@@ -14,16 +14,24 @@ A "step" is one pass of the phoneme-id -> waveform hot path over one batch of sy
 `roofline`: dominant kernel class (HiFi-GAN ResBlock convolutions), CUDA-event timed in the same run.
 `cpu_baseline`: the oracle (a port of the reference's onnxruntime graph) on this box's host cores.
 Prints ONE JSON line on rank 0.
+
+--dump-outputs DIR writes, after the timed steps, what the last timed step computed: the waveform of every utterance
+(float32, `DIR/wav_<i>.npy`) and the frame counts (`DIR/frames.npy`).  Inputs (ids and the seeded noise draws) are the
+same from run to run for the same arguments, so two builds can be compared output for output.
 """
 from __future__ import annotations
 
 import argparse
+import atexit
 import json
 import os
+import shutil
 import subprocess
 import sys
 import threading
 import time
+
+import tempfile
 
 import numpy as np
 
@@ -37,16 +45,6 @@ SR = 22050
 HOP = 256
 
 
-def ncu_traffic():
-    """dram__bytes_read.sum + dram__bytes_write.sum per launch of the dominant kernel from the committed
-    `ncu --set full` capture (profiles/ncu_traffic.json), or null."""
-    p = os.path.join(ROOT, "profiles", "ncu_traffic.json")
-    if os.path.exists(p):
-        with open(p) as f:
-            return json.load(f)
-    return None
-
-
 def read_peaks():
     p = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(p):
@@ -54,7 +52,8 @@ def read_peaks():
             d = json.load(f)
         return {"hbm_gbs": d["hbm_gbs"], "bf16_tflops": d["bf16_tflops"],
                 "bf16_tflops_sustained": d.get("bf16_tflops_sustained", d["bf16_tflops"]), "source": "measured"}
-    return {"hbm_gbs": 6650.0, "bf16_tflops": 1590.0, "bf16_tflops_sustained": 1400.0, "source": "fallback"}
+    # H100 SXM data sheet (700 W): 3.35 TB/s HBM3, 989 dense BF16 TFLOP/s
+    return {"hbm_gbs": 3350.0, "bf16_tflops": 989.0, "bf16_tflops_sustained": 989.0, "source": "fallback"}
 
 
 class ClockSampler:
@@ -156,6 +155,21 @@ def cpu_reference(quality: str, n_phonemes: int, n_utts: int, threads: int):
     return audio, time.perf_counter() - t0
 
 
+MAX_DUMP_BYTES = 64 << 20
+
+
+def dump_outputs(d, job):
+    """The waveforms a caller of the timed path receives (SynthesisJob.fetch), float32, one file per utterance, and the
+    frame counts.  Past 64 MB in all, each waveform is cut to a fixed prefix of equal share."""
+    os.makedirs(d, exist_ok=True)
+    wavs = [a.samples.as_slice().astype(np.float32) for a in job.fetch()]
+    job.close()
+    cap = MAX_DUMP_BYTES // (4 * max(len(wavs), 1)) - 64
+    for i, w in enumerate(wavs):
+        np.save(os.path.join(d, f"wav_{i:03d}.npy"), w[:cap])
+    np.save(os.path.join(d, "frames.npy"), np.array([len(w) // HOP for w in wavs], dtype=np.float64))
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
@@ -168,6 +182,7 @@ def main():
     ap.add_argument("--no-c5", action="store_true", help="skip the C5 mixed-length corpus")
     ap.add_argument("--c5-utts", type=int, default=1024)
     ap.add_argument("--no-secondary", action="store_true", help="skip the C1 / C3 secondary lines (N = 1)")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="write the last timed step's waveforms as DIR/*.npy")
     args = ap.parse_args()
 
     from sonata_b200 import workload
@@ -178,7 +193,7 @@ def main():
     cfg_desc = {"workload": f"{args.workload}: synthetic-{quality} (en_US-lessac-{quality} architecture), "
                             f"{B} x {NPH}-phoneme utterances per GPU, scales [0.667,1,0.8]",
                 "quality": quality, "batch_per_gpu": B, "phonemes": NPH, "ids_per_utt": 2 * NPH + 2,
-                "l2": "working set (>5 GB of activations per step) far exceeds the 126 MB L2",
+                "l2": "working set (>5 GB of activations per step) far exceeds the 50 MB L2",
                 "parallelism": (f"dp{world}: one process per GPU; rank 0 is the frontend (NCCL broadcast of ids, all-reduce of frame "
                                 "counts; utterances are independent, no collective on the waveform path)" if world > 1 else "dp1")}
     cores = os.cpu_count() or 1
@@ -224,6 +239,10 @@ def main():
     if not os.path.exists(_native.LIB_PATH):
         from sonata_b200 import build as _b
         _b.build()
+    # generated voices go to a temporary directory: the tree may be read-only
+    if not os.environ.get("SONATA_B200_VOICE_DIR"):
+        os.environ["SONATA_B200_VOICE_DIR"] = tempfile.mkdtemp(prefix="sonata_voices_")
+        atexit.register(shutil.rmtree, os.environ["SONATA_B200_VOICE_DIR"], True)
     torch.cuda.set_device(local_rank)
     if world > 1:
         dist.init_process_group("nccl", device_id=torch.device("cuda", local_rank))
@@ -271,15 +290,21 @@ def main():
             for k in ("ms", "flops", "bytes", "launches"):
                 acc[k] += r[k]
 
-    def step_device(record):
-        """device-resident pass (results stay in HBM); returns this rank's (audio seconds, device ms)"""
+    kept = []
+
+    def step_device(record, keep=False):
+        """device-resident pass (results stay in HBM); returns this rank's (audio seconds, device ms).  keep: the job
+        stays open (in `kept`) so that its results can be fetched after the timed region"""
         if fe is None:
             job = SynthesisJob(model, all_batches)
             ms = job.run()
             samples = job.lengths()[1]
             if record:
                 add_profile(job.profile())
-            job.close()
+            if keep:
+                kept.append(job)
+            else:
+                job.close()
             return sum(samples) / SR, ms
         fe.synthesize(all_batches if rank == 0 else None, device_only=True)
         owner, samples = fe.last_table
@@ -309,10 +334,14 @@ def main():
     t0 = time.perf_counter()
     audio_local, dev_ms = 0.0, 0.0
     for s in range(args.steps):
-        a_, ms = step_device(True)
+        a_, ms = step_device(True, keep=bool(args.dump_outputs) and s == args.steps - 1)
         audio_local += a_; dev_ms += ms
     barrier()
     wall = time.perf_counter() - t0
+    if args.dump_outputs and rank == 0:
+        if fe is not None:
+            raise SystemExit("--dump-outputs needs --gpus 1")
+        dump_outputs(args.dump_outputs, kept.pop())
     clocks = sampler.stop()
     launches = int(lib.sb200_launch_count()) - launches0
     wall_max, audio_total = reduce_pair(wall, audio_local)
@@ -425,8 +454,7 @@ def main():
         roofline = {
             "bound": "hbm", "kernel": ("conv_tc_kernel" if args.backend >= 1 else "conv_simt_kernel") + " on dec.mrf* (HiFi-GAN ResBlock dilated Conv1d + residual; largest share of the step)",
             "achieved": ach_gbs, "peak": peaks["hbm_gbs"], "unit": "GB/s", "frac": ach_gbs / peaks["hbm_gbs"],
-            "peak_source": f"{peaks['source']} (MEASURED_PEAKS.json hbm_gbs)" if peaks["source"] == "measured" else "fallback 6.65 TB/s",
-            "traffic": ncu_traffic(),
+            "peak_source": f"{peaks['source']} (MEASURED_PEAKS.json hbm_gbs)" if peaks["source"] == "measured" else "fallback: H100 SXM data sheet, 3.35 TB/s",
             "launches": mrf_l, "avg_launch_ms": mrf_ms / mrf_l if mrf_l else None,
             "bytes_per_launch": mrf_bytes / mrf_l if mrf_l else None,
             "share_of_step": mrf_ms / all_ms if all_ms else None,
@@ -451,13 +479,13 @@ def main():
             cpu_base = {"value": a_ / w_, "unit": "audio-s/s", "cores": threads, "kind": "port", "host_cpus": cores,
                         "sample": f"{n_s} utterances of the workload ({NPH} phonemes each), B=1 sequential like speak_batch, "
                                   f"PyTorch-CPU port of the reference graph, torch threads auto-tuned to {threads} of {cores}"}
-        backend_desc = {1: "tcgen05: bf16x2 split (flow, decoder) + chunk-flushed 3xTF32 (text encoder, duration predictor)",
-                        2: "tcgen05 bf16x2 (flow, decoder), fp32 CUDA cores (encoder, duration predictor)", 0: "fp32-simt"}[args.backend]
+        backend_desc = {1: "wgmma: bf16x2 split (flow, decoder) + chunk-flushed 3xTF32 (text encoder, duration predictor)",
+                        2: "wgmma bf16x2 (flow, decoder), fp32 CUDA cores (encoder, duration predictor)", 0: "fp32-simt"}[args.backend]
         line = {
             "metric": "audio-sec/sec", "value": value, "unit": "audio-s/s", "n_gpus": world, "steps": args.steps,
             "warmup": W, "ms_per_step": 1e3 * wall_max / args.steps, "higher_is_better": True,
             "scaling": "weak", "vs_baseline": None,
-            "dtype": "f32 io; tcgen05 with split operands (2 x bf16 flow/decoder, 3 x tf32 encoder/predictor), fp32 accumulate",
+            "dtype": "f32 io; wgmma with split operands (2 x bf16 flow/decoder, 3 x tf32 encoder/predictor), fp32 accumulate",
             "data": "synthetic", "config": cfg_desc,
             "device_ms_per_step": dev_ms_max / args.steps, "audio_s_per_step": audio_total / args.steps,
             "backend": backend_desc, "clocks": clocks, "gpu_launches": launches,

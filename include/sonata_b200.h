@@ -1,9 +1,9 @@
 /*
- * sonata_b200.h — C ABI of libsonata_b200.so: the B200-native replacement for the one hot path of
+ * sonata_b200.h — C ABI of libsonata_b200.so: the H100-native replacement for the one hot path of
  * mush42/sonata, the Piper/VITS phoneme -> waveform synthesis that the reference delegates to
  * onnxruntime (`ort::Session::run`, crates/sonata/models/piper/src/lib.rs:362-379).
  *
- * A Rust `impl SonataModel for B200Vits` (or any FFI host) binds exactly these symbols; each entry
+ * A Rust `impl SonataModel for H100Vits` (or any FFI host) binds exactly these symbols; each entry
  * point cites the reference interface it replaces.  Plain pointers and sizes only — no torch /
  * CUDA types cross this boundary.  All functions are thread-safe per voice (the reference calls
  * `speak_one_sentence` concurrently from rayon workers on one model, synth/src/lib.rs:316-320).
@@ -181,11 +181,10 @@ int32_t sb200_job_profile(const sb200_job* job, sb200_region_stat* out, int32_t 
 /* one convolution on caller data through either backend (kernel unit tests):
  * y[rows][cout] (=|+=) scale * (act(bias + conv_k,dil(lrelu_slope(x))) + res); w is [cout][cin][k];
  * act 0 none, 1 relu, 2 tanh*sigmoid gate (y is [rows][cout/2]); rows >= valid_rows are masked. */
-/* Test hook: the launch configuration the planner of backend 1 (tcgen05 bf16x2 conv) / 2 (tcgen05 3xTF32 conv) would choose
+/* Test hook: the launch configuration the planner of backend 1 (wgmma bf16x2 conv) / 2 (wgmma 3xTF32 conv) would choose
  * for one convolution of `rows` output rows -- nothing is allocated or launched, so it also works without a GPU.
- * out16, backend 1: {nt, image rows, m-tiles, n-tiles, resident, cat, tma_epilogue, pairs, act. stages, weight stages,
- * staging tiles, smem bytes, tma_in, v8, tmem columns, window rows}; backend 2: {nth, image rows, m-pairs, n-tiles, act.
- * stages, weight stages, chunk K-blocks, smem bytes, tmem columns, window rows, 0...}.  Returns 0, or 19 if unsupported. */
+ * out16, backend 1: {nt, image rows, m-tiles, n-tiles, ring stages, smem bytes, window rows, 0...}; backend 2: {nth, image
+ * rows, m-tiles, n-tiles, ring stages, chunk K-blocks, smem bytes, window rows, 0...}.  Returns 0, or 19 if unsupported. */
 int32_t sb200_debug_plan(int32_t backend, int64_t rows, int32_t cin, int32_t cout, int32_t k, int32_t dil, int32_t act,
                          int32_t has_res, int32_t accumulate, int32_t* out16);
 int32_t sb200_debug_conv(int32_t device, int32_t backend, const float* x, int32_t rows, int32_t cin, const float* w,
@@ -194,7 +193,7 @@ int32_t sb200_debug_conv(int32_t device, int32_t backend, const float* x, int32_
                          sb200_error* err);
 /* kernels launched by this library since load (host-side counter) */
 uint64_t sb200_launch_count(void);
-/* select the contraction backend: 0 = fp32 CUDA-core implicit GEMM, 1 = tcgen05 (3xTF32) where
+/* select the contraction backend: 0 = fp32 CUDA-core implicit GEMM, 1 = wgmma (3xTF32) where
  * implemented; returns the previous value */
 int32_t sb200_set_backend(sb200_voice* v, int32_t backend);
 

@@ -1,4 +1,4 @@
-"""Builds sonata_b200/lib/libsonata_b200.so with nvcc for sm_100a (cross-compiles without a GPU)."""
+"""Builds sonata_b200/lib/libsonata_b200.so with nvcc for sm_90a (cross-compiles without a GPU)."""
 from __future__ import annotations
 
 import os
@@ -11,9 +11,9 @@ CSRC = os.path.join(HERE, "csrc")
 OBJ = os.path.join(os.path.dirname(HERE), "build", os.environ.get("SB200_OBJ_DIR", "obj"))
 LIB = os.environ.get("SB200_LIB_OUT") or os.path.join(HERE, "lib", "libsonata_b200.so")
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
-FLAGS = ["-O3", "-std=c++17", "-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo",
+FLAGS = ["-O3", "-std=c++17", "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo",
          "-Xcompiler", "-fPIC", "-Xcompiler", "-Wall", "-Xcompiler", "-Wno-unused-function"] + \
-        os.environ.get("SB200_NVCC_EXTRA", "").split()     # e.g. -DSB200_TC_TRACE_BUILD (tools/trace_tc.py)
+        os.environ.get("SB200_NVCC_EXTRA", "").split()     # extra nvcc flags, e.g. -DNDEBUG
 
 
 def _newer(src: str, dst: str, deps) -> bool:
@@ -48,7 +48,7 @@ def build(force: bool = False, verbose: bool = False) -> str:
             if verbose and out:
                 sys.stderr.write(out)
     if jobs or not os.path.exists(LIB):
-        run([NVCC, "-shared", "-o", LIB] + objs + ["-gencode", "arch=compute_100a,code=sm_100a"])
+        run([NVCC, "-shared", "-o", LIB] + objs + ["-gencode", "arch=compute_90a,code=sm_90a"])
     return LIB
 
 

@@ -1,5 +1,5 @@
 """`sonata` command-line frontend (SURVEY §8f row N4): the argument set and the JSON-lines protocol of the reference
-CLI (crates/frontends/cli/src/main.rs:32-260) over the B200 engine.
+CLI (crates/frontends/cli/src/main.rs:32-260) over the H100 engine.
 
     python -m sonata_b200.cli voice.onnx.json -f phonemes.txt -o out.wav --mode parallel
     echo '{"text": "hɛloʊ", "mode": "realtime", "chunk_size": 100}' | python -m sonata_b200.cli voice.onnx.json > pcm.raw
@@ -24,7 +24,7 @@ MODES = ("lazy", "parallel", "realtime")
 
 
 def build_parser() -> argparse.ArgumentParser:
-    ap = argparse.ArgumentParser(prog="sonata", description="B200-native Piper/VITS synthesis (phoneme input)")
+    ap = argparse.ArgumentParser(prog="sonata", description="H100-native Piper/VITS synthesis (phoneme input)")
     ap.add_argument("config", help="Model config (<voice>.onnx.json)")
     ap.add_argument("-f", "--input-file", help="Input text file (default stdin: one JSON request per line)")
     ap.add_argument("-o", "--output-file", help="Output WAV file (default stdout: raw i16 PCM)")

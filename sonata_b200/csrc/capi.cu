@@ -113,7 +113,7 @@ double now_ms() {
 
 extern "C" {
 
-const char* sb200_version(void) { return "sonata_b200 0.1.0 (sm_100a)"; }
+const char* sb200_version(void) { return "sonata_b200 0.1.0 (sm_90a)"; }
 void sb200_string_free(char* s) { free(s); }
 void sb200_ids_free(int64_t* ids) { free(ids); }
 void sb200_buffer_free(float* p) { free(p); }
@@ -400,16 +400,14 @@ int32_t sb200_debug_plan(int32_t backend, int64_t rows, int32_t cin, int32_t cou
     p.x = stand_in; p.ldx = cin; p.rows_in = R; p.cin = cin; p.in_slope = 0.1f;
     p.w = stand_in; p.bias = stand_in; p.ldw = cout; p.cout = cout;
     p.tc_nt = cout <= 128 ? cout : (cout % 128 == 0 ? 128 : (cout % 96 == 0 ? 96 : 0));      // voice.cu tc_tile_for
-    p.wtc = p.tc_nt ? stand_in : nullptr; p.wcat = (p.tc_nt && p.tc_nt <= 64) ? stand_in : nullptr; p.wtf = stand_in;
+    p.wtc = p.tc_nt ? stand_in : nullptr; p.wtf = stand_in;
     p.ntaps = k;
     for (int t = 0; t < k; t++) p.tap_off[t] = (t - (k - 1) / 2) * dil;
     p.min_off = p.tap_off[0]; p.span = (k - 1) * dil;
     p.rows_q = R; p.orow_mul = 1; p.orow_add = 0;
     p.act = act; p.scale = 1.f; p.res = has_res ? stand_in : nullptr; p.ldres = cout;
     p.y0 = stand_in; p.ldy0 = ycols; p.acc0 = accumulate; p.split = cout; p.y1 = stand_in; p.ldy1 = ycols; p.acc1 = accumulate;
-    plan_assume_tensor_maps() = true;
     const bool ok = backend == 2 ? conv_tf_plan_info(p, out16) : conv_tc_plan_info(p, out16);
-    plan_assume_tensor_maps() = false;
     return ok ? 0 : 19;
 }
 
@@ -433,39 +431,21 @@ int32_t sb200_debug_conv(int32_t device, int32_t backend, const float* x, int32_
         SB_CUDA(cudaMalloc(&dend, 4)); SB_CUDA(cudaMemcpy(dend, &valid_rows, 4, cudaMemcpyHostToDevice));
         ConvArgs p{};
         p.x = dx; p.ldx = cin; p.rows_in = R; p.cin = cin; p.in_slope = in_slope;
-        p.w = cw.w; p.bias = cw.bias; p.ldw = cw.ldw; p.cout = cw.cout; p.wtc = cw.wtc; p.tc_nt = cw.tc_nt; p.wcat = cw.wcat;
+        p.w = cw.w; p.bias = cw.bias; p.ldw = cw.ldw; p.cout = cw.cout; p.wtc = cw.wtc; p.tc_nt = cw.tc_nt;
         p.ntaps = cw.ntaps; memcpy(p.tap_off, cw.tap_off, sizeof(p.tap_off)); p.min_off = cw.min_off; p.span = cw.span;
         p.rows_q = R; p.orow_mul = 1; p.orow_add = 0;
         p.map = RowMap{dend, R, 1, R};
         p.act = act; p.scale = scale; p.res = dres; p.ldres = cout;
         p.y0 = dy; p.ldy0 = ycols; p.acc0 = accumulate; p.split = cout; p.y1 = dy; p.ldy1 = ycols; p.acc1 = accumulate;
         if (res && getenv("SB200_DEBUG_RES_IS_X") && cin == cout) { p.res = dx; p.ldres = cin; }   // ResBlock aliasing (timing only)
-        long long* dtrace = nullptr;
-        const bool want_trace = backend == 1 && getenv("SB200_TC_TRACE") != nullptr;
-        if (want_trace) { SB_CUDA(cudaMalloc(&dtrace, 48 * 8 * 8)); SB_CUDA(cudaMemset(dtrace, 0, 48 * 8 * 8)); }
         p.wtf = cw.wtf;
         if (backend == 2) {
             if (!conv_tf_supported(p)) throw Error(19, "conv shape not supported by the tf32 chunk-flush backend");
             launch_conv_tf(p, 0);
         } else if (backend == 1) {
-            if (!conv_tc_supported(p)) throw Error(19, "conv shape not supported by the tcgen05 backend");
-            if (want_trace) launch_conv_tc(p, 0); // warm-up before the traced run (timing only: RMW cases run twice)
-            p.trace = dtrace;
+            if (!conv_tc_supported(p)) throw Error(19, "conv shape not supported by the wgmma backend");
             launch_conv_tc(p, 0);
         } else launch_conv_simt(p, 0);
-        if (want_trace) {
-            SB_CUDA(cudaDeviceSynchronize());
-            std::vector<long long> t(48 * 8);
-            SB_CUDA(cudaMemcpy(t.data(), dtrace, 48 * 8 * 8, cudaMemcpyDeviceToHost));
-            const long long t0 = t[0];
-            fprintf(stderr, "tile: prod_issue prod_landed prod_conv | mma_afull mma_issued | epi_accfull epi_tmem epi_stored  (cycles rel. to first issue)\n");
-            for (int i = 0; i < 48; i++) {
-                fprintf(stderr, "%3d:", i);
-                for (int k = 0; k < 8; k++) fprintf(stderr, " %9lld", t[i * 8 + k] ? t[i * 8 + k] - t0 : -1LL);
-                fprintf(stderr, "\n");
-            }
-            cudaFree(dtrace);
-        }
         cudaError_t e = cudaDeviceSynchronize();
         if (e == cudaSuccess) e = cudaMemcpy(y, dy, (size_t)rows * ycols * 4, cudaMemcpyDeviceToHost);
         cudaFree(dx); cudaFree(dy); cudaFree(dend); if (dres) cudaFree(dres);

@@ -1,4 +1,4 @@
-// Shared declarations for libsonata_b200 (sm_100a only).
+// Shared declarations for libsonata_b200 (sm_90a only).
 //
 // Activation layout everywhere: TIME-MAJOR fp32 matrices  A[row][channel]  (channel contiguous).
 // A "row" is one time step (phoneme id at the X level, frame at the Y level, sample-group at the
@@ -42,13 +42,11 @@ enum ConvAct { ACT_NONE = 0, ACT_RELU = 1, ACT_GATE = 2 };
 struct ConvArgs {
     const float* x; int ldx; int rows_in; int cin; float in_slope;
     const float* w; const float* bias; int ldw; int cout;
-    const float* wtc; int tc_nt;                                  // tcgen05 weight images (conv_tc.cu) or null
-    const float* wcat;                                            // hi/lo-stacked tap-pair images (conv_tc.cu cat mode) or null
+    const float* wtc; int tc_nt;                                  // bf16 hi/lo weight images (conv_tc.cu) or null
     const float* wtf;                                             // tf32 hi/lo images (conv_tf.cu) or null
     int ntaps; int tap_off[SB_MAX_TAPS]; int min_off; int span;   // span = max_off - min_off
     int rows_q; int orow_mul; int orow_add;
-    int phase_cols;                                               // >0: fused polyphase ConvTranspose (tcgen05 path only)
-    long long* trace;                                             // optional per-role clock64() timeline (debug)
+    int phase_cols;                                               // >0: fused polyphase ConvTranspose (conv_tc.cu only)
     RowMap map;                                                   // validity of q
     int act; float scale;
     const float* res; int ldres;
@@ -97,9 +95,9 @@ struct PerDeviceOnce {
 };
 
 // Programmatic dependent launch.  The step is a chain of ~170-200 dependent kernels; at single-utterance sizes most of
-// them run for 5-30 us, so the launch gap and each kernel's prologue (mbarrier init, TMEM allocation, tensor-map fetch)
+// them run for 5-30 us, so the launch gap and each kernel's prologue (mbarrier init, weight fetch)
 // are a visible part of the step.  Every kernel of the library is launched with the programmatic-stream-serialization
-// attribute and starts with pdl_wait() BEFORE its first access to global memory (tcgen05 kernels: after their prologue),
+// attribute and starts with pdl_wait() BEFORE its first access to global memory (wgmma kernels: after their weight fetch is issued),
 // after a pdl_trigger() at its very top: the following kernels' CTAs may become resident and run their own prologues (and
 // fetch their weights, which no kernel writes) while this kernel is still working; their pdl_wait() returns only when the
 // preceding grid has completed and its writes are visible.  Nothing before a pdl_wait() touches memory another kernel
@@ -133,8 +131,6 @@ void launch_conv_tc(const ConvArgs& a, cudaStream_t st);
 bool try_launch_conv_tc(const ConvArgs& a, cudaStream_t st);
 size_t conv_tc_weight_floats(int cin, int cout, int ntaps, int nt);
 void conv_tc_build_weights(const float* wt, int ldw, int cin, int cout, int ntaps, int nt, float* out);
-size_t conv_tc_cat_weight_floats(int cin, int cout, int ntaps, int nt);
-void conv_tc_build_weights_cat(const float* wt, int ldw, int cin, int cout, int ntaps, int nt, float* out);
 bool conv_tf_supported(const ConvArgs& a);
 bool conv_tf_plan_info(const ConvArgs& a, int* out16);
 void launch_conv_tf(const ConvArgs& a, cudaStream_t st);

@@ -3,7 +3,7 @@
 // This is the correctness reference for every dense contraction on the path (text-encoder 1x1 /
 // k3 convs, duration-predictor 1x1s, WaveNet k5 convs, HiFi-GAN k3..k11 dilated convs and the
 // polyphase ConvTranspose1d), i.e. what onnxruntime's MLAS im2col+SGEMM does on the reference
-// side of `session.run` (piper/src/lib.rs:362-379).  The tcgen05 kernel (conv_tc.cu) implements
+// side of `session.run` (piper/src/lib.rs:362-379).  The wgmma kernel (conv_tc.cu) implements
 // the same ConvArgs contract for the big ResBlock / WaveNet contractions.
 //
 // Tiling: CTA = 256 threads, BM x BN output tile, K loop over (32-channel chunk, tap).

@@ -1,58 +1,40 @@
-// tcgen05 implicit-GEMM Conv1d with a 2-term BF16 split ("bf16x2", fp32 accumulate in TMEM), sm_100a.
+// wgmma implicit-GEMM Conv1d with a 2-term BF16 split ("bf16x2", fp32 accumulate in registers), sm_90a.
 //
 // Same contract as conv_simt.cu (ConvArgs): out[q][n] = epi(bias[n] + sum_t sum_c f(x[q+off_t][c]) w[t][c][n]).
-// GEMM view per tile: D[128 rows x NT cols] (fp32, TMEM) += A_t[128 x 32] . W_t[32 x NT] over (32-channel
-// K-block, tap).
+// GEMM view per tile: D[128 rows x NT cols] += A_t[128 x 32] . W_t[32 x NT] over (32-channel K-block, tap).
 //
 // Precision.  A single reduced-precision MMA misses the 1e-3 waveform tolerance (TF32: 1.9e-3 / 3.6e-3 on
 // the medium / high voice).  Every operand is therefore split  v = hi + lo,  hi = bf16_rn(v),
 // lo = bf16_rn(v - hi)  (16 mantissa bits together) and three MMAs accumulate  hi*hi + lo*hi + hi*lo.
-// End-to-end waveform error 2e-5 / 3.5e-5 (oracle emulation) -- the same as a 3xTF32 split, which was
-// implemented first and needs TWICE the MMA instructions (K = 8 per tf32 MMA vs 16 per bf16 MMA).  That
-// matters because a measured ~80-cycle floor applies to every M=128 SS-mode MMA whatever its N
-// (tools/micro/mma_bench.cu: 81.4 / 80.1 / 79.6 cycles at N = 32 / 64 / 128), and the hot layers here
-// have N = C_out = 32..128.
+// End-to-end waveform error 2e-5 / 3.5e-5 (oracle emulation) -- the same as a 3xTF32 split at half the MMAs
+// (K = 16 per bf16 MMA against 8 per tf32 MMA).
 //
-// Data path:
-//   * activations: one TMA tensor load per stage (cp.async.bulk.tensor.2d: box = 32 channels x window rows,
-//     unswizzled, zero-filled outside the array; fallbacks: one linear bulk copy when rows are contiguous, or
-//     cp.async / LDGSTS) brings the raw fp32 (128 + span)-row WINDOW of a K-block into the smem ring, several
-//     stages ahead; the producer warps then apply the leaky-ReLU prologue, split hi/lo and rewrite each
-//     128-byte row IN PLACE as  [hi: 32 ch bf16 | lo: 32 ch bf16]  in the canonical K-major SWIZZLE_128B
-//     layout (row r at r*128 B, 16-B chunk c at (c ^ (r & 7))).  A tap is only a descriptor whose start
-//     address is shifted by off_t rows (the swizzle is a function of the absolute smem address), so a k-tap
-//     conv stages its input once and issues k x 6 (cat mode: k x 4) MMAs on it;
-//   * weights: pre-split, pre-swizzled tile images written at voice-load time; one cp.async.bulk (UBLKCP)
-//     per (K-block, tap) stage, resident in smem for the whole CTA when they fit; otherwise streamed through a
-//     ring -- on large launches ONE ring for both half-pipelines, which then walk the two m-tiles of a pair
-//     that shares the n-tile, so a stage is fetched from L2 once per 256 output rows;
-//   * MMA: tcgen05.mma.kind::f16 (UTCHMMA), issued from warp-uniform code under elect.sync;
-//     tcgen05.commit releases ring slots / publishes the accumulator;
-//   * epilogue, MODE 0 (general): tcgen05.ld 32x32b.x32 (LDTM) -> bias / gate / residual / scale /
-//     accumulate -> HBM with 256-bit row-per-thread accesses, the residual / read-modify-write operands
-//     prefetched before the accumulator is awaited;
-//   * epilogue, MODE 2 (32- and 64-channel outputs in one column tile): the residual and read-modify-write
-//     operands of a 32-column chunk arrive by TMA tensor loads into SWIZZLE_128B staging tiles, the result is
-//     written over the residual tile in place and leaves with one TMA tensor store per chunk, issued by an
-//     agent lane of the idle weight warp (resident weights) or by thread 0 of the epilogue group itself
-//     (streamed weights) -- the SM's load/store path sees no global traffic at all (that path, not HBM,
-//     bounded these layers: its row-per-thread accesses also slow the producers' conversion 2x);
-// Persistent CTAs (one per SM) walk tiles blockIdx.x, +gridDim.x, ...; mbarrier pipelines (activation
-// ring, weight ring, 4-stage TMEM accumulator ring, MODE 2 staging) run across tile boundaries.
-// Warps: w0/w1 MMA issuers on alternating tiles (w0 also allocates TMEM), w2/w3 weight producers and
-// MODE 2 TMA agents, w4-7 / w8-11 two activation-producer groups, w12-15 / w16-19 two epilogue groups (one
-// per half-pipeline).  Every mbarrier wait carries a watchdog that traps instead of hanging the GPU.
+// One CTA = one 128-row x NT-column tile, two warpgroups (rows 0-63 / 64-127), a two-stage ring over K-blocks:
+//   * activations: the raw fp32 (128 + span)-row WINDOW of a K-block (32 channels = one 128-byte row) arrives by
+//     cp.async (rows outside the array zero-filled); all threads then apply the leaky-ReLU prologue, split hi/lo and
+//     rewrite each row IN PLACE as [hi: 32 ch bf16 | lo: 32 ch bf16] in the K-major SWIZZLE_128B layout (row r at
+//     r*128 B, 16-B chunk c at (c ^ (r & 7))).  A tap is the same window read from a row offset: the A operand
+//     comes from registers (wgmma with A in registers), loaded per thread from the swizzled image at any row,
+//     so a k-tap conv stages its input once;
+//   * weights: pre-split, pre-swizzled images written at voice-load time; one cp.async.bulk (TMA) per tap of the
+//     K-block, completion on an mbarrier; the next K-block's window and weights load while this one computes;
+//   * MMA: wgmma.mma_async m64nNTk16 (B from shared memory by descriptor), six per (tap, K-block) and warpgroup;
+//   * epilogue: bias / gate / ReLU / residual / scale / accumulate straight from the accumulator registers.
+// Every mbarrier wait carries a watchdog that traps instead of hanging the GPU.
 #include "tc_common.cuh"
-#include <cuda.h>
 #include <stdlib.h>
 #include <string.h>
-#include <unordered_map>
 
 namespace sb200 {
 
-static int tc_num_sms() {
+int wg_num_sms() {
     static int n = 0;
-    if (!n) { int dev = 0; cudaGetDevice(&dev); cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev); if (n <= 0) n = 148; }
+    if (!n) {
+        int dev = 0;
+        if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess)
+            cudaGetLastError();
+        if (n <= 0) n = 132;
+    }
     return n;
 }
 
@@ -60,734 +42,221 @@ namespace {
 
 using namespace tcx;
 
-__device__ __forceinline__ void tma_load_2d(uint32_t dst, const CUtensorMap* tm, uint32_t bar, int c0, int c1) {
-    asm volatile("cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
-                 ::"r"(dst), "l"(tm), "r"(bar), "r"(c0), "r"(c1) : "memory");
-}
-
 struct TcLaunch {
     int nt;          // columns per CTA tile (multiple of 32, <= 128)
-    int wnt;         // rows of a weight IMAGE (the voice's tile width); nt == wnt, or wnt / 2 on small launches: the CTA
-                     // then takes half an image (a 64-row half keeps the image's swizzle: 64 % 8 == 0)
+    int wnt;         // rows of a weight IMAGE (the voice's tile width); nt == wnt, or a part of it (a multiple of 32 rows that
+                     // divides it: every part keeps the image's swizzle, 32 % 8 == 0)
     int win;         // window rows (multiple of 8)
-    int na;          // activation ring stages PER PIPELINE
-    int ws;          // weight stages: all (K-block, tap) stages when resident (shared), else ring stages PER PIPELINE
-    int resident;    // weights loaded once per CTA (single n-tile, short K loop)
-    int tmem_cols;   // power of two >= 4*nt (two accumulator stages per pipeline)
     int ntiles_m, ntiles_n;
-    uint32_t idesc;
-    int bulk_in;     // input rows are contiguous 128-B rows (ldx == 32): a window is ONE block -> one TMA bulk copy
-    int tma_in;      // the window of a K-block arrives by ONE TMA tensor load (box 32 channels x win rows; rows outside
-                     // the array are zero-filled by the engine): no LDGSTS traffic through the LSU / L1TEX pipe
-    int depth;       // window loads in flight per pipeline (< na: see plan())
-    int v8;          // every epilogue operand is 32-byte aligned: 256-bit global accesses
-    int tma_st;      // MODE 2: output tile leaves through a TMA tensor store
-    int pairs;       // streamed weights: the CTA walks PAIRS of m-tiles that share the n-tile (pipeline p takes member p), and the
-                     // two pipelines consume ONE weight ring -- every stage is fetched from L2 once per 256 output rows
-    int nstg;        // MODE 2: staging tiles per pipeline (1 = residual-in / output, 2 = + previous value of an accumulated buffer)
-    // "cat" mode (nt <= 64, resident weights): the weight image of a tap stacks the hi rows and the lo rows along N,
-    // so  A_hi x [W_hi ; W_lo]  is ONE MMA of N = 2*nt (columns [0,nt) = hi*hi, [nt,2nt) = hi*lo) and  A_lo x W_hi
-    // accumulates into the first nt columns: 2 MMAs instead of 3 per (tap, K-step).  One thread can issue an
-    // M=128 MMA only every ~85-100 cycles whatever N is, and once the epilogue traffic moved to the TMA engine
-    // the MMA issue loop was the longest stage of the 32-channel layers.  The epilogue adds the two column halves.
-    int cat;
-    int accw;        // TMEM columns per accumulator stage (nt, or 2*nt in cat mode)
-    uint32_t idesc2; // instruction descriptor with N = 2*nt
 };
 
-constexpr int TC_MAXCH = 7;             // 32-B input pieces per producer thread per stage (win <= 224 rows)
-constexpr int TC_GROUP = 128;           // threads per producer group
-constexpr int TC_PROD0 = 4;             // first activation-producer warp
-constexpr int TC_EPI0 = 12;             // first epilogue warp
-constexpr int TC2_THREADS = 640;        // w0/w1 MMA issuers, w2/w3 weight producers, w4-7 / w8-11 activation groups,
-                                        // w12-15 / w16-19 epilogue groups (pipeline 0 / 1)
-constexpr int TC_MAX_ASTAGES = 4;       // per pipeline
-constexpr int TC_MAX_WRING = 44;        // barrier slots for the resident weight set (or 2 x ring)
-constexpr int TC_OUT_BYTES = 128 * 128;  // MODE 2: one staged output tile (128 rows x 32 fp32), two per pipeline
+constexpr int TC_THREADS = 256;         // two warpgroups: tile rows [0, 64) and [64, 128)
+constexpr int TC_STAGES = 2;
 
-// The CTA runs TWO independent half-pipelines (p = 0 / 1 own tiles tl = p, p+2, ...): one thread can issue an
-// M=128 MMA only every ~83 cycles whatever N is, while two issuing warps double the aggregate rate
-// (tools/micro/mma_bench.cu: N=32 385 -> 774 MAC/clk/SM, N=128 1572 -> 2046 = peak).  Each pipeline has its
-// own activation ring, weight ring and accumulator pair, so no mbarrier can be lapped by the other pipeline.
-// MODE 0: plain mapping (one tap per MMA, N = nt).
-// MODE 2: plain mapping for 32-channel outputs with the tile written by ONE TMA tensor store from a swizzled
-// shared-memory staging tile (see the epilogue).
-template <int MODE>
-__global__ void __launch_bounds__(TC2_THREADS, 1) conv_tc_kernel(const ConvArgs a, const TcLaunch L,
-                                                                  const __grid_constant__ CUtensorMap tm_out,
-                                                                  const __grid_constant__ CUtensorMap tm_res,
-                                                                  const __grid_constant__ CUtensorMap tm_x) {
+template <int NT>
+__global__ void __launch_bounds__(TC_THREADS, 1) conv_tc_kernel(const ConvArgs a, const TcLaunch L) {
     pdl_trigger();
-    if (threadIdx.x == 0) TC_TRACE(a, 47, 0);                   // launch-level stamps live in row 47 of the trace
     extern __shared__ __align__(1024) uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-    const uint32_t a_buf = (uint32_t)L.win * 128u;              // one [hi|lo] window image
-    const uint32_t w_stage = (uint32_t)L.nt * (L.cat ? 256u : 128u);   // one weight image: a tap ([hi|lo] rows), or in cat mode
-                                                                // a PAIR of taps ([hi_t|hi_t+1] rows, then [lo_t|lo_t+1] rows)
-    const int wslots = L.resident ? L.ws : 2 * L.ws;
-    uint8_t* A0 = smem;                                         // [2][na] stages
-    uint8_t* W0 = A0 + (size_t)2 * L.na * a_buf;                // resident: [ws]; ring: [2][ws]
-    uint8_t* EX = W0 + (size_t)wslots * w_stage;                // MODE 2: [2 pipelines][2] staging tiles
-    uint64_t* bars = reinterpret_cast<uint64_t*>(EX + (MODE == 2 ? 2 * L.nstg * TC_OUT_BYTES : 0));
-    uint64_t* w_full = bars;                               // [TC_MAX_WRING]
-    uint64_t* w_empty = w_full + TC_MAX_WRING;             // [TC_MAX_WRING]
-    uint64_t* a_full = w_empty + TC_MAX_WRING;             // [2][TC_MAX_ASTAGES]
-    uint64_t* a_empty = a_full + 2 * TC_MAX_ASTAGES;       // [2][TC_MAX_ASTAGES]
-    uint64_t* acc_full = a_empty + 2 * TC_MAX_ASTAGES;     // [4]  (index = pipeline + 2 * stage)
-    uint64_t* acc_empty = acc_full + 4;                    // [4]
-    uint64_t* raw_full = acc_empty + 4;                    // [2][TC_MAX_ASTAGES] bulk-loaded raw windows
-    uint64_t* staged = raw_full + 2 * TC_MAX_ASTAGES;      // [2] MODE 2: output tile staged by the 128 epilogue threads
-    uint64_t* epi_full = staged + 2;                       // [2] MODE 2: residual / previous-value tiles landed (TMA)
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(epi_full + 2);
-
+    const uint32_t a_buf = (uint32_t)L.win * 128u;               // one window image
+    const uint32_t w_tap = (uint32_t)NT * 128u;                  // one tap of a weight stage ([hi|lo] rows)
+    const uint32_t w_buf = (uint32_t)a.ntaps * w_tap;
+    const uint32_t A0 = smem_u32(smem), W0 = A0 + TC_STAGES * a_buf;
+    uint64_t* bars = reinterpret_cast<uint64_t*>(smem + TC_STAGES * (a_buf + w_buf));
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+    const int m_tile = (int)blockIdx.x / L.ntiles_n, n_tile = (int)blockIdx.x % L.ntiles_n;
     const int nkb = a.cin / 32;
-    const int per_tile = nkb * a.ntaps;
-    const int npairs = (a.ntaps + 1) >> 1;
-    const int wper = L.cat ? nkb * npairs : per_tile;            // weight images per tile
-    // tile tl of this CTA -> (m-tile, n-tile).  Plain: tiles blockIdx.x, +gridDim.x, ... over (m, n).  Pairs: the same walk
-    // over (m-pair, n); tile 2k + p is member p of the CTA's k-th pair (an odd m-tile count leaves one empty member whose
-    // rows lie past the end of the array: loads are zero-filled, nothing is stored).
-    const int total_tiles = L.pairs ? ((L.ntiles_m + 1) / 2) * L.ntiles_n : L.ntiles_m * L.ntiles_n;
-    const int my_units = (total_tiles - (int)blockIdx.x + (int)gridDim.x - 1) / (int)gridDim.x;
-    const int my_tiles = L.pairs ? 2 * my_units : my_units;
-    auto tile_m = [&](int tl) {
-        if (L.pairs) return 2 * (((int)blockIdx.x + (tl >> 1) * (int)gridDim.x) / L.ntiles_n) + (tl & 1);
-        return ((int)blockIdx.x + tl * (int)gridDim.x) / L.ntiles_n;
-    };
-    auto tile_n = [&](int tl) {
-        if (L.pairs) return ((int)blockIdx.x + (tl >> 1) * (int)gridDim.x) % L.ntiles_n;
-        return ((int)blockIdx.x + tl * (int)gridDim.x) % L.ntiles_n;
-    };
 
-    if (warp == 3) {
-        // all barriers are initialised by one warp in parallel (a single thread doing the ~120 inits one after the other
-        // was ~2 us of every launch); bars[] order: w_full, w_empty, a_full, a_empty, acc_full, acc_empty, raw_full,
-        // staged, epi_full
-        constexpr int NB = 2 * TC_MAX_WRING + 6 * TC_MAX_ASTAGES + 12;
-        for (int i = lane; i < NB; i += 32) {
-            const int j = i - 2 * TC_MAX_WRING;
-            const uint32_t cnt = j < 0 ? ((L.pairs && i >= TC_MAX_WRING) ? 2u : 1u) : j < 8 ? (uint32_t)TC_GROUP : j < 20 ? 1u : j < 24 ? 128u : j < 32 ? 1u : j < 34 ? 128u : 1u;
-            mbar_init(smem_u32(&bars[i]), cnt);
-        }
+    if (tid == 0) {
+        for (int s = 0; s < TC_STAGES; s++) mbar_init(smem_u32(&bars[s]), 1);
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-        if (lane == 0) {                       // descriptor fetches overlap the rest of the prologue
-            if (L.tma_in) asm volatile("prefetch.tensormap [%0];" ::"l"(&tm_x) : "memory");
-            if (MODE == 2) {
-                asm volatile("prefetch.tensormap [%0];" ::"l"(&tm_out) : "memory");
-                if (a.res) asm volatile("prefetch.tensormap [%0];" ::"l"(&tm_res) : "memory");
-            }
-        }
     }
-    if (warp == 0) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)),
-                     "r"((uint32_t)L.tmem_cols) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
-    if (threadIdx.x == 0) TC_TRACE(a, 47, 1);
-    // everything above (barriers, TMEM, tensor-map prefetch) overlapped the previous kernels' tails; from here on global
-    // memory written by them is read -- except by the weight warps, whose bulk copies read constants (their TMA-agent
-    // part waits before its first fetch)
-    if (warp != 2 && warp != 3) pdl_wait();
-    if (threadIdx.x == 0) TC_TRACE(a, 47, 2);
 
-    // MODE 2 staging traffic (used by the TMA-agent warps, or by the epilogue groups themselves when the weight warps
-    // are busy streaming)
-    const int nch = L.nt / 32;                       // MODE 2: 32-column chunks per tile, one staged item each
-    // MODE 2 item `it` of pipeline pp: tile pp + 2 * (it / nch), chunk it % nch
-    auto item_row = [&](int pp, int it) { return tile_m(pp + 2 * (it / nch)) * 128; };
-    auto agent_fetch = [&](int pp, int it) {
-        const uint32_t st = smem_u32(EX + (size_t)pp * L.nstg * TC_OUT_BYTES);     // [0] residual-in / output, [1] previous
-        const uint32_t bytes = (a.res ? TC_OUT_BYTES : 0) + (a.acc0 ? TC_OUT_BYTES : 0);
-        // nothing to fetch: still publish "staging tile free" (the previous store has been read out)
-        if (!bytes) { mbar_arrive(smem_u32(&epi_full[pp])); return; }
-        const int r0 = item_row(pp, it), c0 = (it % nch) * 32;
-        mbar_expect_tx(smem_u32(&epi_full[pp]), bytes);
-        if (a.res) tma_load_2d(st, &tm_res, smem_u32(&epi_full[pp]), c0, r0);
-        if (a.acc0) tma_load_2d(st + TC_OUT_BYTES, &tm_out, smem_u32(&epi_full[pp]), c0, r0);
+    // weight stage kb: tap t is rows [part * NT, part * NT + NT) of image (n-tile of the voice, kb, t)
+    const int vf = L.wnt / NT;
+    const size_t w_image = (size_t)L.wnt * 128u;
+    const uint8_t* wsrc = reinterpret_cast<const uint8_t*>(a.wtc) + (size_t)(n_tile / vf) * nkb * a.ntaps * w_image +
+                          (size_t)(n_tile % vf) * w_tap;
+    auto issue_w = [&](int kb, int s) {
+        if (tid == 0) {
+            const uint32_t bar = smem_u32(&bars[s]);
+            mbar_expect_tx(bar, w_buf);
+            for (int t = 0; t < a.ntaps; t++)
+                bulk_g2s(W0 + s * w_buf + t * w_tap, wsrc + (size_t)(kb * a.ntaps + t) * w_image, w_tap, bar);
+        }
     };
-    auto agent_store = [&](int pp, int it) {
-        const uint32_t st = smem_u32(EX + (size_t)pp * L.nstg * TC_OUT_BYTES);
-        asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];"
-                     ::"l"(&tm_out), "r"(st), "r"((it % nch) * 32), "r"(item_row(pp, it)) : "memory");
-        asm volatile("cp.async.bulk.commit_group;" ::: "memory");
-        asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");
+    // window of K-block kb: raw fp32 rows, linear (row r at r * 128 B)
+    const int rbase = m_tile * 128 + a.min_off;
+    auto issue_a = [&](int kb, int s) {
+        for (int idx = tid; idx < L.win * 8; idx += TC_THREADS) {
+            const int gr = rbase + (idx >> 3);
+            const bool ok = gr >= 0 && gr < a.rows_in;
+            const float* src = ok ? a.x + (size_t)gr * a.ldx + kb * 32 + (idx & 7) * 4 : a.x;
+            cp_async16(A0 + s * a_buf + (uint32_t)idx * 16u, src, ok ? 16u : 0u);
+        }
+        cp_async_commit();
     };
 
-    if (warp < 2) {
-        // ===================== MMA issuer of pipeline p = warp =====================
-        // The WHOLE warp walks the loop with warp-uniform values (descriptors live in uniform registers, no
-        // R2UR waterfall loops); only the tcgen05 instructions sit under elect.sync.
-        // K-major SWIZZLE_128B descriptor (cute::UMMA::SmemDescriptor v1): start>>4 | LBO 1<<16 | SBO (1024>>4)<<32 |
-        // version 1<<46 | layout SWIZZLE_128B 2<<61; "matrix base offset" stays 0 even for row-shifted starts
-        // (measured: a non-zero base offset breaks every k > 1 case).
-        const int p = warp;
-        const uint64_t desc_hi = ((uint64_t)1 << 16) | ((uint64_t)(1024 >> 4) << 32) | ((uint64_t)1 << 46) | ((uint64_t)2 << 61);
-        uint8_t* Ap = A0 + (size_t)p * L.na * a_buf;
-        const bool own_ring = !L.resident && !L.pairs;           // pairs: one ring of 2 * ws slots for both pipelines
-        uint8_t* Wp = own_ring ? W0 + (size_t)p * L.ws * w_stage : W0;
-        uint64_t* wf = own_ring ? w_full + p * L.ws : w_full;
-        uint64_t* we = own_ring ? w_empty + p * L.ws : w_empty;
-        const int wr = L.pairs ? 2 * L.ws : L.ws;                 // ring slots seen by this pipeline
-        int lit = 0, lwit = 0;                 // pipeline-local stage / weight-stage counters
-        for (int tl = p, lt = 0; tl < my_tiles; tl += 2, lt++) {
-            const int accs = lt & 1;           // accumulator stage within the pipeline
-            const int acc = p + 2 * accs;
-            mbar_wait(smem_u32(&acc_empty[acc]), (uint32_t)(((lt >> 1) & 1) ^ 1));
-            tc_fence_after();
-            const uint32_t dcol = tmem_base + (uint32_t)(acc * L.accw);
-            for (int kb = 0; kb < nkb; kb++, lit++) {
-                const int as = lit % L.na;
-                mbar_wait(smem_u32(&a_full[p * TC_MAX_ASTAGES + as]), (uint32_t)((lit / L.na) & 1));
-                tc_fence_after();
-                if (p == 0 && lane == 0 && kb == 0) TC_TRACE(a, lt, 3);
-                if (p == 0 && lane == 0 && lit < 7) TC_TRACE(a, 40 + lit, 4);
-                const uint32_t aimg = smem_u32(Ap + (size_t)as * a_buf) >> 4;
-                for (int t = 0; t < a.ntaps; t++) {
-                    int ws;
-                    // a streamed cat image holds a PAIR of taps: it is awaited at the even tap and released after the odd
-                    // (or last) one
-                    const bool pair_done = !L.cat || (t & 1) || t == a.ntaps - 1;
-                    if (L.resident) {
-                        ws = L.cat ? kb * npairs + (t >> 1) : kb * a.ntaps + t;
-                        if (lt == 0) { mbar_wait(smem_u32(&wf[ws]), 0); tc_fence_after(); }   // loaded once, stays
-                    } else {
-                        ws = lwit % wr;
-                        if (!L.cat || !(t & 1)) {
-                            mbar_wait(smem_u32(&wf[ws]), (uint32_t)((lwit / wr) & 1));
-                            tc_fence_after();
-                        }
-                    }
-                    const uint32_t wimg = (smem_u32(Wp + (size_t)ws * w_stage) >> 4) + (L.cat ? (uint32_t)(t & 1) * 4u : 0u);
-                    const uint32_t arow = aimg + (uint32_t)(a.tap_off[t] - a.min_off) * 8u;      // rows * 128 B >> 4
-                    if (L.cat) {
-                        if (elect_one()) {
+    issue_w(0, 0);                                      // weights are constants: fetched before the predecessor finishes
+    pdl_wait();
+    issue_a(0, 0);
+
+    const int wg = warp >> 2, g = lane >> 2, c = lane & 3;
+    const int r0 = wg * 64 + (warp & 3) * 16 + g;       // tile rows r0 and r0 + 8 of this thread
+    float acc[NT / 2];
 #pragma unroll
-                            for (int ks = 0; ks < 2; ks++) {
-                                const uint64_t dah = desc_hi | (uint64_t)(arow + ks * 2);
-                                const uint64_t dal = desc_hi | (uint64_t)(arow + 4 + ks * 2);
-                                const uint64_t dw = desc_hi | (uint64_t)(wimg + ks * 2);
-                                tc_mma_bf16(dcol, dah, dw, L.idesc2, (kb | t | ks) ? 1u : 0u);   // [hi*hi | hi*lo]
-                                tc_mma_bf16(dcol, dal, dw, L.idesc, 1u);                          // lo*hi -> first nt columns
-                            }
-                            if (!L.resident && pair_done) tc_commit(smem_u32(&we[ws]));
-                        }
-                    } else if (elect_one()) {
-#pragma unroll
-                        for (int ks = 0; ks < 2; ks++) {                 // two K = 16 steps inside the 64-B hi half
-                            const uint64_t dah = desc_hi | (uint64_t)(arow + ks * 2);
-                            const uint64_t dal = desc_hi | (uint64_t)(arow + 4 + ks * 2);   // lo half starts at byte 64
-                            const uint64_t dwh = desc_hi | (uint64_t)(wimg + ks * 2);
-                            const uint64_t dwl = desc_hi | (uint64_t)(wimg + 4 + ks * 2);
-                            tc_mma_bf16(dcol, dah, dwh, L.idesc, (kb | t | ks) ? 1u : 0u);
-                            tc_mma_bf16(dcol, dal, dwh, L.idesc, 1u);
-                            tc_mma_bf16(dcol, dah, dwl, L.idesc, 1u);
-                        }
-                        if (!L.resident) tc_commit(smem_u32(&we[ws]));   // slot reusable once these MMAs retire
-                    }
-                    __syncwarp();
-                    if (pair_done) lwit++;
-                }
-                if (elect_one()) tc_commit(smem_u32(&a_empty[p * TC_MAX_ASTAGES + as]));
-                __syncwarp();
-                if (p == 0 && lane == 0 && lit < 7) TC_TRACE(a, 40 + lit, 5);
-            }
-            if (elect_one()) tc_commit(smem_u32(&acc_full[acc]));
-            __syncwarp();
-            if (p == 0 && lane == 0) TC_TRACE(a, lt, 4);
-        }
-    } else if (warp < 4) {
-        // ===================== weight producer of pipeline p = warp - 2 =====================
-        const int p = warp - 2;
-        // a stage is one image, or the `nt`-row part of an image that is `wnt` rows tall (see TcLaunch::wnt)
-        const size_t w_image = (size_t)L.wnt * (L.cat ? 256u : 128u);
-        const int nstream = L.cat ? wper : per_tile;             // streamed stages per tile
-        auto w_image0 = [&](int n_tile) {
-            const int vf = L.wnt / L.nt;
-            return reinterpret_cast<const uint8_t*>(a.wtc) + (size_t)(n_tile / vf) * nstream * w_image + (size_t)(n_tile % vf) * w_stage;
-        };
-        {
-        if (lane == 0) {
-            if (L.resident) {
-                if (p == 0) {
-                    const uint8_t* wsrc = reinterpret_cast<const uint8_t*>(a.wtc);
-                    for (int s = 0; s < wper; s++) {
-                        mbar_expect_tx(smem_u32(&w_full[s]), w_stage);
-                        bulk_g2s(smem_u32(W0 + (size_t)s * w_stage), wsrc + (size_t)s * w_stage, w_stage, smem_u32(&w_full[s]));
-                    }
-                }
-            } else if (L.pairs) {
-                if (p == 0) {                                   // one stream feeds both pipelines (w_empty counts two commits)
-                    const int wr = 2 * L.ws;
-                    int lwit = 0;
-                    for (int tl = 0; tl < my_tiles; tl += 2) {
-                        const uint8_t* wsrc = w_image0(tile_n(tl));
-                        for (int i = 0; i < nstream; i++, lwit++) {
-                            const int ws = lwit % wr;
-                            mbar_wait(smem_u32(&w_empty[ws]), (uint32_t)(((lwit / wr) & 1) ^ 1));
-                            mbar_expect_tx(smem_u32(&w_full[ws]), w_stage);
-                            bulk_g2s(smem_u32(W0 + (size_t)ws * w_stage), wsrc + (size_t)i * w_image, w_stage, smem_u32(&w_full[ws]));
-                        }
-                    }
-                }
-            } else {
-                uint8_t* Wp = W0 + (size_t)p * L.ws * w_stage;
-                uint64_t* wf = w_full + p * L.ws;
-                uint64_t* we = w_empty + p * L.ws;
-                int lwit = 0;
-                for (int tl = p; tl < my_tiles; tl += 2) {
-                    const uint8_t* wsrc = w_image0(tile_n(tl));
-                    for (int i = 0; i < nstream; i++, lwit++) {
-                        const int ws = lwit % L.ws;
-                        mbar_wait(smem_u32(&we[ws]), (uint32_t)(((lwit / L.ws) & 1) ^ 1));
-                        mbar_expect_tx(smem_u32(&wf[ws]), w_stage);
-                        bulk_g2s(smem_u32(Wp + (size_t)ws * w_stage), wsrc + (size_t)i * w_image, w_stage, smem_u32(&wf[ws]));
-                    }
-                }
-            }
-        }
-        if (MODE == 2 && L.resident) {
-            // ---- TMA agent of pipeline p (the weight warps are idle once the resident weights are in): stores the
-            // staged output chunk, waits until the engine has read it, then fetches the residual / previous-value
-            // chunk of the pipeline's next item into the same staging buffers.  The epilogue threads never wait for
-            // a store and never touch global memory.
-            if (lane == 0) {
-                pdl_wait();                                                           // residual / previous tiles: predecessor data
-                const int nitems = ((my_tiles - p + 1) / 2) * nch;
-                if (nitems) agent_fetch(p, 0);
-                for (int it = 0; it < nitems; it++) {
-                    mbar_wait(smem_u32(&staged[p]), (uint32_t)(it & 1));
-                    agent_store(p, it);
-                    if (it + 1 < nitems) agent_fetch(p, it + 1);
-                }
-                asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");   // stores complete before the CTA retires
-            }
-        }
-        }
-        __syncwarp();
-    } else if (warp < TC_EPI0) {
-        // ===================== activation producers: group p feeds pipeline p =====================
-        // Raw fp32 rows (32 ch = 128 B) are cp.async'ed (LDGSTS, zero-fill outside the array) straight into the
-        // ring, na-1 stages ahead, and converted IN PLACE to the [hi|lo] bf16 image of the same 128 bytes: the
-        // four lanes that share a row read their 32-B pieces, __syncwarp(), then overwrite the row.
-        const int p = (warp - TC_PROD0) >> 2;
-        const int gt = tid - TC_PROD0 * 32 - p * TC_GROUP;
-        const int npiece = L.win * 4;                  // 32-B pieces (8 channels) per stage
-        const float slope = a.in_slope;
-        uint8_t* Ap = A0 + (size_t)p * L.na * a_buf;
-        const int nloc = (my_tiles - p + 1) / 2;       // tiles owned by this pipeline
-        const int nst = nloc * nkb;                    // stages to produce
-        const int depth = L.depth;                     // stages in flight
-        auto issue_stage = [&](int j) {
-            const int lt = j / nkb, kb = j - lt * nkb;
-            const int rbase = tile_m(p + 2 * lt) * 128 + a.min_off;
-            const int as = j % L.na;
-            if (p == 0 && gt == 0 && j < 7) TC_TRACE(a, 40 + j, 3);       // rows 40..46: stage j of the first tile(s)
-            mbar_wait(smem_u32(&a_empty[p * TC_MAX_ASTAGES + as]), (uint32_t)(((j / L.na) & 1) ^ 1));
-            if (p == 0 && gt == 0 && kb == 0) TC_TRACE(a, lt, 0);
-            if (p == 0 && gt == 0 && j < 7) TC_TRACE(a, 40 + j, 0);
-            const uint32_t img = smem_u32(Ap + (size_t)as * a_buf);
-            const float* xk = a.x + kb * 32;
-            if (L.tma_in) {
-                if (gt == 0) {
-                    mbar_expect_tx(smem_u32(&raw_full[p * TC_MAX_ASTAGES + as]), a_buf);
-                    tma_load_2d(img, &tm_x, smem_u32(&raw_full[p * TC_MAX_ASTAGES + as]), kb * 32, rbase);
-                }
-            } else if (L.bulk_in && rbase >= 0 && rbase + L.win <= a.rows_in) {
-                // contiguous 32-channel rows: the whole window is one block -> one TMA bulk copy (keeps the window
-                // traffic out of the LSU / L1 miss queue; measured +1.4 %)
-                if (gt == 0) {
-                    mbar_expect_tx(smem_u32(&raw_full[p * TC_MAX_ASTAGES + as]), a_buf);
-                    bulk_g2s(img, xk + (size_t)rbase * 32, a_buf, smem_u32(&raw_full[p * TC_MAX_ASTAGES + as]));
-                }
-            } else
-#pragma unroll
-            for (int u = 0; u < TC_MAXCH; u++) {
-                const int idx = gt + u * TC_GROUP;
-                if (idx < npiece) {
-                    const int gr = rbase + (idx >> 2);
-                    const bool ok = gr >= 0 && gr < a.rows_in;
-                    const float* src = ok ? xk + (size_t)gr * a.ldx + (idx & 3) * 8 : a.x;
-                    const uint32_t dst = img + (uint32_t)idx * 32u;
-                    const uint32_t nbytes = ok ? 16u : 0u;
-                    asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(dst), "l"(src), "r"(nbytes) : "memory");
-                    asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(dst + 16u), "l"(src + 4), "r"(nbytes) : "memory");
-                }
-            }
-            asm volatile("cp.async.commit_group;" ::: "memory");
-        };
-        int ji = 0;
-        uint32_t rawpar = 0;                           // per-stage phase parity of raw_full (bulk-loaded stages only)
-        for (; ji < depth && ji < nst; ji++) issue_stage(ji);
-        for (int j = 0; j < nst; j++) {
-            const int pending = ji - 1 - j;            // younger groups allowed to stay in flight
-            if (pending >= 3) asm volatile("cp.async.wait_group 3;" ::: "memory");
-            else if (pending == 2) asm volatile("cp.async.wait_group 2;" ::: "memory");
-            else if (pending == 1) asm volatile("cp.async.wait_group 1;" ::: "memory");
-            else asm volatile("cp.async.wait_group 0;" ::: "memory");
-            {
-                const int lt_ = j / nkb;
-                const int rb_ = tile_m(p + 2 * lt_) * 128 + a.min_off;
-                if (L.tma_in || (L.bulk_in && rb_ >= 0 && rb_ + L.win <= a.rows_in)) {
-                    const int as_ = j % L.na;
-                    mbar_wait(smem_u32(&raw_full[p * TC_MAX_ASTAGES + as_]), (rawpar >> as_) & 1u);
-                    rawpar ^= 1u << as_;
-                }
-            }
-            __syncwarp();
-            if (p == 0 && gt == 0 && (j % nkb) == 0) TC_TRACE(a, j / nkb, 1);
-            if (p == 0 && gt == 0 && j < 7) TC_TRACE(a, 40 + j, 1);
-            const int as = j % L.na;
-            const uint32_t img = smem_u32(Ap + (size_t)as * a_buf);   // explicit ld/st.shared (the manual 1024-B
-                                                                       // alignment hides the address space from nvcc)
-#pragma unroll
-            for (int u = 0; u < TC_MAXCH; u++) {
-                const int idx = gt + u * TC_GROUP;
-                const bool live = idx < npiece;        // warp-uniform per u except in the last partial warp
-                // Bank-conflict-free order: the 8 lanes of a quarter-warp cover two rows; odd rows take their two
-                // 16-byte chunks in the opposite order, so the 8 accesses of one instruction hit 8 different bank
-                // groups (shared-memory bandwidth, shared with the tensor core's operand fetch, bounds these layers).
-                const uint32_t odd = (uint32_t)(idx >> 2) & 1u;
-                float4 v0 = make_float4(0.f, 0.f, 0.f, 0.f), v1 = v0;
-                if (live) {
-                    const float4 t0 = lds128(img + (uint32_t)idx * 32u + odd * 16u);
-                    const float4 t1 = lds128(img + (uint32_t)idx * 32u + 16u - odd * 16u);
-                    v0 = odd ? t1 : t0;
-                    v1 = odd ? t0 : t1;
-                }
-                __syncwarp();                          // every lane of the row has read before anyone overwrites
-                if (live) {
-                    const int r = idx >> 2, c = idx & 3;
-                    float e[8] = {v0.x, v0.y, v0.z, v0.w, v1.x, v1.y, v1.z, v1.w};
-                    if (slope != 1.f) {
-#pragma unroll
-                        for (int i = 0; i < 8; i++) e[i] = fmaxf(e[i], e[i] * slope);   // leaky ReLU, 0 < slope < 1
-                    }
-                    uint4 hi, lo;
-                    hi.x = split2(e[0], e[1], lo.x);
-                    hi.y = split2(e[2], e[3], lo.y);
-                    hi.z = split2(e[4], e[5], lo.z);
-                    hi.w = split2(e[6], e[7], lo.w);
-                    const uint32_t rowb = (uint32_t)r * 128u;
-                    const uint32_t sw = (uint32_t)(r & 7);
-                    const uint4 first = odd ? lo : hi, second = odd ? hi : lo;      // same trick for the two stores
-                    sts128u(img + rowb + (((uint32_t)(c + 4 * odd) ^ sw) << 4), first);
-                    sts128u(img + rowb + (((uint32_t)(c + 4 - 4 * odd) ^ sw) << 4), second);
-                }
-            }
-            fence_async_smem();                       // generic-proxy stores -> visible to the tensor core
-            mbar_arrive(smem_u32(&a_full[p * TC_MAX_ASTAGES + as]));
-            if (p == 0 && gt == 0 && (j % nkb) == nkb - 1) TC_TRACE(a, j / nkb, 2);
-            if (p == 0 && gt == 0 && j < 7) TC_TRACE(a, 40 + j, 2);
-            if (ji < nst) { issue_stage(ji); ji++; }
-        }
-    } else {
-        // ===================== epilogue: warps 12-15 serve pipeline 0, warps 16-19 pipeline 1 =====================
-        // (one TMEM lane quadrant per warp).  The residual and the read-modify-write operand of chunk 0 are
-        // folded into one addend  m = res*scale + prev  and prefetched BEFORE the accumulator is awaited.
-        const int p = (warp - TC_EPI0) >> 2;
-        const int quad = warp & 3;
-        const int row = quad * 32 + lane;
-        if constexpr (MODE == 2) {
-            // ---- 32-channel output, row-per-thread math, but every global operand of the epilogue moves through the
-            // TMA engine: the residual and previous-value tiles arrive in SWIZZLE_128B staging tiles (16-byte chunk
-            // c of row r at c ^ (r & 7): conflict-free 128-bit accesses for a row-per-thread owner), the result is
-            // written over the residual tile in place and leaves with one tensor store issued by the agent warp.
-            // A row-per-thread LDG/STG touches 32 different lines per instruction (one L1TEX data-pipe wavefront
-            // per thread); ncu showed that pipe 83 % busy, two thirds of it global wavefronts, while HBM and L2
-            // sat at 40 %.
-            const uint32_t st = smem_u32(EX + (size_t)p * L.nstg * TC_OUT_BYTES) + (uint32_t)row * 128u;
-            const uint32_t sw = (uint32_t)(row & 7);
-            int it = 0;
-            // streamed weights keep warps 2 / 3 busy: the epilogue group is its own TMA agent (thread 0 stores the chunk
-            // once the group's 128 threads have staged it, and fetches the next operands into the same buffers)
-            const bool self = !L.resident;
-            const int nitems = ((my_tiles - p + 1) / 2) * nch;
-            if (self && row == 0 && nitems) agent_fetch(p, 0);
-            for (int tl = p, lt = 0; tl < my_tiles; tl += 2, lt++) {
-                const int q = tile_m(tl) * 128 + row;
-                const int acc = p + 2 * (lt & 1);
-                const bool valid = q < a.rows_q && row_valid(a.map, q);
-                mbar_wait(smem_u32(&acc_full[acc]), (uint32_t)((lt >> 1) & 1));
-                tc_fence_after();
-                if (p == 0 && warp == TC_EPI0 && lane == 0) TC_TRACE(a, lt, 5);
-                for (int ch = 0; ch < nch; ch++, it++) {
-                    float o[32];
-                    tmem_ld32(tmem_base + ((uint32_t)(quad * 32) << 16) + (uint32_t)(acc * L.accw + ch * 32), o);
-                    if (L.cat) {                  // second column half: the hi*lo products
-                        float t[32];
-                        tmem_ld32(tmem_base + ((uint32_t)(quad * 32) << 16) + (uint32_t)(acc * L.accw + L.nt + ch * 32), t);
-#pragma unroll
-                        for (int j = 0; j < 32; j++) o[j] += t[j];
-                    }
-                    if (ch == nch - 1) {          // accumulator fully read: hand it back to its MMA warp
-                        tc_fence_before();
-                        mbar_arrive(smem_u32(&acc_empty[acc]));
-                        if (p == 0 && warp == TC_EPI0 && lane == 0) TC_TRACE(a, lt, 6);
-                    }
-                    if (a.bias) {
-#pragma unroll
-                        for (int j = 0; j < 32; j += 4) {
-                            const float4 b = *reinterpret_cast<const float4*>(a.bias + ch * 32 + j);
-                            o[j] += b.x; o[j + 1] += b.y; o[j + 2] += b.z; o[j + 3] += b.w;
-                        }
-                    }
-                    if (a.act == ACT_RELU) {
-#pragma unroll
-                        for (int j = 0; j < 32; j++) o[j] = fmaxf(o[j], 0.f);
-                    }
-                    mbar_wait(smem_u32(&epi_full[p]), (uint32_t)(it & 1));     // operands landed AND staging tile free
-                    // gap rows are written as zeros (accumulated buffers hold zeros there already); rows past the end of
-                    // the array are clipped by the tensor map
-#pragma unroll
-                    for (int c = 0; c < 8; c++) {
-                        const uint32_t off = (((uint32_t)c ^ sw) << 4);
-                        float4 r = make_float4(0.f, 0.f, 0.f, 0.f), pv = r;
-                        if (a.res) r = lds128(st + off);
-                        if (a.acc0) pv = lds128(st + TC_OUT_BYTES + off);
-                        uint4 u;
-                        u.x = __float_as_uint(valid ? fmaf(o[4 * c] + r.x, a.scale, pv.x) : 0.f);
-                        u.y = __float_as_uint(valid ? fmaf(o[4 * c + 1] + r.y, a.scale, pv.y) : 0.f);
-                        u.z = __float_as_uint(valid ? fmaf(o[4 * c + 2] + r.z, a.scale, pv.z) : 0.f);
-                        u.w = __float_as_uint(valid ? fmaf(o[4 * c + 3] + r.w, a.scale, pv.w) : 0.f);
-                        sts128u(st + off, u);
-                    }
-                    fence_async_smem();                                  // generic-proxy stores -> visible to the TMA engine
-                    if (self) {
-                        asm volatile("bar.sync %0, 128;" ::"r"(1 + p) : "memory");
-                        if (row == 0) {
-                            agent_store(p, it);
-                            if (it + 1 < nitems) agent_fetch(p, it + 1);
-                        }
-                    } else mbar_arrive(smem_u32(&staged[p]));
-                }
-                if (p == 0 && warp == TC_EPI0 && lane == 0) TC_TRACE(a, lt, 7);
-            }
-            if (self && row == 0) asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");   // stores complete before the CTA retires
+    for (int i = 0; i < NT / 2; i++) acc[i] = 0.f;
+
+    for (int kb = 0; kb < nkb; kb++) {
+        const int s = kb & 1;
+        if (kb + 1 < nkb) {                             // stage s ^ 1 was released at the end of the previous K-block
+            issue_w(kb + 1, s ^ 1);
+            issue_a(kb + 1, s ^ 1);
+            cp_async_wait<1>();
         } else {
-        const bool gate = a.act == ACT_GATE;
-        for (int tl = p, lt = 0; tl < my_tiles; tl += 2, lt++) {
-            const int q = tile_m(tl) * 128 + row;
-            const int n0 = tile_n(tl) * L.nt;
-            const int acc = p + 2 * (lt & 1);
-            const bool inrange = q < a.rows_q;
-            const bool valid = inrange && row_valid(a.map, q);
-            const size_t orow0 = (size_t)q * a.orow_mul + a.orow_add;
-            float m[32];
-            // phase-fused ConvTranspose (phase_cols > 0): column block n / phase_cols is the output phase,
-            // i.e. output row q*u + phase and column n % phase_cols
-            auto prefetch = [&](int ch) {
-                int n = n0 + ch * 32;
-                const bool live = valid && n < a.cout && !gate;
-                size_t orow = orow0;
-                if (a.phase_cols) { orow += (size_t)(n / a.phase_cols); n %= a.phase_cols; }
-                const bool lo_side = n < a.split;
-                const bool accum = lo_side ? a.acc0 : a.acc1;
+            cp_async_wait<0>();
+        }
+        __syncthreads();
+        // in-place conversion, 32-byte pieces (8 channels); the four lanes of a row sit in one warp: all read, then write.
+        // Odd rows take their two 16-byte chunks in the opposite order (bank-conflict-free quarter-warps).
+        const uint32_t img = A0 + s * a_buf;
+        const int npiece = L.win * 4;
+        const float slope = a.in_slope;
+        for (int base = 0; base < npiece; base += TC_THREADS) {
+            const int idx = base + tid;
+            const bool live = idx < npiece;
+            const uint32_t odd = (uint32_t)(idx >> 2) & 1u;
+            float4 v0 = make_float4(0.f, 0.f, 0.f, 0.f), v1 = v0;
+            if (live) {
+                const float4 t0 = lds128(img + (uint32_t)idx * 32u + odd * 16u);
+                const float4 t1 = lds128(img + (uint32_t)idx * 32u + 16u - odd * 16u);
+                v0 = odd ? t1 : t0;
+                v1 = odd ? t0 : t1;
+            }
+            __syncwarp();
+            if (live) {
+                const int r = idx >> 2, cc = idx & 3;
+                float e[8] = {v0.x, v0.y, v0.z, v0.w, v1.x, v1.y, v1.z, v1.w};
+                if (slope != 1.f) {
 #pragma unroll
-                for (int j = 0; j < 32; j++) m[j] = 0.f;
-                if (a.res && live) {
-                    const float* src = a.res + orow * a.ldres + n;
-#pragma unroll
-                    for (int j = 0; j < 32; j += 8) {
-                        float r[8];
-                        if (L.v8) ldg256(src + j, r);
-                        else {
-                            const float4 r0 = *reinterpret_cast<const float4*>(src + j), r1 = *reinterpret_cast<const float4*>(src + j + 4);
-                            r[0] = r0.x; r[1] = r0.y; r[2] = r0.z; r[3] = r0.w; r[4] = r1.x; r[5] = r1.y; r[6] = r1.z; r[7] = r1.w;
-                        }
-#pragma unroll
-                        for (int e = 0; e < 8; e++) m[j + e] = r[e] * a.scale;
-                    }
+                    for (int i = 0; i < 8; i++) e[i] = fmaxf(e[i], e[i] * slope);   // leaky ReLU, 0 < slope < 1
                 }
-                if (accum && live) {
-                    const float* src = lo_side ? a.y0 + orow * a.ldy0 + n : a.y1 + orow * a.ldy1 + (n - a.split);
+                uint4 hi, lo;
+                hi.x = split2(e[0], e[1], lo.x);
+                hi.y = split2(e[2], e[3], lo.y);
+                hi.z = split2(e[4], e[5], lo.z);
+                hi.w = split2(e[6], e[7], lo.w);
+                const uint4 first = odd ? lo : hi, second = odd ? hi : lo;
+                sts128u(sw128(img, r, cc + 4 * (int)odd), first);
+                sts128u(sw128(img, r, cc + 4 - 4 * (int)odd), second);
+            }
+        }
+        __syncthreads();
+        mbar_wait(smem_u32(&bars[s]), (uint32_t)((kb >> 1) & 1));
+        const uint32_t wst = W0 + s * w_buf;
+        for (int t = 0; t < a.ntaps; t++) {
+            const int R0 = r0 + a.tap_off[t] - a.min_off, R1 = R0 + 8;
+            uint32_t ah[2][4], al[2][4];
 #pragma unroll
-                    for (int j = 0; j < 32; j += 8) {
-                        float r[8];
-                        if (L.v8) ldg256(src + j, r);
-                        else {
-                            const float4 r0 = *reinterpret_cast<const float4*>(src + j), r1 = *reinterpret_cast<const float4*>(src + j + 4);
-                            r[0] = r0.x; r[1] = r0.y; r[2] = r0.z; r[3] = r0.w; r[4] = r1.x; r[5] = r1.y; r[6] = r1.z; r[7] = r1.w;
-                        }
+            for (int ks = 0; ks < 2; ks++) {
+                ah[ks][0] = lds32(sw128(img, R0, 2 * ks) + 4u * c);
+                ah[ks][1] = lds32(sw128(img, R1, 2 * ks) + 4u * c);
+                ah[ks][2] = lds32(sw128(img, R0, 2 * ks + 1) + 4u * c);
+                ah[ks][3] = lds32(sw128(img, R1, 2 * ks + 1) + 4u * c);
+                al[ks][0] = lds32(sw128(img, R0, 4 + 2 * ks) + 4u * c);
+                al[ks][1] = lds32(sw128(img, R1, 4 + 2 * ks) + 4u * c);
+                al[ks][2] = lds32(sw128(img, R0, 5 + 2 * ks) + 4u * c);
+                al[ks][3] = lds32(sw128(img, R1, 5 + 2 * ks) + 4u * c);
+            }
+            const uint32_t wimg = wst + t * w_tap;
+            acc_fence<NT / 2>(acc);
+            wg_fence();
 #pragma unroll
-                        for (int e = 0; e < 8; e++) m[j + e] += r[e];
-                    }
-                }
-            };
-            prefetch(0);
-            mbar_wait(smem_u32(&acc_full[acc]), (uint32_t)((lt >> 1) & 1));
-            tc_fence_after();
-            if (p == 0 && warp == TC_EPI0 && lane == 0) TC_TRACE(a, lt, 5);
-            for (int ch = 0; ch < nch; ch++) {
-                float o[32];
-                tmem_ld32(tmem_base + ((uint32_t)(quad * 32) << 16) + (uint32_t)(acc * L.accw + ch * 32), o);   // (cat mode: MODE 2 only)
-                if (ch == nch - 1) {          // accumulator fully read: hand it back to its MMA warp
-                    tc_fence_before();
-                    mbar_arrive(smem_u32(&acc_empty[acc]));
-                    if (p == 0 && warp == TC_EPI0 && lane == 0) TC_TRACE(a, lt, 6);
-                }
-                int n = n0 + ch * 32;
-                if (ch > 0) prefetch(ch);
-                if (!inrange || n >= a.cout) continue;
-                const int nb = n;                       // bias / weight column
+            for (int ks = 0; ks < 2; ks++) {                // two K = 16 steps inside the 64-byte hi half
+                const uint64_t dwh = sw128_desc(wimg + 32u * ks);
+                const uint64_t dwl = sw128_desc(wimg + 64u + 32u * ks);   // lo half starts at byte 64
+                wgmma_rs<WG_BF16, NT>(acc, ah[ks], dwh);
+                wgmma_rs<WG_BF16, NT>(acc, al[ks], dwh);
+                wgmma_rs<WG_BF16, NT>(acc, ah[ks], dwl);
+            }
+            wg_commit();
+            wg_wait0();
+            acc_fence<NT / 2>(acc);
+        }
+        __syncthreads();                                // stage s fully read: the next iteration refills it
+    }
+
+    // ===================== epilogue: thread owns rows r0, r0 + 8 and column pairs 8j + 2c =====================
+    const int n0 = n_tile * NT;
+    const bool gate = a.act == ACT_GATE;
+#pragma unroll
+    for (int h = 0; h < 2; h++) {
+        const int q = m_tile * 128 + r0 + 8 * h;
+        if (q >= a.rows_q) continue;
+        const bool valid = row_valid(a.map, q);
+        const size_t orow0 = (size_t)q * a.orow_mul + a.orow_add;
+#pragma unroll
+        for (int j = 0; j < NT / 8; j++) {
+            const int nb = n0 + 8 * j + 2 * c;          // bias / weight column of the pair's first element
+            if (nb >= a.cout) continue;
+            float o[2] = {acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1]};
+            if (a.bias) { o[0] += a.bias[nb]; o[1] += a.bias[nb + 1]; }
+            if (gate) {
+                // phase-fused ConvTranspose never gates: the pair (2k, 2k+1) gives output column k
+                a.y0[orow0 * a.ldy0 + (nb >> 1)] = valid ? tanhf(o[0]) * (1.f / (1.f + expf(-o[1]))) * a.scale : 0.f;
+                continue;
+            }
+            if (a.act == ACT_RELU) { o[0] = fmaxf(o[0], 0.f); o[1] = fmaxf(o[1], 0.f); }
+#pragma unroll
+            for (int e = 0; e < 2; e++) {
+                // phase-fused ConvTranspose (phase_cols > 0): column block n / phase_cols is the output phase, i.e. output
+                // row q*u + phase and column n % phase_cols
+                int n = nb + e;
                 size_t orow = orow0;
                 if (a.phase_cols) { orow += (size_t)(n / a.phase_cols); n %= a.phase_cols; }
                 const bool lo_side = n < a.split;
                 const int accum = lo_side ? a.acc0 : a.acc1;
-                if (a.bias) {
-#pragma unroll
-                    for (int j = 0; j < 32; j += 4) {
-                        const float4 b = *reinterpret_cast<const float4*>(a.bias + nb + j);
-                        o[j] += b.x; o[j + 1] += b.y; o[j + 2] += b.z; o[j + 3] += b.w;
-                    }
-                }
-                if (gate) {
-                    float* dst = a.y0 + orow * a.ldy0 + (n >> 1);
-#pragma unroll
-                    for (int j = 0; j < 16; j += 8) {
-                        float g[8];
-#pragma unroll
-                        for (int e = 0; e < 8; e++)
-                            g[e] = valid ? tanhf(o[2 * (j + e)]) * (1.f / (1.f + expf(-o[2 * (j + e) + 1]))) * a.scale : 0.f;
-                        if (L.v8) stg256(dst + j, g);
-                        else {
-                            *reinterpret_cast<float4*>(dst + j) = make_float4(g[0], g[1], g[2], g[3]);
-                            *reinterpret_cast<float4*>(dst + j + 4) = make_float4(g[4], g[5], g[6], g[7]);
-                        }
-                    }
-                    continue;
-                }
-                if (a.act == ACT_RELU) {
-#pragma unroll
-                    for (int j = 0; j < 32; j++) o[j] = fmaxf(o[j], 0.f);
-                }
-                if (accum && !valid) continue;     // accumulated buffers keep their zeros in gap rows
-#pragma unroll
-                for (int j = 0; j < 32; j++) o[j] = valid ? fmaf(o[j], a.scale, m[j]) : 0.f;
+                if (accum && !valid) continue;          // accumulated buffers keep their zeros in gap rows
+                float m = 0.f;
+                if (a.res && valid) m = a.res[orow * a.ldres + n] * a.scale;
                 float* dst = lo_side ? a.y0 + orow * a.ldy0 + n : a.y1 + orow * a.ldy1 + (n - a.split);
-#pragma unroll
-                for (int j = 0; j < 32; j += 8) {
-                    if (L.v8) stg256(dst + j, o + j);
-                    else {
-                        *reinterpret_cast<float4*>(dst + j) = make_float4(o[j], o[j + 1], o[j + 2], o[j + 3]);
-                        *reinterpret_cast<float4*>(dst + j + 4) = make_float4(o[j + 4], o[j + 5], o[j + 6], o[j + 7]);
-                    }
-                }
+                if (accum && valid) m += *dst;
+                *dst = valid ? fmaf(o[e], a.scale, m) : 0.f;
             }
-            if (p == 0 && warp == TC_EPI0 && lane == 0) TC_TRACE(a, lt, 7);
-        }
         }
     }
-    tc_fence_before();
-    __syncthreads();
-    if (threadIdx.x == 0) TC_TRACE(a, 47, 3);
-    if (warp == 0) {
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"((uint32_t)L.tmem_cols)
-                     : "memory");
-    }
 }
 
-// [rows][cols] fp32 view of an output buffer: 128-row x 32-column boxes, SWIZZLE_128B in shared memory
-bool make_out_map(CUtensorMap* tm, float* base, int cols, int rows, int ld) {
-    return tensor_map_2d(tm, base, (unsigned long long)cols, (unsigned long long)rows, (unsigned long long)ld, 32, 128, true);
+size_t smem_bytes(const ConvArgs& a, int nt, int win) {
+    return (size_t)TC_STAGES * ((size_t)win * 128 + (size_t)a.ntaps * nt * 128) + TC_STAGES * 8;
 }
 
-// [rows][cin] fp32 view of a conv input: boxes of 32 channels x win rows, linear (unswizzled) in shared memory --
-// exactly the raw window image the producers convert in place
-bool make_in_map(CUtensorMap* tm, const float* base, int rows, int cin, int ld, int win) {
-    return tensor_map_2d(tm, base, (unsigned long long)cin, (unsigned long long)rows, (unsigned long long)ld, 32, (unsigned)win, false);
-}
-
-// 256-bit epilogue accesses need 32-byte aligned rows and column blocks for every operand that is used
-bool epi_v8_ok(const ConvArgs& a) {
-    if (SB_ENV_ONCE("SB200_TC_NOV8")) return false;
-    auto al = [](const void* p, int ld) { return p == nullptr || ((reinterpret_cast<uintptr_t>(p) & 31) == 0 && (ld & 7) == 0); };
-    const int half = a.act == ACT_GATE ? 2 : 1;       // the gate halves the column index
-    if (a.split % (8 * half) != 0 && a.split < a.cout) return false;
-    if (a.phase_cols && (a.phase_cols & 7)) return false;
-    return al(a.res, a.ldres) && al(a.y0, a.ldy0) && al(a.y1, a.ldy1);
-}
-
-bool plan(const ConvArgs& a, TcLaunch& L, size_t& smem, bool allow_tma_st = true) {
-    if (!a.wtc || a.tc_nt <= 0 || a.tc_nt > 128) return false;
-    L.nt = L.wnt = a.tc_nt;
-    L.v8 = epi_v8_ok(a) ? 1 : 0;
-    // TMA-staged epilogue: one output buffer, plain row mapping, whole 32-column chunks (32 / 64 / 128 output channels in
-    // ONE column tile).  SB200_TC_TMAST_MAXC caps the channel count (A/B against the row-per-thread epilogue).
-    int tmast_maxc = 64;
-    { const char* e = SB_ENV_ONCE("SB200_TC_TMAST_MAXC"); if (e) tmast_maxc = atoi(e); }
-    L.tma_st = (allow_tma_st && L.v8 && (a.cout == 32 || a.cout == 64 || a.cout == 128) && a.cout <= tmast_maxc && L.nt == a.cout &&
-                a.act != ACT_GATE && !a.phase_cols && a.split >= a.cout && a.orow_mul == 1 && have_tensor_maps() &&
-                !SB_ENV_ONCE("SB200_TC_NOTMAST")) ? 1 : 0;
-    if (a.res && (a.ldres & 3)) L.tma_st = 0;
-    L.nstg = a.acc0 ? 2 : 1;
-    // Small launches (a single utterance): a 128-column tile costs 160 cycles per MMA from its one issuing warp and a
-    // 128-column epilogue, ~25 us for a k5 layer, while most SMs idle: take the narrowest part of an image (a multiple of
-    // 32 rows that divides it) that still leaves no more tiles than SMs.  Not for the layers of the TMA-staged epilogue:
-    // their arithmetic (cat mode, epilogue rounding) differs from MODE 0, and an utterance must come out bit-identical
-    // whether it is synthesised alone or in a batch (tested); tile WIDTH alone changes no summation order.
-    if (!L.tma_st && a.cout % a.tc_nt == 0 && !SB_ENV_ONCE("SB200_TC_NOHALF")) {
-        const int mt = (a.rows_q + 127) / 128;
-        for (int nt = 32; nt < a.tc_nt; nt += 32)
-            if (a.tc_nt % nt == 0 && mt * (a.cout / nt) <= tc_num_sms()) { L.nt = nt; break; }
-    }
+bool plan(const ConvArgs& a, TcLaunch& L, size_t& smem) {
+    if (!a.wtc || a.tc_nt <= 0 || a.tc_nt > 128 || a.tc_nt % 32) return false;
+    L.wnt = a.tc_nt;
     L.win = (128 + a.span + 7) & ~7;
-    if (L.win * 4 > TC_MAXCH * TC_GROUP) return false;
-    L.cat = 0; L.accw = L.nt; L.idesc2 = 0;
-    // kind::f16 instruction descriptor: D fp32 (1<<4), A = B = BF16 (1<<7, 1<<10), K-major both, N>>3, M>>4
-    L.idesc = (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(L.nt >> 3) << 17) | ((uint32_t)(128 >> 4) << 24);
-    L.ntiles_m = (a.rows_q + 127) / 128;
+    const int mt = (a.rows_q + 127) / 128;
+    // The widest part of an image whose two stages fit; on small launches (a single utterance) the narrowest part that
+    // still leaves no more tiles than SMs, so that more SMs share the work.  Tile width changes no summation order: an
+    // utterance comes out bit-identical whether it is synthesised alone or in a batch.
+    L.nt = 0;
+    for (int nt = a.tc_nt; nt >= 32; nt -= 32)
+        if (a.tc_nt % nt == 0 && smem_bytes(a, nt, L.win) <= WG_SMEM_BUDGET) { L.nt = nt; break; }
+    if (!L.nt) return false;
+    if (a.cout % a.tc_nt == 0)
+        for (int nt = 32; nt < L.nt; nt += 32)
+            if (L.nt % nt == 0 && mt * (a.cout / nt) <= wg_num_sms()) { L.nt = nt; break; }
+    L.ntiles_m = mt;
     L.ntiles_n = (a.cout + L.nt - 1) / L.nt;
-    const size_t a_buf = (size_t)L.win * 128;
-    const size_t w_stage = (size_t)L.nt * 128;
-    const int per_tile = (a.cin / 32) * a.ntaps;
-    const size_t budget = 225 * 1024 - 2048;
-    const size_t bar_bytes = (2 * TC_MAX_WRING + 6 * TC_MAX_ASTAGES + 12) * 8 + 16 + (L.tma_st ? 2 * L.nstg * TC_OUT_BYTES : 0);
-    L.bulk_in = (SB_ENV_ONCE("SB200_TC_NOBULKIN") == nullptr && a.ldx == 32 && a.cin == 32) ? 1 : 0;
-    L.tma_in = (have_tensor_maps() && L.win <= 256 && (a.ldx & 3) == 0 && (reinterpret_cast<uintptr_t>(a.x) & 15) == 0 &&
-                !SB_ENV_ONCE("SB200_TC_NOTMAIN")) ? 1 : 0;
-    L.resident = (L.ntiles_n == 1 && per_tile <= TC_MAX_WRING && per_tile * w_stage + 4 * a_buf + bar_bytes <= budget) ? 1 : 0;
-    if (L.tma_st && !L.resident && SB_ENV_ONCE("SB200_TC_TMAST_RESONLY")) return plan(a, L, smem, false);
-    // (small launches keep one tile per CTA: with fewer tiles than 2 x SMs, pairing halves the CTAs and couples two tiles to
-    //  one weight stream for nothing -- C1 flow 0.90 -> 1.00 ms)
-    L.pairs = (!L.resident && L.ntiles_m * L.ntiles_n >= 2 * tc_num_sms() && !SB_ENV_ONCE("SB200_TC_NOPAIRS")) ? 1 : 0;
-    const int wper_cat = (a.cin / 32) * ((a.ntaps + 1) / 2);
-    // cat mode: with resident weights when the (larger) cat images still fit; with streamed weights always (a stage is then
-    // a tap PAIR; SB200_TC_NOCATSTREAM keeps those layers on three MMAs per step)
-    if (a.wcat && L.tma_st && L.nt <= 64 && !SB_ENV_ONCE("SB200_TC_NOCAT") &&
-        (L.resident ? wper_cat * 2 * w_stage + 4 * a_buf + bar_bytes <= budget : !SB_ENV_ONCE("SB200_TC_NOCATSTREAM"))) {
-        L.cat = 1; L.accw = 2 * L.nt;
-        L.idesc2 = (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)((2 * L.nt) >> 3) << 17) | ((uint32_t)(128 >> 4) << 24);
-    }
-    auto total = [&]() { return (size_t)2 * L.na * a_buf + (size_t)(L.resident ? L.ws : 2 * L.ws) * w_stage * (L.cat ? 2 : 1) + bar_bytes; };
-    // ring depths for the current (resident, cat) choice; false when even the minimum does not fit
-    auto fit = [&]() {
-        L.tmem_cols = 32;
-        while (L.tmem_cols < 4 * L.accw) L.tmem_cols <<= 1;
-        const int nstream = L.cat ? wper_cat : per_tile;
-        L.ws = L.resident ? nstream : (nstream < 4 ? nstream : 4);
-        if (!L.resident && L.ws < 2) L.ws = 2;
-        L.na = TC_MAX_ASTAGES;
-        { const char* e = SB_ENV_ONCE("SB200_TC_NA"); if (e) L.na = atoi(e); }     // tuning knob
-        // (Giving the activation ring priority over a streamed weight ring -- na = 4 / ws = 2 instead of na = 2 / ws = 4 --
-        //  was measured: flow -1.5 %, 128-channel ResBlocks +3.5 %, 64-channel k = 11 layers +9 %: not adopted.)
-        while (L.na > 2 && total() > budget) L.na--;
-        while (!L.resident && L.ws > 2 && total() > budget) L.ws--;
-        return total() <= budget;
-    };
-    if (!fit()) {
-        if (!(L.cat && !L.resident)) return false;
-        L.cat = 0; L.accw = L.nt; L.idesc2 = 0;          // the doubled stages of a streamed cat ring do not fit: three MMAs per step
-        if (!fit()) return false;
-    }
-    L.depth = L.na - 1;
-    { const char* e = SB_ENV_ONCE("SB200_TC_DEPTH"); if (e && atoi(e) >= 1 && atoi(e) < L.na) L.depth = atoi(e); }
-    smem = total() + 2048;
+    smem = smem_bytes(a, L.nt, L.win) + 1024;
     return true;
+}
+
+template <int NT> void launch_nt(const ConvArgs& a, const TcLaunch& L, size_t smem, cudaStream_t st) {
+    static PerDeviceOnce once;
+    once.run([] { cudaFuncSetAttribute(conv_tc_kernel<NT>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024); });
+    launch_pdl(conv_tc_kernel<NT>, dim3(L.ntiles_m * L.ntiles_n), dim3(TC_THREADS), smem, st, a, L);
 }
 
 uint16_t bf16_rn_host(float f) {
@@ -801,45 +270,11 @@ float bf16_to_float_host(uint16_t h) {
 
 }  // namespace
 
-bool tensor_map_2d(CUtensorMap* tm, const void* base, unsigned long long cols, unsigned long long rows, unsigned long long ld,
-                   unsigned box_cols, unsigned box_rows, bool swizzle128) {
-    TensorMapEncodeFn enc = tensor_map_encoder();
-    if (!enc) return false;
-    struct Key {
-        const void* base; unsigned long long cols, rows, ld; unsigned bc, br; bool sw;
-        bool operator==(const Key& o) const { return base == o.base && cols == o.cols && rows == o.rows && ld == o.ld && bc == o.bc && br == o.br && sw == o.sw; }
-    };
-    struct Hash {
-        size_t operator()(const Key& k) const {
-            size_t h = reinterpret_cast<size_t>(k.base);
-            for (unsigned long long v : {k.cols, k.rows, k.ld, (unsigned long long)k.bc, (unsigned long long)k.br, (unsigned long long)k.sw})
-                h = (h ^ (size_t)v) * 0x9E3779B97F4A7C15ull;
-            return h;
-        }
-    };
-    thread_local std::unordered_map<Key, CUtensorMap, Hash> cache;
-    const Key key{base, cols, rows, ld, box_cols, box_rows, swizzle128};
-    auto it = cache.find(key);
-    if (it != cache.end()) { *tm = it->second; return true; }
-    const cuuint64_t dims[2] = {(cuuint64_t)cols, (cuuint64_t)rows};
-    const cuuint64_t strides[1] = {(cuuint64_t)ld * 4};
-    const cuuint32_t box[2] = {box_cols, box_rows};
-    const cuuint32_t estr[2] = {1, 1};
-    if (enc(tm, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, const_cast<void*>(base), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-            swizzle128 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_NONE,
-            CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) != CUDA_SUCCESS)
-        return false;
-    if (cache.size() > 4096) cache.clear();
-    cache.emplace(key, *tm);
-    return true;
-}
-
 // planning only (no launch): the configuration the launcher would choose; see sb200_debug_plan
 bool conv_tc_plan_info(const ConvArgs& a, int* out) {
     TcLaunch L{}; size_t smem = 0;
     if (a.cin % 32 || a.cout % 32 || a.ntaps > SB_MAX_TAPS || !plan(a, L, smem)) return false;
-    const int v[16] = {L.nt, L.wnt, L.ntiles_m, L.ntiles_n, L.resident, L.cat, L.tma_st, L.pairs, L.na, L.ws, L.nstg, (int)smem,
-                       L.tma_in, L.v8, L.tmem_cols, L.win};
+    const int v[16] = {L.nt, L.wnt, L.ntiles_m, L.ntiles_n, TC_STAGES, (int)smem, L.win, 0, 0, 0, 0, 0, 0, 0, 0, 0};
     for (int i = 0; i < 16; i++) out[i] = v[i];
     return true;
 }
@@ -857,41 +292,15 @@ void launch_conv_tc(const ConvArgs& a, cudaStream_t st) {
 // plans ONCE and launches; false (nothing launched) when the shape is not supported
 bool try_launch_conv_tc(const ConvArgs& a, cudaStream_t st) {
     if (a.cin % 32 || a.cout % 32 || a.ntaps > SB_MAX_TAPS) return false;
-    static PerDeviceOnce once;
-    once.run([] {
-        cudaFuncSetAttribute(conv_tc_kernel<0>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
-        cudaFuncSetAttribute(conv_tc_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
-    });
+    if ((a.ldx & 3) || (reinterpret_cast<uintptr_t>(a.x) & 15)) return false;     // 16-byte cp.async window rows
     TcLaunch L; size_t smem;
-    ConvArgs v;
-    CUtensorMap tm, tmr, tmx;
-    memset(&tm, 0, sizeof(tm));
-    memset(&tmr, 0, sizeof(tmr));
-    memset(&tmx, 0, sizeof(tmx));
     if (!plan(a, L, smem)) return false;
-    auto grid_of = [&]() {
-        const int units = L.pairs ? ((L.ntiles_m + 1) / 2) * L.ntiles_n : L.ntiles_m * L.ntiles_n;
-        return units < tc_num_sms() ? units : tc_num_sms();
-    };
-    int grid = grid_of();
-    v = a;
-    if (L.cat) v.wtc = a.wcat;
-    if (L.tma_in && !make_in_map(&tmx, a.x, a.rows_in, a.cin, a.ldx, L.win)) L.tma_in = 0;
-    if (L.tma_st) {
-        if (make_out_map(&tm, a.y0 + (size_t)a.orow_add * a.ldy0, a.cout, a.rows_q, a.ldy0) &&
-            (!a.res || make_out_map(&tmr, const_cast<float*>(a.res) + (size_t)a.orow_add * a.ldres, a.cout, a.rows_q, a.ldres))) {
-            launch_pdl(conv_tc_kernel<2>, dim3(grid), dim3(TC2_THREADS), smem, st, v, L, tm, tmr, tmx);
-            g_launch_count++;
-            check_launch("conv_tc_tma");
-            return true;
-        }
-        if (!plan(a, L, smem, false)) return false;          // no tensor map for these buffers: row-per-thread epilogue
-        grid = grid_of();
-        v = a;
-        if (L.cat) v.wtc = a.wcat;
-        if (L.tma_in && !make_in_map(&tmx, a.x, a.rows_in, a.cin, a.ldx, L.win)) L.tma_in = 0;
+    switch (L.nt) {
+        case 32: launch_nt<32>(a, L, smem, st); break;
+        case 64: launch_nt<64>(a, L, smem, st); break;
+        case 96: launch_nt<96>(a, L, smem, st); break;
+        default: launch_nt<128>(a, L, smem, st); break;
     }
-    launch_pdl(conv_tc_kernel<0>, dim3(grid), dim3(TC2_THREADS), smem, st, v, L, tm, tmr, tmx);
     g_launch_count++;
     check_launch("conv_tc");
     return true;
@@ -926,43 +335,6 @@ void conv_tc_build_weights(const float* wt /*[ntaps][cin][ldw]*/, int ldw, int c
                         img[(size_t)n * 64 + (size_t)(((ch + 4) ^ (n & 7)) << 3) + e] = l;
                     }
                 o += (size_t)nt * 64;
-            }
-}
-
-// cat-mode images: [n-tile][K-block][tap pair] images of 2*nt rows x 128 B; row n < nt = [hi of tap 2p : 32 ch |
-// hi of tap 2p+1 : 32 ch], row nt + n = the lo parts, K-major SWIZZLE_128B.  Same total size as the plain images
-// (plus one half-empty image when the tap count is odd).
-size_t conv_tc_cat_weight_floats(int cin, int cout, int ntaps, int nt) {
-    const int ntiles = (cout + nt - 1) / nt;
-    return (size_t)ntiles * (cin / 32) * ((ntaps + 1) / 2) * 2 * nt * 32;
-}
-
-void conv_tc_build_weights_cat(const float* wt /*[ntaps][cin][ldw]*/, int ldw, int cin, int cout, int ntaps, int nt,
-                               float* out) {
-    const int ntiles = (cout + nt - 1) / nt, nkb = cin / 32, npairs = (ntaps + 1) / 2;
-    uint16_t* o16 = reinterpret_cast<uint16_t*>(out);
-    memset(o16, 0, conv_tc_cat_weight_floats(cin, cout, ntaps, nt) * 4);
-    size_t o = 0;
-    for (int j = 0; j < ntiles; j++)
-        for (int kb = 0; kb < nkb; kb++)
-            for (int pr = 0; pr < npairs; pr++) {
-                uint16_t* img = o16 + o;
-                for (int h = 0; h < 2; h++) {
-                    const int t = 2 * pr + h;
-                    if (t >= ntaps) continue;
-                    for (int n = 0; n < nt; n++)
-                        for (int c = 0; c < 32; c++) {
-                            const int col = j * nt + n;
-                            const float v = col < cout ? wt[((size_t)t * cin + kb * 32 + c) * ldw + col] : 0.f;
-                            const uint16_t hi = bf16_rn_host(v);
-                            const uint16_t lo = bf16_rn_host(v - bf16_to_float_host(hi));
-                            const int ch = h * 4 + (c >> 3), e = c & 7;
-                            const int rl = nt + n;
-                            img[(size_t)n * 64 + (size_t)((ch ^ (n & 7)) << 3) + e] = hi;
-                            img[(size_t)rl * 64 + (size_t)((ch ^ (rl & 7)) << 3) + e] = lo;
-                        }
-                }
-                o += (size_t)2 * nt * 64;
             }
 }
 

@@ -1,35 +1,29 @@
-// tcgen05 implicit-GEMM Conv1d in error-compensated TF32 ("3xTF32") with CHUNK-FLUSHED accumulation, sm_100a.
+// wgmma implicit-GEMM Conv1d in error-compensated TF32 ("3xTF32") with CHUNK-FLUSHED accumulation, sm_90a.
 //
 // Used for the contractions whose result reaches the duration predictor: text-encoder qkv / o / ffn / proj and the
 // duration predictor's 1x1 convs (what onnxruntime's MLAS SGEMM computes inside `session.run`,
 // piper/src/lib.rs:362-379).  ceil(exp(logw)) is a cliff (SURVEY fact 4), so these layers need fp32-class accuracy:
 //   * operands are split  v = hi + lo,  hi = v with the low 13 mantissa bits cleared (exactly a tf32 number),
 //     lo = tf32_rn(v - hi); three MMAs accumulate  hi*hi + lo*hi + hi*lo  (the dropped lo*lo term is 2^-22);
-//   * the tensor core's fp32 accumulator TRUNCATES (profiles/notes_r01.md item 4: error grows linearly with the
-//     number of accumulating MMAs).  The K loop is therefore cut into chunks of 64 channels (1x1 convs) or
-//     32 channels x 3 taps; each chunk accumulates into a fresh TMEM accumulator and the epilogue warps add the
-//     finished chunk into a round-to-nearest fp32 running sum in registers while the next chunk is computed
-//     (two accumulator stages per issuer).  tools/emu_tc_accuracy.py: max error of a K = 2304 contraction
-//     2.5e-6 vs 5.4e-6 for the fp32 FMA chain of conv_simt.cu and 8.4e-5 without the flush.
+//   * the tensor core's fp32 accumulation loses accuracy as the number of accumulating MMAs grows.  The K loop is
+//     therefore cut into chunks of 64 channels (1x1 convs) or 32 channels x k taps; each chunk accumulates into a
+//     fresh register accumulator that is then added into a round-to-nearest fp32 running sum.
+//     tools/emu_tc_accuracy.py: max error of a K = 2304 contraction 2.5e-6 vs 5.4e-6 for the fp32 FMA chain of
+//     conv_simt.cu and 8.4e-5 without the flush.
 //
-// Tiling.  One persistent CTA per SM walks "pair tiles": TWO 128-row m-tiles x one n-tile of NTH <= 96 columns.
-// One thread can issue an M=128 MMA only every ~83 cycles whatever N is (tools/micro/mma_bench.cu), so the CTA has
-// two issuing warps; issuer h owns m-tile h of the pair (its own activation ring and accumulator pair) and both
-// read the SAME weight stage -- a weight image is fetched from L2 once per 256 output rows.
-//   * activations: one TMA tensor load per (m-tile, 32-channel K-block) brings the raw fp32 (128 + span)-row window
-//     into shared memory already in the K-major SWIZZLE_128B layout (32 fp32 = one 128-byte row); two converter
-//     warps rewrite it as the hi image in place and write the lo image beside it (same swizzled offsets, so the
-//     conversion is element-wise).  A tap is the same image with the descriptor start shifted by whole rows.
-//   * weights: hi / lo images pre-split at voice-load time, one cp.async.bulk per (K-block, tap) stage.
-//   * epilogue: tcgen05.ld of each finished chunk -> running sums (96 registers per thread); after the last chunk
-//     bias / ReLU / residual / scale / accumulate and 256-bit row-per-thread stores.
-// Warps: w0/w1 MMA issuers (w0 allocates TMEM), w2 weight loader, w3 activation loader, w4-7 converters,
-// w8-11 / w12-15 epilogue groups of issuer 0 / 1.  Every mbarrier wait carries the watchdog of tc_common.cuh.
+// One CTA = one 128-row x NT-column tile (NT = 96 / 64 / 32), two warpgroups (rows 0-63 / 64-127), a two-stage ring
+// over 32-channel K-blocks:
+//   * activations: the raw fp32 (128 + span)-row window arrives by cp.async straight into the K-major SWIZZLE_128B
+//     layout (32 fp32 = one 128-byte row, rows / columns outside the array zero-filled); all threads rewrite it as the
+//     hi image in place and write the lo image beside it (same swizzled offsets: the conversion is element-wise).
+//     The A operand comes from registers (wgmma with A in registers), loaded from any row offset: a tap is a shift.
+//   * weights: hi / lo images pre-split at voice-load time, one cp.async.bulk (TMA) per image, mbarrier completion.
+//   * epilogue: bias / ReLU / residual / scale / accumulate (or a transposed store) from the running sums.
 //
-// GM = 1 instantiation ("grouped GEMM", the two contractions of the relative-position attention): the B operand is
-// not a pre-split weight image but a second ACTIVATION matrix (K for Q.K^T, V^T for P.V), fetched by TMA tensor loads
-// and split by the converter warps like A; tiles come from a host-built table (one entry per (utterance, head,
-// m-tile pair, n-tile) with its own K extent), so ragged batches need no padding.  Four converter warps (16 warps).
+// GM = 1 ("grouped GEMM", the two contractions of the relative-position attention): the B operand is not a pre-split
+// weight image but a second ACTIVATION matrix (K for Q.K^T, V^T for P.V), loaded and split like A; tiles come from a
+// host-built table (one entry per (utterance, head, m-tile pair, n-tile) with its own K extent), so ragged batches need
+// no padding.  A CTA takes one m-tile of a table entry.
 #include "tc_common.cuh"
 #include <stdlib.h>
 #include <string.h>
@@ -40,392 +34,226 @@ namespace {
 
 using namespace tcx;
 
-constexpr int TF_WARP_WLOAD = 2, TF_WARP_ALOAD = 3, TF_WARP_CONV0 = 4;
-template <int GM> struct TfCfg {
-    static constexpr int NCONV = 128;                              // converter threads (64 could not keep up with two issuers on
-                                                                   // 1x1 layers: 2 x 128 rows per 12 MMAs; ncu: tensor pipe 17 %)
-    static constexpr int WARP_EPI0 = TF_WARP_CONV0 + NCONV / 32;   // first epilogue warp
-    static constexpr int THREADS = (WARP_EPI0 + 8) * 32;
-};
-constexpr int TF_NA_MAX = 4, TF_NW_MAX = 8;
-constexpr int TF_NTH_MAX = 96;
+constexpr int TF_THREADS = 256;
+constexpr int TF_STAGES = 2;
 
 struct TfLaunch {
-    int nth;         // columns of a tile (per issuer and per weight stage): 96 / 64 / 32
+    int nth;         // columns of a tile: 96 / 64 / 32
     int wnth;        // rows of a weight IMAGE (tf_nth_for); nth == wnth, or 32 on small launches: the CTA then takes a 32-row
-                     // part of the hi image and of the lo image (two copies per stage; 32 % 8 == 0 keeps the swizzle)
+                     // part of the hi image and of the lo image (32 % 8 == 0 keeps the swizzle)
     int win;         // window rows (multiple of 8)
-    int na, nw;      // activation ring stages per issuer, weight ring stages
-    int ntiles_mp;   // pairs of 128-row m-tiles
-    int ntiles_n;
+    int ntiles_m, ntiles_n;
     int chunk_kb;    // K-blocks per flush chunk
-    int tmem_cols;
-    uint32_t idesc;
 };
 
-__device__ __forceinline__ void tma_load_2d(uint32_t dst, const CUtensorMap* tm, uint32_t bar, int c0, int c1) {
-    asm volatile("cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
-                 ::"r"(dst), "l"(tm), "r"(bar), "r"(c0), "r"(c1) : "memory");
-}
-__device__ __forceinline__ void tc_mma_tf32(uint32_t d_tmem, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, {%5, %5, %5, %5}, p;\n\t}"
-        ::"r"(d_tmem), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate), "r"(0u) : "memory");
-}
+// GM = 1 operands: A [a_rows][a_cols] and B [b_rows][b_cols] (rows = output columns), K along the columns
+struct TfOperands {
+    const float* a; int a_rows, a_cols, lda;
+    const float* b; int b_rows, b_cols, ldb;
+    const TfTile* tiles;
+};
+
 __device__ __forceinline__ float tf32_rn(float v) {
     uint32_t r;
     asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(r) : "f"(v));
     return __uint_as_float(r);
 }
 
-template <int GM>
-__global__ void __launch_bounds__(TfCfg<GM>::THREADS, 1) conv_tf_kernel(const ConvArgs a, const TfLaunch L,
-                                                                         const __grid_constant__ CUtensorMap tm_x,
-                                                                         const __grid_constant__ CUtensorMap tm_b,
-                                                                         const TfTile* __restrict__ tiles) {
-    constexpr int TF_NCONV = TfCfg<GM>::NCONV;
-    constexpr int TF_WARP_EPI0 = TfCfg<GM>::WARP_EPI0;
+template <int GM, int NT>
+__global__ void __launch_bounds__(TF_THREADS, 1) conv_tf_kernel(const ConvArgs a, const TfLaunch L, const TfOperands G) {
     pdl_trigger();
     extern __shared__ __align__(1024) uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
+    const int ntaps = GM ? 1 : a.ntaps;
     const uint32_t a_img = (uint32_t)L.win * 128u;               // one image (hi or lo) of a window
-    const uint32_t w_img = (uint32_t)L.nth * 128u;               // one image (hi or lo) of a weight stage
-    uint8_t* A0 = smem;                                          // [2 issuers][na][hi | lo]
-    uint8_t* W0 = A0 + (size_t)2 * L.na * 2 * a_img;             // [nw][hi | lo]
-    uint64_t* bars = reinterpret_cast<uint64_t*>(W0 + (size_t)L.nw * 2 * w_img);
-    uint64_t* w_full = bars;                                     // [TF_NW_MAX]
-    uint64_t* w_empty = w_full + TF_NW_MAX;                      // [TF_NW_MAX]  (2 arrivals: both issuers)
-    uint64_t* raw_full = w_empty + TF_NW_MAX;                    // [2][TF_NA_MAX]  TMA landed
-    uint64_t* a_full = raw_full + 2 * TF_NA_MAX;                 // [2][TF_NA_MAX]  converted
-    uint64_t* a_empty = a_full + 2 * TF_NA_MAX;                  // [2][TF_NA_MAX]
-    uint64_t* acc_full = a_empty + 2 * TF_NA_MAX;                // [2][2]
-    uint64_t* acc_empty = acc_full + 4;                          // [2][2]
-    uint64_t* wraw_full = acc_empty + 4;                         // [TF_NW_MAX]  GM: B operand landed (TMA), not yet split
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(wraw_full + TF_NW_MAX);
-
+    const uint32_t w_img = (uint32_t)NT * 128u;                  // one image (hi or lo) of a tap
+    const uint32_t w_buf = (uint32_t)ntaps * 2u * w_img;
+    const uint32_t A0 = smem_u32(smem), W0 = A0 + TF_STAGES * 2 * a_img;   // [stage][hi | lo], [stage][tap][hi | lo]
+    uint64_t* bars = reinterpret_cast<uint64_t*>(smem + TF_STAGES * (2 * a_img + w_buf));
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-    const int nkb_conv = a.cin / 32;
-    const int total_tiles = GM ? L.ntiles_mp : L.ntiles_mp * L.ntiles_n;
-    auto tile_nkb = [&](int tl) -> int { return GM ? tiles[(int)blockIdx.x + tl * (int)gridDim.x].nkb : nkb_conv; };
-    const int my_tiles = (total_tiles - (int)blockIdx.x + (int)gridDim.x - 1) / (int)gridDim.x;
 
-    if (warp == TF_WARP_ALOAD) {
-        // barriers initialised by one warp in parallel; bars[] order: w_full, w_empty, raw_full, a_full, a_empty, acc_full,
-        // acc_empty, wraw_full
-        constexpr int NB = 3 * TF_NW_MAX + 6 * TF_NA_MAX + 8;
-        for (int i = lane; i < NB; i += 32) {
-            uint32_t cnt = 1;
-            if (i < TF_NW_MAX) cnt = GM ? TF_NCONV : 1;                                          // w_full
-            else if (i < 2 * TF_NW_MAX) cnt = 2;                                                 // w_empty
-            else if (i < 2 * TF_NW_MAX + 2 * TF_NA_MAX) cnt = 1;                                 // raw_full
-            else if (i < 2 * TF_NW_MAX + 4 * TF_NA_MAX) cnt = TF_NCONV;                          // a_full
-            else if (i < 2 * TF_NW_MAX + 6 * TF_NA_MAX + 4) cnt = 1;                             // a_empty, acc_full
-            else if (i < 2 * TF_NW_MAX + 6 * TF_NA_MAX + 8) cnt = 128;                           // acc_empty
-            mbar_init(smem_u32(&bars[i]), cnt);                                                  // (rest: wraw_full, 1)
-        }
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-        if (lane == 0) {
-            asm volatile("prefetch.tensormap [%0];" ::"l"(&tm_x) : "memory");
-            if (GM) asm volatile("prefetch.tensormap [%0];" ::"l"(&tm_b) : "memory");
-        }
-    }
-    if (warp == 0) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)),
-                     "r"((uint32_t)L.tmem_cols) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    tc_fence_before();
-    __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
-    // everything above (barriers, TMEM, tensor-map prefetch) overlapped the previous kernels' tails; from here on global
-    // memory written by them is read -- except by the weight loader of the conv form, whose bulk copies read constants
-    if (GM || warp != TF_WARP_WLOAD) pdl_wait();
-
-    if (warp < 2) {
-        // ===================== MMA issuer h: m-tile h of every pair tile =====================
-        // warp-uniform loop, tcgen05 instructions under elect.sync (see conv_tc.cu).  K-major SWIZZLE_128B
-        // descriptor: start>>4 | LBO 1<<16 | SBO (1024>>4)<<32 | version 1<<46 | SWIZZLE_128B 2<<61.
-        const int h = warp;
-        const uint64_t desc_hi = ((uint64_t)1 << 16) | ((uint64_t)(1024 >> 4) << 32) | ((uint64_t)1 << 46) | ((uint64_t)2 << 61);
-        int li = 0, lw = 0, lc = 0;            // activation-stage, weight-stage and chunk counters
-        for (int tl = 0; tl < my_tiles; tl++) {
-            const int nkb = tile_nkb(tl);
-            for (int kb = 0; kb < nkb; kb++, li++) {
-                const int cpos = kb % L.chunk_kb;
-                const int st = lc & 1;
-                if (cpos == 0) {
-                    mbar_wait(smem_u32(&acc_empty[h * 2 + st]), (uint32_t)(((lc >> 1) & 1) ^ 1));
-                    tc_fence_after();
-                }
-                const uint32_t dcol = tmem_base + (uint32_t)((h * 2 + st) * L.nth);
-                const int as = li % L.na;
-                mbar_wait(smem_u32(&a_full[h * TF_NA_MAX + as]), (uint32_t)((li / L.na) & 1));
-                tc_fence_after();
-                const uint32_t ahi = smem_u32(A0 + (size_t)((h * L.na + as) * 2) * a_img) >> 4;
-                const uint32_t alo = ahi + (a_img >> 4);
-                for (int t = 0; t < a.ntaps; t++, lw++) {
-                    const int ws = lw % L.nw;
-                    mbar_wait(smem_u32(&w_full[ws]), (uint32_t)((lw / L.nw) & 1));
-                    tc_fence_after();
-                    const uint32_t whi = smem_u32(W0 + (size_t)ws * 2 * w_img) >> 4;
-                    const uint32_t wlo = whi + (w_img >> 4);
-                    const uint32_t arow = (uint32_t)(a.tap_off[t] - a.min_off) * 8u;       // rows * 128 B >> 4
-                    if (elect_one()) {
-#pragma unroll
-                        for (int ks = 0; ks < 4; ks++) {                  // four K = 8 steps inside the 128-byte row
-                            const uint64_t dah = desc_hi | (uint64_t)(ahi + arow + ks * 2);
-                            const uint64_t dal = desc_hi | (uint64_t)(alo + arow + ks * 2);
-                            const uint64_t dwh = desc_hi | (uint64_t)(whi + ks * 2);
-                            const uint64_t dwl = desc_hi | (uint64_t)(wlo + ks * 2);
-                            tc_mma_tf32(dcol, dah, dwh, L.idesc, (cpos | t | ks) ? 1u : 0u);
-                            tc_mma_tf32(dcol, dal, dwh, L.idesc, 1u);
-                            tc_mma_tf32(dcol, dah, dwl, L.idesc, 1u);
-                        }
-                        tc_commit(smem_u32(&w_empty[ws]));
-                    }
-                    __syncwarp();
-                }
-                if (elect_one()) tc_commit(smem_u32(&a_empty[h * TF_NA_MAX + as]));
-                __syncwarp();
-                if (cpos == L.chunk_kb - 1 || kb == nkb - 1) {
-                    if (elect_one()) tc_commit(smem_u32(&acc_full[h * 2 + st]));
-                    __syncwarp();
-                    lc++;
-                }
-            }
-        }
-    } else if (warp == TF_WARP_WLOAD) {
-        // ===================== weight loader: one bulk copy per (K-block, tap) stage =====================
-        if (lane == 0 && GM) {
-            // B operand = activations: one TMA tensor load (32 K-columns x nth rows) per K-block into the hi image slot
-            int lw = 0;
-            for (int tl = 0; tl < my_tiles; tl++) {
-                const TfTile T = tiles[(int)blockIdx.x + tl * (int)gridDim.x];
-                for (int kb = 0; kb < T.nkb; kb++, lw++) {
-                    const int ws = lw % L.nw;
-                    mbar_wait(smem_u32(&w_empty[ws]), (uint32_t)(((lw / L.nw) & 1) ^ 1));
-                    mbar_expect_tx(smem_u32(&wraw_full[ws]), w_img);
-                    tma_load_2d(smem_u32(W0 + (size_t)ws * 2 * w_img), &tm_b, smem_u32(&wraw_full[ws]), T.b_col0 + kb * 32, T.b_row0);
-                }
-            }
-        } else if (lane == 0) {
-            const int per_tile = nkb_conv * a.ntaps;
-            const uint32_t w_stage = 2 * w_img;
-            int lw = 0;
-            const int vf = L.wnth / L.nth;                       // tile = 1 / vf of an image
-            const size_t src_img = (size_t)L.wnth * 128u;        // one image in the voice (a stage = hi image + lo image)
-            for (int tl = 0; tl < my_tiles; tl++) {
-                const int tg = (int)blockIdx.x + tl * (int)gridDim.x;
-                const int n_tile = tg % L.ntiles_n;
-                const uint8_t* wsrc = reinterpret_cast<const uint8_t*>(a.wtf) + (size_t)(n_tile / vf) * per_tile * 2 * src_img +
-                                      (size_t)(n_tile % vf) * w_img;
-                for (int i = 0; i < per_tile; i++, lw++) {
-                    const int ws = lw % L.nw;
-                    mbar_wait(smem_u32(&w_empty[ws]), (uint32_t)(((lw / L.nw) & 1) ^ 1));
-                    mbar_expect_tx(smem_u32(&w_full[ws]), w_stage);
-                    const uint8_t* st = wsrc + (size_t)i * 2 * src_img;
-                    if (vf == 1) bulk_g2s(smem_u32(W0 + (size_t)ws * w_stage), st, w_stage, smem_u32(&w_full[ws]));
-                    else {
-                        bulk_g2s(smem_u32(W0 + (size_t)ws * w_stage), st, w_img, smem_u32(&w_full[ws]));
-                        bulk_g2s(smem_u32(W0 + (size_t)ws * w_stage + w_img), st + src_img, w_img, smem_u32(&w_full[ws]));
-                    }
-                }
-            }
-        }
-        __syncwarp();
-    } else if (warp == TF_WARP_ALOAD) {
-        // ===================== activation loader: raw fp32 window -> the hi image slot (swizzled by the TMA engine) ======
-        if (lane == 0) {
-            int li = 0;
-            for (int tl = 0; tl < my_tiles; tl++) {
-                const int tg = (int)blockIdx.x + tl * (int)gridDim.x;
-                const int mp = tg / L.ntiles_n;
-                TfTile T{};
-                if (GM) T = tiles[tg];
-                const int nkb = GM ? T.nkb : nkb_conv;
-                for (int kb = 0; kb < nkb; kb++, li++) {
-                    const int as = li % L.na;
-                    for (int h = 0; h < 2; h++) {
-                        mbar_wait(smem_u32(&a_empty[h * TF_NA_MAX + as]), (uint32_t)(((li / L.na) & 1) ^ 1));
-                        mbar_expect_tx(smem_u32(&raw_full[h * TF_NA_MAX + as]), a_img);
-                        tma_load_2d(smem_u32(A0 + (size_t)((h * L.na + as) * 2) * a_img), &tm_x,
-                                    smem_u32(&raw_full[h * TF_NA_MAX + as]), (GM ? T.a_col0 : 0) + kb * 32,
-                                    GM ? T.a_row0[h] : (mp * 2 + h) * 128 + a.min_off);
-                    }
-                }
-            }
-        }
-        __syncwarp();
-    } else if (warp < TF_WARP_EPI0) {
-        // ===================== converters: hi = v with 13 low mantissa bits cleared (in place), lo = tf32_rn(v - hi) ====
-        const int ct = tid - TF_WARP_CONV0 * 32;
-        const int nchunk = L.win * 8;                  // 16-byte chunks per image
-        const float slope = GM ? 1.f : a.in_slope;
-        auto split_image = [&](uint32_t hi_img, uint32_t lo_img, int n16) {
-            for (int idx = ct; idx < n16; idx += TF_NCONV) {
-                float4 v = lds128(hi_img + (uint32_t)idx * 16u);
-                if (slope != 1.f) {
-                    v.x = fmaxf(v.x, v.x * slope); v.y = fmaxf(v.y, v.y * slope);
-                    v.z = fmaxf(v.z, v.z * slope); v.w = fmaxf(v.w, v.w * slope);
-                }
-                uint4 hi, lo;
-                hi.x = __float_as_uint(v.x) & 0xffffe000u; hi.y = __float_as_uint(v.y) & 0xffffe000u;
-                hi.z = __float_as_uint(v.z) & 0xffffe000u; hi.w = __float_as_uint(v.w) & 0xffffe000u;
-                lo.x = __float_as_uint(tf32_rn(v.x - __uint_as_float(hi.x)));
-                lo.y = __float_as_uint(tf32_rn(v.y - __uint_as_float(hi.y)));
-                lo.z = __float_as_uint(tf32_rn(v.z - __uint_as_float(hi.z)));
-                lo.w = __float_as_uint(tf32_rn(v.w - __uint_as_float(hi.w)));
-                sts128u(hi_img + (uint32_t)idx * 16u, hi);
-                sts128u(lo_img + (uint32_t)idx * 16u, lo);
-            }
-            fence_async_smem();                        // generic-proxy stores -> visible to the tensor core
-        };
-        int li = 0, lw = 0;
-        for (int tl = 0; tl < my_tiles; tl++) {
-            const int nkb = tile_nkb(tl);
-            for (int kb = 0; kb < nkb; kb++, li++) {
-                const int as = li % L.na;
-                for (int h = 0; h < 2; h++) {
-                    mbar_wait(smem_u32(&raw_full[h * TF_NA_MAX + as]), (uint32_t)((li / L.na) & 1));
-                    const uint32_t hi_img = smem_u32(A0 + (size_t)((h * L.na + as) * 2) * a_img);
-                    split_image(hi_img, hi_img + a_img, nchunk);
-                    mbar_arrive(smem_u32(&a_full[h * TF_NA_MAX + as]));
-                }
-                if (GM) {                              // the B operand of this K-block (same order as the issuers consume)
-                    const int ws = lw % L.nw;
-                    mbar_wait(smem_u32(&wraw_full[ws]), (uint32_t)((lw / L.nw) & 1));
-                    const uint32_t hi_img = smem_u32(W0 + (size_t)ws * 2 * w_img);
-                    split_image(hi_img, hi_img + w_img, L.nth * 8);
-                    mbar_arrive(smem_u32(&w_full[ws]));
-                    lw++;
-                }
-            }
-        }
+    TfTile T{};
+    int h = 0, m_tile = 0, n_tile = 0, nkb = a.cin / 32;
+    if (GM) {
+        T = G.tiles[blockIdx.x >> 1];
+        h = (int)blockIdx.x & 1;
+        nkb = T.nkb;
     } else {
-        // ===================== epilogue group h: chunk sums -> fp32 running sums -> output =====================
-        const int h = (warp - TF_WARP_EPI0) >> 2;
-        const int quad = warp & 3;                     // TMEM lane quadrant this warp may read
-        const int row = quad * 32 + lane;
-        int lc = 0;
-        for (int tl = 0; tl < my_tiles; tl++) {
-            const int tg = (int)blockIdx.x + tl * (int)gridDim.x;
-            const int q = ((tg / L.ntiles_n) * 2 + h) * 128 + row;
-            const int n0 = (tg % L.ntiles_n) * L.nth;
-            TfTile T{};
-            if (GM) T = tiles[tg];
-            const int nchunks = ((GM ? T.nkb : nkb_conv) + L.chunk_kb - 1) / L.chunk_kb;
-            float run[TF_NTH_MAX];
-#pragma unroll
-            for (int j = 0; j < TF_NTH_MAX; j++) run[j] = 0.f;
-            for (int c = 0; c < nchunks; c++, lc++) {
-                const int st = lc & 1;
-                mbar_wait(smem_u32(&acc_full[h * 2 + st]), (uint32_t)((lc >> 1) & 1));
-                tc_fence_after();
-                const uint32_t tcol = tmem_base + ((uint32_t)(quad * 32) << 16) + (uint32_t)((h * 2 + st) * L.nth);
-#pragma unroll
-                for (int p = 0; p < TF_NTH_MAX / 16; p++) {
-                    if (p * 16 < L.nth) {
-                        float t[16];
-                        tmem_ld16(tcol + (uint32_t)(p * 16), t);
-#pragma unroll
-                        for (int j = 0; j < 16; j++) run[p * 16 + j] += t[j];
-                    }
-                }
-                tc_fence_before();
-                mbar_arrive(smem_u32(&acc_empty[h * 2 + st]));
-            }
-            if (GM) {
-                // grouped GEMM: out = acc * scale (+ res), rows of this m-tile that belong to the utterance only
-                if (row >= T.rows_valid[h]) continue;
-                float* dst = a.y0 + T.out_off[h] + (size_t)row * a.ldy0;
-                const float* rsrc = a.res ? a.res + T.out_off[h] + (size_t)row * a.ldres : nullptr;
-#pragma unroll
-                for (int p = 0; p < TF_NTH_MAX / 8; p++) {
-                    if (p * 8 < L.nth) {
-                        float o[8], r[8];
-#pragma unroll
-                        for (int j = 0; j < 8; j++) r[j] = 0.f;
-                        if (rsrc) ldg256(rsrc + p * 8, r);
-#pragma unroll
-                        for (int j = 0; j < 8; j++) o[j] = fmaf(run[p * 8 + j], a.scale, r[j]);
-                        stg256(dst + p * 8, o);
-                    }
-                }
-                continue;
-            }
-            if (q >= a.rows_q) continue;
-            const bool valid = row_valid(a.map, q);
-            if (a.yt && n0 >= a.yt_col0) {
-                // transposed output tile (V of the fused q/k/v projection: the P.V contraction wants keys contiguous):
-                // yt[column][row]; the 32 lanes of a warp own 32 consecutive rows, so every store instruction writes one
-                // 128-byte line
-                float* dst = a.yt + (size_t)(n0 - a.yt_col0) * a.ldyt + q;
-#pragma unroll
-                for (int j = 0; j < TF_NTH_MAX; j++) {
-                    if (j < L.nth) {
-                        float o = run[j] + (a.bias ? a.bias[n0 + j] : 0.f);
-                        if (a.act == ACT_RELU) o = fmaxf(o, 0.f);
-                        dst[(size_t)j * a.ldyt] = valid ? o * a.scale : 0.f;
-                    }
-                }
-                continue;
-            }
-            if (a.acc0 && !valid) continue;            // accumulated buffers keep their zeros in gap rows
-            const size_t orow = (size_t)q + a.orow_add;
-#pragma unroll
-            for (int p = 0; p < TF_NTH_MAX / 8; p++) {
-                if (p * 8 < L.nth) {
-                    const int n = n0 + p * 8;
-                    float o[8];
-#pragma unroll
-                    for (int j = 0; j < 8; j++) o[j] = run[p * 8 + j];
-                    if (a.bias) {
-                        const float4 b0 = *reinterpret_cast<const float4*>(a.bias + n), b1 = *reinterpret_cast<const float4*>(a.bias + n + 4);
-                        o[0] += b0.x; o[1] += b0.y; o[2] += b0.z; o[3] += b0.w; o[4] += b1.x; o[5] += b1.y; o[6] += b1.z; o[7] += b1.w;
-                    }
-                    if (a.act == ACT_RELU) {
-#pragma unroll
-                        for (int j = 0; j < 8; j++) o[j] = fmaxf(o[j], 0.f);
-                    }
-                    float m[8];
-#pragma unroll
-                    for (int j = 0; j < 8; j++) m[j] = 0.f;
-                    if (a.res && valid) {
-                        float r[8];
-                        ldg256(a.res + orow * a.ldres + n, r);
-#pragma unroll
-                        for (int j = 0; j < 8; j++) m[j] = r[j] * a.scale;
-                    }
-                    if (a.acc0 && valid) {
-                        float r[8];
-                        ldg256(a.y0 + orow * a.ldy0 + n, r);
-#pragma unroll
-                        for (int j = 0; j < 8; j++) m[j] += r[j];
-                    }
-#pragma unroll
-                    for (int j = 0; j < 8; j++) o[j] = valid ? fmaf(o[j], a.scale, m[j]) : 0.f;
-                    stg256(a.y0 + orow * a.ldy0 + n, o);
-                }
+        m_tile = (int)blockIdx.x / L.ntiles_n;
+        n_tile = (int)blockIdx.x % L.ntiles_n;
+    }
+    if (tid == 0) {
+        for (int s = 0; s < TF_STAGES; s++) mbar_init(smem_u32(&bars[s]), 1);
+        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    }
+    __syncthreads();
+
+    // conv form: weight stage kb = (hi, lo) image pairs of every tap, rows [part * NT, +NT) of the voice's images
+    const int vf = L.wnth / NT;
+    const size_t src_img = (size_t)L.wnth * 128u;
+    const uint8_t* wsrc = GM ? nullptr : reinterpret_cast<const uint8_t*>(a.wtf) + (size_t)(n_tile / vf) * nkb * ntaps * 2 * src_img +
+                                         (size_t)(n_tile % vf) * w_img;
+    auto issue_w = [&](int kb, int s) {
+        if (tid == 0) {
+            const uint32_t bar = smem_u32(&bars[s]);
+            mbar_expect_tx(bar, w_buf);
+            for (int t = 0; t < ntaps; t++) {
+                const uint8_t* st = wsrc + (size_t)(kb * ntaps + t) * 2 * src_img;
+                bulk_g2s(W0 + s * w_buf + t * 2 * w_img, st, w_img, bar);
+                bulk_g2s(W0 + s * w_buf + t * 2 * w_img + w_img, st + src_img, w_img, bar);
             }
         }
+    };
+    // rows [row0, row0 + nrows) x columns [col0, col0 + 32) of a [rows][cols] matrix -> swizzled raw image
+    auto load_rows = [&](uint32_t img, const float* base, int ld, int rows, int cols, int row0, int col0, int nrows) {
+        for (int idx = tid; idx < nrows * 8; idx += TF_THREADS) {
+            const int r = idx >> 3, ch = idx & 7;
+            const int gr = row0 + r, gc = col0 + ch * 4;
+            const int nval = gr >= 0 && gr < rows ? min(max(cols - gc, 0), 4) : 0;
+            cp_async16(sw128(img, r, ch), nval ? base + (size_t)gr * ld + gc : base, (uint32_t)nval * 4u);
+        }
+    };
+    auto issue_a = [&](int kb, int s) {
+        const uint32_t img = A0 + s * 2 * a_img;
+        if (GM) {
+            load_rows(img, G.a, G.lda, G.a_rows, G.a_cols, T.a_row0[h], T.a_col0 + kb * 32, 128);
+            load_rows(W0 + s * w_buf, G.b, G.ldb, G.b_rows, G.b_cols, T.b_row0, T.b_col0 + kb * 32, NT);
+        } else {
+            load_rows(img, a.x, a.ldx, a.rows_in, a.cin, m_tile * 128 + a.min_off, kb * 32, L.win);
+        }
+        cp_async_commit();
+    };
+    // hi = v with 13 low mantissa bits cleared (in place), lo = tf32_rn(v - hi) at the same offset of the next image
+    auto split_image = [&](uint32_t hi_img, uint32_t lo_img, int n16, float slope) {
+        for (int idx = tid; idx < n16; idx += TF_THREADS) {
+            float4 v = lds128(hi_img + (uint32_t)idx * 16u);
+            if (slope != 1.f) {
+                v.x = fmaxf(v.x, v.x * slope); v.y = fmaxf(v.y, v.y * slope);
+                v.z = fmaxf(v.z, v.z * slope); v.w = fmaxf(v.w, v.w * slope);
+            }
+            uint4 hi, lo;
+            hi.x = __float_as_uint(v.x) & 0xffffe000u; hi.y = __float_as_uint(v.y) & 0xffffe000u;
+            hi.z = __float_as_uint(v.z) & 0xffffe000u; hi.w = __float_as_uint(v.w) & 0xffffe000u;
+            lo.x = __float_as_uint(tf32_rn(v.x - __uint_as_float(hi.x)));
+            lo.y = __float_as_uint(tf32_rn(v.y - __uint_as_float(hi.y)));
+            lo.z = __float_as_uint(tf32_rn(v.z - __uint_as_float(hi.z)));
+            lo.w = __float_as_uint(tf32_rn(v.w - __uint_as_float(hi.w)));
+            sts128u(hi_img + (uint32_t)idx * 16u, hi);
+            sts128u(lo_img + (uint32_t)idx * 16u, lo);
+        }
+    };
+
+    if (!GM) issue_w(0, 0);                             // weights are constants: fetched before the predecessor finishes
+    pdl_wait();
+    issue_a(0, 0);
+
+    const int wg = warp >> 2, g = lane >> 2, c = lane & 3;
+    const int r0 = wg * 64 + (warp & 3) * 16 + g;       // tile rows r0 and r0 + 8 of this thread
+    float acc[NT / 2], run[NT / 2];
+#pragma unroll
+    for (int i = 0; i < NT / 2; i++) { acc[i] = 0.f; run[i] = 0.f; }
+
+    for (int kb = 0; kb < nkb; kb++) {
+        const int s = kb & 1;
+        if (kb + 1 < nkb) {
+            if (!GM) issue_w(kb + 1, s ^ 1);
+            issue_a(kb + 1, s ^ 1);
+            cp_async_wait<1>();
+        } else {
+            cp_async_wait<0>();
+        }
+        __syncthreads();
+        const uint32_t ahi = A0 + s * 2 * a_img, alo = ahi + a_img;
+        const uint32_t wst = W0 + s * w_buf;
+        split_image(ahi, alo, L.win * 8, GM ? 1.f : a.in_slope);
+        if (GM) split_image(wst, wst + w_img, NT * 8, 1.f);
+        if (GM) fence_async_smem();
+        __syncthreads();
+        if (!GM) mbar_wait(smem_u32(&bars[s]), (uint32_t)((kb >> 1) & 1));
+        for (int t = 0; t < ntaps; t++) {
+            const int R0 = r0 + (GM ? 0 : a.tap_off[t] - a.min_off), R1 = R0 + 8;
+            const uint32_t whi = wst + t * 2 * w_img, wlo = whi + w_img;
+#pragma unroll
+            for (int half = 0; half < 2; half++) {      // two K = 8 steps per register load
+                uint32_t fh[2][4], fl[2][4];
+#pragma unroll
+                for (int u = 0; u < 2; u++) {
+                    const int ks = 2 * half + u;
+                    fh[u][0] = lds32(sw128(ahi, R0, 2 * ks) + 4u * c);
+                    fh[u][1] = lds32(sw128(ahi, R1, 2 * ks) + 4u * c);
+                    fh[u][2] = lds32(sw128(ahi, R0, 2 * ks + 1) + 4u * c);
+                    fh[u][3] = lds32(sw128(ahi, R1, 2 * ks + 1) + 4u * c);
+                    fl[u][0] = lds32(sw128(alo, R0, 2 * ks) + 4u * c);
+                    fl[u][1] = lds32(sw128(alo, R1, 2 * ks) + 4u * c);
+                    fl[u][2] = lds32(sw128(alo, R0, 2 * ks + 1) + 4u * c);
+                    fl[u][3] = lds32(sw128(alo, R1, 2 * ks + 1) + 4u * c);
+                }
+                acc_fence<NT / 2>(acc);
+                wg_fence();
+#pragma unroll
+                for (int u = 0; u < 2; u++) {
+                    const int ks = 2 * half + u;
+                    const uint64_t dwh = sw128_desc(whi + 32u * ks), dwl = sw128_desc(wlo + 32u * ks);
+                    wgmma_rs<WG_TF32, NT>(acc, fh[u], dwh);
+                    wgmma_rs<WG_TF32, NT>(acc, fl[u], dwh);
+                    wgmma_rs<WG_TF32, NT>(acc, fh[u], dwl);
+                }
+                wg_commit();
+                wg_wait0();
+                acc_fence<NT / 2>(acc);
+            }
+        }
+        if (kb % L.chunk_kb == L.chunk_kb - 1 || kb == nkb - 1) {   // chunk finished: flush into the running sums
+#pragma unroll
+            for (int i = 0; i < NT / 2; i++) { run[i] += acc[i]; acc[i] = 0.f; }
+        }
+        __syncthreads();                                // stage s fully read: the next iteration refills it
     }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 0) {
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"((uint32_t)L.tmem_cols)
-                     : "memory");
+
+    // ===================== epilogue: thread owns rows r0, r0 + 8 and column pairs 8j + 2c =====================
+#pragma unroll
+    for (int hh = 0; hh < 2; hh++) {
+        const int row = r0 + 8 * hh;
+        if (GM) {
+            // grouped GEMM: out = acc * scale (+ res), rows of this m-tile that belong to the utterance only
+            if (row >= T.rows_valid[h]) continue;
+            float* dst = a.y0 + T.out_off[h] + (size_t)row * a.ldy0;
+            const float* rsrc = a.res ? a.res + T.out_off[h] + (size_t)row * a.ldres : nullptr;
+#pragma unroll
+            for (int j = 0; j < NT / 8; j++)
+#pragma unroll
+                for (int e = 0; e < 2; e++) {
+                    const int n = 8 * j + 2 * c + e;
+                    dst[n] = fmaf(run[4 * j + 2 * hh + e], a.scale, rsrc ? rsrc[n] : 0.f);
+                }
+            continue;
+        }
+        const int q = m_tile * 128 + row;
+        if (q >= a.rows_q) continue;
+        const bool valid = row_valid(a.map, q);
+        const size_t orow = (size_t)q + a.orow_add;
+#pragma unroll
+        for (int j = 0; j < NT / 8; j++)
+#pragma unroll
+            for (int e = 0; e < 2; e++) {
+                const int n = n_tile * NT + 8 * j + 2 * c + e;
+                float o = run[4 * j + 2 * hh + e] + (a.bias ? a.bias[n] : 0.f);
+                if (a.act == ACT_RELU) o = fmaxf(o, 0.f);
+                if (a.yt && n >= a.yt_col0) {
+                    // transposed output (V of the fused q/k/v projection: the P.V contraction wants keys contiguous)
+                    a.yt[(size_t)(n - a.yt_col0) * a.ldyt + q] = valid ? o * a.scale : 0.f;
+                    continue;
+                }
+                if (a.acc0 && !valid) continue;         // accumulated buffers keep their zeros in gap rows
+                float m = 0.f;
+                if (a.res && valid) m = a.res[orow * a.ldres + n] * a.scale;
+                if (a.acc0 && valid) m += a.y0[orow * a.ldy0 + n];
+                a.y0[orow * a.ldy0 + n] = valid ? fmaf(o, a.scale, m) : 0.f;
+            }
     }
 }
 
-// Column tile.  k-tap layers (ffn): 96 columns -- an activation stage feeds 3 x 12 MMAs, so two ring stages hide the
-// load + conversion latency (ncu: tensor pipe ~50 %).  1x1 layers: an activation stage feeds only 12 MMAs (~1000 cycles)
-// while a TMA load + conversion takes ~2000, so they want THREE stages per issuer, which only fits next to 64-column
-// weight stages (ncu with 96 columns / 2 stages: tensor pipe 12-20 %, 35-57 TFLOP/s against 150-160 for the k3 layers).
-int tf_num_sms();
-
+// Column tile.  k-tap layers (ffn): 96 columns; 1x1 layers: 64 columns.  Images are built at this width.
 int tf_nth_for(int cout, int ntaps) {
     if (ntaps == 1 && cout % 64 == 0) return 64;
     if (cout % 96 == 0) return 96;
@@ -433,54 +261,44 @@ int tf_nth_for(int cout, int ntaps) {
     if (cout % 32 == 0) return 32;
     return 0;
 }
-constexpr size_t TF_SMEM_BUDGET = 227 * 1024 - 1024;     // opt-in maximum minus the slack of the manual 1024-byte alignment
+
+size_t smem_bytes(int win, int ntaps, int nth) {
+    return (size_t)TF_STAGES * (2 * (size_t)win * 128 + (size_t)ntaps * 2 * nth * 128) + TF_STAGES * 8;
+}
 
 bool plan(const ConvArgs& a, TfLaunch& L, size_t& smem) {
     if (!a.wtf || a.cin % 32 || a.cout % 32 || a.ntaps < 1 || a.ntaps > SB_MAX_TAPS) return false;
     if (a.act == ACT_GATE || a.split < a.cout || a.orow_mul != 1 || a.phase_cols) return false;
-    if (!have_tensor_maps()) return false;
-    auto al32 = [](const void* p, int ld) { return p == nullptr || ((reinterpret_cast<uintptr_t>(p) & 31) == 0 && (ld & 7) == 0); };
-    if (!al32(a.y0, a.ldy0) || !al32(a.res, a.ldres)) return false;
     if ((a.ldx & 3) || (reinterpret_cast<uintptr_t>(a.x) & 15)) return false;
     L.nth = L.wnth = tf_nth_for(a.cout, a.ntaps);
     if (!L.nth) return false;
     L.win = (128 + a.span + 7) & ~7;
-    if (L.win > 256) return false;
-    L.ntiles_mp = (a.rows_q + 255) / 256;
-    // Small launches (a single utterance): 32-column tiles on more SMs -- the K loop of a tile costs the same number of
-    // MMAs whatever its width, but each is cheaper and the flush / epilogue of a tile shrinks with its width.
-    if (L.wnth > 32 && L.ntiles_mp * (a.cout / 32) <= tf_num_sms() && !SB_ENV_ONCE("SB200_TF_NONARROW")) L.nth = 32;
+    if (smem_bytes(L.win, a.ntaps, 32) > WG_SMEM_BUDGET) return false;
+    L.ntiles_m = (a.rows_q + 127) / 128;
+    // Small launches (a single utterance), or a weight stage too large for two stages: 32-column parts of the images.
+    // Tile width changes no summation order.
+    if (L.wnth > 32 && (L.ntiles_m * (a.cout / 32) <= wg_num_sms() || smem_bytes(L.win, a.ntaps, L.wnth) > WG_SMEM_BUDGET))
+        L.nth = 32;
     L.ntiles_n = a.cout / L.nth;
     L.chunk_kb = a.ntaps == 1 ? 2 : 1;
-    { const char* e = SB_ENV_ONCE("SB200_TF_CHUNK"); if (e && atoi(e) >= 1) L.chunk_kb = atoi(e); }     // accuracy experiments
-    L.tmem_cols = 32;
-    while (L.tmem_cols < 4 * L.nth) L.tmem_cols <<= 1;
-    // kind::tf32 instruction descriptor: D fp32 (1<<4), A = B = TF32 (2<<7, 2<<10), K-major both, N>>3, M>>4
-    L.idesc = (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)(L.nth >> 3) << 17) | ((uint32_t)(128 >> 4) << 24);
-    const size_t a_img = (size_t)L.win * 128, w_stage = (size_t)L.nth * 256;
-    const size_t bar_bytes = (3 * TF_NW_MAX + 6 * TF_NA_MAX + 8) * 8 + 16;
-    const size_t budget = TF_SMEM_BUDGET;
-    L.na = 2; L.nw = 2;
-    auto total = [&]() { return (size_t)2 * L.na * 2 * a_img + (size_t)L.nw * w_stage + bar_bytes; };
-    if (total() > budget) return false;
-    if (a.ntaps == 1) {
-        // 1x1: activation stages first (see tf_nth_for), then whatever is left for the weight ring
-        while (L.na < 3) { L.na++; if (total() > budget) { L.na--; break; } }
-        while (L.nw < 4) { L.nw++; if (total() > budget) { L.nw--; break; } }
-    } else {
-        // weight stages turn over ntaps times faster than activation stages: deepen the weight ring first
-        while (L.nw < TF_NW_MAX && L.nw < 2 * a.ntaps + 2) { L.nw++; if (total() > budget) { L.nw--; break; } }
-        while (L.na < TF_NA_MAX) { L.na++; if (total() > budget) { L.na--; break; } }
-    }
-    { const char* e = SB_ENV_ONCE("SB200_TF_NW"); if (e && atoi(e) >= 2 && atoi(e) <= TF_NW_MAX) { const int o = L.nw; L.nw = atoi(e); if (total() > budget) L.nw = o; } }
-    smem = total() + 1024;
+    smem = smem_bytes(L.win, a.ntaps, L.nth) + 1024;
     return true;
 }
 
-int tf_num_sms() {
-    static int n = 0;
-    if (!n) { int dev = 0; cudaGetDevice(&dev); cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev); if (n <= 0) n = 148; }
-    return n;
+template <int GM, int NT> void launch_nt(dim3 grid, size_t smem, cudaStream_t st, const ConvArgs& a, const TfLaunch& L,
+                                         const TfOperands& G) {
+    static PerDeviceOnce once;
+    once.run([] { cudaFuncSetAttribute(conv_tf_kernel<GM, NT>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024); });
+    launch_pdl(conv_tf_kernel<GM, NT>, grid, dim3(TF_THREADS), smem, st, a, L, G);
+}
+
+template <int GM> void launch_any(int nth, dim3 grid, size_t smem, cudaStream_t st, const ConvArgs& a, const TfLaunch& L,
+                                  const TfOperands& G) {
+    switch (nth) {
+        case 32: launch_nt<GM, 32>(grid, smem, st, a, L, G); break;
+        case 64: launch_nt<GM, 64>(grid, smem, st, a, L, G); break;
+        default: launch_nt<GM, 96>(grid, smem, st, a, L, G); break;
+    }
 }
 
 uint32_t tf32_rn_host(float f) {        // round to nearest, ties away from zero (cvt.rna.tf32.f32)
@@ -496,7 +314,7 @@ uint32_t tf32_rn_host(float f) {        // round to nearest, ties away from zero
 bool conv_tf_plan_info(const ConvArgs& a, int* out) {
     TfLaunch L{}; size_t smem = 0;
     if (!plan(a, L, smem)) return false;
-    const int v[16] = {L.nth, L.wnth, L.ntiles_mp, L.ntiles_n, L.na, L.nw, L.chunk_kb, (int)smem, L.tmem_cols, L.win, 0, 0, 0, 0, 0, 0};
+    const int v[16] = {L.nth, L.wnth, L.ntiles_m, L.ntiles_n, TF_STAGES, L.chunk_kb, (int)smem, L.win, 0, 0, 0, 0, 0, 0, 0, 0};
     for (int i = 0; i < 16; i++) out[i] = v[i];
     return true;
 }
@@ -512,59 +330,29 @@ void launch_conv_tf(const ConvArgs& a, cudaStream_t st) {
 
 // plans ONCE and launches; false (nothing launched) when the shape is not supported
 bool try_launch_conv_tf(const ConvArgs& a, cudaStream_t st) {
-    static PerDeviceOnce once;
-    once.run([] {
-        cudaFuncSetAttribute(conv_tf_kernel<0>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
-        cudaFuncSetAttribute(conv_tf_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
-    });
     TfLaunch L; size_t smem;
-    CUtensorMap tmx;
-    if (!plan(a, L, smem) ||
-        !tensor_map_2d(&tmx, a.x, (unsigned long long)a.cin, (unsigned long long)a.rows_in, (unsigned long long)a.ldx, 32, (unsigned)L.win, true))
-        return false;
-    const int tiles = L.ntiles_mp * L.ntiles_n;
-    const int grid = tiles < tf_num_sms() ? tiles : tf_num_sms();
-    launch_pdl(conv_tf_kernel<0>, dim3(grid), dim3(TfCfg<0>::THREADS), smem, st, a, L, tmx, tmx, nullptr);
+    if (!plan(a, L, smem)) return false;
+    launch_any<0>(L.nth, dim3(L.ntiles_m * L.ntiles_n), smem, st, a, L, TfOperands{});
     g_launch_count++;
     check_launch("conv_tf");
     return true;
 }
 
 bool gemm_tf_supported(const TfGemm& g) {
-    if (!have_tensor_maps()) return false;
     if (g.nth != 96 && g.nth != 64 && g.nth != 32) return false;
-    auto al = [](const void* p, int ld, int a) { return p == nullptr || ((reinterpret_cast<uintptr_t>(p) & (a - 1)) == 0 && (ld & 3) == 0); };
-    return al(g.a, g.lda, 16) && al(g.b, g.ldb, 16) && al(g.y, g.ldy, 32) && (g.ldy & 7) == 0 && al(g.res, g.ldy, 32);
+    auto al = [](const void* p, int ld) { return p == nullptr || ((reinterpret_cast<uintptr_t>(p) & 15) == 0 && (ld & 3) == 0); };
+    return al(g.a, g.lda) && al(g.b, g.ldb);
 }
 
 void launch_gemm_tf(const TfGemm& g, cudaStream_t st) {
-    static PerDeviceOnce once;
-    once.run([] {
-        cudaFuncSetAttribute(conv_tf_kernel<0>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
-        cudaFuncSetAttribute(conv_tf_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
-    });
     if (g.ntiles <= 0) return;
     ConvArgs a{};
     a.in_slope = 1.f; a.ntaps = 1; a.cin = 32; a.cout = g.nth;
     a.y0 = g.y; a.ldy0 = g.ldy; a.res = g.res; a.ldres = g.ldy; a.scale = g.scale; a.split = g.nth; a.orow_mul = 1;
     TfLaunch L{};
-    L.nth = L.wnth = g.nth; L.win = 128; L.ntiles_mp = g.ntiles; L.ntiles_n = 1; L.chunk_kb = 2;
-    L.tmem_cols = 32;
-    while (L.tmem_cols < 4 * L.nth) L.tmem_cols <<= 1;
-    L.idesc = (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)(L.nth >> 3) << 17) | ((uint32_t)(128 >> 4) << 24);
-    const size_t a_img = 128 * 128, w_stage = (size_t)L.nth * 256;
-    const size_t bar_bytes = (3 * TF_NW_MAX + 6 * TF_NA_MAX + 8) * 8 + 16;
-    const size_t budget = TF_SMEM_BUDGET;
-    L.na = 2; L.nw = 2;
-    auto total = [&]() { return (size_t)2 * L.na * 2 * a_img + (size_t)L.nw * w_stage + bar_bytes; };
-    while (L.na < 3) { L.na++; if (total() > budget) { L.na--; break; } }     // one K-block = 12 MMAs: activation stages first
-    while (L.nw < 4) { L.nw++; if (total() > budget) { L.nw--; break; } }
-    CUtensorMap tma, tmb;
-    if (!tensor_map_2d(&tma, g.a, (unsigned long long)g.a_cols, (unsigned long long)g.a_rows, (unsigned long long)g.lda, 32, 128, true) ||
-        !tensor_map_2d(&tmb, g.b, (unsigned long long)g.b_cols, (unsigned long long)g.b_rows, (unsigned long long)g.ldb, 32, (unsigned)g.nth, true))
-        throw_launch_error("gemm_tf: tensor map encoding failed");
-    const int grid = g.ntiles < tf_num_sms() ? g.ntiles : tf_num_sms();
-    launch_pdl(conv_tf_kernel<1>, dim3(grid), dim3(TfCfg<1>::THREADS), total() + 1024, st, a, L, tma, tmb, g.tiles);
+    L.nth = L.wnth = g.nth; L.win = 128; L.ntiles_m = 2 * g.ntiles; L.ntiles_n = 1; L.chunk_kb = 2;
+    const TfOperands G{g.a, g.a_rows, g.a_cols, g.lda, g.b, g.b_rows, g.b_cols, g.ldb, g.tiles};
+    launch_any<1>(g.nth, dim3(2 * g.ntiles), smem_bytes(128, 1, g.nth) + 1024, st, a, L, G);
     g_launch_count++;
     check_launch("gemm_tf");
 }

@@ -126,7 +126,7 @@ Job* create_job(Voice* v, const long long* ids, const size_t* offs, size_t B, co
         // Small jobs (a single utterance): narrower column tiles put the same MMAs on more SMs (conv_tf.cu plan()); tile
         // width changes no summation order, so results do not depend on it.
         {
-            int sms = 148, dev = 0;
+            int sms = 132, dev = 0;
             if (cudaGetDevice(&dev) == cudaSuccess) cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
             long long wide_s = 0, wide_o = 0;
             for (size_t b = 0; b < B; b++) {
@@ -205,7 +205,7 @@ struct Runner {
         float* y1 = nullptr; int ldy1 = 0; int acc1 = 0;
         int orow_mul = 1, orow_add = 0;
         bool tc_ok = false;
-        bool tf_ok = false;    // duration-critical layer: tcgen05 3xTF32 with chunk-flushed accumulation (conv_tf.cu)
+        bool tf_ok = false;    // duration-critical layer: wgmma 3xTF32 with chunk-flushed accumulation (conv_tf.cu)
         float* yt = nullptr; int yt_col0 = 0, ldyt = 0;     // conv_tf only: column tiles >= yt_col0 stored transposed
     };
     // bias of a conv: the voice's, or this call's speaker-conditioned one (multi-speaker voices)
@@ -213,7 +213,7 @@ struct Runner {
     void conv(const ConvW& w, const float* x, int ldx, const Level& lin, const Opt& o) {
         ConvArgs p{};
         p.x = x; p.ldx = ldx; p.rows_in = lin.map.rows; p.cin = w.cin; p.in_slope = o.in_slope;
-        p.w = w.w; p.bias = bias_of(w); p.ldw = w.ldw; p.cout = w.cout; p.wtc = w.wtc; p.tc_nt = w.tc_nt; p.wcat = w.wcat; p.wtf = w.wtf;
+        p.w = w.w; p.bias = bias_of(w); p.ldw = w.ldw; p.cout = w.cout; p.wtc = w.wtc; p.tc_nt = w.tc_nt; p.wtf = w.wtf;
         p.ntaps = w.ntaps; memcpy(p.tap_off, w.tap_off, sizeof(p.tap_off)); p.min_off = w.min_off; p.span = w.span;
         p.rows_q = lin.map.rows; p.orow_mul = o.orow_mul; p.orow_add = o.orow_add;
         p.map = lin.map;
@@ -222,7 +222,7 @@ struct Runner {
         p.y1 = o.y1; p.ldy1 = o.ldy1; p.acc1 = o.acc1;
         p.yt = o.yt; p.yt_col0 = o.yt_col0; p.ldyt = o.ldyt;
 
-        // backend 1 (default): tcgen05 everywhere; 2: tcgen05 flow / decoder, fp32 CUDA cores for the text encoder and
+        // backend 1 (default): wgmma everywhere; 2: wgmma flow / decoder, fp32 CUDA cores for the text encoder and
         // the duration predictor (the round-1 configuration, kept for A/B runs); 0: fp32 CUDA cores everywhere
         // (each try_launch plans once and returns false without launching when the shape is not supported)
         if (v.backend == 1 && o.tf_ok && try_launch_conv_tf(p, st)) {}
@@ -290,7 +290,7 @@ void run_decoder(Runner& R, const Level& LY, const float* s, float* d_wav, const
         R.begin("dec.up" + std::to_string(i));
         bool fused_done = false;
         if (v.backend >= 1 && st.fused.wtc) {
-            // tcgen05 path: all u phases in one launch (input read once, N = u*cout columns)
+            // tensor-core path: all u phases in one launch (input read once, N = u*cout columns)
             ConvArgs pa{};
             pa.x = cur; pa.ldx = st.cin; pa.rows_in = Lin.map.rows; pa.cin = st.cin; pa.in_slope = 0.1f;
             pa.w = nullptr; pa.bias = st.fused.bias; pa.ldw = st.fused.ldw; pa.cout = st.fused.cout;
@@ -521,7 +521,7 @@ void Job::run(float* d_out, size_t d_out_cap) {
 
     // ---------------- text encoder ----------------
     // Every contraction here reaches the duration predictor, and ceil(duration) is a cliff: the dense layers and the two
-    // attention contractions run on conv_tf.cu (tcgen05, error-compensated tf32, chunk-flushed accumulation: fp32-class
+    // attention contractions run on conv_tf.cu (wgmma, error-compensated tf32, chunk-flushed accumulation: fp32-class
     // accuracy, DESIGN.md section 4); backend 0 / 2 keep them on the fp32 CUDA-core kernels.
     R.begin("enc");
     launch_embed(d_ids_rows, V.emb, sqrtf((float)H), xa, RX, H, st);

@@ -48,8 +48,7 @@ struct Arch {
 struct ConvW {
     float* w = nullptr;
     float* bias = nullptr;
-    float* wtc = nullptr; int tc_nt = 0;     // tcgen05 hi/lo swizzled weight images
-    float* wcat = nullptr;                   // hi/lo-stacked tap-pair images (conv_tc.cu cat mode), column tiles <= 64
+    float* wtc = nullptr; int tc_nt = 0;     // bf16 hi/lo swizzled weight images (conv_tc.cu)
     float* wtf = nullptr;                    // tf32 hi/lo images (conv_tf.cu): text-encoder / duration-predictor layers
     int cin = 0, cout = 0, ldw = 0, ntaps = 0;
     int cond_off = -1;                       // multi-speaker voices: offset of this conv's per-call effective bias (Job::d_cond)
@@ -62,7 +61,7 @@ struct DDSW { float* wdw[3]; float* bdw[3]; ConvW c1x1[3]; float *g1[3], *b1[3],
 struct CFlowW { float* pre_w; float* pre_b; DDSW dds; ConvW proj; int ccol, tcol; };
 struct CouplingW { ConvW pre; std::vector<ConvW> in, rs; ConvW post; int cond_off, tgt_off; };
 struct ResBW { int k; std::vector<int> dils; std::vector<ConvW> c1, c2; };
-struct UpStageW { int u, k, cin, cout; std::vector<ConvW> phase; ConvW fused; std::vector<ResBW> res; };   // fused: all phases as one N = u*cout conv (tcgen05 path)
+struct UpStageW { int u, k, cin, cout; std::vector<ConvW> phase; ConvW fused; std::vector<ResBW> res; };   // fused: all phases as one N = u*cout conv (tensor-core path)
 
 struct SynthConfig { long long speaker = 0; bool has_speaker = false; float noise_scale = 0.667f, length_scale = 1.f, noise_w = 0.8f; };
 
@@ -102,8 +101,8 @@ struct Voice {
     int c_last = 0;
     size_t weight_bytes = 0;
 
-    int backend = 1;                // 1 (default): tcgen05 everywhere (bf16x2 split for flow + decoder, chunk-flushed 3xTF32 for the text
-                                    // encoder + duration predictor); 2: tcgen05 flow + decoder, fp32 CUDA cores for encoder + predictor;
+    int backend = 1;                // 1 (default): wgmma everywhere (bf16x2 split for flow + decoder, chunk-flushed 3xTF32 for the text
+                                    // encoder + duration predictor); 2: wgmma flow + decoder, fp32 CUDA cores for encoder + predictor;
                                     // 0: fp32 CUDA cores everywhere
     unsigned long long noise_seed = 0x5eed5eedULL;
     std::mutex pool_mu;

@@ -1,4 +1,4 @@
-// Non-GEMM stages of the Piper/VITS path as sm_100a kernels: embedding, channel LayerNorm
+// Non-GEMM stages of the Piper/VITS path as sm_90a kernels: embedding, channel LayerNorm
 // (warp-shuffle reductions), DDSConv depthwise stage, relative-position attention, the
 // duration-predictor spline flow, the duration ceil/scan, the monotonic-alignment expansion
 // (generate_path restated as a gather), conv_post+tanh and the Philox noise source.

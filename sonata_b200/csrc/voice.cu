@@ -79,7 +79,7 @@ int tc_tile_for(int cout) {
     return 0;
 }
 
-// tcgen05 weight images for a finished ConvW whose [ntaps][cin][ldw] host copy is `wt`
+// tensor-core weight images for a finished ConvW whose [ntaps][cin][ldw] host copy is `wt`
 void add_tc_images(Uploader& U, ConvW& c, const std::vector<float>& wt) {
     if (c.cin % 32 || c.cout % 32) return;
     if (U.want_tf && c.ldw >= c.cout) {
@@ -96,11 +96,6 @@ void add_tc_images(Uploader& U, ConvW& c, const std::vector<float>& wt) {
     conv_tc_build_weights(wt.data(), c.ldw, c.cin, c.cout, c.ntaps, nt, img.data());
     c.wtc = U.up(img);
     c.tc_nt = nt;
-    if (nt <= 64) {
-        std::vector<float> cat(conv_tc_cat_weight_floats(c.cin, c.cout, c.ntaps, nt));
-        conv_tc_build_weights_cat(wt.data(), c.ldw, c.cin, c.cout, c.ntaps, nt, cat.data());
-        c.wcat = U.up(cat);
-    }
 }
 
 // Conv1d weight [cout][cin][k] (+bias) -> ConvW with taps (t - (k-1)/2) * dil.

@@ -1,7 +1,7 @@
 """Piper voice import: ONNX initialisers -> the SVW weight container the library loads (SURVEY §8f row N1).
 
 The reference loads a voice as `<name>.onnx` + `<name>.onnx.json` (crates/sonata/models/piper/src/lib.rs:88-110) and
-hands the graph to onnxruntime.  This module reads only what the B200 path needs from such a file -- the graph's
+hands the graph to onnxruntime.  This module reads only what the CUDA path needs from such a file -- the graph's
 INITIALISERS (the trained tensors) -- with a small protobuf wire-format reader (no `onnx` package offline), maps them
 onto the parameter names of Piper's `SynthesizerTrn` (the names `voicegen.tensor_specs` uses), folds weight
 normalisation where the export kept it (`weight_g`, `weight_v` or `parametrizations.weight.original0/1`), checks every

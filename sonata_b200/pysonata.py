@@ -1,5 +1,5 @@
 """`pysonata`-shaped binding (SURVEY §8f row N4): the classes and method names of the reference's pyo3 module
-(crates/frontends/python/src/lib.rs:43-457) over the B200 engine, so a script written against `pysonata` runs
+(crates/frontends/python/src/lib.rs:43-457) over the H100 engine, so a script written against `pysonata` runs
 with `import sonata_b200.pysonata as pysonata`.
 
     Sonata.with_piper(PiperModel(cfg)).synthesize_parallel(text, AudioOutputConfig(volume=80))  -> WaveSamples ...

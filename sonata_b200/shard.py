@@ -210,7 +210,7 @@ class Frontend:
       all    : per-utterance sample counts  --NCCL all-reduce (n int64)-->  exact layout of the result segment
       rank r : device -> host copy of its waveforms straight into ITS SLICE of a page-locked host segment shared by
                all ranks -- N PCIe links in parallel instead of funnelling every GPU's audio through rank 0
-               (NCCL gather + one copy: 80k audio-s/s at N = 8 against 174k for per-rank buffers, profiles/notes_r01.md)
+               (NCCL gather + one copy)
       rank 0 : after a barrier, reads every waveform from the same pages (zero-copy numpy views)
 
     `pcm16=True` delivers peak-normalised i16 PCM converted on the device (`to_i16_vec`, samples.rs:51-75): what

@@ -9,7 +9,7 @@ if ROOT not in sys.path:
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on an H100)")
 
 
 def pytest_collection_modifyitems(config, items):
@@ -21,7 +21,7 @@ def pytest_collection_modifyitems(config, items):
         has_gpu = False
     if has_gpu:
         return
-    skip = pytest.mark.skip(reason="no CUDA device visible (gpu-marked tests run on the B200 box)")
+    skip = pytest.mark.skip(reason="no CUDA device visible (gpu-marked tests need an H100)")
     for it in items:
         if "gpu" in it.keywords:
             it.add_marker(skip)

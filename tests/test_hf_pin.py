@@ -25,7 +25,7 @@ from sonata_b200 import PiperSynthesisConfig, voicegen  # noqa: E402
 
 HF_GOLD = sorted(glob.glob(os.path.join(HERE, "golden", "hf", "*.npz")))
 TOL_ORACLE = 2e-5       # fp32 vs fp32, different operation order (measured 2e-6 .. 4e-6)
-TOL_WAV = 1e-3          # BASELINE.json: "waveform max-abs error <1e-3" (measured: see profiles/notes_r02.md)
+TOL_WAV = 1e-3          # BASELINE.json: "waveform max-abs error <1e-3"
 
 
 def _weights_crc(t):

@@ -98,7 +98,7 @@ CASES = [
     (128 * 299, 128, 128, 7, 1, 0.1, 0, True, 1.0, False, None),
 ]
 
-# backend 2 = conv_tf.cu (tcgen05 3xTF32 with chunk-flushed accumulation; the text-encoder / duration-predictor
+# backend 2 = conv_tf.cu (wgmma 3xTF32 with chunk-flushed accumulation; the text-encoder / duration-predictor
 # layers): fp32-class accuracy is the point, so these cases are held to TF_TOL against the fp64 reference (the fp32
 # FMA chain of backend 0 measures 2e-6 .. 1e-5 on the same cases).  Shapes: every (cin, cout, k) of the encoder and
 # the duration predictor, all three column tiles (96 / 64 / 32), ragged row counts (odd number of 128-row tiles in

@@ -1,8 +1,7 @@
 """CPU emulation of tensor-core accumulation error, to decide whether the text encoder / duration predictor can leave
 the fp32 CUDA cores (round-2 planning; see DESIGN.md §4: `ceil(exp(logw))` is a cliff).
 
-Model (calibrated against one hardware measurement, profiles/notes_r01.md item 4: a K = 2816 contraction through the
-bf16x2 tcgen05 path showed 7.7e-5 max error where fp32 FMA shows 7e-6):
+Model (to be checked against a run of tools/conv_unit.py on the target GPU):
   * operands are rounded to the MMA's input format (bf16: 8 significant bits, tf32: 11) and split v = hi + lo;
   * one MMA adds an EXACT partial sum of its K-step (16 products for bf16, 8 for tf32) to the fp32 accumulator and the
     accumulator is rounded TOWARD ZERO (`--acc rn` switches to round-to-nearest for comparison);
