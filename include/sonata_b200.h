@@ -161,7 +161,9 @@ void sb200_latent_free(sb200_latent* z);
 
 /* ---- introspection for tests / bench ---- */
 /* Copy a named intermediate of the LAST run of `job` to host (time-major fp32, valid rows of
- * utterance b only).  Names: "x","stats","logw","z_p","z","dec.pre","dec.up<i>","dec.mrf<i>".
+ * utterance b only).  Names: "x","stats","logw","z_p","z","dec.pre","dec.up<i>","dec.mrf<i>", and the first encoder
+ * layer's attention "qkv0","att0"; on the tensor-core attention also "p0" (head-0 probabilities) and "vt0" (V, returned
+ * channel-major as [hidden][T]).
  * Returns rows via *rows, cols via *cols; data malloc'ed (free with sb200_buffer_free). */
 int32_t sb200_job_debug_fetch(sb200_job* job, const char* name, size_t b, float** data, size_t* rows, size_t* cols,
                               sb200_error* err);
@@ -178,19 +180,28 @@ typedef struct sb200_region_stat {
 } sb200_region_stat;
 /* region statistics of the last run of `job`; returns the number written (<= cap) */
 int32_t sb200_job_profile(const sb200_job* job, sb200_region_stat* out, int32_t cap);
-/* one convolution on caller data through either backend (kernel unit tests):
- * y[rows][cout] (=|+=) scale * (act(bias + conv_k,dil(lrelu_slope(x))) + res); w is [cout][cin][k];
- * act 0 none, 1 relu, 2 tanh*sigmoid gate (y is [rows][cout/2]); rows >= valid_rows are masked. */
 /* Test hook: the launch configuration the planner of backend 1 (wgmma bf16x2 conv) / 2 (wgmma 3xTF32 conv) would choose
  * for one convolution of `rows` output rows -- nothing is allocated or launched, so it also works without a GPU.
  * out16, backend 1: {nt, image rows, m-tiles, n-tiles, ring stages, smem bytes, window rows, 0...}; backend 2: {nth, image
  * rows, m-tiles, n-tiles, ring stages, chunk K-blocks, smem bytes, window rows, 0...}.  Returns 0, or 19 if unsupported. */
 int32_t sb200_debug_plan(int32_t backend, int64_t rows, int32_t cin, int32_t cout, int32_t k, int32_t dil, int32_t act,
                          int32_t has_res, int32_t accumulate, int32_t* out16);
+/* one convolution on caller data through backend 0 (fp32 CUDA cores), 1 (wgmma bf16x2) or 2 (wgmma 3xTF32), for kernel
+ * unit tests: y[rows][cout] (=|+=) scale * (act(bias + conv_k,dil(lrelu_slope(x))) + res); w is [cout][cin][k];
+ * act 0 none, 1 relu, 2 tanh*sigmoid gate (y is [rows][cout/2]); rows >= valid_rows are masked. */
 int32_t sb200_debug_conv(int32_t device, int32_t backend, const float* x, int32_t rows, int32_t cin, const float* w,
                          const float* bias, int32_t cout, int32_t k, int32_t dil, float in_slope, int32_t act,
                          const float* res, float scale, int32_t accumulate, float* y, int32_t valid_rows,
                          sb200_error* err);
+/* sb200_debug_conv with the engine's full row map and both output buffers.  Row q is valid iff
+ * q < seg_end[q / gran] * seg_mul (seg_end has one entry per granule of `rows`, as the engine's segment tables); invalid
+ * rows come out 0, or keep y's contents where that buffer accumulates.  Output columns n < split go to
+ * y0[rows][min(split, cout or cout/2)] (accumulated when acc0), the rest to y1[rows][cout - split] (when acc1);
+ * split = cout (or < 0) means y0 only. */
+int32_t sb200_debug_conv_ex(int32_t device, int32_t backend, const float* x, int32_t rows, int32_t cin, const float* w,
+                            const float* bias, int32_t cout, int32_t k, int32_t dil, float in_slope, int32_t act,
+                            const float* res, float scale, const int32_t* seg_end, int32_t gran, int32_t seg_mul,
+                            float* y0, int32_t acc0, int32_t split, float* y1, int32_t acc1, sb200_error* err);
 /* kernels launched by this library since load (host-side counter) */
 uint64_t sb200_launch_count(void);
 /* select the contraction backend: 0 = fp32 CUDA-core implicit GEMM, 1 = wgmma (3xTF32) where

@@ -4,6 +4,7 @@
 #include "../../include/sonata_b200.h"
 #include "engine.h"
 #include "tc_common.cuh"
+#include <algorithm>
 #include <chrono>
 #include <cstring>
 #include <deque>
@@ -355,10 +356,15 @@ int32_t sb200_job_debug_fetch(sb200_job* job, const char* name, size_t b, float*
         const int U = j.dbg_level[name];
         const int C = it->second.second;
         size_t r0, nr;
-        if (U == 0) { r0 = (size_t)j.xsegs[b].off; nr = (size_t)j.xsegs[b].len; }
+        if (U <= 0) { r0 = (size_t)j.xsegs[b].off; nr = (size_t)j.xsegs[b].len; }
         else { r0 = (size_t)j.fsegs[b].off * U; nr = (size_t)j.fsegs[b].len * U; }
         *data = (float*)malloc(nr * C * 4 + 4);
         SB_CUDA(cudaSetDevice(j.v->device));
+        if (U < 0) {        // transposed [C][RX]: the utterance's columns of every row -> [C][len]
+            SB_CUDA(cudaMemcpy2D(*data, nr * 4, it->second.first + r0, (size_t)j.RX * 4, nr * 4, (size_t)C, cudaMemcpyDeviceToHost));
+            *rows = (size_t)C; *cols = nr;
+            return;
+        }
         SB_CUDA(cudaMemcpy(*data, it->second.first + r0 * C, nr * C * 4, cudaMemcpyDeviceToHost));
         *rows = nr; *cols = (size_t)C;
     });
@@ -411,32 +417,45 @@ int32_t sb200_debug_plan(int32_t backend, int64_t rows, int32_t cin, int32_t cou
     return ok ? 0 : 19;
 }
 
-int32_t sb200_debug_conv(int32_t device, int32_t backend, const float* x, int32_t rows, int32_t cin, const float* w,
-                         const float* bias, int32_t cout, int32_t k, int32_t dil, float in_slope, int32_t act,
-                         const float* res, float scale, int32_t accumulate, float* y, int32_t valid_rows,
-                         sb200_error* err) {
+int32_t sb200_debug_conv_ex(int32_t device, int32_t backend, const float* x, int32_t rows, int32_t cin, const float* w,
+                            const float* bias, int32_t cout, int32_t k, int32_t dil, float in_slope, int32_t act,
+                            const float* res, float scale, const int32_t* seg_end, int32_t gran, int32_t seg_mul,
+                            float* y0, int32_t acc0, int32_t split, float* y1, int32_t acc1, sb200_error* err) {
     return guarded(err, [&] {
+        if (rows <= 0 || gran <= 0 || seg_mul <= 0 || !seg_end) throw Error(19, "debug conv: bad row map");
+        if (split < 0 || split > cout) split = cout;
+        if (split < cout && (act == ACT_GATE || !y1)) throw Error(19, "debug conv: a split output needs y1 and no gate");
         SB_CUDA(cudaSetDevice(device));
         Voice tmp; tmp.device = device;
         ConvW cw = debug_make_conv(tmp, w, bias, cout, cin, k, dil);
         const int R = (rows + 255) / 256 * 256;
         const int ycols = act == ACT_GATE ? cout / 2 : cout;
-        float *dx, *dy, *dres = nullptr; int* dend;
+        const int ld0 = std::min(split, ycols), ld1 = cout - split;    // y0 [rows][ld0], y1 [rows][ld1]
+        const int ngran = (R + gran - 1) / gran;
+        std::vector<int> ends(ngran, 0);                                // granules past the caller's table: all gap rows
+        for (int g = 0; g < ngran && g * gran < rows; g++) ends[g] = seg_end[g];
+        float *dx, *dy0 = nullptr, *dy1 = nullptr, *dres = nullptr; int* dend;
         SB_CUDA(cudaMalloc(&dx, (size_t)R * cin * 4)); SB_CUDA(cudaMemset(dx, 0, (size_t)R * cin * 4));
         SB_CUDA(cudaMemcpy(dx, x, (size_t)rows * cin * 4, cudaMemcpyHostToDevice));
-        SB_CUDA(cudaMalloc(&dy, (size_t)R * ycols * 4)); SB_CUDA(cudaMemset(dy, 0, (size_t)R * ycols * 4));
-        SB_CUDA(cudaMemcpy(dy, y, (size_t)rows * ycols * 4, cudaMemcpyHostToDevice));
+        auto upload_y = [&](float*& d, const float* h, int ld) {
+            if (ld <= 0) return;
+            SB_CUDA(cudaMalloc(&d, (size_t)R * ld * 4)); SB_CUDA(cudaMemset(d, 0, (size_t)R * ld * 4));
+            SB_CUDA(cudaMemcpy(d, h, (size_t)rows * ld * 4, cudaMemcpyHostToDevice));
+        };
+        upload_y(dy0, y0, ld0);
+        upload_y(dy1, y1, ld1);
         if (res) { SB_CUDA(cudaMalloc(&dres, (size_t)R * cout * 4)); SB_CUDA(cudaMemset(dres, 0, (size_t)R * cout * 4));
                    SB_CUDA(cudaMemcpy(dres, res, (size_t)rows * cout * 4, cudaMemcpyHostToDevice)); }
-        SB_CUDA(cudaMalloc(&dend, 4)); SB_CUDA(cudaMemcpy(dend, &valid_rows, 4, cudaMemcpyHostToDevice));
+        SB_CUDA(cudaMalloc(&dend, (size_t)ngran * 4)); SB_CUDA(cudaMemcpy(dend, ends.data(), (size_t)ngran * 4, cudaMemcpyHostToDevice));
         ConvArgs p{};
         p.x = dx; p.ldx = cin; p.rows_in = R; p.cin = cin; p.in_slope = in_slope;
         p.w = cw.w; p.bias = cw.bias; p.ldw = cw.ldw; p.cout = cw.cout; p.wtc = cw.wtc; p.tc_nt = cw.tc_nt;
         p.ntaps = cw.ntaps; memcpy(p.tap_off, cw.tap_off, sizeof(p.tap_off)); p.min_off = cw.min_off; p.span = cw.span;
         p.rows_q = R; p.orow_mul = 1; p.orow_add = 0;
-        p.map = RowMap{dend, R, 1, R};
+        p.map = RowMap{dend, gran, seg_mul, R};
         p.act = act; p.scale = scale; p.res = dres; p.ldres = cout;
-        p.y0 = dy; p.ldy0 = ycols; p.acc0 = accumulate; p.split = cout; p.y1 = dy; p.ldy1 = ycols; p.acc1 = accumulate;
+        p.y0 = dy0 ? dy0 : dy1; p.ldy0 = dy0 ? ld0 : ld1; p.acc0 = acc0; p.split = split;
+        p.y1 = dy1 ? dy1 : dy0; p.ldy1 = dy1 ? ld1 : ld0; p.acc1 = acc1;
         if (res && getenv("SB200_DEBUG_RES_IS_X") && cin == cout) { p.res = dx; p.ldres = cin; }   // ResBlock aliasing (timing only)
         p.wtf = cw.wtf;
         if (backend == 2) {
@@ -447,10 +466,24 @@ int32_t sb200_debug_conv(int32_t device, int32_t backend, const float* x, int32_
             launch_conv_tc(p, 0);
         } else launch_conv_simt(p, 0);
         cudaError_t e = cudaDeviceSynchronize();
-        if (e == cudaSuccess) e = cudaMemcpy(y, dy, (size_t)rows * ycols * 4, cudaMemcpyDeviceToHost);
-        cudaFree(dx); cudaFree(dy); cudaFree(dend); if (dres) cudaFree(dres);
+        if (e == cudaSuccess && dy0) e = cudaMemcpy(y0, dy0, (size_t)rows * ld0 * 4, cudaMemcpyDeviceToHost);
+        if (e == cudaSuccess && dy1) e = cudaMemcpy(y1, dy1, (size_t)rows * ld1 * 4, cudaMemcpyDeviceToHost);
+        cudaFree(dx); cudaFree(dend);
+        if (dy0) cudaFree(dy0);
+        if (dy1) cudaFree(dy1);
+        if (dres) cudaFree(dres);
         if (e != cudaSuccess) throw Error(19, std::string("CUDA error: ") + cudaGetErrorString(e));
     });
+}
+
+int32_t sb200_debug_conv(int32_t device, int32_t backend, const float* x, int32_t rows, int32_t cin, const float* w,
+                         const float* bias, int32_t cout, int32_t k, int32_t dil, float in_slope, int32_t act,
+                         const float* res, float scale, int32_t accumulate, float* y, int32_t valid_rows,
+                         sb200_error* err) {
+    // one segment [0, valid_rows): a single granule spanning the whole (256-row padded) launch
+    const int32_t R = (rows + 255) / 256 * 256;
+    return sb200_debug_conv_ex(device, backend, x, rows, cin, w, bias, cout, k, dil, in_slope, act, res, scale, &valid_rows,
+                               R, 1, y, accumulate, cout, nullptr, accumulate, err);
 }
 
 uint64_t sb200_launch_count(void) { return g_launch_count; }

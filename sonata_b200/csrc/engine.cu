@@ -417,7 +417,7 @@ void Job::run(float* d_out, size_t d_out_cap) {
                            (tc_att ? (size_t)a.heads * RX * att_tp + 2 * (size_t)RX * H : 0);
     const size_t tile_bytes = (tiles_s.size() + tiles_o.size()) * sizeof(TfTile);
     const size_t p1_bytes = xfloats * 4 + (size_t)RX * 20 + B * 64 + tile_bytes + (1 << 20) + (size_t)V.cond_rows * 4 + 1024 +
-                            (debug ? (size_t)RX * (4 * H + att_tp) * 4 + 4096 : 0);
+                            (debug ? (size_t)RX * (5 * H + att_tp) * 4 + 4096 : 0);
     // The arena must also hold phase 2; sizes are only known after the durations come back, so phase 1
     // runs in the front of the arena and phase 2 re-plans behind it (growing = realloc would lose phase-1
     // results, so grow conservatively up front from the mean-duration estimate, then verify).
@@ -543,7 +543,7 @@ void Job::run(float* d_out, size_t d_out_cap) {
             launch_attention(qkv, 3 * H, e.relk, e.relv, a.window, att, H, H, a.heads, d_xsegs, (int)B, max_tx, st);
         }
         { double f = 0; for (auto& s : xsegs) f += 4.0 * (double)s.len * s.len * H; R.count(f, 16.0 * LX.valid_rows * H); }
-        if (debug && l == 0) {      // first-layer attention operands / result (tools/debug_att.py)
+        if (debug && l == 0) {      // first-layer attention operands / result (tests/test_gpu_parity.py)
             float* qk = C.dev.get<float>((size_t)RX * 3 * H);
             float* at = C.dev.get<float>((size_t)RX * H);
             SB_CUDA(cudaMemcpyAsync(qk, qkv, (size_t)RX * 3 * H * 4, cudaMemcpyDeviceToDevice, st));
@@ -553,6 +553,10 @@ void Job::run(float* d_out, size_t d_out_cap) {
                 float* sp = C.dev.get<float>((size_t)RX * att_tp);
                 SB_CUDA(cudaMemcpyAsync(sp, att_s, (size_t)RX * att_tp * 4, cudaMemcpyDeviceToDevice, st));
                 dbg["p0"] = {sp, att_tp}; dbg_level["p0"] = 0;     // head 0 probabilities
+                // V went only to att_vt (the V columns of qkv0 are not written on this path): captured as [H][RX]
+                float* vt = C.dev.get<float>((size_t)H * RX);
+                SB_CUDA(cudaMemcpyAsync(vt, att_vt, (size_t)H * RX * 4, cudaMemcpyDeviceToDevice, st));
+                dbg["vt0"] = {vt, H}; dbg_level["vt0"] = -1;
             }
         }
         { Runner::Opt o; o.y0 = xb; o.ldy0 = H; o.tf_ok = true; R.conv(e.o, att, H, LX, o); }

@@ -181,7 +181,8 @@ struct Job {
     float* d_wav = nullptr; bool wav_external = false;
     float* d_cond = nullptr;       // effective biases of the speaker-conditioned convs for this call
     std::map<std::string, std::pair<float*, int>> dbg;   // name -> (device ptr, cols)
-    std::map<std::string, int> dbg_level;                // name -> U (rows per frame) or 0 for X level
+    std::map<std::string, int> dbg_level;                // name -> U (rows per frame), 0 for X level, -1 for an X-level
+                                                         // buffer stored transposed ([cols][RX])
     std::vector<Region> regions;
     float last_ms = 0;
     bool ran = false;

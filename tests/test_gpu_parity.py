@@ -182,13 +182,69 @@ def test_unscreened_duration_flips_are_cliff_cases():
 @pytest.mark.parametrize("backend", [1, 0], ids=BACKEND_IDS)
 def test_conv_kernels_against_torch(backend, lib_built):
     """Kernel-level unit check of both contraction backends (same ConvArgs contract): 1x1 / dilated k-tap,
-    leaky-ReLU prologue, gate / ReLU / residual / scale / accumulate epilogues, masked rows, and the
-    multi-tile path of the wgmma kernel (many 128-row tiles, narrow and wide column tiles)."""
+    leaky-ReLU prologue, gate / ReLU / residual / scale / accumulate epilogues, masked rows (exactly 0, or untouched
+    under accumulate), and launches of the wgmma kernel on both sides of each tile-narrowing edge."""
     from conv_unit import CASES, run_case
     for c in CASES:
         err, msg = run_case(backend, *c)
         assert err is not None, (c, msg)
         assert err < 1e-4, (c, err)
+
+
+def _supported(backend, cin, cout, k, dil, act, res, acc):
+    if backend == 0:
+        return True
+    import ctypes
+    from sonata_b200 import _native
+    o = (ctypes.c_int32 * 16)()
+    return _native.lib().sb200_debug_plan(backend, 4096, cin, cout, k, dil, act, int(res), int(acc), o) == 0
+
+
+@pytest.mark.parametrize("backend", [1, 0, 2], ids=BACKEND_IDS + ["tf32x3"])
+def test_conv_multi_segment_row_map(backend, lib_built):
+    """Several segments with gap rows in one launch, through the engine's row map (segment end per granule, seg_mul rows
+    per frame at decoder levels): ragged ends inside a 128-row tile, a segment shorter than the conv's halo.  Gap rows
+    come out exactly 0, or keep their (non-zero) prior contents bit for bit under accumulate."""
+    from conv_unit import SEG_CASES, TF_TOL, run_segments
+    ran = 0
+    for lens, gran, seg_mul, cin, cout, k, dil, slope, act, res, scale, acc in SEG_CASES:
+        if not _supported(backend, cin, cout, k, dil, act, res, acc):
+            continue
+        err, gaps_ok = run_segments(backend, lens, gran, seg_mul, cin, cout, k, dil, slope, act, res, scale, acc)
+        assert gaps_ok, (lens, gran, seg_mul, cin, cout, k, acc)
+        assert err < (TF_TOL if backend == 2 else 1e-4), (lens, gran, seg_mul, cin, cout, k, err)
+        ran += 1
+    assert ran >= 3
+
+
+@pytest.mark.parametrize("backend", [1, 0, 2], ids=BACKEND_IDS + ["tf32x3"])
+def test_conv_split_outputs(backend, lib_built):
+    """The two-buffer epilogue of the flow's WaveNet res/skip layers: columns [0, H) accumulate into the residual
+    stream, [H, 2H) into the skip sum (written on the first layer, accumulated after), each half checked on its own.
+    The 3xTF32 kernel has no split epilogue (the encoder never splits): its planner must refuse the launch."""
+    from conv_unit import SPLIT_CASES, run_split
+    if backend == 2:
+        with pytest.raises(AssertionError, match="not supported"):
+            run_split(2, *SPLIT_CASES[0], 0)
+        return
+    for lens, H, k in SPLIT_CASES:
+        for acc1 in (0, 1):
+            (e0, g0), (e1, g1) = run_split(backend, lens, H, k, acc1)
+            assert g0 and g1, (lens, acc1, g0, g1)
+            assert e0 < 1e-4 and e1 < 1e-4, (lens, acc1, e0, e1)
+
+
+def test_conv_results_do_not_depend_on_tile_width(lib_built):
+    """Bit-identity across tile widths at kernel level: each flow / decoder shape (bf16x2) and encoder shape (3xTF32) runs
+    once per column-tile width its planner can choose (row counts found by asking the planner, on this device's SM
+    count), the larger launches fed the same leading rows.  Every output row whose receptive field lies inside all
+    inputs must be bitwise equal: a wgmma m64nNk16 / k8 gives an output element the same bits at every N."""
+    from conv_unit import WIDTH_CASES, width_invariance
+    for case in WIDTH_CASES:
+        launches, res = width_invariance(*case)
+        assert len(launches) >= 2, (case, launches)
+        for nt, rows, same in res:
+            assert same, (case, launches, nt, rows)
 
 
 def test_conv_tf_kernel_fp32_class_accuracy(lib_built):
@@ -200,6 +256,143 @@ def test_conv_tf_kernel_fp32_class_accuracy(lib_built):
         err, msg = run_case(2, *c)
         assert err is not None, (c, msg)
         assert err < TF_TOL, (c, err)
+
+
+def _ids_of_length(n, utt):
+    """n ids (any n, odd included): a synthetic utterance cut to length."""
+    return workload.synthetic_ids(n // 2 + 1, utt=utt)[:n]
+
+
+def _attention_job(m, lens, simt, monkeypatch):
+    """Layer-0 attention captures of one job on the medium voice (debug run), per utterance."""
+    if simt:
+        monkeypatch.setenv("SB200_ATT_SIMT", "1")
+    else:
+        monkeypatch.delenv("SB200_ATT_SIMT", raising=False)
+    ids = [_ids_of_length(n, 300 + i) for i, n in enumerate(lens)]
+    job = SynthesisJob(m, ids, debug=True)
+    job.run()
+    out = []
+    for b in range(len(ids)):
+        d = {k: job.debug_fetch(k, b) for k in ("qkv0", "att0", "x", "logw")}
+        for k in ("p0", "vt0"):
+            try:
+                d[k] = job.debug_fetch(k, b)
+            except sonata_b200.OperationError:
+                pass
+        d["ids"], d["cum"] = ids[b], job.durations(b)
+        out.append(d)
+    job.close()
+    monkeypatch.delenv("SB200_ATT_SIMT", raising=False)
+    return out
+
+
+# One job per softmax regime of the tensor-core attention (rows in 20 / 40 registers, kernels_misc.cu), lengths batched so
+# segment offsets and gap rows are exercised: T = 1, odd T, T = 32k +- 1 (the softmax zero-fills keys to the next multiple
+# of 32, the K extent of P.V), T <= 128 (the second 128-row m-tile of a tile pair has no valid row), T = 640 / 641; and
+# T = 1281, past the tensor-core attention's limit, on the fp32 attention.
+ATT_JOBS = {
+    "nreg20": (1, 2, 31, 32, 33, 63, 65, 97, 127, 128, 129, 255, 257, 639, 640),
+    "nreg40": (3, 95, 641, 1279, 1280),
+    "fp32_fallback": (1281, 33),
+}
+
+
+@pytest.mark.parametrize("regime", list(ATT_JOBS))
+def test_tensor_core_attention_against_fp64(regime, models, monkeypatch):
+    """Layer 0 of the text encoder on the default backend against float64 (tests/att_reference.py):
+    * q / k / v projection, V through its transposed store, against x0 . Wqkv^T + b at the 3xTF32 conv tolerance;
+    * the same job with SB200_ATT_SIMT=1 (V stored untransposed by the same conv kernel): Q / K and V bit for bit;
+    * att0 of the fp32 CUDA-core attention (the SB200_ATT_SIMT=1 run, and both runs of the job past 1280 ids, which
+      takes that kernel whatever the setting) against the fp64 attention of the kernel's own Q / K / V, within the
+      T-scaled fp32 bound att_reference.fp32_att_bound;
+    * att0 of the tensor-core attention, both heads, against the same reference, within
+      ATT_MULT x (the fp32 attention's error on the same inputs) + ATT_FLOOR x max|ref|;
+    * head-0 probabilities p0 against the fp64 softmax, within ATT_MULT x the error of a float32 softmax computed on the
+      host + ATT_FLOOR (absolute; probabilities are <= 1), zero keys [T, round_up(T, 32)), rows summing to 1 within a
+      T-scaled few ulp.  For p0 the floor is what binds: measured 0 .. 5.3e-7 against a float32 host error of
+      0 .. 1.5e-7, while a score GEMM on a single TF32 MMA or two of its three split products is off by 1e-4 or more.
+    att0 errors measured on an H100 SXM are listed beside ATT_MULT in tests/att_reference.py.  Run with -s to print the
+    per-utterance table."""
+    import att_reference as ar
+    from conv_unit import TF_TOL
+    m = models("medium"); _det(m)
+    lens = ATT_JOBS[regime]
+    t = voicegen.make_tensors("medium")
+    a = voicegen.ARCH["medium"]
+    H, heads, D = a["hidden"], a["heads"], a["hidden"] // a["heads"]
+    relk, relv = ar.rel_embeddings(t, 0)
+    tc = _attention_job(m, lens, False, monkeypatch)
+    simt = _attention_job(m, lens, True, monkeypatch)
+    on_tc = regime != "fp32_fallback"
+    report = []
+    for n, u, s in zip(lens, tc, simt):
+        assert u["qkv0"].shape == (n, 3 * H) and u["att0"].shape == (n, H)
+        assert ("vt0" in u) == on_tc and ("p0" in u) == on_tc
+        q, k = u["qkv0"][:, :H], u["qkv0"][:, H:2 * H]
+        v = u["vt0"].T if on_tc else u["qkv0"][:, 2 * H:]
+        _, refs = ar.project_qkv(t, 0, u["ids"])
+        for got, ref in zip((q, k, v), refs):
+            assert float(np.abs(got - ref).max()) < TF_TOL * max(1.0, float(np.abs(ref).max())), n
+        # transposed store: the fp32-attention run stores V untransposed through the same conv_tf kernel
+        assert np.array_equal(s["qkv0"][:, :2 * H], u["qkv0"][:, :2 * H]), n
+        assert np.array_equal(s["qkv0"][:, 2 * H:], v), n
+        Ps, ref = ar.attention(q, k, v, relk, relv, heads)
+        e_tc = float(np.abs(u["att0"] - ref).max())
+        e_simt = float(np.abs(s["att0"] - ref).max())
+        scale = float(np.abs(ref).max())
+        bound = ar.ATT_MULT * e_simt + ar.ATT_FLOOR * scale
+        row = {"T": n, "tc": e_tc, "simt": e_simt, "max_ref": scale, "bound": bound,
+               "simt_bound": ar.fp32_att_bound(n, scale)}
+        assert e_simt <= ar.fp32_att_bound(n, scale), row                             # the fp32 kernel on its own
+        assert on_tc or np.array_equal(u["att0"], s["att0"]), n                        # past 1280 ids: the same kernel
+        assert e_tc <= bound, row
+        if on_tc:
+            p0 = u["p0"]
+            tz = (n + 31) // 32 * 32
+            assert p0.shape[1] >= tz and not p0[:, n:tz].any(), n                    # zero-filled keys of the P.V K extent
+            sums = p0[:, :n].astype(np.float64).sum(1)
+            assert float(np.abs(sums - 1.0).max()) <= (n / 32 + 8) * 2.0 ** -23, (n, float(np.abs(sums - 1.0).max()))
+            P32, _ = ar.attention_head(*(np.asarray(x, dtype=np.float32)[:, :D] for x in (q, k, v)),
+                                       relk.astype(np.float32), relv.astype(np.float32))
+            e_p = float(np.abs(p0[:, :n] - Ps[0]).max())
+            e_p32 = float(np.abs(P32 - Ps[0]).max())
+            row.update(p0=e_p, p0_fp32=e_p32)
+            assert e_p <= ar.ATT_MULT * e_p32 + ar.ATT_FLOOR, row
+        report.append(row)
+    print(regime, "\n" + "\n".join(" ".join(f"{k}={v:.3g}" if isinstance(v, float) else f"{k}={v}" for k, v in r.items())
+                                   for r in report))
+
+
+def test_attention_bits_do_not_depend_on_batch(models):
+    """Utterances synthesised alone (both attention GEMMs on narrow column tiles: 32 keys / 32 head columns) and inside a
+    batch of 32 (64 / 96-column tiles, and wider conv tiles everywhere): att0, p0, x, logw and the durations are bitwise
+    equal.  The sizes sit far from the width switch of engine.cu create_job (checked below)."""
+    m = models("medium"); _det(m)
+    sms = torch.cuda.get_device_properties(0).multi_processor_count
+    lens = [202 + 2 * (u % 24) for u in range(32)]                   # 202 .. 248 ids
+    ids = [_ids_of_length(n, 400 + u) for u, n in enumerate(lens)]
+
+    def widths(ls):     # the attention GEMM tile widths create_job picks (2 heads, 96-wide)
+        ws = sum(2 * ((n + 255) // 256) * ((n + 63) // 64) for n in ls)
+        wo = sum(2 * ((n + 255) // 256) for n in ls)
+        return (32 if ws * 2 <= sms else 64), (32 if wo * 3 <= sms else 96), ws * 2 / sms, wo * 3 / sms
+    assert widths(lens)[:2] == (64, 96) and min(widths(lens)[2:]) > 1.3
+    job = SynthesisJob(m, ids, debug=True)
+    job.run()
+    for b in (0, 13, 31):
+        assert widths([lens[b]])[:2] == (32, 32) and max(widths([lens[b]])[2:]) < 0.5
+        solo = SynthesisJob(m, [ids[b]], debug=True)
+        solo.run()
+        tz = (lens[b] + 31) // 32 * 32
+        for name in ("att0", "p0", "x", "logw", "stats"):
+            x, y = job.debug_fetch(name, b), solo.debug_fetch(name, 0)
+            if name == "p0":
+                x, y = x[:, :tz], y[:, :tz]
+            assert np.array_equal(x, y), (b, name, float(np.abs(x - y).max()))
+        assert np.array_equal(job.durations(b), solo.durations(0)), b
+        solo.close()
+    job.close()
 
 
 def test_device_i16_matches_host_to_i16_vec(models):
@@ -228,7 +421,7 @@ def test_batched_equals_sequential(models):
     for b, ids in enumerate(batches):
         alone = m.infer_with_values(ids)
         assert len(alone) == len(together[b])
-        assert float(np.abs(alone.samples.as_slice() - together[b].samples.as_slice()).max()) < 1e-5
+        assert np.array_equal(alone.samples.as_slice(), together[b].samples.as_slice())     # DESIGN.md §4: same bits
 
 
 def test_speak_api_surface(models, oracle_weights):
@@ -284,8 +477,7 @@ def test_full_size_properties(models):
         assert np.isfinite(s).all() and np.abs(s).max() <= 1.0
     # utterance 5 of the big batch == the same utterance alone (batch-size independence)
     alone = m.infer_with_values(batches[5]).samples.as_slice()
-    assert alone.shape == auds[5].samples.as_slice().shape
-    assert float(np.abs(alone - auds[5].samples.as_slice()).max()) < 1e-5
+    assert np.array_equal(alone, auds[5].samples.as_slice())
     prof = {p["name"]: p for p in job.profile()}
     assert prof["dec.mrf2"]["launches"] == 6 and prof["dec.mrf2"]["ms"] > 0
     assert prof["dec.up2"]["launches"] == 1          # phase-fused ConvTranspose on the tensor-core backend

@@ -98,6 +98,52 @@ def test_relative_attention_matches_naive():
         assert torch.allclose(got, ref, atol=1e-5), T
 
 
+@pytest.mark.parametrize("n", [7, 300])
+def test_attention_reference_matches_oracle_mha(n):
+    """tests/att_reference.py (the fp64 reference the CUDA attention is held to) against the oracle's `_mha` on layer 0
+    of the medium voice: the band-by-band restatement and the oracle's rel_to_abs / abs_to_rel reshapes must agree, so
+    they cannot share a misreading of the relative-position indexing.  conv_o is applied to the reference in float64."""
+    import att_reference as ar
+    t = voicegen.make_tensors("medium")
+    a = voicegen.ARCH["medium"]
+    ids = vo.synthetic_ids(n // 2, utt=4)[:n]
+    x0, (q, k, v) = ar.project_qkv(t, 0, ids)
+    relk, relv = ar.rel_embeddings(t, 0)
+    Ps, out = ar.attention(q, k, v, relk, relv, a["heads"])
+    assert all(np.allclose(P.sum(1), 1.0, rtol=0, atol=1e-12) for P in Ps)
+    p = "enc_p.encoder.attn_layers.0."
+    wo = np.asarray(t[p + "conv_o.weight"], dtype=np.float64)[:, :, 0]
+    got = out @ wo.T + np.asarray(t[p + "conv_o.bias"], dtype=np.float64)
+    W64 = vo.to_torch(t, torch.float64)
+    ref = vo._mha(W64, p, torch.from_numpy(x0.T[None].copy()), a)[0].T.numpy()
+    assert got.shape == ref.shape == (n, a["hidden"])
+    assert float(np.abs(got - ref).max()) < 1e-10 * max(1.0, float(np.abs(ref).max()))
+
+
+def test_pv_emulation_places_degraded_splits_above_attention_bound():
+    """The accuracy bound of the tensor-core attention (att_reference.ATT_MULT x the fp32 kernel's error + a floor) is
+    tight enough to catch a degraded P.V contraction.  CPU emulation (tools/emu_tc_accuracy.py model) of head 0 of
+    layer 0 at T = 1280 keys, the longest utterance the tensor-core attention takes, with the fp32 kernel's summation
+    order standing in for the fp32 kernel: the 3xTF32 chunk-flushed contraction lands below the bound; a single TF32
+    MMA, two of the three split products, and the accumulation without the chunk flush each land above it.  Emulated
+    (max |err|, |P.V| <= 2.3): fp32 kernel order 5.3e-6 (5.3e-6 measured on an H100 at T = 1280), 3xTF32 flushed
+    1.8e-6, bound 1.5e-5; 1xTF32 1.3e-3, 2 products 8.3e-4, no flush 2.6e-5."""
+    import att_reference as ar
+    t = voicegen.make_tensors("medium")
+    ids = vo.synthetic_ids(640, utt=9)[:1280]
+    _, (q, k, v) = ar.project_qkv(t, 0, ids)
+    relk, relv = ar.rel_embeddings(t, 0)
+    D = q.shape[1] // voicegen.ARCH["medium"]["heads"]
+    P, _ = ar.attention_head(q[:, :D], k[:, :D], v[:, :D], relk, relv)
+    V = v[:, :D].astype(np.float32)
+    e = ar.emulated_pv_errors(P, V)
+    bound = ar.ATT_MULT * e["fp32_simt"] + ar.ATT_FLOOR * float(np.abs(P @ V).max())
+    print({key: f"{val:.2e}" for key, val in e.items()}, f"bound {bound:.2e}", f"max|P.V| {float(np.abs(P @ V).max()):.2f}")
+    assert e["3xtf32"] <= bound, (e, bound)
+    for degraded in ("1xtf32", "2_products", "no_flush"):
+        assert e[degraded] > bound, (degraded, e, bound)
+
+
 def _rqs_forward(x, uw, uh, ud, B=5.0):
     """transforms.rational_quadratic_spline(inverse=False), scalar restatement."""
     nb = len(uw)

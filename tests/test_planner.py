@@ -3,9 +3,10 @@ only, nothing is launched, so this runs without a GPU.
 
 The property that matters most: the reference's `speak_batch` is a loop of B=1 runs, and this implementation promises
 the same bits for an utterance whether it is synthesised alone or inside a batch (`test_batched_equals_sequential`,
-`test_frontends_on_the_device` check it on the device).  The planners pick tile widths from the launch SIZE -- which
-changes no summation order -- but the choice that DOES change arithmetic (the chunk length of the flushed
-accumulation) must depend on the layer's shape alone."""
+`test_frontends_on_the_device` check it on the device, with exact equality).  The planners pick tile widths from the
+launch SIZE -- which changes no summation order: a wgmma gives an output element the same bits at every N, which
+`test_conv_results_do_not_depend_on_tile_width` checks on the device for each width -- but the choice that DOES change
+arithmetic (the chunk length of the flushed accumulation) must depend on the layer's shape alone."""
 import ctypes as C
 
 import pytest
@@ -78,6 +79,23 @@ def test_arithmetic_class_does_not_depend_on_launch_size(q):
             if nth < wnth:
                 assert mt * (lay[1] // 32) <= SMS or not two_stages_fit(win, lay[2], wnth, 2), (lay, rows, p)
         assert len(chunks) == 1, (lay, chunks)
+
+
+def test_tile_width_cases_reach_several_widths():
+    """The device-side bit-identity check (tools/conv_unit.py WIDTH_CASES) launches each shape once per tile width the
+    planner picks over launch sizes: every shape must reach at least two widths, the narrowest being 32 columns, and
+    the narrowing edges the kernel cases straddle must be where the planner switches."""
+    import os
+    import sys
+    sys.path.insert(0, os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "tools"))
+    import conv_unit as cu
+    for case in cu.WIDTH_CASES:
+        w = cu.tile_width_launches(*case)
+        assert len(w) >= 2 and min(w) == 32, (case, w)
+    for cout, nt, lay in ((64, 32, (64, 64, 7, 12, ACT_NONE, 1, 1)), (384, 32, (192, 384, 5, 1, ACT_GATE, 0, 0)),
+                          (256, 32, (256, 256, 11, 5, ACT_NONE, 1, 0))):
+        e = cu.narrow_edge(cout, nt)
+        assert plan(1, e, *lay)[0] == nt and plan(1, e + 1, *lay)[0] > nt, (cout, e)
 
 
 def test_hot_layers_get_the_configurations_design_md_describes():

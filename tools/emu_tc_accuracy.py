@@ -10,6 +10,7 @@ Model (to be checked against a run of tools/conv_unit.py on the target GPU):
     `mma.sync` kernel with register accumulators could do for free).
 
 Usage:  python tools/emu_tc_accuracy.py            (prints a table; pure numpy, ~1 minute)
+The attention's P.V contraction is emulated by tests/att_reference.py (emulated_pv_errors) on the synthetic voice.
 """
 import argparse
 
@@ -35,11 +36,14 @@ def to_f32(x64: np.ndarray, mode: str) -> np.ndarray:
     return np.where(over, np.nextafter(y, np.float32(0)), y).astype(np.float32)
 
 
-def emulate(x, w, fmt, acc_mode, chunk):
-    """x [M,K], w [K,N] fp32 -> emulated tensor-core result [M,N] fp32."""
+def emulate(x, w, fmt, acc_mode, chunk, products=("hh", "lh", "hl")):
+    """x [M,K], w [K,N] fp32 -> emulated tensor-core result [M,N] fp32.  `products`: which of the split products
+    (x part, w part) each K-step issues, in order; ("hh",) is a single unsplit MMA."""
     bits, kstep = (8, 16) if fmt == "bf16" else (11, 8)
     xh = round_to_bits(x, bits); xl = round_to_bits(x - xh, bits)
     wh = round_to_bits(w, bits); wl = round_to_bits(w - wh, bits)
+    parts = {"h": (xh, wh), "l": (xl, wl)}
+    pairs = [(parts[p[0]][0], parts[p[1]][1]) for p in products]
     M, K = x.shape
     N = w.shape[1]
     total = np.zeros((M, N), dtype=np.float32)
@@ -47,7 +51,7 @@ def emulate(x, w, fmt, acc_mode, chunk):
     steps = 0
     for k0 in range(0, K, kstep):
         sl = slice(k0, k0 + kstep)
-        for a, b in ((xh, wh), (xl, wh), (xh, wl)):
+        for a, b in pairs:
             part = a[:, sl].astype(np.float64) @ b[sl].astype(np.float64)      # exact enough: 16 products in fp64
             acc = to_f32(acc.astype(np.float64) + part, acc_mode)
         steps += 1
