@@ -163,7 +163,9 @@ void sb200_latent_free(sb200_latent* z);
 /* Copy a named intermediate of the LAST run of `job` to host (time-major fp32, valid rows of
  * utterance b only).  Names: "x","stats","logw","z_p","z","dec.pre","dec.up<i>","dec.mrf<i>", and the first encoder
  * layer's attention "qkv0","att0"; on the tensor-core attention also "p0" (head-0 probabilities) and "vt0" (V, returned
- * channel-major as [hidden][T]).
+ * channel-major as [hidden][T]).  Duration predictor: "dp.g" (the flows' conditioning, [T][hidden]) and, per coupling
+ * flow s = 0, 1, 2 in application order, "dp.f<s>.in" / "dp.f<s>.out" (the two-channel z before / after it, [T][2]),
+ * "dp.f<s>.h" (the DDSConv output, [T][hidden]) and "dp.f<s>.h29" (the spline parameters, [T][32], 29 used).
  * Returns rows via *rows, cols via *cols; data malloc'ed (free with sb200_buffer_free). */
 int32_t sb200_job_debug_fetch(sb200_job* job, const char* name, size_t b, float** data, size_t* rows, size_t* cols,
                               sb200_error* err);
@@ -202,6 +204,18 @@ int32_t sb200_debug_conv_ex(int32_t device, int32_t backend, const float* x, int
                             const float* bias, int32_t cout, int32_t k, int32_t dil, float in_slope, int32_t act,
                             const float* res, float scale, const int32_t* seg_end, int32_t gran, int32_t seg_mul,
                             float* y0, int32_t acc0, int32_t split, float* y1, int32_t acc1, sb200_error* err);
+/* The duration predictor's spline inverse (10 bins, tails at +-5) on caller data, for kernel unit tests: z is [rows][2],
+ * h29 [rows][ldh >= 29] holds per row 10 width logits, 10 height logits and 9 derivative logits, used as given (the
+ * engine divides the width / height logits by sqrt(hidden) first).  z[r][tcol] is replaced by its inverse for rows
+ * r < valid_rows and set to 0 for the rest; z[r][1 - tcol] is left alone.  z is updated in place. */
+int32_t sb200_debug_spline(int32_t device, const float* h29, int32_t ldh, float* z, int32_t rows, int32_t tcol,
+                           int32_t valid_rows, sb200_error* err);
+/* The duration kernel on caller data: per segment b (rows [seg_off[b], seg_off[b] + seg_len[b]) of z [rows][2]),
+ * logw = (z[:,0] - m0) * exp(-logs0), cum = inclusive scan of ceil(exp(logw) * length_scale), y_len[b] = max(sum, 1).
+ * cum and y_len saturate at INT32_MAX.  logw / cum rows outside every segment keep what the caller passed in. */
+int32_t sb200_debug_durations(int32_t device, const float* z, int32_t rows, const int32_t* seg_off, const int32_t* seg_len,
+                              int32_t nseg, float m0, float logs0, float length_scale, float* logw, int32_t* cum,
+                              int32_t* y_len, sb200_error* err);
 /* kernels launched by this library since load (host-side counter) */
 uint64_t sb200_launch_count(void);
 /* select the contraction backend: 0 = fp32 CUDA-core implicit GEMM, 1 = wgmma (3xTF32) where

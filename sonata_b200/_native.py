@@ -99,6 +99,11 @@ SIGNATURES = {
                                         C.c_float, C.c_int32, C.POINTER(C.c_float), C.c_float, C.POINTER(C.c_int32),
                                         C.c_int32, C.c_int32, C.POINTER(C.c_float), C.c_int32, C.c_int32,
                                         C.POINTER(C.c_float), C.c_int32, _ERR]),
+    "sb200_debug_spline": (C.c_int32, [C.c_int32, C.POINTER(C.c_float), C.c_int32, C.POINTER(C.c_float), C.c_int32,
+                                       C.c_int32, C.c_int32, _ERR]),
+    "sb200_debug_durations": (C.c_int32, [C.c_int32, C.POINTER(C.c_float), C.c_int32, C.POINTER(C.c_int32),
+                                          C.POINTER(C.c_int32), C.c_int32, C.c_float, C.c_float, C.c_float,
+                                          C.POINTER(C.c_float), C.POINTER(C.c_int32), C.POINTER(C.c_int32), _ERR]),
     "sb200_launch_count": (C.c_uint64, []),
     "sb200_set_backend": (C.c_int32, [_P, C.c_int32]),
 }

@@ -486,6 +486,56 @@ int32_t sb200_debug_conv(int32_t device, int32_t backend, const float* x, int32_
                                R, 1, y, accumulate, cout, nullptr, accumulate, err);
 }
 
+int32_t sb200_debug_spline(int32_t device, const float* h29, int32_t ldh, float* z, int32_t rows, int32_t tcol,
+                           int32_t valid_rows, sb200_error* err) {
+    return guarded(err, [&] {
+        if (rows <= 0 || ldh < 29 || (tcol != 0 && tcol != 1) || valid_rows < 0 || valid_rows > rows)
+            throw Error(19, "debug spline: bad arguments");
+        SB_CUDA(cudaSetDevice(device));
+        const int R = (rows + 255) / 256 * 256;                          // one granule spanning the padded launch
+        float *dh, *dz; int* dend;
+        SB_CUDA(cudaMalloc(&dh, (size_t)R * ldh * 4)); SB_CUDA(cudaMemset(dh, 0, (size_t)R * ldh * 4));
+        SB_CUDA(cudaMemcpy(dh, h29, (size_t)rows * ldh * 4, cudaMemcpyHostToDevice));
+        SB_CUDA(cudaMalloc(&dz, (size_t)R * 2 * 4)); SB_CUDA(cudaMemset(dz, 0, (size_t)R * 2 * 4));
+        SB_CUDA(cudaMemcpy(dz, z, (size_t)rows * 2 * 4, cudaMemcpyHostToDevice));
+        SB_CUDA(cudaMalloc(&dend, 4)); SB_CUDA(cudaMemcpy(dend, &valid_rows, 4, cudaMemcpyHostToDevice));
+        launch_spline(dh, ldh, dz, tcol, 10, 1.f, RowMap{dend, R, 1, R}, 0);
+        cudaError_t e = cudaDeviceSynchronize();
+        if (e == cudaSuccess) e = cudaMemcpy(z, dz, (size_t)rows * 2 * 4, cudaMemcpyDeviceToHost);
+        cudaFree(dh); cudaFree(dz); cudaFree(dend);
+        if (e != cudaSuccess) throw Error(19, std::string("CUDA error: ") + cudaGetErrorString(e));
+    });
+}
+
+int32_t sb200_debug_durations(int32_t device, const float* z, int32_t rows, const int32_t* seg_off, const int32_t* seg_len,
+                              int32_t nseg, float m0, float logs0, float length_scale, float* logw, int32_t* cum,
+                              int32_t* y_len, sb200_error* err) {
+    return guarded(err, [&] {
+        if (rows <= 0 || nseg <= 0 || !seg_off || !seg_len) throw Error(19, "debug durations: bad arguments");
+        std::vector<SegInfo> segs(nseg);
+        for (int b = 0; b < nseg; b++) {
+            if (seg_off[b] < 0 || seg_len[b] < 0 || (long long)seg_off[b] + seg_len[b] > rows)
+                throw Error(19, "debug durations: segment outside the rows");
+            segs[b] = SegInfo{seg_off[b], seg_len[b]};
+        }
+        SB_CUDA(cudaSetDevice(device));
+        float *dz, *dlogw; int *dcum, *dylen; SegInfo* dseg;
+        SB_CUDA(cudaMalloc(&dz, (size_t)rows * 2 * 4)); SB_CUDA(cudaMemcpy(dz, z, (size_t)rows * 2 * 4, cudaMemcpyHostToDevice));
+        SB_CUDA(cudaMalloc(&dlogw, (size_t)rows * 4)); SB_CUDA(cudaMemcpy(dlogw, logw, (size_t)rows * 4, cudaMemcpyHostToDevice));
+        SB_CUDA(cudaMalloc(&dcum, (size_t)rows * 4)); SB_CUDA(cudaMemcpy(dcum, cum, (size_t)rows * 4, cudaMemcpyHostToDevice));
+        SB_CUDA(cudaMalloc(&dylen, (size_t)nseg * 4));
+        SB_CUDA(cudaMalloc(&dseg, (size_t)nseg * sizeof(SegInfo)));
+        SB_CUDA(cudaMemcpy(dseg, segs.data(), (size_t)nseg * sizeof(SegInfo), cudaMemcpyHostToDevice));
+        launch_durations(dz, m0, logs0, length_scale, dseg, nseg, dlogw, dcum, dylen, 0);
+        cudaError_t e = cudaDeviceSynchronize();
+        if (e == cudaSuccess) e = cudaMemcpy(logw, dlogw, (size_t)rows * 4, cudaMemcpyDeviceToHost);
+        if (e == cudaSuccess) e = cudaMemcpy(cum, dcum, (size_t)rows * 4, cudaMemcpyDeviceToHost);
+        if (e == cudaSuccess) e = cudaMemcpy(y_len, dylen, (size_t)nseg * 4, cudaMemcpyDeviceToHost);
+        cudaFree(dz); cudaFree(dlogw); cudaFree(dcum); cudaFree(dylen); cudaFree(dseg);
+        if (e != cudaSuccess) throw Error(19, std::string("CUDA error: ") + cudaGetErrorString(e));
+    });
+}
+
 uint64_t sb200_launch_count(void) { return g_launch_count; }
 int32_t sb200_set_backend(sb200_voice* v, int32_t backend) { int32_t p = v->v->backend; v->v->backend = backend; return p; }
 

@@ -417,7 +417,8 @@ void Job::run(float* d_out, size_t d_out_cap) {
                            (tc_att ? (size_t)a.heads * RX * att_tp + 2 * (size_t)RX * H : 0);
     const size_t tile_bytes = (tiles_s.size() + tiles_o.size()) * sizeof(TfTile);
     const size_t p1_bytes = xfloats * 4 + (size_t)RX * 20 + B * 64 + tile_bytes + (1 << 20) + (size_t)V.cond_rows * 4 + 1024 +
-                            (debug ? (size_t)RX * (5 * H + att_tp) * 4 + 4096 : 0);
+                            (debug ? (size_t)RX * (5 * H + att_tp) * 4 + 4096 +
+                                     V.dp_flows.size() * ((size_t)RX * (H + 36) * 4 + 1024) : 0);
     // The arena must also hold phase 2; sizes are only known after the durations come back, so phase 1
     // runs in the front of the arena and phase 2 re-plans behind it (growing = realloc would lose phase-1
     // results, so grow conservatively up front from the mean-duration estimate, then verify).
@@ -577,13 +578,26 @@ void Job::run(float* d_out, size_t d_out_cap) {
     R.dds(V.dp_dds, d0, t1, t2, LX);
     { Runner::Opt o; o.y0 = g; o.ldy0 = H; o.tf_ok = true; R.conv(V.dp_proj, d0, H, LX, o); }
     launch_scale_copy2(d_epsw, cfg.noise_w, zz, LX.map, st);
-    for (const CFlowW& cf : V.dp_flows) {
+    if (debug) { dbg["dp.g"] = {g, H}; dbg_level["dp.g"] = 0; }
+    // debug: each flow's input, DDSConv output, spline parameters and output (zz, d0 and h29 are reused: copies)
+    auto capture = [&](const std::string& name, const float* src, int cols) {
+        float* cp = C.dev.get<float>((size_t)RX * cols);
+        SB_CUDA(cudaMemcpyAsync(cp, src, (size_t)RX * cols * 4, cudaMemcpyDeviceToDevice, st));
+        dbg[name] = {cp, cols}; dbg_level[name] = 0;
+    };
+    for (size_t s = 0; s < V.dp_flows.size(); s++) {
+        const CFlowW& cf = V.dp_flows[s];
+        const std::string fs = "dp.f" + std::to_string(s) + ".";
+        if (debug) capture(fs + "in", zz, 2);
         launch_flow_pre(zz, cf.ccol, cf.pre_w, cf.pre_b, g, d0, H, LX.map, st);
         R.count(2.0 * LX.valid_rows * H, 8.0 * LX.valid_rows * H);
         R.dds(cf.dds, d0, t1, t2, LX);
+        if (debug) capture(fs + "h", d0, H);
         { Runner::Opt o; o.y0 = h29; o.ldy0 = 32; o.tf_ok = true; R.conv(cf.proj, d0, H, LX, o); }
+        if (debug) capture(fs + "h29", h29, 32);
         launch_spline(h29, 32, zz, cf.tcol, a.dp_bins, 1.0f / sqrtf((float)H), LX.map, st);
         R.count(0, 4.0 * LX.valid_rows * 34);
+        if (debug) capture(fs + "out", zz, 2);
     }
     launch_durations(zz, V.ea_m0, V.ea_logs0, cfg.length_scale, d_xsegs, (int)B, logw, d_cum, d_ylen, st);
     R.end();

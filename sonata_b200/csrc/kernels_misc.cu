@@ -5,6 +5,7 @@
 // The reference executes all of these inside onnxruntime (piper/src/lib.rs:362-379); the
 // arithmetic restated here follows oracle/vits_oracle.py function by function.
 #include "common.cuh"
+#include <climits>
 #include <math.h>
 
 namespace sb200 {
@@ -453,9 +454,14 @@ __global__ void spline_kernel(const float* __restrict__ h29, int ldh, float* __r
     const float a = t * e + in_h * (delta - in_d);
     const float b = in_h * in_d - t * e;
     const float c = -delta * t;
-    const float disc = b * b - 4.f * a * c;
+    // At the top of a bin disc = h^2 d_{k+1}^2 exactly, but in fp32 it is the difference of two O(4 h^2 delta^2) terms and
+    // can round below zero, where sqrtf gives NaN (the fp32 graph does).  Clamped, the root is the fp64 answer to within
+    // the condition of the inverse (DESIGN.md section 4).
+    const float disc = fmaxf(b * b - 4.f * a * c, 0.f);
     const float root = (2.f * c) / (-b - sqrtf(disc));
-    z[2 * r + tcol] = root * in_w + in_cw;
+    // the exact inverse of an input in [-B, B] lies in [-B, B]; in fp32 the root of an end bin can overshoot B by up to
+    // ~1.4e-4 (hundreds of ulp, saturated and sigma-10 logits), which the next flow would take as its identity tail
+    z[2 * r + tcol] = fminf(fmaxf(root * in_w + in_cw, -B), B);
 }
 
 // z[r][0..1] = eps[r][0..1] * s   (oracle: sdp_reverse  z = eps_w * noise_w)
@@ -470,42 +476,47 @@ __global__ void scale_copy2_kernel(const float* __restrict__ eps, float s, float
 
 // ------------------------------------------------------------------ durations: ceil + inclusive scan
 // oracle: sdp_reverse() tail (ElementwiseAffine^-1) + durations()
+// The scan runs in 64 bits and cum / y_len saturate at INT_MAX: a duration past 2^31 - 1 frames (or a NaN / inf one)
+// must reach the host as an overlong frame count, which it rejects, not wrap into a plausible one.
+__device__ __forceinline__ int sat_int(long long v) { return (int)min(v, (long long)INT_MAX); }
+
 __global__ void __launch_bounds__(256) durations_kernel(const float* __restrict__ z, float m0, float logs0,
                                                         float length_scale, const SegInfo* __restrict__ segs,
                                                         float* __restrict__ logw, int* __restrict__ cum,
                                                         int* __restrict__ y_len) {
     pdl_trigger(); pdl_wait();
     const SegInfo sg = segs[blockIdx.x];
-    __shared__ int warp_tot[8];
-    __shared__ int carry_s;
+    __shared__ long long warp_tot[8];
+    __shared__ long long carry_s;
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     if (tid == 0) carry_s = 0;
     __syncthreads();
     const float einv = expf(-logs0);
     for (int base = 0; base < sg.len; base += 256) {
         const int i = base + tid;
-        int w = 0;
+        long long w = 0;
         if (i < sg.len) {
             const float lw = (z[2 * (sg.off + i)] - m0) * einv;
             logw[sg.off + i] = lw;
-            w = (int)ceilf(expf(lw) * length_scale);
+            const float wc = ceilf(expf(lw) * length_scale);
+            w = wc < 2147483648.f ? (long long)(int)wc : (long long)INT_MAX;     // NaN and inf saturate too
         }
-        int s = w;
+        long long s = w;
 #pragma unroll
         for (int o = 1; o < 32; o <<= 1) {
-            const int t = __shfl_up_sync(0xffffffffu, s, o);
+            const long long t = __shfl_up_sync(0xffffffffu, s, o);
             if (lane >= o) s += t;
         }
         if (lane == 31) warp_tot[warp] = s;
         __syncthreads();
-        int pre = carry_s;
+        long long pre = carry_s;
         for (int k = 0; k < warp; k++) pre += warp_tot[k];
-        if (i < sg.len) cum[sg.off + i] = pre + s;
+        if (i < sg.len) cum[sg.off + i] = sat_int(pre + s);
         __syncthreads();
         if (tid == 255) carry_s = pre + s;
         __syncthreads();
     }
-    if (tid == 0) y_len[blockIdx.x] = max(carry_s, 1);
+    if (tid == 0) y_len[blockIdx.x] = sat_int(max(carry_s, 1LL));
 }
 
 // ------------------------------------------------------------------ alignment expansion (one warp per frame)

@@ -144,6 +144,121 @@ def test_pv_emulation_places_degraded_splits_above_attention_bound():
         assert e[degraded] > bound, (degraded, e, bound)
 
 
+@pytest.mark.parametrize("nspk,sid,n", [(1, None, 41), (4, 3, 300)])
+def test_dp_reference_matches_oracle_sdp_reverse(nspk, sid, n):
+    """tests/dp_reference.py (the float64 restatement the CUDA duration predictor is held to) against the oracle's
+    `sdp_reverse` in float64, on the medium voice and the 4-speaker medium voice at sid 3, noise_w 0.8: dp.g, every
+    flow's output and logw.  The oracle flips z between the flows; the reference keeps the columns fixed."""
+    import dp_reference as dr
+    t = voicegen.make_tensors("medium", n_speakers=nspk)
+    W64 = vo.to_torch(t, torch.float64)
+    a = vo.arch_of(W64)
+    ids = vo.synthetic_ids(n // 2, utt=6)[:n]
+    x64, _, _ = vo.text_encoder(W64, torch.as_tensor(ids).view(1, -1), a)
+    eps = np.random.default_rng(2).standard_normal((n, 2))
+    st = {}
+    logw = vo.sdp_reverse(W64, x64, torch.from_numpy(eps.T[None].copy()), 0.8, a, stages=st,
+                          g=vo.speaker_embedding(W64, sid))[0, 0].numpy()
+    g = dr.dp_cond(t, x64[0].T.numpy(), sid)
+    z = eps * 0.8
+    for s in range(3):
+        h29 = dr.flow_h29(t, s, dr.flow_h(t, s, z, g))
+        uw, uh, ud = h29[:, :10] / np.sqrt(a["hidden"]), h29[:, 10:20] / np.sqrt(a["hidden"]), h29[:, 20:29]
+        tc = dr.flow_cols(s)[1]
+        z = z.copy()
+        z[:, tc] = dr.rqs_inverse(z[:, tc], uw, uh, ud)
+        ora = st[f"dp.flow{dr.FLOWS[s]}"][0].T.numpy()
+        assert float(np.abs((z[:, ::-1] if s % 2 == 0 else z) - ora).max()) < 1e-10, s
+    m0 = float(W64["dp.flows.0.m"].reshape(-1)[0])
+    logs0 = float(W64["dp.flows.0.logs"].reshape(-1)[0])
+    assert float(np.abs(dr.ea_inverse(z[:, 0], m0, logs0) - logw).max()) < 1e-10
+
+
+def test_dp_bound_catches_degraded_variants(oracle_weights):
+    """The bound of the duration predictor's DDSConv stages (dp_reference.DP_MULT x the fp32 oracle's error + DP_FLOOR)
+    is tight enough to catch a degraded kernel.  On flow 0's DDSConv of a 201-id utterance (noise_w 0.8), float32
+    emulations with a tanh GELU, LN eps 1e-6, or a 1x1 on one TF32 product each land above it, and the correct float32
+    chain below it.  A single-pass variance only loses accuracy where |mean| >> std, which this predictor's LN inputs
+    are not: it is shown above the bound on flow 0's first LN input rows shifted by 64 (LN removes a common offset
+    exactly)."""
+    import dp_reference as dr
+    t = voicegen.make_tensors("medium")
+    W32, W64 = oracle_weights("medium"), vo.to_torch(t, torch.float64)
+    a = vo.arch_of(W64)
+    ids = vo.synthetic_ids(100, utt=5)
+    x = vo.text_encoder(W64, torch.as_tensor(ids).view(1, -1), a)[0][0].T.numpy().astype(np.float32)
+    g = dr.dp_cond(t, x).astype(np.float32)
+    z = (np.random.default_rng(0).standard_normal((len(ids), 2)) * 0.8).astype(np.float32)
+    ref = dr.flow_h(t, 0, z, g)
+    p = "dp.flows.7."
+    zc = torch.from_numpy(z[:, 1].copy()).view(1, 1, -1)
+    h32 = vo._dds(W32, p + "convs.", vo._conv(W32, p + "pre", zc), a, g=torch.from_numpy(g.T[None].copy()))[0].T.numpy()
+    bound = dr.DP_MULT * float(np.abs(h32 - ref).max()) + dr.DP_FLOOR
+    err = {k: float(np.abs(dr.flow_h(t, 0, z, g, np.float32, **v) - ref).max())
+           for k, v in (("fp32", {}), ("tanh_gelu", dict(tanh=True)), ("ln_eps_1e-6", dict(eps=1e-6)),
+                        ("one_tf32_1x1", dict(one_tf32=True)))}
+    y = dr.depthwise(dr.flow_pre(t, 0, z, g), t[p + "convs.convs_sep.0.weight"], t[p + "convs.convs_sep.0.bias"], 1)
+    y = (y + 64.0).astype(np.float32)
+    gm, bt = t[p + "convs.norms_1.0.gamma"], t[p + "convs.norms_1.0.beta"]
+    ln_ref = dr.layer_norm(y.astype(np.float64), gm, bt)
+    ln_bound = dr.DP_MULT * float(np.abs(dr.layer_norm(y, gm, bt, np.float32) - ln_ref).max()) + dr.DP_FLOOR
+    err["one_pass_var"] = float(np.abs(dr.layer_norm(y, gm, bt, np.float32, one_pass=True) - ln_ref).max())
+    print({k: f"{v:.2e}" for k, v in err.items()}, f"bound {bound:.2e}", f"LN bound {ln_bound:.2e}")
+    assert err["fp32"] <= bound, (err, bound)
+    for k in ("tanh_gelu", "ln_eps_1e-6", "one_tf32_1x1"):
+        assert err[k] > bound, (k, err, bound)
+    assert err["one_pass_var"] > ln_bound, (err, ln_bound)
+
+
+def test_spline_bound_catches_wrong_splines():
+    """The element-wise bound of the spline kernel (dp_reference.spline_error_bound) is tight enough to catch a wrong
+    spline: on every edge parameter set and input of the kernel test, the kernel's arithmetic emulated on the host with
+    d_k and d_{k+1} swapped, or with 1.9 delta for 2 delta in e, lands above it (by a factor of 40 or more), and the
+    correct arithmetic (contracted or not) lies within it."""
+    import dp_reference as dr
+    rng = np.random.default_rng(7)
+    worst = {}
+    for name, uw, uh, ud in dr.edge_params(rng):
+        _, _, ch = dr.spline_fp32(np.zeros(1, np.float32), uw[None], uh[None], ud[None])
+        y = dr.edge_inputs(ch[0])
+        y = y[(y >= -5) & (y <= 5)]
+        p = [np.repeat(a[None], len(y), 0) for a in (uw, uh, ud)]
+        ref, bound = dr.spline_error_bound(y, *p)
+        for fused in (True, False):
+            assert np.all(np.abs(dr.spline_fp32(y, *p, fused)[0] - ref) <= bound), (name, fused)
+        for defect in ("swap_d", "e_1.9"):
+            r = float(np.max(np.abs(dr.spline_fp32(y, *p, defect=defect)[0] - ref) / bound))
+            worst[defect] = min(worst.get(defect, np.inf), r)
+            assert r > 1, (name, defect, r)
+    print({k: f"{v:.0f}x the bound at least" for k, v in worst.items()})
+
+
+def test_spline_fp32_emulation_meets_negative_discriminants():
+    """dp_reference.spline_fp32 (spline_kernel's arithmetic in float32 on the host) finds fp32 discriminants below zero
+    just under the knots of spline parameters with logits of std 3 -- where the unclamped kernel, like the fp32 graph,
+    returns NaN -- and the clamped formula stays finite there and matches float64 away from such points."""
+    import dp_reference as dr
+    rng = np.random.default_rng(1)
+    n = 300
+    uw, uh, ud = (rng.normal(0, 3, (n, k)).astype(np.float32) for k in (10, 10, 9))
+    _, _, ch = dr.spline_fp32(np.zeros(n, np.float32), uw, uh, ud)
+    y = np.concatenate([(ch[:, k] - np.float32(d)).astype(np.float32) for k in range(1, 10)
+                        for d in np.geomspace(1e-7, 1e-4, 20)])
+    r = np.tile(np.arange(n), 9 * 20)
+    out, disc, _ = dr.spline_fp32(y, uw[r], uh[r], ud[r])
+    assert int((disc < 0).sum()) > 0
+    assert np.isfinite(out).all() and (np.abs(out) <= 5).all()
+    o32 = vo._rqs_inverse(torch.from_numpy(y).view(1, 1, -1), torch.from_numpy(uw[r]).view(1, 1, -1, 10),
+                          torch.from_numpy(uh[r]).view(1, 1, -1, 10), torch.from_numpy(ud[r]).view(1, 1, -1, 9))
+    assert bool(torch.isnan(o32).any())                 # the fp32 graph itself
+    ref = dr.rqs_inverse(y.astype(np.float64), uw[r], uh[r], ud[r])
+    assert float(np.median(np.abs(out - ref))) < 1e-5
+    # forward / inverse round trip in float64
+    x = rng.uniform(-5, 5, n)
+    yy, _ = dr.rqs_forward(x, uw, uh, ud)
+    assert float(np.abs(dr.rqs_inverse(yy, uw, uh, ud) - x).max()) < 1e-6
+
+
 def _rqs_forward(x, uw, uh, ud, B=5.0):
     """transforms.rational_quadratic_spline(inverse=False), scalar restatement."""
     nb = len(uw)
