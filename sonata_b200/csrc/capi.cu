@@ -247,23 +247,11 @@ int32_t sb200_job_fetch(sb200_job* job, sb200_audio* outs, sb200_error* err) {
 int32_t sb200_job_fetch_i16(sb200_job* job, int16_t** outs, size_t* lens, sb200_error* err) {
     return guarded(err, [&] {
         Job& j = *job->j;
-        if (!j.ran || j.encode_only) throw Error(19, "job has not produced audio");
-        Voice& v = *j.v;
-        SB_CUDA(cudaSetDevice(v.device));
-        const int hop = v.a.hop();
-        long long mx = 0;
-        for (size_t b = 0; b < j.B; b++) mx = std::max<long long>(mx, (long long)j.y_len[b] * hop);
-        short* d_i16 = nullptr; unsigned* d_max = nullptr;
-        SB_CUDA(cudaMallocAsync(&d_i16, (size_t)j.total_samples * 2 + 16, j.ctx->stream));
-        SB_CUDA(cudaMallocAsync(&d_max, sizeof(unsigned) * j.B, j.ctx->stream));
-        launch_i16(j.d_wav, j.d_fsegs, (int)j.B, hop, mx, d_max, d_i16, PcmPost{}, j.ctx->stream);
+        SB_CUDA(cudaSetDevice(j.v->device));
+        const int hop = j.v->a.hop();
         PinnedBlock* blk = pin_acquire((size_t)j.total_samples * 2 + 16);
-        cudaError_t e = cudaMemcpyAsync(blk->base, d_i16, (size_t)j.total_samples * 2, cudaMemcpyDeviceToHost, j.ctx->stream);
-        cudaFreeAsync(d_i16, j.ctx->stream);
-        cudaFreeAsync(d_max, j.ctx->stream);
-        if (e == cudaSuccess) e = cudaStreamSynchronize(j.ctx->stream);
-        if (e != cudaSuccess) { pin_release(blk); throw Error(19, std::string("CUDA error: ") + cudaGetErrorString(e)); }
-        const int16_t* h = reinterpret_cast<const int16_t*>(blk->base);
+        int16_t* h = reinterpret_cast<int16_t*>(blk->base);
+        try { job_i16_to_host(j, 1.f, h); } catch (...) { pin_release(blk); throw; }
         for (size_t b = 0; b < j.B; b++) {
             const size_t n = (size_t)j.y_len[b] * hop;
             outs[b] = (int16_t*)malloc(n * 2 + 2);
@@ -287,18 +275,7 @@ int32_t sb200_job_copy_out(sb200_job* job, void* dst, size_t cap, int32_t format
         const size_t bytes = n * (format == 1 ? 2 : 4);
         if (bytes > cap) throw Error(19, "destination buffer is too small for the synthesis result");
         if (format == 1) {
-            const int hop = v.a.hop();
-            long long mx = 0;
-            for (size_t b = 0; b < j.B; b++) mx = std::max<long long>(mx, (long long)j.y_len[b] * hop);
-            short* d_i16 = nullptr; unsigned* d_max = nullptr;
-            SB_CUDA(cudaMallocAsync(&d_i16, n * 2 + 16, st));
-            SB_CUDA(cudaMallocAsync(&d_max, sizeof(unsigned) * j.B, st));
-            launch_i16(j.d_wav, j.d_fsegs, (int)j.B, hop, mx, d_max, d_i16, PcmPost{}, st);
-            cudaError_t e = cudaMemcpyAsync(dst, d_i16, bytes, cudaMemcpyDeviceToHost, st);
-            cudaFreeAsync(d_i16, st);
-            cudaFreeAsync(d_max, st);
-            if (e == cudaSuccess) e = cudaStreamSynchronize(st);
-            if (e != cudaSuccess) throw Error(19, std::string("CUDA error: ") + cudaGetErrorString(e));
+            job_i16_to_host(j, 1.f, static_cast<int16_t*>(dst));
         } else {
             SB_CUDA(cudaMemcpyAsync(dst, j.d_wav, bytes, cudaMemcpyDeviceToHost, st));
             SB_CUDA(cudaStreamSynchronize(st));

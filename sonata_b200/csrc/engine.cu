@@ -5,6 +5,7 @@
 // (:433-435) becomes ONE pass whose per-utterance results equal the B=1 results.
 #include "engine.h"
 #include <algorithm>
+#include <array>
 #include <cmath>
 #include <cstring>
 #include <cstdlib>
@@ -28,22 +29,19 @@ inline int round_up(int x, int m) { return (x + m - 1) / m * m; }
 }  // namespace
 
 // ------------------------------------------------------------------ Context
-void Context::ensure_dev(size_t bytes) {
-    if (bytes <= dev.cap) return;
-    if (dev.base) SB_CUDA(cudaFree(dev.base));
-    dev.base = nullptr; dev.cap = 0;
-    const size_t want = bytes + bytes / 8 + (64u << 20);
+// Arenas grow with headroom, so a warmed-up context allocates nothing in steady state.
+void Arena::reserve(size_t bytes) {
+    used = 0;
+    if (bytes <= cap) return;
+    release();
+    const size_t want = pinned ? bytes * 2 : bytes + bytes / 8 + (64u << 20);
     void* p = nullptr;
-    SB_CUDA(cudaMalloc(&p, want));
-    dev.base = (char*)p; dev.cap = want;
+    SB_CUDA(pinned ? cudaMallocHost(&p, want) : cudaMalloc(&p, want));
+    base = (char*)p; cap = want;
 }
-void Context::ensure_pin(size_t bytes) {
-    if (bytes <= pin_cap) return;
-    if (pin) cudaFreeHost(pin);
-    pin = nullptr; pin_cap = 0;
-    void* p = nullptr;
-    SB_CUDA(cudaMallocHost(&p, bytes * 2));
-    pin = (char*)p; pin_cap = bytes * 2;
+void Arena::release() {
+    if (base) pinned ? cudaFreeHost(base) : cudaFree(base);
+    base = nullptr; cap = 0; used = 0;
 }
 cudaEvent_t Context::next_event() {
     if (events_used == events.size()) {
@@ -54,8 +52,9 @@ cudaEvent_t Context::next_event() {
     return events[events_used++];
 }
 Context::~Context() {
-    if (dev.base) cudaFree(dev.base);
-    if (pin) cudaFreeHost(pin);
+    dev_id.release();
+    dev_frame.release();
+    pin.release();
     for (auto e : events) cudaEventDestroy(e);
     if (stream) cudaStreamDestroy(stream);
 }
@@ -254,39 +253,169 @@ struct Runner {
 void h2d(void* dst, const void* src, size_t bytes, cudaStream_t st) {
     SB_CUDA(cudaMemcpyAsync(dst, src, bytes, cudaMemcpyHostToDevice, st));
 }
+void d2d(float* dst, const float* src, size_t n, cudaStream_t st) {
+    SB_CUDA(cudaMemcpyAsync(dst, src, n * 4, cudaMemcpyDeviceToDevice, st));
+}
+
+void expose(Job& j, const std::string& name, float* p, int cols, int level) {
+    j.dbg[name] = {p, cols};
+    j.dbg_level[name] = level;
+}
+
+// Each workspace below hands out its buffers in one carve(dev, pin).  plan() runs it on dry arenas to learn the sizes,
+// makes room in the context's arenas and carves again for real, so no size is written down twice.
+template <typename Carve> void plan(Arena& dev, Arena& pin, Carve&& carve) {
+    Arena dry_dev, dry_pin;
+    dry_dev.dry = dry_pin.dry = true;
+    carve(dry_dev, dry_pin);
+    dev.reserve(dry_dev.used);
+    pin.reserve(dry_pin.used);
+    carve(dev, pin);
+}
+
+// Id level (phase 1): X tables, encoder and duration-predictor activations, and with debug the captures.
+struct IdBufs {
+    int *ids_rows_h, *xend_h, *xseg_of_h, *ylen_h; SegInfo* xsegs_h; TfTile* tiles_h;     // pinned staging
+    int *ids_rows, *xend, *xseg_of_gran, *cum, *ylen; SegInfo* xsegs; TfTile* tiles;
+    float *xa, *xb, *qkv, *att, *ffn, *stats, *d0, *t1, *t2, *g, *h29, *zz, *logw;
+    float *att_s, *att_vt, *att_orel;          // tensor-core attention: scores of every head, V^T, relative-value term
+    float *epsw, *cond;
+    float *qkv0, *att0, *p0, *vt0;             // debug: layer 0's attention operands and result
+    std::vector<std::array<float*, 4>> dpf;    // debug: each duration flow's input, DDSConv output, spline parameters, output
+
+    void carve(Arena& dev, Arena& pin, const Job& j, bool tc_att) {
+        const Voice& v = *j.v; const Arch& a = v.a;
+        const int RX = j.RX, nxg = RX / GX, H = a.hidden;
+        const size_t B = j.B, ntiles = j.tiles_s.size() + j.tiles_o.size();
+        auto rows = [&](int cols) { return dev.get<float>((size_t)RX * cols); };
+        ids_rows_h = pin.get<int>(RX); xend_h = pin.get<int>(nxg); xseg_of_h = pin.get<int>(nxg);
+        xsegs_h = pin.get<SegInfo>(B); ylen_h = pin.get<int>(B);
+        tiles_h = tc_att ? pin.get<TfTile>(ntiles) : nullptr;
+        ids_rows = dev.get<int>(RX); xend = dev.get<int>(nxg); xseg_of_gran = dev.get<int>(nxg); xsegs = dev.get<SegInfo>(B);
+        cum = dev.get<int>(RX); ylen = dev.get<int>(B);
+        tiles = tc_att ? dev.get<TfTile>(ntiles) : nullptr;
+        xa = rows(H); xb = rows(H); qkv = rows(3 * H); att = rows(H); ffn = rows(a.filter); stats = rows(2 * a.inter);
+        d0 = rows(H); t1 = rows(H); t2 = rows(H); g = rows(H); h29 = rows(32); zz = rows(2); logw = rows(1);
+        att_s = att_vt = att_orel = nullptr;
+        if (tc_att) { att_s = dev.get<float>((size_t)a.heads * RX * j.att_tp); att_vt = rows(H); att_orel = rows(H); }
+        epsw = j.cfg.noise_w != 0.f ? rows(2) : nullptr;
+        cond = v.num_speakers > 1 ? dev.get<float>((size_t)v.cond_rows) : nullptr;
+        qkv0 = att0 = p0 = vt0 = nullptr;
+        dpf.clear();
+        if (j.debug) {
+            qkv0 = rows(3 * H); att0 = rows(H);
+            if (tc_att) { p0 = rows(j.att_tp); vt0 = rows(H); }
+            dpf.resize(v.dp_flows.size());
+            for (auto& f : dpf) f = {rows(2), rows(H), rows(32), rows(2)};
+        }
+    }
+};
+
+// Frame-level tables (segment end and owner of every GY-frame tile, the segment list) and their pinned mirrors.
+struct FrameTables {
+    int *yend, *ftile; FrameSeg* fsegs;
+    int *yend_h, *ftile_h; FrameSeg* fsegs_h;
+    void carve(Arena& dev, Arena& pin, const Job& j) {
+        const int ntile = j.RY / GY; const size_t B = j.fsegs.size();
+        yend = dev.get<int>(ntile); ftile = dev.get<int>(ntile); fsegs = dev.get<FrameSeg>(B);
+        yend_h = pin.get<int>(ntile); ftile_h = pin.get<int>(ntile); fsegs_h = pin.get<FrameSeg>(B);
+    }
+};
+
+// Decoder over RY frames: conv_pre's output, then ping-pong stage buffers sized for the widest stage, or with debug one
+// set per stage so every stage can be fetched.
+struct DecoderBufs {
+    float* p0;
+    std::vector<std::array<float*, 5>> stage;    // per upsampling stage: up, ys, tmp[3]
+    void carve(Arena& dev, const Voice& v, int RY, bool debug) {
+        p0 = dev.get<float>((size_t)RY * v.a.up_init);
+        stage.assign(v.ups.size(), {});
+        int U = 1;
+        if (debug) {
+            for (size_t i = 0; i < v.ups.size(); i++) {
+                U *= v.ups[i].u;
+                for (auto& b : stage[i]) b = dev.get<float>((size_t)RY * U * v.ups[i].cout);
+            }
+            return;
+        }
+        size_t max_elems = 0;
+        for (auto& st : v.ups) { U *= st.u; max_elems = std::max(max_elems, (size_t)RY * U * st.cout); }
+        const int ntmp = (v.a.resblock == 2) ? 2 : 4;
+        float* pool[6] = {nullptr};
+        for (int i = 0; i < 2 + ntmp; i++) pool[i] = dev.get<float>(max_elems);
+        for (size_t i = 0; i < v.ups.size(); i++)
+            stage[i] = {pool[2], pool[i & 1], pool[3], ntmp > 2 ? pool[4] : nullptr, ntmp > 2 ? pool[5] : nullptr};
+    }
+    void expose_to(Job& j) const {
+        const Voice& v = *j.v;
+        expose(j, "dec.pre", p0, v.a.up_init, 1);
+        int U = 1;
+        for (size_t i = 0; i < v.ups.size(); i++) {
+            U *= v.ups[i].u;
+            expose(j, "dec.up" + std::to_string(i), stage[i][0], v.ups[i].cout, U);
+            expose(j, "dec.mrf" + std::to_string(i), stage[i][1], v.ups[i].cout, U);
+        }
+    }
+};
+
+// Frame level of a synthesis pass (phase 2): tables, the latent, the flow's scratch, and unless the pass stops after
+// the flow the decoder and (when the caller passed no buffer) the waveforms.
+struct FrameBufs {
+    FrameTables y;
+    float *s, *epsz, *zp, *h, *acts, *outb, *wav;
+    DecoderBufs dec;
+    void carve(Arena& dev, Arena& pin, const Job& j, bool own_wav) {
+        const Arch& a = j.v->a;
+        const size_t RY = (size_t)j.RY;
+        y.carve(dev, pin, j);
+        s = dev.get<float>(RY * a.inter);
+        epsz = j.cfg.noise_scale != 0.f ? dev.get<float>(RY * a.inter) : nullptr;
+        zp = j.debug ? dev.get<float>(RY * a.inter) : nullptr;
+        h = dev.get<float>(RY * a.hidden); acts = dev.get<float>(RY * a.hidden); outb = dev.get<float>(RY * a.hidden);
+        wav = nullptr;
+        if (j.encode_only) return;
+        if (own_wav) wav = dev.get<float>((size_t)j.total_samples + 4);
+        dec.carve(dev, *j.v, j.RY, j.debug);
+    }
+};
+
+// One streaming decoder chunk: speaker biases, tables, the latent slice, the decoder, the waveform, the PCM scratch
+// when the chunk leaves as i16, and the pinned slot the result is copied to.
+struct ChunkBufs {
+    float* cond;
+    FrameTables y;
+    float *s, *wav;
+    DecoderBufs dec;
+    short* i16; unsigned* max;
+    float* out_h;
+    void carve(Arena& dev, Arena& pin, const Job& j, bool pcm) {
+        const Voice& v = *j.v;
+        cond = v.num_speakers > 1 ? dev.get<float>((size_t)v.cond_rows) : nullptr;
+        y.carve(dev, pin, j);
+        s = dev.get<float>((size_t)j.RY * v.a.inter);
+        wav = dev.get<float>((size_t)j.total_samples + 4);
+        dec.carve(dev, v, j.RY, false);
+        i16 = pcm ? dev.get<short>((size_t)j.total_samples + 8) : nullptr;
+        max = pcm ? dev.get<unsigned>(4) : nullptr;
+        out_h = pin.get<float>((size_t)j.total_samples);
+    }
+};
 
 // decoder over an already-laid-out Y level: s [RY][inter] (gap rows zero) -> wav
-void run_decoder(Runner& R, const Level& LY, const float* s, float* d_wav, const FrameSeg* d_fsegs,
-                 const int* d_ftile, const int* d_yend) {
-    Voice& v = R.v; const Arch& a = R.a; Job& j = R.j; Context& c = R.c;
+void run_decoder(Runner& R, const Level& LY, const FrameTables& y, const DecoderBufs& d, const float* s, float* d_wav) {
+    Voice& v = R.v; const Arch& a = R.a;
     const int RY = LY.map.rows;
     R.begin("dec.pre");
-    float* p0 = c.dev.get<float>((size_t)RY * a.up_init);
-    { Runner::Opt o; o.y0 = p0; o.ldy0 = a.up_init; o.tc_ok = true; R.conv(v.conv_pre, s, a.inter, LY, o); }
+    { Runner::Opt o; o.y0 = d.p0; o.ldy0 = a.up_init; o.tc_ok = true; R.conv(v.conv_pre, s, a.inter, LY, o); }
     R.end();
-    if (j.debug) { j.dbg["dec.pre"] = {p0, a.up_init}; j.dbg_level["dec.pre"] = 1; }
 
-    // ping-pong stage buffers (debug: one set per stage so every stage can be fetched)
-    size_t max_elems = 0;
-    { int U = 1; for (auto& st : v.ups) { U *= st.u; max_elems = std::max(max_elems, (size_t)RY * U * st.cout); } }
-    const int ntmp = (a.resblock == 2) ? 2 : 4;
-    float* pool[6] = {nullptr};
-    if (!j.debug) for (int i = 0; i < 2 + ntmp; i++) pool[i] = c.dev.get<float>(max_elems);
-
-    const float* cur = p0; Level Lin = LY; int U = 1;
+    const float* cur = d.p0; Level Lin = LY; int U = 1;
     for (size_t i = 0; i < v.ups.size(); i++) {
         const UpStageW& st = v.ups[i];
         const int Uo = U * st.u;
-        Level Lo; Lo.map = {d_yend, GY * Uo, Uo, RY * Uo}; Lo.valid_rows = LY.valid_rows * Uo;
-        const size_t elems = (size_t)RY * Uo * st.cout;
-        float *up, *ys, *tmp[3];
-        if (j.debug) {
-            up = c.dev.get<float>(elems); ys = c.dev.get<float>(elems);
-            for (int t = 0; t < 3; t++) tmp[t] = c.dev.get<float>(elems);
-        } else {
-            ys = pool[i & 1]; up = pool[2];
-            tmp[0] = pool[3]; tmp[1] = ntmp > 2 ? pool[4] : nullptr; tmp[2] = ntmp > 2 ? pool[5] : nullptr;
-        }
+        Level Lo; Lo.map = {y.yend, GY * Uo, Uo, RY * Uo}; Lo.valid_rows = LY.valid_rows * Uo;
+        float *up = d.stage[i][0], *ys = d.stage[i][1];
+        float* const* tmp = &d.stage[i][2];
         R.begin("dec.up" + std::to_string(i));
         bool fused_done = false;
         if (v.backend >= 1 && st.fused.wtc) {
@@ -335,20 +464,16 @@ void run_decoder(Runner& R, const Level& LY, const float* s, float* d_wav, const
             }
         }
         R.end();
-        if (j.debug) {
-            j.dbg["dec.up" + std::to_string(i)] = {up, st.cout}; j.dbg_level["dec.up" + std::to_string(i)] = Uo;
-            j.dbg["dec.mrf" + std::to_string(i)] = {ys, st.cout}; j.dbg_level["dec.mrf" + std::to_string(i)] = Uo;
-        }
         cur = ys; Lin = Lo; U = Uo;
     }
     R.begin("dec.post");
-    launch_conv_post(cur, v.c_last, v.conv_post_w, d_wav, d_fsegs, d_ftile, U, Lin.map, R.st);
+    launch_conv_post(cur, v.c_last, v.conv_post_w, d_wav, y.fsegs, y.ftile, U, Lin.map, R.st);
     R.count(2.0 * Lin.valid_rows * v.c_last * 7, 4.0 * Lin.valid_rows * (v.c_last + 1));
     R.end();
 }
 
-// Build the Y-level tables for given per-utterance frame counts; uploads them; returns the level.
-Level build_y_layout(Job& j, Context& c, cudaStream_t st, const std::vector<int>& y_len, int hop) {
+// Lays out the frame level for given per-utterance frame counts (host side: segments, rows, output offsets).
+void lay_out_frames(Job& j, const std::vector<int>& y_len, int hop) {
     const size_t B = y_len.size();
     j.fsegs.resize(B);
     int cur = 0; long long out = 0;
@@ -362,38 +487,24 @@ Level build_y_layout(Job& j, Context& c, cudaStream_t st, const std::vector<int>
         cur += round_up(y_len[b] + HY, GY);
     }
     j.RY = cur; j.total_samples = out;
+}
+
+// Fills the frame-level tables through their pinned mirrors; returns the level.
+Level upload_frames(const Job& j, const FrameTables& t, cudaStream_t st) {
+    const size_t B = j.fsegs.size();
     const int ntile = j.RY / GY;
-    std::vector<int> yend(ntile, 0), ftile(ntile, 0);
+    Level L; L.map = {t.yend, GY, 1, j.RY}; L.valid_rows = 0;
     for (size_t b = 0; b < B; b++) {
         const int t0 = j.fsegs[b].off / GY;
         const int t1 = (b + 1 < B ? j.fsegs[b + 1].off : j.RY) / GY;
-        for (int t = t0; t < t1; t++) { yend[t] = j.fsegs[b].off + j.fsegs[b].len; ftile[t] = (int)b; }
+        for (int k = t0; k < t1; k++) { t.yend_h[k] = j.fsegs[b].off + j.fsegs[b].len; t.ftile_h[k] = (int)b; }
+        L.valid_rows += j.fsegs[b].len;
     }
-    j.d_yend = c.dev.get<int>(ntile);
-    j.d_ftile = c.dev.get<int>(ntile);
-    j.d_fsegs = c.dev.get<FrameSeg>(B);
-    const size_t need = 2 * ntile * sizeof(int) + B * sizeof(FrameSeg);
-    // staging lives in the second half of the pinned buffer (the first half holds the X tables)
-    char* pin = c.pin + c.pin_cap / 2;
-    if (need > c.pin_cap / 2) throw Error(19, "internal: pinned staging too small");
-    memcpy(pin, yend.data(), ntile * sizeof(int));
-    memcpy(pin + ntile * sizeof(int), ftile.data(), ntile * sizeof(int));
-    memcpy(pin + 2 * ntile * sizeof(int), j.fsegs.data(), B * sizeof(FrameSeg));
-    h2d(j.d_yend, pin, ntile * sizeof(int), st);
-    h2d(j.d_ftile, pin + ntile * sizeof(int), ntile * sizeof(int), st);
-    h2d(j.d_fsegs, pin + 2 * ntile * sizeof(int), B * sizeof(FrameSeg), st);
-    Level L; L.map = {j.d_yend, GY, 1, j.RY};
-    L.valid_rows = 0; for (int y : y_len) L.valid_rows += y;
+    memcpy(t.fsegs_h, j.fsegs.data(), B * sizeof(FrameSeg));
+    h2d(t.yend, t.yend_h, ntile * sizeof(int), st);
+    h2d(t.ftile, t.ftile_h, ntile * sizeof(int), st);
+    h2d(t.fsegs, t.fsegs_h, B * sizeof(FrameSeg), st);
     return L;
-}
-
-size_t decoder_bytes(const Voice& v, int RY, bool debug) {
-    const Arch& a = v.a;
-    size_t tot = (size_t)RY * a.up_init * 4 + 4096;
-    size_t max_elems = 0, sum = 0; int U = 1;
-    for (auto& st : v.ups) { U *= st.u; const size_t e = (size_t)RY * U * st.cout; max_elems = std::max(max_elems, e); sum += e; }
-    tot += debug ? sum * 5 * 4 : max_elems * 6 * 4;
-    return tot + (1 << 20);
 }
 
 }  // namespace
@@ -407,117 +518,83 @@ void Job::run(float* d_out, size_t d_out_cap) {
     C.events_used = 0;
     if (!C.ev_begin) { SB_CUDA(cudaEventCreate(&C.ev_begin)); SB_CUDA(cudaEventCreate(&C.ev_end)); }
 
-    // ---------------- phase 1 workspace ----------------
+    // ---------------- id level (phase 1) workspace ----------------
     // tensor-core attention (two grouped GEMMs around a softmax): default backend, 96-wide heads, rows that fit the
     // softmax kernel's registers; otherwise the fp32 CUDA-core attention kernel
     const bool tc_att = V.backend == 1 && H / a.heads == 96 && max_tx <= 1280 && getenv("SB200_ATT_SIMT") == nullptr;
-    // xa xb qkv(3H) att d0 t1 t2 g = 10 H; ffn; stats; h29 32; zz 2 + eps_w 2; logw 1; + attention scratch (scores for
-    // every head, V^T, relative-value term)
-    const size_t xfloats = (size_t)RX * (H * 10 + F + 2 * I + 32 + 2 + 2 + 1) +
-                           (tc_att ? (size_t)a.heads * RX * att_tp + 2 * (size_t)RX * H : 0);
-    const size_t tile_bytes = (tiles_s.size() + tiles_o.size()) * sizeof(TfTile);
-    const size_t p1_bytes = xfloats * 4 + (size_t)RX * 20 + B * 64 + tile_bytes + (1 << 20) + (size_t)V.cond_rows * 4 + 1024 +
-                            (debug ? (size_t)RX * (5 * H + att_tp) * 4 + 4096 +
-                                     V.dp_flows.size() * ((size_t)RX * (H + 36) * 4 + 1024) : 0);
-    // The arena must also hold phase 2; sizes are only known after the durations come back, so phase 1
-    // runs in the front of the arena and phase 2 re-plans behind it (growing = realloc would lose phase-1
-    // results, so grow conservatively up front from the mean-duration estimate, then verify).
-    const double est_frames = 4.0 * (double)ids.size() + 256.0 * B;
-    size_t est_p2 = decoder_bytes(V, (int)std::min<double>(est_frames, 2.0e9 / 256), debug) + (size_t)(est_frames * I * 4 * 6);
-    C.ensure_dev(p1_bytes + est_p2);
-    C.ensure_pin(std::max<size_t>((size_t)RX * 12 + B * 64 + tile_bytes + (1 << 16), 1 << 20));
-    C.dev.used = 0; C.dev.dry = false;
+    IdBufs x;
+    plan(C.dev_id, C.pin, [&](Arena& dev, Arena& pin) { x.carve(dev, pin, *this, tc_att); });
+    d_cum = x.cum; d_cond = x.cond;
     Runner R(*this);
 
     SB_CUDA(cudaEventRecord(C.ev_begin, st));
     // tables
     const int nxg = RX / GX;
-    std::vector<int> xend(nxg, 0), xseg_of(nxg, 0);
-    int* ids_rows_h = reinterpret_cast<int*>(C.pin);
-    for (int r = 0; r < RX; r++) ids_rows_h[r] = -1;
+    std::fill(x.ids_rows_h, x.ids_rows_h + RX, -1);
+    std::fill(x.xend_h, x.xend_h + nxg, 0);
+    std::fill(x.xseg_of_h, x.xseg_of_h + nxg, 0);
     for (size_t b = 0; b < B; b++) {
         const SegInfo& s = xsegs[b];
-        for (int i = 0; i < s.len; i++) ids_rows_h[s.off + i] = (int)ids[offs[b] + i];
+        for (int i = 0; i < s.len; i++) x.ids_rows_h[s.off + i] = (int)ids[offs[b] + i];
         const int g0 = s.off / GX, g1 = (b + 1 < B ? xsegs[b + 1].off : RX) / GX;
-        for (int g = g0; g < g1; g++) { xend[g] = s.off + s.len; xseg_of[g] = (int)b; }
+        for (int g = g0; g < g1; g++) { x.xend_h[g] = s.off + s.len; x.xseg_of_h[g] = (int)b; }
     }
-    int* xend_h = ids_rows_h + RX;
-    memcpy(xend_h, xend.data(), nxg * sizeof(int));
-    int* xseg_of_h = xend_h + nxg;
-    memcpy(xseg_of_h, xseg_of.data(), nxg * sizeof(int));
-    SegInfo* xsegs_h = reinterpret_cast<SegInfo*>(xseg_of_h + nxg);
-    memcpy(xsegs_h, xsegs.data(), B * sizeof(SegInfo));
-    // result slot of the frame counts, then (8-byte aligned) the attention tile tables
-    const size_t ylen_off = ((size_t)RX * 4 + (size_t)nxg * 8 + B * sizeof(SegInfo) + 63) & ~(size_t)63;
-    const size_t tiles_off = (ylen_off + B * sizeof(int) + 63) & ~(size_t)63;
-    TfTile* tiles_h = reinterpret_cast<TfTile*>(C.pin + tiles_off);
-    d_ids_rows = C.dev.get<int>(RX); d_xend = C.dev.get<int>(nxg); d_xseg_of_gran = C.dev.get<int>(nxg); d_xsegs = C.dev.get<SegInfo>(B);
-    d_cum = C.dev.get<int>(RX); d_ylen = C.dev.get<int>(B);
-    h2d(d_ids_rows, ids_rows_h, (size_t)RX * 4, st);
-    h2d(d_xend, xend_h, (size_t)nxg * 4, st);
-    h2d(d_xseg_of_gran, xseg_of_h, (size_t)nxg * 4, st);
-    h2d(d_xsegs, xsegs_h, B * sizeof(SegInfo), st);
-    d_tiles_s = d_tiles_o = nullptr;
+    memcpy(x.xsegs_h, xsegs.data(), B * sizeof(SegInfo));
+    h2d(x.ids_rows, x.ids_rows_h, (size_t)RX * 4, st);
+    h2d(x.xend, x.xend_h, (size_t)nxg * 4, st);
+    h2d(x.xseg_of_gran, x.xseg_of_h, (size_t)nxg * 4, st);
+    h2d(x.xsegs, x.xsegs_h, B * sizeof(SegInfo), st);
     if (tc_att) {
-        memcpy(tiles_h, tiles_s.data(), tiles_s.size() * sizeof(TfTile));
-        memcpy(tiles_h + tiles_s.size(), tiles_o.data(), tiles_o.size() * sizeof(TfTile));
-        d_tiles_s = C.dev.get<TfTile>(tiles_s.size() + tiles_o.size());
-        d_tiles_o = d_tiles_s + tiles_s.size();
-        h2d(d_tiles_s, tiles_h, tile_bytes, st);
+        memcpy(x.tiles_h, tiles_s.data(), tiles_s.size() * sizeof(TfTile));
+        memcpy(x.tiles_h + tiles_s.size(), tiles_o.data(), tiles_o.size() * sizeof(TfTile));
+        h2d(x.tiles, x.tiles_h, (tiles_s.size() + tiles_o.size()) * sizeof(TfTile), st);
     }
 
-    Level LX; LX.map = {d_xend, GX, 1, RX}; LX.valid_rows = (long long)ids.size();
-    float* xa = C.dev.get<float>((size_t)RX * H);
-    float* xb = C.dev.get<float>((size_t)RX * H);
-    float* qkv = C.dev.get<float>((size_t)RX * 3 * H);
-    float* att = C.dev.get<float>((size_t)RX * H);
-    float* ffn = C.dev.get<float>((size_t)RX * F);
-    float* stats = C.dev.get<float>((size_t)RX * 2 * I);
-    float* d0 = C.dev.get<float>((size_t)RX * H);
-    float* t1 = C.dev.get<float>((size_t)RX * H);
-    float* t2 = C.dev.get<float>((size_t)RX * H);
-    float* g = C.dev.get<float>((size_t)RX * H);
-    float* h29 = C.dev.get<float>((size_t)RX * 32);
-    float* zz = C.dev.get<float>((size_t)RX * 2);
-    float* logw = C.dev.get<float>((size_t)RX);
-    float *att_s = nullptr, *att_vt = nullptr, *att_orel = nullptr;
+    Level LX; LX.map = {x.xend, GX, 1, RX}; LX.valid_rows = (long long)ids.size();
     TfGemm gs{}, go{};
     bool tc_att_ok = tc_att;
     if (tc_att) {
-        att_s = C.dev.get<float>((size_t)a.heads * RX * att_tp);
-        att_vt = C.dev.get<float>((size_t)H * RX);
-        att_orel = C.dev.get<float>((size_t)RX * H);
-        gs.a = qkv; gs.a_rows = RX; gs.a_cols = 3 * H; gs.lda = 3 * H;
-        gs.b = qkv; gs.b_rows = RX; gs.b_cols = 3 * H; gs.ldb = 3 * H;
-        gs.nth = att_nth_s; gs.y = att_s; gs.ldy = att_tp; gs.res = nullptr; gs.scale = 1.0f / sqrtf((float)(H / a.heads));
-        gs.tiles = d_tiles_s; gs.ntiles = (int)tiles_s.size();
-        go.a = att_s; go.a_rows = a.heads * RX; go.a_cols = att_tp; go.lda = att_tp;
-        go.b = att_vt; go.b_rows = H; go.b_cols = RX; go.ldb = RX;
-        go.nth = att_nth_o; go.y = att; go.ldy = H; go.res = att_orel; go.scale = 1.f;
-        go.tiles = d_tiles_o; go.ntiles = (int)tiles_o.size();
+        gs.a = x.qkv; gs.a_rows = RX; gs.a_cols = 3 * H; gs.lda = 3 * H;
+        gs.b = x.qkv; gs.b_rows = RX; gs.b_cols = 3 * H; gs.ldb = 3 * H;
+        gs.nth = att_nth_s; gs.y = x.att_s; gs.ldy = att_tp; gs.res = nullptr; gs.scale = 1.0f / sqrtf((float)(H / a.heads));
+        gs.tiles = x.tiles; gs.ntiles = (int)tiles_s.size();
+        go.a = x.att_s; go.a_rows = a.heads * RX; go.a_cols = att_tp; go.lda = att_tp;
+        go.b = x.att_vt; go.b_rows = H; go.b_cols = RX; go.ldb = RX;
+        go.nth = att_nth_o; go.y = x.att; go.ldy = H; go.res = x.att_orel; go.scale = 1.f;
+        go.tiles = x.tiles + tiles_s.size(); go.ntiles = (int)tiles_o.size();
         tc_att_ok = gemm_tf_supported(gs) && gemm_tf_supported(go);
     }
-    d_epsw = nullptr;
-    if (cfg.noise_w != 0.f) {
-        d_epsw = C.dev.get<float>((size_t)RX * 2);
+    if (debug) {
+        expose(*this, "x", x.xa, H, 0); expose(*this, "stats", x.stats, 2 * I, 0);
+        expose(*this, "qkv0", x.qkv0, 3 * H, 0); expose(*this, "att0", x.att0, H, 0);
+        if (tc_att_ok) {
+            expose(*this, "p0", x.p0, att_tp, 0);      // head 0 probabilities
+            expose(*this, "vt0", x.vt0, H, -1);        // stored as [H][RX]
+        }
+        expose(*this, "dp.g", x.g, H, 0); expose(*this, "logw", x.logw, 1, 0);
+        for (size_t s = 0; s < x.dpf.size(); s++) {
+            const std::string fs = "dp.f" + std::to_string(s) + ".";
+            expose(*this, fs + "in", x.dpf[s][0], 2, 0); expose(*this, fs + "h", x.dpf[s][1], H, 0);
+            expose(*this, fs + "h29", x.dpf[s][2], 32, 0); expose(*this, fs + "out", x.dpf[s][3], 2, 0);
+        }
+    }
+    if (x.epsw) {
         if (!eps_w.empty()) {
             std::vector<float> stage((size_t)RX * 2, 0.f);
             for (size_t b = 0; b < B; b++)
                 if (!eps_w[b].empty()) memcpy(stage.data() + (size_t)xsegs[b].off * 2, eps_w[b].data(), eps_w[b].size() * 4);
-            SB_CUDA(cudaMemcpyAsync(d_epsw, stage.data(), stage.size() * 4, cudaMemcpyHostToDevice, st));
+            SB_CUDA(cudaMemcpyAsync(x.epsw, stage.data(), stage.size() * 4, cudaMemcpyHostToDevice, st));
             SB_CUDA(cudaStreamSynchronize(st));   // `stage` is pageable; injection is a test-only path
         } else {
-            launch_randn(d_epsw, (long long)RX * 2, V.noise_seed, 2 * noise_call, st);
+            launch_randn(x.epsw, (long long)RX * 2, V.noise_seed, 2 * noise_call, st);
         }
     }
 
     // ---------------- speaker conditioning (multi-speaker voices) ----------------
-    d_cond = nullptr;
-    if (V.num_speakers > 1) {
+    if (x.cond) {
         const long long sid = cfg.has_speaker ? cfg.speaker : 0;      // piper/src/lib.rs:353-358: speaker.unwrap_or(0)
         if (sid < 0 || sid >= V.emb_rows) throw Error(19, "Failed to run model inference. Error: speaker id out of range");
-        d_cond = C.dev.get<float>((size_t)V.cond_rows);
-        launch_cond_bias(V.cond_w, V.cond_base, V.emb_g + (size_t)sid * V.gin, V.cond_rows, V.gin, d_cond, st);
+        launch_cond_bias(V.cond_w, V.cond_base, V.emb_g + (size_t)sid * V.gin, V.cond_rows, V.gin, x.cond, st);
     }
 
     // ---------------- text encoder ----------------
@@ -525,89 +602,72 @@ void Job::run(float* d_out, size_t d_out_cap) {
     // attention contractions run on conv_tf.cu (wgmma, error-compensated tf32, chunk-flushed accumulation: fp32-class
     // accuracy, DESIGN.md section 4); backend 0 / 2 keep them on the fp32 CUDA-core kernels.
     R.begin("enc");
-    launch_embed(d_ids_rows, V.emb, sqrtf((float)H), xa, RX, H, st);
+    launch_embed(x.ids_rows, V.emb, sqrtf((float)H), x.xa, RX, H, st);
     R.count(0, 4.0 * LX.valid_rows * H);
     for (int l = 0; l < a.layers; l++) {
         const EncLayer& e = V.enc[l];
         {
-            Runner::Opt o; o.y0 = qkv; o.ldy0 = 3 * H; o.tf_ok = true;
-            if (tc_att_ok) { o.yt = att_vt; o.yt_col0 = 2 * H; o.ldyt = RX; }       // V leaves transposed: [H][RX]
-            R.conv(e.qkv, xa, H, LX, o);
+            Runner::Opt o; o.y0 = x.qkv; o.ldy0 = 3 * H; o.tf_ok = true;
+            if (tc_att_ok) { o.yt = x.att_vt; o.yt_col0 = 2 * H; o.ldyt = RX; }       // V leaves transposed: [H][RX]
+            R.conv(e.qkv, x.xa, H, LX, o);
         }
         if (tc_att_ok) {
             launch_gemm_tf(gs, st);
-            launch_attn_softmax(att_s, att_tp, qkv, 3 * H, e.relk, e.relv, a.window, att_orel, H, H, a.heads, RX, d_xsegs,
-                                d_xseg_of_gran, GX, max_tx, st);
+            launch_attn_softmax(x.att_s, att_tp, x.qkv, 3 * H, e.relk, e.relv, a.window, x.att_orel, H, H, a.heads, RX,
+                                x.xsegs, x.xseg_of_gran, GX, max_tx, st);
             launch_gemm_tf(go, st);
             R.count(0, 0, 2);
         } else {
-            launch_attention(qkv, 3 * H, e.relk, e.relv, a.window, att, H, H, a.heads, d_xsegs, (int)B, max_tx, st);
+            launch_attention(x.qkv, 3 * H, e.relk, e.relv, a.window, x.att, H, H, a.heads, x.xsegs, (int)B, max_tx, st);
         }
         { double f = 0; for (auto& s : xsegs) f += 4.0 * (double)s.len * s.len * H; R.count(f, 16.0 * LX.valid_rows * H); }
         if (debug && l == 0) {      // first-layer attention operands / result (tests/test_gpu_parity.py)
-            float* qk = C.dev.get<float>((size_t)RX * 3 * H);
-            float* at = C.dev.get<float>((size_t)RX * H);
-            SB_CUDA(cudaMemcpyAsync(qk, qkv, (size_t)RX * 3 * H * 4, cudaMemcpyDeviceToDevice, st));
-            SB_CUDA(cudaMemcpyAsync(at, att, (size_t)RX * H * 4, cudaMemcpyDeviceToDevice, st));
-            dbg["qkv0"] = {qk, 3 * H}; dbg_level["qkv0"] = 0; dbg["att0"] = {at, H}; dbg_level["att0"] = 0;
+            d2d(x.qkv0, x.qkv, (size_t)RX * 3 * H, st);
+            d2d(x.att0, x.att, (size_t)RX * H, st);
             if (tc_att_ok) {
-                float* sp = C.dev.get<float>((size_t)RX * att_tp);
-                SB_CUDA(cudaMemcpyAsync(sp, att_s, (size_t)RX * att_tp * 4, cudaMemcpyDeviceToDevice, st));
-                dbg["p0"] = {sp, att_tp}; dbg_level["p0"] = 0;     // head 0 probabilities
-                // V went only to att_vt (the V columns of qkv0 are not written on this path): captured as [H][RX]
-                float* vt = C.dev.get<float>((size_t)H * RX);
-                SB_CUDA(cudaMemcpyAsync(vt, att_vt, (size_t)H * RX * 4, cudaMemcpyDeviceToDevice, st));
-                dbg["vt0"] = {vt, H}; dbg_level["vt0"] = -1;
+                d2d(x.p0, x.att_s, (size_t)RX * att_tp, st);
+                // V went only to att_vt (the V columns of qkv0 are not written on this path)
+                d2d(x.vt0, x.att_vt, (size_t)H * RX, st);
             }
         }
-        { Runner::Opt o; o.y0 = xb; o.ldy0 = H; o.tf_ok = true; R.conv(e.o, att, H, LX, o); }
-        launch_ln(xa, xb, nullptr, e.g1, e.b1, xa, H, 0, LX.map, st);
+        { Runner::Opt o; o.y0 = x.xb; o.ldy0 = H; o.tf_ok = true; R.conv(e.o, x.att, H, LX, o); }
+        launch_ln(x.xa, x.xb, nullptr, e.g1, e.b1, x.xa, H, 0, LX.map, st);
         R.count(0, 12.0 * LX.valid_rows * H);
-        { Runner::Opt o; o.act = ACT_RELU; o.y0 = ffn; o.ldy0 = F; o.tf_ok = true; R.conv(e.ffn1, xa, H, LX, o); }
-        { Runner::Opt o; o.y0 = xb; o.ldy0 = H; o.tf_ok = true; R.conv(e.ffn2, ffn, F, LX, o); }
-        launch_ln(xa, xb, nullptr, e.g2, e.b2, xa, H, 0, LX.map, st);
+        { Runner::Opt o; o.act = ACT_RELU; o.y0 = x.ffn; o.ldy0 = F; o.tf_ok = true; R.conv(e.ffn1, x.xa, H, LX, o); }
+        { Runner::Opt o; o.y0 = x.xb; o.ldy0 = H; o.tf_ok = true; R.conv(e.ffn2, x.ffn, F, LX, o); }
+        launch_ln(x.xa, x.xb, nullptr, e.g2, e.b2, x.xa, H, 0, LX.map, st);
         R.count(0, 12.0 * LX.valid_rows * H);
     }
-    { Runner::Opt o; o.y0 = stats; o.ldy0 = 2 * I; o.tf_ok = true; R.conv(V.enc_proj, xa, H, LX, o); }
+    { Runner::Opt o; o.y0 = x.stats; o.ldy0 = 2 * I; o.tf_ok = true; R.conv(V.enc_proj, x.xa, H, LX, o); }
     R.end();
-    if (debug) { dbg["x"] = {xa, H}; dbg_level["x"] = 0; dbg["stats"] = {stats, 2 * I}; dbg_level["stats"] = 0; }
 
     // ---------------- stochastic duration predictor (reverse) ----------------
     R.begin("dp");
-    { Runner::Opt o; o.y0 = d0; o.ldy0 = H; o.tf_ok = true; R.conv(V.dp_pre, xa, H, LX, o); }
-    R.dds(V.dp_dds, d0, t1, t2, LX);
-    { Runner::Opt o; o.y0 = g; o.ldy0 = H; o.tf_ok = true; R.conv(V.dp_proj, d0, H, LX, o); }
-    launch_scale_copy2(d_epsw, cfg.noise_w, zz, LX.map, st);
-    if (debug) { dbg["dp.g"] = {g, H}; dbg_level["dp.g"] = 0; }
-    // debug: each flow's input, DDSConv output, spline parameters and output (zz, d0 and h29 are reused: copies)
-    auto capture = [&](const std::string& name, const float* src, int cols) {
-        float* cp = C.dev.get<float>((size_t)RX * cols);
-        SB_CUDA(cudaMemcpyAsync(cp, src, (size_t)RX * cols * 4, cudaMemcpyDeviceToDevice, st));
-        dbg[name] = {cp, cols}; dbg_level[name] = 0;
-    };
+    { Runner::Opt o; o.y0 = x.d0; o.ldy0 = H; o.tf_ok = true; R.conv(V.dp_pre, x.xa, H, LX, o); }
+    R.dds(V.dp_dds, x.d0, x.t1, x.t2, LX);
+    { Runner::Opt o; o.y0 = x.g; o.ldy0 = H; o.tf_ok = true; R.conv(V.dp_proj, x.d0, H, LX, o); }
+    launch_scale_copy2(x.epsw, cfg.noise_w, x.zz, LX.map, st);
+    // debug: zz, d0 and h29 are reused by every flow, so each flow's stages are captured as copies
     for (size_t s = 0; s < V.dp_flows.size(); s++) {
         const CFlowW& cf = V.dp_flows[s];
-        const std::string fs = "dp.f" + std::to_string(s) + ".";
-        if (debug) capture(fs + "in", zz, 2);
-        launch_flow_pre(zz, cf.ccol, cf.pre_w, cf.pre_b, g, d0, H, LX.map, st);
+        if (debug) d2d(x.dpf[s][0], x.zz, (size_t)RX * 2, st);
+        launch_flow_pre(x.zz, cf.ccol, cf.pre_w, cf.pre_b, x.g, x.d0, H, LX.map, st);
         R.count(2.0 * LX.valid_rows * H, 8.0 * LX.valid_rows * H);
-        R.dds(cf.dds, d0, t1, t2, LX);
-        if (debug) capture(fs + "h", d0, H);
-        { Runner::Opt o; o.y0 = h29; o.ldy0 = 32; o.tf_ok = true; R.conv(cf.proj, d0, H, LX, o); }
-        if (debug) capture(fs + "h29", h29, 32);
-        launch_spline(h29, 32, zz, cf.tcol, a.dp_bins, 1.0f / sqrtf((float)H), LX.map, st);
+        R.dds(cf.dds, x.d0, x.t1, x.t2, LX);
+        if (debug) d2d(x.dpf[s][1], x.d0, (size_t)RX * H, st);
+        { Runner::Opt o; o.y0 = x.h29; o.ldy0 = 32; o.tf_ok = true; R.conv(cf.proj, x.d0, H, LX, o); }
+        if (debug) d2d(x.dpf[s][2], x.h29, (size_t)RX * 32, st);
+        launch_spline(x.h29, 32, x.zz, cf.tcol, a.dp_bins, 1.0f / sqrtf((float)H), LX.map, st);
         R.count(0, 4.0 * LX.valid_rows * 34);
-        if (debug) capture(fs + "out", zz, 2);
+        if (debug) d2d(x.dpf[s][3], x.zz, (size_t)RX * 2, st);
     }
-    launch_durations(zz, V.ea_m0, V.ea_logs0, cfg.length_scale, d_xsegs, (int)B, logw, d_cum, d_ylen, st);
+    launch_durations(x.zz, V.ea_m0, V.ea_logs0, cfg.length_scale, x.xsegs, (int)B, x.logw, x.cum, x.ylen, st);
     R.end();
-    if (debug) { dbg["logw"] = {logw, 1}; dbg_level["logw"] = 0; }
 
     // ---------------- host learns the frame counts (the graph's data-dependent shape) ----------------
-    int* ylen_h = reinterpret_cast<int*>(C.pin + ylen_off);
-    SB_CUDA(cudaMemcpyAsync(ylen_h, d_ylen, B * sizeof(int), cudaMemcpyDeviceToHost, st));
+    SB_CUDA(cudaMemcpyAsync(x.ylen_h, x.ylen, B * sizeof(int), cudaMemcpyDeviceToHost, st));
     SB_CUDA(cudaStreamSynchronize(st));
-    y_len.assign(ylen_h, ylen_h + B);
+    y_len.assign(x.ylen_h, x.ylen_h + B);
     long long tot_frames = 0;
     for (int y : y_len) tot_frames += y;
     if (tot_frames > (long long)(2.0e9 / 256 / 4)) throw Error(19, "Failed to run model inference. Error: predicted durations are unreasonably long");
@@ -616,82 +676,55 @@ void Job::run(float* d_out, size_t d_out_cap) {
             if (!eps_z[b].empty() && eps_z_frames[b] != (size_t)y_len[b])
                 throw Error(19, "injected eps_z has " + std::to_string(eps_z_frames[b]) + " frames but the model produced " + std::to_string(y_len[b]));
 
-    // ---------------- phase 2 workspace (plan, then make sure it fits behind phase 1) ----------------
-    {
-        int cur = 0;
-        for (int y : y_len) cur += round_up(y + HY, GY);
-        const size_t need = C.dev.used + decoder_bytes(V, cur, debug) + (size_t)cur * (size_t)(5 * I + 3 * H) * 4 +
-                            (size_t)tot_frames * a.hop() * 4 + (8 << 20);
-        if (need > C.dev.cap) {
-            // grow: allocate a bigger arena and carry the phase-1 results over
-            Arena old = C.dev;
-            C.dev.base = nullptr; C.dev.cap = 0;
-            void* p = nullptr;
-            SB_CUDA(cudaMalloc(&p, need + need / 8));
-            C.dev.base = (char*)p; C.dev.cap = need + need / 8; C.dev.used = old.used;
-            SB_CUDA(cudaMemcpyAsync(C.dev.base, old.base, old.used, cudaMemcpyDeviceToDevice, st));
-            SB_CUDA(cudaStreamSynchronize(st));
-            const ptrdiff_t delta = C.dev.base - old.base;
-            auto mv = [&](auto*& ptr) { if (ptr) ptr = reinterpret_cast<std::remove_reference_t<decltype(ptr)>>(reinterpret_cast<char*>(ptr) + delta); };
-            mv(d_ids_rows); mv(d_xend); mv(d_xsegs); mv(d_cum); mv(d_ylen); mv(d_epsw); mv(d_xseg_of_gran); mv(d_tiles_s); mv(d_tiles_o); mv(d_cond);
-            mv(xa); mv(stats); mv(logw);
-            for (auto& kv : dbg) kv.second.first = reinterpret_cast<float*>(reinterpret_cast<char*>(kv.second.first) + delta);
-            SB_CUDA(cudaFree(old.base));
-        }
+    // ---------------- frame level (phase 2) workspace ----------------
+    // The stream is idle here, so the pinned staging of the X tables can be reused for the Y tables.
+    lay_out_frames(*this, y_len, a.hop());
+    FrameBufs f;
+    plan(C.dev_frame, C.pin, [&](Arena& dev, Arena& pin) { f.carve(dev, pin, *this, d_out == nullptr); });
+    d_fsegs = f.y.fsegs;
+    if (debug) {
+        expose(*this, "z_p", f.zp, I, 1); expose(*this, "z", f.s, I, 1);
+        if (!encode_only) f.dec.expose_to(*this);
     }
-    Level LY = build_y_layout(*this, C, st, y_len, a.hop());
+    Level LY = upload_frames(*this, f.y, st);
 
     // ---------------- alignment expansion ----------------
     R.begin("align");
-    float* s = C.dev.get<float>((size_t)RY * I);
-    d_epsz = nullptr;
-    if (cfg.noise_scale != 0.f) {
-        d_epsz = C.dev.get<float>((size_t)RY * I);
+    if (f.epsz) {
         if (!eps_z.empty()) {
             std::vector<float> stage((size_t)RY * I, 0.f);
             for (size_t b = 0; b < B; b++)
                 if (!eps_z[b].empty()) memcpy(stage.data() + (size_t)fsegs[b].off * I, eps_z[b].data(), eps_z[b].size() * 4);
-            SB_CUDA(cudaMemcpyAsync(d_epsz, stage.data(), stage.size() * 4, cudaMemcpyHostToDevice, st));
+            SB_CUDA(cudaMemcpyAsync(f.epsz, stage.data(), stage.size() * 4, cudaMemcpyHostToDevice, st));
             SB_CUDA(cudaStreamSynchronize(st));
         } else {
-            launch_randn(d_epsz, (long long)RY * I, V.noise_seed, 2 * noise_call + 1, st);
+            launch_randn(f.epsz, (long long)RY * I, V.noise_seed, 2 * noise_call + 1, st);
         }
     }
-    launch_expand(stats, 2 * I, I, d_cum, d_epsz, cfg.noise_scale, s, d_fsegs, d_ftile, LY.map, st);
+    launch_expand(x.stats, 2 * I, I, x.cum, f.epsz, cfg.noise_scale, f.s, f.y.fsegs, f.y.ftile, LY.map, st);
     R.count(0, 4.0 * LY.valid_rows * 3 * I);
     R.end();
-    float* zp_dbg = nullptr;
-    if (debug) {
-        zp_dbg = C.dev.get<float>((size_t)RY * I);
-        SB_CUDA(cudaMemcpyAsync(zp_dbg, s, (size_t)RY * I * 4, cudaMemcpyDeviceToDevice, st));
-        dbg["z_p"] = {zp_dbg, I}; dbg_level["z_p"] = 1;
-    }
+    if (debug) d2d(f.zp, f.s, (size_t)RY * I, st);
 
     // ---------------- residual-coupling flow (reverse) ----------------
     R.begin("flow");
-    float* h = C.dev.get<float>((size_t)RY * H);
-    float* acts = C.dev.get<float>((size_t)RY * H);
-    float* outb = C.dev.get<float>((size_t)RY * H);
-    const int half = I / 2;
     for (const CouplingW& cp : V.flows) {
-        { Runner::Opt o; o.y0 = h; o.ldy0 = H; o.tc_ok = true; R.conv(cp.pre, s + cp.cond_off, I, LY, o); }
+        { Runner::Opt o; o.y0 = f.h; o.ldy0 = H; o.tc_ok = true; R.conv(cp.pre, f.s + cp.cond_off, I, LY, o); }
         const int n = (int)cp.in.size();
         for (int l = 0; l < n; l++) {
-            { Runner::Opt o; o.act = ACT_GATE; o.y0 = acts; o.ldy0 = H; o.tc_ok = true; R.conv(cp.in[l], h, H, LY, o); }
+            { Runner::Opt o; o.act = ACT_GATE; o.y0 = f.acts; o.ldy0 = H; o.tc_ok = true; R.conv(cp.in[l], f.h, H, LY, o); }
             Runner::Opt o; o.tc_ok = true;
-            if (l < n - 1) { o.y0 = h; o.ldy0 = H; o.acc0 = 1; o.split = H; o.y1 = outb; o.ldy1 = H; o.acc1 = l > 0; }
-            else { o.split = 0; o.y0 = outb; o.ldy0 = H; o.y1 = outb; o.ldy1 = H; o.acc1 = l > 0; }
-            R.conv(cp.rs[l], acts, H, LY, o);
+            if (l < n - 1) { o.y0 = f.h; o.ldy0 = H; o.acc0 = 1; o.split = H; o.y1 = f.outb; o.ldy1 = H; o.acc1 = l > 0; }
+            else { o.split = 0; o.y0 = f.outb; o.ldy0 = H; o.y1 = f.outb; o.ldy1 = H; o.acc1 = l > 0; }
+            R.conv(cp.rs[l], f.acts, H, LY, o);
         }
-        { Runner::Opt o; o.y0 = s + cp.tgt_off; o.ldy0 = I; o.acc0 = 1; o.scale = -1.f; o.tc_ok = true; R.conv(cp.post, outb, H, LY, o); }
+        { Runner::Opt o; o.y0 = f.s + cp.tgt_off; o.ldy0 = I; o.acc0 = 1; o.scale = -1.f; o.tc_ok = true; R.conv(cp.post, f.outb, H, LY, o); }
     }
-    (void)half;
     R.end();
-    if (debug) { dbg["z"] = {s, I}; dbg_level["z"] = 1; }
 
     // ---------------- HiFi-GAN ----------------
     if (encode_only) {
-        z_dev = s;
+        z_dev = f.s;
         SB_CUDA(cudaEventRecord(C.ev_end, st));
         SB_CUDA(cudaStreamSynchronize(st));
         SB_CUDA(cudaGetLastError());
@@ -701,11 +734,11 @@ void Job::run(float* d_out, size_t d_out_cap) {
     }
     if (d_out) {
         if ((size_t)total_samples > d_out_cap) throw Error(19, "caller-provided device output buffer is too small");
-        d_wav = d_out; wav_external = true;
+        d_wav = d_out;
     } else {
-        d_wav = C.dev.get<float>((size_t)total_samples + 4); wav_external = false;
+        d_wav = f.wav;
     }
-    run_decoder(R, LY, s, d_wav, d_fsegs, d_ftile, d_yend);
+    run_decoder(R, LY, f.y, f.dec, f.s, d_wav);
     SB_CUDA(cudaEventRecord(C.ev_end, st));
     SB_CUDA(cudaStreamSynchronize(st));
     SB_CUDA(cudaGetLastError());
@@ -734,49 +767,46 @@ Latent* encode_latent(Voice* v, const long long* ids, size_t n) {
 
 namespace {
 // decoder on z[lo:hi) with the result left on the device (job-owned arena): shared by the f32 and the PCM entry points
-float* decode_chunk_device(Voice* v, const Latent* z, long long lo, long long hi, Job& j, size_t extra_bytes) {
+ChunkBufs decode_chunk_device(Voice* v, const Latent* z, long long lo, long long hi, Job& j, bool pcm) {
     if (lo < 0 || hi > z->frames || lo >= hi) throw Error(19, "Invalid model audio output");
     const Arch& a = v->a;
     j.v = v; j.B = 1; j.ctx = v->acquire();
     Context& C = *j.ctx;
     SB_CUDA(cudaSetDevice(v->device));
     const int n = (int)(hi - lo);
-    const int RY = round_up(n + HY, GY);
-    C.ensure_dev(decoder_bytes(*v, RY, false) + (size_t)RY * a.inter * 4 + (size_t)n * a.hop() * 4 + extra_bytes + (size_t)v->cond_rows * 4 + (4 << 20));
-    C.ensure_pin(std::max<size_t>(1 << 20, (size_t)n * a.hop() * 4 + 4096));
-    C.dev.used = 0; C.events_used = 0;
+    lay_out_frames(j, std::vector<int>{n}, a.hop());
+    ChunkBufs b;
+    plan(C.dev_frame, C.pin, [&](Arena& dev, Arena& pin) { b.carve(dev, pin, j, pcm); });
+    j.d_cond = b.cond; j.d_fsegs = b.y.fsegs; j.d_wav = b.wav;
+    C.events_used = 0;
     if (!C.ev_begin) { SB_CUDA(cudaEventCreate(&C.ev_begin)); SB_CUDA(cudaEventCreate(&C.ev_end)); }
     cudaStream_t st = C.stream;
     Runner R(j);
     SB_CUDA(cudaEventRecord(C.ev_begin, st));
-    if (v->num_speakers > 1) {       // decoder.onnx takes the encoder's `g` (piper/src/lib.rs:706-735, 739-743)
+    if (b.cond) {       // decoder.onnx takes the encoder's `g` (piper/src/lib.rs:706-735, 739-743)
         if (z->sid < 0 || z->sid >= v->emb_rows) throw Error(19, "Failed to run model inference. Error: speaker id out of range");
-        j.d_cond = C.dev.get<float>((size_t)v->cond_rows);
-        launch_cond_bias(v->cond_w, v->cond_base, v->emb_g + (size_t)z->sid * v->gin, v->cond_rows, v->gin, j.d_cond, st);
+        launch_cond_bias(v->cond_w, v->cond_base, v->emb_g + (size_t)z->sid * v->gin, v->cond_rows, v->gin, b.cond, st);
     }
-    Level LY = build_y_layout(j, C, st, std::vector<int>{n}, a.hop());
-    float* s = C.dev.get<float>((size_t)RY * a.inter);
-    launch_fill_zero(s, (long long)RY * a.inter, st);
-    SB_CUDA(cudaMemcpyAsync(s, z->z + (size_t)lo * a.inter, (size_t)n * a.inter * 4, cudaMemcpyDeviceToDevice, st));
-    float* d_wav = C.dev.get<float>((size_t)j.total_samples + 4);
-    run_decoder(R, LY, s, d_wav, j.d_fsegs, j.d_ftile, j.d_yend);
+    Level LY = upload_frames(j, b.y, st);
+    launch_fill_zero(b.s, (long long)j.RY * a.inter, st);
+    SB_CUDA(cudaMemcpyAsync(b.s, z->z + (size_t)lo * a.inter, (size_t)n * a.inter * 4, cudaMemcpyDeviceToDevice, st));
+    run_decoder(R, LY, b.y, b.dec, b.s, b.wav);
     SB_CUDA(cudaEventRecord(C.ev_end, st));
-    return d_wav;
+    return b;
 }
 }  // namespace
 
 void decode_latent_chunk(Voice* v, const Latent* z, long long lo, long long hi, std::vector<float>& out, float* ms) {
     Job j;
-    float* d_wav = decode_chunk_device(v, z, lo, hi, j, 0);
+    const ChunkBufs b = decode_chunk_device(v, z, lo, hi, j, false);
     Context& C = *j.ctx;
     cudaStream_t st = C.stream;
     // through the context's page-locked staging buffer: a DMA copy instead of a pageable one
     const size_t bytes = (size_t)j.total_samples * 4;
-    SB_CUDA(cudaMemcpyAsync(C.pin, d_wav, bytes, cudaMemcpyDeviceToHost, st));
+    SB_CUDA(cudaMemcpyAsync(b.out_h, b.wav, bytes, cudaMemcpyDeviceToHost, st));
     SB_CUDA(cudaStreamSynchronize(st));
     SB_CUDA(cudaGetLastError());
-    out.resize((size_t)j.total_samples);
-    memcpy(out.data(), C.pin, bytes);
+    out.assign(b.out_h, b.out_h + j.total_samples);
     if (ms) cudaEventElapsedTime(ms, C.ev_begin, C.ev_end);
 }
 
@@ -793,7 +823,7 @@ void decode_latent_chunk_pcm(Voice* v, const Latent* z, long long lo, long long 
     Job j;
     const int hop = v->a.hop();
     const size_t total = (size_t)(hi - lo) * hop;
-    float* d_wav = decode_chunk_device(v, z, lo, hi, j, total * 2 + 4096);
+    const ChunkBufs b = decode_chunk_device(v, z, lo, hi, j, true);
     Context& C = *j.ctx;
     cudaStream_t st = C.stream;
     PcmPost post;
@@ -801,41 +831,45 @@ void decode_latent_chunk_pcm(Voice* v, const Latent* z, long long lo, long long 
     const long long m = (long long)total - post.trim_lo - post.trim_hi;
     if (m <= 0) throw Error(19, "Invalid model audio output");
     if (fade > 0) fill_fade(post, fade, m);
-    short* d_i16 = C.dev.get<short>(total + 8);
-    unsigned* d_max = C.dev.get<unsigned>(4);
-    launch_i16(d_wav, j.d_fsegs, 1, hop, (long long)total, d_max, d_i16, post, st);
-    SB_CUDA(cudaMemcpyAsync(C.pin, d_i16, (size_t)m * 2, cudaMemcpyDeviceToHost, st));
+    launch_i16(b.wav, b.y.fsegs, 1, hop, (long long)total, b.max, b.i16, post, st);
+    int16_t* h = reinterpret_cast<int16_t*>(b.out_h);
+    SB_CUDA(cudaMemcpyAsync(h, b.i16, (size_t)m * 2, cudaMemcpyDeviceToHost, st));
     SB_CUDA(cudaStreamSynchronize(st));
     SB_CUDA(cudaGetLastError());
-    out.resize((size_t)m);
-    memcpy(out.data(), C.pin, (size_t)m * 2);
+    out.assign(h, h + m);
     if (ms) cudaEventElapsedTime(ms, C.ev_begin, C.ev_end);
 }
 
-// Peak-normalised 16-bit PCM of every utterance of a finished job (to_i16_vec after the linear gain), converted on the
-// device and copied through the context's page-locked staging buffer.
-void job_pcm16(Job& j, float gain, std::vector<std::vector<int16_t>>& out) {
+void job_i16_to_host(Job& j, float gain, int16_t* dst) {
     if (!j.ran || j.encode_only) throw Error(19, "job has not produced audio");
-    Voice& v = *j.v; Context& C = *j.ctx;
-    SB_CUDA(cudaSetDevice(v.device));
-    cudaStream_t st = C.stream;
-    const int hop = v.a.hop();
+    SB_CUDA(cudaSetDevice(j.v->device));
+    cudaStream_t st = j.ctx->stream;
+    const int hop = j.v->a.hop();
     const size_t n = (size_t)j.total_samples;
     long long mx = 0;
     for (size_t b = 0; b < j.B; b++) mx = std::max<long long>(mx, (long long)j.y_len[b] * hop);
+    // stream-ordered scratch, returned to the pool at once: device memory held after a run does not grow
     short* d_i16 = nullptr; unsigned* d_max = nullptr;
     SB_CUDA(cudaMallocAsync(&d_i16, n * 2 + 16, st));
     SB_CUDA(cudaMallocAsync(&d_max, sizeof(unsigned) * j.B, st));
     PcmPost post; post.gain = gain;
     launch_i16(j.d_wav, j.d_fsegs, (int)j.B, hop, mx, d_max, d_i16, post, st);
-    C.ensure_pin(n * 2 + 4096);                    // the tables staged there were consumed by the pass
-    cudaError_t e = cudaMemcpyAsync(C.pin, d_i16, n * 2, cudaMemcpyDeviceToHost, st);
+    cudaError_t e = cudaMemcpyAsync(dst, d_i16, n * 2, cudaMemcpyDeviceToHost, st);
     cudaFreeAsync(d_i16, st);
     cudaFreeAsync(d_max, st);
     if (e == cudaSuccess) e = cudaStreamSynchronize(st);
     if (e != cudaSuccess) throw Error(19, std::string("CUDA error: ") + cudaGetErrorString(e));
+}
+
+// Peak-normalised 16-bit PCM of every utterance of a finished job, through the context's page-locked staging buffer.
+void job_pcm16(Job& j, float gain, std::vector<std::vector<int16_t>>& out) {
+    Context& C = *j.ctx;
+    SB_CUDA(cudaSetDevice(j.v->device));
+    C.pin.reserve((size_t)j.total_samples * 2);
+    int16_t* h = C.pin.get<int16_t>((size_t)j.total_samples);
+    job_i16_to_host(j, gain, h);
+    const int hop = j.v->a.hop();
     out.resize(j.B);
-    const int16_t* h = reinterpret_cast<const int16_t*>(C.pin);
     for (size_t b = 0; b < j.B; b++)
         out[b].assign(h + j.fsegs[b].out_off, h + j.fsegs[b].out_off + (size_t)j.y_len[b] * hop);
 }

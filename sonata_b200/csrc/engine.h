@@ -120,29 +120,33 @@ ConvW debug_make_conv(Voice& v, const float* w, const float* bias, int cout, int
 
 struct Region { std::string name; cudaEvent_t e0, e1; double flops = 0, bytes = 0; int launches = 0; float ms = 0; };
 
+// Bump allocator over one device (or page-locked host) buffer.  A dry arena hands out no memory and only counts bytes:
+// a workspace is carved once dry to learn its size, reserve()d, then carved for real (engine.cu plan()).
 struct Arena {
+    bool pinned = false;    // page-locked host memory instead of device memory
+    bool dry = false;
     char* base = nullptr;
     size_t cap = 0, used = 0;
-    bool dry = false;
     void* alloc(size_t bytes) {
         const size_t a = (used + 255) & ~(size_t)255;
         used = a + bytes;
         if (dry) return nullptr;
-        if (used > cap) throw Error(19, "internal: device arena overflow");
+        if (used > cap) throw Error(19, "internal: arena overflow");
         return base + a;
     }
     template <typename T> T* get(size_t n) { return reinterpret_cast<T*>(alloc(n * sizeof(T))); }
+    void reserve(size_t bytes);   // empties the arena and makes room for `bytes` (growing frees the old buffer)
+    void release();
 };
 
 struct Context {
     int device = 0;
     cudaStream_t stream = nullptr;
-    Arena dev;          // device workspace
-    char* pin = nullptr; size_t pin_cap = 0;   // pinned staging for small tables
+    Arena dev_id;       // id level of a pass: lives until the job is freed (stats, durations, speaker biases, captures)
+    Arena dev_frame;    // frame level of a pass (latent, flow, decoder, waveforms), or one streaming decoder chunk
+    Arena pin{true};    // page-locked staging: tables on the way in, results on the way out
     std::vector<cudaEvent_t> events; size_t events_used = 0;
     cudaEvent_t ev_begin = nullptr, ev_end = nullptr;
-    void ensure_dev(size_t bytes);
-    void ensure_pin(size_t bytes);
     cudaEvent_t next_event();
     ~Context();
 };
@@ -169,16 +173,14 @@ struct Job {
     // Y layout
     int RY = 0; std::vector<FrameSeg> fsegs; std::vector<int> y_len;
     long long total_samples = 0;
-    // device pointers (ctx arena)
-    int *d_ids_rows = nullptr, *d_xend = nullptr, *d_cum = nullptr, *d_ylen = nullptr, *d_yend = nullptr, *d_ftile = nullptr;
-    SegInfo* d_xsegs = nullptr; FrameSeg* d_fsegs = nullptr;
     // tensor-core attention (conv_tf.cu grouped GEMMs): tile tables built with the X layout, same for every layer
     std::vector<TfTile> tiles_s, tiles_o;      // Q.K^T tiles, P.V tiles
     int att_tp = 0;                            // key columns of a score row (multiple of 96)
     int att_nth_s = 64, att_nth_o = 96;   // column tiles of the two attention GEMMs (narrower when the job is small)
-    int* d_xseg_of_gran = nullptr; TfTile *d_tiles_s = nullptr, *d_tiles_o = nullptr;
-    float *d_epsw = nullptr, *d_epsz = nullptr;
-    float* d_wav = nullptr; bool wav_external = false;
+    // device results read after the pass (context arenas)
+    int* d_cum = nullptr;
+    FrameSeg* d_fsegs = nullptr;
+    float* d_wav = nullptr;
     float* d_cond = nullptr;       // effective biases of the speaker-conditioned convs for this call
     std::map<std::string, std::pair<float*, int>> dbg;   // name -> (device ptr, cols)
     std::map<std::string, int> dbg_level;                // name -> U (rows per frame), 0 for X level, -1 for an X-level
@@ -208,5 +210,9 @@ void decode_latent_chunk(Voice* v, const Latent* z, long long lo, long long hi, 
 void decode_latent_chunk_pcm(Voice* v, const Latent* z, long long lo, long long hi, long long trim_lo_frames,
                              long long trim_hi_frames, int fade, float gain, std::vector<int16_t>& out, float* ms);
 void job_pcm16(Job& j, float gain, std::vector<std::vector<int16_t>>& out);
+// Peak-normalised 16-bit PCM of every utterance of a finished job (to_i16_vec after a linear gain), converted on the
+// device and copied to `dst`: total_samples values laid out like the job's waveforms, in host memory that is best
+// page-locked (a DMA copy).
+void job_i16_to_host(Job& j, float gain, int16_t* dst);
 
 }  // namespace sb200

@@ -186,11 +186,10 @@ std::vector<std::vector<float>> speak_sentences_f32(Voice* v, const std::vector<
     std::unique_ptr<Job> j(create_job(v, ids.data(), offs.data(), ph.size(), nullptr, nullptr, nullptr, false));
     j->run(nullptr, 0);
     Context& C = *j->ctx;
-    const size_t bytes = (size_t)j->total_samples * 4;
-    C.ensure_pin(bytes + 4096);
-    SB_CUDA(cudaMemcpyAsync(C.pin, j->d_wav, bytes, cudaMemcpyDeviceToHost, C.stream));
+    C.pin.reserve((size_t)j->total_samples * 4);
+    float* all = C.pin.get<float>((size_t)j->total_samples);
+    SB_CUDA(cudaMemcpyAsync(all, j->d_wav, (size_t)j->total_samples * 4, cudaMemcpyDeviceToHost, C.stream));
     SB_CUDA(cudaStreamSynchronize(C.stream));
-    const float* all = reinterpret_cast<const float*>(C.pin);
     std::vector<std::vector<float>> out;
     for (size_t b = 0; b < ph.size(); b++)
         out.emplace_back(all + j->fsegs[b].out_off, all + j->fsegs[b].out_off + (size_t)j->y_len[b] * v->a.hop());

@@ -424,6 +424,37 @@ def test_batched_equals_sequential(models):
         assert np.array_equal(alone.samples.as_slice(), together[b].samples.as_slice())     # DESIGN.md §4: same bits
 
 
+def test_workspace_growth_keeps_results(voice_paths):
+    """A context's two device arenas and its pinned staging are sized from each job's own buffers and grow between jobs.
+    Jobs run in turn from one thread (so the voice hands back the same context) must give the bits each gets on a
+    freshly loaded model, whose workspace fits that job exactly: a short job, 32 x 256 ids at length_scale 3 (both
+    arenas and the staging grow), a short debug job (captures added to both levels), the long job again."""
+    short = [workload.synthetic_ids(n, utt=90 + i) for i, n in enumerate((12, 30))]
+    long_ = [workload.synthetic_ids(256, utt=u) for u in range(32)]
+    calls = [(short, 1.0, False), (long_, 3.0, False), (short, 1.0, True), (long_, 3.0, False)]
+
+    def run(m, ids, length_scale, debug):
+        m.set_fallback_synthesis_config(PiperSynthesisConfig(None, 0.0, length_scale, 0.0))
+        job = SynthesisJob(m, ids, debug=debug)
+        job.run()
+        out = [a.samples.as_slice().copy() for a in job.fetch()]
+        job.close()
+        return out
+
+    fresh = []
+    for call in calls:
+        m = sonata_b200.from_config_path(voice_paths["medium"], device=0)
+        fresh.append(run(m, *call))
+        m.close()
+    m = sonata_b200.from_config_path(voice_paths["medium"], device=0)
+    for call, want in zip(calls, fresh):
+        got = run(m, *call)
+        assert len(got) == len(want)
+        for g, w in zip(got, want):
+            assert np.array_equal(g, w)
+    m.close()
+
+
 def test_speak_api_surface(models, oracle_weights):
     m = models("medium"); _det(m)
     ph = "hɛloʊ wɜːld"
