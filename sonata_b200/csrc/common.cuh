@@ -64,13 +64,14 @@ struct TfTile {
     int b_row0;           // first row of the B block
     int b_col0;           // first K column in B
     int nkb;              // 32-column K-blocks
+    int kcols;            // K columns that hold data (from a_col0 / b_col0); the rest of the last K-block reads as zeros
     int rows_valid[2];    // rows of m-tile h that are stored
     long long out_off[2]; // element offset of (row 0, column 0) of m-tile h's output block in y (and res)
 };
 struct TfGemm {
     const float* a; int a_rows, a_cols, lda;      // A [a_rows][a_cols], K along the columns
     const float* b; int b_rows, b_cols, ldb;      // B [b_rows][b_cols], rows = output columns
-    int nth;                                      // B rows (= output columns) per tile: 96 / 64 / 32
+    int nth;                                      // B rows (= output columns) per tile: 96 / 64 / 48 / 32
     float* y; int ldy; const float* res; float scale;
     const TfTile* tiles; int ntiles;              // device table
 };

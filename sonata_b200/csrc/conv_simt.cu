@@ -232,6 +232,9 @@ int conv_simt_bn_for(int cout) {
 }
 
 void launch_conv_simt(const ConvArgs& a, cudaStream_t st) {
+    // the K loop walks whole 32-channel chunks: other widths would silently drop channels (voice.cu widens x_low's
+    // 48-channel coupling halves to 96 for this reason too)
+    if (a.cin % BK) throw_launch_error("conv_simt: input channels must be a multiple of 32");
     const int bn = conv_simt_bn_for(a.cout);
     switch (bn) {
         case 32: launch_cfg<256, 8, 4, 1>(a, st); break;

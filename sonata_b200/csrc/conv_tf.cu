@@ -23,7 +23,9 @@
 // GM = 1 ("grouped GEMM", the two contractions of the relative-position attention): the B operand is not a pre-split
 // weight image but a second ACTIVATION matrix (K for Q.K^T, V^T for P.V), loaded and split like A; tiles come from a
 // host-built table (one entry per (utterance, head, m-tile pair, n-tile) with its own K extent), so ragged batches need
-// no padding.  A CTA takes one m-tile of a table entry.
+// no padding.  A CTA takes one m-tile of a table entry.  A K extent that ends inside a 32-column K-block (48-wide heads:
+// Q.K^T has K = 48) zero-fills the rest of that block in BOTH operands: the columns beyond are the next head's
+// activations, not zeros.  48-wide heads also give P.V its 48-column tiles (m64n48k8).
 #include "tc_common.cuh"
 #include <stdlib.h>
 #include <string.h>
@@ -38,7 +40,7 @@ constexpr int TF_THREADS = 256;
 constexpr int TF_STAGES = 2;
 
 struct TfLaunch {
-    int nth;         // columns of a tile: 96 / 64 / 32
+    int nth;         // columns of a tile: 96 / 64 / 32 (grouped GEMM also 48)
     int wnth;        // rows of a weight IMAGE (tf_nth_for); nth == wnth, or 32 on small launches: the CTA then takes a 32-row
                      // part of the hi image and of the lo image (32 % 8 == 0 keeps the swizzle)
     int win;         // window rows (multiple of 8)
@@ -116,8 +118,8 @@ __global__ void __launch_bounds__(TF_THREADS, 1) conv_tf_kernel(const ConvArgs a
     auto issue_a = [&](int kb, int s) {
         const uint32_t img = A0 + s * 2 * a_img;
         if (GM) {
-            load_rows(img, G.a, G.lda, G.a_rows, G.a_cols, T.a_row0[h], T.a_col0 + kb * 32, 128);
-            load_rows(W0 + s * w_buf, G.b, G.ldb, G.b_rows, G.b_cols, T.b_row0, T.b_col0 + kb * 32, NT);
+            load_rows(img, G.a, G.lda, G.a_rows, min(G.a_cols, T.a_col0 + T.kcols), T.a_row0[h], T.a_col0 + kb * 32, 128);
+            load_rows(W0 + s * w_buf, G.b, G.ldb, G.b_rows, min(G.b_cols, T.b_col0 + T.kcols), T.b_row0, T.b_col0 + kb * 32, NT);
         } else {
             load_rows(img, a.x, a.ldx, a.rows_in, a.cin, m_tile * 128 + a.min_off, kb * 32, L.win);
         }
@@ -301,6 +303,13 @@ template <int GM> void launch_any(int nth, dim3 grid, size_t smem, cudaStream_t 
     }
 }
 
+// the grouped GEMM also takes 48-column tiles (P.V of 48-wide attention heads)
+void launch_gemm_any(int nth, dim3 grid, size_t smem, cudaStream_t st, const ConvArgs& a, const TfLaunch& L,
+                     const TfOperands& G) {
+    if (nth == 48) launch_nt<1, 48>(grid, smem, st, a, L, G);
+    else launch_any<1>(nth, grid, smem, st, a, L, G);
+}
+
 uint32_t tf32_rn_host(float f) {        // round to nearest, ties away from zero (cvt.rna.tf32.f32)
     uint32_t b; memcpy(&b, &f, 4);
     if ((b & 0x7f800000u) == 0x7f800000u) return b;
@@ -339,7 +348,7 @@ bool try_launch_conv_tf(const ConvArgs& a, cudaStream_t st) {
 }
 
 bool gemm_tf_supported(const TfGemm& g) {
-    if (g.nth != 96 && g.nth != 64 && g.nth != 32) return false;
+    if (g.nth != 96 && g.nth != 64 && g.nth != 48 && g.nth != 32) return false;
     auto al = [](const void* p, int ld) { return p == nullptr || ((reinterpret_cast<uintptr_t>(p) & 15) == 0 && (ld & 3) == 0); };
     return al(g.a, g.lda) && al(g.b, g.ldb);
 }
@@ -352,7 +361,7 @@ void launch_gemm_tf(const TfGemm& g, cudaStream_t st) {
     TfLaunch L{};
     L.nth = L.wnth = g.nth; L.win = 128; L.ntiles_m = 2 * g.ntiles; L.ntiles_n = 1; L.chunk_kb = 2;
     const TfOperands G{g.a, g.a_rows, g.a_cols, g.lda, g.b, g.b_rows, g.b_cols, g.ldb, g.tiles};
-    launch_any<1>(g.nth, dim3(2 * g.ntiles), smem_bytes(128, 1, g.nth) + 1024, st, a, L, G);
+    launch_gemm_any(g.nth, dim3(2 * g.ntiles), smem_bytes(128, 1, g.nth) + 1024, st, a, L, G);
     g_launch_count++;
     check_launch("gemm_tf");
 }

@@ -154,7 +154,8 @@ Job* create_job(Voice* v, const long long* ids, const size_t* offs, size_t B, co
                             s.a_row0[m] = off + (mp * 2 + m) * 128;
                             s.out_off[m] = ((long long)h * j->RX + s.a_row0[m]) * j->att_tp + (long long)nt * ks;
                         }
-                        s.a_col0 = h * D; s.b_row0 = off + nt * ks; s.b_col0 = H + h * D; s.nkb = D / 32;
+                        // 48-wide heads: the second K-block is half used and zero-filled past the head
+                        s.a_col0 = h * D; s.b_row0 = off + nt * ks; s.b_col0 = H + h * D; s.nkb = (D + 31) / 32; s.kcols = D;
                         j->tiles_s.push_back(s);
                     }
                     // P.V: K runs over the utterance's keys in blocks of 32 (the softmax zero-fills up to the block end)
@@ -164,7 +165,7 @@ Job* create_job(Voice* v, const long long* ids, const size_t* offs, size_t B, co
                             o.a_row0[m] = h * j->RX + off + (mp * 2 + m) * 128;
                             o.out_off[m] = (long long)(off + (mp * 2 + m) * 128) * H + (long long)h * D + c0;
                         }
-                        o.a_col0 = 0; o.b_row0 = h * D + c0; o.b_col0 = off; o.nkb = (T + 31) / 32;
+                        o.a_col0 = 0; o.b_row0 = h * D + c0; o.b_col0 = off; o.nkb = (T + 31) / 32; o.kcols = o.nkb * 32;
                         j->tiles_o.push_back(o);
                     }
                 }
@@ -519,9 +520,10 @@ void Job::run(float* d_out, size_t d_out_cap) {
     if (!C.ev_begin) { SB_CUDA(cudaEventCreate(&C.ev_begin)); SB_CUDA(cudaEventCreate(&C.ev_end)); }
 
     // ---------------- id level (phase 1) workspace ----------------
-    // tensor-core attention (two grouped GEMMs around a softmax): default backend, 96-wide heads, rows that fit the
-    // softmax kernel's registers; otherwise the fp32 CUDA-core attention kernel
-    const bool tc_att = V.backend == 1 && H / a.heads == 96 && max_tx <= 1280 && getenv("SB200_ATT_SIMT") == nullptr;
+    // tensor-core attention (two grouped GEMMs around a softmax): default backend, 96- or 48-wide heads, rows that fit
+    // the softmax kernel's registers; otherwise the fp32 CUDA-core attention kernel
+    const int D = H / a.heads;
+    const bool tc_att = V.backend == 1 && (D == 96 || D == 48) && max_tx <= 1280 && getenv("SB200_ATT_SIMT") == nullptr;
     IdBufs x;
     plan(C.dev_id, C.pin, [&](Arena& dev, Arena& pin) { x.carve(dev, pin, *this, tc_att); });
     d_cum = x.cum; d_cond = x.cond;

@@ -288,7 +288,8 @@ __global__ void __launch_bounds__(2 * D) attention_kernel(const float* __restric
 // one warp per (row, head) adds the relative-key logits on the |j - i| <= window band, takes the softmax over the
 // utterance's keys IN PLACE, zero-fills the row up to the next multiple of 32 keys (the K extent of the second GEMM) and
 // writes the relative-value term  orel[row][head*D + c] = sum_d p[i][i+d] E_v[d+w][c],  which the second GEMM adds as
-// its residual.  The whole row lives in registers (NREG x 32 keys).  oracle: _mha()
+// its residual.  The whole row lives in registers (NREG x 32 keys).  Lane l holds head channels l + 32k (k < ceil(D/32);
+// 48-wide heads leave lanes 16-31 idle in the second).  oracle: _mha()
 template <int D, int NREG>
 __global__ void __launch_bounds__(256) attn_softmax_kernel(float* __restrict__ S, int Tp, const float* __restrict__ qkv,
                                                            int ldq, const float* __restrict__ relk,
@@ -306,16 +307,17 @@ __global__ void __launch_bounds__(256) attn_softmax_kernel(float* __restrict__ S
     if (i < 0 || i >= T) return;                       // gap row
     float* Sr = S + ((size_t)head * RX + q) * Tp;
     const int nrel = 2 * window + 1;
-    constexpr int NV = D / 32;
+    constexpr int NV = (D + 31) / 32;
+    auto has = [&](int k) { return D % 32 == 0 || lane + 32 * k < D; };
     const float qs = rsqrtf((float)D);
     float qv[NV];
 #pragma unroll
-    for (int k = 0; k < NV; k++) qv[k] = qkv[(size_t)q * ldq + head * D + lane + 32 * k] * qs;
+    for (int k = 0; k < NV; k++) qv[k] = has(k) ? qkv[(size_t)q * ldq + head * D + lane + 32 * k] * qs : 0.f;
     float mine = 0.f;                                  // lane d keeps the logit of relative offset d - window
     for (int d = 0; d < nrel; d++) {
         float s = 0.f;
 #pragma unroll
-        for (int k = 0; k < NV; k++) s = fmaf(qv[k], relk[d * D + lane + 32 * k], s);
+        for (int k = 0; k < NV; k++) if (has(k)) s = fmaf(qv[k], relk[d * D + lane + 32 * k], s);
         s = warp_sum(s);
         if (lane == d) mine = s;
     }
@@ -360,10 +362,10 @@ __global__ void __launch_bounds__(256) attn_softmax_kernel(float* __restrict__ S
     for (int d = 0; d < nrel; d++) {
         const float p = __shfl_sync(0xffffffffu, pb, d);
 #pragma unroll
-        for (int k = 0; k < NV; k++) acc[k] = fmaf(p, relv[d * D + lane + 32 * k], acc[k]);
+        for (int k = 0; k < NV; k++) if (has(k)) acc[k] = fmaf(p, relv[d * D + lane + 32 * k], acc[k]);
     }
 #pragma unroll
-    for (int k = 0; k < NV; k++) orel[(size_t)q * ldo + head * D + lane + 32 * k] = acc[k];
+    for (int k = 0; k < NV; k++) if (has(k)) orel[(size_t)q * ldo + head * D + lane + 32 * k] = acc[k];
 }
 
 // ------------------------------------------------------------------ duration-predictor flow pieces
@@ -804,11 +806,10 @@ void launch_attn_softmax(float* S, int Tp, const float* qkv, int ldq, const floa
                          int gran, int max_len, cudaStream_t st) {
     const int D = H / heads;
     dim3 grid((RX + 7) / 8, heads);
-    if (D != 96 || max_len > 1280 || 2 * window + 1 > 32) throw_launch_error("attn_softmax: unsupported head size / length");
-    if (max_len <= 640)
-        launch_pdl(attn_softmax_kernel<96, 20>, dim3(grid), dim3(256), 0, st, S, Tp, qkv, ldq, relk, relv, window, orel, ldo, RX, segs, seg_of_gran, gran);
-    else
-        launch_pdl(attn_softmax_kernel<96, 40>, dim3(grid), dim3(256), 0, st, S, Tp, qkv, ldq, relk, relv, window, orel, ldo, RX, segs, seg_of_gran, gran);
+    if ((D != 96 && D != 48) || max_len > 1280 || 2 * window + 1 > 32) throw_launch_error("attn_softmax: unsupported head size / length");
+    auto k = D == 96 ? (max_len <= 640 ? attn_softmax_kernel<96, 20> : attn_softmax_kernel<96, 40>)
+                     : (max_len <= 640 ? attn_softmax_kernel<48, 20> : attn_softmax_kernel<48, 40>);
+    launch_pdl(k, dim3(grid), dim3(256), 0, st, S, Tp, qkv, ldq, relk, relv, window, orel, ldo, RX, segs, seg_of_gran, gran);
     g_launch_count++;
 }
 

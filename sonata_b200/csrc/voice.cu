@@ -172,6 +172,24 @@ DDSW load_dds(Uploader& U, const TensorMap& m, const std::string& p, int C, int 
     return d;
 }
 
+// `t` with axis `axis` widened to `width`: source index i lands at `off` + i (reversed: `off` + n-1-i), the rest is zero
+HostTensor widen(const HostTensor& t, int width, int axis, int off, bool reversed) {
+    HostTensor o;
+    o.dims = t.dims;
+    const int n = t.dims[axis];
+    o.dims[axis] = width;
+    size_t outer = 1, inner = 1;
+    for (int d = 0; d < axis; d++) outer *= (size_t)t.dims[d];
+    for (size_t d = axis + 1; d < t.dims.size(); d++) inner *= (size_t)t.dims[d];
+    o.f.assign(outer * width * inner, 0.f);
+    for (size_t a = 0; a < outer; a++)
+        for (int i = 0; i < n; i++) {
+            const int k = off + (reversed ? n - 1 - i : i);
+            memcpy(o.f.data() + (a * width + k) * inner, t.f.data() + (a * n + i) * inner, inner * sizeof(float));
+        }
+    return o;
+}
+
 uint32_t first_code_point(const std::string& s) {
     if (s.empty()) return 0;
     const unsigned char c = (unsigned char)s[0];
@@ -316,8 +334,9 @@ Voice* load_voice(const std::string& config_path, int device) {
             a.res_dils.emplace_back(rd.i.begin() + (size_t)i * rd.dims[1], rd.i.begin() + (size_t)(i + 1) * rd.dims[1]);
     }
     const int H = a.hidden, I = a.inter;
-    if (H % 32 || I % 64 || a.filter % 32 || (a.flow_n & 1) || a.dp_bins != 10 || a.dp_kernel != 3 || a.hop() != 256)
-        throw Error(17, "unsupported voice architecture");
+    if (H % 32 || I % 32 || (I & 1) || a.filter % 32 || (a.flow_n & 1) || a.dp_bins != 10 || a.dp_kernel != 3 || a.hop() != 256)
+        throw Error(17, "unsupported voice architecture (hidden " + std::to_string(H) + ", inter " + std::to_string(I) +
+                        ", filter " + std::to_string(a.filter) + ", hop " + std::to_string(a.hop()) + ")");
     const int D = H / a.heads;
     if (D != 96 && D != 48) throw Error(17, "unsupported attention head size");
     if (H != 96 && H != 192 && H != 256) throw Error(17, "unsupported hidden width (LayerNorm kernels: 96 / 192 / 256)");
@@ -379,12 +398,28 @@ Voice* load_voice(const std::string& config_path, int device) {
             CouplingW c;
             c.cond_off = reversed ? half : 0;
             c.tgt_off = reversed ? 0 : half;
-            c.pre = conv_named(U, m, p + "pre", 1, true, nullptr, reversed ? &rev : nullptr);
+            if (half % 32 == 0) {
+                c.pre = conv_named(U, m, p + "pre", 1, true, nullptr, reversed ? &rev : nullptr);
+            } else {
+                // A half that is not a whole number of 32-channel K-blocks (x_low: 48 of 96) keeps the tensor-core convs
+                // by widening pre and post to all `inter` channels of z: pre reads the target half with zero weights,
+                // post writes the conditioning half with zero weights and bias.  Exact zeros change no sum.
+                const HostTensor w = widen(T(m, p + "pre.weight"), I, 1, c.cond_off, reversed);
+                c.pre = make_conv(U, {&w}, {&T(m, p + "pre.bias")}, 1);
+                c.cond_off = 0;
+            }
             for (int l = 0; l < a.wn_layers; l++) {
                 c.in.push_back(conv_named(U, m, p + "enc.in_layers." + std::to_string(l), 1, true, &gate));
                 c.rs.push_back(conv_named(U, m, p + "enc.res_skip_layers." + std::to_string(l)));
             }
-            c.post = conv_named(U, m, p + "post", 1, true, reversed ? &rev : nullptr);
+            if (half % 32 == 0) {
+                c.post = conv_named(U, m, p + "post", 1, true, reversed ? &rev : nullptr);
+            } else {
+                const HostTensor w = widen(T(m, p + "post.weight"), I, 0, c.tgt_off, reversed);
+                const HostTensor b = widen(T(m, p + "post.bias"), I, 0, c.tgt_off, reversed);
+                c.post = make_conv(U, {&w}, {&b}, 1);
+                c.tgt_off = 0;
+            }
             v->flows.push_back(c);
         }
     }

@@ -156,21 +156,35 @@ def _fold_weight_norm(t: Dict[str, np.ndarray]) -> Dict[str, np.ndarray]:
     return out
 
 
-def detect_quality(t: Dict[str, np.ndarray]) -> str:
-    w = t.get("dec.conv_pre.weight")
-    if w is None:
-        raise ValueError("`dec.conv_pre.weight` not found: initialisers do not carry Piper's parameter names")
-    for q, a in voicegen.ARCH.items():
-        if a["up_init"] == int(w.shape[0]):
-            return q
-    raise ValueError(f"unsupported decoder width {w.shape[0]} (known: " +
-                     ", ".join(f"{q}={a['up_init']}" for q, a in voicegen.ARCH.items()) + ")")
+def detect_quality(t: Dict[str, np.ndarray], cfg: dict | None = None) -> str:
+    """The voice architecture from tensor shapes: the text encoder's width (`enc_p.emb.weight`), then the decoder's
+    (`dec.conv_pre`).  Qualities with the same tensors (low and medium) are told apart by the config's
+    `audio.quality`, then its `audio.sample_rate`; without a config the 22.05 kHz one is taken."""
+    emb, pre = t.get("enc_p.emb.weight"), t.get("dec.conv_pre.weight")
+    if emb is None or pre is None:
+        raise ValueError("`enc_p.emb.weight` / `dec.conv_pre.weight` not found: initialisers do not carry Piper's "
+                         "parameter names")
+    shape = (int(emb.shape[-1]), int(pre.shape[0]))
+    known = sorted(voicegen.ARCH.items())
+    cands = [q for q, a in known if (a["hidden"], a["up_init"]) == shape]
+    if not cands:
+        raise ValueError(f"unsupported voice architecture: encoder width {shape[0]}, decoder width {shape[1]} (known: " +
+                         ", ".join(f"{q}={a['hidden']}/{a['up_init']}" for q, a in known) + ")")
+    audio = (cfg or {}).get("audio", {})
+    for pick in (lambda q: q == audio.get("quality"),
+                 lambda q: voicegen.ARCH[q]["sample_rate"] == audio.get("sample_rate", 22050)):
+        hit = [q for q in cands if pick(q)]
+        if len(hit) == 1:
+            return hit[0]
+    if len(cands) == 1:
+        return cands[0]
+    raise ValueError(f"tensors fit {', '.join(cands)}; the config's audio.quality / sample_rate do not pick one")
 
 
-def convert_tensors(inits: Dict[str, np.ndarray]) -> Tuple[str, Dict[str, np.ndarray]]:
+def convert_tensors(inits: Dict[str, np.ndarray], cfg: dict | None = None) -> Tuple[str, Dict[str, np.ndarray]]:
     """Initialisers -> exactly the tensors of `voicegen.tensor_specs(arch)`, fp32, shapes verified."""
     t = _fold_weight_norm(inits)
-    quality = detect_quality(t)
+    quality = detect_quality(t, cfg)
     specs = voicegen.tensor_specs(voicegen.ARCH[quality])
     eg = t.get("emb_g.weight")
     if eg is not None:                               # multi-speaker voice
@@ -197,9 +211,9 @@ def convert_tensors(inits: Dict[str, np.ndarray]) -> Tuple[str, Dict[str, np.nda
 
 def import_voice(onnx_path: str, config_path: str, out_dir: str) -> str:
     """Writes `<out_dir>/<name>.onnx.json` (copy) + `<out_dir>/<name>.svw`; returns the config path to load."""
-    quality, tensors = convert_tensors(read_initializers(onnx_path))
     with open(config_path) as f:
         cfg = json.load(f)
+    quality, tensors = convert_tensors(read_initializers(onnx_path), cfg)
     n_spk = int(tensors["emb_g.weight"].shape[0]) if "emb_g.weight" in tensors else 1
     if int(cfg.get("num_speakers", 1)) > 1 and n_spk < int(cfg["num_speakers"]):
         raise ValueError(f"config says num_speakers = {cfg['num_speakers']} but the model embeds {n_spk} speaker(s)")

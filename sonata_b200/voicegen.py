@@ -37,6 +37,11 @@ ARCH = {
         sample_rate=22050,
     ),
 }
+# Piper's x_low: the medium decoder behind a 96-wide text encoder and flow (48-wide attention heads), at 16 kHz.
+ARCH["x_low"] = dict(ARCH["medium"], hidden=96, inter=96, filter=384, sample_rate=16000)
+# Piper's low: the medium architecture at 16 kHz.  Same tensors as medium, so it shares medium's gains.
+ARCH["low"] = dict(ARCH["medium"], sample_rate=16000)
+_GAINS_OF = {"low": "medium"}
 
 _DATA_DIR = os.path.join(os.path.dirname(os.path.abspath(__file__)), "data")
 
@@ -206,7 +211,7 @@ def hp_tensors(a: dict) -> "OrderedDict[str, np.ndarray]":
 
 
 def load_gains(quality: str) -> dict:
-    p = os.path.join(_DATA_DIR, f"gains_{quality}.json")
+    p = os.path.join(_DATA_DIR, f"gains_{_GAINS_OF.get(quality, quality)}.json")
     if not os.path.exists(p):
         return {}
     with open(p) as f:
