@@ -113,6 +113,15 @@ int32_t sb200_speak_ids(sb200_voice* v, const int64_t* ids, size_t n, sb200_audi
 /* batched infer_with_values: utterance b = ids_packed[offsets[b] .. offsets[b+1]) */
 int32_t sb200_speak_batch_ids(sb200_voice* v, const int64_t* ids_packed, const size_t* offsets, size_t batch,
                               sb200_audio* outs, sb200_error* err);
+/* sb200_speak_batch_ids with one synthesis config per utterance (speaker and scales, the per-request options of the
+ * reference's CLI and gRPC service), still as one batched pass.  cfgs[b] applies to utterance b; NULL = the voice's
+ * fallback config for every utterance, i.e. sb200_speak_batch_ids.  Each entry is checked like
+ * sb200_set_fallback_synthesis_config (a speaker must be in the voice's speaker_id_map; has_speaker == 0 means
+ * speaker 0); an invalid entry fails the call with OPERATION_ERROR naming the utterance.  Utterance b's result equals
+ * a single-utterance call with cfgs[b] as the fallback config, except for the on-device noise: its draws depend on
+ * the utterance's position in the batch. */
+int32_t sb200_speak_batch_ids_configs(sb200_voice* v, const int64_t* ids_packed, const size_t* offsets, size_t batch,
+                                      const sb200_synth_config* cfgs, sb200_audio* outs, sb200_error* err);
 
 /* ---- job API: the same batched pass split into its host<->device steps (bench / multi-GPU plumbing) ----
  * create  : copies ids to the device (H2D).  `eps_w` / `eps_z` optionally inject the graph's two
@@ -126,6 +135,12 @@ int32_t sb200_job_create(sb200_voice* v, const int64_t* ids_packed, const size_t
                          sb200_job** out, sb200_error* err);
 /* keep every intermediate of the next run fetchable through sb200_job_debug_fetch (tests only) */
 int32_t sb200_job_set_debug(sb200_job* job, int32_t on);
+/* Per-utterance synthesis configs for the next sb200_job_run: cfgs[0 .. batch), or NULL for the voice's fallback config
+ * (what a new job starts with, read at create time) for every utterance.  Entries are checked like
+ * sb200_set_fallback_synthesis_config; an invalid one fails with OPERATION_ERROR naming the utterance and leaves the
+ * job's configs unchanged.  Philox noise (no eps_w / eps_z given) depends on each utterance's batch position, as it
+ * always has: only injected noise makes a mixed batch equal its utterances run alone. */
+int32_t sb200_job_set_configs(sb200_job* job, const sb200_synth_config* cfgs, sb200_error* err);
 int32_t sb200_job_run(sb200_job* job, float* d_out, size_t d_out_capacity, float* device_ms, sb200_error* err);
 int32_t sb200_job_fetch(sb200_job* job, sb200_audio* outs, sb200_error* err);
 size_t sb200_job_batch(const sb200_job* job);

@@ -64,10 +64,13 @@ SIGNATURES = {
     "sb200_speak_ids": (C.c_int32, [_P, C.POINTER(C.c_int64), C.c_size_t, C.POINTER(sb200_audio), _ERR]),
     "sb200_speak_batch_ids": (C.c_int32, [_P, C.POINTER(C.c_int64), C.POINTER(C.c_size_t), C.c_size_t,
                                           C.POINTER(sb200_audio), _ERR]),
+    "sb200_speak_batch_ids_configs": (C.c_int32, [_P, C.POINTER(C.c_int64), C.POINTER(C.c_size_t), C.c_size_t,
+                                                  C.POINTER(sb200_synth_config), C.POINTER(sb200_audio), _ERR]),
     "sb200_job_create": (C.c_int32, [_P, C.POINTER(C.c_int64), C.POINTER(C.c_size_t), C.c_size_t,
                                      C.POINTER(C.POINTER(C.c_float)), C.POINTER(C.POINTER(C.c_float)),
                                      C.POINTER(C.c_size_t), C.POINTER(_P), _ERR]),
     "sb200_job_set_debug": (C.c_int32, [_P, C.c_int32]),
+    "sb200_job_set_configs": (C.c_int32, [_P, C.POINTER(sb200_synth_config), _ERR]),
     "sb200_job_run": (C.c_int32, [_P, C.c_void_p, C.c_size_t, C.POINTER(C.c_float), _ERR]),
     "sb200_job_fetch": (C.c_int32, [_P, C.POINTER(sb200_audio), _ERR]),
     "sb200_job_fetch_i16": (C.c_int32, [_P, C.POINTER(C.POINTER(C.c_int16)), C.POINTER(C.c_size_t), _ERR]),

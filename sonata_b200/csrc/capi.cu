@@ -152,6 +152,14 @@ static void cfg_out(const SynthConfig& c, sb200_synth_config* o) {
     o->speaker = c.speaker; o->has_speaker = c.has_speaker ? 1 : 0;
     o->noise_scale = c.noise_scale; o->length_scale = c.length_scale; o->noise_w = c.noise_w;
 }
+static std::vector<SynthConfig> cfgs_in(const sb200_synth_config* c, size_t n) {
+    std::vector<SynthConfig> out(n);
+    for (size_t b = 0; b < n; b++) {
+        out[b].speaker = c[b].speaker; out[b].has_speaker = c[b].has_speaker != 0;
+        out[b].noise_scale = c[b].noise_scale; out[b].length_scale = c[b].length_scale; out[b].noise_w = c[b].noise_w;
+    }
+    return out;
+}
 int32_t sb200_get_default_synthesis_config(const sb200_voice* v, sb200_synth_config* out, sb200_error* err) {
     return guarded(err, [&] {   // always Some(0), piper/src/lib.rs:444-451
         SynthConfig c = v->v->factory_cfg; c.speaker = 0; c.has_speaker = true; cfg_out(c, out);
@@ -165,9 +173,7 @@ int32_t sb200_set_fallback_synthesis_config(sb200_voice* v, const sb200_synth_co
         std::unique_lock<std::shared_mutex> g(v->v->cfg_mu);
         v->v->cfg.length_scale = c->length_scale; v->v->cfg.noise_scale = c->noise_scale; v->v->cfg.noise_w = c->noise_w;
         if (c->has_speaker) {
-            bool found = false;
-            for (auto& kv : v->v->speaker_id_map) if (kv.second == c->speaker) found = true;
-            if (!found) throw Error(19, "No speaker was found with the given id `" + std::to_string(c->speaker) + "`");
+            check_config(*v->v, cfgs_in(c, 1)[0], "");
             v->v->cfg.speaker = c->speaker; v->v->cfg.has_speaker = true;
         }
     });
@@ -194,19 +200,24 @@ int32_t sb200_phonemes_to_input_ids(const sb200_voice* v, const char* ph, int64_
     });
 }
 
-int32_t sb200_speak_batch_ids(sb200_voice* v, const int64_t* ids, const size_t* offsets, size_t batch,
-                              sb200_audio* outs, sb200_error* err) {
+int32_t sb200_speak_batch_ids_configs(sb200_voice* v, const int64_t* ids, const size_t* offsets, size_t batch,
+                                      const sb200_synth_config* cfgs, sb200_audio* outs, sb200_error* err) {
     return guarded(err, [&] {
         const double t0 = now_ms();
         static_assert(sizeof(long long) == sizeof(int64_t), "");
         std::unique_ptr<Job> j(create_job(v->v.get(), reinterpret_cast<const long long*>(ids), offsets, batch, nullptr,
                                           nullptr, nullptr, false));
+        if (cfgs) set_job_configs(*j, cfgs_in(cfgs, batch).data());
         j->run(nullptr, 0);
         fetch_audio(*j, outs, 0.f);
         const float wall = (float)(now_ms() - t0);
         for (size_t b = 0; b < batch; b++)
             outs[b].inference_ms = wall * (j->total_samples ? (float)outs[b].len / (float)j->total_samples : 0.f);
     });
+}
+int32_t sb200_speak_batch_ids(sb200_voice* v, const int64_t* ids, const size_t* offsets, size_t batch,
+                              sb200_audio* outs, sb200_error* err) {
+    return sb200_speak_batch_ids_configs(v, ids, offsets, batch, nullptr, outs, err);
 }
 int32_t sb200_speak_ids(sb200_voice* v, const int64_t* ids, size_t n, sb200_audio* out, sb200_error* err) {
     const size_t offs[2] = {0, n};
@@ -238,6 +249,12 @@ int32_t sb200_job_create(sb200_voice* v, const int64_t* ids, const size_t* offse
     });
 }
 int32_t sb200_job_set_debug(sb200_job* job, int32_t on) { job->j->debug = on != 0; return 0; }
+int32_t sb200_job_set_configs(sb200_job* job, const sb200_synth_config* cfgs, sb200_error* err) {
+    return guarded(err, [&] {
+        Job& j = *job->j;
+        set_job_configs(j, cfgs ? cfgs_in(cfgs, j.B).data() : nullptr);
+    });
+}
 int32_t sb200_job_run(sb200_job* job, float* d_out, size_t cap, float* device_ms, sb200_error* err) {
     return guarded(err, [&] { job->j->run(d_out, cap); if (device_ms) *device_ms = job->j->last_ms; });
 }
@@ -496,19 +513,22 @@ int32_t sb200_debug_durations(int32_t device, const float* z, int32_t rows, cons
             segs[b] = SegInfo{seg_off[b], seg_len[b]};
         }
         SB_CUDA(cudaSetDevice(device));
-        float *dz, *dlogw; int *dcum, *dylen; SegInfo* dseg;
+        float *dz, *dlogw, *dscale; int *dcum, *dylen; SegInfo* dseg;
+        const std::vector<float> scales(nseg, length_scale);
+        SB_CUDA(cudaMalloc(&dscale, (size_t)nseg * 4));
+        SB_CUDA(cudaMemcpy(dscale, scales.data(), (size_t)nseg * 4, cudaMemcpyHostToDevice));
         SB_CUDA(cudaMalloc(&dz, (size_t)rows * 2 * 4)); SB_CUDA(cudaMemcpy(dz, z, (size_t)rows * 2 * 4, cudaMemcpyHostToDevice));
         SB_CUDA(cudaMalloc(&dlogw, (size_t)rows * 4)); SB_CUDA(cudaMemcpy(dlogw, logw, (size_t)rows * 4, cudaMemcpyHostToDevice));
         SB_CUDA(cudaMalloc(&dcum, (size_t)rows * 4)); SB_CUDA(cudaMemcpy(dcum, cum, (size_t)rows * 4, cudaMemcpyHostToDevice));
         SB_CUDA(cudaMalloc(&dylen, (size_t)nseg * 4));
         SB_CUDA(cudaMalloc(&dseg, (size_t)nseg * sizeof(SegInfo)));
         SB_CUDA(cudaMemcpy(dseg, segs.data(), (size_t)nseg * sizeof(SegInfo), cudaMemcpyHostToDevice));
-        launch_durations(dz, m0, logs0, length_scale, dseg, nseg, dlogw, dcum, dylen, 0);
+        launch_durations(dz, m0, logs0, dscale, dseg, nseg, dlogw, dcum, dylen, 0);
         cudaError_t e = cudaDeviceSynchronize();
         if (e == cudaSuccess) e = cudaMemcpy(logw, dlogw, (size_t)rows * 4, cudaMemcpyDeviceToHost);
         if (e == cudaSuccess) e = cudaMemcpy(cum, dcum, (size_t)rows * 4, cudaMemcpyDeviceToHost);
         if (e == cudaSuccess) e = cudaMemcpy(y_len, dylen, (size_t)nseg * 4, cudaMemcpyDeviceToHost);
-        cudaFree(dz); cudaFree(dlogw); cudaFree(dcum); cudaFree(dylen); cudaFree(dseg);
+        cudaFree(dz); cudaFree(dlogw); cudaFree(dcum); cudaFree(dylen); cudaFree(dseg); cudaFree(dscale);
         if (e != cudaSuccess) throw Error(19, std::string("CUDA error: ") + cudaGetErrorString(e));
     });
 }

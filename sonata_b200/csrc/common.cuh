@@ -54,7 +54,17 @@ struct ConvArgs {
     float* y1; int ldy1; int acc1;                                // columns [split, cout)
     float* yt; int yt_col0; int ldyt;                             // conv_tf.cu: column tiles >= yt_col0 are stored TRANSPOSED,
                                                                   // yt[(n - yt_col0) * ldyt + q] (row index contiguous)
+    const int* bias_slot; int ldbias;                             // per-row bias: row q adds bias[bias_slot[q / map.gran] * ldbias + n]
+                                                                  // (speaker-conditioned convs of a batch with several speakers)
 };
+
+// Epilogue view of GEMM row q >= 0: its validity (row_valid) and its bias row (the conv's own, or with a slot table the
+// one of q's slot), sharing one granule division.
+__device__ __forceinline__ const float* conv_row(const ConvArgs& a, int q, bool& valid) {
+    const int g = q / a.map.gran;
+    valid = q < a.map.rows && q < a.map.seg_end[g] * a.map.seg_mul;
+    return a.bias_slot ? a.bias + (size_t)a.bias_slot[g] * a.ldbias : a.bias;
+}
 
 // One tile of a grouped GEMM on conv_tf.cu's kernel (the attention contractions): two 128-row m-tiles of A against
 // one block of nth B rows over `nkb` 32-column K-blocks;  C = scale * A . B^T (+ res).
@@ -167,12 +177,13 @@ void launch_flow_pre(const float* z, int zcol, const float* w, const float* b, c
 // z[r][tcol] = RQS^-1(z[r][tcol]; params h29[r][0..3*bins-1))
 void launch_spline(const float* h29, int ldh, float* z, int tcol, int bins, float inv_sqrt_filter,
                    RowMap map, cudaStream_t st);
-// logw = (z[:,0]-m0)*exp(-logs0); w = exp(logw)*length_scale; w_ceil; per-segment inclusive scan
-void launch_durations(const float* z, float m0, float logs0, float length_scale, const SegInfo* segs, int nseg,
+// logw = (z[:,0]-m0)*exp(-logs0); w = exp(logw)*length_scale[b]; w_ceil; per-segment inclusive scan
+void launch_durations(const float* z, float m0, float logs0, const float* length_scale, const SegInfo* segs, int nseg,
                       float* logw, int* cum, int* y_len, cudaStream_t st);
 struct FrameSeg { int off; int len; int xoff; int xlen; long long out_off; };
-// z_p rows: gather m_p/logs_p of the token whose cumulative duration covers the frame, add noise
-void launch_expand(const float* stats, int ldst, int I, const int* cum, const float* eps, float noise_scale,
+// z_p rows: gather m_p/logs_p of the token whose cumulative duration covers the frame, add noise scaled by the noise_scale
+// of the frame's segment (ftile_seg)
+void launch_expand(const float* stats, int ldst, int I, const int* cum, const float* eps, const float* noise_scale,
                    float* zp, const FrameSeg* fsegs, const int* ftile_seg, RowMap ymap, cudaStream_t st);
 // wav = tanh(conv_k7(lrelu_{0.01}(x)))  ->  compact per-segment output
 void launch_conv_post(const float* x, int C, const float* w /*[7][C]*/, float* wav, const FrameSeg* fsegs,
@@ -184,10 +195,13 @@ struct PcmPost { float gain = 1.f; int fade_n = 0; long long trim_lo = 0, trim_h
 void launch_i16(const float* wav, const FrameSeg* fsegs, int nseg, int hop, long long max_samples, unsigned* maxbits,
                 short* out, const PcmPost& post, cudaStream_t st);
 void launch_randn(float* out, long long n, unsigned long long seed, unsigned long long stream_id, cudaStream_t st);
-void launch_scale_copy2(const float* eps, float s, float* z, RowMap map, cudaStream_t st);   // z[r][0..1] = eps*s
+// z[r][0..1] = eps * s[seg_of_gran[r / map.gran]]
+void launch_scale_copy2(const float* eps, const float* s, const int* seg_of_gran, float* z, RowMap map, cudaStream_t st);
 void launch_fill_zero(float* p, long long n, cudaStream_t st);
-// out[r] = base[r] + sum_k w[r][k] * g[k]   (speaker conditioning: effective biases of the conditioned convs)
-void launch_cond_bias(const float* w, const float* base, const float* g, int rows, int gin, float* out, cudaStream_t st);
+// out[s][r] = base[r] + sum_k w[r][k] * emb_g[sid[s]][k]  for every slot s < nslots   (speaker conditioning: effective
+// biases of the conditioned convs, one set per distinct speaker of a batch)
+void launch_cond_bias(const float* w, const float* base, const float* emb_g, const int* sid, int nslots, int rows, int gin,
+                      float* out, cudaStream_t st);
 
 // launch-configuration errors are not sticky and would otherwise be lost: throw immediately
 void check_launch(const char* what);

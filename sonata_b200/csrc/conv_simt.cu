@@ -157,7 +157,8 @@ __global__ void __launch_bounds__(256, 2) conv_simt_kernel(const ConvArgs a) {
     for (int i = 0; i < TM; i++) {
         const int q = q0 + ty + i * TY;
         if (q >= a.rows_q) continue;
-        const bool valid = row_valid(a.map, q);
+        bool valid;
+        const float* bias = conv_row(a, q, valid);
         const size_t orow = (size_t)q * a.orow_mul + a.orow_add;
 #pragma unroll
         for (int v = 0; v < NV; v++) {
@@ -165,7 +166,7 @@ __global__ void __launch_bounds__(256, 2) conv_simt_kernel(const ConvArgs a) {
             if (n >= a.cout) continue;
             float o[VW];
 #pragma unroll
-            for (int e = 0; e < VW; e++) o[e] = acc[i][v * VW + e] + (a.bias ? a.bias[n + e] : 0.f);
+            for (int e = 0; e < VW; e++) o[e] = acc[i][v * VW + e] + (bias ? bias[n + e] : 0.f);
             if (a.act == ACT_GATE) {
                 // columns are interleaved (tanh_j, sigmoid_j) pairs -> VW/2 outputs at column n/2
                 float g[VW / 2];

@@ -194,14 +194,15 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv_tc_kernel(const ConvArgs a
     for (int h = 0; h < 2; h++) {
         const int q = m_tile * 128 + r0 + 8 * h;
         if (q >= a.rows_q) continue;
-        const bool valid = row_valid(a.map, q);
+        bool valid;
+        const float* bias = conv_row(a, q, valid);
         const size_t orow0 = (size_t)q * a.orow_mul + a.orow_add;
 #pragma unroll
         for (int j = 0; j < NT / 8; j++) {
             const int nb = n0 + 8 * j + 2 * c;          // bias / weight column of the pair's first element
             if (nb >= a.cout) continue;
             float o[2] = {acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1]};
-            if (a.bias) { o[0] += a.bias[nb]; o[1] += a.bias[nb + 1]; }
+            if (bias) { o[0] += bias[nb]; o[1] += bias[nb + 1]; }
             if (gate) {
                 // phase-fused ConvTranspose never gates: the pair (2k, 2k+1) gives output column k
                 a.y0[orow0 * a.ldy0 + (nb >> 1)] = valid ? tanhf(o[0]) * (1.f / (1.f + expf(-o[1]))) * a.scale : 0.f;

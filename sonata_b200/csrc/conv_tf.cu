@@ -232,14 +232,15 @@ __global__ void __launch_bounds__(TF_THREADS, 1) conv_tf_kernel(const ConvArgs a
         }
         const int q = m_tile * 128 + row;
         if (q >= a.rows_q) continue;
-        const bool valid = row_valid(a.map, q);
+        bool valid;
+        const float* bias = conv_row(a, q, valid);
         const size_t orow = (size_t)q + a.orow_add;
 #pragma unroll
         for (int j = 0; j < NT / 8; j++)
 #pragma unroll
             for (int e = 0; e < 2; e++) {
                 const int n = n_tile * NT + 8 * j + 2 * c + e;
-                float o = run[4 * j + 2 * hh + e] + (a.bias ? a.bias[n] : 0.f);
+                float o = run[4 * j + 2 * hh + e] + (bias ? bias[n] : 0.f);
                 if (a.act == ACT_RELU) o = fmaxf(o, 0.f);
                 if (a.yt && n >= a.yt_col0) {
                     // transposed output (V of the fused q/k/v projection: the P.V contraction wants keys contiguous)

@@ -87,10 +87,7 @@ Job* create_job(Voice* v, const long long* ids, const size_t* offs, size_t B, co
         throw Error(19, "Failed to run model inference. Error: voice was loaded config-only (device -1); libsonata_b200 has no CPU path");
     std::unique_ptr<Job> j(new Job());
     j->v = v; j->B = B; j->debug = debug;
-    {
-        std::shared_lock<std::shared_mutex> g(v->cfg_mu);   // read lock, like piper/src/lib.rs:343
-        j->cfg = v->cfg;
-    }
+    set_job_configs(*j, nullptr);
     j->offs.assign(offs, offs + B + 1);
     j->ids.assign(ids + offs[0], ids + offs[B]);
     const size_t base = offs[0];
@@ -178,6 +175,23 @@ Job* create_job(Voice* v, const long long* ids, const size_t* offs, size_t B, co
     return j.release();
 }
 
+void check_config(const Voice& v, const SynthConfig& c, const std::string& who) {
+    if (!c.has_speaker) return;
+    for (auto& kv : v.speaker_id_map)
+        if (kv.second == c.speaker) return;
+    throw Error(19, who + "No speaker was found with the given id `" + std::to_string(c.speaker) + "`");
+}
+
+void set_job_configs(Job& j, const SynthConfig* cfgs) {
+    if (!cfgs) {
+        std::shared_lock<std::shared_mutex> g(j.v->cfg_mu);   // read lock, like piper/src/lib.rs:343
+        j.cfgs.assign(j.B, j.v->cfg);
+        return;
+    }
+    for (size_t b = 0; b < j.B; b++) check_config(*j.v, cfgs[b], "utterance " + std::to_string(b) + ": ");
+    j.cfgs.assign(cfgs, cfgs + j.B);
+}
+
 namespace {
 
 struct Runner {
@@ -208,12 +222,16 @@ struct Runner {
         bool tf_ok = false;    // duration-critical layer: wgmma 3xTF32 with chunk-flushed accumulation (conv_tf.cu)
         float* yt = nullptr; int yt_col0 = 0, ldyt = 0;     // conv_tf only: column tiles >= yt_col0 stored transposed
     };
-    // bias of a conv: the voice's, or this call's speaker-conditioned one (multi-speaker voices)
-    const float* bias_of(const ConvW& w) const { return (j.d_cond && w.cond_off >= 0) ? j.d_cond + w.cond_off : w.bias; }
+    // bias of a conv: the voice's, or on a multi-speaker voice the speaker-conditioned one of each row's slot
+    void bias_of(const ConvW& w, const Level& lin, ConvArgs& p) const {
+        if (!j.d_cond || w.cond_off < 0) { p.bias = w.bias; return; }
+        if (!lin.bias_slot) throw Error(19, "internal: a speaker-conditioned conv on a level without a slot table");
+        p.bias = j.d_cond + w.cond_off; p.bias_slot = lin.bias_slot; p.ldbias = v.cond_rows;
+    }
     void conv(const ConvW& w, const float* x, int ldx, const Level& lin, const Opt& o) {
         ConvArgs p{};
         p.x = x; p.ldx = ldx; p.rows_in = lin.map.rows; p.cin = w.cin; p.in_slope = o.in_slope;
-        p.w = w.w; p.bias = bias_of(w); p.ldw = w.ldw; p.cout = w.cout; p.wtc = w.wtc; p.tc_nt = w.tc_nt; p.wtf = w.wtf;
+        p.w = w.w; bias_of(w, lin, p); p.ldw = w.ldw; p.cout = w.cout; p.wtc = w.wtc; p.tc_nt = w.tc_nt; p.wtf = w.wtf;
         p.ntaps = w.ntaps; memcpy(p.tap_off, w.tap_off, sizeof(p.tap_off)); p.min_off = w.min_off; p.span = w.span;
         p.rows_q = lin.map.rows; p.orow_mul = o.orow_mul; p.orow_add = o.orow_add;
         p.map = lin.map;
@@ -277,10 +295,13 @@ template <typename Carve> void plan(Arena& dev, Arena& pin, Carve&& carve) {
 // Id level (phase 1): X tables, encoder and duration-predictor activations, and with debug the captures.
 struct IdBufs {
     int *ids_rows_h, *xend_h, *xseg_of_h, *ylen_h; SegInfo* xsegs_h; TfTile* tiles_h;     // pinned staging
+    float* scales_h; int *xslot_h, *sid_h;
     int *ids_rows, *xend, *xseg_of_gran, *cum, *ylen; SegInfo* xsegs; TfTile* tiles;
+    float* scales;                             // per utterance: noise_w [B], length_scale [B], noise_scale [B]
+    int *xslot, *sid;                          // multi-speaker voices: speaker slot of every X granule, speaker of every slot
     float *xa, *xb, *qkv, *att, *ffn, *stats, *d0, *t1, *t2, *g, *h29, *zz, *logw;
     float *att_s, *att_vt, *att_orel;          // tensor-core attention: scores of every head, V^T, relative-value term
-    float *epsw, *cond;
+    float *epsw, *cond;                        // cond: [slot][cond_rows]
     float *qkv0, *att0, *p0, *vt0;             // debug: layer 0's attention operands and result
     std::vector<std::array<float*, 4>> dpf;    // debug: each duration flow's input, DDSConv output, spline parameters, output
 
@@ -292,15 +313,23 @@ struct IdBufs {
         ids_rows_h = pin.get<int>(RX); xend_h = pin.get<int>(nxg); xseg_of_h = pin.get<int>(nxg);
         xsegs_h = pin.get<SegInfo>(B); ylen_h = pin.get<int>(B);
         tiles_h = tc_att ? pin.get<TfTile>(ntiles) : nullptr;
+        const bool multi = v.num_speakers > 1;
+        const size_t nslots = j.slot_sid.size();
+        scales_h = pin.get<float>(3 * B);
+        xslot_h = multi ? pin.get<int>(nxg) : nullptr; sid_h = multi ? pin.get<int>(nslots) : nullptr;
         ids_rows = dev.get<int>(RX); xend = dev.get<int>(nxg); xseg_of_gran = dev.get<int>(nxg); xsegs = dev.get<SegInfo>(B);
         cum = dev.get<int>(RX); ylen = dev.get<int>(B);
         tiles = tc_att ? dev.get<TfTile>(ntiles) : nullptr;
+        scales = dev.get<float>(3 * B);
+        xslot = multi ? dev.get<int>(nxg) : nullptr; sid = multi ? dev.get<int>(nslots) : nullptr;
         xa = rows(H); xb = rows(H); qkv = rows(3 * H); att = rows(H); ffn = rows(a.filter); stats = rows(2 * a.inter);
         d0 = rows(H); t1 = rows(H); t2 = rows(H); g = rows(H); h29 = rows(32); zz = rows(2); logw = rows(1);
         att_s = att_vt = att_orel = nullptr;
         if (tc_att) { att_s = dev.get<float>((size_t)a.heads * RX * j.att_tp); att_vt = rows(H); att_orel = rows(H); }
-        epsw = j.cfg.noise_w != 0.f ? rows(2) : nullptr;
-        cond = v.num_speakers > 1 ? dev.get<float>((size_t)v.cond_rows) : nullptr;
+        bool any_noise_w = false;
+        for (const SynthConfig& c : j.cfgs) any_noise_w |= c.noise_w != 0.f;
+        epsw = any_noise_w ? rows(2) : nullptr;
+        cond = multi ? dev.get<float>(nslots * v.cond_rows) : nullptr;
         qkv0 = att0 = p0 = vt0 = nullptr;
         dpf.clear();
         if (j.debug) {
@@ -312,14 +341,18 @@ struct IdBufs {
     }
 };
 
-// Frame-level tables (segment end and owner of every GY-frame tile, the segment list) and their pinned mirrors.
+// Frame-level tables (segment end, owner and on multi-speaker voices speaker slot of every GY-frame tile, the segment
+// list) and their pinned mirrors.
 struct FrameTables {
-    int *yend, *ftile; FrameSeg* fsegs;
-    int *yend_h, *ftile_h; FrameSeg* fsegs_h;
+    int *yend, *ftile, *yslot; FrameSeg* fsegs;
+    int *yend_h, *ftile_h, *yslot_h; FrameSeg* fsegs_h;
     void carve(Arena& dev, Arena& pin, const Job& j) {
         const int ntile = j.RY / GY; const size_t B = j.fsegs.size();
+        const bool multi = j.v->num_speakers > 1;
         yend = dev.get<int>(ntile); ftile = dev.get<int>(ntile); fsegs = dev.get<FrameSeg>(B);
         yend_h = pin.get<int>(ntile); ftile_h = pin.get<int>(ntile); fsegs_h = pin.get<FrameSeg>(B);
+        yslot = multi ? dev.get<int>(ntile) : nullptr;
+        yslot_h = multi ? pin.get<int>(ntile) : nullptr;
     }
 };
 
@@ -370,7 +403,9 @@ struct FrameBufs {
         const size_t RY = (size_t)j.RY;
         y.carve(dev, pin, j);
         s = dev.get<float>(RY * a.inter);
-        epsz = j.cfg.noise_scale != 0.f ? dev.get<float>(RY * a.inter) : nullptr;
+        bool any_noise = false;
+        for (const SynthConfig& c : j.cfgs) any_noise |= c.noise_scale != 0.f;
+        epsz = any_noise ? dev.get<float>(RY * a.inter) : nullptr;
         zp = j.debug ? dev.get<float>(RY * a.inter) : nullptr;
         h = dev.get<float>(RY * a.hidden); acts = dev.get<float>(RY * a.hidden); outb = dev.get<float>(RY * a.hidden);
         wav = nullptr;
@@ -384,6 +419,7 @@ struct FrameBufs {
 // when the chunk leaves as i16, and the pinned slot the result is copied to.
 struct ChunkBufs {
     float* cond;
+    int *sid, *sid_h;
     FrameTables y;
     float *s, *wav;
     DecoderBufs dec;
@@ -391,7 +427,10 @@ struct ChunkBufs {
     float* out_h;
     void carve(Arena& dev, Arena& pin, const Job& j, bool pcm) {
         const Voice& v = *j.v;
-        cond = v.num_speakers > 1 ? dev.get<float>((size_t)v.cond_rows) : nullptr;
+        const bool multi = v.num_speakers > 1;
+        cond = multi ? dev.get<float>((size_t)v.cond_rows) : nullptr;
+        sid = multi ? dev.get<int>(1) : nullptr;
+        sid_h = multi ? pin.get<int>(1) : nullptr;
         y.carve(dev, pin, j);
         s = dev.get<float>((size_t)j.RY * v.a.inter);
         wav = dev.get<float>((size_t)j.total_samples + 4);
@@ -494,17 +533,21 @@ void lay_out_frames(Job& j, const std::vector<int>& y_len, int hop) {
 Level upload_frames(const Job& j, const FrameTables& t, cudaStream_t st) {
     const size_t B = j.fsegs.size();
     const int ntile = j.RY / GY;
-    Level L; L.map = {t.yend, GY, 1, j.RY}; L.valid_rows = 0;
+    Level L; L.map = {t.yend, GY, 1, j.RY}; L.valid_rows = 0; L.bias_slot = t.yslot;
     for (size_t b = 0; b < B; b++) {
         const int t0 = j.fsegs[b].off / GY;
         const int t1 = (b + 1 < B ? j.fsegs[b + 1].off : j.RY) / GY;
-        for (int k = t0; k < t1; k++) { t.yend_h[k] = j.fsegs[b].off + j.fsegs[b].len; t.ftile_h[k] = (int)b; }
+        for (int k = t0; k < t1; k++) {
+            t.yend_h[k] = j.fsegs[b].off + j.fsegs[b].len; t.ftile_h[k] = (int)b;
+            if (t.yslot_h) t.yslot_h[k] = j.slot_of[b];
+        }
         L.valid_rows += j.fsegs[b].len;
     }
     memcpy(t.fsegs_h, j.fsegs.data(), B * sizeof(FrameSeg));
     h2d(t.yend, t.yend_h, ntile * sizeof(int), st);
     h2d(t.ftile, t.ftile_h, ntile * sizeof(int), st);
     h2d(t.fsegs, t.fsegs_h, B * sizeof(FrameSeg), st);
+    if (t.yslot) h2d(t.yslot, t.yslot_h, ntile * sizeof(int), st);
     return L;
 }
 
@@ -524,6 +567,18 @@ void Job::run(float* d_out, size_t d_out_cap) {
     // the softmax kernel's registers; otherwise the fp32 CUDA-core attention kernel
     const int D = H / a.heads;
     const bool tc_att = V.backend == 1 && (D == 96 || D == 48) && max_tx <= 1280 && getenv("SB200_ATT_SIMT") == nullptr;
+    // speaker slots: one set of conditioned biases per distinct speaker of the batch, not per utterance
+    slot_of.assign(B, 0); slot_sid.clear();
+    if (V.num_speakers > 1) {
+        for (size_t b = 0; b < B; b++) {
+            const long long sid = cfgs[b].has_speaker ? cfgs[b].speaker : 0;   // piper/src/lib.rs:353-358: speaker.unwrap_or(0)
+            if (sid < 0 || sid >= V.emb_rows)
+                throw Error(19, "Failed to run model inference. Error: speaker id out of range (utterance " + std::to_string(b) + ")");
+            const auto it = std::find(slot_sid.begin(), slot_sid.end(), (int)sid);
+            slot_of[b] = (int)(it - slot_sid.begin());
+            if (it == slot_sid.end()) slot_sid.push_back((int)sid);
+        }
+    }
     IdBufs x;
     plan(C.dev_id, C.pin, [&](Arena& dev, Arena& pin) { x.carve(dev, pin, *this, tc_att); });
     d_cum = x.cum; d_cond = x.cond;
@@ -540,19 +595,27 @@ void Job::run(float* d_out, size_t d_out_cap) {
         for (int i = 0; i < s.len; i++) x.ids_rows_h[s.off + i] = (int)ids[offs[b] + i];
         const int g0 = s.off / GX, g1 = (b + 1 < B ? xsegs[b + 1].off : RX) / GX;
         for (int g = g0; g < g1; g++) { x.xend_h[g] = s.off + s.len; x.xseg_of_h[g] = (int)b; }
+        x.scales_h[b] = cfgs[b].noise_w; x.scales_h[B + b] = cfgs[b].length_scale; x.scales_h[2 * B + b] = cfgs[b].noise_scale;
     }
     memcpy(x.xsegs_h, xsegs.data(), B * sizeof(SegInfo));
     h2d(x.ids_rows, x.ids_rows_h, (size_t)RX * 4, st);
     h2d(x.xend, x.xend_h, (size_t)nxg * 4, st);
     h2d(x.xseg_of_gran, x.xseg_of_h, (size_t)nxg * 4, st);
     h2d(x.xsegs, x.xsegs_h, B * sizeof(SegInfo), st);
+    h2d(x.scales, x.scales_h, 3 * B * sizeof(float), st);
+    if (x.xslot) {
+        for (int g = 0; g < nxg; g++) x.xslot_h[g] = slot_of[x.xseg_of_h[g]];
+        std::copy(slot_sid.begin(), slot_sid.end(), x.sid_h);
+        h2d(x.xslot, x.xslot_h, (size_t)nxg * 4, st);
+        h2d(x.sid, x.sid_h, slot_sid.size() * 4, st);
+    }
     if (tc_att) {
         memcpy(x.tiles_h, tiles_s.data(), tiles_s.size() * sizeof(TfTile));
         memcpy(x.tiles_h + tiles_s.size(), tiles_o.data(), tiles_o.size() * sizeof(TfTile));
         h2d(x.tiles, x.tiles_h, (tiles_s.size() + tiles_o.size()) * sizeof(TfTile), st);
     }
 
-    Level LX; LX.map = {x.xend, GX, 1, RX}; LX.valid_rows = (long long)ids.size();
+    Level LX; LX.map = {x.xend, GX, 1, RX}; LX.valid_rows = (long long)ids.size(); LX.bias_slot = x.xslot;
     TfGemm gs{}, go{};
     bool tc_att_ok = tc_att;
     if (tc_att) {
@@ -593,11 +656,7 @@ void Job::run(float* d_out, size_t d_out_cap) {
     }
 
     // ---------------- speaker conditioning (multi-speaker voices) ----------------
-    if (x.cond) {
-        const long long sid = cfg.has_speaker ? cfg.speaker : 0;      // piper/src/lib.rs:353-358: speaker.unwrap_or(0)
-        if (sid < 0 || sid >= V.emb_rows) throw Error(19, "Failed to run model inference. Error: speaker id out of range");
-        launch_cond_bias(V.cond_w, V.cond_base, V.emb_g + (size_t)sid * V.gin, V.cond_rows, V.gin, x.cond, st);
-    }
+    if (x.cond) launch_cond_bias(V.cond_w, V.cond_base, V.emb_g, x.sid, (int)slot_sid.size(), V.cond_rows, V.gin, x.cond, st);
 
     // ---------------- text encoder ----------------
     // Every contraction here reaches the duration predictor, and ceil(duration) is a cliff: the dense layers and the two
@@ -648,7 +707,7 @@ void Job::run(float* d_out, size_t d_out_cap) {
     { Runner::Opt o; o.y0 = x.d0; o.ldy0 = H; o.tf_ok = true; R.conv(V.dp_pre, x.xa, H, LX, o); }
     R.dds(V.dp_dds, x.d0, x.t1, x.t2, LX);
     { Runner::Opt o; o.y0 = x.g; o.ldy0 = H; o.tf_ok = true; R.conv(V.dp_proj, x.d0, H, LX, o); }
-    launch_scale_copy2(x.epsw, cfg.noise_w, x.zz, LX.map, st);
+    launch_scale_copy2(x.epsw, x.scales, x.xseg_of_gran, x.zz, LX.map, st);
     // debug: zz, d0 and h29 are reused by every flow, so each flow's stages are captured as copies
     for (size_t s = 0; s < V.dp_flows.size(); s++) {
         const CFlowW& cf = V.dp_flows[s];
@@ -663,7 +722,7 @@ void Job::run(float* d_out, size_t d_out_cap) {
         R.count(0, 4.0 * LX.valid_rows * 34);
         if (debug) d2d(x.dpf[s][3], x.zz, (size_t)RX * 2, st);
     }
-    launch_durations(x.zz, V.ea_m0, V.ea_logs0, cfg.length_scale, x.xsegs, (int)B, x.logw, x.cum, x.ylen, st);
+    launch_durations(x.zz, V.ea_m0, V.ea_logs0, x.scales + B, x.xsegs, (int)B, x.logw, x.cum, x.ylen, st);
     R.end();
 
     // ---------------- host learns the frame counts (the graph's data-dependent shape) ----------------
@@ -703,7 +762,7 @@ void Job::run(float* d_out, size_t d_out_cap) {
             launch_randn(f.epsz, (long long)RY * I, V.noise_seed, 2 * noise_call + 1, st);
         }
     }
-    launch_expand(x.stats, 2 * I, I, x.cum, f.epsz, cfg.noise_scale, f.s, f.y.fsegs, f.y.ftile, LY.map, st);
+    launch_expand(x.stats, 2 * I, I, x.cum, f.epsz, x.scales + 2 * B, f.s, f.y.fsegs, f.y.ftile, LY.map, st);
     R.count(0, 4.0 * LY.valid_rows * 3 * I);
     R.end();
     if (debug) d2d(f.zp, f.s, (size_t)RY * I, st);
@@ -759,7 +818,7 @@ Latent* encode_latent(Voice* v, const long long* ids, size_t n) {
     j->run(nullptr, 0);
     std::unique_ptr<Latent> L(new Latent());
     L->v = v; L->frames = j->y_len[0];
-    L->sid = j->cfg.has_speaker ? j->cfg.speaker : 0;
+    L->sid = j->cfgs[0].has_speaker ? j->cfgs[0].speaker : 0;
     const size_t bytes = (size_t)L->frames * v->a.inter * 4;
     SB_CUDA(cudaMalloc(&L->z, bytes));
     const float* src = j->z_dev + (size_t)j->fsegs[0].off * v->a.inter;
@@ -777,6 +836,10 @@ ChunkBufs decode_chunk_device(Voice* v, const Latent* z, long long lo, long long
     SB_CUDA(cudaSetDevice(v->device));
     const int n = (int)(hi - lo);
     lay_out_frames(j, std::vector<int>{n}, a.hop());
+    // decoder.onnx takes the encoder's `g` (piper/src/lib.rs:706-735, 739-743): one speaker slot
+    if (v->num_speakers > 1 && (z->sid < 0 || z->sid >= v->emb_rows))
+        throw Error(19, "Failed to run model inference. Error: speaker id out of range");
+    j.slot_of.assign(1, 0); j.slot_sid.assign(1, (int)z->sid);
     ChunkBufs b;
     plan(C.dev_frame, C.pin, [&](Arena& dev, Arena& pin) { b.carve(dev, pin, j, pcm); });
     j.d_cond = b.cond; j.d_fsegs = b.y.fsegs; j.d_wav = b.wav;
@@ -785,9 +848,10 @@ ChunkBufs decode_chunk_device(Voice* v, const Latent* z, long long lo, long long
     cudaStream_t st = C.stream;
     Runner R(j);
     SB_CUDA(cudaEventRecord(C.ev_begin, st));
-    if (b.cond) {       // decoder.onnx takes the encoder's `g` (piper/src/lib.rs:706-735, 739-743)
-        if (z->sid < 0 || z->sid >= v->emb_rows) throw Error(19, "Failed to run model inference. Error: speaker id out of range");
-        launch_cond_bias(v->cond_w, v->cond_base, v->emb_g + (size_t)z->sid * v->gin, v->cond_rows, v->gin, b.cond, st);
+    if (b.cond) {
+        b.sid_h[0] = j.slot_sid[0];
+        h2d(b.sid, b.sid_h, sizeof(int), st);
+        launch_cond_bias(v->cond_w, v->cond_base, v->emb_g, b.sid, 1, v->cond_rows, v->gin, b.cond, st);
     }
     Level LY = upload_frames(j, b.y, st);
     launch_fill_zero(b.s, (long long)j.RY * a.inter, st);

@@ -154,12 +154,15 @@ struct Context {
 struct Level {          // one time resolution of the packed batch
     RowMap map;
     long long valid_rows = 0;
+    const int* bias_slot = nullptr;   // speaker slot of every granule (multi-speaker voices), for the conditioned convs
 };
 
 struct Job {
     Voice* v = nullptr;
     Context* ctx = nullptr;
-    SynthConfig cfg;
+    std::vector<SynthConfig> cfgs;    // one per utterance: the voice's fallback config unless set_job_configs changed it
+    std::vector<int> slot_of;         // per utterance: its speaker slot (index into slot_sid)
+    std::vector<int> slot_sid;        // per slot: the speaker id, distinct, in order of first use
     size_t B = 0;
     bool debug = false;
     bool encode_only = false;     // stop after the flow (streaming 'encoder.onnx' half)
@@ -181,7 +184,7 @@ struct Job {
     int* d_cum = nullptr;
     FrameSeg* d_fsegs = nullptr;
     float* d_wav = nullptr;
-    float* d_cond = nullptr;       // effective biases of the speaker-conditioned convs for this call
+    float* d_cond = nullptr;       // effective biases of the speaker-conditioned convs for this call, [slot][cond_rows]
     std::map<std::string, std::pair<float*, int>> dbg;   // name -> (device ptr, cols)
     std::map<std::string, int> dbg_level;                // name -> U (rows per frame), 0 for X level, -1 for an X-level
                                                          // buffer stored transposed ([cols][RX])
@@ -195,6 +198,12 @@ struct Job {
 
 Job* create_job(Voice* v, const long long* ids, const size_t* offs, size_t B, const float* const* eps_w,
                 const float* const* eps_z, const size_t* eps_z_frames, bool debug);
+// Checks a synthesis config against the voice like sb200_set_fallback_synthesis_config: a speaker, when given, must be
+// a value of the voice's speaker_id_map.  `who` prefixes the error message.
+void check_config(const Voice& v, const SynthConfig& c, const std::string& who);
+// Per-utterance configs of the job's next run: cfgs[0 .. B), or the voice's fallback config for every utterance when
+// cfgs is null.  Every entry is checked first; on an error the job keeps its configs.
+void set_job_configs(Job& j, const SynthConfig* cfgs);
 
 struct Latent {
     Voice* v = nullptr;

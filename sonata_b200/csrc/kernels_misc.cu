@@ -466,14 +466,17 @@ __global__ void spline_kernel(const float* __restrict__ h29, int ldh, float* __r
     z[2 * r + tcol] = fminf(fmaxf(root * in_w + in_cw, -B), B);
 }
 
-// z[r][0..1] = eps[r][0..1] * s   (oracle: sdp_reverse  z = eps_w * noise_w)
-__global__ void scale_copy2_kernel(const float* __restrict__ eps, float s, float* __restrict__ z, RowMap map) {
+// z[r][0..1] = eps[r][0..1] * noise_w of r's segment   (oracle: sdp_reverse  z = eps_w * noise_w).  A segment whose
+// noise_w is 0 gets exact zeros, as a call without noise does (eps * 0 would give -0 for a negative draw).
+__global__ void scale_copy2_kernel(const float* __restrict__ eps, const float* __restrict__ s,
+                                   const int* __restrict__ seg_of_gran, float* __restrict__ z, RowMap map) {
     pdl_trigger(); pdl_wait();
     const int r = blockIdx.x * blockDim.x + threadIdx.x;
     if (r >= map.rows) return;
-    const bool v = row_valid(map, r) && eps != nullptr;
-    z[2 * r] = v ? eps[2 * r] * s : 0.f;
-    z[2 * r + 1] = v ? eps[2 * r + 1] * s : 0.f;
+    const float sr = (eps != nullptr && row_valid(map, r)) ? s[seg_of_gran[r / map.gran]] : 0.f;
+    const bool v = sr != 0.f;
+    z[2 * r] = v ? eps[2 * r] * sr : 0.f;
+    z[2 * r + 1] = v ? eps[2 * r + 1] * sr : 0.f;
 }
 
 // ------------------------------------------------------------------ durations: ceil + inclusive scan
@@ -483,11 +486,13 @@ __global__ void scale_copy2_kernel(const float* __restrict__ eps, float s, float
 __device__ __forceinline__ int sat_int(long long v) { return (int)min(v, (long long)INT_MAX); }
 
 __global__ void __launch_bounds__(256) durations_kernel(const float* __restrict__ z, float m0, float logs0,
-                                                        float length_scale, const SegInfo* __restrict__ segs,
+                                                        const float* __restrict__ length_scales,
+                                                        const SegInfo* __restrict__ segs,
                                                         float* __restrict__ logw, int* __restrict__ cum,
                                                         int* __restrict__ y_len) {
     pdl_trigger(); pdl_wait();
     const SegInfo sg = segs[blockIdx.x];
+    const float length_scale = length_scales[blockIdx.x];
     __shared__ long long warp_tot[8];
     __shared__ long long carry_s;
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
@@ -525,7 +530,7 @@ __global__ void __launch_bounds__(256) durations_kernel(const float* __restrict_
 // oracle: expand()   frame j takes token i iff cum[i-1] <= j < cum[i]
 __global__ void __launch_bounds__(256) expand_kernel(const float* __restrict__ stats, int ldst, int I,
                                                      const int* __restrict__ cum, const float* __restrict__ eps,
-                                                     float noise_scale, float* __restrict__ zp,
+                                                     const float* __restrict__ noise_scales, float* __restrict__ zp,
                                                      const FrameSeg* __restrict__ fsegs,
                                                      const int* __restrict__ ftile_seg, RowMap ymap) {
     pdl_trigger(); pdl_wait();
@@ -537,7 +542,10 @@ __global__ void __launch_bounds__(256) expand_kernel(const float* __restrict__ s
         for (int c = lane; c < I; c += 32) o[c] = 0.f;
         return;
     }
-    const FrameSeg fs = fsegs[ftile_seg[r / ymap.gran]];
+    const int seg = ftile_seg[r / ymap.gran];
+    const FrameSeg fs = fsegs[seg];
+    // a segment whose noise_scale is 0 takes the no-noise branch (no `eps * 0` term, which could be -0)
+    const float noise_scale = eps ? noise_scales[seg] : 0.f;
     const int j = r - fs.off;
     const int* cm = cum + fs.xoff;
     int lo = 0, hi = fs.xlen;          // first i with cm[i] > j
@@ -721,13 +729,15 @@ __global__ void randn_kernel(float* __restrict__ out, long long n, unsigned long
         if (i4 * 4 + e < n) out[i4 * 4 + e] = v[e];
 }
 
-// speaker conditioning: one warp per row of the stacked 1x1 conditioning convs
+// speaker conditioning: one warp per row of the stacked 1x1 conditioning convs, one grid row (blockIdx.y) per speaker slot
 __global__ void __launch_bounds__(256) cond_bias_kernel(const float* __restrict__ w, const float* __restrict__ base,
-                                                        const float* __restrict__ g, int rows, int gin,
-                                                        float* __restrict__ out) {
+                                                        const float* __restrict__ emb_g, const int* __restrict__ sid,
+                                                        int rows, int gin, float* __restrict__ out) {
     pdl_trigger(); pdl_wait();
     const int r = blockIdx.x * 8 + (threadIdx.x >> 5), lane = threadIdx.x & 31;
     if (r >= rows) return;
+    const float* g = emb_g + (size_t)sid[blockIdx.y] * gin;
+    out += (size_t)blockIdx.y * rows;
     float s = 0.f;
     for (int k = lane; k < gin; k += 32) s = fmaf(w[(size_t)r * gin + k], g[k], s);
     s = warp_sum(s);
@@ -827,18 +837,18 @@ void launch_spline(const float* h29, int ldh, float* z, int tcol, int bins, floa
     g_launch_count++;
 }
 
-void launch_scale_copy2(const float* eps, float s, float* z, RowMap map, cudaStream_t st) {
-    launch_pdl(scale_copy2_kernel, dim3((map.rows + 255) / 256), dim3(256), 0, st, eps, s, z, map);
+void launch_scale_copy2(const float* eps, const float* s, const int* seg_of_gran, float* z, RowMap map, cudaStream_t st) {
+    launch_pdl(scale_copy2_kernel, dim3((map.rows + 255) / 256), dim3(256), 0, st, eps, s, seg_of_gran, z, map);
     g_launch_count++;
 }
 
-void launch_durations(const float* z, float m0, float logs0, float length_scale, const SegInfo* segs, int nseg,
+void launch_durations(const float* z, float m0, float logs0, const float* length_scale, const SegInfo* segs, int nseg,
                       float* logw, int* cum, int* y_len, cudaStream_t st) {
     launch_pdl(durations_kernel, dim3(nseg), dim3(256), 0, st, z, m0, logs0, length_scale, segs, logw, cum, y_len);
     g_launch_count++;
 }
 
-void launch_expand(const float* stats, int ldst, int I, const int* cum, const float* eps, float noise_scale,
+void launch_expand(const float* stats, int ldst, int I, const int* cum, const float* eps, const float* noise_scale,
                    float* zp, const FrameSeg* fsegs, const int* ftile_seg, RowMap ymap, cudaStream_t st) {
     launch_pdl(expand_kernel, dim3((ymap.rows + 7) / 8), dim3(256), 0, st, stats, ldst, I, cum, eps, noise_scale, zp, fsegs, ftile_seg, ymap);
     g_launch_count++;
@@ -878,8 +888,9 @@ void launch_randn(float* out, long long n, unsigned long long seed, unsigned lon
     g_launch_count++;
 }
 
-void launch_cond_bias(const float* w, const float* base, const float* g, int rows, int gin, float* out, cudaStream_t st) {
-    launch_pdl(cond_bias_kernel, dim3((rows + 7) / 8), dim3(256), 0, st, w, base, g, rows, gin, out);
+void launch_cond_bias(const float* w, const float* base, const float* emb_g, const int* sid, int nslots, int rows, int gin,
+                      float* out, cudaStream_t st) {
+    launch_pdl(cond_bias_kernel, dim3((rows + 7) / 8, nslots), dim3(256), 0, st, w, base, emb_g, sid, rows, gin, out);
     g_launch_count++;
 }
 

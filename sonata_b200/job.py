@@ -10,16 +10,18 @@ import numpy as np
 
 from . import _native as N
 from .core import Audio
-from .piper import _check, _take_audio
+from .piper import _check, _config_array, _take_audio
 
 
 class SynthesisJob:
     def __init__(self, model, batches: Sequence[Sequence[int]], eps_w: Optional[Sequence] = None,
-                 eps_z: Optional[Sequence] = None, debug: bool = False):
+                 eps_z: Optional[Sequence] = None, debug: bool = False, configs: Optional[Sequence] = None):
+        """`configs`: one PiperSynthesisConfig per utterance (see set_configs); None keeps the voice's fallback config."""
         self._m = model
         self._lib = model._lib
         n = len(batches)
         self.batch = n
+        _config_array(configs, n)             # argument errors before the job exists
         packed = np.ascontiguousarray(np.concatenate([np.asarray(b, dtype=np.int64) for b in batches]))
         offs = np.zeros(n + 1, dtype=np.uint64)
         offs[1:] = np.cumsum([len(b) for b in batches])
@@ -50,6 +52,14 @@ class SynthesisJob:
             C.byref(err)), err)
         if debug:
             self._lib.sb200_job_set_debug(self._h, 1)
+        if configs is not None:
+            self.set_configs(configs)
+
+    def set_configs(self, configs: Optional[Sequence]) -> None:
+        """Per-utterance PiperSynthesisConfigs for the next run, or None for the voice's fallback config.  A wrong
+        length or an unknown speaker raises OperationError and leaves the job's configs as they were."""
+        err = N.sb200_error()
+        _check(self._lib.sb200_job_set_configs(self._h, _config_array(configs, self.batch), C.byref(err)), err)
 
     def run(self, d_out_ptr: int = 0, capacity: int = 0) -> float:
         ms, err = C.c_float(), N.sb200_error()

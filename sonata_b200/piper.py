@@ -31,6 +31,22 @@ class PiperSynthesisConfig:
     noise_w: float = 0.8
 
 
+def _config_array(configs: Optional[Sequence["PiperSynthesisConfig"]], n: int):
+    """The C image of per-utterance synthesis configs (None stays None: the voice's fallback config for everyone)."""
+    if configs is None:
+        return None
+    configs = list(configs)
+    if len(configs) != n:
+        raise OperationError(f"Invalid configuration for Vits Model: {len(configs)} configs for {n} utterances")
+    arr = (N.sb200_synth_config * n)()
+    for i, c in enumerate(configs):
+        if not isinstance(c, PiperSynthesisConfig):
+            raise OperationError(f"Invalid configuration for Vits Model (utterance {i})")
+        arr[i] = N.sb200_synth_config(c.speaker or 0, 0 if c.speaker is None else 1, c.noise_scale, c.length_scale,
+                                      c.noise_w)
+    return arr
+
+
 def _check(rc: int, err: N.sb200_error):
     if rc != 0:
         msg = ""
@@ -163,10 +179,16 @@ class _VitsCommons:
         _check(self._lib.sb200_speak_one_sentence(self._h, phonemes.encode("utf-8"), C.byref(a), C.byref(err)), err)
         return _take_audio(a)
 
-    def speak_batch(self, phoneme_batches: Sequence[str]) -> List[Audio]:
+    def speak_batch(self, phoneme_batches: Sequence[str],
+                    configs: Optional[Sequence[PiperSynthesisConfig]] = None) -> List[Audio]:
+        """`configs`: one PiperSynthesisConfig per utterance (speaker and scales), still synthesised as one pass;
+        None uses the fallback config for every utterance."""
         n = len(phoneme_batches)
+        _config_array(configs, n)             # argument errors before any id mapping
         if n == 0:
             return []
+        if configs is not None:
+            return self.infer_batch_with_values([self.phonemes_to_input_ids(p) for p in phoneme_batches], configs)
         arr = (C.c_char_p * n)(*[p.encode("utf-8") for p in phoneme_batches])
         outs = (N.sb200_audio * n)()
         err = N.sb200_error()
@@ -181,15 +203,21 @@ class _VitsCommons:
                                          C.byref(err)), err)
         return _take_audio(a)
 
-    def infer_batch_with_values(self, batches: Sequence[Sequence[int]]) -> List[Audio]:
+    def infer_batch_with_values(self, batches: Sequence[Sequence[int]],
+                                configs: Optional[Sequence[PiperSynthesisConfig]] = None) -> List[Audio]:
+        """Batched infer_with_values.  `configs`: one PiperSynthesisConfig per utterance (speaker and scales), or None
+        for the fallback config; each utterance's result equals a single-utterance call with its config as the
+        fallback, except for the on-device noise, whose draws depend on the batch position."""
         n = len(batches)
+        cfgs = _config_array(configs, n)
         packed = np.ascontiguousarray(np.concatenate([np.asarray(b, dtype=np.int64) for b in batches]))
         offs = np.zeros(n + 1, dtype=np.uint64)
         offs[1:] = np.cumsum([len(b) for b in batches])
         outs = (N.sb200_audio * n)()
         err = N.sb200_error()
-        _check(self._lib.sb200_speak_batch_ids(self._h, packed.ctypes.data_as(C.POINTER(C.c_int64)),
-                                               offs.ctypes.data_as(C.POINTER(C.c_size_t)), n, outs, C.byref(err)), err)
+        _check(self._lib.sb200_speak_batch_ids_configs(self._h, packed.ctypes.data_as(C.POINTER(C.c_int64)),
+                                                       offs.ctypes.data_as(C.POINTER(C.c_size_t)), n, cfgs, outs,
+                                                       C.byref(err)), err)
         return [_take_audio(outs[i]) for i in range(n)]
 
     def _cfg(self, fn) -> PiperSynthesisConfig:

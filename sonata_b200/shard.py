@@ -215,8 +215,9 @@ class Frontend:
 
     `pcm16=True` delivers peak-normalised i16 PCM converted on the device (`to_i16_vec`, samples.rs:51-75): what
     libsonata's callback receives, at half the device->host bytes.  Every device / host buffer is allocated once and
-    reused; the collectives carry only ids and length tables.  `run_local(ids_list, dst, capacity, fmt)` is the per-rank
-    synthesis hook (default: the CUDA job of `model`); the gloo tests pass a deterministic stand-in."""
+    reused; the collectives carry only ids, per-utterance configs and length tables.  `run_local(ids_list, dst, capacity,
+    fmt)` is the per-rank synthesis hook (default: the CUDA job of `model`), called with `configs=` (the shard's configs in
+    its utterance order) only when the caller gave configs; the gloo tests pass a deterministic stand-in."""
 
     def __init__(self, model=None, group=None, pcm16: bool = False, pin: bool = True, run_local: Optional[Callable] = None):
         self.model, self.group, self.pcm16 = model, group, pcm16
@@ -233,11 +234,31 @@ class Frontend:
         self.last_profile = []
 
     # -- collective plumbing ----------------------------------------------------------------------------------------
-    FIRST_BLOCK = 1 << 18      # int64 elements (2 MB) of the first broadcast: [n, total, lens, owner, ids ...]
+    FIRST_BLOCK = 1 << 18      # int64 elements (2 MB) of the first broadcast: [n, total, has_cfg, lens, owner, ids ...,
+    #                            configs: 4 words per utterance when has_cfg]
 
-    def _bcast_ids(self, batches):
-        """ONE broadcast of a fixed-size block carries the header and (for up to ~260k ids) everything else; a second
-        broadcast follows only for larger inputs.  Host staging buffers are page-locked and reused."""
+    @staticmethod
+    def _encode_configs(configs) -> np.ndarray:
+        """int64 image of per-utterance PiperSynthesisConfigs: speaker (-1 for None), then the bits of noise_scale,
+        length_scale and noise_w as float64 (exact for any Python float)."""
+        out = np.empty((len(configs), 4), dtype=np.int64)
+        out[:, 0] = [-1 if c.speaker is None else int(c.speaker) for c in configs]
+        out[:, 1:] = np.array([[c.noise_scale, c.length_scale, c.noise_w] for c in configs],
+                              dtype=np.float64).reshape(-1, 3).view(np.int64)
+        return out.reshape(-1)
+
+    @staticmethod
+    def _decode_configs(words: np.ndarray) -> list:
+        from .piper import PiperSynthesisConfig
+        w = words.reshape(-1, 4)
+        f = np.ascontiguousarray(w[:, 1:]).view(np.float64)
+        return [PiperSynthesisConfig(None if s < 0 else int(s), float(a), float(b), float(c))
+                for s, (a, b, c) in zip(w[:, 0].tolist(), f.tolist())]
+
+    def _bcast_ids(self, batches, configs=None):
+        """ONE broadcast of a fixed-size block carries the header and (for up to ~260k ids) everything else, the
+        per-utterance configs included; a second broadcast follows only for larger inputs.  Host staging buffers are
+        page-locked and reused."""
         rank, world = dist.get_rank(self.group), dist.get_world_size(self.group)
         dev = _dev(self.group)
         fb = self.FIRST_BLOCK
@@ -251,15 +272,18 @@ class Frontend:
             owner = np.zeros(len(batches), dtype=np.int64)
             for r, p in enumerate(lpt_partition(lens.tolist(), world)):
                 owner[p] = r
-            total = 2 + 2 * len(batches) + int(lens.sum())
+            n0 = len(batches)
+            ids_end = 3 + 2 * n0 + int(lens.sum())
+            total = ids_end + (4 * n0 if configs is not None else 0)
             if self._host.numel() < total:
                 self._host = torch.empty(int(total * 1.5), dtype=torch.int64, pin_memory=self._host.is_pinned())
             h = self._host.numpy()
-            h[0], h[1] = len(batches), total
-            n0 = len(batches)
-            h[2:2 + n0] = lens
-            h[2 + n0:2 + 2 * n0] = owner
-            np.concatenate([np.asarray(b, dtype=np.int64) for b in batches], out=h[2 + 2 * n0:total])
+            h[0], h[1], h[2] = n0, total, configs is not None
+            h[3:3 + n0] = lens
+            h[3 + n0:3 + 2 * n0] = owner
+            np.concatenate([np.asarray(b, dtype=np.int64) for b in batches], out=h[3 + 2 * n0:ids_end])
+            if configs is not None:
+                h[ids_end:total] = self._encode_configs(configs)
             self._payload.copy_(self._host[:fb], non_blocking=True)
         dist.broadcast(self._payload, 0, group=self.group)
         if rank != 0:
@@ -285,18 +309,29 @@ class Frontend:
                     torch.cuda.current_stream().synchronize()
         flat = self._host.numpy()
         n = int(flat[0])
-        lens, owner = flat[2:2 + n], flat[2 + n:2 + 2 * n].copy()
-        offs = 2 + 2 * n + np.concatenate([[0], np.cumsum(lens)])
+        lens, owner = flat[3:3 + n], flat[3 + n:3 + 2 * n].copy()
+        offs = 3 + 2 * n + np.concatenate([[0], np.cumsum(lens)])
         mine = np.nonzero(owner == rank)[0]
-        return n, owner, mine, [flat[offs[i]:offs[i + 1]].copy() for i in mine]
+        my_cfgs = None
+        if flat[2]:
+            words = flat[offs[-1]:offs[-1] + 4 * n].reshape(n, 4)
+            my_cfgs = self._decode_configs(words[mine])
+        return n, owner, mine, [flat[offs[i]:offs[i + 1]].copy() for i in mine], my_cfgs
 
-    def synthesize(self, batches: Optional[Sequence[np.ndarray]], device_only: bool = False):
+    def synthesize(self, batches: Optional[Sequence[np.ndarray]], device_only: bool = False,
+                   configs: Optional[Sequence] = None):
         """Collective.  Rank 0 passes every utterance's ids and gets the waveforms back in utterance order (views into
         the shared segment, valid until the next call); the other ranks pass None and get None.
-        `device_only`: stop after the passes (results stay in each GPU's memory): the device-resident timing of bench.py."""
+        `device_only`: stop after the passes (results stay in each GPU's memory): the device-resident timing of bench.py.
+        `configs` (rank 0): one PiperSynthesisConfig per utterance; they travel with the ids and each rank runs its
+        shard with its utterances' configs.  None: the voice's fallback config everywhere."""
         rank, world = dist.get_rank(self.group), dist.get_world_size(self.group)
         dev = _dev(self.group)
-        n, owner, mine, my_ids = self._bcast_ids(batches)
+        if rank == 0 and configs is not None and len(configs) != len(batches):
+            from .core import OperationError
+            raise OperationError(f"Invalid configuration for Vits Model: {len(configs)} configs for {len(batches)} utterances")
+        n, owner, mine, my_ids, my_cfgs = self._bcast_ids(batches, configs)
+        extra = {} if my_cfgs is None else {"configs": my_cfgs}
         bps = 2 if self.pcm16 else 4
         fmt = 1 if self.pcm16 else 0
         # two-step because the layout of the segment depends on every rank's frame counts: run first (waveforms stay on
@@ -306,13 +341,13 @@ class Frontend:
             from .job import SynthesisJob
             samples_local = []
             if my_ids:
-                job = SynthesisJob(self.model, my_ids)
+                job = SynthesisJob(self.model, my_ids, configs=my_cfgs)
                 self.last_device_ms = job.run()
                 samples_local = job.lengths()[1]
                 if self.collect_profile:
                     self.last_profile = job.profile()
         else:
-            samples_local = self.run_local(my_ids, None, 0, fmt) if my_ids else []
+            samples_local = self.run_local(my_ids, None, 0, fmt, **extra) if my_ids else []
         if self._lens is None or self._lens.numel() < n:
             cap = max(n, 1024)
             self._lens = torch.zeros(cap, dtype=torch.int64, device=dev)
@@ -346,7 +381,8 @@ class Frontend:
             if job is not None:
                 job.copy_out(self.seg.address + start, my_bytes, fmt)
             else:
-                self.run_local(my_ids, self.seg.view(start, my_bytes, np.int16 if self.pcm16 else np.float32), my_bytes, fmt)
+                self.run_local(my_ids, self.seg.view(start, my_bytes, np.int16 if self.pcm16 else np.float32), my_bytes, fmt,
+                               **extra)
         if job is not None:
             job.close()
         dist.barrier(group=self.group)
