@@ -174,6 +174,28 @@ int32_t sb200_decode_chunk(sb200_voice* v, const sb200_latent* z, int64_t frame_
                            sb200_audio* out, sb200_error* err);
 void sb200_latent_free(sb200_latent* z);
 
+/* ---- many realtime streams at once: SpeechStreamer (piper/src/lib.rs:765-858) for K clients, as the gRPC server's
+ * SynthesizeUtteranceRealtime (grpc/src/main.rs:356-383) holds them, in one pass per step ----
+ * Batched infer_encoder (:537-574): one encoder pass over `batch` utterances -> outs[b], each freed with
+ * sb200_latent_free in any order (they share one device allocation, released with the last) and sharing ownership of
+ * the voice like sb200_encode_ids' latents.  cfgs: one per utterance as for sb200_speak_batch_ids_configs (NULL = the
+ * fallback config for every utterance); a bad entry fails the call naming the utterance.  As there, the on-device noise
+ * draws depend on the utterance's position in the batch. */
+int32_t sb200_encode_batch_ids_configs(sb200_voice* v, const int64_t* ids_packed, const size_t* offsets, size_t batch,
+                                       const sb200_synth_config* cfgs, sb200_latent** outs, sb200_error* err);
+/* n calls of sb200_decode_chunk (decoder.onnx on z[:, :, lo:hi], :793-840) as ONE decoder pass: outs[k] gets
+ * 256*(hi[k]-lo[k]) samples, bit for bit what sb200_decode_chunk(zs[k], lo[k], hi[k]) returns.  Every latent must come
+ * from `v` and satisfy 0 <= lo < hi <= frames; errors name the chunk.  n = 0 does nothing. */
+int32_t sb200_decode_chunks(sb200_voice* v, const sb200_latent* const* zs, const int64_t* lo, const int64_t* hi, size_t n,
+                            sb200_audio* outs, sb200_error* err);
+/* The same pass, each chunk leaving as what libsonata's SYNTH_MODE_REALTIME emits for it: trim_lo_frames[k] /
+ * trim_hi_frames[k] overlap frames dropped (NULL = none; piper :811-826), crossfade(fade) (samples.rs:144-157; 0 = none),
+ * linear gain[k] (NULL = 1; synth/src/lib.rs:84-86), then to_i16_vec (samples.rs:51-75) normalised to the chunk's own
+ * peak.  outs[k] receives a malloc'ed buffer of lens[k] samples: free with sb200_i16_free. */
+int32_t sb200_decode_chunks_i16(sb200_voice* v, const sb200_latent* const* zs, const int64_t* lo, const int64_t* hi,
+                                const int64_t* trim_lo_frames, const int64_t* trim_hi_frames, size_t n, int32_t fade,
+                                const float* gain, int16_t** outs, size_t* lens, sb200_error* err);
+
 /* ---- introspection for tests / bench ---- */
 /* Copy a named intermediate of the LAST run of `job` to host (time-major fp32, valid rows of
  * utterance b only).  Names: "x","stats","logw","z_p","z","dec.pre","dec.up<i>","dec.mrf<i>", and the first encoder

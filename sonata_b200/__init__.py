@@ -9,10 +9,11 @@ include/sonata_b200.h).  There is no CPU path.
 """
 from .core import (Audio, AudioInfo, AudioSamples, FailedToLoadResource, OperationError, Phonemes,
                    PhonemizationError, SonataError)
-from .synth import AudioOutputConfig, SonataSpeechSynthesizer
-from .piper import (AdaptiveMelChunker, PiperSynthesisConfig, SpeechStreamer, VitsModel, VitsStreamingModel,
-                    from_config_path)
+from .synth import AudioOutputConfig, RealtimeBatch, SonataSpeechSynthesizer
+from .piper import (AdaptiveMelChunker, PiperSynthesisConfig, SpeechStreamer, StreamBatch, VitsModel,
+                    VitsStreamingModel, from_config_path)
 
 __all__ = ["Audio", "AudioInfo", "AudioSamples", "FailedToLoadResource", "OperationError", "Phonemes",
            "PhonemizationError", "SonataError", "AdaptiveMelChunker", "PiperSynthesisConfig", "SpeechStreamer",
-           "VitsModel", "VitsStreamingModel", "from_config_path", "AudioOutputConfig", "SonataSpeechSynthesizer"]
+           "StreamBatch", "VitsModel", "VitsStreamingModel", "from_config_path", "AudioOutputConfig",
+           "SonataSpeechSynthesizer", "RealtimeBatch"]

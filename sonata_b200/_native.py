@@ -85,6 +85,14 @@ SIGNATURES = {
     "sb200_latent_frames": (C.c_int64, [_P]),
     "sb200_decode_chunk": (C.c_int32, [_P, _P, C.c_int64, C.c_int64, C.POINTER(sb200_audio), _ERR]),
     "sb200_latent_free": (None, [_P]),
+    "sb200_encode_batch_ids_configs": (C.c_int32, [_P, C.POINTER(C.c_int64), C.POINTER(C.c_size_t), C.c_size_t,
+                                                   C.POINTER(sb200_synth_config), C.POINTER(_P), _ERR]),
+    "sb200_decode_chunks": (C.c_int32, [_P, C.POINTER(_P), C.POINTER(C.c_int64), C.POINTER(C.c_int64), C.c_size_t,
+                                        C.POINTER(sb200_audio), _ERR]),
+    "sb200_decode_chunks_i16": (C.c_int32, [_P, C.POINTER(_P), C.POINTER(C.c_int64), C.POINTER(C.c_int64),
+                                            C.POINTER(C.c_int64), C.POINTER(C.c_int64), C.c_size_t, C.c_int32,
+                                            C.POINTER(C.c_float), C.POINTER(C.POINTER(C.c_int16)),
+                                            C.POINTER(C.c_size_t), _ERR]),
     "sb200_job_debug_fetch": (C.c_int32, [_P, C.c_char_p, C.c_size_t, C.POINTER(C.POINTER(C.c_float)),
                                           C.POINTER(C.c_size_t), C.POINTER(C.c_size_t), _ERR]),
     "sb200_buffer_free": (None, [C.POINTER(C.c_float)]),

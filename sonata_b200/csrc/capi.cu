@@ -341,6 +341,63 @@ int32_t sb200_decode_chunk(sb200_voice* v, const sb200_latent* z, int64_t lo, in
 }
 void sb200_latent_free(sb200_latent* z) { delete z; }
 
+int32_t sb200_encode_batch_ids_configs(sb200_voice* v, const int64_t* ids, const size_t* offsets, size_t batch,
+                                       const sb200_synth_config* cfgs, sb200_latent** outs, sb200_error* err) {
+    return guarded(err, [&] {
+        const std::vector<SynthConfig> c = cfgs ? cfgs_in(cfgs, batch) : std::vector<SynthConfig>();
+        std::vector<Latent*> ls = encode_latents(v->v.get(), reinterpret_cast<const long long*>(ids), offsets, batch,
+                                                 cfgs ? c.data() : nullptr);
+        for (size_t b = 0; b < batch; b++) outs[b] = new sb200_latent{ls[b], v->v};
+    });
+}
+
+namespace {
+std::vector<const Latent*> latents_of(const sb200_latent* const* zs, size_t n) {
+    std::vector<const Latent*> out(n);
+    for (size_t k = 0; k < n; k++) {
+        if (!zs[k]) throw Error(19, "chunk " + std::to_string(k) + ": null latent");
+        out[k] = zs[k]->l;
+    }
+    return out;
+}
+}  // namespace
+
+int32_t sb200_decode_chunks(sb200_voice* v, const sb200_latent* const* zs, const int64_t* lo, const int64_t* hi, size_t n,
+                            sb200_audio* outs, sb200_error* err) {
+    return guarded(err, [&] {
+        static_assert(sizeof(long long) == sizeof(int64_t), "");
+        const std::vector<const Latent*> ls = latents_of(zs, n);
+        std::vector<std::vector<float>> w; float ms = 0;
+        decode_latent_chunks(v->v.get(), ls.data(), reinterpret_cast<const long long*>(lo),
+                             reinterpret_cast<const long long*>(hi), n, w, &ms);
+        size_t total = 0;
+        for (auto& x : w) total += x.size();
+        for (size_t k = 0; k < n; k++) {
+            outs[k].data = (float*)malloc(w[k].size() * 4 + 4);
+            memcpy(outs[k].data, w[k].data(), w[k].size() * 4);
+            outs[k].len = w[k].size(); outs[k].sample_rate = (uint32_t)v->v->sample_rate;
+            outs[k].inference_ms = ms * (total ? (float)w[k].size() / (float)total : 0.f);
+        }
+    });
+}
+
+int32_t sb200_decode_chunks_i16(sb200_voice* v, const sb200_latent* const* zs, const int64_t* lo, const int64_t* hi,
+                                const int64_t* trim_lo_frames, const int64_t* trim_hi_frames, size_t n, int32_t fade,
+                                const float* gain, int16_t** outs, size_t* lens, sb200_error* err) {
+    return guarded(err, [&] {
+        const std::vector<const Latent*> ls = latents_of(zs, n);
+        std::vector<std::vector<int16_t>> w;
+        decode_latent_chunks_pcm(v->v.get(), ls.data(), reinterpret_cast<const long long*>(lo),
+                                 reinterpret_cast<const long long*>(hi), reinterpret_cast<const long long*>(trim_lo_frames),
+                                 reinterpret_cast<const long long*>(trim_hi_frames), n, fade, gain, w, nullptr);
+        for (size_t k = 0; k < n; k++) {
+            outs[k] = (int16_t*)malloc(w[k].size() * 2 + 2);
+            memcpy(outs[k], w[k].data(), w[k].size() * 2);
+            lens[k] = w[k].size();
+        }
+    });
+}
+
 // ---- introspection ----
 int32_t sb200_job_debug_fetch(sb200_job* job, const char* name, size_t b, float** data, size_t* rows, size_t* cols, sb200_error* err) {
     return guarded(err, [&] {

@@ -192,12 +192,17 @@ void launch_conv_post(const float* x, int C, const float* w /*[7][C]*/, float* w
 // what the reference applies to a chunk before the 16-bit conversion (see kernels_misc.cu): overlap trim (samples),
 // crossfade table of fade_n <= 48 entries, linear gain.  Default = plain to_i16_vec.
 struct PcmPost { float gain = 1.f; int fade_n = 0; long long trim_lo = 0, trim_hi = 0; float tab[48] = {0}; };
-void launch_i16(const float* wav, const FrameSeg* fsegs, int nseg, int hop, long long max_samples, unsigned* maxbits,
-                short* out, const PcmPost& post, cudaStream_t st);
+// posts: device array, one entry per segment; max_samples: the longest segment (before trimming), sizes the grid
+void launch_i16(const float* wav, const FrameSeg* fsegs, const PcmPost* posts, int nseg, int hop, long long max_samples,
+                unsigned* maxbits, short* out, cudaStream_t st);
+// One row range of a frame level taken from a latent: rows [off, off + len) of the level are rows [lo, lo + len) of src.
+struct GatherSeg { const float* src; long long lo; int off; int len; };
+// s[r] = the source row of r's segment (tile_seg: segment of every gran-row tile), or exact zeros past its end.
+// cols is a multiple of 4 and every src is 16-byte aligned.
+void launch_gather_rows(const GatherSeg* segs, const int* tile_seg, int gran, int rows, int cols, float* s, cudaStream_t st);
 void launch_randn(float* out, long long n, unsigned long long seed, unsigned long long stream_id, cudaStream_t st);
 // z[r][0..1] = eps * s[seg_of_gran[r / map.gran]]
 void launch_scale_copy2(const float* eps, const float* s, const int* seg_of_gran, float* z, RowMap map, cudaStream_t st);
-void launch_fill_zero(float* p, long long n, cudaStream_t st);
 // out[s][r] = base[r] + sum_k w[r][k] * emb_g[sid[s]][k]  for every slot s < nslots   (speaker conditioning: effective
 // biases of the conditioned convs, one set per distinct speaker of a batch)
 void launch_cond_bias(const float* w, const float* base, const float* emb_g, const int* sid, int nslots, int rows, int gin,

@@ -415,28 +415,35 @@ struct FrameBufs {
     }
 };
 
-// One streaming decoder chunk: speaker biases, tables, the latent slice, the decoder, the waveform, the PCM scratch
-// when the chunk leaves as i16, and the pinned slot the result is copied to.
+// One pass of streaming decoder chunks: speaker biases of every slot, tables, the gather table and the latent slices,
+// the decoder, the waveforms, the PCM scratch when the chunks leave as i16, and the pinned block the packed result is
+// copied to.
 struct ChunkBufs {
     float* cond;
     int *sid, *sid_h;
     FrameTables y;
+    GatherSeg *src, *src_h;
     float *s, *wav;
     DecoderBufs dec;
+    PcmPost *post, *post_h;
     short* i16; unsigned* max;
     float* out_h;
     void carve(Arena& dev, Arena& pin, const Job& j, bool pcm) {
         const Voice& v = *j.v;
         const bool multi = v.num_speakers > 1;
-        cond = multi ? dev.get<float>((size_t)v.cond_rows) : nullptr;
-        sid = multi ? dev.get<int>(1) : nullptr;
-        sid_h = multi ? pin.get<int>(1) : nullptr;
+        const size_t n = j.fsegs.size(), nslots = j.slot_sid.size();
+        cond = multi ? dev.get<float>(nslots * v.cond_rows) : nullptr;
+        sid = multi ? dev.get<int>(nslots) : nullptr;
+        sid_h = multi ? pin.get<int>(nslots) : nullptr;
         y.carve(dev, pin, j);
+        src = dev.get<GatherSeg>(n); src_h = pin.get<GatherSeg>(n);
         s = dev.get<float>((size_t)j.RY * v.a.inter);
         wav = dev.get<float>((size_t)j.total_samples + 4);
         dec.carve(dev, v, j.RY, false);
+        post = pcm ? dev.get<PcmPost>(n) : nullptr;
+        post_h = pcm ? pin.get<PcmPost>(n) : nullptr;
         i16 = pcm ? dev.get<short>((size_t)j.total_samples + 8) : nullptr;
-        max = pcm ? dev.get<unsigned>(4) : nullptr;
+        max = pcm ? dev.get<unsigned>(n) : nullptr;
         out_h = pin.get<float>((size_t)j.total_samples);
     }
 };
@@ -809,71 +816,38 @@ void Job::run(float* d_out, size_t d_out_cap) {
 }
 
 // ====================================================================== streaming halves
-Latent::~Latent() { if (z) { cudaSetDevice(v->device); cudaFree(z); } }
+std::vector<Latent*> encode_latents(Voice* v, const long long* ids, const size_t* offs, size_t B, const SynthConfig* cfgs) {
+    std::unique_ptr<Job> j(create_job(v, ids, offs, B, nullptr, nullptr, nullptr, false));
+    if (cfgs) set_job_configs(*j, cfgs);
+    j->encode_only = true;
+    j->run(nullptr, 0);
+    const size_t I = (size_t)v->a.inter;
+    size_t total = 0;
+    for (int f : j->y_len) total += (size_t)f;
+    // one allocation for the whole pass: cudaMalloc synchronises the device, so B of them would stall other streams B times
+    float* p = nullptr;
+    SB_CUDA(cudaMalloc(&p, std::max<size_t>(total, 1) * I * 4));
+    const int dev = v->device;
+    std::shared_ptr<float> mem(p, [dev](float* q) { cudaSetDevice(dev); cudaFree(q); });
+    std::vector<std::unique_ptr<Latent>> ls(B);
+    size_t row = 0;
+    for (size_t b = 0; b < B; b++) {
+        Latent& L = *(ls[b] = std::unique_ptr<Latent>(new Latent()));
+        L.v = v; L.mem = mem; L.z = p + row * I; L.frames = j->y_len[b];
+        L.sid = j->cfgs[b].has_speaker ? j->cfgs[b].speaker : 0;
+        SB_CUDA(cudaMemcpyAsync(L.z, j->z_dev + (size_t)j->fsegs[b].off * I, (size_t)L.frames * I * 4,
+                                cudaMemcpyDeviceToDevice, j->ctx->stream));
+        row += (size_t)L.frames;
+    }
+    SB_CUDA(cudaStreamSynchronize(j->ctx->stream));
+    std::vector<Latent*> out(B);
+    for (size_t b = 0; b < B; b++) out[b] = ls[b].release();
+    return out;
+}
 
 Latent* encode_latent(Voice* v, const long long* ids, size_t n) {
     const size_t offs[2] = {0, n};
-    std::unique_ptr<Job> j(create_job(v, ids, offs, 1, nullptr, nullptr, nullptr, false));
-    j->encode_only = true;
-    j->run(nullptr, 0);
-    std::unique_ptr<Latent> L(new Latent());
-    L->v = v; L->frames = j->y_len[0];
-    L->sid = j->cfgs[0].has_speaker ? j->cfgs[0].speaker : 0;
-    const size_t bytes = (size_t)L->frames * v->a.inter * 4;
-    SB_CUDA(cudaMalloc(&L->z, bytes));
-    const float* src = j->z_dev + (size_t)j->fsegs[0].off * v->a.inter;
-    SB_CUDA(cudaMemcpy(L->z, src, bytes, cudaMemcpyDeviceToDevice));
-    return L.release();
-}
-
-namespace {
-// decoder on z[lo:hi) with the result left on the device (job-owned arena): shared by the f32 and the PCM entry points
-ChunkBufs decode_chunk_device(Voice* v, const Latent* z, long long lo, long long hi, Job& j, bool pcm) {
-    if (lo < 0 || hi > z->frames || lo >= hi) throw Error(19, "Invalid model audio output");
-    const Arch& a = v->a;
-    j.v = v; j.B = 1; j.ctx = v->acquire();
-    Context& C = *j.ctx;
-    SB_CUDA(cudaSetDevice(v->device));
-    const int n = (int)(hi - lo);
-    lay_out_frames(j, std::vector<int>{n}, a.hop());
-    // decoder.onnx takes the encoder's `g` (piper/src/lib.rs:706-735, 739-743): one speaker slot
-    if (v->num_speakers > 1 && (z->sid < 0 || z->sid >= v->emb_rows))
-        throw Error(19, "Failed to run model inference. Error: speaker id out of range");
-    j.slot_of.assign(1, 0); j.slot_sid.assign(1, (int)z->sid);
-    ChunkBufs b;
-    plan(C.dev_frame, C.pin, [&](Arena& dev, Arena& pin) { b.carve(dev, pin, j, pcm); });
-    j.d_cond = b.cond; j.d_fsegs = b.y.fsegs; j.d_wav = b.wav;
-    C.events_used = 0;
-    if (!C.ev_begin) { SB_CUDA(cudaEventCreate(&C.ev_begin)); SB_CUDA(cudaEventCreate(&C.ev_end)); }
-    cudaStream_t st = C.stream;
-    Runner R(j);
-    SB_CUDA(cudaEventRecord(C.ev_begin, st));
-    if (b.cond) {
-        b.sid_h[0] = j.slot_sid[0];
-        h2d(b.sid, b.sid_h, sizeof(int), st);
-        launch_cond_bias(v->cond_w, v->cond_base, v->emb_g, b.sid, 1, v->cond_rows, v->gin, b.cond, st);
-    }
-    Level LY = upload_frames(j, b.y, st);
-    launch_fill_zero(b.s, (long long)j.RY * a.inter, st);
-    SB_CUDA(cudaMemcpyAsync(b.s, z->z + (size_t)lo * a.inter, (size_t)n * a.inter * 4, cudaMemcpyDeviceToDevice, st));
-    run_decoder(R, LY, b.y, b.dec, b.s, b.wav);
-    SB_CUDA(cudaEventRecord(C.ev_end, st));
-    return b;
-}
-}  // namespace
-
-void decode_latent_chunk(Voice* v, const Latent* z, long long lo, long long hi, std::vector<float>& out, float* ms) {
-    Job j;
-    const ChunkBufs b = decode_chunk_device(v, z, lo, hi, j, false);
-    Context& C = *j.ctx;
-    cudaStream_t st = C.stream;
-    // through the context's page-locked staging buffer: a DMA copy instead of a pageable one
-    const size_t bytes = (size_t)j.total_samples * 4;
-    SB_CUDA(cudaMemcpyAsync(b.out_h, b.wav, bytes, cudaMemcpyDeviceToHost, st));
-    SB_CUDA(cudaStreamSynchronize(st));
-    SB_CUDA(cudaGetLastError());
-    out.assign(b.out_h, b.out_h + j.total_samples);
-    if (ms) cudaEventElapsedTime(ms, C.ev_begin, C.ev_end);
+    return encode_latents(v, ids, offs, 1, nullptr)[0];
 }
 
 // crossfade table of AudioSamples::crossfade (audio/ops/src/samples.rs:144-157) for a buffer of `len` samples
@@ -884,26 +858,148 @@ static void fill_fade(PcmPost& p, int fade, long long len) {
     for (int i = 0; i < p.fade_n; i++) p.tab[i] = sinf(((float)i / att) * 3.14159265358979f / 2.0f);
 }
 
-void decode_latent_chunk_pcm(Voice* v, const Latent* z, long long lo, long long hi, long long trim_lo_frames,
-                             long long trim_hi_frames, int fade, float gain, std::vector<int16_t>& out, float* ms) {
+namespace {
+// The PCM post-path of one chunk pass: per-chunk trims, crossfade table and gain.
+struct ChunkPcm { const long long *trim_lo, *trim_hi; int fade; const float* gain; };
+
+// One decoder pass over chunks z[k][lo[k] : hi[k]), k < n, laid out as the segments of one frame level: the result is
+// left on the device (job-owned arena), and with `pcm` converted to i16.  Every check runs before any device work.
+// Errors name the chunk and its frame range, except through the single-chunk entry points (`single`), which keep
+// the messages they always gave.
+ChunkBufs decode_chunks_device(Voice* v, const Latent* const* z, const long long* lo, const long long* hi, size_t n,
+                               Job& j, const ChunkPcm* pcm, bool single) {
+    const Arch& a = v->a;
+    const int hop = a.hop();
+    std::vector<int> len(n);
+    j.slot_of.assign(n, 0); j.slot_sid.clear();
+    auto fail = [single](size_t k, const std::string& what, const std::string& detail) {
+        throw Error(19, single ? what : "chunk " + std::to_string(k) + ": " + what + detail);
+    };
+    for (size_t k = 0; k < n; k++) {
+        if (!z[k] || z[k]->v != v) fail(k, "the latent was not encoded by this voice", "");
+        if (lo[k] < 0 || lo[k] >= hi[k] || hi[k] > z[k]->frames)
+            fail(k, "Invalid model audio output", " (frames [" + std::to_string(lo[k]) + ", " + std::to_string(hi[k]) +
+                                                  ") of a latent of " + std::to_string(z[k]->frames) + ")");
+        if (pcm) {
+            const long long tl = pcm->trim_lo ? pcm->trim_lo[k] : 0, th = pcm->trim_hi ? pcm->trim_hi[k] : 0;
+            if (tl < 0 || th < 0 || tl + th >= hi[k] - lo[k]) fail(k, "Invalid model audio output", " (trim)");
+        }
+        // decoder.onnx takes the encoder's `g` (piper/src/lib.rs:706-735, 739-743): one speaker slot per distinct sid
+        if (v->num_speakers > 1) {
+            const long long sid = z[k]->sid;
+            if (sid < 0 || sid >= v->emb_rows) fail(k, "Failed to run model inference. Error: speaker id out of range", "");
+            const auto it = std::find(j.slot_sid.begin(), j.slot_sid.end(), (int)sid);
+            j.slot_of[k] = (int)(it - j.slot_sid.begin());
+            if (it == j.slot_sid.end()) j.slot_sid.push_back((int)sid);
+        }
+        len[k] = (int)(hi[k] - lo[k]);
+    }
+    j.v = v; j.B = n; j.ctx = v->acquire();
+    Context& C = *j.ctx;
+    SB_CUDA(cudaSetDevice(v->device));
+    lay_out_frames(j, len, hop);
+    ChunkBufs b;
+    plan(C.dev_frame, C.pin, [&](Arena& dev, Arena& pin) { b.carve(dev, pin, j, pcm != nullptr); });
+    j.d_cond = b.cond; j.d_fsegs = b.y.fsegs; j.d_wav = b.wav;
+    C.events_used = 0;
+    if (!C.ev_begin) { SB_CUDA(cudaEventCreate(&C.ev_begin)); SB_CUDA(cudaEventCreate(&C.ev_end)); }
+    cudaStream_t st = C.stream;
+    Runner R(j);
+    SB_CUDA(cudaEventRecord(C.ev_begin, st));
+    if (b.cond) {
+        std::copy(j.slot_sid.begin(), j.slot_sid.end(), b.sid_h);
+        h2d(b.sid, b.sid_h, j.slot_sid.size() * sizeof(int), st);
+        launch_cond_bias(v->cond_w, v->cond_base, v->emb_g, b.sid, (int)j.slot_sid.size(), v->cond_rows, v->gin, b.cond, st);
+    }
+    Level LY = upload_frames(j, b.y, st);
+    for (size_t k = 0; k < n; k++) b.src_h[k] = GatherSeg{z[k]->z, lo[k], j.fsegs[k].off, len[k]};
+    h2d(b.src, b.src_h, n * sizeof(GatherSeg), st);
+    launch_gather_rows(b.src, b.y.ftile, GY, j.RY, a.inter, b.s, st);
+    run_decoder(R, LY, b.y, b.dec, b.s, b.wav);
+    if (pcm) {
+        long long longest = 0;
+        for (size_t k = 0; k < n; k++) {
+            PcmPost& p = b.post_h[k];
+            p = PcmPost();
+            p.gain = pcm->gain ? pcm->gain[k] : 1.f;
+            p.trim_lo = (pcm->trim_lo ? pcm->trim_lo[k] : 0) * hop;
+            p.trim_hi = (pcm->trim_hi ? pcm->trim_hi[k] : 0) * hop;
+            if (pcm->fade > 0) fill_fade(p, pcm->fade, (long long)len[k] * hop - p.trim_lo - p.trim_hi);
+            longest = std::max(longest, (long long)len[k] * hop);
+        }
+        h2d(b.post, b.post_h, n * sizeof(PcmPost), st);
+        launch_i16(b.wav, b.y.fsegs, b.post, (int)n, hop, longest, b.max, b.i16, st);
+    }
+    SB_CUDA(cudaEventRecord(C.ev_end, st));
+    return b;
+}
+
+void chunks_f32(Voice* v, const Latent* const* z, const long long* lo, const long long* hi, size_t n,
+                std::vector<std::vector<float>>& out, float* ms, bool single) {
+    out.clear();
+    if (ms) *ms = 0.f;
+    if (n == 0) return;
     Job j;
-    const int hop = v->a.hop();
-    const size_t total = (size_t)(hi - lo) * hop;
-    const ChunkBufs b = decode_chunk_device(v, z, lo, hi, j, true);
+    const ChunkBufs b = decode_chunks_device(v, z, lo, hi, n, j, nullptr, single);
     Context& C = *j.ctx;
     cudaStream_t st = C.stream;
-    PcmPost post;
-    post.gain = gain; post.trim_lo = trim_lo_frames * hop; post.trim_hi = trim_hi_frames * hop;
-    const long long m = (long long)total - post.trim_lo - post.trim_hi;
-    if (m <= 0) throw Error(19, "Invalid model audio output");
-    if (fade > 0) fill_fade(post, fade, m);
-    launch_i16(b.wav, b.y.fsegs, 1, hop, (long long)total, b.max, b.i16, post, st);
-    int16_t* h = reinterpret_cast<int16_t*>(b.out_h);
-    SB_CUDA(cudaMemcpyAsync(h, b.i16, (size_t)m * 2, cudaMemcpyDeviceToHost, st));
+    // one copy of the packed waveforms through the context's page-locked staging buffer (a DMA copy, not a pageable one)
+    SB_CUDA(cudaMemcpyAsync(b.out_h, b.wav, (size_t)j.total_samples * 4, cudaMemcpyDeviceToHost, st));
     SB_CUDA(cudaStreamSynchronize(st));
     SB_CUDA(cudaGetLastError());
-    out.assign(h, h + m);
+    const int hop = v->a.hop();
+    out.resize(n);
+    for (size_t k = 0; k < n; k++)
+        out[k].assign(b.out_h + j.fsegs[k].out_off, b.out_h + j.fsegs[k].out_off + (size_t)j.fsegs[k].len * hop);
     if (ms) cudaEventElapsedTime(ms, C.ev_begin, C.ev_end);
+}
+
+void chunks_pcm(Voice* v, const Latent* const* z, const long long* lo, const long long* hi, const ChunkPcm& pcm, size_t n,
+                std::vector<std::vector<int16_t>>& out, float* ms, bool single) {
+    out.clear();
+    if (ms) *ms = 0.f;
+    if (n == 0) return;
+    Job j;
+    const ChunkBufs b = decode_chunks_device(v, z, lo, hi, n, j, &pcm, single);
+    Context& C = *j.ctx;
+    cudaStream_t st = C.stream;
+    int16_t* h = reinterpret_cast<int16_t*>(b.out_h);
+    SB_CUDA(cudaMemcpyAsync(h, b.i16, (size_t)j.total_samples * 2, cudaMemcpyDeviceToHost, st));
+    SB_CUDA(cudaStreamSynchronize(st));
+    SB_CUDA(cudaGetLastError());
+    out.resize(n);
+    for (size_t k = 0; k < n; k++) {
+        const PcmPost& p = b.post_h[k];
+        const long long m = (long long)j.fsegs[k].len * v->a.hop() - p.trim_lo - p.trim_hi;
+        out[k].assign(h + j.fsegs[k].out_off, h + j.fsegs[k].out_off + m);
+    }
+    if (ms) cudaEventElapsedTime(ms, C.ev_begin, C.ev_end);
+}
+
+}  // namespace
+
+void decode_latent_chunks(Voice* v, const Latent* const* z, const long long* lo, const long long* hi, size_t n,
+                          std::vector<std::vector<float>>& out, float* ms) {
+    chunks_f32(v, z, lo, hi, n, out, ms, false);
+}
+
+void decode_latent_chunk(Voice* v, const Latent* z, long long lo, long long hi, std::vector<float>& out, float* ms) {
+    std::vector<std::vector<float>> o;
+    chunks_f32(v, &z, &lo, &hi, 1, o, ms, true);
+    out.swap(o[0]);
+}
+
+void decode_latent_chunks_pcm(Voice* v, const Latent* const* z, const long long* lo, const long long* hi,
+                              const long long* trim_lo_frames, const long long* trim_hi_frames, size_t n, int fade,
+                              const float* gain, std::vector<std::vector<int16_t>>& out, float* ms) {
+    chunks_pcm(v, z, lo, hi, ChunkPcm{trim_lo_frames, trim_hi_frames, fade, gain}, n, out, ms, false);
+}
+
+void decode_latent_chunk_pcm(Voice* v, const Latent* z, long long lo, long long hi, long long trim_lo_frames,
+                             long long trim_hi_frames, int fade, float gain, std::vector<int16_t>& out, float* ms) {
+    std::vector<std::vector<int16_t>> o;
+    chunks_pcm(v, &z, &lo, &hi, ChunkPcm{&trim_lo_frames, &trim_hi_frames, fade, &gain}, 1, o, ms, true);
+    out.swap(o[0]);
 }
 
 void job_i16_to_host(Job& j, float gain, int16_t* dst) {
@@ -915,14 +1011,19 @@ void job_i16_to_host(Job& j, float gain, int16_t* dst) {
     long long mx = 0;
     for (size_t b = 0; b < j.B; b++) mx = std::max<long long>(mx, (long long)j.y_len[b] * hop);
     // stream-ordered scratch, returned to the pool at once: device memory held after a run does not grow
-    short* d_i16 = nullptr; unsigned* d_max = nullptr;
+    short* d_i16 = nullptr; unsigned* d_max = nullptr; PcmPost* d_post = nullptr;
     SB_CUDA(cudaMallocAsync(&d_i16, n * 2 + 16, st));
     SB_CUDA(cudaMallocAsync(&d_max, sizeof(unsigned) * j.B, st));
+    SB_CUDA(cudaMallocAsync(&d_post, sizeof(PcmPost) * j.B, st));
     PcmPost post; post.gain = gain;
-    launch_i16(j.d_wav, j.d_fsegs, (int)j.B, hop, mx, d_max, d_i16, post, st);
+    const std::vector<PcmPost> posts(j.B, post);
+    // pageable source: the call returns once the entries are staged, so `posts` may go out of scope before the copy runs
+    SB_CUDA(cudaMemcpyAsync(d_post, posts.data(), sizeof(PcmPost) * j.B, cudaMemcpyHostToDevice, st));
+    launch_i16(j.d_wav, j.d_fsegs, d_post, (int)j.B, hop, mx, d_max, d_i16, st);
     cudaError_t e = cudaMemcpyAsync(dst, d_i16, n * 2, cudaMemcpyDeviceToHost, st);
     cudaFreeAsync(d_i16, st);
     cudaFreeAsync(d_max, st);
+    cudaFreeAsync(d_post, st);
     if (e == cudaSuccess) e = cudaStreamSynchronize(st);
     if (e != cudaSuccess) throw Error(19, std::string("CUDA error: ") + cudaGetErrorString(e));
 }

@@ -208,14 +208,25 @@ void set_job_configs(Job& j, const SynthConfig* cfgs);
 struct Latent {
     Voice* v = nullptr;
     long long sid = 0;    // speaker of the encoder pass (the reference hands `g` from encoder.onnx to decoder.onnx)
-    float* z = nullptr;   // device [frames][inter]
+    std::shared_ptr<float> mem;   // device allocation shared by the latents of one encoder pass, freed with the last
+    float* z = nullptr;   // device [frames][inter], inside `mem`
     long long frames = 0;
-    ~Latent();
 };
+// One encoder pass over B utterances (cfgs: one per utterance, or null for the voice's fallback config) -> B latents
+// sharing one device allocation.  The caller owns the returned pointers.
+std::vector<Latent*> encode_latents(Voice* v, const long long* ids, const size_t* offs, size_t B, const SynthConfig* cfgs);
 Latent* encode_latent(Voice* v, const long long* ids, size_t n);
+// One frame-level decoder pass over n chunks z[k][lo[k] : hi[k]) of latents of `v`; out[k] gets chunk k's waveform.
+// Chunk k equals the same chunk decoded alone, bit for bit.  ms: the pass's device time.
+void decode_latent_chunks(Voice* v, const Latent* const* z, const long long* lo, const long long* hi, size_t n,
+                          std::vector<std::vector<float>>& out, float* ms);
 void decode_latent_chunk(Voice* v, const Latent* z, long long lo, long long hi, std::vector<float>& out, float* ms);
-// the same chunk as peak-normalised i16 PCM with the reference's post-path done on the DEVICE: drop trim_lo / trim_hi
-// overlap frames, crossfade(fade) (samples.rs:144-157), linear gain, to_i16_vec (samples.rs:51-75)
+// the same chunks as peak-normalised i16 PCM with the reference's post-path done on the DEVICE, per chunk: drop
+// trim_lo / trim_hi overlap frames (null: none), crossfade(fade) (samples.rs:144-157), linear gain (null: 1),
+// to_i16_vec (samples.rs:51-75) normalised to the chunk's own peak
+void decode_latent_chunks_pcm(Voice* v, const Latent* const* z, const long long* lo, const long long* hi,
+                              const long long* trim_lo_frames, const long long* trim_hi_frames, size_t n, int fade,
+                              const float* gain, std::vector<std::vector<int16_t>>& out, float* ms);
 void decode_latent_chunk_pcm(Voice* v, const Latent* z, long long lo, long long hi, long long trim_lo_frames,
                              long long trim_hi_frames, int fade, float gain, std::vector<int16_t>& out, float* ms);
 void job_pcm16(Job& j, float gain, std::vector<std::vector<int16_t>>& out);

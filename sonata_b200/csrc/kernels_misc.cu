@@ -653,43 +653,64 @@ __global__ void __launch_bounds__(256) conv_post_kernel(const float* __restrict_
 // order); halves the device->host bytes of a synthesis result.  `PcmPost` folds in what the reference does to a
 // chunk before that conversion: trimming the overlap frames of a streamed chunk (piper/src/lib.rs:811-826),
 // crossfade(42) (samples.rs:144-157; the sine table is computed by the host so both sides use the same floats) and
-// the linear volume gain of AudioOutputConfig (synth/src/lib.rs:84-86).
-__device__ __forceinline__ float pcm_value(const float* __restrict__ x, long long i, long long m, const PcmPost& p) {
-    float v = x[i];
-    if (p.fade_n > 0) {
-        if (i < p.fade_n) v = __fmul_rn(v, p.tab[i]);
-        else if (i >= m - p.fade_n) v = __fmul_rn(v, p.tab[m - 1 - i]);
+// the linear volume gain of AudioOutputConfig (synth/src/lib.rs:84-86).  Every segment (blockIdx.y) has its own
+// PcmPost, so one launch converts the chunks of many streams, each normalised to its own peak.
+struct PcmSeg {                                // one segment's PcmPost, scalars in registers
+    const float* x; long long n; float gain; int fade_n; const float* tab;
+};
+__device__ __forceinline__ PcmSeg pcm_seg(const float* wav, const FrameSeg& fs, const PcmPost* p, int hop) {
+    const long long trim_lo = p->trim_lo;
+    return {wav + fs.out_off + trim_lo, (long long)fs.len * hop - trim_lo - p->trim_hi, p->gain, p->fade_n, p->tab};
+}
+__device__ __forceinline__ float pcm_value(const PcmSeg& s, long long i) {
+    float v = s.x[i];
+    if (s.fade_n > 0) {
+        if (i < s.fade_n) v = __fmul_rn(v, s.tab[i]);
+        else if (i >= s.n - s.fade_n) v = __fmul_rn(v, s.tab[s.n - 1 - i]);
     }
-    return p.gain == 1.f ? v : __fmul_rn(v, p.gain);
+    return s.gain == 1.f ? v : __fmul_rn(v, s.gain);
 }
 
-__global__ void i16_absmax_kernel(const float* __restrict__ wav, const FrameSeg* __restrict__ fsegs, int hop,
-                                  unsigned* __restrict__ maxbits, const PcmPost post) {
+__global__ void i16_absmax_kernel(const float* __restrict__ wav, const FrameSeg* __restrict__ fsegs,
+                                  const PcmPost* __restrict__ posts, int hop, unsigned* __restrict__ maxbits) {
     pdl_trigger(); pdl_wait();
-    const FrameSeg fs = fsegs[blockIdx.y];
-    const long long n = (long long)fs.len * hop - post.trim_lo - post.trim_hi;
-    const float* x = wav + fs.out_off + post.trim_lo;
+    const PcmSeg s = pcm_seg(wav, fsegs[blockIdx.y], posts + blockIdx.y, hop);
     float m = 0.f;
-    for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x)
-        m = fmaxf(m, fabsf(pcm_value(x, i, n, post)));
+    for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < s.n; i += (long long)gridDim.x * blockDim.x)
+        m = fmaxf(m, fabsf(pcm_value(s, i)));
     m = warp_max(m);
     if ((threadIdx.x & 31) == 0 && m > 0.f) atomicMax(maxbits + blockIdx.y, __float_as_uint(m));   // non-negative floats
                                                                                                   // order like their bits
 }
 
-__global__ void i16_convert_kernel(const float* __restrict__ wav, const FrameSeg* __restrict__ fsegs, int hop,
-                                   const unsigned* __restrict__ maxbits, short* __restrict__ out, const PcmPost post) {
+__global__ void i16_convert_kernel(const float* __restrict__ wav, const FrameSeg* __restrict__ fsegs,
+                                   const PcmPost* __restrict__ posts, int hop, const unsigned* __restrict__ maxbits,
+                                   short* __restrict__ out) {
     pdl_trigger(); pdl_wait();
     const FrameSeg fs = fsegs[blockIdx.y];
-    const long long n = (long long)fs.len * hop - post.trim_lo - post.trim_hi;
-    const float* x = wav + fs.out_off + post.trim_lo;
+    const PcmSeg s = pcm_seg(wav, fs, posts + blockIdx.y, hop);
     short* y = out + fs.out_off;
     const float amax = fmaxf(__uint_as_float(maxbits[blockIdx.y]), 1.1920928955078125e-07f);
     const float scale = __fdiv_rn(32767.0f, amax);
-    for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
-        const float v = fminf(fmaxf(__fmul_rn(pcm_value(x, i, n, post), scale), -32768.0f), 32767.0f);
+    for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < s.n; i += (long long)gridDim.x * blockDim.x) {
+        const float v = fminf(fmaxf(__fmul_rn(pcm_value(s, i), scale), -32768.0f), 32767.0f);
         y[i] = (short)(int)v;                      // truncating cast
     }
+}
+
+// Frame-level input of a chunk pass: every row is a plain 16-byte copy of its segment's latent row or exact zeros, so a
+// chunk's rows hold the same bits whatever else shares the pass.
+__global__ void gather_rows_kernel(const GatherSeg* __restrict__ segs, const int* __restrict__ tile_seg, int gran, int c4,
+                                   long long n4, float4* __restrict__ s) {
+    pdl_trigger(); pdl_wait();
+    const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n4) return;
+    const int r = (int)(i / c4), c = (int)(i - (long long)r * c4);
+    const GatherSeg g = segs[tile_seg[r / gran]];
+    const int k = r - g.off;                   // >= 0: a segment's tiles start at its first row
+    float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
+    if (k < g.len) v = reinterpret_cast<const float4*>(g.src)[(g.lo + k) * c4 + c];
+    s[i] = v;
 }
 
 // ------------------------------------------------------------------ Philox4x32-10 -> N(0,1)
@@ -742,12 +763,6 @@ __global__ void __launch_bounds__(256) cond_bias_kernel(const float* __restrict_
     for (int k = lane; k < gin; k += 32) s = fmaf(w[(size_t)r * gin + k], g[k], s);
     s = warp_sum(s);
     if (lane == 0) out[r] = base[r] + s;
-}
-
-__global__ void fill_zero_kernel(float4* p, long long n4) {
-    pdl_trigger(); pdl_wait();
-    const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i < n4) p[i] = make_float4(0.f, 0.f, 0.f, 0.f);
 }
 
 template <typename K>
@@ -869,17 +884,25 @@ void launch_conv_post(const float* x, int C, const float* w, float* wav, const F
     g_launch_count++;
 }
 
-void launch_i16(const float* wav, const FrameSeg* fsegs, int nseg, int hop, long long max_samples, unsigned* maxbits,
-                short* out, const PcmPost& post, cudaStream_t st) {
+void launch_i16(const float* wav, const FrameSeg* fsegs, const PcmPost* posts, int nseg, int hop, long long max_samples,
+                unsigned* maxbits, short* out, cudaStream_t st) {
     if (nseg <= 0) return;
     cudaMemsetAsync(maxbits, 0, sizeof(unsigned) * nseg, st);
     int bx = (int)((max_samples + 256 * 8 - 1) / (256 * 8));
     if (bx < 1) bx = 1;
     if (bx > 1024) bx = 1024;
     dim3 grid(bx, nseg);
-    launch_pdl(i16_absmax_kernel, dim3(grid), dim3(256), 0, st, wav, fsegs, hop, maxbits, post);
-    launch_pdl(i16_convert_kernel, dim3(grid), dim3(256), 0, st, wav, fsegs, hop, maxbits, out, post);
+    launch_pdl(i16_absmax_kernel, dim3(grid), dim3(256), 0, st, wav, fsegs, posts, hop, maxbits);
+    launch_pdl(i16_convert_kernel, dim3(grid), dim3(256), 0, st, wav, fsegs, posts, hop, maxbits, out);
     g_launch_count += 2;
+}
+
+void launch_gather_rows(const GatherSeg* segs, const int* tile_seg, int gran, int rows, int cols, float* s, cudaStream_t st) {
+    if (cols % 4 != 0) throw_launch_error("gather_rows: channel count must be a multiple of 4");
+    const long long n4 = (long long)rows * (cols / 4);
+    launch_pdl(gather_rows_kernel, dim3((unsigned)((n4 + 255) / 256)), dim3(256), 0, st, segs, tile_seg, gran, cols / 4, n4,
+               reinterpret_cast<float4*>(s));
+    g_launch_count++;
 }
 
 void launch_randn(float* out, long long n, unsigned long long seed, unsigned long long stream_id, cudaStream_t st) {
@@ -891,12 +914,6 @@ void launch_randn(float* out, long long n, unsigned long long seed, unsigned lon
 void launch_cond_bias(const float* w, const float* base, const float* emb_g, const int* sid, int nslots, int rows, int gin,
                       float* out, cudaStream_t st) {
     launch_pdl(cond_bias_kernel, dim3((rows + 7) / 8, nslots), dim3(256), 0, st, w, base, emb_g, sid, rows, gin, out);
-    g_launch_count++;
-}
-
-void launch_fill_zero(float* p, long long n, cudaStream_t st) {
-    const long long n4 = n / 4;
-    launch_pdl(fill_zero_kernel, dim3((unsigned)((n4 + 255) / 256)), dim3(256), 0, st, reinterpret_cast<float4*>(p), n4);
     g_launch_count++;
 }
 

@@ -327,12 +327,208 @@ class VitsStreamingModel(_VitsCommons):
                                           C.byref(err)), err)
         return EncoderOutputs(self, h)
 
+    def infer_encoder_batch(self, batches: Sequence[Sequence[int]],
+                            configs: Optional[Sequence[PiperSynthesisConfig]] = None) -> List[EncoderOutputs]:
+        """infer_encoder over many utterances in one encoder pass.  `configs`: one PiperSynthesisConfig per utterance,
+        or None for the fallback config; each latent equals infer_encoder alone with its config as the fallback,
+        except for the on-device noise, whose draws depend on the batch position."""
+        n = len(batches)
+        cfgs = _config_array(configs, n)
+        if any(len(b) == 0 for b in batches):
+            raise OperationError("Failed to run model inference. Error: empty input sequence")
+        if n == 0:
+            return []
+        packed = np.ascontiguousarray(np.concatenate([np.asarray(b, dtype=np.int64) for b in batches]))
+        offs = np.zeros(n + 1, dtype=np.uint64)
+        offs[1:] = np.cumsum([len(b) for b in batches])
+        outs = (C.c_void_p * n)()
+        err = N.sb200_error()
+        _check(self._lib.sb200_encode_batch_ids_configs(self._h, packed.ctypes.data_as(C.POINTER(C.c_int64)),
+                                                        offs.ctypes.data_as(C.POINTER(C.c_size_t)), n, cfgs, outs,
+                                                        C.byref(err)), err)
+        return [EncoderOutputs(self, C.c_void_p(outs[i])) for i in range(n)]
+
+    def infer_decoder_batch(self, chunks: Sequence[tuple], pcm16: bool = False, fade: int = 0,
+                            gains: Optional[Sequence[float]] = None) -> list:
+        """Many `EncoderOutputs.infer_decoder(lo, hi)` calls as one decoder pass.  `chunks`: (encoder outputs, lo, hi)
+        per chunk; each result equals that chunk decoded alone, bit for bit.
+
+        With pcm16, a chunk may be (encoder outputs, lo, hi, trim_lo, trim_hi) and each result is what the realtime
+        mode emits for it as int16: trim_lo / trim_hi overlap frames dropped, crossfade(fade), gains[k] (None: 1),
+        peak-normalised to the chunk's own peak."""
+        n = len(chunks)
+        lo, hi = np.zeros(n, np.int64), np.zeros(n, np.int64)
+        tlo, thi = np.zeros(n, np.int64), np.zeros(n, np.int64)
+        hs = (C.c_void_p * n)()
+        for k, c in enumerate(chunks):
+            if len(c) not in ((3, 5) if pcm16 else (3,)):
+                raise OperationError(f"Invalid decoder chunk {k}: expected (encoder outputs, lo, hi"
+                                     + (", trim_lo, trim_hi)" if pcm16 else ")"))
+            enc = c[0]
+            if not isinstance(enc, EncoderOutputs) or enc._m is not self or not enc._h:
+                raise OperationError(f"Invalid decoder chunk {k}: encoder outputs of another model")
+            lo[k], hi[k] = int(c[1]), int(c[2])
+            if len(c) == 5:
+                tlo[k], thi[k] = int(c[3]), int(c[4])
+            hs[k] = enc._h.value
+        if gains is not None and len(gains) != n:
+            raise OperationError(f"Invalid decoder gains: {len(gains)} gains for {n} chunks")
+        if n == 0:
+            return []
+        p64 = lambda a: a.ctypes.data_as(C.POINTER(C.c_int64))
+        err = N.sb200_error()
+        if not pcm16:
+            outs = (N.sb200_audio * n)()
+            _check(self._lib.sb200_decode_chunks(self._h, hs, p64(lo), p64(hi), n, outs, C.byref(err)), err)
+            return [_take_audio(outs[k]).samples for k in range(n)]
+        g = None if gains is None else np.ascontiguousarray(gains, dtype=np.float32)
+        outs = (C.POINTER(C.c_int16) * n)()
+        lens = (C.c_size_t * n)()
+        _check(self._lib.sb200_decode_chunks_i16(self._h, hs, p64(lo), p64(hi), p64(tlo), p64(thi), n, int(fade),
+                                                 None if g is None else g.ctypes.data_as(C.POINTER(C.c_float)), outs,
+                                                 lens, C.byref(err)), err)
+        res = []
+        for k in range(n):
+            res.append(np.ctypeslib.as_array(outs[k], (lens[k],)).copy() if lens[k] else np.zeros(0, np.int16))
+            self._lib.sb200_i16_free(outs[k])
+        return res
+
     def supports_streaming_output(self) -> bool:
         return True
 
     def stream_synthesis(self, phonemes: str, chunk_size: int, chunk_padding: int) -> SpeechStreamer:
         ids = self.phonemes_to_input_ids(phonemes)
         return SpeechStreamer(self.infer_encoder(ids), chunk_size, chunk_padding)
+
+
+class _Stream:
+    """One sentence of a StreamBatch: its latent and its own chunk schedule, with SpeechStreamer's one-shot rule."""
+
+    def __init__(self, key, enc, chunk_size: int, chunk_padding: int):
+        self.key, self.enc = key, enc
+        self.chunker = AdaptiveMelChunker(enc.num_frames, chunk_size, chunk_padding)
+        self.one_shot = enc.num_frames <= (chunk_size * 2 + chunk_padding * 2)
+
+    def next_chunk(self):
+        """(lo, hi, audio slice or None): the frames to decode next, and how SpeechStreamer.__next__ trims them (None:
+        the one-shot chunk, returned as decoded)."""
+        (m0, m1), (a0, a1) = next(self.chunker)
+        if self.one_shot:
+            self.chunker.consume()
+            return 0, self.enc.num_frames, None
+        return m0, self.enc.num_frames if m1 is None else m1, slice(a0, a1)
+
+    @property
+    def done(self) -> bool:
+        return self.chunker.last_end_index is None
+
+
+def _check_chunking(chunk_size, chunk_padding):
+    if not isinstance(chunk_size, int) or chunk_size < 1:
+        raise OperationError(f"Invalid chunk size {chunk_size!r}: expected a positive integer")
+    if not isinstance(chunk_padding, int) or chunk_padding < 0:
+        raise OperationError(f"Invalid chunk padding {chunk_padding!r}: expected a non-negative integer")
+
+
+class StreamBatch:
+    """Many realtime streams served together (a server holding K `stream_synthesis` clients).
+
+    `add` admits a sentence (phonemes or ids) with an optional PiperSynthesisConfig (None: the fallback config); a
+    config whose speaker the voice does not have is refused there.  Each `step` encodes every stream added since the
+    last step in ONE encoder pass, then decodes the next chunk of every active stream in ONE decoder pass, and returns
+    [(key, AudioSamples)] in admission order.  Each stream keeps its own AdaptiveMelChunker, trim, one-shot rule and
+    crossfade(42), so its chunks are exactly what `stream_synthesis` yields for that sentence with its config as the
+    fallback.
+
+    One stream's failure stays that stream's, as with one `stream_synthesis` per client: when a batched pass raises,
+    its streams are run one at a time, and a stream whose own encoder or decoder work fails gets its SonataError as
+    its item, (key, error), once, and ends.  The other streams carry on."""
+
+    def __init__(self, model, chunk_size: int, chunk_padding: int):
+        _check_chunking(chunk_size, chunk_padding)
+        self.model = model
+        self.chunk_size, self.chunk_padding = chunk_size, chunk_padding
+        self._pending: list = []      # (key, ids, config, chunk_size) not yet encoded
+        self._active: List[_Stream] = []
+        self._next_key = 0
+
+    def add(self, ids_or_phonemes, config: Optional[PiperSynthesisConfig] = None) -> int:
+        return self._add(ids_or_phonemes, config, self.chunk_size)
+
+    def _add(self, ids_or_phonemes, config, chunk_size: int) -> int:
+        if config is not None and not isinstance(config, PiperSynthesisConfig):
+            raise OperationError("Invalid configuration for Vits Model")
+        if config is not None and config.speaker is not None and config.speaker not in (self.model.get_speakers() or {}):
+            raise OperationError(f"No speaker was found with the given id `{config.speaker}`")     # as check_config
+        _check_chunking(chunk_size, self.chunk_padding)
+        if isinstance(ids_or_phonemes, str):
+            ids = self.model.phonemes_to_input_ids(ids_or_phonemes)
+        else:
+            ids = [int(i) for i in ids_or_phonemes]
+        if not ids:
+            raise OperationError("Failed to run model inference. Error: empty input sequence")
+        key = self._next_key
+        self._next_key += 1
+        self._pending.append((key, ids, config, chunk_size))
+        return key
+
+    def __len__(self) -> int:
+        """Streams added and not yet finished."""
+        return len(self._pending) + len(self._active)
+
+    def __contains__(self, key) -> bool:
+        """Whether stream `key` has chunks still to come."""
+        return any(p[0] == key for p in self._pending) or any(s.key == key for s in self._active)
+
+    def step(self) -> List[tuple]:
+        out = []
+        active = self._active
+        if self._pending:
+            pend, self._pending = self._pending, []
+            fallback = None
+            if any(p[2] is not None for p in pend):
+                fallback = self.model.get_fallback_synthesis_config()
+
+            def encode(ps):
+                configs = None if fallback is None else [fallback if p[2] is None else p[2] for p in ps]
+                return self.model.infer_encoder_batch([p[1] for p in ps], configs)
+            for p, (enc, err) in zip(pend, _each_or_alone(encode, pend)):
+                if err is not None:
+                    out.append((p[0], err))
+                else:
+                    active.append(_Stream(p[0], enc, p[3], self.chunk_padding))
+        plan = [(s,) + s.next_chunk() for s in active]
+        failed = set()
+        decoded = _each_or_alone(lambda pl: self.model.infer_decoder_batch([(s.enc, lo, hi) for s, lo, hi, _ in pl]),
+                                 plan) if plan else []
+        for (s, _, _, trim), (a, err) in zip(plan, decoded):
+            if err is not None:
+                out.append((s.key, err))
+                failed.add(s.key)
+                continue
+            if trim is not None:
+                a = AudioSamples(a.as_slice()[trim])
+                a.crossfade(42)
+            out.append((s.key, a))
+        self._active = [s for s in active if not s.done and s.key not in failed]
+        return out
+
+
+def _each_or_alone(call, items):
+    """call(items) as one pass -> [(result, None)]; when that pass raises a SonataError, each item alone, so an item's
+    failure is reported as its own (None, error) and the others still get their results."""
+    try:
+        return [(r, None) for r in call(items)]
+    except SonataError as e:
+        if len(items) == 1:
+            return [(None, e)]
+    out = []
+    for it in items:
+        try:
+            out.append((call([it])[0], None))
+        except SonataError as e:
+            out.append((None, e))
+    return out
 
 
 def from_config_path(config_path, device: int = 0):

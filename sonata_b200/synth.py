@@ -75,6 +75,21 @@ class AudioOutputConfig:
         return Audio(self.apply_to_raw_samples(s), audio.info.sample_rate, audio.inference_ms)
 
 
+def next_chunk_size(chunk_size: int, produced: int) -> int:
+    """The realtime mode's chunk-size growth rule (synth/src/lib.rs:348-356): before every sentence after the first,
+    the chunk size is multiplied by the number of chunks produced so far (chunk_factor = 1)."""
+    return chunk_size * 1 * produced if produced != 0 else chunk_size
+
+
+def _sentences(model, text: str) -> List[str]:
+    """SpeechSynthesisTaskProvider::get_phonemes (:256-258), or newline-separated phoneme sentences when the model has
+    no phonemizer."""
+    try:
+        return model.phonemize_text(text).to_vec()
+    except SonataError:
+        return [s for s in text.split("\n") if s.strip()]
+
+
 class SonataSpeechSynthesizer:
     """synth/src/lib.rs:119-203.  `text` is a phoneme string; sentences are separated by newlines when the
     model has no phonemizer (the espeak-ng front-end is outside this repo)."""
@@ -82,12 +97,8 @@ class SonataSpeechSynthesizer:
     def __init__(self, model):
         self.model = model
 
-    # -- SpeechSynthesisTaskProvider::get_phonemes (:256-258)
     def _phonemes(self, text: str) -> List[str]:
-        try:
-            return self.model.phonemize_text(text).to_vec()
-        except SonataError:
-            return [s for s in text.split("\n") if s.strip()]
+        return _sentences(self.model, text)
 
     def _process(self, audio: Audio, cfg: Optional[AudioOutputConfig]) -> Audio:
         return cfg.apply(audio) if cfg is not None else audio
@@ -113,8 +124,7 @@ class SonataSpeechSynthesizer:
             cs, produced = chunk_size, 0
             try:
                 for ph in self._phonemes(text):
-                    if produced != 0:
-                        cs = cs * 1 * produced                      # chunk_factor = 1 (:348-356)
+                    cs = next_chunk_size(cs, produced)
                     n = 0
                     for chunk in self.model.stream_synthesis(ph, cs, chunk_padding):
                         q.put(output_config.apply_to_raw_samples(chunk) if output_config else chunk)
@@ -151,3 +161,78 @@ class SonataSpeechSynthesizer:
 
     def audio_output_info(self):
         return self.model.audio_output_info()
+
+
+class _Request:
+    def __init__(self, key, ids, output_config, config, chunk_size):
+        self.key, self.ids, self.output_config, self.config = key, ids, output_config, config
+        self.cs, self.produced, self.n, self.next = chunk_size, 0, 0, 0
+
+
+class RealtimeBatch:
+    """Many realtime requests of one or more sentences served together: `synthesize_streamed` for K clients, with every
+    step of every client in one encoder pass (sentences that start) and one decoder pass (the next chunk of each).
+
+    `add(text, output_config, config)` admits a request (config: its PiperSynthesisConfig, None for the fallback);
+    `step()` returns [(key, AudioSamples)].  A request's items are exactly what
+    `synthesize_streamed(text, output_config, chunk_size, chunk_padding)` yields with `config` as the fallback: the
+    chunk-size growth rule across its sentences, volume on every chunk and the appended silence after each sentence.
+    Each sentence's ids are mapped and the config's speaker checked at `add`, so a bad request raises there; a request
+    whose synthesis fails later gets its SonataError as its last item, (key, error), and the others carry on."""
+
+    def __init__(self, model, chunk_size: int = 72, chunk_padding: int = 3):
+        from .piper import StreamBatch
+        self.model = model
+        self.chunk_size = chunk_size
+        self._streams = StreamBatch(model, chunk_size, chunk_padding)
+        self._sr = model.audio_output_info().sample_rate
+        self._by_stream = {}          # stream key -> request of the sentence it speaks
+        self._next_key = 0
+
+    def add(self, text: str, output_config: Optional[AudioOutputConfig] = None, config=None) -> int:
+        from .piper import PiperSynthesisConfig
+        if output_config is not None:
+            output_config._check_supported()
+        if config is not None and not isinstance(config, PiperSynthesisConfig):
+            raise OperationError("Invalid configuration for Vits Model")
+        if config is not None and config.speaker is not None and config.speaker not in (self.model.get_speakers() or {}):
+            raise OperationError(f"No speaker was found with the given id `{config.speaker}`")
+        ids = [self.model.phonemes_to_input_ids(ph) for ph in _sentences(self.model, text)]
+        if any(len(i) == 0 for i in ids):
+            raise OperationError("Failed to run model inference. Error: empty input sequence")
+        req = _Request(self._next_key, ids, output_config, config, self.chunk_size)
+        self._next_key += 1
+        self._start_sentence(req)
+        return req.key
+
+    def _start_sentence(self, req: _Request) -> None:
+        if req.next == len(req.ids):
+            return
+        req.cs = next_chunk_size(req.cs, req.produced)
+        req.n = 0
+        self._by_stream[self._streams._add(req.ids[req.next], req.config, req.cs)] = req
+        req.next += 1
+
+    def __len__(self) -> int:
+        """Requests added and not yet finished."""
+        return len(self._by_stream)
+
+    def step(self) -> List[tuple]:
+        out = []
+        for skey, chunk in self._streams.step():
+            req = self._by_stream[skey]
+            if isinstance(chunk, SonataError):          # the request ends with its error, as synthesize_streamed's
+                del self._by_stream[skey]               # channel delivers it (:368-371); the others carry on
+                out.append((req.key, chunk))
+                continue
+            oc = req.output_config
+            out.append((req.key, oc.apply_to_raw_samples(chunk) if oc else chunk))
+            req.n += 1
+            if skey in self._streams:
+                continue
+            del self._by_stream[skey]                  # the sentence is done
+            req.produced += req.n
+            if oc and oc.appended_silence_ms:
+                out.append((req.key, oc.generate_silence(oc.appended_silence_ms, self._sr)))
+            self._start_sentence(req)
+        return out
