@@ -100,6 +100,11 @@ int64_t sb200_speaker_name_to_id(const sb200_voice* v, const char* name);
 int32_t sb200_phonemes_to_input_ids(const sb200_voice* v, const char* phonemes_utf8, int64_t** ids, size_t* n,
                                     sb200_error* err);
 void sb200_ids_free(int64_t* ids);
+/* sb200_phonemes_to_input_ids plus, per id, where it came from: src_char[i] is the index, in Unicode characters of
+ * `phonemes_utf8`, of the character id i was mapped from.  A pad id belongs to the character before it; bos and eos get
+ * -1; dropped characters own no id.  Both arrays are malloc'ed (free each with sb200_ids_free). */
+int32_t sb200_phonemes_to_input_ids_map(const sb200_voice* v, const char* phonemes_utf8, int64_t** ids,
+                                        int64_t** src_char, size_t* n, sb200_error* err);
 
 /* ---- synthesis ---- */
 /* SonataModel::speak_one_sentence(phonemes: String) (piper/src/lib.rs:439-443) */
@@ -123,6 +128,25 @@ int32_t sb200_speak_batch_ids(sb200_voice* v, const int64_t* ids_packed, const s
 int32_t sb200_speak_batch_ids_configs(sb200_voice* v, const int64_t* ids_packed, const size_t* offsets, size_t batch,
                                       const sb200_synth_config* cfgs, sb200_audio* outs, sb200_error* err);
 
+/* ---- per-phoneme durations: control them, and read when each id is spoken ----
+ * Duration controls are per id, packed like ids_packed (one entry per id of the batch):
+ *   scale_packed[i]  (finite, >= 0): id i lasts ceil((exp(logw) * length_scale) * scale) frames, the product rounded in
+ *                    that order, so a scale of exactly 1.0 gives the bits of a call without scales;
+ *   frames_packed[i] (-1 or >= 0) : >= 0 fixes id i's frame count (its predicted duration is still computed and
+ *                    ignored); -1 keeps the predicted count.
+ * Either array may be NULL (none of that kind).  All-1.0 scales and all -1 frames give the same bits as no controls.
+ * A bad entry fails with OPERATION_ERROR naming the utterance and the id.  0 frames are allowed: the id is skipped; an
+ * utterance whose ids all get 0 frames is 1 frame long, as a prediction summing to 0 always was.
+ * Frames per id (the reference's `p_duration`) come packed like ids_packed; samples of id i = frames * 256. */
+/* sb200_speak_batch_ids_configs with duration controls; id_frames_out (NULL: not wanted) receives the frames per id,
+ * packed like ids_packed.  With NULL controls and NULL id_frames_out this is sb200_speak_batch_ids_configs, bit for bit.
+ * Utterance b equals its single-utterance call with the same config and controls, except for the on-device noise:
+ * its draws depend on the utterance's position in the batch. */
+int32_t sb200_speak_batch_ids_durations(sb200_voice* v, const int64_t* ids_packed, const size_t* offsets, size_t batch,
+                                        const sb200_synth_config* cfgs, const float* scale_packed,
+                                        const int32_t* frames_packed, sb200_audio* outs, int32_t* id_frames_out,
+                                        sb200_error* err);
+
 /* ---- job API: the same batched pass split into its host<->device steps (bench / multi-GPU plumbing) ----
  * create  : copies ids to the device (H2D).  `eps_w` / `eps_z` optionally inject the graph's two
  *           RandomNormalLike draws (time-major: eps_w[b] = f32[T_x][2], eps_z[b] = f32[T_y][inter]);
@@ -141,6 +165,14 @@ int32_t sb200_job_set_debug(sb200_job* job, int32_t on);
  * job's configs unchanged.  Philox noise (no eps_w / eps_z given) depends on each utterance's batch position, as it
  * always has: only injected noise makes a mixed batch equal its utterances run alone. */
 int32_t sb200_job_set_configs(sb200_job* job, const sb200_synth_config* cfgs, sb200_error* err);
+/* Duration controls (see sb200_speak_batch_ids_durations) for the next sb200_job_run; NULL / NULL restores the default
+ * (a job without controls, what a new job starts with).  Every entry is checked first; an invalid one fails with
+ * OPERATION_ERROR naming the utterance and the id, and leaves the job's controls as they were. */
+int32_t sb200_job_set_durations(sb200_job* job, const float* scale_packed, const int32_t* frames_packed, sb200_error* err);
+/* Frames per id of the last run, packed like ids_packed, into out_packed[0 .. capacity): one device->host copy of the
+ * whole batch's cumulative durations, made on the first call after a run.  Fails before a run, or when capacity is
+ * smaller than the number of ids. */
+int32_t sb200_job_id_frames(sb200_job* job, int32_t* out_packed, size_t capacity, sb200_error* err);
 int32_t sb200_job_run(sb200_job* job, float* d_out, size_t d_out_capacity, float* device_ms, sb200_error* err);
 int32_t sb200_job_fetch(sb200_job* job, sb200_audio* outs, sb200_error* err);
 size_t sb200_job_batch(const sb200_job* job);
@@ -183,6 +215,15 @@ void sb200_latent_free(sb200_latent* z);
  * draws depend on the utterance's position in the batch. */
 int32_t sb200_encode_batch_ids_configs(sb200_voice* v, const int64_t* ids_packed, const size_t* offsets, size_t batch,
                                        const sb200_synth_config* cfgs, sb200_latent** outs, sb200_error* err);
+/* sb200_encode_batch_ids_configs with duration controls (see sb200_speak_batch_ids_durations); NULL / NULL is that call,
+ * bit for bit.  Each latent keeps its ids' frame counts: sb200_latent_id_frames. */
+int32_t sb200_encode_batch_ids_durations(sb200_voice* v, const int64_t* ids_packed, const size_t* offsets, size_t batch,
+                                         const sb200_synth_config* cfgs, const float* scale_packed,
+                                         const int32_t* frames_packed, sb200_latent** outs, sb200_error* err);
+/* The encoder's `p_duration` (piper/src/lib.rs:675, 706-717) as frames per id of the latent's utterance (their sum is
+ * its frame count, except that an utterance whose ids all got 0 frames is 1 frame long).  Returns the number of ids;
+ * writes them to out only when capacity is at least that (call with NULL, 0 to learn the size). */
+int64_t sb200_latent_id_frames(const sb200_latent* z, int32_t* out, size_t capacity);
 /* n calls of sb200_decode_chunk (decoder.onnx on z[:, :, lo:hi], :793-840) as ONE decoder pass: outs[k] gets
  * 256*(hi[k]-lo[k]) samples, bit for bit what sb200_decode_chunk(zs[k], lo[k], hi[k]) returns.  Every latent must come
  * from `v` and satisfy 0 <= lo < hi <= frames; errors name the chunk.  n = 0 does nothing. */

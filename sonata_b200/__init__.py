@@ -7,13 +7,13 @@ Public surface mirrors the reference crates on that path:
 All arithmetic runs in sonata_b200/lib/libsonata_b200.so (hand-written sm_90a CUDA, C ABI in
 include/sonata_b200.h).  There is no CPU path.
 """
-from .core import (Audio, AudioInfo, AudioSamples, FailedToLoadResource, OperationError, Phonemes,
+from .core import (Audio, AudioInfo, AudioSamples, FailedToLoadResource, OperationError, PhonemeAlignment, Phonemes,
                    PhonemizationError, SonataError)
 from .synth import AudioOutputConfig, RealtimeBatch, SonataSpeechSynthesizer
 from .piper import (AdaptiveMelChunker, PiperSynthesisConfig, SpeechStreamer, StreamBatch, VitsModel,
                     VitsStreamingModel, from_config_path)
 
-__all__ = ["Audio", "AudioInfo", "AudioSamples", "FailedToLoadResource", "OperationError", "Phonemes",
+__all__ = ["Audio", "AudioInfo", "AudioSamples", "FailedToLoadResource", "OperationError", "PhonemeAlignment", "Phonemes",
            "PhonemizationError", "SonataError", "AdaptiveMelChunker", "PiperSynthesisConfig", "SpeechStreamer",
            "StreamBatch", "VitsModel", "VitsStreamingModel", "from_config_path", "AudioOutputConfig",
            "SonataSpeechSynthesizer", "RealtimeBatch"]

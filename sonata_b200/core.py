@@ -63,6 +63,14 @@ class Phonemes:
 
 
 @dataclass
+class PhonemeAlignment:
+    """When one phoneme of an utterance is spoken: `num_samples` samples of its audio from `start_sample` on."""
+    phoneme: str
+    start_sample: int
+    num_samples: int
+
+
+@dataclass
 class AudioInfo:
     sample_rate: int
     num_channels: int = 1

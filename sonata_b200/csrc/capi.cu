@@ -200,20 +200,43 @@ int32_t sb200_phonemes_to_input_ids(const sb200_voice* v, const char* ph, int64_
     });
 }
 
-int32_t sb200_speak_batch_ids_configs(sb200_voice* v, const int64_t* ids, const size_t* offsets, size_t batch,
-                                      const sb200_synth_config* cfgs, sb200_audio* outs, sb200_error* err) {
+int32_t sb200_phonemes_to_input_ids_map(const sb200_voice* v, const char* ph, int64_t** ids, int64_t** src_char,
+                                        size_t* n, sb200_error* err) {
+    return guarded(err, [&] {
+        std::vector<long long> src;
+        std::vector<long long> r = v->v->phonemes_to_ids(ph, &src);
+        *ids = (int64_t*)malloc(r.size() * sizeof(int64_t));
+        *src_char = (int64_t*)malloc(r.size() * sizeof(int64_t));
+        for (size_t i = 0; i < r.size(); i++) { (*ids)[i] = r[i]; (*src_char)[i] = src[i]; }
+        *n = r.size();
+    });
+}
+
+int32_t sb200_speak_batch_ids_durations(sb200_voice* v, const int64_t* ids, const size_t* offsets, size_t batch,
+                                        const sb200_synth_config* cfgs, const float* scale_packed,
+                                        const int32_t* frames_packed, sb200_audio* outs, int32_t* id_frames_out,
+                                        sb200_error* err) {
     return guarded(err, [&] {
         const double t0 = now_ms();
         static_assert(sizeof(long long) == sizeof(int64_t), "");
         std::unique_ptr<Job> j(create_job(v->v.get(), reinterpret_cast<const long long*>(ids), offsets, batch, nullptr,
                                           nullptr, nullptr, false));
         if (cfgs) set_job_configs(*j, cfgs_in(cfgs, batch).data());
+        set_job_durations(*j, scale_packed, frames_packed);
         j->run(nullptr, 0);
         fetch_audio(*j, outs, 0.f);
+        if (id_frames_out) {
+            const std::vector<int>& f = job_id_frames(*j);
+            std::copy(f.begin(), f.end(), id_frames_out);
+        }
         const float wall = (float)(now_ms() - t0);
         for (size_t b = 0; b < batch; b++)
             outs[b].inference_ms = wall * (j->total_samples ? (float)outs[b].len / (float)j->total_samples : 0.f);
     });
+}
+int32_t sb200_speak_batch_ids_configs(sb200_voice* v, const int64_t* ids, const size_t* offsets, size_t batch,
+                                      const sb200_synth_config* cfgs, sb200_audio* outs, sb200_error* err) {
+    return sb200_speak_batch_ids_durations(v, ids, offsets, batch, cfgs, nullptr, nullptr, outs, nullptr, err);
 }
 int32_t sb200_speak_batch_ids(sb200_voice* v, const int64_t* ids, const size_t* offsets, size_t batch,
                               sb200_audio* outs, sb200_error* err) {
@@ -253,6 +276,19 @@ int32_t sb200_job_set_configs(sb200_job* job, const sb200_synth_config* cfgs, sb
     return guarded(err, [&] {
         Job& j = *job->j;
         set_job_configs(j, cfgs ? cfgs_in(cfgs, j.B).data() : nullptr);
+    });
+}
+int32_t sb200_job_set_durations(sb200_job* job, const float* scale_packed, const int32_t* frames_packed, sb200_error* err) {
+    return guarded(err, [&] { set_job_durations(*job->j, scale_packed, frames_packed); });
+}
+int32_t sb200_job_id_frames(sb200_job* job, int32_t* out_packed, size_t capacity, sb200_error* err) {
+    return guarded(err, [&] {
+        Job& j = *job->j;
+        if (!out_packed) throw Error(19, "null destination");
+        const std::vector<int>& f = job_id_frames(j);
+        if (capacity < f.size())
+            throw Error(19, "capacity " + std::to_string(capacity) + " is smaller than the job's " + std::to_string(f.size()) + " ids");
+        std::copy(f.begin(), f.end(), out_packed);
     });
 }
 int32_t sb200_job_run(sb200_job* job, float* d_out, size_t cap, float* device_ms, sb200_error* err) {
@@ -341,14 +377,24 @@ int32_t sb200_decode_chunk(sb200_voice* v, const sb200_latent* z, int64_t lo, in
 }
 void sb200_latent_free(sb200_latent* z) { delete z; }
 
-int32_t sb200_encode_batch_ids_configs(sb200_voice* v, const int64_t* ids, const size_t* offsets, size_t batch,
-                                       const sb200_synth_config* cfgs, sb200_latent** outs, sb200_error* err) {
+int32_t sb200_encode_batch_ids_durations(sb200_voice* v, const int64_t* ids, const size_t* offsets, size_t batch,
+                                         const sb200_synth_config* cfgs, const float* scale_packed,
+                                         const int32_t* frames_packed, sb200_latent** outs, sb200_error* err) {
     return guarded(err, [&] {
         const std::vector<SynthConfig> c = cfgs ? cfgs_in(cfgs, batch) : std::vector<SynthConfig>();
         std::vector<Latent*> ls = encode_latents(v->v.get(), reinterpret_cast<const long long*>(ids), offsets, batch,
-                                                 cfgs ? c.data() : nullptr);
+                                                 cfgs ? c.data() : nullptr, scale_packed, frames_packed);
         for (size_t b = 0; b < batch; b++) outs[b] = new sb200_latent{ls[b], v->v};
     });
+}
+int32_t sb200_encode_batch_ids_configs(sb200_voice* v, const int64_t* ids, const size_t* offsets, size_t batch,
+                                       const sb200_synth_config* cfgs, sb200_latent** outs, sb200_error* err) {
+    return sb200_encode_batch_ids_durations(v, ids, offsets, batch, cfgs, nullptr, nullptr, outs, err);
+}
+int64_t sb200_latent_id_frames(const sb200_latent* z, int32_t* out, size_t capacity) {
+    const std::vector<int>& f = z->l->id_frames;
+    if (out && capacity >= f.size()) std::copy(f.begin(), f.end(), out);
+    return (int64_t)f.size();
 }
 
 namespace {

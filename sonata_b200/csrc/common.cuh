@@ -177,9 +177,11 @@ void launch_flow_pre(const float* z, int zcol, const float* w, const float* b, c
 // z[r][tcol] = RQS^-1(z[r][tcol]; params h29[r][0..3*bins-1))
 void launch_spline(const float* h29, int ldh, float* z, int tcol, int bins, float inv_sqrt_filter,
                    RowMap map, cudaStream_t st);
-// logw = (z[:,0]-m0)*exp(-logs0); w = exp(logw)*length_scale[b]; w_ceil; per-segment inclusive scan
+// logw = (z[:,0]-m0)*exp(-logs0); w = exp(logw)*length_scale[b]; w_ceil; per-segment inclusive scan.  Optional per-id
+// controls at the id level (null: none): w_ceil = ceil(w * dur_scale[r]), and dur_frames[r] >= 0 replaces w_ceil.
 void launch_durations(const float* z, float m0, float logs0, const float* length_scale, const SegInfo* segs, int nseg,
-                      float* logw, int* cum, int* y_len, cudaStream_t st);
+                      float* logw, int* cum, int* y_len, cudaStream_t st, const float* dur_scale = nullptr,
+                      const int* dur_frames = nullptr);
 struct FrameSeg { int off; int len; int xoff; int xlen; long long out_off; };
 // z_p rows: gather m_p/logs_p of the token whose cumulative duration covers the frame, add noise scaled by the noise_scale
 // of the frame's segment (ftile_seg)

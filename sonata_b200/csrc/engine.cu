@@ -192,6 +192,22 @@ void set_job_configs(Job& j, const SynthConfig* cfgs) {
     j.cfgs.assign(cfgs, cfgs + j.B);
 }
 
+void set_job_durations(Job& j, const float* scale, const int* frames) {
+    for (size_t b = 0; b < j.B; b++)
+        for (size_t i = j.offs[b]; i < j.offs[b + 1]; i++) {
+            auto fail = [&](const std::string& what) {
+                throw Error(19, "utterance " + std::to_string(b) + ", id " + std::to_string(i - j.offs[b]) + ": " + what);
+            };
+            if (scale && !(std::isfinite(scale[i]) && scale[i] >= 0.f))
+                fail("duration scale " + std::to_string(scale[i]) + " is not a finite value >= 0");
+            if (frames && frames[i] < -1)
+                fail("fixed duration " + std::to_string(frames[i]) + " is neither -1 (predicted) nor a frame count >= 0");
+        }
+    const size_t n = j.ids.size();
+    if (scale) j.dur_scale.assign(scale, scale + n); else j.dur_scale.clear();
+    if (frames) j.dur_frames.assign(frames, frames + n); else j.dur_frames.clear();
+}
+
 namespace {
 
 struct Runner {
@@ -302,6 +318,7 @@ struct IdBufs {
     float *xa, *xb, *qkv, *att, *ffn, *stats, *d0, *t1, *t2, *g, *h29, *zz, *logw;
     float *att_s, *att_vt, *att_orel;          // tensor-core attention: scores of every head, V^T, relative-value term
     float *epsw, *cond;                        // cond: [slot][cond_rows]
+    float *dscale, *dscale_h; int *dframes, *dframes_h;   // per-id duration controls (only when the job has them)
     float *qkv0, *att0, *p0, *vt0;             // debug: layer 0's attention operands and result
     std::vector<std::array<float*, 4>> dpf;    // debug: each duration flow's input, DDSConv output, spline parameters, output
 
@@ -330,6 +347,9 @@ struct IdBufs {
         for (const SynthConfig& c : j.cfgs) any_noise_w |= c.noise_w != 0.f;
         epsw = any_noise_w ? rows(2) : nullptr;
         cond = multi ? dev.get<float>(nslots * v.cond_rows) : nullptr;
+        const bool scaled = !j.dur_scale.empty(), fixed = !j.dur_frames.empty();
+        dscale = scaled ? dev.get<float>(RX) : nullptr; dscale_h = scaled ? pin.get<float>(RX) : nullptr;
+        dframes = fixed ? dev.get<int>(RX) : nullptr; dframes_h = fixed ? pin.get<int>(RX) : nullptr;
         qkv0 = att0 = p0 = vt0 = nullptr;
         dpf.clear();
         if (j.debug) {
@@ -558,14 +578,45 @@ Level upload_frames(const Job& j, const FrameTables& t, cudaStream_t st) {
     return L;
 }
 
+// Starts the copy of the batch's cum rows (up to the end of the last utterance: one copy, gap rows included) into the
+// context's page-locked staging, on the job's stream; the caller synchronises.  The pass is over, so the staging of its
+// tables is free.
+const int* stage_cum(Job& j) {
+    const SegInfo& last = j.xsegs[j.B - 1];
+    const size_t n = (size_t)last.off + (size_t)last.len;
+    Context& C = *j.ctx;
+    C.pin.reserve(n * sizeof(int));
+    int* h = C.pin.get<int>(n);
+    SB_CUDA(cudaMemcpyAsync(h, j.d_cum, n * sizeof(int), cudaMemcpyDeviceToHost, C.stream));
+    return h;
+}
+
+// Frames per id of utterance b, from the staged cum rows.
+void cum_to_frames(const Job& j, const int* cum, size_t b, int* out) {
+    const int* c = cum + j.xsegs[b].off;
+    int prev = 0;
+    for (int i = 0; i < j.xsegs[b].len; i++) { out[i] = c[i] - prev; prev = c[i]; }
+}
+
 }  // namespace
+
+const std::vector<int>& job_id_frames(Job& j) {
+    if (!j.ran) throw Error(19, "job has not run: no per-id frame counts yet");
+    if (!j.id_frames.empty()) return j.id_frames;
+    SB_CUDA(cudaSetDevice(j.v->device));
+    const int* h = stage_cum(j);
+    SB_CUDA(cudaStreamSynchronize(j.ctx->stream));
+    j.id_frames.resize(j.ids.size());
+    for (size_t b = 0; b < j.B; b++) cum_to_frames(j, h, b, j.id_frames.data() + j.offs[b]);
+    return j.id_frames;
+}
 
 void Job::run(float* d_out, size_t d_out_cap) {
     Voice& V = *v; Context& C = *ctx; const Arch& a = V.a;
     SB_CUDA(cudaSetDevice(V.device));
     cudaStream_t st = C.stream;
     const int H = a.hidden, I = a.inter, F = a.filter;
-    regions.clear(); dbg.clear(); dbg_level.clear();
+    regions.clear(); dbg.clear(); dbg_level.clear(); id_frames.clear();
     C.events_used = 0;
     if (!C.ev_begin) { SB_CUDA(cudaEventCreate(&C.ev_begin)); SB_CUDA(cudaEventCreate(&C.ev_end)); }
 
@@ -615,6 +666,17 @@ void Job::run(float* d_out, size_t d_out_cap) {
         std::copy(slot_sid.begin(), slot_sid.end(), x.sid_h);
         h2d(x.xslot, x.xslot_h, (size_t)nxg * 4, st);
         h2d(x.sid, x.sid_h, slot_sid.size() * 4, st);
+    }
+    if (x.dscale || x.dframes) {
+        if (x.dscale) std::fill(x.dscale_h, x.dscale_h + RX, 1.f);
+        if (x.dframes) std::fill(x.dframes_h, x.dframes_h + RX, -1);
+        for (size_t b = 0; b < B; b++) {
+            const int r0 = xsegs[b].off;
+            if (x.dscale) std::copy(dur_scale.begin() + offs[b], dur_scale.begin() + offs[b + 1], x.dscale_h + r0);
+            if (x.dframes) std::copy(dur_frames.begin() + offs[b], dur_frames.begin() + offs[b + 1], x.dframes_h + r0);
+        }
+        if (x.dscale) h2d(x.dscale, x.dscale_h, (size_t)RX * 4, st);
+        if (x.dframes) h2d(x.dframes, x.dframes_h, (size_t)RX * 4, st);
     }
     if (tc_att) {
         memcpy(x.tiles_h, tiles_s.data(), tiles_s.size() * sizeof(TfTile));
@@ -729,7 +791,8 @@ void Job::run(float* d_out, size_t d_out_cap) {
         R.count(0, 4.0 * LX.valid_rows * 34);
         if (debug) d2d(x.dpf[s][3], x.zz, (size_t)RX * 2, st);
     }
-    launch_durations(x.zz, V.ea_m0, V.ea_logs0, x.scales + B, x.xsegs, (int)B, x.logw, x.cum, x.ylen, st);
+    launch_durations(x.zz, V.ea_m0, V.ea_logs0, x.scales + B, x.xsegs, (int)B, x.logw, x.cum, x.ylen, st, x.dscale,
+                     x.dframes);
     R.end();
 
     // ---------------- host learns the frame counts (the graph's data-dependent shape) ----------------
@@ -816,9 +879,11 @@ void Job::run(float* d_out, size_t d_out_cap) {
 }
 
 // ====================================================================== streaming halves
-std::vector<Latent*> encode_latents(Voice* v, const long long* ids, const size_t* offs, size_t B, const SynthConfig* cfgs) {
+std::vector<Latent*> encode_latents(Voice* v, const long long* ids, const size_t* offs, size_t B, const SynthConfig* cfgs,
+                                    const float* scale, const int* frames) {
     std::unique_ptr<Job> j(create_job(v, ids, offs, B, nullptr, nullptr, nullptr, false));
     if (cfgs) set_job_configs(*j, cfgs);
+    set_job_durations(*j, scale, frames);
     j->encode_only = true;
     j->run(nullptr, 0);
     const size_t I = (size_t)v->a.inter;
@@ -839,7 +904,12 @@ std::vector<Latent*> encode_latents(Voice* v, const long long* ids, const size_t
                                 cudaMemcpyDeviceToDevice, j->ctx->stream));
         row += (size_t)L.frames;
     }
+    const int* cum = stage_cum(*j);
     SB_CUDA(cudaStreamSynchronize(j->ctx->stream));
+    for (size_t b = 0; b < B; b++) {
+        ls[b]->id_frames.resize(j->offs[b + 1] - j->offs[b]);
+        cum_to_frames(*j, cum, b, ls[b]->id_frames.data());
+    }
     std::vector<Latent*> out(B);
     for (size_t b = 0; b < B; b++) out[b] = ls[b].release();
     return out;

@@ -112,7 +112,10 @@ struct Voice {
     ~Voice();
     Context* acquire();
     void release(Context* c);
-    std::vector<long long> phonemes_to_ids(const char* utf8) const;
+    // Piper's [bos, (id, pad)*, eos] ids of a phoneme string.  src_char (optional) receives, per id, the index in
+    // Unicode characters of the input character it came from (a pad belongs to the character before it; bos and eos
+    // get -1).
+    std::vector<long long> phonemes_to_ids(const char* utf8, std::vector<long long>* src_char = nullptr) const;
 };
 
 Voice* load_voice(const std::string& config_path, int device);
@@ -170,6 +173,9 @@ struct Job {
     unsigned long long noise_call = 0;
     // host copies of inputs
     std::vector<long long> ids; std::vector<size_t> offs;
+    // per-id duration controls, packed like ids (empty: none; set_job_durations)
+    std::vector<float> dur_scale; std::vector<int> dur_frames;
+    std::vector<int> id_frames;       // frames per id of the last run, packed like ids: filled by job_id_frames
     std::vector<std::vector<float>> eps_w, eps_z; std::vector<size_t> eps_z_frames;
     // X layout
     int RX = 0; std::vector<SegInfo> xsegs; int max_tx = 0;
@@ -204,6 +210,14 @@ void check_config(const Voice& v, const SynthConfig& c, const std::string& who);
 // Per-utterance configs of the job's next run: cfgs[0 .. B), or the voice's fallback config for every utterance when
 // cfgs is null.  Every entry is checked first; on an error the job keeps its configs.
 void set_job_configs(Job& j, const SynthConfig* cfgs);
+// Per-id duration controls of the job's next run, each packed like the job's ids (one entry per id) or null: scales
+// (finite, >= 0) multiply the predicted duration before its ceil, frames (-1 = predicted, or >= 0) replace it.  Every
+// entry is checked first; an error names the utterance and the id, and leaves the job's controls as they were.  Null
+// and null restores the default (no controls, the kernel reads none).
+void set_job_durations(Job& j, const float* scale, const int* frames);
+// Frames per id of the job's last run, packed like its ids: one device->host copy of the batch's cum rows through the
+// context's page-locked staging, differenced on the host.  Cached until the next run.
+const std::vector<int>& job_id_frames(Job& j);
 
 struct Latent {
     Voice* v = nullptr;
@@ -211,10 +225,13 @@ struct Latent {
     std::shared_ptr<float> mem;   // device allocation shared by the latents of one encoder pass, freed with the last
     float* z = nullptr;   // device [frames][inter], inside `mem`
     long long frames = 0;
+    std::vector<int> id_frames;   // frames per id of the encoder pass (the reference's p_duration)
 };
-// One encoder pass over B utterances (cfgs: one per utterance, or null for the voice's fallback config) -> B latents
-// sharing one device allocation.  The caller owns the returned pointers.
-std::vector<Latent*> encode_latents(Voice* v, const long long* ids, const size_t* offs, size_t B, const SynthConfig* cfgs);
+// One encoder pass over B utterances (cfgs: one per utterance, or null for the voice's fallback config; scale / frames:
+// per-id duration controls as for set_job_durations, or null) -> B latents sharing one device allocation.  The caller
+// owns the returned pointers.
+std::vector<Latent*> encode_latents(Voice* v, const long long* ids, const size_t* offs, size_t B, const SynthConfig* cfgs,
+                                    const float* scale = nullptr, const int* frames = nullptr);
 Latent* encode_latent(Voice* v, const long long* ids, size_t n);
 // One frame-level decoder pass over n chunks z[k][lo[k] : hi[k]) of latents of `v`; out[k] gets chunk k's waveform.
 // Chunk k equals the same chunk decoded alone, bit for bit.  ms: the pass's device time.

@@ -483,11 +483,18 @@ __global__ void scale_copy2_kernel(const float* __restrict__ eps, const float* _
 // oracle: sdp_reverse() tail (ElementwiseAffine^-1) + durations()
 // The scan runs in 64 bits and cum / y_len saturate at INT_MAX: a duration past 2^31 - 1 frames (or a NaN / inf one)
 // must reach the host as an overlong frame count, which it rejects, not wrap into a plausible one.
+// Optional per-id controls, at the id level like logw (null: none):
+//   dur_scale  : the predicted count is ceil((exp(logw) * length_scale) * s); the product is rounded in that order, so
+//                s = 1 gives the bits of a call without scales
+//   dur_frames : a value >= 0 replaces the count (no ceil involved); -1 keeps the predicted one
+// logw is written for every id either way.
 __device__ __forceinline__ int sat_int(long long v) { return (int)min(v, (long long)INT_MAX); }
 
 __global__ void __launch_bounds__(256) durations_kernel(const float* __restrict__ z, float m0, float logs0,
                                                         const float* __restrict__ length_scales,
                                                         const SegInfo* __restrict__ segs,
+                                                        const float* __restrict__ dur_scale,
+                                                        const int* __restrict__ dur_frames,
                                                         float* __restrict__ logw, int* __restrict__ cum,
                                                         int* __restrict__ y_len) {
     pdl_trigger(); pdl_wait();
@@ -503,10 +510,17 @@ __global__ void __launch_bounds__(256) durations_kernel(const float* __restrict_
         const int i = base + tid;
         long long w = 0;
         if (i < sg.len) {
-            const float lw = (z[2 * (sg.off + i)] - m0) * einv;
-            logw[sg.off + i] = lw;
-            const float wc = ceilf(expf(lw) * length_scale);
+            const int row = sg.off + i;
+            const float lw = (z[2 * row] - m0) * einv;
+            logw[row] = lw;
+            float wf = expf(lw) * length_scale;
+            if (dur_scale) wf = wf * dur_scale[row];
+            const float wc = ceilf(wf);
             w = wc < 2147483648.f ? (long long)(int)wc : (long long)INT_MAX;     // NaN and inf saturate too
+            if (dur_frames) {
+                const int f = dur_frames[row];
+                if (f >= 0) w = f;
+            }
         }
         long long s = w;
 #pragma unroll
@@ -858,8 +872,9 @@ void launch_scale_copy2(const float* eps, const float* s, const int* seg_of_gran
 }
 
 void launch_durations(const float* z, float m0, float logs0, const float* length_scale, const SegInfo* segs, int nseg,
-                      float* logw, int* cum, int* y_len, cudaStream_t st) {
-    launch_pdl(durations_kernel, dim3(nseg), dim3(256), 0, st, z, m0, logs0, length_scale, segs, logw, cum, y_len);
+                      float* logw, int* cum, int* y_len, cudaStream_t st, const float* dur_scale, const int* dur_frames) {
+    launch_pdl(durations_kernel, dim3(nseg), dim3(256), 0, st, z, m0, logs0, length_scale, segs, dur_scale, dur_frames,
+               logw, cum, y_len);
     g_launch_count++;
 }
 

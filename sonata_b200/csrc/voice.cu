@@ -215,7 +215,7 @@ ConvW debug_make_conv(Voice& v, const float* w, const float* bias, int cout, int
 }
 
 // VitsModelCommons::phonemes_to_input_ids + get_meta_ids (piper/src/lib.rs:173-179, 232-250)
-std::vector<long long> Voice::phonemes_to_ids(const char* utf8) const {
+std::vector<long long> Voice::phonemes_to_ids(const char* utf8, std::vector<long long>* src_char) const {
     auto meta = [&](char ch) -> long long {
         auto it = phoneme_first_id.find((uint32_t)ch);
         if (it == phoneme_first_id.end())
@@ -225,8 +225,9 @@ std::vector<long long> Voice::phonemes_to_ids(const char* utf8) const {
     const long long pad = meta('_'), bos = meta('^'), eos = meta('$');
     std::vector<long long> ids;
     ids.push_back(bos);
+    if (src_char) src_char->assign(1, -1);
     const unsigned char* s = reinterpret_cast<const unsigned char*>(utf8);
-    while (*s) {
+    for (long long ch = 0; *s; ch++) {
         uint32_t cp; int n;
         if (*s < 0x80) { cp = *s; n = 1; }
         else if ((*s >> 5) == 6) { cp = *s & 0x1F; n = 2; }
@@ -242,9 +243,11 @@ std::vector<long long> Voice::phonemes_to_ids(const char* utf8) const {
         if (it != phoneme_first_id.end()) {   // unknown phonemes are dropped silently (:243)
             ids.push_back(it->second);
             ids.push_back(pad);
+            if (src_char) { src_char->push_back(ch); src_char->push_back(ch); }
         }
     }
     ids.push_back(eos);
+    if (src_char) src_char->push_back(-1);
     return ids;
 }
 

@@ -10,7 +10,7 @@ import numpy as np
 
 from . import _native as N
 from .core import Audio
-from .piper import _check, _config_array, _take_audio
+from .piper import _check, _config_array, _duration_arrays, _ptr, _take_audio
 
 
 class SynthesisJob:
@@ -21,6 +21,7 @@ class SynthesisJob:
         self._lib = model._lib
         n = len(batches)
         self.batch = n
+        self._lens = [len(b) for b in batches]
         _config_array(configs, n)             # argument errors before the job exists
         packed = np.ascontiguousarray(np.concatenate([np.asarray(b, dtype=np.int64) for b in batches]))
         offs = np.zeros(n + 1, dtype=np.uint64)
@@ -60,6 +61,23 @@ class SynthesisJob:
         length or an unknown speaker raises OperationError and leaves the job's configs as they were."""
         err = N.sb200_error()
         _check(self._lib.sb200_job_set_configs(self._h, _config_array(configs, self.batch), C.byref(err)), err)
+
+    def set_durations(self, scales: Optional[Sequence] = None, frames: Optional[Sequence] = None) -> None:
+        """Per-id duration controls for the next run (see VitsModel.infer_batch_with_durations): scales[b] / frames[b]
+        hold one value per id of utterance b, or None.  None and None restores the default.  A bad entry raises
+        OperationError naming the utterance and the id, and leaves the job's controls as they were."""
+        sc, fr = _duration_arrays(self._lens, scales, frames)
+        err = N.sb200_error()
+        _check(self._lib.sb200_job_set_durations(self._h, _ptr(sc, C.c_float), _ptr(fr, C.c_int32), C.byref(err)), err)
+
+    def id_frames(self) -> List[np.ndarray]:
+        """Frames per id of the last run, one int32 array per utterance (one device->host copy for the batch)."""
+        total = int(sum(self._lens))
+        out = np.zeros(total, np.int32)
+        err = N.sb200_error()
+        _check(self._lib.sb200_job_id_frames(self._h, _ptr(out, C.c_int32), total, C.byref(err)), err)
+        offs = np.concatenate([[0], np.cumsum(self._lens)]).astype(int)
+        return [out[offs[b]:offs[b + 1]].copy() for b in range(self.batch)]
 
     def run(self, d_out_ptr: int = 0, capacity: int = 0) -> float:
         ms, err = C.c_float(), N.sb200_error()

@@ -9,13 +9,16 @@ in the reference too.
 from __future__ import annotations
 
 import ctypes as C
+import math
+import numbers
 from dataclasses import dataclass
-from typing import Iterator, List, Optional, Sequence
+from typing import Iterator, List, Optional, Sequence, Tuple
 
 import numpy as np
 
 from . import _native as N
-from .core import Audio, AudioInfo, AudioSamples, OperationError, Phonemes, PhonemizationError, SonataError
+from .core import (Audio, AudioInfo, AudioSamples, OperationError, PhonemeAlignment, Phonemes, PhonemizationError,
+                   SonataError)
 
 MIN_CHUNK_SIZE = 44      # piper/src/lib.rs:18
 MAX_CHUNK_SIZE = 1024    # piper/src/lib.rs:19
@@ -45,6 +48,106 @@ def _config_array(configs: Optional[Sequence["PiperSynthesisConfig"]], n: int):
         arr[i] = N.sb200_synth_config(c.speaker or 0, 0 if c.speaker is None else 1, c.noise_scale, c.length_scale,
                                       c.noise_w)
     return arr
+
+
+def _per_utterance(values, n: int, what: str) -> list:
+    if isinstance(values, (str, bytes)) or not hasattr(values, "__len__"):
+        raise OperationError(f"Invalid {what}: expected one entry (or None) per utterance")
+    values = list(values)
+    if len(values) != n:
+        raise OperationError(f"Invalid {what}: {len(values)} entries for {n} utterances")
+    return values
+
+
+def _scale_value(x, b: int, i: int, unit: str = "id") -> float:
+    if isinstance(x, bool) or not isinstance(x, numbers.Real):
+        raise OperationError(f"utterance {b}, {unit} {i}: duration scale {x!r} is not a number")
+    x = float(x)
+    if not (math.isfinite(x) and x >= 0.0):
+        raise OperationError(f"utterance {b}, {unit} {i}: duration scale {x} is not a finite value >= 0")
+    return x
+
+
+def _numeric(v, kinds):
+    """v as a 1-D numpy array when its dtype kind is one of `kinds` (the vectorised checks), else None."""
+    a = v if isinstance(v, np.ndarray) else np.asarray(v) if not isinstance(v, (str, bytes)) else None
+    return a.reshape(-1) if a is not None and a.dtype.kind in kinds and a.ndim <= 1 else None
+
+
+def _duration_arrays(lens: Sequence[int], duration_scales=None, durations=None):
+    """The packed C images of per-id duration controls, checked as the library checks them: (scales f32, frames i32),
+    each None when not given.  duration_scales[b] / durations[b] hold one value per id of utterance b, or None for an
+    utterance without that control (scale 1.0, frames -1: its plain result).  Numeric arrays are checked in one
+    vectorised pass; anything else element by element, which also names the first bad element."""
+    n = len(lens)
+    total = int(sum(lens))
+    scales = frames = None
+    if duration_scales is not None:
+        scales = np.ones(total, np.float32)
+        pos = 0
+        for b, v in enumerate(_per_utterance(duration_scales, n, "duration scales")):
+            if v is not None:
+                a = _numeric(v, "fiu")
+                if a is None:
+                    v = list(v)
+                    a = np.array([_scale_value(x, b, i) for i, x in enumerate(v)] if len(v) == lens[b] else v)
+                if a.size != lens[b]:
+                    raise OperationError(f"utterance {b}: {a.size} duration scales for {lens[b]} ids")
+                f = a.astype(np.float32)
+                bad = np.nonzero(~(np.isfinite(f) & (f >= 0)))[0]
+                if bad.size:
+                    _scale_value(float(f[bad[0]]), b, int(bad[0]))
+                scales[pos:pos + lens[b]] = f
+            pos += lens[b]
+    if durations is not None:
+        frames = np.full(total, -1, np.int32)
+        pos = 0
+        for b, v in enumerate(_per_utterance(durations, n, "durations")):
+            if v is not None:
+                a = _numeric(v, "iu")
+                if a is None:
+                    v = list(v)
+                    if len(v) == lens[b]:
+                        for i, x in enumerate(v):
+                            if isinstance(x, bool) or not isinstance(x, numbers.Integral):
+                                raise OperationError(f"utterance {b}, id {i}: fixed duration {x!r} is not an integer")
+                    a = np.array([int(x) for x in v], dtype=object)
+                if a.size != lens[b]:
+                    raise OperationError(f"utterance {b}: {a.size} durations for {lens[b]} ids")
+                bad = np.nonzero((a < -1) | (a > 2**31 - 1))[0]
+                if bad.size:
+                    raise OperationError(f"utterance {b}, id {int(bad[0])}: fixed duration {int(a[bad[0]])} is neither "
+                                         "-1 (predicted) nor a frame count >= 0")
+                frames[pos:pos + lens[b]] = a.astype(np.int64)
+            pos += lens[b]
+    return scales, frames
+
+
+def _ptr(a, ctype):
+    return None if a is None else a.ctypes.data_as(C.POINTER(ctype))
+
+
+def _alignment(phonemes: str, src_char: Sequence[int], frames: Sequence[int], n_samples: int) -> List[PhonemeAlignment]:
+    """Groups per-id frame counts by the character each id came from: bos (`^`), one entry per kept character (its id
+    and its pad) and eos (`$`), contiguous from sample 0.  An utterance whose ids all got 0 frames is still one frame
+    long; that frame (after every id) goes to the last entry, so the entries always end at n_samples."""
+    total = int(sum(int(f) for f in frames))
+    hop = n_samples // max(total, 1)
+    out: List[PhonemeAlignment] = []
+    start, i = 0, 0
+    while i < len(frames):
+        src = int(src_char[i])
+        j, f = i, 0
+        while j < len(frames) and int(src_char[j]) == src and not (src < 0 and j > i):
+            f += int(frames[j])
+            j += 1
+        ph = phonemes[src] if src >= 0 else ("^" if i == 0 else "$")
+        out.append(PhonemeAlignment(ph, start, f * hop))
+        start += f * hop
+        i = j
+    if out and start != n_samples:
+        out[-1].num_samples += n_samples - start
+    return out
 
 
 def _check(rc: int, err: N.sb200_error):
@@ -174,6 +277,19 @@ class _VitsCommons:
         self._lib.sb200_ids_free(ids)
         return out
 
+    def phonemes_to_input_ids_map(self, phonemes: str) -> Tuple[List[int], List[int]]:
+        """phonemes_to_input_ids plus, per id, the index (in characters of `phonemes`) of the character it came from: a
+        pad belongs to the character before it, bos and eos get -1, dropped characters own no id."""
+        ids, src = C.POINTER(C.c_int64)(), C.POINTER(C.c_int64)()
+        n = C.c_size_t()
+        err = N.sb200_error()
+        _check(self._lib.sb200_phonemes_to_input_ids_map(self._h, phonemes.encode("utf-8"), C.byref(ids), C.byref(src),
+                                                         C.byref(n), C.byref(err)), err)
+        out = ([int(ids[i]) for i in range(n.value)], [int(src[i]) for i in range(n.value)])
+        self._lib.sb200_ids_free(ids)
+        self._lib.sb200_ids_free(src)
+        return out
+
     def speak_one_sentence(self, phonemes: str) -> Audio:
         a, err = N.sb200_audio(), N.sb200_error()
         _check(self._lib.sb200_speak_one_sentence(self._h, phonemes.encode("utf-8"), C.byref(a), C.byref(err)), err)
@@ -219,6 +335,65 @@ class _VitsCommons:
                                                        offs.ctypes.data_as(C.POINTER(C.c_size_t)), n, cfgs, outs,
                                                        C.byref(err)), err)
         return [_take_audio(outs[i]) for i in range(n)]
+
+    def infer_batch_with_durations(self, batches: Sequence[Sequence[int]],
+                                   configs: Optional[Sequence[PiperSynthesisConfig]] = None,
+                                   duration_scales: Optional[Sequence] = None,
+                                   durations: Optional[Sequence] = None) -> List[Tuple[Audio, np.ndarray]]:
+        """infer_batch_with_values with per-id duration control, returning (audio, frames per id) per utterance.
+
+        duration_scales[b]: one scale (finite, >= 0) per id of utterance b, applied before the duration's ceil, so 1.0
+        gives the plain result bit for bit; durations[b]: one frame count per id, -1 for "predicted" or >= 0 to fix it.
+        Either list, or any of its entries, may be None.  The frame counts times 256 are each id's samples; an
+        utterance whose ids all got 0 frames is still one frame long."""
+        n = len(batches)
+        cfgs = _config_array(configs, n)
+        lens = [len(b) for b in batches]
+        scales, frames = _duration_arrays(lens, duration_scales, durations)
+        if n == 0:
+            return []
+        if any(x == 0 for x in lens):
+            raise OperationError("Failed to run model inference. Error: empty input sequence")
+        packed = np.ascontiguousarray(np.concatenate([np.asarray(b, dtype=np.int64) for b in batches]))
+        offs = np.zeros(n + 1, dtype=np.uint64)
+        offs[1:] = np.cumsum(lens)
+        outs = (N.sb200_audio * n)()
+        id_frames = np.zeros(int(offs[-1]), np.int32)
+        err = N.sb200_error()
+        _check(self._lib.sb200_speak_batch_ids_durations(
+            self._h, packed.ctypes.data_as(C.POINTER(C.c_int64)), offs.ctypes.data_as(C.POINTER(C.c_size_t)), n, cfgs,
+            _ptr(scales, C.c_float), _ptr(frames, C.c_int32), outs, _ptr(id_frames, C.c_int32), C.byref(err)), err)
+        return [(_take_audio(outs[b]), id_frames[int(offs[b]):int(offs[b + 1])].copy()) for b in range(n)]
+
+    def speak_batch_with_alignment(self, phoneme_batches: Sequence[str],
+                                   configs: Optional[Sequence[PiperSynthesisConfig]] = None,
+                                   duration_scales: Optional[Sequence] = None) -> List[Tuple[Audio, List[PhonemeAlignment]]]:
+        """speak_batch that also says when each phoneme is spoken: per utterance (audio, alignment), the alignment
+        holding one entry for bos (`^`), one per kept phoneme character (its id and its trailing pad) and one for eos
+        (`$`), contiguous from sample 0 to len(audio).
+
+        duration_scales[b] (or None): one scale per character of phoneme_batches[b], applied to that character's id and
+        pad; characters the voice drops have no entry and their scales are ignored."""
+        n = len(phoneme_batches)
+        _config_array(configs, n)
+        per_char = None if duration_scales is None else _per_utterance(duration_scales, n, "duration scales")
+        maps = [self.phonemes_to_input_ids_map(p) for p in phoneme_batches]
+        id_scales = None
+        if per_char is not None:
+            id_scales = []
+            for b, (ph, (ids, src)) in enumerate(zip(phoneme_batches, maps)):
+                v = per_char[b]
+                if v is None:
+                    id_scales.append(None)
+                    continue
+                v = list(v) if not isinstance(v, np.ndarray) else v.reshape(-1).tolist()
+                if len(v) != len(ph):
+                    raise OperationError(f"utterance {b}: {len(v)} duration scales for {len(ph)} characters")
+                kept = {c: _scale_value(v[c], b, c, "character") for c in sorted(set(src)) if c >= 0}
+                id_scales.append([1.0 if c < 0 else kept[c] for c in src])
+        res = self.infer_batch_with_durations([m[0] for m in maps], configs, id_scales)
+        return [(audio, _alignment(ph, src, frames, len(audio)))
+                for ph, (_, src), (audio, frames) in zip(phoneme_batches, maps, res)]
 
     def _cfg(self, fn) -> PiperSynthesisConfig:
         c, err = N.sb200_synth_config(), N.sb200_error()
@@ -277,6 +452,10 @@ class EncoderOutputs:
     def __init__(self, model: "_VitsCommons", handle: C.c_void_p):
         self._m, self._h = model, handle
         self.num_frames = int(model._lib.sb200_latent_frames(handle))
+        # frames per id of the encoder pass (the reference's optional `p_duration` output)
+        n = int(model._lib.sb200_latent_id_frames(handle, None, 0))
+        self.p_duration = np.zeros(n, np.int32)
+        model._lib.sb200_latent_id_frames(handle, _ptr(self.p_duration, C.c_int32), n)
 
     def infer_decoder(self, lo: int = 0, hi: Optional[int] = None) -> AudioSamples:
         hi = self.num_frames if hi is None else hi
@@ -328,12 +507,16 @@ class VitsStreamingModel(_VitsCommons):
         return EncoderOutputs(self, h)
 
     def infer_encoder_batch(self, batches: Sequence[Sequence[int]],
-                            configs: Optional[Sequence[PiperSynthesisConfig]] = None) -> List[EncoderOutputs]:
+                            configs: Optional[Sequence[PiperSynthesisConfig]] = None,
+                            duration_scales: Optional[Sequence] = None,
+                            durations: Optional[Sequence] = None) -> List[EncoderOutputs]:
         """infer_encoder over many utterances in one encoder pass.  `configs`: one PiperSynthesisConfig per utterance,
         or None for the fallback config; each latent equals infer_encoder alone with its config as the fallback,
-        except for the on-device noise, whose draws depend on the batch position."""
+        except for the on-device noise, whose draws depend on the batch position.  `duration_scales` / `durations`:
+        per-id duration controls as for infer_batch_with_durations; each output's `p_duration` holds its frames per id."""
         n = len(batches)
         cfgs = _config_array(configs, n)
+        scales, frames = _duration_arrays([len(b) for b in batches], duration_scales, durations)
         if any(len(b) == 0 for b in batches):
             raise OperationError("Failed to run model inference. Error: empty input sequence")
         if n == 0:
@@ -343,9 +526,10 @@ class VitsStreamingModel(_VitsCommons):
         offs[1:] = np.cumsum([len(b) for b in batches])
         outs = (C.c_void_p * n)()
         err = N.sb200_error()
-        _check(self._lib.sb200_encode_batch_ids_configs(self._h, packed.ctypes.data_as(C.POINTER(C.c_int64)),
-                                                        offs.ctypes.data_as(C.POINTER(C.c_size_t)), n, cfgs, outs,
-                                                        C.byref(err)), err)
+        _check(self._lib.sb200_encode_batch_ids_durations(self._h, packed.ctypes.data_as(C.POINTER(C.c_int64)),
+                                                          offs.ctypes.data_as(C.POINTER(C.c_size_t)), n, cfgs,
+                                                          _ptr(scales, C.c_float), _ptr(frames, C.c_int32), outs,
+                                                          C.byref(err)), err)
         return [EncoderOutputs(self, C.c_void_p(outs[i])) for i in range(n)]
 
     def infer_decoder_batch(self, chunks: Sequence[tuple], pcm16: bool = False, fade: int = 0,
