@@ -262,10 +262,14 @@ typedef struct sb200_region_stat {
 int32_t sb200_job_profile(const sb200_job* job, sb200_region_stat* out, int32_t cap);
 /* Test hook: the launch configuration the planner of backend 1 (wgmma bf16x2 conv) / 2 (wgmma 3xTF32 conv) would choose
  * for one convolution of `rows` output rows -- nothing is allocated or launched, so it also works without a GPU.
- * out16, backend 1: {nt, image rows, m-tiles, n-tiles, ring stages, smem bytes, window rows, 0...}; backend 2: {nth, image
- * rows, m-tiles, n-tiles, ring stages, chunk K-blocks, smem bytes, window rows, 0...}.  Returns 0, or 19 if unsupported. */
+ * out16, backend 1: {nt, image rows, m-tiles, n-tiles, ring stages, smem bytes, window rows, grid CTAs, weights resident
+ * (0/1), CTAs per SM, 0...}; backend 2: {nth, image rows, m-tiles, n-tiles, ring stages, chunk K-blocks, smem bytes, window
+ * rows, 0...}.  Returns 0, or 19 if unsupported. */
 int32_t sb200_debug_plan(int32_t backend, int64_t rows, int32_t cin, int32_t cout, int32_t k, int32_t dil, int32_t act,
                          int32_t has_res, int32_t accumulate, int32_t* out16);
+/* Test hook: at most `cap` CTAs per launch of backend 1's persistent conv kernel from now on in this process (0: no cap;
+ * the launch still takes one CTA per column tile).  Results do not depend on it.  Returns the previous cap. */
+int32_t sb200_debug_conv_grid_cap(int32_t cap);
 /* one convolution on caller data through backend 0 (fp32 CUDA cores), 1 (wgmma bf16x2) or 2 (wgmma 3xTF32), for kernel
  * unit tests: y[rows][cout] (=|+=) scale * (act(bias + conv_k,dil(lrelu_slope(x))) + res); w is [cout][cin][k];
  * act 0 none, 1 relu, 2 tanh*sigmoid gate (y is [rows][cout/2]); rows >= valid_rows are masked. */

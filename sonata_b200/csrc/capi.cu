@@ -514,6 +514,12 @@ int32_t sb200_debug_plan(int32_t backend, int64_t rows, int32_t cin, int32_t cou
     return ok ? 0 : 19;
 }
 
+int32_t sb200_debug_conv_grid_cap(int32_t cap) {
+    const int32_t old = g_conv_tc_grid_cap;
+    g_conv_tc_grid_cap = cap > 0 ? cap : 0;
+    return old;
+}
+
 int32_t sb200_debug_conv_ex(int32_t device, int32_t backend, const float* x, int32_t rows, int32_t cin, const float* w,
                             const float* bias, int32_t cout, int32_t k, int32_t dil, float in_slope, int32_t act,
                             const float* res, float scale, const int32_t* seg_end, int32_t gran, int32_t seg_mul,

@@ -140,6 +140,7 @@ bool conv_tc_supported(const ConvArgs& a);
 bool conv_tc_plan_info(const ConvArgs& a, int* out16);     // planning only, see sb200_debug_plan
 void launch_conv_tc(const ConvArgs& a, cudaStream_t st);
 bool try_launch_conv_tc(const ConvArgs& a, cudaStream_t st);
+extern int g_conv_tc_grid_cap;     // at most this many CTAs per conv_tc launch (0: no cap); see sb200_debug_conv_grid_cap
 size_t conv_tc_weight_floats(int cin, int cout, int ntaps, int nt);
 void conv_tc_build_weights(const float* wt, int ldw, int cin, int cout, int ntaps, int nt, float* out);
 bool conv_tf_supported(const ConvArgs& a);

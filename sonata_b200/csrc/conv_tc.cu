@@ -9,23 +9,39 @@
 // End-to-end waveform error 2e-5 / 3.5e-5 (oracle emulation) -- the same as a 3xTF32 split at half the MMAs
 // (K = 16 per bf16 MMA against 8 per tf32 MMA).
 //
-// One CTA = one 128-row x NT-column tile, two warpgroups (rows 0-63 / 64-127), a two-stage ring over K-blocks:
+// Persistent CTAs: the grid is as many CTAs as can be resident at once, and each walks a static list of 128-row x
+// NT-column tiles.  A CTA keeps one n-tile (blockIdx % ntiles_n) and takes the m-tiles blockIdx / ntiles_n + i * (grid /
+// ntiles_n): the CTAs of one m-tile run side by side, so the re-reads of its window come from L2.  Two warpgroups
+// (rows 0-63 / 64-127) and a two-stage ring over the CTA's flat sequence of (tile, K-block) steps, so the next tile's
+// first window loads while this tile runs its MMAs and its epilogue:
 //   * activations: the raw fp32 (128 + span)-row WINDOW of a K-block (32 channels = one 128-byte row) arrives by
 //     cp.async (rows outside the array zero-filled); all threads then apply the leaky-ReLU prologue, split hi/lo and
 //     rewrite each row IN PLACE as [hi: 32 ch bf16 | lo: 32 ch bf16] in the K-major SWIZZLE_128B layout (row r at
 //     r*128 B, 16-B chunk c at (c ^ (r & 7))).  A tap is the same window read from a row offset: the A operand
 //     comes from registers (wgmma with A in registers), loaded per thread from the swizzled image at any row,
 //     so a k-tap conv stages its input once;
-//   * weights: pre-split, pre-swizzled images written at voice-load time; one cp.async.bulk (TMA) per tap of the
-//     K-block, completion on an mbarrier; the next K-block's window and weights load while this one computes;
-//   * MMA: wgmma.mma_async m64nNTk16 (B from shared memory by descriptor), six per (tap, K-block) and warpgroup;
-//   * epilogue: bias / gate / ReLU / residual / scale / accumulate straight from the accumulator registers.
+//   * weights: pre-split, pre-swizzled images written at voice-load time, one cp.async.bulk (TMA) per tap image,
+//     completion on an mbarrier.  RESIDENT when the layer has at most two K-blocks (then all of the n-tile's images
+//     take no more shared memory than two ring stages would): fetched once per CTA, before pdl_wait().  Otherwise each
+//     ring stage holds one K-block's taps, loading with that step's window;
+//   * MMA: wgmma.mma_async m64nNTk16 (B from shared memory by descriptor), six per (tap, K-block) and warpgroup, one
+//     commit group per tap.  On tiles of up to 64 columns the A fragments are double-buffered across taps: the next
+//     tap's fragments load while this tap's MMAs run (wait_group 1).  The issue order per accumulator is (K-block, tap,
+//     K step, hi*hi, lo*hi, hi*lo) either way, so every output keeps its bits;
+//   * epilogue: bias / gate / ReLU / residual / scale / accumulate straight from the accumulator registers; on tiles of
+//     up to 64 columns a column pair is one 8-byte access where the output layout allows it, and four pairs issue their
+//     residual / accumulated reads before any of them stores.
+// Registers are capped for 2 CTAs per SM (-Xptxas -v: 98 / 122 / 96 / 110 registers at NT = 32 / 64 / 96 / 128, no
+// spills), so the shared memory of a plan decides whether one or two CTAs share an SM.
 // Every mbarrier wait carries a watchdog that traps instead of hanging the GPU.
 #include "tc_common.cuh"
+#include <algorithm>
 #include <stdlib.h>
 #include <string.h>
 
 namespace sb200 {
+
+int g_conv_tc_grid_cap = 0;
 
 int wg_num_sms() {
     static int n = 0;
@@ -48,24 +64,31 @@ struct TcLaunch {
                      // divides it: every part keeps the image's swizzle, 32 % 8 == 0)
     int win;         // window rows (multiple of 8)
     int ntiles_m, ntiles_n;
+    int grid;        // CTAs: a multiple of ntiles_n, at most ntiles_m * ntiles_n
+    int resident;    // 1: every weight image of the CTA's n-tile stays in shared memory; 0: one K-block per ring stage
+    int pairs;       // 1: a column pair may be one 8-byte access to res / y0 / y1 (aligned, no phase mapping, no gate)
 };
 
 constexpr int TC_THREADS = 256;         // two warpgroups: tile rows [0, 64) and [64, 128)
 constexpr int TC_STAGES = 2;
 
 template <int NT>
-__global__ void __launch_bounds__(TC_THREADS, 1) conv_tc_kernel(const ConvArgs a, const TcLaunch L) {
+__global__ void __launch_bounds__(TC_THREADS, 2) conv_tc_kernel(const ConvArgs a, const TcLaunch L) {
     pdl_trigger();
     extern __shared__ __align__(1024) uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-    const uint32_t a_buf = (uint32_t)L.win * 128u;               // one window image
-    const uint32_t w_tap = (uint32_t)NT * 128u;                  // one tap of a weight stage ([hi|lo] rows)
-    const uint32_t w_buf = (uint32_t)a.ntaps * w_tap;
-    const uint32_t A0 = smem_u32(smem), W0 = A0 + TC_STAGES * a_buf;
-    uint64_t* bars = reinterpret_cast<uint64_t*>(smem + TC_STAGES * (a_buf + w_buf));
-    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-    const int m_tile = (int)blockIdx.x / L.ntiles_n, n_tile = (int)blockIdx.x % L.ntiles_n;
     const int nkb = a.cin / 32;
+    const uint32_t a_buf = (uint32_t)L.win * 128u;               // one window image
+    const uint32_t w_tap = (uint32_t)NT * 128u;                  // one tap of a weight image ([hi|lo] rows)
+    const uint32_t w_kb = (uint32_t)a.ntaps * w_tap;             // the taps of one K-block
+    const uint32_t w_bytes = L.resident ? (uint32_t)nkb * w_kb : TC_STAGES * w_kb;
+    const uint32_t A0 = smem_u32(smem), W0 = A0 + TC_STAGES * a_buf;
+    uint64_t* bars = reinterpret_cast<uint64_t*>(smem + TC_STAGES * a_buf + w_bytes);
+    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+    const int n_tile = (int)blockIdx.x % L.ntiles_n, m_first = (int)blockIdx.x / L.ntiles_n;
+    const int m_step = (int)gridDim.x / L.ntiles_n;
+    const int nsteps = (L.ntiles_m - m_first + m_step - 1) / m_step * nkb;   // step j: m-tile m_first + j / nkb * m_step,
+                                                                             // K-block j % nkb
 
     if (tid == 0) {
         for (int s = 0; s < TC_STAGES; s++) mbar_init(smem_u32(&bars[s]), 1);
@@ -73,22 +96,23 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv_tc_kernel(const ConvArgs a
     }
     __syncthreads();
 
-    // weight stage kb: tap t is rows [part * NT, part * NT + NT) of image (n-tile of the voice, kb, t)
+    // K-block kb, tap t of the n-tile: rows [part * NT, part * NT + NT) of image (n-tile of the voice, kb, t)
     const int vf = L.wnt / NT;
     const size_t w_image = (size_t)L.wnt * 128u;
     const uint8_t* wsrc = reinterpret_cast<const uint8_t*>(a.wtc) + (size_t)(n_tile / vf) * nkb * a.ntaps * w_image +
                           (size_t)(n_tile % vf) * w_tap;
-    auto issue_w = [&](int kb, int s) {
+    // images [kb0 * ntaps, (kb0 + nkb_) * ntaps) to dst, completion on bars[s]
+    auto issue_w = [&](int kb0, int nkb_, uint32_t dst, int s) {
         if (tid == 0) {
             const uint32_t bar = smem_u32(&bars[s]);
-            mbar_expect_tx(bar, w_buf);
-            for (int t = 0; t < a.ntaps; t++)
-                bulk_g2s(W0 + s * w_buf + t * w_tap, wsrc + (size_t)(kb * a.ntaps + t) * w_image, w_tap, bar);
+            mbar_expect_tx(bar, (uint32_t)nkb_ * w_kb);
+            for (int i = 0; i < nkb_ * a.ntaps; i++)
+                bulk_g2s(dst + i * w_tap, wsrc + (size_t)(kb0 * a.ntaps + i) * w_image, w_tap, bar);
         }
     };
-    // window of K-block kb: raw fp32 rows, linear (row r at r * 128 B)
-    const int rbase = m_tile * 128 + a.min_off;
-    auto issue_a = [&](int kb, int s) {
+    // window of step j: raw fp32 rows, linear (row r at r * 128 B)
+    auto issue_a = [&](int j, int s) {
+        const int kb = j % nkb, rbase = (m_first + j / nkb * m_step) * 128 + a.min_off;
         for (int idx = tid; idx < L.win * 8; idx += TC_THREADS) {
             const int gr = rbase + (idx >> 3);
             const bool ok = gr >= 0 && gr < a.rows_in;
@@ -98,7 +122,9 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv_tc_kernel(const ConvArgs a
         cp_async_commit();
     };
 
-    issue_w(0, 0);                                      // weights are constants: fetched before the predecessor finishes
+    // weights are constants: fetched before the predecessor finishes
+    if (L.resident) issue_w(0, nkb, W0, 0);
+    else issue_w(0, 1, W0, 0);
     pdl_wait();
     issue_a(0, 0);
 
@@ -108,11 +134,13 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv_tc_kernel(const ConvArgs a
 #pragma unroll
     for (int i = 0; i < NT / 2; i++) acc[i] = 0.f;
 
-    for (int kb = 0; kb < nkb; kb++) {
-        const int s = kb & 1;
-        if (kb + 1 < nkb) {                             // stage s ^ 1 was released at the end of the previous K-block
-            issue_w(kb + 1, s ^ 1);
-            issue_a(kb + 1, s ^ 1);
+    const int n0 = n_tile * NT;
+
+    for (int j = 0; j < nsteps; j++) {
+        const int s = j & 1, kb = j % nkb;
+        if (j + 1 < nsteps) {                           // stage s ^ 1 was released at the end of the previous step
+            if (!L.resident) issue_w((j + 1) % nkb, 1, W0 + (s ^ 1) * w_kb, s ^ 1);
+            issue_a(j + 1, s ^ 1);
             cp_async_wait<1>();
         } else {
             cp_async_wait<0>();
@@ -153,11 +181,16 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv_tc_kernel(const ConvArgs a
             }
         }
         __syncthreads();
-        mbar_wait(smem_u32(&bars[s]), (uint32_t)((kb >> 1) & 1));
-        const uint32_t wst = W0 + s * w_buf;
-        for (int t = 0; t < a.ntaps; t++) {
+        uint32_t wst;
+        if (L.resident) {
+            if (j == 0) mbar_wait<false>(smem_u32(&bars[0]), 0);
+            wst = W0 + kb * w_kb;
+        } else {
+            mbar_wait<false>(smem_u32(&bars[s]), (uint32_t)((j >> 1) & 1));
+            wst = W0 + s * w_kb;
+        }
+        auto load_frag = [&](int t, uint32_t (&ah)[2][4], uint32_t (&al)[2][4]) {
             const int R0 = r0 + a.tap_off[t] - a.min_off, R1 = R0 + 8;
-            uint32_t ah[2][4], al[2][4];
 #pragma unroll
             for (int ks = 0; ks < 2; ks++) {
                 ah[ks][0] = lds32(sw128(img, R0, 2 * ks) + 4u * c);
@@ -169,8 +202,9 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv_tc_kernel(const ConvArgs a
                 al[ks][2] = lds32(sw128(img, R0, 5 + 2 * ks) + 4u * c);
                 al[ks][3] = lds32(sw128(img, R1, 5 + 2 * ks) + 4u * c);
             }
+        };
+        auto mma_tap = [&](int t, const uint32_t (&ah)[2][4], const uint32_t (&al)[2][4]) {
             const uint32_t wimg = wst + t * w_tap;
-            acc_fence<NT / 2>(acc);
             wg_fence();
 #pragma unroll
             for (int ks = 0; ks < 2; ks++) {                // two K = 16 steps inside the 64-byte hi half
@@ -181,83 +215,208 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv_tc_kernel(const ConvArgs a
                 wgmma_rs<WG_BF16, NT>(acc, ah[ks], dwl);
             }
             wg_commit();
-            wg_wait0();
-            acc_fence<NT / 2>(acc);
+        };
+        uint32_t ah0[2][4], al0[2][4];
+        acc_fence<NT / 2>(acc);
+        if constexpr (NT <= 64) {
+            // even taps use fragment set 0, odd taps set 1; after a tap is issued, wait_group 1 retires the tap before
+            // it, whose set the next tap reloads
+            uint32_t ah1[2][4], al1[2][4];
+            for (int t = 0; t < a.ntaps; t += 2) {
+                load_frag(t, ah0, al0);
+                mma_tap(t, ah0, al0);
+                wg_wait1();
+                if (t + 1 < a.ntaps) {
+                    load_frag(t + 1, ah1, al1);
+                    mma_tap(t + 1, ah1, al1);
+                    wg_wait1();
+                }
+            }
+        } else {
+            // one fragment set: a second one does not fit the 128 registers per thread of two CTAs per SM next to the
+            // 64- or 48-register accumulator
+            for (int t = 0; t < a.ntaps; t++) {
+                load_frag(t, ah0, al0);
+                mma_tap(t, ah0, al0);
+                wg_wait0();
+            }
         }
-        __syncthreads();                                // stage s fully read: the next iteration refills it
-    }
+        wg_wait0();
+        acc_fence<NT / 2>(acc);
+        __syncthreads();                                // stage s fully read: the next step refills it
+        if (kb < nkb - 1) continue;
 
-    // ===================== epilogue: thread owns rows r0, r0 + 8 and column pairs 8j + 2c =====================
-    const int n0 = n_tile * NT;
-    const bool gate = a.act == ACT_GATE;
+        // ===================== epilogue: thread owns rows r0, r0 + 8 and column pairs 8p + 2c =====================
+        const int m_tile = m_first + j / nkb * m_step;
+        const bool gate = a.act == ACT_GATE;
+        if (NT <= 64 && L.pairs && !gate) {        // (on wider tiles this path costs the registers of a second CTA per SM)
+            // Both columns of a pair on one side of the split (split is even): the per-element rule of the general path,
+            // 8 bytes at a time.  A group of the thread's pairs issues all its global reads before any of them stores: the
+            // compiler may not move a load above a store to a buffer that could alias it, so interleaved, every pair
+            // would wait for a memory round trip of its own.
+            constexpr int NP = NT / 8, G = 4;                     // pairs per row; pairs per read group
+            bool live[2], valid[2];
+            const float* bias[2];
+            size_t orow0[2];
 #pragma unroll
-    for (int h = 0; h < 2; h++) {
-        const int q = m_tile * 128 + r0 + 8 * h;
-        if (q >= a.rows_q) continue;
-        bool valid;
-        const float* bias = conv_row(a, q, valid);
-        const size_t orow0 = (size_t)q * a.orow_mul + a.orow_add;
-#pragma unroll
-        for (int j = 0; j < NT / 8; j++) {
-            const int nb = n0 + 8 * j + 2 * c;          // bias / weight column of the pair's first element
-            if (nb >= a.cout) continue;
-            float o[2] = {acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1]};
-            if (bias) { o[0] += bias[nb]; o[1] += bias[nb + 1]; }
-            if (gate) {
-                // phase-fused ConvTranspose never gates: the pair (2k, 2k+1) gives output column k
-                a.y0[orow0 * a.ldy0 + (nb >> 1)] = valid ? tanhf(o[0]) * (1.f / (1.f + expf(-o[1]))) * a.scale : 0.f;
-                continue;
+            for (int h = 0; h < 2; h++) {
+                const int q = m_tile * 128 + r0 + 8 * h;
+                live[h] = q < a.rows_q;
+                valid[h] = false;
+                bias[h] = live[h] ? conv_row(a, q, valid[h]) : nullptr;
+                orow0[h] = (size_t)q * a.orow_mul + a.orow_add;
             }
-            if (a.act == ACT_RELU) { o[0] = fmaxf(o[0], 0.f); o[1] = fmaxf(o[1], 0.f); }
 #pragma unroll
-            for (int e = 0; e < 2; e++) {
-                // phase-fused ConvTranspose (phase_cols > 0): column block n / phase_cols is the output phase, i.e. output
-                // row q*u + phase and column n % phase_cols
-                int n = nb + e;
-                size_t orow = orow0;
-                if (a.phase_cols) { orow += (size_t)(n / a.phase_cols); n %= a.phase_cols; }
-                const bool lo_side = n < a.split;
-                const int accum = lo_side ? a.acc0 : a.acc1;
-                if (accum && !valid) continue;          // accumulated buffers keep their zeros in gap rows
-                float m = 0.f;
-                if (a.res && valid) m = a.res[orow * a.ldres + n] * a.scale;
-                float* dst = lo_side ? a.y0 + orow * a.ldy0 + n : a.y1 + orow * a.ldy1 + (n - a.split);
-                if (accum && valid) m += *dst;
-                *dst = valid ? fmaf(o[e], a.scale, m) : 0.f;
+            for (int k0 = 0; k0 < 2 * NP; k0 += G) {
+                float2 rv[G], dv[G];
+#pragma unroll
+                for (int i = 0; i < G; i++) {
+                    const int h = (k0 + i) / NP, nb = n0 + 8 * ((k0 + i) % NP) + 2 * c;
+                    rv[i] = dv[i] = make_float2(0.f, 0.f);
+                    if (!live[h] || nb >= a.cout || !valid[h]) continue;
+                    const bool lo_side = nb < a.split;
+                    if (a.res) rv[i] = *reinterpret_cast<const float2*>(a.res + orow0[h] * a.ldres + nb);
+                    if (lo_side ? a.acc0 : a.acc1)
+                        dv[i] = *reinterpret_cast<const float2*>(lo_side ? a.y0 + orow0[h] * a.ldy0 + nb
+                                                                         : a.y1 + orow0[h] * a.ldy1 + (nb - a.split));
+                }
+#pragma unroll
+                for (int i = 0; i < G; i++) {
+                    const int h = (k0 + i) / NP, p = (k0 + i) % NP, nb = n0 + 8 * p + 2 * c;
+                    if (!live[h] || nb >= a.cout) continue;
+                    float o[2] = {acc[4 * p + 2 * h], acc[4 * p + 2 * h + 1]};
+                    if (bias[h]) { o[0] += bias[h][nb]; o[1] += bias[h][nb + 1]; }
+                    if (a.act == ACT_RELU) { o[0] = fmaxf(o[0], 0.f); o[1] = fmaxf(o[1], 0.f); }
+                    const bool lo_side = nb < a.split;
+                    const int accum = lo_side ? a.acc0 : a.acc1;
+                    if (accum && !valid[h]) continue;
+                    float2 m = make_float2(0.f, 0.f);
+                    if (a.res && valid[h]) { m.x = rv[i].x * a.scale; m.y = rv[i].y * a.scale; }
+                    if (accum && valid[h]) { m.x += dv[i].x; m.y += dv[i].y; }
+                    *reinterpret_cast<float2*>(lo_side ? a.y0 + orow0[h] * a.ldy0 + nb : a.y1 + orow0[h] * a.ldy1 + (nb - a.split)) =
+                        valid[h] ? make_float2(fmaf(o[0], a.scale, m.x), fmaf(o[1], a.scale, m.y)) : make_float2(0.f, 0.f);
+                }
+            }
+        } else {
+#pragma unroll
+            for (int h = 0; h < 2; h++) {
+                const int q = m_tile * 128 + r0 + 8 * h;
+                if (q >= a.rows_q) continue;
+                bool valid;
+                const float* bias = conv_row(a, q, valid);
+                const size_t orow0 = (size_t)q * a.orow_mul + a.orow_add;
+#pragma unroll
+                for (int p = 0; p < NT / 8; p++) {
+                    const int nb = n0 + 8 * p + 2 * c;      // bias / weight column of the pair's first element
+                    if (nb >= a.cout) continue;
+                    float o[2] = {acc[4 * p + 2 * h], acc[4 * p + 2 * h + 1]};
+                    if (bias) { o[0] += bias[nb]; o[1] += bias[nb + 1]; }
+                    if (gate) {
+                        // phase-fused ConvTranspose never gates: the pair (2k, 2k+1) gives output column k
+                        a.y0[orow0 * a.ldy0 + (nb >> 1)] = valid ? tanhf(o[0]) * (1.f / (1.f + expf(-o[1]))) * a.scale : 0.f;
+                        continue;
+                    }
+                    if (a.act == ACT_RELU) { o[0] = fmaxf(o[0], 0.f); o[1] = fmaxf(o[1], 0.f); }
+#pragma unroll
+                    for (int e = 0; e < 2; e++) {
+                        // phase-fused ConvTranspose (phase_cols > 0): column block n / phase_cols is the output phase, i.e.
+                        // output row q*u + phase and column n % phase_cols
+                        int n = nb + e;
+                        size_t orow = orow0;
+                        if (a.phase_cols) { orow += (size_t)(n / a.phase_cols); n %= a.phase_cols; }
+                        const bool lo_side = n < a.split;
+                        const int accum = lo_side ? a.acc0 : a.acc1;
+                        if (accum && !valid) continue;      // accumulated buffers keep their zeros in gap rows
+                        float m = 0.f;
+                        if (a.res && valid) m = a.res[orow * a.ldres + n] * a.scale;
+                        float* dst = lo_side ? a.y0 + orow * a.ldy0 + n : a.y1 + orow * a.ldy1 + (n - a.split);
+                        if (accum && valid) m += *dst;
+                        *dst = valid ? fmaf(o[e], a.scale, m) : 0.f;
+                    }
+                }
             }
         }
+#pragma unroll
+        for (int i = 0; i < NT / 2; i++) acc[i] = 0.f;
     }
 }
 
-size_t smem_bytes(const ConvArgs& a, int nt, int win) {
-    return (size_t)TC_STAGES * ((size_t)win * 128 + (size_t)a.ntaps * nt * 128) + TC_STAGES * 8;
+// Every K-block's images when resident (nkb <= TC_STAGES: never more than the ring's two stages), else two stages.
+size_t smem_bytes(const ConvArgs& a, int nt, int win, bool resident) {
+    const size_t w_kb = (size_t)a.ntaps * nt * 128;
+    return (size_t)TC_STAGES * win * 128 + (resident ? (size_t)(a.cin / 32) : (size_t)TC_STAGES) * w_kb + TC_STAGES * 8;
 }
+
+template <int NT> void allow_smem() {
+    static PerDeviceOnce once;
+    once.run([] { cudaFuncSetAttribute(conv_tc_kernel<NT>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024); });
+}
+
+template <int NT> int occupancy(size_t smem) {
+    allow_smem<NT>();
+    int n = 0;
+    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, conv_tc_kernel<NT>, TC_THREADS, smem) != cudaSuccess) {
+        cudaGetLastError();
+        n = 0;
+    }
+    return n;
+}
+
+// CTAs of conv_tc_kernel<nt> with `smem` bytes of dynamic shared memory that fit on one SM: the occupancy API's answer,
+// cached per (nt, smem KB) -- every plan's smem is 16 bytes past a multiple of 1024, so the KB is exact.  Without a
+// device, the bound of the 228 KB of shared memory per SM (1 KB of it reserved per CTA) alone.
+int ctas_per_sm(int nt, size_t smem) {
+    static int cache[4][256];
+    int& slot = cache[nt / 32 - 1][std::min<size_t>(smem >> 10, 255)];
+    int n = __atomic_load_n(&slot, __ATOMIC_RELAXED);
+    if (n > 0) return n;
+    switch (nt) {
+        case 32: n = occupancy<32>(smem); break;
+        case 64: n = occupancy<64>(smem); break;
+        case 96: n = occupancy<96>(smem); break;
+        default: n = occupancy<128>(smem); break;
+    }
+    if (n > 0) {
+        __atomic_store_n(&slot, n, __ATOMIC_RELAXED);
+        return n;
+    }
+    return std::max(1, std::min(2048 / TC_THREADS, (int)((228u * 1024u) / (smem + 1024))));
+}
+
+bool aligned8(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 7) == 0; }
 
 bool plan(const ConvArgs& a, TcLaunch& L, size_t& smem) {
     if (!a.wtc || a.tc_nt <= 0 || a.tc_nt > 128 || a.tc_nt % 32) return false;
     L.wnt = a.tc_nt;
     L.win = (128 + a.span + 7) & ~7;
     const int mt = (a.rows_q + 127) / 128;
-    // The widest part of an image whose two stages fit; on small launches (a single utterance) the narrowest part that
-    // still leaves no more tiles than SMs, so that more SMs share the work.  Tile width changes no summation order: an
-    // utterance comes out bit-identical whether it is synthesised alone or in a batch.
+    // The widest part of an image whose two ring stages fit; on small launches (a single utterance) the narrowest part
+    // that still leaves no more tiles than SMs, so that more SMs share the work.  Tile width changes no summation order:
+    // an utterance comes out bit-identical whether it is synthesised alone or in a batch.
     L.nt = 0;
     for (int nt = a.tc_nt; nt >= 32; nt -= 32)
-        if (a.tc_nt % nt == 0 && smem_bytes(a, nt, L.win) <= WG_SMEM_BUDGET) { L.nt = nt; break; }
+        if (a.tc_nt % nt == 0 && smem_bytes(a, nt, L.win, false) <= WG_SMEM_BUDGET) { L.nt = nt; break; }
     if (!L.nt) return false;
     if (a.cout % a.tc_nt == 0)
         for (int nt = 32; nt < L.nt; nt += 32)
             if (L.nt % nt == 0 && mt * (a.cout / nt) <= wg_num_sms()) { L.nt = nt; break; }
     L.ntiles_m = mt;
     L.ntiles_n = (a.cout + L.nt - 1) / L.nt;
-    smem = smem_bytes(a, L.nt, L.win) + 1024;
+    L.resident = a.cin / 32 <= TC_STAGES;
+    smem = smem_bytes(a, L.nt, L.win, L.resident) + 1024;
+    // Persistent grid: every CTA that fits at once, rounded down to whole m-tiles (a CTA keeps its n-tile); a launch of
+    // no more tiles than that runs one tile per CTA.
+    int grid = wg_num_sms() * ctas_per_sm(L.nt, smem);
+    if (g_conv_tc_grid_cap > 0) grid = std::min(grid, g_conv_tc_grid_cap);
+    L.grid = std::min(std::max(L.ntiles_n, grid / L.ntiles_n * L.ntiles_n), L.ntiles_m * L.ntiles_n);
+    L.pairs = !a.phase_cols && a.act != ACT_GATE && a.split % 2 == 0 && aligned8(a.y0) && aligned8(a.y1) &&
+              a.ldy0 % 2 == 0 && a.ldy1 % 2 == 0 && (!a.res || (aligned8(a.res) && a.ldres % 2 == 0));
     return true;
 }
 
 template <int NT> void launch_nt(const ConvArgs& a, const TcLaunch& L, size_t smem, cudaStream_t st) {
-    static PerDeviceOnce once;
-    once.run([] { cudaFuncSetAttribute(conv_tc_kernel<NT>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024); });
-    launch_pdl(conv_tc_kernel<NT>, dim3(L.ntiles_m * L.ntiles_n), dim3(TC_THREADS), smem, st, a, L);
+    allow_smem<NT>();
+    launch_pdl(conv_tc_kernel<NT>, dim3(L.grid), dim3(TC_THREADS), smem, st, a, L);
 }
 
 uint16_t bf16_rn_host(float f) {
@@ -275,7 +434,8 @@ float bf16_to_float_host(uint16_t h) {
 bool conv_tc_plan_info(const ConvArgs& a, int* out) {
     TcLaunch L{}; size_t smem = 0;
     if (a.cin % 32 || a.cout % 32 || a.ntaps > SB_MAX_TAPS || !plan(a, L, smem)) return false;
-    const int v[16] = {L.nt, L.wnt, L.ntiles_m, L.ntiles_n, TC_STAGES, (int)smem, L.win, 0, 0, 0, 0, 0, 0, 0, 0, 0};
+    const int v[16] = {L.nt, L.wnt, L.ntiles_m, L.ntiles_n, TC_STAGES, (int)smem, L.win, L.grid, L.resident,
+                       ctas_per_sm(L.nt, smem), 0, 0, 0, 0, 0, 0};
     for (int i = 0; i < 16; i++) out[i] = v[i];
     return true;
 }

@@ -38,7 +38,9 @@ __device__ __forceinline__ bool mbar_try(uint32_t bar, uint32_t parity) {
         : "=r"(ok) : "r"(bar), "r"(parity) : "memory");
     return ok != 0;
 }
-__device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
+// kPrint = false traps without the message: printf is a function call, and ptxas serializes every wgmma of a kernel that
+// keeps wgmma groups in flight (wait_group 1) and contains a call (conv_tc.cu)
+template <bool kPrint = true> __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
     unsigned spins = 0;
     unsigned long long t0 = 0;
     while (!mbar_try(bar, parity)) {
@@ -47,7 +49,8 @@ __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
         asm volatile("mov.u64 %0, %globaltimer;" : "=l"(now));
         if (t0 == 0) t0 = now;
         if (now - t0 > 2000000000ull) {   // 2 s: a pipeline bug must fail loudly, never hang the GPU
-            printf("wgmma conv: mbarrier watchdog (block %d thread %d bar %u parity %u)\n", blockIdx.x, threadIdx.x, bar, parity);
+            if (kPrint)
+                printf("wgmma conv: mbarrier watchdog (block %d thread %d bar %u parity %u)\n", blockIdx.x, threadIdx.x, bar, parity);
             asm volatile("trap;");
         }
     }
@@ -79,6 +82,7 @@ __device__ __forceinline__ uint64_t sw128_desc(uint32_t saddr) {
 __device__ __forceinline__ void wg_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wg_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wg_wait0() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
+__device__ __forceinline__ void wg_wait1() { asm volatile("wgmma.wait_group.sync.aligned 1;" ::: "memory"); }
 // pins accumulator registers in place around the asynchronous MMAs (no read or write may move across)
 template <int NREG> __device__ __forceinline__ void acc_fence(float* d) {
 #pragma unroll

@@ -2,7 +2,7 @@
 Usage: python tools/conv_unit.py <backend> [quick | i,j,...]
 
 Backends: 0 = conv_simt.cu (fp32 CUDA cores), 1 = conv_tc.cu (wgmma bf16x2), 2 = conv_tf.cu (wgmma 3xTF32, chunk-flushed).
-On the wgmma kernels one CTA computes one 128-row tile of NT columns.  NT is the width of the voice's weight image, or a
+On the wgmma kernels a CTA computes 128-row tiles of NT columns.  NT is the width of the voice's weight image, or a
 32-column multiple part of it when the launch is small: the planners narrow the tile while m-tiles x (cout / NT) <= SMs
 (`narrow_edge`).  The hook pads a launch to a multiple of 256 rows, like the engine's segment tables."""
 import ctypes as C
@@ -203,7 +203,7 @@ CASES = [
     (E256, 256, 256, 11, 5, 0.1, 0, True, 1.0, False, E256 - 50),
     (E256 + 77, 256, 256, 11, 5, 0.1, 0, True, 1.0, False, None),
     (333, 192, 96, 1, 1, 1.0, 0, True, -1.0, True, 301),
-    # many more tiles than SMs (one CTA per tile, several waves): the 32- and 64-channel ResBlock layers of the last
+    # many more tiles than SMs (several tiles per CTA): the 32- and 64-channel ResBlock layers of the last
     # decoder stages, every (k, dilation) of ResBlock2 / ResBlock1, ragged tails inside a warp's 32 rows, accumulate /
     # residual / scale, ReLU, no residual
     (SMS * 128 * 3 + 384, 32, 32, 3, 2, 0.1, 0, True, 1.0, False, SMS * 128 * 3 + 300),
