@@ -46,7 +46,6 @@ struct ConvArgs {
     const float* wtf;                                             // tf32 hi/lo images (conv_tf.cu) or null
     int ntaps; int tap_off[SB_MAX_TAPS]; int min_off; int span;   // span = max_off - min_off
     int rows_q; int orow_mul; int orow_add;
-    int phase_cols;                                               // >0: fused polyphase ConvTranspose (conv_tc.cu only)
     RowMap map;                                                   // validity of q
     int act; float scale;
     const float* res; int ldres;

@@ -11,28 +11,34 @@
 //
 // Persistent CTAs: the grid is as many CTAs as can be resident at once, and each walks a static list of 128-row x
 // NT-column tiles.  A CTA keeps one n-tile (blockIdx % ntiles_n) and takes the m-tiles blockIdx / ntiles_n + i * (grid /
-// ntiles_n): the CTAs of one m-tile run side by side, so the re-reads of its window come from L2.  Two warpgroups
-// (rows 0-63 / 64-127) and a two-stage ring over the CTA's flat sequence of (tile, K-block) steps, so the next tile's
-// first window loads while this tile runs its MMAs and its epilogue:
+// ntiles_n): the CTAs of one m-tile run side by side, so the re-reads of its window come from L2.
+//
+// Warp-specialized: producer warps load and convert (one warpgroup on 32-column tiles, two on wider ones, which run one
+// CTA per SM), two MMA warpgroups (tile rows 0-63 / 64-127) run the MMAs and the epilogue.  They hand off through a two-stage ring over the CTA's flat sequence of (tile, K-block) steps; each
+// stage has a full and an empty mbarrier.  While the MMA warpgroups work on one step, the producer loads and converts the
+// next (a deeper ring, where shared memory allowed one, was slower: DESIGN.md section 3):
 //   * activations: the raw fp32 (128 + span)-row WINDOW of a K-block (32 channels = one 128-byte row) arrives by
-//     cp.async (rows outside the array zero-filled); all threads then apply the leaky-ReLU prologue, split hi/lo and
-//     rewrite each row IN PLACE as [hi: 32 ch bf16 | lo: 32 ch bf16] in the K-major SWIZZLE_128B layout (row r at
-//     r*128 B, 16-B chunk c at (c ^ (r & 7))).  A tap is the same window read from a row offset: the A operand
-//     comes from registers (wgmma with A in registers), loaded per thread from the swizzled image at any row,
-//     so a k-tap conv stages its input once;
-//   * weights: pre-split, pre-swizzled images written at voice-load time, one cp.async.bulk (TMA) per tap image,
-//     completion on an mbarrier.  RESIDENT when the layer has at most two K-blocks (then all of the n-tile's images
-//     take no more shared memory than two ring stages would): fetched once per CTA, before pdl_wait().  Otherwise each
-//     ring stage holds one K-block's taps, loading with that step's window;
+//     cp.async (rows outside the array zero-filled); the producer then applies the leaky-ReLU prologue, splits hi/lo and
+//     rewrites each row IN PLACE as [hi: 32 ch bf16 | lo: 32 ch bf16] in the K-major SWIZZLE_128B layout (row r at
+//     r*128 B, 16-B chunk c at (c ^ (r & 7))), and arrives on the stage's full barrier.  A tap is the same window read
+//     from a row offset: the A operand comes from registers (wgmma with A in registers), loaded per thread from the
+//     swizzled image at any row, so a k-tap conv stages its input once;
+//   * weights: pre-split, pre-swizzled images written at voice-load time, one cp.async.bulk (TMA) per tap image.
+//     RESIDENT when the layer has at most two K-blocks (then all of the n-tile's images take no more shared memory than
+//     two ring stages would): fetched once per CTA, before pdl_wait(), on a barrier of their own.  Otherwise each ring
+//     stage holds one K-block's taps, counted in bytes on the stage's full barrier;
 //   * MMA: wgmma.mma_async m64nNTk16 (B from shared memory by descriptor), six per (tap, K-block) and warpgroup, one
-//     commit group per tap.  On tiles of up to 64 columns the A fragments are double-buffered across taps: the next
-//     tap's fragments load while this tap's MMAs run (wait_group 1).  The issue order per accumulator is (K-block, tap,
-//     K step, hi*hi, lo*hi, hi*lo) either way, so every output keeps its bits;
-//   * epilogue: bias / gate / ReLU / residual / scale / accumulate straight from the accumulator registers; on tiles of
-//     up to 64 columns a column pair is one 8-byte access where the output layout allows it, and four pairs issue their
-//     residual / accumulated reads before any of them stores.
-// Registers are capped for 2 CTAs per SM (-Xptxas -v: 98 / 122 / 96 / 110 registers at NT = 32 / 64 / 96 / 128, no
-// spills), so the shared memory of a plan decides whether one or two CTAs share an SM.
+//     commit group per tap; the A fragments are double-buffered across taps (the next tap's load while this tap's MMAs
+//     run, wait_group 1).  The issue order per accumulator is (K-block, tap, K step, hi*hi, lo*hi, hi*lo), so every
+//     output keeps its bits.  Once a step's MMAs have retired, the MMA warpgroups arrive on the stage's empty barrier,
+//     before the epilogue, so the producer refills it while they store;
+//   * epilogue: bias / gate / ReLU / residual / scale / accumulate straight from the accumulator registers; a column
+//     pair is one 8-byte access where the output layout allows it, and groups of pairs issue their residual /
+//     accumulated reads before any of them stores.  On tiles wider than 32 columns the first group's reads are issued
+//     before the tile's last K-block runs its MMAs.
+// Registers (setmaxnreg): 32-column tiles run 2 CTAs per SM at 80 registers per thread, the producer dropping to 40 and
+// the MMA warpgroups rising to 96; wider tiles run one CTA per SM at 128, split 32 (two producer warpgroups) / 224.
+// -Xptxas -v: no spills at any NT.
 // Every mbarrier wait carries a watchdog that traps instead of hanging the GPU.
 #include "tc_common.cuh"
 #include <algorithm>
@@ -66,68 +72,143 @@ struct TcLaunch {
     int ntiles_m, ntiles_n;
     int grid;        // CTAs: a multiple of ntiles_n, at most ntiles_m * ntiles_n
     int resident;    // 1: every weight image of the CTA's n-tile stays in shared memory; 0: one K-block per ring stage
-    int pairs;       // 1: a column pair may be one 8-byte access to res / y0 / y1 (aligned, no phase mapping, no gate)
+    int pairs;       // 1: a column pair may be one 8-byte access to res / y0 / y1 (aligned, no gate)
 };
 
-constexpr int TC_THREADS = 256;         // two warpgroups: tile rows [0, 64) and [64, 128)
+constexpr int TC_CONSUMERS = 256;       // two MMA warpgroups: tile rows [0, 64) and [64, 128)
 constexpr int TC_STAGES = 2;
+constexpr int TC_BAR_BYTES = 64;        // full[TC_STAGES], empty[TC_STAGES], resident weights
+
+// Roles and register split per tile width.  32-column tiles run 2 CTAs per SM (their shared memory would allow more;
+// registers decide) with one producer warpgroup: 80 registers at launch -> producer 40 / MMA warpgroups 96.  Wider tiles
+// run one CTA per SM, and there the conversion of one warpgroup alone sets the pace of layers with short MMAs (the
+// 64-channel ResBlocks), so two producer warpgroups share each window: 128 -> 32 / 224.
+template <int NT> struct TcRoles {
+    static constexpr int ctas = NT == 32 ? 2 : 1;
+    static constexpr int producers = NT == 32 ? 128 : 256;   // window and weight loads, in-place conversion
+    static constexpr int threads = TC_CONSUMERS + producers;
+    static constexpr int launch = (65536 / (threads * ctas)) & ~7;
+    static constexpr int producer_regs = NT == 32 ? 40 : 32;
+    static constexpr int consumer_regs = ((launch * threads - producer_regs * producers) / TC_CONSUMERS) & ~7;
+};
 
 template <int NT>
-__global__ void __launch_bounds__(TC_THREADS, 2) conv_tc_kernel(const ConvArgs a, const TcLaunch L) {
+__global__ void __launch_bounds__(TcRoles<NT>::threads, TcRoles<NT>::ctas) conv_tc_kernel(const ConvArgs a, const TcLaunch L) {
+    constexpr int NPROD = TcRoles<NT>::producers;
     pdl_trigger();
     extern __shared__ __align__(1024) uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-    const int nkb = a.cin / 32;
+    const int nkb = a.cin / 32, S = TC_STAGES;
     const uint32_t a_buf = (uint32_t)L.win * 128u;               // one window image
     const uint32_t w_tap = (uint32_t)NT * 128u;                  // one tap of a weight image ([hi|lo] rows)
     const uint32_t w_kb = (uint32_t)a.ntaps * w_tap;             // the taps of one K-block
-    const uint32_t w_bytes = L.resident ? (uint32_t)nkb * w_kb : TC_STAGES * w_kb;
-    const uint32_t A0 = smem_u32(smem), W0 = A0 + TC_STAGES * a_buf;
-    uint64_t* bars = reinterpret_cast<uint64_t*>(smem + TC_STAGES * a_buf + w_bytes);
-    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+    const uint32_t w_bytes = L.resident ? (uint32_t)nkb * w_kb : (uint32_t)S * w_kb;
+    const uint32_t A0 = smem_u32(smem), W0 = A0 + S * a_buf;
+    const uint32_t FULL = A0 + S * a_buf + w_bytes;              // full[s]: stage s converted (and its weights landed)
+    const uint32_t EMPTY = FULL + 8u * TC_STAGES;                // empty[s]: both MMA warpgroups done reading stage s
+    const uint32_t WRES = EMPTY + 8u * TC_STAGES;                // resident weights landed
+    const int tid = threadIdx.x;
     const int n_tile = (int)blockIdx.x % L.ntiles_n, m_first = (int)blockIdx.x / L.ntiles_n;
     const int m_step = (int)gridDim.x / L.ntiles_n;
     const int nsteps = (L.ntiles_m - m_first + m_step - 1) / m_step * nkb;   // step j: m-tile m_first + j / nkb * m_step,
-                                                                             // K-block j % nkb
+                                                                             // K-block j % nkb, ring stage j % S
 
     if (tid == 0) {
-        for (int s = 0; s < TC_STAGES; s++) mbar_init(smem_u32(&bars[s]), 1);
+        for (int s = 0; s < S; s++) {
+            mbar_init(FULL + 8u * s, NPROD + (L.resident ? 0 : 1));   // + the weights' expect_tx arrival
+            mbar_init(EMPTY + 8u * s, TC_CONSUMERS);
+        }
+        mbar_init(WRES, 1);
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
     __syncthreads();
 
-    // K-block kb, tap t of the n-tile: rows [part * NT, part * NT + NT) of image (n-tile of the voice, kb, t)
-    const int vf = L.wnt / NT;
-    const size_t w_image = (size_t)L.wnt * 128u;
-    const uint8_t* wsrc = reinterpret_cast<const uint8_t*>(a.wtc) + (size_t)(n_tile / vf) * nkb * a.ntaps * w_image +
-                          (size_t)(n_tile % vf) * w_tap;
-    // images [kb0 * ntaps, (kb0 + nkb_) * ntaps) to dst, completion on bars[s]
-    auto issue_w = [&](int kb0, int nkb_, uint32_t dst, int s) {
-        if (tid == 0) {
-            const uint32_t bar = smem_u32(&bars[s]);
-            mbar_expect_tx(bar, (uint32_t)nkb_ * w_kb);
-            for (int i = 0; i < nkb_ * a.ntaps; i++)
-                bulk_g2s(dst + i * w_tap, wsrc + (size_t)(kb0 * a.ntaps + i) * w_image, w_tap, bar);
-        }
-    };
-    // window of step j: raw fp32 rows, linear (row r at r * 128 B)
-    auto issue_a = [&](int j, int s) {
-        const int kb = j % nkb, rbase = (m_first + j / nkb * m_step) * 128 + a.min_off;
-        for (int idx = tid; idx < L.win * 8; idx += TC_THREADS) {
-            const int gr = rbase + (idx >> 3);
-            const bool ok = gr >= 0 && gr < a.rows_in;
-            const float* src = ok ? a.x + (size_t)gr * a.ldx + kb * 32 + (idx & 7) * 4 : a.x;
-            cp_async16(A0 + s * a_buf + (uint32_t)idx * 16u, src, ok ? 16u : 0u);
-        }
-        cp_async_commit();
-    };
+    if (tid >= TC_CONSUMERS) {
+        // ============================= producer warpgroup(s): loads and in-place conversion =============================
+        setmaxnreg_dec<TcRoles<NT>::producer_regs>();
+        const int ptid = tid - TC_CONSUMERS;
+        // K-block kb, tap t of the n-tile: rows [part * NT, part * NT + NT) of image (n-tile of the voice, kb, t)
+        const int vf = L.wnt / NT;
+        const size_t w_image = (size_t)L.wnt * 128u;
+        const uint8_t* wsrc = reinterpret_cast<const uint8_t*>(a.wtc) + (size_t)(n_tile / vf) * nkb * a.ntaps * w_image +
+                              (size_t)(n_tile % vf) * w_tap;
+        // images [kb0 * ntaps, (kb0 + nkb_) * ntaps) to dst, completion on bar
+        auto issue_w = [&](int kb0, int nkb_, uint32_t dst, uint32_t bar) {
+            if (ptid == 0) {
+                mbar_expect_tx(bar, (uint32_t)nkb_ * w_kb);
+                for (int i = 0; i < nkb_ * a.ntaps; i++)
+                    bulk_g2s(dst + i * w_tap, wsrc + (size_t)(kb0 * a.ntaps + i) * w_image, w_tap, bar);
+            }
+        };
+        // window of step j: raw fp32 rows, linear (row r at r * 128 B)
+        auto issue_a = [&](int j, int s) {
+            const int kb = j % nkb, rbase = (m_first + j / nkb * m_step) * 128 + a.min_off;
+            for (int idx = ptid; idx < L.win * 8; idx += NPROD) {
+                const int gr = rbase + (idx >> 3);
+                const bool ok = gr >= 0 && gr < a.rows_in;
+                const float* src = ok ? a.x + (size_t)gr * a.ldx + kb * 32 + (idx & 7) * 4 : a.x;
+                cp_async16(A0 + s * a_buf + (uint32_t)idx * 16u, src, ok ? 16u : 0u);
+            }
+            cp_async_commit();
+        };
 
-    // weights are constants: fetched before the predecessor finishes
-    if (L.resident) issue_w(0, nkb, W0, 0);
-    else issue_w(0, 1, W0, 0);
+        // weights are constants: fetched before the predecessor finishes
+        if (L.resident) issue_w(0, nkb, W0, WRES);
+        else issue_w(0, 1, W0, FULL);
+        pdl_wait();
+
+        // Step j refills stage j % 2 once the MMA warpgroups have released it (step j - 2), and loads and converts it
+        // while they run step j - 1.
+        for (int j = 0; j < nsteps; j++) {
+            const int s = j & 1;
+            if (j >= S) mbar_wait<false>(EMPTY + 8u * s, (uint32_t)((j / S - 1) & 1));
+            if (!L.resident && j > 0) issue_w(j % nkb, 1, W0 + s * w_kb, FULL + 8u * s);
+            issue_a(j, s);
+            cp_async_wait<0>();
+            named_bar_sync(1, NPROD);            // every producer's part of the window has landed
+            // in-place conversion, 32-byte pieces (8 channels); the four lanes of a row sit in one warp: all read, then
+            // write.  Odd rows take their two 16-byte chunks in the opposite order (bank-conflict-free quarter-warps).
+            const uint32_t img = A0 + s * a_buf;
+            const int npiece = L.win * 4;
+            const float slope = a.in_slope;
+            for (int base = 0; base < npiece; base += NPROD) {
+                const int idx = base + ptid;
+                const bool live = idx < npiece;
+                const uint32_t odd = (uint32_t)(idx >> 2) & 1u;
+                float4 v0 = make_float4(0.f, 0.f, 0.f, 0.f), v1 = v0;
+                if (live) {
+                    const float4 t0 = lds128(img + (uint32_t)idx * 32u + odd * 16u);
+                    const float4 t1 = lds128(img + (uint32_t)idx * 32u + 16u - odd * 16u);
+                    v0 = odd ? t1 : t0;
+                    v1 = odd ? t0 : t1;
+                }
+                __syncwarp();
+                if (live) {
+                    const int r = idx >> 2, cc = idx & 3;
+                    float e[8] = {v0.x, v0.y, v0.z, v0.w, v1.x, v1.y, v1.z, v1.w};
+                    if (slope != 1.f) {
+#pragma unroll
+                        for (int i = 0; i < 8; i++) e[i] = fmaxf(e[i], e[i] * slope);   // leaky ReLU, 0 < slope < 1
+                    }
+                    uint4 hi, lo;
+                    hi.x = split2(e[0], e[1], lo.x);
+                    hi.y = split2(e[2], e[3], lo.y);
+                    hi.z = split2(e[4], e[5], lo.z);
+                    hi.w = split2(e[6], e[7], lo.w);
+                    const uint4 first = odd ? lo : hi, second = odd ? hi : lo;
+                    sts128u(sw128(img, r, cc + 4 * (int)odd), first);
+                    sts128u(sw128(img, r, cc + 4 - 4 * (int)odd), second);
+                }
+            }
+            mbar_arrive(FULL + 8u * s);
+        }
+        return;
+    }
+
+    // ================================ two MMA warpgroups: fragments, wgmma, epilogue ================================
+    setmaxnreg_inc<TcRoles<NT>::consumer_regs>();
     pdl_wait();
-    issue_a(0, 0);
-
+    const int warp = tid >> 5, lane = tid & 31;
     const int wg = warp >> 2, g = lane >> 2, c = lane & 3;
     const int r0 = wg * 64 + (warp & 3) * 16 + g;       // tile rows r0 and r0 + 8 of this thread
     float acc[NT / 2];
@@ -135,60 +216,71 @@ __global__ void __launch_bounds__(TC_THREADS, 2) conv_tc_kernel(const ConvArgs a
     for (int i = 0; i < NT / 2; i++) acc[i] = 0.f;
 
     const int n0 = n_tile * NT;
+    const bool gate = a.act == ACT_GATE;
+    const bool grouped = L.pairs && !gate;
+    // Grouped epilogue: both columns of a pair on one side of the split (split is even), the per-element rule of the
+    // general path 8 bytes at a time.  A group of the thread's pairs issues all its global reads before any of them
+    // stores: the compiler may not move a load above a store to a buffer that could alias it, so interleaved, every
+    // pair would wait for a memory round trip of its own.  On tiles wider than 32 columns, the first group's reads go out
+    // before the tile's last K-block runs its MMAs, and each later group's before the previous group stores.
+    constexpr int NP = NT / 8, G = NT == 32 ? 4 : 8, NG = 2 * NP / G;   // pairs per row; pairs per group; groups
+    constexpr bool EARLY = NT > 32;     // at 2 CTAs per SM (96 registers), one group's reads at a time, after the MMAs
+    bool live[2], valid[2];
+    const float* bias[2];
+    size_t orow0[2];
+    auto load_group = [&](int k0, float2 (&rv)[G], float2 (&dv)[G]) {
+#pragma unroll
+        for (int i = 0; i < G; i++) {
+            const int h = (k0 + i) / NP, nb = n0 + 8 * ((k0 + i) % NP) + 2 * c;
+            rv[i] = dv[i] = make_float2(0.f, 0.f);
+            if (!live[h] || nb >= a.cout || !valid[h]) continue;
+            const bool lo_side = nb < a.split;
+            if (a.res) rv[i] = *reinterpret_cast<const float2*>(a.res + orow0[h] * a.ldres + nb);
+            if (lo_side ? a.acc0 : a.acc1)
+                dv[i] = *reinterpret_cast<const float2*>(lo_side ? a.y0 + orow0[h] * a.ldy0 + nb
+                                                                 : a.y1 + orow0[h] * a.ldy1 + (nb - a.split));
+        }
+    };
+    auto store_group = [&](int k0, const float2 (&rv)[G], const float2 (&dv)[G]) {
+#pragma unroll
+        for (int i = 0; i < G; i++) {
+            const int h = (k0 + i) / NP, p = (k0 + i) % NP, nb = n0 + 8 * p + 2 * c;
+            if (!live[h] || nb >= a.cout) continue;
+            float o[2] = {acc[4 * p + 2 * h], acc[4 * p + 2 * h + 1]};
+            if (bias[h]) { o[0] += bias[h][nb]; o[1] += bias[h][nb + 1]; }
+            if (a.act == ACT_RELU) { o[0] = fmaxf(o[0], 0.f); o[1] = fmaxf(o[1], 0.f); }
+            const bool lo_side = nb < a.split;
+            const int accum = lo_side ? a.acc0 : a.acc1;
+            if (accum && !valid[h]) continue;
+            float2 m = make_float2(0.f, 0.f);
+            if (a.res && valid[h]) { m.x = rv[i].x * a.scale; m.y = rv[i].y * a.scale; }
+            if (accum && valid[h]) { m.x += dv[i].x; m.y += dv[i].y; }
+            *reinterpret_cast<float2*>(lo_side ? a.y0 + orow0[h] * a.ldy0 + nb : a.y1 + orow0[h] * a.ldy1 + (nb - a.split)) =
+                valid[h] ? make_float2(fmaf(o[0], a.scale, m.x), fmaf(o[1], a.scale, m.y)) : make_float2(0.f, 0.f);
+        }
+    };
 
     for (int j = 0; j < nsteps; j++) {
         const int s = j & 1, kb = j % nkb;
-        if (j + 1 < nsteps) {                           // stage s ^ 1 was released at the end of the previous step
-            if (!L.resident) issue_w((j + 1) % nkb, 1, W0 + (s ^ 1) * w_kb, s ^ 1);
-            issue_a(j + 1, s ^ 1);
-            cp_async_wait<1>();
-        } else {
-            cp_async_wait<0>();
-        }
-        __syncthreads();
-        // in-place conversion, 32-byte pieces (8 channels); the four lanes of a row sit in one warp: all read, then write.
-        // Odd rows take their two 16-byte chunks in the opposite order (bank-conflict-free quarter-warps).
-        const uint32_t img = A0 + s * a_buf;
-        const int npiece = L.win * 4;
-        const float slope = a.in_slope;
-        for (int base = 0; base < npiece; base += TC_THREADS) {
-            const int idx = base + tid;
-            const bool live = idx < npiece;
-            const uint32_t odd = (uint32_t)(idx >> 2) & 1u;
-            float4 v0 = make_float4(0.f, 0.f, 0.f, 0.f), v1 = v0;
-            if (live) {
-                const float4 t0 = lds128(img + (uint32_t)idx * 32u + odd * 16u);
-                const float4 t1 = lds128(img + (uint32_t)idx * 32u + 16u - odd * 16u);
-                v0 = odd ? t1 : t0;
-                v1 = odd ? t0 : t1;
-            }
-            __syncwarp();
-            if (live) {
-                const int r = idx >> 2, cc = idx & 3;
-                float e[8] = {v0.x, v0.y, v0.z, v0.w, v1.x, v1.y, v1.z, v1.w};
-                if (slope != 1.f) {
+        const int m_tile = m_first + j / nkb * m_step;
+        const bool last_kb = kb == nkb - 1;
+        float2 rv[2][G], dv[2][G];
+        auto first_group = [&]() {
 #pragma unroll
-                    for (int i = 0; i < 8; i++) e[i] = fmaxf(e[i], e[i] * slope);   // leaky ReLU, 0 < slope < 1
-                }
-                uint4 hi, lo;
-                hi.x = split2(e[0], e[1], lo.x);
-                hi.y = split2(e[2], e[3], lo.y);
-                hi.z = split2(e[4], e[5], lo.z);
-                hi.w = split2(e[6], e[7], lo.w);
-                const uint4 first = odd ? lo : hi, second = odd ? hi : lo;
-                sts128u(sw128(img, r, cc + 4 * (int)odd), first);
-                sts128u(sw128(img, r, cc + 4 - 4 * (int)odd), second);
+            for (int h = 0; h < 2; h++) {
+                const int q = m_tile * 128 + r0 + 8 * h;
+                live[h] = q < a.rows_q;
+                valid[h] = false;
+                bias[h] = live[h] ? conv_row(a, q, valid[h]) : nullptr;
+                orow0[h] = (size_t)q * a.orow_mul + a.orow_add;
             }
-        }
-        __syncthreads();
-        uint32_t wst;
-        if (L.resident) {
-            if (j == 0) mbar_wait<false>(smem_u32(&bars[0]), 0);
-            wst = W0 + kb * w_kb;
-        } else {
-            mbar_wait<false>(smem_u32(&bars[s]), (uint32_t)((j >> 1) & 1));
-            wst = W0 + s * w_kb;
-        }
+            load_group(0, rv[0], dv[0]);
+        };
+        if (EARLY && last_kb && grouped) first_group();
+        mbar_wait<false>(FULL + 8u * s, (uint32_t)((j >> 1) & 1));
+        if (L.resident && j == 0) mbar_wait<false>(WRES, 0);
+        const uint32_t img = A0 + s * a_buf;
+        const uint32_t wst = L.resident ? W0 + kb * w_kb : W0 + s * w_kb;
         auto load_frag = [&](int t, uint32_t (&ah)[2][4], uint32_t (&al)[2][4]) {
             const int R0 = r0 + a.tap_off[t] - a.min_off, R1 = R0 + 8;
 #pragma unroll
@@ -216,86 +308,34 @@ __global__ void __launch_bounds__(TC_THREADS, 2) conv_tc_kernel(const ConvArgs a
             }
             wg_commit();
         };
-        uint32_t ah0[2][4], al0[2][4];
+        // even taps use fragment set 0, odd taps set 1; after a tap is issued, wait_group 1 retires the tap before it,
+        // whose set the next tap reloads.  The issue order per accumulator is (tap, K step, hi*hi, lo*hi, hi*lo).
+        uint32_t ah0[2][4], al0[2][4], ah1[2][4], al1[2][4];
         acc_fence<NT / 2>(acc);
-        if constexpr (NT <= 64) {
-            // even taps use fragment set 0, odd taps set 1; after a tap is issued, wait_group 1 retires the tap before
-            // it, whose set the next tap reloads
-            uint32_t ah1[2][4], al1[2][4];
-            for (int t = 0; t < a.ntaps; t += 2) {
-                load_frag(t, ah0, al0);
-                mma_tap(t, ah0, al0);
+        for (int t = 0; t < a.ntaps; t += 2) {
+            load_frag(t, ah0, al0);
+            mma_tap(t, ah0, al0);
+            wg_wait1();
+            if (t + 1 < a.ntaps) {
+                load_frag(t + 1, ah1, al1);
+                mma_tap(t + 1, ah1, al1);
                 wg_wait1();
-                if (t + 1 < a.ntaps) {
-                    load_frag(t + 1, ah1, al1);
-                    mma_tap(t + 1, ah1, al1);
-                    wg_wait1();
-                }
-            }
-        } else {
-            // one fragment set: a second one does not fit the 128 registers per thread of two CTAs per SM next to the
-            // 64- or 48-register accumulator
-            for (int t = 0; t < a.ntaps; t++) {
-                load_frag(t, ah0, al0);
-                mma_tap(t, ah0, al0);
-                wg_wait0();
             }
         }
         wg_wait0();
         acc_fence<NT / 2>(acc);
-        __syncthreads();                                // stage s fully read: the next step refills it
-        if (kb < nkb - 1) continue;
+        mbar_arrive(EMPTY + 8u * s);                    // stage s fully read: the producer may refill it
+        if (!last_kb) continue;
 
         // ===================== epilogue: thread owns rows r0, r0 + 8 and column pairs 8p + 2c =====================
-        const int m_tile = m_first + j / nkb * m_step;
-        const bool gate = a.act == ACT_GATE;
-        if (NT <= 64 && L.pairs && !gate) {        // (on wider tiles this path costs the registers of a second CTA per SM)
-            // Both columns of a pair on one side of the split (split is even): the per-element rule of the general path,
-            // 8 bytes at a time.  A group of the thread's pairs issues all its global reads before any of them stores: the
-            // compiler may not move a load above a store to a buffer that could alias it, so interleaved, every pair
-            // would wait for a memory round trip of its own.
-            constexpr int NP = NT / 8, G = 4;                     // pairs per row; pairs per read group
-            bool live[2], valid[2];
-            const float* bias[2];
-            size_t orow0[2];
+        if (grouped) {
+            if (!EARLY) first_group();
 #pragma unroll
-            for (int h = 0; h < 2; h++) {
-                const int q = m_tile * 128 + r0 + 8 * h;
-                live[h] = q < a.rows_q;
-                valid[h] = false;
-                bias[h] = live[h] ? conv_row(a, q, valid[h]) : nullptr;
-                orow0[h] = (size_t)q * a.orow_mul + a.orow_add;
-            }
-#pragma unroll
-            for (int k0 = 0; k0 < 2 * NP; k0 += G) {
-                float2 rv[G], dv[G];
-#pragma unroll
-                for (int i = 0; i < G; i++) {
-                    const int h = (k0 + i) / NP, nb = n0 + 8 * ((k0 + i) % NP) + 2 * c;
-                    rv[i] = dv[i] = make_float2(0.f, 0.f);
-                    if (!live[h] || nb >= a.cout || !valid[h]) continue;
-                    const bool lo_side = nb < a.split;
-                    if (a.res) rv[i] = *reinterpret_cast<const float2*>(a.res + orow0[h] * a.ldres + nb);
-                    if (lo_side ? a.acc0 : a.acc1)
-                        dv[i] = *reinterpret_cast<const float2*>(lo_side ? a.y0 + orow0[h] * a.ldy0 + nb
-                                                                         : a.y1 + orow0[h] * a.ldy1 + (nb - a.split));
-                }
-#pragma unroll
-                for (int i = 0; i < G; i++) {
-                    const int h = (k0 + i) / NP, p = (k0 + i) % NP, nb = n0 + 8 * p + 2 * c;
-                    if (!live[h] || nb >= a.cout) continue;
-                    float o[2] = {acc[4 * p + 2 * h], acc[4 * p + 2 * h + 1]};
-                    if (bias[h]) { o[0] += bias[h][nb]; o[1] += bias[h][nb + 1]; }
-                    if (a.act == ACT_RELU) { o[0] = fmaxf(o[0], 0.f); o[1] = fmaxf(o[1], 0.f); }
-                    const bool lo_side = nb < a.split;
-                    const int accum = lo_side ? a.acc0 : a.acc1;
-                    if (accum && !valid[h]) continue;
-                    float2 m = make_float2(0.f, 0.f);
-                    if (a.res && valid[h]) { m.x = rv[i].x * a.scale; m.y = rv[i].y * a.scale; }
-                    if (accum && valid[h]) { m.x += dv[i].x; m.y += dv[i].y; }
-                    *reinterpret_cast<float2*>(lo_side ? a.y0 + orow0[h] * a.ldy0 + nb : a.y1 + orow0[h] * a.ldy1 + (nb - a.split)) =
-                        valid[h] ? make_float2(fmaf(o[0], a.scale, m.x), fmaf(o[1], a.scale, m.y)) : make_float2(0.f, 0.f);
-                }
+            for (int k = 0; k < NG; k++) {
+                const int b = EARLY ? k & 1 : 0;
+                if (EARLY && k + 1 < NG) load_group((k + 1) * G, rv[b ^ 1], dv[b ^ 1]);
+                if (!EARLY && k > 0) load_group(k * G, rv[0], dv[0]);
+                store_group(k * G, rv[b], dv[b]);
             }
         } else {
 #pragma unroll
@@ -312,24 +352,20 @@ __global__ void __launch_bounds__(TC_THREADS, 2) conv_tc_kernel(const ConvArgs a
                     float o[2] = {acc[4 * p + 2 * h], acc[4 * p + 2 * h + 1]};
                     if (bias) { o[0] += bias[nb]; o[1] += bias[nb + 1]; }
                     if (gate) {
-                        // phase-fused ConvTranspose never gates: the pair (2k, 2k+1) gives output column k
+                        // the pair (2k, 2k+1) gives output column k
                         a.y0[orow0 * a.ldy0 + (nb >> 1)] = valid ? tanhf(o[0]) * (1.f / (1.f + expf(-o[1]))) * a.scale : 0.f;
                         continue;
                     }
                     if (a.act == ACT_RELU) { o[0] = fmaxf(o[0], 0.f); o[1] = fmaxf(o[1], 0.f); }
 #pragma unroll
                     for (int e = 0; e < 2; e++) {
-                        // phase-fused ConvTranspose (phase_cols > 0): column block n / phase_cols is the output phase, i.e.
-                        // output row q*u + phase and column n % phase_cols
-                        int n = nb + e;
-                        size_t orow = orow0;
-                        if (a.phase_cols) { orow += (size_t)(n / a.phase_cols); n %= a.phase_cols; }
+                        const int n = nb + e;
                         const bool lo_side = n < a.split;
                         const int accum = lo_side ? a.acc0 : a.acc1;
                         if (accum && !valid) continue;      // accumulated buffers keep their zeros in gap rows
                         float m = 0.f;
-                        if (a.res && valid) m = a.res[orow * a.ldres + n] * a.scale;
-                        float* dst = lo_side ? a.y0 + orow * a.ldy0 + n : a.y1 + orow * a.ldy1 + (n - a.split);
+                        if (a.res && valid) m = a.res[orow0 * a.ldres + n] * a.scale;
+                        float* dst = lo_side ? a.y0 + orow0 * a.ldy0 + n : a.y1 + orow0 * a.ldy1 + (n - a.split);
                         if (accum && valid) m += *dst;
                         *dst = valid ? fmaf(o[e], a.scale, m) : 0.f;
                     }
@@ -344,7 +380,7 @@ __global__ void __launch_bounds__(TC_THREADS, 2) conv_tc_kernel(const ConvArgs a
 // Every K-block's images when resident (nkb <= TC_STAGES: never more than the ring's two stages), else two stages.
 size_t smem_bytes(const ConvArgs& a, int nt, int win, bool resident) {
     const size_t w_kb = (size_t)a.ntaps * nt * 128;
-    return (size_t)TC_STAGES * win * 128 + (resident ? (size_t)(a.cin / 32) : (size_t)TC_STAGES) * w_kb + TC_STAGES * 8;
+    return (size_t)TC_STAGES * win * 128 + (resident ? (size_t)(a.cin / 32) : (size_t)TC_STAGES) * w_kb + TC_BAR_BYTES;
 }
 
 template <int NT> void allow_smem() {
@@ -355,7 +391,7 @@ template <int NT> void allow_smem() {
 template <int NT> int occupancy(size_t smem) {
     allow_smem<NT>();
     int n = 0;
-    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, conv_tc_kernel<NT>, TC_THREADS, smem) != cudaSuccess) {
+    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, conv_tc_kernel<NT>, TcRoles<NT>::threads, smem) != cudaSuccess) {
         cudaGetLastError();
         n = 0;
     }
@@ -363,8 +399,9 @@ template <int NT> int occupancy(size_t smem) {
 }
 
 // CTAs of conv_tc_kernel<nt> with `smem` bytes of dynamic shared memory that fit on one SM: the occupancy API's answer,
-// cached per (nt, smem KB) -- every plan's smem is 16 bytes past a multiple of 1024, so the KB is exact.  Without a
-// device, the bound of the 228 KB of shared memory per SM (1 KB of it reserved per CTA) alone.
+// cached per (nt, smem KB) -- every plan's smem is TC_BAR_BYTES past a multiple of 1024, so the KB is exact.  Without a
+// device, the kernel's register bound (TcRoles::ctas) and that of the 228 KB of shared memory per SM (1 KB of it
+// reserved per CTA).
 int ctas_per_sm(int nt, size_t smem) {
     static int cache[4][256];
     int& slot = cache[nt / 32 - 1][std::min<size_t>(smem >> 10, 255)];
@@ -380,7 +417,8 @@ int ctas_per_sm(int nt, size_t smem) {
         __atomic_store_n(&slot, n, __ATOMIC_RELAXED);
         return n;
     }
-    return std::max(1, std::min(2048 / TC_THREADS, (int)((228u * 1024u) / (smem + 1024))));
+    const int by_regs = nt == 32 ? TcRoles<32>::ctas : TcRoles<128>::ctas;
+    return std::max(1, std::min(by_regs, (int)((228u * 1024u) / (smem + 1024))));
 }
 
 bool aligned8(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 7) == 0; }
@@ -409,14 +447,14 @@ bool plan(const ConvArgs& a, TcLaunch& L, size_t& smem) {
     int grid = wg_num_sms() * ctas_per_sm(L.nt, smem);
     if (g_conv_tc_grid_cap > 0) grid = std::min(grid, g_conv_tc_grid_cap);
     L.grid = std::min(std::max(L.ntiles_n, grid / L.ntiles_n * L.ntiles_n), L.ntiles_m * L.ntiles_n);
-    L.pairs = !a.phase_cols && a.act != ACT_GATE && a.split % 2 == 0 && aligned8(a.y0) && aligned8(a.y1) &&
+    L.pairs = a.act != ACT_GATE && a.split % 2 == 0 && aligned8(a.y0) && aligned8(a.y1) &&
               a.ldy0 % 2 == 0 && a.ldy1 % 2 == 0 && (!a.res || (aligned8(a.res) && a.ldres % 2 == 0));
     return true;
 }
 
 template <int NT> void launch_nt(const ConvArgs& a, const TcLaunch& L, size_t smem, cudaStream_t st) {
     allow_smem<NT>();
-    launch_pdl(conv_tc_kernel<NT>, dim3(L.grid), dim3(TC_THREADS), smem, st, a, L);
+    launch_pdl(conv_tc_kernel<NT>, dim3(L.grid), dim3(TcRoles<NT>::threads), smem, st, a, L);
 }
 
 uint16_t bf16_rn_host(float f) {

@@ -271,7 +271,7 @@ size_t smem_bytes(int win, int ntaps, int nth) {
 
 bool plan(const ConvArgs& a, TfLaunch& L, size_t& smem) {
     if (!a.wtf || a.cin % 32 || a.cout % 32 || a.ntaps < 1 || a.ntaps > SB_MAX_TAPS) return false;
-    if (a.act == ACT_GATE || a.split < a.cout || a.orow_mul != 1 || a.phase_cols) return false;
+    if (a.act == ACT_GATE || a.split < a.cout || a.orow_mul != 1) return false;
     if ((a.ldx & 3) || (reinterpret_cast<uintptr_t>(a.x) & 15)) return false;
     L.nth = L.wnth = tf_nth_for(a.cout, a.ntaps);
     if (!L.nth) return false;

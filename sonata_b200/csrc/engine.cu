@@ -486,16 +486,18 @@ void run_decoder(Runner& R, const Level& LY, const FrameTables& y, const Decoder
         R.begin("dec.up" + std::to_string(i));
         bool fused_done = false;
         if (v.backend >= 1 && st.fused.wtc) {
-            // tensor-core path: all u phases in one launch (input read once, N = u*cout columns)
+            // tensor-core path: all u phases in one launch (input read once, N = u*cout columns).  Column block p of
+            // GEMM row q is output row q*u + p, column n % cout, so with ldy0 = u*cout the output is the GEMM's own
+            // row-major matrix: an ordinary conv.
             ConvArgs pa{};
             pa.x = cur; pa.ldx = st.cin; pa.rows_in = Lin.map.rows; pa.cin = st.cin; pa.in_slope = 0.1f;
             pa.w = nullptr; pa.bias = st.fused.bias; pa.ldw = st.fused.ldw; pa.cout = st.fused.cout;
             pa.wtc = st.fused.wtc; pa.tc_nt = st.fused.tc_nt;
             pa.ntaps = st.fused.ntaps; memcpy(pa.tap_off, st.fused.tap_off, sizeof(pa.tap_off));
             pa.min_off = st.fused.min_off; pa.span = st.fused.span;
-            pa.rows_q = Lin.map.rows; pa.orow_mul = st.u; pa.orow_add = 0; pa.phase_cols = st.cout;
+            pa.rows_q = Lin.map.rows; pa.orow_mul = 1; pa.orow_add = 0;
             pa.map = Lin.map; pa.act = ACT_NONE; pa.scale = 1.f;
-            pa.y0 = up; pa.ldy0 = st.cout; pa.split = st.fused.cout; pa.y1 = up; pa.ldy1 = st.cout;
+            pa.y0 = up; pa.ldy0 = st.fused.cout; pa.split = st.fused.cout; pa.y1 = up; pa.ldy1 = st.fused.cout;
             if (try_launch_conv_tc(pa, R.st)) {
                 const double vr = (double)Lin.valid_rows;
                 R.count(2.0 * vr * st.cin * st.cout * st.k, 4.0 * (vr * (st.cin + (double)st.u * st.cout) + (double)st.cin * st.cout * st.k));

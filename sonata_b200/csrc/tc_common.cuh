@@ -29,6 +29,14 @@ __device__ __forceinline__ void mbar_init(uint32_t bar, uint32_t count) {
 __device__ __forceinline__ void mbar_expect_tx(uint32_t bar, uint32_t bytes) {
     asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(bytes) : "memory");
 }
+// one arrival (release: the thread's earlier shared-memory reads and writes are ordered before the phase completes)
+__device__ __forceinline__ void mbar_arrive(uint32_t bar) {
+    asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory");
+}
+// barrier `id` (1..15) over the `nthreads` threads of some warps of the CTA
+__device__ __forceinline__ void named_bar_sync(int id, int nthreads) {
+    asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
+}
 __device__ __forceinline__ bool mbar_try(uint32_t bar, uint32_t parity) {
     uint32_t ok;
     asm volatile(
@@ -68,6 +76,9 @@ __device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commi
 // generic-proxy shared-memory stores -> visible to the tensor core's operand reads (async proxy)
 __device__ __forceinline__ void fence_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 template <int N> __device__ __forceinline__ void cp_async_wait() { asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory"); }
+// warpgroup-wide register budget change (every thread of the warpgroup executes it)
+template <int N> __device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N)); }
+template <int N> __device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N)); }
 
 // K-major SWIZZLE_128B: row r of an image at r * 128 B, 16-byte chunk c at (c ^ (r & 7)); images start 1024-byte aligned.
 __device__ __forceinline__ uint32_t sw128(uint32_t img, int row, int chunk) {
