@@ -267,6 +267,11 @@ int32_t sb200_job_profile(const sb200_job* job, sb200_region_stat* out, int32_t 
  * rows, 0...}.  Returns 0, or 19 if unsupported. */
 int32_t sb200_debug_plan(int32_t backend, int64_t rows, int32_t cin, int32_t cout, int32_t k, int32_t dil, int32_t act,
                          int32_t has_res, int32_t accumulate, int32_t* out16);
+/* Test hook: the same plan of backend 1, and whether its epilogue operands (residual, accumulated output) are staged in
+ * shared memory while the tile's MMAs run: *staging_bytes is their shared memory per CTA, 0 when not staged.  Returns 0,
+ * or 19 if unsupported. */
+int32_t sb200_debug_plan_staging(int64_t rows, int32_t cin, int32_t cout, int32_t k, int32_t dil, int32_t act,
+                                 int32_t has_res, int32_t accumulate, int32_t* staging_bytes);
 /* Test hook: at most `cap` CTAs per launch of backend 1's persistent conv kernel from now on in this process (0: no cap;
  * the launch still takes one CTA per column tile).  Results do not depend on it.  Returns the previous cap. */
 int32_t sb200_debug_conv_grid_cap(int32_t cap);

@@ -113,6 +113,8 @@ SIGNATURES = {
     "sb200_job_profile": (C.c_int32, [_P, C.POINTER(sb200_region_stat), C.c_int32]),
     "sb200_debug_plan": (C.c_int32, [C.c_int32, C.c_int64, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
                                       C.c_int32, C.POINTER(C.c_int32)]),
+    "sb200_debug_plan_staging": (C.c_int32, [C.c_int64, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
+                                              C.c_int32, C.c_int32, C.POINTER(C.c_int32)]),
     "sb200_debug_conv_grid_cap": (C.c_int32, [C.c_int32]),
     "sb200_debug_conv": (C.c_int32, [C.c_int32, C.c_int32, C.POINTER(C.c_float), C.c_int32, C.c_int32,
                                      C.POINTER(C.c_float), C.POINTER(C.c_float), C.c_int32, C.c_int32, C.c_int32,

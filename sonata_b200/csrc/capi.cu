@@ -489,8 +489,8 @@ int32_t sb200_job_profile(const sb200_job* job, sb200_region_stat* out, int32_t 
     }
     return n;
 }
-int32_t sb200_debug_plan(int32_t backend, int64_t rows, int32_t cin, int32_t cout, int32_t k, int32_t dil, int32_t act,
-                         int32_t has_res, int32_t accumulate, int32_t* out16) {
+static int32_t debug_plan(int32_t backend, int64_t rows, int32_t cin, int32_t cout, int32_t k, int32_t dil, int32_t act,
+                          int32_t has_res, int32_t accumulate, int32_t* out16, int32_t* staging_bytes) {
     // Planning only: nothing is allocated or launched, so this also runs where there is no GPU (host-logic tests); tensor
     // maps are assumed available, as on any sm_90+ driver.  Buffers are described by stand-in addresses (the planners look
     // at alignment only).  Layer conventions as in sb200_debug_conv / the engine's ResBlock and flow layers.
@@ -510,8 +510,18 @@ int32_t sb200_debug_plan(int32_t backend, int64_t rows, int32_t cin, int32_t cou
     p.rows_q = R; p.orow_mul = 1; p.orow_add = 0;
     p.act = act; p.scale = 1.f; p.res = has_res ? stand_in : nullptr; p.ldres = cout;
     p.y0 = stand_in; p.ldy0 = ycols; p.acc0 = accumulate; p.split = cout; p.y1 = stand_in; p.ldy1 = ycols; p.acc1 = accumulate;
-    const bool ok = backend == 2 ? conv_tf_plan_info(p, out16) : conv_tc_plan_info(p, out16);
+    const bool ok = backend == 2 ? conv_tf_plan_info(p, out16) : conv_tc_plan_info(p, out16, staging_bytes);
     return ok ? 0 : 19;
+}
+int32_t sb200_debug_plan(int32_t backend, int64_t rows, int32_t cin, int32_t cout, int32_t k, int32_t dil, int32_t act,
+                         int32_t has_res, int32_t accumulate, int32_t* out16) {
+    return debug_plan(backend, rows, cin, cout, k, dil, act, has_res, accumulate, out16, nullptr);
+}
+int32_t sb200_debug_plan_staging(int64_t rows, int32_t cin, int32_t cout, int32_t k, int32_t dil, int32_t act,
+                                 int32_t has_res, int32_t accumulate, int32_t* staging_bytes) {
+    int32_t out16[16];
+    if (!staging_bytes) return 19;
+    return debug_plan(1, rows, cin, cout, k, dil, act, has_res, accumulate, out16, staging_bytes);
 }
 
 int32_t sb200_debug_conv_grid_cap(int32_t cap) {

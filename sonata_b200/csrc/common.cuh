@@ -136,7 +136,8 @@ inline void launch_pdl(void (*kern)(KArgs...), dim3 grid, dim3 block, size_t sme
 void launch_conv_simt(const ConvArgs& a, cudaStream_t st);
 int conv_simt_bn_for(int cout);
 bool conv_tc_supported(const ConvArgs& a);
-bool conv_tc_plan_info(const ConvArgs& a, int* out16);     // planning only, see sb200_debug_plan
+// planning only, see sb200_debug_plan; *staging_bytes: the staged epilogue operands' shared memory (0: not staged)
+bool conv_tc_plan_info(const ConvArgs& a, int* out16, int* staging_bytes = nullptr);
 void launch_conv_tc(const ConvArgs& a, cudaStream_t st);
 bool try_launch_conv_tc(const ConvArgs& a, cudaStream_t st);
 extern int g_conv_tc_grid_cap;     // at most this many CTAs per conv_tc launch (0: no cap); see sb200_debug_conv_grid_cap

@@ -32,13 +32,20 @@
 //     run, wait_group 1).  The issue order per accumulator is (K-block, tap, K step, hi*hi, lo*hi, hi*lo), so every
 //     output keeps its bits.  Once a step's MMAs have retired, the MMA warpgroups arrive on the stage's empty barrier,
 //     before the epilogue, so the producer refills it while they store;
+//   * staged epilogue operands: on tiles wider than 32 columns, where they fit beside the ring at the same tile width
+//     and CTAs per SM, the producers
+//     also fetch each tile's residual and accumulated output (16-byte cp.async into one SWIZZLE_128B image per 32
+//     columns, rows past the array zero-filled) while the MMA warpgroups run the tile's MMAs.  They complete on a
+//     barrier of their own (cp.async.mbarrier.arrive), and the MMA warpgroups release the buffer on another once they
+//     hold the operands in registers, before they store;
 //   * epilogue: bias / gate / ReLU / residual / scale / accumulate straight from the accumulator registers; a column
-//     pair is one 8-byte access where the output layout allows it, and groups of pairs issue their residual /
-//     accumulated reads before any of them stores.  On tiles wider than 32 columns the first group's reads are issued
-//     before the tile's last K-block runs its MMAs.
+//     pair is one 8-byte access where the output layout allows it.  Staged launches read the operands from shared
+//     memory; the others issue a group of pairs' global reads before any of them stores (on tiles wider than 32
+//     columns the first group's before the tile's last K-block runs its MMAs).
 // Registers (setmaxnreg): 32-column tiles run 2 CTAs per SM at 80 registers per thread, the producer dropping to 40 and
 // the MMA warpgroups rising to 96; wider tiles run one CTA per SM at 128, split 32 (two producer warpgroups) / 224.
-// -Xptxas -v: no spills at any NT.
+// -Xptxas -v: no spills at NT = 32; 24 / 44 bytes of spill stores / loads at NT >= 64 (loop-invariant values, reloaded
+// from L1).
 // Every mbarrier wait carries a watchdog that traps instead of hanging the GPU.
 #include "tc_common.cuh"
 #include <algorithm>
@@ -73,11 +80,26 @@ struct TcLaunch {
     int grid;        // CTAs: a multiple of ntiles_n, at most ntiles_m * ntiles_n
     int resident;    // 1: every weight image of the CTA's n-tile stays in shared memory; 0: one K-block per ring stage
     int pairs;       // 1: a column pair may be one 8-byte access to res / y0 / y1 (aligned, no gate)
+    int stage;       // 1: the producers stage each tile's residual / accumulated output in shared memory (needs pairs)
 };
 
 constexpr int TC_CONSUMERS = 256;       // two MMA warpgroups: tile rows [0, 64) and [64, 128)
 constexpr int TC_STAGES = 2;
-constexpr int TC_BAR_BYTES = 64;        // full[TC_STAGES], empty[TC_STAGES], resident weights
+// full[TC_STAGES], empty[TC_STAGES], resident weights, staging full / free.  They live in the 1024 bytes of alignment
+// slack (before the aligned base when it leaves room, else after the data), so they take no shared memory of their own.
+constexpr int TC_BAR_BYTES = 64;
+
+// Staged epilogue operand: 128 rows x nt fp32, one 16 KB SWIZZLE_128B image per 32 columns.  Element (r, col) at
+// sw128(slab col / 32, r, (col % 32) / 4) + 4 (col % 4): the epilogue's float2 reads (rows g / g + 8, columns 8p + 2c)
+// of a warp hit distinct banks, where a linear [128][nt] tile would be 4-way conflicted.
+__device__ __forceinline__ uint32_t stg_addr(uint32_t base, int row, int col) {
+    return sw128(base + (uint32_t)(col >> 5) * 16384u, row, (col >> 2) & 7) + 4u * (uint32_t)(col & 3);
+}
+// v, through a move the compiler cannot hoist out of a loop
+__device__ __forceinline__ uint32_t opaque(uint32_t v) {
+    asm volatile("mov.b32 %0, %0;" : "+r"(v));
+    return v;
+}
 
 // Roles and register split per tile width.  32-column tiles run 2 CTAs per SM (their shared memory would allow more;
 // registers decide) with one producer warpgroup: 80 registers at launch -> producer 40 / MMA warpgroups 96.  Wider tiles
@@ -97,16 +119,24 @@ __global__ void __launch_bounds__(TcRoles<NT>::threads, TcRoles<NT>::ctas) conv_
     constexpr int NPROD = TcRoles<NT>::producers;
     pdl_trigger();
     extern __shared__ __align__(1024) uint8_t smem_raw[];
-    uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
     const int nkb = a.cin / 32, S = TC_STAGES;
+    const bool acc_any = a.acc0 || a.acc1;
+    const bool stage = NT > 32 && L.stage;                       // the planner stages wider tiles only
     const uint32_t a_buf = (uint32_t)L.win * 128u;               // one window image
     const uint32_t w_tap = (uint32_t)NT * 128u;                  // one tap of a weight image ([hi|lo] rows)
     const uint32_t w_kb = (uint32_t)a.ntaps * w_tap;             // the taps of one K-block
     const uint32_t w_bytes = L.resident ? (uint32_t)nkb * w_kb : (uint32_t)S * w_kb;
-    const uint32_t A0 = smem_u32(smem), W0 = A0 + S * a_buf;
-    const uint32_t FULL = A0 + S * a_buf + w_bytes;              // full[s]: stage s converted (and its weights landed)
+    const uint32_t stg_op = 128u * NT * 4u;                      // one staged epilogue operand
+    const uint32_t raw = smem_u32(smem_raw), A0 = (raw + 1023u) & ~1023u, W0 = A0 + S * a_buf;
+    const uint32_t SRES = W0 + w_bytes;                          // staged residual
+    const uint32_t SACC = SRES + (stage && a.res ? stg_op : 0u);   // staged accumulated output
+    const uint32_t data_end = SACC + (stage && acc_any ? stg_op : 0u);
+    const uint32_t FULL = A0 - raw >= (uint32_t)TC_BAR_BYTES ? raw : data_end;   // full[s]: stage s converted (and its
+                                                                                  // weights landed)
     const uint32_t EMPTY = FULL + 8u * TC_STAGES;                // empty[s]: both MMA warpgroups done reading stage s
     const uint32_t WRES = EMPTY + 8u * TC_STAGES;                // resident weights landed
+    const uint32_t SFULL = WRES + 8u;                            // a tile's epilogue operands landed
+    const uint32_t SFREE = SFULL + 8u;                           // the MMA warpgroups hold them in registers
     const int tid = threadIdx.x;
     const int n_tile = (int)blockIdx.x % L.ntiles_n, m_first = (int)blockIdx.x / L.ntiles_n;
     const int m_step = (int)gridDim.x / L.ntiles_n;
@@ -119,6 +149,8 @@ __global__ void __launch_bounds__(TcRoles<NT>::threads, TcRoles<NT>::ctas) conv_
             mbar_init(EMPTY + 8u * s, TC_CONSUMERS);
         }
         mbar_init(WRES, 1);
+        mbar_init(SFULL, NPROD);                                  // one cp.async arrival per producer thread
+        mbar_init(SFREE, TC_CONSUMERS);
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
     __syncthreads();
@@ -151,6 +183,33 @@ __global__ void __launch_bounds__(TcRoles<NT>::threads, TcRoles<NT>::ctas) conv_
             }
             cp_async_commit();
         };
+        // epilogue operands of the CTA's tile t, once the MMA warpgroups have taken tile t - 1's: 16-byte pieces of the
+        // residual and of the accumulated output (columns < split from y0 when acc0, >= split from y1 when acc1), rows
+        // past the array and sides that are not accumulated zero-filled; completion on SFULL
+        // A thread keeps one 16-byte column piece and walks the rows (NT = 96: 240 of the 256 threads, 10 rows a pass).
+        // Its per-thread values are recomputed per tile from an opaque copy of ptid: the producers' 32 / 40 registers do
+        // not hold them across the window loop.
+        constexpr int CPR = NT / 4, RSTEP = NPROD / CPR;     // pieces per row; rows per pass
+        auto issue_stage = [&](int t) {
+            if (t > 0) mbar_wait<false>(SFREE, (uint32_t)((t - 1) & 1));
+            const int pt = (int)opaque((uint32_t)ptid);
+            if (pt < RSTEP * CPR) {
+                const int col = 4 * (pt % CPR), nb = n_tile * NT + col;
+                const bool lo_side = nb < a.split;
+                const bool rd_res = a.res && nb < a.cout, rd_acc = (lo_side ? a.acc0 : a.acc1) && nb < a.cout;
+                const float* acc_src = lo_side ? a.y0 + nb : a.y1 + (nb - a.split);
+                const int ld_acc = lo_side ? a.ldy0 : a.ldy1;
+                for (int r = pt / CPR; r < 128; r += RSTEP) {
+                    const int q = (m_first + t * m_step) * 128 + r;
+                    const size_t orow = (size_t)q * a.orow_mul + a.orow_add;
+                    const bool ok_res = rd_res && q < a.rows_q, ok_acc = rd_acc && q < a.rows_q;
+                    if (a.res) cp_async16(stg_addr(SRES, r, col), ok_res ? a.res + nb + orow * a.ldres : a.x, ok_res ? 16u : 0u);
+                    if (acc_any) cp_async16(stg_addr(SACC, r, col), ok_acc ? acc_src + orow * ld_acc : a.x, ok_acc ? 16u : 0u);
+                }
+            }
+            cp_async_commit();
+            cp_async_mbar_arrive(SFULL);
+        };
 
         // weights are constants: fetched before the predecessor finishes
         if (L.resident) issue_w(0, nkb, W0, WRES);
@@ -158,13 +217,20 @@ __global__ void __launch_bounds__(TcRoles<NT>::threads, TcRoles<NT>::ctas) conv_
         pdl_wait();
 
         // Step j refills stage j % 2 once the MMA warpgroups have released it (step j - 2), and loads and converts it
-        // while they run step j - 1.
+        // while they run step j - 1.  Tile t's epilogue operands are issued at step t * nkb + 1, after that step's window
+        // (so they never hold it up), when tile t - 1's epilogue has just taken its operands: they land while tile t's
+        // MMAs run.  With one K-block per tile, the last tile's go out after the loop.
         for (int j = 0; j < nsteps; j++) {
             const int s = j & 1;
             if (j >= S) mbar_wait<false>(EMPTY + 8u * s, (uint32_t)((j / S - 1) & 1));
             if (!L.resident && j > 0) issue_w(j % nkb, 1, W0 + s * w_kb, FULL + 8u * s);
             issue_a(j, s);
-            cp_async_wait<0>();
+            if (stage && j > 0 && (j - 1) % nkb == 0) {
+                issue_stage((j - 1) / nkb);
+                cp_async_wait<1>();              // the window; the staged operands complete on SFULL
+            } else {
+                cp_async_wait<0>();
+            }
             named_bar_sync(1, NPROD);            // every producer's part of the window has landed
             // in-place conversion, 32-byte pieces (8 channels); the four lanes of a row sit in one warp: all read, then
             // write.  Odd rows take their two 16-byte chunks in the opposite order (bank-conflict-free quarter-warps).
@@ -202,6 +268,8 @@ __global__ void __launch_bounds__(TcRoles<NT>::threads, TcRoles<NT>::ctas) conv_
             }
             mbar_arrive(FULL + 8u * s);
         }
+        if (stage && nkb == 1) issue_stage(nsteps - 1);
+        cp_async_wait<0>();
         return;
     }
 
@@ -222,9 +290,11 @@ __global__ void __launch_bounds__(TcRoles<NT>::threads, TcRoles<NT>::ctas) conv_
     // general path 8 bytes at a time.  A group of the thread's pairs issues all its global reads before any of them
     // stores: the compiler may not move a load above a store to a buffer that could alias it, so interleaved, every
     // pair would wait for a memory round trip of its own.  On tiles wider than 32 columns, the first group's reads go out
-    // before the tile's last K-block runs its MMAs, and each later group's before the previous group stores.
+    // before the tile's last K-block runs its MMAs, and each later group's before the previous group stores.  Staged
+    // launches (L.stage) take a group's operands from the staging buffer the producers filled during the MMAs instead.
     constexpr int NP = NT / 8, G = NT == 32 ? 4 : 8, NG = 2 * NP / G;   // pairs per row; pairs per group; groups
     constexpr bool EARLY = NT > 32;     // at 2 CTAs per SM (96 registers), one group's reads at a time, after the MMAs
+    const bool early = EARLY && grouped && !stage;
     bool live[2], valid[2];
     const float* bias[2];
     size_t orow0[2];
@@ -239,6 +309,19 @@ __global__ void __launch_bounds__(TcRoles<NT>::threads, TcRoles<NT>::ctas) conv_
             if (lo_side ? a.acc0 : a.acc1)
                 dv[i] = *reinterpret_cast<const float2*>(lo_side ? a.y0 + orow0[h] * a.ldy0 + nb
                                                                  : a.y1 + orow0[h] * a.ldy1 + (nb - a.split));
+        }
+    };
+    // stg_addr(base, r0 + 8h, 8p + 2c) = base + thread part + (h, p, g >> 1) part.  The thread part and g >> 1 pass
+    // through an opaque move per tile (`opaque`), so the compiler computes each pair's address where it is read instead
+    // of keeping all of them in registers across the tile loop.
+    const uint32_t stg_thread = (uint32_t)r0 * 128u + ((uint32_t)((c >> 1) ^ (g & 1)) << 4) + 8u * (uint32_t)(c & 1);
+    auto lds_group = [&](int k0, uint32_t thr, uint32_t gh, float2 (&rv)[G], float2 (&dv)[G]) {
+#pragma unroll
+        for (int i = 0; i < G; i++) {
+            const int h = (k0 + i) / NP, p = (k0 + i) % NP;
+            const uint32_t off = thr + (uint32_t)(p >> 2) * 16384u + (uint32_t)h * 1024u + (((uint32_t)(p & 3) ^ gh) << 5);
+            if (a.res) rv[i] = lds64(SRES + off);
+            if (acc_any) dv[i] = lds64(SACC + off);
         }
     };
     auto store_group = [&](int k0, const float2 (&rv)[G], const float2 (&dv)[G]) {
@@ -265,7 +348,7 @@ __global__ void __launch_bounds__(TcRoles<NT>::threads, TcRoles<NT>::ctas) conv_
         const int m_tile = m_first + j / nkb * m_step;
         const bool last_kb = kb == nkb - 1;
         float2 rv[2][G], dv[2][G];
-        auto first_group = [&]() {
+        auto rows_of_tile = [&]() {
 #pragma unroll
             for (int h = 0; h < 2; h++) {
                 const int q = m_tile * 128 + r0 + 8 * h;
@@ -274,9 +357,11 @@ __global__ void __launch_bounds__(TcRoles<NT>::threads, TcRoles<NT>::ctas) conv_
                 bias[h] = live[h] ? conv_row(a, q, valid[h]) : nullptr;
                 orow0[h] = (size_t)q * a.orow_mul + a.orow_add;
             }
-            load_group(0, rv[0], dv[0]);
         };
-        if (EARLY && last_kb && grouped) first_group();
+        if (early && last_kb) {
+            rows_of_tile();
+            load_group(0, rv[0], dv[0]);
+        }
         mbar_wait<false>(FULL + 8u * s, (uint32_t)((j >> 1) & 1));
         if (L.resident && j == 0) mbar_wait<false>(WRES, 0);
         const uint32_t img = A0 + s * a_buf;
@@ -328,8 +413,21 @@ __global__ void __launch_bounds__(TcRoles<NT>::threads, TcRoles<NT>::ctas) conv_
         if (!last_kb) continue;
 
         // ===================== epilogue: thread owns rows r0, r0 + 8 and column pairs 8p + 2c =====================
-        if (grouped) {
-            if (!EARLY) first_group();
+        if (grouped && stage) {
+            rows_of_tile();
+            mbar_wait<false>(SFULL, (uint32_t)((j / nkb) & 1));
+            const uint32_t thr = opaque(stg_thread), gh = opaque((uint32_t)g >> 1);
+#pragma unroll
+            for (int k = 0; k < NG; k++) {
+                lds_group(k * G, thr, gh, rv[0], dv[0]);
+                if (k == NG - 1) mbar_arrive(SFREE);    // the producers may stage the next tile
+                store_group(k * G, rv[0], dv[0]);
+            }
+        } else if (grouped) {
+            if (!EARLY) {
+                rows_of_tile();
+                load_group(0, rv[0], dv[0]);
+            }
 #pragma unroll
             for (int k = 0; k < NG; k++) {
                 const int b = EARLY ? k & 1 : 0;
@@ -377,10 +475,12 @@ __global__ void __launch_bounds__(TcRoles<NT>::threads, TcRoles<NT>::ctas) conv_
     }
 }
 
-// Every K-block's images when resident (nkb <= TC_STAGES: never more than the ring's two stages), else two stages.
-size_t smem_bytes(const ConvArgs& a, int nt, int win, bool resident) {
+// Two window stages; every K-block's images when resident (nkb <= TC_STAGES: never more than the ring's two stages),
+// else two stages; `staged` epilogue operands.  The barriers sit in the alignment slack.
+size_t smem_bytes(const ConvArgs& a, int nt, int win, bool resident, int staged) {
     const size_t w_kb = (size_t)a.ntaps * nt * 128;
-    return (size_t)TC_STAGES * win * 128 + (resident ? (size_t)(a.cin / 32) : (size_t)TC_STAGES) * w_kb + TC_BAR_BYTES;
+    return (size_t)TC_STAGES * win * 128 + (resident ? (size_t)(a.cin / 32) : (size_t)TC_STAGES) * w_kb +
+           (size_t)staged * 128 * nt * 4;
 }
 
 template <int NT> void allow_smem() {
@@ -399,7 +499,7 @@ template <int NT> int occupancy(size_t smem) {
 }
 
 // CTAs of conv_tc_kernel<nt> with `smem` bytes of dynamic shared memory that fit on one SM: the occupancy API's answer,
-// cached per (nt, smem KB) -- every plan's smem is TC_BAR_BYTES past a multiple of 1024, so the KB is exact.  Without a
+// cached per (nt, smem KB) -- every plan's smem is a multiple of 1024, so the KB is exact.  Without a
 // device, the kernel's register bound (TcRoles::ctas) and that of the 228 KB of shared memory per SM (1 KB of it
 // reserved per CTA).
 int ctas_per_sm(int nt, size_t smem) {
@@ -422,6 +522,16 @@ int ctas_per_sm(int nt, size_t smem) {
 }
 
 bool aligned8(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 7) == 0; }
+bool aligned16(const void* p, int ld) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0 && ld % 4 == 0; }
+
+// Epilogue operands the producers can stage in 16-byte pieces: 0 (nothing to read, gate, or misaligned), 1 or 2.
+int staged_operands(const ConvArgs& a, const TcLaunch& L) {
+    const bool acc = a.acc0 || a.acc1;
+    if (!L.pairs || (!a.res && !acc) || a.split % 4) return 0;
+    if (a.res && !aligned16(a.res, a.ldres)) return 0;
+    if ((a.acc0 && !aligned16(a.y0, a.ldy0)) || (a.acc1 && !aligned16(a.y1, a.ldy1))) return 0;
+    return (a.res ? 1 : 0) + (acc ? 1 : 0);
+}
 
 bool plan(const ConvArgs& a, TcLaunch& L, size_t& smem) {
     if (!a.wtc || a.tc_nt <= 0 || a.tc_nt > 128 || a.tc_nt % 32) return false;
@@ -433,7 +543,7 @@ bool plan(const ConvArgs& a, TcLaunch& L, size_t& smem) {
     // an utterance comes out bit-identical whether it is synthesised alone or in a batch.
     L.nt = 0;
     for (int nt = a.tc_nt; nt >= 32; nt -= 32)
-        if (a.tc_nt % nt == 0 && smem_bytes(a, nt, L.win, false) <= WG_SMEM_BUDGET) { L.nt = nt; break; }
+        if (a.tc_nt % nt == 0 && smem_bytes(a, nt, L.win, false, 0) <= WG_SMEM_BUDGET) { L.nt = nt; break; }
     if (!L.nt) return false;
     if (a.cout % a.tc_nt == 0)
         for (int nt = 32; nt < L.nt; nt += 32)
@@ -441,14 +551,21 @@ bool plan(const ConvArgs& a, TcLaunch& L, size_t& smem) {
     L.ntiles_m = mt;
     L.ntiles_n = (a.cout + L.nt - 1) / L.nt;
     L.resident = a.cin / 32 <= TC_STAGES;
-    smem = smem_bytes(a, L.nt, L.win, L.resident) + 1024;
+    L.pairs = a.act != ACT_GATE && a.split % 2 == 0 && aligned8(a.y0) && aligned8(a.y1) &&
+              a.ldy0 % 2 == 0 && a.ldy1 % 2 == 0 && (!a.res || (aligned8(a.res) && a.ldres % 2 == 0));
+    smem = smem_bytes(a, L.nt, L.win, L.resident, 0) + 1024;
+    // Staged epilogue operands only where they fit beside the ring at the same tile width and CTAs per SM, and only on
+    // tiles wider than 32 columns: two 32-column CTAs per SM with staging take 227 of the SM's 228 KB of shared memory,
+    // which leaves the smallest L1 carve-out, and the 32-channel ResBlocks ran 3-7 % slower staged (DESIGN.md section 3).
+    const int nst = staged_operands(a, L);
+    const size_t staged = smem_bytes(a, L.nt, L.win, L.resident, nst) + 1024;
+    L.stage = L.nt > 32 && nst > 0 && staged - 1024 <= WG_SMEM_BUDGET && ctas_per_sm(L.nt, staged) == ctas_per_sm(L.nt, smem);
+    if (L.stage) smem = staged;
     // Persistent grid: every CTA that fits at once, rounded down to whole m-tiles (a CTA keeps its n-tile); a launch of
     // no more tiles than that runs one tile per CTA.
     int grid = wg_num_sms() * ctas_per_sm(L.nt, smem);
     if (g_conv_tc_grid_cap > 0) grid = std::min(grid, g_conv_tc_grid_cap);
     L.grid = std::min(std::max(L.ntiles_n, grid / L.ntiles_n * L.ntiles_n), L.ntiles_m * L.ntiles_n);
-    L.pairs = a.act != ACT_GATE && a.split % 2 == 0 && aligned8(a.y0) && aligned8(a.y1) &&
-              a.ldy0 % 2 == 0 && a.ldy1 % 2 == 0 && (!a.res || (aligned8(a.res) && a.ldres % 2 == 0));
     return true;
 }
 
@@ -469,12 +586,13 @@ float bf16_to_float_host(uint16_t h) {
 }  // namespace
 
 // planning only (no launch): the configuration the launcher would choose; see sb200_debug_plan
-bool conv_tc_plan_info(const ConvArgs& a, int* out) {
+bool conv_tc_plan_info(const ConvArgs& a, int* out, int* staging_bytes) {
     TcLaunch L{}; size_t smem = 0;
     if (a.cin % 32 || a.cout % 32 || a.ntaps > SB_MAX_TAPS || !plan(a, L, smem)) return false;
     const int v[16] = {L.nt, L.wnt, L.ntiles_m, L.ntiles_n, TC_STAGES, (int)smem, L.win, L.grid, L.resident,
                        ctas_per_sm(L.nt, smem), 0, 0, 0, 0, 0, 0};
     for (int i = 0; i < 16; i++) out[i] = v[i];
+    if (staging_bytes) *staging_bytes = L.stage ? staged_operands(a, L) * 128 * L.nt * 4 : 0;
     return true;
 }
 
