@@ -417,6 +417,7 @@ struct DecoderBufs {
 struct FrameBufs {
     FrameTables y;
     float *s, *epsz, *zp, *h, *acts, *outb, *wav;
+    std::vector<float*> flow;                  // debug: z after each coupling layer, in the engine's channel order
     DecoderBufs dec;
     void carve(Arena& dev, Arena& pin, const Job& j, bool own_wav) {
         const Arch& a = j.v->a;
@@ -427,6 +428,8 @@ struct FrameBufs {
         for (const SynthConfig& c : j.cfgs) any_noise |= c.noise_scale != 0.f;
         epsz = any_noise ? dev.get<float>(RY * a.inter) : nullptr;
         zp = j.debug ? dev.get<float>(RY * a.inter) : nullptr;
+        flow.assign(j.debug ? j.v->flows.size() : 0, nullptr);
+        for (auto& p : flow) p = dev.get<float>(RY * a.inter);
         h = dev.get<float>(RY * a.hidden); acts = dev.get<float>(RY * a.hidden); outb = dev.get<float>(RY * a.hidden);
         wav = nullptr;
         if (j.encode_only) return;
@@ -817,6 +820,10 @@ void Job::run(float* d_out, size_t d_out_cap) {
     d_fsegs = f.y.fsegs;
     if (debug) {
         expose(*this, "z_p", f.zp, I, 1); expose(*this, "z", f.s, I, 1);
+        // flow.{f}: z after the coupling layer of the graph's flow.flows.{2f} (f = flow_n - 1 first).  The graph's Flip
+        // layers are folded into the weights, so z keeps z_p's channel order throughout: after an odd number of
+        // couplings the graph's z is this capture reversed along channels, after an even number it is the capture.
+        for (size_t s = 0; s < f.flow.size(); s++) expose(*this, "flow." + std::to_string(a.flow_n - 1 - (int)s), f.flow[s], I, 1);
         if (!encode_only) f.dec.expose_to(*this);
     }
     Level LY = upload_frames(*this, f.y, st);
@@ -841,7 +848,8 @@ void Job::run(float* d_out, size_t d_out_cap) {
 
     // ---------------- residual-coupling flow (reverse) ----------------
     R.begin("flow");
-    for (const CouplingW& cp : V.flows) {
+    for (size_t step = 0; step < V.flows.size(); step++) {
+        const CouplingW& cp = V.flows[step];
         { Runner::Opt o; o.y0 = f.h; o.ldy0 = H; o.tc_ok = true; R.conv(cp.pre, f.s + cp.cond_off, I, LY, o); }
         const int n = (int)cp.in.size();
         for (int l = 0; l < n; l++) {
@@ -852,6 +860,7 @@ void Job::run(float* d_out, size_t d_out_cap) {
             R.conv(cp.rs[l], f.acts, H, LY, o);
         }
         { Runner::Opt o; o.y0 = f.s + cp.tgt_off; o.ldy0 = I; o.acc0 = 1; o.scale = -1.f; o.tc_ok = true; R.conv(cp.post, f.outb, H, LY, o); }
+        if (debug) d2d(f.flow[step], f.s, (size_t)RY * I, st);
     }
     R.end();
 
