@@ -110,6 +110,28 @@ double now_ms() {
     return std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now().time_since_epoch()).count();
 }
 
+// Device buffers of one debug hook call, freed however the call ends (an SB_CUDA that throws included).
+struct DeviceBuffers {
+    std::vector<void*> ptrs;
+    DeviceBuffers() = default;
+    DeviceBuffers(const DeviceBuffers&) = delete;
+    DeviceBuffers& operator=(const DeviceBuffers&) = delete;
+    ~DeviceBuffers() { for (void* p : ptrs) cudaFree(p); }
+    template <typename T> T* alloc(size_t n) {
+        void* p = nullptr;
+        SB_CUDA(cudaMalloc(&p, n * sizeof(T)));
+        ptrs.push_back(p);
+        return static_cast<T*>(p);
+    }
+    // n elements: the m of host array h, then zeros
+    template <typename T> T* upload(const T* h, size_t m, size_t n) {
+        T* d = alloc<T>(n);
+        if (n > m) SB_CUDA(cudaMemset(d, 0, n * sizeof(T)));
+        SB_CUDA(cudaMemcpy(d, h, m * sizeof(T), cudaMemcpyHostToDevice));
+        return d;
+    }
+};
+
 }  // namespace
 
 extern "C" {
@@ -497,19 +519,15 @@ static int32_t debug_plan(int32_t backend, int64_t rows, int32_t cin, int32_t co
     if (!out16 || cin <= 0 || cout <= 0 || k <= 0 || k > SB_MAX_TAPS || dil <= 0 || rows <= 0) return 19;
     static float anchor[64];
     float* const stand_in = reinterpret_cast<float*>((reinterpret_cast<uintptr_t>(anchor) + 127) & ~(uintptr_t)127);
-    ConvArgs p{};
+    ConvW w = conv_layout(cin, cout, centred_taps(k, dil), false);
+    w.w = w.bias = w.wtf = stand_in;
+    w.tc_nt = tc_tile_for(cout);
+    w.wtc = w.tc_nt ? stand_in : nullptr;
     const int R = (int)((rows + 255) / 256 * 256);
-    const int ycols = act == ACT_GATE ? cout / 2 : cout;
-    p.x = stand_in; p.ldx = cin; p.rows_in = R; p.cin = cin; p.in_slope = 0.1f;
-    p.w = stand_in; p.bias = stand_in; p.ldw = cout; p.cout = cout;
-    p.tc_nt = cout <= 128 ? cout : (cout % 128 == 0 ? 128 : (cout % 96 == 0 ? 96 : 0));      // voice.cu tc_tile_for
-    p.wtc = p.tc_nt ? stand_in : nullptr; p.wtf = stand_in;
-    p.ntaps = k;
-    for (int t = 0; t < k; t++) p.tap_off[t] = (t - (k - 1) / 2) * dil;
-    p.min_off = p.tap_off[0]; p.span = (k - 1) * dil;
-    p.rows_q = R; p.orow_mul = 1; p.orow_add = 0;
-    p.act = act; p.scale = 1.f; p.res = has_res ? stand_in : nullptr; p.ldres = cout;
-    p.y0 = stand_in; p.ldy0 = ycols; p.acc0 = accumulate; p.split = cout; p.y1 = stand_in; p.ldy1 = ycols; p.acc1 = accumulate;
+    ConvCall c;
+    c.in_slope = 0.1f; c.act = act; c.res = has_res ? stand_in : nullptr; c.ldres = cout;
+    c.y0 = c.y1 = stand_in; c.ldy0 = c.ldy1 = act == ACT_GATE ? cout / 2 : cout; c.acc0 = c.acc1 = accumulate;
+    const ConvArgs p = conv_args(w, stand_in, cin, RowMap{nullptr, R, 1, R}, c);
     const bool ok = backend == 2 ? conv_tf_plan_info(p, out16) : conv_tc_plan_info(p, out16, staging_bytes);
     return ok ? 0 : 19;
 }
@@ -547,45 +565,26 @@ int32_t sb200_debug_conv_ex(int32_t device, int32_t backend, const float* x, int
         const int ngran = (R + gran - 1) / gran;
         std::vector<int> ends(ngran, 0);                                // granules past the caller's table: all gap rows
         for (int g = 0; g < ngran && g * gran < rows; g++) ends[g] = seg_end[g];
-        float *dx, *dy0 = nullptr, *dy1 = nullptr, *dres = nullptr; int* dend;
-        SB_CUDA(cudaMalloc(&dx, (size_t)R * cin * 4)); SB_CUDA(cudaMemset(dx, 0, (size_t)R * cin * 4));
-        SB_CUDA(cudaMemcpy(dx, x, (size_t)rows * cin * 4, cudaMemcpyHostToDevice));
-        auto upload_y = [&](float*& d, const float* h, int ld) {
-            if (ld <= 0) return;
-            SB_CUDA(cudaMalloc(&d, (size_t)R * ld * 4)); SB_CUDA(cudaMemset(d, 0, (size_t)R * ld * 4));
-            SB_CUDA(cudaMemcpy(d, h, (size_t)rows * ld * 4, cudaMemcpyHostToDevice));
-        };
-        upload_y(dy0, y0, ld0);
-        upload_y(dy1, y1, ld1);
-        if (res) { SB_CUDA(cudaMalloc(&dres, (size_t)R * cout * 4)); SB_CUDA(cudaMemset(dres, 0, (size_t)R * cout * 4));
-                   SB_CUDA(cudaMemcpy(dres, res, (size_t)rows * cout * 4, cudaMemcpyHostToDevice)); }
-        SB_CUDA(cudaMalloc(&dend, (size_t)ngran * 4)); SB_CUDA(cudaMemcpy(dend, ends.data(), (size_t)ngran * 4, cudaMemcpyHostToDevice));
-        ConvArgs p{};
-        p.x = dx; p.ldx = cin; p.rows_in = R; p.cin = cin; p.in_slope = in_slope;
-        p.w = cw.w; p.bias = cw.bias; p.ldw = cw.ldw; p.cout = cw.cout; p.wtc = cw.wtc; p.tc_nt = cw.tc_nt;
-        p.ntaps = cw.ntaps; memcpy(p.tap_off, cw.tap_off, sizeof(p.tap_off)); p.min_off = cw.min_off; p.span = cw.span;
-        p.rows_q = R; p.orow_mul = 1; p.orow_add = 0;
-        p.map = RowMap{dend, gran, seg_mul, R};
-        p.act = act; p.scale = scale; p.res = dres; p.ldres = cout;
-        p.y0 = dy0 ? dy0 : dy1; p.ldy0 = dy0 ? ld0 : ld1; p.acc0 = acc0; p.split = split;
-        p.y1 = dy1 ? dy1 : dy0; p.ldy1 = dy1 ? ld1 : ld0; p.acc1 = acc1;
-        if (res && getenv("SB200_DEBUG_RES_IS_X") && cin == cout) { p.res = dx; p.ldres = cin; }   // ResBlock aliasing (timing only)
-        p.wtf = cw.wtf;
+        DeviceBuffers d;
+        float* dx = d.upload(x, (size_t)rows * cin, (size_t)R * cin);
+        float* dy0 = ld0 > 0 ? d.upload(y0, (size_t)rows * ld0, (size_t)R * ld0) : nullptr;
+        float* dy1 = ld1 > 0 ? d.upload(y1, (size_t)rows * ld1, (size_t)R * ld1) : nullptr;
+        const float* dres = res ? d.upload(res, (size_t)rows * cout, (size_t)R * cout) : nullptr;
+        const int* dend = d.upload(ends.data(), (size_t)ngran, (size_t)ngran);
+        ConvCall c;
+        c.in_slope = in_slope; c.act = act; c.scale = scale; c.res = dres; c.ldres = cout;
+        c.y0 = dy0 ? dy0 : dy1; c.ldy0 = dy0 ? ld0 : ld1; c.acc0 = acc0; c.split = split;
+        c.y1 = dy1 ? dy1 : dy0; c.ldy1 = dy1 ? ld1 : ld0; c.acc1 = acc1;
+        if (res && getenv("SB200_DEBUG_RES_IS_X") && cin == cout) { c.res = dx; c.ldres = cin; }   // ResBlock aliasing (timing only)
+        const ConvArgs p = conv_args(cw, dx, cin, RowMap{dend, gran, seg_mul, R}, c);
         if (backend == 2) {
-            if (!conv_tf_supported(p)) throw Error(19, "conv shape not supported by the tf32 chunk-flush backend");
-            launch_conv_tf(p, 0);
+            if (!try_launch_conv_tf(p, 0)) throw Error(19, "conv shape not supported by the tf32 chunk-flush backend");
         } else if (backend == 1) {
-            if (!conv_tc_supported(p)) throw Error(19, "conv shape not supported by the wgmma backend");
-            launch_conv_tc(p, 0);
+            if (!try_launch_conv_tc(p, 0)) throw Error(19, "conv shape not supported by the wgmma backend");
         } else launch_conv_simt(p, 0);
-        cudaError_t e = cudaDeviceSynchronize();
-        if (e == cudaSuccess && dy0) e = cudaMemcpy(y0, dy0, (size_t)rows * ld0 * 4, cudaMemcpyDeviceToHost);
-        if (e == cudaSuccess && dy1) e = cudaMemcpy(y1, dy1, (size_t)rows * ld1 * 4, cudaMemcpyDeviceToHost);
-        cudaFree(dx); cudaFree(dend);
-        if (dy0) cudaFree(dy0);
-        if (dy1) cudaFree(dy1);
-        if (dres) cudaFree(dres);
-        if (e != cudaSuccess) throw Error(19, std::string("CUDA error: ") + cudaGetErrorString(e));
+        SB_CUDA(cudaDeviceSynchronize());
+        if (dy0) SB_CUDA(cudaMemcpy(y0, dy0, (size_t)rows * ld0 * 4, cudaMemcpyDeviceToHost));
+        if (dy1) SB_CUDA(cudaMemcpy(y1, dy1, (size_t)rows * ld1 * 4, cudaMemcpyDeviceToHost));
     });
 }
 
@@ -606,17 +605,13 @@ int32_t sb200_debug_spline(int32_t device, const float* h29, int32_t ldh, float*
             throw Error(19, "debug spline: bad arguments");
         SB_CUDA(cudaSetDevice(device));
         const int R = (rows + 255) / 256 * 256;                          // one granule spanning the padded launch
-        float *dh, *dz; int* dend;
-        SB_CUDA(cudaMalloc(&dh, (size_t)R * ldh * 4)); SB_CUDA(cudaMemset(dh, 0, (size_t)R * ldh * 4));
-        SB_CUDA(cudaMemcpy(dh, h29, (size_t)rows * ldh * 4, cudaMemcpyHostToDevice));
-        SB_CUDA(cudaMalloc(&dz, (size_t)R * 2 * 4)); SB_CUDA(cudaMemset(dz, 0, (size_t)R * 2 * 4));
-        SB_CUDA(cudaMemcpy(dz, z, (size_t)rows * 2 * 4, cudaMemcpyHostToDevice));
-        SB_CUDA(cudaMalloc(&dend, 4)); SB_CUDA(cudaMemcpy(dend, &valid_rows, 4, cudaMemcpyHostToDevice));
+        DeviceBuffers d;
+        const float* dh = d.upload(h29, (size_t)rows * ldh, (size_t)R * ldh);
+        float* dz = d.upload(z, (size_t)rows * 2, (size_t)R * 2);
+        const int* dend = d.upload(&valid_rows, 1, 1);
         launch_spline(dh, ldh, dz, tcol, 10, 1.f, RowMap{dend, R, 1, R}, 0);
-        cudaError_t e = cudaDeviceSynchronize();
-        if (e == cudaSuccess) e = cudaMemcpy(z, dz, (size_t)rows * 2 * 4, cudaMemcpyDeviceToHost);
-        cudaFree(dh); cudaFree(dz); cudaFree(dend);
-        if (e != cudaSuccess) throw Error(19, std::string("CUDA error: ") + cudaGetErrorString(e));
+        SB_CUDA(cudaDeviceSynchronize());
+        SB_CUDA(cudaMemcpy(z, dz, (size_t)rows * 2 * 4, cudaMemcpyDeviceToHost));
     });
 }
 
@@ -632,23 +627,19 @@ int32_t sb200_debug_durations(int32_t device, const float* z, int32_t rows, cons
             segs[b] = SegInfo{seg_off[b], seg_len[b]};
         }
         SB_CUDA(cudaSetDevice(device));
-        float *dz, *dlogw, *dscale; int *dcum, *dylen; SegInfo* dseg;
         const std::vector<float> scales(nseg, length_scale);
-        SB_CUDA(cudaMalloc(&dscale, (size_t)nseg * 4));
-        SB_CUDA(cudaMemcpy(dscale, scales.data(), (size_t)nseg * 4, cudaMemcpyHostToDevice));
-        SB_CUDA(cudaMalloc(&dz, (size_t)rows * 2 * 4)); SB_CUDA(cudaMemcpy(dz, z, (size_t)rows * 2 * 4, cudaMemcpyHostToDevice));
-        SB_CUDA(cudaMalloc(&dlogw, (size_t)rows * 4)); SB_CUDA(cudaMemcpy(dlogw, logw, (size_t)rows * 4, cudaMemcpyHostToDevice));
-        SB_CUDA(cudaMalloc(&dcum, (size_t)rows * 4)); SB_CUDA(cudaMemcpy(dcum, cum, (size_t)rows * 4, cudaMemcpyHostToDevice));
-        SB_CUDA(cudaMalloc(&dylen, (size_t)nseg * 4));
-        SB_CUDA(cudaMalloc(&dseg, (size_t)nseg * sizeof(SegInfo)));
-        SB_CUDA(cudaMemcpy(dseg, segs.data(), (size_t)nseg * sizeof(SegInfo), cudaMemcpyHostToDevice));
+        DeviceBuffers d;
+        const float* dscale = d.upload(scales.data(), (size_t)nseg, (size_t)nseg);
+        const float* dz = d.upload(z, (size_t)rows * 2, (size_t)rows * 2);
+        float* dlogw = d.upload(logw, (size_t)rows, (size_t)rows);
+        int* dcum = d.upload(cum, (size_t)rows, (size_t)rows);
+        int* dylen = d.alloc<int>((size_t)nseg);
+        const SegInfo* dseg = d.upload(segs.data(), (size_t)nseg, (size_t)nseg);
         launch_durations(dz, m0, logs0, dscale, dseg, nseg, dlogw, dcum, dylen, 0);
-        cudaError_t e = cudaDeviceSynchronize();
-        if (e == cudaSuccess) e = cudaMemcpy(logw, dlogw, (size_t)rows * 4, cudaMemcpyDeviceToHost);
-        if (e == cudaSuccess) e = cudaMemcpy(cum, dcum, (size_t)rows * 4, cudaMemcpyDeviceToHost);
-        if (e == cudaSuccess) e = cudaMemcpy(y_len, dylen, (size_t)nseg * 4, cudaMemcpyDeviceToHost);
-        cudaFree(dz); cudaFree(dlogw); cudaFree(dcum); cudaFree(dylen); cudaFree(dseg); cudaFree(dscale);
-        if (e != cudaSuccess) throw Error(19, std::string("CUDA error: ") + cudaGetErrorString(e));
+        SB_CUDA(cudaDeviceSynchronize());
+        SB_CUDA(cudaMemcpy(logw, dlogw, (size_t)rows * 4, cudaMemcpyDeviceToHost));
+        SB_CUDA(cudaMemcpy(cum, dcum, (size_t)rows * 4, cudaMemcpyDeviceToHost));
+        SB_CUDA(cudaMemcpy(y_len, dylen, (size_t)nseg * 4, cudaMemcpyDeviceToHost));
     });
 }
 

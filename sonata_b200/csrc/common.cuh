@@ -135,24 +135,20 @@ inline void launch_pdl(void (*kern)(KArgs...), dim3 grid, dim3 block, size_t sme
 
 void launch_conv_simt(const ConvArgs& a, cudaStream_t st);
 int conv_simt_bn_for(int cout);
-bool conv_tc_supported(const ConvArgs& a);
 // planning only, see sb200_debug_plan; *staging_bytes: the staged epilogue operands' shared memory (0: not staged)
 bool conv_tc_plan_info(const ConvArgs& a, int* out16, int* staging_bytes = nullptr);
-void launch_conv_tc(const ConvArgs& a, cudaStream_t st);
+// try_launch_conv_tc / _tf plan once and launch; false (nothing launched) when the kernel does not take the shape
 bool try_launch_conv_tc(const ConvArgs& a, cudaStream_t st);
 extern int g_conv_tc_grid_cap;     // at most this many CTAs per conv_tc launch (0: no cap); see sb200_debug_conv_grid_cap
 size_t conv_tc_weight_floats(int cin, int cout, int ntaps, int nt);
 void conv_tc_build_weights(const float* wt, int ldw, int cin, int cout, int ntaps, int nt, float* out);
-bool conv_tf_supported(const ConvArgs& a);
 bool conv_tf_plan_info(const ConvArgs& a, int* out16);
-void launch_conv_tf(const ConvArgs& a, cudaStream_t st);
 bool try_launch_conv_tf(const ConvArgs& a, cudaStream_t st);
 size_t conv_tf_weight_floats(int cin, int cout, int ntaps);
 void conv_tf_build_weights(const float* wt, int ldw, int cin, int cout, int ntaps, float* out);
 bool gemm_tf_supported(const TfGemm& g);
 void launch_gemm_tf(const TfGemm& g, cudaStream_t st);
 void throw_launch_error(const char* what);
-      // column tile the SIMT kernel will use for this cout (for weight padding)
 
 struct SegInfo { int off; int len; };   // rows
 

@@ -596,16 +596,6 @@ bool conv_tc_plan_info(const ConvArgs& a, int* out, int* staging_bytes) {
     return true;
 }
 
-bool conv_tc_supported(const ConvArgs& a) {
-    TcLaunch L; size_t smem;
-    if (a.cin % 32 || a.cout % 32 || a.ntaps > SB_MAX_TAPS) return false;
-    return plan(a, L, smem);
-}
-
-void launch_conv_tc(const ConvArgs& a, cudaStream_t st) {
-    if (!try_launch_conv_tc(a, st)) launch_conv_simt(a, st);
-}
-
 // plans ONCE and launches; false (nothing launched) when the shape is not supported
 bool try_launch_conv_tc(const ConvArgs& a, cudaStream_t st) {
     if (a.cin % 32 || a.cout % 32 || a.ntaps > SB_MAX_TAPS) return false;

@@ -329,15 +329,6 @@ bool conv_tf_plan_info(const ConvArgs& a, int* out) {
     return true;
 }
 
-bool conv_tf_supported(const ConvArgs& a) {
-    TfLaunch L; size_t smem;
-    return plan(a, L, smem);
-}
-
-void launch_conv_tf(const ConvArgs& a, cudaStream_t st) {
-    if (!try_launch_conv_tf(a, st)) launch_conv_simt(a, st);
-}
-
 // plans ONCE and launches; false (nothing launched) when the shape is not supported
 bool try_launch_conv_tf(const ConvArgs& a, cudaStream_t st) {
     TfLaunch L; size_t smem;

@@ -19,6 +19,19 @@ void check_launch(const char* what) {
     if (e != cudaSuccess) throw Error(19, std::string("CUDA launch failed (") + what + "): " + cudaGetErrorString(e));
 }
 
+ConvArgs conv_args(const ConvW& w, const float* x, int ldx, const RowMap& map, const ConvCall& c) {
+    ConvArgs p{};
+    p.x = x; p.ldx = ldx; p.rows_in = map.rows; p.cin = w.cin; p.in_slope = c.in_slope;
+    p.w = w.w; p.bias = w.bias; p.ldw = w.ldw; p.cout = w.cout; p.wtc = w.wtc; p.tc_nt = w.tc_nt; p.wtf = w.wtf;
+    p.ntaps = w.ntaps; memcpy(p.tap_off, w.tap_off, sizeof(p.tap_off)); p.min_off = w.min_off; p.span = w.span;
+    p.rows_q = map.rows; p.orow_mul = c.orow_mul; p.orow_add = c.orow_add;
+    p.map = map;
+    p.act = c.act; p.scale = c.scale; p.res = c.res; p.ldres = c.ldres;
+    p.y0 = c.y0; p.ldy0 = c.ldy0; p.acc0 = c.acc0; p.split = c.split < 0 ? w.cout : c.split;
+    p.y1 = c.y1; p.ldy1 = c.ldy1; p.acc1 = c.acc1;
+    p.yt = c.yt; p.yt_col0 = c.yt_col0; p.ldyt = c.ldyt;
+    return p;
+}
 
 namespace {
 constexpr int GX = 64;     // X-level granule (ids)
@@ -227,47 +240,26 @@ struct Runner {
         if (cur) { cur->flops += flops; cur->bytes += bytes; cur->launches += launches; }
     }
 
-    // generic conv launch
-    struct Opt {
-        float in_slope = 1.f; int act = ACT_NONE; float scale = 1.f;
-        const float* res = nullptr; int ldres = 0;
-        float* y0 = nullptr; int ldy0 = 0; int acc0 = 0; int split = -1;
-        float* y1 = nullptr; int ldy1 = 0; int acc1 = 0;
-        int orow_mul = 1, orow_add = 0;
-        bool tc_ok = false;
-        bool tf_ok = false;    // duration-critical layer: wgmma 3xTF32 with chunk-flushed accumulation (conv_tf.cu)
-        float* yt = nullptr; int yt_col0 = 0, ldyt = 0;     // conv_tf only: column tiles >= yt_col0 stored transposed
-    };
-    // bias of a conv: the voice's, or on a multi-speaker voice the speaker-conditioned one of each row's slot
-    void bias_of(const ConvW& w, const Level& lin, ConvArgs& p) const {
-        if (!j.d_cond || w.cond_off < 0) { p.bias = w.bias; return; }
-        if (!lin.bias_slot) throw Error(19, "internal: a speaker-conditioned conv on a level without a slot table");
-        p.bias = j.d_cond + w.cond_off; p.bias_slot = lin.bias_slot; p.ldbias = v.cond_rows;
-    }
-    void conv(const ConvW& w, const float* x, int ldx, const Level& lin, const Opt& o) {
-        ConvArgs p{};
-        p.x = x; p.ldx = ldx; p.rows_in = lin.map.rows; p.cin = w.cin; p.in_slope = o.in_slope;
-        p.w = w.w; bias_of(w, lin, p); p.ldw = w.ldw; p.cout = w.cout; p.wtc = w.wtc; p.tc_nt = w.tc_nt; p.wtf = w.wtf;
-        p.ntaps = w.ntaps; memcpy(p.tap_off, w.tap_off, sizeof(p.tap_off)); p.min_off = w.min_off; p.span = w.span;
-        p.rows_q = lin.map.rows; p.orow_mul = o.orow_mul; p.orow_add = o.orow_add;
-        p.map = lin.map;
-        p.act = o.act; p.scale = o.scale; p.res = o.res; p.ldres = o.ldres;
-        p.y0 = o.y0; p.ldy0 = o.ldy0; p.acc0 = o.acc0; p.split = o.split < 0 ? w.cout : o.split;
-        p.y1 = o.y1; p.ldy1 = o.ldy1; p.acc1 = o.acc1;
-        p.yt = o.yt; p.yt_col0 = o.yt_col0; p.ldyt = o.ldyt;
-
-        // backend 1 (default): wgmma everywhere; 2: wgmma flow / decoder, fp32 CUDA cores for the text encoder and
-        // the duration predictor (the round-1 configuration, kept for A/B runs); 0: fp32 CUDA cores everywhere
-        // (each try_launch plans once and returns false without launching when the shape is not supported)
-        if (v.backend == 1 && o.tf_ok && try_launch_conv_tf(p, st)) {}
+    void conv(const ConvW& w, const float* x, int ldx, const Level& lin, const ConvCall& o) {
+        ConvArgs p = conv_args(w, x, ldx, lin.map, o);
+        // on a multi-speaker voice, the speaker-conditioned bias of each row's slot
+        if (j.d_cond && w.cond_off >= 0) {
+            if (!lin.bias_slot) throw Error(19, "internal: a speaker-conditioned conv on a level without a slot table");
+            p.bias = j.d_cond + w.cond_off; p.bias_slot = lin.bias_slot; p.ldbias = v.cond_rows;
+        }
+        // The layer's images name the kernels that can run it.  Backend 1 (default): conv_tf, else conv_tc; 2: conv_tc
+        // (the text encoder and the duration predictor on fp32 CUDA cores, kept for A/B runs); 0: fp32 CUDA cores
+        // everywhere.  Each try_launch plans once and returns false without launching when the shape is not supported.
+        if (v.backend == 1 && w.wtf && try_launch_conv_tf(p, st)) {}
         else if (o.yt) throw Error(19, "internal: a transposed conv output needs the conv_tf kernel");
-        else if (v.backend >= 1 && o.tc_ok && try_launch_conv_tc(p, st)) {}
+        else if (v.backend >= 1 && w.wtc && try_launch_conv_tc(p, st)) {}
+        else if (!w.w) throw Error(19, "internal: no kernel for a conv without fp32 weights");
         else launch_conv_simt(p, st);
         const double vr = (double)lin.valid_rows;
         const int cout_w = (o.act == ACT_GATE) ? w.cout / 2 : w.cout;
-        count(2.0 * vr * w.cin * w.cout * w.ntaps,
+        count(2.0 * vr * w.macs,
               4.0 * (vr * (w.cin + cout_w + ((o.res && o.res != x) ? w.cout : 0) + ((o.acc0 | o.acc1) ? w.cout : 0)) +
-                     (double)w.ntaps * w.cin * w.cout));
+                     (double)w.macs));
     }
 
     void dds(const DDSW& d, float* x, float* t1, float* t2, const Level& L) {
@@ -276,7 +268,7 @@ struct Runner {
         for (int i = 0; i < 3; i++) {
             launch_dw_ln_gelu(x, d.wdw[i], d.bdw[i], a.dp_kernel, dil, d.g1[i], d.b1[i], t1, C, L.map, st);
             count(2.0 * L.valid_rows * C * a.dp_kernel, 8.0 * L.valid_rows * C);
-            Opt o; o.y0 = t2; o.ldy0 = C; o.tf_ok = true;
+            ConvCall o; o.y0 = t2; o.ldy0 = C;
             conv(d.c1x1[i], t1, C, L, o);
             launch_ln(t2, nullptr, x, d.g2[i], d.b2[i], x, C, 1, L.map, st);
             count(0, 12.0 * L.valid_rows * C);
@@ -476,7 +468,7 @@ void run_decoder(Runner& R, const Level& LY, const FrameTables& y, const Decoder
     Voice& v = R.v; const Arch& a = R.a;
     const int RY = LY.map.rows;
     R.begin("dec.pre");
-    { Runner::Opt o; o.y0 = d.p0; o.ldy0 = a.up_init; o.tc_ok = true; R.conv(v.conv_pre, s, a.inter, LY, o); }
+    { ConvCall o; o.y0 = d.p0; o.ldy0 = a.up_init; R.conv(v.conv_pre, s, a.inter, LY, o); }
     R.end();
 
     const float* cur = d.p0; Level Lin = LY; int U = 1;
@@ -487,29 +479,16 @@ void run_decoder(Runner& R, const Level& LY, const FrameTables& y, const Decoder
         float *up = d.stage[i][0], *ys = d.stage[i][1];
         float* const* tmp = &d.stage[i][2];
         R.begin("dec.up" + std::to_string(i));
-        bool fused_done = false;
         if (v.backend >= 1 && st.fused.wtc) {
-            // tensor-core path: all u phases in one launch (input read once, N = u*cout columns).  Column block p of
-            // GEMM row q is output row q*u + p, column n % cout, so with ldy0 = u*cout the output is the GEMM's own
-            // row-major matrix: an ordinary conv.
-            ConvArgs pa{};
-            pa.x = cur; pa.ldx = st.cin; pa.rows_in = Lin.map.rows; pa.cin = st.cin; pa.in_slope = 0.1f;
-            pa.w = nullptr; pa.bias = st.fused.bias; pa.ldw = st.fused.ldw; pa.cout = st.fused.cout;
-            pa.wtc = st.fused.wtc; pa.tc_nt = st.fused.tc_nt;
-            pa.ntaps = st.fused.ntaps; memcpy(pa.tap_off, st.fused.tap_off, sizeof(pa.tap_off));
-            pa.min_off = st.fused.min_off; pa.span = st.fused.span;
-            pa.rows_q = Lin.map.rows; pa.orow_mul = 1; pa.orow_add = 0;
-            pa.map = Lin.map; pa.act = ACT_NONE; pa.scale = 1.f;
-            pa.y0 = up; pa.ldy0 = st.fused.cout; pa.split = st.fused.cout; pa.y1 = up; pa.ldy1 = st.fused.cout;
-            if (try_launch_conv_tc(pa, R.st)) {
-                const double vr = (double)Lin.valid_rows;
-                R.count(2.0 * vr * st.cin * st.cout * st.k, 4.0 * (vr * (st.cin + (double)st.u * st.cout) + (double)st.cin * st.cout * st.k));
-                fused_done = true;
+            // all u phases in one launch (input read once, N = u*cout columns).  Column block p of GEMM row q is output
+            // row q*u + p, column n % cout, so with ldy0 = u*cout the output is the GEMM's own row-major matrix.
+            ConvCall o; o.in_slope = 0.1f; o.y0 = up; o.ldy0 = st.fused.cout;
+            R.conv(st.fused, cur, st.cin, Lin, o);
+        } else {
+            for (int p = 0; p < st.u; p++) {
+                ConvCall o; o.in_slope = 0.1f; o.y0 = up; o.ldy0 = st.cout; o.orow_mul = st.u; o.orow_add = p;
+                R.conv(st.phase[p], cur, st.cin, Lin, o);
             }
-        }
-        for (int p = 0; p < st.u && !fused_done; p++) {
-            Runner::Opt o; o.in_slope = 0.1f; o.y0 = up; o.ldy0 = st.cout; o.orow_mul = st.u; o.orow_add = p; o.tc_ok = true;
-            R.conv(st.phase[p], cur, st.cin, Lin, o);
         }
         R.end();
         R.begin("dec.mrf" + std::to_string(i));
@@ -522,11 +501,11 @@ void run_decoder(Runner& R, const Level& LY, const FrameTables& y, const Decoder
                 const bool last = (m + 1 == nd);
                 const float* cin_ptr = xb;
                 if (a.resblock != 2) {
-                    Runner::Opt o1; o1.in_slope = 0.1f; o1.y0 = tmp[0]; o1.ldy0 = st.cout; o1.tc_ok = true;
+                    ConvCall o1; o1.in_slope = 0.1f; o1.y0 = tmp[0]; o1.ldy0 = st.cout;
                     R.conv(rb.c1[m], xb, st.cout, Lo, o1);
                     cin_ptr = tmp[0];
                 }
-                Runner::Opt o; o.in_slope = 0.1f; o.res = xb; o.ldres = st.cout; o.tc_ok = true;
+                ConvCall o; o.in_slope = 0.1f; o.res = xb; o.ldres = st.cout;
                 float* dst;
                 if (last) { dst = ys; o.scale = third; o.acc0 = jb > 0 ? 1 : 0; }
                 else dst = (a.resblock == 2) ? tmp[0] : tmp[1 + (m & 1)];
@@ -742,7 +721,7 @@ void Job::run(float* d_out, size_t d_out_cap) {
     for (int l = 0; l < a.layers; l++) {
         const EncLayer& e = V.enc[l];
         {
-            Runner::Opt o; o.y0 = x.qkv; o.ldy0 = 3 * H; o.tf_ok = true;
+            ConvCall o; o.y0 = x.qkv; o.ldy0 = 3 * H;
             if (tc_att_ok) { o.yt = x.att_vt; o.yt_col0 = 2 * H; o.ldyt = RX; }       // V leaves transposed: [H][RX]
             R.conv(e.qkv, x.xa, H, LX, o);
         }
@@ -765,22 +744,22 @@ void Job::run(float* d_out, size_t d_out_cap) {
                 d2d(x.vt0, x.att_vt, (size_t)H * RX, st);
             }
         }
-        { Runner::Opt o; o.y0 = x.xb; o.ldy0 = H; o.tf_ok = true; R.conv(e.o, x.att, H, LX, o); }
+        { ConvCall o; o.y0 = x.xb; o.ldy0 = H; R.conv(e.o, x.att, H, LX, o); }
         launch_ln(x.xa, x.xb, nullptr, e.g1, e.b1, x.xa, H, 0, LX.map, st);
         R.count(0, 12.0 * LX.valid_rows * H);
-        { Runner::Opt o; o.act = ACT_RELU; o.y0 = x.ffn; o.ldy0 = F; o.tf_ok = true; R.conv(e.ffn1, x.xa, H, LX, o); }
-        { Runner::Opt o; o.y0 = x.xb; o.ldy0 = H; o.tf_ok = true; R.conv(e.ffn2, x.ffn, F, LX, o); }
+        { ConvCall o; o.act = ACT_RELU; o.y0 = x.ffn; o.ldy0 = F; R.conv(e.ffn1, x.xa, H, LX, o); }
+        { ConvCall o; o.y0 = x.xb; o.ldy0 = H; R.conv(e.ffn2, x.ffn, F, LX, o); }
         launch_ln(x.xa, x.xb, nullptr, e.g2, e.b2, x.xa, H, 0, LX.map, st);
         R.count(0, 12.0 * LX.valid_rows * H);
     }
-    { Runner::Opt o; o.y0 = x.stats; o.ldy0 = 2 * I; o.tf_ok = true; R.conv(V.enc_proj, x.xa, H, LX, o); }
+    { ConvCall o; o.y0 = x.stats; o.ldy0 = 2 * I; R.conv(V.enc_proj, x.xa, H, LX, o); }
     R.end();
 
     // ---------------- stochastic duration predictor (reverse) ----------------
     R.begin("dp");
-    { Runner::Opt o; o.y0 = x.d0; o.ldy0 = H; o.tf_ok = true; R.conv(V.dp_pre, x.xa, H, LX, o); }
+    { ConvCall o; o.y0 = x.d0; o.ldy0 = H; R.conv(V.dp_pre, x.xa, H, LX, o); }
     R.dds(V.dp_dds, x.d0, x.t1, x.t2, LX);
-    { Runner::Opt o; o.y0 = x.g; o.ldy0 = H; o.tf_ok = true; R.conv(V.dp_proj, x.d0, H, LX, o); }
+    { ConvCall o; o.y0 = x.g; o.ldy0 = H; R.conv(V.dp_proj, x.d0, H, LX, o); }
     launch_scale_copy2(x.epsw, x.scales, x.xseg_of_gran, x.zz, LX.map, st);
     // debug: zz, d0 and h29 are reused by every flow, so each flow's stages are captured as copies
     for (size_t s = 0; s < V.dp_flows.size(); s++) {
@@ -790,7 +769,7 @@ void Job::run(float* d_out, size_t d_out_cap) {
         R.count(2.0 * LX.valid_rows * H, 8.0 * LX.valid_rows * H);
         R.dds(cf.dds, x.d0, x.t1, x.t2, LX);
         if (debug) d2d(x.dpf[s][1], x.d0, (size_t)RX * H, st);
-        { Runner::Opt o; o.y0 = x.h29; o.ldy0 = 32; o.tf_ok = true; R.conv(cf.proj, x.d0, H, LX, o); }
+        { ConvCall o; o.y0 = x.h29; o.ldy0 = 32; R.conv(cf.proj, x.d0, H, LX, o); }
         if (debug) d2d(x.dpf[s][2], x.h29, (size_t)RX * 32, st);
         launch_spline(x.h29, 32, x.zz, cf.tcol, a.dp_bins, 1.0f / sqrtf((float)H), LX.map, st);
         R.count(0, 4.0 * LX.valid_rows * 34);
@@ -850,16 +829,16 @@ void Job::run(float* d_out, size_t d_out_cap) {
     R.begin("flow");
     for (size_t step = 0; step < V.flows.size(); step++) {
         const CouplingW& cp = V.flows[step];
-        { Runner::Opt o; o.y0 = f.h; o.ldy0 = H; o.tc_ok = true; R.conv(cp.pre, f.s + cp.cond_off, I, LY, o); }
+        { ConvCall o; o.y0 = f.h; o.ldy0 = H; R.conv(cp.pre, f.s + cp.cond_off, I, LY, o); }
         const int n = (int)cp.in.size();
         for (int l = 0; l < n; l++) {
-            { Runner::Opt o; o.act = ACT_GATE; o.y0 = f.acts; o.ldy0 = H; o.tc_ok = true; R.conv(cp.in[l], f.h, H, LY, o); }
-            Runner::Opt o; o.tc_ok = true;
+            { ConvCall o; o.act = ACT_GATE; o.y0 = f.acts; o.ldy0 = H; R.conv(cp.in[l], f.h, H, LY, o); }
+            ConvCall o;
             if (l < n - 1) { o.y0 = f.h; o.ldy0 = H; o.acc0 = 1; o.split = H; o.y1 = f.outb; o.ldy1 = H; o.acc1 = l > 0; }
             else { o.split = 0; o.y0 = f.outb; o.ldy0 = H; o.y1 = f.outb; o.ldy1 = H; o.acc1 = l > 0; }
             R.conv(cp.rs[l], f.acts, H, LY, o);
         }
-        { Runner::Opt o; o.y0 = f.s + cp.tgt_off; o.ldy0 = I; o.acc0 = 1; o.scale = -1.f; o.tc_ok = true; R.conv(cp.post, f.outb, H, LY, o); }
+        { ConvCall o; o.y0 = f.s + cp.tgt_off; o.ldy0 = I; o.acc0 = 1; o.scale = -1.f; R.conv(cp.post, f.outb, H, LY, o); }
         if (debug) d2d(f.flow[step], f.s, (size_t)RY * I, st);
     }
     R.end();

@@ -45,23 +45,48 @@ struct Arch {
     int hop() const { int h = 1; for (int u : up_rates) h *= u; return h; }
 };
 
+// One convolution layer: its shape (conv_layout) and the weight images of the kernels that can run it.  A layer carries
+// only the images of its kernels, and Runner::conv picks the kernel from the images it finds.
 struct ConvW {
-    float* w = nullptr;
+    float* w = nullptr;                      // fp32 [ntaps][cin][ldw] (conv_simt.cu); null on the phase-fused ConvTranspose
     float* bias = nullptr;
-    float* wtc = nullptr; int tc_nt = 0;     // bf16 hi/lo swizzled weight images (conv_tc.cu)
+    float* wtc = nullptr; int tc_nt = 0;     // bf16 hi/lo swizzled weight images (conv_tc.cu): flow and decoder layers
     float* wtf = nullptr;                    // tf32 hi/lo images (conv_tf.cu): text-encoder / duration-predictor layers
     int cin = 0, cout = 0, ldw = 0, ntaps = 0;
+    int macs = 0;                            // multiply-adds per output row (profile counters)
     int cond_off = -1;                       // multi-speaker voices: offset of this conv's per-call effective bias (Job::d_cond)
     int tap_off[SB_MAX_TAPS] = {0};
     int min_off = 0, span = 0;
 };
+
+// Tap offsets (t - (k-1)/2) * dil, t < k, of a centred Conv1d of kernel size k.
+std::vector<int> centred_taps(int k, int dil);
+// The shape of a conv with taps `offs` and no weights: ntaps, tap_off, min_off, span, macs = ntaps * cin * cout, and ldw
+// padded to conv_simt's column tile (pad_ldw) or equal to cout.
+ConvW conv_layout(int cin, int cout, const std::vector<int>& offs, bool pad_ldw = true);
+// Column tile of conv_tc's weight image for `cout` output columns; 0: the kernel takes no such layer.
+int tc_tile_for(int cout);
+
+// What a call site adds to a layer: input activation, epilogue and outputs (the ConvArgs fields of the same names).
+struct ConvCall {
+    float in_slope = 1.f; int act = ACT_NONE; float scale = 1.f;
+    const float* res = nullptr; int ldres = 0;
+    float* y0 = nullptr; int ldy0 = 0; int acc0 = 0; int split = -1;     // split < 0: every column goes to y0
+    float* y1 = nullptr; int ldy1 = 0; int acc1 = 0;
+    int orow_mul = 1, orow_add = 0;
+    float* yt = nullptr; int yt_col0 = 0, ldyt = 0;     // conv_tf only: column tiles >= yt_col0 stored transposed
+};
+// Launch arguments of layer `w` over the rows of `map`, reading x [map.rows][ldx]; the bias is the layer's own.
+ConvArgs conv_args(const ConvW& w, const float* x, int ldx, const RowMap& map, const ConvCall& c);
 
 struct EncLayer { ConvW qkv, o, ffn1, ffn2; float *relk, *relv, *g1, *b1, *g2, *b2; };
 struct DDSW { float* wdw[3]; float* bdw[3]; ConvW c1x1[3]; float *g1[3], *b1[3], *g2[3], *b2[3]; };
 struct CFlowW { float* pre_w; float* pre_b; DDSW dds; ConvW proj; int ccol, tcol; };
 struct CouplingW { ConvW pre; std::vector<ConvW> in, rs; ConvW post; int cond_off, tgt_off; };
 struct ResBW { int k; std::vector<int> dils; std::vector<ConvW> c1, c2; };
-struct UpStageW { int u, k, cin, cout; std::vector<ConvW> phase; ConvW fused; std::vector<ResBW> res; };   // fused: all phases as one N = u*cout conv (tensor-core path)
+// phase: one fp32 conv per output phase (backend 0, or when fused has no image); fused: all phases as one N = u*cout
+// conv with bf16 images only (backends 1 and 2)
+struct UpStageW { int u, k, cin, cout; std::vector<ConvW> phase; ConvW fused; std::vector<ResBW> res; };
 
 struct SynthConfig { long long speaker = 0; bool has_speaker = false; float noise_scale = 0.667f, length_scale = 1.f, noise_w = 0.8f; };
 
@@ -99,11 +124,10 @@ struct Voice {
     float *cond_w = nullptr, *cond_base = nullptr; int cond_rows = 0;
     float* conv_post_w = nullptr;   // [7][C_last]
     int c_last = 0;
-    size_t weight_bytes = 0;
 
     int backend = 1;                // 1 (default): wgmma everywhere (bf16x2 split for flow + decoder, chunk-flushed 3xTF32 for the text
                                     // encoder + duration predictor); 2: wgmma flow + decoder, fp32 CUDA cores for encoder + predictor;
-                                    // 0: fp32 CUDA cores everywhere
+                                    // 0: fp32 CUDA cores everywhere.  Runner::conv applies it to the images each layer carries.
     unsigned long long noise_seed = 0x5eed5eedULL;
     std::mutex pool_mu;
     std::vector<Context*> pool;

@@ -61,28 +61,29 @@ const HostTensor& T(const TensorMap& m, const std::string& n) {
 
 struct Uploader {
     Voice* v;
-    bool want_tf = false;      // also build the tf32 hi/lo images of conv_tf.cu (layers that feed the duration predictor)
     float* up(const std::vector<float>& h) {
         float* d = nullptr;
         SB_CUDA(cudaMalloc(&d, h.size() * sizeof(float) + 16));
         SB_CUDA(cudaMemcpy(d, h.data(), h.size() * sizeof(float), cudaMemcpyHostToDevice));
         v->dev_allocs.push_back(d);
-        v->weight_bytes += h.size() * sizeof(float);
         return d;
     }
 };
 
-int tc_tile_for(int cout) {
-    if (cout <= 128) return cout;
-    if (cout % 128 == 0) return 128;
-    if (cout % 96 == 0) return 96;
-    return 0;
-}
+// Weight images of a conv, one per kernel that reads it: conv_simt.cu, conv_tf.cu, conv_tc.cu.
+enum ConvImages { IMG_F32 = 1, IMG_TF32 = 2, IMG_BF16 = 4 };
+// text encoder and duration predictor: conv_tf on backend 1, conv_simt on backends 0 and 2
+constexpr int ENC_IMAGES = IMG_F32 | IMG_TF32;
+// flow and decoder: conv_tc on backends 1 and 2, conv_simt on backend 0
+constexpr int DEC_IMAGES = IMG_F32 | IMG_BF16;
 
-// tensor-core weight images for a finished ConvW whose [ntaps][cin][ldw] host copy is `wt`
-void add_tc_images(Uploader& U, ConvW& c, const std::vector<float>& wt) {
+// Uploads the bias bt [ldw] and the requested images of weights wt [ntaps][cin][ldw] of a laid-out conv.  A
+// tensor-core image is built only for a shape its kernel takes.
+void upload_conv(Uploader& U, ConvW& c, const std::vector<float>& wt, const std::vector<float>& bt, int images) {
+    if (images & IMG_F32) c.w = U.up(wt);
+    c.bias = U.up(bt);
     if (c.cin % 32 || c.cout % 32) return;
-    if (U.want_tf && c.ldw >= c.cout) {
+    if (images & IMG_TF32) {
         const size_t nf = conv_tf_weight_floats(c.cin, c.cout, c.ntaps);
         if (nf) {
             std::vector<float> img(nf);
@@ -91,18 +92,18 @@ void add_tc_images(Uploader& U, ConvW& c, const std::vector<float>& wt) {
         }
     }
     const int nt = tc_tile_for(c.cout);
-    if (!nt) return;
+    if (!(images & IMG_BF16) || !nt) return;
     std::vector<float> img(conv_tc_weight_floats(c.cin, c.cout, c.ntaps, nt));
     conv_tc_build_weights(wt.data(), c.ldw, c.cin, c.cout, c.ntaps, nt, img.data());
     c.wtc = U.up(img);
     c.tc_nt = nt;
 }
 
-// Conv1d weight [cout][cin][k] (+bias) -> ConvW with taps (t - (k-1)/2) * dil.
+// Conv1d weight [cout][cin][k] (+bias) -> ConvW with centred taps of dilation `dil` and the given images.
 // `perm_out`: output column n takes source row perm_out[n]; `perm_in` likewise for inputs.
-ConvW make_conv(Uploader& U, const std::vector<const HostTensor*>& ws, const std::vector<const HostTensor*>& bs,
-                int dil, const std::vector<int>* perm_out = nullptr, const std::vector<int>* perm_in = nullptr,
-                int pad_cout_to = 0) {
+ConvW make_conv(Uploader& U, int images, const std::vector<const HostTensor*>& ws,
+                const std::vector<const HostTensor*>& bs, int dil, const std::vector<int>* perm_out = nullptr,
+                const std::vector<int>* perm_in = nullptr, int pad_cout_to = 0) {
     const int cin = ws[0]->dims[1], k = ws[0]->dims[2];
     int cout = 0;
     for (auto* w : ws) cout += w->dims[0];
@@ -117,19 +118,7 @@ ConvW make_conv(Uploader& U, const std::vector<const HostTensor*>& ws, const std
             r += ws[s]->dims[0];
         }
     }
-    ConvW c;
-    c.cin = cin; c.ntaps = k;
-    c.cout = pad_cout_to ? pad_cout_to : cout;
-    const int bn = conv_simt_bn_for(c.cout);
-    c.ldw = (c.cout + bn - 1) / bn * bn;
-    if (k > SB_MAX_TAPS) throw Error(17, "conv kernel too wide");
-    c.min_off = 0; int mx = 0;
-    for (int t = 0; t < k; t++) {
-        c.tap_off[t] = (t - (k - 1) / 2) * dil;
-        c.min_off = std::min(c.min_off, c.tap_off[t]);
-        mx = std::max(mx, c.tap_off[t]);
-    }
-    c.span = mx - c.min_off;
+    ConvW c = conv_layout(cin, pad_cout_to ? pad_cout_to : cout, centred_taps(k, dil));
     std::vector<float> wt((size_t)k * cin * c.ldw, 0.f), bt(c.ldw, 0.f);
     for (int n = 0; n < cout; n++) {
         const int sn = perm_out ? (*perm_out)[n] : n;
@@ -140,20 +129,19 @@ ConvW make_conv(Uploader& U, const std::vector<const HostTensor*>& ws, const std
                 wt[((size_t)t * cin + ci) * c.ldw + n] = wcat[((size_t)sn * cin + sc) * k + t];
         }
     }
-    c.w = U.up(wt);
-    c.bias = U.up(bt);
-    add_tc_images(U, c, wt);
+    upload_conv(U, c, wt, bt, images);
     return c;
 }
 
-ConvW conv_named(Uploader& U, const TensorMap& m, const std::string& name, int dil = 1, bool has_bias = true,
-                 const std::vector<int>* perm_out = nullptr, const std::vector<int>* perm_in = nullptr,
-                 int pad_cout_to = 0) {
+ConvW conv_named(Uploader& U, int images, const TensorMap& m, const std::string& name, int dil = 1,
+                 bool has_bias = true, const std::vector<int>* perm_out = nullptr,
+                 const std::vector<int>* perm_in = nullptr, int pad_cout_to = 0) {
     std::vector<const HostTensor*> bs;
     if (has_bias) bs.push_back(&T(m, name + ".bias")); else bs.push_back(nullptr);
-    return make_conv(U, {&T(m, name + ".weight")}, bs, dil, perm_out, perm_in, pad_cout_to);
+    return make_conv(U, images, {&T(m, name + ".weight")}, bs, dil, perm_out, perm_in, pad_cout_to);
 }
 
+// DDSConv of the duration predictor
 DDSW load_dds(Uploader& U, const TensorMap& m, const std::string& p, int C, int k) {
     DDSW d;
     for (int i = 0; i < 3; i++) {
@@ -163,7 +151,7 @@ DDSW load_dds(Uploader& U, const TensorMap& m, const std::string& p, int C, int 
             for (int t = 0; t < k; t++) wt[(size_t)t * C + c] = w.f[(size_t)c * k + t];
         d.wdw[i] = U.up(wt);
         d.bdw[i] = U.up(T(m, p + "convs_sep." + std::to_string(i) + ".bias").f);
-        d.c1x1[i] = conv_named(U, m, p + "convs_1x1." + std::to_string(i));
+        d.c1x1[i] = conv_named(U, ENC_IMAGES, m, p + "convs_1x1." + std::to_string(i));
         d.g1[i] = U.up(T(m, p + "norms_1." + std::to_string(i) + ".gamma").f);
         d.b1[i] = U.up(T(m, p + "norms_1." + std::to_string(i) + ".beta").f);
         d.g2[i] = U.up(T(m, p + "norms_2." + std::to_string(i) + ".gamma").f);
@@ -203,15 +191,41 @@ uint32_t first_code_point(const std::string& s) {
 
 }  // namespace
 
-// test hook: build a ConvW (both backends' weight layouts) from a raw [cout][cin][k] tensor
+std::vector<int> centred_taps(int k, int dil) {
+    std::vector<int> offs(k);
+    for (int t = 0; t < k; t++) offs[t] = (t - (k - 1) / 2) * dil;
+    return offs;
+}
+
+ConvW conv_layout(int cin, int cout, const std::vector<int>& offs, bool pad_ldw) {
+    if (offs.empty() || offs.size() > SB_MAX_TAPS) throw Error(17, "unsupported conv kernel size");
+    ConvW c;
+    c.cin = cin; c.cout = cout; c.ntaps = (int)offs.size();
+    c.macs = c.ntaps * cin * cout;
+    const int bn = pad_ldw ? conv_simt_bn_for(cout) : 1;
+    c.ldw = (cout + bn - 1) / bn * bn;
+    std::copy(offs.begin(), offs.end(), c.tap_off);
+    c.min_off = *std::min_element(offs.begin(), offs.end());
+    c.span = *std::max_element(offs.begin(), offs.end()) - c.min_off;
+    return c;
+}
+
+int tc_tile_for(int cout) {
+    if (cout <= 128) return cout;
+    if (cout % 128 == 0) return 128;
+    if (cout % 96 == 0) return 96;
+    return 0;
+}
+
+// test hook: build a ConvW with every kernel's weight images from a raw [cout][cin][k] tensor (tools/conv_unit.py runs
+// one conv on each backend)
 ConvW debug_make_conv(Voice& v, const float* w, const float* bias, int cout, int cin, int k, int dil) {
     HostTensor hw, hb;
     hw.dims = {cout, cin, k}; hw.f.assign(w, w + (size_t)cout * cin * k);
     hb.dims = {cout}; hb.f.assign(cout, 0.f);
     if (bias) hb.f.assign(bias, bias + cout);
     Uploader U{&v};
-    U.want_tf = true;
-    return make_conv(U, {&hw}, {&hb}, dil);
+    return make_conv(U, IMG_F32 | IMG_TF32 | IMG_BF16, {&hw}, {&hb}, dil);
 }
 
 // VitsModelCommons::phonemes_to_input_ids + get_meta_ids (piper/src/lib.rs:173-179, 232-250)
@@ -345,14 +359,13 @@ Voice* load_voice(const std::string& config_path, int device) {
     if (H != 96 && H != 192 && H != 256) throw Error(17, "unsupported hidden width (LayerNorm kernels: 96 / 192 / 256)");
 
     Uploader U{v.get()};
-    U.want_tf = true;          // text encoder + duration predictor: error-compensated tf32 with chunked accumulation
     v->emb = U.up(T(m, "enc_p.emb.weight").f);
     for (int l = 0; l < a.layers; l++) {
         EncLayer e;
         const std::string p = "enc_p.encoder.attn_layers." + std::to_string(l) + ".";
-        e.qkv = make_conv(U, {&T(m, p + "conv_q.weight"), &T(m, p + "conv_k.weight"), &T(m, p + "conv_v.weight")},
+        e.qkv = make_conv(U, ENC_IMAGES, {&T(m, p + "conv_q.weight"), &T(m, p + "conv_k.weight"), &T(m, p + "conv_v.weight")},
                           {&T(m, p + "conv_q.bias"), &T(m, p + "conv_k.bias"), &T(m, p + "conv_v.bias")}, 1);
-        e.o = conv_named(U, m, p + "conv_o");
+        e.o = conv_named(U, ENC_IMAGES, m, p + "conv_o");
         e.relk = U.up(T(m, p + "emb_rel_k").f);
         e.relv = U.up(T(m, p + "emb_rel_v").f);
         const std::string n1 = "enc_p.encoder.norm_layers_1." + std::to_string(l);
@@ -360,14 +373,14 @@ Voice* load_voice(const std::string& config_path, int device) {
         e.g1 = U.up(T(m, n1 + ".gamma").f); e.b1 = U.up(T(m, n1 + ".beta").f);
         e.g2 = U.up(T(m, n2 + ".gamma").f); e.b2 = U.up(T(m, n2 + ".beta").f);
         const std::string f = "enc_p.encoder.ffn_layers." + std::to_string(l) + ".";
-        e.ffn1 = conv_named(U, m, f + "conv_1");
-        e.ffn2 = conv_named(U, m, f + "conv_2");
+        e.ffn1 = conv_named(U, ENC_IMAGES, m, f + "conv_1");
+        e.ffn2 = conv_named(U, ENC_IMAGES, m, f + "conv_2");
         v->enc.push_back(e);
     }
-    v->enc_proj = conv_named(U, m, "enc_p.proj");
+    v->enc_proj = conv_named(U, ENC_IMAGES, m, "enc_p.proj");
 
-    v->dp_pre = conv_named(U, m, "dp.pre");
-    v->dp_proj = conv_named(U, m, "dp.proj");
+    v->dp_pre = conv_named(U, ENC_IMAGES, m, "dp.pre");
+    v->dp_proj = conv_named(U, ENC_IMAGES, m, "dp.proj");
     v->dp_dds = load_dds(U, m, "dp.convs.", H, a.dp_kernel);
     {
         // reversed(flows)[:-2] + [EA]: Flip, CF4^-1, Flip, CF3^-1, Flip, CF2^-1, Flip, EA^-1.  The flips
@@ -379,7 +392,7 @@ Voice* load_voice(const std::string& config_path, int device) {
             cf.pre_w = U.up(T(m, p + "pre.weight").f);
             cf.pre_b = U.up(T(m, p + "pre.bias").f);
             cf.dds = load_dds(U, m, p + "convs.", H, a.dp_kernel);
-            cf.proj = conv_named(U, m, p + "proj", 1, true, nullptr, nullptr, 32);
+            cf.proj = conv_named(U, ENC_IMAGES, m, p + "proj", 1, true, nullptr, nullptr, 32);
             cf.ccol = (s % 2 == 0) ? 1 : 0;
             cf.tcol = 1 - cf.ccol;
             v->dp_flows.push_back(cf);
@@ -387,7 +400,6 @@ Voice* load_voice(const std::string& config_path, int device) {
         v->ea_m0 = T(m, "dp.flows.0.m").f[0];
         v->ea_logs0 = T(m, "dp.flows.0.logs").f[0];
     }
-    U.want_tf = false;
     {
         const int half = I / 2;
         std::vector<int> rev(half);
@@ -402,31 +414,31 @@ Voice* load_voice(const std::string& config_path, int device) {
             c.cond_off = reversed ? half : 0;
             c.tgt_off = reversed ? 0 : half;
             if (half % 32 == 0) {
-                c.pre = conv_named(U, m, p + "pre", 1, true, nullptr, reversed ? &rev : nullptr);
+                c.pre = conv_named(U, DEC_IMAGES, m, p + "pre", 1, true, nullptr, reversed ? &rev : nullptr);
             } else {
                 // A half that is not a whole number of 32-channel K-blocks (x_low: 48 of 96) keeps the tensor-core convs
                 // by widening pre and post to all `inter` channels of z: pre reads the target half with zero weights,
                 // post writes the conditioning half with zero weights and bias.  Exact zeros change no sum.
                 const HostTensor w = widen(T(m, p + "pre.weight"), I, 1, c.cond_off, reversed);
-                c.pre = make_conv(U, {&w}, {&T(m, p + "pre.bias")}, 1);
+                c.pre = make_conv(U, DEC_IMAGES, {&w}, {&T(m, p + "pre.bias")}, 1);
                 c.cond_off = 0;
             }
             for (int l = 0; l < a.wn_layers; l++) {
-                c.in.push_back(conv_named(U, m, p + "enc.in_layers." + std::to_string(l), 1, true, &gate));
-                c.rs.push_back(conv_named(U, m, p + "enc.res_skip_layers." + std::to_string(l)));
+                c.in.push_back(conv_named(U, DEC_IMAGES, m, p + "enc.in_layers." + std::to_string(l), 1, true, &gate));
+                c.rs.push_back(conv_named(U, DEC_IMAGES, m, p + "enc.res_skip_layers." + std::to_string(l)));
             }
             if (half % 32 == 0) {
-                c.post = conv_named(U, m, p + "post", 1, true, reversed ? &rev : nullptr);
+                c.post = conv_named(U, DEC_IMAGES, m, p + "post", 1, true, reversed ? &rev : nullptr);
             } else {
                 const HostTensor w = widen(T(m, p + "post.weight"), I, 0, c.tgt_off, reversed);
                 const HostTensor b = widen(T(m, p + "post.bias"), I, 0, c.tgt_off, reversed);
-                c.post = make_conv(U, {&w}, {&b}, 1);
+                c.post = make_conv(U, DEC_IMAGES, {&w}, {&b}, 1);
                 c.tgt_off = 0;
             }
             v->flows.push_back(c);
         }
     }
-    v->conv_pre = conv_named(U, m, "dec.conv_pre");
+    v->conv_pre = conv_named(U, DEC_IMAGES, m, "dec.conv_pre");
     {
         int C = a.up_init;
         const int nk = (int)a.res_kernels.size();
@@ -435,56 +447,46 @@ Voice* load_voice(const std::string& config_path, int device) {
             st.u = a.up_rates[i]; st.k = a.up_kernels[i]; st.cin = C; st.cout = C / 2;
             const HostTensor& w = T(m, "dec.ups." + std::to_string(i) + ".weight");   // [cin][cout][k]
             const HostTensor& b = T(m, "dec.ups." + std::to_string(i) + ".bias");
+            // polyphase: output n = q*u + p reads input q + off through kernel index p + pad - off*u, for every off that
+            // puts the index in [0, k)
             const int pad = (st.k - st.u) / 2;
-            // polyphase: output n = q*u + p reads inputs q - d for every d with 0 <= d*u + p + pad < k
-            for (int p = 0; p < st.u; p++) {
-                const int pp = p + pad;
-                std::vector<int> ds;
-                for (int d = -st.k; d <= st.k; d++) { const int kk = d * st.u + pp; if (kk >= 0 && kk < st.k) ds.push_back(d); }
-                ConvW c;
-                c.cin = st.cin; c.cout = st.cout; c.ntaps = (int)ds.size();
-                const int bn = conv_simt_bn_for(c.cout);
-                c.ldw = (c.cout + bn - 1) / bn * bn;
-                c.min_off = 1 << 30; int mx = -(1 << 30);
-                std::vector<float> wt((size_t)c.ntaps * c.cin * c.ldw, 0.f), bt(c.ldw, 0.f);
+            auto kidx = [&](int p, int off) { const int kk = p + pad - off * st.u; return kk >= 0 && kk < st.k ? kk : -1; };
+            // phase p's weights, for the taps of c, into columns [col0, col0 + cout) of wt [ntaps][cin][ldw]
+            auto put_phase = [&](const ConvW& c, int p, int col0, std::vector<float>& wt) {
                 for (int t = 0; t < c.ntaps; t++) {
-                    c.tap_off[t] = -ds[t];
-                    c.min_off = std::min(c.min_off, c.tap_off[t]); mx = std::max(mx, c.tap_off[t]);
-                    const int kk = ds[t] * st.u + pp;
+                    const int kk = kidx(p, c.tap_off[t]);
+                    if (kk < 0) continue;
                     for (int ci = 0; ci < c.cin; ci++)
-                        for (int n = 0; n < c.cout; n++)
-                            wt[((size_t)t * c.cin + ci) * c.ldw + n] = w.f[((size_t)ci * st.cout + n) * st.k + kk];
+                        for (int n = 0; n < st.cout; n++)
+                            wt[((size_t)t * c.cin + ci) * c.ldw + col0 + n] = w.f[((size_t)ci * st.cout + n) * st.k + kk];
                 }
-                c.span = mx - c.min_off;
-                for (int n = 0; n < c.cout; n++) bt[n] = b.f[n];
-                c.w = U.up(wt); c.bias = U.up(bt);
-                add_tc_images(U, c, wt);
+            };
+            std::vector<int> all;    // union of the phases' taps
+            for (int p = 0; p < st.u; p++) {
+                std::vector<int> offs;      // descending: the order in which the fp32 kernel sums the taps
+                for (int off = st.k; off >= -st.k; off--)
+                    if (kidx(p, off) >= 0) offs.push_back(off);
+                ConvW c = conv_layout(st.cin, st.cout, offs);
+                std::vector<float> wt((size_t)c.ntaps * c.cin * c.ldw, 0.f), bt(c.ldw, 0.f);
+                put_phase(c, p, 0, wt);
+                std::copy(b.f.begin(), b.f.begin() + st.cout, bt.begin());
+                upload_conv(U, c, wt, bt, IMG_F32);
                 st.phase.push_back(c);
+                for (int off : offs)
+                    if (std::find(all.begin(), all.end(), off) == all.end()) all.push_back(off);
             }
-            {
-                // all phases as ONE conv: taps = union of the phase taps, column p*cout + co = phase p, channel co
-                std::vector<int> offs;
-                for (auto& ph : st.phase) for (int t = 0; t < ph.ntaps; t++)
-                    if (std::find(offs.begin(), offs.end(), ph.tap_off[t]) == offs.end()) offs.push_back(ph.tap_off[t]);
-                std::sort(offs.begin(), offs.end());
-                ConvW f;
-                f.cin = st.cin; f.cout = st.u * st.cout; f.ntaps = (int)offs.size(); f.ldw = f.cout;
-                f.min_off = offs.front(); f.span = offs.back() - offs.front();
+            if (all.size() <= SB_MAX_TAPS && st.cout % 32 == 0) {
+                // all phases as ONE conv (conv_tc): taps = union of the phase taps, column p*cout + co = phase p,
+                // channel co.  Its zero taps are no work: macs counts the ConvTranspose's own.
+                std::sort(all.begin(), all.end());
+                ConvW f = conv_layout(st.cin, st.u * st.cout, all, false);
+                f.macs = st.cin * st.cout * st.k;
                 std::vector<float> wt((size_t)f.ntaps * f.cin * f.ldw, 0.f), bt(f.ldw, 0.f);
                 for (int p = 0; p < st.u; p++) {
-                    const int pp = p + pad;
-                    for (int t = 0; t < f.ntaps; t++) {
-                        f.tap_off[t] = offs[t];
-                        const int kk = -offs[t] * st.u + pp;       // tap offset = -d, kernel index = d*u + p + pad
-                        if (kk < 0 || kk >= st.k) continue;
-                        for (int ci = 0; ci < f.cin; ci++)
-                            for (int n = 0; n < st.cout; n++)
-                                wt[((size_t)t * f.cin + ci) * f.ldw + p * st.cout + n] = w.f[((size_t)ci * st.cout + n) * st.k + kk];
-                    }
-                    for (int n = 0; n < st.cout; n++) bt[p * st.cout + n] = b.f[n];
+                    put_phase(f, p, p * st.cout, wt);
+                    std::copy(b.f.begin(), b.f.begin() + st.cout, bt.begin() + p * st.cout);
                 }
-                f.bias = U.up(bt);
-                if (f.ntaps <= SB_MAX_TAPS && st.cout % 32 == 0) add_tc_images(U, f, wt);
+                upload_conv(U, f, wt, bt, IMG_BF16);
                 st.fused = f;
             }
             C /= 2;
@@ -492,10 +494,10 @@ Voice* load_voice(const std::string& config_path, int device) {
                 ResBW rb; rb.k = a.res_kernels[j]; rb.dils = a.res_dils[j];
                 const std::string p = "dec.resblocks." + std::to_string(i * nk + j) + ".";
                 for (size_t d = 0; d < rb.dils.size(); d++) {
-                    if (a.resblock == 2) rb.c1.push_back(conv_named(U, m, p + "convs." + std::to_string(d), rb.dils[d]));
+                    if (a.resblock == 2) rb.c1.push_back(conv_named(U, DEC_IMAGES, m, p + "convs." + std::to_string(d), rb.dils[d]));
                     else {
-                        rb.c1.push_back(conv_named(U, m, p + "convs1." + std::to_string(d), rb.dils[d]));
-                        rb.c2.push_back(conv_named(U, m, p + "convs2." + std::to_string(d), 1));
+                        rb.c1.push_back(conv_named(U, DEC_IMAGES, m, p + "convs1." + std::to_string(d), rb.dils[d]));
+                        rb.c2.push_back(conv_named(U, DEC_IMAGES, m, p + "convs2." + std::to_string(d), 1));
                     }
                 }
                 st.res.push_back(rb);

@@ -27,12 +27,28 @@ def plan(backend, rows, cin, cout, k, dil, act=ACT_NONE, res=0, acc=0):
     return None if rc else list(o)
 
 
+def phase_fused_layers(q):
+    """(cin, cout, k, dil, act, res, acc) of each ConvTranspose1d run as one conv of u*cout columns.  Its taps are the
+    union of the phases' taps, derived as voice.cu does: output q*u + p reads input q + off through kernel index
+    p + pad - off*u.  On every shipped voice that union is {-1, 0, 1}, a centred k = 3 conv."""
+    a = voicegen.ARCH[q]
+    L, ch = [], a["up_init"]
+    for u, k in zip(a["up_rates"], a["up_kernels"]):
+        pad = (k - u) // 2
+        taps = {off for p in range(u) for off in range(-k, k + 1) if 0 <= p + pad - off * u < k}
+        assert taps == {-1, 0, 1}, (q, u, k, taps)
+        L.append((ch, u * (ch // 2), 3, 1, ACT_NONE, 0, 0))
+        ch //= 2
+    return L
+
+
 def decoder_and_flow_layers(q):
-    """(cin, cout, k, dil, act, res, acc) of every conv_tc layer of a voice (the phase-fused transposed convs aside)."""
+    """(cin, cout, k, dil, act, res, acc) of every conv_tc layer of a voice."""
     a = voicegen.ARCH[q]
     H, half = a["hidden"], a["inter"] // 2
     L = {(half, H, 1, 1, ACT_NONE, 0, 0), (H, 2 * H, a["flow_kernel"], 1, ACT_GATE, 0, 0), (H, 2 * H, 1, 1, ACT_NONE, 0, 1),
          (H, H, 1, 1, ACT_NONE, 0, 1), (H, half, 1, 1, ACT_NONE, 0, 0), (a["inter"], a["up_init"], 7, 1, ACT_NONE, 0, 0)}
+    L |= set(phase_fused_layers(q))
     ch = a["up_init"]
     for _ in a["up_rates"]:
         ch //= 2
@@ -79,6 +95,16 @@ def test_arithmetic_class_does_not_depend_on_launch_size(q):
             if nth < wnth:
                 assert mt * (lay[1] // 32) <= SMS or not two_stages_fit(win, lay[2], wnth, 2), (lay, rows, p)
         assert len(chunks) == 1, (lay, chunks)
+
+
+@pytest.mark.parametrize("q", ["medium", "high", "x_low", "low"])
+def test_phase_fused_transposed_convs_plan_at_every_size(q):
+    """The phase-fused ConvTranspose carries bf16 images only (its phases keep fp32 ones for backend 0), so on the
+    tensor-core backends conv_tc must take it at every launch size."""
+    for lay in phase_fused_layers(q):
+        for rows in ROWS:
+            p = plan(1, rows, *lay)
+            assert p is not None and p[5] <= SMEM_MAX, (q, lay, rows, p)
 
 
 def test_tile_width_cases_reach_several_widths():
