@@ -123,8 +123,8 @@ int32_t sb200_speak_batch_ids(sb200_voice* v, const int64_t* ids_packed, const s
  * fallback config for every utterance, i.e. sb200_speak_batch_ids.  Each entry is checked like
  * sb200_set_fallback_synthesis_config (a speaker must be in the voice's speaker_id_map; has_speaker == 0 means
  * speaker 0); an invalid entry fails the call with OPERATION_ERROR naming the utterance.  Utterance b's result equals
- * a single-utterance call with cfgs[b] as the fallback config, except for the on-device noise: its draws depend on
- * the utterance's position in the batch. */
+ * a single-utterance call with cfgs[b] as the fallback config, except for the on-device noise of an unseeded utterance:
+ * its draws depend on the utterance's position in the batch (see sb200_speak_batch_ids_seeded). */
 int32_t sb200_speak_batch_ids_configs(sb200_voice* v, const int64_t* ids_packed, const size_t* offsets, size_t batch,
                                       const sb200_synth_config* cfgs, sb200_audio* outs, sb200_error* err);
 
@@ -140,12 +140,27 @@ int32_t sb200_speak_batch_ids_configs(sb200_voice* v, const int64_t* ids_packed,
  * Frames per id (the reference's `p_duration`) come packed like ids_packed; samples of id i = frames * 256. */
 /* sb200_speak_batch_ids_configs with duration controls; id_frames_out (NULL: not wanted) receives the frames per id,
  * packed like ids_packed.  With NULL controls and NULL id_frames_out this is sb200_speak_batch_ids_configs, bit for bit.
- * Utterance b equals its single-utterance call with the same config and controls, except for the on-device noise:
- * its draws depend on the utterance's position in the batch. */
+ * Utterance b equals its single-utterance call with the same config and controls, except for the on-device noise of an
+ * unseeded utterance: its draws depend on the utterance's position in the batch. */
 int32_t sb200_speak_batch_ids_durations(sb200_voice* v, const int64_t* ids_packed, const size_t* offsets, size_t batch,
                                         const sb200_synth_config* cfgs, const float* scale_packed,
                                         const int32_t* frames_packed, sb200_audio* outs, int32_t* id_frames_out,
                                         sb200_error* err);
+
+/* ---- noise seeds: reproducible default-noise synthesis ----
+ * The graph draws eps_w [T_x][2] (scaled by noise_w) and eps_z [T_y][inter] (scaled by noise_scale).  Unseeded, they
+ * are Philox draws of the voice's call counter and the utterance's place in the packed batch.  A seeded utterance's
+ * draws are a function of its seed, the tensor, the row (id or frame index) and the column only, so the utterance
+ * equals itself run alone, bit for bit, whatever shares its batch, on every backend and every voice handle of the same
+ * file, and the noise of frame t does not depend on how many frames follow it.
+ * seeds[b] is utterance b's seed (any 64-bit value) when seeded[b] is 1; seeded[b] = 0 keeps its positional noise
+ * (bit for bit what a call without seeds gives it); seeded == NULL with seeds != NULL seeds every utterance; seeds ==
+ * NULL is a call without seeds.  A flag other than 0 / 1 fails with OPERATION_ERROR naming the utterance. */
+/* sb200_speak_batch_ids_durations with noise seeds; NULL seeds is that call, bit for bit. */
+int32_t sb200_speak_batch_ids_seeded(sb200_voice* v, const int64_t* ids_packed, const size_t* offsets, size_t batch,
+                                     const sb200_synth_config* cfgs, const float* scale_packed,
+                                     const int32_t* frames_packed, const uint64_t* seeds, const int32_t* seeded,
+                                     sb200_audio* outs, int32_t* id_frames_out, sb200_error* err);
 
 /* ---- job API: the same batched pass split into its host<->device steps (bench / multi-GPU plumbing) ----
  * create  : copies ids to the device (H2D).  `eps_w` / `eps_z` optionally inject the graph's two
@@ -162,13 +177,19 @@ int32_t sb200_job_set_debug(sb200_job* job, int32_t on);
 /* Per-utterance synthesis configs for the next sb200_job_run: cfgs[0 .. batch), or NULL for the voice's fallback config
  * (what a new job starts with, read at create time) for every utterance.  Entries are checked like
  * sb200_set_fallback_synthesis_config; an invalid one fails with OPERATION_ERROR naming the utterance and leaves the
- * job's configs unchanged.  Philox noise (no eps_w / eps_z given) depends on each utterance's batch position, as it
- * always has: only injected noise makes a mixed batch equal its utterances run alone. */
+ * job's configs unchanged.  Philox noise (no eps_w / eps_z given) of an unseeded utterance depends on its batch
+ * position, as it always has: injected noise or a seed (sb200_job_set_seeds) makes a mixed batch equal its utterances
+ * run alone. */
 int32_t sb200_job_set_configs(sb200_job* job, const sb200_synth_config* cfgs, sb200_error* err);
 /* Duration controls (see sb200_speak_batch_ids_durations) for the next sb200_job_run; NULL / NULL restores the default
  * (a job without controls, what a new job starts with).  Every entry is checked first; an invalid one fails with
  * OPERATION_ERROR naming the utterance and the id, and leaves the job's controls as they were. */
 int32_t sb200_job_set_durations(sb200_job* job, const float* scale_packed, const int32_t* frames_packed, sb200_error* err);
+/* Noise seeds (see sb200_speak_batch_ids_seeded) for the next sb200_job_run; seeds == NULL restores positional noise
+ * (what a new job starts with).  Seeds on a job created with injected eps_w / eps_z fail with OPERATION_ERROR, as does
+ * a bad flag; either leaves the job's seeds as they were.  With debug on, the run's noise is fetchable as "eps_w"
+ * ([T_x][2]) and "eps_z" ([T_y][inter]) when its scale is not 0 for some utterance. */
+int32_t sb200_job_set_seeds(sb200_job* job, const uint64_t* seeds, const int32_t* seeded, sb200_error* err);
 /* Frames per id of the last run, packed like ids_packed, into out_packed[0 .. capacity): one device->host copy of the
  * whole batch's cumulative durations, made on the first call after a run.  Fails before a run, or when capacity is
  * smaller than the number of ids. */
@@ -212,7 +233,7 @@ void sb200_latent_free(sb200_latent* z);
  * sb200_latent_free in any order (they share one device allocation, released with the last) and sharing ownership of
  * the voice like sb200_encode_ids' latents.  cfgs: one per utterance as for sb200_speak_batch_ids_configs (NULL = the
  * fallback config for every utterance); a bad entry fails the call naming the utterance.  As there, the on-device noise
- * draws depend on the utterance's position in the batch. */
+ * draws of an unseeded utterance depend on its position in the batch (see sb200_encode_batch_ids_seeded). */
 int32_t sb200_encode_batch_ids_configs(sb200_voice* v, const int64_t* ids_packed, const size_t* offsets, size_t batch,
                                        const sb200_synth_config* cfgs, sb200_latent** outs, sb200_error* err);
 /* sb200_encode_batch_ids_configs with duration controls (see sb200_speak_batch_ids_durations); NULL / NULL is that call,
@@ -220,6 +241,12 @@ int32_t sb200_encode_batch_ids_configs(sb200_voice* v, const int64_t* ids_packed
 int32_t sb200_encode_batch_ids_durations(sb200_voice* v, const int64_t* ids_packed, const size_t* offsets, size_t batch,
                                          const sb200_synth_config* cfgs, const float* scale_packed,
                                          const int32_t* frames_packed, sb200_latent** outs, sb200_error* err);
+/* sb200_encode_batch_ids_durations with noise seeds (see sb200_speak_batch_ids_seeded); NULL seeds is that call, bit for
+ * bit.  A seeded latent equals the `z` of the same utterance synthesised with the same seed. */
+int32_t sb200_encode_batch_ids_seeded(sb200_voice* v, const int64_t* ids_packed, const size_t* offsets, size_t batch,
+                                      const sb200_synth_config* cfgs, const float* scale_packed,
+                                      const int32_t* frames_packed, const uint64_t* seeds, const int32_t* seeded,
+                                      sb200_latent** outs, sb200_error* err);
 /* The encoder's `p_duration` (piper/src/lib.rs:675, 706-717) as frames per id of the latent's utterance (their sum is
  * its frame count, except that an utterance whose ids all got 0 frames is 1 frame long).  Returns the number of ids;
  * writes them to out only when capacity is at least that (call with NULL, 0 to learn the size). */

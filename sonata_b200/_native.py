@@ -72,13 +72,18 @@ SIGNATURES = {
                                                     C.POINTER(sb200_synth_config), C.POINTER(C.c_float),
                                                     C.POINTER(C.c_int32), C.POINTER(sb200_audio), C.POINTER(C.c_int32),
                                                     _ERR]),
+    "sb200_speak_batch_ids_seeded": (C.c_int32, [_P, C.POINTER(C.c_int64), C.POINTER(C.c_size_t), C.c_size_t,
+                                                 C.POINTER(sb200_synth_config), C.POINTER(C.c_float),
+                                                 C.POINTER(C.c_int32), C.POINTER(C.c_uint64), C.POINTER(C.c_int32),
+                                                 C.POINTER(sb200_audio), C.POINTER(C.c_int32), _ERR]),
     "sb200_job_create": (C.c_int32, [_P, C.POINTER(C.c_int64), C.POINTER(C.c_size_t), C.c_size_t,
                                      C.POINTER(C.POINTER(C.c_float)), C.POINTER(C.POINTER(C.c_float)),
                                      C.POINTER(C.c_size_t), C.POINTER(_P), _ERR]),
     "sb200_job_set_debug": (C.c_int32, [_P, C.c_int32]),
     "sb200_job_set_configs": (C.c_int32, [_P, C.POINTER(sb200_synth_config), _ERR]),
     "sb200_job_set_durations": (C.c_int32, [_P, C.POINTER(C.c_float), C.POINTER(C.c_int32), _ERR]),
-    "sb200_job_id_frames": (C.c_int32, [_P, C.POINTER(C.c_int32), C.c_size_t, _ERR]),
+    "sb200_job_set_seeds": (C.c_int32, [_P, C.POINTER(C.c_uint64), C.POINTER(C.c_int32), _ERR]),
+    "sb200_job_id_frames":(C.c_int32, [_P, C.POINTER(C.c_int32), C.c_size_t, _ERR]),
     "sb200_job_run": (C.c_int32, [_P, C.c_void_p, C.c_size_t, C.POINTER(C.c_float), _ERR]),
     "sb200_job_fetch": (C.c_int32, [_P, C.POINTER(sb200_audio), _ERR]),
     "sb200_job_fetch_i16": (C.c_int32, [_P, C.POINTER(C.POINTER(C.c_int16)), C.POINTER(C.c_size_t), _ERR]),
@@ -98,7 +103,11 @@ SIGNATURES = {
     "sb200_encode_batch_ids_durations": (C.c_int32, [_P, C.POINTER(C.c_int64), C.POINTER(C.c_size_t), C.c_size_t,
                                                      C.POINTER(sb200_synth_config), C.POINTER(C.c_float),
                                                      C.POINTER(C.c_int32), C.POINTER(_P), _ERR]),
-    "sb200_latent_id_frames": (C.c_int64, [_P, C.POINTER(C.c_int32), C.c_size_t]),
+    "sb200_encode_batch_ids_seeded": (C.c_int32, [_P, C.POINTER(C.c_int64), C.POINTER(C.c_size_t), C.c_size_t,
+                                                  C.POINTER(sb200_synth_config), C.POINTER(C.c_float),
+                                                  C.POINTER(C.c_int32), C.POINTER(C.c_uint64), C.POINTER(C.c_int32),
+                                                  C.POINTER(_P), _ERR]),
+    "sb200_latent_id_frames":(C.c_int64, [_P, C.POINTER(C.c_int32), C.c_size_t]),
     "sb200_decode_chunks": (C.c_int32, [_P, C.POINTER(_P), C.POINTER(C.c_int64), C.POINTER(C.c_int64), C.c_size_t,
                                         C.POINTER(sb200_audio), _ERR]),
     "sb200_decode_chunks_i16": (C.c_int32, [_P, C.POINTER(_P), C.POINTER(C.c_int64), C.POINTER(C.c_int64),

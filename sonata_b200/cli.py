@@ -39,13 +39,16 @@ def build_parser() -> argparse.ArgumentParser:
     ap.add_argument("--silence", type=int, help="Extra silence (ms) appended to each sentence")
     ap.add_argument("--chunk-size", type=int)
     ap.add_argument("--chunk-padding", type=int)
+    ap.add_argument("--seed", type=int, help="Noise seed [0, 2^64): sentence i uses seed + i, so the same input and seed "
+                                          "give the same samples (default: positional noise)")
     ap.add_argument("--device", type=int, default=int(os.environ.get("SONATA_B200_DEVICE", "0")))
     return ap
 
 
 def process_request(synth: SonataSpeechSynthesizer, default_cfg: PiperSynthesisConfig, req: dict,
                     output_file: Optional[str], out=None) -> None:
-    """process_synthesis_request (main.rs:126-165)"""
+    """process_synthesis_request (main.rs:126-165).  `seed` (optional): the request's noise seed, see
+    synth.sentence_seed."""
     out = out or sys.stdout.buffer
     synth.model.set_fallback_synthesis_config(PiperSynthesisConfig(
         req.get("speaker_id"),
@@ -54,16 +57,18 @@ def process_request(synth: SonataSpeechSynthesizer, default_cfg: PiperSynthesisC
         req["noise_w"] if req.get("noise_w") is not None else default_cfg.noise_w))
     oc = AudioOutputConfig(req.get("rate"), req.get("volume"), req.get("pitch"), req.get("appended_silence_ms"))
     text = req["text"]
+    seed = req.get("seed")
     if output_file:
-        synth.synthesize_to_file(output_file, text, oc)
+        synth.synthesize_to_file(output_file, text, oc, seed=seed)
         return
     mode = (req.get("mode") or "lazy").lower()
     if mode == "lazy":
-        stream = (a.samples for a in synth.synthesize_lazy(text, oc))
+        stream = (a.samples for a in synth.synthesize_lazy(text, oc, seed=seed))
     elif mode == "parallel":
-        stream = (a.samples for a in synth.synthesize_parallel(text, oc))
+        stream = (a.samples for a in synth.synthesize_parallel(text, oc, seed=seed))
     elif mode == "realtime":
-        stream = synth.synthesize_streamed(text, oc, req.get("chunk_size") or 100, req.get("chunk_padding") or 3)
+        stream = synth.synthesize_streamed(text, oc, req.get("chunk_size") or 100, req.get("chunk_padding") or 3,
+                                          seed=seed)
     else:
         raise ValueError(f"unknown synthesis mode `{mode}`")
     for samples in stream:
@@ -82,13 +87,15 @@ def main(argv=None) -> int:
         req = {"text": text, "mode": args.mode, "speaker_id": args.speaker_id, "length_scale": args.length_scale,
                "noise_scale": args.noise_scale, "noise_w": args.noise_w, "rate": args.rate, "volume": args.volume,
                "pitch": args.pitch, "appended_silence_ms": args.silence, "chunk_size": args.chunk_size,
-               "chunk_padding": args.chunk_padding}
+               "chunk_padding": args.chunk_padding, "seed": args.seed}
         process_request(synth, default_cfg, req, args.output_file)
     else:
         for i, line in enumerate(sys.stdin):
             if not line.strip():
                 continue
             req = json.loads(line)
+            if req.get("seed") is None:
+                req["seed"] = args.seed
             out_file = None
             if args.output_file:
                 stem, ext = os.path.splitext(args.output_file)

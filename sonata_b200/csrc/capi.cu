@@ -234,17 +234,19 @@ int32_t sb200_phonemes_to_input_ids_map(const sb200_voice* v, const char* ph, in
     });
 }
 
-int32_t sb200_speak_batch_ids_durations(sb200_voice* v, const int64_t* ids, const size_t* offsets, size_t batch,
-                                        const sb200_synth_config* cfgs, const float* scale_packed,
-                                        const int32_t* frames_packed, sb200_audio* outs, int32_t* id_frames_out,
-                                        sb200_error* err) {
+int32_t sb200_speak_batch_ids_seeded(sb200_voice* v, const int64_t* ids, const size_t* offsets, size_t batch,
+                                     const sb200_synth_config* cfgs, const float* scale_packed,
+                                     const int32_t* frames_packed, const uint64_t* seeds, const int32_t* seeded,
+                                     sb200_audio* outs, int32_t* id_frames_out, sb200_error* err) {
     return guarded(err, [&] {
         const double t0 = now_ms();
         static_assert(sizeof(long long) == sizeof(int64_t), "");
+        static_assert(sizeof(unsigned long long) == sizeof(uint64_t), "");
         std::unique_ptr<Job> j(create_job(v->v.get(), reinterpret_cast<const long long*>(ids), offsets, batch, nullptr,
                                           nullptr, nullptr, false));
         if (cfgs) set_job_configs(*j, cfgs_in(cfgs, batch).data());
         set_job_durations(*j, scale_packed, frames_packed);
+        set_job_seeds(*j, reinterpret_cast<const unsigned long long*>(seeds), seeded);
         j->run(nullptr, 0);
         fetch_audio(*j, outs, 0.f);
         if (id_frames_out) {
@@ -255,6 +257,13 @@ int32_t sb200_speak_batch_ids_durations(sb200_voice* v, const int64_t* ids, cons
         for (size_t b = 0; b < batch; b++)
             outs[b].inference_ms = wall * (j->total_samples ? (float)outs[b].len / (float)j->total_samples : 0.f);
     });
+}
+int32_t sb200_speak_batch_ids_durations(sb200_voice* v, const int64_t* ids, const size_t* offsets, size_t batch,
+                                        const sb200_synth_config* cfgs, const float* scale_packed,
+                                        const int32_t* frames_packed, sb200_audio* outs, int32_t* id_frames_out,
+                                        sb200_error* err) {
+    return sb200_speak_batch_ids_seeded(v, ids, offsets, batch, cfgs, scale_packed, frames_packed, nullptr, nullptr, outs,
+                                        id_frames_out, err);
 }
 int32_t sb200_speak_batch_ids_configs(sb200_voice* v, const int64_t* ids, const size_t* offsets, size_t batch,
                                       const sb200_synth_config* cfgs, sb200_audio* outs, sb200_error* err) {
@@ -302,6 +311,9 @@ int32_t sb200_job_set_configs(sb200_job* job, const sb200_synth_config* cfgs, sb
 }
 int32_t sb200_job_set_durations(sb200_job* job, const float* scale_packed, const int32_t* frames_packed, sb200_error* err) {
     return guarded(err, [&] { set_job_durations(*job->j, scale_packed, frames_packed); });
+}
+int32_t sb200_job_set_seeds(sb200_job* job, const uint64_t* seeds, const int32_t* seeded, sb200_error* err) {
+    return guarded(err, [&] { set_job_seeds(*job->j, reinterpret_cast<const unsigned long long*>(seeds), seeded); });
 }
 int32_t sb200_job_id_frames(sb200_job* job, int32_t* out_packed, size_t capacity, sb200_error* err) {
     return guarded(err, [&] {
@@ -399,15 +411,23 @@ int32_t sb200_decode_chunk(sb200_voice* v, const sb200_latent* z, int64_t lo, in
 }
 void sb200_latent_free(sb200_latent* z) { delete z; }
 
-int32_t sb200_encode_batch_ids_durations(sb200_voice* v, const int64_t* ids, const size_t* offsets, size_t batch,
-                                         const sb200_synth_config* cfgs, const float* scale_packed,
-                                         const int32_t* frames_packed, sb200_latent** outs, sb200_error* err) {
+int32_t sb200_encode_batch_ids_seeded(sb200_voice* v, const int64_t* ids, const size_t* offsets, size_t batch,
+                                      const sb200_synth_config* cfgs, const float* scale_packed,
+                                      const int32_t* frames_packed, const uint64_t* seeds, const int32_t* seeded,
+                                      sb200_latent** outs, sb200_error* err) {
     return guarded(err, [&] {
         const std::vector<SynthConfig> c = cfgs ? cfgs_in(cfgs, batch) : std::vector<SynthConfig>();
         std::vector<Latent*> ls = encode_latents(v->v.get(), reinterpret_cast<const long long*>(ids), offsets, batch,
-                                                 cfgs ? c.data() : nullptr, scale_packed, frames_packed);
+                                                 cfgs ? c.data() : nullptr, scale_packed, frames_packed,
+                                                 reinterpret_cast<const unsigned long long*>(seeds), seeded);
         for (size_t b = 0; b < batch; b++) outs[b] = new sb200_latent{ls[b], v->v};
     });
+}
+int32_t sb200_encode_batch_ids_durations(sb200_voice* v, const int64_t* ids, const size_t* offsets, size_t batch,
+                                         const sb200_synth_config* cfgs, const float* scale_packed,
+                                         const int32_t* frames_packed, sb200_latent** outs, sb200_error* err) {
+    return sb200_encode_batch_ids_seeded(v, ids, offsets, batch, cfgs, scale_packed, frames_packed, nullptr, nullptr, outs,
+                                         err);
 }
 int32_t sb200_encode_batch_ids_configs(sb200_voice* v, const int64_t* ids, const size_t* offsets, size_t batch,
                                        const sb200_synth_config* cfgs, sb200_latent** outs, sb200_error* err) {

@@ -200,6 +200,15 @@ struct GatherSeg { const float* src; long long lo; int off; int len; };
 // cols is a multiple of 4 and every src is 16-byte aligned.
 void launch_gather_rows(const GatherSeg* segs, const int* tile_seg, int gran, int rows, int cols, float* s, cudaStream_t st);
 void launch_randn(float* out, long long n, unsigned long long seed, unsigned long long stream_id, cudaStream_t st);
+// One utterance's noise seed (seeded = 0: positional noise).
+struct NoiseSeed { unsigned long long seed; int seeded; int pad; };
+// launch_randn's buffer of map.rows x cols values, except that the valid rows of seeded segments (segment of a row:
+// seg_of_gran, its first row: segs[].off) get the keyed draws of their segment's seed and tensor `tag` (0: eps_w,
+// 1: eps_z), a function of the row within the utterance and the column only (kernels_misc.cu).
+void launch_randn_seeded(float* out, int cols, unsigned tag, unsigned long long seed, unsigned long long stream_id,
+                         const NoiseSeed* seeds, const SegInfo* segs, const int* seg_of_gran, RowMap map, cudaStream_t st);
+void launch_randn_seeded(float* out, int cols, unsigned tag, unsigned long long seed, unsigned long long stream_id,
+                         const NoiseSeed* seeds, const FrameSeg* segs, const int* seg_of_gran, RowMap map, cudaStream_t st);
 // z[r][0..1] = eps * s[seg_of_gran[r / map.gran]]
 void launch_scale_copy2(const float* eps, const float* s, const int* seg_of_gran, float* z, RowMap map, cudaStream_t st);
 // out[s][r] = base[r] + sum_k w[r][k] * emb_g[sid[s]][k]  for every slot s < nslots   (speaker conditioning: effective

@@ -221,6 +221,21 @@ void set_job_durations(Job& j, const float* scale, const int* frames) {
     if (frames) j.dur_frames.assign(frames, frames + n); else j.dur_frames.clear();
 }
 
+void set_job_seeds(Job& j, const unsigned long long* seeds, const int* seeded) {
+    if (!seeds) { j.seeds.clear(); return; }
+    std::vector<NoiseSeed> s(j.B);
+    bool any = false;
+    for (size_t b = 0; b < j.B; b++) {
+        const int f = seeded ? seeded[b] : 1;
+        if (f != 0 && f != 1) throw Error(19, "utterance " + std::to_string(b) + ": seeded flag " + std::to_string(f) + " is neither 0 nor 1");
+        if (f && (!j.eps_w.empty() || !j.eps_z.empty()))     // injection zero-fills the utterances it leaves out
+            throw Error(19, "utterance " + std::to_string(b) + ": a noise seed on a job with injected eps_w / eps_z");
+        s[b] = NoiseSeed{f ? seeds[b] : 0ull, f, 0};
+        any |= f != 0;
+    }
+    if (any) j.seeds.swap(s); else j.seeds.clear();
+}
+
 namespace {
 
 struct Runner {
@@ -311,6 +326,7 @@ struct IdBufs {
     float *att_s, *att_vt, *att_orel;          // tensor-core attention: scores of every head, V^T, relative-value term
     float *epsw, *cond;                        // cond: [slot][cond_rows]
     float *dscale, *dscale_h; int *dframes, *dframes_h;   // per-id duration controls (only when the job has them)
+    NoiseSeed *seeds, *seeds_h;                // per utterance (only when the job has seeds; read at both levels)
     float *qkv0, *att0, *p0, *vt0;             // debug: layer 0's attention operands and result
     std::vector<std::array<float*, 4>> dpf;    // debug: each duration flow's input, DDSConv output, spline parameters, output
 
@@ -342,7 +358,9 @@ struct IdBufs {
         const bool scaled = !j.dur_scale.empty(), fixed = !j.dur_frames.empty();
         dscale = scaled ? dev.get<float>(RX) : nullptr; dscale_h = scaled ? pin.get<float>(RX) : nullptr;
         dframes = fixed ? dev.get<int>(RX) : nullptr; dframes_h = fixed ? pin.get<int>(RX) : nullptr;
-        qkv0 = att0 = p0 = vt0 = nullptr;
+        const bool seeded = !j.seeds.empty();
+        seeds = seeded ? dev.get<NoiseSeed>(B) : nullptr; seeds_h = seeded ? pin.get<NoiseSeed>(B) : nullptr;
+        qkv0 =att0 = p0 = vt0 = nullptr;
         dpf.clear();
         if (j.debug) {
             qkv0 = rows(3 * H); att0 = rows(H);
@@ -662,6 +680,10 @@ void Job::run(float* d_out, size_t d_out_cap) {
         if (x.dscale) h2d(x.dscale, x.dscale_h, (size_t)RX * 4, st);
         if (x.dframes) h2d(x.dframes, x.dframes_h, (size_t)RX * 4, st);
     }
+    if (x.seeds) {
+        std::copy(seeds.begin(), seeds.end(), x.seeds_h);
+        h2d(x.seeds, x.seeds_h, B * sizeof(NoiseSeed), st);
+    }
     if (tc_att) {
         memcpy(x.tiles_h, tiles_s.data(), tiles_s.size() * sizeof(TfTile));
         memcpy(x.tiles_h + tiles_s.size(), tiles_o.data(), tiles_o.size() * sizeof(TfTile));
@@ -703,9 +725,12 @@ void Job::run(float* d_out, size_t d_out_cap) {
                 if (!eps_w[b].empty()) memcpy(stage.data() + (size_t)xsegs[b].off * 2, eps_w[b].data(), eps_w[b].size() * 4);
             SB_CUDA(cudaMemcpyAsync(x.epsw, stage.data(), stage.size() * 4, cudaMemcpyHostToDevice, st));
             SB_CUDA(cudaStreamSynchronize(st));   // `stage` is pageable; injection is a test-only path
+        } else if (x.seeds) {
+            launch_randn_seeded(x.epsw, 2, 0, V.noise_seed, 2 * noise_call, x.seeds, x.xsegs, x.xseg_of_gran, LX.map, st);
         } else {
             launch_randn(x.epsw, (long long)RX * 2, V.noise_seed, 2 * noise_call, st);
         }
+        if (debug) expose(*this, "eps_w", x.epsw, 2, 0);
     }
 
     // ---------------- speaker conditioning (multi-speaker voices) ----------------
@@ -816,9 +841,12 @@ void Job::run(float* d_out, size_t d_out_cap) {
                 if (!eps_z[b].empty()) memcpy(stage.data() + (size_t)fsegs[b].off * I, eps_z[b].data(), eps_z[b].size() * 4);
             SB_CUDA(cudaMemcpyAsync(f.epsz, stage.data(), stage.size() * 4, cudaMemcpyHostToDevice, st));
             SB_CUDA(cudaStreamSynchronize(st));
+        } else if (x.seeds) {
+            launch_randn_seeded(f.epsz, I, 1, V.noise_seed, 2 * noise_call + 1, x.seeds, f.y.fsegs, f.y.ftile, LY.map, st);
         } else {
             launch_randn(f.epsz, (long long)RY * I, V.noise_seed, 2 * noise_call + 1, st);
         }
+        if (debug) expose(*this, "eps_z", f.epsz, I, 1);
     }
     launch_expand(x.stats, 2 * I, I, x.cum, f.epsz, x.scales + 2 * B, f.s, f.y.fsegs, f.y.ftile, LY.map, st);
     R.count(0, 4.0 * LY.valid_rows * 3 * I);
@@ -870,10 +898,12 @@ void Job::run(float* d_out, size_t d_out_cap) {
 
 // ====================================================================== streaming halves
 std::vector<Latent*> encode_latents(Voice* v, const long long* ids, const size_t* offs, size_t B, const SynthConfig* cfgs,
-                                    const float* scale, const int* frames) {
+                                    const float* scale, const int* frames, const unsigned long long* seeds,
+                                    const int* seeded) {
     std::unique_ptr<Job> j(create_job(v, ids, offs, B, nullptr, nullptr, nullptr, false));
     if (cfgs) set_job_configs(*j, cfgs);
     set_job_durations(*j, scale, frames);
+    set_job_seeds(*j, seeds, seeded);
     j->encode_only = true;
     j->run(nullptr, 0);
     const size_t I = (size_t)v->a.inter;

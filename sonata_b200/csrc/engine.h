@@ -201,6 +201,7 @@ struct Job {
     std::vector<float> dur_scale; std::vector<int> dur_frames;
     std::vector<int> id_frames;       // frames per id of the last run, packed like ids: filled by job_id_frames
     std::vector<std::vector<float>> eps_w, eps_z; std::vector<size_t> eps_z_frames;
+    std::vector<NoiseSeed> seeds;     // one per utterance, empty when none is seeded (set_job_seeds)
     // X layout
     int RX = 0; std::vector<SegInfo> xsegs; int max_tx = 0;
     // Y layout
@@ -239,6 +240,12 @@ void set_job_configs(Job& j, const SynthConfig* cfgs);
 // entry is checked first; an error names the utterance and the id, and leaves the job's controls as they were.  Null
 // and null restores the default (no controls, the kernel reads none).
 void set_job_durations(Job& j, const float* scale, const int* frames);
+// Per-utterance noise seeds of the job's next run: utterance b is seeded when seeded[b] is 1 (every utterance when
+// seeded is null), and its eps_w / eps_z are then keyed draws of seeds[b] that do not depend on the batch
+// (kernels_misc.cu randn_seg_kernel); seeded[b] = 0 keeps its positional noise.  Null seeds restores positional noise
+// for all.  Flags other than 0 / 1, or seeds on a job with injected noise, fail naming the utterance and leave the job
+// as it was.
+void set_job_seeds(Job& j, const unsigned long long* seeds, const int* seeded);
 // Frames per id of the job's last run, packed like its ids: one device->host copy of the batch's cum rows through the
 // context's page-locked staging, differenced on the host.  Cached until the next run.
 const std::vector<int>& job_id_frames(Job& j);
@@ -252,10 +259,11 @@ struct Latent {
     std::vector<int> id_frames;   // frames per id of the encoder pass (the reference's p_duration)
 };
 // One encoder pass over B utterances (cfgs: one per utterance, or null for the voice's fallback config; scale / frames:
-// per-id duration controls as for set_job_durations, or null) -> B latents sharing one device allocation.  The caller
-// owns the returned pointers.
+// per-id duration controls as for set_job_durations, or null; seeds / seeded: noise seeds as for set_job_seeds) -> B
+// latents sharing one device allocation.  The caller owns the returned pointers.
 std::vector<Latent*> encode_latents(Voice* v, const long long* ids, const size_t* offs, size_t B, const SynthConfig* cfgs,
-                                    const float* scale = nullptr, const int* frames = nullptr);
+                                    const float* scale = nullptr, const int* frames = nullptr,
+                                    const unsigned long long* seeds = nullptr, const int* seeded = nullptr);
 Latent* encode_latent(Voice* v, const long long* ids, size_t n);
 // One frame-level decoder pass over n chunks z[k][lo[k] : hi[k]) of latents of `v`; out[k] gets chunk k's waveform.
 // Chunk k equals the same chunk decoded alone, bit for bit.  ms: the pass's device time.

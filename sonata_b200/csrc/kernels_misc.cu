@@ -739,13 +739,10 @@ __device__ __forceinline__ void philox_round(unsigned& c0, unsigned& c1, unsigne
     c0 = n0; c1 = n1; c2 = n2; c3 = n3;
 }
 
-__global__ void randn_kernel(float* __restrict__ out, long long n, unsigned long long seed,
-                             unsigned long long stream_id) {
-    pdl_trigger(); pdl_wait();
-    const long long i4 = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i4 * 4 >= n) return;
-    unsigned c0 = (unsigned)i4, c1 = (unsigned)(i4 >> 32), c2 = (unsigned)stream_id, c3 = (unsigned)(stream_id >> 32);
-    unsigned k0 = (unsigned)seed, k1 = (unsigned)(seed >> 32);
+// Four N(0,1) values from one Philox4x32-10 block of counter (c0..c3) under key (k0, k1), by Box-Muller
+// (tests/noise_reference.py restates it on the host).
+__device__ __forceinline__ void philox_normal4(unsigned c0, unsigned c1, unsigned c2, unsigned c3, unsigned k0,
+                                               unsigned k1, float v[4]) {
 #pragma unroll
     for (int r = 0; r < 10; r++) {
         philox_round(c0, c1, c2, c3, k0, k1);
@@ -759,7 +756,52 @@ __global__ void randn_kernel(float* __restrict__ out, long long n, unsigned long
     float s0, cs0, s1, cs1;
     sincosf(6.283185307179586f * u1, &s0, &cs0);
     sincosf(6.283185307179586f * u3, &s1, &cs1);
-    const float v[4] = {r0 * cs0, r0 * s0, r1 * cs1, r1 * s1};
+    v[0] = r0 * cs0; v[1] = r0 * s0; v[2] = r1 * cs1; v[3] = r1 * s1;
+}
+
+// Positional noise: quad i4 of the buffer is counter (i4, i4 >> 32, stream_id, stream_id >> 32) under the voice's key.
+__global__ void randn_kernel(float* __restrict__ out, long long n, unsigned long long seed,
+                             unsigned long long stream_id) {
+    pdl_trigger(); pdl_wait();
+    const long long i4 = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i4 * 4 >= n) return;
+    float v[4];
+    philox_normal4((unsigned)i4, (unsigned)(i4 >> 32), (unsigned)stream_id, (unsigned)(stream_id >> 32), (unsigned)seed,
+                   (unsigned)(seed >> 32), v);
+    for (int e = 0; e < 4; e++)
+        if (i4 * 4 + e < n) out[i4 * 4 + e] = v[e];
+}
+
+// randn_kernel's buffer [rows][cols] with keyed draws for seeded segments.  The quad starting at row r, column c
+// belongs to the segment of r's granule; when r is a valid row of a seeded segment it is counter (q, q >> 32, tag, 0)
+// under key (seed, seed >> 32), q = ((r - off) * cols + c) / 4, off the segment's first row.  That draw depends on the
+// seed, the tensor (tag), the row within the utterance and the column only, never on the batch around it.  Every other
+// quad (gap rows, unseeded segments) gets randn_kernel's value at the same flat index.  cols is 2 at the id level
+// (segments start on 64-row boundaries, so a quad never leaves its segment; the second row of the last quad of an odd
+// length segment is a gap row that takes the keyed value, and no consumer reads it) and inter, a multiple of 4, at the
+// frame level.
+template <typename Seg>
+__global__ void randn_seg_kernel(float* __restrict__ out, long long n, unsigned long long seed,
+                                 unsigned long long stream_id, int cols, unsigned tag,
+                                 const NoiseSeed* __restrict__ seeds, const Seg* __restrict__ segs,
+                                 const int* __restrict__ seg_of_gran, RowMap map) {
+    pdl_trigger(); pdl_wait();
+    const long long i4 = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i4 * 4 >= n) return;
+    const int r = (int)(i4 * 4 / cols), c = (int)(i4 * 4 - (long long)r * cols);
+    unsigned c0 = (unsigned)i4, c1 = (unsigned)(i4 >> 32), c2 = (unsigned)stream_id, c3 = (unsigned)(stream_id >> 32);
+    unsigned long long key = seed;
+    if (row_valid(map, r)) {
+        const int s = seg_of_gran[r / map.gran];
+        const NoiseSeed ns = seeds[s];
+        if (ns.seeded) {
+            const unsigned long long q = ((unsigned long long)(r - segs[s].off) * (unsigned)cols + (unsigned)c) >> 2;
+            c0 = (unsigned)q; c1 = (unsigned)(q >> 32); c2 = tag; c3 = 0u;
+            key = ns.seed;
+        }
+    }
+    float v[4];
+    philox_normal4(c0, c1, c2, c3, (unsigned)key, (unsigned)(key >> 32), v);
     for (int e = 0; e < 4; e++)
         if (i4 * 4 + e < n) out[i4 * 4 + e] = v[e];
 }
@@ -924,6 +966,23 @@ void launch_randn(float* out, long long n, unsigned long long seed, unsigned lon
     const long long n4 = (n + 3) / 4;
     launch_pdl(randn_kernel, dim3((unsigned)((n4 + 255) / 256)), dim3(256), 0, st, out, n, seed, stream_id);
     g_launch_count++;
+}
+
+template <typename Seg>
+static void randn_seg(float* out, int cols, unsigned tag, unsigned long long seed, unsigned long long stream_id,
+                      const NoiseSeed* seeds, const Seg* segs, const int* seg_of_gran, RowMap map, cudaStream_t st) {
+    const long long n = (long long)map.rows * cols, n4 = (n + 3) / 4;
+    launch_pdl(randn_seg_kernel<Seg>, dim3((unsigned)((n4 + 255) / 256)), dim3(256), 0, st, out, n, seed, stream_id, cols,
+               tag, seeds, segs, seg_of_gran, map);
+    g_launch_count++;
+}
+void launch_randn_seeded(float* out, int cols, unsigned tag, unsigned long long seed, unsigned long long stream_id,
+                         const NoiseSeed* seeds, const SegInfo* segs, const int* seg_of_gran, RowMap map, cudaStream_t st) {
+    randn_seg(out, cols, tag, seed, stream_id, seeds, segs, seg_of_gran, map, st);
+}
+void launch_randn_seeded(float* out, int cols, unsigned tag, unsigned long long seed, unsigned long long stream_id,
+                         const NoiseSeed* seeds, const FrameSeg* segs, const int* seg_of_gran, RowMap map, cudaStream_t st) {
+    randn_seg(out, cols, tag, seed, stream_id, seeds, segs, seg_of_gran, map, st);
 }
 
 void launch_cond_bias(const float* w, const float* base, const float* emb_g, const int* sid, int nslots, int rows, int gin,

@@ -10,19 +10,22 @@ import numpy as np
 
 from . import _native as N
 from .core import Audio
-from .piper import _check, _config_array, _duration_arrays, _ptr, _take_audio
+from .piper import _check, _config_array, _duration_arrays, _ptr, _seed_arrays, _take_audio
 
 
 class SynthesisJob:
     def __init__(self, model, batches: Sequence[Sequence[int]], eps_w: Optional[Sequence] = None,
-                 eps_z: Optional[Sequence] = None, debug: bool = False, configs: Optional[Sequence] = None):
-        """`configs`: one PiperSynthesisConfig per utterance (see set_configs); None keeps the voice's fallback config."""
+                 eps_z: Optional[Sequence] = None, debug: bool = False, configs: Optional[Sequence] = None,
+                 seeds: Optional[Sequence] = None):
+        """`configs`: one PiperSynthesisConfig per utterance (see set_configs); None keeps the voice's fallback config.
+        `seeds`: noise seeds (see set_seeds)."""
         self._m = model
         self._lib = model._lib
         n = len(batches)
         self.batch = n
         self._lens = [len(b) for b in batches]
         _config_array(configs, n)             # argument errors before the job exists
+        _seed_arrays(seeds, n)
         packed = np.ascontiguousarray(np.concatenate([np.asarray(b, dtype=np.int64) for b in batches]))
         offs = np.zeros(n + 1, dtype=np.uint64)
         offs[1:] = np.cumsum([len(b) for b in batches])
@@ -55,6 +58,8 @@ class SynthesisJob:
             self._lib.sb200_job_set_debug(self._h, 1)
         if configs is not None:
             self.set_configs(configs)
+        if seeds is not None:
+            self.set_seeds(seeds)
 
     def set_configs(self, configs: Optional[Sequence]) -> None:
         """Per-utterance PiperSynthesisConfigs for the next run, or None for the voice's fallback config.  A wrong
@@ -69,6 +74,15 @@ class SynthesisJob:
         sc, fr = _duration_arrays(self._lens, scales, frames)
         err = N.sb200_error()
         _check(self._lib.sb200_job_set_durations(self._h, _ptr(sc, C.c_float), _ptr(fr, C.c_int32), C.byref(err)), err)
+
+    def set_seeds(self, seeds: Optional[Sequence]) -> None:
+        """Per-utterance noise seeds for the next run (see VitsModel.infer_batch_with_values): an int in [0, 2**64) or
+        None per utterance; None for the whole list restores positional noise.  With debug on, the run's draws are
+        fetchable as "eps_w" and "eps_z".  A bad entry, or seeds on a job with injected noise, raises OperationError
+        and leaves the job's seeds as they were."""
+        sv, sf = _seed_arrays(seeds, self.batch)
+        err = N.sb200_error()
+        _check(self._lib.sb200_job_set_seeds(self._h, _ptr(sv, C.c_uint64), _ptr(sf, C.c_int32), C.byref(err)), err)
 
     def id_frames(self) -> List[np.ndarray]:
         """Frames per id of the last run, one int32 array per utterance (one device->host copy for the batch)."""

@@ -123,6 +123,26 @@ def _duration_arrays(lens: Sequence[int], duration_scales=None, durations=None):
     return scales, frames
 
 
+def _seed_arrays(seeds, n: int):
+    """The C image of per-utterance noise seeds: (seeds u64, seeded i32), or (None, None) when `seeds` is None or holds
+    no seed.  seeds[b] is an int in [0, 2**64) or None (utterance b keeps its positional noise)."""
+    if seeds is None:
+        return None, None
+    vals = np.zeros(n, np.uint64)
+    flags = np.zeros(n, np.int32)
+    for b, s in enumerate(_per_utterance(seeds, n, "noise seeds")):
+        if s is None:
+            continue
+        if isinstance(s, bool) or not isinstance(s, numbers.Integral):
+            raise OperationError(f"utterance {b}: noise seed {s!r} is not an integer")
+        if not 0 <= int(s) < 2**64:
+            raise OperationError(f"utterance {b}: noise seed {int(s)} is not in [0, 2**64)")
+        vals[b], flags[b] = int(s), 1
+    if not flags.any():
+        return None, None
+    return vals, flags
+
+
 def _ptr(a, ctype):
     return None if a is None else a.ctypes.data_as(C.POINTER(ctype))
 
@@ -296,15 +316,18 @@ class _VitsCommons:
         return _take_audio(a)
 
     def speak_batch(self, phoneme_batches: Sequence[str],
-                    configs: Optional[Sequence[PiperSynthesisConfig]] = None) -> List[Audio]:
+                    configs: Optional[Sequence[PiperSynthesisConfig]] = None, seeds: Optional[Sequence] = None) -> List[Audio]:
         """`configs`: one PiperSynthesisConfig per utterance (speaker and scales), still synthesised as one pass;
-        None uses the fallback config for every utterance."""
+        None uses the fallback config for every utterance.  `seeds`: noise seeds as for infer_batch_with_values."""
         n = len(phoneme_batches)
         _config_array(configs, n)             # argument errors before any id mapping
+        sv, _ = _seed_arrays(seeds, n)
         if n == 0:
             return []
-        if configs is not None:
-            return self.infer_batch_with_values([self.phonemes_to_input_ids(p) for p in phoneme_batches], configs)
+        if configs is not None or sv is not None:
+            extra = {} if sv is None else {"seeds": seeds}
+            return self.infer_batch_with_values([self.phonemes_to_input_ids(p) for p in phoneme_batches], configs,
+                                                **extra)
         arr = (C.c_char_p * n)(*[p.encode("utf-8") for p in phoneme_batches])
         outs = (N.sb200_audio * n)()
         err = N.sb200_error()
@@ -320,12 +343,20 @@ class _VitsCommons:
         return _take_audio(a)
 
     def infer_batch_with_values(self, batches: Sequence[Sequence[int]],
-                                configs: Optional[Sequence[PiperSynthesisConfig]] = None) -> List[Audio]:
+                                configs: Optional[Sequence[PiperSynthesisConfig]] = None,
+                                seeds: Optional[Sequence] = None) -> List[Audio]:
         """Batched infer_with_values.  `configs`: one PiperSynthesisConfig per utterance (speaker and scales), or None
         for the fallback config; each utterance's result equals a single-utterance call with its config as the
-        fallback, except for the on-device noise, whose draws depend on the batch position."""
+        fallback, except for the on-device noise of an unseeded utterance, whose draws depend on the batch position.
+
+        `seeds`: one noise seed per utterance, an int in [0, 2**64) or None.  A seeded utterance's noise depends on its
+        seed alone, so its result is the same bits in any batch, on any call and on any handle of the voice; an
+        unseeded one keeps the positional noise of a call without seeds."""
         n = len(batches)
         cfgs = _config_array(configs, n)
+        sv, _ = _seed_arrays(seeds, n)
+        if sv is not None:
+            return [a for a, _ in self.infer_batch_with_durations(batches, configs, seeds=seeds)]
         packed = np.ascontiguousarray(np.concatenate([np.asarray(b, dtype=np.int64) for b in batches]))
         offs = np.zeros(n + 1, dtype=np.uint64)
         offs[1:] = np.cumsum([len(b) for b in batches])
@@ -339,17 +370,20 @@ class _VitsCommons:
     def infer_batch_with_durations(self, batches: Sequence[Sequence[int]],
                                    configs: Optional[Sequence[PiperSynthesisConfig]] = None,
                                    duration_scales: Optional[Sequence] = None,
-                                   durations: Optional[Sequence] = None) -> List[Tuple[Audio, np.ndarray]]:
+                                   durations: Optional[Sequence] = None,
+                                   seeds: Optional[Sequence] = None) -> List[Tuple[Audio, np.ndarray]]:
         """infer_batch_with_values with per-id duration control, returning (audio, frames per id) per utterance.
 
         duration_scales[b]: one scale (finite, >= 0) per id of utterance b, applied before the duration's ceil, so 1.0
         gives the plain result bit for bit; durations[b]: one frame count per id, -1 for "predicted" or >= 0 to fix it.
         Either list, or any of its entries, may be None.  The frame counts times 256 are each id's samples; an
-        utterance whose ids all got 0 frames is still one frame long."""
+        utterance whose ids all got 0 frames is still one frame long.  `seeds`: as for infer_batch_with_values; a
+        seeded frame's noise depends on its index only, so controls that move frames never reshuffle it."""
         n = len(batches)
         cfgs = _config_array(configs, n)
         lens = [len(b) for b in batches]
         scales, frames = _duration_arrays(lens, duration_scales, durations)
+        sv, sf = _seed_arrays(seeds, n)
         if n == 0:
             return []
         if any(x == 0 for x in lens):
@@ -360,22 +394,26 @@ class _VitsCommons:
         outs = (N.sb200_audio * n)()
         id_frames = np.zeros(int(offs[-1]), np.int32)
         err = N.sb200_error()
-        _check(self._lib.sb200_speak_batch_ids_durations(
+        _check(self._lib.sb200_speak_batch_ids_seeded(
             self._h, packed.ctypes.data_as(C.POINTER(C.c_int64)), offs.ctypes.data_as(C.POINTER(C.c_size_t)), n, cfgs,
-            _ptr(scales, C.c_float), _ptr(frames, C.c_int32), outs, _ptr(id_frames, C.c_int32), C.byref(err)), err)
+            _ptr(scales, C.c_float), _ptr(frames, C.c_int32), _ptr(sv, C.c_uint64), _ptr(sf, C.c_int32), outs,
+            _ptr(id_frames, C.c_int32), C.byref(err)), err)
         return [(_take_audio(outs[b]), id_frames[int(offs[b]):int(offs[b + 1])].copy()) for b in range(n)]
 
     def speak_batch_with_alignment(self, phoneme_batches: Sequence[str],
                                    configs: Optional[Sequence[PiperSynthesisConfig]] = None,
-                                   duration_scales: Optional[Sequence] = None) -> List[Tuple[Audio, List[PhonemeAlignment]]]:
+                                   duration_scales: Optional[Sequence] = None,
+                                   seeds: Optional[Sequence] = None) -> List[Tuple[Audio, List[PhonemeAlignment]]]:
         """speak_batch that also says when each phoneme is spoken: per utterance (audio, alignment), the alignment
         holding one entry for bos (`^`), one per kept phoneme character (its id and its trailing pad) and one for eos
         (`$`), contiguous from sample 0 to len(audio).
 
         duration_scales[b] (or None): one scale per character of phoneme_batches[b], applied to that character's id and
-        pad; characters the voice drops have no entry and their scales are ignored."""
+        pad; characters the voice drops have no entry and their scales are ignored.  `seeds`: as for
+        infer_batch_with_values."""
         n = len(phoneme_batches)
         _config_array(configs, n)
+        _seed_arrays(seeds, n)
         per_char = None if duration_scales is None else _per_utterance(duration_scales, n, "duration scales")
         maps = [self.phonemes_to_input_ids_map(p) for p in phoneme_batches]
         id_scales = None
@@ -391,7 +429,8 @@ class _VitsCommons:
                     raise OperationError(f"utterance {b}: {len(v)} duration scales for {len(ph)} characters")
                 kept = {c: _scale_value(v[c], b, c, "character") for c in sorted(set(src)) if c >= 0}
                 id_scales.append([1.0 if c < 0 else kept[c] for c in src])
-        res = self.infer_batch_with_durations([m[0] for m in maps], configs, id_scales)
+        extra = {} if seeds is None else {"seeds": seeds}
+        res = self.infer_batch_with_durations([m[0] for m in maps], configs, id_scales, **extra)
         return [(audio, _alignment(ph, src, frames, len(audio)))
                 for ph, (_, src), (audio, frames) in zip(phoneme_batches, maps, res)]
 
@@ -435,7 +474,7 @@ class _VitsCommons:
     def supports_streaming_output(self) -> bool:
         return False
 
-    def stream_synthesis(self, phonemes: str, chunk_size: int, chunk_padding: int):
+    def stream_synthesis(self, phonemes: str, chunk_size: int, chunk_padding: int, seed: Optional[int] = None):
         raise OperationError("Streaming synthesis is not supported for this model")
 
     def set_backend(self, backend: int) -> int:
@@ -509,14 +548,18 @@ class VitsStreamingModel(_VitsCommons):
     def infer_encoder_batch(self, batches: Sequence[Sequence[int]],
                             configs: Optional[Sequence[PiperSynthesisConfig]] = None,
                             duration_scales: Optional[Sequence] = None,
-                            durations: Optional[Sequence] = None) -> List[EncoderOutputs]:
+                            durations: Optional[Sequence] = None,
+                            seeds: Optional[Sequence] = None) -> List[EncoderOutputs]:
         """infer_encoder over many utterances in one encoder pass.  `configs`: one PiperSynthesisConfig per utterance,
         or None for the fallback config; each latent equals infer_encoder alone with its config as the fallback,
-        except for the on-device noise, whose draws depend on the batch position.  `duration_scales` / `durations`:
-        per-id duration controls as for infer_batch_with_durations; each output's `p_duration` holds its frames per id."""
+        except for the on-device noise of an unseeded utterance, whose draws depend on the batch position.
+        `duration_scales` / `durations`: per-id duration controls as for infer_batch_with_durations; each output's
+        `p_duration` holds its frames per id.  `seeds`: noise seeds as for infer_batch_with_values; a seeded latent
+        equals the `z` of the same utterance synthesised with the same seed."""
         n = len(batches)
         cfgs = _config_array(configs, n)
         scales, frames = _duration_arrays([len(b) for b in batches], duration_scales, durations)
+        sv, sf = _seed_arrays(seeds, n)
         if any(len(b) == 0 for b in batches):
             raise OperationError("Failed to run model inference. Error: empty input sequence")
         if n == 0:
@@ -526,10 +569,11 @@ class VitsStreamingModel(_VitsCommons):
         offs[1:] = np.cumsum([len(b) for b in batches])
         outs = (C.c_void_p * n)()
         err = N.sb200_error()
-        _check(self._lib.sb200_encode_batch_ids_durations(self._h, packed.ctypes.data_as(C.POINTER(C.c_int64)),
-                                                          offs.ctypes.data_as(C.POINTER(C.c_size_t)), n, cfgs,
-                                                          _ptr(scales, C.c_float), _ptr(frames, C.c_int32), outs,
-                                                          C.byref(err)), err)
+        _check(self._lib.sb200_encode_batch_ids_seeded(self._h, packed.ctypes.data_as(C.POINTER(C.c_int64)),
+                                                       offs.ctypes.data_as(C.POINTER(C.c_size_t)), n, cfgs,
+                                                       _ptr(scales, C.c_float), _ptr(frames, C.c_int32),
+                                                       _ptr(sv, C.c_uint64), _ptr(sf, C.c_int32), outs,
+                                                       C.byref(err)), err)
         return [EncoderOutputs(self, C.c_void_p(outs[i])) for i in range(n)]
 
     def infer_decoder_batch(self, chunks: Sequence[tuple], pcm16: bool = False, fade: int = 0,
@@ -580,9 +624,13 @@ class VitsStreamingModel(_VitsCommons):
     def supports_streaming_output(self) -> bool:
         return True
 
-    def stream_synthesis(self, phonemes: str, chunk_size: int, chunk_padding: int) -> SpeechStreamer:
+    def stream_synthesis(self, phonemes: str, chunk_size: int, chunk_padding: int,
+                         seed: Optional[int] = None) -> SpeechStreamer:
+        """`seed`: the sentence's noise seed (see infer_batch_with_values), or None for positional noise."""
+        _seed_arrays([seed], 1)
         ids = self.phonemes_to_input_ids(phonemes)
-        return SpeechStreamer(self.infer_encoder(ids), chunk_size, chunk_padding)
+        enc = self.infer_encoder(ids) if seed is None else self.infer_encoder_batch([ids], seeds=[seed])[0]
+        return SpeechStreamer(enc, chunk_size, chunk_padding)
 
 
 class _Stream:
@@ -632,16 +680,19 @@ class StreamBatch:
         _check_chunking(chunk_size, chunk_padding)
         self.model = model
         self.chunk_size, self.chunk_padding = chunk_size, chunk_padding
-        self._pending: list = []      # (key, ids, config, chunk_size) not yet encoded
+        self._pending: list = []      # (key, ids, config, chunk_size, seed) not yet encoded
         self._active: List[_Stream] = []
         self._next_key = 0
 
-    def add(self, ids_or_phonemes, config: Optional[PiperSynthesisConfig] = None) -> int:
-        return self._add(ids_or_phonemes, config, self.chunk_size)
+    def add(self, ids_or_phonemes, config: Optional[PiperSynthesisConfig] = None, seed: Optional[int] = None) -> int:
+        """`seed`: the stream's noise seed (see infer_batch_with_values); a seeded stream yields what
+        `stream_synthesis(..., seed=seed)` yields, whatever other streams share its encoder pass."""
+        return self._add(ids_or_phonemes, config, self.chunk_size, seed)
 
-    def _add(self, ids_or_phonemes, config, chunk_size: int) -> int:
+    def _add(self, ids_or_phonemes, config, chunk_size: int, seed: Optional[int] = None) -> int:
         if config is not None and not isinstance(config, PiperSynthesisConfig):
             raise OperationError("Invalid configuration for Vits Model")
+        _seed_arrays([seed], 1)
         if config is not None and config.speaker is not None and config.speaker not in (self.model.get_speakers() or {}):
             raise OperationError(f"No speaker was found with the given id `{config.speaker}`")     # as check_config
         _check_chunking(chunk_size, self.chunk_padding)
@@ -653,7 +704,7 @@ class StreamBatch:
             raise OperationError("Failed to run model inference. Error: empty input sequence")
         key = self._next_key
         self._next_key += 1
-        self._pending.append((key, ids, config, chunk_size))
+        self._pending.append((key, ids, config, chunk_size, seed))
         return key
 
     def __len__(self) -> int:
@@ -675,7 +726,9 @@ class StreamBatch:
 
             def encode(ps):
                 configs = None if fallback is None else [fallback if p[2] is None else p[2] for p in ps]
-                return self.model.infer_encoder_batch([p[1] for p in ps], configs)
+                if all(p[4] is None for p in ps):
+                    return self.model.infer_encoder_batch([p[1] for p in ps], configs)
+                return self.model.infer_encoder_batch([p[1] for p in ps], configs, seeds=[p[4] for p in ps])
             for p, (enc, err) in zip(pend, _each_or_alone(encode, pend)):
                 if err is not None:
                     out.append((p[0], err))

@@ -217,7 +217,8 @@ class Frontend:
     libsonata's callback receives, at half the device->host bytes.  Every device / host buffer is allocated once and
     reused; the collectives carry only ids, per-utterance configs and length tables.  `run_local(ids_list, dst, capacity,
     fmt)` is the per-rank synthesis hook (default: the CUDA job of `model`), called with `configs=` (the shard's configs in
-    its utterance order) only when the caller gave configs; the gloo tests pass a deterministic stand-in."""
+    its utterance order) only when the caller gave configs, and `seeds=` likewise; the gloo tests pass a deterministic
+    stand-in."""
 
     def __init__(self, model=None, group=None, pcm16: bool = False, pin: bool = True, run_local: Optional[Callable] = None):
         self.model, self.group, self.pcm16 = model, group, pcm16
@@ -234,8 +235,8 @@ class Frontend:
         self.last_profile = []
 
     # -- collective plumbing ----------------------------------------------------------------------------------------
-    FIRST_BLOCK = 1 << 18      # int64 elements (2 MB) of the first broadcast: [n, total, has_cfg, lens, owner, ids ...,
-    #                            configs: 4 words per utterance when has_cfg]
+    FIRST_BLOCK = 1 << 18      # int64 elements (2 MB) of the first broadcast: [n, total, has, lens, owner, ids ...,
+    #                            configs: 4 words per utterance when has & 1, seeds: 2 words per utterance when has & 2]
 
     @staticmethod
     def _encode_configs(configs) -> np.ndarray:
@@ -255,10 +256,27 @@ class Frontend:
         return [PiperSynthesisConfig(None if s < 0 else int(s), float(a), float(b), float(c))
                 for s, (a, b, c) in zip(w[:, 0].tolist(), f.tolist())]
 
-    def _bcast_ids(self, batches, configs=None):
+    @staticmethod
+    def _encode_seeds(seeds, n: int) -> np.ndarray:
+        """int64 image of per-utterance noise seeds: [seeded flag, the seed's 64 bits] per utterance."""
+        from .piper import _seed_arrays
+        vals, flags = _seed_arrays(seeds, n)
+        out = np.zeros((n, 2), dtype=np.int64)
+        if vals is not None:
+            out[:, 0] = flags
+            out[:, 1] = vals.view(np.int64)
+        return out.reshape(-1)
+
+    @staticmethod
+    def _decode_seeds(words: np.ndarray) -> list:
+        w = np.ascontiguousarray(words.reshape(-1, 2))
+        vals = w[:, 1].view(np.uint64)
+        return [int(v) if f else None for f, v in zip(w[:, 0].tolist(), vals.tolist())]
+
+    def _bcast_ids(self, batches, configs=None, seeds=None):
         """ONE broadcast of a fixed-size block carries the header and (for up to ~260k ids) everything else, the
         per-utterance configs included; a second broadcast follows only for larger inputs.  Host staging buffers are
-        page-locked and reused."""
+        page-locked and reused.  Seeds, when given, follow the configs; without them the block is what it always was."""
         rank, world = dist.get_rank(self.group), dist.get_world_size(self.group)
         dev = _dev(self.group)
         fb = self.FIRST_BLOCK
@@ -274,16 +292,20 @@ class Frontend:
                 owner[p] = r
             n0 = len(batches)
             ids_end = 3 + 2 * n0 + int(lens.sum())
-            total = ids_end + (4 * n0 if configs is not None else 0)
+            seed_words = None if seeds is None else self._encode_seeds(seeds, n0)
+            cfg_end = ids_end + (4 * n0 if configs is not None else 0)
+            total = cfg_end + (0 if seed_words is None else seed_words.size)
             if self._host.numel() < total:
                 self._host = torch.empty(int(total * 1.5), dtype=torch.int64, pin_memory=self._host.is_pinned())
             h = self._host.numpy()
-            h[0], h[1], h[2] = n0, total, configs is not None
+            h[0], h[1], h[2] = n0, total, (configs is not None) | (2 if seed_words is not None else 0)
             h[3:3 + n0] = lens
             h[3 + n0:3 + 2 * n0] = owner
             np.concatenate([np.asarray(b, dtype=np.int64) for b in batches], out=h[3 + 2 * n0:ids_end])
             if configs is not None:
-                h[ids_end:total] = self._encode_configs(configs)
+                h[ids_end:cfg_end] = self._encode_configs(configs)
+            if seed_words is not None:
+                h[cfg_end:total] = seed_words
             self._payload.copy_(self._host[:fb], non_blocking=True)
         dist.broadcast(self._payload, 0, group=self.group)
         if rank != 0:
@@ -312,26 +334,37 @@ class Frontend:
         lens, owner = flat[3:3 + n], flat[3 + n:3 + 2 * n].copy()
         offs = 3 + 2 * n + np.concatenate([[0], np.cumsum(lens)])
         mine = np.nonzero(owner == rank)[0]
-        my_cfgs = None
-        if flat[2]:
-            words = flat[offs[-1]:offs[-1] + 4 * n].reshape(n, 4)
+        my_cfgs = my_seeds = None
+        end = offs[-1]
+        if flat[2] & 1:
+            words = flat[end:end + 4 * n].reshape(n, 4)
             my_cfgs = self._decode_configs(words[mine])
-        return n, owner, mine, [flat[offs[i]:offs[i + 1]].copy() for i in mine], my_cfgs
+            end += 4 * n
+        if flat[2] & 2:
+            my_seeds = self._decode_seeds(flat[end:end + 2 * n].reshape(n, 2)[mine])
+        return n, owner, mine, [flat[offs[i]:offs[i + 1]].copy() for i in mine], my_cfgs, my_seeds
 
     def synthesize(self, batches: Optional[Sequence[np.ndarray]], device_only: bool = False,
-                   configs: Optional[Sequence] = None):
+                   configs: Optional[Sequence] = None, seeds: Optional[Sequence] = None):
         """Collective.  Rank 0 passes every utterance's ids and gets the waveforms back in utterance order (views into
         the shared segment, valid until the next call); the other ranks pass None and get None.
         `device_only`: stop after the passes (results stay in each GPU's memory): the device-resident timing of bench.py.
         `configs` (rank 0): one PiperSynthesisConfig per utterance; they travel with the ids and each rank runs its
-        shard with its utterances' configs.  None: the voice's fallback config everywhere."""
+        shard with its utterances' configs.  None: the voice's fallback config everywhere.
+        `seeds` (rank 0): one noise seed (int in [0, 2**64) or None) per utterance, as for
+        VitsModel.infer_batch_with_values; a seeded utterance's samples do not depend on the rank or shard it lands on."""
         rank, world = dist.get_rank(self.group), dist.get_world_size(self.group)
         dev = _dev(self.group)
         if rank == 0 and configs is not None and len(configs) != len(batches):
             from .core import OperationError
             raise OperationError(f"Invalid configuration for Vits Model: {len(configs)} configs for {len(batches)} utterances")
-        n, owner, mine, my_ids, my_cfgs = self._bcast_ids(batches, configs)
+        if rank == 0 and seeds is not None:
+            from .piper import _seed_arrays
+            _seed_arrays(seeds, len(batches))           # argument errors before any collective
+        n, owner, mine, my_ids, my_cfgs, my_seeds = self._bcast_ids(batches, configs, seeds)
         extra = {} if my_cfgs is None else {"configs": my_cfgs}
+        if my_seeds is not None:
+            extra["seeds"] = my_seeds
         bps = 2 if self.pcm16 else 4
         fmt = 1 if self.pcm16 else 0
         # two-step because the layout of the segment depends on every rank's frame counts: run first (waveforms stay on
@@ -341,7 +374,7 @@ class Frontend:
             from .job import SynthesisJob
             samples_local = []
             if my_ids:
-                job = SynthesisJob(self.model, my_ids, configs=my_cfgs)
+                job = SynthesisJob(self.model, my_ids, configs=my_cfgs, seeds=my_seeds)
                 self.last_device_ms = job.run()
                 samples_local = job.lengths()[1]
                 if self.collect_profile:

@@ -81,6 +81,15 @@ def next_chunk_size(chunk_size: int, produced: int) -> int:
     return chunk_size * 1 * produced if produced != 0 else chunk_size
 
 
+def sentence_seed(seed: Optional[int], i: int) -> Optional[int]:
+    """The noise seed of sentence i of a request seeded with `seed`: (seed + i) mod 2**64, so every sentence has its
+    own noise and a request's audio depends on its seed alone.  None (an unseeded request) stays None.  Raises
+    OperationError when `seed` is not an int in [0, 2**64)."""
+    from .piper import _seed_arrays
+    _seed_arrays([seed], 1)
+    return None if seed is None else (int(seed) + i) % 2**64
+
+
 def _sentences(model, text: str) -> List[str]:
     """SpeechSynthesisTaskProvider::get_phonemes (:256-258), or newline-separated phoneme sentences when the model has
     no phonemizer."""
@@ -103,30 +112,47 @@ class SonataSpeechSynthesizer:
     def _process(self, audio: Audio, cfg: Optional[AudioOutputConfig]) -> Audio:
         return cfg.apply(audio) if cfg is not None else audio
 
-    def synthesize_lazy(self, text: str, output_config: Optional[AudioOutputConfig] = None) -> Iterator[Audio]:
-        for ph in self._phonemes(text):
-            yield self._process(self.model.speak_one_sentence(ph), output_config)
+    # `seed` (every mode): the request's noise seed, sentence i seeded with sentence_seed(seed, i); None keeps the
+    # positional noise.
 
-    def synthesize_parallel(self, text: str, output_config: Optional[AudioOutputConfig] = None) -> Iterator[Audio]:
+    def synthesize_lazy(self, text: str, output_config: Optional[AudioOutputConfig] = None,
+                        seed: Optional[int] = None) -> Iterator[Audio]:
+        sentence_seed(seed, 0)
+        for i, ph in enumerate(self._phonemes(text)):
+            a = (self.model.speak_one_sentence(ph) if seed is None
+                 else self.model.speak_batch([ph], seeds=[sentence_seed(seed, i)])[0])
+            yield self._process(a, output_config)
+
+    def synthesize_parallel(self, text: str, output_config: Optional[AudioOutputConfig] = None,
+                            seed: Optional[int] = None) -> Iterator[Audio]:
+        sentence_seed(seed, 0)
         ph = self._phonemes(text)
-        results = self.model.speak_batch(ph) if ph else []        # one batched pass == the rayon fan-out + collect
+        if not ph:
+            results = []
+        elif seed is None:
+            results = self.model.speak_batch(ph)                  # one batched pass == the rayon fan-out + collect
+        else:
+            results = self.model.speak_batch(ph, seeds=[sentence_seed(seed, i) for i in range(len(ph))])
         return iter([self._process(a, output_config) for a in results])
 
     def synthesize_streamed(self, text: str, output_config: Optional[AudioOutputConfig] = None,
-                            chunk_size: int = 72, chunk_padding: int = 3) -> Iterator[AudioSamples]:
+                            chunk_size: int = 72, chunk_padding: int = 3,
+                            seed: Optional[int] = None) -> Iterator[AudioSamples]:
         """RealtimeSpeechStream (:337-382): a background producer pushes chunks into an unbounded channel;
         chunk_size is multiplied by the number of chunks already produced for every following sentence."""
+        sentence_seed(seed, 0)
         sr = self.model.audio_output_info().sample_rate
+        extra = lambda i: {} if seed is None else {"seed": sentence_seed(seed, i)}
         q: "queue.Queue" = queue.Queue()
         done = object()
 
         def producer():
             cs, produced = chunk_size, 0
             try:
-                for ph in self._phonemes(text):
+                for i, ph in enumerate(self._phonemes(text)):
                     cs = next_chunk_size(cs, produced)
                     n = 0
-                    for chunk in self.model.stream_synthesis(ph, cs, chunk_padding):
+                    for chunk in self.model.stream_synthesis(ph, cs, chunk_padding, **extra(i)):
                         q.put(output_config.apply_to_raw_samples(chunk) if output_config else chunk)
                         n += 1
                     produced += n
@@ -145,9 +171,10 @@ class SonataSpeechSynthesizer:
                 raise item
             yield item
 
-    def synthesize_to_file(self, filename, text: str, output_config: Optional[AudioOutputConfig] = None) -> None:
+    def synthesize_to_file(self, filename, text: str, output_config: Optional[AudioOutputConfig] = None,
+                           seed: Optional[int] = None) -> None:
         """:168-198 — parallel mode, concatenated, peak-normalised i16 WAV."""
-        parts = [a.samples.as_slice() for a in self.synthesize_parallel(text, output_config)]
+        parts = [a.samples.as_slice() for a in self.synthesize_parallel(text, output_config, seed=seed)]
         if not parts or sum(len(p) for p in parts) == 0:
             raise OperationError("No speech data to write")
         Audio(AudioSamples(np.concatenate(parts)), self.model.audio_output_info().sample_rate).save_to_file(filename)
@@ -164,8 +191,8 @@ class SonataSpeechSynthesizer:
 
 
 class _Request:
-    def __init__(self, key, ids, output_config, config, chunk_size):
-        self.key, self.ids, self.output_config, self.config = key, ids, output_config, config
+    def __init__(self, key, ids, output_config, config, chunk_size, seed=None):
+        self.key, self.ids, self.output_config, self.config, self.seed = key, ids, output_config, config, seed
         self.cs, self.produced, self.n, self.next = chunk_size, 0, 0, 0
 
 
@@ -189,8 +216,11 @@ class RealtimeBatch:
         self._by_stream = {}          # stream key -> request of the sentence it speaks
         self._next_key = 0
 
-    def add(self, text: str, output_config: Optional[AudioOutputConfig] = None, config=None) -> int:
+    def add(self, text: str, output_config: Optional[AudioOutputConfig] = None, config=None,
+            seed: Optional[int] = None) -> int:
+        """`seed`: the request's noise seed, as for synthesize_streamed."""
         from .piper import PiperSynthesisConfig
+        sentence_seed(seed, 0)
         if output_config is not None:
             output_config._check_supported()
         if config is not None and not isinstance(config, PiperSynthesisConfig):
@@ -200,7 +230,7 @@ class RealtimeBatch:
         ids = [self.model.phonemes_to_input_ids(ph) for ph in _sentences(self.model, text)]
         if any(len(i) == 0 for i in ids):
             raise OperationError("Failed to run model inference. Error: empty input sequence")
-        req = _Request(self._next_key, ids, output_config, config, self.chunk_size)
+        req = _Request(self._next_key, ids, output_config, config, self.chunk_size, seed)
         self._next_key += 1
         self._start_sentence(req)
         return req.key
@@ -210,7 +240,7 @@ class RealtimeBatch:
             return
         req.cs = next_chunk_size(req.cs, req.produced)
         req.n = 0
-        self._by_stream[self._streams._add(req.ids[req.next], req.config, req.cs)] = req
+        self._by_stream[self._streams._add(req.ids[req.next], req.config, req.cs, sentence_seed(req.seed, req.next))] = req
         req.next += 1
 
     def __len__(self) -> int:
