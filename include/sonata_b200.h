@@ -162,6 +162,22 @@ int32_t sb200_speak_batch_ids_seeded(sb200_voice* v, const int64_t* ids_packed, 
                                      const int32_t* frames_packed, const uint64_t* seeds, const int32_t* seeded,
                                      sb200_audio* outs, int32_t* id_frames_out, sb200_error* err);
 
+/* ---- output sample rate: results resampled on the device ----
+ * An output rate is 8000, 11025, 16000, 22050, 24000, 32000, 44100 or 48000 Hz; 0 or the voice's own rate means no
+ * resampling, bit for bit what a call without rates returns.  Any other value fails with OPERATION_ERROR naming the
+ * utterance.  The resampler is scipy.signal.resample_poly's default: with up/down the reduced ratio out/in, H = 10 *
+ * max(up, down) and h = firwin(2H + 1, 1 / max(up, down), window=('kaiser', 5.0)) * up (designed in double, rounded to
+ * f32), an utterance of n samples becomes ceil(n * up / down) samples,
+ *     y[j] = sum_i x[i] * h[j*down + H - i*up]  over 0 <= i < n with 0 <= j*down + H - i*up <= 2H,
+ * each sum one fmaf chain in ascending i, so a resampled utterance has the same bits in any batch.
+ * sb200_speak_batch_ids_seeded with output_rates[b] the rate of utterance b (outs[b].sample_rate reports it); NULL
+ * rates is that call, bit for bit. */
+int32_t sb200_speak_batch_ids_rates(sb200_voice* v, const int64_t* ids_packed, const size_t* offsets, size_t batch,
+                                    const sb200_synth_config* cfgs, const float* scale_packed,
+                                    const int32_t* frames_packed, const uint64_t* seeds, const int32_t* seeded,
+                                    const uint32_t* output_rates, sb200_audio* outs, int32_t* id_frames_out,
+                                    sb200_error* err);
+
 /* ---- job API: the same batched pass split into its host<->device steps (bench / multi-GPU plumbing) ----
  * create  : copies ids to the device (H2D).  `eps_w` / `eps_z` optionally inject the graph's two
  *           RandomNormalLike draws (time-major: eps_w[b] = f32[T_x][2], eps_z[b] = f32[T_y][inter]);
@@ -190,6 +206,13 @@ int32_t sb200_job_set_durations(sb200_job* job, const float* scale_packed, const
  * a bad flag; either leaves the job's seeds as they were.  With debug on, the run's noise is fetchable as "eps_w"
  * ([T_x][2]) and "eps_z" ([T_y][inter]) when its scale is not 0 for some utterance. */
 int32_t sb200_job_set_seeds(sb200_job* job, const uint64_t* seeds, const int32_t* seeded, sb200_error* err);
+/* Output rates (see sb200_speak_batch_ids_rates) for the next sb200_job_run: rates[0 .. batch), or NULL for none (what
+ * a new job starts with).  An unsupported entry fails with OPERATION_ERROR naming the utterance and leaves the job's
+ * rates as they were.  After a run with rates, every result call reports the resampled signal: the d_out of
+ * sb200_job_run (its capacity counts resampled samples), sb200_job_fetch (sample_rate per utterance),
+ * sb200_job_fetch_i16, sb200_job_copy_out (both formats) and the samples and out_offsets of sb200_job_lengths; its
+ * frames stay frame counts.  sb200_job_profile reports the resampling launch as the region "resample". */
+int32_t sb200_job_set_output_rates(sb200_job* job, const uint32_t* rates, sb200_error* err);
 /* Frames per id of the last run, packed like ids_packed, into out_packed[0 .. capacity): one device->host copy of the
  * whole batch's cumulative durations, made on the first call after a run.  Fails before a run, or when capacity is
  * smaller than the number of ids. */
@@ -264,6 +287,27 @@ int32_t sb200_decode_chunks_i16(sb200_voice* v, const sb200_latent* const* zs, c
                                 const int64_t* trim_lo_frames, const int64_t* trim_hi_frames, size_t n, int32_t fade,
                                 const float* gain, int16_t** outs, size_t* lens, sb200_error* err);
 
+/* ---- streams at an output sample rate (see sb200_speak_batch_ids_rates) ----
+ * A resampler is one stream's state on the device: the last K - 1 <= 2H/up of its inputs (K taps per phase) and the
+ * counts of inputs consumed and outputs emitted.  out_rate must be a supported rate other than the voice's own (a
+ * stream at the voice's rate needs none); otherwise OPERATION_ERROR.  It shares ownership of the voice. */
+typedef struct sb200_resampler sb200_resampler;
+int32_t sb200_resampler_create(sb200_voice* v, uint32_t out_rate, sb200_resampler** out, sb200_error* err);
+void sb200_resampler_free(sb200_resampler* r);
+/* sb200_decode_chunks_i16's pass and post-path (trims, crossfade(fade), gain) per chunk, then chunk k appended to its
+ * stream's resampler resamplers[k] (NULL: the chunk leaves at the voice's rate after the post-path).  Chunk k emits
+ * every output whose inputs have all arrived (the rest, 10-28 inputs at the supported rates, are held back) and, when
+ * last[k] is 1 (last NULL: none), every output left, reading zeros past the stream's end; the resampler then takes no
+ * more chunks.  A chunk may emit 0 samples.  The concatenation of a stream's outputs is, bit for bit, its whole input
+ * resampled at once (sb200_debug_resample).  format 0: outs[k] is f32; 1: i16 normalised to the emitted chunk's own
+ * peak (to_i16_vec).  outs[k] is malloc'ed, lens[k] samples: free with free() (sb200_i16_free / sb200_buffer_free).
+ * A resampler appearing twice, made for another voice or already flushed fails with OPERATION_ERROR naming the chunk,
+ * before any state changes. */
+int32_t sb200_decode_chunks_resampled(sb200_voice* v, const sb200_latent* const* zs, const int64_t* lo, const int64_t* hi,
+                                      const int64_t* trim_lo_frames, const int64_t* trim_hi_frames, size_t n,
+                                      int32_t fade, const float* gain, sb200_resampler* const* resamplers,
+                                      const int32_t* last, int32_t format, void** outs, size_t* lens, sb200_error* err);
+
 /* ---- introspection for tests / bench ---- */
 /* Copy a named intermediate of the LAST run of `job` to host (time-major fp32, valid rows of
  * utterance b only).  Names: "x","stats","logw","z_p","z","dec.pre","dec.up<i>","dec.mrf<i>", and the first encoder
@@ -330,6 +374,20 @@ int32_t sb200_debug_spline(int32_t device, const float* h29, int32_t ldh, float*
 int32_t sb200_debug_durations(int32_t device, const float* z, int32_t rows, const int32_t* seg_off, const int32_t* seg_len,
                               int32_t nseg, float m0, float logs0, float length_scale, float* logw, int32_t* cum,
                               int32_t* y_len, sb200_error* err);
+/* Test hook: the resampling filter from in_rate to out_rate (see sb200_speak_batch_ids_rates), no device needed.
+ * *up / *down receive the reduced ratio, and taps[0 .. 2H] the f32 taps in natural order when cap >= 2H + 1
+ * (H = 10 * max(up, down)).  Returns 0, or 19 when out_rate is not a supported rate or equals in_rate. */
+int32_t sb200_debug_resample_filter(int32_t in_rate, int32_t out_rate, float* taps, size_t cap, int32_t* up,
+                                    int32_t* down);
+/* Test hook, no device needed: the samples a stream resampled from in_rate to out_rate emits per chunk when its chunks
+ * bring chunk_lens[0 .. n) inputs and the last one flushes it.  emitted[k] receives chunk k's count.  Returns 0, or 19
+ * for an unsupported rate or a negative length. */
+int32_t sb200_debug_resample_emit(int32_t in_rate, int32_t out_rate, const int64_t* chunk_lens, size_t n,
+                                  int64_t* emitted);
+/* The resampling kernel over one caller buffer x[0 .. n) from in_rate to out_rate: y receives ceil(n * up / down)
+ * samples, bit for bit what a job resampling an utterance of those samples returns. */
+int32_t sb200_debug_resample(int32_t device, const float* x, size_t n, int32_t in_rate, int32_t out_rate, float* y,
+                             sb200_error* err);
 /* kernels launched by this library since load (host-side counter) */
 uint64_t sb200_launch_count(void);
 /* select the contraction backend: 0 = fp32 CUDA-core implicit GEMM, 1 = wgmma (3xTF32) where

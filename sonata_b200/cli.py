@@ -41,6 +41,8 @@ def build_parser() -> argparse.ArgumentParser:
     ap.add_argument("--chunk-padding", type=int)
     ap.add_argument("--seed", type=int, help="Noise seed [0, 2^64): sentence i uses seed + i, so the same input and seed "
                                           "give the same samples (default: positional noise)")
+    ap.add_argument("--output-rate", type=int, help="Output sample rate in Hz (8000, 11025, 16000, 22050, 24000, 32000, "
+                                                  "44100 or 48000; default the voice's), resampled on the GPU")
     ap.add_argument("--device", type=int, default=int(os.environ.get("SONATA_B200_DEVICE", "0")))
     return ap
 
@@ -48,7 +50,7 @@ def build_parser() -> argparse.ArgumentParser:
 def process_request(synth: SonataSpeechSynthesizer, default_cfg: PiperSynthesisConfig, req: dict,
                     output_file: Optional[str], out=None) -> None:
     """process_synthesis_request (main.rs:126-165).  `seed` (optional): the request's noise seed, see
-    synth.sentence_seed."""
+    synth.sentence_seed.  `output_rate` (optional): the sample rate of the WAV or raw PCM written."""
     out = out or sys.stdout.buffer
     synth.model.set_fallback_synthesis_config(PiperSynthesisConfig(
         req.get("speaker_id"),
@@ -58,17 +60,18 @@ def process_request(synth: SonataSpeechSynthesizer, default_cfg: PiperSynthesisC
     oc = AudioOutputConfig(req.get("rate"), req.get("volume"), req.get("pitch"), req.get("appended_silence_ms"))
     text = req["text"]
     seed = req.get("seed")
+    rate = {"output_rate": req["output_rate"]} if req.get("output_rate") else {}
     if output_file:
-        synth.synthesize_to_file(output_file, text, oc, seed=seed)
+        synth.synthesize_to_file(output_file, text, oc, seed=seed, **rate)
         return
     mode = (req.get("mode") or "lazy").lower()
     if mode == "lazy":
-        stream = (a.samples for a in synth.synthesize_lazy(text, oc, seed=seed))
+        stream = (a.samples for a in synth.synthesize_lazy(text, oc, seed=seed, **rate))
     elif mode == "parallel":
-        stream = (a.samples for a in synth.synthesize_parallel(text, oc, seed=seed))
+        stream = (a.samples for a in synth.synthesize_parallel(text, oc, seed=seed, **rate))
     elif mode == "realtime":
         stream = synth.synthesize_streamed(text, oc, req.get("chunk_size") or 100, req.get("chunk_padding") or 3,
-                                          seed=seed)
+                                          seed=seed, **rate)
     else:
         raise ValueError(f"unknown synthesis mode `{mode}`")
     for samples in stream:
@@ -87,7 +90,7 @@ def main(argv=None) -> int:
         req = {"text": text, "mode": args.mode, "speaker_id": args.speaker_id, "length_scale": args.length_scale,
                "noise_scale": args.noise_scale, "noise_w": args.noise_w, "rate": args.rate, "volume": args.volume,
                "pitch": args.pitch, "appended_silence_ms": args.silence, "chunk_size": args.chunk_size,
-               "chunk_padding": args.chunk_padding, "seed": args.seed}
+               "chunk_padding": args.chunk_padding, "seed": args.seed, "output_rate": args.output_rate}
         process_request(synth, default_cfg, req, args.output_file)
     else:
         for i, line in enumerate(sys.stdin):
@@ -96,6 +99,8 @@ def main(argv=None) -> int:
             req = json.loads(line)
             if req.get("seed") is None:
                 req["seed"] = args.seed
+            if req.get("output_rate") is None:
+                req["output_rate"] = args.output_rate
             out_file = None
             if args.output_file:
                 stem, ext = os.path.splitext(args.output_file)

@@ -22,6 +22,10 @@ struct sb200_latent {
     Latent* l; std::shared_ptr<Voice> keep;
     ~sb200_latent() { delete l; }
 };
+struct sb200_resampler {
+    Resampler* r; std::shared_ptr<Voice> keep;
+    ~sb200_resampler() { delete r; }
+};
 
 namespace {
 
@@ -90,18 +94,17 @@ void fetch_audio(Job& j, sb200_audio* outs, float wall_ms) {
     if (!j.ran || j.encode_only) throw Error(19, "job has not produced audio");
     Voice& v = *j.v;
     SB_CUDA(cudaSetDevice(v.device));
-    PinnedBlock* blk = pin_acquire((size_t)j.total_samples * 4 + 16);
-    cudaError_t e = cudaMemcpyAsync(blk->base, j.d_wav, (size_t)j.total_samples * 4, cudaMemcpyDeviceToHost, j.ctx->stream);
+    PinnedBlock* blk = pin_acquire((size_t)j.out_total * 4 + 16);
+    cudaError_t e = cudaMemcpyAsync(blk->base, j.d_wav, (size_t)j.out_total * 4, cudaMemcpyDeviceToHost, j.ctx->stream);
     if (e == cudaSuccess) e = cudaStreamSynchronize(j.ctx->stream);
     if (e != cudaSuccess) { pin_release(blk); throw Error(19, std::string("CUDA error: ") + cudaGetErrorString(e)); }
     blk->refs = (int)j.B;
-    const int hop = v.a.hop();
     std::lock_guard<std::mutex> g(g_pin_mu);
     for (size_t b = 0; b < j.B; b++) {
-        outs[b].data = blk->base + j.fsegs[b].out_off;
-        outs[b].len = (size_t)j.y_len[b] * hop;
-        outs[b].sample_rate = (uint32_t)v.sample_rate;
-        outs[b].inference_ms = wall_ms * (j.total_samples ? (float)outs[b].len / (float)j.total_samples : 0.f);
+        outs[b].data = blk->base + j.osegs[b].out_off;
+        outs[b].len = (size_t)j.osegs[b].len * j.out_hop;
+        outs[b].sample_rate = (uint32_t)j.osr[b];
+        outs[b].inference_ms = wall_ms * (j.out_total ? (float)outs[b].len / (float)j.out_total : 0.f);
         g_owner[outs[b].data] = blk;
     }
 }
@@ -234,19 +237,25 @@ int32_t sb200_phonemes_to_input_ids_map(const sb200_voice* v, const char* ph, in
     });
 }
 
-int32_t sb200_speak_batch_ids_seeded(sb200_voice* v, const int64_t* ids, const size_t* offsets, size_t batch,
-                                     const sb200_synth_config* cfgs, const float* scale_packed,
-                                     const int32_t* frames_packed, const uint64_t* seeds, const int32_t* seeded,
-                                     sb200_audio* outs, int32_t* id_frames_out, sb200_error* err) {
+int32_t sb200_speak_batch_ids_rates(sb200_voice* v, const int64_t* ids, const size_t* offsets, size_t batch,
+                                    const sb200_synth_config* cfgs, const float* scale_packed,
+                                    const int32_t* frames_packed, const uint64_t* seeds, const int32_t* seeded,
+                                    const uint32_t* output_rates, sb200_audio* outs, int32_t* id_frames_out,
+                                    sb200_error* err) {
     return guarded(err, [&] {
         const double t0 = now_ms();
         static_assert(sizeof(long long) == sizeof(int64_t), "");
         static_assert(sizeof(unsigned long long) == sizeof(uint64_t), "");
+        if (output_rates)       // before the job: the rates are checked against the voice's config alone
+            for (size_t b = 0; b < batch; b++)
+                if (output_rates[b] != 0 && output_rates[b] != (uint32_t)v->v->sample_rate)
+                    resample_ratio(v->v->sample_rate, output_rates[b], "utterance " + std::to_string(b) + ": ");
         std::unique_ptr<Job> j(create_job(v->v.get(), reinterpret_cast<const long long*>(ids), offsets, batch, nullptr,
                                           nullptr, nullptr, false));
         if (cfgs) set_job_configs(*j, cfgs_in(cfgs, batch).data());
         set_job_durations(*j, scale_packed, frames_packed);
         set_job_seeds(*j, reinterpret_cast<const unsigned long long*>(seeds), seeded);
+        set_job_output_rates(*j, output_rates);
         j->run(nullptr, 0);
         fetch_audio(*j, outs, 0.f);
         if (id_frames_out) {
@@ -255,8 +264,15 @@ int32_t sb200_speak_batch_ids_seeded(sb200_voice* v, const int64_t* ids, const s
         }
         const float wall = (float)(now_ms() - t0);
         for (size_t b = 0; b < batch; b++)
-            outs[b].inference_ms = wall * (j->total_samples ? (float)outs[b].len / (float)j->total_samples : 0.f);
+            outs[b].inference_ms = wall * (j->out_total ? (float)outs[b].len / (float)j->out_total : 0.f);
     });
+}
+int32_t sb200_speak_batch_ids_seeded(sb200_voice* v, const int64_t* ids, const size_t* offsets, size_t batch,
+                                     const sb200_synth_config* cfgs, const float* scale_packed,
+                                     const int32_t* frames_packed, const uint64_t* seeds, const int32_t* seeded,
+                                     sb200_audio* outs, int32_t* id_frames_out, sb200_error* err) {
+    return sb200_speak_batch_ids_rates(v, ids, offsets, batch, cfgs, scale_packed, frames_packed, seeds, seeded, nullptr,
+                                       outs, id_frames_out, err);
 }
 int32_t sb200_speak_batch_ids_durations(sb200_voice* v, const int64_t* ids, const size_t* offsets, size_t batch,
                                         const sb200_synth_config* cfgs, const float* scale_packed,
@@ -315,6 +331,9 @@ int32_t sb200_job_set_durations(sb200_job* job, const float* scale_packed, const
 int32_t sb200_job_set_seeds(sb200_job* job, const uint64_t* seeds, const int32_t* seeded, sb200_error* err) {
     return guarded(err, [&] { set_job_seeds(*job->j, reinterpret_cast<const unsigned long long*>(seeds), seeded); });
 }
+int32_t sb200_job_set_output_rates(sb200_job* job, const uint32_t* rates, sb200_error* err) {
+    return guarded(err, [&] { set_job_output_rates(*job->j, rates); });
+}
 int32_t sb200_job_id_frames(sb200_job* job, int32_t* out_packed, size_t capacity, sb200_error* err) {
     return guarded(err, [&] {
         Job& j = *job->j;
@@ -335,14 +354,13 @@ int32_t sb200_job_fetch_i16(sb200_job* job, int16_t** outs, size_t* lens, sb200_
     return guarded(err, [&] {
         Job& j = *job->j;
         SB_CUDA(cudaSetDevice(j.v->device));
-        const int hop = j.v->a.hop();
-        PinnedBlock* blk = pin_acquire((size_t)j.total_samples * 2 + 16);
+        PinnedBlock* blk = pin_acquire((size_t)j.out_total * 2 + 16);
         int16_t* h = reinterpret_cast<int16_t*>(blk->base);
         try { job_i16_to_host(j, 1.f, h); } catch (...) { pin_release(blk); throw; }
         for (size_t b = 0; b < j.B; b++) {
-            const size_t n = (size_t)j.y_len[b] * hop;
+            const size_t n = (size_t)j.osegs[b].len * j.out_hop;
             outs[b] = (int16_t*)malloc(n * 2 + 2);
-            memcpy(outs[b], h + j.fsegs[b].out_off, n * 2);
+            memcpy(outs[b], h + j.osegs[b].out_off, n * 2);
             lens[b] = n;
         }
         pin_release(blk);
@@ -358,7 +376,7 @@ int32_t sb200_job_copy_out(sb200_job* job, void* dst, size_t cap, int32_t format
         Voice& v = *j.v;
         SB_CUDA(cudaSetDevice(v.device));
         cudaStream_t st = j.ctx->stream;
-        const size_t n = (size_t)j.total_samples;
+        const size_t n = (size_t)j.out_total;
         const size_t bytes = n * (format == 1 ? 2 : 4);
         if (bytes > cap) throw Error(19, "destination buffer is too small for the synthesis result");
         if (format == 1) {
@@ -385,11 +403,10 @@ size_t sb200_job_batch(const sb200_job* job) { return job->j->B; }
 int32_t sb200_job_lengths(const sb200_job* job, int64_t* frames, int64_t* samples, int64_t* out_offsets) {
     const Job& j = *job->j;
     if (!j.ran) return 19;
-    const int hop = j.v->a.hop();
     for (size_t b = 0; b < j.B; b++) {
         if (frames) frames[b] = j.y_len[b];
-        if (samples) samples[b] = (int64_t)j.y_len[b] * hop;
-        if (out_offsets) out_offsets[b] = j.fsegs[b].out_off;
+        if (samples) samples[b] = (int64_t)j.osegs[b].len * j.out_hop;
+        if (out_offsets) out_offsets[b] = j.osegs[b].out_off;
     }
     return 0;
 }
@@ -482,6 +499,39 @@ int32_t sb200_decode_chunks_i16(sb200_voice* v, const sb200_latent* const* zs, c
             outs[k] = (int16_t*)malloc(w[k].size() * 2 + 2);
             memcpy(outs[k], w[k].data(), w[k].size() * 2);
             lens[k] = w[k].size();
+        }
+    });
+}
+
+int32_t sb200_resampler_create(sb200_voice* v, uint32_t out_rate, sb200_resampler** out, sb200_error* err) {
+    return guarded(err, [&] {
+        if (!v || !out) throw Error(19, "null argument");
+        *out = new sb200_resampler{create_resampler(v->v.get(), out_rate), v->v};
+    });
+}
+void sb200_resampler_free(sb200_resampler* r) { delete r; }
+
+int32_t sb200_decode_chunks_resampled(sb200_voice* v, const sb200_latent* const* zs, const int64_t* lo, const int64_t* hi,
+                                      const int64_t* trim_lo_frames, const int64_t* trim_hi_frames, size_t n,
+                                      int32_t fade, const float* gain, sb200_resampler* const* resamplers,
+                                      const int32_t* last, int32_t format, void** outs, size_t* lens, sb200_error* err) {
+    return guarded(err, [&] {
+        const std::vector<const Latent*> ls = latents_of(zs, n);
+        if (n > 0 && (!resamplers || !outs || !lens)) throw Error(19, "null argument");
+        std::vector<Resampler*> rs(n);
+        for (size_t k = 0; k < n; k++) rs[k] = resamplers[k] ? resamplers[k]->r : nullptr;
+        std::vector<std::vector<float>> f;
+        std::vector<std::vector<int16_t>> s;
+        decode_latent_chunks_resampled(v->v.get(), ls.data(), reinterpret_cast<const long long*>(lo),
+                                       reinterpret_cast<const long long*>(hi),
+                                       reinterpret_cast<const long long*>(trim_lo_frames),
+                                       reinterpret_cast<const long long*>(trim_hi_frames), n, fade, gain, rs.data(), last,
+                                       format, f, s);
+        for (size_t k = 0; k < n; k++) {
+            const size_t m = format == 1 ? s[k].size() : f[k].size(), es = format == 1 ? 2 : 4;
+            outs[k] = malloc(m * es + 4);
+            memcpy(outs[k], format == 1 ? (const void*)s[k].data() : (const void*)f[k].data(), m * es);
+            lens[k] = m;
         }
     });
 }
@@ -660,6 +710,65 @@ int32_t sb200_debug_durations(int32_t device, const float* z, int32_t rows, cons
         SB_CUDA(cudaMemcpy(logw, dlogw, (size_t)rows * 4, cudaMemcpyDeviceToHost));
         SB_CUDA(cudaMemcpy(cum, dcum, (size_t)rows * 4, cudaMemcpyDeviceToHost));
         SB_CUDA(cudaMemcpy(y_len, dylen, (size_t)nseg * 4, cudaMemcpyDeviceToHost));
+    });
+}
+
+int32_t sb200_debug_resample_filter(int32_t in_rate, int32_t out_rate, float* taps, size_t cap, int32_t* up,
+                                    int32_t* down) {
+    try {
+        const ResampleFilter f = resample_ratio(in_rate, out_rate, "");
+        if (up) *up = f.up;
+        if (down) *down = f.down;
+        if (taps && cap >= (size_t)(2 * f.H + 1)) {
+            const std::vector<float> h = resample_taps(f.up, f.down);
+            std::copy(h.begin(), h.end(), taps);
+        }
+        return 0;
+    } catch (const Error& e) {
+        return e.code;
+    }
+}
+
+int32_t sb200_debug_resample_emit(int32_t in_rate, int32_t out_rate, const int64_t* chunk_lens, size_t n,
+                                  int64_t* emitted) {
+    try {
+        if (!chunk_lens || !emitted) return 19;
+        const ResampleFilter f = resample_ratio(in_rate, out_rate, "");
+        long long consumed = 0, done = 0;
+        for (size_t k = 0; k < n; k++) {
+            if (chunk_lens[k] < 0) return 19;
+            consumed += chunk_lens[k];
+            const long long end = resample_emit_end(f, consumed, k + 1 == n);
+            emitted[k] = end - done;
+            done = end;
+        }
+        return 0;
+    } catch (const Error& e) {
+        return e.code;
+    }
+}
+
+int32_t sb200_debug_resample(int32_t device, const float* x, size_t n, int32_t in_rate, int32_t out_rate, float* y,
+                             sb200_error* err) {
+    return guarded(err, [&] {
+        if (!x || !y || n == 0 || n > (size_t)INT32_MAX) throw Error(19, "debug resample: bad arguments");
+        ResampleFilter f = resample_ratio(in_rate, out_rate, "");
+        const std::vector<float> t = resample_phase_major(resample_taps(f.up, f.down), f.up, f.K);
+        const long long n_out = ((long long)n * f.up + f.down - 1) / f.down;
+        SB_CUDA(cudaSetDevice(device));
+        DeviceBuffers d;
+        f.taps = d.upload(t.data(), t.size(), t.size());
+        const float* dx = d.upload(x, n, n);
+        float* dy = d.alloc<float>((size_t)n_out);
+        const FrameSeg fs{0, (int)n, 0, 0, 0};               // one segment of n samples at hop 1
+        const PcmPost post;
+        const ResampleSeg rs{f.taps, 0, n_out, f.up, f.down, f.H, f.K};
+        const FrameSeg* dfs = d.upload(&fs, 1, 1);
+        const PcmPost* dpost = d.upload(&post, 1, 1);
+        const ResampleSeg* drs = d.upload(&rs, 1, 1);
+        launch_resample(dx, dfs, dpost, 1, drs, 1, n_out, resample_span(f.up, f.down, f.K), dy, 0);
+        SB_CUDA(cudaDeviceSynchronize());
+        SB_CUDA(cudaMemcpy(y, dy, (size_t)n_out * 4, cudaMemcpyDeviceToHost));
     });
 }
 

@@ -194,6 +194,24 @@ struct PcmPost { float gain = 1.f; int fade_n = 0; long long trim_lo = 0, trim_h
 // posts: device array, one entry per segment; max_samples: the longest segment (before trimming), sizes the grid
 void launch_i16(const float* wav, const FrameSeg* fsegs, const PcmPost* posts, int nseg, int hop, long long max_samples,
                 unsigned* maxbits, short* out, cudaStream_t st);
+// Polyphase resampling of one segment (resample_poly's sum, kernels_misc.cu resample_kernel): n_out outputs at
+// out[out_off ..), from the segment's samples as pcm_value reads them.  taps: phase-major [up][K], taps[p][k] =
+// h[p + k*up] (0 past 2H).  up == 0: the segment is copied unchanged.  A stream's chunk continues its stream: the
+// segment's samples are inputs c .. c + n, hist holds the h inputs before them, the outputs written are j0 .. j0 + n_out,
+// and hist_out (null: none) receives the last h_out inputs for the next chunk.  A whole utterance is c = h = j0 = 0.
+struct ResampleSeg {
+    const float* taps; long long out_off, n_out; int up, down, H, K;
+    const float* hist; float* hist_out; long long c, j0; int h, h_out;
+};
+constexpr int RS_OUTS = 1024;     // consecutive outputs per block iteration
+// Shared-memory floats a block needs for one run of RS_OUTS outputs of a segment with this ratio.
+inline int resample_span(int up, int down, int K) {
+    return up > 0 ? (int)(((long long)(RS_OUTS - 1) * down) / up) + K + 1 : 0;
+}
+// One launch over nseg segments (blockIdx.y = segment), each segment with its own ratio; max_out: the most outputs of
+// any segment, smem_floats: the largest resample_span of the segments.
+void launch_resample(const float* wav, const FrameSeg* fsegs, const PcmPost* posts, int hop, const ResampleSeg* segs,
+                     int nseg, long long max_out, int smem_floats, float* out, cudaStream_t st);
 // One row range of a frame level taken from a latent: rows [off, off + len) of the level are rows [lo, lo + len) of src.
 struct GatherSeg { const float* src; long long lo; int off; int len; };
 // s[r] = the source row of r's segment (tile_seg: segment of every gran-row tile), or exact zeros past its end.

@@ -236,6 +236,19 @@ void set_job_seeds(Job& j, const unsigned long long* seeds, const int* seeded) {
     if (any) j.seeds.swap(s); else j.seeds.clear();
 }
 
+void set_job_output_rates(Job& j, const unsigned* rates) {
+    if (!rates) { j.out_rates.clear(); return; }
+    std::vector<int> r(j.B, 0);
+    bool any = false;
+    for (size_t b = 0; b < j.B; b++) {
+        if (rates[b] == 0 || rates[b] == (unsigned)j.v->sample_rate) continue;
+        resample_ratio(j.v->sample_rate, rates[b], "utterance " + std::to_string(b) + ": ");
+        r[b] = (int)rates[b];
+        any = true;
+    }
+    if (any) j.out_rates.swap(r); else j.out_rates.clear();
+}
+
 namespace {
 
 struct Runner {
@@ -423,13 +436,27 @@ struct DecoderBufs {
 };
 
 // Frame level of a synthesis pass (phase 2): tables, the latent, the flow's scratch, and unless the pass stops after
-// the flow the decoder and (when the caller passed no buffer) the waveforms.
+// the flow the decoder and (when the caller passed no buffer) the waveforms.  With output rates the decoder's
+// waveforms are always the pass's own, and the resampled ones go to the caller's buffer or to `rs`, with the tables of
+// the resampling launch.
 struct FrameBufs {
     FrameTables y;
     float *s, *epsz, *zp, *h, *acts, *outb, *wav;
     std::vector<float*> flow;                  // debug: z after each coupling layer, in the engine's channel order
     DecoderBufs dec;
+    float* rs;
+    ResampleSeg *rsegs, *rsegs_h; PcmPost *posts, *posts_h; FrameSeg *osegs, *osegs_h;
     void carve(Arena& dev, Arena& pin, const Job& j, bool own_wav) {
+        rs = nullptr; rsegs = rsegs_h = nullptr; posts = posts_h = nullptr; osegs = osegs_h = nullptr;
+        const bool resample = !j.out_rates.empty() && !j.encode_only;
+        if (resample) {
+            const size_t B = j.B;
+            rsegs = dev.get<ResampleSeg>(B); rsegs_h = pin.get<ResampleSeg>(B);
+            posts = dev.get<PcmPost>(B); posts_h = pin.get<PcmPost>(B);
+            osegs = dev.get<FrameSeg>(B); osegs_h = pin.get<FrameSeg>(B);
+            if (own_wav) rs = dev.get<float>((size_t)j.out_total + 4);
+            own_wav = true;
+        }
         const Arch& a = j.v->a;
         const size_t RY = (size_t)j.RY;
         y.carve(dev, pin, j);
@@ -461,7 +488,15 @@ struct ChunkBufs {
     PcmPost *post, *post_h;
     short* i16; unsigned* max;
     float* out_h;
-    void carve(Arena& dev, Arena& pin, const Job& j, bool pcm) {
+    // streams resampled after the post-path: tables, the resampled chunks and, leaving as i16, their conversion
+    ResampleSeg *rsegs, *rsegs_h; FrameSeg *osegs, *osegs_h; PcmPost *ipost, *ipost_h; float* rs;
+    void carve(Arena& dev, Arena& pin, const Job& j, bool pcm, long long rs_total = -1, bool rs_i16 = false) {
+        const bool resample = rs_total >= 0;
+        const size_t nr = resample ? j.fsegs.size() : 0;
+        rsegs = dev.get<ResampleSeg>(nr); rsegs_h = pin.get<ResampleSeg>(nr);
+        osegs = dev.get<FrameSeg>(nr); osegs_h = pin.get<FrameSeg>(nr);
+        ipost = dev.get<PcmPost>(nr); ipost_h = pin.get<PcmPost>(nr);
+        rs = resample ? dev.get<float>((size_t)rs_total + 4) : nullptr;
         const Voice& v = *j.v;
         const bool multi = v.num_speakers > 1;
         const size_t n = j.fsegs.size(), nslots = j.slot_sid.size();
@@ -475,9 +510,10 @@ struct ChunkBufs {
         dec.carve(dev, v, j.RY, false);
         post = pcm ? dev.get<PcmPost>(n) : nullptr;
         post_h = pcm ? pin.get<PcmPost>(n) : nullptr;
-        i16 = pcm ? dev.get<short>((size_t)j.total_samples + 8) : nullptr;
+        const size_t n_i16 = resample ? (rs_i16 ? (size_t)rs_total : 0) : (size_t)j.total_samples;
+        i16 = pcm ? dev.get<short>(n_i16 + 8) : nullptr;
         max = pcm ? dev.get<unsigned>(n) : nullptr;
-        out_h = pin.get<float>((size_t)j.total_samples);
+        out_h = pin.get<float>(std::max<size_t>((size_t)j.total_samples, resample ? (size_t)rs_total : 0));
     }
 };
 
@@ -556,6 +592,34 @@ void lay_out_frames(Job& j, const std::vector<int>& y_len, int hop) {
         cur += round_up(y_len[b] + HY, GY);
     }
     j.RY = cur; j.total_samples = out;
+}
+
+// What the job hands out (osegs, out_hop, out_total): the frame layout itself without output rates, else one segment of
+// ceil(n * up / down) samples per utterance, back to back.  Returns each utterance's filter (null: not resampled).
+std::vector<const ResampleFilter*> lay_out_output(Job& j, int hop) {
+    std::vector<const ResampleFilter*> filt;
+    j.osr.assign(j.B, j.v->sample_rate);
+    if (j.out_rates.empty() || j.encode_only) {
+        j.osegs = j.fsegs; j.out_hop = hop; j.out_total = j.total_samples;
+        return filt;
+    }
+    for (size_t b = 0; b < j.B; b++)
+        if (j.out_rates[b]) j.osr[b] = j.out_rates[b];
+    filt.assign(j.B, nullptr);
+    j.osegs.assign(j.B, FrameSeg{});
+    long long off = 0;
+    for (size_t b = 0; b < j.B; b++) {
+        const long long n = (long long)j.fsegs[b].len * hop;
+        long long n_out = n;
+        if (j.out_rates[b]) {
+            filt[b] = &voice_resampler(*j.v, j.out_rates[b], "utterance " + std::to_string(b) + ": ");
+            n_out = (n * filt[b]->up + filt[b]->down - 1) / filt[b]->down;
+        }
+        j.osegs[b] = FrameSeg{0, (int)n_out, 0, 0, off};
+        off += n_out;
+    }
+    j.out_hop = 1; j.out_total = off;
+    return filt;
 }
 
 // Fills the frame-level tables through their pinned mirrors; returns the level.
@@ -819,9 +883,11 @@ void Job::run(float* d_out, size_t d_out_cap) {
     // ---------------- frame level (phase 2) workspace ----------------
     // The stream is idle here, so the pinned staging of the X tables can be reused for the Y tables.
     lay_out_frames(*this, y_len, a.hop());
+    const std::vector<const ResampleFilter*> filt = lay_out_output(*this, a.hop());
     FrameBufs f;
     plan(C.dev_frame, C.pin, [&](Arena& dev, Arena& pin) { f.carve(dev, pin, *this, d_out == nullptr); });
     d_fsegs = f.y.fsegs;
+    d_osegs = f.osegs ? f.osegs : d_fsegs;
     if (debug) {
         expose(*this, "z_p", f.zp, I, 1); expose(*this, "z", f.s, I, 1);
         // flow.{f}: z after the coupling layer of the graph's flow.flows.{2f} (f = flow_n - 1 first).  The graph's Flip
@@ -831,6 +897,30 @@ void Job::run(float* d_out, size_t d_out_cap) {
         if (!encode_only) f.dec.expose_to(*this);
     }
     Level LY = upload_frames(*this, f.y, st);
+    long long rs_max_out = 0;
+    int rs_smem = 0;
+    double rs_flops = 0, rs_bytes = 0;
+    if (f.rsegs) {
+        for (size_t b = 0; b < B; b++) {
+            const FrameSeg& o = osegs[b];
+            const ResampleFilter* r = filt[b];
+            f.rsegs_h[b] = r ? ResampleSeg{r->taps, o.out_off, o.len, r->up, r->down, r->H, r->K}
+                             : ResampleSeg{nullptr, o.out_off, o.len, 0, 1, 0, 0};
+            f.posts_h[b] = PcmPost();
+            rs_max_out = std::max<long long>(rs_max_out, o.len);
+            const double n_in = (double)fsegs[b].len * a.hop();
+            rs_bytes += 4.0 * (n_in + o.len);
+            if (r) {
+                rs_smem = std::max(rs_smem, resample_span(r->up, r->down, r->K));
+                rs_flops += 2.0 * (double)o.len * (2.0 * r->H + 1.0) / r->up;
+                rs_bytes += 4.0 * (double)r->up * r->K;
+            }
+        }
+        memcpy(f.osegs_h, osegs.data(), B * sizeof(FrameSeg));
+        h2d(f.rsegs, f.rsegs_h, B * sizeof(ResampleSeg), st);
+        h2d(f.posts, f.posts_h, B * sizeof(PcmPost), st);
+        h2d(f.osegs, f.osegs_h, B * sizeof(FrameSeg), st);
+    }
 
     // ---------------- alignment expansion ----------------
     R.begin("align");
@@ -882,12 +972,18 @@ void Job::run(float* d_out, size_t d_out_cap) {
         return;
     }
     if (d_out) {
-        if ((size_t)total_samples > d_out_cap) throw Error(19, "caller-provided device output buffer is too small");
+        if ((size_t)out_total > d_out_cap) throw Error(19, "caller-provided device output buffer is too small");
         d_wav = d_out;
     } else {
-        d_wav = f.wav;
+        d_wav = f.rs ? f.rs : f.wav;
     }
-    run_decoder(R, LY, f.y, f.dec, f.s, d_wav);
+    run_decoder(R, LY, f.y, f.dec, f.s, f.rsegs ? f.wav : d_wav);
+    if (f.rsegs) {
+        R.begin("resample");
+        launch_resample(f.wav, f.y.fsegs, f.posts, a.hop(), f.rsegs, (int)B, rs_max_out, rs_smem, d_wav, st);
+        R.count(rs_flops, rs_bytes);
+        R.end();
+    }
     SB_CUDA(cudaEventRecord(C.ev_end, st));
     SB_CUDA(cudaStreamSynchronize(st));
     SB_CUDA(cudaGetLastError());
@@ -951,13 +1047,19 @@ static void fill_fade(PcmPost& p, int fade, long long len) {
 namespace {
 // The PCM post-path of one chunk pass: per-chunk trims, crossfade table and gain.
 struct ChunkPcm { const long long *trim_lo, *trim_hi; int fade; const float* gain; };
+// Streams resampled after the post-path: one resampler per chunk (null: none), the flush flags and the output format;
+// segs / ends are filled by the pass, and applied to the resamplers once it has succeeded.
+struct ChunkResample {
+    Resampler* const* rs; const int* last; int format;
+    std::vector<ResampleSeg> segs; std::vector<long long> ends; long long total = 0, max_out = 0; int smem = 0;
+};
 
 // One decoder pass over chunks z[k][lo[k] : hi[k]), k < n, laid out as the segments of one frame level: the result is
 // left on the device (job-owned arena), and with `pcm` converted to i16.  Every check runs before any device work.
 // Errors name the chunk and its frame range, except through the single-chunk entry points (`single`), which keep
 // the messages they always gave.
 ChunkBufs decode_chunks_device(Voice* v, const Latent* const* z, const long long* lo, const long long* hi, size_t n,
-                               Job& j, const ChunkPcm* pcm, bool single) {
+                               Job& j, const ChunkPcm* pcm, bool single, ChunkResample* rsp = nullptr) {
     const Arch& a = v->a;
     const int hop = a.hop();
     std::vector<int> len(n);
@@ -983,13 +1085,51 @@ ChunkBufs decode_chunks_device(Voice* v, const Latent* const* z, const long long
             if (it == j.slot_sid.end()) j.slot_sid.push_back((int)sid);
         }
         len[k] = (int)(hi[k] - lo[k]);
+        if (rsp && rsp->rs[k]) {
+            const Resampler* r = rsp->rs[k];
+            if (r->v != v) fail(k, "the resampler was made for another voice", "");
+            if (r->ended) fail(k, "the resampler's stream has already been flushed", "");
+            for (size_t q = 0; q < k; q++)
+                if (rsp->rs[q] == r) fail(k, "the resampler of chunk " + std::to_string(q) + " appears twice in one call", "");
+            if (rsp->last && rsp->last[k] != 0 && rsp->last[k] != 1)
+                fail(k, "last flag " + std::to_string(rsp->last[k]) + " is neither 0 nor 1", "");
+        }
+    }
+    if (rsp) {
+        rsp->segs.assign(n, ResampleSeg{});
+        rsp->ends.assign(n, 0);
+        long long off = 0;
+        for (size_t k = 0; k < n; k++) {
+            const long long m = (long long)len[k] * hop - (pcm->trim_lo ? pcm->trim_lo[k] : 0) * hop -
+                                (pcm->trim_hi ? pcm->trim_hi[k] : 0) * hop;
+            ResampleSeg& s = rsp->segs[k];
+            s.out_off = off;
+            const Resampler* r = rsp->rs[k];
+            if (!r) {
+                s.n_out = m;
+            } else {
+                const ResampleFilter& f = r->f;
+                const long long N = r->consumed + m;
+                rsp->ends[k] = resample_emit_end(f, N, rsp->last && rsp->last[k]);
+                s.taps = f.taps; s.up = f.up; s.down = f.down; s.H = f.H; s.K = f.K;
+                s.n_out = rsp->ends[k] - r->emitted;
+                s.hist = r->hist[r->cur]; s.hist_out = r->hist[1 - r->cur];
+                s.c = r->consumed; s.j0 = r->emitted; s.h = r->h; s.h_out = (int)std::min<long long>(N, f.K - 1);
+                rsp->smem = std::max(rsp->smem, resample_span(f.up, f.down, f.K));
+            }
+            rsp->max_out = std::max(rsp->max_out, s.n_out);
+            off += s.n_out;
+        }
+        rsp->total = off;
     }
     j.v = v; j.B = n; j.ctx = v->acquire();
     Context& C = *j.ctx;
     SB_CUDA(cudaSetDevice(v->device));
     lay_out_frames(j, len, hop);
     ChunkBufs b;
-    plan(C.dev_frame, C.pin, [&](Arena& dev, Arena& pin) { b.carve(dev, pin, j, pcm != nullptr); });
+    plan(C.dev_frame, C.pin, [&](Arena& dev, Arena& pin) {
+        b.carve(dev, pin, j, pcm != nullptr, rsp ? rsp->total : -1, rsp && rsp->format == 1);
+    });
     j.d_cond = b.cond; j.d_fsegs = b.y.fsegs; j.d_wav = b.wav;
     C.events_used = 0;
     if (!C.ev_begin) { SB_CUDA(cudaEventCreate(&C.ev_begin)); SB_CUDA(cudaEventCreate(&C.ev_end)); }
@@ -1018,10 +1158,61 @@ ChunkBufs decode_chunks_device(Voice* v, const Latent* const* z, const long long
             longest = std::max(longest, (long long)len[k] * hop);
         }
         h2d(b.post, b.post_h, n * sizeof(PcmPost), st);
-        launch_i16(b.wav, b.y.fsegs, b.post, (int)n, hop, longest, b.max, b.i16, st);
+        if (!rsp) {
+            launch_i16(b.wav, b.y.fsegs, b.post, (int)n, hop, longest, b.max, b.i16, st);
+        } else {
+            for (size_t k = 0; k < n; k++) {
+                b.rsegs_h[k] = rsp->segs[k];
+                b.osegs_h[k] = FrameSeg{0, (int)rsp->segs[k].n_out, 0, 0, rsp->segs[k].out_off};
+                b.ipost_h[k] = PcmPost();
+            }
+            h2d(b.rsegs, b.rsegs_h, n * sizeof(ResampleSeg), st);
+            h2d(b.osegs, b.osegs_h, n * sizeof(FrameSeg), st);
+            h2d(b.ipost, b.ipost_h, n * sizeof(PcmPost), st);
+            R.begin("resample");
+            launch_resample(b.wav, b.y.fsegs, b.post, hop, b.rsegs, (int)n, rsp->max_out, rsp->smem, b.rs, st);
+            R.end();
+            if (rsp->format == 1) launch_i16(b.rs, b.osegs, b.ipost, (int)n, 1, rsp->max_out, b.max, b.i16, st);
+        }
     }
     SB_CUDA(cudaEventRecord(C.ev_end, st));
     return b;
+}
+
+void chunks_resampled(Voice* v, const Latent* const* z, const long long* lo, const long long* hi, const ChunkPcm& pcm,
+                      ChunkResample& rsp, size_t n, std::vector<std::vector<float>>& out_f32,
+                      std::vector<std::vector<int16_t>>& out_i16) {
+    out_f32.clear(); out_i16.clear();
+    if (n == 0) return;
+    if (rsp.format != 0 && rsp.format != 1) throw Error(19, "format " + std::to_string(rsp.format) + " is neither 0 (f32) nor 1 (i16)");
+    Job j;
+    const ChunkBufs b = decode_chunks_device(v, z, lo, hi, n, j, &pcm, false, &rsp);
+    cudaStream_t st = j.ctx->stream;
+    const size_t es = rsp.format == 1 ? 2 : 4;
+    SB_CUDA(cudaMemcpyAsync(b.out_h, rsp.format == 1 ? (const void*)b.i16 : (const void*)b.rs, (size_t)rsp.total * es,
+                            cudaMemcpyDeviceToHost, st));
+    SB_CUDA(cudaStreamSynchronize(st));
+    SB_CUDA(cudaGetLastError());
+    for (size_t k = 0; k < n; k++) {
+        Resampler* r = rsp.rs[k];
+        if (!r) continue;
+        const ResampleSeg& s = rsp.segs[k];
+        r->consumed = s.c + ((long long)j.fsegs[k].len * v->a.hop() - b.post_h[k].trim_lo - b.post_h[k].trim_hi);
+        r->emitted = rsp.ends[k];
+        r->cur ^= 1;
+        r->h = s.h_out;
+        r->ended = rsp.last && rsp.last[k];
+    }
+    if (rsp.format == 1) out_i16.resize(n); else out_f32.resize(n);
+    for (size_t k = 0; k < n; k++) {
+        const long long o = rsp.segs[k].out_off, m = rsp.segs[k].n_out;
+        if (rsp.format == 1) {
+            const int16_t* h = reinterpret_cast<const int16_t*>(b.out_h);
+            out_i16[k].assign(h + o, h + o + m);
+        } else {
+            out_f32[k].assign(b.out_h + o, b.out_h + o + m);
+        }
+    }
 }
 
 void chunks_f32(Voice* v, const Latent* const* z, const long long* lo, const long long* hi, size_t n,
@@ -1092,14 +1283,24 @@ void decode_latent_chunk_pcm(Voice* v, const Latent* z, long long lo, long long 
     out.swap(o[0]);
 }
 
+void decode_latent_chunks_resampled(Voice* v, const Latent* const* z, const long long* lo, const long long* hi,
+                                    const long long* trim_lo_frames, const long long* trim_hi_frames, size_t n, int fade,
+                                    const float* gain, Resampler* const* rs, const int* last, int format,
+                                    std::vector<std::vector<float>>& out_f32, std::vector<std::vector<int16_t>>& out_i16) {
+    if (n > 0 && !rs) throw Error(19, "null resampler table");
+    ChunkResample rsp;
+    rsp.rs = rs; rsp.last = last; rsp.format = format;
+    chunks_resampled(v, z, lo, hi, ChunkPcm{trim_lo_frames, trim_hi_frames, fade, gain}, rsp, n, out_f32, out_i16);
+}
+
 void job_i16_to_host(Job& j, float gain, int16_t* dst) {
     if (!j.ran || j.encode_only) throw Error(19, "job has not produced audio");
     SB_CUDA(cudaSetDevice(j.v->device));
     cudaStream_t st = j.ctx->stream;
-    const int hop = j.v->a.hop();
-    const size_t n = (size_t)j.total_samples;
+    const int hop = j.out_hop;
+    const size_t n = (size_t)j.out_total;
     long long mx = 0;
-    for (size_t b = 0; b < j.B; b++) mx = std::max<long long>(mx, (long long)j.y_len[b] * hop);
+    for (size_t b = 0; b < j.B; b++) mx = std::max<long long>(mx, (long long)j.osegs[b].len * hop);
     // stream-ordered scratch, returned to the pool at once: device memory held after a run does not grow
     short* d_i16 = nullptr; unsigned* d_max = nullptr; PcmPost* d_post = nullptr;
     SB_CUDA(cudaMallocAsync(&d_i16, n * 2 + 16, st));
@@ -1109,7 +1310,7 @@ void job_i16_to_host(Job& j, float gain, int16_t* dst) {
     const std::vector<PcmPost> posts(j.B, post);
     // pageable source: the call returns once the entries are staged, so `posts` may go out of scope before the copy runs
     SB_CUDA(cudaMemcpyAsync(d_post, posts.data(), sizeof(PcmPost) * j.B, cudaMemcpyHostToDevice, st));
-    launch_i16(j.d_wav, j.d_fsegs, d_post, (int)j.B, hop, mx, d_max, d_i16, st);
+    launch_i16(j.d_wav, j.d_osegs, d_post, (int)j.B, hop, mx, d_max, d_i16, st);
     cudaError_t e = cudaMemcpyAsync(dst, d_i16, n * 2, cudaMemcpyDeviceToHost, st);
     cudaFreeAsync(d_i16, st);
     cudaFreeAsync(d_max, st);
@@ -1122,13 +1323,12 @@ void job_i16_to_host(Job& j, float gain, int16_t* dst) {
 void job_pcm16(Job& j, float gain, std::vector<std::vector<int16_t>>& out) {
     Context& C = *j.ctx;
     SB_CUDA(cudaSetDevice(j.v->device));
-    C.pin.reserve((size_t)j.total_samples * 2);
-    int16_t* h = C.pin.get<int16_t>((size_t)j.total_samples);
+    C.pin.reserve((size_t)j.out_total * 2);
+    int16_t* h = C.pin.get<int16_t>((size_t)j.out_total);
     job_i16_to_host(j, gain, h);
-    const int hop = j.v->a.hop();
     out.resize(j.B);
     for (size_t b = 0; b < j.B; b++)
-        out[b].assign(h + j.fsegs[b].out_off, h + j.fsegs[b].out_off + (size_t)j.y_len[b] * hop);
+        out[b].assign(h + j.osegs[b].out_off, h + j.osegs[b].out_off + (size_t)j.osegs[b].len * j.out_hop);
 }
 
 }  // namespace sb200

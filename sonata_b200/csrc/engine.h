@@ -90,6 +90,19 @@ struct UpStageW { int u, k, cin, cout; std::vector<ConvW> phase; ConvW fused; st
 
 struct SynthConfig { long long speaker = 0; bool has_speaker = false; float noise_scale = 0.667f, length_scale = 1.f, noise_w = 0.8f; };
 
+// resample_poly's default filter for in_rate -> out_rate (resample.cu): up / down the reduced ratio, H = 10 max(up, down)
+// and 2H + 1 taps; on the device the taps are stored phase-major, K per phase (ResampleSeg).
+struct ResampleFilter { int up = 1, down = 1, H = 0, K = 0; float* taps = nullptr; };
+// The output rates a caller may ask for.  A rate of 0 or equal to the voice's own means no resampling.
+bool output_rate_supported(long long rate);
+// The filter's ratio and shape (no taps) for in_rate -> out_rate; throws OPERATION_ERROR prefixed by `who` when out_rate
+// is not a supported rate or the ratio is too large for the kernel.  in_rate == out_rate is not a resampling ratio.
+ResampleFilter resample_ratio(int in_rate, long long out_rate, const std::string& who);
+// The 2H + 1 taps in natural order, designed in double (firwin with a Kaiser(5.0) window, times up), rounded to f32.
+std::vector<float> resample_taps(int up, int down);
+// The phase-major image of `h`: [up][K], zero past 2H.
+std::vector<float> resample_phase_major(const std::vector<float>& h, int up, int K);
+
 struct Context;   // stream + arenas for one in-flight call
 
 struct Voice {
@@ -132,6 +145,8 @@ struct Voice {
     std::mutex pool_mu;
     std::vector<Context*> pool;
     std::atomic<unsigned long long> call_counter{0};
+    std::mutex rs_mu;
+    std::map<long long, ResampleFilter> rs_filters;   // by output rate, taps on the device: built on first use
 
     ~Voice();
     Context* acquire();
@@ -143,6 +158,8 @@ struct Voice {
 };
 
 Voice* load_voice(const std::string& config_path, int device);
+// The voice's filter to `out_rate` with its phase-major taps on the voice's device, built and cached on first use.
+const ResampleFilter& voice_resampler(Voice& v, long long out_rate, const std::string& who);
 ConvW debug_make_conv(Voice& v, const float* w, const float* bias, int cout, int cin, int k, int dil);
 
 struct Region { std::string name; cudaEvent_t e0, e1; double flops = 0, bytes = 0; int launches = 0; float ms = 0; };
@@ -202,6 +219,8 @@ struct Job {
     std::vector<int> id_frames;       // frames per id of the last run, packed like ids: filled by job_id_frames
     std::vector<std::vector<float>> eps_w, eps_z; std::vector<size_t> eps_z_frames;
     std::vector<NoiseSeed> seeds;     // one per utterance, empty when none is seeded (set_job_seeds)
+    std::vector<int> out_rates;       // one per utterance, 0 = the voice's rate; empty when none resamples
+                                      // (set_job_output_rates)
     // X layout
     int RX = 0; std::vector<SegInfo> xsegs; int max_tx = 0;
     // Y layout
@@ -215,6 +234,12 @@ struct Job {
     int* d_cum = nullptr;
     FrameSeg* d_fsegs = nullptr;
     float* d_wav = nullptr;
+    // What the job hands out: utterance b is d_wav[osegs[b].out_off ..) of osegs[b].len * out_hop samples, and
+    // d_osegs mirrors osegs on the device.  Without output rates these are fsegs, the hop and total_samples; with them,
+    // one segment of len = n_out per utterance at out_hop = 1.
+    std::vector<FrameSeg> osegs; int out_hop = 1; long long out_total = 0;
+    std::vector<int> osr;             // sample rate of each handed-out utterance
+    FrameSeg* d_osegs = nullptr;
     float* d_cond = nullptr;       // effective biases of the speaker-conditioned convs for this call, [slot][cond_rows]
     std::map<std::string, std::pair<float*, int>> dbg;   // name -> (device ptr, cols)
     std::map<std::string, int> dbg_level;                // name -> U (rows per frame), 0 for X level, -1 for an X-level
@@ -246,6 +271,9 @@ void set_job_durations(Job& j, const float* scale, const int* frames);
 // for all.  Flags other than 0 / 1, or seeds on a job with injected noise, fail naming the utterance and leave the job
 // as it was.
 void set_job_seeds(Job& j, const unsigned long long* seeds, const int* seeded);
+// Per-utterance output rates of the job's next run (rates[0 .. B), 0 or the voice's rate: none), or null for none.
+// Every entry is checked first; an unsupported rate fails naming the utterance and leaves the job's rates as they were.
+void set_job_output_rates(Job& j, const unsigned* rates);
 // Frames per id of the job's last run, packed like its ids: one device->host copy of the batch's cum rows through the
 // context's page-locked staging, differenced on the host.  Cached until the next run.
 const std::vector<int>& job_id_frames(Job& j);
@@ -278,6 +306,29 @@ void decode_latent_chunks_pcm(Voice* v, const Latent* const* z, const long long*
                               const float* gain, std::vector<std::vector<int16_t>>& out, float* ms);
 void decode_latent_chunk_pcm(Voice* v, const Latent* z, long long lo, long long hi, long long trim_lo_frames,
                              long long trim_hi_frames, int fade, float gain, std::vector<int16_t>& out, float* ms);
+// One stream's resampling state: the filter to its output rate, the last inputs (two device buffers of K floats each,
+// read and written alternately), and how many inputs it has consumed and outputs it has emitted.
+struct Resampler {
+    Voice* v = nullptr;
+    ResampleFilter f;
+    float* hist[2] = {nullptr, nullptr};
+    int cur = 0, h = 0;
+    long long consumed = 0, emitted = 0;
+    bool ended = false;
+    ~Resampler();
+};
+Resampler* create_resampler(Voice* v, long long out_rate);
+// Outputs of a stream whose first n inputs have arrived: all ceil(n * up / down) once it has ended, else those whose
+// every input has arrived (j * down + H < n * up).
+long long resample_emit_end(const ResampleFilter& f, long long n, bool ended);
+// decode_latent_chunks_pcm's post-path (trim, crossfade, gain) per chunk, then chunk k appended to its stream's
+// resampler rs[k] (null: the chunk is returned at the voice's rate, as that post-path leaves it), emitting every output
+// it can, and flushing the stream when last[k] is 1.  format 0: f32 in out_f32; 1: i16 normalised to each emitted
+// chunk's own peak, in out_i16.  A resampler may appear once per call, and must belong to `v`.
+void decode_latent_chunks_resampled(Voice* v, const Latent* const* z, const long long* lo, const long long* hi,
+                                    const long long* trim_lo_frames, const long long* trim_hi_frames, size_t n, int fade,
+                                    const float* gain, Resampler* const* rs, const int* last, int format,
+                                    std::vector<std::vector<float>>& out_f32, std::vector<std::vector<int16_t>>& out_i16);
 void job_pcm16(Job& j, float gain, std::vector<std::vector<int16_t>>& out);
 // Peak-normalised 16-bit PCM of every utterance of a finished job (to_i16_vec after a linear gain), converted on the
 // device and copied to `dst`: total_samples values laid out like the job's waveforms, in host memory that is best

@@ -5,6 +5,7 @@
 // The reference executes all of these inside onnxruntime (piper/src/lib.rs:362-379); the
 // arithmetic restated here follows oracle/vits_oracle.py function by function.
 #include "common.cuh"
+#include <algorithm>
 #include <climits>
 #include <math.h>
 
@@ -712,6 +713,60 @@ __global__ void i16_convert_kernel(const float* __restrict__ wav, const FrameSeg
     }
 }
 
+// ------------------------------------------------------------------ polyphase resampling (scipy's resample_poly)
+// Output j of a segment of n inputs is  y[j] = sum_i x[i] * h[j*down + H - i*up]  over 0 <= i < n with the tap index in
+// [0, 2H], evaluated as ONE fmaf chain in ascending i starting from 0.  With t = j*down + H, phase p = t % up and
+// i_max = t / up, input i_max - k meets tap h[p + k*up] = taps[p][k].  The chain depends on j, n and the ratio only, so
+// a sample comes out with the same bits whatever buffer, batch or block split it is computed in.  A block computes runs
+// of RS_OUTS consecutive outputs: it stages the input span of the run in shared memory, read through pcm_value (the
+// segment's trim, crossfade and gain), then each thread evaluates its outputs from there, the taps of one output being
+// contiguous in the phase-major table.
+// A stream's segment continues an input sequence: its samples are inputs c .. c + n of the stream, the h inputs before
+// them come from `hist`, and it writes outputs j0 .. j0 + n_out.  Block 0 of the segment also stores the stream's last
+// h_out inputs into `hist_out` (a different buffer, so no block reads what another writes).  Outputs are only emitted
+// once every input they read has arrived (or the stream has ended), so the chain of output j is the same as over the
+// whole stream in one buffer.
+__device__ __forceinline__ float rs_input(const ResampleSeg& r, const PcmSeg& s, long long g) {
+    return g < r.c ? r.hist[g - (r.c - r.h)] : pcm_value(s, g - r.c);
+}
+__global__ void resample_kernel(const float* __restrict__ wav, const FrameSeg* __restrict__ fsegs,
+                                const PcmPost* __restrict__ posts, int hop, const ResampleSeg* __restrict__ segs,
+                                float* __restrict__ out) {
+    extern __shared__ float xs[];
+    pdl_trigger(); pdl_wait();
+    const ResampleSeg r = segs[blockIdx.y];
+    const PcmSeg s = pcm_seg(wav, fsegs[blockIdx.y], posts + blockIdx.y, hop);
+    float* y = out + r.out_off;
+    if (r.up == 0) {
+        for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < s.n; i += (long long)gridDim.x * blockDim.x)
+            y[i] = pcm_value(s, i);
+        return;
+    }
+    const long long N = r.c + s.n;            // inputs of the stream so far
+    if (blockIdx.x == 0 && r.hist_out)
+        for (int q = threadIdx.x; q < r.h_out; q += blockDim.x) r.hist_out[q] = rs_input(r, s, N - r.h_out + q);
+    const int up = r.up, down = r.down, H2 = 2 * r.H, K = r.K;
+    for (long long a = (long long)blockIdx.x * RS_OUTS; a < r.n_out; a += (long long)gridDim.x * RS_OUTS) {
+        const long long j_a = r.j0 + a, j_b = r.j0 + min(a + RS_OUTS, r.n_out);
+        const long long i_lo = max(0ll, (j_a * down + r.H) / up - (K - 1));
+        const long long i_hi = min(((j_b - 1) * down + r.H) / up, N - 1);
+        for (int q = threadIdx.x; q <= (int)(i_hi - i_lo); q += blockDim.x) xs[q] = rs_input(r, s, i_lo + q);
+        __syncthreads();
+        for (long long j = j_a + threadIdx.x; j < j_b; j += blockDim.x) {
+            const long long t = j * down + r.H, im = t / up;
+            const int p = (int)(t - im * up);
+            const int kmax = (int)min((long long)((H2 - p) / up), im);      // i >= 0
+            const int kmin = (int)max(0ll, im - (N - 1));                     // i < N
+            const float* h = r.taps + p * K;
+            const float* x = xs + (int)(im - i_lo);
+            float acc = 0.f;
+            for (int k = kmax; k >= kmin; k--) acc = fmaf(x[-k], __ldg(h + k), acc);
+            y[j - r.j0] = acc;
+        }
+        __syncthreads();
+    }
+}
+
 // Frame-level input of a chunk pass: every row is a plain 16-byte copy of its segment's latent row or exact zeros, so a
 // chunk's rows hold the same bits whatever else shares the pass.
 __global__ void gather_rows_kernel(const GatherSeg* __restrict__ segs, const int* __restrict__ tile_seg, int gran, int c4,
@@ -952,6 +1007,16 @@ void launch_i16(const float* wav, const FrameSeg* fsegs, const PcmPost* posts, i
     launch_pdl(i16_absmax_kernel, dim3(grid), dim3(256), 0, st, wav, fsegs, posts, hop, maxbits);
     launch_pdl(i16_convert_kernel, dim3(grid), dim3(256), 0, st, wav, fsegs, posts, hop, maxbits, out);
     g_launch_count += 2;
+}
+
+void launch_resample(const float* wav, const FrameSeg* fsegs, const PcmPost* posts, int hop, const ResampleSeg* segs,
+                     int nseg, long long max_out, int smem_floats, float* out, cudaStream_t st) {
+    if (nseg <= 0) return;
+    const size_t smem = sizeof(float) * (size_t)smem_floats;
+    if (smem > 48 * 1024) throw_launch_error("resample: input span exceeds 48 KB of shared memory");
+    const long long bx = std::min<long long>(std::max<long long>((max_out + RS_OUTS - 1) / RS_OUTS, 1), 4096);
+    launch_pdl(resample_kernel, dim3((unsigned)bx, nseg), dim3(256), smem, st, wav, fsegs, posts, hop, segs, out);
+    g_launch_count++;
 }
 
 void launch_gather_rows(const GatherSeg* segs, const int* tile_seg, int gran, int rows, int cols, float* s, cudaStream_t st) {

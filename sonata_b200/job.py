@@ -10,15 +10,15 @@ import numpy as np
 
 from . import _native as N
 from .core import Audio
-from .piper import _check, _config_array, _duration_arrays, _ptr, _seed_arrays, _take_audio
+from .piper import _check, _config_array, _duration_arrays, _ptr, _rate_array, _seed_arrays, _take_audio
 
 
 class SynthesisJob:
     def __init__(self, model, batches: Sequence[Sequence[int]], eps_w: Optional[Sequence] = None,
                  eps_z: Optional[Sequence] = None, debug: bool = False, configs: Optional[Sequence] = None,
-                 seeds: Optional[Sequence] = None):
+                 seeds: Optional[Sequence] = None, output_rates: Optional[Sequence] = None):
         """`configs`: one PiperSynthesisConfig per utterance (see set_configs); None keeps the voice's fallback config.
-        `seeds`: noise seeds (see set_seeds)."""
+        `seeds`: noise seeds (see set_seeds).  `output_rates`: output sample rates (see set_output_rates)."""
         self._m = model
         self._lib = model._lib
         n = len(batches)
@@ -26,6 +26,7 @@ class SynthesisJob:
         self._lens = [len(b) for b in batches]
         _config_array(configs, n)             # argument errors before the job exists
         _seed_arrays(seeds, n)
+        _rate_array(output_rates, n)
         packed = np.ascontiguousarray(np.concatenate([np.asarray(b, dtype=np.int64) for b in batches]))
         offs = np.zeros(n + 1, dtype=np.uint64)
         offs[1:] = np.cumsum([len(b) for b in batches])
@@ -60,6 +61,8 @@ class SynthesisJob:
             self.set_configs(configs)
         if seeds is not None:
             self.set_seeds(seeds)
+        if output_rates is not None:
+            self.set_output_rates(output_rates)
 
     def set_configs(self, configs: Optional[Sequence]) -> None:
         """Per-utterance PiperSynthesisConfigs for the next run, or None for the voice's fallback config.  A wrong
@@ -83,6 +86,15 @@ class SynthesisJob:
         sv, sf = _seed_arrays(seeds, self.batch)
         err = N.sb200_error()
         _check(self._lib.sb200_job_set_seeds(self._h, _ptr(sv, C.c_uint64), _ptr(sf, C.c_int32), C.byref(err)), err)
+
+    def set_output_rates(self, rates: Optional[Sequence]) -> None:
+        """Per-utterance output sample rates for the next run (see VitsModel.infer_batch_with_values), or None for the
+        voice's rate throughout.  After such a run, fetch, fetch_i16, copy_out and the samples and offsets of lengths
+        all report the resampled signal.  An unsupported rate raises OperationError naming the utterance and leaves the
+        job's rates as they were."""
+        r = _rate_array(rates, self.batch)
+        err = N.sb200_error()
+        _check(self._lib.sb200_job_set_output_rates(self._h, _ptr(r, C.c_uint32), C.byref(err)), err)
 
     def id_frames(self) -> List[np.ndarray]:
         """Frames per id of the last run, one int32 array per utterance (one device->host copy for the batch)."""

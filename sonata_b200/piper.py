@@ -23,6 +23,7 @@ from .core import (Audio, AudioInfo, AudioSamples, OperationError, PhonemeAlignm
 MIN_CHUNK_SIZE = 44      # piper/src/lib.rs:18
 MAX_CHUNK_SIZE = 1024    # piper/src/lib.rs:19
 HOP = 256                # piper/src/lib.rs:910
+OUTPUT_RATES = (8000, 11025, 16000, 22050, 24000, 32000, 44100, 48000)    # rates results can be resampled to
 
 
 @dataclass
@@ -143,18 +144,45 @@ def _seed_arrays(seeds, n: int):
     return vals, flags
 
 
+def _rate_array(rates, n: int):
+    """The C image of per-utterance output rates (u32), or None when `rates` is None.  rates[b] is one of OUTPUT_RATES,
+    or None / 0 for the voice's own rate; the library also treats the voice's own rate as no resampling."""
+    if rates is None:
+        return None
+    out = np.zeros(n, np.uint32)
+    for b, r in enumerate(_per_utterance(rates, n, "output rates")):
+        if r is None:
+            continue
+        if isinstance(r, bool) or not isinstance(r, numbers.Integral) or (int(r) != 0 and int(r) not in OUTPUT_RATES):
+            raise OperationError(f"utterance {b}: output rate {r!r} Hz is not supported "
+                                 f"({', '.join(map(str, OUTPUT_RATES))}, or 0 / None for the voice's rate)")
+        out[b] = int(r)
+    return out
+
+
+def rate_ratio(in_rate: int, out_rate: Optional[int]) -> Tuple[int, int]:
+    """(up, down): out_rate / in_rate reduced, (1, 1) for no resampling (None, 0 or the same rate)."""
+    if not out_rate or int(out_rate) == int(in_rate):
+        return 1, 1
+    g = math.gcd(int(in_rate), int(out_rate))
+    return int(out_rate) // g, int(in_rate) // g
+
+
 def _ptr(a, ctype):
     return None if a is None else a.ctypes.data_as(C.POINTER(ctype))
 
 
-def _alignment(phonemes: str, src_char: Sequence[int], frames: Sequence[int], n_samples: int) -> List[PhonemeAlignment]:
+def _alignment(phonemes: str, src_char: Sequence[int], frames: Sequence[int], n_samples: int,
+               up: int = 1, down: int = 1) -> List[PhonemeAlignment]:
     """Groups per-id frame counts by the character each id came from: bos (`^`), one entry per kept character (its id
     and its pad) and eos (`$`), contiguous from sample 0.  An utterance whose ids all got 0 frames is still one frame
-    long; that frame (after every id) goes to the last entry, so the entries always end at n_samples."""
+    long; that frame (after every id) goes to the last entry, so the entries always end at n_samples.  Audio resampled
+    by up/down puts the boundary after F frames at ceil(F * hop * up / down)."""
     total = int(sum(int(f) for f in frames))
-    hop = n_samples // max(total, 1)
+    hop = n_samples // max(total, 1) if (up, down) == (1, 1) else HOP
+    at = lambda frames_before: -((-frames_before * hop * up) // down)
     out: List[PhonemeAlignment] = []
-    start, i = 0, 0
+    start, i, fsum = 0, 0, 0
     while i < len(frames):
         src = int(src_char[i])
         j, f = i, 0
@@ -162,8 +190,10 @@ def _alignment(phonemes: str, src_char: Sequence[int], frames: Sequence[int], n_
             f += int(frames[j])
             j += 1
         ph = phonemes[src] if src >= 0 else ("^" if i == 0 else "$")
-        out.append(PhonemeAlignment(ph, start, f * hop))
-        start += f * hop
+        fsum += f
+        end = at(fsum)
+        out.append(PhonemeAlignment(ph, start, end - start))
+        start = end
         i = j
     if out and start != n_samples:
         out[-1].num_samples += n_samples - start
@@ -316,16 +346,21 @@ class _VitsCommons:
         return _take_audio(a)
 
     def speak_batch(self, phoneme_batches: Sequence[str],
-                    configs: Optional[Sequence[PiperSynthesisConfig]] = None, seeds: Optional[Sequence] = None) -> List[Audio]:
+                    configs: Optional[Sequence[PiperSynthesisConfig]] = None, seeds: Optional[Sequence] = None,
+                    output_rates: Optional[Sequence] = None) -> List[Audio]:
         """`configs`: one PiperSynthesisConfig per utterance (speaker and scales), still synthesised as one pass;
-        None uses the fallback config for every utterance.  `seeds`: noise seeds as for infer_batch_with_values."""
+        None uses the fallback config for every utterance.  `seeds`: noise seeds as for infer_batch_with_values.
+        `output_rates`: per-utterance output sample rates as for infer_batch_with_values."""
         n = len(phoneme_batches)
         _config_array(configs, n)             # argument errors before any id mapping
         sv, _ = _seed_arrays(seeds, n)
+        rates = _rate_array(output_rates, n)
         if n == 0:
             return []
-        if configs is not None or sv is not None:
+        if configs is not None or sv is not None or rates is not None:
             extra = {} if sv is None else {"seeds": seeds}
+            if rates is not None:
+                extra["output_rates"] = output_rates
             return self.infer_batch_with_values([self.phonemes_to_input_ids(p) for p in phoneme_batches], configs,
                                                 **extra)
         arr = (C.c_char_p * n)(*[p.encode("utf-8") for p in phoneme_batches])
@@ -344,19 +379,26 @@ class _VitsCommons:
 
     def infer_batch_with_values(self, batches: Sequence[Sequence[int]],
                                 configs: Optional[Sequence[PiperSynthesisConfig]] = None,
-                                seeds: Optional[Sequence] = None) -> List[Audio]:
+                                seeds: Optional[Sequence] = None,
+                                output_rates: Optional[Sequence] = None) -> List[Audio]:
         """Batched infer_with_values.  `configs`: one PiperSynthesisConfig per utterance (speaker and scales), or None
         for the fallback config; each utterance's result equals a single-utterance call with its config as the
         fallback, except for the on-device noise of an unseeded utterance, whose draws depend on the batch position.
 
         `seeds`: one noise seed per utterance, an int in [0, 2**64) or None.  A seeded utterance's noise depends on its
         seed alone, so its result is the same bits in any batch, on any call and on any handle of the voice; an
-        unseeded one keeps the positional noise of a call without seeds."""
+        unseeded one keeps the positional noise of a call without seeds.
+
+        `output_rates`: one output sample rate per utterance, one of OUTPUT_RATES, or None / 0 for the voice's own.
+        The waveform is resampled on the device with scipy.signal.resample_poly's default filter, and the Audio
+        reports the rate it is at."""
         n = len(batches)
         cfgs = _config_array(configs, n)
         sv, _ = _seed_arrays(seeds, n)
-        if sv is not None:
-            return [a for a, _ in self.infer_batch_with_durations(batches, configs, seeds=seeds)]
+        rates = _rate_array(output_rates, n)
+        if sv is not None or rates is not None:
+            return [a for a, _ in self.infer_batch_with_durations(batches, configs, seeds=seeds,
+                                                                  output_rates=output_rates)]
         packed = np.ascontiguousarray(np.concatenate([np.asarray(b, dtype=np.int64) for b in batches]))
         offs = np.zeros(n + 1, dtype=np.uint64)
         offs[1:] = np.cumsum([len(b) for b in batches])
@@ -371,19 +413,22 @@ class _VitsCommons:
                                    configs: Optional[Sequence[PiperSynthesisConfig]] = None,
                                    duration_scales: Optional[Sequence] = None,
                                    durations: Optional[Sequence] = None,
-                                   seeds: Optional[Sequence] = None) -> List[Tuple[Audio, np.ndarray]]:
+                                   seeds: Optional[Sequence] = None,
+                                   output_rates: Optional[Sequence] = None) -> List[Tuple[Audio, np.ndarray]]:
         """infer_batch_with_values with per-id duration control, returning (audio, frames per id) per utterance.
 
         duration_scales[b]: one scale (finite, >= 0) per id of utterance b, applied before the duration's ceil, so 1.0
         gives the plain result bit for bit; durations[b]: one frame count per id, -1 for "predicted" or >= 0 to fix it.
         Either list, or any of its entries, may be None.  The frame counts times 256 are each id's samples; an
         utterance whose ids all got 0 frames is still one frame long.  `seeds`: as for infer_batch_with_values; a
-        seeded frame's noise depends on its index only, so controls that move frames never reshuffle it."""
+        seeded frame's noise depends on its index only, so controls that move frames never reshuffle it.
+        `output_rates`: as for infer_batch_with_values (the frame counts stay frame counts)."""
         n = len(batches)
         cfgs = _config_array(configs, n)
         lens = [len(b) for b in batches]
         scales, frames = _duration_arrays(lens, duration_scales, durations)
         sv, sf = _seed_arrays(seeds, n)
+        rates = _rate_array(output_rates, n)
         if n == 0:
             return []
         if any(x == 0 for x in lens):
@@ -394,26 +439,29 @@ class _VitsCommons:
         outs = (N.sb200_audio * n)()
         id_frames = np.zeros(int(offs[-1]), np.int32)
         err = N.sb200_error()
-        _check(self._lib.sb200_speak_batch_ids_seeded(
+        _check(self._lib.sb200_speak_batch_ids_rates(
             self._h, packed.ctypes.data_as(C.POINTER(C.c_int64)), offs.ctypes.data_as(C.POINTER(C.c_size_t)), n, cfgs,
-            _ptr(scales, C.c_float), _ptr(frames, C.c_int32), _ptr(sv, C.c_uint64), _ptr(sf, C.c_int32), outs,
-            _ptr(id_frames, C.c_int32), C.byref(err)), err)
+            _ptr(scales, C.c_float), _ptr(frames, C.c_int32), _ptr(sv, C.c_uint64), _ptr(sf, C.c_int32),
+            _ptr(rates, C.c_uint32), outs, _ptr(id_frames, C.c_int32), C.byref(err)), err)
         return [(_take_audio(outs[b]), id_frames[int(offs[b]):int(offs[b + 1])].copy()) for b in range(n)]
 
     def speak_batch_with_alignment(self, phoneme_batches: Sequence[str],
                                    configs: Optional[Sequence[PiperSynthesisConfig]] = None,
                                    duration_scales: Optional[Sequence] = None,
-                                   seeds: Optional[Sequence] = None) -> List[Tuple[Audio, List[PhonemeAlignment]]]:
+                                   seeds: Optional[Sequence] = None,
+                                   output_rates: Optional[Sequence] = None) -> List[Tuple[Audio, List[PhonemeAlignment]]]:
         """speak_batch that also says when each phoneme is spoken: per utterance (audio, alignment), the alignment
         holding one entry for bos (`^`), one per kept phoneme character (its id and its trailing pad) and one for eos
         (`$`), contiguous from sample 0 to len(audio).
 
         duration_scales[b] (or None): one scale per character of phoneme_batches[b], applied to that character's id and
         pad; characters the voice drops have no entry and their scales are ignored.  `seeds`: as for
-        infer_batch_with_values."""
+        infer_batch_with_values.  `output_rates`: as for infer_batch_with_values; the alignment is then in samples of
+        the output rate, the boundary after F frames at ceil(F * 256 * up / down)."""
         n = len(phoneme_batches)
         _config_array(configs, n)
         _seed_arrays(seeds, n)
+        _rate_array(output_rates, n)
         per_char = None if duration_scales is None else _per_utterance(duration_scales, n, "duration scales")
         maps = [self.phonemes_to_input_ids_map(p) for p in phoneme_batches]
         id_scales = None
@@ -430,8 +478,12 @@ class _VitsCommons:
                 kept = {c: _scale_value(v[c], b, c, "character") for c in sorted(set(src)) if c >= 0}
                 id_scales.append([1.0 if c < 0 else kept[c] for c in src])
         extra = {} if seeds is None else {"seeds": seeds}
+        if output_rates is not None:
+            extra["output_rates"] = output_rates
         res = self.infer_batch_with_durations([m[0] for m in maps], configs, id_scales, **extra)
-        return [(audio, _alignment(ph, src, frames, len(audio)))
+        voice_rate = self.audio_output_info().sample_rate if output_rates is not None else None
+        ratio = lambda audio: (1, 1) if voice_rate is None else rate_ratio(voice_rate, audio.info.sample_rate)
+        return [(audio, _alignment(ph, src, frames, len(audio), *ratio(audio)))
                 for ph, (_, src), (audio, frames) in zip(phoneme_batches, maps, res)]
 
     def _cfg(self, fn) -> PiperSynthesisConfig:
@@ -511,19 +563,64 @@ class EncoderOutputs:
             pass
 
 
-class SpeechStreamer:
-    """piper/src/lib.rs:765-858: chunked decoder runs with overlap trimming + crossfade(42)."""
+class Resampler:
+    """One stream's output-rate resampler on the device (sb200_resampler_*): it carries the stream's last inputs and
+    counts between chunks, so the concatenation of what it emits is the whole stream resampled at once.  `out_rate`: one
+    of OUTPUT_RATES other than the voice's own."""
 
-    def __init__(self, enc: EncoderOutputs, chunk_size: int, chunk_padding: int):
+    def __init__(self, model: "_VitsCommons", out_rate: int):
+        _rate_array([out_rate], 1)
+        self._m, self.rate, self._h = model, int(out_rate), C.c_void_p()
+        err = N.sb200_error()
+        _check(model._lib.sb200_resampler_create(model._h, int(out_rate), C.byref(self._h), C.byref(err)), err)
+
+    def __del__(self):
+        try:
+            if self._h:
+                self._m._lib.sb200_resampler_free(self._h)
+                self._h = None
+        except Exception:
+            pass
+
+
+def _stream_resampler(model, output_rate) -> Optional[Resampler]:
+    """A Resampler for a stream at output_rate, or None when the stream stays at the voice's rate."""
+    _rate_array([output_rate], 1)
+    if not output_rate or int(output_rate) == model.audio_output_info().sample_rate:
+        return None
+    return Resampler(model, output_rate)
+
+
+def _trim_frames(trim: slice) -> Tuple[int, int]:
+    """The overlap frames a SpeechStreamer audio slice drops at each end."""
+    return (trim.start or 0) // HOP, (-trim.stop // HOP) if trim.stop is not None else 0
+
+
+class SpeechStreamer:
+    """piper/src/lib.rs:765-858: chunked decoder runs with overlap trimming + crossfade(42).  With a resampler, each
+    chunk's trim and crossfade run on the device and the chunk leaves at the resampler's rate."""
+
+    def __init__(self, enc: EncoderOutputs, chunk_size: int, chunk_padding: int,
+                 resampler: Optional[Resampler] = None):
         self.enc = enc
         self.chunker = AdaptiveMelChunker(enc.num_frames, chunk_size, chunk_padding)
         self.one_shot = enc.num_frames <= (chunk_size * 2 + chunk_padding * 2)
+        self.resampler = resampler
 
     def __iter__(self) -> Iterator[AudioSamples]:
         return self
 
     def __next__(self) -> AudioSamples:
         (m0, m1), (a0, a1) = next(self.chunker)
+        if self.resampler is not None:
+            if self.one_shot:
+                self.chunker.consume()
+                chunk, fade = (self.enc, 0, self.enc.num_frames, 0, 0), 0
+            else:
+                hi = self.enc.num_frames if m1 is None else m1
+                chunk, fade = (self.enc, m0, hi) + _trim_frames(slice(a0, a1)), 42
+            return self.enc._m.infer_decoder_batch([chunk], fade=fade, resamplers=[self.resampler],
+                                                   last=[self.chunker.last_end_index is None])[0]
         if self.one_shot:
             self.chunker.consume()
             return self.enc.infer_decoder()
@@ -577,19 +674,25 @@ class VitsStreamingModel(_VitsCommons):
         return [EncoderOutputs(self, C.c_void_p(outs[i])) for i in range(n)]
 
     def infer_decoder_batch(self, chunks: Sequence[tuple], pcm16: bool = False, fade: int = 0,
-                            gains: Optional[Sequence[float]] = None) -> list:
+                            gains: Optional[Sequence[float]] = None, resamplers: Optional[Sequence] = None,
+                            last: Optional[Sequence[bool]] = None) -> list:
         """Many `EncoderOutputs.infer_decoder(lo, hi)` calls as one decoder pass.  `chunks`: (encoder outputs, lo, hi)
         per chunk; each result equals that chunk decoded alone, bit for bit.
 
         With pcm16, a chunk may be (encoder outputs, lo, hi, trim_lo, trim_hi) and each result is what the realtime
         mode emits for it as int16: trim_lo / trim_hi overlap frames dropped, crossfade(fade), gains[k] (None: 1),
-        peak-normalised to the chunk's own peak."""
+        peak-normalised to the chunk's own peak.
+
+        With `resamplers` (one Resampler or None per chunk), chunks may carry trims in either format: after the same
+        post-path each chunk is appended to its stream's resampler and the result is what that stream emits for it at
+        its output rate (AudioSamples, or int16 normalised to the emitted samples' own peak with pcm16); last[k] flushes
+        the stream.  A None resampler returns the chunk after the post-path at the voice's rate."""
         n = len(chunks)
         lo, hi = np.zeros(n, np.int64), np.zeros(n, np.int64)
         tlo, thi = np.zeros(n, np.int64), np.zeros(n, np.int64)
         hs = (C.c_void_p * n)()
         for k, c in enumerate(chunks):
-            if len(c) not in ((3, 5) if pcm16 else (3,)):
+            if len(c) not in ((3, 5) if pcm16 or resamplers is not None else (3,)):
                 raise OperationError(f"Invalid decoder chunk {k}: expected (encoder outputs, lo, hi"
                                      + (", trim_lo, trim_hi)" if pcm16 else ")"))
             enc = c[0]
@@ -605,6 +708,33 @@ class VitsStreamingModel(_VitsCommons):
             return []
         p64 = lambda a: a.ctypes.data_as(C.POINTER(C.c_int64))
         err = N.sb200_error()
+        if resamplers is not None:
+            resamplers = _per_utterance(resamplers, n, "resamplers")
+            rs = (C.c_void_p * n)()
+            for k, r in enumerate(resamplers):
+                if r is not None and (not isinstance(r, Resampler) or not r._h):
+                    raise OperationError(f"chunk {k}: not a Resampler")
+                rs[k] = None if r is None else r._h.value
+            fl = np.zeros(n, np.int32) if last is None else np.array([1 if x else 0 for x in
+                                                                        _per_utterance(last, n, "last flags")], np.int32)
+            g = None if gains is None else np.ascontiguousarray(gains, dtype=np.float32)
+            outs = (C.c_void_p * n)()
+            lens = (C.c_size_t * n)()
+            _check(self._lib.sb200_decode_chunks_resampled(
+                self._h, hs, p64(lo), p64(hi), p64(tlo), p64(thi), n, int(fade),
+                None if g is None else g.ctypes.data_as(C.POINTER(C.c_float)), rs, _ptr(fl, C.c_int32),
+                1 if pcm16 else 0, outs, lens, C.byref(err)), err)
+            res = []
+            for k in range(n):
+                m = int(lens[k])
+                if pcm16:
+                    a = np.ctypeslib.as_array(C.cast(outs[k], C.POINTER(C.c_int16)), (m,)).copy() if m else np.zeros(0, np.int16)
+                else:
+                    a = AudioSamples(np.ctypeslib.as_array(C.cast(outs[k], C.POINTER(C.c_float)), (m,)).copy()
+                                     if m else np.zeros(0, np.float32))
+                self._lib.sb200_i16_free(C.cast(outs[k], C.POINTER(C.c_int16)))
+                res.append(a)
+            return res
         if not pcm16:
             outs = (N.sb200_audio * n)()
             _check(self._lib.sb200_decode_chunks(self._h, hs, p64(lo), p64(hi), n, outs, C.byref(err)), err)
@@ -625,19 +755,21 @@ class VitsStreamingModel(_VitsCommons):
         return True
 
     def stream_synthesis(self, phonemes: str, chunk_size: int, chunk_padding: int,
-                         seed: Optional[int] = None) -> SpeechStreamer:
-        """`seed`: the sentence's noise seed (see infer_batch_with_values), or None for positional noise."""
+                         seed: Optional[int] = None, output_rate: Optional[int] = None) -> SpeechStreamer:
+        """`seed`: the sentence's noise seed (see infer_batch_with_values), or None for positional noise.
+        `output_rate`: the chunks' sample rate (see infer_batch_with_values), the sentence resampled as one stream."""
         _seed_arrays([seed], 1)
+        _rate_array([output_rate], 1)
         ids = self.phonemes_to_input_ids(phonemes)
         enc = self.infer_encoder(ids) if seed is None else self.infer_encoder_batch([ids], seeds=[seed])[0]
-        return SpeechStreamer(enc, chunk_size, chunk_padding)
+        return SpeechStreamer(enc, chunk_size, chunk_padding, _stream_resampler(self, output_rate))
 
 
 class _Stream:
     """One sentence of a StreamBatch: its latent and its own chunk schedule, with SpeechStreamer's one-shot rule."""
 
-    def __init__(self, key, enc, chunk_size: int, chunk_padding: int):
-        self.key, self.enc = key, enc
+    def __init__(self, key, enc, chunk_size: int, chunk_padding: int, resampler: Optional[Resampler] = None):
+        self.key, self.enc, self.resampler = key, enc, resampler
         self.chunker = AdaptiveMelChunker(enc.num_frames, chunk_size, chunk_padding)
         self.one_shot = enc.num_frames <= (chunk_size * 2 + chunk_padding * 2)
 
@@ -670,7 +802,9 @@ class StreamBatch:
     last step in ONE encoder pass, then decodes the next chunk of every active stream in ONE decoder pass, and returns
     [(key, AudioSamples)] in admission order.  Each stream keeps its own AdaptiveMelChunker, trim, one-shot rule and
     crossfade(42), so its chunks are exactly what `stream_synthesis` yields for that sentence with its config as the
-    fallback.
+    fallback.  A stream added with an output rate has its own resampler: its chunks are trimmed, crossfaded and
+    resampled on the device.  Those chunks go through a second decoder pass of the step (a third for one-shot ones,
+    which are not crossfaded), so the streams at the voice's rate keep their pass and their bits.
 
     One stream's failure stays that stream's, as with one `stream_synthesis` per client: when a batched pass raises,
     its streams are run one at a time, and a stream whose own encoder or decoder work fails gets its SonataError as
@@ -680,19 +814,23 @@ class StreamBatch:
         _check_chunking(chunk_size, chunk_padding)
         self.model = model
         self.chunk_size, self.chunk_padding = chunk_size, chunk_padding
-        self._pending: list = []      # (key, ids, config, chunk_size, seed) not yet encoded
+        self._pending: list = []      # (key, ids, config, chunk_size, seed, output rate) not yet encoded
         self._active: List[_Stream] = []
         self._next_key = 0
 
-    def add(self, ids_or_phonemes, config: Optional[PiperSynthesisConfig] = None, seed: Optional[int] = None) -> int:
+    def add(self, ids_or_phonemes, config: Optional[PiperSynthesisConfig] = None, seed: Optional[int] = None,
+            output_rate: Optional[int] = None) -> int:
         """`seed`: the stream's noise seed (see infer_batch_with_values); a seeded stream yields what
-        `stream_synthesis(..., seed=seed)` yields, whatever other streams share its encoder pass."""
-        return self._add(ids_or_phonemes, config, self.chunk_size, seed)
+        `stream_synthesis(..., seed=seed)` yields, whatever other streams share its encoder pass.  `output_rate`: the
+        stream's sample rate, as for stream_synthesis."""
+        return self._add(ids_or_phonemes, config, self.chunk_size, seed, output_rate)
 
-    def _add(self, ids_or_phonemes, config, chunk_size: int, seed: Optional[int] = None) -> int:
+    def _add(self, ids_or_phonemes, config, chunk_size: int, seed: Optional[int] = None,
+             output_rate: Optional[int] = None) -> int:
         if config is not None and not isinstance(config, PiperSynthesisConfig):
             raise OperationError("Invalid configuration for Vits Model")
         _seed_arrays([seed], 1)
+        _rate_array([output_rate], 1)
         if config is not None and config.speaker is not None and config.speaker not in (self.model.get_speakers() or {}):
             raise OperationError(f"No speaker was found with the given id `{config.speaker}`")     # as check_config
         _check_chunking(chunk_size, self.chunk_padding)
@@ -704,7 +842,7 @@ class StreamBatch:
             raise OperationError("Failed to run model inference. Error: empty input sequence")
         key = self._next_key
         self._next_key += 1
-        self._pending.append((key, ids, config, chunk_size, seed))
+        self._pending.append((key, ids, config, chunk_size, seed, output_rate))
         return key
 
     def __len__(self) -> int:
@@ -730,20 +868,37 @@ class StreamBatch:
                     return self.model.infer_encoder_batch([p[1] for p in ps], configs)
                 return self.model.infer_encoder_batch([p[1] for p in ps], configs, seeds=[p[4] for p in ps])
             for p, (enc, err) in zip(pend, _each_or_alone(encode, pend)):
-                if err is not None:
-                    out.append((p[0], err))
-                else:
-                    active.append(_Stream(p[0], enc, p[3], self.chunk_padding))
+                if err is None:
+                    try:
+                        active.append(_Stream(p[0], enc, p[3], self.chunk_padding,
+                                              _stream_resampler(self.model, p[5])))
+                        continue
+                    except SonataError as e:
+                        err = e
+                out.append((p[0], err))
         plan = [(s,) + s.next_chunk() for s in active]
         failed = set()
-        decoded = _each_or_alone(lambda pl: self.model.infer_decoder_batch([(s.enc, lo, hi) for s, lo, hi, _ in pl]),
-                                 plan) if plan else []
-        for (s, _, _, trim), (a, err) in zip(plan, decoded):
+        plain = [p for p in plan if p[0].resampler is None]
+        faded = [p for p in plan if p[0].resampler is not None and p[3] is not None]
+        whole = [p for p in plan if p[0].resampler is not None and p[3] is None]
+
+        def resampled(pl, fade):
+            chunks = [(s.enc, lo, hi) + ((0, 0) if trim is None else _trim_frames(trim)) for s, lo, hi, trim in pl]
+            return self.model.infer_decoder_batch(chunks, fade=fade, resamplers=[p[0].resampler for p in pl],
+                                                  last=[p[0].done for p in pl])
+        decoded = {}
+        for group, call in ((plain, lambda pl: self.model.infer_decoder_batch([(s.enc, lo, hi) for s, lo, hi, _ in pl])),
+                            (faded, lambda pl: resampled(pl, 42)), (whole, lambda pl: resampled(pl, 0))):
+            if group:
+                decoded.update({id(p): r for p, r in zip(group, _each_or_alone(call, group))})
+        for p in plan:
+            s, _, _, trim = p
+            a, err = decoded[id(p)]
             if err is not None:
                 out.append((s.key, err))
                 failed.add(s.key)
                 continue
-            if trim is not None:
+            if trim is not None and s.resampler is None:
                 a = AudioSamples(a.as_slice()[trim])
                 a.crossfade(42)
             out.append((s.key, a))

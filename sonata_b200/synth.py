@@ -90,6 +90,12 @@ def sentence_seed(seed: Optional[int], i: int) -> Optional[int]:
     return None if seed is None else (int(seed) + i) % 2**64
 
 
+def _check_output_rate(rate) -> None:
+    """Raises OperationError unless `rate` is None, 0 or one of piper.OUTPUT_RATES."""
+    from .piper import _rate_array
+    _rate_array([rate], 1)
+
+
 def _sentences(model, text: str) -> List[str]:
     """SpeechSynthesisTaskProvider::get_phonemes (:256-258), or newline-separated phoneme sentences when the model has
     no phonemizer."""
@@ -113,36 +119,48 @@ class SonataSpeechSynthesizer:
         return cfg.apply(audio) if cfg is not None else audio
 
     # `seed` (every mode): the request's noise seed, sentence i seeded with sentence_seed(seed, i); None keeps the
-    # positional noise.
+    # positional noise.  `output_rate` (every mode): the sample rate of the audio handed out, one of
+    # piper.OUTPUT_RATES (None / 0: the voice's), each sentence resampled on the device; appended silence is generated
+    # at that rate.
 
     def synthesize_lazy(self, text: str, output_config: Optional[AudioOutputConfig] = None,
-                        seed: Optional[int] = None) -> Iterator[Audio]:
+                        seed: Optional[int] = None, output_rate: Optional[int] = None) -> Iterator[Audio]:
         sentence_seed(seed, 0)
+        _check_output_rate(output_rate)
         for i, ph in enumerate(self._phonemes(text)):
-            a = (self.model.speak_one_sentence(ph) if seed is None
-                 else self.model.speak_batch([ph], seeds=[sentence_seed(seed, i)])[0])
+            if output_rate:
+                extra = {} if seed is None else {"seeds": [sentence_seed(seed, i)]}
+                a = self.model.speak_batch([ph], output_rates=[output_rate], **extra)[0]
+            else:
+                a = (self.model.speak_one_sentence(ph) if seed is None
+                     else self.model.speak_batch([ph], seeds=[sentence_seed(seed, i)])[0])
             yield self._process(a, output_config)
 
     def synthesize_parallel(self, text: str, output_config: Optional[AudioOutputConfig] = None,
-                            seed: Optional[int] = None) -> Iterator[Audio]:
+                            seed: Optional[int] = None, output_rate: Optional[int] = None) -> Iterator[Audio]:
         sentence_seed(seed, 0)
+        _check_output_rate(output_rate)
         ph = self._phonemes(text)
+        extra = {"output_rates": [output_rate] * len(ph)} if output_rate else {}
         if not ph:
             results = []
         elif seed is None:
-            results = self.model.speak_batch(ph)                  # one batched pass == the rayon fan-out + collect
+            results = self.model.speak_batch(ph, **extra)         # one batched pass == the rayon fan-out + collect
         else:
-            results = self.model.speak_batch(ph, seeds=[sentence_seed(seed, i) for i in range(len(ph))])
+            results = self.model.speak_batch(ph, seeds=[sentence_seed(seed, i) for i in range(len(ph))], **extra)
         return iter([self._process(a, output_config) for a in results])
 
     def synthesize_streamed(self, text: str, output_config: Optional[AudioOutputConfig] = None,
                             chunk_size: int = 72, chunk_padding: int = 3,
-                            seed: Optional[int] = None) -> Iterator[AudioSamples]:
+                            seed: Optional[int] = None, output_rate: Optional[int] = None) -> Iterator[AudioSamples]:
         """RealtimeSpeechStream (:337-382): a background producer pushes chunks into an unbounded channel;
-        chunk_size is multiplied by the number of chunks already produced for every following sentence."""
+        chunk_size is multiplied by the number of chunks already produced for every following sentence.
+        `output_rate`: each sentence is resampled as its own stream (zero history at its start, flushed at its end)."""
         sentence_seed(seed, 0)
-        sr = self.model.audio_output_info().sample_rate
-        extra = lambda i: {} if seed is None else {"seed": sentence_seed(seed, i)}
+        _check_output_rate(output_rate)
+        sr = output_rate or self.model.audio_output_info().sample_rate
+        rate = {"output_rate": output_rate} if output_rate else {}
+        extra = lambda i: dict(rate) if seed is None else dict(rate, seed=sentence_seed(seed, i))
         q: "queue.Queue" = queue.Queue()
         done = object()
 
@@ -172,12 +190,14 @@ class SonataSpeechSynthesizer:
             yield item
 
     def synthesize_to_file(self, filename, text: str, output_config: Optional[AudioOutputConfig] = None,
-                           seed: Optional[int] = None) -> None:
-        """:168-198 — parallel mode, concatenated, peak-normalised i16 WAV."""
-        parts = [a.samples.as_slice() for a in self.synthesize_parallel(text, output_config, seed=seed)]
+                           seed: Optional[int] = None, output_rate: Optional[int] = None) -> None:
+        """:168-198 — parallel mode, concatenated, peak-normalised i16 WAV (at output_rate when given)."""
+        extra = {"output_rate": output_rate} if output_rate else {}
+        parts = [a.samples.as_slice() for a in self.synthesize_parallel(text, output_config, seed=seed, **extra)]
         if not parts or sum(len(p) for p in parts) == 0:
             raise OperationError("No speech data to write")
-        Audio(AudioSamples(np.concatenate(parts)), self.model.audio_output_info().sample_rate).save_to_file(filename)
+        rate = output_rate or self.model.audio_output_info().sample_rate
+        Audio(AudioSamples(np.concatenate(parts)), rate).save_to_file(filename)
 
     # passthroughs of the SonataModel surface (:205-253)
     def speak_one_sentence(self, phonemes: str) -> Audio:
@@ -191,8 +211,9 @@ class SonataSpeechSynthesizer:
 
 
 class _Request:
-    def __init__(self, key, ids, output_config, config, chunk_size, seed=None):
+    def __init__(self, key, ids, output_config, config, chunk_size, seed=None, output_rate=None):
         self.key, self.ids, self.output_config, self.config, self.seed = key, ids, output_config, config, seed
+        self.output_rate = output_rate
         self.cs, self.produced, self.n, self.next = chunk_size, 0, 0, 0
 
 
@@ -217,10 +238,11 @@ class RealtimeBatch:
         self._next_key = 0
 
     def add(self, text: str, output_config: Optional[AudioOutputConfig] = None, config=None,
-            seed: Optional[int] = None) -> int:
-        """`seed`: the request's noise seed, as for synthesize_streamed."""
+            seed: Optional[int] = None, output_rate: Optional[int] = None) -> int:
+        """`seed`: the request's noise seed, `output_rate` its sample rate, as for synthesize_streamed."""
         from .piper import PiperSynthesisConfig
         sentence_seed(seed, 0)
+        _check_output_rate(output_rate)
         if output_config is not None:
             output_config._check_supported()
         if config is not None and not isinstance(config, PiperSynthesisConfig):
@@ -230,7 +252,7 @@ class RealtimeBatch:
         ids = [self.model.phonemes_to_input_ids(ph) for ph in _sentences(self.model, text)]
         if any(len(i) == 0 for i in ids):
             raise OperationError("Failed to run model inference. Error: empty input sequence")
-        req = _Request(self._next_key, ids, output_config, config, self.chunk_size, seed)
+        req = _Request(self._next_key, ids, output_config, config, self.chunk_size, seed, output_rate or None)
         self._next_key += 1
         self._start_sentence(req)
         return req.key
@@ -240,7 +262,9 @@ class RealtimeBatch:
             return
         req.cs = next_chunk_size(req.cs, req.produced)
         req.n = 0
-        self._by_stream[self._streams._add(req.ids[req.next], req.config, req.cs, sentence_seed(req.seed, req.next))] = req
+        rate = {} if req.output_rate is None else {"output_rate": req.output_rate}
+        self._by_stream[self._streams._add(req.ids[req.next], req.config, req.cs, sentence_seed(req.seed, req.next),
+                                           **rate)] = req
         req.next += 1
 
     def __len__(self) -> int:
@@ -263,6 +287,6 @@ class RealtimeBatch:
             del self._by_stream[skey]                  # the sentence is done
             req.produced += req.n
             if oc and oc.appended_silence_ms:
-                out.append((req.key, oc.generate_silence(oc.appended_silence_ms, self._sr)))
+                out.append((req.key, oc.generate_silence(oc.appended_silence_ms, req.output_rate or self._sr)))
             self._start_sentence(req)
         return out
