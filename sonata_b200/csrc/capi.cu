@@ -72,6 +72,20 @@ char* dup_cstr(const std::string& s) {
     return p;
 }
 
+// A copy of `w` in a buffer from malloc, which the caller frees.
+template <typename T> T* malloc_copy(const std::vector<T>& w) {
+    T* p = static_cast<T*>(malloc(w.size() * sizeof(T) + 4));
+    memcpy(p, w.data(), w.size() * sizeof(T));
+    return p;
+}
+// Chunk k's samples w[k] in a buffer of its own from malloc (sb200_i16_free), its length in lens[k].
+template <typename T, typename P> void copy_out(const std::vector<std::vector<T>>& w, P* outs, size_t* lens) {
+    for (size_t k = 0; k < w.size(); k++) {
+        outs[k] = malloc_copy(w[k]);
+        lens[k] = w[k].size();
+    }
+}
+
 template <typename F>
 int32_t guarded(sb200_error* err, F&& f) {
     if (err) { err->code = 0; err->message = nullptr; }
@@ -419,11 +433,13 @@ int32_t sb200_encode_ids(sb200_voice* v, const int64_t* ids, size_t n, sb200_lat
 int64_t sb200_latent_frames(const sb200_latent* z) { return z->l->frames; }
 int32_t sb200_decode_chunk(sb200_voice* v, const sb200_latent* z, int64_t lo, int64_t hi, sb200_audio* out, sb200_error* err) {
     return guarded(err, [&] {
-        std::vector<float> w; float ms = 0;
-        decode_latent_chunk(v->v.get(), z->l, lo, hi, w, &ms);
-        out->data = (float*)malloc(w.size() * 4 + 4);
-        memcpy(out->data, w.data(), w.size() * 4);
-        out->len = w.size(); out->inference_ms = ms; out->sample_rate = (uint32_t)v->v->sample_rate;
+        ChunkPass p;
+        p.chunks = {ChunkSpec{z->l, lo, hi}};
+        p.single = true;
+        ChunkResult r;
+        decode_chunks(v->v.get(), p, r);
+        out->data = malloc_copy(r.f32[0]);
+        out->len = r.f32[0].size(); out->inference_ms = r.ms; out->sample_rate = (uint32_t)v->v->sample_rate;
     });
 }
 void sb200_latent_free(sb200_latent* z) { delete z; }
@@ -457,31 +473,35 @@ int64_t sb200_latent_id_frames(const sb200_latent* z, int32_t* out, size_t capac
 }
 
 namespace {
-std::vector<const Latent*> latents_of(const sb200_latent* const* zs, size_t n) {
-    std::vector<const Latent*> out(n);
+// A pass over chunks zs[k] frames [lo[k], hi[k]), k < n, with trims (null: none) and gains (null: 1).
+ChunkPass chunk_pass(const sb200_latent* const* zs, const int64_t* lo, const int64_t* hi, size_t n,
+                     const int64_t* trim_lo_frames = nullptr, const int64_t* trim_hi_frames = nullptr,
+                     const float* gain = nullptr) {
+    ChunkPass p;
+    p.chunks.resize(n);
     for (size_t k = 0; k < n; k++) {
         if (!zs[k]) throw Error(19, "chunk " + std::to_string(k) + ": null latent");
-        out[k] = zs[k]->l;
+        ChunkSpec& c = p.chunks[k];
+        c.z = zs[k]->l; c.lo = lo[k]; c.hi = hi[k];
+        if (trim_lo_frames) c.trim_lo = trim_lo_frames[k];
+        if (trim_hi_frames) c.trim_hi = trim_hi_frames[k];
+        if (gain) c.gain = gain[k];
     }
-    return out;
+    return p;
 }
 }  // namespace
 
 int32_t sb200_decode_chunks(sb200_voice* v, const sb200_latent* const* zs, const int64_t* lo, const int64_t* hi, size_t n,
                             sb200_audio* outs, sb200_error* err) {
     return guarded(err, [&] {
-        static_assert(sizeof(long long) == sizeof(int64_t), "");
-        const std::vector<const Latent*> ls = latents_of(zs, n);
-        std::vector<std::vector<float>> w; float ms = 0;
-        decode_latent_chunks(v->v.get(), ls.data(), reinterpret_cast<const long long*>(lo),
-                             reinterpret_cast<const long long*>(hi), n, w, &ms);
+        ChunkResult r;
+        decode_chunks(v->v.get(), chunk_pass(zs, lo, hi, n), r);
         size_t total = 0;
-        for (auto& x : w) total += x.size();
+        for (auto& w : r.f32) total += w.size();
         for (size_t k = 0; k < n; k++) {
-            outs[k].data = (float*)malloc(w[k].size() * 4 + 4);
-            memcpy(outs[k].data, w[k].data(), w[k].size() * 4);
-            outs[k].len = w[k].size(); outs[k].sample_rate = (uint32_t)v->v->sample_rate;
-            outs[k].inference_ms = ms * (total ? (float)w[k].size() / (float)total : 0.f);
+            outs[k].data = malloc_copy(r.f32[k]);
+            outs[k].len = r.f32[k].size(); outs[k].sample_rate = (uint32_t)v->v->sample_rate;
+            outs[k].inference_ms = r.ms * (total ? (float)r.f32[k].size() / (float)total : 0.f);
         }
     });
 }
@@ -490,16 +510,11 @@ int32_t sb200_decode_chunks_i16(sb200_voice* v, const sb200_latent* const* zs, c
                                 const int64_t* trim_lo_frames, const int64_t* trim_hi_frames, size_t n, int32_t fade,
                                 const float* gain, int16_t** outs, size_t* lens, sb200_error* err) {
     return guarded(err, [&] {
-        const std::vector<const Latent*> ls = latents_of(zs, n);
-        std::vector<std::vector<int16_t>> w;
-        decode_latent_chunks_pcm(v->v.get(), ls.data(), reinterpret_cast<const long long*>(lo),
-                                 reinterpret_cast<const long long*>(hi), reinterpret_cast<const long long*>(trim_lo_frames),
-                                 reinterpret_cast<const long long*>(trim_hi_frames), n, fade, gain, w, nullptr);
-        for (size_t k = 0; k < n; k++) {
-            outs[k] = (int16_t*)malloc(w[k].size() * 2 + 2);
-            memcpy(outs[k], w[k].data(), w[k].size() * 2);
-            lens[k] = w[k].size();
-        }
+        ChunkPass p = chunk_pass(zs, lo, hi, n, trim_lo_frames, trim_hi_frames, gain);
+        p.fade = fade; p.format = 1;
+        ChunkResult r;
+        decode_chunks(v->v.get(), p, r);
+        copy_out(r.i16, outs, lens);
     });
 }
 
@@ -516,23 +531,16 @@ int32_t sb200_decode_chunks_resampled(sb200_voice* v, const sb200_latent* const*
                                       int32_t fade, const float* gain, sb200_resampler* const* resamplers,
                                       const int32_t* last, int32_t format, void** outs, size_t* lens, sb200_error* err) {
     return guarded(err, [&] {
-        const std::vector<const Latent*> ls = latents_of(zs, n);
+        ChunkPass p = chunk_pass(zs, lo, hi, n, trim_lo_frames, trim_hi_frames, gain);
         if (n > 0 && (!resamplers || !outs || !lens)) throw Error(19, "null argument");
-        std::vector<Resampler*> rs(n);
-        for (size_t k = 0; k < n; k++) rs[k] = resamplers[k] ? resamplers[k]->r : nullptr;
-        std::vector<std::vector<float>> f;
-        std::vector<std::vector<int16_t>> s;
-        decode_latent_chunks_resampled(v->v.get(), ls.data(), reinterpret_cast<const long long*>(lo),
-                                       reinterpret_cast<const long long*>(hi),
-                                       reinterpret_cast<const long long*>(trim_lo_frames),
-                                       reinterpret_cast<const long long*>(trim_hi_frames), n, fade, gain, rs.data(), last,
-                                       format, f, s);
         for (size_t k = 0; k < n; k++) {
-            const size_t m = format == 1 ? s[k].size() : f[k].size(), es = format == 1 ? 2 : 4;
-            outs[k] = malloc(m * es + 4);
-            memcpy(outs[k], format == 1 ? (const void*)s[k].data() : (const void*)f[k].data(), m * es);
-            lens[k] = m;
+            p.chunks[k].rs = resamplers[k] ? resamplers[k]->r : nullptr;
+            if (last) p.chunks[k].last = last[k];
         }
+        p.fade = fade; p.resample = true; p.format = format;
+        ChunkResult r;
+        decode_chunks(v->v.get(), p, r);
+        if (format == 1) copy_out(r.i16, outs, lens); else copy_out(r.f32, outs, lens);
     });
 }
 

@@ -399,6 +399,61 @@ struct FrameTables {
     }
 };
 
+// One resample launch over segments laid out back to back: each segment's ResampleSeg, what the launch is sized by and
+// what the profile counts.
+struct ResamplePlan {
+    std::vector<ResampleSeg> segs;
+    long long total = 0, max_out = 0; int smem = 0;
+    double flops = 0, bytes = 0;
+    // Appends a segment of n_in inputs through `f` (null: copied unchanged).  A whole signal emits every output; with a
+    // stream's resampler `r` (whose filter is f) the segment continues r's stream, emits every output whose inputs have
+    // all arrived, and flushes the stream when `last`.
+    void add(const ResampleFilter* f, long long n_in, const Resampler* r = nullptr, bool last = false) {
+        ResampleSeg s{};
+        s.out_off = total; s.n_out = n_in; s.down = 1;
+        if (f) {
+            const long long N = (r ? r->consumed : 0) + n_in;
+            s.taps = f->taps; s.up = f->up; s.down = f->down; s.H = f->H; s.K = f->K;
+            s.n_out = resample_emit_end(*f, N, !r || last) - (r ? r->emitted : 0);
+            if (r) {
+                s.hist = r->hist[r->cur]; s.hist_out = r->hist[1 - r->cur];
+                s.c = r->consumed; s.j0 = r->emitted; s.h = r->h; s.h_out = (int)std::min<long long>(N, f->K - 1);
+            }
+        }
+        bytes += 4.0 * ((double)n_in + s.n_out);
+        if (f) {
+            smem = std::max(smem, resample_span(f->up, f->down, f->K));
+            flops += 2.0 * (double)s.n_out * (2.0 * f->H + 1.0) / f->up;
+            bytes += 4.0 * (double)f->up * f->K;
+        }
+        max_out = std::max(max_out, s.n_out);
+        total += s.n_out;
+        segs.push_back(s);
+    }
+};
+
+// Device tables of a resample launch and their pinned mirrors: the segments, identity posts (for a launch whose input
+// has no post-path, or for the i16 conversion of its output) and the output segments, n_out samples at out_off.
+struct ResampleTables {
+    ResampleSeg *segs, *segs_h; PcmPost *posts, *posts_h; FrameSeg *osegs, *osegs_h;
+    void carve(Arena& dev, Arena& pin, size_t n) {
+        segs = dev.get<ResampleSeg>(n); segs_h = pin.get<ResampleSeg>(n);
+        posts = dev.get<PcmPost>(n); posts_h = pin.get<PcmPost>(n);
+        osegs = dev.get<FrameSeg>(n); osegs_h = pin.get<FrameSeg>(n);
+    }
+    void upload(const ResamplePlan& p, cudaStream_t st) {
+        const size_t n = p.segs.size();
+        for (size_t k = 0; k < n; k++) {
+            segs_h[k] = p.segs[k];
+            posts_h[k] = PcmPost();
+            osegs_h[k] = FrameSeg{0, (int)p.segs[k].n_out, 0, 0, p.segs[k].out_off};
+        }
+        h2d(segs, segs_h, n * sizeof(ResampleSeg), st);
+        h2d(posts, posts_h, n * sizeof(PcmPost), st);
+        h2d(osegs, osegs_h, n * sizeof(FrameSeg), st);
+    }
+};
+
 // Decoder over RY frames: conv_pre's output, then ping-pong stage buffers sized for the widest stage, or with debug one
 // set per stage so every stage can be fetched.
 struct DecoderBufs {
@@ -438,23 +493,18 @@ struct DecoderBufs {
 // Frame level of a synthesis pass (phase 2): tables, the latent, the flow's scratch, and unless the pass stops after
 // the flow the decoder and (when the caller passed no buffer) the waveforms.  With output rates the decoder's
 // waveforms are always the pass's own, and the resampled ones go to the caller's buffer or to `rs`, with the tables of
-// the resampling launch.
+// the resampling launch `rp`.
 struct FrameBufs {
     FrameTables y;
     float *s, *epsz, *zp, *h, *acts, *outb, *wav;
     std::vector<float*> flow;                  // debug: z after each coupling layer, in the engine's channel order
     DecoderBufs dec;
-    float* rs;
-    ResampleSeg *rsegs, *rsegs_h; PcmPost *posts, *posts_h; FrameSeg *osegs, *osegs_h;
-    void carve(Arena& dev, Arena& pin, const Job& j, bool own_wav) {
-        rs = nullptr; rsegs = rsegs_h = nullptr; posts = posts_h = nullptr; osegs = osegs_h = nullptr;
-        const bool resample = !j.out_rates.empty() && !j.encode_only;
-        if (resample) {
-            const size_t B = j.B;
-            rsegs = dev.get<ResampleSeg>(B); rsegs_h = pin.get<ResampleSeg>(B);
-            posts = dev.get<PcmPost>(B); posts_h = pin.get<PcmPost>(B);
-            osegs = dev.get<FrameSeg>(B); osegs_h = pin.get<FrameSeg>(B);
-            if (own_wav) rs = dev.get<float>((size_t)j.out_total + 4);
+    ResampleTables rt; float* rs;
+    void carve(Arena& dev, Arena& pin, const Job& j, const ResamplePlan& rp, bool own_wav) {
+        rt.carve(dev, pin, rp.segs.size());
+        rs = nullptr;
+        if (!rp.segs.empty()) {
+            if (own_wav) rs = dev.get<float>((size_t)rp.total + 4);
             own_wav = true;
         }
         const Arch& a = j.v->a;
@@ -476,8 +526,8 @@ struct FrameBufs {
 };
 
 // One pass of streaming decoder chunks: speaker biases of every slot, tables, the gather table and the latent slices,
-// the decoder, the waveforms, the PCM scratch when the chunks leave as i16, and the pinned block the packed result is
-// copied to.
+// the decoder and the waveforms; the post-path table when an output stage runs, the resample launch's tables and
+// output, the i16 scratch; and the pinned block the packed result (`total` values) is copied to.
 struct ChunkBufs {
     float* cond;
     int *sid, *sid_h;
@@ -486,19 +536,12 @@ struct ChunkBufs {
     float *s, *wav;
     DecoderBufs dec;
     PcmPost *post, *post_h;
+    ResampleTables rt; float* rs;
     short* i16; unsigned* max;
-    float* out_h;
-    // streams resampled after the post-path: tables, the resampled chunks and, leaving as i16, their conversion
-    ResampleSeg *rsegs, *rsegs_h; FrameSeg *osegs, *osegs_h; PcmPost *ipost, *ipost_h; float* rs;
-    void carve(Arena& dev, Arena& pin, const Job& j, bool pcm, long long rs_total = -1, bool rs_i16 = false) {
-        const bool resample = rs_total >= 0;
-        const size_t nr = resample ? j.fsegs.size() : 0;
-        rsegs = dev.get<ResampleSeg>(nr); rsegs_h = pin.get<ResampleSeg>(nr);
-        osegs = dev.get<FrameSeg>(nr); osegs_h = pin.get<FrameSeg>(nr);
-        ipost = dev.get<PcmPost>(nr); ipost_h = pin.get<PcmPost>(nr);
-        rs = resample ? dev.get<float>((size_t)rs_total + 4) : nullptr;
+    void* out_h;
+    void carve(Arena& dev, Arena& pin, const Job& j, const ChunkPass& p, const ResamplePlan& rp, size_t total) {
         const Voice& v = *j.v;
-        const bool multi = v.num_speakers > 1;
+        const bool multi = v.num_speakers > 1, i16_out = p.format == 1;
         const size_t n = j.fsegs.size(), nslots = j.slot_sid.size();
         cond = multi ? dev.get<float>(nslots * v.cond_rows) : nullptr;
         sid = multi ? dev.get<int>(nslots) : nullptr;
@@ -508,12 +551,13 @@ struct ChunkBufs {
         s = dev.get<float>((size_t)j.RY * v.a.inter);
         wav = dev.get<float>((size_t)j.total_samples + 4);
         dec.carve(dev, v, j.RY, false);
-        post = pcm ? dev.get<PcmPost>(n) : nullptr;
-        post_h = pcm ? pin.get<PcmPost>(n) : nullptr;
-        const size_t n_i16 = resample ? (rs_i16 ? (size_t)rs_total : 0) : (size_t)j.total_samples;
-        i16 = pcm ? dev.get<short>(n_i16 + 8) : nullptr;
-        max = pcm ? dev.get<unsigned>(n) : nullptr;
-        out_h = pin.get<float>(std::max<size_t>((size_t)j.total_samples, resample ? (size_t)rs_total : 0));
+        post = p.resample || i16_out ? dev.get<PcmPost>(n) : nullptr;
+        post_h = p.resample || i16_out ? pin.get<PcmPost>(n) : nullptr;
+        rt.carve(dev, pin, rp.segs.size());
+        rs = p.resample ? dev.get<float>(total + 4) : nullptr;
+        i16 = i16_out ? dev.get<short>(total + 8) : nullptr;
+        max = i16_out ? dev.get<unsigned>(n) : nullptr;
+        out_h = pin.alloc(total * (i16_out ? 2 : 4));
     }
 };
 
@@ -594,32 +638,37 @@ void lay_out_frames(Job& j, const std::vector<int>& y_len, int hop) {
     j.RY = cur; j.total_samples = out;
 }
 
-// What the job hands out (osegs, out_hop, out_total): the frame layout itself without output rates, else one segment of
-// ceil(n * up / down) samples per utterance, back to back.  Returns each utterance's filter (null: not resampled).
-std::vector<const ResampleFilter*> lay_out_output(Job& j, int hop) {
-    std::vector<const ResampleFilter*> filt;
+// What the job hands out (osegs, out_hop, out_total): the frame layout itself without output rates (an empty plan), else
+// the segments of the returned plan, one utterance each at its rate, back to back.
+ResamplePlan lay_out_output(Job& j, int hop) {
+    ResamplePlan p;
     j.osr.assign(j.B, j.v->sample_rate);
     if (j.out_rates.empty() || j.encode_only) {
         j.osegs = j.fsegs; j.out_hop = hop; j.out_total = j.total_samples;
-        return filt;
+        return p;
     }
-    for (size_t b = 0; b < j.B; b++)
-        if (j.out_rates[b]) j.osr[b] = j.out_rates[b];
-    filt.assign(j.B, nullptr);
     j.osegs.assign(j.B, FrameSeg{});
-    long long off = 0;
     for (size_t b = 0; b < j.B; b++) {
-        const long long n = (long long)j.fsegs[b].len * hop;
-        long long n_out = n;
+        const ResampleFilter* f = nullptr;
         if (j.out_rates[b]) {
-            filt[b] = &voice_resampler(*j.v, j.out_rates[b], "utterance " + std::to_string(b) + ": ");
-            n_out = (n * filt[b]->up + filt[b]->down - 1) / filt[b]->down;
+            j.osr[b] = j.out_rates[b];
+            f = &voice_resampler(*j.v, j.out_rates[b], "utterance " + std::to_string(b) + ": ");
         }
-        j.osegs[b] = FrameSeg{0, (int)n_out, 0, 0, off};
-        off += n_out;
+        p.add(f, (long long)j.fsegs[b].len * hop);
+        j.osegs[b] = FrameSeg{0, (int)p.segs[b].n_out, 0, 0, p.segs[b].out_off};
     }
-    j.out_hop = 1; j.out_total = off;
-    return filt;
+    j.out_hop = 1; j.out_total = p.total;
+    return p;
+}
+
+// The resample launch of plan `p` (tables `t`) over the segments of wav, read through `posts`, into out: profile region
+// "resample".
+void run_resample(Runner& R, const ResamplePlan& p, const ResampleTables& t, const float* wav, const FrameSeg* fsegs,
+                  const PcmPost* posts, int hop, float* out) {
+    R.begin("resample");
+    launch_resample(wav, fsegs, posts, hop, t.segs, (int)p.segs.size(), p.max_out, p.smem, out, R.st);
+    R.count(p.flops, p.bytes);
+    R.end();
 }
 
 // Fills the frame-level tables through their pinned mirrors; returns the level.
@@ -883,11 +932,12 @@ void Job::run(float* d_out, size_t d_out_cap) {
     // ---------------- frame level (phase 2) workspace ----------------
     // The stream is idle here, so the pinned staging of the X tables can be reused for the Y tables.
     lay_out_frames(*this, y_len, a.hop());
-    const std::vector<const ResampleFilter*> filt = lay_out_output(*this, a.hop());
+    const ResamplePlan rp = lay_out_output(*this, a.hop());
+    const bool resample = !rp.segs.empty();
     FrameBufs f;
-    plan(C.dev_frame, C.pin, [&](Arena& dev, Arena& pin) { f.carve(dev, pin, *this, d_out == nullptr); });
+    plan(C.dev_frame, C.pin, [&](Arena& dev, Arena& pin) { f.carve(dev, pin, *this, rp, d_out == nullptr); });
     d_fsegs = f.y.fsegs;
-    d_osegs = f.osegs ? f.osegs : d_fsegs;
+    d_osegs = resample ? f.rt.osegs : d_fsegs;
     if (debug) {
         expose(*this, "z_p", f.zp, I, 1); expose(*this, "z", f.s, I, 1);
         // flow.{f}: z after the coupling layer of the graph's flow.flows.{2f} (f = flow_n - 1 first).  The graph's Flip
@@ -897,30 +947,7 @@ void Job::run(float* d_out, size_t d_out_cap) {
         if (!encode_only) f.dec.expose_to(*this);
     }
     Level LY = upload_frames(*this, f.y, st);
-    long long rs_max_out = 0;
-    int rs_smem = 0;
-    double rs_flops = 0, rs_bytes = 0;
-    if (f.rsegs) {
-        for (size_t b = 0; b < B; b++) {
-            const FrameSeg& o = osegs[b];
-            const ResampleFilter* r = filt[b];
-            f.rsegs_h[b] = r ? ResampleSeg{r->taps, o.out_off, o.len, r->up, r->down, r->H, r->K}
-                             : ResampleSeg{nullptr, o.out_off, o.len, 0, 1, 0, 0};
-            f.posts_h[b] = PcmPost();
-            rs_max_out = std::max<long long>(rs_max_out, o.len);
-            const double n_in = (double)fsegs[b].len * a.hop();
-            rs_bytes += 4.0 * (n_in + o.len);
-            if (r) {
-                rs_smem = std::max(rs_smem, resample_span(r->up, r->down, r->K));
-                rs_flops += 2.0 * (double)o.len * (2.0 * r->H + 1.0) / r->up;
-                rs_bytes += 4.0 * (double)r->up * r->K;
-            }
-        }
-        memcpy(f.osegs_h, osegs.data(), B * sizeof(FrameSeg));
-        h2d(f.rsegs, f.rsegs_h, B * sizeof(ResampleSeg), st);
-        h2d(f.posts, f.posts_h, B * sizeof(PcmPost), st);
-        h2d(f.osegs, f.osegs_h, B * sizeof(FrameSeg), st);
-    }
+    if (resample) f.rt.upload(rp, st);
 
     // ---------------- alignment expansion ----------------
     R.begin("align");
@@ -977,13 +1004,8 @@ void Job::run(float* d_out, size_t d_out_cap) {
     } else {
         d_wav = f.rs ? f.rs : f.wav;
     }
-    run_decoder(R, LY, f.y, f.dec, f.s, f.rsegs ? f.wav : d_wav);
-    if (f.rsegs) {
-        R.begin("resample");
-        launch_resample(f.wav, f.y.fsegs, f.posts, a.hop(), f.rsegs, (int)B, rs_max_out, rs_smem, d_wav, st);
-        R.count(rs_flops, rs_bytes);
-        R.end();
-    }
+    run_decoder(R, LY, f.y, f.dec, f.s, resample ? f.wav : d_wav);
+    if (resample) run_resample(R, rp, f.rt, f.wav, f.y.fsegs, f.rt.posts, a.hop(), d_wav);
     SB_CUDA(cudaEventRecord(C.ev_end, st));
     SB_CUDA(cudaStreamSynchronize(st));
     SB_CUDA(cudaGetLastError());
@@ -1044,92 +1066,63 @@ static void fill_fade(PcmPost& p, int fade, long long len) {
     for (int i = 0; i < p.fade_n; i++) p.tab[i] = sinf(((float)i / att) * 3.14159265358979f / 2.0f);
 }
 
-namespace {
-// The PCM post-path of one chunk pass: per-chunk trims, crossfade table and gain.
-struct ChunkPcm { const long long *trim_lo, *trim_hi; int fade; const float* gain; };
-// Streams resampled after the post-path: one resampler per chunk (null: none), the flush flags and the output format;
-// segs / ends are filled by the pass, and applied to the resamplers once it has succeeded.
-struct ChunkResample {
-    Resampler* const* rs; const int* last; int format;
-    std::vector<ResampleSeg> segs; std::vector<long long> ends; long long total = 0, max_out = 0; int smem = 0;
-};
-
-// One decoder pass over chunks z[k][lo[k] : hi[k]), k < n, laid out as the segments of one frame level: the result is
-// left on the device (job-owned arena), and with `pcm` converted to i16.  Every check runs before any device work.
-// Errors name the chunk and its frame range, except through the single-chunk entry points (`single`), which keep
-// the messages they always gave.
-ChunkBufs decode_chunks_device(Voice* v, const Latent* const* z, const long long* lo, const long long* hi, size_t n,
-                               Job& j, const ChunkPcm* pcm, bool single, ChunkResample* rsp = nullptr) {
-    const Arch& a = v->a;
-    const int hop = a.hop();
+// The chunks are laid out as the segments of one frame level.  The pass runs the decoder, then its output stage: the
+// resample launch, which reads the waveforms through the post-path, and the i16 conversion, which applies the post-path
+// itself when no resample launch ran.  The packed result comes back in one copy through the context's page-locked
+// staging, and only then do the resamplers advance.
+void decode_chunks(Voice* v, const ChunkPass& p, ChunkResult& out) {
+    out.f32.clear(); out.i16.clear(); out.ms = 0.f;
+    const size_t n = p.chunks.size();
+    if (n == 0) return;
+    if (p.format != 0 && p.format != 1) throw Error(19, "format " + std::to_string(p.format) + " is neither 0 (f32) nor 1 (i16)");
+    const int hop = v->a.hop();
+    Job j;
     std::vector<int> len(n);
-    j.slot_of.assign(n, 0); j.slot_sid.clear();
-    auto fail = [single](size_t k, const std::string& what, const std::string& detail) {
-        throw Error(19, single ? what : "chunk " + std::to_string(k) + ": " + what + detail);
+    j.slot_of.assign(n, 0);
+    auto fail = [&p](size_t k, const std::string& what, const std::string& detail) {
+        throw Error(19, p.single ? what : "chunk " + std::to_string(k) + ": " + what + detail);
     };
     for (size_t k = 0; k < n; k++) {
-        if (!z[k] || z[k]->v != v) fail(k, "the latent was not encoded by this voice", "");
-        if (lo[k] < 0 || lo[k] >= hi[k] || hi[k] > z[k]->frames)
-            fail(k, "Invalid model audio output", " (frames [" + std::to_string(lo[k]) + ", " + std::to_string(hi[k]) +
-                                                  ") of a latent of " + std::to_string(z[k]->frames) + ")");
-        if (pcm) {
-            const long long tl = pcm->trim_lo ? pcm->trim_lo[k] : 0, th = pcm->trim_hi ? pcm->trim_hi[k] : 0;
-            if (tl < 0 || th < 0 || tl + th >= hi[k] - lo[k]) fail(k, "Invalid model audio output", " (trim)");
-        }
+        const ChunkSpec& c = p.chunks[k];
+        if (!c.z || c.z->v != v) fail(k, "the latent was not encoded by this voice", "");
+        if (c.lo < 0 || c.lo >= c.hi || c.hi > c.z->frames)
+            fail(k, "Invalid model audio output", " (frames [" + std::to_string(c.lo) + ", " + std::to_string(c.hi) +
+                                                  ") of a latent of " + std::to_string(c.z->frames) + ")");
+        if (c.trim_lo < 0 || c.trim_hi < 0 || c.trim_lo + c.trim_hi >= c.hi - c.lo)
+            fail(k, "Invalid model audio output", " (trim)");
         // decoder.onnx takes the encoder's `g` (piper/src/lib.rs:706-735, 739-743): one speaker slot per distinct sid
         if (v->num_speakers > 1) {
-            const long long sid = z[k]->sid;
+            const long long sid = c.z->sid;
             if (sid < 0 || sid >= v->emb_rows) fail(k, "Failed to run model inference. Error: speaker id out of range", "");
             const auto it = std::find(j.slot_sid.begin(), j.slot_sid.end(), (int)sid);
             j.slot_of[k] = (int)(it - j.slot_sid.begin());
             if (it == j.slot_sid.end()) j.slot_sid.push_back((int)sid);
         }
-        len[k] = (int)(hi[k] - lo[k]);
-        if (rsp && rsp->rs[k]) {
-            const Resampler* r = rsp->rs[k];
+        len[k] = (int)(c.hi - c.lo);
+        if (const Resampler* r = c.rs) {
             if (r->v != v) fail(k, "the resampler was made for another voice", "");
             if (r->ended) fail(k, "the resampler's stream has already been flushed", "");
             for (size_t q = 0; q < k; q++)
-                if (rsp->rs[q] == r) fail(k, "the resampler of chunk " + std::to_string(q) + " appears twice in one call", "");
-            if (rsp->last && rsp->last[k] != 0 && rsp->last[k] != 1)
-                fail(k, "last flag " + std::to_string(rsp->last[k]) + " is neither 0 nor 1", "");
+                if (p.chunks[q].rs == r) fail(k, "the resampler of chunk " + std::to_string(q) + " appears twice in one call", "");
+            if (c.last != 0 && c.last != 1) fail(k, "last flag " + std::to_string(c.last) + " is neither 0 nor 1", "");
         }
     }
-    if (rsp) {
-        rsp->segs.assign(n, ResampleSeg{});
-        rsp->ends.assign(n, 0);
-        long long off = 0;
-        for (size_t k = 0; k < n; k++) {
-            const long long m = (long long)len[k] * hop - (pcm->trim_lo ? pcm->trim_lo[k] : 0) * hop -
-                                (pcm->trim_hi ? pcm->trim_hi[k] : 0) * hop;
-            ResampleSeg& s = rsp->segs[k];
-            s.out_off = off;
-            const Resampler* r = rsp->rs[k];
-            if (!r) {
-                s.n_out = m;
-            } else {
-                const ResampleFilter& f = r->f;
-                const long long N = r->consumed + m;
-                rsp->ends[k] = resample_emit_end(f, N, rsp->last && rsp->last[k]);
-                s.taps = f.taps; s.up = f.up; s.down = f.down; s.H = f.H; s.K = f.K;
-                s.n_out = rsp->ends[k] - r->emitted;
-                s.hist = r->hist[r->cur]; s.hist_out = r->hist[1 - r->cur];
-                s.c = r->consumed; s.j0 = r->emitted; s.h = r->h; s.h_out = (int)std::min<long long>(N, f.K - 1);
-                rsp->smem = std::max(rsp->smem, resample_span(f.up, f.down, f.K));
-            }
-            rsp->max_out = std::max(rsp->max_out, s.n_out);
-            off += s.n_out;
-        }
-        rsp->total = off;
+    // samples of each chunk after its trims, and the resample launch
+    std::vector<long long> n_in(n);
+    ResamplePlan rp;
+    for (size_t k = 0; k < n; k++) {
+        const ChunkSpec& c = p.chunks[k];
+        n_in[k] = (c.hi - c.lo - c.trim_lo - c.trim_hi) * hop;
+        if (p.resample) rp.add(c.rs ? &c.rs->f : nullptr, n_in[k], c.rs, c.last != 0);
     }
+
     j.v = v; j.B = n; j.ctx = v->acquire();
     Context& C = *j.ctx;
     SB_CUDA(cudaSetDevice(v->device));
     lay_out_frames(j, len, hop);
+    const size_t total = p.resample ? (size_t)rp.total : (size_t)j.total_samples;
     ChunkBufs b;
-    plan(C.dev_frame, C.pin, [&](Arena& dev, Arena& pin) {
-        b.carve(dev, pin, j, pcm != nullptr, rsp ? rsp->total : -1, rsp && rsp->format == 1);
-    });
+    plan(C.dev_frame, C.pin, [&](Arena& dev, Arena& pin) { b.carve(dev, pin, j, p, rp, total); });
     j.d_cond = b.cond; j.d_fsegs = b.y.fsegs; j.d_wav = b.wav;
     C.events_used = 0;
     if (!C.ev_begin) { SB_CUDA(cudaEventCreate(&C.ev_begin)); SB_CUDA(cudaEventCreate(&C.ev_end)); }
@@ -1142,155 +1135,58 @@ ChunkBufs decode_chunks_device(Voice* v, const Latent* const* z, const long long
         launch_cond_bias(v->cond_w, v->cond_base, v->emb_g, b.sid, (int)j.slot_sid.size(), v->cond_rows, v->gin, b.cond, st);
     }
     Level LY = upload_frames(j, b.y, st);
-    for (size_t k = 0; k < n; k++) b.src_h[k] = GatherSeg{z[k]->z, lo[k], j.fsegs[k].off, len[k]};
+    for (size_t k = 0; k < n; k++) b.src_h[k] = GatherSeg{p.chunks[k].z->z, p.chunks[k].lo, j.fsegs[k].off, len[k]};
     h2d(b.src, b.src_h, n * sizeof(GatherSeg), st);
-    launch_gather_rows(b.src, b.y.ftile, GY, j.RY, a.inter, b.s, st);
+    launch_gather_rows(b.src, b.y.ftile, GY, j.RY, v->a.inter, b.s, st);
     run_decoder(R, LY, b.y, b.dec, b.s, b.wav);
-    if (pcm) {
-        long long longest = 0;
+    if (b.post) {
         for (size_t k = 0; k < n; k++) {
-            PcmPost& p = b.post_h[k];
-            p = PcmPost();
-            p.gain = pcm->gain ? pcm->gain[k] : 1.f;
-            p.trim_lo = (pcm->trim_lo ? pcm->trim_lo[k] : 0) * hop;
-            p.trim_hi = (pcm->trim_hi ? pcm->trim_hi[k] : 0) * hop;
-            if (pcm->fade > 0) fill_fade(p, pcm->fade, (long long)len[k] * hop - p.trim_lo - p.trim_hi);
-            longest = std::max(longest, (long long)len[k] * hop);
+            PcmPost& q = b.post_h[k];
+            q = PcmPost();
+            q.gain = p.chunks[k].gain;
+            q.trim_lo = p.chunks[k].trim_lo * hop;
+            q.trim_hi = p.chunks[k].trim_hi * hop;
+            if (p.fade > 0) fill_fade(q, p.fade, n_in[k]);
         }
         h2d(b.post, b.post_h, n * sizeof(PcmPost), st);
-        if (!rsp) {
-            launch_i16(b.wav, b.y.fsegs, b.post, (int)n, hop, longest, b.max, b.i16, st);
-        } else {
-            for (size_t k = 0; k < n; k++) {
-                b.rsegs_h[k] = rsp->segs[k];
-                b.osegs_h[k] = FrameSeg{0, (int)rsp->segs[k].n_out, 0, 0, rsp->segs[k].out_off};
-                b.ipost_h[k] = PcmPost();
-            }
-            h2d(b.rsegs, b.rsegs_h, n * sizeof(ResampleSeg), st);
-            h2d(b.osegs, b.osegs_h, n * sizeof(FrameSeg), st);
-            h2d(b.ipost, b.ipost_h, n * sizeof(PcmPost), st);
-            R.begin("resample");
-            launch_resample(b.wav, b.y.fsegs, b.post, hop, b.rsegs, (int)n, rsp->max_out, rsp->smem, b.rs, st);
-            R.end();
-            if (rsp->format == 1) launch_i16(b.rs, b.osegs, b.ipost, (int)n, 1, rsp->max_out, b.max, b.i16, st);
-        }
+    }
+    if (p.resample) {
+        b.rt.upload(rp, st);
+        run_resample(R, rp, b.rt, b.wav, b.y.fsegs, b.post, hop, b.rs);
+        if (b.i16) launch_i16(b.rs, b.rt.osegs, b.rt.posts, (int)n, 1, rp.max_out, b.max, b.i16, st);
+    } else if (b.i16) {
+        launch_i16(b.wav, b.y.fsegs, b.post, (int)n, hop, (long long)*std::max_element(len.begin(), len.end()) * hop,
+                   b.max, b.i16, st);
     }
     SB_CUDA(cudaEventRecord(C.ev_end, st));
-    return b;
-}
-
-void chunks_resampled(Voice* v, const Latent* const* z, const long long* lo, const long long* hi, const ChunkPcm& pcm,
-                      ChunkResample& rsp, size_t n, std::vector<std::vector<float>>& out_f32,
-                      std::vector<std::vector<int16_t>>& out_i16) {
-    out_f32.clear(); out_i16.clear();
-    if (n == 0) return;
-    if (rsp.format != 0 && rsp.format != 1) throw Error(19, "format " + std::to_string(rsp.format) + " is neither 0 (f32) nor 1 (i16)");
-    Job j;
-    const ChunkBufs b = decode_chunks_device(v, z, lo, hi, n, j, &pcm, false, &rsp);
-    cudaStream_t st = j.ctx->stream;
-    const size_t es = rsp.format == 1 ? 2 : 4;
-    SB_CUDA(cudaMemcpyAsync(b.out_h, rsp.format == 1 ? (const void*)b.i16 : (const void*)b.rs, (size_t)rsp.total * es,
-                            cudaMemcpyDeviceToHost, st));
+    const void* res = b.i16 ? (const void*)b.i16 : b.rs ? (const void*)b.rs : (const void*)b.wav;
+    SB_CUDA(cudaMemcpyAsync(b.out_h, res, total * (b.i16 ? 2 : 4), cudaMemcpyDeviceToHost, st));
     SB_CUDA(cudaStreamSynchronize(st));
     SB_CUDA(cudaGetLastError());
+
     for (size_t k = 0; k < n; k++) {
-        Resampler* r = rsp.rs[k];
+        Resampler* r = p.chunks[k].rs;
         if (!r) continue;
-        const ResampleSeg& s = rsp.segs[k];
-        r->consumed = s.c + ((long long)j.fsegs[k].len * v->a.hop() - b.post_h[k].trim_lo - b.post_h[k].trim_hi);
-        r->emitted = rsp.ends[k];
+        const ResampleSeg& s = rp.segs[k];
+        r->consumed = s.c + n_in[k];
+        r->emitted = s.j0 + s.n_out;
         r->cur ^= 1;
         r->h = s.h_out;
-        r->ended = rsp.last && rsp.last[k];
+        r->ended = p.chunks[k].last != 0;
     }
-    if (rsp.format == 1) out_i16.resize(n); else out_f32.resize(n);
+    if (b.i16) out.i16.resize(n); else out.f32.resize(n);
     for (size_t k = 0; k < n; k++) {
-        const long long o = rsp.segs[k].out_off, m = rsp.segs[k].n_out;
-        if (rsp.format == 1) {
-            const int16_t* h = reinterpret_cast<const int16_t*>(b.out_h);
-            out_i16[k].assign(h + o, h + o + m);
+        const long long o = p.resample ? rp.segs[k].out_off : j.fsegs[k].out_off;
+        const long long m = p.resample ? rp.segs[k].n_out : n_in[k];
+        if (b.i16) {
+            const int16_t* h = static_cast<const int16_t*>(b.out_h);
+            out.i16[k].assign(h + o, h + o + m);
         } else {
-            out_f32[k].assign(b.out_h + o, b.out_h + o + m);
+            const float* h = static_cast<const float*>(b.out_h);
+            out.f32[k].assign(h + o, h + o + m);
         }
     }
-}
-
-void chunks_f32(Voice* v, const Latent* const* z, const long long* lo, const long long* hi, size_t n,
-                std::vector<std::vector<float>>& out, float* ms, bool single) {
-    out.clear();
-    if (ms) *ms = 0.f;
-    if (n == 0) return;
-    Job j;
-    const ChunkBufs b = decode_chunks_device(v, z, lo, hi, n, j, nullptr, single);
-    Context& C = *j.ctx;
-    cudaStream_t st = C.stream;
-    // one copy of the packed waveforms through the context's page-locked staging buffer (a DMA copy, not a pageable one)
-    SB_CUDA(cudaMemcpyAsync(b.out_h, b.wav, (size_t)j.total_samples * 4, cudaMemcpyDeviceToHost, st));
-    SB_CUDA(cudaStreamSynchronize(st));
-    SB_CUDA(cudaGetLastError());
-    const int hop = v->a.hop();
-    out.resize(n);
-    for (size_t k = 0; k < n; k++)
-        out[k].assign(b.out_h + j.fsegs[k].out_off, b.out_h + j.fsegs[k].out_off + (size_t)j.fsegs[k].len * hop);
-    if (ms) cudaEventElapsedTime(ms, C.ev_begin, C.ev_end);
-}
-
-void chunks_pcm(Voice* v, const Latent* const* z, const long long* lo, const long long* hi, const ChunkPcm& pcm, size_t n,
-                std::vector<std::vector<int16_t>>& out, float* ms, bool single) {
-    out.clear();
-    if (ms) *ms = 0.f;
-    if (n == 0) return;
-    Job j;
-    const ChunkBufs b = decode_chunks_device(v, z, lo, hi, n, j, &pcm, single);
-    Context& C = *j.ctx;
-    cudaStream_t st = C.stream;
-    int16_t* h = reinterpret_cast<int16_t*>(b.out_h);
-    SB_CUDA(cudaMemcpyAsync(h, b.i16, (size_t)j.total_samples * 2, cudaMemcpyDeviceToHost, st));
-    SB_CUDA(cudaStreamSynchronize(st));
-    SB_CUDA(cudaGetLastError());
-    out.resize(n);
-    for (size_t k = 0; k < n; k++) {
-        const PcmPost& p = b.post_h[k];
-        const long long m = (long long)j.fsegs[k].len * v->a.hop() - p.trim_lo - p.trim_hi;
-        out[k].assign(h + j.fsegs[k].out_off, h + j.fsegs[k].out_off + m);
-    }
-    if (ms) cudaEventElapsedTime(ms, C.ev_begin, C.ev_end);
-}
-
-}  // namespace
-
-void decode_latent_chunks(Voice* v, const Latent* const* z, const long long* lo, const long long* hi, size_t n,
-                          std::vector<std::vector<float>>& out, float* ms) {
-    chunks_f32(v, z, lo, hi, n, out, ms, false);
-}
-
-void decode_latent_chunk(Voice* v, const Latent* z, long long lo, long long hi, std::vector<float>& out, float* ms) {
-    std::vector<std::vector<float>> o;
-    chunks_f32(v, &z, &lo, &hi, 1, o, ms, true);
-    out.swap(o[0]);
-}
-
-void decode_latent_chunks_pcm(Voice* v, const Latent* const* z, const long long* lo, const long long* hi,
-                              const long long* trim_lo_frames, const long long* trim_hi_frames, size_t n, int fade,
-                              const float* gain, std::vector<std::vector<int16_t>>& out, float* ms) {
-    chunks_pcm(v, z, lo, hi, ChunkPcm{trim_lo_frames, trim_hi_frames, fade, gain}, n, out, ms, false);
-}
-
-void decode_latent_chunk_pcm(Voice* v, const Latent* z, long long lo, long long hi, long long trim_lo_frames,
-                             long long trim_hi_frames, int fade, float gain, std::vector<int16_t>& out, float* ms) {
-    std::vector<std::vector<int16_t>> o;
-    chunks_pcm(v, &z, &lo, &hi, ChunkPcm{&trim_lo_frames, &trim_hi_frames, fade, &gain}, 1, o, ms, true);
-    out.swap(o[0]);
-}
-
-void decode_latent_chunks_resampled(Voice* v, const Latent* const* z, const long long* lo, const long long* hi,
-                                    const long long* trim_lo_frames, const long long* trim_hi_frames, size_t n, int fade,
-                                    const float* gain, Resampler* const* rs, const int* last, int format,
-                                    std::vector<std::vector<float>>& out_f32, std::vector<std::vector<int16_t>>& out_i16) {
-    if (n > 0 && !rs) throw Error(19, "null resampler table");
-    ChunkResample rsp;
-    rsp.rs = rs; rsp.last = last; rsp.format = format;
-    chunks_resampled(v, z, lo, hi, ChunkPcm{trim_lo_frames, trim_hi_frames, fade, gain}, rsp, n, out_f32, out_i16);
+    cudaEventElapsedTime(&out.ms, C.ev_begin, C.ev_end);
 }
 
 void job_i16_to_host(Job& j, float gain, int16_t* dst) {

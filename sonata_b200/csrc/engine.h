@@ -293,19 +293,6 @@ std::vector<Latent*> encode_latents(Voice* v, const long long* ids, const size_t
                                     const float* scale = nullptr, const int* frames = nullptr,
                                     const unsigned long long* seeds = nullptr, const int* seeded = nullptr);
 Latent* encode_latent(Voice* v, const long long* ids, size_t n);
-// One frame-level decoder pass over n chunks z[k][lo[k] : hi[k]) of latents of `v`; out[k] gets chunk k's waveform.
-// Chunk k equals the same chunk decoded alone, bit for bit.  ms: the pass's device time.
-void decode_latent_chunks(Voice* v, const Latent* const* z, const long long* lo, const long long* hi, size_t n,
-                          std::vector<std::vector<float>>& out, float* ms);
-void decode_latent_chunk(Voice* v, const Latent* z, long long lo, long long hi, std::vector<float>& out, float* ms);
-// the same chunks as peak-normalised i16 PCM with the reference's post-path done on the DEVICE, per chunk: drop
-// trim_lo / trim_hi overlap frames (null: none), crossfade(fade) (samples.rs:144-157), linear gain (null: 1),
-// to_i16_vec (samples.rs:51-75) normalised to the chunk's own peak
-void decode_latent_chunks_pcm(Voice* v, const Latent* const* z, const long long* lo, const long long* hi,
-                              const long long* trim_lo_frames, const long long* trim_hi_frames, size_t n, int fade,
-                              const float* gain, std::vector<std::vector<int16_t>>& out, float* ms);
-void decode_latent_chunk_pcm(Voice* v, const Latent* z, long long lo, long long hi, long long trim_lo_frames,
-                             long long trim_hi_frames, int fade, float gain, std::vector<int16_t>& out, float* ms);
 // One stream's resampling state: the filter to its output rate, the last inputs (two device buffers of K floats each,
 // read and written alternately), and how many inputs it has consumed and outputs it has emitted.
 struct Resampler {
@@ -321,14 +308,37 @@ Resampler* create_resampler(Voice* v, long long out_rate);
 // Outputs of a stream whose first n inputs have arrived: all ceil(n * up / down) once it has ended, else those whose
 // every input has arrived (j * down + H < n * up).
 long long resample_emit_end(const ResampleFilter& f, long long n, bool ended);
-// decode_latent_chunks_pcm's post-path (trim, crossfade, gain) per chunk, then chunk k appended to its stream's
-// resampler rs[k] (null: the chunk is returned at the voice's rate, as that post-path leaves it), emitting every output
-// it can, and flushing the stream when last[k] is 1.  format 0: f32 in out_f32; 1: i16 normalised to each emitted
-// chunk's own peak, in out_i16.  A resampler may appear once per call, and must belong to `v`.
-void decode_latent_chunks_resampled(Voice* v, const Latent* const* z, const long long* lo, const long long* hi,
-                                    const long long* trim_lo_frames, const long long* trim_hi_frames, size_t n, int fade,
-                                    const float* gain, Resampler* const* rs, const int* last, int format,
-                                    std::vector<std::vector<float>>& out_f32, std::vector<std::vector<int16_t>>& out_i16);
+
+// One chunk z[lo, hi) of a latent, and what its pass does to it before it leaves.
+struct ChunkSpec {
+    const Latent* z = nullptr; long long lo = 0, hi = 0;
+    long long trim_lo = 0, trim_hi = 0;   // overlap frames dropped by the post-path
+    float gain = 1.f;                     // linear gain of the post-path
+    Resampler* rs = nullptr;              // the chunk's stream (resample passes; null: none)
+    int last = 0;                         // 1: the chunk ends its stream, which is flushed
+};
+// One frame-level decoder pass over chunks of latents of one voice; chunk k equals the same chunk decoded alone, bit for
+// bit.  Without `resample` or i16, a chunk leaves as the decoder's waveform, and its trims, gain and the fade must keep
+// their defaults.  Otherwise the reference's post-path runs on the device per chunk: drop the trim frames,
+// crossfade(fade) (samples.rs:144-157), the gain.  With `resample` the chunk is then appended to its stream's resampler,
+// emitting every output it can (a chunk without one leaves at the voice's rate as the post-path leaves it); a resampler
+// may appear once per pass and must belong to the voice.  i16: to_i16_vec (samples.rs:51-75) normalised to each emitted
+// chunk's own peak.  Every check runs before any device work and any resampler changes; errors name the chunk, except
+// with `single`, which keeps the single-chunk entry point's messages.
+struct ChunkPass {
+    std::vector<ChunkSpec> chunks;
+    int fade = 0;
+    bool resample = false;
+    int format = 0;                       // 0: f32, 1: i16
+    bool single = false;
+};
+struct ChunkResult {
+    std::vector<std::vector<float>> f32;      // format 0
+    std::vector<std::vector<int16_t>> i16;    // format 1
+    float ms = 0;                             // the pass's device time
+};
+void decode_chunks(Voice* v, const ChunkPass& p, ChunkResult& out);
+
 void job_pcm16(Job& j, float gain, std::vector<std::vector<int16_t>>& out);
 // Peak-normalised 16-bit PCM of every utterance of a finished job (to_i16_vec after a linear gain), converted on the
 // device and copied to `dst`: total_samples values laid out like the job's waveforms, in host memory that is best

@@ -134,12 +134,16 @@ void do_synthesize(Voice* v, const std::string& text, const SynthesisParams& p) 
             std::unique_ptr<Latent> z(encode_latent(v, ids.data(), ids.size()));
             const long long frames = z->frames;
             long long n = 0;
-            std::vector<int16_t> w;
+            ChunkPass cp;                                                           // one chunk, leaving as i16
+            cp.format = 1; cp.single = true;
+            ChunkResult r;
             if (frames <= 2 * chunk + 2 * pad) {                                    // one-shot (piper :785)
-                decode_latent_chunk_pcm(v, z.get(), 0, frames, 0, 0, 0, gain, w, nullptr);
-                n = 1; if (!emit(p, w, 0)) return;
+                cp.chunks = {ChunkSpec{z.get(), 0, frames, 0, 0, gain}};
+                decode_chunks(v, cp, r);
+                n = 1; if (!emit(p, r.i16[0], 0)) return;
             } else {                                                                // AdaptiveMelChunker (piper :886-912)
                 long long last = 0, step = 1; bool more = true;
+                cp.fade = 42;                                                       // trim + crossfade(42)
                 while (more) {
                     const long long cs = std::min<long long>(chunk * step, 1024);
                     const long long start = last == 0 ? 0 : last - 2 * pad, spad = last == 0 ? 0 : pad;
@@ -147,8 +151,9 @@ void do_synthesize(Voice* v, const std::string& text, const SynthesisParams& p) 
                     long long end = cend, epad = pad;
                     if (frames - cend <= 44) { end = frames; epad = 0; more = false; }
                     step++; last = cend;
-                    decode_latent_chunk_pcm(v, z.get(), start, end, spad, epad, 42, gain, w, nullptr);   // trim + crossfade(42)
-                    n++; if (!emit(p, w, 0)) return;
+                    cp.chunks = {ChunkSpec{z.get(), start, end, spad, epad, gain}};
+                    decode_chunks(v, cp, r);
+                    n++; if (!emit(p, r.i16[0], 0)) return;
                 }
             }
             produced += n;

@@ -222,6 +222,17 @@ class _PinnedOwner:
             pass
 
 
+def _take_chunks(lib, outs, lens, dtype) -> list:
+    """Copies of the chunk buffers `outs` (malloc'ed, lens[k] samples of `dtype` each) as numpy arrays; frees them."""
+    ptr = C.POINTER(np.ctypeslib.as_ctypes_type(dtype))
+    res = []
+    for k in range(len(lens)):
+        m = int(lens[k])
+        res.append(np.ctypeslib.as_array(C.cast(outs[k], ptr), (m,)).copy() if m else np.zeros(0, dtype))
+        lib.sb200_i16_free(C.cast(outs[k], C.POINTER(C.c_int16)))
+    return res
+
+
 def _take_audio(a: N.sb200_audio) -> Audio:
     """Zero-copy: the returned samples are a read-only view of the library's pinned host buffer (the
     reference copies `outputs[0]` into a Vec at piper/src/lib.rs:392)."""
@@ -724,17 +735,9 @@ class VitsStreamingModel(_VitsCommons):
                 self._h, hs, p64(lo), p64(hi), p64(tlo), p64(thi), n, int(fade),
                 None if g is None else g.ctypes.data_as(C.POINTER(C.c_float)), rs, _ptr(fl, C.c_int32),
                 1 if pcm16 else 0, outs, lens, C.byref(err)), err)
-            res = []
-            for k in range(n):
-                m = int(lens[k])
-                if pcm16:
-                    a = np.ctypeslib.as_array(C.cast(outs[k], C.POINTER(C.c_int16)), (m,)).copy() if m else np.zeros(0, np.int16)
-                else:
-                    a = AudioSamples(np.ctypeslib.as_array(C.cast(outs[k], C.POINTER(C.c_float)), (m,)).copy()
-                                     if m else np.zeros(0, np.float32))
-                self._lib.sb200_i16_free(C.cast(outs[k], C.POINTER(C.c_int16)))
-                res.append(a)
-            return res
+            if pcm16:
+                return _take_chunks(self._lib, outs, lens, np.int16)
+            return [AudioSamples(a) for a in _take_chunks(self._lib, outs, lens, np.float32)]
         if not pcm16:
             outs = (N.sb200_audio * n)()
             _check(self._lib.sb200_decode_chunks(self._h, hs, p64(lo), p64(hi), n, outs, C.byref(err)), err)
@@ -745,11 +748,7 @@ class VitsStreamingModel(_VitsCommons):
         _check(self._lib.sb200_decode_chunks_i16(self._h, hs, p64(lo), p64(hi), p64(tlo), p64(thi), n, int(fade),
                                                  None if g is None else g.ctypes.data_as(C.POINTER(C.c_float)), outs,
                                                  lens, C.byref(err)), err)
-        res = []
-        for k in range(n):
-            res.append(np.ctypeslib.as_array(outs[k], (lens[k],)).copy() if lens[k] else np.zeros(0, np.int16))
-            self._lib.sb200_i16_free(outs[k])
-        return res
+        return _take_chunks(self._lib, outs, lens, np.int16)
 
     def supports_streaming_output(self) -> bool:
         return True

@@ -210,6 +210,31 @@ def test_i16_equals_facade_realtime_events(voices, lib_built):
         assert _eq(g, e)
 
 
+def test_chunk_entry_points_add_only_their_output_stage_launches(voices):
+    """Over the same chunks every chunk entry point launches what sb200_decode_chunks launches, plus its output stage:
+    the i16 conversion (peak, convert), the resample launch (also when every resampler is null), or both."""
+    from sonata_b200 import _native as N
+    from sonata_b200.piper import Resampler
+    m = voices("medium4")
+    chunks = _chunk_set(_chunk_latents(m))
+    trimmed = [c + ((3, 3) if c[2] - c[1] > 6 else (0, 0)) for c in chunks]
+    rs = [Resampler(m, (8000, 48000)[k % 2]) if k % 3 else None for k in range(len(chunks))]
+
+    def launches(f):
+        n0 = N.lib().sb200_launch_count()
+        f()
+        return N.lib().sb200_launch_count() - n0
+    base = launches(lambda: m.infer_decoder_batch(chunks))
+    assert base > 0
+    assert launches(lambda: chunks[2][0].infer_decoder(chunks[2][1], chunks[2][2])) == \
+        launches(lambda: m.infer_decoder_batch([chunks[2]]))
+    extra = [launches(lambda: m.infer_decoder_batch(trimmed, pcm16=True, fade=42)),
+             launches(lambda: m.infer_decoder_batch(trimmed, fade=42, resamplers=rs)),
+             launches(lambda: m.infer_decoder_batch(trimmed, pcm16=True, fade=42, resamplers=rs)),
+             launches(lambda: m.infer_decoder_batch(trimmed, fade=42, resamplers=[None] * len(chunks)))]
+    assert [e - base for e in extra] == [2, 1, 3, 1]
+
+
 def _alone_stream(m, ids, cfg, cs, pad):
     enc = _alone_latent(m, ids, cfg)
     return [a.as_slice().copy() for a in SpeechStreamer(enc, cs, pad)]
