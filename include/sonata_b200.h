@@ -178,6 +178,31 @@ int32_t sb200_speak_batch_ids_rates(sb200_voice* v, const int64_t* ids_packed, c
                                     const uint32_t* output_rates, sb200_audio* outs, int32_t* id_frames_out,
                                     sb200_error* err);
 
+/* ---- loudness: each utterance measured (ITU-R BS.1770-4, one channel) and scaled to a target on the device ----
+ * Loudness is measured on the signal the caller receives (after resampling, at the output rate).  K-weighting is
+ * libebur128's any-rate design in double: a high shelf (f0 = 1681.974450955533 Hz, G = 3.999843853973347 dB,
+ * Q = 0.7071752369554196, Vb = Vh^0.4996667741545416) then a high-pass (f0 = 38.13547087602444 Hz,
+ * Q = 0.5003270373238773), both with K = tan(pi f0 / rate).  With the step S = (rate + 5) / 10 samples, block j covers
+ * samples [jS, jS + 4S) (floor((n - 4S) / S) + 1 blocks when n >= 4S, else none) and has z_j = sum y^2 / 4S over the
+ * K-weighted signal y, l_j = -0.691 + 10 log10(z_j).  The absolute gate keeps l_j > -70; with Gr = -0.691 +
+ * 10 log10(mean z over those) - 10, the integrated loudness L = -0.691 + 10 log10(mean z over the blocks with
+ * l_j > -70 and l_j > Gr), -inf when no block passes (silence, or under 400 ms).  Filter, energies and gates run in
+ * double.  The gain g = min(10^((T - L) / 20), 1 / peak) (peak: the largest |x|) is computed in double, rounded to f32
+ * and stepped down an ulp while f32(peak * g) > 1, and every sample becomes f32(x * g): normalisation never takes the
+ * sample peak above full scale.  L = -inf or peak = 0 gives g = 1 and the utterance keeps its bits.  An utterance's L,
+ * g and samples do not depend on its batch.  A target is a finite value in [-70, 0] LUFS, or NaN for none; any other
+ * value fails with OPERATION_ERROR naming the utterance.  When some utterance has a target every utterance is
+ * measured, and one without a target keeps its bits (g = 1).  The i16 results (sb200_job_fetch_i16,
+ * sb200_job_copy_out format 1) convert an utterance with a target at the fixed scale, trunc(clamp(y * 32767, -32768,
+ * 32767)), so its level survives; the others keep to_i16_vec.
+ * sb200_speak_batch_ids_rates with target_lufs[b] the target of utterance b; lufs_out / gain_out (either may be NULL)
+ * receive each utterance's L and g when some utterance has a target.  NULL targets is that call, bit for bit. */
+int32_t sb200_speak_batch_ids_loudness(sb200_voice* v, const int64_t* ids_packed, const size_t* offsets, size_t batch,
+                                       const sb200_synth_config* cfgs, const float* scale_packed,
+                                       const int32_t* frames_packed, const uint64_t* seeds, const int32_t* seeded,
+                                       const uint32_t* output_rates, const float* target_lufs, sb200_audio* outs,
+                                       int32_t* id_frames_out, double* lufs_out, float* gain_out, sb200_error* err);
+
 /* ---- job API: the same batched pass split into its host<->device steps (bench / multi-GPU plumbing) ----
  * create  : copies ids to the device (H2D).  `eps_w` / `eps_z` optionally inject the graph's two
  *           RandomNormalLike draws (time-major: eps_w[b] = f32[T_x][2], eps_z[b] = f32[T_y][inter]);
@@ -213,6 +238,15 @@ int32_t sb200_job_set_seeds(sb200_job* job, const uint64_t* seeds, const int32_t
  * sb200_job_fetch_i16, sb200_job_copy_out (both formats) and the samples and out_offsets of sb200_job_lengths; its
  * frames stay frame counts.  sb200_job_profile reports the resampling launch as the region "resample". */
 int32_t sb200_job_set_output_rates(sb200_job* job, const uint32_t* rates, sb200_error* err);
+/* Loudness targets (see sb200_speak_batch_ids_loudness) for the next sb200_job_run: target_lufs[0 .. batch), or NULL
+ * for none (what a new job starts with; so are targets that are all NaN).  A bad entry fails with OPERATION_ERROR naming
+ * the utterance and leaves the job's targets as they were.  A run with targets measures after the decoder and any
+ * resampling, scales the job's result in place (d_out included), and sb200_job_profile reports the launch as the
+ * region "loudness". */
+int32_t sb200_job_set_loudness(sb200_job* job, const float* target_lufs, sb200_error* err);
+/* Each utterance's integrated loudness L (LUFS, -inf when no block passes the gates) and applied gain g of the last run
+ * into lufs[0 .. batch) / gain[0 .. batch) (either may be NULL).  Fails when that run had no targets. */
+int32_t sb200_job_loudness(const sb200_job* job, double* lufs, float* gain, sb200_error* err);
 /* Frames per id of the last run, packed like ids_packed, into out_packed[0 .. capacity): one device->host copy of the
  * whole batch's cumulative durations, made on the first call after a run.  Fails before a run, or when capacity is
  * smaller than the number of ids. */
@@ -388,6 +422,12 @@ int32_t sb200_debug_resample_emit(int32_t in_rate, int32_t out_rate, const int64
  * samples, bit for bit what a job resampling an utterance of those samples returns. */
 int32_t sb200_debug_resample(int32_t device, const float* x, size_t n, int32_t in_rate, int32_t out_rate, float* y,
                              sb200_error* err);
+/* Test hook, no device needed: the K-weighting design at `rate` (see sb200_speak_batch_ids_loudness) into coeffs[0 .. 10):
+ * the shelf's b0, b1, b2, a1, a2, then the high-pass's (a0 = 1).  Returns 0, or 19 for a rate outside 8000 .. 384000. */
+int32_t sb200_debug_loudness_filter(int32_t rate, double* coeffs);
+/* The loudness kernel over one caller buffer x[0 .. n) at `rate`, measured only: *lufs receives its integrated loudness,
+ * bit for bit what a job measures for an utterance of those samples. */
+int32_t sb200_debug_loudness(int32_t device, const float* x, size_t n, int32_t rate, double* lufs, sb200_error* err);
 /* kernels launched by this library since load (host-side counter) */
 uint64_t sb200_launch_count(void);
 /* select the contraction backend: 0 = fp32 CUDA-core implicit GEMM, 1 = wgmma (3xTF32) where

@@ -17,8 +17,9 @@ import sys
 from typing import Optional
 
 from . import from_config_path
+from .core import OperationError
 from .piper import PiperSynthesisConfig
-from .synth import AudioOutputConfig, SonataSpeechSynthesizer
+from .synth import AudioOutputConfig, SonataSpeechSynthesizer, _check_loudness
 
 MODES = ("lazy", "parallel", "realtime")
 
@@ -43,6 +44,10 @@ def build_parser() -> argparse.ArgumentParser:
                                           "give the same samples (default: positional noise)")
     ap.add_argument("--output-rate", type=int, help="Output sample rate in Hz (8000, 11025, 16000, 22050, 24000, 32000, "
                                                   "44100 or 48000; default the voice's), resampled on the GPU")
+    ap.add_argument("--loudness", type=float, metavar="LUFS",
+                    help="Target integrated loudness of every sentence in LUFS, [-70, 0] (ITU-R BS.1770-4; e.g. -23 "
+                         "EBU R128, -16 podcasts), measured and applied on the GPU; output is then written at a fixed "
+                         "scale instead of peak-normalised.  Not in realtime mode")
     ap.add_argument("--device", type=int, default=int(os.environ.get("SONATA_B200_DEVICE", "0")))
     return ap
 
@@ -50,8 +55,17 @@ def build_parser() -> argparse.ArgumentParser:
 def process_request(synth: SonataSpeechSynthesizer, default_cfg: PiperSynthesisConfig, req: dict,
                     output_file: Optional[str], out=None) -> None:
     """process_synthesis_request (main.rs:126-165).  `seed` (optional): the request's noise seed, see
-    synth.sentence_seed.  `output_rate` (optional): the sample rate of the WAV or raw PCM written."""
+    synth.sentence_seed.  `output_rate` (optional): the sample rate of the WAV or raw PCM written.  `loudness`
+    (optional): every sentence's target loudness in LUFS; the PCM is then written at the fixed scale."""
     out = out or sys.stdout.buffer
+    mode = (req.get("mode") or "lazy").lower()
+    loudness = req.get("loudness")
+    if loudness is not None:
+        _check_loudness(loudness)
+        if mode == "realtime" and not output_file:
+            raise OperationError("loudness normalisation is not available in realtime mode: integrated loudness needs "
+                                 "the whole sentence, and realtime mode hands out a sentence's first chunk before its "
+                                 "last one is decoded (use lazy or parallel mode)")
     synth.model.set_fallback_synthesis_config(PiperSynthesisConfig(
         req.get("speaker_id"),
         req["noise_scale"] if req.get("noise_scale") is not None else default_cfg.noise_scale,
@@ -61,21 +75,21 @@ def process_request(synth: SonataSpeechSynthesizer, default_cfg: PiperSynthesisC
     text = req["text"]
     seed = req.get("seed")
     rate = {"output_rate": req["output_rate"]} if req.get("output_rate") else {}
+    loud = {} if loudness is None else {"loudness": loudness}
     if output_file:
-        synth.synthesize_to_file(output_file, text, oc, seed=seed, **rate)
+        synth.synthesize_to_file(output_file, text, oc, seed=seed, **rate, **loud)
         return
-    mode = (req.get("mode") or "lazy").lower()
     if mode == "lazy":
-        stream = (a.samples for a in synth.synthesize_lazy(text, oc, seed=seed, **rate))
+        stream = (a.samples for a in synth.synthesize_lazy(text, oc, seed=seed, **rate, **loud))
     elif mode == "parallel":
-        stream = (a.samples for a in synth.synthesize_parallel(text, oc, seed=seed, **rate))
+        stream = (a.samples for a in synth.synthesize_parallel(text, oc, seed=seed, **rate, **loud))
     elif mode == "realtime":
         stream = synth.synthesize_streamed(text, oc, req.get("chunk_size") or 100, req.get("chunk_padding") or 3,
                                           seed=seed, **rate)
     else:
         raise ValueError(f"unknown synthesis mode `{mode}`")
     for samples in stream:
-        out.write(samples.as_wave_bytes())
+        out.write(samples.as_wave_bytes(fixed_scale=loudness is not None))
         out.flush()
 
 
@@ -90,7 +104,8 @@ def main(argv=None) -> int:
         req = {"text": text, "mode": args.mode, "speaker_id": args.speaker_id, "length_scale": args.length_scale,
                "noise_scale": args.noise_scale, "noise_w": args.noise_w, "rate": args.rate, "volume": args.volume,
                "pitch": args.pitch, "appended_silence_ms": args.silence, "chunk_size": args.chunk_size,
-               "chunk_padding": args.chunk_padding, "seed": args.seed, "output_rate": args.output_rate}
+               "chunk_padding": args.chunk_padding, "seed": args.seed, "output_rate": args.output_rate,
+               "loudness": args.loudness}
         process_request(synth, default_cfg, req, args.output_file)
     else:
         for i, line in enumerate(sys.stdin):
@@ -101,6 +116,8 @@ def main(argv=None) -> int:
                 req["seed"] = args.seed
             if req.get("output_rate") is None:
                 req["output_rate"] = args.output_rate
+            if req.get("loudness") is None:
+                req["loudness"] = args.loudness
             out_file = None
             if args.output_file:
                 stem, ext = os.path.splitext(args.output_file)

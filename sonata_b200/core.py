@@ -115,8 +115,15 @@ class AudioSamples:
         y = np.clip(v * scale, np.float32(-32768.0), np.float32(32767.0))
         return np.trunc(y).astype(np.int16)
 
-    def as_wave_bytes(self) -> bytes:
-        return self.to_i16_vec().astype("<i2").tobytes()
+    def to_i16_fixed(self) -> np.ndarray:
+        """trunc(clamp(x * 32767, -32768, 32767)): 16-bit PCM at a fixed scale, which keeps a loudness-normalised
+        buffer's level (the library's i16 conversion of an utterance with a loudness target)."""
+        y = np.clip(self._v * np.float32(32767.0), np.float32(-32768.0), np.float32(32767.0))
+        return np.trunc(y).astype(np.int16)
+
+    def as_wave_bytes(self, fixed_scale: bool = False) -> bytes:
+        """16-bit little-endian PCM, peak-normalised (to_i16_vec), or at the fixed scale (to_i16_fixed)."""
+        return (self.to_i16_fixed() if fixed_scale else self.to_i16_vec()).astype("<i2").tobytes()
 
     def merge(self, other: "AudioSamples") -> None:
         self._v = np.concatenate([self._v, other._v])
@@ -170,9 +177,10 @@ class Audio:
         d = self.duration_ms()
         return 0.0 if d == 0.0 else self.inference_ms / d
 
-    def save_to_file(self, filename) -> None:
+    def save_to_file(self, filename, fixed_scale: bool = False) -> None:
+        """A 16-bit WAV file, peak-normalised, or at the fixed scale (see AudioSamples.as_wave_bytes)."""
         with wave.open(str(filename), "wb") as w:
             w.setnchannels(self.info.num_channels)
             w.setsampwidth(self.info.sample_width)
             w.setframerate(self.info.sample_rate)
-            w.writeframes(self.as_wave_bytes())
+            w.writeframes(self.samples.as_wave_bytes(fixed_scale))

@@ -6,6 +6,7 @@
 #include "tc_common.cuh"
 #include <algorithm>
 #include <chrono>
+#include <cmath>
 #include <cstring>
 #include <deque>
 
@@ -251,11 +252,18 @@ int32_t sb200_phonemes_to_input_ids_map(const sb200_voice* v, const char* ph, in
     });
 }
 
-int32_t sb200_speak_batch_ids_rates(sb200_voice* v, const int64_t* ids, const size_t* offsets, size_t batch,
-                                    const sb200_synth_config* cfgs, const float* scale_packed,
-                                    const int32_t* frames_packed, const uint64_t* seeds, const int32_t* seeded,
-                                    const uint32_t* output_rates, sb200_audio* outs, int32_t* id_frames_out,
-                                    sb200_error* err) {
+// Measured loudness and applied gains of a job's last run into lufs / gain (either may be null).
+static void job_loudness(const Job& j, double* lufs, float* gain) {
+    if (!j.ran || j.loud_ran.empty()) throw Error(19, "the job's last run measured no loudness (no utterance had a target)");
+    if (lufs) std::copy(j.loud_lufs.begin(), j.loud_lufs.end(), lufs);
+    if (gain) std::copy(j.loud_gain.begin(), j.loud_gain.end(), gain);
+}
+
+int32_t sb200_speak_batch_ids_loudness(sb200_voice* v, const int64_t* ids, const size_t* offsets, size_t batch,
+                                       const sb200_synth_config* cfgs, const float* scale_packed,
+                                       const int32_t* frames_packed, const uint64_t* seeds, const int32_t* seeded,
+                                       const uint32_t* output_rates, const float* target_lufs, sb200_audio* outs,
+                                       int32_t* id_frames_out, double* lufs_out, float* gain_out, sb200_error* err) {
     return guarded(err, [&] {
         const double t0 = now_ms();
         static_assert(sizeof(long long) == sizeof(int64_t), "");
@@ -264,22 +272,33 @@ int32_t sb200_speak_batch_ids_rates(sb200_voice* v, const int64_t* ids, const si
             for (size_t b = 0; b < batch; b++)
                 if (output_rates[b] != 0 && output_rates[b] != (uint32_t)v->v->sample_rate)
                     resample_ratio(v->v->sample_rate, output_rates[b], "utterance " + std::to_string(b) + ": ");
+        const bool loud = check_loudness_targets(target_lufs, batch);
         std::unique_ptr<Job> j(create_job(v->v.get(), reinterpret_cast<const long long*>(ids), offsets, batch, nullptr,
                                           nullptr, nullptr, false));
         if (cfgs) set_job_configs(*j, cfgs_in(cfgs, batch).data());
         set_job_durations(*j, scale_packed, frames_packed);
         set_job_seeds(*j, reinterpret_cast<const unsigned long long*>(seeds), seeded);
         set_job_output_rates(*j, output_rates);
+        set_job_loudness(*j, target_lufs);
         j->run(nullptr, 0);
         fetch_audio(*j, outs, 0.f);
         if (id_frames_out) {
             const std::vector<int>& f = job_id_frames(*j);
             std::copy(f.begin(), f.end(), id_frames_out);
         }
+        if (loud) job_loudness(*j, lufs_out, gain_out);
         const float wall = (float)(now_ms() - t0);
         for (size_t b = 0; b < batch; b++)
             outs[b].inference_ms = wall * (j->out_total ? (float)outs[b].len / (float)j->out_total : 0.f);
     });
+}
+int32_t sb200_speak_batch_ids_rates(sb200_voice* v, const int64_t* ids, const size_t* offsets, size_t batch,
+                                    const sb200_synth_config* cfgs, const float* scale_packed,
+                                    const int32_t* frames_packed, const uint64_t* seeds, const int32_t* seeded,
+                                    const uint32_t* output_rates, sb200_audio* outs, int32_t* id_frames_out,
+                                    sb200_error* err) {
+    return sb200_speak_batch_ids_loudness(v, ids, offsets, batch, cfgs, scale_packed, frames_packed, seeds, seeded,
+                                          output_rates, nullptr, outs, id_frames_out, nullptr, nullptr, err);
 }
 int32_t sb200_speak_batch_ids_seeded(sb200_voice* v, const int64_t* ids, const size_t* offsets, size_t batch,
                                      const sb200_synth_config* cfgs, const float* scale_packed,
@@ -347,6 +366,12 @@ int32_t sb200_job_set_seeds(sb200_job* job, const uint64_t* seeds, const int32_t
 }
 int32_t sb200_job_set_output_rates(sb200_job* job, const uint32_t* rates, sb200_error* err) {
     return guarded(err, [&] { set_job_output_rates(*job->j, rates); });
+}
+int32_t sb200_job_set_loudness(sb200_job* job, const float* target_lufs, sb200_error* err) {
+    return guarded(err, [&] { set_job_loudness(*job->j, target_lufs); });
+}
+int32_t sb200_job_loudness(const sb200_job* job, double* lufs, float* gain, sb200_error* err) {
+    return guarded(err, [&] { job_loudness(*job->j, lufs, gain); });
 }
 int32_t sb200_job_id_frames(sb200_job* job, int32_t* out_packed, size_t capacity, sb200_error* err) {
     return guarded(err, [&] {
@@ -777,6 +802,37 @@ int32_t sb200_debug_resample(int32_t device, const float* x, size_t n, int32_t i
         launch_resample(dx, dfs, dpost, 1, drs, 1, n_out, resample_span(f.up, f.down, f.K), dy, 0);
         SB_CUDA(cudaDeviceSynchronize());
         SB_CUDA(cudaMemcpy(y, dy, (size_t)n_out * 4, cudaMemcpyDeviceToHost));
+    });
+}
+
+int32_t sb200_debug_loudness_filter(int32_t rate, double* coeffs) {
+    try {
+        if (!coeffs) return 19;
+        LoudSeg s{};
+        loudness_design(rate, s);
+        std::copy(s.k, s.k + 10, coeffs);
+        return 0;
+    } catch (const Error& e) {
+        return e.code;
+    }
+}
+
+int32_t sb200_debug_loudness(int32_t device, const float* x, size_t n, int32_t rate, double* lufs, sb200_error* err) {
+    return guarded(err, [&] {
+        if (!x || !lufs || n == 0) throw Error(19, "debug loudness: bad arguments");
+        LoudSeg s{};
+        loudness_design(rate, s);
+        s.off = 0; s.n = (long long)n; s.c0 = 0; s.target = NAN;
+        SB_CUDA(cudaSetDevice(device));
+        DeviceBuffers d;
+        float* dx = d.upload(x, n, n);
+        const LoudSeg* ds = d.upload(&s, 1, 1);
+        double* scratch = d.alloc<double>((size_t)LD_SCRATCH * ((n + s.S - 1) / s.S));
+        double* dl = d.alloc<double>(1);
+        float* dg = d.alloc<float>(1);
+        launch_loudness(dx, ds, 1, scratch, dl, dg, 0);
+        SB_CUDA(cudaDeviceSynchronize());
+        SB_CUDA(cudaMemcpy(lufs, dl, sizeof(double), cudaMemcpyDeviceToHost));
     });
 }
 

@@ -189,8 +189,9 @@ void launch_conv_post(const float* x, int C, const float* w /*[7][C]*/, float* w
                       const int* ftile_seg, int U, RowMap map, cudaStream_t st);
 // per-utterance peak-normalised f32 -> i16 (audio-ops `to_i16_vec`), out indexed like wav
 // what the reference applies to a chunk before the 16-bit conversion (see kernels_misc.cu): overlap trim (samples),
-// crossfade table of fade_n <= 48 entries, linear gain.  Default = plain to_i16_vec.
-struct PcmPost { float gain = 1.f; int fade_n = 0; long long trim_lo = 0, trim_hi = 0; float tab[48] = {0}; };
+// crossfade table of fade_n <= 48 entries, linear gain.  Default = plain to_i16_vec.  fixed_scale = 1 converts at the
+// fixed scale 32767 instead of the segment's peak (loudness-normalised utterances).
+struct PcmPost { float gain = 1.f; int fade_n = 0; long long trim_lo = 0, trim_hi = 0; float tab[48] = {0}; int fixed_scale = 0; };
 // posts: device array, one entry per segment; max_samples: the longest segment (before trimming), sizes the grid
 void launch_i16(const float* wav, const FrameSeg* fsegs, const PcmPost* posts, int nseg, int hop, long long max_samples,
                 unsigned* maxbits, short* out, cudaStream_t st);
@@ -212,6 +213,20 @@ inline int resample_span(int up, int down, int K) {
 // any segment, smem_floats: the largest resample_span of the segments.
 void launch_resample(const float* wav, const FrameSeg* fsegs, const PcmPost* posts, int hop, const ResampleSeg* segs,
                      int nseg, long long max_out, int smem_floats, float* out, cudaStream_t st);
+// Integrated loudness (BS.1770-4, one channel) of one segment, wav[off, off + n) at one rate, and its normalisation in
+// place (kernels_misc.cu loudness_kernel; the filter design is loudness.cu's).  The segment is cut into chunks of S
+// samples, chunk c at scratch[LD_SCRATCH * (c0 + c) ..).  k: the K-weighting cascade, shelf then high-pass, each
+// {b0, b1, b2, a1, a2} (a0 = 1); AS: A^S, row-major, of its state recurrence s' = A s + B x with s = the two biquads'
+// transposed-direct-form-II states {s1, s2, t1, t2}.  target: LUFS, NaN = measured only.
+struct LoudSeg {
+    long long off, n, c0;
+    int S; float target;
+    double k[10], AS[16];
+};
+constexpr int LD_SCRATCH = 6;     // doubles per chunk: its 4 states, its sum of y^2, its peak
+// One launch over nseg segments (blockIdx.x = segment): lufs[b] = the integrated loudness (-inf when no block passes the
+// gates), gain[b] = the gain applied to the segment (1 without a target).
+void launch_loudness(float* wav, const LoudSeg* segs, int nseg, double* scratch, double* lufs, float* gain, cudaStream_t st);
 // One row range of a frame level taken from a latent: rows [off, off + len) of the level are rows [lo, lo + len) of src.
 struct GatherSeg { const float* src; long long lo; int off; int len; };
 // s[r] = the source row of r's segment (tile_seg: segment of every gran-row tile), or exact zeros past its end.

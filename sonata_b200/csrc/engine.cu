@@ -249,6 +249,11 @@ void set_job_output_rates(Job& j, const unsigned* rates) {
     if (any) j.out_rates.swap(r); else j.out_rates.clear();
 }
 
+void set_job_loudness(Job& j, const float* targets) {
+    if (check_loudness_targets(targets, j.B)) j.loud_target.assign(targets, targets + j.B);
+    else j.loud_target.clear();
+}
+
 namespace {
 
 struct Runner {
@@ -454,6 +459,29 @@ struct ResampleTables {
     }
 };
 
+// The loudness launch over what a job hands out: one segment per utterance at its delivered rate, chunk scratch laid out
+// back to back.
+struct LoudnessPlan {
+    std::vector<LoudSeg> segs;
+    long long chunks = 0;
+};
+
+// Device tables of the loudness launch and their pinned mirrors: the segments, the chunk scratch and the results.
+struct LoudnessBufs {
+    LoudSeg *segs = nullptr, *segs_h = nullptr;
+    double* scratch = nullptr;
+    double *lufs = nullptr, *lufs_h = nullptr;
+    float *gain = nullptr, *gain_h = nullptr;
+    void carve(Arena& dev, Arena& pin, const LoudnessPlan& p) {
+        const size_t n = p.segs.size();
+        if (n == 0) return;
+        segs = dev.get<LoudSeg>(n); segs_h = pin.get<LoudSeg>(n);
+        scratch = dev.get<double>((size_t)LD_SCRATCH * std::max<long long>(p.chunks, 1));
+        lufs = dev.get<double>(n); lufs_h = pin.get<double>(n);
+        gain = dev.get<float>(n); gain_h = pin.get<float>(n);
+    }
+};
+
 // Decoder over RY frames: conv_pre's output, then ping-pong stage buffers sized for the widest stage, or with debug one
 // set per stage so every stage can be fetched.
 struct DecoderBufs {
@@ -500,8 +528,10 @@ struct FrameBufs {
     std::vector<float*> flow;                  // debug: z after each coupling layer, in the engine's channel order
     DecoderBufs dec;
     ResampleTables rt; float* rs;
-    void carve(Arena& dev, Arena& pin, const Job& j, const ResamplePlan& rp, bool own_wav) {
+    LoudnessBufs ld;
+    void carve(Arena& dev, Arena& pin, const Job& j, const ResamplePlan& rp, const LoudnessPlan& lp, bool own_wav) {
         rt.carve(dev, pin, rp.segs.size());
+        ld.carve(dev, pin, lp);
         rs = nullptr;
         if (!rp.segs.empty()) {
             if (own_wav) rs = dev.get<float>((size_t)rp.total + 4);
@@ -669,6 +699,41 @@ void run_resample(Runner& R, const ResamplePlan& p, const ResampleTables& t, con
     launch_resample(wav, fsegs, posts, hop, t.segs, (int)p.segs.size(), p.max_out, p.smem, out, R.st);
     R.count(p.flops, p.bytes);
     R.end();
+}
+
+// The loudness launch of a job with targets (an empty plan without): every utterance as the job hands it out, at its
+// rate, with its target or NaN.
+LoudnessPlan lay_out_loudness(const Job& j) {
+    LoudnessPlan p;
+    if (j.loud_target.empty() || j.encode_only) return p;
+    p.segs.resize(j.B);
+    for (size_t b = 0; b < j.B; b++) {
+        LoudSeg& s = p.segs[b];
+        loudness_design(j.osr[b], s);
+        s.off = j.osegs[b].out_off;
+        s.n = (long long)j.osegs[b].len * j.out_hop;
+        s.c0 = p.chunks;
+        s.target = j.loud_target[b];
+        p.chunks += (s.n + s.S - 1) / s.S;
+    }
+    return p;
+}
+
+// The loudness launch of plan `p` over wav in place, and the copy of its results to the pinned mirrors: profile region
+// "loudness".  Its bytes are the samples read and, where a target scales them, written.
+void run_loudness(Runner& R, const LoudnessPlan& p, const LoudnessBufs& t, float* wav) {
+    const size_t n = p.segs.size();
+    double samples = 0, scaled = 0;
+    for (const LoudSeg& s : p.segs) {
+        samples += (double)s.n;
+        if (!std::isnan(s.target)) scaled += (double)s.n;
+    }
+    R.begin("loudness");
+    launch_loudness(wav, t.segs, (int)n, t.scratch, t.lufs, t.gain, R.st);
+    R.count(2.0 * 22.0 * samples, 4.0 * (samples + scaled));
+    R.end();
+    SB_CUDA(cudaMemcpyAsync(t.lufs_h, t.lufs, n * sizeof(double), cudaMemcpyDeviceToHost, R.st));
+    SB_CUDA(cudaMemcpyAsync(t.gain_h, t.gain, n * sizeof(float), cudaMemcpyDeviceToHost, R.st));
 }
 
 // Fills the frame-level tables through their pinned mirrors; returns the level.
@@ -934,8 +999,10 @@ void Job::run(float* d_out, size_t d_out_cap) {
     lay_out_frames(*this, y_len, a.hop());
     const ResamplePlan rp = lay_out_output(*this, a.hop());
     const bool resample = !rp.segs.empty();
+    const LoudnessPlan lp = lay_out_loudness(*this);
+    loud_ran.clear(); loud_lufs.clear(); loud_gain.clear();
     FrameBufs f;
-    plan(C.dev_frame, C.pin, [&](Arena& dev, Arena& pin) { f.carve(dev, pin, *this, rp, d_out == nullptr); });
+    plan(C.dev_frame, C.pin, [&](Arena& dev, Arena& pin) { f.carve(dev, pin, *this, rp, lp, d_out == nullptr); });
     d_fsegs = f.y.fsegs;
     d_osegs = resample ? f.rt.osegs : d_fsegs;
     if (debug) {
@@ -948,6 +1015,10 @@ void Job::run(float* d_out, size_t d_out_cap) {
     }
     Level LY = upload_frames(*this, f.y, st);
     if (resample) f.rt.upload(rp, st);
+    if (!lp.segs.empty()) {
+        std::copy(lp.segs.begin(), lp.segs.end(), f.ld.segs_h);
+        h2d(f.ld.segs, f.ld.segs_h, lp.segs.size() * sizeof(LoudSeg), st);
+    }
 
     // ---------------- alignment expansion ----------------
     R.begin("align");
@@ -1006,11 +1077,17 @@ void Job::run(float* d_out, size_t d_out_cap) {
     }
     run_decoder(R, LY, f.y, f.dec, f.s, resample ? f.wav : d_wav);
     if (resample) run_resample(R, rp, f.rt, f.wav, f.y.fsegs, f.rt.posts, a.hop(), d_wav);
+    if (!lp.segs.empty()) run_loudness(R, lp, f.ld, d_wav);
     SB_CUDA(cudaEventRecord(C.ev_end, st));
     SB_CUDA(cudaStreamSynchronize(st));
     SB_CUDA(cudaGetLastError());
     SB_CUDA(cudaEventElapsedTime(&last_ms, C.ev_begin, C.ev_end));
     for (Region& r : regions) cudaEventElapsedTime(&r.ms, r.e0, r.e1);
+    if (!lp.segs.empty()) {
+        loud_ran = loud_target;
+        loud_lufs.assign(f.ld.lufs_h, f.ld.lufs_h + B);
+        loud_gain.assign(f.ld.gain_h, f.ld.gain_h + B);
+    }
     ran = true;
 }
 
@@ -1203,7 +1280,9 @@ void job_i16_to_host(Job& j, float gain, int16_t* dst) {
     SB_CUDA(cudaMallocAsync(&d_max, sizeof(unsigned) * j.B, st));
     SB_CUDA(cudaMallocAsync(&d_post, sizeof(PcmPost) * j.B, st));
     PcmPost post; post.gain = gain;
-    const std::vector<PcmPost> posts(j.B, post);
+    std::vector<PcmPost> posts(j.B, post);
+    // a loudness-normalised utterance keeps its level: fixed scale instead of its own peak
+    for (size_t b = 0; b < j.loud_ran.size(); b++) posts[b].fixed_scale = std::isnan(j.loud_ran[b]) ? 0 : 1;
     // pageable source: the call returns once the entries are staged, so `posts` may go out of scope before the copy runs
     SB_CUDA(cudaMemcpyAsync(d_post, posts.data(), sizeof(PcmPost) * j.B, cudaMemcpyHostToDevice, st));
     launch_i16(j.d_wav, j.d_osegs, d_post, (int)j.B, hop, mx, d_max, d_i16, st);

@@ -103,6 +103,15 @@ std::vector<float> resample_taps(int up, int down);
 // The phase-major image of `h`: [up][K], zero past 2H.
 std::vector<float> resample_phase_major(const std::vector<float>& h, int up, int K);
 
+// Loudness normalisation (loudness.cu).  Rates the K-weighting filter is designed for: 8 kHz .. 384 kHz.
+bool loudness_rate_supported(long long rate);
+// Fills s.S = (rate + 5) / 10, the cascade s.k (libebur128's design in double) and s.AS = A^S; throws OPERATION_ERROR
+// for an unsupported rate.
+void loudness_design(long long rate, LoudSeg& s);
+// Checks targets t[0 .. B) (null: none): NaN is no target, anything else must be finite and in [-70, 0] LUFS, or the
+// call fails naming the utterance.  Returns whether some utterance has a target.
+bool check_loudness_targets(const float* t, size_t B);
+
 struct Context;   // stream + arenas for one in-flight call
 
 struct Voice {
@@ -221,6 +230,11 @@ struct Job {
     std::vector<NoiseSeed> seeds;     // one per utterance, empty when none is seeded (set_job_seeds)
     std::vector<int> out_rates;       // one per utterance, 0 = the voice's rate; empty when none resamples
                                       // (set_job_output_rates)
+    std::vector<float> loud_target;   // one LUFS target per utterance, NaN = none; empty when none has one
+                                      // (set_job_loudness)
+    // Loudness of the last run: the targets it ran with (empty: it measured nothing), each utterance's integrated
+    // loudness and the gain applied to it
+    std::vector<float> loud_ran; std::vector<double> loud_lufs; std::vector<float> loud_gain;
     // X layout
     int RX = 0; std::vector<SegInfo> xsegs; int max_tx = 0;
     // Y layout
@@ -274,6 +288,10 @@ void set_job_seeds(Job& j, const unsigned long long* seeds, const int* seeded);
 // Per-utterance output rates of the job's next run (rates[0 .. B), 0 or the voice's rate: none), or null for none.
 // Every entry is checked first; an unsupported rate fails naming the utterance and leaves the job's rates as they were.
 void set_job_output_rates(Job& j, const unsigned* rates);
+// Per-utterance loudness targets of the job's next run (targets[0 .. B), NaN: none), or null for none.  With a target,
+// every utterance is measured after the decoder and any resampling, and those with one are scaled to it; see
+// check_loudness_targets for the checks.  A bad entry leaves the job's targets as they were.
+void set_job_loudness(Job& j, const float* targets);
 // Frames per id of the job's last run, packed like its ids: one device->host copy of the batch's cum rows through the
 // context's page-locked staging, differenced on the host.  Cached until the next run.
 const std::vector<int>& job_id_frames(Job& j);
@@ -342,7 +360,7 @@ void decode_chunks(Voice* v, const ChunkPass& p, ChunkResult& out);
 void job_pcm16(Job& j, float gain, std::vector<std::vector<int16_t>>& out);
 // Peak-normalised 16-bit PCM of every utterance of a finished job (to_i16_vec after a linear gain), converted on the
 // device and copied to `dst`: total_samples values laid out like the job's waveforms, in host memory that is best
-// page-locked (a DMA copy).
+// page-locked (a DMA copy).  An utterance the last run gave a loudness target converts at the fixed scale 32767.
 void job_i16_to_host(Job& j, float gain, int16_t* dst);
 
 }  // namespace sb200

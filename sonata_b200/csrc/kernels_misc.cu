@@ -706,7 +706,7 @@ __global__ void i16_convert_kernel(const float* __restrict__ wav, const FrameSeg
     const PcmSeg s = pcm_seg(wav, fs, posts + blockIdx.y, hop);
     short* y = out + fs.out_off;
     const float amax = fmaxf(__uint_as_float(maxbits[blockIdx.y]), 1.1920928955078125e-07f);
-    const float scale = __fdiv_rn(32767.0f, amax);
+    const float scale = posts[blockIdx.y].fixed_scale ? 32767.0f : __fdiv_rn(32767.0f, amax);
     for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < s.n; i += (long long)gridDim.x * blockDim.x) {
         const float v = fminf(fmaxf(__fmul_rn(pcm_value(s, i), scale), -32768.0f), 32767.0f);
         y[i] = (short)(int)v;                      // truncating cast
@@ -765,6 +765,166 @@ __global__ void resample_kernel(const float* __restrict__ wav, const FrameSeg* _
         }
         __syncthreads();
     }
+}
+
+// ------------------------------------------------------------------ integrated loudness (ITU-R BS.1770-4, one channel)
+// One block per segment.  The K-weighting cascade is the only sequential part: (1) every chunk of S samples is filtered
+// from zero state by one thread, which keeps the chunk's end state and peak; (2) thread 0 chains the states,
+// s_{c+1} = A^S s_c + e_c, giving every chunk its true initial state; (3) every full chunk is filtered again from it and
+// its sum of y^2, in sample order, is q_c; (4) block j (samples [jS, jS + 4S)) has z_j = (q_j + .. + q_{j+3}) / 4S and
+// the absolute and relative gates run over the z_j in a fixed tree order; (5) the gain g = min(10^((T - L)/20), 1/peak)
+// scales the segment in place.  Filter, energies and gates are double.  Chunking, chains and reduction orders depend on
+// the segment's samples and S only, so L, g and the output are the same bits in any batch.
+constexpr int LD_THREADS = 256;
+
+// Samples [i0, i1) of x through the cascade from state s (updated), returning the sum of y^2 in sample order.
+__device__ __forceinline__ double kweight_run(const float* __restrict__ x, long long i0, long long i1, const double* k,
+                                              double* s, float* peak) {
+    double s1 = s[0], s2 = s[1], t1 = s[2], t2 = s[3], e = 0.0;
+    float m = 0.f;
+    auto step = [&](float xf) {
+        m = fmaxf(m, fabsf(xf));
+        const double v = (double)xf;
+        const double y1 = fma(k[0], v, s1);
+        s1 = fma(k[1], v, fma(-k[3], y1, s2));
+        s2 = fma(k[2], v, -k[4] * y1);
+        const double y = fma(k[5], y1, t1);
+        t1 = fma(k[6], y1, fma(-k[8], y, t2));
+        t2 = fma(k[7], y1, -k[9] * y);
+        e = fma(y, y, e);
+    };
+    // the lanes of a warp read chunks S samples apart: 16 loads issued together wait for memory once, not 16 times
+    constexpr int V = 16;
+    long long i = i0;
+    for (; i + V <= i1; i += V) {
+        float xv[V];
+#pragma unroll
+        for (int u = 0; u < V; u++) xv[u] = x[i + u];
+#pragma unroll
+        for (int u = 0; u < V; u++) step(xv[u]);
+    }
+    for (; i < i1; i++) step(x[i]);
+    s[0] = s1; s[1] = s2; s[2] = t1; s[3] = t2;
+    *peak = m;
+    return e;
+}
+
+// Fixed-order tree sum over the block (every thread gets the total).
+__device__ __forceinline__ double ld_block_sum(double v, double* red) {
+    __syncthreads();
+    red[threadIdx.x] = v;
+    for (int w = LD_THREADS / 2; w > 0; w >>= 1) {
+        __syncthreads();
+        if (threadIdx.x < w) red[threadIdx.x] += red[threadIdx.x + w];
+    }
+    __syncthreads();
+    return red[0];
+}
+
+__device__ __forceinline__ double ld_block_loudness(double z) { return -0.691 + 10.0 * log10(z); }
+
+__global__ void __launch_bounds__(LD_THREADS) loudness_kernel(float* __restrict__ wav, const LoudSeg* __restrict__ segs,
+                                                              double* __restrict__ scratch, double* __restrict__ lufs,
+                                                              float* __restrict__ gain) {
+    __shared__ double red[LD_THREADS];
+    pdl_trigger(); pdl_wait();
+    const LoudSeg& G = segs[blockIdx.x];
+    const long long n = G.n, S = G.S;
+    float* x = wav + G.off;
+    double* sc = scratch + (long long)LD_SCRATCH * G.c0;
+    double k[10];
+#pragma unroll
+    for (int i = 0; i < 10; i++) k[i] = G.k[i];
+    const long long nch = (n + S - 1) / S, nfull = n / S;
+    // (1) zero-state end states and peaks
+    float peak = 0.f;
+    for (long long c = threadIdx.x; c < nch; c += LD_THREADS) {
+        double s[4] = {0.0, 0.0, 0.0, 0.0};
+        float m;
+        kweight_run(x, c * S, min(n, (c + 1) * S), k, s, &m);
+        double* d = sc + LD_SCRATCH * c;
+        d[0] = s[0]; d[1] = s[1]; d[2] = s[2]; d[3] = s[3];
+        peak = fmaxf(peak, m);
+    }
+    __syncthreads();
+    // (2) initial states, in place of the end states
+    if (threadIdx.x == 0) {
+        double s[4] = {0.0, 0.0, 0.0, 0.0};
+        for (long long c = 0; c + 1 < nch; c++) {
+            double* d = sc + LD_SCRATCH * c;
+            const double e[4] = {d[0], d[1], d[2], d[3]};
+            double t[4];
+#pragma unroll
+            for (int r = 0; r < 4; r++) {
+                double a = e[r];
+#pragma unroll
+                for (int q = 0; q < 4; q++) a = fma(G.AS[4 * r + q], s[q], a);
+                t[r] = a;
+            }
+            d[0] = s[0]; d[1] = s[1]; d[2] = s[2]; d[3] = s[3];
+#pragma unroll
+            for (int r = 0; r < 4; r++) s[r] = t[r];
+        }
+        if (nch > 0) {
+            double* d = sc + LD_SCRATCH * (nch - 1);
+            d[0] = s[0]; d[1] = s[1]; d[2] = s[2]; d[3] = s[3];
+        }
+    }
+    __syncthreads();
+    // (3) energy of every full chunk from its true initial state
+    for (long long c = threadIdx.x; c < nfull; c += LD_THREADS) {
+        double* d = sc + LD_SCRATCH * c;
+        double s[4] = {d[0], d[1], d[2], d[3]};
+        float m;
+        d[4] = kweight_run(x, c * S, (c + 1) * S, k, s, &m);
+    }
+    // peak of the segment (fmaxf of |x|, as i16_absmax_kernel)
+    peak = warp_max(peak);
+    __syncthreads();
+    if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = (double)peak;
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        float m = 0.f;
+        for (int w = 0; w < LD_THREADS / 32; w++) m = fmaxf(m, (float)red[w]);
+        red[LD_THREADS - 1] = (double)m;
+    }
+    __syncthreads();
+    peak = (float)red[LD_THREADS - 1];
+    // (4) gates over the nb blocks
+    const long long nb = n >= 4 * S ? (n - 4 * S) / S + 1 : 0;
+    const double blk = 4.0 * (double)S;
+    auto z_of = [&](long long j) {
+        const double* q = sc + LD_SCRATCH * j + 4;
+        return (((q[0] + q[LD_SCRATCH]) + q[2 * LD_SCRATCH]) + q[3 * LD_SCRATCH]) / blk;
+    };
+    double sum = 0.0, cnt = 0.0;
+    for (long long j = threadIdx.x; j < nb; j += LD_THREADS) {
+        const double z = z_of(j);
+        if (ld_block_loudness(z) > -70.0) { sum += z; cnt += 1.0; }
+    }
+    sum = ld_block_sum(sum, red);
+    cnt = ld_block_sum(cnt, red);
+    double L = -INFINITY;
+    if (cnt > 0.0) {
+        const double rel = ld_block_loudness(sum / cnt) - 10.0;
+        double sum2 = 0.0, cnt2 = 0.0;
+        for (long long j = threadIdx.x; j < nb; j += LD_THREADS) {
+            const double z = z_of(j), l = ld_block_loudness(z);
+            if (l > -70.0 && l > rel) { sum2 += z; cnt2 += 1.0; }
+        }
+        sum2 = ld_block_sum(sum2, red);
+        cnt2 = ld_block_sum(cnt2, red);
+        if (cnt2 > 0.0) L = ld_block_loudness(sum2 / cnt2);
+    }
+    // (5) the gain, never taking the peak above full scale
+    float g = 1.f;
+    if (!isnan(G.target) && L > -INFINITY && peak > 0.f) {
+        g = (float)fmin(exp10(((double)G.target - L) / 20.0), 1.0 / (double)peak);
+        while (__fmul_rn(peak, g) > 1.f) g = nextafterf(g, 0.f);
+    }
+    if (threadIdx.x == 0) { lufs[blockIdx.x] = L; gain[blockIdx.x] = g; }
+    if (g != 1.f)
+        for (long long i = threadIdx.x; i < n; i += LD_THREADS) x[i] = __fmul_rn(x[i], g);
 }
 
 // Frame-level input of a chunk pass: every row is a plain 16-byte copy of its segment's latent row or exact zeros, so a
@@ -1016,6 +1176,12 @@ void launch_resample(const float* wav, const FrameSeg* fsegs, const PcmPost* pos
     if (smem > 48 * 1024) throw_launch_error("resample: input span exceeds 48 KB of shared memory");
     const long long bx = std::min<long long>(std::max<long long>((max_out + RS_OUTS - 1) / RS_OUTS, 1), 4096);
     launch_pdl(resample_kernel, dim3((unsigned)bx, nseg), dim3(256), smem, st, wav, fsegs, posts, hop, segs, out);
+    g_launch_count++;
+}
+
+void launch_loudness(float* wav, const LoudSeg* segs, int nseg, double* scratch, double* lufs, float* gain, cudaStream_t st) {
+    if (nseg <= 0) return;
+    launch_pdl(loudness_kernel, dim3(nseg), dim3(LD_THREADS), 0, st, wav, segs, scratch, lufs, gain);
     g_launch_count++;
 }
 

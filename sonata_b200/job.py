@@ -4,21 +4,24 @@ per-stage intermediates).  Ordinary callers use `VitsModel.speak_*`."""
 from __future__ import annotations
 
 import ctypes as C
-from typing import List, Optional, Sequence
+from typing import List, Optional, Sequence, Tuple
 
 import numpy as np
 
 from . import _native as N
 from .core import Audio
-from .piper import _check, _config_array, _duration_arrays, _ptr, _rate_array, _seed_arrays, _take_audio
+from .piper import (_check, _config_array, _duration_arrays, _loudness_array, _ptr, _rate_array, _seed_arrays,
+                    _take_audio)
 
 
 class SynthesisJob:
     def __init__(self, model, batches: Sequence[Sequence[int]], eps_w: Optional[Sequence] = None,
                  eps_z: Optional[Sequence] = None, debug: bool = False, configs: Optional[Sequence] = None,
-                 seeds: Optional[Sequence] = None, output_rates: Optional[Sequence] = None):
+                 seeds: Optional[Sequence] = None, output_rates: Optional[Sequence] = None,
+                 loudness: Optional[Sequence] = None):
         """`configs`: one PiperSynthesisConfig per utterance (see set_configs); None keeps the voice's fallback config.
-        `seeds`: noise seeds (see set_seeds).  `output_rates`: output sample rates (see set_output_rates)."""
+        `seeds`: noise seeds (see set_seeds).  `output_rates`: output sample rates (see set_output_rates).
+        `loudness`: loudness targets (see set_loudness)."""
         self._m = model
         self._lib = model._lib
         n = len(batches)
@@ -27,6 +30,7 @@ class SynthesisJob:
         _config_array(configs, n)             # argument errors before the job exists
         _seed_arrays(seeds, n)
         _rate_array(output_rates, n)
+        _loudness_array(loudness, n)
         packed = np.ascontiguousarray(np.concatenate([np.asarray(b, dtype=np.int64) for b in batches]))
         offs = np.zeros(n + 1, dtype=np.uint64)
         offs[1:] = np.cumsum([len(b) for b in batches])
@@ -63,6 +67,8 @@ class SynthesisJob:
             self.set_seeds(seeds)
         if output_rates is not None:
             self.set_output_rates(output_rates)
+        if loudness is not None:
+            self.set_loudness(loudness)
 
     def set_configs(self, configs: Optional[Sequence]) -> None:
         """Per-utterance PiperSynthesisConfigs for the next run, or None for the voice's fallback config.  A wrong
@@ -95,6 +101,25 @@ class SynthesisJob:
         r = _rate_array(rates, self.batch)
         err = N.sb200_error()
         _check(self._lib.sb200_job_set_output_rates(self._h, _ptr(r, C.c_uint32), C.byref(err)), err)
+
+    def set_loudness(self, targets: Optional[Sequence]) -> None:
+        """Per-utterance loudness targets for the next run (see VitsModel.infer_batch_with_values): LUFS in [-70, 0] or
+        None per utterance; None for the whole list (or all None) turns loudness off.  A run with targets measures every
+        utterance, scales those with a target in place on the device (d_out included), and fetch_i16 / copy_out(fmt=1)
+        convert those at the fixed scale 32767 instead of their peak.  A bad entry raises OperationError naming the
+        utterance and leaves the job's targets as they were."""
+        t = _loudness_array(targets, self.batch)
+        err = N.sb200_error()
+        _check(self._lib.sb200_job_set_loudness(self._h, _ptr(t, C.c_float), C.byref(err)), err)
+
+    def loudness(self) -> Tuple[np.ndarray, np.ndarray]:
+        """(integrated loudness in LUFS as float64, -inf when no block passes the gates; gain applied as float32) per
+        utterance of the last run, which must have had targets."""
+        lufs = np.zeros(self.batch, np.float64)
+        gain = np.zeros(self.batch, np.float32)
+        err = N.sb200_error()
+        _check(self._lib.sb200_job_loudness(self._h, _ptr(lufs, C.c_double), _ptr(gain, C.c_float), C.byref(err)), err)
+        return lufs, gain
 
     def id_frames(self) -> List[np.ndarray]:
         """Frames per id of the last run, one int32 array per utterance (one device->host copy for the batch)."""

@@ -160,6 +160,25 @@ def _rate_array(rates, n: int):
     return out
 
 
+def _loudness_array(targets, n: int):
+    """The C image of per-utterance loudness targets (f32, NaN for none), or None when `targets` is None or holds no
+    target.  targets[b] is a LUFS value, finite and in [-70, 0], or None / NaN (utterance b is measured only)."""
+    if targets is None:
+        return None
+    out = np.full(n, np.nan, np.float32)
+    for b, t in enumerate(_per_utterance(targets, n, "loudness targets")):
+        if t is None:
+            continue
+        if isinstance(t, bool) or not isinstance(t, numbers.Real):
+            raise OperationError(f"utterance {b}: loudness target {t!r} is not a number")
+        if math.isnan(float(t)):
+            continue
+        if not (math.isfinite(float(t)) and -70.0 <= float(t) <= 0.0):
+            raise OperationError(f"utterance {b}: loudness target {float(t)} LUFS is not a finite value in [-70, 0]")
+        out[b] = float(t)
+    return None if np.isnan(out).all() else out
+
+
 def rate_ratio(in_rate: int, out_rate: Optional[int]) -> Tuple[int, int]:
     """(up, down): out_rate / in_rate reduced, (1, 1) for no resampling (None, 0 or the same rate)."""
     if not out_rate or int(out_rate) == int(in_rate):
@@ -358,20 +377,24 @@ class _VitsCommons:
 
     def speak_batch(self, phoneme_batches: Sequence[str],
                     configs: Optional[Sequence[PiperSynthesisConfig]] = None, seeds: Optional[Sequence] = None,
-                    output_rates: Optional[Sequence] = None) -> List[Audio]:
+                    output_rates: Optional[Sequence] = None, loudness: Optional[Sequence] = None) -> List[Audio]:
         """`configs`: one PiperSynthesisConfig per utterance (speaker and scales), still synthesised as one pass;
         None uses the fallback config for every utterance.  `seeds`: noise seeds as for infer_batch_with_values.
-        `output_rates`: per-utterance output sample rates as for infer_batch_with_values."""
+        `output_rates` / `loudness`: per-utterance output sample rates / loudness targets as for
+        infer_batch_with_values."""
         n = len(phoneme_batches)
         _config_array(configs, n)             # argument errors before any id mapping
         sv, _ = _seed_arrays(seeds, n)
         rates = _rate_array(output_rates, n)
+        loud = _loudness_array(loudness, n)
         if n == 0:
             return []
-        if configs is not None or sv is not None or rates is not None:
+        if configs is not None or sv is not None or rates is not None or loud is not None:
             extra = {} if sv is None else {"seeds": seeds}
             if rates is not None:
                 extra["output_rates"] = output_rates
+            if loud is not None:
+                extra["loudness"] = loudness
             return self.infer_batch_with_values([self.phonemes_to_input_ids(p) for p in phoneme_batches], configs,
                                                 **extra)
         arr = (C.c_char_p * n)(*[p.encode("utf-8") for p in phoneme_batches])
@@ -391,7 +414,8 @@ class _VitsCommons:
     def infer_batch_with_values(self, batches: Sequence[Sequence[int]],
                                 configs: Optional[Sequence[PiperSynthesisConfig]] = None,
                                 seeds: Optional[Sequence] = None,
-                                output_rates: Optional[Sequence] = None) -> List[Audio]:
+                                output_rates: Optional[Sequence] = None,
+                                loudness: Optional[Sequence] = None) -> List[Audio]:
         """Batched infer_with_values.  `configs`: one PiperSynthesisConfig per utterance (speaker and scales), or None
         for the fallback config; each utterance's result equals a single-utterance call with its config as the
         fallback, except for the on-device noise of an unseeded utterance, whose draws depend on the batch position.
@@ -402,14 +426,20 @@ class _VitsCommons:
 
         `output_rates`: one output sample rate per utterance, one of OUTPUT_RATES, or None / 0 for the voice's own.
         The waveform is resampled on the device with scipy.signal.resample_poly's default filter, and the Audio
-        reports the rate it is at."""
+        reports the rate it is at.
+
+        `loudness`: one target integrated loudness per utterance in LUFS (finite, in [-70, 0]) or None.  The delivered
+        signal (after any resampling) is measured on the device as ITU-R BS.1770-4 defines it and scaled to the target,
+        never past a sample peak of 1.0; an utterance under 400 ms or silent keeps its samples, as does one whose target
+        is None (see include/sonata_b200.h, sb200_speak_batch_ids_loudness)."""
         n = len(batches)
         cfgs = _config_array(configs, n)
         sv, _ = _seed_arrays(seeds, n)
         rates = _rate_array(output_rates, n)
-        if sv is not None or rates is not None:
+        loud = _loudness_array(loudness, n)
+        if sv is not None or rates is not None or loud is not None:
             return [a for a, _ in self.infer_batch_with_durations(batches, configs, seeds=seeds,
-                                                                  output_rates=output_rates)]
+                                                                  output_rates=output_rates, loudness=loudness)]
         packed = np.ascontiguousarray(np.concatenate([np.asarray(b, dtype=np.int64) for b in batches]))
         offs = np.zeros(n + 1, dtype=np.uint64)
         offs[1:] = np.cumsum([len(b) for b in batches])
@@ -425,7 +455,8 @@ class _VitsCommons:
                                    duration_scales: Optional[Sequence] = None,
                                    durations: Optional[Sequence] = None,
                                    seeds: Optional[Sequence] = None,
-                                   output_rates: Optional[Sequence] = None) -> List[Tuple[Audio, np.ndarray]]:
+                                   output_rates: Optional[Sequence] = None,
+                                   loudness: Optional[Sequence] = None) -> List[Tuple[Audio, np.ndarray]]:
         """infer_batch_with_values with per-id duration control, returning (audio, frames per id) per utterance.
 
         duration_scales[b]: one scale (finite, >= 0) per id of utterance b, applied before the duration's ceil, so 1.0
@@ -433,13 +464,14 @@ class _VitsCommons:
         Either list, or any of its entries, may be None.  The frame counts times 256 are each id's samples; an
         utterance whose ids all got 0 frames is still one frame long.  `seeds`: as for infer_batch_with_values; a
         seeded frame's noise depends on its index only, so controls that move frames never reshuffle it.
-        `output_rates`: as for infer_batch_with_values (the frame counts stay frame counts)."""
+        `output_rates` / `loudness`: as for infer_batch_with_values (the frame counts stay frame counts)."""
         n = len(batches)
         cfgs = _config_array(configs, n)
         lens = [len(b) for b in batches]
         scales, frames = _duration_arrays(lens, duration_scales, durations)
         sv, sf = _seed_arrays(seeds, n)
         rates = _rate_array(output_rates, n)
+        loud = _loudness_array(loudness, n)
         if n == 0:
             return []
         if any(x == 0 for x in lens):
@@ -450,17 +482,19 @@ class _VitsCommons:
         outs = (N.sb200_audio * n)()
         id_frames = np.zeros(int(offs[-1]), np.int32)
         err = N.sb200_error()
-        _check(self._lib.sb200_speak_batch_ids_rates(
+        _check(self._lib.sb200_speak_batch_ids_loudness(
             self._h, packed.ctypes.data_as(C.POINTER(C.c_int64)), offs.ctypes.data_as(C.POINTER(C.c_size_t)), n, cfgs,
             _ptr(scales, C.c_float), _ptr(frames, C.c_int32), _ptr(sv, C.c_uint64), _ptr(sf, C.c_int32),
-            _ptr(rates, C.c_uint32), outs, _ptr(id_frames, C.c_int32), C.byref(err)), err)
+            _ptr(rates, C.c_uint32), _ptr(loud, C.c_float), outs, _ptr(id_frames, C.c_int32), None, None,
+            C.byref(err)), err)
         return [(_take_audio(outs[b]), id_frames[int(offs[b]):int(offs[b + 1])].copy()) for b in range(n)]
 
     def speak_batch_with_alignment(self, phoneme_batches: Sequence[str],
                                    configs: Optional[Sequence[PiperSynthesisConfig]] = None,
                                    duration_scales: Optional[Sequence] = None,
                                    seeds: Optional[Sequence] = None,
-                                   output_rates: Optional[Sequence] = None) -> List[Tuple[Audio, List[PhonemeAlignment]]]:
+                                   output_rates: Optional[Sequence] = None,
+                                   loudness: Optional[Sequence] = None) -> List[Tuple[Audio, List[PhonemeAlignment]]]:
         """speak_batch that also says when each phoneme is spoken: per utterance (audio, alignment), the alignment
         holding one entry for bos (`^`), one per kept phoneme character (its id and its trailing pad) and one for eos
         (`$`), contiguous from sample 0 to len(audio).
@@ -468,11 +502,13 @@ class _VitsCommons:
         duration_scales[b] (or None): one scale per character of phoneme_batches[b], applied to that character's id and
         pad; characters the voice drops have no entry and their scales are ignored.  `seeds`: as for
         infer_batch_with_values.  `output_rates`: as for infer_batch_with_values; the alignment is then in samples of
-        the output rate, the boundary after F frames at ceil(F * 256 * up / down)."""
+        the output rate, the boundary after F frames at ceil(F * 256 * up / down).  `loudness`: as for
+        infer_batch_with_values; it scales samples and moves no boundary."""
         n = len(phoneme_batches)
         _config_array(configs, n)
         _seed_arrays(seeds, n)
         _rate_array(output_rates, n)
+        _loudness_array(loudness, n)
         per_char = None if duration_scales is None else _per_utterance(duration_scales, n, "duration scales")
         maps = [self.phonemes_to_input_ids_map(p) for p in phoneme_batches]
         id_scales = None
@@ -491,6 +527,8 @@ class _VitsCommons:
         extra = {} if seeds is None else {"seeds": seeds}
         if output_rates is not None:
             extra["output_rates"] = output_rates
+        if loudness is not None:
+            extra["loudness"] = loudness
         res = self.infer_batch_with_durations([m[0] for m in maps], configs, id_scales, **extra)
         voice_rate = self.audio_output_info().sample_rate if output_rates is not None else None
         ratio = lambda audio: (1, 1) if voice_rate is None else rate_ratio(voice_rate, audio.info.sample_rate)

@@ -96,6 +96,12 @@ def _check_output_rate(rate) -> None:
     _rate_array([rate], 1)
 
 
+def _check_loudness(target) -> None:
+    """Raises OperationError unless `target` is None or a loudness target in LUFS, finite and in [-70, 0]."""
+    from .piper import _loudness_array
+    _loudness_array([target], 1)
+
+
 def _sentences(model, text: str) -> List[str]:
     """SpeechSynthesisTaskProvider::get_phonemes (:256-258), or newline-separated phoneme sentences when the model has
     no phonemizer."""
@@ -121,27 +127,38 @@ class SonataSpeechSynthesizer:
     # `seed` (every mode): the request's noise seed, sentence i seeded with sentence_seed(seed, i); None keeps the
     # positional noise.  `output_rate` (every mode): the sample rate of the audio handed out, one of
     # piper.OUTPUT_RATES (None / 0: the voice's), each sentence resampled on the device; appended silence is generated
-    # at that rate.
+    # at that rate.  `loudness` (lazy, parallel and file modes): a target integrated loudness in LUFS, [-70, 0], each
+    # sentence measured and scaled to it on the device before the output config's volume and silence apply.
 
     def synthesize_lazy(self, text: str, output_config: Optional[AudioOutputConfig] = None,
-                        seed: Optional[int] = None, output_rate: Optional[int] = None) -> Iterator[Audio]:
+                        seed: Optional[int] = None, output_rate: Optional[int] = None,
+                        loudness: Optional[float] = None) -> Iterator[Audio]:
         sentence_seed(seed, 0)
         _check_output_rate(output_rate)
+        _check_loudness(loudness)
         for i, ph in enumerate(self._phonemes(text)):
-            if output_rate:
+            if output_rate or loudness is not None:
                 extra = {} if seed is None else {"seeds": [sentence_seed(seed, i)]}
-                a = self.model.speak_batch([ph], output_rates=[output_rate], **extra)[0]
+                if output_rate:
+                    extra["output_rates"] = [output_rate]
+                if loudness is not None:
+                    extra["loudness"] = [loudness]
+                a = self.model.speak_batch([ph], **extra)[0]
             else:
                 a = (self.model.speak_one_sentence(ph) if seed is None
                      else self.model.speak_batch([ph], seeds=[sentence_seed(seed, i)])[0])
             yield self._process(a, output_config)
 
     def synthesize_parallel(self, text: str, output_config: Optional[AudioOutputConfig] = None,
-                            seed: Optional[int] = None, output_rate: Optional[int] = None) -> Iterator[Audio]:
+                            seed: Optional[int] = None, output_rate: Optional[int] = None,
+                            loudness: Optional[float] = None) -> Iterator[Audio]:
         sentence_seed(seed, 0)
         _check_output_rate(output_rate)
+        _check_loudness(loudness)
         ph = self._phonemes(text)
         extra = {"output_rates": [output_rate] * len(ph)} if output_rate else {}
+        if loudness is not None:
+            extra["loudness"] = [loudness] * len(ph)
         if not ph:
             results = []
         elif seed is None:
@@ -190,14 +207,18 @@ class SonataSpeechSynthesizer:
             yield item
 
     def synthesize_to_file(self, filename, text: str, output_config: Optional[AudioOutputConfig] = None,
-                           seed: Optional[int] = None, output_rate: Optional[int] = None) -> None:
-        """:168-198 — parallel mode, concatenated, peak-normalised i16 WAV (at output_rate when given)."""
+                           seed: Optional[int] = None, output_rate: Optional[int] = None,
+                           loudness: Optional[float] = None) -> None:
+        """:168-198 — parallel mode, concatenated, peak-normalised i16 WAV (at output_rate when given).  With
+        `loudness` the WAV is written at the fixed scale (trunc(clamp(x * 32767))), so it keeps the sentences' level."""
         extra = {"output_rate": output_rate} if output_rate else {}
+        if loudness is not None:
+            extra["loudness"] = loudness
         parts = [a.samples.as_slice() for a in self.synthesize_parallel(text, output_config, seed=seed, **extra)]
         if not parts or sum(len(p) for p in parts) == 0:
             raise OperationError("No speech data to write")
         rate = output_rate or self.model.audio_output_info().sample_rate
-        Audio(AudioSamples(np.concatenate(parts)), rate).save_to_file(filename)
+        Audio(AudioSamples(np.concatenate(parts)), rate).save_to_file(filename, fixed_scale=loudness is not None)
 
     # passthroughs of the SonataModel surface (:205-253)
     def speak_one_sentence(self, phonemes: str) -> Audio:
