@@ -260,11 +260,26 @@ size_t sb200_job_batch(const sb200_job* job);
  * outs[b] receives a malloc'ed buffer of lens[b] samples: free with sb200_i16_free. */
 int32_t sb200_job_fetch_i16(sb200_job* job, int16_t** outs, size_t* lens, sb200_error* err);
 void sb200_i16_free(int16_t* p);
+/* G.711 audio for telephony (SIP/RTP PCMU = mu-law, payload type 0; PCMA = A-law, payload type 8), one byte per sample.
+ * The bytes are G.711 of exactly the i16 samples sb200_job_fetch_i16 returns, after utterance b is scaled by gains[b]
+ * (NULL = 1; each must be finite): to_i16_vec, or the fixed scale for an utterance with a loudness target.  The
+ * encoding runs in the same two launches as the i16 conversion; nothing is encoded on the host.  law:
+ * SB200_G711_MULAW (0) or SB200_G711_ALAW (1), as CPython's audioop.lin2ulaw / lin2alaw encode a 16-bit sample
+ * (silence, sample 0, is 0xFF in mu-law and 0xD5 in A-law).  outs[b] receives a malloc'ed buffer of lens[b] bytes:
+ * free with sb200_bytes_free.  A bad law or gain fails with OPERATION_ERROR before anything runs, a gain naming its
+ * utterance. */
+#define SB200_G711_MULAW 0
+#define SB200_G711_ALAW 1
+int32_t sb200_job_fetch_g711(sb200_job* job, int32_t law, const float* gains, uint8_t** outs, size_t* lens,
+                             sb200_error* err);
+void sb200_bytes_free(uint8_t* p);
 int32_t sb200_job_lengths(const sb200_job* job, int64_t* frames, int64_t* samples, int64_t* out_offsets);
 /* Copy the result of a finished job into CALLER-OWNED host memory, utterances back to back in batch order.
  * format 0: f32 samples (what infer_with_values returns, piper/src/lib.rs:382-392);
  * format 1: i16 PCM, peak-normalised per utterance on the device (= AudioSamples::to_i16_vec, samples.rs:51-75;
- *           what libsonata hands to its callback, capi/src/lib.rs:416-438) -- half the device->host bytes.
+ *           what libsonata hands to its callback, capi/src/lib.rs:416-438) -- half the device->host bytes;
+ * format 2 / 3: G.711 mu-law / A-law of the format-1 samples (sb200_job_fetch_g711 with gains 1), one byte per sample.
+ * Any other format fails with OPERATION_ERROR before anything runs.
  * `dst` may be ordinary or page-locked memory (see sb200_host_register), e.g. a slice of a segment shared by the
  * per-GPU worker processes of one frontend.  *written = bytes written; fails if `capacity_bytes` is too small. */
 int32_t sb200_job_copy_out(sb200_job* job, void* dst, size_t capacity_bytes, int32_t format, size_t* written,
@@ -320,6 +335,12 @@ int32_t sb200_decode_chunks(sb200_voice* v, const sb200_latent* const* zs, const
 int32_t sb200_decode_chunks_i16(sb200_voice* v, const sb200_latent* const* zs, const int64_t* lo, const int64_t* hi,
                                 const int64_t* trim_lo_frames, const int64_t* trim_hi_frames, size_t n, int32_t fade,
                                 const float* gain, int16_t** outs, size_t* lens, sb200_error* err);
+/* sb200_decode_chunks_i16's pass, each chunk leaving as the G.711 bytes (law as for sb200_job_fetch_g711) of the i16
+ * samples that call returns for it, from the same launches: outs[k] receives a malloc'ed buffer of lens[k] bytes, free
+ * with sb200_bytes_free.  A bad law fails with OPERATION_ERROR before anything runs. */
+int32_t sb200_decode_chunks_g711(sb200_voice* v, const sb200_latent* const* zs, const int64_t* lo, const int64_t* hi,
+                                 const int64_t* trim_lo_frames, const int64_t* trim_hi_frames, size_t n, int32_t fade,
+                                 const float* gain, int32_t law, uint8_t** outs, size_t* lens, sb200_error* err);
 
 /* ---- streams at an output sample rate (see sb200_speak_batch_ids_rates) ----
  * A resampler is one stream's state on the device: the last K - 1 <= 2H/up of its inputs (K taps per phase) and the
@@ -334,7 +355,9 @@ void sb200_resampler_free(sb200_resampler* r);
  * last[k] is 1 (last NULL: none), every output left, reading zeros past the stream's end; the resampler then takes no
  * more chunks.  A chunk may emit 0 samples.  The concatenation of a stream's outputs is, bit for bit, its whole input
  * resampled at once (sb200_debug_resample).  format 0: outs[k] is f32; 1: i16 normalised to the emitted chunk's own
- * peak (to_i16_vec).  outs[k] is malloc'ed, lens[k] samples: free with free() (sb200_i16_free / sb200_buffer_free).
+ * peak (to_i16_vec); 2 / 3: G.711 mu-law / A-law bytes of those i16 samples, except that gain[k] then scales the
+ * resampled samples just before their conversion (a volume on the delivered audio) rather than the chunk before it.  outs[k] is malloc'ed, lens[k] samples:
+ * free with free() (sb200_i16_free / sb200_buffer_free / sb200_bytes_free).  Another format fails with OPERATION_ERROR.
  * A resampler appearing twice, made for another voice or already flushed fails with OPERATION_ERROR naming the chunk,
  * before any state changes. */
 int32_t sb200_decode_chunks_resampled(sb200_voice* v, const sb200_latent* const* zs, const int64_t* lo, const int64_t* hi,
@@ -428,6 +451,9 @@ int32_t sb200_debug_loudness_filter(int32_t rate, double* coeffs);
 /* The loudness kernel over one caller buffer x[0 .. n) at `rate`, measured only: *lufs receives its integrated loudness,
  * bit for bit what a job measures for an utterance of those samples. */
 int32_t sb200_debug_loudness(int32_t device, const float* x, size_t n, int32_t rate, double* lufs, sb200_error* err);
+/* Test hook: G.711 (law as for sb200_job_fetch_g711) of x[0 .. n) into out[0 .. n).  device -1 runs the host copy of
+ * the encoders (no device needed); otherwise the encoders run on that device over the buffer. */
+int32_t sb200_debug_g711(int32_t device, int32_t law, const int16_t* x, size_t n, uint8_t* out, sb200_error* err);
 /* kernels launched by this library since load (host-side counter) */
 uint64_t sb200_launch_count(void);
 /* select the contraction backend: 0 = fp32 CUDA-core implicit GEMM, 1 = wgmma (3xTF32) where

@@ -102,6 +102,9 @@ SIGNATURES = {
     "sb200_job_fetch": (C.c_int32, [_P, C.POINTER(sb200_audio), _ERR]),
     "sb200_job_fetch_i16": (C.c_int32, [_P, C.POINTER(C.POINTER(C.c_int16)), C.POINTER(C.c_size_t), _ERR]),
     "sb200_i16_free": (None, [C.POINTER(C.c_int16)]),
+    "sb200_job_fetch_g711": (C.c_int32, [_P, C.c_int32, C.POINTER(C.c_float), C.POINTER(C.POINTER(C.c_uint8)),
+                                         C.POINTER(C.c_size_t), _ERR]),
+    "sb200_bytes_free": (None, [C.POINTER(C.c_uint8)]),
     "sb200_job_batch": (C.c_size_t, [_P]),
     "sb200_job_lengths": (C.c_int32, [_P, C.POINTER(C.c_int64), C.POINTER(C.c_int64), C.POINTER(C.c_int64)]),
     "sb200_job_copy_out": (C.c_int32, [_P, C.c_void_p, C.c_size_t, C.c_int32, C.POINTER(C.c_size_t), _ERR]),
@@ -128,6 +131,10 @@ SIGNATURES = {
                                             C.POINTER(C.c_int64), C.POINTER(C.c_int64), C.c_size_t, C.c_int32,
                                             C.POINTER(C.c_float), C.POINTER(C.POINTER(C.c_int16)),
                                             C.POINTER(C.c_size_t), _ERR]),
+    "sb200_decode_chunks_g711": (C.c_int32, [_P, C.POINTER(_P), C.POINTER(C.c_int64), C.POINTER(C.c_int64),
+                                             C.POINTER(C.c_int64), C.POINTER(C.c_int64), C.c_size_t, C.c_int32,
+                                             C.POINTER(C.c_float), C.c_int32, C.POINTER(C.POINTER(C.c_uint8)),
+                                             C.POINTER(C.c_size_t), _ERR]),
     "sb200_job_debug_fetch": (C.c_int32, [_P, C.c_char_p, C.c_size_t, C.POINTER(C.POINTER(C.c_float)),
                                           C.POINTER(C.c_size_t), C.POINTER(C.c_size_t), _ERR]),
     "sb200_buffer_free": (None, [C.POINTER(C.c_float)]),
@@ -168,6 +175,8 @@ SIGNATURES = {
     "sb200_debug_loudness_filter": (C.c_int32, [C.c_int32, C.POINTER(C.c_double)]),
     "sb200_debug_loudness": (C.c_int32, [C.c_int32, C.POINTER(C.c_float), C.c_size_t, C.c_int32, C.POINTER(C.c_double),
                                          _ERR]),
+    "sb200_debug_g711": (C.c_int32, [C.c_int32, C.c_int32, C.POINTER(C.c_int16), C.c_size_t, C.POINTER(C.c_uint8),
+                                     _ERR]),
     "sb200_launch_count": (C.c_uint64, []),
     "sb200_set_backend": (C.c_int32, [_P, C.c_int32]),
 }

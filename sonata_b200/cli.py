@@ -6,7 +6,9 @@ CLI (crates/frontends/cli/src/main.rs:32-260) over the H100 engine.
 
 Without `-f`, one JSON request per stdin line (fields of `SynthesisRequest`, main.rs:78-92); without `-o`, raw 16-bit
 LE PCM (peak-normalised per sentence / chunk like `as_wave_bytes`) goes to stdout; with `-o` and stdin requests the
-files are numbered `<stem>-<n>.<ext>` (main.rs:243-256).  `text` is phonemes, one sentence per line.
+files are numbered `<stem>-<n>.<ext>` (main.rs:243-256).  `text` is phonemes, one sentence per line.  With
+`--encoding mulaw|alaw` (or a JSON "encoding") the output is G.711 instead, encoded on the GPU: raw bytes on stdout,
+or an 8-bit G.711 WAV with `-o`.
 """
 from __future__ import annotations
 
@@ -17,7 +19,7 @@ import sys
 from typing import Optional
 
 from . import from_config_path
-from .core import OperationError
+from .core import ENCODINGS, OperationError, check_encoding
 from .piper import PiperSynthesisConfig
 from .synth import AudioOutputConfig, SonataSpeechSynthesizer, _check_loudness
 
@@ -48,6 +50,9 @@ def build_parser() -> argparse.ArgumentParser:
                     help="Target integrated loudness of every sentence in LUFS, [-70, 0] (ITU-R BS.1770-4; e.g. -23 "
                          "EBU R128, -16 podcasts), measured and applied on the GPU; output is then written at a fixed "
                          "scale instead of peak-normalised.  Not in realtime mode")
+    ap.add_argument("--encoding", choices=("pcm16",) + ENCODINGS,
+                    help="Output encoding: pcm16 (default), or G.711 mulaw / alaw at one byte per sample (telephony: "
+                         "PCMU / PCMA), encoded on the GPU")
     ap.add_argument("--device", type=int, default=int(os.environ.get("SONATA_B200_DEVICE", "0")))
     return ap
 
@@ -60,6 +65,8 @@ def process_request(synth: SonataSpeechSynthesizer, default_cfg: PiperSynthesisC
     out = out or sys.stdout.buffer
     mode = (req.get("mode") or "lazy").lower()
     loudness = req.get("loudness")
+    encoding = req.get("encoding")
+    encoding = None if encoding == "pcm16" else check_encoding(encoding, "request: ")
     if loudness is not None:
         _check_loudness(loudness)
         if mode == "realtime" and not output_file:
@@ -76,20 +83,25 @@ def process_request(synth: SonataSpeechSynthesizer, default_cfg: PiperSynthesisC
     seed = req.get("seed")
     rate = {"output_rate": req["output_rate"]} if req.get("output_rate") else {}
     loud = {} if loudness is None else {"loudness": loudness}
+    enc = {} if encoding is None else {"encoding": encoding}
     if output_file:
-        synth.synthesize_to_file(output_file, text, oc, seed=seed, **rate, **loud)
+        synth.synthesize_to_file(output_file, text, oc, seed=seed, **rate, **loud, **enc)
         return
     if mode == "lazy":
-        stream = (a.samples for a in synth.synthesize_lazy(text, oc, seed=seed, **rate, **loud))
+        stream = synth.synthesize_lazy(text, oc, seed=seed, **rate, **loud, **enc)
     elif mode == "parallel":
-        stream = (a.samples for a in synth.synthesize_parallel(text, oc, seed=seed, **rate, **loud))
+        stream = synth.synthesize_parallel(text, oc, seed=seed, **rate, **loud, **enc)
     elif mode == "realtime":
         stream = synth.synthesize_streamed(text, oc, req.get("chunk_size") or 100, req.get("chunk_padding") or 3,
-                                          seed=seed, **rate)
+                                          seed=seed, **rate, **enc)
     else:
         raise ValueError(f"unknown synthesis mode `{mode}`")
-    for samples in stream:
-        out.write(samples.as_wave_bytes(fixed_scale=loudness is not None))
+    for item in stream:
+        if encoding is not None:                      # G.711 bytes, one per sample
+            out.write(item)
+        else:
+            samples = item if mode == "realtime" else item.samples
+            out.write(samples.as_wave_bytes(fixed_scale=loudness is not None))
         out.flush()
 
 
@@ -105,7 +117,7 @@ def main(argv=None) -> int:
                "noise_scale": args.noise_scale, "noise_w": args.noise_w, "rate": args.rate, "volume": args.volume,
                "pitch": args.pitch, "appended_silence_ms": args.silence, "chunk_size": args.chunk_size,
                "chunk_padding": args.chunk_padding, "seed": args.seed, "output_rate": args.output_rate,
-               "loudness": args.loudness}
+               "loudness": args.loudness, "encoding": args.encoding}
         process_request(synth, default_cfg, req, args.output_file)
     else:
         for i, line in enumerate(sys.stdin):
@@ -118,6 +130,8 @@ def main(argv=None) -> int:
                 req["output_rate"] = args.output_rate
             if req.get("loudness") is None:
                 req["loudness"] = args.loudness
+            if req.get("encoding") is None:
+                req["encoding"] = args.encoding
             out_file = None
             if args.output_file:
                 stem, ext = os.path.splitext(args.output_file)

@@ -79,6 +79,54 @@ class AudioInfo:
 
 _F32_EPS = float(np.finfo(np.float32).eps)
 
+# G.711 encodings a result can be delivered in: the C ABI's law codes (SB200_G711_MULAW / _ALAW), the byte of silence
+# (sample 0) and the WAV format tag (WAVE_FORMAT_MULAW = 7, WAVE_FORMAT_ALAW = 6).
+ENCODINGS = ("mulaw", "alaw")
+G711_LAW = {"mulaw": 0, "alaw": 1}
+G711_SILENCE = {"mulaw": 0xFF, "alaw": 0xD5}
+G711_WAVE_TAG = {"mulaw": 7, "alaw": 6}
+
+
+def check_encoding(encoding, who: str = "") -> Optional[str]:
+    """`encoding` when it is None, "mulaw" or "alaw"; otherwise OperationError prefixed by `who` (e.g. "utterance 3: ")."""
+    if encoding is None or (isinstance(encoding, str) and encoding in ENCODINGS):
+        return encoding
+    raise OperationError(f"{who}encoding {encoding!r} is neither 'mulaw' nor 'alaw' (or None for linear PCM)")
+
+
+def g711_encode(x: np.ndarray, encoding: str) -> np.ndarray:
+    """G.711 bytes (uint8) of 16-bit samples, as CPython's audioop.lin2ulaw / lin2alaw compute them (the Sun g711.c
+    lineage); the library's encoders compute the same bytes on the device."""
+    check_encoding(encoding)
+    if encoding is None:
+        raise OperationError("encoding None is neither 'mulaw' nor 'alaw'")
+    v = np.asarray(x, dtype=np.int16).astype(np.int32).reshape(-1)
+    if encoding == "mulaw":
+        v = v >> 2                                            # 14 bits, arithmetic shift
+        mask = np.where(v < 0, 0x7F, 0xFF)
+        v = np.minimum(np.abs(v), 8159) + 33                  # 33 .. 8192
+        seg = (v[:, None] >= (0x40 << np.arange(8))).sum(axis=1)
+        code = np.where(seg >= 8, 0x7F, (np.minimum(seg, 7) << 4) | ((v >> (np.minimum(seg, 7) + 1)) & 0xF))
+    else:
+        v = v >> 3                                            # 13 bits
+        mask = np.where(v < 0, 0x55, 0xD5)
+        v = np.where(v < 0, -v - 1, v)                        # 0 .. 4095
+        seg = (v[:, None] >= (0x20 << np.arange(8))).sum(axis=1)
+        code = (seg << 4) | ((v >> np.maximum(seg, 1)) & 0xF)
+    return (code ^ mask).astype(np.uint8)
+
+
+def g711_wave_bytes(data: bytes, encoding: str, sample_rate: int) -> bytes:
+    """A mono 8-bit G.711 WAV file holding `data`: an 18-byte `fmt ` chunk (WAVE_FORMAT_MULAW or WAVE_FORMAT_ALAW,
+    block align 1, cbSize 0), a `fact` chunk with the sample count, and the `data` chunk (padded to an even length).
+    Python's `wave` module writes PCM only."""
+    check_encoding(encoding)
+    n = len(data)
+    fmt = struct.pack("<HHIIHHH", G711_WAVE_TAG[encoding], 1, int(sample_rate), int(sample_rate), 1, 8, 0)
+    body = (b"WAVE" + b"fmt " + struct.pack("<I", len(fmt)) + fmt + b"fact" + struct.pack("<II", 4, n)
+            + b"data" + struct.pack("<I", n) + bytes(data) + (b"\0" if n % 2 else b""))
+    return b"RIFF" + struct.pack("<I", len(body)) + body
+
 
 class AudioSamples:
     """struct AudioSamples(Vec<f32>) (audio/ops/src/samples.rs:16-18)."""
@@ -124,6 +172,14 @@ class AudioSamples:
     def as_wave_bytes(self, fixed_scale: bool = False) -> bytes:
         """16-bit little-endian PCM, peak-normalised (to_i16_vec), or at the fixed scale (to_i16_fixed)."""
         return (self.to_i16_fixed() if fixed_scale else self.to_i16_vec()).astype("<i2").tobytes()
+
+    def as_g711_bytes(self, law: str, fixed_scale: bool = False) -> bytes:
+        """G.711 ("mulaw" or "alaw") of the 16-bit samples as_wave_bytes holds, one byte per sample: what the library's
+        G.711 results are, computed here on the host."""
+        check_encoding(law)
+        if law is None:
+            raise OperationError("law None is neither 'mulaw' nor 'alaw'")
+        return g711_encode(self.to_i16_fixed() if fixed_scale else self.to_i16_vec(), law).tobytes()
 
     def merge(self, other: "AudioSamples") -> None:
         self._v = np.concatenate([self._v, other._v])

@@ -406,20 +406,45 @@ int32_t sb200_job_fetch_i16(sb200_job* job, int16_t** outs, size_t* lens, sb200_
     });
 }
 void sb200_i16_free(int16_t* p) { free(p); }
+int32_t sb200_job_fetch_g711(sb200_job* job, int32_t law, const float* gains, uint8_t** outs, size_t* lens,
+                             sb200_error* err) {
+    return guarded(err, [&] {
+        Job& j = *job->j;
+        g711_format(law, "");
+        if (!j.ran || j.encode_only) throw Error(19, "job has not produced audio");
+        if (!outs || !lens) throw Error(19, "null argument");
+        SB_CUDA(cudaSetDevice(j.v->device));
+        PinnedBlock* blk = pin_acquire((size_t)j.out_total + 16);
+        uint8_t* h = reinterpret_cast<uint8_t*>(blk->base);
+        try { job_g711_to_host(j, law, gains, h); } catch (...) { pin_release(blk); throw; }
+        for (size_t b = 0; b < j.B; b++) {
+            const size_t n = (size_t)j.osegs[b].len * j.out_hop;
+            outs[b] = (uint8_t*)malloc(n + 1);
+            memcpy(outs[b], h + j.osegs[b].out_off, n);
+            lens[b] = n;
+        }
+        pin_release(blk);
+    });
+}
+void sb200_bytes_free(uint8_t* p) { free(p); }
 
 int32_t sb200_job_copy_out(sb200_job* job, void* dst, size_t cap, int32_t format, size_t* written, sb200_error* err) {
     return guarded(err, [&] {
         Job& j = *job->j;
+        if (format < PCM_F32 || format > PCM_ALAW)
+            throw Error(19, "format " + std::to_string(format) + " is not 0 (f32), 1 (i16), 2 (mu-law) or 3 (A-law)");
         if (!j.ran || j.encode_only) throw Error(19, "job has not produced audio");
         if (!dst) throw Error(19, "null destination");
         Voice& v = *j.v;
         SB_CUDA(cudaSetDevice(v.device));
         cudaStream_t st = j.ctx->stream;
         const size_t n = (size_t)j.out_total;
-        const size_t bytes = n * (format == 1 ? 2 : 4);
+        const size_t bytes = n * pcm_bytes(format);
         if (bytes > cap) throw Error(19, "destination buffer is too small for the synthesis result");
-        if (format == 1) {
+        if (format == PCM_I16) {
             job_i16_to_host(j, 1.f, static_cast<int16_t*>(dst));
+        } else if (format != PCM_F32) {
+            job_g711_to_host(j, format == PCM_MULAW ? G711_MULAW : G711_ALAW, nullptr, static_cast<uint8_t*>(dst));
         } else {
             SB_CUDA(cudaMemcpyAsync(dst, j.d_wav, bytes, cudaMemcpyDeviceToHost, st));
             SB_CUDA(cudaStreamSynchronize(st));
@@ -543,6 +568,19 @@ int32_t sb200_decode_chunks_i16(sb200_voice* v, const sb200_latent* const* zs, c
     });
 }
 
+int32_t sb200_decode_chunks_g711(sb200_voice* v, const sb200_latent* const* zs, const int64_t* lo, const int64_t* hi,
+                                 const int64_t* trim_lo_frames, const int64_t* trim_hi_frames, size_t n, int32_t fade,
+                                 const float* gain, int32_t law, uint8_t** outs, size_t* lens, sb200_error* err) {
+    return guarded(err, [&] {
+        const int fmt = g711_format(law, "");
+        ChunkPass p = chunk_pass(zs, lo, hi, n, trim_lo_frames, trim_hi_frames, gain);
+        p.fade = fade; p.format = fmt;
+        ChunkResult r;
+        decode_chunks(v->v.get(), p, r);
+        copy_out(r.g711, outs, lens);
+    });
+}
+
 int32_t sb200_resampler_create(sb200_voice* v, uint32_t out_rate, sb200_resampler** out, sb200_error* err) {
     return guarded(err, [&] {
         if (!v || !out) throw Error(19, "null argument");
@@ -565,7 +603,9 @@ int32_t sb200_decode_chunks_resampled(sb200_voice* v, const sb200_latent* const*
         p.fade = fade; p.resample = true; p.format = format;
         ChunkResult r;
         decode_chunks(v->v.get(), p, r);
-        if (format == 1) copy_out(r.i16, outs, lens); else copy_out(r.f32, outs, lens);
+        if (format == PCM_I16) copy_out(r.i16, outs, lens);
+        else if (format == PCM_F32) copy_out(r.f32, outs, lens);
+        else copy_out(r.g711, outs, lens);
     });
 }
 
@@ -833,6 +873,25 @@ int32_t sb200_debug_loudness(int32_t device, const float* x, size_t n, int32_t r
         launch_loudness(dx, ds, 1, scratch, dl, dg, 0);
         SB_CUDA(cudaDeviceSynchronize());
         SB_CUDA(cudaMemcpy(lufs, dl, sizeof(double), cudaMemcpyDeviceToHost));
+    });
+}
+
+int32_t sb200_debug_g711(int32_t device, int32_t law, const int16_t* x, size_t n, uint8_t* out, sb200_error* err) {
+    return guarded(err, [&] {
+        const int fmt = g711_format(law, "");
+        if ((!x || !out) && n > 0) throw Error(19, "debug g711: null buffer");
+        if (device < 0) {
+            for (size_t i = 0; i < n; i++) out[i] = fmt == PCM_MULAW ? g711_ulaw(x[i]) : g711_alaw(x[i]);
+            return;
+        }
+        if (n == 0) return;
+        SB_CUDA(cudaSetDevice(device));
+        DeviceBuffers d;
+        const short* dx = d.upload(reinterpret_cast<const short*>(x), n, n);
+        uint8_t* dy = d.alloc<uint8_t>(n);
+        launch_g711(dx, (long long)n, fmt, dy, 0);
+        SB_CUDA(cudaDeviceSynchronize());
+        SB_CUDA(cudaMemcpy(out, dy, n, cudaMemcpyDeviceToHost));
     });
 }
 

@@ -192,9 +192,39 @@ void launch_conv_post(const float* x, int C, const float* w /*[7][C]*/, float* w
 // crossfade table of fade_n <= 48 entries, linear gain.  Default = plain to_i16_vec.  fixed_scale = 1 converts at the
 // fixed scale 32767 instead of the segment's peak (loudness-normalised utterances).
 struct PcmPost { float gain = 1.f; int fade_n = 0; long long trim_lo = 0, trim_hi = 0; float tab[48] = {0}; int fixed_scale = 0; };
-// posts: device array, one entry per segment; max_samples: the longest segment (before trimming), sizes the grid
-void launch_i16(const float* wav, const FrameSeg* fsegs, const PcmPost* posts, int nseg, int hop, long long max_samples,
-                unsigned* maxbits, short* out, cudaStream_t st);
+// Output formats of a result: 0 f32, 1 i16 PCM, 2 G.711 mu-law, 3 G.711 A-law (one byte per sample).
+enum PcmFormat { PCM_F32 = 0, PCM_I16 = 1, PCM_MULAW = 2, PCM_ALAW = 3 };
+inline size_t pcm_bytes(int fmt) { return fmt == PCM_F32 ? 4 : fmt == PCM_I16 ? 2 : 1; }
+// G.711 of one 16-bit sample, as CPython's audioop.lin2ulaw / lin2alaw (the Sun g711.c lineage) compute it.
+// mu-law: the sample >> 2 (14 bits), clipped to +-8159, biased by 33, segment from its leading bit, one's complement.
+__host__ __device__ inline uint8_t g711_ulaw(int16_t x) {
+    int v = x >> 2;                             // arithmetic shift
+    int mask = 0xFF;
+    if (v < 0) { v = -v; mask = 0x7F; }
+    if (v > 8159) v = 8159;
+    v += 33;                                    // 33 <= v <= 8192
+    int seg = 0;
+    while (seg < 8 && v >= (0x40 << seg)) seg++; // segment ends 0x3F, 0x7F, .., 0x1FFF
+    if (seg >= 8) return (uint8_t)(0x7F ^ mask);
+    return (uint8_t)((((seg << 4) | ((v >> (seg + 1)) & 0xF))) ^ mask);
+}
+// A-law: the sample >> 3 (13 bits), segment and mantissa, even bits inverted (XOR 0x55; 0xD5 also sets the sign bit).
+__host__ __device__ inline uint8_t g711_alaw(int16_t x) {
+    int v = x >> 3;
+    int mask = 0xD5;
+    if (v < 0) { v = -v - 1; mask = 0x55; }    // 0 <= v <= 4095
+    int seg = 0;
+    while (seg < 8 && v >= (0x20 << seg)) seg++; // segment ends 0x1F, 0x3F, .., 0xFFF
+    if (seg >= 8) return (uint8_t)(0x7F ^ mask);
+    const int aval = (seg << 4) | ((seg < 2 ? v >> 1 : v >> seg) & 0xF);
+    return (uint8_t)(aval ^ mask);
+}
+// posts: device array, one entry per segment; max_samples: the longest segment (before trimming), sizes the grid.
+// fmt: PCM_I16 writes short, PCM_MULAW / PCM_ALAW write the G.711 byte of that same short (out is uint8_t).
+void launch_pcm(const float* wav, const FrameSeg* fsegs, const PcmPost* posts, int nseg, int hop, long long max_samples,
+                unsigned* maxbits, int fmt, void* out, cudaStream_t st);
+// out[i] = the G.711 byte (fmt PCM_MULAW / PCM_ALAW) of x[i], i < n: the encoders on the device over a plain buffer.
+void launch_g711(const short* x, long long n, int fmt, uint8_t* out, cudaStream_t st);
 // Polyphase resampling of one segment (resample_poly's sum, kernels_misc.cu resample_kernel): n_out outputs at
 // out[out_off ..), from the segment's samples as pcm_value reads them.  taps: phase-major [up][K], taps[p][k] =
 // h[p + k*up] (0 past 2H).  up == 0: the segment is copied unchanged.  A stream's chunk continues its stream: the

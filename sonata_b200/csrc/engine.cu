@@ -438,7 +438,8 @@ struct ResamplePlan {
 };
 
 // Device tables of a resample launch and their pinned mirrors: the segments, identity posts (for a launch whose input
-// has no post-path, or for the i16 conversion of its output) and the output segments, n_out samples at out_off.
+// has no post-path, or for the i16 conversion of its output; out_gain[k], when given, is output k's gain there) and the
+// output segments, n_out samples at out_off.
 struct ResampleTables {
     ResampleSeg *segs, *segs_h; PcmPost *posts, *posts_h; FrameSeg *osegs, *osegs_h;
     void carve(Arena& dev, Arena& pin, size_t n) {
@@ -446,11 +447,12 @@ struct ResampleTables {
         posts = dev.get<PcmPost>(n); posts_h = pin.get<PcmPost>(n);
         osegs = dev.get<FrameSeg>(n); osegs_h = pin.get<FrameSeg>(n);
     }
-    void upload(const ResamplePlan& p, cudaStream_t st) {
+    void upload(const ResamplePlan& p, cudaStream_t st, const std::vector<float>* out_gain = nullptr) {
         const size_t n = p.segs.size();
         for (size_t k = 0; k < n; k++) {
             segs_h[k] = p.segs[k];
             posts_h[k] = PcmPost();
+            if (out_gain) posts_h[k].gain = (*out_gain)[k];
             osegs_h[k] = FrameSeg{0, (int)p.segs[k].n_out, 0, 0, p.segs[k].out_off};
         }
         h2d(segs, segs_h, n * sizeof(ResampleSeg), st);
@@ -557,7 +559,7 @@ struct FrameBufs {
 
 // One pass of streaming decoder chunks: speaker biases of every slot, tables, the gather table and the latent slices,
 // the decoder and the waveforms; the post-path table when an output stage runs, the resample launch's tables and
-// output, the i16 scratch; and the pinned block the packed result (`total` values) is copied to.
+// output, the i16 or G.711 scratch; and the pinned block the packed result (`total` values) is copied to.
 struct ChunkBufs {
     float* cond;
     int *sid, *sid_h;
@@ -567,11 +569,11 @@ struct ChunkBufs {
     DecoderBufs dec;
     PcmPost *post, *post_h;
     ResampleTables rt; float* rs;
-    short* i16; unsigned* max;
+    void* pcm; unsigned* max;
     void* out_h;
     void carve(Arena& dev, Arena& pin, const Job& j, const ChunkPass& p, const ResamplePlan& rp, size_t total) {
         const Voice& v = *j.v;
-        const bool multi = v.num_speakers > 1, i16_out = p.format == 1;
+        const bool multi = v.num_speakers > 1, i16_out = p.format != PCM_F32;
         const size_t n = j.fsegs.size(), nslots = j.slot_sid.size();
         cond = multi ? dev.get<float>(nslots * v.cond_rows) : nullptr;
         sid = multi ? dev.get<int>(nslots) : nullptr;
@@ -585,9 +587,9 @@ struct ChunkBufs {
         post_h = p.resample || i16_out ? pin.get<PcmPost>(n) : nullptr;
         rt.carve(dev, pin, rp.segs.size());
         rs = p.resample ? dev.get<float>(total + 4) : nullptr;
-        i16 = i16_out ? dev.get<short>(total + 8) : nullptr;
+        pcm = i16_out ? dev.alloc((total + 8) * pcm_bytes(p.format)) : nullptr;
         max = i16_out ? dev.get<unsigned>(n) : nullptr;
-        out_h = pin.alloc(total * (i16_out ? 2 : 4));
+        out_h = pin.alloc(total * pcm_bytes(p.format));
     }
 };
 
@@ -1144,14 +1146,15 @@ static void fill_fade(PcmPost& p, int fade, long long len) {
 }
 
 // The chunks are laid out as the segments of one frame level.  The pass runs the decoder, then its output stage: the
-// resample launch, which reads the waveforms through the post-path, and the i16 conversion, which applies the post-path
-// itself when no resample launch ran.  The packed result comes back in one copy through the context's page-locked
-// staging, and only then do the resamplers advance.
+// resample launch, which reads the waveforms through the post-path, and the i16 (or G.711) conversion, which applies the
+// post-path itself when no resample launch ran.  The packed result comes back in one copy through the context's
+// page-locked staging, and only then do the resamplers advance.
 void decode_chunks(Voice* v, const ChunkPass& p, ChunkResult& out) {
-    out.f32.clear(); out.i16.clear(); out.ms = 0.f;
+    out.f32.clear(); out.i16.clear(); out.g711.clear(); out.ms = 0.f;
     const size_t n = p.chunks.size();
     if (n == 0) return;
-    if (p.format != 0 && p.format != 1) throw Error(19, "format " + std::to_string(p.format) + " is neither 0 (f32) nor 1 (i16)");
+    if (p.format < PCM_F32 || p.format > PCM_ALAW)
+        throw Error(19, "format " + std::to_string(p.format) + " is not 0 (f32), 1 (i16), 2 (mu-law) or 3 (A-law)");
     const int hop = v->a.hop();
     Job j;
     std::vector<int> len(n);
@@ -1216,11 +1219,17 @@ void decode_chunks(Voice* v, const ChunkPass& p, ChunkResult& out) {
     h2d(b.src, b.src_h, n * sizeof(GatherSeg), st);
     launch_gather_rows(b.src, b.y.ftile, GY, j.RY, v->a.inter, b.s, st);
     run_decoder(R, LY, b.y, b.dec, b.s, b.wav);
+    // G.711 of resampled chunks: the gain scales the resampled samples just before the conversion, as a volume on the
+    // delivered audio (resampling x * g is not bit for bit resampling x, then times g)
+    const bool gain_after = p.resample && p.format >= PCM_MULAW;
+    std::vector<float> out_gain;
+    if (gain_after)
+        for (const ChunkSpec& c : p.chunks) out_gain.push_back(c.gain);
     if (b.post) {
         for (size_t k = 0; k < n; k++) {
             PcmPost& q = b.post_h[k];
             q = PcmPost();
-            q.gain = p.chunks[k].gain;
+            q.gain = gain_after ? 1.f : p.chunks[k].gain;
             q.trim_lo = p.chunks[k].trim_lo * hop;
             q.trim_hi = p.chunks[k].trim_hi * hop;
             if (p.fade > 0) fill_fade(q, p.fade, n_in[k]);
@@ -1228,16 +1237,16 @@ void decode_chunks(Voice* v, const ChunkPass& p, ChunkResult& out) {
         h2d(b.post, b.post_h, n * sizeof(PcmPost), st);
     }
     if (p.resample) {
-        b.rt.upload(rp, st);
+        b.rt.upload(rp, st, gain_after ? &out_gain : nullptr);
         run_resample(R, rp, b.rt, b.wav, b.y.fsegs, b.post, hop, b.rs);
-        if (b.i16) launch_i16(b.rs, b.rt.osegs, b.rt.posts, (int)n, 1, rp.max_out, b.max, b.i16, st);
-    } else if (b.i16) {
-        launch_i16(b.wav, b.y.fsegs, b.post, (int)n, hop, (long long)*std::max_element(len.begin(), len.end()) * hop,
-                   b.max, b.i16, st);
+        if (b.pcm) launch_pcm(b.rs, b.rt.osegs, b.rt.posts, (int)n, 1, rp.max_out, b.max, p.format, b.pcm, st);
+    } else if (b.pcm) {
+        launch_pcm(b.wav, b.y.fsegs, b.post, (int)n, hop, (long long)*std::max_element(len.begin(), len.end()) * hop,
+                   b.max, p.format, b.pcm, st);
     }
     SB_CUDA(cudaEventRecord(C.ev_end, st));
-    const void* res = b.i16 ? (const void*)b.i16 : b.rs ? (const void*)b.rs : (const void*)b.wav;
-    SB_CUDA(cudaMemcpyAsync(b.out_h, res, total * (b.i16 ? 2 : 4), cudaMemcpyDeviceToHost, st));
+    const void* res = b.pcm ? (const void*)b.pcm : b.rs ? (const void*)b.rs : (const void*)b.wav;
+    SB_CUDA(cudaMemcpyAsync(b.out_h, res, total * pcm_bytes(p.format), cudaMemcpyDeviceToHost, st));
     SB_CUDA(cudaStreamSynchronize(st));
     SB_CUDA(cudaGetLastError());
 
@@ -1251,13 +1260,16 @@ void decode_chunks(Voice* v, const ChunkPass& p, ChunkResult& out) {
         r->h = s.h_out;
         r->ended = p.chunks[k].last != 0;
     }
-    if (b.i16) out.i16.resize(n); else out.f32.resize(n);
+    if (p.format == PCM_I16) out.i16.resize(n); else if (b.pcm) out.g711.resize(n); else out.f32.resize(n);
     for (size_t k = 0; k < n; k++) {
         const long long o = p.resample ? rp.segs[k].out_off : j.fsegs[k].out_off;
         const long long m = p.resample ? rp.segs[k].n_out : n_in[k];
-        if (b.i16) {
+        if (p.format == PCM_I16) {
             const int16_t* h = static_cast<const int16_t*>(b.out_h);
             out.i16[k].assign(h + o, h + o + m);
+        } else if (b.pcm) {
+            const uint8_t* h = static_cast<const uint8_t*>(b.out_h);
+            out.g711[k].assign(h + o, h + o + m);
         } else {
             const float* h = static_cast<const float*>(b.out_h);
             out.f32[k].assign(h + o, h + o + m);
@@ -1266,32 +1278,57 @@ void decode_chunks(Voice* v, const ChunkPass& p, ChunkResult& out) {
     cudaEventElapsedTime(&out.ms, C.ev_begin, C.ev_end);
 }
 
-void job_i16_to_host(Job& j, float gain, int16_t* dst) {
+namespace {
+// The i16 conversion of a finished job in format `fmt` (PCM_I16 or a G.711 law), utterance b after gains[b].
+void job_pcm_to_host(Job& j, int fmt, const float* gains, void* dst) {
     if (!j.ran || j.encode_only) throw Error(19, "job has not produced audio");
     SB_CUDA(cudaSetDevice(j.v->device));
     cudaStream_t st = j.ctx->stream;
     const int hop = j.out_hop;
-    const size_t n = (size_t)j.out_total;
+    const size_t n = (size_t)j.out_total, bytes = pcm_bytes(fmt);
     long long mx = 0;
     for (size_t b = 0; b < j.B; b++) mx = std::max<long long>(mx, (long long)j.osegs[b].len * hop);
     // stream-ordered scratch, returned to the pool at once: device memory held after a run does not grow
-    short* d_i16 = nullptr; unsigned* d_max = nullptr; PcmPost* d_post = nullptr;
-    SB_CUDA(cudaMallocAsync(&d_i16, n * 2 + 16, st));
+    void* d_pcm = nullptr; unsigned* d_max = nullptr; PcmPost* d_post = nullptr;
+    SB_CUDA(cudaMallocAsync(&d_pcm, n * bytes + 16, st));
     SB_CUDA(cudaMallocAsync(&d_max, sizeof(unsigned) * j.B, st));
     SB_CUDA(cudaMallocAsync(&d_post, sizeof(PcmPost) * j.B, st));
-    PcmPost post; post.gain = gain;
-    std::vector<PcmPost> posts(j.B, post);
+    std::vector<PcmPost> posts(j.B);
+    for (size_t b = 0; b < j.B; b++) posts[b].gain = gains[b];
     // a loudness-normalised utterance keeps its level: fixed scale instead of its own peak
     for (size_t b = 0; b < j.loud_ran.size(); b++) posts[b].fixed_scale = std::isnan(j.loud_ran[b]) ? 0 : 1;
     // pageable source: the call returns once the entries are staged, so `posts` may go out of scope before the copy runs
     SB_CUDA(cudaMemcpyAsync(d_post, posts.data(), sizeof(PcmPost) * j.B, cudaMemcpyHostToDevice, st));
-    launch_i16(j.d_wav, j.d_osegs, d_post, (int)j.B, hop, mx, d_max, d_i16, st);
-    cudaError_t e = cudaMemcpyAsync(dst, d_i16, n * 2, cudaMemcpyDeviceToHost, st);
-    cudaFreeAsync(d_i16, st);
+    launch_pcm(j.d_wav, j.d_osegs, d_post, (int)j.B, hop, mx, d_max, fmt, d_pcm, st);
+    cudaError_t e = cudaMemcpyAsync(dst, d_pcm, n * bytes, cudaMemcpyDeviceToHost, st);
+    cudaFreeAsync(d_pcm, st);
     cudaFreeAsync(d_max, st);
     cudaFreeAsync(d_post, st);
     if (e == cudaSuccess) e = cudaStreamSynchronize(st);
     if (e != cudaSuccess) throw Error(19, std::string("CUDA error: ") + cudaGetErrorString(e));
+}
+}  // namespace
+
+void job_i16_to_host(Job& j, float gain, int16_t* dst) {
+    const std::vector<float> gains(j.B, gain);
+    job_pcm_to_host(j, PCM_I16, gains.data(), dst);
+}
+
+int g711_format(long long law, const std::string& who) {
+    if (law != G711_MULAW && law != G711_ALAW)
+        throw Error(19, who + "G.711 law " + std::to_string(law) + " is neither 0 (mu-law) nor 1 (A-law)");
+    return law == G711_MULAW ? PCM_MULAW : PCM_ALAW;
+}
+
+void job_g711_to_host(Job& j, int law, const float* gains, uint8_t* dst) {
+    const int fmt = g711_format(law, "");
+    std::vector<float> g(j.B, 1.f);
+    for (size_t b = 0; gains && b < j.B; b++) {
+        if (!std::isfinite(gains[b]))
+            throw Error(19, "utterance " + std::to_string(b) + ": gain " + std::to_string(gains[b]) + " is not finite");
+        g[b] = gains[b];
+    }
+    job_pcm_to_host(j, fmt, g.data(), dst);
 }
 
 // Peak-normalised 16-bit PCM of every utterance of a finished job, through the context's page-locked staging buffer.

@@ -341,18 +341,20 @@ struct ChunkSpec {
 // crossfade(fade) (samples.rs:144-157), the gain.  With `resample` the chunk is then appended to its stream's resampler,
 // emitting every output it can (a chunk without one leaves at the voice's rate as the post-path leaves it); a resampler
 // may appear once per pass and must belong to the voice.  i16: to_i16_vec (samples.rs:51-75) normalised to each emitted
-// chunk's own peak.  Every check runs before any device work and any resampler changes; errors name the chunk, except
-// with `single`, which keeps the single-chunk entry point's messages.
+// chunk's own peak; mu-law / A-law: the G.711 bytes of those same i16 samples, from the same launches.  Every check runs
+// before any device work and any resampler changes; errors name the chunk, except with `single`, which keeps the
+// single-chunk entry point's messages.
 struct ChunkPass {
     std::vector<ChunkSpec> chunks;
     int fade = 0;
     bool resample = false;
-    int format = 0;                       // 0: f32, 1: i16
+    int format = 0;                       // PcmFormat: 0 f32, 1 i16, 2 mu-law, 3 A-law
     bool single = false;
 };
 struct ChunkResult {
     std::vector<std::vector<float>> f32;      // format 0
     std::vector<std::vector<int16_t>> i16;    // format 1
+    std::vector<std::vector<uint8_t>> g711;   // formats 2 and 3
     float ms = 0;                             // the pass's device time
 };
 void decode_chunks(Voice* v, const ChunkPass& p, ChunkResult& out);
@@ -362,5 +364,13 @@ void job_pcm16(Job& j, float gain, std::vector<std::vector<int16_t>>& out);
 // device and copied to `dst`: total_samples values laid out like the job's waveforms, in host memory that is best
 // page-locked (a DMA copy).  An utterance the last run gave a loudness target converts at the fixed scale 32767.
 void job_i16_to_host(Job& j, float gain, int16_t* dst);
+// G.711 laws of the C ABI.
+constexpr int G711_MULAW = 0, G711_ALAW = 1;
+// The PcmFormat of G.711 law `law`; throws OPERATION_ERROR prefixed by `who` for any other value.
+int g711_format(long long law, const std::string& who);
+// job_i16_to_host's samples, utterance b after gains[b] (null: 1; each must be finite), encoded with G.711 law `law`
+// in the same launches: one byte per sample in `dst`, laid out like the job's waveforms.  A bad law or gain fails
+// before anything runs.
+void job_g711_to_host(Job& j, int law, const float* gains, uint8_t* dst);
 
 }  // namespace sb200

@@ -698,18 +698,26 @@ __global__ void i16_absmax_kernel(const float* __restrict__ wav, const FrameSeg*
                                                                                                   // order like their bits
 }
 
+// FMT: PCM_I16 stores the 16-bit sample; PCM_MULAW / PCM_ALAW store the G.711 byte of that same sample (common.cuh),
+// so an encoded result is the i16 result encoded, at half its bytes.
+template <int FMT> struct PcmOut { using T = uint8_t; };
+template <> struct PcmOut<PCM_I16> { using T = short; };
+template <int FMT>
 __global__ void i16_convert_kernel(const float* __restrict__ wav, const FrameSeg* __restrict__ fsegs,
                                    const PcmPost* __restrict__ posts, int hop, const unsigned* __restrict__ maxbits,
-                                   short* __restrict__ out) {
+                                   typename PcmOut<FMT>::T* __restrict__ out) {
     pdl_trigger(); pdl_wait();
     const FrameSeg fs = fsegs[blockIdx.y];
     const PcmSeg s = pcm_seg(wav, fs, posts + blockIdx.y, hop);
-    short* y = out + fs.out_off;
+    typename PcmOut<FMT>::T* y = out + fs.out_off;
     const float amax = fmaxf(__uint_as_float(maxbits[blockIdx.y]), 1.1920928955078125e-07f);
     const float scale = posts[blockIdx.y].fixed_scale ? 32767.0f : __fdiv_rn(32767.0f, amax);
     for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < s.n; i += (long long)gridDim.x * blockDim.x) {
         const float v = fminf(fmaxf(__fmul_rn(pcm_value(s, i), scale), -32768.0f), 32767.0f);
-        y[i] = (short)(int)v;                      // truncating cast
+        const short q = (short)(int)v;             // truncating cast
+        if constexpr (FMT == PCM_I16) y[i] = q;
+        else if constexpr (FMT == PCM_MULAW) y[i] = g711_ulaw(q);
+        else y[i] = g711_alaw(q);
     }
 }
 
@@ -1156,8 +1164,9 @@ void launch_conv_post(const float* x, int C, const float* w, float* wav, const F
     g_launch_count++;
 }
 
-void launch_i16(const float* wav, const FrameSeg* fsegs, const PcmPost* posts, int nseg, int hop, long long max_samples,
-                unsigned* maxbits, short* out, cudaStream_t st) {
+void launch_pcm(const float* wav, const FrameSeg* fsegs, const PcmPost* posts, int nseg, int hop, long long max_samples,
+                unsigned* maxbits, int fmt, void* out, cudaStream_t st) {
+    if (fmt != PCM_I16 && fmt != PCM_MULAW && fmt != PCM_ALAW) throw_launch_error("pcm: format is not i16 or G.711");
     if (nseg <= 0) return;
     cudaMemsetAsync(maxbits, 0, sizeof(unsigned) * nseg, st);
     int bx = (int)((max_samples + 256 * 8 - 1) / (256 * 8));
@@ -1165,8 +1174,26 @@ void launch_i16(const float* wav, const FrameSeg* fsegs, const PcmPost* posts, i
     if (bx > 1024) bx = 1024;
     dim3 grid(bx, nseg);
     launch_pdl(i16_absmax_kernel, dim3(grid), dim3(256), 0, st, wav, fsegs, posts, hop, maxbits);
-    launch_pdl(i16_convert_kernel, dim3(grid), dim3(256), 0, st, wav, fsegs, posts, hop, maxbits, out);
+    if (fmt == PCM_I16)
+        launch_pdl(i16_convert_kernel<PCM_I16>, dim3(grid), dim3(256), 0, st, wav, fsegs, posts, hop, maxbits, (short*)out);
+    else if (fmt == PCM_MULAW)
+        launch_pdl(i16_convert_kernel<PCM_MULAW>, dim3(grid), dim3(256), 0, st, wav, fsegs, posts, hop, maxbits, (uint8_t*)out);
+    else
+        launch_pdl(i16_convert_kernel<PCM_ALAW>, dim3(grid), dim3(256), 0, st, wav, fsegs, posts, hop, maxbits, (uint8_t*)out);
     g_launch_count += 2;
+}
+
+// One thread per value: the G.711 byte of x[i] (sb200_debug_g711's device side).
+__global__ void g711_kernel(const short* __restrict__ x, long long n, int fmt, uint8_t* __restrict__ out) {
+    pdl_trigger(); pdl_wait();
+    for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x)
+        out[i] = fmt == PCM_MULAW ? g711_ulaw(x[i]) : g711_alaw(x[i]);
+}
+void launch_g711(const short* x, long long n, int fmt, uint8_t* out, cudaStream_t st) {
+    if (n <= 0) return;
+    const long long bx = std::min<long long>((n + 255) / 256, 4096);
+    launch_pdl(g711_kernel, dim3((unsigned)bx), dim3(256), 0, st, x, n, fmt, out);
+    g_launch_count++;
 }
 
 void launch_resample(const float* wav, const FrameSeg* fsegs, const PcmPost* posts, int hop, const ResampleSeg* segs,

@@ -9,9 +9,9 @@ from typing import List, Optional, Sequence, Tuple
 import numpy as np
 
 from . import _native as N
-from .core import Audio
-from .piper import (_check, _config_array, _duration_arrays, _loudness_array, _ptr, _rate_array, _seed_arrays,
-                    _take_audio)
+from .core import G711_LAW, Audio, OperationError, check_encoding
+from .piper import (_check, _config_array, _duration_arrays, _gain_array, _loudness_array, _ptr, _rate_array,
+                    _seed_arrays, _take_audio, _take_bytes)
 
 
 class SynthesisJob:
@@ -156,9 +156,22 @@ class SynthesisJob:
             self._lib.sb200_i16_free(outs[i])
         return res
 
+    def fetch_g711(self, law: str, gains: Optional[Sequence] = None) -> List[bytes]:
+        """Per-utterance G.711 bytes ("mulaw" or "alaw"), one per sample: the encoding of exactly what fetch_i16
+        returns, after gains[b] (None: 1), computed on the device in the i16 conversion's launches."""
+        if law is None or check_encoding(law) is None:
+            raise OperationError(f"law {law!r} is neither 'mulaw' nor 'alaw'")
+        g = _gain_array(gains, self.batch)
+        outs = (C.POINTER(C.c_uint8) * self.batch)()
+        lens = (C.c_size_t * self.batch)()
+        err = N.sb200_error()
+        _check(self._lib.sb200_job_fetch_g711(self._h, G711_LAW[law], _ptr(g, C.c_float), outs, lens, C.byref(err)), err)
+        return _take_bytes(self._lib, outs, lens)
+
     def copy_out(self, dst_address: int, capacity_bytes: int, fmt: int = 0) -> int:
         """Device -> host copy of the whole result (utterances back to back) into caller memory, e.g. a slice of the
-        host segment shared by the ranks of one frontend; fmt 0 = f32, 1 = peak-normalised i16 PCM.  Returns bytes."""
+        host segment shared by the ranks of one frontend; fmt 0 = f32, 1 = peak-normalised i16 PCM, 2 / 3 = G.711
+        mu-law / A-law of those i16 samples (one byte each).  Returns bytes."""
         wr, err = C.c_size_t(), N.sb200_error()
         _check(self._lib.sb200_job_copy_out(self._h, C.c_void_p(dst_address), capacity_bytes, fmt, C.byref(wr),
                                             C.byref(err)), err)

@@ -17,8 +17,8 @@ from typing import Iterator, List, Optional, Sequence, Tuple
 import numpy as np
 
 from . import _native as N
-from .core import (Audio, AudioInfo, AudioSamples, OperationError, PhonemeAlignment, Phonemes, PhonemizationError,
-                   SonataError)
+from .core import (G711_LAW, Audio, AudioInfo, AudioSamples, OperationError, PhonemeAlignment, Phonemes,
+                   PhonemizationError, SonataError, check_encoding)
 
 MIN_CHUNK_SIZE = 44      # piper/src/lib.rs:18
 MAX_CHUNK_SIZE = 1024    # piper/src/lib.rs:19
@@ -179,6 +179,30 @@ def _loudness_array(targets, n: int):
     return None if np.isnan(out).all() else out
 
 
+def _encoding_list(law, n: int) -> list:
+    """One G.711 encoding ("mulaw" / "alaw") per utterance from `law`: one encoding for all, or one per utterance.  A bad
+    entry raises OperationError naming the utterance."""
+    laws = [law] * n if law is None or isinstance(law, str) else _per_utterance(law, n, "encodings")
+    for b, e in enumerate(laws):
+        if e is None or check_encoding(e, f"utterance {b}: ") is None:
+            raise OperationError(f"utterance {b}: encoding {e!r} is neither 'mulaw' nor 'alaw'")
+    return laws
+
+
+def _gain_array(gains, n: int):
+    """The C image of per-utterance linear gains (f32), or None when `gains` is None (1 for every utterance)."""
+    if gains is None:
+        return None
+    out = np.ones(n, np.float32)
+    for b, g in enumerate(_per_utterance(gains, n, "gains")):
+        if g is None:
+            continue
+        if isinstance(g, bool) or not isinstance(g, numbers.Real) or not math.isfinite(float(g)):
+            raise OperationError(f"utterance {b}: gain {g!r} is not a finite number")
+        out[b] = float(g)
+    return out
+
+
 def rate_ratio(in_rate: int, out_rate: Optional[int]) -> Tuple[int, int]:
     """(up, down): out_rate / in_rate reduced, (1, 1) for no resampling (None, 0 or the same rate)."""
     if not out_rate or int(out_rate) == int(in_rate):
@@ -249,6 +273,15 @@ def _take_chunks(lib, outs, lens, dtype) -> list:
         m = int(lens[k])
         res.append(np.ctypeslib.as_array(C.cast(outs[k], ptr), (m,)).copy() if m else np.zeros(0, dtype))
         lib.sb200_i16_free(C.cast(outs[k], C.POINTER(C.c_int16)))
+    return res
+
+
+def _take_bytes(lib, outs, lens) -> List[bytes]:
+    """Copies of the byte buffers `outs` (malloc'ed, lens[k] bytes each) as bytes; frees them."""
+    res = []
+    for k in range(len(lens)):
+        res.append(C.string_at(outs[k], int(lens[k])) if int(lens[k]) else b"")
+        lib.sb200_bytes_free(C.cast(outs[k], C.POINTER(C.c_uint8)))
     return res
 
 
@@ -535,6 +568,52 @@ class _VitsCommons:
         return [(audio, _alignment(ph, src, frames, len(audio), *ratio(audio)))
                 for ph, (_, src), (audio, frames) in zip(phoneme_batches, maps, res)]
 
+    def infer_batch_g711(self, batches: Sequence[Sequence[int]], law,
+                         configs: Optional[Sequence[PiperSynthesisConfig]] = None, seeds: Optional[Sequence] = None,
+                         output_rates: Optional[Sequence] = None, loudness: Optional[Sequence] = None,
+                         gains: Optional[Sequence] = None) -> List[bytes]:
+        """infer_batch_with_values delivered as G.711 telephony audio: one `bytes` per utterance, one byte per sample.
+        `law`: "mulaw" (PCMU) or "alaw" (PCMA), or one of those per utterance.  The bytes are G.711 of exactly the
+        16-bit samples the i16 route gives (SynthesisJob.fetch_i16): to_i16_vec of the utterance after gains[b] (None:
+        1), or the fixed scale for an utterance with a loudness target.  They are encoded on the device in the i16
+        conversion's launches, so only one byte per sample leaves the card.  `configs`, `seeds`, `output_rates` and
+        `loudness` as for infer_batch_with_values; a batch mixing laws runs one conversion per law."""
+        from .job import SynthesisJob
+        n = len(batches)
+        _config_array(configs, n)
+        _seed_arrays(seeds, n)
+        _rate_array(output_rates, n)
+        _loudness_array(loudness, n)
+        laws = _encoding_list(law, n)
+        _gain_array(gains, n)
+        if n == 0:
+            return []
+        if any(len(b) == 0 for b in batches):
+            raise OperationError("Failed to run model inference. Error: empty input sequence")
+        job = SynthesisJob(self, batches, configs=configs, seeds=seeds, output_rates=output_rates, loudness=loudness)
+        try:
+            job.run()
+            out: List[Optional[bytes]] = [None] * n
+            for e in dict.fromkeys(laws):
+                res = job.fetch_g711(e, gains)
+                for b in range(n):
+                    if laws[b] == e:
+                        out[b] = res[b]
+            return out
+        finally:
+            job.close()
+
+    def speak_batch_g711(self, phoneme_batches: Sequence[str], law,
+                         configs: Optional[Sequence[PiperSynthesisConfig]] = None, seeds: Optional[Sequence] = None,
+                         output_rates: Optional[Sequence] = None, loudness: Optional[Sequence] = None,
+                         gains: Optional[Sequence] = None) -> List[bytes]:
+        """speak_batch delivered as G.711 bytes: infer_batch_g711 over the phonemes' ids."""
+        n = len(phoneme_batches)
+        _config_array(configs, n)
+        _encoding_list(law, n)
+        return self.infer_batch_g711([self.phonemes_to_input_ids(p) for p in phoneme_batches], law, configs, seeds,
+                                     output_rates, loudness, gains)
+
     def _cfg(self, fn) -> PiperSynthesisConfig:
         c, err = N.sb200_synth_config(), N.sb200_error()
         _check(fn(self._h, C.byref(c), C.byref(err)), err)
@@ -647,20 +726,33 @@ def _trim_frames(trim: slice) -> Tuple[int, int]:
 
 class SpeechStreamer:
     """piper/src/lib.rs:765-858: chunked decoder runs with overlap trimming + crossfade(42).  With a resampler, each
-    chunk's trim and crossfade run on the device and the chunk leaves at the resampler's rate."""
+    chunk's trim and crossfade run on the device and the chunk leaves at the resampler's rate.  With an encoding, they
+    run on the device too and each chunk leaves as G.711 bytes of its to_i16_vec after `gain`."""
 
     def __init__(self, enc: EncoderOutputs, chunk_size: int, chunk_padding: int,
-                 resampler: Optional[Resampler] = None):
+                 resampler: Optional[Resampler] = None, encoding: Optional[str] = None, gain: float = 1.0):
         self.enc = enc
         self.chunker = AdaptiveMelChunker(enc.num_frames, chunk_size, chunk_padding)
         self.one_shot = enc.num_frames <= (chunk_size * 2 + chunk_padding * 2)
         self.resampler = resampler
+        self.encoding, self.gain = encoding, gain
 
     def __iter__(self) -> Iterator[AudioSamples]:
         return self
 
     def __next__(self) -> AudioSamples:
         (m0, m1), (a0, a1) = next(self.chunker)
+        if self.encoding is not None:
+            if self.one_shot:
+                self.chunker.consume()
+                chunk, fade = (self.enc, 0, self.enc.num_frames, 0, 0), 0
+            else:
+                hi = self.enc.num_frames if m1 is None else m1
+                chunk, fade = (self.enc, m0, hi) + _trim_frames(slice(a0, a1)), 42
+            rs = {} if self.resampler is None else {"resamplers": [self.resampler],
+                                                    "last": [self.chunker.last_end_index is None]}
+            return self.enc._m.infer_decoder_batch([chunk], fade=fade, gains=[self.gain], encoding=self.encoding,
+                                                   **rs)[0]
         if self.resampler is not None:
             if self.one_shot:
                 self.chunker.consume()
@@ -724,7 +816,7 @@ class VitsStreamingModel(_VitsCommons):
 
     def infer_decoder_batch(self, chunks: Sequence[tuple], pcm16: bool = False, fade: int = 0,
                             gains: Optional[Sequence[float]] = None, resamplers: Optional[Sequence] = None,
-                            last: Optional[Sequence[bool]] = None) -> list:
+                            last: Optional[Sequence[bool]] = None, encoding: Optional[str] = None) -> list:
         """Many `EncoderOutputs.infer_decoder(lo, hi)` calls as one decoder pass.  `chunks`: (encoder outputs, lo, hi)
         per chunk; each result equals that chunk decoded alone, bit for bit.
 
@@ -735,13 +827,20 @@ class VitsStreamingModel(_VitsCommons):
         With `resamplers` (one Resampler or None per chunk), chunks may carry trims in either format: after the same
         post-path each chunk is appended to its stream's resampler and the result is what that stream emits for it at
         its output rate (AudioSamples, or int16 normalised to the emitted samples' own peak with pcm16); last[k] flushes
-        the stream.  A None resampler returns the chunk after the post-path at the voice's rate."""
+        the stream.  A None resampler returns the chunk after the post-path at the voice's rate.
+
+        With `encoding` ("mulaw" or "alaw"; None: none), chunks take pcm16's tuples and each result is `bytes`: G.711 of
+        the int16 samples pcm16 returns for that chunk (with or without resamplers), encoded on the device in the same
+        launches."""
+        check_encoding(encoding)
+        if encoding is not None and pcm16:
+            raise OperationError("pcm16 and an encoding are two output formats: give one")
         n = len(chunks)
         lo, hi = np.zeros(n, np.int64), np.zeros(n, np.int64)
         tlo, thi = np.zeros(n, np.int64), np.zeros(n, np.int64)
         hs = (C.c_void_p * n)()
         for k, c in enumerate(chunks):
-            if len(c) not in ((3, 5) if pcm16 or resamplers is not None else (3,)):
+            if len(c) not in ((3, 5) if pcm16 or encoding or resamplers is not None else (3,)):
                 raise OperationError(f"Invalid decoder chunk {k}: expected (encoder outputs, lo, hi"
                                      + (", trim_lo, trim_hi)" if pcm16 else ")"))
             enc = c[0]
@@ -772,10 +871,20 @@ class VitsStreamingModel(_VitsCommons):
             _check(self._lib.sb200_decode_chunks_resampled(
                 self._h, hs, p64(lo), p64(hi), p64(tlo), p64(thi), n, int(fade),
                 None if g is None else g.ctypes.data_as(C.POINTER(C.c_float)), rs, _ptr(fl, C.c_int32),
-                1 if pcm16 else 0, outs, lens, C.byref(err)), err)
+                G711_LAW[encoding] + 2 if encoding else 1 if pcm16 else 0, outs, lens, C.byref(err)), err)
+            if encoding:
+                return _take_bytes(self._lib, outs, lens)
             if pcm16:
                 return _take_chunks(self._lib, outs, lens, np.int16)
             return [AudioSamples(a) for a in _take_chunks(self._lib, outs, lens, np.float32)]
+        if encoding:
+            g = None if gains is None else np.ascontiguousarray(gains, dtype=np.float32)
+            outs = (C.POINTER(C.c_uint8) * n)()
+            lens = (C.c_size_t * n)()
+            _check(self._lib.sb200_decode_chunks_g711(self._h, hs, p64(lo), p64(hi), p64(tlo), p64(thi), n, int(fade),
+                                                      None if g is None else g.ctypes.data_as(C.POINTER(C.c_float)),
+                                                      G711_LAW[encoding], outs, lens, C.byref(err)), err)
+            return _take_bytes(self._lib, outs, lens)
         if not pcm16:
             outs = (N.sb200_audio * n)()
             _check(self._lib.sb200_decode_chunks(self._h, hs, p64(lo), p64(hi), n, outs, C.byref(err)), err)
@@ -792,21 +901,37 @@ class VitsStreamingModel(_VitsCommons):
         return True
 
     def stream_synthesis(self, phonemes: str, chunk_size: int, chunk_padding: int,
-                         seed: Optional[int] = None, output_rate: Optional[int] = None) -> SpeechStreamer:
+                         seed: Optional[int] = None, output_rate: Optional[int] = None,
+                         encoding: Optional[str] = None, gain: Optional[float] = None) -> SpeechStreamer:
         """`seed`: the sentence's noise seed (see infer_batch_with_values), or None for positional noise.
-        `output_rate`: the chunks' sample rate (see infer_batch_with_values), the sentence resampled as one stream."""
+        `output_rate`: the chunks' sample rate (see infer_batch_with_values), the sentence resampled as one stream.
+        `encoding`: "mulaw" / "alaw" for chunks of G.711 `bytes`: each is G.711 of to_i16_vec of the chunk the stream
+        yields without an encoding, after the linear `gain` (None: 1; encoded streams only), encoded on the device."""
         _seed_arrays([seed], 1)
         _rate_array([output_rate], 1)
+        g = _stream_gain(encoding, gain)
         ids = self.phonemes_to_input_ids(phonemes)
         enc = self.infer_encoder(ids) if seed is None else self.infer_encoder_batch([ids], seeds=[seed])[0]
-        return SpeechStreamer(enc, chunk_size, chunk_padding, _stream_resampler(self, output_rate))
+        return SpeechStreamer(enc, chunk_size, chunk_padding, _stream_resampler(self, output_rate), encoding, g)
+
+
+def _stream_gain(encoding, gain) -> float:
+    """Checks a stream's encoding and gain; the gain as a float (1 when None)."""
+    check_encoding(encoding)
+    if gain is None:
+        return 1.0
+    if encoding is None:
+        raise OperationError("a stream's gain applies before its G.711 encoding: give an encoding with it")
+    return float(_gain_array([gain], 1)[0])
 
 
 class _Stream:
     """One sentence of a StreamBatch: its latent and its own chunk schedule, with SpeechStreamer's one-shot rule."""
 
-    def __init__(self, key, enc, chunk_size: int, chunk_padding: int, resampler: Optional[Resampler] = None):
+    def __init__(self, key, enc, chunk_size: int, chunk_padding: int, resampler: Optional[Resampler] = None,
+                 encoding: Optional[str] = None, gain: float = 1.0):
         self.key, self.enc, self.resampler = key, enc, resampler
+        self.encoding, self.gain = encoding, gain
         self.chunker = AdaptiveMelChunker(enc.num_frames, chunk_size, chunk_padding)
         self.one_shot = enc.num_frames <= (chunk_size * 2 + chunk_padding * 2)
 
@@ -841,7 +966,9 @@ class StreamBatch:
     crossfade(42), so its chunks are exactly what `stream_synthesis` yields for that sentence with its config as the
     fallback.  A stream added with an output rate has its own resampler: its chunks are trimmed, crossfaded and
     resampled on the device.  Those chunks go through a second decoder pass of the step (a third for one-shot ones,
-    which are not crossfaded), so the streams at the voice's rate keep their pass and their bits.
+    which are not crossfaded), so the streams at the voice's rate keep their pass and their bits.  A stream added with
+    an encoding yields G.711 `bytes` (see stream_synthesis); its chunks go through a pass per encoding, output rate or
+    not, and one-shot or not, with its trim, crossfade and gain on the device.
 
     One stream's failure stays that stream's, as with one `stream_synthesis` per client: when a batched pass raises,
     its streams are run one at a time, and a stream whose own encoder or decoder work fails gets its SonataError as
@@ -851,23 +978,24 @@ class StreamBatch:
         _check_chunking(chunk_size, chunk_padding)
         self.model = model
         self.chunk_size, self.chunk_padding = chunk_size, chunk_padding
-        self._pending: list = []      # (key, ids, config, chunk_size, seed, output rate) not yet encoded
+        self._pending: list = []      # (key, ids, config, chunk_size, seed, output rate, encoding, gain) not encoded yet
         self._active: List[_Stream] = []
         self._next_key = 0
 
     def add(self, ids_or_phonemes, config: Optional[PiperSynthesisConfig] = None, seed: Optional[int] = None,
-            output_rate: Optional[int] = None) -> int:
+            output_rate: Optional[int] = None, encoding: Optional[str] = None, gain: Optional[float] = None) -> int:
         """`seed`: the stream's noise seed (see infer_batch_with_values); a seeded stream yields what
-        `stream_synthesis(..., seed=seed)` yields, whatever other streams share its encoder pass.  `output_rate`: the
-        stream's sample rate, as for stream_synthesis."""
-        return self._add(ids_or_phonemes, config, self.chunk_size, seed, output_rate)
+        `stream_synthesis(..., seed=seed)` yields, whatever other streams share its encoder pass.  `output_rate`,
+        `encoding` and `gain`: the stream's sample rate and G.711 encoding, as for stream_synthesis."""
+        return self._add(ids_or_phonemes, config, self.chunk_size, seed, output_rate, encoding, gain)
 
     def _add(self, ids_or_phonemes, config, chunk_size: int, seed: Optional[int] = None,
-             output_rate: Optional[int] = None) -> int:
+             output_rate: Optional[int] = None, encoding: Optional[str] = None, gain: Optional[float] = None) -> int:
         if config is not None and not isinstance(config, PiperSynthesisConfig):
             raise OperationError("Invalid configuration for Vits Model")
         _seed_arrays([seed], 1)
         _rate_array([output_rate], 1)
+        gain = _stream_gain(encoding, gain)
         if config is not None and config.speaker is not None and config.speaker not in (self.model.get_speakers() or {}):
             raise OperationError(f"No speaker was found with the given id `{config.speaker}`")     # as check_config
         _check_chunking(chunk_size, self.chunk_padding)
@@ -879,7 +1007,7 @@ class StreamBatch:
             raise OperationError("Failed to run model inference. Error: empty input sequence")
         key = self._next_key
         self._next_key += 1
-        self._pending.append((key, ids, config, chunk_size, seed, output_rate))
+        self._pending.append((key, ids, config, chunk_size, seed, output_rate, encoding, gain))
         return key
 
     def __len__(self) -> int:
@@ -908,24 +1036,35 @@ class StreamBatch:
                 if err is None:
                     try:
                         active.append(_Stream(p[0], enc, p[3], self.chunk_padding,
-                                              _stream_resampler(self.model, p[5])))
+                                              _stream_resampler(self.model, p[5]), p[6], p[7]))
                         continue
                     except SonataError as e:
                         err = e
                 out.append((p[0], err))
         plan = [(s,) + s.next_chunk() for s in active]
         failed = set()
-        plain = [p for p in plan if p[0].resampler is None]
-        faded = [p for p in plan if p[0].resampler is not None and p[3] is not None]
-        whole = [p for p in plan if p[0].resampler is not None and p[3] is None]
+        # one pass per (encoding, resampled, one-shot): the streams without an encoding first, in their usual passes
+        plain_key = (None, False, False)
+        groups = {plain_key: [], (None, True, False): [], (None, True, True): []}
+        for p in plan:
+            s = p[0]
+            k = plain_key if s.encoding is None and s.resampler is None else (s.encoding, s.resampler is not None,
+                                                                                 p[3] is None)
+            groups.setdefault(k, []).append(p)
 
-        def resampled(pl, fade):
+        def device_post(pl, key):
+            encoding, resampled, whole = key
             chunks = [(s.enc, lo, hi) + ((0, 0) if trim is None else _trim_frames(trim)) for s, lo, hi, trim in pl]
-            return self.model.infer_decoder_batch(chunks, fade=fade, resamplers=[p[0].resampler for p in pl],
-                                                  last=[p[0].done for p in pl])
+            extra = {} if not resampled else {"resamplers": [p[0].resampler for p in pl], "last": [p[0].done for p in pl]}
+            if encoding is not None:
+                extra.update(encoding=encoding, gains=[p[0].gain for p in pl])
+            return self.model.infer_decoder_batch(chunks, fade=0 if whole else 42, **extra)
         decoded = {}
-        for group, call in ((plain, lambda pl: self.model.infer_decoder_batch([(s.enc, lo, hi) for s, lo, hi, _ in pl])),
-                            (faded, lambda pl: resampled(pl, 42)), (whole, lambda pl: resampled(pl, 0))):
+        for key, group in groups.items():
+            if key == plain_key:
+                call = lambda pl: self.model.infer_decoder_batch([(s.enc, lo, hi) for s, lo, hi, _ in pl])
+            else:
+                call = lambda pl, key=key: device_post(pl, key)
             if group:
                 decoded.update({id(p): r for p, r in zip(group, _each_or_alone(call, group))})
         for p in plan:
@@ -935,7 +1074,7 @@ class StreamBatch:
                 out.append((s.key, err))
                 failed.add(s.key)
                 continue
-            if trim is not None and s.resampler is None:
+            if trim is not None and s.resampler is None and s.encoding is None:
                 a = AudioSamples(a.as_slice()[trim])
                 a.crossfade(42)
             out.append((s.key, a))

@@ -24,7 +24,7 @@ from typing import Iterator, List, Optional
 
 import numpy as np
 
-from .core import Audio, AudioSamples, OperationError, SonataError
+from .core import G711_SILENCE, Audio, AudioSamples, OperationError, SonataError, check_encoding, g711_wave_bytes
 
 RATE_RANGE = (0.5, 5.5)      # synth/src/lib.rs:13
 VOLUME_RANGE = (0.0, 1.0)    # :14
@@ -66,6 +66,15 @@ class AudioOutputConfig:
     def generate_silence(self, time_ms: int, sample_rate: int) -> AudioSamples:
         return AudioSamples(np.zeros((time_ms * sample_rate) // 1000, dtype=np.float32))   # :107-116
 
+    def gain(self) -> Optional[float]:
+        """The linear gain of `volume`, or None without one."""
+        return None if self.volume is None else percent_to_param(self.volume, *VOLUME_RANGE)
+
+    def silence_bytes(self, sample_rate: int, encoding: str) -> bytes:
+        """The appended silence in G.711: the code of sample 0 (0xFF mu-law, 0xD5 A-law) per sample."""
+        n = (self.appended_silence_ms * sample_rate) // 1000 if self.appended_silence_ms else 0
+        return bytes([G711_SILENCE[encoding]]) * n
+
     def apply(self, audio: Audio) -> Audio:
         """synth/src/lib.rs:37-54: silence is appended first, then the whole buffer is processed."""
         s = audio.samples
@@ -102,6 +111,12 @@ def _check_loudness(target) -> None:
     _loudness_array([target], 1)
 
 
+def _device_g711(model) -> bool:
+    """Whether `model` encodes G.711 on the device (VitsModel / VitsStreamingModel).  Other SonataModels (fakes in
+    tests) get the host definition, AudioSamples.as_g711_bytes, of the audio they return."""
+    return hasattr(model, "speak_batch_g711")
+
+
 def _sentences(model, text: str) -> List[str]:
     """SpeechSynthesisTaskProvider::get_phonemes (:256-258), or newline-separated phoneme sentences when the model has
     no phonemizer."""
@@ -129,14 +144,47 @@ class SonataSpeechSynthesizer:
     # piper.OUTPUT_RATES (None / 0: the voice's), each sentence resampled on the device; appended silence is generated
     # at that rate.  `loudness` (lazy, parallel and file modes): a target integrated loudness in LUFS, [-70, 0], each
     # sentence measured and scaled to it on the device before the output config's volume and silence apply.
+    # `encoding` (every mode): "mulaw" / "alaw" hands out G.711 `bytes` instead of Audio / AudioSamples: G.711 of the
+    # 16-bit samples of what the mode hands out without it (to_i16_vec per sentence or chunk, or the fixed scale with a
+    # loudness target), the output config's volume applied on the device as a gain before the conversion and its
+    # silence appended as code-of-zero bytes.
+
+    def _g711_batch(self, phs: List[str], encoding: str, seeds, output_rate, loudness,
+                    cfg: Optional[AudioOutputConfig]) -> List[bytes]:
+        """The G.711 bytes of sentences `phs`, one synthesis pass, each followed by its appended silence."""
+        if cfg is not None:
+            cfg._check_supported()
+        n = len(phs)
+        extra = {} if seeds is None else {"seeds": seeds}
+        if output_rate:
+            extra["output_rates"] = [output_rate] * n
+        if loudness is not None:
+            extra["loudness"] = [loudness] * n
+        if not _device_g711(self.model):
+            res = self.model.speak_batch(phs, **extra) if extra else self.model.speak_batch(phs)
+            return [self._process(a, cfg).samples.as_g711_bytes(encoding, fixed_scale=loudness is not None)
+                    for a in res]
+        g = cfg.gain() if cfg is not None else None
+        if g is not None:
+            extra["gains"] = [g] * n
+        res = self.model.speak_batch_g711(phs, encoding, **extra)
+        if cfg is None:
+            return res
+        rate = output_rate or self.model.audio_output_info().sample_rate
+        return [r + cfg.silence_bytes(rate, encoding) for r in res]
 
     def synthesize_lazy(self, text: str, output_config: Optional[AudioOutputConfig] = None,
                         seed: Optional[int] = None, output_rate: Optional[int] = None,
-                        loudness: Optional[float] = None) -> Iterator[Audio]:
+                        loudness: Optional[float] = None, encoding: Optional[str] = None) -> Iterator[Audio]:
         sentence_seed(seed, 0)
         _check_output_rate(output_rate)
         _check_loudness(loudness)
+        check_encoding(encoding)
         for i, ph in enumerate(self._phonemes(text)):
+            if encoding is not None:
+                yield self._g711_batch([ph], encoding, None if seed is None else [sentence_seed(seed, i)], output_rate,
+                                       loudness, output_config)[0]
+                continue
             if output_rate or loudness is not None:
                 extra = {} if seed is None else {"seeds": [sentence_seed(seed, i)]}
                 if output_rate:
@@ -151,11 +199,15 @@ class SonataSpeechSynthesizer:
 
     def synthesize_parallel(self, text: str, output_config: Optional[AudioOutputConfig] = None,
                             seed: Optional[int] = None, output_rate: Optional[int] = None,
-                            loudness: Optional[float] = None) -> Iterator[Audio]:
+                            loudness: Optional[float] = None, encoding: Optional[str] = None) -> Iterator[Audio]:
         sentence_seed(seed, 0)
         _check_output_rate(output_rate)
         _check_loudness(loudness)
+        check_encoding(encoding)
         ph = self._phonemes(text)
+        if encoding is not None:
+            seeds = None if seed is None else [sentence_seed(seed, i) for i in range(len(ph))]
+            return iter(self._g711_batch(ph, encoding, seeds, output_rate, loudness, output_config) if ph else [])
         extra = {"output_rates": [output_rate] * len(ph)} if output_rate else {}
         if loudness is not None:
             extra["loudness"] = [loudness] * len(ph)
@@ -169,15 +221,32 @@ class SonataSpeechSynthesizer:
 
     def synthesize_streamed(self, text: str, output_config: Optional[AudioOutputConfig] = None,
                             chunk_size: int = 72, chunk_padding: int = 3,
-                            seed: Optional[int] = None, output_rate: Optional[int] = None) -> Iterator[AudioSamples]:
+                            seed: Optional[int] = None, output_rate: Optional[int] = None,
+                            encoding: Optional[str] = None) -> Iterator[AudioSamples]:
         """RealtimeSpeechStream (:337-382): a background producer pushes chunks into an unbounded channel;
         chunk_size is multiplied by the number of chunks already produced for every following sentence.
-        `output_rate`: each sentence is resampled as its own stream (zero history at its start, flushed at its end)."""
+        `output_rate`: each sentence is resampled as its own stream (zero history at its start, flushed at its end).
+        `encoding`: every chunk is G.711 bytes of its to_i16_vec after the volume, encoded on the device."""
         sentence_seed(seed, 0)
         _check_output_rate(output_rate)
+        check_encoding(encoding)
+        if encoding is not None and output_config is not None:
+            output_config._check_supported()
         sr = output_rate or self.model.audio_output_info().sample_rate
         rate = {"output_rate": output_rate} if output_rate else {}
+        device = encoding is not None and _device_g711(self.model)
+        if device:
+            rate["encoding"] = encoding
+            if output_config is not None and output_config.gain() is not None:
+                rate["gain"] = output_config.gain()
         extra = lambda i: dict(rate) if seed is None else dict(rate, seed=sentence_seed(seed, i))
+
+        def emit(chunk):
+            if encoding is None:
+                return output_config.apply_to_raw_samples(chunk) if output_config else chunk
+            if device:
+                return chunk
+            return (output_config.apply_to_raw_samples(chunk) if output_config else chunk).as_g711_bytes(encoding)
         q: "queue.Queue" = queue.Queue()
         done = object()
 
@@ -188,11 +257,12 @@ class SonataSpeechSynthesizer:
                     cs = next_chunk_size(cs, produced)
                     n = 0
                     for chunk in self.model.stream_synthesis(ph, cs, chunk_padding, **extra(i)):
-                        q.put(output_config.apply_to_raw_samples(chunk) if output_config else chunk)
+                        q.put(emit(chunk))
                         n += 1
                     produced += n
                     if output_config and output_config.appended_silence_ms:
-                        q.put(output_config.generate_silence(output_config.appended_silence_ms, sr))
+                        q.put(output_config.generate_silence(output_config.appended_silence_ms, sr) if encoding is None
+                              else output_config.silence_bytes(sr, encoding))
             except Exception as e:                                  # errors travel through the channel (:368-371)
                 q.put(e)
             q.put(done)
@@ -208,12 +278,21 @@ class SonataSpeechSynthesizer:
 
     def synthesize_to_file(self, filename, text: str, output_config: Optional[AudioOutputConfig] = None,
                            seed: Optional[int] = None, output_rate: Optional[int] = None,
-                           loudness: Optional[float] = None) -> None:
+                           loudness: Optional[float] = None, encoding: Optional[str] = None) -> None:
         """:168-198 — parallel mode, concatenated, peak-normalised i16 WAV (at output_rate when given).  With
-        `loudness` the WAV is written at the fixed scale (trunc(clamp(x * 32767))), so it keeps the sentences' level."""
+        `loudness` the WAV is written at the fixed scale (trunc(clamp(x * 32767))), so it keeps the sentences' level.
+        With `encoding` the WAV is 8-bit G.711 (WAVE_FORMAT_MULAW / _ALAW, with a `fact` chunk) holding the sentences'
+        bytes as synthesize_parallel hands them out: each sentence converted at its own peak (or the fixed scale)."""
         extra = {"output_rate": output_rate} if output_rate else {}
         if loudness is not None:
             extra["loudness"] = loudness
+        if check_encoding(encoding) is not None:
+            data = b"".join(self.synthesize_parallel(text, output_config, seed=seed, encoding=encoding, **extra))
+            if not data:
+                raise OperationError("No speech data to write")
+            with open(filename, "wb") as f:
+                f.write(g711_wave_bytes(data, encoding, output_rate or self.model.audio_output_info().sample_rate))
+            return
         parts = [a.samples.as_slice() for a in self.synthesize_parallel(text, output_config, seed=seed, **extra)]
         if not parts or sum(len(p) for p in parts) == 0:
             raise OperationError("No speech data to write")
@@ -232,9 +311,9 @@ class SonataSpeechSynthesizer:
 
 
 class _Request:
-    def __init__(self, key, ids, output_config, config, chunk_size, seed=None, output_rate=None):
+    def __init__(self, key, ids, output_config, config, chunk_size, seed=None, output_rate=None, encoding=None):
         self.key, self.ids, self.output_config, self.config, self.seed = key, ids, output_config, config, seed
-        self.output_rate = output_rate
+        self.output_rate, self.encoding = output_rate, encoding
         self.cs, self.produced, self.n, self.next = chunk_size, 0, 0, 0
 
 
@@ -259,11 +338,13 @@ class RealtimeBatch:
         self._next_key = 0
 
     def add(self, text: str, output_config: Optional[AudioOutputConfig] = None, config=None,
-            seed: Optional[int] = None, output_rate: Optional[int] = None) -> int:
-        """`seed`: the request's noise seed, `output_rate` its sample rate, as for synthesize_streamed."""
+            seed: Optional[int] = None, output_rate: Optional[int] = None, encoding: Optional[str] = None) -> int:
+        """`seed`: the request's noise seed, `output_rate` its sample rate and `encoding` its G.711 encoding, as for
+        synthesize_streamed."""
         from .piper import PiperSynthesisConfig
         sentence_seed(seed, 0)
         _check_output_rate(output_rate)
+        check_encoding(encoding)
         if output_config is not None:
             output_config._check_supported()
         if config is not None and not isinstance(config, PiperSynthesisConfig):
@@ -273,7 +354,7 @@ class RealtimeBatch:
         ids = [self.model.phonemes_to_input_ids(ph) for ph in _sentences(self.model, text)]
         if any(len(i) == 0 for i in ids):
             raise OperationError("Failed to run model inference. Error: empty input sequence")
-        req = _Request(self._next_key, ids, output_config, config, self.chunk_size, seed, output_rate or None)
+        req = _Request(self._next_key, ids, output_config, config, self.chunk_size, seed, output_rate or None, encoding)
         self._next_key += 1
         self._start_sentence(req)
         return req.key
@@ -284,6 +365,10 @@ class RealtimeBatch:
         req.cs = next_chunk_size(req.cs, req.produced)
         req.n = 0
         rate = {} if req.output_rate is None else {"output_rate": req.output_rate}
+        if req.encoding is not None:
+            rate["encoding"] = req.encoding
+            if req.output_config is not None and req.output_config.gain() is not None:
+                rate["gain"] = req.output_config.gain()
         self._by_stream[self._streams._add(req.ids[req.next], req.config, req.cs, sentence_seed(req.seed, req.next),
                                            **rate)] = req
         req.next += 1
@@ -301,13 +386,15 @@ class RealtimeBatch:
                 out.append((req.key, chunk))
                 continue
             oc = req.output_config
-            out.append((req.key, oc.apply_to_raw_samples(chunk) if oc else chunk))
+            out.append((req.key, chunk if req.encoding is not None or not oc else oc.apply_to_raw_samples(chunk)))
             req.n += 1
             if skey in self._streams:
                 continue
             del self._by_stream[skey]                  # the sentence is done
             req.produced += req.n
             if oc and oc.appended_silence_ms:
-                out.append((req.key, oc.generate_silence(oc.appended_silence_ms, req.output_rate or self._sr)))
+                sr = req.output_rate or self._sr
+                out.append((req.key, oc.generate_silence(oc.appended_silence_ms, sr) if req.encoding is None
+                            else oc.silence_bytes(sr, req.encoding)))
             self._start_sentence(req)
         return out
