@@ -273,6 +273,27 @@ void sb200_i16_free(int16_t* p);
 int32_t sb200_job_fetch_g711(sb200_job* job, int32_t law, const float* gains, uint8_t** outs, size_t* lens,
                              sb200_error* err);
 void sb200_bytes_free(uint8_t* p);
+/* Lossless FLAC, one complete native stream per utterance (RFC 9639, streamable subset; free with sb200_bytes_free).
+ * Its samples are exactly the i16 samples sb200_job_fetch_i16 returns, after utterance b is scaled by gains[b] (NULL =
+ * 1; each must be finite, as for sb200_job_fetch_g711), at the utterance's delivered sample rate.  The stream:
+ *   - `fLaC`, one metadata block header (last = 1, type 0 STREAMINFO, length 34), STREAMINFO: min = max block size
+ *     4096, the exact min / max frame size (0 without frames), the rate, 1 channel, 16 bits, the total samples and an
+ *     all-zero MD5 ("not computed");
+ *   - fixed-blocksize frames of 4096 samples (the last one shorter): sync 0xFFF8, block-size code 0b1100 (the last
+ *     frame: 0b0110 / 0b0111 with 8- / 16-bit size - 1), the rate's code (11025 Hz: 0b1101 with a 16-bit Hz field),
+ *     mono, 16 bits, the UTF-8-coded frame number and CRC-8;
+ *   - one subframe (no wasted bits): CONSTANT when every sample is equal, else the smallest of FIXED 0-4, LPC 1-8
+ *     (12-bit coefficients, shift 0..15) and VERBATIM, ties in that order; residuals in Rice partitions of order 0-8
+ *     with each partition's optimal parameter (method 0b00, or 0b01 when one exceeds 14), no escapes;
+ *   - zero padding to a byte and CRC-16.
+ * The analysis, layout and packing run on the device; the frame sizes come back first, then only the compressed bytes.
+ * A frame's bytes depend only on its samples and its position in its stream. */
+int32_t sb200_job_fetch_flac(sb200_job* job, const float* gains, uint8_t** outs, size_t* lens, sb200_error* err);
+/* The same encoder over a host buffer x[0 .. n) at sample_rate, on `device`: *out receives a malloc'ed stream of *len
+ * bytes (free with sb200_bytes_free); n = 0 gives the 42-byte header-only stream.  A rate other than the eight output
+ * rates (8000, 11025, 16000, 22050, 24000, 32000, 44100, 48000) fails with OPERATION_ERROR before any device work. */
+int32_t sb200_flac_encode(int32_t device, const int16_t* x, size_t n, uint32_t sample_rate, uint8_t** out, size_t* len,
+                          sb200_error* err);
 int32_t sb200_job_lengths(const sb200_job* job, int64_t* frames, int64_t* samples, int64_t* out_offsets);
 /* Copy the result of a finished job into CALLER-OWNED host memory, utterances back to back in batch order.
  * format 0: f32 samples (what infer_with_values returns, piper/src/lib.rs:382-392);

@@ -105,6 +105,10 @@ SIGNATURES = {
     "sb200_job_fetch_g711": (C.c_int32, [_P, C.c_int32, C.POINTER(C.c_float), C.POINTER(C.POINTER(C.c_uint8)),
                                          C.POINTER(C.c_size_t), _ERR]),
     "sb200_bytes_free": (None, [C.POINTER(C.c_uint8)]),
+    "sb200_job_fetch_flac": (C.c_int32, [_P, C.POINTER(C.c_float), C.POINTER(C.POINTER(C.c_uint8)),
+                                         C.POINTER(C.c_size_t), _ERR]),
+    "sb200_flac_encode": (C.c_int32, [C.c_int32, C.POINTER(C.c_int16), C.c_size_t, C.c_uint32,
+                                      C.POINTER(C.POINTER(C.c_uint8)), C.POINTER(C.c_size_t), _ERR]),
     "sb200_job_batch": (C.c_size_t, [_P]),
     "sb200_job_lengths": (C.c_int32, [_P, C.POINTER(C.c_int64), C.POINTER(C.c_int64), C.POINTER(C.c_int64)]),
     "sb200_job_copy_out": (C.c_int32, [_P, C.c_void_p, C.c_size_t, C.c_int32, C.POINTER(C.c_size_t), _ERR]),

@@ -8,7 +8,8 @@ Without `-f`, one JSON request per stdin line (fields of `SynthesisRequest`, mai
 LE PCM (peak-normalised per sentence / chunk like `as_wave_bytes`) goes to stdout; with `-o` and stdin requests the
 files are numbered `<stem>-<n>.<ext>` (main.rs:243-256).  `text` is phonemes, one sentence per line.  With
 `--encoding mulaw|alaw` (or a JSON "encoding") the output is G.711 instead, encoded on the GPU: raw bytes on stdout,
-or an 8-bit G.711 WAV with `-o`.
+or an 8-bit G.711 WAV with `-o`.  With `--encoding flac` each request is one lossless FLAC stream, encoded on the GPU:
+on stdout, or as the `-o` file (the same bytes either way); realtime mode refuses it.
 """
 from __future__ import annotations
 
@@ -19,7 +20,7 @@ import sys
 from typing import Optional
 
 from . import from_config_path
-from .core import ENCODINGS, OperationError, check_encoding
+from .core import ENCODINGS, FLAC, OperationError, check_encoding
 from .piper import PiperSynthesisConfig
 from .synth import AudioOutputConfig, SonataSpeechSynthesizer, _check_loudness
 
@@ -50,9 +51,10 @@ def build_parser() -> argparse.ArgumentParser:
                     help="Target integrated loudness of every sentence in LUFS, [-70, 0] (ITU-R BS.1770-4; e.g. -23 "
                          "EBU R128, -16 podcasts), measured and applied on the GPU; output is then written at a fixed "
                          "scale instead of peak-normalised.  Not in realtime mode")
-    ap.add_argument("--encoding", choices=("pcm16",) + ENCODINGS,
-                    help="Output encoding: pcm16 (default), or G.711 mulaw / alaw at one byte per sample (telephony: "
-                         "PCMU / PCMA), encoded on the GPU")
+    ap.add_argument("--encoding", choices=("pcm16",) + ENCODINGS + (FLAC,),
+                    help="Output encoding: pcm16 (default), G.711 mulaw / alaw at one byte per sample (telephony: "
+                         "PCMU / PCMA), or lossless flac (one FLAC stream per request, on stdout or in the -o file; "
+                         "not in realtime mode), encoded on the GPU")
     ap.add_argument("--device", type=int, default=int(os.environ.get("SONATA_B200_DEVICE", "0")))
     return ap
 
@@ -66,7 +68,13 @@ def process_request(synth: SonataSpeechSynthesizer, default_cfg: PiperSynthesisC
     mode = (req.get("mode") or "lazy").lower()
     loudness = req.get("loudness")
     encoding = req.get("encoding")
-    encoding = None if encoding == "pcm16" else check_encoding(encoding, "request: ")
+    if encoding == FLAC:
+        if mode == "realtime" and not output_file:
+            raise OperationError("FLAC output is not available in realtime mode: a FLAC stream is one whole file whose "
+                                 "header holds its length, and realtime mode hands out a sentence's first chunk before "
+                                 "its last one is decoded (use lazy or parallel mode)")
+    else:
+        encoding = None if encoding == "pcm16" else check_encoding(encoding, "request: ")
     if loudness is not None:
         _check_loudness(loudness)
         if mode == "realtime" and not output_file:
@@ -86,6 +94,10 @@ def process_request(synth: SonataSpeechSynthesizer, default_cfg: PiperSynthesisC
     enc = {} if encoding is None else {"encoding": encoding}
     if output_file:
         synth.synthesize_to_file(output_file, text, oc, seed=seed, **rate, **loud, **enc)
+        return
+    if encoding == FLAC:                              # the bytes -o writes, one stream per request
+        out.write(synth.synthesize_flac(text, oc, seed=seed, **rate, **loud))
+        out.flush()
         return
     if mode == "lazy":
         stream = synth.synthesize_lazy(text, oc, seed=seed, **rate, **loud, **enc)

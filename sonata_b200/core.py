@@ -128,6 +128,43 @@ def g711_wave_bytes(data: bytes, encoding: str, sample_rate: int) -> bytes:
     return b"RIFF" + struct.pack("<I", len(body)) + body
 
 
+# FLAC is a whole-file format: its STREAMINFO holds the stream's length and frame sizes, so it is written whole (files,
+# batches, jobs) and never handed out piece by piece.
+FLAC = "flac"
+
+
+def refuse_flac(encoding, where: str) -> None:
+    """OperationError when `encoding` is "flac" in `where`, a mode that hands out audio piece by piece."""
+    if isinstance(encoding, str) and encoding == FLAC:
+        raise OperationError(f"{where} cannot deliver 'flac': a FLAC stream is one whole file (STREAMINFO holds its "
+                             "length and frame sizes); use synthesize_to_file, infer_batch_flac / speak_batch_flac or "
+                             "SynthesisJob.fetch_flac")
+
+
+def flac_encode(samples_i16: np.ndarray, sample_rate: int, device: int = 0) -> bytes:
+    """A complete FLAC stream (RFC 9639 streamable subset: mono, 16 bits, blocks of 4096, MD5 left zero) of the 1-D
+    int16 array `samples_i16` at `sample_rate` (one of piper.OUTPUT_RATES), encoded on CUDA device `device` by the
+    library's kernels; nothing is encoded on the host.  Zero samples give the 42-byte header-only stream."""
+    import ctypes as C
+    from . import _native as N
+    from .piper import OUTPUT_RATES, _check
+    if not isinstance(samples_i16, np.ndarray) or samples_i16.dtype != np.int16 or samples_i16.ndim != 1:
+        raise OperationError("flac_encode takes a 1-D numpy array of int16 samples")
+    if isinstance(sample_rate, bool) or not isinstance(sample_rate, (int, np.integer)) or int(sample_rate) not in OUTPUT_RATES:
+        raise OperationError(f"FLAC: sample rate {sample_rate!r} is not one of the output rates {OUTPUT_RATES}")
+    if isinstance(device, bool) or not isinstance(device, (int, np.integer)) or int(device) < 0:
+        raise OperationError(f"device {device!r} is not a CUDA device index")
+    x = np.ascontiguousarray(samples_i16)
+    out, n, err = C.POINTER(C.c_uint8)(), C.c_size_t(), N.sb200_error()
+    lib = N.lib()
+    _check(lib.sb200_flac_encode(int(device), x.ctypes.data_as(C.POINTER(C.c_int16)), x.size, int(sample_rate),
+                                 C.byref(out), C.byref(n), C.byref(err)), err)
+    try:
+        return C.string_at(out, n.value)
+    finally:
+        lib.sb200_bytes_free(out)
+
+
 class AudioSamples:
     """struct AudioSamples(Vec<f32>) (audio/ops/src/samples.rs:16-18)."""
 

@@ -427,6 +427,26 @@ int32_t sb200_job_fetch_g711(sb200_job* job, int32_t law, const float* gains, ui
     });
 }
 void sb200_bytes_free(uint8_t* p) { free(p); }
+int32_t sb200_job_fetch_flac(sb200_job* job, const float* gains, uint8_t** outs, size_t* lens, sb200_error* err) {
+    return guarded(err, [&] {
+        Job& j = *job->j;
+        if (!j.ran || j.encode_only) throw Error(19, "job has not produced audio");
+        if (!outs || !lens) throw Error(19, "null argument");
+        job_flac_to_host(j, gains, outs, lens);
+    });
+}
+int32_t sb200_flac_encode(int32_t device, const int16_t* x, size_t n, uint32_t sample_rate, uint8_t** out, size_t* len,
+                          sb200_error* err) {
+    return guarded(err, [&] {
+        if (!flac_rate_supported(sample_rate))
+            throw Error(19, "FLAC: sample rate " + std::to_string(sample_rate) + " Hz is not one of the output rates");
+        if (!out || !len || (!x && n > 0)) throw Error(19, "null argument");
+        SB_CUDA(cudaSetDevice(device));
+        DeviceBuffers d;
+        const short* dx = n ? d.upload(reinterpret_cast<const short*>(x), n, n) : nullptr;
+        flac_encode(dx, {FlacStream{0, (long long)n, (long long)sample_rate}}, 0, out, len);
+    });
+}
 
 int32_t sb200_job_copy_out(sb200_job* job, void* dst, size_t cap, int32_t format, size_t* written, sb200_error* err) {
     return guarded(err, [&] {

@@ -1279,33 +1279,55 @@ void decode_chunks(Voice* v, const ChunkPass& p, ChunkResult& out) {
 }
 
 namespace {
-// The i16 conversion of a finished job in format `fmt` (PCM_I16 or a G.711 law), utterance b after gains[b].
-void job_pcm_to_host(Job& j, int fmt, const float* gains, void* dst) {
-    if (!j.ran || j.encode_only) throw Error(19, "job has not produced audio");
-    SB_CUDA(cudaSetDevice(j.v->device));
-    cudaStream_t st = j.ctx->stream;
-    const int hop = j.out_hop;
-    const size_t n = (size_t)j.out_total, bytes = pcm_bytes(fmt);
-    long long mx = 0;
-    for (size_t b = 0; b < j.B; b++) mx = std::max<long long>(mx, (long long)j.osegs[b].len * hop);
-    // stream-ordered scratch, returned to the pool at once: device memory held after a run does not grow
+// The i16 conversion of a finished job in format `fmt` (PCM_I16 or a G.711 law), utterance b after gains[b], into
+// stream-ordered scratch laid out like the job's waveforms.  The scratch goes back to the pool with the object, so
+// device memory held after a run does not grow.
+struct JobPcm {
+    cudaStream_t st = nullptr;
     void* d_pcm = nullptr; unsigned* d_max = nullptr; PcmPost* d_post = nullptr;
-    SB_CUDA(cudaMallocAsync(&d_pcm, n * bytes + 16, st));
-    SB_CUDA(cudaMallocAsync(&d_max, sizeof(unsigned) * j.B, st));
-    SB_CUDA(cudaMallocAsync(&d_post, sizeof(PcmPost) * j.B, st));
-    std::vector<PcmPost> posts(j.B);
-    for (size_t b = 0; b < j.B; b++) posts[b].gain = gains[b];
-    // a loudness-normalised utterance keeps its level: fixed scale instead of its own peak
-    for (size_t b = 0; b < j.loud_ran.size(); b++) posts[b].fixed_scale = std::isnan(j.loud_ran[b]) ? 0 : 1;
-    // pageable source: the call returns once the entries are staged, so `posts` may go out of scope before the copy runs
-    SB_CUDA(cudaMemcpyAsync(d_post, posts.data(), sizeof(PcmPost) * j.B, cudaMemcpyHostToDevice, st));
-    launch_pcm(j.d_wav, j.d_osegs, d_post, (int)j.B, hop, mx, d_max, fmt, d_pcm, st);
-    cudaError_t e = cudaMemcpyAsync(dst, d_pcm, n * bytes, cudaMemcpyDeviceToHost, st);
-    cudaFreeAsync(d_pcm, st);
-    cudaFreeAsync(d_max, st);
-    cudaFreeAsync(d_post, st);
-    if (e == cudaSuccess) e = cudaStreamSynchronize(st);
+    JobPcm(Job& j, int fmt, const float* gains) {
+        if (!j.ran || j.encode_only) throw Error(19, "job has not produced audio");
+        SB_CUDA(cudaSetDevice(j.v->device));
+        st = j.ctx->stream;
+        const int hop = j.out_hop;
+        const size_t n = (size_t)j.out_total;
+        long long mx = 0;
+        for (size_t b = 0; b < j.B; b++) mx = std::max<long long>(mx, (long long)j.osegs[b].len * hop);
+        SB_CUDA(cudaMallocAsync(&d_pcm, n * pcm_bytes(fmt) + 16, st));
+        SB_CUDA(cudaMallocAsync(&d_max, sizeof(unsigned) * j.B, st));
+        SB_CUDA(cudaMallocAsync(&d_post, sizeof(PcmPost) * j.B, st));
+        std::vector<PcmPost> posts(j.B);
+        for (size_t b = 0; b < j.B; b++) posts[b].gain = gains[b];
+        // a loudness-normalised utterance keeps its level: fixed scale instead of its own peak
+        for (size_t b = 0; b < j.loud_ran.size(); b++) posts[b].fixed_scale = std::isnan(j.loud_ran[b]) ? 0 : 1;
+        // pageable source: the call returns once the entries are staged, so `posts` may go out of scope before the
+        // copy runs
+        SB_CUDA(cudaMemcpyAsync(d_post, posts.data(), sizeof(PcmPost) * j.B, cudaMemcpyHostToDevice, st));
+        launch_pcm(j.d_wav, j.d_osegs, d_post, (int)j.B, hop, mx, d_max, fmt, d_pcm, st);
+    }
+    ~JobPcm() {
+        cudaFreeAsync(d_pcm, st);
+        cudaFreeAsync(d_max, st);
+        cudaFreeAsync(d_post, st);
+    }
+};
+
+void job_pcm_to_host(Job& j, int fmt, const float* gains, void* dst) {
+    JobPcm pcm(j, fmt, gains);
+    cudaError_t e = cudaMemcpyAsync(dst, pcm.d_pcm, (size_t)j.out_total * pcm_bytes(fmt), cudaMemcpyDeviceToHost, pcm.st);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(pcm.st);
     if (e != cudaSuccess) throw Error(19, std::string("CUDA error: ") + cudaGetErrorString(e));
+}
+
+// gains[0 .. B), each finite, or 1 for every utterance when null.
+std::vector<float> job_gains(const Job& j, const float* gains) {
+    std::vector<float> g(j.B, 1.f);
+    for (size_t b = 0; gains && b < j.B; b++) {
+        if (!std::isfinite(gains[b]))
+            throw Error(19, "utterance " + std::to_string(b) + ": gain " + std::to_string(gains[b]) + " is not finite");
+        g[b] = gains[b];
+    }
+    return g;
 }
 }  // namespace
 
@@ -1322,13 +1344,22 @@ int g711_format(long long law, const std::string& who) {
 
 void job_g711_to_host(Job& j, int law, const float* gains, uint8_t* dst) {
     const int fmt = g711_format(law, "");
-    std::vector<float> g(j.B, 1.f);
-    for (size_t b = 0; gains && b < j.B; b++) {
-        if (!std::isfinite(gains[b]))
-            throw Error(19, "utterance " + std::to_string(b) + ": gain " + std::to_string(gains[b]) + " is not finite");
-        g[b] = gains[b];
-    }
+    const std::vector<float> g = job_gains(j, gains);
     job_pcm_to_host(j, fmt, g.data(), dst);
+}
+
+void job_flac_to_host(Job& j, const float* gains, uint8_t** outs, size_t* lens) {
+    const std::vector<float> g = job_gains(j, gains);
+    if (!j.ran || j.encode_only) throw Error(19, "job has not produced audio");
+    for (size_t b = 0; b < j.B; b++)
+        if (!flac_rate_supported(j.osr[b]))
+            throw Error(19, "utterance " + std::to_string(b) + ": FLAC: sample rate " + std::to_string(j.osr[b]) +
+                                " Hz is not one of the output rates");
+    JobPcm pcm(j, PCM_I16, g.data());
+    std::vector<FlacStream> streams(j.B);
+    for (size_t b = 0; b < j.B; b++)
+        streams[b] = FlacStream{j.osegs[b].out_off, (long long)j.osegs[b].len * j.out_hop, j.osr[b]};
+    flac_encode(static_cast<const short*>(pcm.d_pcm), streams, pcm.st, outs, lens);
 }
 
 // Peak-normalised 16-bit PCM of every utterance of a finished job, through the context's page-locked staging buffer.

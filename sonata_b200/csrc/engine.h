@@ -372,5 +372,21 @@ int g711_format(long long law, const std::string& who);
 // in the same launches: one byte per sample in `dst`, laid out like the job's waveforms.  A bad law or gain fails
 // before anything runs.
 void job_g711_to_host(Job& j, int law, const float* gains, uint8_t* dst);
+// One FLAC stream per utterance of a finished job (flac.cu): the 16-bit samples job_i16_to_host's conversion gives
+// after gains[b] (null: 1; each must be finite), encoded on the device at the utterance's delivered rate.  outs[b]
+// receives a malloc'ed buffer of lens[b] bytes.  A bad gain fails before anything runs.
+void job_flac_to_host(Job& j, const float* gains, uint8_t** outs, size_t* lens);
+
+// ---- FLAC (flac.cu) ----
+constexpr int FLAC_STREAMINFO_BYTES = 42;   // `fLaC`, the block header and STREAMINFO
+// One stream to encode: samples [off, off + n) of a device buffer of 16-bit samples, at `rate` Hz.
+struct FlacStream { long long off = 0, n = 0; long long rate = 0; };
+// Whether `rate` has a FLAC frame-header code here: the eight output rates.
+bool flac_rate_supported(long long rate);
+// A complete FLAC stream (RFC 9639 streamable subset; mono, 16 bits, blocks of 4096) of every entry of `streams`,
+// encoded by the kernels of flac.cu on `st`: outs[s] receives a malloc'ed buffer of lens[s] bytes.  The size table is
+// read back first, then only the compressed bytes.  An unsupported rate fails before any device work.
+void flac_encode(const short* d_x, const std::vector<FlacStream>& streams, cudaStream_t st, uint8_t** outs,
+                 size_t* lens);
 
 }  // namespace sb200

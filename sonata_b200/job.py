@@ -168,6 +168,17 @@ class SynthesisJob:
         _check(self._lib.sb200_job_fetch_g711(self._h, G711_LAW[law], _ptr(g, C.c_float), outs, lens, C.byref(err)), err)
         return _take_bytes(self._lib, outs, lens)
 
+    def fetch_flac(self, gains: Optional[Sequence] = None) -> List[bytes]:
+        """One complete FLAC stream per utterance (see sb200_job_fetch_flac): lossless, of exactly the 16-bit samples
+        fetch_i16 returns after gains[b] (None: 1), at the utterance's delivered rate.  Analysed, laid out and packed on
+        the device; only the compressed bytes leave the card."""
+        g = _gain_array(gains, self.batch)
+        outs = (C.POINTER(C.c_uint8) * self.batch)()
+        lens = (C.c_size_t * self.batch)()
+        err = N.sb200_error()
+        _check(self._lib.sb200_job_fetch_flac(self._h, _ptr(g, C.c_float), outs, lens, C.byref(err)), err)
+        return _take_bytes(self._lib, outs, lens)
+
     def copy_out(self, dst_address: int, capacity_bytes: int, fmt: int = 0) -> int:
         """Device -> host copy of the whole result (utterances back to back) into caller memory, e.g. a slice of the
         host segment shared by the ranks of one frontend; fmt 0 = f32, 1 = peak-normalised i16 PCM, 2 / 3 = G.711

@@ -18,7 +18,7 @@ import numpy as np
 
 from . import _native as N
 from .core import (G711_LAW, Audio, AudioInfo, AudioSamples, OperationError, PhonemeAlignment, Phonemes,
-                   PhonemizationError, SonataError, check_encoding)
+                   PhonemizationError, SonataError, check_encoding, refuse_flac)
 
 MIN_CHUNK_SIZE = 44      # piper/src/lib.rs:18
 MAX_CHUNK_SIZE = 1024    # piper/src/lib.rs:19
@@ -614,6 +614,42 @@ class _VitsCommons:
         return self.infer_batch_g711([self.phonemes_to_input_ids(p) for p in phoneme_batches], law, configs, seeds,
                                      output_rates, loudness, gains)
 
+    def infer_batch_flac(self, batches: Sequence[Sequence[int]],
+                         configs: Optional[Sequence[PiperSynthesisConfig]] = None, seeds: Optional[Sequence] = None,
+                         output_rates: Optional[Sequence] = None, loudness: Optional[Sequence] = None,
+                         gains: Optional[Sequence] = None) -> List[bytes]:
+        """infer_batch_with_values delivered as lossless FLAC: one complete stream (`bytes`) per utterance.  Its samples
+        are exactly the 16-bit samples the i16 route gives (SynthesisJob.fetch_i16): to_i16_vec of the utterance after
+        gains[b] (None: 1), or the fixed scale for an utterance with a loudness target, at its delivered rate.  They are
+        encoded on the device, and only the compressed bytes leave the card.  `configs`, `seeds`, `output_rates` and
+        `loudness` as for infer_batch_with_values."""
+        from .job import SynthesisJob
+        n = len(batches)
+        _config_array(configs, n)
+        _seed_arrays(seeds, n)
+        _rate_array(output_rates, n)
+        _loudness_array(loudness, n)
+        _gain_array(gains, n)
+        if n == 0:
+            return []
+        if any(len(b) == 0 for b in batches):
+            raise OperationError("Failed to run model inference. Error: empty input sequence")
+        job = SynthesisJob(self, batches, configs=configs, seeds=seeds, output_rates=output_rates, loudness=loudness)
+        try:
+            job.run()
+            return job.fetch_flac(gains)
+        finally:
+            job.close()
+
+    def speak_batch_flac(self, phoneme_batches: Sequence[str],
+                         configs: Optional[Sequence[PiperSynthesisConfig]] = None, seeds: Optional[Sequence] = None,
+                         output_rates: Optional[Sequence] = None, loudness: Optional[Sequence] = None,
+                         gains: Optional[Sequence] = None) -> List[bytes]:
+        """speak_batch delivered as FLAC streams: infer_batch_flac over the phonemes' ids."""
+        _config_array(configs, len(phoneme_batches))
+        return self.infer_batch_flac([self.phonemes_to_input_ids(p) for p in phoneme_batches], configs, seeds,
+                                     output_rates, loudness, gains)
+
     def _cfg(self, fn) -> PiperSynthesisConfig:
         c, err = N.sb200_synth_config(), N.sb200_error()
         _check(fn(self._h, C.byref(c), C.byref(err)), err)
@@ -832,6 +868,7 @@ class VitsStreamingModel(_VitsCommons):
         With `encoding` ("mulaw" or "alaw"; None: none), chunks take pcm16's tuples and each result is `bytes`: G.711 of
         the int16 samples pcm16 returns for that chunk (with or without resamplers), encoded on the device in the same
         launches."""
+        refuse_flac(encoding, "a decoder chunk pass")
         check_encoding(encoding)
         if encoding is not None and pcm16:
             raise OperationError("pcm16 and an encoding are two output formats: give one")
@@ -909,6 +946,7 @@ class VitsStreamingModel(_VitsCommons):
         yields without an encoding, after the linear `gain` (None: 1; encoded streams only), encoded on the device."""
         _seed_arrays([seed], 1)
         _rate_array([output_rate], 1)
+        refuse_flac(encoding, "stream_synthesis")
         g = _stream_gain(encoding, gain)
         ids = self.phonemes_to_input_ids(phonemes)
         enc = self.infer_encoder(ids) if seed is None else self.infer_encoder_batch([ids], seeds=[seed])[0]
@@ -995,6 +1033,7 @@ class StreamBatch:
             raise OperationError("Invalid configuration for Vits Model")
         _seed_arrays([seed], 1)
         _rate_array([output_rate], 1)
+        refuse_flac(encoding, "StreamBatch")
         gain = _stream_gain(encoding, gain)
         if config is not None and config.speaker is not None and config.speaker not in (self.model.get_speakers() or {}):
             raise OperationError(f"No speaker was found with the given id `{config.speaker}`")     # as check_config

@@ -24,7 +24,8 @@ from typing import Iterator, List, Optional
 
 import numpy as np
 
-from .core import G711_SILENCE, Audio, AudioSamples, OperationError, SonataError, check_encoding, g711_wave_bytes
+from .core import (FLAC, G711_SILENCE, Audio, AudioSamples, OperationError, SonataError, check_encoding, flac_encode,
+                   g711_wave_bytes, refuse_flac)
 
 RATE_RANGE = (0.5, 5.5)      # synth/src/lib.rs:13
 VOLUME_RANGE = (0.0, 1.0)    # :14
@@ -179,6 +180,7 @@ class SonataSpeechSynthesizer:
         sentence_seed(seed, 0)
         _check_output_rate(output_rate)
         _check_loudness(loudness)
+        refuse_flac(encoding, "synthesize_lazy")
         check_encoding(encoding)
         for i, ph in enumerate(self._phonemes(text)):
             if encoding is not None:
@@ -203,6 +205,7 @@ class SonataSpeechSynthesizer:
         sentence_seed(seed, 0)
         _check_output_rate(output_rate)
         _check_loudness(loudness)
+        refuse_flac(encoding, "synthesize_parallel")
         check_encoding(encoding)
         ph = self._phonemes(text)
         if encoding is not None:
@@ -229,6 +232,7 @@ class SonataSpeechSynthesizer:
         `encoding`: every chunk is G.711 bytes of its to_i16_vec after the volume, encoded on the device."""
         sentence_seed(seed, 0)
         _check_output_rate(output_rate)
+        refuse_flac(encoding, "synthesize_streamed")
         check_encoding(encoding)
         if encoding is not None and output_config is not None:
             output_config._check_supported()
@@ -282,7 +286,13 @@ class SonataSpeechSynthesizer:
         """:168-198 — parallel mode, concatenated, peak-normalised i16 WAV (at output_rate when given).  With
         `loudness` the WAV is written at the fixed scale (trunc(clamp(x * 32767))), so it keeps the sentences' level.
         With `encoding` the WAV is 8-bit G.711 (WAVE_FORMAT_MULAW / _ALAW, with a `fact` chunk) holding the sentences'
-        bytes as synthesize_parallel hands them out: each sentence converted at its own peak (or the fixed scale)."""
+        bytes as synthesize_parallel hands them out: each sentence converted at its own peak (or the fixed scale).
+        With encoding="flac" the file is one FLAC stream (synthesize_flac) instead of a WAV."""
+        if isinstance(encoding, str) and encoding == FLAC:
+            data = self.synthesize_flac(text, output_config, seed=seed, output_rate=output_rate, loudness=loudness)
+            with open(filename, "wb") as f:
+                f.write(data)
+            return
         extra = {"output_rate": output_rate} if output_rate else {}
         if loudness is not None:
             extra["loudness"] = loudness
@@ -293,11 +303,30 @@ class SonataSpeechSynthesizer:
             with open(filename, "wb") as f:
                 f.write(g711_wave_bytes(data, encoding, output_rate or self.model.audio_output_info().sample_rate))
             return
+        self._document(text, output_config, seed, output_rate, loudness).save_to_file(filename,
+                                                                                       fixed_scale=loudness is not None)
+
+    def _document(self, text: str, output_config: Optional[AudioOutputConfig], seed, output_rate, loudness) -> Audio:
+        """The sentences of synthesize_parallel concatenated: what synthesize_to_file writes as a WAV."""
+        extra = {"output_rate": output_rate} if output_rate else {}
+        if loudness is not None:
+            extra["loudness"] = loudness
         parts = [a.samples.as_slice() for a in self.synthesize_parallel(text, output_config, seed=seed, **extra)]
         if not parts or sum(len(p) for p in parts) == 0:
             raise OperationError("No speech data to write")
         rate = output_rate or self.model.audio_output_info().sample_rate
-        Audio(AudioSamples(np.concatenate(parts)), rate).save_to_file(filename, fixed_scale=loudness is not None)
+        return Audio(AudioSamples(np.concatenate(parts)), rate)
+
+    def synthesize_flac(self, text: str, output_config: Optional[AudioOutputConfig] = None,
+                        seed: Optional[int] = None, output_rate: Optional[int] = None,
+                        loudness: Optional[float] = None) -> bytes:
+        """The FLAC file synthesize_to_file(..., encoding="flac") writes: one stream whose decoded samples are exactly
+        the 16-bit samples of the WAV the same call writes without an encoding (the concatenation at the document's
+        peak, or the fixed scale with `loudness`), encoded on the model's device by flac_encode."""
+        doc = self._document(text, output_config, seed, output_rate, loudness)
+        s = doc.samples
+        return flac_encode(s.to_i16_fixed() if loudness is not None else s.to_i16_vec(), doc.info.sample_rate,
+                           getattr(self.model, "device", 0))
 
     # passthroughs of the SonataModel surface (:205-253)
     def speak_one_sentence(self, phonemes: str) -> Audio:
@@ -344,6 +373,7 @@ class RealtimeBatch:
         from .piper import PiperSynthesisConfig
         sentence_seed(seed, 0)
         _check_output_rate(output_rate)
+        refuse_flac(encoding, "RealtimeBatch")
         check_encoding(encoding)
         if output_config is not None:
             output_config._check_supported()
