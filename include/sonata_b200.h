@@ -203,6 +203,32 @@ int32_t sb200_speak_batch_ids_loudness(sb200_voice* v, const int64_t* ids_packed
                                        const uint32_t* output_rates, const float* target_lufs, sb200_audio* outs,
                                        int32_t* id_frames_out, double* lufs_out, float* gain_out, sb200_error* err);
 
+/* ---- pitch and tempo: each utterance's waveform warped by two ratios on the device ----
+ * pitch p in [0.5, 2] multiplies every frequency of the utterance and keeps its duration; tempo t in [0.25, 4] plays it
+ * t times faster and keeps its pitch (delivered length about n / t).  NaN or exactly 1 asks for nothing; any other
+ * value outside its range fails with OPERATION_ERROR naming the utterance, before any device work.  An utterance that
+ * asks for neither keeps its bits.  The stage runs at the voice's rate R on the decoder's waveform x[0 .. n), before any
+ * resampling and loudness, which see its output as they see a waveform.  With alpha = (double)p / (double)t:
+ *  1. Time stretch by alpha (skipped when p == t), WSOLA: Hs = R / 100, N = 2 Hs, D = R / 160 (integer divisions),
+ *     n1 = floor(n alpha + 0.5), frames k < F = ceil(n1 / Hs) at a_k = floor(k Hs / alpha + 0.5) (double), a virtual frame
+ *     -1 at a = -Hs with offset 0.  With q[i] = trunc(clamp(x[i], -1, 1) * 32767) (0 outside x), delta_0 = 0 and for
+ *     k >= 1 delta_k is the delta in [-D, D] maximising sum_{i < N} q[a_{k-1} + delta_{k-1} + Hs + i] q[a_k + delta + i]
+ *     in 64-bit integers, ties to the smaller |delta|, then to the negative one.  With w[i] = 0.5 - 0.5 cos(2 pi i / N),
+ *     s[m] = w[r] x[a_k + delta_k + r] + w[r + Hs] x[a_{k-1} + delta_{k-1} + r + Hs] for k = m / Hs, r = m - k Hs, in f32.
+ *  2. Pitch resampling by p (skipped when p == 1): n2 = floor(n1 / p + 0.5), y[j] = sum_i s[i] h(j p - i) with
+ *     h(u) = c sinc(c u) (0.42 + 0.5 cos(pi u / W) + 0.08 cos(2 pi u / W)) for |u| < W, c = min(1, 1 / p), W = 16 / c;
+ *     positions and phases in double, taps rounded to f32, one fmaf chain in ascending i.
+ * The offsets are exact integers and the waveform stages have a fixed evaluation order, so a warped utterance has the
+ * same bits in any batch.  Per-id frame counts stay frame counts of the unwarped utterance.
+ * sb200_speak_batch_ids_loudness with pitch[b] / tempo[b] the ratios of utterance b (either array may be NULL); NULL and
+ * NULL is that call, bit for bit. */
+int32_t sb200_speak_batch_ids_prosody(sb200_voice* v, const int64_t* ids_packed, const size_t* offsets, size_t batch,
+                                      const sb200_synth_config* cfgs, const float* scale_packed,
+                                      const int32_t* frames_packed, const uint64_t* seeds, const int32_t* seeded,
+                                      const uint32_t* output_rates, const float* target_lufs, const float* pitch,
+                                      const float* tempo, sb200_audio* outs, int32_t* id_frames_out, double* lufs_out,
+                                      float* gain_out, sb200_error* err);
+
 /* ---- job API: the same batched pass split into its host<->device steps (bench / multi-GPU plumbing) ----
  * create  : copies ids to the device (H2D).  `eps_w` / `eps_z` optionally inject the graph's two
  *           RandomNormalLike draws (time-major: eps_w[b] = f32[T_x][2], eps_z[b] = f32[T_y][inter]);
@@ -247,6 +273,15 @@ int32_t sb200_job_set_loudness(sb200_job* job, const float* target_lufs, sb200_e
 /* Each utterance's integrated loudness L (LUFS, -inf when no block passes the gates) and applied gain g of the last run
  * into lufs[0 .. batch) / gain[0 .. batch) (either may be NULL).  Fails when that run had no targets. */
 int32_t sb200_job_loudness(const sb200_job* job, double* lufs, float* gain, sb200_error* err);
+/* Pitch and tempo ratios (see sb200_speak_batch_ids_prosody) for the next sb200_job_run: pitch[0 .. batch) and
+ * tempo[0 .. batch), either or both NULL for none (what a new job starts with; so are ratios that are all NaN or 1).  A
+ * bad entry fails with OPERATION_ERROR naming the utterance and leaves the job's ratios as they were.  After a run with
+ * ratios every result call reports the warped signal, as after a run with output rates, and sb200_job_profile reports
+ * the offset chain and the overlap-add as the region "stretch" and the pitch resampler as "pitch". */
+int32_t sb200_job_set_prosody(sb200_job* job, const float* pitch, const float* tempo, sb200_error* err);
+/* Each utterance's stretched length n1, delivered length before any output-rate resampling n2 and WSOLA frame count F of
+ * the last run into n1[0 .. batch) / n2 / frames (each may be NULL).  Fails when that run had no ratios. */
+int32_t sb200_job_prosody(const sb200_job* job, int64_t* n1, int64_t* n2, int32_t* frames, sb200_error* err);
 /* Frames per id of the last run, packed like ids_packed, into out_packed[0 .. capacity): one device->host copy of the
  * whole batch's cumulative durations, made on the first call after a run.  Fails before a run, or when capacity is
  * smaller than the number of ids. */
@@ -472,6 +507,17 @@ int32_t sb200_debug_loudness_filter(int32_t rate, double* coeffs);
 /* The loudness kernel over one caller buffer x[0 .. n) at `rate`, measured only: *lufs receives its integrated loudness,
  * bit for bit what a job measures for an utterance of those samples. */
 int32_t sb200_debug_loudness(int32_t device, const float* x, size_t n, int32_t rate, double* lufs, sb200_error* err);
+/* Test hook, no device needed: the prosody plan (see sb200_speak_batch_ids_prosody) of n samples at `rate` with the two
+ * ratios: shape6 receives Hs, N, D, n1, n2, F, and positions[0 .. min(F, cap)) the analysis positions a_k.  Returns 0, or
+ * 19 for a ratio out of range or a rate outside 1000 .. 48000. */
+int32_t sb200_debug_prosody_plan(int32_t rate, int64_t n, float pitch, float tempo, int64_t* shape6, int64_t* positions,
+                                 size_t cap);
+/* The prosody kernels over one caller buffer x[0 .. n) at `rate`: y[0 .. n2) receives the result, bit for bit what a job
+ * gives an utterance of those samples, offsets[0 .. F) (NULL: not wanted) its delta_k and stretched[0 .. n1) (NULL: not
+ * wanted) the signal after stage 1 when that stage runs.  Fails when a destination is smaller than the plan says. */
+int32_t sb200_debug_prosody(int32_t device, const float* x, size_t n, int32_t rate, float pitch, float tempo, float* y,
+                            size_t cap, int32_t* offsets, size_t offsets_cap, float* stretched, size_t stretched_cap,
+                            sb200_error* err);
 /* Test hook: G.711 (law as for sb200_job_fetch_g711) of x[0 .. n) into out[0 .. n).  device -1 runs the host copy of
  * the encoders (no device needed); otherwise the encoders run on that device over the buffer. */
 int32_t sb200_debug_g711(int32_t device, int32_t law, const int16_t* x, size_t n, uint8_t* out, sb200_error* err);

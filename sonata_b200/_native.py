@@ -87,6 +87,12 @@ SIGNATURES = {
                                                    C.POINTER(C.c_uint32), C.POINTER(C.c_float), C.POINTER(sb200_audio),
                                                    C.POINTER(C.c_int32), C.POINTER(C.c_double), C.POINTER(C.c_float),
                                                    _ERR]),
+    "sb200_speak_batch_ids_prosody": (C.c_int32, [_P, C.POINTER(C.c_int64), C.POINTER(C.c_size_t), C.c_size_t,
+                                                  C.POINTER(sb200_synth_config), C.POINTER(C.c_float),
+                                                  C.POINTER(C.c_int32), C.POINTER(C.c_uint64), C.POINTER(C.c_int32),
+                                                  C.POINTER(C.c_uint32), C.POINTER(C.c_float), C.POINTER(C.c_float),
+                                                  C.POINTER(C.c_float), C.POINTER(sb200_audio), C.POINTER(C.c_int32),
+                                                  C.POINTER(C.c_double), C.POINTER(C.c_float), _ERR]),
     "sb200_job_create": (C.c_int32, [_P, C.POINTER(C.c_int64), C.POINTER(C.c_size_t), C.c_size_t,
                                      C.POINTER(C.POINTER(C.c_float)), C.POINTER(C.POINTER(C.c_float)),
                                      C.POINTER(C.c_size_t), C.POINTER(_P), _ERR]),
@@ -97,6 +103,8 @@ SIGNATURES = {
     "sb200_job_set_output_rates": (C.c_int32, [_P, C.POINTER(C.c_uint32), _ERR]),
     "sb200_job_set_loudness": (C.c_int32, [_P, C.POINTER(C.c_float), _ERR]),
     "sb200_job_loudness": (C.c_int32, [_P, C.POINTER(C.c_double), C.POINTER(C.c_float), _ERR]),
+    "sb200_job_set_prosody": (C.c_int32, [_P, C.POINTER(C.c_float), C.POINTER(C.c_float), _ERR]),
+    "sb200_job_prosody": (C.c_int32, [_P, C.POINTER(C.c_int64), C.POINTER(C.c_int64), C.POINTER(C.c_int32), _ERR]),
     "sb200_job_id_frames":(C.c_int32, [_P, C.POINTER(C.c_int32), C.c_size_t, _ERR]),
     "sb200_job_run": (C.c_int32, [_P, C.c_void_p, C.c_size_t, C.POINTER(C.c_float), _ERR]),
     "sb200_job_fetch": (C.c_int32, [_P, C.POINTER(sb200_audio), _ERR]),
@@ -179,6 +187,11 @@ SIGNATURES = {
     "sb200_debug_loudness_filter": (C.c_int32, [C.c_int32, C.POINTER(C.c_double)]),
     "sb200_debug_loudness": (C.c_int32, [C.c_int32, C.POINTER(C.c_float), C.c_size_t, C.c_int32, C.POINTER(C.c_double),
                                          _ERR]),
+    "sb200_debug_prosody_plan": (C.c_int32, [C.c_int32, C.c_int64, C.c_float, C.c_float, C.POINTER(C.c_int64),
+                                             C.POINTER(C.c_int64), C.c_size_t]),
+    "sb200_debug_prosody": (C.c_int32, [C.c_int32, C.POINTER(C.c_float), C.c_size_t, C.c_int32, C.c_float, C.c_float,
+                                        C.POINTER(C.c_float), C.c_size_t, C.POINTER(C.c_int32), C.c_size_t,
+                                        C.POINTER(C.c_float), C.c_size_t, _ERR]),
     "sb200_debug_g711": (C.c_int32, [C.c_int32, C.c_int32, C.POINTER(C.c_int16), C.c_size_t, C.POINTER(C.c_uint8),
                                      _ERR]),
     "sb200_launch_count": (C.c_uint64, []),

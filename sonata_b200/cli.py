@@ -21,8 +21,8 @@ from typing import Optional
 
 from . import from_config_path
 from .core import ENCODINGS, FLAC, OperationError, check_encoding
-from .piper import PiperSynthesisConfig
-from .synth import AudioOutputConfig, SonataSpeechSynthesizer, _check_loudness
+from .piper import PiperSynthesisConfig, refuse_prosody
+from .synth import AudioOutputConfig, SonataSpeechSynthesizer, _check_loudness, _check_prosody
 
 MODES = ("lazy", "parallel", "realtime")
 
@@ -51,6 +51,12 @@ def build_parser() -> argparse.ArgumentParser:
                     help="Target integrated loudness of every sentence in LUFS, [-70, 0] (ITU-R BS.1770-4; e.g. -23 "
                          "EBU R128, -16 podcasts), measured and applied on the GPU; output is then written at a fixed "
                          "scale instead of peak-normalised.  Not in realtime mode")
+    ap.add_argument("--pitch-ratio", type=float, metavar="RATIO",
+                    help="Multiply every frequency of the speech by RATIO, [0.5, 2], at the same duration, on the GPU.  "
+                         "Not in realtime mode")
+    ap.add_argument("--tempo", type=float, metavar="RATIO",
+                    help="Play the speech RATIO times faster, [0.25, 4], at the same pitch, on the GPU (a waveform time "
+                         "stretch: unlike --length-scale it keeps the model's articulation).  Not in realtime mode")
     ap.add_argument("--encoding", choices=("pcm16",) + ENCODINGS + (FLAC,),
                     help="Output encoding: pcm16 (default), G.711 mulaw / alaw at one byte per sample (telephony: "
                          "PCMU / PCMA), or lossless flac (one FLAC stream per request, on stdout or in the -o file; "
@@ -63,7 +69,8 @@ def process_request(synth: SonataSpeechSynthesizer, default_cfg: PiperSynthesisC
                     output_file: Optional[str], out=None) -> None:
     """process_synthesis_request (main.rs:126-165).  `seed` (optional): the request's noise seed, see
     synth.sentence_seed.  `output_rate` (optional): the sample rate of the WAV or raw PCM written.  `loudness`
-    (optional): every sentence's target loudness in LUFS; the PCM is then written at the fixed scale."""
+    (optional): every sentence's target loudness in LUFS; the PCM is then written at the fixed scale.  `pitch_ratio` /
+    `tempo` (optional): the ratios every sentence is shifted and played by, in lazy and parallel modes."""
     out = out or sys.stdout.buffer
     mode = (req.get("mode") or "lazy").lower()
     loudness = req.get("loudness")
@@ -81,6 +88,10 @@ def process_request(synth: SonataSpeechSynthesizer, default_cfg: PiperSynthesisC
             raise OperationError("loudness normalisation is not available in realtime mode: integrated loudness needs "
                                  "the whole sentence, and realtime mode hands out a sentence's first chunk before its "
                                  "last one is decoded (use lazy or parallel mode)")
+    pros = {k: req[k] for k in ("pitch_ratio", "tempo") if req.get(k) is not None}
+    _check_prosody(pros.get("pitch_ratio"), pros.get("tempo"))
+    if mode == "realtime" and not output_file:
+        refuse_prosody(pros.get("pitch_ratio"), pros.get("tempo"), "realtime mode")
     synth.model.set_fallback_synthesis_config(PiperSynthesisConfig(
         req.get("speaker_id"),
         req["noise_scale"] if req.get("noise_scale") is not None else default_cfg.noise_scale,
@@ -93,16 +104,16 @@ def process_request(synth: SonataSpeechSynthesizer, default_cfg: PiperSynthesisC
     loud = {} if loudness is None else {"loudness": loudness}
     enc = {} if encoding is None else {"encoding": encoding}
     if output_file:
-        synth.synthesize_to_file(output_file, text, oc, seed=seed, **rate, **loud, **enc)
+        synth.synthesize_to_file(output_file, text, oc, seed=seed, **rate, **loud, **enc, **pros)
         return
     if encoding == FLAC:                              # the bytes -o writes, one stream per request
-        out.write(synth.synthesize_flac(text, oc, seed=seed, **rate, **loud))
+        out.write(synth.synthesize_flac(text, oc, seed=seed, **rate, **loud, **pros))
         out.flush()
         return
     if mode == "lazy":
-        stream = synth.synthesize_lazy(text, oc, seed=seed, **rate, **loud, **enc)
+        stream = synth.synthesize_lazy(text, oc, seed=seed, **rate, **loud, **enc, **pros)
     elif mode == "parallel":
-        stream = synth.synthesize_parallel(text, oc, seed=seed, **rate, **loud, **enc)
+        stream = synth.synthesize_parallel(text, oc, seed=seed, **rate, **loud, **enc, **pros)
     elif mode == "realtime":
         stream = synth.synthesize_streamed(text, oc, req.get("chunk_size") or 100, req.get("chunk_padding") or 3,
                                           seed=seed, **rate, **enc)
@@ -129,7 +140,8 @@ def main(argv=None) -> int:
                "noise_scale": args.noise_scale, "noise_w": args.noise_w, "rate": args.rate, "volume": args.volume,
                "pitch": args.pitch, "appended_silence_ms": args.silence, "chunk_size": args.chunk_size,
                "chunk_padding": args.chunk_padding, "seed": args.seed, "output_rate": args.output_rate,
-               "loudness": args.loudness, "encoding": args.encoding}
+               "loudness": args.loudness, "encoding": args.encoding, "pitch_ratio": args.pitch_ratio,
+               "tempo": args.tempo}
         process_request(synth, default_cfg, req, args.output_file)
     else:
         for i, line in enumerate(sys.stdin):
@@ -144,6 +156,10 @@ def main(argv=None) -> int:
                 req["loudness"] = args.loudness
             if req.get("encoding") is None:
                 req["encoding"] = args.encoding
+            if req.get("pitch_ratio") is None:
+                req["pitch_ratio"] = args.pitch_ratio
+            if req.get("tempo") is None:
+                req["tempo"] = args.tempo
             out_file = None
             if args.output_file:
                 stem, ext = os.path.splitext(args.output_file)

@@ -259,11 +259,23 @@ static void job_loudness(const Job& j, double* lufs, float* gain) {
     if (gain) std::copy(j.loud_gain.begin(), j.loud_gain.end(), gain);
 }
 
-int32_t sb200_speak_batch_ids_loudness(sb200_voice* v, const int64_t* ids, const size_t* offsets, size_t batch,
-                                       const sb200_synth_config* cfgs, const float* scale_packed,
-                                       const int32_t* frames_packed, const uint64_t* seeds, const int32_t* seeded,
-                                       const uint32_t* output_rates, const float* target_lufs, sb200_audio* outs,
-                                       int32_t* id_frames_out, double* lufs_out, float* gain_out, sb200_error* err) {
+// Each utterance's stretched length, delivered length and frame count of a job's last run (each may be null).
+static void job_prosody(const Job& j, int64_t* n1, int64_t* n2, int32_t* frames) {
+    if (!j.ran || j.pros_ran.empty())
+        throw Error(19, "the job's last run had no prosody stage (no utterance asked for a pitch or a tempo)");
+    for (size_t b = 0; b < j.B; b++) {
+        if (n1) n1[b] = j.pros_ran[b].n1;
+        if (n2) n2[b] = j.pros_ran[b].n2;
+        if (frames) frames[b] = j.pros_ran[b].F;
+    }
+}
+
+int32_t sb200_speak_batch_ids_prosody(sb200_voice* v, const int64_t* ids, const size_t* offsets, size_t batch,
+                                      const sb200_synth_config* cfgs, const float* scale_packed,
+                                      const int32_t* frames_packed, const uint64_t* seeds, const int32_t* seeded,
+                                      const uint32_t* output_rates, const float* target_lufs, const float* pitch,
+                                      const float* tempo, sb200_audio* outs, int32_t* id_frames_out, double* lufs_out,
+                                      float* gain_out, sb200_error* err) {
     return guarded(err, [&] {
         const double t0 = now_ms();
         static_assert(sizeof(long long) == sizeof(int64_t), "");
@@ -273,6 +285,7 @@ int32_t sb200_speak_batch_ids_loudness(sb200_voice* v, const int64_t* ids, const
                 if (output_rates[b] != 0 && output_rates[b] != (uint32_t)v->v->sample_rate)
                     resample_ratio(v->v->sample_rate, output_rates[b], "utterance " + std::to_string(b) + ": ");
         const bool loud = check_loudness_targets(target_lufs, batch);
+        check_prosody(pitch, tempo, batch);
         std::unique_ptr<Job> j(create_job(v->v.get(), reinterpret_cast<const long long*>(ids), offsets, batch, nullptr,
                                           nullptr, nullptr, false));
         if (cfgs) set_job_configs(*j, cfgs_in(cfgs, batch).data());
@@ -280,6 +293,7 @@ int32_t sb200_speak_batch_ids_loudness(sb200_voice* v, const int64_t* ids, const
         set_job_seeds(*j, reinterpret_cast<const unsigned long long*>(seeds), seeded);
         set_job_output_rates(*j, output_rates);
         set_job_loudness(*j, target_lufs);
+        set_job_prosody(*j, pitch, tempo);
         j->run(nullptr, 0);
         fetch_audio(*j, outs, 0.f);
         if (id_frames_out) {
@@ -291,6 +305,15 @@ int32_t sb200_speak_batch_ids_loudness(sb200_voice* v, const int64_t* ids, const
         for (size_t b = 0; b < batch; b++)
             outs[b].inference_ms = wall * (j->out_total ? (float)outs[b].len / (float)j->out_total : 0.f);
     });
+}
+int32_t sb200_speak_batch_ids_loudness(sb200_voice* v, const int64_t* ids, const size_t* offsets, size_t batch,
+                                       const sb200_synth_config* cfgs, const float* scale_packed,
+                                       const int32_t* frames_packed, const uint64_t* seeds, const int32_t* seeded,
+                                       const uint32_t* output_rates, const float* target_lufs, sb200_audio* outs,
+                                       int32_t* id_frames_out, double* lufs_out, float* gain_out, sb200_error* err) {
+    return sb200_speak_batch_ids_prosody(v, ids, offsets, batch, cfgs, scale_packed, frames_packed, seeds, seeded,
+                                         output_rates, target_lufs, nullptr, nullptr, outs, id_frames_out, lufs_out,
+                                         gain_out, err);
 }
 int32_t sb200_speak_batch_ids_rates(sb200_voice* v, const int64_t* ids, const size_t* offsets, size_t batch,
                                     const sb200_synth_config* cfgs, const float* scale_packed,
@@ -372,6 +395,12 @@ int32_t sb200_job_set_loudness(sb200_job* job, const float* target_lufs, sb200_e
 }
 int32_t sb200_job_loudness(const sb200_job* job, double* lufs, float* gain, sb200_error* err) {
     return guarded(err, [&] { job_loudness(*job->j, lufs, gain); });
+}
+int32_t sb200_job_set_prosody(sb200_job* job, const float* pitch, const float* tempo, sb200_error* err) {
+    return guarded(err, [&] { set_job_prosody(*job->j, pitch, tempo); });
+}
+int32_t sb200_job_prosody(const sb200_job* job, int64_t* n1, int64_t* n2, int32_t* frames, sb200_error* err) {
+    return guarded(err, [&] { job_prosody(*job->j, n1, n2, frames); });
 }
 int32_t sb200_job_id_frames(sb200_job* job, int32_t* out_packed, size_t capacity, sb200_error* err) {
     return guarded(err, [&] {
@@ -893,6 +922,52 @@ int32_t sb200_debug_loudness(int32_t device, const float* x, size_t n, int32_t r
         launch_loudness(dx, ds, 1, scratch, dl, dg, 0);
         SB_CUDA(cudaDeviceSynchronize());
         SB_CUDA(cudaMemcpy(lufs, dl, sizeof(double), cudaMemcpyDeviceToHost));
+    });
+}
+
+int32_t sb200_debug_prosody_plan(int32_t rate, int64_t n, float pitch, float tempo, int64_t* shape6, int64_t* positions,
+                                 size_t cap) {
+    try {
+        if (!shape6 || n < 0) return 19;
+        check_prosody(&pitch, &tempo, 1);
+        const ProsodyShape s = prosody_shape(rate, n, pitch, tempo);
+        const int64_t out[6] = {s.Hs, s.N, s.D, s.n1, s.n2, s.F};
+        std::copy(out, out + 6, shape6);
+        for (int k = 0; positions && k < s.F && (size_t)k < cap; k++) positions[k] = prosody_analysis(s.Hs, s.alpha, k);
+        return 0;
+    } catch (const Error& e) {
+        return e.code;
+    }
+}
+
+int32_t sb200_debug_prosody(int32_t device, const float* x, size_t n, int32_t rate, float pitch, float tempo, float* y,
+                            size_t cap, int32_t* offsets, size_t offsets_cap, float* stretched, size_t stretched_cap,
+                            sb200_error* err) {
+    return guarded(err, [&] {
+        if (!x || !y || n == 0 || n > (size_t)INT32_MAX) throw Error(19, "debug prosody: bad arguments");
+        check_prosody(&pitch, &tempo, 1);
+        ProsodyPlan p;
+        p.add(prosody_shape(rate, (long long)n, pitch, tempo), 0, (long long)n);
+        const ProsodySeg& g = p.segs[0];
+        if ((size_t)g.n2 > cap || (offsets && (size_t)g.F > offsets_cap) ||
+            (stretched && g.stretch && (size_t)g.n1 > stretched_cap))
+            throw Error(19, "debug prosody: a destination is too small for the result");
+        SB_CUDA(cudaSetDevice(device));
+        DeviceBuffers d;
+        const float* dx = d.upload(x, n, n);
+        const ProsodySeg* dg = d.upload(&g, 1, 1);
+        int* doff = d.alloc<int>((size_t)g.F + 1);
+        float* ds = d.alloc<float>((size_t)p.s_total + 4);
+        float* dy = d.alloc<float>((size_t)g.n2 + 4);
+        if (p.smem_ints) launch_prosody_offsets(dx, dg, 1, p.smem_ints, doff, 0);
+        launch_prosody_ola(dx, dg, 1, p.max_ola, doff, ds, dy, 0);
+        if (p.max_pitch) launch_prosody_pitch(dx, ds, dg, 1, p.max_pitch, dy, 0);
+        SB_CUDA(cudaDeviceSynchronize());
+        SB_CUDA(cudaMemcpy(y, dy, (size_t)g.n2 * 4, cudaMemcpyDeviceToHost));
+        if (offsets && g.F) SB_CUDA(cudaMemcpy(offsets, doff, (size_t)g.F * 4, cudaMemcpyDeviceToHost));
+        // the stretched signal: the scratch when the pitch stage follows, else the result itself
+        if (stretched && g.stretch)
+            SB_CUDA(cudaMemcpy(stretched, g.pitch ? ds : dy, (size_t)g.n1 * 4, cudaMemcpyDeviceToHost));
     });
 }
 

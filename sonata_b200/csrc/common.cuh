@@ -257,6 +257,30 @@ constexpr int LD_SCRATCH = 6;     // doubles per chunk: its 4 states, its sum of
 // One launch over nseg segments (blockIdx.x = segment): lufs[b] = the integrated loudness (-inf when no block passes the
 // gates), gain[b] = the gain applied to the segment (1 without a target).
 void launch_loudness(float* wav, const LoudSeg* segs, int nseg, double* scratch, double* lufs, float* gain, cudaStream_t st);
+// Pitch and tempo of one segment (prosody.cu): x = wav[in_off, in_off + n) is time-stretched by alpha = pitch / tempo
+// (WSOLA: synthesis hop Hs, frame 2 Hs, search radius D, F frames whose offsets go to offsets[d_off ..)) into n1 samples
+// when `stretch`, then resampled by p into n2 samples when `pitch`.  The delivered signal is y[y_off, y_off + n2); with
+// both stages the stretched signal passes through s[s_off, s_off + n1).  With neither, x is copied to y.
+struct ProsodySeg {
+    long long in_off, n, s_off, n1, y_off, n2, d_off;
+    int F, Hs, D, stretch, pitch;
+    double alpha, p;
+};
+// Analysis position of WSOLA frame k: floor(k Hs / alpha + 0.5), every operation exactly rounded in double, so the host
+// plan and the kernels agree; the virtual frame -1 sits at -Hs.
+__host__ __device__ inline long long prosody_analysis(int Hs, double alpha, long long k) {
+    return k < 0 ? -(long long)Hs : (long long)floor((double)(k * Hs) / alpha + 0.5);
+}
+constexpr int PP_OUTS = 256;      // consecutive outputs of the pitch resampler per block iteration
+constexpr int PP_SPAN = 640;      // shared-memory floats of their input span: 255 p + 2 W + 3 at p = 2, W = 32
+// The offset chain (blockIdx.x = segment, one persistent block each; smem_ints: the largest 4 Hs + 2 D of the segments),
+// the overlap-add or copy (max_out: the most samples any segment writes) and the pitch resampler, one launch each.
+void launch_prosody_offsets(const float* wav, const ProsodySeg* segs, int nseg, int smem_ints, int* offsets,
+                            cudaStream_t st);
+void launch_prosody_ola(const float* wav, const ProsodySeg* segs, int nseg, long long max_out, const int* offsets,
+                        float* s, float* y, cudaStream_t st);
+void launch_prosody_pitch(const float* wav, const float* s, const ProsodySeg* segs, int nseg, long long max_out, float* y,
+                          cudaStream_t st);
 // One row range of a frame level taken from a latent: rows [off, off + len) of the level are rows [lo, lo + len) of src.
 struct GatherSeg { const float* src; long long lo; int off; int len; };
 // s[r] = the source row of r's segment (tile_seg: segment of every gran-row tile), or exact zeros past its end.

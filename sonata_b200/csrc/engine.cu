@@ -254,6 +254,13 @@ void set_job_loudness(Job& j, const float* targets) {
     else j.loud_target.clear();
 }
 
+void set_job_prosody(Job& j, const float* pitch, const float* tempo) {
+    if (!check_prosody(pitch, tempo, j.B)) { j.pitch.clear(); j.tempo.clear(); return; }
+    const std::vector<float> none(j.B, NAN);
+    j.pitch.assign(pitch ? pitch : none.data(), (pitch ? pitch : none.data()) + j.B);
+    j.tempo.assign(tempo ? tempo : none.data(), (tempo ? tempo : none.data()) + j.B);
+}
+
 namespace {
 
 struct Runner {
@@ -461,6 +468,33 @@ struct ResampleTables {
     }
 };
 
+// Device buffers of the prosody launches and the pinned mirrors of their tables: the segments, the output segments
+// (n2 samples at y_off, for the launches that read the prosody output), every frame's offset, the stretched signals of
+// the segments that run both stages, and the output unless it goes straight to the caller's buffer.
+struct ProsodyBufs {
+    ProsodySeg *segs = nullptr, *segs_h = nullptr; FrameSeg *osegs = nullptr, *osegs_h = nullptr;
+    int* offsets = nullptr; float *s = nullptr, *y = nullptr;
+    void carve(Arena& dev, Arena& pin, const ProsodyPlan& p, bool own_y) {
+        const size_t n = p.segs.size();
+        y = nullptr;
+        if (n == 0) return;
+        segs = dev.get<ProsodySeg>(n); segs_h = pin.get<ProsodySeg>(n);
+        osegs = dev.get<FrameSeg>(n); osegs_h = pin.get<FrameSeg>(n);
+        offsets = p.d_total ? dev.get<int>((size_t)p.d_total) : nullptr;
+        s = p.s_total ? dev.get<float>((size_t)p.s_total + 4) : nullptr;
+        if (own_y) y = dev.get<float>((size_t)p.y_total + 4);
+    }
+    void upload(const ProsodyPlan& p, cudaStream_t st) {
+        const size_t n = p.segs.size();
+        for (size_t k = 0; k < n; k++) {
+            segs_h[k] = p.segs[k];
+            osegs_h[k] = FrameSeg{0, (int)p.segs[k].n2, 0, 0, p.segs[k].y_off};
+        }
+        h2d(segs, segs_h, n * sizeof(ProsodySeg), st);
+        h2d(osegs, osegs_h, n * sizeof(FrameSeg), st);
+    }
+};
+
 // The loudness launch over what a job hands out: one segment per utterance at its delivered rate, chunk scratch laid out
 // back to back.
 struct LoudnessPlan {
@@ -521,9 +555,10 @@ struct DecoderBufs {
 };
 
 // Frame level of a synthesis pass (phase 2): tables, the latent, the flow's scratch, and unless the pass stops after
-// the flow the decoder and (when the caller passed no buffer) the waveforms.  With output rates the decoder's
-// waveforms are always the pass's own, and the resampled ones go to the caller's buffer or to `rs`, with the tables of
-// the resampling launch `rp`.
+// the flow the decoder and (when the caller passed no buffer) the waveforms.  With prosody or output rates the decoder's
+// waveforms are always the pass's own.  The prosody output (plan `pp`) is the pass's own too unless it is the result
+// and the caller passed a buffer; the resampled waveforms go to the caller's buffer or to `rs`, with the tables of the
+// resampling launch `rp`.
 struct FrameBufs {
     FrameTables y;
     float *s, *epsz, *zp, *h, *acts, *outb, *wav;
@@ -531,14 +566,18 @@ struct FrameBufs {
     DecoderBufs dec;
     ResampleTables rt; float* rs;
     LoudnessBufs ld;
-    void carve(Arena& dev, Arena& pin, const Job& j, const ResamplePlan& rp, const LoudnessPlan& lp, bool own_wav) {
+    ProsodyBufs pr;
+    void carve(Arena& dev, Arena& pin, const Job& j, const ProsodyPlan& pp, const ResamplePlan& rp, const LoudnessPlan& lp,
+               bool own_wav) {
         rt.carve(dev, pin, rp.segs.size());
         ld.carve(dev, pin, lp);
+        pr.carve(dev, pin, pp, own_wav || !rp.segs.empty());
         rs = nullptr;
         if (!rp.segs.empty()) {
             if (own_wav) rs = dev.get<float>((size_t)rp.total + 4);
             own_wav = true;
         }
+        if (!pp.segs.empty()) own_wav = true;
         const Arch& a = j.v->a;
         const size_t RY = (size_t)j.RY;
         y.carve(dev, pin, j);
@@ -670,13 +709,30 @@ void lay_out_frames(Job& j, const std::vector<int>& y_len, int hop) {
     j.RY = cur; j.total_samples = out;
 }
 
-// What the job hands out (osegs, out_hop, out_total): the frame layout itself without output rates (an empty plan), else
-// the segments of the returned plan, one utterance each at its rate, back to back.
-ResamplePlan lay_out_output(Job& j, int hop) {
+// The prosody launches of a job whose utterances ask for a pitch or a tempo (an empty plan when none does): every
+// utterance's decoder waveform, with its ratios or NaN.
+ProsodyPlan lay_out_prosody(const Job& j, int hop) {
+    ProsodyPlan p;
+    if (j.pitch.empty() || j.encode_only) return p;
+    for (size_t b = 0; b < j.B; b++) {
+        const long long n = (long long)j.fsegs[b].len * hop;
+        p.add(prosody_shape(j.v->sample_rate, n, j.pitch[b], j.tempo[b]), j.fsegs[b].out_off, n);
+    }
+    return p;
+}
+
+// What the job hands out (osegs, out_hop, out_total): the frame layout itself without prosody and output rates (an empty
+// plan), the prosody output without output rates (an empty plan too), else the segments of the returned plan, one
+// utterance each at its rate, back to back, resampled from the prosody output when there is one.
+ResamplePlan lay_out_output(Job& j, int hop, const ProsodyPlan& pp) {
     ResamplePlan p;
     j.osr.assign(j.B, j.v->sample_rate);
     if (j.out_rates.empty() || j.encode_only) {
         j.osegs = j.fsegs; j.out_hop = hop; j.out_total = j.total_samples;
+        if (!pp.segs.empty()) {
+            for (size_t b = 0; b < j.B; b++) j.osegs[b] = FrameSeg{0, (int)pp.segs[b].n2, 0, 0, pp.segs[b].y_off};
+            j.out_hop = 1; j.out_total = pp.y_total;
+        }
         return p;
     }
     j.osegs.assign(j.B, FrameSeg{});
@@ -686,7 +742,7 @@ ResamplePlan lay_out_output(Job& j, int hop) {
             j.osr[b] = j.out_rates[b];
             f = &voice_resampler(*j.v, j.out_rates[b], "utterance " + std::to_string(b) + ": ");
         }
-        p.add(f, (long long)j.fsegs[b].len * hop);
+        p.add(f, pp.segs.empty() ? (long long)j.fsegs[b].len * hop : pp.segs[b].n2);
         j.osegs[b] = FrameSeg{0, (int)p.segs[b].n_out, 0, 0, p.segs[b].out_off};
     }
     j.out_hop = 1; j.out_total = p.total;
@@ -700,6 +756,22 @@ void run_resample(Runner& R, const ResamplePlan& p, const ResampleTables& t, con
     R.begin("resample");
     launch_resample(wav, fsegs, posts, hop, t.segs, (int)p.segs.size(), p.max_out, p.smem, out, R.st);
     R.count(p.flops, p.bytes);
+    R.end();
+}
+
+// The prosody launches of plan `p` (buffers `t`) over the segments of wav into y: profile regions "stretch" (the offset
+// chain and the overlap-add, which also copies the segments without a ratio) and "pitch".
+void run_prosody(Runner& R, const ProsodyPlan& p, const ProsodyBufs& t, const float* wav, float* y) {
+    const int n = (int)p.segs.size();
+    R.begin("stretch");
+    if (p.smem_ints) launch_prosody_offsets(wav, t.segs, n, p.smem_ints, t.offsets, R.st);
+    launch_prosody_ola(wav, t.segs, n, p.max_ola, t.offsets, t.s, y, R.st);
+    R.count(p.stretch_flops, p.stretch_bytes, p.smem_ints ? 2 : 1);
+    R.end();
+    if (p.max_pitch == 0) return;
+    R.begin("pitch");
+    launch_prosody_pitch(wav, t.s, t.segs, n, p.max_pitch, y, R.st);
+    R.count(p.pitch_flops, p.pitch_bytes);
     R.end();
 }
 
@@ -999,14 +1071,16 @@ void Job::run(float* d_out, size_t d_out_cap) {
     // ---------------- frame level (phase 2) workspace ----------------
     // The stream is idle here, so the pinned staging of the X tables can be reused for the Y tables.
     lay_out_frames(*this, y_len, a.hop());
-    const ResamplePlan rp = lay_out_output(*this, a.hop());
+    const ProsodyPlan pp = lay_out_prosody(*this, a.hop());
+    const bool prosody = !pp.segs.empty();
+    const ResamplePlan rp = lay_out_output(*this, a.hop(), pp);
     const bool resample = !rp.segs.empty();
     const LoudnessPlan lp = lay_out_loudness(*this);
-    loud_ran.clear(); loud_lufs.clear(); loud_gain.clear();
+    loud_ran.clear(); loud_lufs.clear(); loud_gain.clear(); pros_ran.clear();
     FrameBufs f;
-    plan(C.dev_frame, C.pin, [&](Arena& dev, Arena& pin) { f.carve(dev, pin, *this, rp, lp, d_out == nullptr); });
+    plan(C.dev_frame, C.pin, [&](Arena& dev, Arena& pin) { f.carve(dev, pin, *this, pp, rp, lp, d_out == nullptr); });
     d_fsegs = f.y.fsegs;
-    d_osegs = resample ? f.rt.osegs : d_fsegs;
+    d_osegs = resample ? f.rt.osegs : prosody ? f.pr.osegs : d_fsegs;
     if (debug) {
         expose(*this, "z_p", f.zp, I, 1); expose(*this, "z", f.s, I, 1);
         // flow.{f}: z after the coupling layer of the graph's flow.flows.{2f} (f = flow_n - 1 first).  The graph's Flip
@@ -1016,6 +1090,7 @@ void Job::run(float* d_out, size_t d_out_cap) {
         if (!encode_only) f.dec.expose_to(*this);
     }
     Level LY = upload_frames(*this, f.y, st);
+    if (prosody) f.pr.upload(pp, st);
     if (resample) f.rt.upload(rp, st);
     if (!lp.segs.empty()) {
         std::copy(lp.segs.begin(), lp.segs.end(), f.ld.segs_h);
@@ -1075,16 +1150,24 @@ void Job::run(float* d_out, size_t d_out_cap) {
         if ((size_t)out_total > d_out_cap) throw Error(19, "caller-provided device output buffer is too small");
         d_wav = d_out;
     } else {
-        d_wav = f.rs ? f.rs : f.wav;
+        d_wav = f.rs ? f.rs : f.pr.y ? f.pr.y : f.wav;
     }
-    run_decoder(R, LY, f.y, f.dec, f.s, resample ? f.wav : d_wav);
-    if (resample) run_resample(R, rp, f.rt, f.wav, f.y.fsegs, f.rt.posts, a.hop(), d_wav);
+    run_decoder(R, LY, f.y, f.dec, f.s, resample || prosody ? f.wav : d_wav);
+    // the output stage: prosody on the decoder's waveform, the resample launch on what that left, loudness on the result
+    const float* staged = f.wav; const FrameSeg* staged_segs = f.y.fsegs; int staged_hop = a.hop();
+    if (prosody) {
+        float* py = resample ? f.pr.y : d_wav;
+        run_prosody(R, pp, f.pr, f.wav, py);
+        staged = py; staged_segs = f.pr.osegs; staged_hop = 1;
+    }
+    if (resample) run_resample(R, rp, f.rt, staged, staged_segs, f.rt.posts, staged_hop, d_wav);
     if (!lp.segs.empty()) run_loudness(R, lp, f.ld, d_wav);
     SB_CUDA(cudaEventRecord(C.ev_end, st));
     SB_CUDA(cudaStreamSynchronize(st));
     SB_CUDA(cudaGetLastError());
     SB_CUDA(cudaEventElapsedTime(&last_ms, C.ev_begin, C.ev_end));
     for (Region& r : regions) cudaEventElapsedTime(&r.ms, r.e0, r.e1);
+    pros_ran = pp.shapes;
     if (!lp.segs.empty()) {
         loud_ran = loud_target;
         loud_lufs.assign(f.ld.lufs_h, f.ld.lufs_h + B);

@@ -112,6 +112,28 @@ void loudness_design(long long rate, LoudSeg& s);
 // call fails naming the utterance.  Returns whether some utterance has a target.
 bool check_loudness_targets(const float* t, size_t B);
 
+// Pitch and tempo (prosody.cu).  What one utterance of n samples at `rate` becomes with its two ratios: the WSOLA
+// frame sizes (synthesis hop Hs = rate / 100, frame N = 2 Hs, search radius D = rate / 160), the stretch factor
+// alpha = pitch / tempo, the stretched length n1 = floor(n alpha + 0.5) in F = ceil(n1 / Hs) frames (stage skipped when
+// pitch == tempo: n1 = n, F = 0) and the delivered length n2 = floor(n1 / pitch + 0.5) (stage skipped when pitch is 1).
+struct ProsodyShape { int Hs, N, D, F; long long n1, n2; bool stretch, pitch; double alpha, p; };
+// NaN or 1 asks for nothing.  Throws OPERATION_ERROR for a rate without frame sizes or a result too long to index.
+ProsodyShape prosody_shape(int rate, long long n, float pitch, float tempo);
+// Checks pitch[0 .. B) and tempo[0 .. B) (either may be null): NaN or 1 is none, anything else must be finite and in
+// [0.5, 2] (pitch) or [0.25, 4] (tempo), or the call fails naming the utterance.  Returns whether some utterance asks.
+bool check_prosody(const float* pitch, const float* tempo, size_t B);
+// The three prosody launches over segments laid out back to back: each segment's ProsodySeg, the sizes of the offsets,
+// the stretched scratch and the output, what the launches are sized by and what the profile counts.
+struct ProsodyPlan {
+    std::vector<ProsodySeg> segs;
+    std::vector<ProsodyShape> shapes;
+    long long s_total = 0, y_total = 0, d_total = 0, max_ola = 0, max_pitch = 0, steps = 0;
+    int smem_ints = 0;
+    double stretch_flops = 0, stretch_bytes = 0, pitch_flops = 0, pitch_bytes = 0;
+    // Appends the segment wav[in_off, in_off + n) with shape `sh`.
+    void add(const ProsodyShape& sh, long long in_off, long long n);
+};
+
 struct Context;   // stream + arenas for one in-flight call
 
 struct Voice {
@@ -232,6 +254,9 @@ struct Job {
                                       // (set_job_output_rates)
     std::vector<float> loud_target;   // one LUFS target per utterance, NaN = none; empty when none has one
                                       // (set_job_loudness)
+    std::vector<float> pitch, tempo;  // one ratio per utterance each, NaN = none; both empty when no utterance asks
+                                      // (set_job_prosody)
+    std::vector<ProsodyShape> pros_ran;   // each utterance's shape in the last run (empty: it ran no prosody stage)
     // Loudness of the last run: the targets it ran with (empty: it measured nothing), each utterance's integrated
     // loudness and the gain applied to it
     std::vector<float> loud_ran; std::vector<double> loud_lufs; std::vector<float> loud_gain;
@@ -249,8 +274,8 @@ struct Job {
     FrameSeg* d_fsegs = nullptr;
     float* d_wav = nullptr;
     // What the job hands out: utterance b is d_wav[osegs[b].out_off ..) of osegs[b].len * out_hop samples, and
-    // d_osegs mirrors osegs on the device.  Without output rates these are fsegs, the hop and total_samples; with them,
-    // one segment of len = n_out per utterance at out_hop = 1.
+    // d_osegs mirrors osegs on the device.  Without prosody or output rates these are fsegs, the hop and total_samples;
+    // with either, one segment of len = its delivered samples per utterance at out_hop = 1.
     std::vector<FrameSeg> osegs; int out_hop = 1; long long out_total = 0;
     std::vector<int> osr;             // sample rate of each handed-out utterance
     FrameSeg* d_osegs = nullptr;
@@ -292,6 +317,10 @@ void set_job_output_rates(Job& j, const unsigned* rates);
 // every utterance is measured after the decoder and any resampling, and those with one are scaled to it; see
 // check_loudness_targets for the checks.  A bad entry leaves the job's targets as they were.
 void set_job_loudness(Job& j, const float* targets);
+// Per-utterance pitch and tempo ratios of the job's next run (each [0 .. B) or null; NaN or 1: none).  With a ratio, the
+// utterance's waveform is time-stretched and pitch-resampled right after the decoder, before any resampling and
+// loudness; see check_prosody for the checks.  A bad entry leaves the job's ratios as they were.
+void set_job_prosody(Job& j, const float* pitch, const float* tempo);
 // Frames per id of the job's last run, packed like its ids: one device->host copy of the batch's cum rows through the
 // context's page-locked staging, differenced on the host.  Cached until the next run.
 const std::vector<int>& job_id_frames(Job& j);

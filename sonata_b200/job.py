@@ -10,18 +10,20 @@ import numpy as np
 
 from . import _native as N
 from .core import G711_LAW, Audio, OperationError, check_encoding
-from .piper import (_check, _config_array, _duration_arrays, _gain_array, _loudness_array, _ptr, _rate_array,
-                    _seed_arrays, _take_audio, _take_bytes)
+from .piper import (_check, _config_array, _duration_arrays, _gain_array, _loudness_array, _prosody_arrays, _ptr,
+                    _rate_array, _seed_arrays, _take_audio, _take_bytes)
 
 
 class SynthesisJob:
     def __init__(self, model, batches: Sequence[Sequence[int]], eps_w: Optional[Sequence] = None,
                  eps_z: Optional[Sequence] = None, debug: bool = False, configs: Optional[Sequence] = None,
                  seeds: Optional[Sequence] = None, output_rates: Optional[Sequence] = None,
-                 loudness: Optional[Sequence] = None):
+                 loudness: Optional[Sequence] = None, pitches: Optional[Sequence] = None,
+                 tempos: Optional[Sequence] = None):
         """`configs`: one PiperSynthesisConfig per utterance (see set_configs); None keeps the voice's fallback config.
         `seeds`: noise seeds (see set_seeds).  `output_rates`: output sample rates (see set_output_rates).
-        `loudness`: loudness targets (see set_loudness)."""
+        `loudness`: loudness targets (see set_loudness).  `pitches` / `tempos`: pitch and tempo ratios (see
+        set_prosody)."""
         self._m = model
         self._lib = model._lib
         n = len(batches)
@@ -31,6 +33,7 @@ class SynthesisJob:
         _seed_arrays(seeds, n)
         _rate_array(output_rates, n)
         _loudness_array(loudness, n)
+        _prosody_arrays(pitches, tempos, n)
         packed = np.ascontiguousarray(np.concatenate([np.asarray(b, dtype=np.int64) for b in batches]))
         offs = np.zeros(n + 1, dtype=np.uint64)
         offs[1:] = np.cumsum([len(b) for b in batches])
@@ -69,6 +72,8 @@ class SynthesisJob:
             self.set_output_rates(output_rates)
         if loudness is not None:
             self.set_loudness(loudness)
+        if pitches is not None or tempos is not None:
+            self.set_prosody(pitches, tempos)
 
     def set_configs(self, configs: Optional[Sequence]) -> None:
         """Per-utterance PiperSynthesisConfigs for the next run, or None for the voice's fallback config.  A wrong
@@ -120,6 +125,26 @@ class SynthesisJob:
         err = N.sb200_error()
         _check(self._lib.sb200_job_loudness(self._h, _ptr(lufs, C.c_double), _ptr(gain, C.c_float), C.byref(err)), err)
         return lufs, gain
+
+    def set_prosody(self, pitches: Optional[Sequence] = None, tempos: Optional[Sequence] = None) -> None:
+        """Per-utterance pitch and tempo ratios for the next run (see VitsModel.infer_batch_with_values): a ratio or
+        None per utterance in each list; None for a whole list, or lists of None / NaN / 1.0, turn that control off.
+        After a run with ratios, fetch, fetch_i16, fetch_g711, fetch_flac, copy_out and the samples and offsets of
+        lengths all report the warped signal.  A bad entry raises OperationError naming the utterance and leaves the
+        job's ratios as they were."""
+        p, t = _prosody_arrays(pitches, tempos, self.batch)
+        err = N.sb200_error()
+        _check(self._lib.sb200_job_set_prosody(self._h, _ptr(p, C.c_float), _ptr(t, C.c_float), C.byref(err)), err)
+
+    def prosody(self) -> Tuple[np.ndarray, np.ndarray, np.ndarray]:
+        """(stretched length n1, delivered length before any output-rate resampling n2, WSOLA frames F) per utterance of
+        the last run, which must have had ratios."""
+        n1, n2 = np.zeros(self.batch, np.int64), np.zeros(self.batch, np.int64)
+        frames = np.zeros(self.batch, np.int32)
+        err = N.sb200_error()
+        _check(self._lib.sb200_job_prosody(self._h, _ptr(n1, C.c_int64), _ptr(n2, C.c_int64), _ptr(frames, C.c_int32),
+                                           C.byref(err)), err)
+        return n1, n2, frames
 
     def id_frames(self) -> List[np.ndarray]:
         """Frames per id of the last run, one int32 array per utterance (one device->host copy for the batch)."""

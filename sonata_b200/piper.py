@@ -179,6 +179,50 @@ def _loudness_array(targets, n: int):
     return None if np.isnan(out).all() else out
 
 
+PITCH_RANGE = (0.5, 2.0)     # pitch ratios a result can be shifted by
+TEMPO_RANGE = (0.25, 4.0)    # tempo ratios a result can be played at
+
+
+def _ratio_array(values, n: int, what: str, lo: float, hi: float):
+    if values is None:
+        return None
+    out = np.full(n, np.nan, np.float32)
+    for b, v in enumerate(_per_utterance(values, n, f"{what} ratios")):
+        if v is None:
+            continue
+        if isinstance(v, bool) or not isinstance(v, numbers.Real):
+            raise OperationError(f"utterance {b}: {what} ratio {v!r} is not a number")
+        if math.isnan(float(v)) or float(v) == 1.0:
+            continue
+        if not (math.isfinite(float(v)) and lo <= float(v) <= hi):
+            raise OperationError(f"utterance {b}: {what} ratio {float(v)} is not a finite value in [{lo}, {hi}]")
+        out[b] = float(v)
+    return None if np.isnan(out).all() else out
+
+
+def _prosody_arrays(pitches, tempos, n: int):
+    """The C images of per-utterance pitch and tempo ratios: (pitch f32, tempo f32), NaN for none, each None when not
+    given or when no utterance asks.  pitches[b] is a ratio in PITCH_RANGE, tempos[b] one in TEMPO_RANGE, or None / NaN /
+    1.0 for an utterance that keeps its samples."""
+    return _ratio_array(pitches, n, "pitch", *PITCH_RANGE), _ratio_array(tempos, n, "tempo", *TEMPO_RANGE)
+
+
+def _prosody_kwargs(pitches, tempos) -> dict:
+    out = {} if pitches is None else {"pitches": pitches}
+    if tempos is not None:
+        out["tempos"] = tempos
+    return out
+
+
+def refuse_prosody(pitch, tempo, where: str) -> None:
+    """OperationError when `where`, a mode that hands out a sentence chunk by chunk, is asked for a pitch or tempo
+    ratio."""
+    if any(a is not None for a in _prosody_arrays([pitch], [tempo], 1)):
+        raise OperationError(f"{where} cannot shift pitch or tempo: the time stretch walks a whole sentence frame by "
+                             "frame, and this mode hands out a sentence's first chunk before its last one is decoded "
+                             "(use the lazy, parallel or file modes, speak_batch or a SynthesisJob)")
+
+
 def _encoding_list(law, n: int) -> list:
     """One G.711 encoding ("mulaw" / "alaw") per utterance from `law`: one encoding for all, or one per utterance.  A bad
     entry raises OperationError naming the utterance."""
@@ -216,14 +260,19 @@ def _ptr(a, ctype):
 
 
 def _alignment(phonemes: str, src_char: Sequence[int], frames: Sequence[int], n_samples: int,
-               up: int = 1, down: int = 1) -> List[PhonemeAlignment]:
+               up: int = 1, down: int = 1, warped: bool = False) -> List[PhonemeAlignment]:
     """Groups per-id frame counts by the character each id came from: bos (`^`), one entry per kept character (its id
     and its pad) and eos (`$`), contiguous from sample 0.  An utterance whose ids all got 0 frames is still one frame
     long; that frame (after every id) goes to the last entry, so the entries always end at n_samples.  Audio resampled
-    by up/down puts the boundary after F frames at ceil(F * hop * up / down)."""
+    by up/down puts the boundary after F frames at ceil(F * hop * up / down).  `warped` (a pitch or tempo ratio changed
+    the length): the boundary after F of the utterance's T frames is at floor(F * n_samples / T + 0.5), whatever the
+    output rate; the time stretch moves a sample by at most D = rate // 160 input samples from that linear map, so a
+    boundary is accurate to within D / tempo samples of the warped signal."""
     total = int(sum(int(f) for f in frames))
     hop = n_samples // max(total, 1) if (up, down) == (1, 1) else HOP
     at = lambda frames_before: -((-frames_before * hop * up) // down)
+    if warped:
+        at = lambda frames_before: (2 * frames_before * n_samples + max(total, 1)) // (2 * max(total, 1))
     out: List[PhonemeAlignment] = []
     start, i, fsum = 0, 0, 0
     while i < len(frames):
@@ -410,20 +459,24 @@ class _VitsCommons:
 
     def speak_batch(self, phoneme_batches: Sequence[str],
                     configs: Optional[Sequence[PiperSynthesisConfig]] = None, seeds: Optional[Sequence] = None,
-                    output_rates: Optional[Sequence] = None, loudness: Optional[Sequence] = None) -> List[Audio]:
+                    output_rates: Optional[Sequence] = None, loudness: Optional[Sequence] = None,
+                    pitches: Optional[Sequence] = None, tempos: Optional[Sequence] = None) -> List[Audio]:
         """`configs`: one PiperSynthesisConfig per utterance (speaker and scales), still synthesised as one pass;
         None uses the fallback config for every utterance.  `seeds`: noise seeds as for infer_batch_with_values.
-        `output_rates` / `loudness`: per-utterance output sample rates / loudness targets as for
-        infer_batch_with_values."""
+        `output_rates` / `loudness` / `pitches` / `tempos`: per-utterance output sample rates, loudness targets and
+        pitch and tempo ratios as for infer_batch_with_values."""
         n = len(phoneme_batches)
         _config_array(configs, n)             # argument errors before any id mapping
         sv, _ = _seed_arrays(seeds, n)
         rates = _rate_array(output_rates, n)
         loud = _loudness_array(loudness, n)
+        pros = any(a is not None for a in _prosody_arrays(pitches, tempos, n))
         if n == 0:
             return []
-        if configs is not None or sv is not None or rates is not None or loud is not None:
+        if configs is not None or sv is not None or rates is not None or loud is not None or pros:
             extra = {} if sv is None else {"seeds": seeds}
+            if pros:
+                extra.update(_prosody_kwargs(pitches, tempos))
             if rates is not None:
                 extra["output_rates"] = output_rates
             if loud is not None:
@@ -448,7 +501,8 @@ class _VitsCommons:
                                 configs: Optional[Sequence[PiperSynthesisConfig]] = None,
                                 seeds: Optional[Sequence] = None,
                                 output_rates: Optional[Sequence] = None,
-                                loudness: Optional[Sequence] = None) -> List[Audio]:
+                                loudness: Optional[Sequence] = None, pitches: Optional[Sequence] = None,
+                                tempos: Optional[Sequence] = None) -> List[Audio]:
         """Batched infer_with_values.  `configs`: one PiperSynthesisConfig per utterance (speaker and scales), or None
         for the fallback config; each utterance's result equals a single-utterance call with its config as the
         fallback, except for the on-device noise of an unseeded utterance, whose draws depend on the batch position.
@@ -464,15 +518,24 @@ class _VitsCommons:
         `loudness`: one target integrated loudness per utterance in LUFS (finite, in [-70, 0]) or None.  The delivered
         signal (after any resampling) is measured on the device as ITU-R BS.1770-4 defines it and scaled to the target,
         never past a sample peak of 1.0; an utterance under 400 ms or silent keeps its samples, as does one whose target
-        is None (see include/sonata_b200.h, sb200_speak_batch_ids_loudness)."""
+        is None (see include/sonata_b200.h, sb200_speak_batch_ids_loudness).
+
+        `pitches` / `tempos`: one ratio per utterance, or None.  A pitch p in PITCH_RANGE multiplies every frequency of
+        the utterance and keeps its duration; a tempo t in TEMPO_RANGE plays it t times faster at the same pitch (about
+        len / t samples), keeping the model's articulation where a small length_scale would ask the duration predictor
+        for durations it never saw.  Both are signal processing on the decoder's waveform on the device (WSOLA, then a
+        windowed-sinc resampler; sb200_speak_batch_ids_prosody), before any resampling and loudness; None, NaN or 1.0
+        leaves the utterance's samples as they are, bit for bit."""
         n = len(batches)
         cfgs = _config_array(configs, n)
         sv, _ = _seed_arrays(seeds, n)
         rates = _rate_array(output_rates, n)
         loud = _loudness_array(loudness, n)
-        if sv is not None or rates is not None or loud is not None:
+        pros = any(a is not None for a in _prosody_arrays(pitches, tempos, n))
+        if sv is not None or rates is not None or loud is not None or pros:
             return [a for a, _ in self.infer_batch_with_durations(batches, configs, seeds=seeds,
-                                                                  output_rates=output_rates, loudness=loudness)]
+                                                                  output_rates=output_rates, loudness=loudness,
+                                                                  **(_prosody_kwargs(pitches, tempos) if pros else {}))]
         packed = np.ascontiguousarray(np.concatenate([np.asarray(b, dtype=np.int64) for b in batches]))
         offs = np.zeros(n + 1, dtype=np.uint64)
         offs[1:] = np.cumsum([len(b) for b in batches])
@@ -489,7 +552,8 @@ class _VitsCommons:
                                    durations: Optional[Sequence] = None,
                                    seeds: Optional[Sequence] = None,
                                    output_rates: Optional[Sequence] = None,
-                                   loudness: Optional[Sequence] = None) -> List[Tuple[Audio, np.ndarray]]:
+                                   loudness: Optional[Sequence] = None, pitches: Optional[Sequence] = None,
+                                   tempos: Optional[Sequence] = None) -> List[Tuple[Audio, np.ndarray]]:
         """infer_batch_with_values with per-id duration control, returning (audio, frames per id) per utterance.
 
         duration_scales[b]: one scale (finite, >= 0) per id of utterance b, applied before the duration's ceil, so 1.0
@@ -497,7 +561,8 @@ class _VitsCommons:
         Either list, or any of its entries, may be None.  The frame counts times 256 are each id's samples; an
         utterance whose ids all got 0 frames is still one frame long.  `seeds`: as for infer_batch_with_values; a
         seeded frame's noise depends on its index only, so controls that move frames never reshuffle it.
-        `output_rates` / `loudness`: as for infer_batch_with_values (the frame counts stay frame counts)."""
+        `output_rates` / `loudness` / `pitches` / `tempos`: as for infer_batch_with_values (the frame counts stay frame
+        counts of the utterance before any warp)."""
         n = len(batches)
         cfgs = _config_array(configs, n)
         lens = [len(b) for b in batches]
@@ -505,6 +570,7 @@ class _VitsCommons:
         sv, sf = _seed_arrays(seeds, n)
         rates = _rate_array(output_rates, n)
         loud = _loudness_array(loudness, n)
+        pit, tem = _prosody_arrays(pitches, tempos, n)
         if n == 0:
             return []
         if any(x == 0 for x in lens):
@@ -515,11 +581,11 @@ class _VitsCommons:
         outs = (N.sb200_audio * n)()
         id_frames = np.zeros(int(offs[-1]), np.int32)
         err = N.sb200_error()
-        _check(self._lib.sb200_speak_batch_ids_loudness(
+        _check(self._lib.sb200_speak_batch_ids_prosody(
             self._h, packed.ctypes.data_as(C.POINTER(C.c_int64)), offs.ctypes.data_as(C.POINTER(C.c_size_t)), n, cfgs,
             _ptr(scales, C.c_float), _ptr(frames, C.c_int32), _ptr(sv, C.c_uint64), _ptr(sf, C.c_int32),
-            _ptr(rates, C.c_uint32), _ptr(loud, C.c_float), outs, _ptr(id_frames, C.c_int32), None, None,
-            C.byref(err)), err)
+            _ptr(rates, C.c_uint32), _ptr(loud, C.c_float), _ptr(pit, C.c_float), _ptr(tem, C.c_float), outs,
+            _ptr(id_frames, C.c_int32), None, None, C.byref(err)), err)
         return [(_take_audio(outs[b]), id_frames[int(offs[b]):int(offs[b + 1])].copy()) for b in range(n)]
 
     def speak_batch_with_alignment(self, phoneme_batches: Sequence[str],
@@ -527,7 +593,8 @@ class _VitsCommons:
                                    duration_scales: Optional[Sequence] = None,
                                    seeds: Optional[Sequence] = None,
                                    output_rates: Optional[Sequence] = None,
-                                   loudness: Optional[Sequence] = None) -> List[Tuple[Audio, List[PhonemeAlignment]]]:
+                                   loudness: Optional[Sequence] = None, pitches: Optional[Sequence] = None,
+                                   tempos: Optional[Sequence] = None) -> List[Tuple[Audio, List[PhonemeAlignment]]]:
         """speak_batch that also says when each phoneme is spoken: per utterance (audio, alignment), the alignment
         holding one entry for bos (`^`), one per kept phoneme character (its id and its trailing pad) and one for eos
         (`$`), contiguous from sample 0 to len(audio).
@@ -536,12 +603,18 @@ class _VitsCommons:
         pad; characters the voice drops have no entry and their scales are ignored.  `seeds`: as for
         infer_batch_with_values.  `output_rates`: as for infer_batch_with_values; the alignment is then in samples of
         the output rate, the boundary after F frames at ceil(F * 256 * up / down).  `loudness`: as for
-        infer_batch_with_values; it scales samples and moves no boundary."""
+        infer_batch_with_values; it scales samples and moves no boundary.  `pitches` / `tempos`: as for
+        infer_batch_with_values; an utterance with a ratio has every boundary scaled by delivered / original length
+        (floor(F * len(audio) / T + 0.5) after F of its T frames), accurate to within (rate // 160) / tempo samples of
+        the warped signal because the time stretch takes each frame from within that many samples of the linear map."""
         n = len(phoneme_batches)
         _config_array(configs, n)
         _seed_arrays(seeds, n)
         _rate_array(output_rates, n)
         _loudness_array(loudness, n)
+        pit, tem = _prosody_arrays(pitches, tempos, n)
+        warped = [(pit is not None and not np.isnan(pit[b])) or (tem is not None and not np.isnan(tem[b]))
+                  for b in range(n)]
         per_char = None if duration_scales is None else _per_utterance(duration_scales, n, "duration scales")
         maps = [self.phonemes_to_input_ids_map(p) for p in phoneme_batches]
         id_scales = None
@@ -562,22 +635,26 @@ class _VitsCommons:
             extra["output_rates"] = output_rates
         if loudness is not None:
             extra["loudness"] = loudness
+        if any(warped):
+            extra.update(_prosody_kwargs(pitches, tempos))
         res = self.infer_batch_with_durations([m[0] for m in maps], configs, id_scales, **extra)
         voice_rate = self.audio_output_info().sample_rate if output_rates is not None else None
         ratio = lambda audio: (1, 1) if voice_rate is None else rate_ratio(voice_rate, audio.info.sample_rate)
-        return [(audio, _alignment(ph, src, frames, len(audio), *ratio(audio)))
-                for ph, (_, src), (audio, frames) in zip(phoneme_batches, maps, res)]
+        return [(audio, _alignment(ph, src, frames, len(audio), *ratio(audio), warped=w))
+                for ph, (_, src), (audio, frames), w in zip(phoneme_batches, maps, res, warped)]
 
     def infer_batch_g711(self, batches: Sequence[Sequence[int]], law,
                          configs: Optional[Sequence[PiperSynthesisConfig]] = None, seeds: Optional[Sequence] = None,
                          output_rates: Optional[Sequence] = None, loudness: Optional[Sequence] = None,
-                         gains: Optional[Sequence] = None) -> List[bytes]:
+                         gains: Optional[Sequence] = None, pitches: Optional[Sequence] = None,
+                         tempos: Optional[Sequence] = None) -> List[bytes]:
         """infer_batch_with_values delivered as G.711 telephony audio: one `bytes` per utterance, one byte per sample.
         `law`: "mulaw" (PCMU) or "alaw" (PCMA), or one of those per utterance.  The bytes are G.711 of exactly the
         16-bit samples the i16 route gives (SynthesisJob.fetch_i16): to_i16_vec of the utterance after gains[b] (None:
         1), or the fixed scale for an utterance with a loudness target.  They are encoded on the device in the i16
         conversion's launches, so only one byte per sample leaves the card.  `configs`, `seeds`, `output_rates` and
-        `loudness` as for infer_batch_with_values; a batch mixing laws runs one conversion per law."""
+        `loudness` as for infer_batch_with_values, and so are `pitches` and `tempos`; a batch mixing laws runs one
+        conversion per law."""
         from .job import SynthesisJob
         n = len(batches)
         _config_array(configs, n)
@@ -586,11 +663,13 @@ class _VitsCommons:
         _loudness_array(loudness, n)
         laws = _encoding_list(law, n)
         _gain_array(gains, n)
+        _prosody_arrays(pitches, tempos, n)
         if n == 0:
             return []
         if any(len(b) == 0 for b in batches):
             raise OperationError("Failed to run model inference. Error: empty input sequence")
-        job = SynthesisJob(self, batches, configs=configs, seeds=seeds, output_rates=output_rates, loudness=loudness)
+        job = SynthesisJob(self, batches, configs=configs, seeds=seeds, output_rates=output_rates, loudness=loudness,
+                           pitches=pitches, tempos=tempos)
         try:
             job.run()
             out: List[Optional[bytes]] = [None] * n
@@ -606,23 +685,25 @@ class _VitsCommons:
     def speak_batch_g711(self, phoneme_batches: Sequence[str], law,
                          configs: Optional[Sequence[PiperSynthesisConfig]] = None, seeds: Optional[Sequence] = None,
                          output_rates: Optional[Sequence] = None, loudness: Optional[Sequence] = None,
-                         gains: Optional[Sequence] = None) -> List[bytes]:
+                         gains: Optional[Sequence] = None, pitches: Optional[Sequence] = None,
+                         tempos: Optional[Sequence] = None) -> List[bytes]:
         """speak_batch delivered as G.711 bytes: infer_batch_g711 over the phonemes' ids."""
         n = len(phoneme_batches)
         _config_array(configs, n)
         _encoding_list(law, n)
         return self.infer_batch_g711([self.phonemes_to_input_ids(p) for p in phoneme_batches], law, configs, seeds,
-                                     output_rates, loudness, gains)
+                                     output_rates, loudness, gains, pitches, tempos)
 
     def infer_batch_flac(self, batches: Sequence[Sequence[int]],
                          configs: Optional[Sequence[PiperSynthesisConfig]] = None, seeds: Optional[Sequence] = None,
                          output_rates: Optional[Sequence] = None, loudness: Optional[Sequence] = None,
-                         gains: Optional[Sequence] = None) -> List[bytes]:
+                         gains: Optional[Sequence] = None, pitches: Optional[Sequence] = None,
+                         tempos: Optional[Sequence] = None) -> List[bytes]:
         """infer_batch_with_values delivered as lossless FLAC: one complete stream (`bytes`) per utterance.  Its samples
         are exactly the 16-bit samples the i16 route gives (SynthesisJob.fetch_i16): to_i16_vec of the utterance after
         gains[b] (None: 1), or the fixed scale for an utterance with a loudness target, at its delivered rate.  They are
-        encoded on the device, and only the compressed bytes leave the card.  `configs`, `seeds`, `output_rates` and
-        `loudness` as for infer_batch_with_values."""
+        encoded on the device, and only the compressed bytes leave the card.  `configs`, `seeds`, `output_rates`,
+        `loudness`, `pitches` and `tempos` as for infer_batch_with_values."""
         from .job import SynthesisJob
         n = len(batches)
         _config_array(configs, n)
@@ -630,11 +711,13 @@ class _VitsCommons:
         _rate_array(output_rates, n)
         _loudness_array(loudness, n)
         _gain_array(gains, n)
+        _prosody_arrays(pitches, tempos, n)
         if n == 0:
             return []
         if any(len(b) == 0 for b in batches):
             raise OperationError("Failed to run model inference. Error: empty input sequence")
-        job = SynthesisJob(self, batches, configs=configs, seeds=seeds, output_rates=output_rates, loudness=loudness)
+        job = SynthesisJob(self, batches, configs=configs, seeds=seeds, output_rates=output_rates, loudness=loudness,
+                           pitches=pitches, tempos=tempos)
         try:
             job.run()
             return job.fetch_flac(gains)
@@ -644,11 +727,12 @@ class _VitsCommons:
     def speak_batch_flac(self, phoneme_batches: Sequence[str],
                          configs: Optional[Sequence[PiperSynthesisConfig]] = None, seeds: Optional[Sequence] = None,
                          output_rates: Optional[Sequence] = None, loudness: Optional[Sequence] = None,
-                         gains: Optional[Sequence] = None) -> List[bytes]:
+                         gains: Optional[Sequence] = None, pitches: Optional[Sequence] = None,
+                         tempos: Optional[Sequence] = None) -> List[bytes]:
         """speak_batch delivered as FLAC streams: infer_batch_flac over the phonemes' ids."""
         _config_array(configs, len(phoneme_batches))
         return self.infer_batch_flac([self.phonemes_to_input_ids(p) for p in phoneme_batches], configs, seeds,
-                                     output_rates, loudness, gains)
+                                     output_rates, loudness, gains, pitches, tempos)
 
     def _cfg(self, fn) -> PiperSynthesisConfig:
         c, err = N.sb200_synth_config(), N.sb200_error()
@@ -939,11 +1023,14 @@ class VitsStreamingModel(_VitsCommons):
 
     def stream_synthesis(self, phonemes: str, chunk_size: int, chunk_padding: int,
                          seed: Optional[int] = None, output_rate: Optional[int] = None,
-                         encoding: Optional[str] = None, gain: Optional[float] = None) -> SpeechStreamer:
+                         encoding: Optional[str] = None, gain: Optional[float] = None,
+                         pitch: Optional[float] = None, tempo: Optional[float] = None) -> SpeechStreamer:
         """`seed`: the sentence's noise seed (see infer_batch_with_values), or None for positional noise.
         `output_rate`: the chunks' sample rate (see infer_batch_with_values), the sentence resampled as one stream.
         `encoding`: "mulaw" / "alaw" for chunks of G.711 `bytes`: each is G.711 of to_i16_vec of the chunk the stream
-        yields without an encoding, after the linear `gain` (None: 1; encoded streams only), encoded on the device."""
+        yields without an encoding, after the linear `gain` (None: 1; encoded streams only), encoded on the device.
+        `pitch` / `tempo`: ratios as for infer_batch_with_values, refused here unless neutral (refuse_prosody)."""
+        refuse_prosody(pitch, tempo, "stream_synthesis")
         _seed_arrays([seed], 1)
         _rate_array([output_rate], 1)
         refuse_flac(encoding, "stream_synthesis")
@@ -1021,10 +1108,13 @@ class StreamBatch:
         self._next_key = 0
 
     def add(self, ids_or_phonemes, config: Optional[PiperSynthesisConfig] = None, seed: Optional[int] = None,
-            output_rate: Optional[int] = None, encoding: Optional[str] = None, gain: Optional[float] = None) -> int:
+            output_rate: Optional[int] = None, encoding: Optional[str] = None, gain: Optional[float] = None,
+            pitch: Optional[float] = None, tempo: Optional[float] = None) -> int:
         """`seed`: the stream's noise seed (see infer_batch_with_values); a seeded stream yields what
         `stream_synthesis(..., seed=seed)` yields, whatever other streams share its encoder pass.  `output_rate`,
-        `encoding` and `gain`: the stream's sample rate and G.711 encoding, as for stream_synthesis."""
+        `encoding` and `gain`: the stream's sample rate and G.711 encoding, as for stream_synthesis; `pitch` / `tempo`
+        are refused unless neutral, as there."""
+        refuse_prosody(pitch, tempo, "StreamBatch")
         return self._add(ids_or_phonemes, config, self.chunk_size, seed, output_rate, encoding, gain)
 
     def _add(self, ids_or_phonemes, config, chunk_size: int, seed: Optional[int] = None,

@@ -12,6 +12,9 @@
 `AudioOutputConfig` (rate / volume / pitch through Sonic, appended silence) is CPU post-processing after
 the path (SURVEY §2 row 7, out of scope): appended silence and volume are honoured (pure sample
 arithmetic); a non-neutral rate or pitch raises OperationError instead of silently being ignored.
+Sonic's percent controls stay out of scope; pitch and tempo exist as ratio controls instead, the
+`pitch_ratio=` and `tempo=` keywords of the lazy, parallel and file modes, which run on the GPU
+(`VitsModel.infer_batch_with_values`).  How the percent scale would map onto them is undecided.
 The model argument is anything with the `SonataModel` surface (`sonata_b200.VitsModel`, or a fake in
 the CPU tests) — like the reference's `Arc<dyn SonataModel + Send + Sync>`.
 """
@@ -112,6 +115,22 @@ def _check_loudness(target) -> None:
     _loudness_array([target], 1)
 
 
+def _check_prosody(pitch_ratio, tempo) -> None:
+    """Raises OperationError unless each is None or a ratio in piper.PITCH_RANGE / piper.TEMPO_RANGE."""
+    from .piper import _prosody_arrays
+    _prosody_arrays([pitch_ratio], [tempo], 1)
+
+
+def _prosody_extra(n: int, pitch_ratio, tempo) -> dict:
+    """The per-utterance keywords of n sentences that share a request's pitch ratio and tempo ({} without either)."""
+    from .piper import _prosody_arrays
+    p, t = _prosody_arrays([pitch_ratio], [tempo], 1)
+    out = {} if p is None else {"pitches": [pitch_ratio] * n}
+    if t is not None:
+        out["tempos"] = [tempo] * n
+    return out
+
+
 def _device_g711(model) -> bool:
     """Whether `model` encodes G.711 on the device (VitsModel / VitsStreamingModel).  Other SonataModels (fakes in
     tests) get the host definition, AudioSamples.as_g711_bytes, of the audio they return."""
@@ -148,10 +167,12 @@ class SonataSpeechSynthesizer:
     # `encoding` (every mode): "mulaw" / "alaw" hands out G.711 `bytes` instead of Audio / AudioSamples: G.711 of the
     # 16-bit samples of what the mode hands out without it (to_i16_vec per sentence or chunk, or the fixed scale with a
     # loudness target), the output config's volume applied on the device as a gain before the conversion and its
-    # silence appended as code-of-zero bytes.
+    # silence appended as code-of-zero bytes.  `pitch_ratio` / `tempo` (lazy, parallel and file modes): each sentence's
+    # frequencies multiplied by the ratio at the same duration / played that many times faster at the same pitch, on
+    # the device before any resampling and loudness (piper.PITCH_RANGE, piper.TEMPO_RANGE).
 
     def _g711_batch(self, phs: List[str], encoding: str, seeds, output_rate, loudness,
-                    cfg: Optional[AudioOutputConfig]) -> List[bytes]:
+                    cfg: Optional[AudioOutputConfig], pitch_ratio=None, tempo=None) -> List[bytes]:
         """The G.711 bytes of sentences `phs`, one synthesis pass, each followed by its appended silence."""
         if cfg is not None:
             cfg._check_supported()
@@ -161,6 +182,7 @@ class SonataSpeechSynthesizer:
             extra["output_rates"] = [output_rate] * n
         if loudness is not None:
             extra["loudness"] = [loudness] * n
+        extra.update(_prosody_extra(n, pitch_ratio, tempo))
         if not _device_g711(self.model):
             res = self.model.speak_batch(phs, **extra) if extra else self.model.speak_batch(phs)
             return [self._process(a, cfg).samples.as_g711_bytes(encoding, fixed_scale=loudness is not None)
@@ -176,19 +198,22 @@ class SonataSpeechSynthesizer:
 
     def synthesize_lazy(self, text: str, output_config: Optional[AudioOutputConfig] = None,
                         seed: Optional[int] = None, output_rate: Optional[int] = None,
-                        loudness: Optional[float] = None, encoding: Optional[str] = None) -> Iterator[Audio]:
+                        loudness: Optional[float] = None, encoding: Optional[str] = None,
+                        pitch_ratio: Optional[float] = None, tempo: Optional[float] = None) -> Iterator[Audio]:
         sentence_seed(seed, 0)
         _check_output_rate(output_rate)
         _check_loudness(loudness)
+        _check_prosody(pitch_ratio, tempo)
         refuse_flac(encoding, "synthesize_lazy")
         check_encoding(encoding)
+        pros = _prosody_extra(1, pitch_ratio, tempo)
         for i, ph in enumerate(self._phonemes(text)):
             if encoding is not None:
                 yield self._g711_batch([ph], encoding, None if seed is None else [sentence_seed(seed, i)], output_rate,
-                                       loudness, output_config)[0]
+                                       loudness, output_config, pitch_ratio, tempo)[0]
                 continue
-            if output_rate or loudness is not None:
-                extra = {} if seed is None else {"seeds": [sentence_seed(seed, i)]}
+            if output_rate or loudness is not None or pros:
+                extra = dict(pros) if seed is None else dict(pros, seeds=[sentence_seed(seed, i)])
                 if output_rate:
                     extra["output_rates"] = [output_rate]
                 if loudness is not None:
@@ -201,17 +226,21 @@ class SonataSpeechSynthesizer:
 
     def synthesize_parallel(self, text: str, output_config: Optional[AudioOutputConfig] = None,
                             seed: Optional[int] = None, output_rate: Optional[int] = None,
-                            loudness: Optional[float] = None, encoding: Optional[str] = None) -> Iterator[Audio]:
+                            loudness: Optional[float] = None, encoding: Optional[str] = None,
+                            pitch_ratio: Optional[float] = None, tempo: Optional[float] = None) -> Iterator[Audio]:
         sentence_seed(seed, 0)
         _check_output_rate(output_rate)
         _check_loudness(loudness)
+        _check_prosody(pitch_ratio, tempo)
         refuse_flac(encoding, "synthesize_parallel")
         check_encoding(encoding)
         ph = self._phonemes(text)
         if encoding is not None:
             seeds = None if seed is None else [sentence_seed(seed, i) for i in range(len(ph))]
-            return iter(self._g711_batch(ph, encoding, seeds, output_rate, loudness, output_config) if ph else [])
+            return iter(self._g711_batch(ph, encoding, seeds, output_rate, loudness, output_config, pitch_ratio, tempo)
+                        if ph else [])
         extra = {"output_rates": [output_rate] * len(ph)} if output_rate else {}
+        extra.update(_prosody_extra(len(ph), pitch_ratio, tempo))
         if loudness is not None:
             extra["loudness"] = [loudness] * len(ph)
         if not ph:
@@ -225,11 +254,15 @@ class SonataSpeechSynthesizer:
     def synthesize_streamed(self, text: str, output_config: Optional[AudioOutputConfig] = None,
                             chunk_size: int = 72, chunk_padding: int = 3,
                             seed: Optional[int] = None, output_rate: Optional[int] = None,
-                            encoding: Optional[str] = None) -> Iterator[AudioSamples]:
+                            encoding: Optional[str] = None, pitch_ratio: Optional[float] = None,
+                            tempo: Optional[float] = None) -> Iterator[AudioSamples]:
         """RealtimeSpeechStream (:337-382): a background producer pushes chunks into an unbounded channel;
         chunk_size is multiplied by the number of chunks already produced for every following sentence.
         `output_rate`: each sentence is resampled as its own stream (zero history at its start, flushed at its end).
-        `encoding`: every chunk is G.711 bytes of its to_i16_vec after the volume, encoded on the device."""
+        `encoding`: every chunk is G.711 bytes of its to_i16_vec after the volume, encoded on the device.
+        `pitch_ratio` / `tempo`: refused here unless neutral (see piper.refuse_prosody)."""
+        from .piper import refuse_prosody
+        refuse_prosody(pitch_ratio, tempo, "synthesize_streamed")
         sentence_seed(seed, 0)
         _check_output_rate(output_rate)
         refuse_flac(encoding, "synthesize_streamed")
@@ -282,20 +315,26 @@ class SonataSpeechSynthesizer:
 
     def synthesize_to_file(self, filename, text: str, output_config: Optional[AudioOutputConfig] = None,
                            seed: Optional[int] = None, output_rate: Optional[int] = None,
-                           loudness: Optional[float] = None, encoding: Optional[str] = None) -> None:
+                           loudness: Optional[float] = None, encoding: Optional[str] = None,
+                           pitch_ratio: Optional[float] = None, tempo: Optional[float] = None) -> None:
         """:168-198 — parallel mode, concatenated, peak-normalised i16 WAV (at output_rate when given).  With
         `loudness` the WAV is written at the fixed scale (trunc(clamp(x * 32767))), so it keeps the sentences' level.
         With `encoding` the WAV is 8-bit G.711 (WAVE_FORMAT_MULAW / _ALAW, with a `fact` chunk) holding the sentences'
         bytes as synthesize_parallel hands them out: each sentence converted at its own peak (or the fixed scale).
         With encoding="flac" the file is one FLAC stream (synthesize_flac) instead of a WAV."""
         if isinstance(encoding, str) and encoding == FLAC:
-            data = self.synthesize_flac(text, output_config, seed=seed, output_rate=output_rate, loudness=loudness)
+            data = self.synthesize_flac(text, output_config, seed=seed, output_rate=output_rate, loudness=loudness,
+                                        pitch_ratio=pitch_ratio, tempo=tempo)
             with open(filename, "wb") as f:
                 f.write(data)
             return
         extra = {"output_rate": output_rate} if output_rate else {}
         if loudness is not None:
             extra["loudness"] = loudness
+        if pitch_ratio is not None:
+            extra["pitch_ratio"] = pitch_ratio
+        if tempo is not None:
+            extra["tempo"] = tempo
         if check_encoding(encoding) is not None:
             data = b"".join(self.synthesize_parallel(text, output_config, seed=seed, encoding=encoding, **extra))
             if not data:
@@ -303,14 +342,19 @@ class SonataSpeechSynthesizer:
             with open(filename, "wb") as f:
                 f.write(g711_wave_bytes(data, encoding, output_rate or self.model.audio_output_info().sample_rate))
             return
-        self._document(text, output_config, seed, output_rate, loudness).save_to_file(filename,
-                                                                                       fixed_scale=loudness is not None)
+        self._document(text, output_config, seed, output_rate, loudness, pitch_ratio, tempo).save_to_file(
+            filename, fixed_scale=loudness is not None)
 
-    def _document(self, text: str, output_config: Optional[AudioOutputConfig], seed, output_rate, loudness) -> Audio:
+    def _document(self, text: str, output_config: Optional[AudioOutputConfig], seed, output_rate, loudness,
+                  pitch_ratio=None, tempo=None) -> Audio:
         """The sentences of synthesize_parallel concatenated: what synthesize_to_file writes as a WAV."""
         extra = {"output_rate": output_rate} if output_rate else {}
         if loudness is not None:
             extra["loudness"] = loudness
+        if pitch_ratio is not None:
+            extra["pitch_ratio"] = pitch_ratio
+        if tempo is not None:
+            extra["tempo"] = tempo
         parts = [a.samples.as_slice() for a in self.synthesize_parallel(text, output_config, seed=seed, **extra)]
         if not parts or sum(len(p) for p in parts) == 0:
             raise OperationError("No speech data to write")
@@ -319,11 +363,12 @@ class SonataSpeechSynthesizer:
 
     def synthesize_flac(self, text: str, output_config: Optional[AudioOutputConfig] = None,
                         seed: Optional[int] = None, output_rate: Optional[int] = None,
-                        loudness: Optional[float] = None) -> bytes:
+                        loudness: Optional[float] = None, pitch_ratio: Optional[float] = None,
+                        tempo: Optional[float] = None) -> bytes:
         """The FLAC file synthesize_to_file(..., encoding="flac") writes: one stream whose decoded samples are exactly
         the 16-bit samples of the WAV the same call writes without an encoding (the concatenation at the document's
         peak, or the fixed scale with `loudness`), encoded on the model's device by flac_encode."""
-        doc = self._document(text, output_config, seed, output_rate, loudness)
+        doc = self._document(text, output_config, seed, output_rate, loudness, pitch_ratio, tempo)
         s = doc.samples
         return flac_encode(s.to_i16_fixed() if loudness is not None else s.to_i16_vec(), doc.info.sample_rate,
                            getattr(self.model, "device", 0))
@@ -367,10 +412,12 @@ class RealtimeBatch:
         self._next_key = 0
 
     def add(self, text: str, output_config: Optional[AudioOutputConfig] = None, config=None,
-            seed: Optional[int] = None, output_rate: Optional[int] = None, encoding: Optional[str] = None) -> int:
+            seed: Optional[int] = None, output_rate: Optional[int] = None, encoding: Optional[str] = None,
+            pitch_ratio: Optional[float] = None, tempo: Optional[float] = None) -> int:
         """`seed`: the request's noise seed, `output_rate` its sample rate and `encoding` its G.711 encoding, as for
-        synthesize_streamed."""
-        from .piper import PiperSynthesisConfig
+        synthesize_streamed; `pitch_ratio` / `tempo` are refused unless neutral, as there."""
+        from .piper import PiperSynthesisConfig, refuse_prosody
+        refuse_prosody(pitch_ratio, tempo, "RealtimeBatch")
         sentence_seed(seed, 0)
         _check_output_rate(output_rate)
         refuse_flac(encoding, "RealtimeBatch")
