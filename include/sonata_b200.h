@@ -421,6 +421,40 @@ int32_t sb200_decode_chunks_resampled(sb200_voice* v, const sb200_latent* const*
                                       int32_t fade, const float* gain, sb200_resampler* const* resamplers,
                                       const int32_t* last, int32_t format, void** outs, size_t* lens, sb200_error* err);
 
+/* ---- streams with a pitch and a tempo (see sb200_speak_batch_ids_prosody) ----
+ * A prosody stream is one stream's pitch / tempo state on the device: the tail of its input the WSOLA search and the
+ * overlap-add still read (fewer than max(ceil(2 Hs / alpha), Hs) + 2 D + N samples), the tail of the stretched signal
+ * the pitch resampler still reads (at most 2 W + 4 samples, W = 16 max(1, pitch) <= 32), the deltas of its last two
+ * frames, and its counts.  pitch in [0.5, 2] and tempo in [0.25, 4] as for the batch calls (NaN or 1: none); neutral
+ * ratios, or ratios out of range, fail with OPERATION_ERROR.  It shares ownership of the voice. */
+typedef struct sb200_prosody_stream sb200_prosody_stream;
+int32_t sb200_prosody_stream_create(sb200_voice* v, float pitch, float tempo, sb200_prosody_stream** out,
+                                    sb200_error* err);
+void sb200_prosody_stream_free(sb200_prosody_stream* s);
+/* The "stretch" and "pitch" device time (ms) of the last chunk pass the stream was in (0: none ran). */
+int32_t sb200_prosody_stream_profile(const sb200_prosody_stream* s, float* stretch_ms, float* pitch_ms);
+/* sb200_decode_chunks_resampled with a prosody stream per chunk, warps[k] (NULL: none; warps NULL: none at all, which
+ * is sb200_decode_chunks_resampled bit for bit).  Chunk k's samples after the post-path (trims, crossfade(fade) and,
+ * except for G.711, gain[k]) are appended to warps[k]; what it emits then goes to resamplers[k] (or leaves at the
+ * voice's rate) and to the conversion, with gain[k] where sb200_decode_chunks_resampled applies it.
+ * Contract: the concatenation of what a prosody stream emits is, bit for bit, sb200_debug_prosody of the concatenation
+ * of the samples appended to it.  Those are the chunks after this call's post-path on the device, which are the chunks
+ * sb200_decode_chunks_resampled returns for a NULL resampler: their crossfade table is computed by this library
+ * (sinf), so on the faded samples they can differ by an ulp from a crossfade applied on the host with another sine
+ * (as a plain Python stream's chunks are).  Emission rule, with a_k = floor(k Hs / alpha + 0.5) (a_{-1} = -Hs) and C the inputs
+ * consumed: frame k's delta is known once max(a_{k-1} + D + Hs + N, a_k + D + N) <= C (frames 0 .. K - 1, each known
+ * one in order); stretched samples min(K Hs, floor(C alpha + 0.5)) are computed (C when pitch == tempo); output j is
+ * emitted once ceil(j pitch + W) <= that count (every stretched sample when pitch is 1).  None of this depends on the
+ * stream's final length.  The chunk with last[k] = 1 emits everything up to n2, reading zeros past the stream's end,
+ * and the stream then takes no more chunks.  A chunk may emit 0 samples.  A prosody stream appearing twice, made for
+ * another voice or already flushed, or a last flag other than 0 / 1, fails with OPERATION_ERROR naming the chunk before
+ * any device work or state change. */
+int32_t sb200_decode_chunks_warped(sb200_voice* v, const sb200_latent* const* zs, const int64_t* lo, const int64_t* hi,
+                                   const int64_t* trim_lo_frames, const int64_t* trim_hi_frames, size_t n, int32_t fade,
+                                   const float* gain, sb200_resampler* const* resamplers,
+                                   sb200_prosody_stream* const* warps, const int32_t* last, int32_t format, void** outs,
+                                   size_t* lens, sb200_error* err);
+
 /* ---- introspection for tests / bench ---- */
 /* Copy a named intermediate of the LAST run of `job` to host (time-major fp32, valid rows of
  * utterance b only).  Names: "x","stats","logw","z_p","z","dec.pre","dec.up<i>","dec.mrf<i>", and the first encoder
@@ -518,6 +552,17 @@ int32_t sb200_debug_prosody_plan(int32_t rate, int64_t n, float pitch, float tem
 int32_t sb200_debug_prosody(int32_t device, const float* x, size_t n, int32_t rate, float pitch, float tempo, float* y,
                             size_t cap, int32_t* offsets, size_t offsets_cap, float* stretched, size_t stretched_cap,
                             sb200_error* err);
+/* Test hook, no device needed: the samples a prosody stream with these ratios at `rate` emits per chunk (the rule of
+ * sb200_decode_chunks_warped) when its chunks bring chunk_lens[0 .. n_chunks) inputs and the last one ends it.
+ * emitted[k] receives chunk k's count.  Returns 0, or 19 for bad ratios, a bad rate or a negative length. */
+int32_t sb200_debug_prosody_stream_plan(int32_t rate, float pitch, float tempo, const int64_t* chunk_lens, size_t n_chunks,
+                                        int64_t* emitted);
+/* A fresh prosody stream on `device` fed x[0 .. sum chunk_lens) in chunks of chunk_lens[0 .. n_chunks), the last one
+ * ending it, with no decoder involved: y receives the concatenated outputs (cap: its size), lens[k] chunk k's count,
+ * and offsets[0 .. F) (NULL: not wanted) every frame's delta as its chunk computed it. */
+int32_t sb200_debug_prosody_stream(int32_t device, const float* x, const int64_t* chunk_lens, size_t n_chunks,
+                                   int32_t rate, float pitch, float tempo, float* y, size_t cap, int64_t* lens,
+                                   int32_t* offsets, size_t offsets_cap, sb200_error* err);
 /* Test hook: G.711 (law as for sb200_job_fetch_g711) of x[0 .. n) into out[0 .. n).  device -1 runs the host copy of
  * the encoders (no device needed); otherwise the encoders run on that device over the buffer. */
 int32_t sb200_debug_g711(int32_t device, int32_t law, const int16_t* x, size_t n, uint8_t* out, sb200_error* err);

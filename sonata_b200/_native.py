@@ -180,6 +180,18 @@ SIGNATURES = {
                                                   C.POINTER(C.c_int64), C.POINTER(C.c_int64), C.c_size_t, C.c_int32,
                                                   C.POINTER(C.c_float), C.POINTER(_P), C.POINTER(C.c_int32), C.c_int32,
                                                   C.POINTER(C.c_void_p), C.POINTER(C.c_size_t), _ERR]),
+    "sb200_prosody_stream_create": (C.c_int32, [_P, C.c_float, C.c_float, C.POINTER(_P), _ERR]),
+    "sb200_prosody_stream_free": (None, [_P]),
+    "sb200_prosody_stream_profile": (C.c_int32, [_P, C.POINTER(C.c_float), C.POINTER(C.c_float)]),
+    "sb200_decode_chunks_warped": (C.c_int32, [_P, C.POINTER(_P), C.POINTER(C.c_int64), C.POINTER(C.c_int64),
+                                               C.POINTER(C.c_int64), C.POINTER(C.c_int64), C.c_size_t, C.c_int32,
+                                               C.POINTER(C.c_float), C.POINTER(_P), C.POINTER(_P), C.POINTER(C.c_int32),
+                                               C.c_int32, C.POINTER(C.c_void_p), C.POINTER(C.c_size_t), _ERR]),
+    "sb200_debug_prosody_stream_plan": (C.c_int32, [C.c_int32, C.c_float, C.c_float, C.POINTER(C.c_int64), C.c_size_t,
+                                                    C.POINTER(C.c_int64)]),
+    "sb200_debug_prosody_stream": (C.c_int32, [C.c_int32, C.POINTER(C.c_float), C.POINTER(C.c_int64), C.c_size_t,
+                                               C.c_int32, C.c_float, C.c_float, C.POINTER(C.c_float), C.c_size_t,
+                                               C.POINTER(C.c_int64), C.POINTER(C.c_int32), C.c_size_t, _ERR]),
     "sb200_debug_resample_emit": (C.c_int32, [C.c_int32, C.c_int32, C.POINTER(C.c_int64), C.c_size_t,
                                               C.POINTER(C.c_int64)]),
     "sb200_debug_resample": (C.c_int32, [C.c_int32, C.POINTER(C.c_float), C.c_size_t, C.c_int32, C.c_int32,

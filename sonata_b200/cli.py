@@ -21,7 +21,7 @@ from typing import Optional
 
 from . import from_config_path
 from .core import ENCODINGS, FLAC, OperationError, check_encoding
-from .piper import PiperSynthesisConfig, refuse_prosody
+from .piper import PiperSynthesisConfig, VitsStreamingModel, refuse_prosody
 from .synth import AudioOutputConfig, SonataSpeechSynthesizer, _check_loudness, _check_prosody
 
 MODES = ("lazy", "parallel", "realtime")
@@ -90,7 +90,7 @@ def process_request(synth: SonataSpeechSynthesizer, default_cfg: PiperSynthesisC
                                  "last one is decoded (use lazy or parallel mode)")
     pros = {k: req[k] for k in ("pitch_ratio", "tempo") if req.get(k) is not None}
     _check_prosody(pros.get("pitch_ratio"), pros.get("tempo"))
-    if mode == "realtime" and not output_file:
+    if mode == "realtime" and not output_file and not isinstance(synth.model, VitsStreamingModel):
         refuse_prosody(pros.get("pitch_ratio"), pros.get("tempo"), "realtime mode")
     synth.model.set_fallback_synthesis_config(PiperSynthesisConfig(
         req.get("speaker_id"),
@@ -116,7 +116,7 @@ def process_request(synth: SonataSpeechSynthesizer, default_cfg: PiperSynthesisC
         stream = synth.synthesize_parallel(text, oc, seed=seed, **rate, **loud, **enc, **pros)
     elif mode == "realtime":
         stream = synth.synthesize_streamed(text, oc, req.get("chunk_size") or 100, req.get("chunk_padding") or 3,
-                                          seed=seed, **rate, **enc)
+                                          seed=seed, **rate, **enc, **pros)
     else:
         raise ValueError(f"unknown synthesis mode `{mode}`")
     for item in stream:

@@ -23,6 +23,10 @@ struct sb200_latent {
     Latent* l; std::shared_ptr<Voice> keep;
     ~sb200_latent() { delete l; }
 };
+struct sb200_prosody_stream {
+    ProsodyStream* p; std::shared_ptr<Voice> keep;
+    ~sb200_prosody_stream() { delete p; }
+};
 struct sb200_resampler {
     Resampler* r; std::shared_ptr<Voice> keep;
     ~sb200_resampler() { delete r; }
@@ -638,15 +642,43 @@ int32_t sb200_resampler_create(sb200_voice* v, uint32_t out_rate, sb200_resample
 }
 void sb200_resampler_free(sb200_resampler* r) { delete r; }
 
+int32_t sb200_prosody_stream_create(sb200_voice* v, float pitch, float tempo, sb200_prosody_stream** out,
+                                    sb200_error* err) {
+    return guarded(err, [&] {
+        if (!v || !out) throw Error(19, "null argument");
+        Voice* w = v->v.get();
+        if (w->device < 0 || !w->emb)
+            throw Error(19, "Failed to run model inference. Error: voice was loaded config-only (device -1); libsonata_b200 has no CPU path");
+        *out = new sb200_prosody_stream{create_prosody_stream(w, w->device, w->sample_rate, pitch, tempo), v->v};
+    });
+}
+void sb200_prosody_stream_free(sb200_prosody_stream* s) { delete s; }
+int32_t sb200_prosody_stream_profile(const sb200_prosody_stream* s, float* stretch_ms, float* pitch_ms) {
+    if (!s) return 19;
+    if (stretch_ms) *stretch_ms = s->p->last_ms[0];
+    if (pitch_ms) *pitch_ms = s->p->last_ms[1];
+    return 0;
+}
+
 int32_t sb200_decode_chunks_resampled(sb200_voice* v, const sb200_latent* const* zs, const int64_t* lo, const int64_t* hi,
                                       const int64_t* trim_lo_frames, const int64_t* trim_hi_frames, size_t n,
                                       int32_t fade, const float* gain, sb200_resampler* const* resamplers,
                                       const int32_t* last, int32_t format, void** outs, size_t* lens, sb200_error* err) {
+    return sb200_decode_chunks_warped(v, zs, lo, hi, trim_lo_frames, trim_hi_frames, n, fade, gain, resamplers, nullptr,
+                                      last, format, outs, lens, err);
+}
+
+int32_t sb200_decode_chunks_warped(sb200_voice* v, const sb200_latent* const* zs, const int64_t* lo, const int64_t* hi,
+                                   const int64_t* trim_lo_frames, const int64_t* trim_hi_frames, size_t n, int32_t fade,
+                                   const float* gain, sb200_resampler* const* resamplers,
+                                   sb200_prosody_stream* const* warps, const int32_t* last, int32_t format, void** outs,
+                                   size_t* lens, sb200_error* err) {
     return guarded(err, [&] {
         ChunkPass p = chunk_pass(zs, lo, hi, n, trim_lo_frames, trim_hi_frames, gain);
         if (n > 0 && (!resamplers || !outs || !lens)) throw Error(19, "null argument");
         for (size_t k = 0; k < n; k++) {
             p.chunks[k].rs = resamplers[k] ? resamplers[k]->r : nullptr;
+            p.chunks[k].ps = warps && warps[k] ? warps[k]->p : nullptr;
             if (last) p.chunks[k].last = last[k];
         }
         p.fade = fade; p.resample = true; p.format = format;
@@ -968,6 +1000,77 @@ int32_t sb200_debug_prosody(int32_t device, const float* x, size_t n, int32_t ra
         // the stretched signal: the scratch when the pitch stage follows, else the result itself
         if (stretched && g.stretch)
             SB_CUDA(cudaMemcpy(stretched, g.pitch ? ds : dy, (size_t)g.n1 * 4, cudaMemcpyDeviceToHost));
+    });
+}
+
+int32_t sb200_debug_prosody_stream_plan(int32_t rate, float pitch, float tempo, const int64_t* chunk_lens, size_t n_chunks,
+                                        int64_t* emitted) {
+    try {
+        if (n_chunks > 0 && (!chunk_lens || !emitted)) return 19;
+        const std::vector<long long> e =
+            prosody_stream_plan(rate, pitch, tempo, reinterpret_cast<const long long*>(chunk_lens), n_chunks);
+        std::copy(e.begin(), e.end(), emitted);
+        return 0;
+    } catch (const Error& e) {
+        return e.code;
+    }
+}
+
+int32_t sb200_debug_prosody_stream(int32_t device, const float* x, const int64_t* chunk_lens, size_t n_chunks,
+                                   int32_t rate, float pitch, float tempo, float* y, size_t cap, int64_t* lens,
+                                   int32_t* offsets, size_t offsets_cap, sb200_error* err) {
+    return guarded(err, [&] {
+        if (!x || !chunk_lens || !y || !lens || n_chunks == 0) throw Error(19, "debug prosody stream: bad arguments");
+        long long total = 0;
+        for (size_t k = 0; k < n_chunks; k++) {
+            if (chunk_lens[k] < 0) throw Error(19, "debug prosody stream: negative chunk length");
+            total += chunk_lens[k];
+        }
+        const std::vector<long long> e =
+            prosody_stream_plan(rate, pitch, tempo, reinterpret_cast<const long long*>(chunk_lens), n_chunks);
+        long long out_total = 0;
+        for (long long m : e) out_total += m;
+        if ((size_t)out_total > cap) throw Error(19, "debug prosody stream: the destination is too small for the result");
+        SB_CUDA(cudaSetDevice(device));
+        std::unique_ptr<ProsodyStream> ps(create_prosody_stream(nullptr, device, rate, pitch, tempo));
+        if (offsets && ps->sh.stretch &&
+            (size_t)prosody_shape(rate, total, pitch, tempo).F > offsets_cap)
+            throw Error(19, "debug prosody stream: the offsets destination is too small");
+        // buffers for the largest pass: windows of at most the history plus the whole input, every frame and output
+        const ProsodyShape whole = prosody_shape(rate, total, pitch, tempo);
+        DeviceBuffers d;
+        const float* dx = d.upload(x, (size_t)total, (size_t)total + 4);
+        const PcmPost post;
+        const PcmPost* dpost = d.upload(&post, 1, 1);
+        FrameSeg* dfs = d.alloc<FrameSeg>(1);
+        ProsodySeg* dg = d.alloc<ProsodySeg>(1);
+        ProsodyCarry* dc = d.alloc<ProsodyCarry>(1);
+        float* win = d.alloc<float>((size_t)ps->cap_in + (size_t)total + 4);
+        float* ds = d.alloc<float>((size_t)ps->cap_s + (size_t)whole.n1 + 4);
+        int* doff = d.alloc<int>((size_t)whole.F + 4);
+        float* dy = d.alloc<float>((size_t)out_total + 4);
+        long long in_at = 0, out_at = 0;
+        for (size_t k = 0; k < n_chunks; k++) {
+            const bool last = k + 1 == n_chunks;
+            const ProsodyStep t = prosody_stream_step(*ps, chunk_lens[k], last);
+            ProsodyPlan p;
+            p.add_stream(*ps, t);
+            const ProsodyCarry c = prosody_carry(*ps, t, 0);
+            // the chunk as one segment of single samples at in_at
+            const FrameSeg fs{0, (int)chunk_lens[k], 0, 0, in_at};
+            SB_CUDA(cudaMemcpy(dfs, &fs, sizeof(fs), cudaMemcpyHostToDevice));
+            SB_CUDA(cudaMemcpy(dg, &p.segs[0], sizeof(ProsodySeg), cudaMemcpyHostToDevice));
+            SB_CUDA(cudaMemcpy(dc, &c, sizeof(c), cudaMemcpyHostToDevice));
+            launch_prosody_stream_stretch(p, dg, dc, dx, dfs, dpost, 1, win, ds, doff, dy, 0);
+            if (p.max_pitch) launch_prosody_pitch(win, ds, dg, 1, p.max_pitch, dy, 0);
+            SB_CUDA(cudaDeviceSynchronize());
+            SB_CUDA(cudaMemcpy(y + out_at, dy, (size_t)p.y_total * 4, cudaMemcpyDeviceToHost));
+            if (offsets && t.k1 > t.k0)
+                SB_CUDA(cudaMemcpy(offsets + t.k0, doff + 2, (size_t)(t.k1 - t.k0) * 4, cudaMemcpyDeviceToHost));
+            lens[k] = p.y_total;
+            out_at += p.y_total; in_at += chunk_lens[k];
+            prosody_stream_advance(*ps, t, last);
+        }
     });
 }
 

@@ -192,6 +192,22 @@ void launch_conv_post(const float* x, int C, const float* w /*[7][C]*/, float* w
 // crossfade table of fade_n <= 48 entries, linear gain.  Default = plain to_i16_vec.  fixed_scale = 1 converts at the
 // fixed scale 32767 instead of the segment's peak (loudness-normalised utterances).
 struct PcmPost { float gain = 1.f; int fade_n = 0; long long trim_lo = 0, trim_hi = 0; float tab[48] = {0}; int fixed_scale = 0; };
+// One segment's PcmPost with its scalars in registers, and sample i of the segment after it (kernels_misc.cu).
+struct PcmSeg {
+    const float* x; long long n; float gain; int fade_n; const float* tab;
+};
+__device__ __forceinline__ PcmSeg pcm_seg(const float* wav, const FrameSeg& fs, const PcmPost* p, int hop) {
+    const long long trim_lo = p->trim_lo;
+    return {wav + fs.out_off + trim_lo, (long long)fs.len * hop - trim_lo - p->trim_hi, p->gain, p->fade_n, p->tab};
+}
+__device__ __forceinline__ float pcm_value(const PcmSeg& s, long long i) {
+    float v = s.x[i];
+    if (s.fade_n > 0) {
+        if (i < s.fade_n) v = __fmul_rn(v, s.tab[i]);
+        else if (i >= s.n - s.fade_n) v = __fmul_rn(v, s.tab[s.n - 1 - i]);
+    }
+    return s.gain == 1.f ? v : __fmul_rn(v, s.gain);
+}
 // Output formats of a result: 0 f32, 1 i16 PCM, 2 G.711 mu-law, 3 G.711 A-law (one byte per sample).
 enum PcmFormat { PCM_F32 = 0, PCM_I16 = 1, PCM_MULAW = 2, PCM_ALAW = 3 };
 inline size_t pcm_bytes(int fmt) { return fmt == PCM_F32 ? 4 : fmt == PCM_I16 ? 2 : 1; }
@@ -261,10 +277,29 @@ void launch_loudness(float* wav, const LoudSeg* segs, int nseg, double* scratch,
 // (WSOLA: synthesis hop Hs, frame 2 Hs, search radius D, F frames whose offsets go to offsets[d_off ..)) into n1 samples
 // when `stretch`, then resampled by p into n2 samples when `pitch`.  The delivered signal is y[y_off, y_off + n2); with
 // both stages the stretched signal passes through s[s_off, s_off + n1).  With neither, x is copied to y.
+// A segment is a window of its signal, at absolute positions: wav[in_off] is input x0 (inputs at n and past it read as
+// zeros), offsets[d_off] is frame d0's delta, s[s_off] is stretched sample s0 (n1: the stretched samples known; the
+// pitch stage reads none past it).  The launches compute the offsets of frames [k0, k1), stretched samples [m0, m1)
+// and outputs [j0, j1), written from y[y_off] (the stretched samples too when there is no pitch stage, j0 = m0).  A
+// whole utterance is x0 = s0 = d0 = m0 = j0 = k0 = 0, k1 = F, m1 = n1, j1 = n2; a stream's chunk pass is a later window
+// of its stream (ProsodyStream), the frames before k0 known from earlier passes and staged at offsets[d_off].
 struct ProsodySeg {
     long long in_off, n, s_off, n1, y_off, n2, d_off;
     int F, Hs, D, stretch, pitch;
     double alpha, p;
+    long long x0, s0, m0, m1, j0, j1;
+    int k0, k1, d0;
+};
+// What a stream's chunk pass stages before the prosody launches and carries after them (prosody.cu): the chunk's
+// samples after the post-path (fsegs / posts entry `chunk`) follow h_in history inputs in the segment's input window,
+// h_s stretched samples of history start its stretched window and the deltas of frames d0, d0 + 1 start its offsets.
+// Afterwards in_keep inputs from window position in_from, s_keep stretched samples from s_from and the two deltas from
+// d_from go to the stream's other buffers.
+struct ProsodyCarry {
+    int chunk, h_in, h_s, in_keep, s_keep;
+    long long in_from, s_from, d_from;
+    const float *in_hist, *s_hist; const int* d_hist;
+    float *in_next, *s_next; int* d_next;
 };
 // Analysis position of WSOLA frame k: floor(k Hs / alpha + 0.5), every operation exactly rounded in double, so the host
 // plan and the kernels agree; the virtual frame -1 sits at -Hs.
@@ -281,6 +316,13 @@ void launch_prosody_ola(const float* wav, const ProsodySeg* segs, int nseg, long
                         float* s, float* y, cudaStream_t st);
 void launch_prosody_pitch(const float* wav, const float* s, const ProsodySeg* segs, int nseg, long long max_out, float* y,
                           cudaStream_t st);
+// A stream pass's staging (before the launches above; chunks read from src through fsegs / posts, max_in: the longest
+// window) and carry (after the overlap-add; max_keep: the longest tail), one launch each over the nseg segments.
+void launch_prosody_stage(const float* src, const FrameSeg* fsegs, const PcmPost* posts, int hop, const ProsodySeg* segs,
+                          const ProsodyCarry* cs, int nseg, long long max_in, float* wav, float* s, int* offsets,
+                          cudaStream_t st);
+void launch_prosody_carry(const float* wav, const float* s, const int* offsets, const ProsodySeg* segs,
+                          const ProsodyCarry* cs, int nseg, long long max_keep, cudaStream_t st);
 // One row range of a frame level taken from a latent: rows [off, off + len) of the level are rows [lo, lo + len) of src.
 struct GatherSeg { const float* src; long long lo; int off; int len; };
 // s[r] = the source row of r's segment (tile_seg: segment of every gran-row tile), or exact zeros past its end.

@@ -610,7 +610,13 @@ struct ChunkBufs {
     ResampleTables rt; float* rs;
     void* pcm; unsigned* max;
     void* out_h;
-    void carve(Arena& dev, Arena& pin, const Job& j, const ChunkPass& p, const ResamplePlan& rp, size_t total) {
+    // warped chunks (plan `pp`): the prosody tables, windows and offsets, the output after the waveforms in `wav`, and
+    // the resample launch's input table (the prosody output for a warped chunk, the post-path's chunk for the others)
+    ProsodySeg *pseg = nullptr, *pseg_h = nullptr; ProsodyCarry *pcar = nullptr, *pcar_h = nullptr;
+    float *px = nullptr, *ps = nullptr; int* poff = nullptr;
+    FrameSeg *rin = nullptr, *rin_h = nullptr; PcmPost *rpost = nullptr, *rpost_h = nullptr;
+    void carve(Arena& dev, Arena& pin, const Job& j, const ChunkPass& p, const ResamplePlan& rp, const ProsodyPlan& pp,
+               size_t total) {
         const Voice& v = *j.v;
         const bool multi = v.num_speakers > 1, i16_out = p.format != PCM_F32;
         const size_t n = j.fsegs.size(), nslots = j.slot_sid.size();
@@ -620,7 +626,16 @@ struct ChunkBufs {
         y.carve(dev, pin, j);
         src = dev.get<GatherSeg>(n); src_h = pin.get<GatherSeg>(n);
         s = dev.get<float>((size_t)j.RY * v.a.inter);
-        wav = dev.get<float>((size_t)j.total_samples + 4);
+        wav = dev.get<float>((size_t)j.total_samples + (size_t)pp.y_total + 4);
+        if (const size_t m = pp.segs.size()) {
+            pseg = dev.get<ProsodySeg>(m); pseg_h = pin.get<ProsodySeg>(m);
+            pcar = dev.get<ProsodyCarry>(m); pcar_h = pin.get<ProsodyCarry>(m);
+            px = dev.get<float>((size_t)pp.in_total + 4);
+            ps = dev.get<float>((size_t)pp.s_total + 4);
+            poff = dev.get<int>((size_t)pp.d_total + 2);
+            rin = dev.get<FrameSeg>(n); rin_h = pin.get<FrameSeg>(n);
+            rpost = dev.get<PcmPost>(n); rpost_h = pin.get<PcmPost>(n);
+        }
         dec.carve(dev, v, j.RY, false);
         post = p.resample || i16_out ? dev.get<PcmPost>(n) : nullptr;
         post_h = p.resample || i16_out ? pin.get<PcmPost>(n) : nullptr;
@@ -1229,11 +1244,12 @@ static void fill_fade(PcmPost& p, int fade, long long len) {
 }
 
 // The chunks are laid out as the segments of one frame level.  The pass runs the decoder, then its output stage: the
-// resample launch, which reads the waveforms through the post-path, and the i16 (or G.711) conversion, which applies the
-// post-path itself when no resample launch ran.  The packed result comes back in one copy through the context's
-// page-locked staging, and only then do the resamplers advance.
+// prosody launches of the chunks with a pitch / tempo stream, which read the waveforms through the post-path, the
+// resample launch, which reads their output or the waveforms through the post-path, and the i16 (or G.711) conversion,
+// which applies the post-path itself when no resample launch ran.  The packed result comes back in one copy through the
+// context's page-locked staging, and only then do the resamplers and prosody streams advance.
 void decode_chunks(Voice* v, const ChunkPass& p, ChunkResult& out) {
-    out.f32.clear(); out.i16.clear(); out.g711.clear(); out.ms = 0.f;
+    out.f32.clear(); out.i16.clear(); out.g711.clear(); out.ms = out.stretch_ms = out.pitch_ms = 0.f;
     const size_t n = p.chunks.size();
     if (n == 0) return;
     if (p.format < PCM_F32 || p.format > PCM_ALAW)
@@ -1267,16 +1283,35 @@ void decode_chunks(Voice* v, const ChunkPass& p, ChunkResult& out) {
             if (r->ended) fail(k, "the resampler's stream has already been flushed", "");
             for (size_t q = 0; q < k; q++)
                 if (p.chunks[q].rs == r) fail(k, "the resampler of chunk " + std::to_string(q) + " appears twice in one call", "");
-            if (c.last != 0 && c.last != 1) fail(k, "last flag " + std::to_string(c.last) + " is neither 0 nor 1", "");
         }
+        if (const ProsodyStream* w = c.ps) {
+            if (!p.resample) fail(k, "a prosody stream needs a resampled chunk pass", "");
+            if (w->v != v) fail(k, "the prosody stream was made for another voice", "");
+            if (w->ended) fail(k, "the prosody stream has already been flushed", "");
+            for (size_t q = 0; q < k; q++)
+                if (p.chunks[q].ps == w)
+                    fail(k, "the prosody stream of chunk " + std::to_string(q) + " appears twice in one call", "");
+        }
+        if ((c.rs || c.ps) && c.last != 0 && c.last != 1)
+            fail(k, "last flag " + std::to_string(c.last) + " is neither 0 nor 1", "");
     }
-    // samples of each chunk after its trims, and the resample launch
-    std::vector<long long> n_in(n);
+    // samples of each chunk after its trims, what its prosody stream emits for them, and the resample launch
+    std::vector<long long> n_in(n), n_res(n);     // n_res: what the resample launch takes (a warped chunk's output)
+    std::vector<ProsodyStep> steps(n);
+    std::vector<int> warped;
+    ProsodyPlan pp;
     ResamplePlan rp;
     for (size_t k = 0; k < n; k++) {
         const ChunkSpec& c = p.chunks[k];
         n_in[k] = (c.hi - c.lo - c.trim_lo - c.trim_hi) * hop;
-        if (p.resample) rp.add(c.rs ? &c.rs->f : nullptr, n_in[k], c.rs, c.last != 0);
+        n_res[k] = n_in[k];
+        if (c.ps) {
+            steps[k] = prosody_stream_step(*c.ps, n_in[k], c.last != 0);
+            pp.add_stream(*c.ps, steps[k]);
+            warped.push_back((int)k);
+            n_res[k] = steps[k].j1 - steps[k].j0;
+        }
+        if (p.resample) rp.add(c.rs ? &c.rs->f : nullptr, n_res[k], c.rs, c.last != 0);
     }
 
     j.v = v; j.B = n; j.ctx = v->acquire();
@@ -1285,7 +1320,7 @@ void decode_chunks(Voice* v, const ChunkPass& p, ChunkResult& out) {
     lay_out_frames(j, len, hop);
     const size_t total = p.resample ? (size_t)rp.total : (size_t)j.total_samples;
     ChunkBufs b;
-    plan(C.dev_frame, C.pin, [&](Arena& dev, Arena& pin) { b.carve(dev, pin, j, p, rp, total); });
+    plan(C.dev_frame, C.pin, [&](Arena& dev, Arena& pin) { b.carve(dev, pin, j, p, rp, pp, total); });
     j.d_cond = b.cond; j.d_fsegs = b.y.fsegs; j.d_wav = b.wav;
     C.events_used = 0;
     if (!C.ev_begin) { SB_CUDA(cudaEventCreate(&C.ev_begin)); SB_CUDA(cudaEventCreate(&C.ev_end)); }
@@ -1319,9 +1354,43 @@ void decode_chunks(Voice* v, const ChunkPass& p, ChunkResult& out) {
         }
         h2d(b.post, b.post_h, n * sizeof(PcmPost), st);
     }
+    // warped chunks: prosody on the post-path's samples, then the resample launch reads its output (n samples at
+    // `off` as a segment of ceil(n / hop) frames less a trim, with no post-path of its own)
+    const FrameSeg* rs_in = b.y.fsegs; const PcmPost* rs_post = b.post;
+    if (!warped.empty()) {
+        float* py = b.wav + j.total_samples;
+        for (size_t q = 0; q < warped.size(); q++) {
+            b.pseg_h[q] = pp.segs[q];
+            b.pcar_h[q] = prosody_carry(*p.chunks[warped[q]].ps, steps[warped[q]], warped[q]);
+        }
+        h2d(b.pseg, b.pseg_h, warped.size() * sizeof(ProsodySeg), st);
+        h2d(b.pcar, b.pcar_h, warped.size() * sizeof(ProsodyCarry), st);
+        R.begin("stretch");
+        launch_prosody_stream_stretch(pp, b.pseg, b.pcar, b.wav, b.y.fsegs, b.post, hop, b.px, b.ps, b.poff, py, st);
+        R.count(pp.stretch_flops, pp.stretch_bytes, 2 + (pp.smem_ints ? 1 : 0) + (pp.max_ola ? 1 : 0));
+        R.end();
+        if (pp.max_pitch) {
+            R.begin("pitch");
+            launch_prosody_pitch(b.px, b.ps, b.pseg, (int)warped.size(), pp.max_pitch, py, st);
+            R.count(pp.pitch_flops, pp.pitch_bytes);
+            R.end();
+        }
+        std::copy(j.fsegs.begin(), j.fsegs.end(), b.rin_h);
+        std::copy(b.post_h, b.post_h + n, b.rpost_h);
+        for (size_t q = 0; q < warped.size(); q++) {
+            const ProsodySeg& g = pp.segs[q];
+            const long long m = g.j1 - g.j0, frames = (m + hop - 1) / hop;
+            b.rin_h[warped[q]] = FrameSeg{0, (int)frames, 0, 0, j.total_samples + g.y_off};
+            b.rpost_h[warped[q]] = PcmPost();
+            b.rpost_h[warped[q]].trim_hi = frames * hop - m;
+        }
+        h2d(b.rin, b.rin_h, n * sizeof(FrameSeg), st);
+        h2d(b.rpost, b.rpost_h, n * sizeof(PcmPost), st);
+        rs_in = b.rin; rs_post = b.rpost;
+    }
     if (p.resample) {
         b.rt.upload(rp, st, gain_after ? &out_gain : nullptr);
-        run_resample(R, rp, b.rt, b.wav, b.y.fsegs, b.post, hop, b.rs);
+        run_resample(R, rp, b.rt, b.wav, rs_in, rs_post, hop, b.rs);
         if (b.pcm) launch_pcm(b.rs, b.rt.osegs, b.rt.posts, (int)n, 1, rp.max_out, b.max, p.format, b.pcm, st);
     } else if (b.pcm) {
         launch_pcm(b.wav, b.y.fsegs, b.post, (int)n, hop, (long long)*std::max_element(len.begin(), len.end()) * hop,
@@ -1337,11 +1406,21 @@ void decode_chunks(Voice* v, const ChunkPass& p, ChunkResult& out) {
         Resampler* r = p.chunks[k].rs;
         if (!r) continue;
         const ResampleSeg& s = rp.segs[k];
-        r->consumed = s.c + n_in[k];
+        r->consumed = s.c + n_res[k];
         r->emitted = s.j0 + s.n_out;
         r->cur ^= 1;
         r->h = s.h_out;
         r->ended = p.chunks[k].last != 0;
+    }
+    for (Region& g : j.regions) {
+        if (g.name != "stretch" && g.name != "pitch") continue;
+        cudaEventElapsedTime(&g.ms, g.e0, g.e1);
+        (g.name == "stretch" ? out.stretch_ms : out.pitch_ms) = g.ms;
+    }
+    for (int k : warped) {
+        ProsodyStream& w = *p.chunks[k].ps;
+        prosody_stream_advance(w, steps[k], p.chunks[k].last != 0);
+        w.last_ms[0] = out.stretch_ms; w.last_ms[1] = out.pitch_ms;
     }
     if (p.format == PCM_I16) out.i16.resize(n); else if (b.pcm) out.g711.resize(n); else out.f32.resize(n);
     for (size_t k = 0; k < n; k++) {

@@ -124,15 +124,66 @@ ProsodyShape prosody_shape(int rate, long long n, float pitch, float tempo);
 bool check_prosody(const float* pitch, const float* tempo, size_t B);
 // The three prosody launches over segments laid out back to back: each segment's ProsodySeg, the sizes of the offsets,
 // the stretched scratch and the output, what the launches are sized by and what the profile counts.
+struct Voice;
+struct ProsodyStream;
+struct ProsodyStep;
 struct ProsodyPlan {
     std::vector<ProsodySeg> segs;
     std::vector<ProsodyShape> shapes;
     long long s_total = 0, y_total = 0, d_total = 0, max_ola = 0, max_pitch = 0, steps = 0;
+    long long in_total = 0, max_in = 0, max_keep = 0;     // streams: the input windows, the staging and carry sizes
     int smem_ints = 0;
     double stretch_flops = 0, stretch_bytes = 0, pitch_flops = 0, pitch_bytes = 0;
     // Appends the segment wav[in_off, in_off + n) with shape `sh`.
     void add(const ProsodyShape& sh, long long in_off, long long n);
+    // Appends stream ps's window for its chunk pass step t; its input window goes to wav[in_total ..) of the pass.
+    void add_stream(const ProsodyStream& ps, const ProsodyStep& t);
 };
+
+// One stream's pitch and tempo state (prosody.cu): the shape of its ratios, its counts (inputs consumed, frames whose
+// delta is known, stretched samples computed, outputs emitted, and the history held of the inputs and the stretched
+// signal) and, on the device, two sets of buffers read and written alternately: the input tail (at most cap_in), the
+// stretched tail (at most cap_s, with both stages) and the deltas of the last two known frames.
+struct ProsodyCounts { long long consumed = 0, frames = 0, stretched = 0, emitted = 0; int h_in = 0, h_s = 0; };
+struct ProsodyStream {
+    Voice* v = nullptr;
+    int device = 0, rate = 0;
+    float pitch = 1.f, tempo = 1.f;
+    ProsodyShape sh{};                    // Hs, N, D, alpha, p and the stages (lengths unused)
+    int cap_in = 0, cap_s = 0;
+    void* mem = nullptr;
+    float* in_hist[2] = {nullptr, nullptr}; float* s_hist[2] = {nullptr, nullptr}; int* d_hist[2] = {nullptr, nullptr};
+    int cur = 0;
+    ProsodyCounts c;
+    bool ended = false;
+    float last_ms[2] = {0.f, 0.f};        // the "stretch" and "pitch" device time of the last pass it was in
+    ~ProsodyStream();
+};
+// What one chunk pass does to a stream: n_in new inputs, the frames [k0, k1), stretched samples [m0, m1) and outputs
+// [j0, j1) it computes, the first absolute positions of its input and stretched windows (x0, s0), where the tails the
+// next pass reads start (in_from, s_from), and the counts after it.  Computed on the host from the counts alone.
+struct ProsodyStep {
+    long long n_in, x0, s0, m0, m1, j0, j1, in_from, s_from;
+    int k0, k1;
+    ProsodyCounts next;
+};
+// Checks the ratios (one must ask for something) and sizes the history; no device memory.
+void prosody_stream_init(ProsodyStream& ps, int rate, float pitch, float tempo);
+ProsodyStream* create_prosody_stream(Voice* v, int device, int rate, float pitch, float tempo);
+// The emission rule (include/sonata_b200.h, sb200_decode_chunks_warped).  Throws OPERATION_ERROR only on an internal
+// inconsistency.
+ProsodyStep prosody_stream_step(const ProsodyStream& ps, long long n_in, bool last);
+// The stage / carry entry of chunk `chunk` for step t of ps.
+ProsodyCarry prosody_carry(const ProsodyStream& ps, const ProsodyStep& t, int chunk);
+// The launches of a stream pass's "stretch" region: staging, the offset chain, the overlap-add and the carry.  The
+// pitch stage is launch_prosody_pitch over the same tables.
+void launch_prosody_stream_stretch(const ProsodyPlan& p, const ProsodySeg* segs, const ProsodyCarry* cs,
+                                   const float* src, const FrameSeg* fsegs, const PcmPost* posts, int hop, float* x,
+                                   float* s, int* offsets, float* y, cudaStream_t st);
+// After the pass has synchronised: the counts become t's and the buffers swap.
+void prosody_stream_advance(ProsodyStream& ps, const ProsodyStep& t, bool last);
+// Outputs per chunk of a stream with these ratios whose chunks bring chunk_lens[0 .. n) inputs, the last one ending it.
+std::vector<long long> prosody_stream_plan(int rate, float pitch, float tempo, const long long* chunk_lens, size_t n);
 
 struct Context;   // stream + arenas for one in-flight call
 
@@ -362,6 +413,7 @@ struct ChunkSpec {
     long long trim_lo = 0, trim_hi = 0;   // overlap frames dropped by the post-path
     float gain = 1.f;                     // linear gain of the post-path
     Resampler* rs = nullptr;              // the chunk's stream (resample passes; null: none)
+    ProsodyStream* ps = nullptr;          // the chunk's pitch / tempo stream (resample passes; null: none)
     int last = 0;                         // 1: the chunk ends its stream, which is flushed
 };
 // One frame-level decoder pass over chunks of latents of one voice; chunk k equals the same chunk decoded alone, bit for
@@ -369,7 +421,9 @@ struct ChunkSpec {
 // their defaults.  Otherwise the reference's post-path runs on the device per chunk: drop the trim frames,
 // crossfade(fade) (samples.rs:144-157), the gain.  With `resample` the chunk is then appended to its stream's resampler,
 // emitting every output it can (a chunk without one leaves at the voice's rate as the post-path leaves it); a resampler
-// may appear once per pass and must belong to the voice.  i16: to_i16_vec (samples.rs:51-75) normalised to each emitted
+// may appear once per pass and must belong to the voice.  A chunk with a prosody stream (resample passes only) is warped
+// first, and what that stream emits is what the resampler, or the voice-rate copy, takes; the same rules hold for
+// prosody streams.  i16: to_i16_vec (samples.rs:51-75) normalised to each emitted
 // chunk's own peak; mu-law / A-law: the G.711 bytes of those same i16 samples, from the same launches.  Every check runs
 // before any device work and any resampler changes; errors name the chunk, except with `single`, which keeps the
 // single-chunk entry point's messages.
@@ -385,6 +439,7 @@ struct ChunkResult {
     std::vector<std::vector<int16_t>> i16;    // format 1
     std::vector<std::vector<uint8_t>> g711;   // formats 2 and 3
     float ms = 0;                             // the pass's device time
+    float stretch_ms = 0, pitch_ms = 0;       // its "stretch" and "pitch" regions (0: none ran)
 };
 void decode_chunks(Voice* v, const ChunkPass& p, ChunkResult& out);
 

@@ -669,22 +669,8 @@ __global__ void __launch_bounds__(256) conv_post_kernel(const float* __restrict_
 // chunk before that conversion: trimming the overlap frames of a streamed chunk (piper/src/lib.rs:811-826),
 // crossfade(42) (samples.rs:144-157; the sine table is computed by the host so both sides use the same floats) and
 // the linear volume gain of AudioOutputConfig (synth/src/lib.rs:84-86).  Every segment (blockIdx.y) has its own
-// PcmPost, so one launch converts the chunks of many streams, each normalised to its own peak.
-struct PcmSeg {                                // one segment's PcmPost, scalars in registers
-    const float* x; long long n; float gain; int fade_n; const float* tab;
-};
-__device__ __forceinline__ PcmSeg pcm_seg(const float* wav, const FrameSeg& fs, const PcmPost* p, int hop) {
-    const long long trim_lo = p->trim_lo;
-    return {wav + fs.out_off + trim_lo, (long long)fs.len * hop - trim_lo - p->trim_hi, p->gain, p->fade_n, p->tab};
-}
-__device__ __forceinline__ float pcm_value(const PcmSeg& s, long long i) {
-    float v = s.x[i];
-    if (s.fade_n > 0) {
-        if (i < s.fade_n) v = __fmul_rn(v, s.tab[i]);
-        else if (i >= s.n - s.fade_n) v = __fmul_rn(v, s.tab[s.n - 1 - i]);
-    }
-    return s.gain == 1.f ? v : __fmul_rn(v, s.gain);
-}
+// PcmPost, so one launch converts the chunks of many streams, each normalised to its own peak.  A segment is read
+// through pcm_seg / pcm_value (common.cuh).
 
 __global__ void i16_absmax_kernel(const float* __restrict__ wav, const FrameSeg* __restrict__ fsegs,
                                   const PcmPost* __restrict__ posts, int hop, unsigned* __restrict__ maxbits) {

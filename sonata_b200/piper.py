@@ -839,6 +839,46 @@ def _stream_resampler(model, output_rate) -> Optional[Resampler]:
     return Resampler(model, output_rate)
 
 
+class ProsodyStream:
+    """One stream's pitch and tempo state on the device (sb200_prosody_stream_*): it carries the tails of the stream's
+    input and stretched signal, and its last frames' offsets, between chunks, so the concatenation of what it emits is
+    the whole stream warped at once.  `pitch` / `tempo`: ratios as for infer_batch_with_values, not both neutral."""
+
+    def __init__(self, model: "_VitsCommons", pitch=None, tempo=None):
+        p, t = _prosody_arrays([pitch], [tempo], 1)
+        if p is None and t is None:
+            raise OperationError("a prosody stream needs a pitch or a tempo ratio other than 1 (None, NaN or 1: none)")
+        self._m, self._h = model, C.c_void_p()
+        self.pitch = None if p is None else float(p[0])
+        self.tempo = None if t is None else float(t[0])
+        err = N.sb200_error()
+        _check(model._lib.sb200_prosody_stream_create(model._h, float("nan") if p is None else float(p[0]),
+                                                      float("nan") if t is None else float(t[0]), C.byref(self._h),
+                                                      C.byref(err)), err)
+
+    def last_pass_ms(self) -> Tuple[float, float]:
+        """The "stretch" and "pitch" device time (ms) of the last chunk pass this stream was in."""
+        s, p = C.c_float(), C.c_float()
+        self._m._lib.sb200_prosody_stream_profile(self._h, C.byref(s), C.byref(p))
+        return float(s.value), float(p.value)
+
+    def __del__(self):
+        try:
+            if self._h:
+                self._m._lib.sb200_prosody_stream_free(self._h)
+                self._h = None
+        except Exception:
+            pass
+
+
+def _stream_prosody(model, pitch, tempo) -> Optional[ProsodyStream]:
+    """A ProsodyStream for a stream with these ratios, or None when neither asks for anything."""
+    p, t = _prosody_arrays([pitch], [tempo], 1)
+    if p is None and t is None:
+        return None
+    return ProsodyStream(model, pitch, tempo)
+
+
 def _trim_frames(trim: slice) -> Tuple[int, int]:
     """The overlap frames a SpeechStreamer audio slice drops at each end."""
     return (trim.start or 0) // HOP, (-trim.stop // HOP) if trim.stop is not None else 0
@@ -850,38 +890,37 @@ class SpeechStreamer:
     run on the device too and each chunk leaves as G.711 bytes of its to_i16_vec after `gain`."""
 
     def __init__(self, enc: EncoderOutputs, chunk_size: int, chunk_padding: int,
-                 resampler: Optional[Resampler] = None, encoding: Optional[str] = None, gain: float = 1.0):
+                 resampler: Optional[Resampler] = None, encoding: Optional[str] = None, gain: float = 1.0,
+                 warp: Optional[ProsodyStream] = None):
         self.enc = enc
         self.chunker = AdaptiveMelChunker(enc.num_frames, chunk_size, chunk_padding)
         self.one_shot = enc.num_frames <= (chunk_size * 2 + chunk_padding * 2)
         self.resampler = resampler
         self.encoding, self.gain = encoding, gain
+        self.warp = warp
 
     def __iter__(self) -> Iterator[AudioSamples]:
         return self
 
     def __next__(self) -> AudioSamples:
         (m0, m1), (a0, a1) = next(self.chunker)
-        if self.encoding is not None:
+        # encoded, resampled or warped: the post-path runs on the device, then the stream's resampler / prosody stream
+        if self.encoding is not None or self.resampler is not None or self.warp is not None:
             if self.one_shot:
                 self.chunker.consume()
                 chunk, fade = (self.enc, 0, self.enc.num_frames, 0, 0), 0
             else:
                 hi = self.enc.num_frames if m1 is None else m1
                 chunk, fade = (self.enc, m0, hi) + _trim_frames(slice(a0, a1)), 42
-            rs = {} if self.resampler is None else {"resamplers": [self.resampler],
-                                                    "last": [self.chunker.last_end_index is None]}
-            return self.enc._m.infer_decoder_batch([chunk], fade=fade, gains=[self.gain], encoding=self.encoding,
-                                                   **rs)[0]
-        if self.resampler is not None:
-            if self.one_shot:
-                self.chunker.consume()
-                chunk, fade = (self.enc, 0, self.enc.num_frames, 0, 0), 0
-            else:
-                hi = self.enc.num_frames if m1 is None else m1
-                chunk, fade = (self.enc, m0, hi) + _trim_frames(slice(a0, a1)), 42
-            return self.enc._m.infer_decoder_batch([chunk], fade=fade, resamplers=[self.resampler],
-                                                   last=[self.chunker.last_end_index is None])[0]
+            kw = {}
+            if self.resampler is not None or self.warp is not None:     # whether this chunk ends the stream: after
+                kw.update(resamplers=[self.resampler],                  # the one-shot consume()
+                          last=[self.chunker.last_end_index is None])
+            if self.warp is not None:
+                kw["warps"] = [self.warp]
+            if self.encoding is not None:
+                kw.update(gains=[self.gain], encoding=self.encoding)
+            return self.enc._m.infer_decoder_batch([chunk], fade=fade, **kw)[0]
         if self.one_shot:
             self.chunker.consume()
             return self.enc.infer_decoder()
@@ -936,7 +975,8 @@ class VitsStreamingModel(_VitsCommons):
 
     def infer_decoder_batch(self, chunks: Sequence[tuple], pcm16: bool = False, fade: int = 0,
                             gains: Optional[Sequence[float]] = None, resamplers: Optional[Sequence] = None,
-                            last: Optional[Sequence[bool]] = None, encoding: Optional[str] = None) -> list:
+                            last: Optional[Sequence[bool]] = None, encoding: Optional[str] = None,
+                            warps: Optional[Sequence] = None) -> list:
         """Many `EncoderOutputs.infer_decoder(lo, hi)` calls as one decoder pass.  `chunks`: (encoder outputs, lo, hi)
         per chunk; each result equals that chunk decoded alone, bit for bit.
 
@@ -951,7 +991,11 @@ class VitsStreamingModel(_VitsCommons):
 
         With `encoding` ("mulaw" or "alaw"; None: none), chunks take pcm16's tuples and each result is `bytes`: G.711 of
         the int16 samples pcm16 returns for that chunk (with or without resamplers), encoded on the device in the same
-        launches."""
+        launches.
+
+        With `warps` (one ProsodyStream or None per chunk; chunks may carry trims, as with resamplers), chunk k after
+        the post-path is appended to its prosody stream first, and what that emits goes on to resamplers[k] (None
+        entries, or resamplers None: the voice's rate) and the conversion; last[k] flushes both streams."""
         refuse_flac(encoding, "a decoder chunk pass")
         check_encoding(encoding)
         if encoding is not None and pcm16:
@@ -961,7 +1005,7 @@ class VitsStreamingModel(_VitsCommons):
         tlo, thi = np.zeros(n, np.int64), np.zeros(n, np.int64)
         hs = (C.c_void_p * n)()
         for k, c in enumerate(chunks):
-            if len(c) not in ((3, 5) if pcm16 or encoding or resamplers is not None else (3,)):
+            if len(c) not in ((3, 5) if pcm16 or encoding or resamplers is not None or warps is not None else (3,)):
                 raise OperationError(f"Invalid decoder chunk {k}: expected (encoder outputs, lo, hi"
                                      + (", trim_lo, trim_hi)" if pcm16 else ")"))
             enc = c[0]
@@ -977,22 +1021,35 @@ class VitsStreamingModel(_VitsCommons):
             return []
         p64 = lambda a: a.ctypes.data_as(C.POINTER(C.c_int64))
         err = N.sb200_error()
-        if resamplers is not None:
-            resamplers = _per_utterance(resamplers, n, "resamplers")
+        if resamplers is not None or warps is not None:
+            resamplers = _per_utterance([None] * n if resamplers is None else resamplers, n, "resamplers")
             rs = (C.c_void_p * n)()
             for k, r in enumerate(resamplers):
                 if r is not None and (not isinstance(r, Resampler) or not r._h):
                     raise OperationError(f"chunk {k}: not a Resampler")
                 rs[k] = None if r is None else r._h.value
+            ws = None
+            if warps is not None:
+                ws = (C.c_void_p * n)()
+                for k, w in enumerate(_per_utterance(warps, n, "warps")):
+                    if w is not None and (not isinstance(w, ProsodyStream) or not w._h):
+                        raise OperationError(f"chunk {k}: not a ProsodyStream")
+                    ws[k] = None if w is None else w._h.value
             fl = np.zeros(n, np.int32) if last is None else np.array([1 if x else 0 for x in
                                                                         _per_utterance(last, n, "last flags")], np.int32)
             g = None if gains is None else np.ascontiguousarray(gains, dtype=np.float32)
             outs = (C.c_void_p * n)()
             lens = (C.c_size_t * n)()
-            _check(self._lib.sb200_decode_chunks_resampled(
-                self._h, hs, p64(lo), p64(hi), p64(tlo), p64(thi), n, int(fade),
-                None if g is None else g.ctypes.data_as(C.POINTER(C.c_float)), rs, _ptr(fl, C.c_int32),
-                G711_LAW[encoding] + 2 if encoding else 1 if pcm16 else 0, outs, lens, C.byref(err)), err)
+            fmt = G711_LAW[encoding] + 2 if encoding else 1 if pcm16 else 0
+            gp = None if g is None else g.ctypes.data_as(C.POINTER(C.c_float))
+            if ws is None:
+                _check(self._lib.sb200_decode_chunks_resampled(
+                    self._h, hs, p64(lo), p64(hi), p64(tlo), p64(thi), n, int(fade), gp, rs, _ptr(fl, C.c_int32), fmt,
+                    outs, lens, C.byref(err)), err)
+            else:
+                _check(self._lib.sb200_decode_chunks_warped(
+                    self._h, hs, p64(lo), p64(hi), p64(tlo), p64(thi), n, int(fade), gp, rs, ws, _ptr(fl, C.c_int32),
+                    fmt, outs, lens, C.byref(err)), err)
             if encoding:
                 return _take_bytes(self._lib, outs, lens)
             if pcm16:
@@ -1029,15 +1086,20 @@ class VitsStreamingModel(_VitsCommons):
         `output_rate`: the chunks' sample rate (see infer_batch_with_values), the sentence resampled as one stream.
         `encoding`: "mulaw" / "alaw" for chunks of G.711 `bytes`: each is G.711 of to_i16_vec of the chunk the stream
         yields without an encoding, after the linear `gain` (None: 1; encoded streams only), encoded on the device.
-        `pitch` / `tempo`: ratios as for infer_batch_with_values, refused here unless neutral (refuse_prosody)."""
-        refuse_prosody(pitch, tempo, "stream_synthesis")
+        `pitch` / `tempo`: ratios as for infer_batch_with_values, the sentence warped as one stream on the device
+        (ProsodyStream): the concatenation of the chunks is the sentence the stream yields without ratios, warped at
+        once, then resampled and encoded as without ratios."""
+        if not isinstance(self, VitsStreamingModel):
+            refuse_prosody(pitch, tempo, "stream_synthesis")
+        _prosody_arrays([pitch], [tempo], 1)
         _seed_arrays([seed], 1)
         _rate_array([output_rate], 1)
         refuse_flac(encoding, "stream_synthesis")
         g = _stream_gain(encoding, gain)
         ids = self.phonemes_to_input_ids(phonemes)
         enc = self.infer_encoder(ids) if seed is None else self.infer_encoder_batch([ids], seeds=[seed])[0]
-        return SpeechStreamer(enc, chunk_size, chunk_padding, _stream_resampler(self, output_rate), encoding, g)
+        return SpeechStreamer(enc, chunk_size, chunk_padding, _stream_resampler(self, output_rate), encoding, g,
+                              _stream_prosody(self, pitch, tempo))
 
 
 def _stream_gain(encoding, gain) -> float:
@@ -1054,9 +1116,10 @@ class _Stream:
     """One sentence of a StreamBatch: its latent and its own chunk schedule, with SpeechStreamer's one-shot rule."""
 
     def __init__(self, key, enc, chunk_size: int, chunk_padding: int, resampler: Optional[Resampler] = None,
-                 encoding: Optional[str] = None, gain: float = 1.0):
+                 encoding: Optional[str] = None, gain: float = 1.0, warp: Optional[ProsodyStream] = None):
         self.key, self.enc, self.resampler = key, enc, resampler
         self.encoding, self.gain = encoding, gain
+        self.warp = warp
         self.chunker = AdaptiveMelChunker(enc.num_frames, chunk_size, chunk_padding)
         self.one_shot = enc.num_frames <= (chunk_size * 2 + chunk_padding * 2)
 
@@ -1112,15 +1175,19 @@ class StreamBatch:
             pitch: Optional[float] = None, tempo: Optional[float] = None) -> int:
         """`seed`: the stream's noise seed (see infer_batch_with_values); a seeded stream yields what
         `stream_synthesis(..., seed=seed)` yields, whatever other streams share its encoder pass.  `output_rate`,
-        `encoding` and `gain`: the stream's sample rate and G.711 encoding, as for stream_synthesis; `pitch` / `tempo`
-        are refused unless neutral, as there."""
-        refuse_prosody(pitch, tempo, "StreamBatch")
-        return self._add(ids_or_phonemes, config, self.chunk_size, seed, output_rate, encoding, gain)
+        `encoding` and `gain`: the stream's sample rate and G.711 encoding, as for stream_synthesis; `pitch` / `tempo`:
+        its ratios, as there.  A warped stream's chunks go through passes of their own, so the other streams keep their
+        passes and their bits."""
+        if not isinstance(self.model, VitsStreamingModel):
+            refuse_prosody(pitch, tempo, "StreamBatch")
+        return self._add(ids_or_phonemes, config, self.chunk_size, seed, output_rate, encoding, gain, pitch, tempo)
 
     def _add(self, ids_or_phonemes, config, chunk_size: int, seed: Optional[int] = None,
-             output_rate: Optional[int] = None, encoding: Optional[str] = None, gain: Optional[float] = None) -> int:
+             output_rate: Optional[int] = None, encoding: Optional[str] = None, gain: Optional[float] = None,
+             pitch: Optional[float] = None, tempo: Optional[float] = None) -> int:
         if config is not None and not isinstance(config, PiperSynthesisConfig):
             raise OperationError("Invalid configuration for Vits Model")
+        _prosody_arrays([pitch], [tempo], 1)
         _seed_arrays([seed], 1)
         _rate_array([output_rate], 1)
         refuse_flac(encoding, "StreamBatch")
@@ -1136,7 +1203,7 @@ class StreamBatch:
             raise OperationError("Failed to run model inference. Error: empty input sequence")
         key = self._next_key
         self._next_key += 1
-        self._pending.append((key, ids, config, chunk_size, seed, output_rate, encoding, gain))
+        self._pending.append((key, ids, config, chunk_size, seed, output_rate, encoding, gain, pitch, tempo))
         return key
 
     def __len__(self) -> int:
@@ -1165,26 +1232,31 @@ class StreamBatch:
                 if err is None:
                     try:
                         active.append(_Stream(p[0], enc, p[3], self.chunk_padding,
-                                              _stream_resampler(self.model, p[5]), p[6], p[7]))
+                                              _stream_resampler(self.model, p[5]), p[6], p[7],
+                                              _stream_prosody(self.model, p[8], p[9])))
                         continue
                     except SonataError as e:
                         err = e
                 out.append((p[0], err))
         plan = [(s,) + s.next_chunk() for s in active]
         failed = set()
-        # one pass per (encoding, resampled, one-shot): the streams without an encoding first, in their usual passes
-        plain_key = (None, False, False)
-        groups = {plain_key: [], (None, True, False): [], (None, True, True): []}
+        # one pass per (encoding, resampled, one-shot, warped): the streams without an encoding first, in their usual
+        # passes; warped streams in passes of their own
+        plain_key = (None, False, False, False)
+        groups = {plain_key: [], (None, True, False, False): [], (None, True, True, False): []}
         for p in plan:
             s = p[0]
-            k = plain_key if s.encoding is None and s.resampler is None else (s.encoding, s.resampler is not None,
-                                                                                 p[3] is None)
+            plain = s.encoding is None and s.resampler is None and s.warp is None
+            k = plain_key if plain else (s.encoding, s.resampler is not None, p[3] is None, s.warp is not None)
             groups.setdefault(k, []).append(p)
 
         def device_post(pl, key):
-            encoding, resampled, whole = key
+            encoding, resampled, whole, warped = key
             chunks = [(s.enc, lo, hi) + ((0, 0) if trim is None else _trim_frames(trim)) for s, lo, hi, trim in pl]
-            extra = {} if not resampled else {"resamplers": [p[0].resampler for p in pl], "last": [p[0].done for p in pl]}
+            extra = {} if not (resampled or warped) else {"resamplers": [p[0].resampler for p in pl],
+                                                          "last": [p[0].done for p in pl]}
+            if warped:
+                extra["warps"] = [p[0].warp for p in pl]
             if encoding is not None:
                 extra.update(encoding=encoding, gains=[p[0].gain for p in pl])
             return self.model.infer_decoder_batch(chunks, fade=0 if whole else 42, **extra)
@@ -1203,7 +1275,7 @@ class StreamBatch:
                 out.append((s.key, err))
                 failed.add(s.key)
                 continue
-            if trim is not None and s.resampler is None and s.encoding is None:
+            if trim is not None and s.resampler is None and s.encoding is None and s.warp is None:
                 a = AudioSamples(a.as_slice()[trim])
                 a.crossfade(42)
             out.append((s.key, a))

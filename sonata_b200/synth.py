@@ -131,6 +131,19 @@ def _prosody_extra(n: int, pitch_ratio, tempo) -> dict:
     return out
 
 
+def _stream_prosody_extra(model, pitch_ratio, tempo, where: str) -> dict:
+    """The stream_synthesis keywords of a streaming request's ratios ({} without either).  A model that is not one of
+    this library's streaming voices cannot warp a stream on the device and refuses by name (piper.refuse_prosody)."""
+    from .piper import VitsStreamingModel, _prosody_arrays, refuse_prosody
+    if not isinstance(model, VitsStreamingModel):
+        refuse_prosody(pitch_ratio, tempo, where)
+    p, t = _prosody_arrays([pitch_ratio], [tempo], 1)
+    out = {} if p is None else {"pitch": pitch_ratio}
+    if t is not None:
+        out["tempo"] = tempo
+    return out
+
+
 def _device_g711(model) -> bool:
     """Whether `model` encodes G.711 on the device (VitsModel / VitsStreamingModel).  Other SonataModels (fakes in
     tests) get the host definition, AudioSamples.as_g711_bytes, of the audio they return."""
@@ -260,9 +273,9 @@ class SonataSpeechSynthesizer:
         chunk_size is multiplied by the number of chunks already produced for every following sentence.
         `output_rate`: each sentence is resampled as its own stream (zero history at its start, flushed at its end).
         `encoding`: every chunk is G.711 bytes of its to_i16_vec after the volume, encoded on the device.
-        `pitch_ratio` / `tempo`: refused here unless neutral (see piper.refuse_prosody)."""
-        from .piper import refuse_prosody
-        refuse_prosody(pitch_ratio, tempo, "synthesize_streamed")
+        `pitch_ratio` / `tempo`: every sentence warped as its own stream on the device (a fresh piper.ProsodyStream,
+        flushed at its end); appended silence is not warped."""
+        pros = _stream_prosody_extra(self.model, pitch_ratio, tempo, "synthesize_streamed")
         sentence_seed(seed, 0)
         _check_output_rate(output_rate)
         refuse_flac(encoding, "synthesize_streamed")
@@ -276,6 +289,7 @@ class SonataSpeechSynthesizer:
             rate["encoding"] = encoding
             if output_config is not None and output_config.gain() is not None:
                 rate["gain"] = output_config.gain()
+        rate.update(pros)
         extra = lambda i: dict(rate) if seed is None else dict(rate, seed=sentence_seed(seed, i))
 
         def emit(chunk):
@@ -415,9 +429,9 @@ class RealtimeBatch:
             seed: Optional[int] = None, output_rate: Optional[int] = None, encoding: Optional[str] = None,
             pitch_ratio: Optional[float] = None, tempo: Optional[float] = None) -> int:
         """`seed`: the request's noise seed, `output_rate` its sample rate and `encoding` its G.711 encoding, as for
-        synthesize_streamed; `pitch_ratio` / `tempo` are refused unless neutral, as there."""
-        from .piper import PiperSynthesisConfig, refuse_prosody
-        refuse_prosody(pitch_ratio, tempo, "RealtimeBatch")
+        synthesize_streamed, and `pitch_ratio` / `tempo` its ratios, each sentence warped as its own stream, as there."""
+        from .piper import PiperSynthesisConfig
+        pros = _stream_prosody_extra(self.model, pitch_ratio, tempo, "RealtimeBatch")
         sentence_seed(seed, 0)
         _check_output_rate(output_rate)
         refuse_flac(encoding, "RealtimeBatch")
@@ -432,6 +446,7 @@ class RealtimeBatch:
         if any(len(i) == 0 for i in ids):
             raise OperationError("Failed to run model inference. Error: empty input sequence")
         req = _Request(self._next_key, ids, output_config, config, self.chunk_size, seed, output_rate or None, encoding)
+        req.prosody = pros
         self._next_key += 1
         self._start_sentence(req)
         return req.key
@@ -446,6 +461,7 @@ class RealtimeBatch:
             rate["encoding"] = req.encoding
             if req.output_config is not None and req.output_config.gain() is not None:
                 rate["gain"] = req.output_config.gain()
+        rate.update(req.prosody)
         self._by_stream[self._streams._add(req.ids[req.next], req.config, req.cs, sentence_seed(req.seed, req.next),
                                            **rate)] = req
         req.next += 1

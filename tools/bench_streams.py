@@ -12,9 +12,11 @@ K, one JSON line:
                     out (and how many streams had at least one)
   pad_frac          StreamBatch only: padding rows of the decoder passes' frame levels over all their rows (each chunk
                     occupies whole 128-frame granules)
-The device name and power limit are printed first, read in the same run.
+The device name and power limit are printed first, read in the same run.  With --ratios the arms are StreamBatch runs
+with every stream at one pair of pitch / tempo ratios (none, pitch 1.25, tempo 1.5, pitch 0.8 with tempo 2), whose lines
+add the "stretch" and "pitch" device ms per step; audio_s_per_s is then at the delivered length.
 
-  python tools/bench_streams.py [--ks 1,8,32,128] [--reps 1]
+  python tools/bench_streams.py [--ks 1,8,32,128] [--reps 1] [--ratios]
 """
 import argparse
 import atexit
@@ -86,6 +88,50 @@ def run_batch(model, batches, sr):
     return wall, [arrivals[k] for k in keys], [lens[k] for k in keys], {"pad_frac": round(pad, 4)}
 
 
+RATIO_ARMS = {"none": {}, "pitch_1.25": {"pitch": 1.25}, "tempo_1.5": {"tempo": 1.5},
+              "pitch_0.8_tempo_2": {"pitch": 0.8, "tempo": 2.0}}
+
+
+def run_ratios(model, batches, sr, ratios):
+    """StreamBatch with every stream at `ratios`: the batch arm's figures plus the "stretch" and "pitch" device ms per
+    step (each warped pass's regions, summed over the passes of a step, averaged over the steps)."""
+    from sonata_b200 import StreamBatch
+    decode = model.infer_decoder_batch
+    prof = {"stretch": 0.0, "pitch": 0.0}
+
+    def timed(chunks, **kw):
+        out = decode(chunks, **kw)
+        w = next((w for w in kw.get("warps") or [] if w is not None), None)
+        if w is not None:
+            s, p = w.last_pass_ms()
+            prof["stretch"] += s
+            prof["pitch"] += p
+        return out
+    model.infer_decoder_batch = timed
+    steps = 0
+    try:
+        sb = StreamBatch(model, CHUNK, PAD)
+        t0 = time.perf_counter()
+        keys = [sb.add(ids, **ratios) for ids in batches]
+        arrivals = {k: [] for k in keys}
+        lens = {k: [] for k in keys}
+        while len(sb):
+            out = sb.step()
+            steps += 1
+            t = time.perf_counter() - t0
+            for key, a in out:
+                if isinstance(a, Exception):
+                    raise a
+                arrivals[key].append(t)
+                lens[key].append(len(a))
+        wall = time.perf_counter() - t0
+    finally:
+        del model.infer_decoder_batch
+    return wall, [arrivals[k] for k in keys], [lens[k] for k in keys], {
+        "stretch_ms_per_step": round(prof["stretch"] / max(steps, 1), 3),
+        "pitch_ms_per_step": round(prof["pitch"] / max(steps, 1), 3), "steps": steps}
+
+
 def run_threads(model, batches, sr):
     from sonata_b200 import SpeechStreamer
     k = len(batches)
@@ -119,6 +165,9 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--ks", default="1,8,32,128")
     ap.add_argument("--reps", type=int, default=1, help="timed runs per arm and K (each line is one run)")
+    ap.add_argument("--ratios", action="store_true",
+                    help="StreamBatch arms with pitch / tempo ratios instead (no ratios, pitch 1.25, tempo 1.5, pitch "
+                         "0.8 with tempo 2), alternated in each rep; audio_s_per_s is at the delivered length")
     args = ap.parse_args()
 
     import torch
@@ -140,6 +189,8 @@ def main():
     ks = [int(k) for k in args.ks.split(",")]
     batches = [[int(i) for i in workload.synthetic_ids(PHONEMES, utt=u)] for u in range(max(ks))]
     arms = {"stream_batch": run_batch, "threads": run_threads}
+    if args.ratios:
+        arms = {name: (lambda m, b, s, r=r: run_ratios(m, b, s, r)) for name, r in RATIO_ARMS.items()}
     for k in ks:
         for name, fn in arms.items():            # warm-up: modules, arenas and pinned blocks at this K
             fn(model, batches[:k], sr)
