@@ -354,6 +354,10 @@ struct IdBufs {
     NoiseSeed *seeds, *seeds_h;                // per utterance (only when the job has seeds; read at both levels)
     float *qkv0, *att0, *p0, *vt0;             // debug: layer 0's attention operands and result
     std::vector<std::array<float*, 4>> dpf;    // debug: each duration flow's input, DDSConv output, spline parameters, output
+    float* emb0;                               // debug: the scaled embedding, before layer 0
+    // debug: each encoder layer's stages, ENC_* order (vt only with the tensor-core attention, stored [H][RX])
+    enum { ENC_QKV, ENC_VT, ENC_ATT, ENC_O, ENC_LN1, ENC_FFN1, ENC_FFN2, ENC_LN2, ENC_NCAP };
+    std::vector<std::array<float*, ENC_NCAP>> encl;
 
     void carve(Arena& dev, Arena& pin, const Job& j, bool tc_att) {
         const Voice& v = *j.v; const Arch& a = v.a;
@@ -386,12 +390,18 @@ struct IdBufs {
         const bool seeded = !j.seeds.empty();
         seeds = seeded ? dev.get<NoiseSeed>(B) : nullptr; seeds_h = seeded ? pin.get<NoiseSeed>(B) : nullptr;
         qkv0 =att0 = p0 = vt0 = nullptr;
+        emb0 = nullptr;
         dpf.clear();
+        encl.clear();
         if (j.debug) {
             qkv0 = rows(3 * H); att0 = rows(H);
             if (tc_att) { p0 = rows(j.att_tp); vt0 = rows(H); }
             dpf.resize(v.dp_flows.size());
             for (auto& f : dpf) f = {rows(2), rows(H), rows(32), rows(2)};
+            emb0 = rows(H);
+            encl.resize(a.layers);
+            for (auto& e : encl)
+                e = {rows(3 * H), tc_att ? rows(H) : nullptr, rows(H), rows(H), rows(H), rows(a.filter), rows(H), rows(H)};
         }
     }
 };
@@ -984,6 +994,16 @@ void Job::run(float* d_out, size_t d_out_cap) {
             expose(*this, fs + "in", x.dpf[s][0], 2, 0); expose(*this, fs + "h", x.dpf[s][1], H, 0);
             expose(*this, fs + "h29", x.dpf[s][2], 32, 0); expose(*this, fs + "out", x.dpf[s][3], 2, 0);
         }
+        expose(*this, "enc.emb", x.emb0, H, 0);
+        for (int l = 0; l < a.layers; l++) {
+            const std::string p = "enc." + std::to_string(l) + ".";
+            const auto& c = x.encl[l];
+            expose(*this, p + "qkv", c[IdBufs::ENC_QKV], 3 * H, 0);
+            if (tc_att_ok) expose(*this, p + "vt", c[IdBufs::ENC_VT], H, -1);   // stored as [H][RX]
+            expose(*this, p + "att", c[IdBufs::ENC_ATT], H, 0); expose(*this, p + "o", c[IdBufs::ENC_O], H, 0);
+            expose(*this, p + "ln1", c[IdBufs::ENC_LN1], H, 0); expose(*this, p + "ffn1", c[IdBufs::ENC_FFN1], F, 0);
+            expose(*this, p + "ffn2", c[IdBufs::ENC_FFN2], H, 0); expose(*this, p + "ln2", c[IdBufs::ENC_LN2], H, 0);
+        }
     }
     if (x.epsw) {
         if (!eps_w.empty()) {
@@ -1010,12 +1030,19 @@ void Job::run(float* d_out, size_t d_out_cap) {
     R.begin("enc");
     launch_embed(x.ids_rows, V.emb, sqrtf((float)H), x.xa, RX, H, st);
     R.count(0, 4.0 * LX.valid_rows * H);
+    // debug: every stage is copied right after its launch (xa and xb are overwritten in place)
+    if (debug) d2d(x.emb0, x.xa, (size_t)RX * H, st);
     for (int l = 0; l < a.layers; l++) {
         const EncLayer& e = V.enc[l];
+        float* const* cap = debug ? x.encl[l].data() : nullptr;
         {
             ConvCall o; o.y0 = x.qkv; o.ldy0 = 3 * H;
             if (tc_att_ok) { o.yt = x.att_vt; o.yt_col0 = 2 * H; o.ldyt = RX; }       // V leaves transposed: [H][RX]
             R.conv(e.qkv, x.xa, H, LX, o);
+        }
+        if (cap) {
+            d2d(cap[IdBufs::ENC_QKV], x.qkv, (size_t)RX * 3 * H, st);
+            if (tc_att_ok) d2d(cap[IdBufs::ENC_VT], x.att_vt, (size_t)H * RX, st);
         }
         if (tc_att_ok) {
             launch_gemm_tf(gs, st);
@@ -1036,13 +1063,19 @@ void Job::run(float* d_out, size_t d_out_cap) {
                 d2d(x.vt0, x.att_vt, (size_t)H * RX, st);
             }
         }
+        if (cap) d2d(cap[IdBufs::ENC_ATT], x.att, (size_t)RX * H, st);
         { ConvCall o; o.y0 = x.xb; o.ldy0 = H; R.conv(e.o, x.att, H, LX, o); }
+        if (cap) d2d(cap[IdBufs::ENC_O], x.xb, (size_t)RX * H, st);
         launch_ln(x.xa, x.xb, nullptr, e.g1, e.b1, x.xa, H, 0, LX.map, st);
         R.count(0, 12.0 * LX.valid_rows * H);
+        if (cap) d2d(cap[IdBufs::ENC_LN1], x.xa, (size_t)RX * H, st);
         { ConvCall o; o.act = ACT_RELU; o.y0 = x.ffn; o.ldy0 = F; R.conv(e.ffn1, x.xa, H, LX, o); }
+        if (cap) d2d(cap[IdBufs::ENC_FFN1], x.ffn, (size_t)RX * F, st);
         { ConvCall o; o.y0 = x.xb; o.ldy0 = H; R.conv(e.ffn2, x.ffn, F, LX, o); }
+        if (cap) d2d(cap[IdBufs::ENC_FFN2], x.xb, (size_t)RX * H, st);
         launch_ln(x.xa, x.xb, nullptr, e.g2, e.b2, x.xa, H, 0, LX.map, st);
         R.count(0, 12.0 * LX.valid_rows * H);
+        if (cap) d2d(cap[IdBufs::ENC_LN2], x.xa, (size_t)RX * H, st);
     }
     { ConvCall o; o.y0 = x.stats; o.ldy0 = 2 * I; R.conv(V.enc_proj, x.xa, H, LX, o); }
     R.end();

@@ -253,15 +253,28 @@ TF_CASES = [
     (18432, 192, 576, 1, 1, 1.0, 0, False, 1.0, False, 18000),
     (18432, 768, 192, 3, 1, 1.0, 0, True, 1.0, False, None),
     (18432 + 128, 192, 768, 3, 1, 1.0, 1, False, 1.0, False, None),
+    # x_low (96 hidden channels): qkv, conv_o, ffn1, ffn2 and proj of the encoder, the duration predictor's 96 -> 96 and
+    # 96 -> 32 1x1 layers, the single-utterance ffn2 shape and a many-tile ffn2 with a residual
+    (256, 96, 288, 1, 1, 1.0, 0, False, 1.0, False, None),
+    (256, 96, 96, 1, 1, 1.0, 0, False, 1.0, False, 201),
+    (256, 96, 384, 3, 1, 1.0, 1, False, 1.0, False, None),
+    (256, 384, 96, 3, 1, 1.0, 0, False, 1.0, False, 255),
+    (256, 96, 192, 1, 1, 1.0, 0, False, 1.0, False, None),
+    (300, 96, 96, 1, 1, 1.0, 0, True, 0.5, True, 290),
+    (256, 96, 32, 1, 1, 1.0, 0, False, 1.0, False, None),
+    (512, 384, 96, 3, 1, 1.0, 0, False, 1.0, False, 258),
+    (18432, 384, 96, 3, 1, 1.0, 0, True, 1.0, False, 18000),
 ]
 
 # Several segments in one launch (the engine's packed batches).  (lens, gran, seg_mul, cin, cout, k, dil, slope, act, res,
 # scale, acc): X-level granules of 64 ids with segment ends ragged inside a 128-row tile and a 2-row segment shorter than
-# the conv's halo; Y-level granules of 128 frames; a decoder level at U = 4 / 8 rows per frame (gran = 128 U, seg_mul = U).
+# the conv's halo (also at x_low's 96 / 384 channels); Y-level granules of 128 frames; a decoder level at U = 4 / 8 rows per frame (gran = 128 U, seg_mul = U).
 SEG_CASES = [
     ((50, 2, 100, 77, 3), 64, 1, 192, 192, 3, 1, 1.0, 0, False, 1.0, False),
     ((50, 2, 100, 77, 3), 64, 1, 192, 576, 1, 1, 1.0, 0, False, 1.0, True),
     ((50, 2, 100, 77, 3), 64, 1, 192, 768, 3, 1, 1.0, 1, True, 0.5, True),
+    ((50, 2, 100, 77, 3, 48), 64, 1, 96, 384, 3, 1, 1.0, 1, False, 1.0, False),
+    ((50, 2, 100, 77, 3, 48), 64, 1, 384, 96, 3, 1, 1.0, 0, True, 1.0, False),
     ((130, 2, 5, 300), 128, 1, 192, 384, 5, 1, 1.0, 2, False, 1.0, False),
     ((130, 2, 5, 300), 128, 1, 128, 128, 11, 5, 0.1, 0, True, 1 / 3, True),
     ((3, 20, 7, 1), 512, 4, 64, 64, 7, 12, 0.1, 0, True, 1 / 3, True),
