@@ -700,7 +700,7 @@ int32_t sb200_job_debug_fetch(sb200_job* job, const char* name, size_t b, float*
         const int C = it->second.second;
         size_t r0, nr;
         if (U <= 0) { r0 = (size_t)j.xsegs[b].off; nr = (size_t)j.xsegs[b].len; }
-        else { r0 = (size_t)j.fsegs[b].off * U; nr = (size_t)j.fsegs[b].len * U; }
+        else { r0 = (size_t)j.frames.fsegs[b].off * U; nr = (size_t)j.frames.fsegs[b].len * U; }
         *data = (float*)malloc(nr * C * 4 + 4);
         SB_CUDA(cudaSetDevice(j.v->device));
         if (U < 0) {        // transposed [C][RX]: the utterance's columns of every row -> [C][len]

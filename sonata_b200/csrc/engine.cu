@@ -263,14 +263,17 @@ void set_job_prosody(Job& j, const float* pitch, const float* tempo) {
 
 namespace {
 
+// Launches of one pass on context c's stream, each counted in the profile region of `regions` open at the time.  cond:
+// the effective biases of the speaker-conditioned convs, [slot][cond_rows] (null on a single-speaker voice).
 struct Runner {
-    Job& j; Voice& v; Context& c; const Arch& a; cudaStream_t st;
+    Voice& v; Context& c; std::vector<Region>& regions; const float* cond; const Arch& a; cudaStream_t st;
     Region* cur = nullptr;
-    Runner(Job& job) : j(job), v(*job.v), c(*job.ctx), a(job.v->a), st(job.ctx->stream) {}
+    Runner(Voice& voice, Context& ctx, std::vector<Region>& regs, const float* cond_bias)
+        : v(voice), c(ctx), regions(regs), cond(cond_bias), a(voice.a), st(ctx.stream) {}
 
     void begin(const std::string& name) {
-        j.regions.emplace_back();
-        cur = &j.regions.back();
+        regions.emplace_back();
+        cur = &regions.back();
         cur->name = name;
         cur->e0 = c.next_event(); cur->e1 = c.next_event();
         cudaEventRecord(cur->e0, st);
@@ -283,9 +286,9 @@ struct Runner {
     void conv(const ConvW& w, const float* x, int ldx, const Level& lin, const ConvCall& o) {
         ConvArgs p = conv_args(w, x, ldx, lin.map, o);
         // on a multi-speaker voice, the speaker-conditioned bias of each row's slot
-        if (j.d_cond && w.cond_off >= 0) {
+        if (cond && w.cond_off >= 0) {
             if (!lin.bias_slot) throw Error(19, "internal: a speaker-conditioned conv on a level without a slot table");
-            p.bias = j.d_cond + w.cond_off; p.bias_slot = lin.bias_slot; p.ldbias = v.cond_rows;
+            p.bias = cond + w.cond_off; p.bias_slot = lin.bias_slot; p.ldbias = v.cond_rows;
         }
         // The layer's images name the kernels that can run it.  Backend 1 (default): conv_tf, else conv_tc; 2: conv_tc
         // (the text encoder and the duration predictor on fp32 CUDA cores, kept for A/B runs); 0: fp32 CUDA cores
@@ -317,9 +320,6 @@ struct Runner {
     }
 };
 
-void h2d(void* dst, const void* src, size_t bytes, cudaStream_t st) {
-    SB_CUDA(cudaMemcpyAsync(dst, src, bytes, cudaMemcpyHostToDevice, st));
-}
 void d2d(float* dst, const float* src, size_t n, cudaStream_t st) {
     SB_CUDA(cudaMemcpyAsync(dst, src, n * 4, cudaMemcpyDeviceToDevice, st));
 }
@@ -340,18 +340,63 @@ template <typename Carve> void plan(Arena& dev, Arena& pin, Carve&& carve) {
     carve(dev, pin);
 }
 
+// A table the host fills and the device reads, or the reverse: the device table `d` and its page-locked mirror `h`,
+// carved together with one element count, so every copy moves exactly the carved table.  Unset (null) when not carved.
+template <typename T> struct Staged {
+    T* d = nullptr; T* h = nullptr; size_t n = 0;
+    void carve(Arena& dev, Arena& pin, size_t count) { n = count; d = dev.get<T>(n); h = pin.get<T>(n); }
+    void upload(cudaStream_t st) const { SB_CUDA(cudaMemcpyAsync(d, h, n * sizeof(T), cudaMemcpyHostToDevice, st)); }
+    void download(cudaStream_t st) const { SB_CUDA(cudaMemcpyAsync(h, d, n * sizeof(T), cudaMemcpyDeviceToHost, st)); }
+};
+
+// Gives the next segment of a pass the slot of speaker `sid`, a new one for a speaker not seen before; false when sid
+// is not a speaker of the voice.  On a single-speaker voice every segment has slot 0 and the pass has no slots.
+bool assign_slot(FrameLayout& l, const Voice& v, long long sid) {
+    if (v.num_speakers <= 1) { l.slot_of.push_back(0); return true; }
+    if (sid < 0 || sid >= v.emb_rows) return false;
+    const auto it = std::find(l.slot_sid.begin(), l.slot_sid.end(), (int)sid);
+    l.slot_of.push_back((int)(it - l.slot_sid.begin()));
+    if (it == l.slot_sid.end()) l.slot_sid.push_back((int)sid);
+    return true;
+}
+
+// Speaker conditioning of a pass with speaker slots: the speaker of every slot and the effective biases of the
+// speaker-conditioned convs, [slot][cond_rows].  Unset without slots.
+struct SpeakerBias {
+    Staged<int> sid; float* cond = nullptr;
+    void carve(Arena& dev, Arena& pin, const Voice& v, const FrameLayout& l) {
+        if (l.slot_sid.empty()) return;
+        cond = dev.get<float>(l.slot_sid.size() * v.cond_rows);
+        sid.carve(dev, pin, l.slot_sid.size());
+    }
+    // Fills the speaker table and launches the computation of the biases.
+    void run(const Voice& v, const FrameLayout& l, cudaStream_t st) const {
+        if (!cond) return;
+        std::copy(l.slot_sid.begin(), l.slot_sid.end(), sid.h);
+        sid.upload(st);
+        launch_cond_bias(v.cond_w, v.cond_base, v.emb_g, sid.d, (int)sid.n, v.cond_rows, v.gin, cond, st);
+    }
+};
+
+// The start of a pass on context c: its events are taken again from the first, and ev_begin is recorded.
+void begin_pass(Context& c) {
+    c.events_used = 0;
+    if (!c.ev_begin) { SB_CUDA(cudaEventCreate(&c.ev_begin)); SB_CUDA(cudaEventCreate(&c.ev_end)); }
+    SB_CUDA(cudaEventRecord(c.ev_begin, c.stream));
+}
+
 // Id level (phase 1): X tables, encoder and duration-predictor activations, and with debug the captures.
 struct IdBufs {
-    int *ids_rows_h, *xend_h, *xseg_of_h, *ylen_h; SegInfo* xsegs_h; TfTile* tiles_h;     // pinned staging
-    float* scales_h; int *xslot_h, *sid_h;
-    int *ids_rows, *xend, *xseg_of_gran, *cum, *ylen; SegInfo* xsegs; TfTile* tiles;
-    float* scales;                             // per utterance: noise_w [B], length_scale [B], noise_scale [B]
-    int *xslot, *sid;                          // multi-speaker voices: speaker slot of every X granule, speaker of every slot
+    Staged<int> ids_rows, xend, xseg_of_gran, ylen; Staged<SegInfo> xsegs; Staged<TfTile> tiles;
+    Staged<float> scales;                      // per utterance: noise_w [B], length_scale [B], noise_scale [B]
+    Staged<int> xslot;                         // multi-speaker voices: speaker slot of every X granule
+    SpeakerBias spk;
+    int* cum;
     float *xa, *xb, *qkv, *att, *ffn, *stats, *d0, *t1, *t2, *g, *h29, *zz, *logw;
     float *att_s, *att_vt, *att_orel;          // tensor-core attention: scores of every head, V^T, relative-value term
-    float *epsw, *cond;                        // cond: [slot][cond_rows]
-    float *dscale, *dscale_h; int *dframes, *dframes_h;   // per-id duration controls (only when the job has them)
-    NoiseSeed *seeds, *seeds_h;                // per utterance (only when the job has seeds; read at both levels)
+    float* epsw;
+    Staged<float> dscale; Staged<int> dframes; // per-id duration controls (only when the job has them)
+    Staged<NoiseSeed> seeds;                   // per utterance (only when the job has seeds; read at both levels)
     float *qkv0, *att0, *p0, *vt0;             // debug: layer 0's attention operands and result
     std::vector<std::array<float*, 4>> dpf;    // debug: each duration flow's input, DDSConv output, spline parameters, output
     float* emb0;                               // debug: the scaled embedding, before layer 0
@@ -364,18 +409,13 @@ struct IdBufs {
         const int RX = j.RX, nxg = RX / GX, H = a.hidden;
         const size_t B = j.B, ntiles = j.tiles_s.size() + j.tiles_o.size();
         auto rows = [&](int cols) { return dev.get<float>((size_t)RX * cols); };
-        ids_rows_h = pin.get<int>(RX); xend_h = pin.get<int>(nxg); xseg_of_h = pin.get<int>(nxg);
-        xsegs_h = pin.get<SegInfo>(B); ylen_h = pin.get<int>(B);
-        tiles_h = tc_att ? pin.get<TfTile>(ntiles) : nullptr;
-        const bool multi = v.num_speakers > 1;
-        const size_t nslots = j.slot_sid.size();
-        scales_h = pin.get<float>(3 * B);
-        xslot_h = multi ? pin.get<int>(nxg) : nullptr; sid_h = multi ? pin.get<int>(nslots) : nullptr;
-        ids_rows = dev.get<int>(RX); xend = dev.get<int>(nxg); xseg_of_gran = dev.get<int>(nxg); xsegs = dev.get<SegInfo>(B);
-        cum = dev.get<int>(RX); ylen = dev.get<int>(B);
-        tiles = tc_att ? dev.get<TfTile>(ntiles) : nullptr;
-        scales = dev.get<float>(3 * B);
-        xslot = multi ? dev.get<int>(nxg) : nullptr; sid = multi ? dev.get<int>(nslots) : nullptr;
+        ids_rows.carve(dev, pin, RX); xend.carve(dev, pin, nxg); xseg_of_gran.carve(dev, pin, nxg);
+        xsegs.carve(dev, pin, B); ylen.carve(dev, pin, B);
+        if (tc_att) tiles.carve(dev, pin, ntiles);
+        scales.carve(dev, pin, 3 * B);
+        if (!j.frames.slot_sid.empty()) xslot.carve(dev, pin, nxg);
+        spk.carve(dev, pin, v, j.frames);
+        cum = dev.get<int>(RX);
         xa = rows(H); xb = rows(H); qkv = rows(3 * H); att = rows(H); ffn = rows(a.filter); stats = rows(2 * a.inter);
         d0 = rows(H); t1 = rows(H); t2 = rows(H); g = rows(H); h29 = rows(32); zz = rows(2); logw = rows(1);
         att_s = att_vt = att_orel = nullptr;
@@ -383,12 +423,9 @@ struct IdBufs {
         bool any_noise_w = false;
         for (const SynthConfig& c : j.cfgs) any_noise_w |= c.noise_w != 0.f;
         epsw = any_noise_w ? rows(2) : nullptr;
-        cond = multi ? dev.get<float>(nslots * v.cond_rows) : nullptr;
-        const bool scaled = !j.dur_scale.empty(), fixed = !j.dur_frames.empty();
-        dscale = scaled ? dev.get<float>(RX) : nullptr; dscale_h = scaled ? pin.get<float>(RX) : nullptr;
-        dframes = fixed ? dev.get<int>(RX) : nullptr; dframes_h = fixed ? pin.get<int>(RX) : nullptr;
-        const bool seeded = !j.seeds.empty();
-        seeds = seeded ? dev.get<NoiseSeed>(B) : nullptr; seeds_h = seeded ? pin.get<NoiseSeed>(B) : nullptr;
+        if (!j.dur_scale.empty()) dscale.carve(dev, pin, RX);
+        if (!j.dur_frames.empty()) dframes.carve(dev, pin, RX);
+        if (!j.seeds.empty()) seeds.carve(dev, pin, B);
         qkv0 =att0 = p0 = vt0 = nullptr;
         emb0 = nullptr;
         dpf.clear();
@@ -407,17 +444,13 @@ struct IdBufs {
 };
 
 // Frame-level tables (segment end, owner and on multi-speaker voices speaker slot of every GY-frame tile, the segment
-// list) and their pinned mirrors.
+// list) of layout l.
 struct FrameTables {
-    int *yend, *ftile, *yslot; FrameSeg* fsegs;
-    int *yend_h, *ftile_h, *yslot_h; FrameSeg* fsegs_h;
-    void carve(Arena& dev, Arena& pin, const Job& j) {
-        const int ntile = j.RY / GY; const size_t B = j.fsegs.size();
-        const bool multi = j.v->num_speakers > 1;
-        yend = dev.get<int>(ntile); ftile = dev.get<int>(ntile); fsegs = dev.get<FrameSeg>(B);
-        yend_h = pin.get<int>(ntile); ftile_h = pin.get<int>(ntile); fsegs_h = pin.get<FrameSeg>(B);
-        yslot = multi ? dev.get<int>(ntile) : nullptr;
-        yslot_h = multi ? pin.get<int>(ntile) : nullptr;
+    Staged<int> yend, ftile, yslot; Staged<FrameSeg> fsegs;
+    void carve(Arena& dev, Arena& pin, const FrameLayout& l) {
+        const int ntile = l.RY / GY;
+        yend.carve(dev, pin, ntile); ftile.carve(dev, pin, ntile); fsegs.carve(dev, pin, l.fsegs.size());
+        if (!l.slot_sid.empty()) yslot.carve(dev, pin, ntile);
     }
 };
 
@@ -458,50 +491,51 @@ struct ResamplePlan {
 // has no post-path, or for the i16 conversion of its output; out_gain[k], when given, is output k's gain there) and the
 // output segments, n_out samples at out_off.
 struct ResampleTables {
-    ResampleSeg *segs, *segs_h; PcmPost *posts, *posts_h; FrameSeg *osegs, *osegs_h;
+    Staged<ResampleSeg> segs; Staged<PcmPost> posts; Staged<FrameSeg> osegs;
     void carve(Arena& dev, Arena& pin, size_t n) {
-        segs = dev.get<ResampleSeg>(n); segs_h = pin.get<ResampleSeg>(n);
-        posts = dev.get<PcmPost>(n); posts_h = pin.get<PcmPost>(n);
-        osegs = dev.get<FrameSeg>(n); osegs_h = pin.get<FrameSeg>(n);
+        segs.carve(dev, pin, n); posts.carve(dev, pin, n); osegs.carve(dev, pin, n);
     }
     void upload(const ResamplePlan& p, cudaStream_t st, const std::vector<float>* out_gain = nullptr) {
-        const size_t n = p.segs.size();
-        for (size_t k = 0; k < n; k++) {
-            segs_h[k] = p.segs[k];
-            posts_h[k] = PcmPost();
-            if (out_gain) posts_h[k].gain = (*out_gain)[k];
-            osegs_h[k] = FrameSeg{0, (int)p.segs[k].n_out, 0, 0, p.segs[k].out_off};
+        for (size_t k = 0; k < p.segs.size(); k++) {
+            segs.h[k] = p.segs[k];
+            posts.h[k] = PcmPost();
+            if (out_gain) posts.h[k].gain = (*out_gain)[k];
+            osegs.h[k] = FrameSeg{0, (int)p.segs[k].n_out, 0, 0, p.segs[k].out_off};
         }
-        h2d(segs, segs_h, n * sizeof(ResampleSeg), st);
-        h2d(posts, posts_h, n * sizeof(PcmPost), st);
-        h2d(osegs, osegs_h, n * sizeof(FrameSeg), st);
+        segs.upload(st); posts.upload(st); osegs.upload(st);
     }
 };
 
-// Device buffers of the prosody launches and the pinned mirrors of their tables: the segments, the output segments
-// (n2 samples at y_off, for the launches that read the prosody output), every frame's offset, the stretched signals of
-// the segments that run both stages, and the output unless it goes straight to the caller's buffer.
+// Device buffers of the prosody launches of plan p and the pinned mirrors of their tables: the segments, every frame's
+// offset, the stretched signals of the segments that run both stages, and the output unless it goes elsewhere.  A plan
+// of whole signals adds the output segments (n2 samples at y_off, for the launches that read the prosody output); a
+// plan of stream windows the carry entry of every window and the staged input windows.
 struct ProsodyBufs {
-    ProsodySeg *segs = nullptr, *segs_h = nullptr; FrameSeg *osegs = nullptr, *osegs_h = nullptr;
-    int* offsets = nullptr; float *s = nullptr, *y = nullptr;
+    Staged<ProsodySeg> segs; Staged<FrameSeg> osegs; Staged<ProsodyCarry> carry;
+    int* offsets = nullptr; float *x = nullptr, *s = nullptr, *y = nullptr;
     void carve(Arena& dev, Arena& pin, const ProsodyPlan& p, bool own_y) {
         const size_t n = p.segs.size();
         y = nullptr;
         if (n == 0) return;
-        segs = dev.get<ProsodySeg>(n); segs_h = pin.get<ProsodySeg>(n);
-        osegs = dev.get<FrameSeg>(n); osegs_h = pin.get<FrameSeg>(n);
+        segs.carve(dev, pin, n);
+        if (p.in_total) {
+            carry.carve(dev, pin, n);
+            x = dev.get<float>((size_t)p.in_total + 4);
+        } else {
+            osegs.carve(dev, pin, n);
+        }
         offsets = p.d_total ? dev.get<int>((size_t)p.d_total) : nullptr;
         s = p.s_total ? dev.get<float>((size_t)p.s_total + 4) : nullptr;
         if (own_y) y = dev.get<float>((size_t)p.y_total + 4);
     }
-    void upload(const ProsodyPlan& p, cudaStream_t st) {
-        const size_t n = p.segs.size();
-        for (size_t k = 0; k < n; k++) {
-            segs_h[k] = p.segs[k];
-            osegs_h[k] = FrameSeg{0, (int)p.segs[k].n2, 0, 0, p.segs[k].y_off};
+    // Fills and uploads the segments and, for whole signals, the output segments; a stream pass fills the carry.
+    void upload(const ProsodyPlan& p, cudaStream_t st) const {
+        for (size_t k = 0; k < p.segs.size(); k++) {
+            segs.h[k] = p.segs[k];
+            if (osegs.d) osegs.h[k] = FrameSeg{0, (int)p.segs[k].n2, 0, 0, p.segs[k].y_off};
         }
-        h2d(segs, segs_h, n * sizeof(ProsodySeg), st);
-        h2d(osegs, osegs_h, n * sizeof(FrameSeg), st);
+        segs.upload(st);
+        if (osegs.d) osegs.upload(st);
     }
 };
 
@@ -514,17 +548,15 @@ struct LoudnessPlan {
 
 // Device tables of the loudness launch and their pinned mirrors: the segments, the chunk scratch and the results.
 struct LoudnessBufs {
-    LoudSeg *segs = nullptr, *segs_h = nullptr;
+    Staged<LoudSeg> segs;
     double* scratch = nullptr;
-    double *lufs = nullptr, *lufs_h = nullptr;
-    float *gain = nullptr, *gain_h = nullptr;
+    Staged<double> lufs; Staged<float> gain;
     void carve(Arena& dev, Arena& pin, const LoudnessPlan& p) {
         const size_t n = p.segs.size();
         if (n == 0) return;
-        segs = dev.get<LoudSeg>(n); segs_h = pin.get<LoudSeg>(n);
+        segs.carve(dev, pin, n);
         scratch = dev.get<double>((size_t)LD_SCRATCH * std::max<long long>(p.chunks, 1));
-        lufs = dev.get<double>(n); lufs_h = pin.get<double>(n);
-        gain = dev.get<float>(n); gain_h = pin.get<float>(n);
+        lufs.carve(dev, pin, n); gain.carve(dev, pin, n);
     }
 };
 
@@ -589,8 +621,8 @@ struct FrameBufs {
         }
         if (!pp.segs.empty()) own_wav = true;
         const Arch& a = j.v->a;
-        const size_t RY = (size_t)j.RY;
-        y.carve(dev, pin, j);
+        const size_t RY = (size_t)j.frames.RY;
+        y.carve(dev, pin, j.frames);
         s = dev.get<float>(RY * a.inter);
         bool any_noise = false;
         for (const SynthConfig& c : j.cfgs) any_noise |= c.noise_scale != 0.f;
@@ -601,54 +633,41 @@ struct FrameBufs {
         h = dev.get<float>(RY * a.hidden); acts = dev.get<float>(RY * a.hidden); outb = dev.get<float>(RY * a.hidden);
         wav = nullptr;
         if (j.encode_only) return;
-        if (own_wav) wav = dev.get<float>((size_t)j.total_samples + 4);
-        dec.carve(dev, *j.v, j.RY, j.debug);
+        if (own_wav) wav = dev.get<float>((size_t)j.frames.total_samples + 4);
+        dec.carve(dev, *j.v, j.frames.RY, j.debug);
     }
 };
 
-// One pass of streaming decoder chunks: speaker biases of every slot, tables, the gather table and the latent slices,
-// the decoder and the waveforms; the post-path table when an output stage runs, the resample launch's tables and
-// output, the i16 or G.711 scratch; and the pinned block the packed result (`total` values) is copied to.
+// One pass of streaming decoder chunks (layout l): speaker biases of every slot, tables, the gather table and the
+// latent slices, the decoder and the waveforms; the post-path table when an output stage runs, the resample launch's
+// tables and output, the i16 or G.711 scratch; and the pinned block the packed result (`total` values) is copied to.
 struct ChunkBufs {
-    float* cond;
-    int *sid, *sid_h;
+    SpeakerBias spk;
     FrameTables y;
-    GatherSeg *src, *src_h;
+    Staged<GatherSeg> src;
     float *s, *wav;
     DecoderBufs dec;
-    PcmPost *post, *post_h;
+    Staged<PcmPost> post;
     ResampleTables rt; float* rs;
     void* pcm; unsigned* max;
     void* out_h;
-    // warped chunks (plan `pp`): the prosody tables, windows and offsets, the output after the waveforms in `wav`, and
-    // the resample launch's input table (the prosody output for a warped chunk, the post-path's chunk for the others)
-    ProsodySeg *pseg = nullptr, *pseg_h = nullptr; ProsodyCarry *pcar = nullptr, *pcar_h = nullptr;
-    float *px = nullptr, *ps = nullptr; int* poff = nullptr;
-    FrameSeg *rin = nullptr, *rin_h = nullptr; PcmPost *rpost = nullptr, *rpost_h = nullptr;
-    void carve(Arena& dev, Arena& pin, const Job& j, const ChunkPass& p, const ResamplePlan& rp, const ProsodyPlan& pp,
-               size_t total) {
-        const Voice& v = *j.v;
-        const bool multi = v.num_speakers > 1, i16_out = p.format != PCM_F32;
-        const size_t n = j.fsegs.size(), nslots = j.slot_sid.size();
-        cond = multi ? dev.get<float>(nslots * v.cond_rows) : nullptr;
-        sid = multi ? dev.get<int>(nslots) : nullptr;
-        sid_h = multi ? pin.get<int>(nslots) : nullptr;
-        y.carve(dev, pin, j);
-        src = dev.get<GatherSeg>(n); src_h = pin.get<GatherSeg>(n);
-        s = dev.get<float>((size_t)j.RY * v.a.inter);
-        wav = dev.get<float>((size_t)j.total_samples + (size_t)pp.y_total + 4);
-        if (const size_t m = pp.segs.size()) {
-            pseg = dev.get<ProsodySeg>(m); pseg_h = pin.get<ProsodySeg>(m);
-            pcar = dev.get<ProsodyCarry>(m); pcar_h = pin.get<ProsodyCarry>(m);
-            px = dev.get<float>((size_t)pp.in_total + 4);
-            ps = dev.get<float>((size_t)pp.s_total + 4);
-            poff = dev.get<int>((size_t)pp.d_total + 2);
-            rin = dev.get<FrameSeg>(n); rin_h = pin.get<FrameSeg>(n);
-            rpost = dev.get<PcmPost>(n); rpost_h = pin.get<PcmPost>(n);
-        }
-        dec.carve(dev, v, j.RY, false);
-        post = p.resample || i16_out ? dev.get<PcmPost>(n) : nullptr;
-        post_h = p.resample || i16_out ? pin.get<PcmPost>(n) : nullptr;
+    // warped chunks (plan `pp`): the prosody buffers, the output after the waveforms in `wav`, and the resample
+    // launch's input table (the prosody output for a warped chunk, the post-path's chunk for the others)
+    ProsodyBufs pr;
+    Staged<FrameSeg> rin; Staged<PcmPost> rpost;
+    void carve(Arena& dev, Arena& pin, const Voice& v, const FrameLayout& l, const ChunkPass& p, const ResamplePlan& rp,
+               const ProsodyPlan& pp, size_t total) {
+        const bool i16_out = p.format != PCM_F32;
+        const size_t n = l.fsegs.size();
+        spk.carve(dev, pin, v, l);
+        y.carve(dev, pin, l);
+        src.carve(dev, pin, n);
+        s = dev.get<float>((size_t)l.RY * v.a.inter);
+        wav = dev.get<float>((size_t)l.total_samples + (size_t)pp.y_total + 4);
+        pr.carve(dev, pin, pp, false);
+        if (!pp.segs.empty()) { rin.carve(dev, pin, n); rpost.carve(dev, pin, n); }
+        dec.carve(dev, v, l.RY, false);
+        if (p.resample || i16_out) post.carve(dev, pin, n);
         rt.carve(dev, pin, rp.segs.size());
         rs = p.resample ? dev.get<float>(total + 4) : nullptr;
         pcm = i16_out ? dev.alloc((total + 8) * pcm_bytes(p.format)) : nullptr;
@@ -669,7 +688,7 @@ void run_decoder(Runner& R, const Level& LY, const FrameTables& y, const Decoder
     for (size_t i = 0; i < v.ups.size(); i++) {
         const UpStageW& st = v.ups[i];
         const int Uo = U * st.u;
-        Level Lo; Lo.map = {y.yend, GY * Uo, Uo, RY * Uo}; Lo.valid_rows = LY.valid_rows * Uo;
+        Level Lo; Lo.map = {y.yend.d, GY * Uo, Uo, RY * Uo}; Lo.valid_rows = LY.valid_rows * Uo;
         float *up = d.stage[i][0], *ys = d.stage[i][1];
         float* const* tmp = &d.stage[i][2];
         R.begin("dec.up" + std::to_string(i));
@@ -712,26 +731,27 @@ void run_decoder(Runner& R, const Level& LY, const FrameTables& y, const Decoder
         cur = ys; Lin = Lo; U = Uo;
     }
     R.begin("dec.post");
-    launch_conv_post(cur, v.c_last, v.conv_post_w, d_wav, y.fsegs, y.ftile, U, Lin.map, R.st);
+    launch_conv_post(cur, v.c_last, v.conv_post_w, d_wav, y.fsegs.d, y.ftile.d, U, Lin.map, R.st);
     R.count(2.0 * Lin.valid_rows * v.c_last * 7, 4.0 * Lin.valid_rows * (v.c_last + 1));
     R.end();
 }
 
-// Lays out the frame level for given per-utterance frame counts (host side: segments, rows, output offsets).
-void lay_out_frames(Job& j, const std::vector<int>& y_len, int hop) {
+// Lays out the frame level for given per-segment frame counts (host side: segments, rows, output offsets).  xsegs: the
+// X segments the frames come from (a job's utterances), or none (a chunk pass).
+void lay_out_frames(FrameLayout& l, const std::vector<int>& y_len, int hop, const std::vector<SegInfo>& xsegs) {
     const size_t B = y_len.size();
-    j.fsegs.resize(B);
+    l.fsegs.resize(B);
     int cur = 0; long long out = 0;
     for (size_t b = 0; b < B; b++) {
-        FrameSeg& f = j.fsegs[b];
+        FrameSeg& f = l.fsegs[b];
         f.off = cur; f.len = y_len[b];
-        f.xoff = b < j.xsegs.size() ? j.xsegs[b].off : 0;
-        f.xlen = b < j.xsegs.size() ? j.xsegs[b].len : 0;
+        f.xoff = b < xsegs.size() ? xsegs[b].off : 0;
+        f.xlen = b < xsegs.size() ? xsegs[b].len : 0;
         f.out_off = out;
         out += (long long)y_len[b] * hop;
         cur += round_up(y_len[b] + HY, GY);
     }
-    j.RY = cur; j.total_samples = out;
+    l.RY = cur; l.total_samples = out;
 }
 
 // The prosody launches of a job whose utterances ask for a pitch or a tempo (an empty plan when none does): every
@@ -740,8 +760,9 @@ ProsodyPlan lay_out_prosody(const Job& j, int hop) {
     ProsodyPlan p;
     if (j.pitch.empty() || j.encode_only) return p;
     for (size_t b = 0; b < j.B; b++) {
-        const long long n = (long long)j.fsegs[b].len * hop;
-        p.add(prosody_shape(j.v->sample_rate, n, j.pitch[b], j.tempo[b]), j.fsegs[b].out_off, n);
+        const FrameSeg& f = j.frames.fsegs[b];
+        const long long n = (long long)f.len * hop;
+        p.add(prosody_shape(j.v->sample_rate, n, j.pitch[b], j.tempo[b]), f.out_off, n);
     }
     return p;
 }
@@ -753,7 +774,7 @@ ResamplePlan lay_out_output(Job& j, int hop, const ProsodyPlan& pp) {
     ResamplePlan p;
     j.osr.assign(j.B, j.v->sample_rate);
     if (j.out_rates.empty() || j.encode_only) {
-        j.osegs = j.fsegs; j.out_hop = hop; j.out_total = j.total_samples;
+        j.osegs = j.frames.fsegs; j.out_hop = hop; j.out_total = j.frames.total_samples;
         if (!pp.segs.empty()) {
             for (size_t b = 0; b < j.B; b++) j.osegs[b] = FrameSeg{0, (int)pp.segs[b].n2, 0, 0, pp.segs[b].y_off};
             j.out_hop = 1; j.out_total = pp.y_total;
@@ -767,7 +788,7 @@ ResamplePlan lay_out_output(Job& j, int hop, const ProsodyPlan& pp) {
             j.osr[b] = j.out_rates[b];
             f = &voice_resampler(*j.v, j.out_rates[b], "utterance " + std::to_string(b) + ": ");
         }
-        p.add(f, pp.segs.empty() ? (long long)j.fsegs[b].len * hop : pp.segs[b].n2);
+        p.add(f, pp.segs.empty() ? (long long)j.frames.fsegs[b].len * hop : pp.segs[b].n2);
         j.osegs[b] = FrameSeg{0, (int)p.segs[b].n_out, 0, 0, p.segs[b].out_off};
     }
     j.out_hop = 1; j.out_total = p.total;
@@ -779,7 +800,7 @@ ResamplePlan lay_out_output(Job& j, int hop, const ProsodyPlan& pp) {
 void run_resample(Runner& R, const ResamplePlan& p, const ResampleTables& t, const float* wav, const FrameSeg* fsegs,
                   const PcmPost* posts, int hop, float* out) {
     R.begin("resample");
-    launch_resample(wav, fsegs, posts, hop, t.segs, (int)p.segs.size(), p.max_out, p.smem, out, R.st);
+    launch_resample(wav, fsegs, posts, hop, t.segs.d, (int)p.segs.size(), p.max_out, p.smem, out, R.st);
     R.count(p.flops, p.bytes);
     R.end();
 }
@@ -789,13 +810,13 @@ void run_resample(Runner& R, const ResamplePlan& p, const ResampleTables& t, con
 void run_prosody(Runner& R, const ProsodyPlan& p, const ProsodyBufs& t, const float* wav, float* y) {
     const int n = (int)p.segs.size();
     R.begin("stretch");
-    if (p.smem_ints) launch_prosody_offsets(wav, t.segs, n, p.smem_ints, t.offsets, R.st);
-    launch_prosody_ola(wav, t.segs, n, p.max_ola, t.offsets, t.s, y, R.st);
+    if (p.smem_ints) launch_prosody_offsets(wav, t.segs.d, n, p.smem_ints, t.offsets, R.st);
+    launch_prosody_ola(wav, t.segs.d, n, p.max_ola, t.offsets, t.s, y, R.st);
     R.count(p.stretch_flops, p.stretch_bytes, p.smem_ints ? 2 : 1);
     R.end();
     if (p.max_pitch == 0) return;
     R.begin("pitch");
-    launch_prosody_pitch(wav, t.s, t.segs, n, p.max_pitch, y, R.st);
+    launch_prosody_pitch(wav, t.s, t.segs.d, n, p.max_pitch, y, R.st);
     R.count(p.pitch_flops, p.pitch_bytes);
     R.end();
 }
@@ -828,32 +849,31 @@ void run_loudness(Runner& R, const LoudnessPlan& p, const LoudnessBufs& t, float
         if (!std::isnan(s.target)) scaled += (double)s.n;
     }
     R.begin("loudness");
-    launch_loudness(wav, t.segs, (int)n, t.scratch, t.lufs, t.gain, R.st);
+    launch_loudness(wav, t.segs.d, (int)n, t.scratch, t.lufs.d, t.gain.d, R.st);
     R.count(2.0 * 22.0 * samples, 4.0 * (samples + scaled));
     R.end();
-    SB_CUDA(cudaMemcpyAsync(t.lufs_h, t.lufs, n * sizeof(double), cudaMemcpyDeviceToHost, R.st));
-    SB_CUDA(cudaMemcpyAsync(t.gain_h, t.gain, n * sizeof(float), cudaMemcpyDeviceToHost, R.st));
+    t.lufs.download(R.st);
+    t.gain.download(R.st);
 }
 
-// Fills the frame-level tables through their pinned mirrors; returns the level.
-Level upload_frames(const Job& j, const FrameTables& t, cudaStream_t st) {
-    const size_t B = j.fsegs.size();
-    const int ntile = j.RY / GY;
-    Level L; L.map = {t.yend, GY, 1, j.RY}; L.valid_rows = 0; L.bias_slot = t.yslot;
+// Fills the frame-level tables of layout l through their pinned mirrors; returns the level.
+Level upload_frames(const FrameLayout& l, const FrameTables& t, cudaStream_t st) {
+    const size_t B = l.fsegs.size();
+    Level L; L.map = {t.yend.d, GY, 1, l.RY}; L.valid_rows = 0; L.bias_slot = t.yslot.d;
     for (size_t b = 0; b < B; b++) {
-        const int t0 = j.fsegs[b].off / GY;
-        const int t1 = (b + 1 < B ? j.fsegs[b + 1].off : j.RY) / GY;
+        const int t0 = l.fsegs[b].off / GY;
+        const int t1 = (b + 1 < B ? l.fsegs[b + 1].off : l.RY) / GY;
         for (int k = t0; k < t1; k++) {
-            t.yend_h[k] = j.fsegs[b].off + j.fsegs[b].len; t.ftile_h[k] = (int)b;
-            if (t.yslot_h) t.yslot_h[k] = j.slot_of[b];
+            t.yend.h[k] = l.fsegs[b].off + l.fsegs[b].len; t.ftile.h[k] = (int)b;
+            if (t.yslot.d) t.yslot.h[k] = l.slot_of[b];
         }
-        L.valid_rows += j.fsegs[b].len;
+        L.valid_rows += l.fsegs[b].len;
     }
-    memcpy(t.fsegs_h, j.fsegs.data(), B * sizeof(FrameSeg));
-    h2d(t.yend, t.yend_h, ntile * sizeof(int), st);
-    h2d(t.ftile, t.ftile_h, ntile * sizeof(int), st);
-    h2d(t.fsegs, t.fsegs_h, B * sizeof(FrameSeg), st);
-    if (t.yslot) h2d(t.yslot, t.yslot_h, ntile * sizeof(int), st);
+    std::copy(l.fsegs.begin(), l.fsegs.end(), t.fsegs.h);
+    t.yend.upload(st);
+    t.ftile.upload(st);
+    t.fsegs.upload(st);
+    if (t.yslot.d) t.yslot.upload(st);
     return L;
 }
 
@@ -896,89 +916,74 @@ void Job::run(float* d_out, size_t d_out_cap) {
     cudaStream_t st = C.stream;
     const int H = a.hidden, I = a.inter, F = a.filter;
     regions.clear(); dbg.clear(); dbg_level.clear(); id_frames.clear();
-    C.events_used = 0;
-    if (!C.ev_begin) { SB_CUDA(cudaEventCreate(&C.ev_begin)); SB_CUDA(cudaEventCreate(&C.ev_end)); }
 
     // ---------------- id level (phase 1) workspace ----------------
     // tensor-core attention (two grouped GEMMs around a softmax): default backend, 96- or 48-wide heads, rows that fit
     // the softmax kernel's registers; otherwise the fp32 CUDA-core attention kernel
     const int D = H / a.heads;
     const bool tc_att = V.backend == 1 && (D == 96 || D == 48) && max_tx <= 1280 && getenv("SB200_ATT_SIMT") == nullptr;
-    // speaker slots: one set of conditioned biases per distinct speaker of the batch, not per utterance
-    slot_of.assign(B, 0); slot_sid.clear();
-    if (V.num_speakers > 1) {
-        for (size_t b = 0; b < B; b++) {
-            const long long sid = cfgs[b].has_speaker ? cfgs[b].speaker : 0;   // piper/src/lib.rs:353-358: speaker.unwrap_or(0)
-            if (sid < 0 || sid >= V.emb_rows)
-                throw Error(19, "Failed to run model inference. Error: speaker id out of range (utterance " + std::to_string(b) + ")");
-            const auto it = std::find(slot_sid.begin(), slot_sid.end(), (int)sid);
-            slot_of[b] = (int)(it - slot_sid.begin());
-            if (it == slot_sid.end()) slot_sid.push_back((int)sid);
-        }
-    }
+    frames.slot_of.clear(); frames.slot_sid.clear();
+    for (size_t b = 0; b < B; b++)      // piper/src/lib.rs:353-358: speaker.unwrap_or(0)
+        if (!assign_slot(frames, V, cfgs[b].has_speaker ? cfgs[b].speaker : 0))
+            throw Error(19, "Failed to run model inference. Error: speaker id out of range (utterance " + std::to_string(b) + ")");
     IdBufs x;
     plan(C.dev_id, C.pin, [&](Arena& dev, Arena& pin) { x.carve(dev, pin, *this, tc_att); });
-    d_cum = x.cum; d_cond = x.cond;
-    Runner R(*this);
+    d_cum = x.cum;
+    Runner R(V, C, regions, x.spk.cond);
 
-    SB_CUDA(cudaEventRecord(C.ev_begin, st));
+    begin_pass(C);
     // tables
     const int nxg = RX / GX;
-    std::fill(x.ids_rows_h, x.ids_rows_h + RX, -1);
-    std::fill(x.xend_h, x.xend_h + nxg, 0);
-    std::fill(x.xseg_of_h, x.xseg_of_h + nxg, 0);
+    std::fill(x.ids_rows.h, x.ids_rows.h + RX, -1);
+    std::fill(x.xend.h, x.xend.h + nxg, 0);
+    std::fill(x.xseg_of_gran.h, x.xseg_of_gran.h + nxg, 0);
     for (size_t b = 0; b < B; b++) {
         const SegInfo& s = xsegs[b];
-        for (int i = 0; i < s.len; i++) x.ids_rows_h[s.off + i] = (int)ids[offs[b] + i];
+        for (int i = 0; i < s.len; i++) x.ids_rows.h[s.off + i] = (int)ids[offs[b] + i];
         const int g0 = s.off / GX, g1 = (b + 1 < B ? xsegs[b + 1].off : RX) / GX;
-        for (int g = g0; g < g1; g++) { x.xend_h[g] = s.off + s.len; x.xseg_of_h[g] = (int)b; }
-        x.scales_h[b] = cfgs[b].noise_w; x.scales_h[B + b] = cfgs[b].length_scale; x.scales_h[2 * B + b] = cfgs[b].noise_scale;
+        for (int g = g0; g < g1; g++) { x.xend.h[g] = s.off + s.len; x.xseg_of_gran.h[g] = (int)b; }
+        x.scales.h[b] = cfgs[b].noise_w; x.scales.h[B + b] = cfgs[b].length_scale; x.scales.h[2 * B + b] = cfgs[b].noise_scale;
     }
-    memcpy(x.xsegs_h, xsegs.data(), B * sizeof(SegInfo));
-    h2d(x.ids_rows, x.ids_rows_h, (size_t)RX * 4, st);
-    h2d(x.xend, x.xend_h, (size_t)nxg * 4, st);
-    h2d(x.xseg_of_gran, x.xseg_of_h, (size_t)nxg * 4, st);
-    h2d(x.xsegs, x.xsegs_h, B * sizeof(SegInfo), st);
-    h2d(x.scales, x.scales_h, 3 * B * sizeof(float), st);
-    if (x.xslot) {
-        for (int g = 0; g < nxg; g++) x.xslot_h[g] = slot_of[x.xseg_of_h[g]];
-        std::copy(slot_sid.begin(), slot_sid.end(), x.sid_h);
-        h2d(x.xslot, x.xslot_h, (size_t)nxg * 4, st);
-        h2d(x.sid, x.sid_h, slot_sid.size() * 4, st);
+    std::copy(xsegs.begin(), xsegs.end(), x.xsegs.h);
+    x.ids_rows.upload(st);
+    x.xend.upload(st);
+    x.xseg_of_gran.upload(st);
+    x.xsegs.upload(st);
+    x.scales.upload(st);
+    if (x.xslot.d) {
+        for (int g = 0; g < nxg; g++) x.xslot.h[g] = frames.slot_of[x.xseg_of_gran.h[g]];
+        x.xslot.upload(st);
     }
-    if (x.dscale || x.dframes) {
-        if (x.dscale) std::fill(x.dscale_h, x.dscale_h + RX, 1.f);
-        if (x.dframes) std::fill(x.dframes_h, x.dframes_h + RX, -1);
-        for (size_t b = 0; b < B; b++) {
-            const int r0 = xsegs[b].off;
-            if (x.dscale) std::copy(dur_scale.begin() + offs[b], dur_scale.begin() + offs[b + 1], x.dscale_h + r0);
-            if (x.dframes) std::copy(dur_frames.begin() + offs[b], dur_frames.begin() + offs[b + 1], x.dframes_h + r0);
-        }
-        if (x.dscale) h2d(x.dscale, x.dscale_h, (size_t)RX * 4, st);
-        if (x.dframes) h2d(x.dframes, x.dframes_h, (size_t)RX * 4, st);
-    }
-    if (x.seeds) {
-        std::copy(seeds.begin(), seeds.end(), x.seeds_h);
-        h2d(x.seeds, x.seeds_h, B * sizeof(NoiseSeed), st);
+    // per-id duration controls: each id's value on its X row, `none` on the gap rows
+    auto per_id = [&](const auto& t, const auto& vals, auto none) {
+        if (!t.d) return;
+        std::fill(t.h, t.h + RX, none);
+        for (size_t b = 0; b < B; b++) std::copy(vals.begin() + offs[b], vals.begin() + offs[b + 1], t.h + xsegs[b].off);
+        t.upload(st);
+    };
+    per_id(x.dscale, dur_scale, 1.f);
+    per_id(x.dframes, dur_frames, -1);
+    if (x.seeds.d) {
+        std::copy(seeds.begin(), seeds.end(), x.seeds.h);
+        x.seeds.upload(st);
     }
     if (tc_att) {
-        memcpy(x.tiles_h, tiles_s.data(), tiles_s.size() * sizeof(TfTile));
-        memcpy(x.tiles_h + tiles_s.size(), tiles_o.data(), tiles_o.size() * sizeof(TfTile));
-        h2d(x.tiles, x.tiles_h, (tiles_s.size() + tiles_o.size()) * sizeof(TfTile), st);
+        std::copy(tiles_o.begin(), tiles_o.end(), std::copy(tiles_s.begin(), tiles_s.end(), x.tiles.h));
+        x.tiles.upload(st);
     }
 
-    Level LX; LX.map = {x.xend, GX, 1, RX}; LX.valid_rows = (long long)ids.size(); LX.bias_slot = x.xslot;
+    Level LX; LX.map = {x.xend.d, GX, 1, RX}; LX.valid_rows = (long long)ids.size(); LX.bias_slot = x.xslot.d;
     TfGemm gs{}, go{};
     bool tc_att_ok = tc_att;
     if (tc_att) {
         gs.a = x.qkv; gs.a_rows = RX; gs.a_cols = 3 * H; gs.lda = 3 * H;
         gs.b = x.qkv; gs.b_rows = RX; gs.b_cols = 3 * H; gs.ldb = 3 * H;
         gs.nth = att_nth_s; gs.y = x.att_s; gs.ldy = att_tp; gs.res = nullptr; gs.scale = 1.0f / sqrtf((float)(H / a.heads));
-        gs.tiles = x.tiles; gs.ntiles = (int)tiles_s.size();
+        gs.tiles = x.tiles.d; gs.ntiles = (int)tiles_s.size();
         go.a = x.att_s; go.a_rows = a.heads * RX; go.a_cols = att_tp; go.lda = att_tp;
         go.b = x.att_vt; go.b_rows = H; go.b_cols = RX; go.ldb = RX;
         go.nth = att_nth_o; go.y = x.att; go.ldy = H; go.res = x.att_orel; go.scale = 1.f;
-        go.tiles = x.tiles + tiles_s.size(); go.ntiles = (int)tiles_o.size();
+        go.tiles = x.tiles.d + tiles_s.size(); go.ntiles = (int)tiles_o.size();
         tc_att_ok = gemm_tf_supported(gs) && gemm_tf_supported(go);
     }
     if (debug) {
@@ -1012,8 +1017,9 @@ void Job::run(float* d_out, size_t d_out_cap) {
                 if (!eps_w[b].empty()) memcpy(stage.data() + (size_t)xsegs[b].off * 2, eps_w[b].data(), eps_w[b].size() * 4);
             SB_CUDA(cudaMemcpyAsync(x.epsw, stage.data(), stage.size() * 4, cudaMemcpyHostToDevice, st));
             SB_CUDA(cudaStreamSynchronize(st));   // `stage` is pageable; injection is a test-only path
-        } else if (x.seeds) {
-            launch_randn_seeded(x.epsw, 2, 0, V.noise_seed, 2 * noise_call, x.seeds, x.xsegs, x.xseg_of_gran, LX.map, st);
+        } else if (x.seeds.d) {
+            launch_randn_seeded(x.epsw, 2, 0, V.noise_seed, 2 * noise_call, x.seeds.d, x.xsegs.d, x.xseg_of_gran.d, LX.map,
+                                st);
         } else {
             launch_randn(x.epsw, (long long)RX * 2, V.noise_seed, 2 * noise_call, st);
         }
@@ -1021,14 +1027,14 @@ void Job::run(float* d_out, size_t d_out_cap) {
     }
 
     // ---------------- speaker conditioning (multi-speaker voices) ----------------
-    if (x.cond) launch_cond_bias(V.cond_w, V.cond_base, V.emb_g, x.sid, (int)slot_sid.size(), V.cond_rows, V.gin, x.cond, st);
+    x.spk.run(V, frames, st);
 
     // ---------------- text encoder ----------------
     // Every contraction here reaches the duration predictor, and ceil(duration) is a cliff: the dense layers and the two
     // attention contractions run on conv_tf.cu (wgmma, error-compensated tf32, chunk-flushed accumulation: fp32-class
     // accuracy, DESIGN.md section 4); backend 0 / 2 keep them on the fp32 CUDA-core kernels.
     R.begin("enc");
-    launch_embed(x.ids_rows, V.emb, sqrtf((float)H), x.xa, RX, H, st);
+    launch_embed(x.ids_rows.d, V.emb, sqrtf((float)H), x.xa, RX, H, st);
     R.count(0, 4.0 * LX.valid_rows * H);
     // debug: every stage is copied right after its launch (xa and xb are overwritten in place)
     if (debug) d2d(x.emb0, x.xa, (size_t)RX * H, st);
@@ -1047,11 +1053,11 @@ void Job::run(float* d_out, size_t d_out_cap) {
         if (tc_att_ok) {
             launch_gemm_tf(gs, st);
             launch_attn_softmax(x.att_s, att_tp, x.qkv, 3 * H, e.relk, e.relv, a.window, x.att_orel, H, H, a.heads, RX,
-                                x.xsegs, x.xseg_of_gran, GX, max_tx, st);
+                                x.xsegs.d, x.xseg_of_gran.d, GX, max_tx, st);
             launch_gemm_tf(go, st);
             R.count(0, 0, 2);
         } else {
-            launch_attention(x.qkv, 3 * H, e.relk, e.relv, a.window, x.att, H, H, a.heads, x.xsegs, (int)B, max_tx, st);
+            launch_attention(x.qkv, 3 * H, e.relk, e.relv, a.window, x.att, H, H, a.heads, x.xsegs.d, (int)B, max_tx, st);
         }
         { double f = 0; for (auto& s : xsegs) f += 4.0 * (double)s.len * s.len * H; R.count(f, 16.0 * LX.valid_rows * H); }
         if (debug && l == 0) {      // first-layer attention operands / result (tests/test_gpu_parity.py)
@@ -1085,7 +1091,7 @@ void Job::run(float* d_out, size_t d_out_cap) {
     { ConvCall o; o.y0 = x.d0; o.ldy0 = H; R.conv(V.dp_pre, x.xa, H, LX, o); }
     R.dds(V.dp_dds, x.d0, x.t1, x.t2, LX);
     { ConvCall o; o.y0 = x.g; o.ldy0 = H; R.conv(V.dp_proj, x.d0, H, LX, o); }
-    launch_scale_copy2(x.epsw, x.scales, x.xseg_of_gran, x.zz, LX.map, st);
+    launch_scale_copy2(x.epsw, x.scales.d, x.xseg_of_gran.d, x.zz, LX.map, st);
     // debug: zz, d0 and h29 are reused by every flow, so each flow's stages are captured as copies
     for (size_t s = 0; s < V.dp_flows.size(); s++) {
         const CFlowW& cf = V.dp_flows[s];
@@ -1100,14 +1106,14 @@ void Job::run(float* d_out, size_t d_out_cap) {
         R.count(0, 4.0 * LX.valid_rows * 34);
         if (debug) d2d(x.dpf[s][3], x.zz, (size_t)RX * 2, st);
     }
-    launch_durations(x.zz, V.ea_m0, V.ea_logs0, x.scales + B, x.xsegs, (int)B, x.logw, x.cum, x.ylen, st, x.dscale,
-                     x.dframes);
+    launch_durations(x.zz, V.ea_m0, V.ea_logs0, x.scales.d + B, x.xsegs.d, (int)B, x.logw, x.cum, x.ylen.d, st,
+                     x.dscale.d, x.dframes.d);
     R.end();
 
     // ---------------- host learns the frame counts (the graph's data-dependent shape) ----------------
-    SB_CUDA(cudaMemcpyAsync(x.ylen_h, x.ylen, B * sizeof(int), cudaMemcpyDeviceToHost, st));
+    x.ylen.download(st);
     SB_CUDA(cudaStreamSynchronize(st));
-    y_len.assign(x.ylen_h, x.ylen_h + B);
+    y_len.assign(x.ylen.h, x.ylen.h + B);
     long long tot_frames = 0;
     for (int y : y_len) tot_frames += y;
     if (tot_frames > (long long)(2.0e9 / 256 / 4)) throw Error(19, "Failed to run model inference. Error: predicted durations are unreasonably long");
@@ -1118,7 +1124,7 @@ void Job::run(float* d_out, size_t d_out_cap) {
 
     // ---------------- frame level (phase 2) workspace ----------------
     // The stream is idle here, so the pinned staging of the X tables can be reused for the Y tables.
-    lay_out_frames(*this, y_len, a.hop());
+    lay_out_frames(frames, y_len, a.hop(), xsegs);
     const ProsodyPlan pp = lay_out_prosody(*this, a.hop());
     const bool prosody = !pp.segs.empty();
     const ResamplePlan rp = lay_out_output(*this, a.hop(), pp);
@@ -1127,8 +1133,7 @@ void Job::run(float* d_out, size_t d_out_cap) {
     loud_ran.clear(); loud_lufs.clear(); loud_gain.clear(); pros_ran.clear();
     FrameBufs f;
     plan(C.dev_frame, C.pin, [&](Arena& dev, Arena& pin) { f.carve(dev, pin, *this, pp, rp, lp, d_out == nullptr); });
-    d_fsegs = f.y.fsegs;
-    d_osegs = resample ? f.rt.osegs : prosody ? f.pr.osegs : d_fsegs;
+    d_osegs = resample ? f.rt.osegs.d : prosody ? f.pr.osegs.d : f.y.fsegs.d;
     if (debug) {
         expose(*this, "z_p", f.zp, I, 1); expose(*this, "z", f.s, I, 1);
         // flow.{f}: z after the coupling layer of the graph's flow.flows.{2f} (f = flow_n - 1 first).  The graph's Flip
@@ -1137,31 +1142,33 @@ void Job::run(float* d_out, size_t d_out_cap) {
         for (size_t s = 0; s < f.flow.size(); s++) expose(*this, "flow." + std::to_string(a.flow_n - 1 - (int)s), f.flow[s], I, 1);
         if (!encode_only) f.dec.expose_to(*this);
     }
-    Level LY = upload_frames(*this, f.y, st);
+    Level LY = upload_frames(frames, f.y, st);
     if (prosody) f.pr.upload(pp, st);
     if (resample) f.rt.upload(rp, st);
     if (!lp.segs.empty()) {
-        std::copy(lp.segs.begin(), lp.segs.end(), f.ld.segs_h);
-        h2d(f.ld.segs, f.ld.segs_h, lp.segs.size() * sizeof(LoudSeg), st);
+        std::copy(lp.segs.begin(), lp.segs.end(), f.ld.segs.h);
+        f.ld.segs.upload(st);
     }
 
     // ---------------- alignment expansion ----------------
     R.begin("align");
+    const int RY = frames.RY;
     if (f.epsz) {
         if (!eps_z.empty()) {
             std::vector<float> stage((size_t)RY * I, 0.f);
             for (size_t b = 0; b < B; b++)
-                if (!eps_z[b].empty()) memcpy(stage.data() + (size_t)fsegs[b].off * I, eps_z[b].data(), eps_z[b].size() * 4);
+                if (!eps_z[b].empty()) memcpy(stage.data() + (size_t)frames.fsegs[b].off * I, eps_z[b].data(), eps_z[b].size() * 4);
             SB_CUDA(cudaMemcpyAsync(f.epsz, stage.data(), stage.size() * 4, cudaMemcpyHostToDevice, st));
             SB_CUDA(cudaStreamSynchronize(st));
-        } else if (x.seeds) {
-            launch_randn_seeded(f.epsz, I, 1, V.noise_seed, 2 * noise_call + 1, x.seeds, f.y.fsegs, f.y.ftile, LY.map, st);
+        } else if (x.seeds.d) {
+            launch_randn_seeded(f.epsz, I, 1, V.noise_seed, 2 * noise_call + 1, x.seeds.d, f.y.fsegs.d, f.y.ftile.d, LY.map,
+                                st);
         } else {
             launch_randn(f.epsz, (long long)RY * I, V.noise_seed, 2 * noise_call + 1, st);
         }
         if (debug) expose(*this, "eps_z", f.epsz, I, 1);
     }
-    launch_expand(x.stats, 2 * I, I, x.cum, f.epsz, x.scales + 2 * B, f.s, f.y.fsegs, f.y.ftile, LY.map, st);
+    launch_expand(x.stats, 2 * I, I, x.cum, f.epsz, x.scales.d + 2 * B, f.s, f.y.fsegs.d, f.y.ftile.d, LY.map, st);
     R.count(0, 4.0 * LY.valid_rows * 3 * I);
     R.end();
     if (debug) d2d(f.zp, f.s, (size_t)RY * I, st);
@@ -1202,13 +1209,13 @@ void Job::run(float* d_out, size_t d_out_cap) {
     }
     run_decoder(R, LY, f.y, f.dec, f.s, resample || prosody ? f.wav : d_wav);
     // the output stage: prosody on the decoder's waveform, the resample launch on what that left, loudness on the result
-    const float* staged = f.wav; const FrameSeg* staged_segs = f.y.fsegs; int staged_hop = a.hop();
+    const float* staged = f.wav; const FrameSeg* staged_segs = f.y.fsegs.d; int staged_hop = a.hop();
     if (prosody) {
         float* py = resample ? f.pr.y : d_wav;
         run_prosody(R, pp, f.pr, f.wav, py);
-        staged = py; staged_segs = f.pr.osegs; staged_hop = 1;
+        staged = py; staged_segs = f.pr.osegs.d; staged_hop = 1;
     }
-    if (resample) run_resample(R, rp, f.rt, staged, staged_segs, f.rt.posts, staged_hop, d_wav);
+    if (resample) run_resample(R, rp, f.rt, staged, staged_segs, f.rt.posts.d, staged_hop, d_wav);
     if (!lp.segs.empty()) run_loudness(R, lp, f.ld, d_wav);
     SB_CUDA(cudaEventRecord(C.ev_end, st));
     SB_CUDA(cudaStreamSynchronize(st));
@@ -1218,8 +1225,8 @@ void Job::run(float* d_out, size_t d_out_cap) {
     pros_ran = pp.shapes;
     if (!lp.segs.empty()) {
         loud_ran = loud_target;
-        loud_lufs.assign(f.ld.lufs_h, f.ld.lufs_h + B);
-        loud_gain.assign(f.ld.gain_h, f.ld.gain_h + B);
+        loud_lufs.assign(f.ld.lufs.h, f.ld.lufs.h + B);
+        loud_gain.assign(f.ld.gain.h, f.ld.gain.h + B);
     }
     ran = true;
 }
@@ -1248,7 +1255,7 @@ std::vector<Latent*> encode_latents(Voice* v, const long long* ids, const size_t
         Latent& L = *(ls[b] = std::unique_ptr<Latent>(new Latent()));
         L.v = v; L.mem = mem; L.z = p + row * I; L.frames = j->y_len[b];
         L.sid = j->cfgs[b].has_speaker ? j->cfgs[b].speaker : 0;
-        SB_CUDA(cudaMemcpyAsync(L.z, j->z_dev + (size_t)j->fsegs[b].off * I, (size_t)L.frames * I * 4,
+        SB_CUDA(cudaMemcpyAsync(L.z, j->z_dev + (size_t)j->frames.fsegs[b].off * I, (size_t)L.frames * I * 4,
                                 cudaMemcpyDeviceToDevice, j->ctx->stream));
         row += (size_t)L.frames;
     }
@@ -1288,9 +1295,8 @@ void decode_chunks(Voice* v, const ChunkPass& p, ChunkResult& out) {
     if (p.format < PCM_F32 || p.format > PCM_ALAW)
         throw Error(19, "format " + std::to_string(p.format) + " is not 0 (f32), 1 (i16), 2 (mu-law) or 3 (A-law)");
     const int hop = v->a.hop();
-    Job j;
+    FrameLayout l;
     std::vector<int> len(n);
-    j.slot_of.assign(n, 0);
     auto fail = [&p](size_t k, const std::string& what, const std::string& detail) {
         throw Error(19, p.single ? what : "chunk " + std::to_string(k) + ": " + what + detail);
     };
@@ -1302,14 +1308,8 @@ void decode_chunks(Voice* v, const ChunkPass& p, ChunkResult& out) {
                                                   ") of a latent of " + std::to_string(c.z->frames) + ")");
         if (c.trim_lo < 0 || c.trim_hi < 0 || c.trim_lo + c.trim_hi >= c.hi - c.lo)
             fail(k, "Invalid model audio output", " (trim)");
-        // decoder.onnx takes the encoder's `g` (piper/src/lib.rs:706-735, 739-743): one speaker slot per distinct sid
-        if (v->num_speakers > 1) {
-            const long long sid = c.z->sid;
-            if (sid < 0 || sid >= v->emb_rows) fail(k, "Failed to run model inference. Error: speaker id out of range", "");
-            const auto it = std::find(j.slot_sid.begin(), j.slot_sid.end(), (int)sid);
-            j.slot_of[k] = (int)(it - j.slot_sid.begin());
-            if (it == j.slot_sid.end()) j.slot_sid.push_back((int)sid);
-        }
+        // decoder.onnx takes the encoder's `g` (piper/src/lib.rs:706-735, 739-743)
+        if (!assign_slot(l, *v, c.z->sid)) fail(k, "Failed to run model inference. Error: speaker id out of range", "");
         len[k] = (int)(c.hi - c.lo);
         if (const Resampler* r = c.rs) {
             if (r->v != v) fail(k, "the resampler was made for another voice", "");
@@ -1347,28 +1347,23 @@ void decode_chunks(Voice* v, const ChunkPass& p, ChunkResult& out) {
         if (p.resample) rp.add(c.rs ? &c.rs->f : nullptr, n_res[k], c.rs, c.last != 0);
     }
 
-    j.v = v; j.B = n; j.ctx = v->acquire();
-    Context& C = *j.ctx;
+    const auto release = [v](Context* c) { v->release(c); };
+    const std::unique_ptr<Context, decltype(release)> ctx(v->acquire(), release);
+    Context& C = *ctx;
     SB_CUDA(cudaSetDevice(v->device));
-    lay_out_frames(j, len, hop);
-    const size_t total = p.resample ? (size_t)rp.total : (size_t)j.total_samples;
+    lay_out_frames(l, len, hop, {});
+    const size_t total = p.resample ? (size_t)rp.total : (size_t)l.total_samples;
     ChunkBufs b;
-    plan(C.dev_frame, C.pin, [&](Arena& dev, Arena& pin) { b.carve(dev, pin, j, p, rp, pp, total); });
-    j.d_cond = b.cond; j.d_fsegs = b.y.fsegs; j.d_wav = b.wav;
-    C.events_used = 0;
-    if (!C.ev_begin) { SB_CUDA(cudaEventCreate(&C.ev_begin)); SB_CUDA(cudaEventCreate(&C.ev_end)); }
+    plan(C.dev_frame, C.pin, [&](Arena& dev, Arena& pin) { b.carve(dev, pin, *v, l, p, rp, pp, total); });
     cudaStream_t st = C.stream;
-    Runner R(j);
-    SB_CUDA(cudaEventRecord(C.ev_begin, st));
-    if (b.cond) {
-        std::copy(j.slot_sid.begin(), j.slot_sid.end(), b.sid_h);
-        h2d(b.sid, b.sid_h, j.slot_sid.size() * sizeof(int), st);
-        launch_cond_bias(v->cond_w, v->cond_base, v->emb_g, b.sid, (int)j.slot_sid.size(), v->cond_rows, v->gin, b.cond, st);
-    }
-    Level LY = upload_frames(j, b.y, st);
-    for (size_t k = 0; k < n; k++) b.src_h[k] = GatherSeg{p.chunks[k].z->z, p.chunks[k].lo, j.fsegs[k].off, len[k]};
-    h2d(b.src, b.src_h, n * sizeof(GatherSeg), st);
-    launch_gather_rows(b.src, b.y.ftile, GY, j.RY, v->a.inter, b.s, st);
+    std::vector<Region> regions;
+    Runner R(*v, C, regions, b.spk.cond);
+    begin_pass(C);
+    b.spk.run(*v, l, st);
+    Level LY = upload_frames(l, b.y, st);
+    for (size_t k = 0; k < n; k++) b.src.h[k] = GatherSeg{p.chunks[k].z->z, p.chunks[k].lo, l.fsegs[k].off, len[k]};
+    b.src.upload(st);
+    launch_gather_rows(b.src.d, b.y.ftile.d, GY, l.RY, v->a.inter, b.s, st);
     run_decoder(R, LY, b.y, b.dec, b.s, b.wav);
     // G.711 of resampled chunks: the gain scales the resampled samples just before the conversion, as a volume on the
     // delivered audio (resampling x * g is not bit for bit resampling x, then times g)
@@ -1376,57 +1371,56 @@ void decode_chunks(Voice* v, const ChunkPass& p, ChunkResult& out) {
     std::vector<float> out_gain;
     if (gain_after)
         for (const ChunkSpec& c : p.chunks) out_gain.push_back(c.gain);
-    if (b.post) {
+    if (b.post.d) {
         for (size_t k = 0; k < n; k++) {
-            PcmPost& q = b.post_h[k];
+            PcmPost& q = b.post.h[k];
             q = PcmPost();
             q.gain = gain_after ? 1.f : p.chunks[k].gain;
             q.trim_lo = p.chunks[k].trim_lo * hop;
             q.trim_hi = p.chunks[k].trim_hi * hop;
             if (p.fade > 0) fill_fade(q, p.fade, n_in[k]);
         }
-        h2d(b.post, b.post_h, n * sizeof(PcmPost), st);
+        b.post.upload(st);
     }
     // warped chunks: prosody on the post-path's samples, then the resample launch reads its output (n samples at
     // `off` as a segment of ceil(n / hop) frames less a trim, with no post-path of its own)
-    const FrameSeg* rs_in = b.y.fsegs; const PcmPost* rs_post = b.post;
+    const FrameSeg* rs_in = b.y.fsegs.d; const PcmPost* rs_post = b.post.d;
     if (!warped.empty()) {
-        float* py = b.wav + j.total_samples;
-        for (size_t q = 0; q < warped.size(); q++) {
-            b.pseg_h[q] = pp.segs[q];
-            b.pcar_h[q] = prosody_carry(*p.chunks[warped[q]].ps, steps[warped[q]], warped[q]);
-        }
-        h2d(b.pseg, b.pseg_h, warped.size() * sizeof(ProsodySeg), st);
-        h2d(b.pcar, b.pcar_h, warped.size() * sizeof(ProsodyCarry), st);
+        float* py = b.wav + l.total_samples;
+        b.pr.upload(pp, st);
+        for (size_t q = 0; q < warped.size(); q++)
+            b.pr.carry.h[q] = prosody_carry(*p.chunks[warped[q]].ps, steps[warped[q]], warped[q]);
+        b.pr.carry.upload(st);
         R.begin("stretch");
-        launch_prosody_stream_stretch(pp, b.pseg, b.pcar, b.wav, b.y.fsegs, b.post, hop, b.px, b.ps, b.poff, py, st);
+        launch_prosody_stream_stretch(pp, b.pr.segs.d, b.pr.carry.d, b.wav, b.y.fsegs.d, b.post.d, hop, b.pr.x, b.pr.s,
+                                      b.pr.offsets, py, st);
         R.count(pp.stretch_flops, pp.stretch_bytes, 2 + (pp.smem_ints ? 1 : 0) + (pp.max_ola ? 1 : 0));
         R.end();
         if (pp.max_pitch) {
             R.begin("pitch");
-            launch_prosody_pitch(b.px, b.ps, b.pseg, (int)warped.size(), pp.max_pitch, py, st);
+            launch_prosody_pitch(b.pr.x, b.pr.s, b.pr.segs.d, (int)warped.size(), pp.max_pitch, py, st);
             R.count(pp.pitch_flops, pp.pitch_bytes);
             R.end();
         }
-        std::copy(j.fsegs.begin(), j.fsegs.end(), b.rin_h);
-        std::copy(b.post_h, b.post_h + n, b.rpost_h);
+        std::copy(l.fsegs.begin(), l.fsegs.end(), b.rin.h);
+        std::copy(b.post.h, b.post.h + n, b.rpost.h);
         for (size_t q = 0; q < warped.size(); q++) {
             const ProsodySeg& g = pp.segs[q];
             const long long m = g.j1 - g.j0, frames = (m + hop - 1) / hop;
-            b.rin_h[warped[q]] = FrameSeg{0, (int)frames, 0, 0, j.total_samples + g.y_off};
-            b.rpost_h[warped[q]] = PcmPost();
-            b.rpost_h[warped[q]].trim_hi = frames * hop - m;
+            b.rin.h[warped[q]] = FrameSeg{0, (int)frames, 0, 0, l.total_samples + g.y_off};
+            b.rpost.h[warped[q]] = PcmPost();
+            b.rpost.h[warped[q]].trim_hi = frames * hop - m;
         }
-        h2d(b.rin, b.rin_h, n * sizeof(FrameSeg), st);
-        h2d(b.rpost, b.rpost_h, n * sizeof(PcmPost), st);
-        rs_in = b.rin; rs_post = b.rpost;
+        b.rin.upload(st);
+        b.rpost.upload(st);
+        rs_in = b.rin.d; rs_post = b.rpost.d;
     }
     if (p.resample) {
         b.rt.upload(rp, st, gain_after ? &out_gain : nullptr);
         run_resample(R, rp, b.rt, b.wav, rs_in, rs_post, hop, b.rs);
-        if (b.pcm) launch_pcm(b.rs, b.rt.osegs, b.rt.posts, (int)n, 1, rp.max_out, b.max, p.format, b.pcm, st);
+        if (b.pcm) launch_pcm(b.rs, b.rt.osegs.d, b.rt.posts.d, (int)n, 1, rp.max_out, b.max, p.format, b.pcm, st);
     } else if (b.pcm) {
-        launch_pcm(b.wav, b.y.fsegs, b.post, (int)n, hop, (long long)*std::max_element(len.begin(), len.end()) * hop,
+        launch_pcm(b.wav, b.y.fsegs.d, b.post.d, (int)n, hop, (long long)*std::max_element(len.begin(), len.end()) * hop,
                    b.max, p.format, b.pcm, st);
     }
     SB_CUDA(cudaEventRecord(C.ev_end, st));
@@ -1445,7 +1439,7 @@ void decode_chunks(Voice* v, const ChunkPass& p, ChunkResult& out) {
         r->h = s.h_out;
         r->ended = p.chunks[k].last != 0;
     }
-    for (Region& g : j.regions) {
+    for (Region& g : regions) {
         if (g.name != "stretch" && g.name != "pitch") continue;
         cudaEventElapsedTime(&g.ms, g.e0, g.e1);
         (g.name == "stretch" ? out.stretch_ms : out.pitch_ms) = g.ms;
@@ -1457,7 +1451,7 @@ void decode_chunks(Voice* v, const ChunkPass& p, ChunkResult& out) {
     }
     if (p.format == PCM_I16) out.i16.resize(n); else if (b.pcm) out.g711.resize(n); else out.f32.resize(n);
     for (size_t k = 0; k < n; k++) {
-        const long long o = p.resample ? rp.segs[k].out_off : j.fsegs[k].out_off;
+        const long long o = p.resample ? rp.segs[k].out_off : l.fsegs[k].out_off;
         const long long m = p.resample ? rp.segs[k].n_out : n_in[k];
         if (p.format == PCM_I16) {
             const int16_t* h = static_cast<const int16_t*>(b.out_h);

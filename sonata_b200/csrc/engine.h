@@ -54,7 +54,7 @@ struct ConvW {
     float* wtf = nullptr;                    // tf32 hi/lo images (conv_tf.cu): text-encoder / duration-predictor layers
     int cin = 0, cout = 0, ldw = 0, ntaps = 0;
     int macs = 0;                            // multiply-adds per output row (profile counters)
-    int cond_off = -1;                       // multi-speaker voices: offset of this conv's per-call effective bias (Job::d_cond)
+    int cond_off = -1;                       // multi-speaker voices: offset of this conv's per-call effective bias (Runner::cond)
     int tap_off[SB_MAX_TAPS] = {0};
     int min_off = 0, span = 0;
 };
@@ -283,12 +283,19 @@ struct Level {          // one time resolution of the packed batch
     const int* bias_slot = nullptr;   // speaker slot of every granule (multi-speaker voices), for the conditioned convs
 };
 
+// The frame level of a pass, one segment per utterance (a job) or chunk (a chunk pass), and its speaker slots.
+struct FrameLayout {
+    std::vector<FrameSeg> fsegs;
+    int RY = 0;
+    long long total_samples = 0;
+    std::vector<int> slot_of;         // per segment: its speaker slot (index into slot_sid; 0 on single-speaker voices)
+    std::vector<int> slot_sid;        // per slot: the speaker id, distinct, in order of first use (empty: one speaker)
+};
+
 struct Job {
     Voice* v = nullptr;
     Context* ctx = nullptr;
     std::vector<SynthConfig> cfgs;    // one per utterance: the voice's fallback config unless set_job_configs changed it
-    std::vector<int> slot_of;         // per utterance: its speaker slot (index into slot_sid)
-    std::vector<int> slot_sid;        // per slot: the speaker id, distinct, in order of first use
     size_t B = 0;
     bool debug = false;
     bool encode_only = false;     // stop after the flow (streaming 'encoder.onnx' half)
@@ -314,15 +321,13 @@ struct Job {
     // X layout
     int RX = 0; std::vector<SegInfo> xsegs; int max_tx = 0;
     // Y layout
-    int RY = 0; std::vector<FrameSeg> fsegs; std::vector<int> y_len;
-    long long total_samples = 0;
+    FrameLayout frames; std::vector<int> y_len;
     // tensor-core attention (conv_tf.cu grouped GEMMs): tile tables built with the X layout, same for every layer
     std::vector<TfTile> tiles_s, tiles_o;      // Q.K^T tiles, P.V tiles
     int att_tp = 0;                            // key columns of a score row (multiple of 96)
     int att_nth_s = 64, att_nth_o = 96;   // column tiles of the two attention GEMMs (narrower when the job is small)
     // device results read after the pass (context arenas)
     int* d_cum = nullptr;
-    FrameSeg* d_fsegs = nullptr;
     float* d_wav = nullptr;
     // What the job hands out: utterance b is d_wav[osegs[b].out_off ..) of osegs[b].len * out_hop samples, and
     // d_osegs mirrors osegs on the device.  Without prosody or output rates these are fsegs, the hop and total_samples;
@@ -330,7 +335,6 @@ struct Job {
     std::vector<FrameSeg> osegs; int out_hop = 1; long long out_total = 0;
     std::vector<int> osr;             // sample rate of each handed-out utterance
     FrameSeg* d_osegs = nullptr;
-    float* d_cond = nullptr;       // effective biases of the speaker-conditioned convs for this call, [slot][cond_rows]
     std::map<std::string, std::pair<float*, int>> dbg;   // name -> (device ptr, cols)
     std::map<std::string, int> dbg_level;                // name -> U (rows per frame), 0 for X level, -1 for an X-level
                                                          // buffer stored transposed ([cols][RX])

@@ -191,13 +191,14 @@ std::vector<std::vector<float>> speak_sentences_f32(Voice* v, const std::vector<
     std::unique_ptr<Job> j(create_job(v, ids.data(), offs.data(), ph.size(), nullptr, nullptr, nullptr, false));
     j->run(nullptr, 0);
     Context& C = *j->ctx;
-    C.pin.reserve((size_t)j->total_samples * 4);
-    float* all = C.pin.get<float>((size_t)j->total_samples);
-    SB_CUDA(cudaMemcpyAsync(all, j->d_wav, (size_t)j->total_samples * 4, cudaMemcpyDeviceToHost, C.stream));
+    const FrameLayout& l = j->frames;
+    C.pin.reserve((size_t)l.total_samples * 4);
+    float* all = C.pin.get<float>((size_t)l.total_samples);
+    SB_CUDA(cudaMemcpyAsync(all, j->d_wav, (size_t)l.total_samples * 4, cudaMemcpyDeviceToHost, C.stream));
     SB_CUDA(cudaStreamSynchronize(C.stream));
     std::vector<std::vector<float>> out;
     for (size_t b = 0; b < ph.size(); b++)
-        out.emplace_back(all + j->fsegs[b].out_off, all + j->fsegs[b].out_off + (size_t)j->y_len[b] * v->a.hop());
+        out.emplace_back(all + l.fsegs[b].out_off, all + l.fsegs[b].out_off + (size_t)j->y_len[b] * v->a.hop());
     return out;
 }
 
