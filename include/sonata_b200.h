@@ -509,6 +509,19 @@ int32_t sb200_debug_conv_ex(int32_t device, int32_t backend, const float* x, int
                             const float* bias, int32_t cout, int32_t k, int32_t dil, float in_slope, int32_t act,
                             const float* res, float scale, const int32_t* seg_end, int32_t gran, int32_t seg_mul,
                             float* y0, int32_t acc0, int32_t split, float* y1, int32_t acc1, sb200_error* err);
+/* A whole 64-channel HiFi-GAN ResBlock2 stage through its fused kernel (backend 1), for kernel unit tests:
+ * y[rows][64] = (1/nbr) sum_b (x1_b + conv_{ks[b], dils[2b+1]}(lrelu_0.1(x1_b)) + bias),
+ * x1_b = x + conv_{ks[b], dils[2b]}(lrelu_0.1(x)) + bias, each conv as sb200_debug_conv_ex runs it with that residual and
+ * scale (1 / nbr on the second conv, which accumulates from the second branch on).  w holds the 2 nbr weights
+ * [64][64][ks[b]] back to back in the order (branch, conv), bias the 2 nbr biases [64].  Row validity as in
+ * sb200_debug_conv_ex; invalid rows come out 0.  Honours sb200_debug_conv_grid_cap. */
+int32_t sb200_debug_resblock2_stage(int32_t device, const float* x, int32_t rows, int32_t nbr, const int32_t* ks,
+                                    const int32_t* dils, const float* w, const float* bias, const int32_t* seg_end,
+                                    int32_t gran, int32_t seg_mul, float* y, sb200_error* err);
+/* Test hook: the fused ResBlock2 stage kernel's plan for such a stage over `rows` rows -- nothing is allocated or
+ * launched.  out8 = {tile rows, x window rows, x1 rows, weight ring slots, dynamic shared memory bytes, grid CTAs,
+ * threads per CTA, registers per CTA}.  Returns 0, or 19 if the kernel does not take the stage. */
+int32_t sb200_debug_resblock2_plan(int64_t rows, int32_t nbr, const int32_t* ks, const int32_t* dils, int32_t* out8);
 /* The duration predictor's spline inverse (10 bins, tails at +-5) on caller data, for kernel unit tests: z is [rows][2],
  * h29 [rows][ldh >= 29] holds per row 10 width logits, 10 height logits and 9 derivative logits, used as given (the
  * engine divides the width / height logits by sqrt(hidden) first).  z[r][tcol] is replaced by its inverse for rows

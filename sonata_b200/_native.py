@@ -167,6 +167,12 @@ SIGNATURES = {
                                         C.c_float, C.c_int32, C.POINTER(C.c_float), C.c_float, C.POINTER(C.c_int32),
                                         C.c_int32, C.c_int32, C.POINTER(C.c_float), C.c_int32, C.c_int32,
                                         C.POINTER(C.c_float), C.c_int32, _ERR]),
+    "sb200_debug_resblock2_stage": (C.c_int32, [C.c_int32, C.POINTER(C.c_float), C.c_int32, C.c_int32,
+                                                C.POINTER(C.c_int32), C.POINTER(C.c_int32), C.POINTER(C.c_float),
+                                                C.POINTER(C.c_float), C.POINTER(C.c_int32), C.c_int32, C.c_int32,
+                                                C.POINTER(C.c_float), _ERR]),
+    "sb200_debug_resblock2_plan": (C.c_int32, [C.c_int64, C.c_int32, C.POINTER(C.c_int32), C.POINTER(C.c_int32),
+                                               C.POINTER(C.c_int32)]),
     "sb200_debug_spline": (C.c_int32, [C.c_int32, C.POINTER(C.c_float), C.c_int32, C.POINTER(C.c_float), C.c_int32,
                                        C.c_int32, C.c_int32, _ERR]),
     "sb200_debug_durations": (C.c_int32, [C.c_int32, C.POINTER(C.c_float), C.c_int32, C.POINTER(C.c_int32),

@@ -154,6 +154,20 @@ struct DeviceBuffers {
     }
 };
 
+// The branches of a 64-channel ResBlock2 stage of kernel sizes ks[b] and dilations dils[2b], dils[2b + 1]; each conv's
+// ConvW from `make` (weights and images, or only the shape).  False on a malformed description.
+template <typename Make> bool debug_stage(int32_t nbr, const int32_t* ks, const int32_t* dils, std::vector<ResBW>& res, Make&& make) {
+    if (nbr <= 0 || !ks || !dils) return false;
+    res.assign(nbr, ResBW{});
+    for (int b = 0; b < nbr; b++) {
+        if (ks[b] <= 0 || ks[b] > SB_MAX_TAPS || dils[2 * b] <= 0 || dils[2 * b + 1] <= 0) return false;
+        res[b].k = ks[b];
+        res[b].dils = {dils[2 * b], dils[2 * b + 1]};
+        for (int cv = 0; cv < 2; cv++) res[b].c1.push_back(make(b, cv));
+    }
+    return true;
+}
+
 }  // namespace
 
 extern "C" {
@@ -809,6 +823,50 @@ int32_t sb200_debug_conv_ex(int32_t device, int32_t backend, const float* x, int
         SB_CUDA(cudaDeviceSynchronize());
         if (dy0) SB_CUDA(cudaMemcpy(y0, dy0, (size_t)rows * ld0 * 4, cudaMemcpyDeviceToHost));
         if (dy1) SB_CUDA(cudaMemcpy(y1, dy1, (size_t)rows * ld1 * 4, cudaMemcpyDeviceToHost));
+    });
+}
+
+int32_t sb200_debug_resblock2_plan(int64_t rows, int32_t nbr, const int32_t* ks, const int32_t* dils, int32_t* out8) {
+    if (!out8 || rows <= 0 || rows > (1 << 30)) return 19;
+    static float anchor[64];
+    float* const stand_in = reinterpret_cast<float*>((reinterpret_cast<uintptr_t>(anchor) + 127) & ~(uintptr_t)127);
+    std::vector<ResBW> res;
+    const bool ok = debug_stage(nbr, ks, dils, res, [&](int b, int cv) {
+        ConvW w = conv_layout(64, 64, centred_taps(ks[b], dils[2 * b + cv]), false);
+        w.w = w.bias = w.wtc = stand_in;
+        w.tc_nt = tc_tile_for(64);
+        return w;
+    });
+    return ok && resblock2_tc_plan(res, (int)rows, out8) ? 0 : 19;
+}
+
+int32_t sb200_debug_resblock2_stage(int32_t device, const float* x, int32_t rows, int32_t nbr, const int32_t* ks,
+                                    const int32_t* dils, const float* w, const float* bias, const int32_t* seg_end,
+                                    int32_t gran, int32_t seg_mul, float* y, sb200_error* err) {
+    return guarded(err, [&] {
+        if (rows <= 0 || gran <= 0 || seg_mul <= 0 || !seg_end || !x || !w || !bias || !y)
+            throw Error(19, "debug resblock2 stage: bad arguments");
+        SB_CUDA(cudaSetDevice(device));
+        Voice tmp; tmp.device = device;
+        std::vector<ResBW> res;
+        size_t woff = 0;
+        const bool ok = debug_stage(nbr, ks, dils, res, [&](int b, int cv) {
+            const float* wb = w + woff;
+            woff += (size_t)64 * 64 * ks[b];
+            return debug_make_conv(tmp, wb, bias + (size_t)(2 * b + cv) * 64, 64, 64, ks[b], dils[2 * b + cv]);
+        });
+        if (!ok || !resblock2_tc_plan(res, rows, nullptr)) throw Error(19, "debug resblock2 stage: shape not supported");
+        const int R = (rows + 255) / 256 * 256;
+        const int ngran = (R + gran - 1) / gran;
+        std::vector<int> ends(ngran, 0);
+        for (int g = 0; g < ngran && g * gran < rows; g++) ends[g] = seg_end[g];
+        DeviceBuffers d;
+        const float* dx = d.upload(x, (size_t)rows * 64, (size_t)R * 64);
+        float* dy = d.alloc<float>((size_t)R * 64);
+        const int* dend = d.upload(ends.data(), (size_t)ngran, (size_t)ngran);
+        launch_resblock2_tc(res, dx, dy, RowMap{dend, gran, seg_mul, R}, 0);
+        SB_CUDA(cudaDeviceSynchronize());
+        SB_CUDA(cudaMemcpy(y, dy, (size_t)rows * 64 * 4, cudaMemcpyDeviceToHost));
     });
 }
 

@@ -705,6 +705,20 @@ void run_decoder(Runner& R, const Level& LY, const FrameTables& y, const Decoder
         }
         R.end();
         R.begin("dec.mrf" + std::to_string(i));
+        // A 64-channel ResBlock2 stage is one fused launch: it reads its input once and writes the mean once, where the
+        // six layer-wise convs each read and write a full activation.  The 32- and 128-channel stages stay layer-wise
+        // (DESIGN.md section 3).
+        if (v.backend >= 1 && a.resblock == 2 && st.cout == 64 && resblock2_tc_plan(st.res, Lo.map.rows, nullptr)) {
+            launch_resblock2_tc(st.res, up, ys, Lo.map, R.st);
+            const double vr = (double)Lo.valid_rows;
+            double macs = 0;
+            for (const ResBW& rb : st.res)
+                for (const ConvW& w : rb.c1) macs += w.macs;
+            R.count(2.0 * vr * macs, 4.0 * (vr * 2 * st.cout + macs));
+            R.end();
+            cur = ys; Lin = Lo; U = Uo;
+            continue;
+        }
         const float third = 1.0f / (float)st.res.size();
         for (size_t jb = 0; jb < st.res.size(); jb++) {
             const ResBW& rb = st.res[jb];

@@ -84,6 +84,12 @@ struct DDSW { float* wdw[3]; float* bdw[3]; ConvW c1x1[3]; float *g1[3], *b1[3],
 struct CFlowW { float* pre_w; float* pre_b; DDSW dds; ConvW proj; int ccol, tcol; };
 struct CouplingW { ConvW pre; std::vector<ConvW> in, rs; ConvW post; int cond_off, tgt_off; };
 struct ResBW { int k; std::vector<int> dils; std::vector<ConvW> c1, c2; };
+// A ResBlock2 stage (branches res[b], convs c1[0] and c1[1]) of 64 channels as one launch (resblock_tc.cu):
+// y = mean over b of x1_b + conv(lrelu(x1_b)), x1_b = x + conv(lrelu(x)), bit-identical to the six conv_tc launches.
+// resblock2_tc_plan: false when the stage's shape is not one the kernel takes; out8 (or null) = {tile rows, x window
+// rows, x1 rows, weight ring slots, dynamic shared memory bytes, grid CTAs for `rows`, threads, registers of one CTA}.
+bool resblock2_tc_plan(const std::vector<ResBW>& res, int rows, int* out8);
+void launch_resblock2_tc(const std::vector<ResBW>& res, const float* x, float* y, const RowMap& map, cudaStream_t st);
 // phase: one fp32 conv per output phase (backend 0, or when fused has no image); fused: all phases as one N = u*cout
 // conv with bf16 images only (backends 1 and 2)
 struct UpStageW { int u, k, cin, cout; std::vector<ConvW> phase; ConvW fused; std::vector<ResBW> res; };
