@@ -53,6 +53,7 @@ struct ConvArgs {
     float* y1; int ldy1; int acc1;                                // columns [split, cout)
     float* yt; int yt_col0; int ldyt;                             // conv_tf.cu: column tiles >= yt_col0 are stored TRANSPOSED,
                                                                   // yt[(n - yt_col0) * ldyt + q] (row index contiguous)
+    int yt_keep;                                                  // and, when set, also to y0 as the other columns are
     const int* bias_slot; int ldbias;                             // per-row bias: row q adds bias[bias_slot[q / map.gran] * ldbias + n]
                                                                   // (speaker-conditioned convs of a batch with several speakers)
 };
@@ -160,7 +161,10 @@ void launch_ln(const float* x, const float* res1, const float* res2, const float
 // out = GELU(LN(depthwise_conv_k(x, dilation)))   (DDSConv first half)
 void launch_dw_ln_gelu(const float* x, const float* wdw /*[k][C]*/, const float* bdw, int k, int dil,
                        const float* gamma, const float* beta, float* out, int C, RowMap map, cudaStream_t st);
-// Relative-position softmax between the two attention GEMMs (in place on the score rows): see kernels_misc.cu
+// The longest utterance the tensor-core attention takes: the softmax keeps a score row in 40 registers of 32 lanes.
+constexpr int ATT_TC_MAX = 1280;
+// Relative-position softmax between the two attention GEMMs (in place on the score rows): see kernels_misc.cu.  max_len:
+// the longest utterance on this path (<= ATT_TC_MAX); rows of longer ones are left to launch_attention.
 void launch_attn_softmax(float* S, int Tp, const float* qkv, int ldq, const float* relk, const float* relv, int window,
                          float* orel, int ldo, int H, int heads, int RX, const SegInfo* segs, const int* seg_of_gran,
                          int gran, int max_len, cudaStream_t st);

@@ -245,7 +245,7 @@ __global__ void __launch_bounds__(TF_THREADS, 1) conv_tf_kernel(const ConvArgs a
                 if (a.yt && n >= a.yt_col0) {
                     // transposed output (V of the fused q/k/v projection: the P.V contraction wants keys contiguous)
                     a.yt[(size_t)(n - a.yt_col0) * a.ldyt + q] = valid ? o * a.scale : 0.f;
-                    continue;
+                    if (!a.yt_keep) continue;
                 }
                 if (a.acc0 && !valid) continue;         // accumulated buffers keep their zeros in gap rows
                 float m = 0.f;

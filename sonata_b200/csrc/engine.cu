@@ -29,7 +29,7 @@ ConvArgs conv_args(const ConvW& w, const float* x, int ldx, const RowMap& map, c
     p.act = c.act; p.scale = c.scale; p.res = c.res; p.ldres = c.ldres;
     p.y0 = c.y0; p.ldy0 = c.ldy0; p.acc0 = c.acc0; p.split = c.split < 0 ? w.cout : c.split;
     p.y1 = c.y1; p.ldy1 = c.ldy1; p.acc1 = c.acc1;
-    p.yt = c.yt; p.yt_col0 = c.yt_col0; p.ldyt = c.ldyt;
+    p.yt = c.yt; p.yt_col0 = c.yt_col0; p.ldyt = c.ldyt; p.yt_keep = c.yt_keep;
     return p;
 }
 
@@ -118,20 +118,26 @@ Job* create_job(Voice* v, const long long* ids, const size_t* offs, size_t B, co
         for (size_t b = 0; b < B; b++) if (eps_z[b]) j->eps_z[b].assign(eps_z[b], eps_z[b] + eps_z_frames[b] * (size_t)v->a.inter);
     }
     // X layout
+    const int H = v->a.hidden, heads = v->a.heads, D = H / heads;
     int cur = 0;
     for (size_t b = 0; b < B; b++) {
         const int n = (int)(j->offs[b + 1] - j->offs[b]);
+        // attention_kernel keeps a score row per query in shared memory; any utterance may run on it (every one past
+        // ATT_TC_MAX ids, every one on backends 0 / 2)
+        if (attention_smem_bytes(n, D) > 220 * 1024)
+            throw Error(19, "Failed to run model inference. Error: sentence too long for one pass (utterance " +
+                                std::to_string(b) + ": " + std::to_string(n) + " ids)");
         j->xsegs.push_back({cur, n});
-        j->max_tx = std::max(j->max_tx, n);
+        if (n <= ATT_TC_MAX) j->att_tc_len = std::max(j->att_tc_len, n);
         cur += round_up(n + HX, GX);
     }
     j->RX = round_up(cur, 256);
     {
-        // Tile tables of the two attention GEMMs (conv_tf.cu, grouped mode).  S[head][row][key] = Q.K^T / sqrt(D):
-        // A = Q rows, B = K rows of the fused q/k/v activation [RX][3H]; O = P.V: A = P rows of S viewed as
-        // [heads*RX][Tp], B = V^T [H][RX] (the q/k/v projection stores V transposed).
-        const int H = v->a.hidden, heads = v->a.heads, D = H / heads;
-        j->att_tp = round_up(std::max(j->max_tx, 1), 64);      // key tile of the Q.K^T GEMM (64: see conv_tf.cu tf_nth_for)
+        // Tile tables of the two attention GEMMs (conv_tf.cu, grouped mode), over the utterances of at most ATT_TC_MAX
+        // ids.  S[head][row][key] = Q.K^T / sqrt(D): A = Q rows, B = K rows of the fused q/k/v activation [RX][3H];
+        // O = P.V: A = P rows of S viewed as [heads*RX][Tp], B = V^T [H][RX] (the q/k/v projection stores V transposed).
+        auto on_tc = [&](size_t b) { return j->xsegs[b].len <= ATT_TC_MAX; };
+        j->att_tp = round_up(std::max(j->att_tc_len, 1), 64);  // key tile of the Q.K^T GEMM (64: see conv_tf.cu tf_nth_for)
         // Small jobs (a single utterance): narrower column tiles put the same MMAs on more SMs (conv_tf.cu plan()); tile
         // width changes no summation order, so results do not depend on it.
         {
@@ -139,6 +145,7 @@ Job* create_job(Voice* v, const long long* ids, const size_t* offs, size_t B, co
             if (cudaGetDevice(&dev) == cudaSuccess) cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
             long long wide_s = 0, wide_o = 0;
             for (size_t b = 0; b < B; b++) {
+                if (!on_tc(b)) continue;
                 const int T = j->xsegs[b].len;
                 wide_s += (long long)heads * ((T + 255) / 256) * ((T + 63) / 64);
                 wide_o += (long long)heads * ((T + 255) / 256);
@@ -148,6 +155,7 @@ Job* create_job(Voice* v, const long long* ids, const size_t* offs, size_t B, co
         }
         const int ks = j->att_nth_s, ko = j->att_nth_o;
         for (size_t b = 0; b < B; b++) {
+            if (!on_tc(b)) continue;
             const int off = j->xsegs[b].off, T = j->xsegs[b].len;
             const int nmp = (T + 255) / 256, nnt = (T + ks - 1) / ks;
             for (int h = 0; h < heads; h++)
@@ -181,8 +189,6 @@ Job* create_job(Voice* v, const long long* ids, const size_t* offs, size_t B, co
                 }
         }
     }
-    if (attention_smem_bytes(j->max_tx, v->a.hidden / v->a.heads) > 220 * 1024)
-        throw Error(19, "Failed to run model inference. Error: sentence too long for one pass (" + std::to_string(j->max_tx) + " ids)");
     j->noise_call = ++v->call_counter;
     j->ctx = v->acquire();
     return j.release();
@@ -388,6 +394,7 @@ void begin_pass(Context& c) {
 // Id level (phase 1): X tables, encoder and duration-predictor activations, and with debug the captures.
 struct IdBufs {
     Staged<int> ids_rows, xend, xseg_of_gran, ylen; Staged<SegInfo> xsegs; Staged<TfTile> tiles;
+    Staged<SegInfo> att_segs;                  // the utterances on the fp32 attention kernel
     Staged<float> scales;                      // per utterance: noise_w [B], length_scale [B], noise_scale [B]
     Staged<int> xslot;                         // multi-speaker voices: speaker slot of every X granule
     SpeakerBias spk;
@@ -404,7 +411,7 @@ struct IdBufs {
     enum { ENC_QKV, ENC_VT, ENC_ATT, ENC_O, ENC_LN1, ENC_FFN1, ENC_FFN2, ENC_LN2, ENC_NCAP };
     std::vector<std::array<float*, ENC_NCAP>> encl;
 
-    void carve(Arena& dev, Arena& pin, const Job& j, bool tc_att) {
+    void carve(Arena& dev, Arena& pin, const Job& j, bool tc_att, size_t n_simt) {
         const Voice& v = *j.v; const Arch& a = v.a;
         const int RX = j.RX, nxg = RX / GX, H = a.hidden;
         const size_t B = j.B, ntiles = j.tiles_s.size() + j.tiles_o.size();
@@ -412,6 +419,7 @@ struct IdBufs {
         ids_rows.carve(dev, pin, RX); xend.carve(dev, pin, nxg); xseg_of_gran.carve(dev, pin, nxg);
         xsegs.carve(dev, pin, B); ylen.carve(dev, pin, B);
         if (tc_att) tiles.carve(dev, pin, ntiles);
+        if (n_simt) att_segs.carve(dev, pin, n_simt);
         scales.carve(dev, pin, 3 * B);
         if (!j.frames.slot_sid.empty()) xslot.carve(dev, pin, nxg);
         spk.carve(dev, pin, v, j.frames);
@@ -932,16 +940,24 @@ void Job::run(float* d_out, size_t d_out_cap) {
     regions.clear(); dbg.clear(); dbg_level.clear(); id_frames.clear();
 
     // ---------------- id level (phase 1) workspace ----------------
-    // tensor-core attention (two grouped GEMMs around a softmax): default backend, 96- or 48-wide heads, rows that fit
-    // the softmax kernel's registers; otherwise the fp32 CUDA-core attention kernel
+    // Each utterance takes the attention it would take alone: the tensor-core attention (two grouped GEMMs around a
+    // softmax) on the default backend with 96- or 48-wide heads when it has at most ATT_TC_MAX ids (the softmax keeps a
+    // row in registers), otherwise the fp32 CUDA-core attention kernel, launched over those utterances only.  A batch
+    // with utterances on both routes runs both in every layer.
     const int D = H / a.heads;
-    const bool tc_att = V.backend == 1 && (D == 96 || D == 48) && max_tx <= 1280 && getenv("SB200_ATT_SIMT") == nullptr;
+    const bool tc_voice = V.backend == 1 && (D == 96 || D == 48) && getenv("SB200_ATT_SIMT") == nullptr;
+    const bool tc_att = tc_voice && !tiles_s.empty();
+    std::vector<SegInfo> simt_segs;
+    int simt_len = 0;
+    for (const SegInfo& s : xsegs)
+        if (!tc_voice || s.len > ATT_TC_MAX) { simt_segs.push_back(s); simt_len = std::max(simt_len, s.len); }
+    const bool simt_att = !simt_segs.empty();
     frames.slot_of.clear(); frames.slot_sid.clear();
     for (size_t b = 0; b < B; b++)      // piper/src/lib.rs:353-358: speaker.unwrap_or(0)
         if (!assign_slot(frames, V, cfgs[b].has_speaker ? cfgs[b].speaker : 0))
             throw Error(19, "Failed to run model inference. Error: speaker id out of range (utterance " + std::to_string(b) + ")");
     IdBufs x;
-    plan(C.dev_id, C.pin, [&](Arena& dev, Arena& pin) { x.carve(dev, pin, *this, tc_att); });
+    plan(C.dev_id, C.pin, [&](Arena& dev, Arena& pin) { x.carve(dev, pin, *this, tc_att, simt_segs.size()); });
     d_cum = x.cum;
     Runner R(V, C, regions, x.spk.cond);
 
@@ -985,10 +1001,13 @@ void Job::run(float* d_out, size_t d_out_cap) {
         std::copy(tiles_o.begin(), tiles_o.end(), std::copy(tiles_s.begin(), tiles_s.end(), x.tiles.h));
         x.tiles.upload(st);
     }
+    if (simt_att) {
+        std::copy(simt_segs.begin(), simt_segs.end(), x.att_segs.h);
+        x.att_segs.upload(st);
+    }
 
     Level LX; LX.map = {x.xend.d, GX, 1, RX}; LX.valid_rows = (long long)ids.size(); LX.bias_slot = x.xslot.d;
     TfGemm gs{}, go{};
-    bool tc_att_ok = tc_att;
     if (tc_att) {
         gs.a = x.qkv; gs.a_rows = RX; gs.a_cols = 3 * H; gs.lda = 3 * H;
         gs.b = x.qkv; gs.b_rows = RX; gs.b_cols = 3 * H; gs.ldb = 3 * H;
@@ -998,13 +1017,13 @@ void Job::run(float* d_out, size_t d_out_cap) {
         go.b = x.att_vt; go.b_rows = H; go.b_cols = RX; go.ldb = RX;
         go.nth = att_nth_o; go.y = x.att; go.ldy = H; go.res = x.att_orel; go.scale = 1.f;
         go.tiles = x.tiles.d + tiles_s.size(); go.ntiles = (int)tiles_o.size();
-        tc_att_ok = gemm_tf_supported(gs) && gemm_tf_supported(go);
+        if (!gemm_tf_supported(gs) || !gemm_tf_supported(go)) throw Error(19, "internal: attention GEMM operands conv_tf does not take");
     }
     if (debug) {
         expose(*this, "x", x.xa, H, 0); expose(*this, "stats", x.stats, 2 * I, 0);
         expose(*this, "qkv0", x.qkv0, 3 * H, 0); expose(*this, "att0", x.att0, H, 0);
-        if (tc_att_ok) {
-            expose(*this, "p0", x.p0, att_tp, 0);      // head 0 probabilities
+        if (tc_att) {
+            expose(*this, "p0", x.p0, att_tp, 0);      // head 0 probabilities; zero rows for utterances past ATT_TC_MAX
             expose(*this, "vt0", x.vt0, H, -1);        // stored as [H][RX]
         }
         expose(*this, "dp.g", x.g, H, 0); expose(*this, "logw", x.logw, 1, 0);
@@ -1018,7 +1037,7 @@ void Job::run(float* d_out, size_t d_out_cap) {
             const std::string p = "enc." + std::to_string(l) + ".";
             const auto& c = x.encl[l];
             expose(*this, p + "qkv", c[IdBufs::ENC_QKV], 3 * H, 0);
-            if (tc_att_ok) expose(*this, p + "vt", c[IdBufs::ENC_VT], H, -1);   // stored as [H][RX]
+            if (tc_att) expose(*this, p + "vt", c[IdBufs::ENC_VT], H, -1);   // stored as [H][RX]
             expose(*this, p + "att", c[IdBufs::ENC_ATT], H, 0); expose(*this, p + "o", c[IdBufs::ENC_O], H, 0);
             expose(*this, p + "ln1", c[IdBufs::ENC_LN1], H, 0); expose(*this, p + "ffn1", c[IdBufs::ENC_FFN1], F, 0);
             expose(*this, p + "ffn2", c[IdBufs::ENC_FFN2], H, 0); expose(*this, p + "ln2", c[IdBufs::ENC_LN2], H, 0);
@@ -1056,30 +1075,37 @@ void Job::run(float* d_out, size_t d_out_cap) {
         const EncLayer& e = V.enc[l];
         float* const* cap = debug ? x.encl[l].data() : nullptr;
         {
+            // V leaves transposed for the P.V GEMM, [H][RX]; with both routes also in qkv's V columns for attention_kernel
             ConvCall o; o.y0 = x.qkv; o.ldy0 = 3 * H;
-            if (tc_att_ok) { o.yt = x.att_vt; o.yt_col0 = 2 * H; o.ldyt = RX; }       // V leaves transposed: [H][RX]
+            if (tc_att) { o.yt = x.att_vt; o.yt_col0 = 2 * H; o.ldyt = RX; o.yt_keep = simt_att; }
             R.conv(e.qkv, x.xa, H, LX, o);
         }
         if (cap) {
             d2d(cap[IdBufs::ENC_QKV], x.qkv, (size_t)RX * 3 * H, st);
-            if (tc_att_ok) d2d(cap[IdBufs::ENC_VT], x.att_vt, (size_t)H * RX, st);
+            if (tc_att) d2d(cap[IdBufs::ENC_VT], x.att_vt, (size_t)H * RX, st);
         }
-        if (tc_att_ok) {
+        int att_launches = 0;
+        if (tc_att) {
             launch_gemm_tf(gs, st);
             launch_attn_softmax(x.att_s, att_tp, x.qkv, 3 * H, e.relk, e.relv, a.window, x.att_orel, H, H, a.heads, RX,
-                                x.xsegs.d, x.xseg_of_gran.d, GX, max_tx, st);
+                                x.xsegs.d, x.xseg_of_gran.d, GX, att_tc_len, st);
             launch_gemm_tf(go, st);
-            R.count(0, 0, 2);
-        } else {
-            launch_attention(x.qkv, 3 * H, e.relk, e.relv, a.window, x.att, H, H, a.heads, x.xsegs.d, (int)B, max_tx, st);
+            att_launches += 3;
         }
-        { double f = 0; for (auto& s : xsegs) f += 4.0 * (double)s.len * s.len * H; R.count(f, 16.0 * LX.valid_rows * H); }
+        if (simt_att) {
+            launch_attention(x.qkv, 3 * H, e.relk, e.relv, a.window, x.att, H, H, a.heads, x.att_segs.d,
+                             (int)simt_segs.size(), simt_len, st);
+            att_launches += 1;
+        }
+        { double f = 0; for (auto& s : xsegs) f += 4.0 * (double)s.len * s.len * H; R.count(f, 16.0 * LX.valid_rows * H, att_launches); }
         if (debug && l == 0) {      // first-layer attention operands / result (tests/test_gpu_parity.py)
             d2d(x.qkv0, x.qkv, (size_t)RX * 3 * H, st);
             d2d(x.att0, x.att, (size_t)RX * H, st);
-            if (tc_att_ok) {
+            if (tc_att) {
                 d2d(x.p0, x.att_s, (size_t)RX * att_tp, st);
-                // V went only to att_vt (the V columns of qkv0 are not written on this path)
+                for (const SegInfo& s : simt_segs)         // score rows no kernel of this path wrote
+                    SB_CUDA(cudaMemsetAsync(x.p0 + (size_t)s.off * att_tp, 0, (size_t)s.len * att_tp * sizeof(float), st));
+                // V went to att_vt; the V columns of qkv0 hold it too only when some utterance is on attention_kernel
                 d2d(x.vt0, x.att_vt, (size_t)H * RX, st);
             }
         }

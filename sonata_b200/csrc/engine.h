@@ -75,6 +75,7 @@ struct ConvCall {
     float* y1 = nullptr; int ldy1 = 0; int acc1 = 0;
     int orow_mul = 1, orow_add = 0;
     float* yt = nullptr; int yt_col0 = 0, ldyt = 0;     // conv_tf only: column tiles >= yt_col0 stored transposed
+    int yt_keep = 0;                                    // ... and also untransposed to y0
 };
 // Launch arguments of layer `w` over the rows of `map`, reading x [map.rows][ldx]; the bias is the layer's own.
 ConvArgs conv_args(const ConvW& w, const float* x, int ldx, const RowMap& map, const ConvCall& c);
@@ -325,12 +326,14 @@ struct Job {
     // loudness and the gain applied to it
     std::vector<float> loud_ran; std::vector<double> loud_lufs; std::vector<float> loud_gain;
     // X layout
-    int RX = 0; std::vector<SegInfo> xsegs; int max_tx = 0;
+    int RX = 0; std::vector<SegInfo> xsegs;
     // Y layout
     FrameLayout frames; std::vector<int> y_len;
-    // tensor-core attention (conv_tf.cu grouped GEMMs): tile tables built with the X layout, same for every layer
+    // tensor-core attention (conv_tf.cu grouped GEMMs): tile tables built with the X layout, same for every layer, of
+    // the utterances of at most ATT_TC_MAX ids (the only ones the path takes: Job::run)
     std::vector<TfTile> tiles_s, tiles_o;      // Q.K^T tiles, P.V tiles
-    int att_tp = 0;                            // key columns of a score row (multiple of 96)
+    int att_tc_len = 0;                        // the longest of those utterances (0: none)
+    int att_tp = 0;                            // key columns of a score row (multiple of 64)
     int att_nth_s = 64, att_nth_o = 96;   // column tiles of the two attention GEMMs (narrower when the job is small)
     // device results read after the pass (context arenas)
     int* d_cum = nullptr;

@@ -290,7 +290,8 @@ __global__ void __launch_bounds__(2 * D) attention_kernel(const float* __restric
 // utterance's keys IN PLACE, zero-fills the row up to the next multiple of 32 keys (the K extent of the second GEMM) and
 // writes the relative-value term  orel[row][head*D + c] = sum_d p[i][i+d] E_v[d+w][c],  which the second GEMM adds as
 // its residual.  The whole row lives in registers (NREG x 32 keys).  Lane l holds head channels l + 32k (k < ceil(D/32);
-// 48-wide heads leave lanes 16-31 idle in the second).  oracle: _mha()
+// 48-wide heads leave lanes 16-31 idle in the second).  The launcher picks NREG from the longest utterance of the job
+// on this path; rows of longer utterances, which run on attention_kernel, are skipped.  oracle: _mha()
 template <int D, int NREG>
 __global__ void __launch_bounds__(256) attn_softmax_kernel(float* __restrict__ S, int Tp, const float* __restrict__ qkv,
                                                            int ldq, const float* __restrict__ relk,
@@ -306,6 +307,7 @@ __global__ void __launch_bounds__(256) attn_softmax_kernel(float* __restrict__ S
     const SegInfo sg = segs[seg_of_gran[q / gran]];
     const int i = q - sg.off, T = sg.len;
     if (i < 0 || i >= T) return;                       // gap row
+    if (T > 32 * NREG) return;                         // an utterance longer than the registers hold: on attention_kernel
     float* Sr = S + ((size_t)head * RX + q) * Tp;
     const int nrel = 2 * window + 1;
     constexpr int NV = (D + 31) / 32;
@@ -1096,7 +1098,7 @@ void launch_attn_softmax(float* S, int Tp, const float* qkv, int ldq, const floa
                          int gran, int max_len, cudaStream_t st) {
     const int D = H / heads;
     dim3 grid((RX + 7) / 8, heads);
-    if ((D != 96 && D != 48) || max_len > 1280 || 2 * window + 1 > 32) throw_launch_error("attn_softmax: unsupported head size / length");
+    if ((D != 96 && D != 48) || max_len > ATT_TC_MAX || 2 * window + 1 > 32) throw_launch_error("attn_softmax: unsupported head size / length");
     auto k = D == 96 ? (max_len <= 640 ? attn_softmax_kernel<96, 20> : attn_softmax_kernel<96, 40>)
                      : (max_len <= 640 ? attn_softmax_kernel<48, 20> : attn_softmax_kernel<48, 40>);
     launch_pdl(k, dim3(grid), dim3(256), 0, st, S, Tp, qkv, ldq, relk, relv, window, orel, ldo, RX, segs, seg_of_gran, gran);

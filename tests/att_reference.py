@@ -19,19 +19,22 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 #     T          1        31-65           95-257          639-641         1279-1280
 #     fp32     1.2e-7   4.1e-7-8.1e-7    5.8e-7-1.3e-6    2.7e-6-2.9e-6   5.0e-6-5.3e-6
 #     wgmma    5.9e-7   1.8e-6-3.4e-6    2.9e-6-3.6e-6    3.6e-6-3.8e-6   3.9e-6-4.1e-6
-# (the fp32 fallback at T = 1281: 5.5e-6).  The CPU emulation in test_oracle.py puts a P.V contraction with a single
-# TF32 MMA (1.3e-3), two of the three split products (8.3e-4), or no chunk flush (2.6e-5) at T = 1280 above this
-# bound (1.5e-5 there); the chunk-flushed 3xTF32 contraction emulates at 1.8e-6.
+# (the fp32 attention at T = 1281: 5.5e-6; at its length limits, measured on an H100 80GB HBM3 at a 700 W power
+# limit by tests/test_attention_routing_gpu.py -s: medium T = 3004, 1.22e-5 at |ref| 2.49 (83 ulp of max |ref|), and
+# x_low T = 3244, 1.24e-5 at |ref| 2.30 (90 ulp), both 0.42 of fp32_att_bound).  The CPU emulation in test_oracle.py
+# puts a P.V contraction with a single TF32 MMA (1.3e-3), two of the three split products (8.3e-4), or no chunk flush
+# (2.6e-5) at T = 1280 above this bound (1.5e-5 there); the chunk-flushed 3xTF32 contraction emulates at 1.8e-6.
 ATT_MULT = 2.0
 ATT_FLOOR = 2e-6
 
 
 def fp32_att_bound(T, scale):
-    """Bound of the fp32 CUDA-core attention kernel itself (backends 0 / 2, and every job past 1280 ids), so that it is not
-    only the tensor-core path's yardstick: (8 + T / 16) ulp of max |ref|.  Each output of that kernel sums its T
+    """Bound of the fp32 CUDA-core attention kernel itself (backends 0 / 2, and every utterance past 1280 ids), so that it
+    is not only the tensor-core path's yardstick: (8 + T / 16) ulp of max |ref|.  Each output of that kernel sums its T
     products in four fp32 FMA chains of T / 4 keys; measured on the H100 above, its error grows as ~T / 35 ulp of max |ref|
-    (0.8 ulp at T = 1, 3.7 at 63, 19 at 640, 35 at 1280, 37 at 1281), which leaves at least 1.9x margin at every length
-    tested, while a wrong band index, a dropped term or a reduced-precision accumulation lands orders of magnitude above."""
+    (0.8 ulp at T = 1, 3.7 at 63, 19 at 640, 35 at 1280, 37 at 1281, 83 at 3004, 90 at 3244), which leaves at least
+    1.9x margin at every length tested, while a wrong band index, a dropped term or a reduced-precision accumulation
+    lands orders of magnitude above."""
     return (8 + T / 16) * 2.0 ** -24 * scale
 
 

@@ -26,7 +26,7 @@ Every stage evaluates through an `Arith`:
 Keyword mutations of an Arith model plausible kernel mistakes, for the CPU test that shows the bounds catch them.
 
 Bounds (stage_check), each at least 2x above the worst value measured on an H100 SXM (80 GB HBM3, 700 W power limit) by
-tests/test_encoder_gpu.py -s (medium / high / x_low voices; edge batches of 1 .. 1281 ids on backend 1, backend 1 with
+tests/test_encoder_gpu.py -s (medium / high / x_low voices; edge batches of 1 .. 3004 ids on backend 1, backend 1 with
 the fp32 attention and backend 0; medium 32 x 256 and high 1 x 512 phonemes on backend 1):
     enc.emb      bit for bit with float32(emb) * float32(sqrt(H)).
     backend 1 contractions (qkv, o, ffn1 after the ReLU, ffn2, stats), per 128-row tile:
@@ -61,7 +61,7 @@ F32_MULT = 4.0          # the same on backend 0: at most 0.24 (the kernels' erro
 F32_FLOOR = 2.0 ** -22
 LN_MULT = 4.0           # both LayerNorms, every backend: at most 0.31
 LN_FLOOR = 2.0 ** -22
-ATT_MULT = 4.0          # fp32 attention kernel (backend 0, SB200_ATT_SIMT=1, T > 1280): at most 0.19; tensor-core
+ATT_MULT = 4.0          # fp32 attention kernel (backend 0, SB200_ATT_SIMT=1, T > 1280): at most 0.23; tensor-core
 ATT_FLOOR = 2.0 ** -18  # attention: at most 0.41.  The floor is the tensor-core path's: its split operands leave up to
                         # 4.7e-6 at |ref| 2.3 at any T (att_reference.py), which 2^-22 (0.46 for the fp32 kernel at
                         # ATT_MULT 4) put at 1.7x the bound.  At T = 1280 this bound is ~1.5e-5, near an unflushed P.V's

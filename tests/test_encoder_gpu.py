@@ -25,13 +25,15 @@ pytestmark = pytest.mark.gpu
 
 # One job per batch.  T <= w and T = 2w + 1: the clipped relative band; 31 / 32 / 33: the softmax's 32-key zero fill;
 # 48: n + HX lands on the 64-id granule; 63 / 64 / 65: granule edges; 127 .. 257: conv_tf's 128-row tiles; 639 .. 1280:
-# both softmax register regimes and the tensor-core limit; 1281: the whole job on the fp32 attention.
+# both softmax register regimes and the tensor-core limit; 1281 and 3004 (the longest utterance the fp32 attention takes
+# with 96-wide heads) on the fp32 attention, beside 33, 1280 and 2 on the tensor cores: a job on both routes.
 EDGE_BATCHES = {
     "short": (1, 2, 4, 5, 9, 10, 31, 32, 33, 48, 63, 64, 65),
     "tiles": (127, 128, 129, 255, 257, 3),
     "softmax": (639, 640, 641, 1280, 2),
-    "fallback": (1281, 33),
+    "fallback": (1281, 33, 1280, 3004, 2),
 }
+TC_MAX = 1280       # the longest utterance on the tensor-core attention
 VOICES = ("medium", "high", "x_low")
 # name -> (backend, fp32 attention forced)
 CONFIGS = {"b1": (1, False), "b1_fp32att": (1, True), "b0": (0, False)}
@@ -81,11 +83,13 @@ def _run(m, ids, backend, simt, monkeypatch, debug=True):
 
 
 def _captures(job, t, utts, ids):
-    """Per utterance: every enc.* capture, x, stats and the ids.  On the tensor-core attention path V reaches only the
-    transposed capture enc.{l}.vt, which takes the place of qkv's V columns."""
+    """Per utterance: every enc.* capture, x, stats and the ids.  On a job with tensor-core attention V reaches the
+    transposed capture enc.{l}.vt, which takes the place of qkv's V columns; on a job that also has utterances on the
+    fp32 attention it reaches qkv's V columns too, with the same bits."""
     a = er.arch(t)
     H = a["hidden"]
     names = [s[0] for s in er.stages(t)]
+    both = max(len(i) for i in ids) > TC_MAX and min(len(i) for i in ids) <= TC_MAX
     out = []
     for b in utts:
         c = {n: job.debug_fetch(n, b) for n in names}
@@ -96,6 +100,8 @@ def _captures(job, t, utts, ids):
                 vt = job.debug_fetch(f"enc.{l}.vt", b)
             except sonata_b200.OperationError:
                 continue
+            if both:
+                assert np.array_equal(c[f"enc.{l}.qkv"][:, 2 * H:], vt.T), (l, len(ids[b]))
             c[f"enc.{l}.qkv"] = c[f"enc.{l}.qkv"].copy()
             c[f"enc.{l}.qkv"][:, 2 * H:] = vt.T
             c[f"enc.{l}.vt"] = vt

@@ -290,12 +290,14 @@ def _attention_job(m, lens, simt, monkeypatch):
 # One job per softmax regime of the tensor-core attention (rows in 20 / 40 registers, kernels_misc.cu), lengths batched so
 # segment offsets and gap rows are exercised: T = 1, odd T, T = 32k +- 1 (the softmax zero-fills keys to the next multiple
 # of 32, the K extent of P.V), T <= 128 (the second 128-row m-tile of a tile pair has no valid row), T = 640 / 641; and
-# T = 1281, past the tensor-core attention's limit, on the fp32 attention.
+# a job on both routes: T = 1281 and 2000, past the tensor-core attention's limit, on the fp32 attention, beside 33 and
+# 1280 on the tensor cores.
 ATT_JOBS = {
     "nreg20": (1, 2, 31, 32, 33, 63, 65, 97, 127, 128, 129, 255, 257, 639, 640),
     "nreg40": (3, 95, 641, 1279, 1280),
-    "fp32_fallback": (1281, 33),
+    "mixed": (1281, 33, 1280, 2000),
 }
+TC_MAX = 1280       # the longest utterance on the tensor-core attention
 
 
 @pytest.mark.parametrize("regime", list(ATT_JOBS))
@@ -303,15 +305,17 @@ def test_tensor_core_attention_against_fp64(regime, models, monkeypatch):
     """Layer 0 of the text encoder on the default backend against float64 (tests/att_reference.py):
     * q / k / v projection, V through its transposed store, against x0 . Wqkv^T + b at the 3xTF32 conv tolerance;
     * the same job with SB200_ATT_SIMT=1 (V stored untransposed by the same conv kernel): Q / K and V bit for bit;
-    * att0 of the fp32 CUDA-core attention (the SB200_ATT_SIMT=1 run, and both runs of the job past 1280 ids, which
-      takes that kernel whatever the setting) against the fp64 attention of the kernel's own Q / K / V, within the
-      T-scaled fp32 bound att_reference.fp32_att_bound;
-    * att0 of the tensor-core attention, both heads, against the same reference, within
+      in the job on both routes V goes both ways, and qkv0's V columns equal vt0 transposed;
+    * att0 of the fp32 CUDA-core attention (the SB200_ATT_SIMT=1 run, and both runs of every utterance past 1280 ids,
+      which takes that kernel whatever the setting and must give the same bits in both) against the fp64 attention of
+      the kernel's own Q / K / V, within the T-scaled fp32 bound att_reference.fp32_att_bound;
+    * att0 of the tensor-core attention (utterances of at most 1280 ids), both heads, against the same reference, within
       ATT_MULT x (the fp32 attention's error on the same inputs) + ATT_FLOOR x max|ref|;
     * head-0 probabilities p0 against the fp64 softmax, within ATT_MULT x the error of a float32 softmax computed on the
       host + ATT_FLOOR (absolute; probabilities are <= 1), zero keys [T, round_up(T, 32)), rows summing to 1 within a
       T-scaled few ulp.  For p0 the floor is what binds: measured 0 .. 5.3e-7 against a float32 host error of
-      0 .. 1.5e-7, while a score GEMM on a single TF32 MMA or two of its three split products is off by 1e-4 or more.
+      0 .. 1.5e-7, while a score GEMM on a single TF32 MMA or two of its three split products is off by 1e-4 or more;
+      the p0 rows of utterances on the fp32 attention are zero.
     att0 errors measured on an H100 SXM are listed beside ATT_MULT in tests/att_reference.py.  Run with -s to print the
     per-utterance table."""
     import att_reference as ar
@@ -324,13 +328,16 @@ def test_tensor_core_attention_against_fp64(regime, models, monkeypatch):
     relk, relv = ar.rel_embeddings(t, 0)
     tc = _attention_job(m, lens, False, monkeypatch)
     simt = _attention_job(m, lens, True, monkeypatch)
-    on_tc = regime != "fp32_fallback"
+    both = max(lens) > TC_MAX
     report = []
     for n, u, s in zip(lens, tc, simt):
+        on_tc = n <= TC_MAX
         assert u["qkv0"].shape == (n, 3 * H) and u["att0"].shape == (n, H)
-        assert ("vt0" in u) == on_tc and ("p0" in u) == on_tc
+        assert "vt0" in u and "p0" in u and "p0" not in s and "vt0" not in s      # the job has a tensor-core utterance
         q, k = u["qkv0"][:, :H], u["qkv0"][:, H:2 * H]
-        v = u["vt0"].T if on_tc else u["qkv0"][:, 2 * H:]
+        v = u["vt0"].T
+        if both:                                                                      # V stored both ways
+            assert np.array_equal(u["qkv0"][:, 2 * H:], v), n
         _, refs = ar.project_qkv(t, 0, u["ids"])
         for got, ref in zip((q, k, v), refs):
             assert float(np.abs(got - ref).max()) < TF_TOL * max(1.0, float(np.abs(ref).max())), n
@@ -347,7 +354,9 @@ def test_tensor_core_attention_against_fp64(regime, models, monkeypatch):
         assert e_simt <= ar.fp32_att_bound(n, scale), row                             # the fp32 kernel on its own
         assert on_tc or np.array_equal(u["att0"], s["att0"]), n                        # past 1280 ids: the same kernel
         assert e_tc <= bound, row
-        if on_tc:
+        if not on_tc:
+            assert not u["p0"].any(), n
+        else:
             p0 = u["p0"]
             tz = (n + 31) // 32 * 32
             assert p0.shape[1] >= tz and not p0[:, n:tz].any(), n                    # zero-filled keys of the P.V K extent
