@@ -468,6 +468,20 @@ int32_t sb200_job_debug_fetch(sb200_job* job, const char* name, size_t b, float*
 void sb200_buffer_free(float* p);
 /* cumulative durations (int32 per id) of utterance b */
 int32_t sb200_job_debug_durations(sb200_job* job, size_t b, int32_t** cum, size_t* n, sb200_error* err);
+/* One stage of one chunk of sb200_debug_decode_chunks: rows x cols floats, time-major. */
+typedef struct sb200_chunk_capture {
+    char name[32];
+    size_t chunk;         /* index of the chunk in the call */
+    size_t rows, cols;
+    float* data;
+} sb200_chunk_capture;
+/* Test hook: sb200_decode_chunks' pass over chunks zs[k] frames [lo[k], hi[k]) with every decoder stage captured; the
+ * same kernels run and the waveforms are bit for bit that call's.  *caps receives *n_caps records, for each chunk in
+ * order: "z" (the latent rows the pass gathered, [hi - lo][inter]), "dec.pre", "dec.up<i>", "dec.mrf<i>" (the names,
+ * channel order and rows per frame of sb200_job_debug_fetch) and "wav" (the chunk's samples, one column).  Each holds
+ * the chunk's own (hi - lo) * U rows.  Records and data are one malloc'ed block: free *caps with free(). */
+int32_t sb200_debug_decode_chunks(sb200_voice* v, const sb200_latent* const* zs, const int64_t* lo, const int64_t* hi,
+                                  size_t n, sb200_chunk_capture** caps, size_t* n_caps, sb200_error* err);
 
 typedef struct sb200_region_stat {
     char name[32];

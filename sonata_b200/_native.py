@@ -36,6 +36,11 @@ class sb200_region_stat(C.Structure):
                 ("launches", C.c_int32)]
 
 
+class sb200_chunk_capture(C.Structure):
+    _fields_ = [("name", C.c_char * 32), ("chunk", C.c_size_t), ("rows", C.c_size_t), ("cols", C.c_size_t),
+                ("data", C.POINTER(C.c_float))]
+
+
 _P = C.c_void_p
 _ERR = C.POINTER(sb200_error)
 
@@ -152,6 +157,8 @@ SIGNATURES = {
     "sb200_buffer_free": (None, [C.POINTER(C.c_float)]),
     "sb200_job_debug_durations": (C.c_int32, [_P, C.c_size_t, C.POINTER(C.POINTER(C.c_int32)),
                                               C.POINTER(C.c_size_t), _ERR]),
+    "sb200_debug_decode_chunks": (C.c_int32, [_P, C.POINTER(_P), C.POINTER(C.c_int64), C.POINTER(C.c_int64), C.c_size_t,
+                                              C.POINTER(C.POINTER(sb200_chunk_capture)), C.POINTER(C.c_size_t), _ERR]),
     "sb200_job_profile": (C.c_int32, [_P, C.POINTER(sb200_region_stat), C.c_int32]),
     "sb200_debug_plan": (C.c_int32, [C.c_int32, C.c_int64, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
                                       C.c_int32, C.POINTER(C.c_int32)]),

@@ -737,6 +737,42 @@ int32_t sb200_job_debug_durations(sb200_job* job, size_t b, int32_t** cum, size_
         *n = len;
     });
 }
+int32_t sb200_debug_decode_chunks(sb200_voice* v, const sb200_latent* const* zs, const int64_t* lo, const int64_t* hi,
+                                  size_t n, sb200_chunk_capture** caps, size_t* n_caps, sb200_error* err) {
+    return guarded(err, [&] {
+        if (!caps || !n_caps) throw Error(19, "null argument");
+        *caps = nullptr; *n_caps = 0;
+        ChunkPass p = chunk_pass(zs, lo, hi, n);
+        p.debug = true;
+        ChunkResult r;
+        decode_chunks(v->v.get(), p, r);
+        if (n == 0) return;
+        // per chunk: the stages in order, then the waveform; records first, their data after them in the same block
+        const size_t per = r.captures.size() + 1, count = n * per;
+        size_t floats = 0;
+        for (size_t k = 0; k < n; k++) {
+            for (const ChunkCapture& c : r.captures) floats += c.rows[k].size();
+            floats += r.f32[k].size();
+        }
+        char* block = static_cast<char*>(malloc(count * sizeof(sb200_chunk_capture) + floats * 4 + 4));
+        if (!block) throw Error(19, "out of host memory");
+        sb200_chunk_capture* rec = reinterpret_cast<sb200_chunk_capture*>(block);
+        float* data = reinterpret_cast<float*>(block + count * sizeof(sb200_chunk_capture));
+        const auto put = [&](const std::string& name, size_t k, const std::vector<float>& x, size_t cols) {
+            memset(rec, 0, sizeof(*rec));
+            strncpy(rec->name, name.c_str(), sizeof(rec->name) - 1);
+            rec->chunk = k; rec->rows = x.size() / cols; rec->cols = cols; rec->data = data;
+            std::copy(x.begin(), x.end(), data);
+            data += x.size(); rec++;
+        };
+        for (size_t k = 0; k < n; k++) {
+            for (const ChunkCapture& c : r.captures) put(c.name, k, c.rows[k], (size_t)c.cols);
+            put("wav", k, r.f32[k], 1);
+        }
+        *caps = reinterpret_cast<sb200_chunk_capture*>(block);
+        *n_caps = count;
+    });
+}
 int32_t sb200_job_profile(const sb200_job* job, sb200_region_stat* out, int32_t cap) {
     const Job& j = *job->j;
     int32_t n = 0;

@@ -592,15 +592,18 @@ struct DecoderBufs {
         for (size_t i = 0; i < v.ups.size(); i++)
             stage[i] = {pool[2], pool[i & 1], pool[3], ntmp > 2 ? pool[4] : nullptr, ntmp > 2 ? pool[5] : nullptr};
     }
-    void expose_to(Job& j) const {
-        const Voice& v = *j.v;
-        expose(j, "dec.pre", p0, v.a.up_init, 1);
+    // f(name, buffer, columns, rows per frame) of every stage in order (with debug, each its own buffer)
+    template <typename F> void each_stage(const Voice& v, F&& f) const {
+        f("dec.pre", p0, v.a.up_init, 1);
         int U = 1;
         for (size_t i = 0; i < v.ups.size(); i++) {
             U *= v.ups[i].u;
-            expose(j, "dec.up" + std::to_string(i), stage[i][0], v.ups[i].cout, U);
-            expose(j, "dec.mrf" + std::to_string(i), stage[i][1], v.ups[i].cout, U);
+            f("dec.up" + std::to_string(i), stage[i][0], v.ups[i].cout, U);
+            f("dec.mrf" + std::to_string(i), stage[i][1], v.ups[i].cout, U);
         }
+    }
+    void expose_to(Job& j) const {
+        each_stage(*j.v, [&](const std::string& name, float* p, int cols, int U) { expose(j, name, p, cols, U); });
     }
 };
 
@@ -647,8 +650,9 @@ struct FrameBufs {
 };
 
 // One pass of streaming decoder chunks (layout l): speaker biases of every slot, tables, the gather table and the
-// latent slices, the decoder and the waveforms; the post-path table when an output stage runs, the resample launch's
-// tables and output, the i16 or G.711 scratch; and the pinned block the packed result (`total` values) is copied to.
+// latent slices, the decoder (one buffer per stage for a debug pass) and the waveforms; the post-path table when an
+// output stage runs, the resample launch's tables and output, the i16 or G.711 scratch; and the pinned block the packed
+// result (`total` values) is copied to.
 struct ChunkBufs {
     SpeakerBias spk;
     FrameTables y;
@@ -674,7 +678,7 @@ struct ChunkBufs {
         wav = dev.get<float>((size_t)l.total_samples + (size_t)pp.y_total + 4);
         pr.carve(dev, pin, pp, false);
         if (!pp.segs.empty()) { rin.carve(dev, pin, n); rpost.carve(dev, pin, n); }
-        dec.carve(dev, v, l.RY, false);
+        dec.carve(dev, v, l.RY, p.debug);
         if (p.resample || i16_out) post.carve(dev, pin, n);
         rt.carve(dev, pin, rp.segs.size());
         rs = p.resample ? dev.get<float>(total + 4) : nullptr;
@@ -1329,11 +1333,15 @@ static void fill_fade(PcmPost& p, int fade, long long len) {
 // which applies the post-path itself when no resample launch ran.  The packed result comes back in one copy through the
 // context's page-locked staging, and only then do the resamplers and prosody streams advance.
 void decode_chunks(Voice* v, const ChunkPass& p, ChunkResult& out) {
-    out.f32.clear(); out.i16.clear(); out.g711.clear(); out.ms = out.stretch_ms = out.pitch_ms = 0.f;
+    out.f32.clear(); out.i16.clear(); out.g711.clear(); out.captures.clear();
+    out.ms = out.stretch_ms = out.pitch_ms = 0.f;
     const size_t n = p.chunks.size();
     if (n == 0) return;
     if (p.format < PCM_F32 || p.format > PCM_ALAW)
         throw Error(19, "format " + std::to_string(p.format) + " is not 0 (f32), 1 (i16), 2 (mu-law) or 3 (A-law)");
+    if (p.debug && (p.format != PCM_F32 || p.resample))
+        throw Error(19, "a chunk pass with captures returns the decoder's f32 waveforms only: no resampling, prosody or "
+                        "PCM output");
     const int hop = v->a.hop();
     FrameLayout l;
     std::vector<int> len(n);
@@ -1505,6 +1513,20 @@ void decode_chunks(Voice* v, const ChunkPass& p, ChunkResult& out) {
         }
     }
     cudaEventElapsedTime(&out.ms, C.ev_begin, C.ev_end);
+    if (p.debug) {
+        // each chunk's rows of every stage, straight from the pass's own buffers (the stream has synchronised)
+        const auto capture = [&](const std::string& name, const float* src, int cols, int U) {
+            ChunkCapture c{name, cols, U, std::vector<std::vector<float>>(n)};
+            for (size_t k = 0; k < n; k++) {
+                const size_t r0 = (size_t)l.fsegs[k].off * U, nr = (size_t)len[k] * U;
+                c.rows[k].resize(nr * cols);
+                SB_CUDA(cudaMemcpy(c.rows[k].data(), src + r0 * cols, nr * cols * 4, cudaMemcpyDeviceToHost));
+            }
+            out.captures.push_back(std::move(c));
+        };
+        capture("z", b.s, v->a.inter, 1);
+        b.dec.each_stage(*v, capture);
+    }
 }
 
 namespace {

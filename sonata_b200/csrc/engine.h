@@ -439,13 +439,23 @@ struct ChunkSpec {
 // prosody streams.  i16: to_i16_vec (samples.rs:51-75) normalised to each emitted
 // chunk's own peak; mu-law / A-law: the G.711 bytes of those same i16 samples, from the same launches.  Every check runs
 // before any device work and any resampler changes; errors name the chunk, except with `single`, which keeps the
-// single-chunk entry point's messages.
+// single-chunk entry point's messages.  With `debug` the decoder keeps one buffer per stage and every stage is copied
+// out per chunk after the pass (ChunkResult::captures); the launches are the same.  Such a pass is format 0 without
+// `resample`.
 struct ChunkPass {
     std::vector<ChunkSpec> chunks;
     int fade = 0;
     bool resample = false;
     int format = 0;                       // PcmFormat: 0 f32, 1 i16, 2 mu-law, 3 A-law
     bool single = false;
+    bool debug = false;
+};
+// One stage of a debug chunk pass: "z" (the gathered latent rows), then the DecoderBufs::expose_to names; rows[k] is
+// chunk k's (hi - lo) * level rows of `cols` values, time-major.
+struct ChunkCapture {
+    std::string name;
+    int cols = 0, level = 1;
+    std::vector<std::vector<float>> rows;
 };
 struct ChunkResult {
     std::vector<std::vector<float>> f32;      // format 0
@@ -453,6 +463,7 @@ struct ChunkResult {
     std::vector<std::vector<uint8_t>> g711;   // formats 2 and 3
     float ms = 0;                             // the pass's device time
     float stretch_ms = 0, pitch_ms = 0;       // its "stretch" and "pitch" regions (0: none ran)
+    std::vector<ChunkCapture> captures;       // ChunkPass::debug only
 };
 void decode_chunks(Voice* v, const ChunkPass& p, ChunkResult& out);
 

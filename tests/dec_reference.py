@@ -44,6 +44,12 @@ POST_SLOPE = 0.01       # before conv_post (torch's default)
 #     dec.mrf{i}, ResBlock2         max |err| 5.6e-6 .. 1.1e-5   at most 0.33: 3.0x margin
 #     dec.mrf{i}, ResBlock1         max |err| 1.1e-5 .. 3.8e-5   at most 0.77 at mult 4 (high dec.mrf0, full size),
 #                                                                so mult 8 there: about 0.4, 2.5x margin
+# Streaming decoder chunk passes, same H100, held to the same bounds (tests/test_chunk_decoder_gpu.py -s): the edge pass
+# of each voice and backend (chunks of 1, 2, 127 .. 129, 180, 200 frames and whole latents of 290 .. 1030 frames) and
+# 32 chunks of 51 frames on medium, largest fraction of the bound on any tile of any chunk:
+#     dec.pre, dec.up{i}            max |err| 1.6e-5 .. 3.1e-5   at most 0.44
+#     dec.mrf{i}, ResBlock2         max |err| 5.5e-6 .. 9.3e-6   at most 0.34
+#     dec.mrf{i}, ResBlock1         max |err| 1.1e-5 .. 2.2e-5   at most 0.37 at mult 8
 # tests/test_flow_decoder_host.py shows each emulated kernel mistake at least 3x above this bound.
 TC_MULT = 4.0
 TC_MULT_RB1 = 8.0
@@ -55,7 +61,8 @@ TC_FLOOR = 2.0 ** -20
 # output (a blocked host GEMM accumulates more accurately than the CUDA-core kernels: conv_pre's 1344-term sums on
 # backend 0 measured 7x the error of torch's fp32 CPU conv).
 # Measured on the H100 above (same runs): max |err| 6.1e-7 .. 5.6e-6 on backend 0's stages and 4.9e-7 .. 1.0e-6 on the
-# waveform, at most 0.31 of the bound: 3.2x margin.
+# waveform, at most 0.31 of the bound: 3.2x margin.  Chunk passes (same runs as above): max |err| 5.4e-7 .. 4.7e-6 on
+# backend 0's stages, at most 0.31, and 4.8e-7 .. 6.0e-7 on the waveform, at most 0.23.
 F32_MULT = 4.0
 F32_FLOOR = 2.0 ** -21
 
@@ -329,6 +336,32 @@ def stages(T, sid=None):
         out.append((f"dec.mrf{i}", f"dec.up{i}", lambda x, ar, i=i: dec_mrf(T, i, x, ar)))
         prev = f"dec.mrf{i}"
     out.append(("wav", prev, lambda x, ar: dec_post(T, x, ar)))
+    return out
+
+
+def chunk_halo(T):
+    """{stage: (left, right)} for z and the decoder stages: how many rows at each edge of a chunk (a slice of a latent
+    decoded alone, every conv zero-padded at the slice's edges) may differ from the same rows of the whole latent
+    decoded at once, in the stage's own rows (frames x U).  The rows between them read only rows of the slice, at every
+    stage before them.  A centred conv of kernel k and dilation d adds d (k - 1) / 2 rows each side; a ConvTranspose of
+    stride u, kernel k and padding p = (k - u) / 2 turns h rows into h u + k - p - u on the left (output row o reads
+    input rows ceil((o + p - k + 1) / u) .. floor((o + p) / u)) and h u + p on the right; a stage's ResBlocks run side
+    by side, so the MRF adds the largest of their chains."""
+    a = arch(T)
+    out = {"z": (0, 0)}
+    h = (3, 3)                                           # conv_pre, k = 7
+    out["dec.pre"] = h
+    for i, (u, k) in enumerate(zip(a["up_rates"], a["up_kernels"])):
+        p = (k - u) // 2
+        h = (max(0, h[0] * u + k - p - u), h[1] * u + p)
+        out[f"dec.up{i}"] = h
+        grow = 0
+        for rk, rd in zip(a["res_kernels"], a["res_dils"]):
+            per = [d * (rk - 1) // 2 + ((rk - 1) // 2 if a["resblock"] == 1 else 0) for d in rd]
+            grow = max(grow, sum(per))
+        h = (h[0] + grow, h[1] + grow)
+        out[f"dec.mrf{i}"] = h
+    out["wav"] = (h[0] + 3, h[1] + 3)                    # conv_post, k = 7
     return out
 
 

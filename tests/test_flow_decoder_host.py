@@ -117,6 +117,46 @@ def test_bound_catches_xlow_padding_weight():
         src = f"flow.{f}"
 
 
+def _decoder_chain(t, z):
+    """The float64 decoder stages from z (dec.pre .. wav) on the CPU, as numpy."""
+    ar = dr.Arith("f64")
+    ar.dev = torch.device("cpu")           # one deterministic device, so equal inputs give equal bits
+    res = {"z": ar.t(z)}
+    for name, src, fn in dr.stages(t):
+        if not name.startswith("flow."):
+            res[name] = fn(res[src], ar)
+    return {k: dr._np(v) for k, v in res.items()}
+
+
+@pytest.mark.parametrize("voice", ["x_low", "high"])
+def test_chunk_halo_bounds_the_receptive_field(voice):
+    """dec_reference.chunk_halo against the float64 chain: z is changed outside a slice [lo, hi) of a 64-frame window,
+    and every row of every stage that chunk_halo calls interior to the slice keeps its bits; the row just past the halo
+    on either side (one row less of halo) changes at every stage, so the halo is also no larger than it must be.  The
+    changed rows are BIG times larger than z: the farthest rows reach a stage through one edge tap of every conv on the
+    way, and at z's own scale that contribution falls below float64 rounding by the high voice's dec.mrf3."""
+    BIG = 1e12
+    t = voicegen.make_tensors(voice)
+    a = dr.arch(t)
+    halo = dr.chunk_halo(t)
+    lo, hi, n = 16, 48, 64
+    rng = np.random.default_rng(11)
+    z = rng.standard_normal((n, a["inter"]))
+    z2 = z.copy()
+    z2[:lo] = BIG * rng.standard_normal((lo, a["inter"]))
+    z2[hi:] = BIG * rng.standard_normal((n - hi, a["inter"]))
+    r1, r2 = _decoder_chain(t, z), _decoder_chain(t, z2)
+    assert set(halo) == set(r1)
+    for name, (left, right) in halo.items():
+        U = r1[name].shape[0] // n
+        i0, i1 = lo * U + left, hi * U - right
+        assert i0 < i1, (voice, name, left, right)
+        assert np.array_equal(r1[name][i0:i1], r2[name][i0:i1]), (voice, name)
+        if name != "z":
+            assert not np.array_equal(r1[name][i0 - 1], r2[name][i0 - 1]), (voice, name, "left")
+            assert not np.array_equal(r1[name][i1], r2[name][i1]), (voice, name, "right")
+
+
 @pytest.mark.parametrize("voice", ["medium", "high"])
 def test_bound_catches_conv_post_edge_tap(voice):
     """conv_post dropping the taps that cross a 512-row block edge lands at least 3x above the fp32-class waveform bound."""

@@ -32,6 +32,7 @@ def test_struct_layouts_match_header():
     assert ctypes.sizeof(_native.sb200_synth_config) == 24
     assert ctypes.sizeof(_native.sb200_audio_info) == 12
     assert ctypes.sizeof(_native.sb200_region_stat) == 64
+    assert ctypes.sizeof(_native.sb200_chunk_capture) == 64
 
 
 # ---------------------------------------------------------------- config / id mapping (piper/src/lib.rs:112-250)
