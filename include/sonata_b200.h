@@ -229,6 +229,44 @@ int32_t sb200_speak_batch_ids_prosody(sb200_voice* v, const int64_t* ids_packed,
                                       const float* tempo, sb200_audio* outs, int32_t* id_frames_out, double* lufs_out,
                                       float* gain_out, sb200_error* err);
 
+/* ---- pitch contours: a pitch ratio per id, each id keeping its duration ----
+ * A contour gives each id of an utterance its own pitch ratio, packed like ids_packed: a finite value in [0.5, 2], or
+ * NaN or exactly 1 for none.  Every frequency in the samples an id produces is multiplied by its ratio, and with the
+ * utterance's tempo t (1 without one) each id lasts its unwarped length / t.  A contour combines with a tempo but not
+ * with the utterance's pitch ratio: an utterance with both fails with OPERATION_ERROR naming it, and a bad entry fails
+ * naming the utterance and the id, before any device work.  A contour of NaN / 1 only asks for nothing.  In double
+ * (Hs, N, D, the quantisation, the tie rule, the window and the sinc kernel as for sb200_speak_batch_ids_prosody), on
+ * the decoder's n = 256 T_y samples:
+ *  1. Pieces.  Id i covers input samples [256 C_{i-1}, 256 C_i) (C: cumulative frames).  Ids with 0 frames are dropped,
+ *     and runs of consecutive remaining ids with equal f32 ratios (NaN -> 1) merge into one piece: pieces r = 1 .. m with
+ *     0 = B_0 < .. < B_m = n and ratios p_r.  An utterance whose ids all have 0 frames is one piece with ratio 1.  One
+ *     piece is planned as the utterance ratio p_1 (so a uniform contour has the bits of that pitch ratio).
+ *  2. Stretch (skipped when every alpha_r = 1): alpha_r = (double)p_r / (double)t, S_0 = 0,
+ *     S_r = S_{r-1} + (B_r - B_{r-1}) * alpha_r, n1 = floor(S_m + 0.5), F = ceil(n1 / Hs).  Frame k lies in the piece
+ *     with S_{r-1} <= k Hs < S_r (the last piece: k Hs >= S_{m-1}) and a_k = floor(B_{r-1} + (k Hs - S_{r-1}) / alpha_r
+ *     + 0.5); the virtual frame -1 stays at -Hs.  The offsets and the overlap-add are those of the utterance ratios.
+ *  3. Pitch (skipped when every p_r = 1): Q_0 = 0, Q_r = Q_{r-1} + (S_r - S_{r-1}) / p_r for r < m,
+ *     n2 = floor(Q_{m-1} + (n1 - S_{m-1}) / p_m + 0.5).  Output j lies in the piece with Q_{r-1} <= j < Q_r (the last
+ *     one open-ended) at pos = S_{r-1} + (j - Q_{r-1}) * p_r, and y[j] = sum_i s[i] h_r(pos - i) over 0 <= i < n1 with
+ *     |pos - i| < W_r, c_r = min(1, 1 / p_r), W_r = 16 / c_r; phases in double, taps rounded to f32, one fmaf chain in
+ *     ascending i.
+ *  4. Delivered ends.  Id i, ending at input sample b with B_{r-1} < b <= B_r (r = 1 for b = 0), ends at
+ *     floor(Q_{r-1} + ((b - B_{r-1}) * alpha_r) / p_r + 0.5); the last id ends at n2.  With an output rate up / down a
+ *     delivered end beta is at ceil(beta * up / down) of the resampled signal, as frame boundaries are.
+ * Every expression is evaluated as written, each operation rounded (no fused multiply-add), so with one piece each one is
+ * the utterance-ratio formula.  With t = 1 every end but the last is the unwarped 256 C_i, and the last, n2, is within
+ * one sample of n.  Utterances without a contour get the same ends from the one piece of their ratios.
+ * sb200_speak_batch_ids_prosody with pitch_packed (NULL: none) the contours of the batch, packed like ids_packed, and
+ * bounds_out (NULL: not wanted) each id's delivered end before any output-rate resampling, packed like ids_packed.
+ * NULL pitch_packed and NULL bounds_out is that call, bit for bit. */
+int32_t sb200_speak_batch_ids_contour(sb200_voice* v, const int64_t* ids_packed, const size_t* offsets, size_t batch,
+                                      const sb200_synth_config* cfgs, const float* scale_packed,
+                                      const int32_t* frames_packed, const uint64_t* seeds, const int32_t* seeded,
+                                      const uint32_t* output_rates, const float* target_lufs, const float* pitch,
+                                      const float* tempo, const float* pitch_packed, sb200_audio* outs,
+                                      int32_t* id_frames_out, int64_t* bounds_out, double* lufs_out, float* gain_out,
+                                      sb200_error* err);
+
 /* ---- job API: the same batched pass split into its host<->device steps (bench / multi-GPU plumbing) ----
  * create  : copies ids to the device (H2D).  `eps_w` / `eps_z` optionally inject the graph's two
  *           RandomNormalLike draws (time-major: eps_w[b] = f32[T_x][2], eps_z[b] = f32[T_y][inter]);
@@ -282,6 +320,16 @@ int32_t sb200_job_set_prosody(sb200_job* job, const float* pitch, const float* t
 /* Each utterance's stretched length n1, delivered length before any output-rate resampling n2 and WSOLA frame count F of
  * the last run into n1[0 .. batch) / n2 / frames (each may be NULL).  Fails when that run had no ratios. */
 int32_t sb200_job_prosody(const sb200_job* job, int64_t* n1, int64_t* n2, int32_t* frames, sb200_error* err);
+/* A pitch contour (see sb200_speak_batch_ids_contour) for the next sb200_job_run, packed like ids_packed, or NULL for none
+ * (what a new job starts with; so is a contour that is all NaN or 1).  Checked like sb200_job_set_durations: a bad entry
+ * fails with OPERATION_ERROR naming the utterance and the id, and an utterance with a pitch ratio set by
+ * sb200_job_set_prosody fails naming the utterance; either leaves the job as it was.  A run with a contour copies the
+ * batch's cumulative durations to the host with the frame counts, and after it every result call reports the warped
+ * signal, as after a run with ratios. */
+int32_t sb200_job_set_pitch_contour(sb200_job* job, const float* pitch_packed, sb200_error* err);
+/* Each id's delivered end in the last run (see sb200_speak_batch_ids_contour), at the voice's rate, packed like
+ * ids_packed, into out_packed[0 .. capacity).  Fails before a run, or when capacity is smaller than the number of ids. */
+int32_t sb200_job_prosody_bounds(sb200_job* job, int64_t* out_packed, size_t capacity, sb200_error* err);
 /* Frames per id of the last run, packed like ids_packed, into out_packed[0 .. capacity): one device->host copy of the
  * whole batch's cumulative durations, made on the first call after a run.  Fails before a run, or when capacity is
  * smaller than the number of ids. */
@@ -579,6 +627,18 @@ int32_t sb200_debug_prosody_plan(int32_t rate, int64_t n, float pitch, float tem
 int32_t sb200_debug_prosody(int32_t device, const float* x, size_t n, int32_t rate, float pitch, float tempo, float* y,
                             size_t cap, int32_t* offsets, size_t offsets_cap, float* stretched, size_t stretched_cap,
                             sb200_error* err);
+/* Test hook, no device needed: the plan of a pitch contour (see sb200_speak_batch_ids_contour) over n samples at `rate`
+ * whose id i ends at input sample ends[i] (non-decreasing, the last one at n unless all are 0) with ratio ratios[i], and
+ * the tempo: shape6 receives Hs, N, D, n1, n2, F, positions[0 .. min(F, cap)) the a_k and bounds[0 .. n_ids) (NULL: not
+ * wanted) each id's delivered end.  Returns 0, or 19 for a bad ratio, tempo, end or rate. */
+int32_t sb200_debug_prosody_contour_plan(int32_t rate, int64_t n, const int64_t* ends, const float* ratios, size_t n_ids,
+                                         float tempo, int64_t* shape6, int64_t* positions, size_t cap, int64_t* bounds);
+/* The prosody kernels over one caller buffer x[0 .. n) with that contour: y[0 .. n2), offsets[0 .. F) and
+ * stretched[0 .. n1) as for sb200_debug_prosody, bit for bit what a job gives an utterance of those samples and ends. */
+int32_t sb200_debug_prosody_contour(int32_t device, const float* x, size_t n, int32_t rate, const int64_t* ends,
+                                    const float* ratios, size_t n_ids, float tempo, float* y, size_t cap,
+                                    int32_t* offsets, size_t offsets_cap, float* stretched, size_t stretched_cap,
+                                    sb200_error* err);
 /* Test hook, no device needed: the samples a prosody stream with these ratios at `rate` emits per chunk (the rule of
  * sb200_decode_chunks_warped) when its chunks bring chunk_lens[0 .. n_chunks) inputs and the last one ends it.
  * emitted[k] receives chunk k's count.  Returns 0, or 19 for bad ratios, a bad rate or a negative length. */

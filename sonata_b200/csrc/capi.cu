@@ -288,12 +288,13 @@ static void job_prosody(const Job& j, int64_t* n1, int64_t* n2, int32_t* frames)
     }
 }
 
-int32_t sb200_speak_batch_ids_prosody(sb200_voice* v, const int64_t* ids, const size_t* offsets, size_t batch,
+int32_t sb200_speak_batch_ids_contour(sb200_voice* v, const int64_t* ids, const size_t* offsets, size_t batch,
                                       const sb200_synth_config* cfgs, const float* scale_packed,
                                       const int32_t* frames_packed, const uint64_t* seeds, const int32_t* seeded,
                                       const uint32_t* output_rates, const float* target_lufs, const float* pitch,
-                                      const float* tempo, sb200_audio* outs, int32_t* id_frames_out, double* lufs_out,
-                                      float* gain_out, sb200_error* err) {
+                                      const float* tempo, const float* pitch_packed, sb200_audio* outs,
+                                      int32_t* id_frames_out, int64_t* bounds_out, double* lufs_out, float* gain_out,
+                                      sb200_error* err) {
     return guarded(err, [&] {
         const double t0 = now_ms();
         static_assert(sizeof(long long) == sizeof(int64_t), "");
@@ -304,6 +305,7 @@ int32_t sb200_speak_batch_ids_prosody(sb200_voice* v, const int64_t* ids, const 
                     resample_ratio(v->v->sample_rate, output_rates[b], "utterance " + std::to_string(b) + ": ");
         const bool loud = check_loudness_targets(target_lufs, batch);
         check_prosody(pitch, tempo, batch);
+        check_pitch_contour(pitch_packed, offsets, batch, pitch);
         std::unique_ptr<Job> j(create_job(v->v.get(), reinterpret_cast<const long long*>(ids), offsets, batch, nullptr,
                                           nullptr, nullptr, false));
         if (cfgs) set_job_configs(*j, cfgs_in(cfgs, batch).data());
@@ -312,17 +314,32 @@ int32_t sb200_speak_batch_ids_prosody(sb200_voice* v, const int64_t* ids, const 
         set_job_output_rates(*j, output_rates);
         set_job_loudness(*j, target_lufs);
         set_job_prosody(*j, pitch, tempo);
+        set_job_pitch_contour(*j, pitch_packed);
         j->run(nullptr, 0);
         fetch_audio(*j, outs, 0.f);
         if (id_frames_out) {
             const std::vector<int>& f = job_id_frames(*j);
             std::copy(f.begin(), f.end(), id_frames_out);
         }
+        if (bounds_out) {
+            const std::vector<long long> e = job_prosody_bounds(*j);
+            std::copy(e.begin(), e.end(), bounds_out);
+        }
         if (loud) job_loudness(*j, lufs_out, gain_out);
         const float wall = (float)(now_ms() - t0);
         for (size_t b = 0; b < batch; b++)
             outs[b].inference_ms = wall * (j->out_total ? (float)outs[b].len / (float)j->out_total : 0.f);
     });
+}
+int32_t sb200_speak_batch_ids_prosody(sb200_voice* v, const int64_t* ids, const size_t* offsets, size_t batch,
+                                      const sb200_synth_config* cfgs, const float* scale_packed,
+                                      const int32_t* frames_packed, const uint64_t* seeds, const int32_t* seeded,
+                                      const uint32_t* output_rates, const float* target_lufs, const float* pitch,
+                                      const float* tempo, sb200_audio* outs, int32_t* id_frames_out, double* lufs_out,
+                                      float* gain_out, sb200_error* err) {
+    return sb200_speak_batch_ids_contour(v, ids, offsets, batch, cfgs, scale_packed, frames_packed, seeds, seeded,
+                                         output_rates, target_lufs, pitch, tempo, nullptr, outs, id_frames_out, nullptr,
+                                         lufs_out, gain_out, err);
 }
 int32_t sb200_speak_batch_ids_loudness(sb200_voice* v, const int64_t* ids, const size_t* offsets, size_t batch,
                                        const sb200_synth_config* cfgs, const float* scale_packed,
@@ -419,6 +436,19 @@ int32_t sb200_job_set_prosody(sb200_job* job, const float* pitch, const float* t
 }
 int32_t sb200_job_prosody(const sb200_job* job, int64_t* n1, int64_t* n2, int32_t* frames, sb200_error* err) {
     return guarded(err, [&] { job_prosody(*job->j, n1, n2, frames); });
+}
+int32_t sb200_job_set_pitch_contour(sb200_job* job, const float* pitch_packed, sb200_error* err) {
+    return guarded(err, [&] { set_job_pitch_contour(*job->j, pitch_packed); });
+}
+int32_t sb200_job_prosody_bounds(sb200_job* job, int64_t* out_packed, size_t capacity, sb200_error* err) {
+    return guarded(err, [&] {
+        Job& j = *job->j;
+        if (!out_packed || capacity < j.ids.size())
+            throw Error(19, "prosody bounds: the destination holds " + std::to_string(capacity) + " entries, the job has " +
+                                std::to_string(j.ids.size()) + " ids");
+        const std::vector<long long> e = job_prosody_bounds(j);
+        std::copy(e.begin(), e.end(), out_packed);
+    });
 }
 int32_t sb200_job_id_frames(sb200_job* job, int32_t* out_packed, size_t capacity, sb200_error* err) {
     return guarded(err, [&] {
@@ -1092,6 +1122,70 @@ int32_t sb200_debug_prosody(int32_t device, const float* x, size_t n, int32_t ra
         SB_CUDA(cudaMemcpy(y, dy, (size_t)g.n2 * 4, cudaMemcpyDeviceToHost));
         if (offsets && g.F) SB_CUDA(cudaMemcpy(offsets, doff, (size_t)g.F * 4, cudaMemcpyDeviceToHost));
         // the stretched signal: the scratch when the pitch stage follows, else the result itself
+        if (stretched && g.stretch)
+            SB_CUDA(cudaMemcpy(stretched, g.pitch ? ds : dy, (size_t)g.n1 * 4, cudaMemcpyDeviceToHost));
+    });
+}
+
+int32_t sb200_debug_prosody_contour_plan(int32_t rate, int64_t n, const int64_t* ends, const float* ratios, size_t n_ids,
+                                         float tempo, int64_t* shape6, int64_t* positions, size_t cap, int64_t* bounds) {
+    try {
+        if (!shape6 || !ends || !ratios || n_ids == 0 || n <= 0) return 19;
+        const size_t offs[2] = {0, n_ids};
+        check_pitch_contour(ratios, offs, 1, nullptr);
+        check_prosody(nullptr, &tempo, 1);
+        std::vector<ContourPiece> pc;
+        const ProsodyShape s = prosody_contour_plan(rate, n, reinterpret_cast<const long long*>(ends), ratios, n_ids, NAN,
+                                                    tempo, pc, reinterpret_cast<long long*>(bounds));
+        const int64_t out[6] = {s.Hs, s.N, s.D, s.n1, s.n2, s.F};
+        std::copy(out, out + 6, shape6);
+        // the positions as the offset chain computes them, with the piece carried from frame to frame
+        for (int k = 0; positions && k < s.F && (size_t)k < cap; k++) {
+            if (pc.empty()) { positions[k] = prosody_analysis(s.Hs, s.alpha, k); continue; }
+            size_t r = 0;
+            while (r + 2 < pc.size() && (double)((long long)k * s.Hs) >= pc[r + 1].S) r++;
+            positions[k] = (long long)std::floor(pc[r].B + ((double)((long long)k * s.Hs) - pc[r].S) / pc[r].alpha + 0.5);
+        }
+        return 0;
+    } catch (const Error& e) {
+        return e.code;
+    }
+}
+
+int32_t sb200_debug_prosody_contour(int32_t device, const float* x, size_t n, int32_t rate, const int64_t* ends,
+                                    const float* ratios, size_t n_ids, float tempo, float* y, size_t cap,
+                                    int32_t* offsets, size_t offsets_cap, float* stretched, size_t stretched_cap,
+                                    sb200_error* err) {
+    return guarded(err, [&] {
+        if (!x || !y || !ends || !ratios || n_ids == 0 || n == 0 || n > (size_t)INT32_MAX)
+            throw Error(19, "debug prosody contour: bad arguments");
+        const size_t offs[2] = {0, n_ids};
+        check_pitch_contour(ratios, offs, 1, nullptr);
+        check_prosody(nullptr, &tempo, 1);
+        std::vector<ContourPiece> pc;
+        ProsodyPlan p;
+        p.add(prosody_contour_plan(rate, (long long)n, reinterpret_cast<const long long*>(ends), ratios, n_ids, NAN, tempo,
+                                   pc, nullptr),
+              0, (long long)n, &pc);
+        const ProsodySeg& g = p.segs[0];
+        if ((size_t)g.n2 > cap || (offsets && (size_t)g.F > offsets_cap) ||
+            (stretched && g.stretch && (size_t)g.n1 > stretched_cap))
+            throw Error(19, "debug prosody contour: a destination is too small for the result");
+        SB_CUDA(cudaSetDevice(device));
+        DeviceBuffers d;
+        const float* dx = d.upload(x, n, n);
+        const ProsodySeg* dg = d.upload(&g, 1, 1);
+        const ContourPiece* dpc = p.pieces.empty() ? nullptr : d.upload(p.pieces.data(), p.pieces.size(), p.pieces.size());
+        int* doff = d.alloc<int>((size_t)g.F + 1);
+        long long* dap = d.alloc<long long>((size_t)g.F + 1);
+        float* ds = d.alloc<float>((size_t)p.s_total + 4);
+        float* dy = d.alloc<float>((size_t)g.n2 + 4);
+        if (p.smem_ints) launch_prosody_offsets(dx, dg, 1, p.smem_ints, doff, 0, dpc, dap);
+        launch_prosody_ola(dx, dg, 1, p.max_ola, doff, ds, dy, 0, dap);
+        if (p.max_pitch) launch_prosody_pitch(dx, ds, dg, 1, p.max_pitch, dy, 0, dpc);
+        SB_CUDA(cudaDeviceSynchronize());
+        SB_CUDA(cudaMemcpy(y, dy, (size_t)g.n2 * 4, cudaMemcpyDeviceToHost));
+        if (offsets && g.F) SB_CUDA(cudaMemcpy(offsets, doff, (size_t)g.F * 4, cudaMemcpyDeviceToHost));
         if (stretched && g.stretch)
             SB_CUDA(cudaMemcpy(stretched, g.pitch ? ds : dy, (size_t)g.n1 * 4, cudaMemcpyDeviceToHost));
     });

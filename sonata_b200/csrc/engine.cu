@@ -261,10 +261,19 @@ void set_job_loudness(Job& j, const float* targets) {
 }
 
 void set_job_prosody(Job& j, const float* pitch, const float* tempo) {
-    if (!check_prosody(pitch, tempo, j.B)) { j.pitch.clear(); j.tempo.clear(); return; }
+    const bool any = check_prosody(pitch, tempo, j.B);
+    if (!j.contour.empty()) check_pitch_contour(j.contour.data(), j.offs.data(), j.B, pitch);
+    if (!any) { j.pitch.clear(); j.tempo.clear(); return; }
     const std::vector<float> none(j.B, NAN);
     j.pitch.assign(pitch ? pitch : none.data(), (pitch ? pitch : none.data()) + j.B);
     j.tempo.assign(tempo ? tempo : none.data(), (tempo ? tempo : none.data()) + j.B);
+}
+
+void set_job_pitch_contour(Job& j, const float* packed) {
+    if (check_pitch_contour(packed, j.offs.data(), j.B, j.pitch.empty() ? nullptr : j.pitch.data()))
+        j.contour.assign(packed, packed + j.ids.size());
+    else
+        j.contour.clear();
 }
 
 namespace {
@@ -399,6 +408,7 @@ struct IdBufs {
     Staged<int> xslot;                         // multi-speaker voices: speaker slot of every X granule
     SpeakerBias spk;
     int* cum;
+    int* cum_h;                                // pinned mirror of cum (only when the job has a pitch contour)
     float *xa, *xb, *qkv, *att, *ffn, *stats, *d0, *t1, *t2, *g, *h29, *zz, *logw;
     float *att_s, *att_vt, *att_orel;          // tensor-core attention: scores of every head, V^T, relative-value term
     float* epsw;
@@ -424,6 +434,7 @@ struct IdBufs {
         if (!j.frames.slot_sid.empty()) xslot.carve(dev, pin, nxg);
         spk.carve(dev, pin, v, j.frames);
         cum = dev.get<int>(RX);
+        cum_h = j.contour.empty() ? nullptr : pin.get<int>(RX);
         xa = rows(H); xb = rows(H); qkv = rows(3 * H); att = rows(H); ffn = rows(a.filter); stats = rows(2 * a.inter);
         d0 = rows(H); t1 = rows(H); t2 = rows(H); g = rows(H); h29 = rows(32); zz = rows(2); logw = rows(1);
         att_s = att_vt = att_orel = nullptr;
@@ -520,12 +531,18 @@ struct ResampleTables {
 // plan of stream windows the carry entry of every window and the staged input windows.
 struct ProsodyBufs {
     Staged<ProsodySeg> segs; Staged<FrameSeg> osegs; Staged<ProsodyCarry> carry;
+    Staged<ContourPiece> pieces;               // the contours' piece tables (only when a segment has one)
+    long long* apos = nullptr;                 // and their analysis positions, indexed like the offsets
     int* offsets = nullptr; float *x = nullptr, *s = nullptr, *y = nullptr;
     void carve(Arena& dev, Arena& pin, const ProsodyPlan& p, bool own_y) {
         const size_t n = p.segs.size();
         y = nullptr;
         if (n == 0) return;
         segs.carve(dev, pin, n);
+        if (!p.pieces.empty()) {
+            pieces.carve(dev, pin, p.pieces.size());
+            apos = dev.get<long long>((size_t)p.d_total);
+        }
         if (p.in_total) {
             carry.carve(dev, pin, n);
             x = dev.get<float>((size_t)p.in_total + 4);
@@ -544,6 +561,10 @@ struct ProsodyBufs {
         }
         segs.upload(st);
         if (osegs.d) osegs.upload(st);
+        if (pieces.d) {
+            std::copy(p.pieces.begin(), p.pieces.end(), pieces.h);
+            pieces.upload(st);
+        }
     }
 };
 
@@ -780,15 +801,36 @@ void lay_out_frames(FrameLayout& l, const std::vector<int>& y_len, int hop, cons
     l.RY = cur; l.total_samples = out;
 }
 
-// The prosody launches of a job whose utterances ask for a pitch or a tempo (an empty plan when none does): every
-// utterance's decoder waveform, with its ratios or NaN.
-ProsodyPlan lay_out_prosody(const Job& j, int hop) {
+// The prosody launches of a job whose utterances ask for a pitch, a tempo or a contour (an empty plan when none does):
+// every utterance's decoder waveform, with its ratios or NaN.  With a contour (cum: the batch's cum rows on the host),
+// every utterance is planned from its ids' ends, and bounds receives each id's delivered end, packed like the ids.
+ProsodyPlan lay_out_prosody(const Job& j, int hop, const std::vector<int>& cum, std::vector<long long>& bounds) {
     ProsodyPlan p;
-    if (j.pitch.empty() || j.encode_only) return p;
+    bounds.clear();
+    if ((j.pitch.empty() && j.contour.empty()) || j.encode_only) return p;
+    if (j.contour.empty()) {
+        for (size_t b = 0; b < j.B; b++) {
+            const FrameSeg& f = j.frames.fsegs[b];
+            const long long n = (long long)f.len * hop;
+            p.add(prosody_shape(j.v->sample_rate, n, j.pitch[b], j.tempo[b]), f.out_off, n);
+        }
+        return p;
+    }
+    bounds.resize(j.ids.size());
+    std::vector<long long> ends;
+    std::vector<ContourPiece> pieces;
     for (size_t b = 0; b < j.B; b++) {
         const FrameSeg& f = j.frames.fsegs[b];
         const long long n = (long long)f.len * hop;
-        p.add(prosody_shape(j.v->sample_rate, n, j.pitch[b], j.tempo[b]), f.out_off, n);
+        const size_t n_ids = j.offs[b + 1] - j.offs[b];
+        ends.resize(n_ids);
+        for (size_t i = 0; i < n_ids; i++) ends[i] = (long long)cum[j.xsegs[b].off + i] * hop;
+        const float* r = j.contour.data() + j.offs[b];
+        const bool has = std::any_of(r, r + n_ids, [](float v) { return !std::isnan(v) && v != 1.f; });
+        const float pitch = j.pitch.empty() ? NAN : j.pitch[b], tempo = j.tempo.empty() ? NAN : j.tempo[b];
+        const ProsodyShape sh = prosody_contour_plan(j.v->sample_rate, n, ends.data(), has ? r : nullptr, n_ids, pitch,
+                                                     tempo, pieces, bounds.data() + j.offs[b]);
+        p.add(sh, f.out_off, n, &pieces);
     }
     return p;
 }
@@ -836,13 +878,13 @@ void run_resample(Runner& R, const ResamplePlan& p, const ResampleTables& t, con
 void run_prosody(Runner& R, const ProsodyPlan& p, const ProsodyBufs& t, const float* wav, float* y) {
     const int n = (int)p.segs.size();
     R.begin("stretch");
-    if (p.smem_ints) launch_prosody_offsets(wav, t.segs.d, n, p.smem_ints, t.offsets, R.st);
-    launch_prosody_ola(wav, t.segs.d, n, p.max_ola, t.offsets, t.s, y, R.st);
+    if (p.smem_ints) launch_prosody_offsets(wav, t.segs.d, n, p.smem_ints, t.offsets, R.st, t.pieces.d, t.apos);
+    launch_prosody_ola(wav, t.segs.d, n, p.max_ola, t.offsets, t.s, y, R.st, t.apos);
     R.count(p.stretch_flops, p.stretch_bytes, p.smem_ints ? 2 : 1);
     R.end();
     if (p.max_pitch == 0) return;
     R.begin("pitch");
-    launch_prosody_pitch(wav, t.s, t.segs.d, n, p.max_pitch, y, R.st);
+    launch_prosody_pitch(wav, t.s, t.segs.d, n, p.max_pitch, y, R.st, t.pieces.d);
     R.count(p.pitch_flops, p.pitch_bytes);
     R.end();
 }
@@ -934,6 +976,25 @@ const std::vector<int>& job_id_frames(Job& j) {
     j.id_frames.resize(j.ids.size());
     for (size_t b = 0; b < j.B; b++) cum_to_frames(j, h, b, j.id_frames.data() + j.offs[b]);
     return j.id_frames;
+}
+
+std::vector<long long> job_prosody_bounds(Job& j) {
+    if (!j.ran) throw Error(19, "the job has not run");
+    if (!j.pros_bounds.empty()) return j.pros_bounds;
+    const std::vector<int>& f = job_id_frames(j);
+    std::vector<long long> out(j.ids.size()), ends;
+    std::vector<ContourPiece> pieces;
+    const int hop = j.v->a.hop();
+    for (size_t b = 0; b < j.B; b++) {
+        const size_t n_ids = j.offs[b + 1] - j.offs[b];
+        ends.resize(n_ids);
+        long long c = 0;
+        for (size_t i = 0; i < n_ids; i++) { c += f[j.offs[b] + i]; ends[i] = c * hop; }
+        prosody_contour_plan(j.v->sample_rate, (long long)std::max(c, 1ll) * hop, ends.data(), nullptr, n_ids,
+                             j.pitch_ran.empty() ? NAN : j.pitch_ran[b], j.tempo_ran.empty() ? NAN : j.tempo_ran[b],
+                             pieces, out.data() + j.offs[b]);
+    }
+    return out;
 }
 
 void Job::run(float* d_out, size_t d_out_cap) {
@@ -1156,8 +1217,10 @@ void Job::run(float* d_out, size_t d_out_cap) {
 
     // ---------------- host learns the frame counts (the graph's data-dependent shape) ----------------
     x.ylen.download(st);
+    if (x.cum_h) SB_CUDA(cudaMemcpyAsync(x.cum_h, x.cum, (size_t)RX * sizeof(int), cudaMemcpyDeviceToHost, st));
     SB_CUDA(cudaStreamSynchronize(st));
     y_len.assign(x.ylen.h, x.ylen.h + B);
+    const std::vector<int> cum_host = x.cum_h ? std::vector<int>(x.cum_h, x.cum_h + RX) : std::vector<int>();
     long long tot_frames = 0;
     for (int y : y_len) tot_frames += y;
     if (tot_frames > (long long)(2.0e9 / 256 / 4)) throw Error(19, "Failed to run model inference. Error: predicted durations are unreasonably long");
@@ -1169,12 +1232,13 @@ void Job::run(float* d_out, size_t d_out_cap) {
     // ---------------- frame level (phase 2) workspace ----------------
     // The stream is idle here, so the pinned staging of the X tables can be reused for the Y tables.
     lay_out_frames(frames, y_len, a.hop(), xsegs);
-    const ProsodyPlan pp = lay_out_prosody(*this, a.hop());
+    std::vector<long long> bounds;
+    const ProsodyPlan pp = lay_out_prosody(*this, a.hop(), cum_host, bounds);
     const bool prosody = !pp.segs.empty();
     const ResamplePlan rp = lay_out_output(*this, a.hop(), pp);
     const bool resample = !rp.segs.empty();
     const LoudnessPlan lp = lay_out_loudness(*this);
-    loud_ran.clear(); loud_lufs.clear(); loud_gain.clear(); pros_ran.clear();
+    loud_ran.clear(); loud_lufs.clear(); loud_gain.clear(); pros_ran.clear(); pros_bounds.clear();
     FrameBufs f;
     plan(C.dev_frame, C.pin, [&](Arena& dev, Arena& pin) { f.carve(dev, pin, *this, pp, rp, lp, d_out == nullptr); });
     d_osegs = resample ? f.rt.osegs.d : prosody ? f.pr.osegs.d : f.y.fsegs.d;
@@ -1267,6 +1331,8 @@ void Job::run(float* d_out, size_t d_out_cap) {
     SB_CUDA(cudaEventElapsedTime(&last_ms, C.ev_begin, C.ev_end));
     for (Region& r : regions) cudaEventElapsedTime(&r.ms, r.e0, r.e1);
     pros_ran = pp.shapes;
+    pros_bounds.swap(bounds);
+    pitch_ran = pitch; tempo_ran = tempo;
     if (!lp.segs.empty()) {
         loud_ran = loud_target;
         loud_lufs.assign(f.ld.lufs.h, f.ld.lufs.h + B);

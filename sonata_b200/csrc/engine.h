@@ -129,20 +129,35 @@ ProsodyShape prosody_shape(int rate, long long n, float pitch, float tempo);
 // Checks pitch[0 .. B) and tempo[0 .. B) (either may be null): NaN or 1 is none, anything else must be finite and in
 // [0.5, 2] (pitch) or [0.25, 4] (tempo), or the call fails naming the utterance.  Returns whether some utterance asks.
 bool check_prosody(const float* pitch, const float* tempo, size_t B);
+// Checks a pitch contour packed[0 .. offs[B]) of B utterances (utterance b: ids [offs[b], offs[b + 1])): NaN or 1 is
+// none, anything else must be finite and in [0.5, 2], and an utterance with a contour must not also have a pitch ratio
+// (pitch: one per utterance, or null), or the call fails naming the utterance (and the id).  Returns whether some
+// utterance has a contour.
+bool check_pitch_contour(const float* packed, const size_t* offs, size_t B, const float* pitch);
+// The plan of one utterance of n samples whose id i ends at input sample ends[i] (non-decreasing; the last one at n
+// unless every id is empty) with pitch ratio ratios[i] (NaN or 1: none; ratios null: the utterance ratio `pitch` for
+// every id) and the utterance's tempo (include/sonata_b200.h, sb200_speak_batch_ids_contour).  Returns the shape;
+// pieces receives the piece table and its sentinel when the ids make two or more pieces, and is emptied when they make
+// one, which is planned as the utterance ratio it equals.  bounds[0 .. n_ids) (may be null) receives each id's delivered
+// end.  Throws OPERATION_ERROR for bad ends, a rate without frame sizes or a result too long to index.
+ProsodyShape prosody_contour_plan(int rate, long long n, const long long* ends, const float* ratios, size_t n_ids,
+                                  float pitch, float tempo, std::vector<ContourPiece>& pieces, long long* bounds);
 // The three prosody launches over segments laid out back to back: each segment's ProsodySeg, the sizes of the offsets,
-// the stretched scratch and the output, what the launches are sized by and what the profile counts.
+// the stretched scratch and the output, what the launches are sized by and what the profile counts.  Segments with a
+// contour add their piece tables to `pieces`, and the plan then needs a d_total table of analysis positions.
 struct Voice;
 struct ProsodyStream;
 struct ProsodyStep;
 struct ProsodyPlan {
     std::vector<ProsodySeg> segs;
     std::vector<ProsodyShape> shapes;
+    std::vector<ContourPiece> pieces;
     long long s_total = 0, y_total = 0, d_total = 0, max_ola = 0, max_pitch = 0, steps = 0;
     long long in_total = 0, max_in = 0, max_keep = 0;     // streams: the input windows, the staging and carry sizes
     int smem_ints = 0;
     double stretch_flops = 0, stretch_bytes = 0, pitch_flops = 0, pitch_bytes = 0;
-    // Appends the segment wav[in_off, in_off + n) with shape `sh`.
-    void add(const ProsodyShape& sh, long long in_off, long long n);
+    // Appends the segment wav[in_off, in_off + n) with shape `sh` and, when it has one, its contour's piece table.
+    void add(const ProsodyShape& sh, long long in_off, long long n, const std::vector<ContourPiece>* contour = nullptr);
     // Appends stream ps's window for its chunk pass step t; its input window goes to wav[in_total ..) of the pass.
     void add_stream(const ProsodyStream& ps, const ProsodyStep& t);
 };
@@ -321,7 +336,11 @@ struct Job {
                                       // (set_job_loudness)
     std::vector<float> pitch, tempo;  // one ratio per utterance each, NaN = none; both empty when no utterance asks
                                       // (set_job_prosody)
+    std::vector<float> contour;       // per-id pitch ratios, packed like ids, NaN or 1 = none; empty when no utterance
+                                      // has a contour (set_job_pitch_contour)
     std::vector<ProsodyShape> pros_ran;   // each utterance's shape in the last run (empty: it ran no prosody stage)
+    std::vector<float> pitch_ran, tempo_ran;   // the ratios the last run had (empty: none)
+    std::vector<long long> pros_bounds;   // each id's delivered end in the last run when it had a contour (else empty)
     // Loudness of the last run: the targets it ran with (empty: it measured nothing), each utterance's integrated
     // loudness and the gain applied to it
     std::vector<float> loud_ran; std::vector<double> loud_lufs; std::vector<float> loud_gain;
@@ -385,6 +404,13 @@ void set_job_loudness(Job& j, const float* targets);
 // utterance's waveform is time-stretched and pitch-resampled right after the decoder, before any resampling and
 // loudness; see check_prosody for the checks.  A bad entry leaves the job's ratios as they were.
 void set_job_prosody(Job& j, const float* pitch, const float* tempo);
+// Per-id pitch ratios of the job's next run, packed like its ids (NaN or 1: none), or null for none; see
+// check_pitch_contour for the checks, which also refuse an utterance with a pitch ratio.  A bad entry leaves the job's
+// contour as it was.  Each utterance with a contour runs the prosody stage with its pieces (prosody_contour_plan).
+void set_job_pitch_contour(Job& j, const float* packed);
+// Each id's delivered end (prosody_contour_plan) in the job's last run, packed like its ids, at the voice's rate: kept
+// from the run when it had a contour, else computed from job_id_frames and the ratios it had.
+std::vector<long long> job_prosody_bounds(Job& j);
 // Frames per id of the job's last run, packed like its ids: one device->host copy of the batch's cum rows through the
 // context's page-locked staging, differenced on the host.  Cached until the next run.
 const std::vector<int>& job_id_frames(Job& j);

@@ -51,6 +51,86 @@ ProsodyShape prosody_shape(int rate, long long n, float pitch, float tempo) {
     return s;
 }
 
+bool check_pitch_contour(const float* packed, const size_t* offs, size_t B, const float* pitch) {
+    if (!packed) return false;
+    bool any = false;
+    for (size_t b = 0; b < B; b++) {
+        bool has = false;
+        for (size_t i = offs[b]; i < offs[b + 1]; i++) {
+            if (!prosody_asked(packed[i])) continue;
+            if (!(std::isfinite(packed[i]) && packed[i] >= 0.5f && packed[i] <= 2.f))
+                throw Error(19, "utterance " + std::to_string(b) + ", id " + std::to_string(i - offs[b]) +
+                                    ": pitch ratio " + std::to_string(packed[i]) +
+                                    " is not a finite value in [0.5, 2] (NaN or 1: none)");
+            has = true;
+        }
+        if (has && pitch && prosody_asked(pitch[b]))
+            throw Error(19, "utterance " + std::to_string(b) +
+                                ": a pitch contour and a pitch ratio together (give one or the other)");
+        any |= has;
+    }
+    return any;
+}
+
+// The pieces, their knots and the delivered ends, each expression evaluated in the order the header states it (the
+// host compiler does not contract them: no FMA for the default x86-64 target).
+ProsodyShape prosody_contour_plan(int rate, long long n, const long long* ends, const float* ratios, size_t n_ids,
+                                  float pitch, float tempo, std::vector<ContourPiece>& pieces, long long* bounds) {
+    struct Run { long long b0, b1; float p; };
+    std::vector<Run> runs;
+    const float p_utt = prosody_asked(pitch) ? pitch : 1.f;
+    long long prev = 0;
+    for (size_t i = 0; i < n_ids; i++) {
+        if (ends[i] < prev || ends[i] > n)
+            throw Error(19, "prosody contour: id " + std::to_string(i) + " ends at " + std::to_string(ends[i]) +
+                                ", before the id ahead of it or past the utterance's " + std::to_string(n) + " samples");
+        const float r = ratios ? (prosody_asked(ratios[i]) ? ratios[i] : 1.f) : p_utt;
+        if (ends[i] > prev) {
+            if (!runs.empty() && runs.back().p == r) runs.back().b1 = ends[i];
+            else runs.push_back(Run{prev, ends[i], r});
+        }
+        prev = ends[i];
+    }
+    if (runs.empty()) runs.push_back(Run{0, n, ratios ? 1.f : p_utt});
+    else if (prev != n) throw Error(19, "prosody contour: the last id ends at " + std::to_string(prev) + ", not at " +
+                                            std::to_string(n));
+    const size_t m = runs.size();
+    const double t = (double)(prosody_asked(tempo) ? tempo : 1.f);
+    std::vector<long long> B(m + 1, 0);
+    std::vector<double> S(m + 1, 0.0), Q(m, 0.0), al(m), pr(m);
+    for (size_t r = 0; r < m; r++) {
+        pr[r] = (double)runs[r].p; al[r] = pr[r] / t;
+        B[r + 1] = runs[r].b1;
+        S[r + 1] = S[r] + (double)(B[r + 1] - B[r]) * al[r];
+    }
+    for (size_t r = 0; r + 1 < m; r++) Q[r + 1] = Q[r] + (S[r + 1] - S[r]) / pr[r];
+    pieces.clear();
+    ProsodyShape sh;
+    if (m == 1) {
+        sh = prosody_shape(rate, n, runs[0].p, tempo);
+    } else {
+        sh = prosody_shape(rate, n, NAN, NAN);
+        sh.stretch = sh.pitch = true;
+        sh.alpha = 1.0; sh.p = *std::max_element(pr.begin(), pr.end());      // p: what the profile's tap count uses
+        const double n1 = std::floor(S[m] + 0.5);
+        const double n2 = std::floor(Q[m - 1] + (n1 - S[m - 1]) / pr[m - 1] + 0.5);
+        if (n1 > INT_MAX || n2 > INT_MAX) throw Error(19, "prosody: the stretched utterance is unreasonably long");
+        sh.n1 = (long long)n1; sh.n2 = (long long)n2;
+        sh.F = (int)((sh.n1 + sh.Hs - 1) / sh.Hs);
+        for (size_t r = 0; r < m; r++) pieces.push_back(ContourPiece{B[r], S[r], Q[r], al[r], pr[r]});
+        pieces.push_back(ContourPiece{n, INFINITY, INFINITY, 1.0, 1.0});
+    }
+    if (bounds) {
+        size_t r = 0;
+        for (size_t i = 0; i < n_ids; i++) {
+            while (ends[i] > B[r + 1]) r++;          // the piece with B_{r-1} < b <= B_r (the first one for b = 0)
+            bounds[i] = (long long)std::floor(Q[r] + ((double)(ends[i] - B[r]) * al[r]) / pr[r] + 0.5);
+        }
+        if (n_ids) bounds[n_ids - 1] = sh.n2;
+    }
+    return sh;
+}
+
 // ------------------------------------------------------------------ kernel 1: the offset chain
 // One block per segment walks its frames in order.  For frame k it stages q around where the previous frame would
 // continue (c = a_{k-1} + delta_{k-1} + Hs) and around a_k, every thread scores lags l, l + blockDim, .. as 64-bit
@@ -68,7 +148,8 @@ __device__ __forceinline__ bool pr_better(long long s1, int d1, long long s0, in
 }
 
 __global__ void __launch_bounds__(PR_THREADS)
-prosody_offsets_kernel(const float* __restrict__ wav, const ProsodySeg* __restrict__ segs, int* __restrict__ offsets) {
+prosody_offsets_kernel(const float* __restrict__ wav, const ProsodySeg* __restrict__ segs, int* __restrict__ offsets,
+                       const ContourPiece* __restrict__ pieces, long long* __restrict__ apos) {
     extern __shared__ int pq[];
     __shared__ long long ws[PR_THREADS / 32];
     __shared__ int wd[PR_THREADS / 32];
@@ -80,13 +161,30 @@ prosody_offsets_kernel(const float* __restrict__ wav, const ProsodySeg* __restri
     const int Hs = g.Hs, N = 2 * Hs, D = g.D, L = 2 * D + 1;
     int* ref = pq;
     int* cand = pq + N;
-    if (g.k0 == 0 && threadIdx.x == 0) out[0] = 0;
+    // a contour (whole utterances only): the piece of frame k is carried from frame to frame, and a_k goes to ap[k]
+    const ContourPiece* pc = g.c_n ? pieces + g.c_off : nullptr;
+    long long* ap = g.c_n ? apos + g.d_off : nullptr;
+    int r = 0;
+    if (g.k0 == 0 && threadIdx.x == 0) {
+        out[0] = 0;
+        if (pc) ap[0] = 0;
+    }
     // the frame before the first one computed: frame 0 (delta 0, at 0) or the last one an earlier pass computed
     const int k_first = max(g.k0, 1);
     long long a_prev = prosody_analysis(Hs, g.alpha, k_first - 1);
     int d_prev = k_first == 1 ? 0 : out[k_first - 1];
     for (int k = k_first; k < g.k1; k++) {
-        const long long a = prosody_analysis(Hs, g.alpha, k), c = a_prev + d_prev + Hs;
+        long long a;
+        if (pc) {
+            // a_k = floor(B + (k Hs - S) / alpha + 0.5) in the piece with S <= k Hs, every operation rounded as the host
+            const double kh = (double)((long long)k * Hs);
+            while (r + 1 < g.c_n && kh >= pc[r + 1].S) r++;
+            a = (long long)floor(__dadd_rn(__dadd_rn((double)pc[r].B, __ddiv_rn(__dsub_rn(kh, pc[r].S), pc[r].alpha)), 0.5));
+            if (threadIdx.x == 0) ap[k] = a;
+        } else {
+            a = prosody_analysis(Hs, g.alpha, k);
+        }
+        const long long c = a_prev + d_prev + Hs;
         for (int i = threadIdx.x; i < N; i += PR_THREADS) ref[i] = pr_quant(x, g.x0, g.n, c + i);
         for (int i = threadIdx.x; i < N + 2 * D; i += PR_THREADS) cand[i] = pr_quant(x, g.x0, g.n, a - D + i);
         __syncthreads();
@@ -121,7 +219,8 @@ prosody_offsets_kernel(const float* __restrict__ wav, const ProsodySeg* __restri
 __device__ __forceinline__ float pr_window(int i, int N) { return (float)(0.5 - 0.5 * cospi(2.0 * (double)i / (double)N)); }
 
 __global__ void prosody_ola_kernel(const float* __restrict__ wav, const ProsodySeg* __restrict__ segs,
-                                   const int* __restrict__ offsets, float* __restrict__ s, float* __restrict__ y) {
+                                   const int* __restrict__ offsets, float* __restrict__ s, float* __restrict__ y,
+                                   const long long* __restrict__ apos) {
     pdl_trigger(); pdl_wait();
     const ProsodySeg g = segs[blockIdx.y];
     const float* x = wav + g.in_off;
@@ -136,10 +235,13 @@ __global__ void prosody_ola_kernel(const float* __restrict__ wav, const ProsodyS
     const long long ob = g.pitch ? g.s0 : g.m0;
     const int* dl = offsets + g.d_off - g.d0;
     const int Hs = g.Hs, N = 2 * Hs;
+    const long long* ap = g.c_n ? apos + g.d_off : nullptr;      // a contour's analysis positions, from the offset chain
     for (long long m = g.m0 + i0; m < g.m1; m += step) {
         const int k = (int)(m / Hs), r = (int)(m - (long long)k * Hs);
-        const long long p1 = prosody_analysis(Hs, g.alpha, k) + dl[k] + r;
-        const long long p0 = prosody_analysis(Hs, g.alpha, k - 1) + (k > 0 ? dl[k - 1] : 0) + r + Hs;
+        const long long a1 = ap ? ap[k] : prosody_analysis(Hs, g.alpha, k);
+        const long long a0 = ap ? (k > 0 ? ap[k - 1] : -(long long)Hs) : prosody_analysis(Hs, g.alpha, k - 1);
+        const long long p1 = a1 + dl[k] + r;
+        const long long p0 = a0 + (k > 0 ? dl[k - 1] : 0) + r + Hs;
         const float x1 = p1 >= 0 && p1 < g.n ? x[p1 - g.x0] : 0.f, x0 = p0 >= 0 && p0 < g.n ? x[p0 - g.x0] : 0.f;
         out[m - ob] = __fadd_rn(__fmul_rn(pr_window(r, N), x1), __fmul_rn(pr_window(r + Hs, N), x0));
     }
@@ -150,11 +252,34 @@ __global__ void prosody_ola_kernel(const float* __restrict__ wav, const ProsodyS
 // h(u) = c sinc(c u) (0.42 + 0.5 cos(pi u / W) + 0.08 cos(2 pi u / W)), c = min(1, 1 / p), W = 16 / c.  The position j p
 // and the phases are double: sin(pi c u) and cos(pi u / W) are evaluated once at the first tap and rotated by the
 // constant per-tap angle after it; a tap is rounded to f32 as (sin(pi c u) * window) / (pi u).  A block stages the input
-// span of PP_OUTS consecutive outputs in shared memory.  The chain of output j depends on j, p and n1 alone.
+// span of PP_OUTS consecutive outputs in shared memory.  The chain of output j depends on j, p and n1 alone.  With a
+// contour, output j takes the position S + (j - Q) p of its piece and that piece's c, W and rotations, and the block
+// stages the union of its outputs' spans.
+__device__ __forceinline__ float pp_chain(const float* __restrict__ xs, long long lo, long long i0, long long i1,
+                                          double pos, double c, double W, double sdc, double cdc, double sdw,
+                                          double cdw) {
+    const double pi = 3.14159265358979323846;
+    double u = pos - (double)i0, su, cu, sw, cw;
+    sincospi(c * u, &su, &cu);
+    sincospi(u / W, &sw, &cw);
+    float acc = 0.f;
+    for (long long i = i0; i <= i1; i++) {
+        const double win = 0.42 + 0.5 * cw + 0.08 * (2.0 * cw * cw - 1.0);
+        const float h = u == 0.0 ? (float)(c * win) : (float)(su * win) / (float)(pi * u);
+        acc = fmaf(xs[i - lo], h, acc);
+        const double su2 = su * cdc - cu * sdc, sw2 = sw * cdw - cw * sdw;      // one tap on: u - 1
+        cu = cu * cdc + su * sdc; su = su2;
+        cw = cw * cdw + sw * sdw; sw = sw2;
+        u -= 1.0;
+    }
+    return acc;
+}
+
 __global__ void __launch_bounds__(PP_OUTS)
 prosody_pitch_kernel(const float* __restrict__ wav, const float* __restrict__ s, const ProsodySeg* __restrict__ segs,
-                     float* __restrict__ y) {
+                     float* __restrict__ y, const ContourPiece* __restrict__ pieces) {
     __shared__ float xs[PP_SPAN];
+    __shared__ long long span[2];
     pdl_trigger(); pdl_wait();
     const ProsodySeg g = segs[blockIdx.y];
     if (!g.pitch) return;
@@ -162,34 +287,55 @@ prosody_pitch_kernel(const float* __restrict__ wav, const float* __restrict__ s,
     const float* in = g.stretch ? s + g.s_off : wav + g.in_off;
     const long long ib = g.stretch ? g.s0 : g.x0;
     float* out = y + g.y_off - g.j0;
-    const double pi = 3.14159265358979323846, p = g.p, c = p > 1.0 ? 1.0 / p : 1.0, W = 16.0 / c;
-    double sdc, cdc, sdw, cdw;            // the per-tap rotations: pi c and pi / W
-    sincospi(c, &sdc, &cdc);
-    sincospi(1.0 / W, &sdw, &cdw);
+    if (g.c_n == 0) {
+        const double p = g.p, c = p > 1.0 ? 1.0 / p : 1.0, W = 16.0 / c;
+        double sdc, cdc, sdw, cdw;            // the per-tap rotations: pi c and pi / W
+        sincospi(c, &sdc, &cdc);
+        sincospi(1.0 / W, &sdw, &cdw);
+        for (long long a = g.j0 + (long long)blockIdx.x * PP_OUTS; a < g.j1; a += (long long)gridDim.x * PP_OUTS) {
+            const long long jb = min(a + (long long)PP_OUTS, g.j1);
+            const long long lo = max(0ll, (long long)floor((double)a * p - W) + 1);
+            const long long hi = min(g.n1 - 1, (long long)ceil((double)(jb - 1) * p + W) - 1);
+            for (int q = threadIdx.x; q <= (int)(hi - lo); q += PP_OUTS) xs[q] = in[lo + q - ib];
+            __syncthreads();
+            const long long j = a + threadIdx.x;
+            if (j < jb) {
+                const double pos = (double)j * p;
+                const long long i0 = max(lo, (long long)floor(pos - W) + 1), i1 = min(hi, (long long)ceil(pos + W) - 1);
+                out[j] = pp_chain(xs, lo, i0, i1, pos, c, W, sdc, cdc, sdw, cdw);
+            }
+            __syncthreads();
+        }
+        return;
+    }
+    const ContourPiece* pc = pieces + g.c_off;
     for (long long a = g.j0 + (long long)blockIdx.x * PP_OUTS; a < g.j1; a += (long long)gridDim.x * PP_OUTS) {
         const long long jb = min(a + (long long)PP_OUTS, g.j1);
-        const long long lo = max(0ll, (long long)floor((double)a * p - W) + 1);
-        const long long hi = min(g.n1 - 1, (long long)ceil((double)(jb - 1) * p + W) - 1);
+        // the piece of the block's first output (the last one with Q <= a), then each output's own
+        int r = 0;
+        for (int top = g.c_n - 1; r < top;) {
+            const int mid = (r + top + 1) / 2;
+            if (pc[mid].Q <= (double)a) r = mid; else top = mid - 1;
+        }
+        const long long j = a + threadIdx.x;
+        const bool live = j < jb;
+        if (live)
+            while ((double)j >= pc[r + 1].Q) r++;           // the sentinel's Q is +inf
+        const double p = pc[r].p, c = p > 1.0 ? 1.0 / p : 1.0, W = 16.0 / c;
+        const double pos = __dadd_rn(pc[r].S, __dmul_rn(__dsub_rn((double)j, pc[r].Q), p));
+        const long long i0 = max(0ll, (long long)floor(pos - W) + 1), i1 = min(g.n1 - 1, (long long)ceil(pos + W) - 1);
+        if (threadIdx.x == 0) { span[0] = LLONG_MAX; span[1] = LLONG_MIN; }
+        __syncthreads();
+        if (live) { atomicMin(&span[0], i0); atomicMax(&span[1], i1); }
+        __syncthreads();
+        const long long lo = span[0], hi = span[1];
         for (int q = threadIdx.x; q <= (int)(hi - lo); q += PP_OUTS) xs[q] = in[lo + q - ib];
         __syncthreads();
-        const long long j = a + threadIdx.x;
-        if (j < jb) {
-            const double pos = (double)j * p;
-            const long long i0 = max(lo, (long long)floor(pos - W) + 1), i1 = min(hi, (long long)ceil(pos + W) - 1);
-            double u = pos - (double)i0, su, cu, sw, cw;
-            sincospi(c * u, &su, &cu);
-            sincospi(u / W, &sw, &cw);
-            float acc = 0.f;
-            for (long long i = i0; i <= i1; i++) {
-                const double win = 0.42 + 0.5 * cw + 0.08 * (2.0 * cw * cw - 1.0);
-                const float h = u == 0.0 ? (float)(c * win) : (float)(su * win) / (float)(pi * u);
-                acc = fmaf(xs[i - lo], h, acc);
-                const double su2 = su * cdc - cu * sdc, sw2 = sw * cdw - cw * sdw;      // one tap on: u - 1
-                cu = cu * cdc + su * sdc; su = su2;
-                cw = cw * cdw + sw * sdw; sw = sw2;
-                u -= 1.0;
-            }
-            out[j] = acc;
+        if (live) {
+            double sdc, cdc, sdw, cdw;
+            sincospi(c, &sdc, &cdc);
+            sincospi(1.0 / W, &sdw, &cdw);
+            out[j] = pp_chain(xs, lo, i0, i1, pos, c, W, sdc, cdc, sdw, cdw);
         }
         __syncthreads();
     }
@@ -234,25 +380,27 @@ unsigned grid_for(long long n, int per_block) {
 }  // namespace
 
 void launch_prosody_offsets(const float* wav, const ProsodySeg* segs, int nseg, int smem_ints, int* offsets,
-                            cudaStream_t st) {
+                            cudaStream_t st, const ContourPiece* pieces, long long* apos) {
     if (nseg <= 0) return;
     const size_t smem = sizeof(int) * (size_t)smem_ints;
     if (smem > 48 * 1024) throw_launch_error("prosody: frame staging exceeds 48 KB of shared memory");
-    launch_pdl(prosody_offsets_kernel, dim3(nseg), dim3(PR_THREADS), smem, st, wav, segs, offsets);
+    launch_pdl(prosody_offsets_kernel, dim3(nseg), dim3(PR_THREADS), smem, st, wav, segs, offsets, pieces, apos);
     g_launch_count++;
 }
 
 void launch_prosody_ola(const float* wav, const ProsodySeg* segs, int nseg, long long max_out, const int* offsets,
-                        float* s, float* y, cudaStream_t st) {
+                        float* s, float* y, cudaStream_t st, const long long* apos) {
     if (nseg <= 0) return;
-    launch_pdl(prosody_ola_kernel, dim3(grid_for(max_out, 1024), nseg), dim3(256), 0, st, wav, segs, offsets, s, y);
+    launch_pdl(prosody_ola_kernel, dim3(grid_for(max_out, 1024), nseg), dim3(256), 0, st, wav, segs, offsets, s, y,
+               apos);
     g_launch_count++;
 }
 
 void launch_prosody_pitch(const float* wav, const float* s, const ProsodySeg* segs, int nseg, long long max_out, float* y,
-                          cudaStream_t st) {
+                          cudaStream_t st, const ContourPiece* pieces) {
     if (nseg <= 0) return;
-    launch_pdl(prosody_pitch_kernel, dim3(grid_for(max_out, PP_OUTS), nseg), dim3(PP_OUTS), 0, st, wav, s, segs, y);
+    launch_pdl(prosody_pitch_kernel, dim3(grid_for(max_out, PP_OUTS), nseg), dim3(PP_OUTS), 0, st, wav, s, segs, y,
+               pieces);
     g_launch_count++;
 }
 
@@ -273,8 +421,12 @@ void launch_prosody_carry(const float* wav, const float* s, const int* offsets, 
 }
 
 // ------------------------------------------------------------------ the launches of a plan
-void ProsodyPlan::add(const ProsodyShape& sh, long long in_off, long long n) {
+void ProsodyPlan::add(const ProsodyShape& sh, long long in_off, long long n, const std::vector<ContourPiece>* contour) {
     ProsodySeg g{};
+    if (contour && !contour->empty()) {
+        g.c_off = (int)pieces.size(); g.c_n = (int)contour->size() - 1;
+        pieces.insert(pieces.end(), contour->begin(), contour->end());
+    }
     g.in_off = in_off; g.n = n; g.n1 = sh.n1; g.n2 = sh.n2;
     g.F = sh.F; g.Hs = sh.Hs; g.D = sh.D; g.stretch = sh.stretch; g.pitch = sh.pitch; g.alpha = sh.alpha; g.p = sh.p;
     g.k1 = sh.F; g.m1 = sh.n1; g.j1 = sh.n2;      // the whole utterance: every other window field 0

@@ -10,8 +10,8 @@ import numpy as np
 
 from . import _native as N
 from .core import G711_LAW, Audio, OperationError, check_encoding
-from .piper import (_check, _config_array, _duration_arrays, _gain_array, _loudness_array, _prosody_arrays, _ptr,
-                    _rate_array, _seed_arrays, _take_audio, _take_bytes)
+from .piper import (_check, _config_array, _contour_arrays, _duration_arrays, _gain_array, _loudness_array,
+                    _prosody_arrays, _ptr, _rate_array, _seed_arrays, _take_audio, _take_bytes)
 
 
 class SynthesisJob:
@@ -19,11 +19,11 @@ class SynthesisJob:
                  eps_z: Optional[Sequence] = None, debug: bool = False, configs: Optional[Sequence] = None,
                  seeds: Optional[Sequence] = None, output_rates: Optional[Sequence] = None,
                  loudness: Optional[Sequence] = None, pitches: Optional[Sequence] = None,
-                 tempos: Optional[Sequence] = None):
+                 tempos: Optional[Sequence] = None, pitch_contours: Optional[Sequence] = None):
         """`configs`: one PiperSynthesisConfig per utterance (see set_configs); None keeps the voice's fallback config.
         `seeds`: noise seeds (see set_seeds).  `output_rates`: output sample rates (see set_output_rates).
         `loudness`: loudness targets (see set_loudness).  `pitches` / `tempos`: pitch and tempo ratios (see
-        set_prosody)."""
+        set_prosody).  `pitch_contours`: per-id pitch ratios (see set_pitch_contours)."""
         self._m = model
         self._lib = model._lib
         n = len(batches)
@@ -33,7 +33,7 @@ class SynthesisJob:
         _seed_arrays(seeds, n)
         _rate_array(output_rates, n)
         _loudness_array(loudness, n)
-        _prosody_arrays(pitches, tempos, n)
+        _contour_arrays(self._lens, pitch_contours, _prosody_arrays(pitches, tempos, n)[0])
         packed = np.ascontiguousarray(np.concatenate([np.asarray(b, dtype=np.int64) for b in batches]))
         offs = np.zeros(n + 1, dtype=np.uint64)
         offs[1:] = np.cumsum([len(b) for b in batches])
@@ -74,6 +74,8 @@ class SynthesisJob:
             self.set_loudness(loudness)
         if pitches is not None or tempos is not None:
             self.set_prosody(pitches, tempos)
+        if pitch_contours is not None:
+            self.set_pitch_contours(pitch_contours)
 
     def set_configs(self, configs: Optional[Sequence]) -> None:
         """Per-utterance PiperSynthesisConfigs for the next run, or None for the voice's fallback config.  A wrong
@@ -145,6 +147,26 @@ class SynthesisJob:
         _check(self._lib.sb200_job_prosody(self._h, _ptr(n1, C.c_int64), _ptr(n2, C.c_int64), _ptr(frames, C.c_int32),
                                            C.byref(err)), err)
         return n1, n2, frames
+
+    def set_pitch_contours(self, contours: Optional[Sequence]) -> None:
+        """Per-id pitch ratios for the next run (see VitsModel.infer_batch_with_values): contours[b] holds one ratio per
+        id of utterance b, or is None; None for the whole list, or ratios that are all None / NaN / 1.0, turn contours
+        off.  A contour combines with the job's tempos and not with its pitch ratios.  After a run with a contour the
+        results report the warped signal, as after set_prosody, and prosody_bounds gives each id's delivered end.  A bad
+        entry raises OperationError naming the utterance and the id, and leaves the job's contours as they were."""
+        c = _contour_arrays(self._lens, contours)
+        err = N.sb200_error()
+        _check(self._lib.sb200_job_set_pitch_contour(self._h, _ptr(c, C.c_float), C.byref(err)), err)
+
+    def prosody_bounds(self) -> List[np.ndarray]:
+        """Each id's delivered end in the last run, at the voice's rate, one int64 array per utterance (see
+        sb200_job_prosody_bounds)."""
+        total = int(sum(self._lens))
+        out = np.zeros(total, np.int64)
+        err = N.sb200_error()
+        _check(self._lib.sb200_job_prosody_bounds(self._h, _ptr(out, C.c_int64), total, C.byref(err)), err)
+        offs = np.concatenate([[0], np.cumsum(self._lens)]).astype(int)
+        return [out[offs[b]:offs[b + 1]].copy() for b in range(self.batch)]
 
     def id_frames(self) -> List[np.ndarray]:
         """Frames per id of the last run, one int32 array per utterance (one device->host copy for the batch)."""

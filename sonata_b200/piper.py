@@ -207,6 +207,49 @@ def _prosody_arrays(pitches, tempos, n: int):
     return _ratio_array(pitches, n, "pitch", *PITCH_RANGE), _ratio_array(tempos, n, "tempo", *TEMPO_RANGE)
 
 
+def _contour_value(x, b: int, i: int, unit: str = "id") -> float:
+    if x is None:
+        return math.nan
+    if isinstance(x, bool) or not isinstance(x, numbers.Real):
+        raise OperationError(f"utterance {b}, {unit} {i}: pitch ratio {x!r} is not a number")
+    x = float(x)
+    if not (math.isnan(x) or x == 1.0 or (math.isfinite(x) and PITCH_RANGE[0] <= x <= PITCH_RANGE[1])):
+        raise OperationError(f"utterance {b}, {unit} {i}: pitch ratio {x} is not a finite value in "
+                             f"[{PITCH_RANGE[0]}, {PITCH_RANGE[1]}] (NaN or 1: none)")
+    return x
+
+
+def _contour_arrays(lens: Sequence[int], pitch_contours=None, pitches=None):
+    """The packed C image of per-id pitch ratios (f32, NaN for none), checked as the library checks them, or None when
+    not given or when no utterance has a contour.  pitch_contours[b] holds one ratio per id of utterance b (in
+    PITCH_RANGE, or None / NaN / 1.0 for none), or is None.  An utterance with a contour may not also have a pitch ratio
+    in `pitches` (the C image of _prosody_arrays, or None).  Numeric arrays are checked in one vectorised pass; anything
+    else element by element, which also names the first bad element."""
+    if pitch_contours is None:
+        return None
+    n = len(lens)
+    out = np.full(int(sum(lens)), np.nan, np.float32)
+    pos = 0
+    for b, v in enumerate(_per_utterance(pitch_contours, n, "pitch contours")):
+        if v is not None:
+            a = _numeric(v, "fiu")
+            if a is None:
+                v = list(v)
+                a = np.array([_contour_value(x, b, i) for i, x in enumerate(v)] if len(v) == lens[b] else v)
+            if a.size != lens[b]:
+                raise OperationError(f"utterance {b}: {a.size} pitch ratios for {lens[b]} ids")
+            f = a.astype(np.float32)
+            asked = ~np.isnan(f) & (f != 1)
+            bad = np.nonzero(asked & ~(np.isfinite(f) & (f >= PITCH_RANGE[0]) & (f <= PITCH_RANGE[1])))[0]
+            if bad.size:
+                _contour_value(float(f[bad[0]]), b, int(bad[0]))
+            if asked.any() and pitches is not None and not np.isnan(pitches[b]):
+                raise OperationError(f"utterance {b}: a pitch contour and a pitch ratio together (give one or the other)")
+            out[pos:pos + lens[b]] = f
+        pos += lens[b]
+    return None if (np.isnan(out) | (out == 1)).all() else out
+
+
 def _prosody_kwargs(pitches, tempos) -> dict:
     out = {} if pitches is None else {"pitches": pitches}
     if tempos is not None:
@@ -260,14 +303,17 @@ def _ptr(a, ctype):
 
 
 def _alignment(phonemes: str, src_char: Sequence[int], frames: Sequence[int], n_samples: int,
-               up: int = 1, down: int = 1, warped: bool = False) -> List[PhonemeAlignment]:
+               up: int = 1, down: int = 1, warped: bool = False,
+               bounds: Optional[Sequence[int]] = None) -> List[PhonemeAlignment]:
     """Groups per-id frame counts by the character each id came from: bos (`^`), one entry per kept character (its id
     and its pad) and eos (`$`), contiguous from sample 0.  An utterance whose ids all got 0 frames is still one frame
     long; that frame (after every id) goes to the last entry, so the entries always end at n_samples.  Audio resampled
     by up/down puts the boundary after F frames at ceil(F * hop * up / down).  `warped` (a pitch or tempo ratio changed
     the length): the boundary after F of the utterance's T frames is at floor(F * n_samples / T + 0.5), whatever the
     output rate; the time stretch moves a sample by at most D = rate // 160 input samples from that linear map, so a
-    boundary is accurate to within D / tempo samples of the warped signal."""
+    boundary is accurate to within D / tempo samples of the warped signal.  `bounds` (a pitch contour): each id's
+    delivered end at the voice's rate (sb200_speak_batch_ids_contour); an entry ends where its last id does, at
+    ceil(end * up / down)."""
     total = int(sum(int(f) for f in frames))
     hop = n_samples // max(total, 1) if (up, down) == (1, 1) else HOP
     at = lambda frames_before: -((-frames_before * hop * up) // down)
@@ -283,7 +329,7 @@ def _alignment(phonemes: str, src_char: Sequence[int], frames: Sequence[int], n_
             j += 1
         ph = phonemes[src] if src >= 0 else ("^" if i == 0 else "$")
         fsum += f
-        end = at(fsum)
+        end = at(fsum) if bounds is None else -((-int(bounds[j - 1]) * up) // down)
         out.append(PhonemeAlignment(ph, start, end - start))
         start = end
         i = j
@@ -460,11 +506,13 @@ class _VitsCommons:
     def speak_batch(self, phoneme_batches: Sequence[str],
                     configs: Optional[Sequence[PiperSynthesisConfig]] = None, seeds: Optional[Sequence] = None,
                     output_rates: Optional[Sequence] = None, loudness: Optional[Sequence] = None,
-                    pitches: Optional[Sequence] = None, tempos: Optional[Sequence] = None) -> List[Audio]:
+                    pitches: Optional[Sequence] = None, tempos: Optional[Sequence] = None,
+                    pitch_contours: Optional[Sequence] = None) -> List[Audio]:
         """`configs`: one PiperSynthesisConfig per utterance (speaker and scales), still synthesised as one pass;
         None uses the fallback config for every utterance.  `seeds`: noise seeds as for infer_batch_with_values.
         `output_rates` / `loudness` / `pitches` / `tempos`: per-utterance output sample rates, loudness targets and
-        pitch and tempo ratios as for infer_batch_with_values."""
+        pitch and tempo ratios as for infer_batch_with_values.  `pitch_contours`: as for speak_batch_with_alignment,
+        one ratio per phoneme character."""
         n = len(phoneme_batches)
         _config_array(configs, n)             # argument errors before any id mapping
         sv, _ = _seed_arrays(seeds, n)
@@ -473,6 +521,11 @@ class _VitsCommons:
         pros = any(a is not None for a in _prosody_arrays(pitches, tempos, n))
         if n == 0:
             return []
+        if pitch_contours is not None:
+            return [a for a, _ in self.speak_batch_with_alignment(phoneme_batches, configs, seeds=seeds,
+                                                                  output_rates=output_rates, loudness=loudness,
+                                                                  pitches=pitches, tempos=tempos,
+                                                                  pitch_contours=pitch_contours)]
         if configs is not None or sv is not None or rates is not None or loud is not None or pros:
             extra = {} if sv is None else {"seeds": seeds}
             if pros:
@@ -502,7 +555,8 @@ class _VitsCommons:
                                 seeds: Optional[Sequence] = None,
                                 output_rates: Optional[Sequence] = None,
                                 loudness: Optional[Sequence] = None, pitches: Optional[Sequence] = None,
-                                tempos: Optional[Sequence] = None) -> List[Audio]:
+                                tempos: Optional[Sequence] = None,
+                                pitch_contours: Optional[Sequence] = None) -> List[Audio]:
         """Batched infer_with_values.  `configs`: one PiperSynthesisConfig per utterance (speaker and scales), or None
         for the fallback config; each utterance's result equals a single-utterance call with its config as the
         fallback, except for the on-device noise of an unseeded utterance, whose draws depend on the batch position.
@@ -525,17 +579,27 @@ class _VitsCommons:
         len / t samples), keeping the model's articulation where a small length_scale would ask the duration predictor
         for durations it never saw.  Both are signal processing on the decoder's waveform on the device (WSOLA, then a
         windowed-sinc resampler; sb200_speak_batch_ids_prosody), before any resampling and loudness; None, NaN or 1.0
-        leaves the utterance's samples as they are, bit for bit."""
+        leaves the utterance's samples as they are, bit for bit.
+
+        `pitch_contours`: one pitch ratio per id for each utterance (in PITCH_RANGE, or None / NaN / 1.0 for none), or
+        None.  Each id's samples are shifted by its own ratio and the id keeps its duration (divided by the utterance's
+        tempo, which a contour combines with; an utterance's pitch ratio does not).  A contour whose ratio is the same
+        on every id gives the bits of that pitch ratio (sb200_speak_batch_ids_contour)."""
         n = len(batches)
         cfgs = _config_array(configs, n)
         sv, _ = _seed_arrays(seeds, n)
         rates = _rate_array(output_rates, n)
         loud = _loudness_array(loudness, n)
-        pros = any(a is not None for a in _prosody_arrays(pitches, tempos, n))
-        if sv is not None or rates is not None or loud is not None or pros:
+        pit, tem = _prosody_arrays(pitches, tempos, n)
+        pros = pit is not None or tem is not None
+        contour = _contour_arrays([len(b) for b in batches], pitch_contours, pit)
+        if sv is not None or rates is not None or loud is not None or pros or contour is not None:
+            extra = _prosody_kwargs(pitches, tempos) if pros else {}
+            if contour is not None:
+                extra["pitch_contours"] = pitch_contours
             return [a for a, _ in self.infer_batch_with_durations(batches, configs, seeds=seeds,
                                                                   output_rates=output_rates, loudness=loudness,
-                                                                  **(_prosody_kwargs(pitches, tempos) if pros else {}))]
+                                                                  **extra)]
         packed = np.ascontiguousarray(np.concatenate([np.asarray(b, dtype=np.int64) for b in batches]))
         offs = np.zeros(n + 1, dtype=np.uint64)
         offs[1:] = np.cumsum([len(b) for b in batches])
@@ -553,7 +617,8 @@ class _VitsCommons:
                                    seeds: Optional[Sequence] = None,
                                    output_rates: Optional[Sequence] = None,
                                    loudness: Optional[Sequence] = None, pitches: Optional[Sequence] = None,
-                                   tempos: Optional[Sequence] = None) -> List[Tuple[Audio, np.ndarray]]:
+                                   tempos: Optional[Sequence] = None,
+                                   pitch_contours: Optional[Sequence] = None) -> List[Tuple[Audio, np.ndarray]]:
         """infer_batch_with_values with per-id duration control, returning (audio, frames per id) per utterance.
 
         duration_scales[b]: one scale (finite, >= 0) per id of utterance b, applied before the duration's ceil, so 1.0
@@ -561,8 +626,14 @@ class _VitsCommons:
         Either list, or any of its entries, may be None.  The frame counts times 256 are each id's samples; an
         utterance whose ids all got 0 frames is still one frame long.  `seeds`: as for infer_batch_with_values; a
         seeded frame's noise depends on its index only, so controls that move frames never reshuffle it.
-        `output_rates` / `loudness` / `pitches` / `tempos`: as for infer_batch_with_values (the frame counts stay frame
-        counts of the utterance before any warp)."""
+        `output_rates` / `loudness` / `pitches` / `tempos` / `pitch_contours`: as for infer_batch_with_values (the
+        frame counts stay frame counts of the utterance before any warp)."""
+        return [(a, f) for a, f, _ in self._speak_ids(batches, configs, duration_scales, durations, seeds, output_rates,
+                                                       loudness, pitches, tempos, pitch_contours)]
+
+    def _speak_ids(self, batches, configs, duration_scales, durations, seeds, output_rates, loudness, pitches, tempos,
+                   pitch_contours) -> List[Tuple[Audio, np.ndarray, Optional[np.ndarray]]]:
+        """infer_batch_with_durations with each id's delivered end (None without a contour) per utterance."""
         n = len(batches)
         cfgs = _config_array(configs, n)
         lens = [len(b) for b in batches]
@@ -571,6 +642,7 @@ class _VitsCommons:
         rates = _rate_array(output_rates, n)
         loud = _loudness_array(loudness, n)
         pit, tem = _prosody_arrays(pitches, tempos, n)
+        contour = _contour_arrays(lens, pitch_contours, pit)
         if n == 0:
             return []
         if any(x == 0 for x in lens):
@@ -581,12 +653,23 @@ class _VitsCommons:
         outs = (N.sb200_audio * n)()
         id_frames = np.zeros(int(offs[-1]), np.int32)
         err = N.sb200_error()
-        _check(self._lib.sb200_speak_batch_ids_prosody(
-            self._h, packed.ctypes.data_as(C.POINTER(C.c_int64)), offs.ctypes.data_as(C.POINTER(C.c_size_t)), n, cfgs,
-            _ptr(scales, C.c_float), _ptr(frames, C.c_int32), _ptr(sv, C.c_uint64), _ptr(sf, C.c_int32),
-            _ptr(rates, C.c_uint32), _ptr(loud, C.c_float), _ptr(pit, C.c_float), _ptr(tem, C.c_float), outs,
-            _ptr(id_frames, C.c_int32), None, None, C.byref(err)), err)
-        return [(_take_audio(outs[b]), id_frames[int(offs[b]):int(offs[b + 1])].copy()) for b in range(n)]
+        bounds = None
+        if contour is None:
+            _check(self._lib.sb200_speak_batch_ids_prosody(
+                self._h, packed.ctypes.data_as(C.POINTER(C.c_int64)), offs.ctypes.data_as(C.POINTER(C.c_size_t)), n,
+                cfgs, _ptr(scales, C.c_float), _ptr(frames, C.c_int32), _ptr(sv, C.c_uint64), _ptr(sf, C.c_int32),
+                _ptr(rates, C.c_uint32), _ptr(loud, C.c_float), _ptr(pit, C.c_float), _ptr(tem, C.c_float), outs,
+                _ptr(id_frames, C.c_int32), None, None, C.byref(err)), err)
+        else:
+            bounds = np.zeros(int(offs[-1]), np.int64)
+            _check(self._lib.sb200_speak_batch_ids_contour(
+                self._h, packed.ctypes.data_as(C.POINTER(C.c_int64)), offs.ctypes.data_as(C.POINTER(C.c_size_t)), n,
+                cfgs, _ptr(scales, C.c_float), _ptr(frames, C.c_int32), _ptr(sv, C.c_uint64), _ptr(sf, C.c_int32),
+                _ptr(rates, C.c_uint32), _ptr(loud, C.c_float), _ptr(pit, C.c_float), _ptr(tem, C.c_float),
+                _ptr(contour, C.c_float), outs, _ptr(id_frames, C.c_int32), _ptr(bounds, C.c_int64), None, None,
+                C.byref(err)), err)
+        cut = lambda a, b: None if a is None else a[int(offs[b]):int(offs[b + 1])].copy()
+        return [(_take_audio(outs[b]), cut(id_frames, b), cut(bounds, b)) for b in range(n)]
 
     def speak_batch_with_alignment(self, phoneme_batches: Sequence[str],
                                    configs: Optional[Sequence[PiperSynthesisConfig]] = None,
@@ -594,7 +677,8 @@ class _VitsCommons:
                                    seeds: Optional[Sequence] = None,
                                    output_rates: Optional[Sequence] = None,
                                    loudness: Optional[Sequence] = None, pitches: Optional[Sequence] = None,
-                                   tempos: Optional[Sequence] = None) -> List[Tuple[Audio, List[PhonemeAlignment]]]:
+                                   tempos: Optional[Sequence] = None, pitch_contours: Optional[Sequence] = None
+                                   ) -> List[Tuple[Audio, List[PhonemeAlignment]]]:
         """speak_batch that also says when each phoneme is spoken: per utterance (audio, alignment), the alignment
         holding one entry for bos (`^`), one per kept phoneme character (its id and its trailing pad) and one for eos
         (`$`), contiguous from sample 0 to len(audio).
@@ -606,7 +690,12 @@ class _VitsCommons:
         infer_batch_with_values; it scales samples and moves no boundary.  `pitches` / `tempos`: as for
         infer_batch_with_values; an utterance with a ratio has every boundary scaled by delivered / original length
         (floor(F * len(audio) / T + 0.5) after F of its T frames), accurate to within (rate // 160) / tempo samples of
-        the warped signal because the time stretch takes each frame from within that many samples of the linear map."""
+        the warped signal because the time stretch takes each frame from within that many samples of the linear map.
+
+        pitch_contours[b] (or None): one pitch ratio per character of phoneme_batches[b] (in PITCH_RANGE, or None / NaN
+        / 1.0 for none), applied to that character's id and pad, bos and eos keeping their pitch; see
+        infer_batch_with_values.  An utterance with a contour is aligned from each id's delivered end
+        (sb200_speak_batch_ids_contour), exact rather than scaled: with no tempo a boundary stays where it was."""
         n = len(phoneme_batches)
         _config_array(configs, n)
         _seed_arrays(seeds, n)
@@ -616,7 +705,23 @@ class _VitsCommons:
         warped = [(pit is not None and not np.isnan(pit[b])) or (tem is not None and not np.isnan(tem[b]))
                   for b in range(n)]
         per_char = None if duration_scales is None else _per_utterance(duration_scales, n, "duration scales")
+        char_contours = None if pitch_contours is None else _per_utterance(pitch_contours, n, "pitch contours")
         maps = [self.phonemes_to_input_ids_map(p) for p in phoneme_batches]
+        id_contours = None
+        if char_contours is not None:
+            id_contours = []
+            for b, (ph, (ids, src)) in enumerate(zip(phoneme_batches, maps)):
+                v = char_contours[b]
+                if v is None:
+                    id_contours.append(None)
+                    continue
+                v = list(v) if not isinstance(v, np.ndarray) else v.reshape(-1).tolist()
+                if len(v) != len(ph):
+                    raise OperationError(f"utterance {b}: {len(v)} pitch ratios for {len(ph)} characters")
+                kept = {c: _contour_value(v[c], b, c, "character") for c in sorted(set(src)) if c >= 0}
+                id_contours.append([1.0 if c < 0 else kept[c] for c in src])
+            if _contour_arrays([len(m[0]) for m in maps], id_contours, pit) is None:
+                id_contours = None
         id_scales = None
         if per_char is not None:
             id_scales = []
@@ -637,11 +742,19 @@ class _VitsCommons:
             extra["loudness"] = loudness
         if any(warped):
             extra.update(_prosody_kwargs(pitches, tempos))
-        res = self.infer_batch_with_durations([m[0] for m in maps], configs, id_scales, **extra)
+        if id_contours is None:
+            res = [(a, f, None) for a, f in self.infer_batch_with_durations([m[0] for m in maps], configs, id_scales,
+                                                                            **extra)]
+        else:
+            res = self._speak_ids([m[0] for m in maps], configs, id_scales, None, extra.get("seeds"),
+                                  extra.get("output_rates"), extra.get("loudness"), extra.get("pitches"),
+                                  extra.get("tempos"), id_contours)
         voice_rate = self.audio_output_info().sample_rate if output_rates is not None else None
         ratio = lambda audio: (1, 1) if voice_rate is None else rate_ratio(voice_rate, audio.info.sample_rate)
-        return [(audio, _alignment(ph, src, frames, len(audio), *ratio(audio), warped=w))
-                for ph, (_, src), (audio, frames), w in zip(phoneme_batches, maps, res, warped)]
+        shaped = [id_contours is not None and c is not None and any(not (math.isnan(x) or x == 1.0) for x in c)
+                  for c in (id_contours or [None] * n)]
+        return [(audio, _alignment(ph, src, frames, len(audio), *ratio(audio), warped=w, bounds=bounds if c else None))
+                for ph, (_, src), (audio, frames, bounds), w, c in zip(phoneme_batches, maps, res, warped, shaped)]
 
     def infer_batch_g711(self, batches: Sequence[Sequence[int]], law,
                          configs: Optional[Sequence[PiperSynthesisConfig]] = None, seeds: Optional[Sequence] = None,

@@ -11,6 +11,15 @@ step synthesises the batch and fetches the f32 result to the host.  Six arms:
   (f) host        : arm (a)'s result put through the numpy specification (tests/prosody_reference.py) at pitch 1.25,
                     one thread.
 
+With --contour the arms are pitch contours instead (the host arm is skipped):
+
+  (a) none             : no ratios;
+  (b) pitch            : every utterance at pitch 1.25;
+  (c) contour_uniform  : a contour of 1.25 on every id, which must give arm (b)'s bits (checked once, reported as
+                         "same_bits_as_pitch");
+  (d) contour_question : 1 on the first 75 % of each utterance's ids, then rising in five steps to 1.3;
+  (e) contour_mixed    : per-id ratios drawn from {0.8, 1, 1.25} with a fixed seed.
+
 The arms alternate over --rounds rounds of --steps steps each, so drift in the card's clocks reaches every arm alike.
 Prints the device name and power limit, then one JSON line per arm: wall and device ms per step (medians over rounds,
 and the spread), the device time, algorithmic bytes and operations of the "stretch" and "pitch" regions, and the
@@ -43,6 +52,7 @@ def main():
     ap.add_argument("--utts", type=int, default=32)
     ap.add_argument("--phonemes", type=int, default=256)
     ap.add_argument("--no-host", action="store_true", help="skip the host arm")
+    ap.add_argument("--contour", action="store_true", help="the pitch-contour arms instead")
     args = ap.parse_args()
 
     import torch
@@ -68,7 +78,21 @@ def main():
     arms = {"a_none": {}, "b_pitch_1.25": dict(pitches=[1.25] * n), "c_tempo_1.5": dict(tempos=[1.5] * n),
             "d_pitch_0.8_tempo_2": dict(pitches=[0.8] * n, tempos=[2.0] * n),
             "e_pitch_48k_lufs": dict(pitches=[1.25] * n, output_rates=[48000] * n, loudness=[-16.0] * n)}
-    if not args.no_host:
+    if args.contour:
+        import numpy as np
+
+        def question(k):
+            c = [1.0] * k
+            rise = k - int(0.75 * k)
+            for i in range(int(0.75 * k), k):
+                c[i] = 1.0 + 0.06 * (1 + (i - int(0.75 * k)) * 5 // rise)
+            return c
+        rng = np.random.default_rng(1234)
+        arms = {"a_none": {}, "b_pitch_1.25": dict(pitches=[1.25] * n),
+                "c_contour_uniform_1.25": dict(pitch_contours=[[1.25] * len(b) for b in batches]),
+                "d_contour_question": dict(pitch_contours=[question(len(b)) for b in batches]),
+                "e_contour_mixed": dict(pitch_contours=[list(rng.choice([0.8, 1.0, 1.25], len(b))) for b in batches])}
+    elif not args.no_host:
         arms["f_host_pitch_1.25"] = "host"
 
     def step(arm):
@@ -85,6 +109,15 @@ def main():
         return audio_s, ms, reg, frames
 
     print(json.dumps(device_info()), flush=True)
+    same_bits = None
+    if args.contour:
+        def samples(arm):
+            job = SynthesisJob(model, batches, seeds=seeds, **arm)
+            job.run()
+            out = [a.samples.as_slice().tobytes() for a in job.fetch()]
+            job.close()
+            return out
+        same_bits = samples(arms["b_pitch_1.25"]) == samples(arms["c_contour_uniform_1.25"])
     for arm in arms.values():
         for _ in range(max(args.warmup, 1) if arm != "host" else 1):
             step(arm)
@@ -121,6 +154,8 @@ def main():
                "audio_s_per_s_wall": round(med("audio") / (med("wall") / 1e3), 1)}
         for k, v in r["reg"].items():
             out[k + "_bytes"], out[k + "_ops"] = v["bytes"], v["flops"]
+        if name.startswith("c_contour") and same_bits is not None:
+            out["same_bits_as_pitch"] = same_bits
         if r["frames"] > 1:
             out["longest_utterance_frames"] = r["frames"]
             out["stretch_us_per_frame_step"] = round(med("stretch") * 1e3 / (r["frames"] - 1), 3)
