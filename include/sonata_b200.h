@@ -502,6 +502,37 @@ int32_t sb200_decode_chunks_warped(sb200_voice* v, const sb200_latent* const* zs
                                    const float* gain, sb200_resampler* const* resamplers,
                                    sb200_prosody_stream* const* warps, const int32_t* last, int32_t format, void** outs,
                                    size_t* lens, sb200_error* err);
+/* ---- streams with a pitch contour (see sb200_speak_batch_ids_contour) ----
+ * A prosody stream for latent z's sentence with pitch_per_id[0 .. n_ids) (one ratio per id of z, n_ids its id count;
+ * values as for sb200_speak_batch_ids_contour, NaN or 1: none) and a tempo (NaN or 1: none).  Its plan is fixed at
+ * creation from the latent's frames: n = 256 T_y inputs, id i ending at 256 C_i (C: cumulative frames), pieces, knots
+ * and delivered ends as in sb200_speak_batch_ids_contour.  A bad ratio fails naming the id, a contour and tempo that
+ * together ask for nothing, a wrong n_ids or another voice's latent fail too, all with OPERATION_ERROR before any device
+ * work.  The piece table is uploaded once, into the stream's own allocation.
+ * Contract: join the chunks a contoured stream emits through sb200_decode_chunks_warped; the result is, bit for bit,
+ * sb200_debug_prosody_contour (n, ends = 256 C_i, the ratios and the tempo) of the joined samples appended to it (the
+ * chunks after the post-path, as for a ratio stream), then resampled and converted as without a contour.  The joined
+ * trimmed chunks of a stream cover frames [0, T_y) exactly, so the chunk that ends the stream must bring the total to
+ * n and no chunk may take it past n; otherwise that pass fails with OPERATION_ERROR (internal) before any device work,
+ * and the stream is left as it was.  A contour that merges into one piece
+ * is the ratio stream of that pitch (same chunk counts, same bits).
+ * Emission rule, generalising sb200_decode_chunks_warped's (which it is with one piece): pieces r = 1 .. m with knots
+ * B, S, Q as in sb200_speak_batch_ids_contour, alpha_r = p_r / t, W_r = 16 / min(1, 1 / p_r) and W_max = max_r W_r; C
+ * the inputs consumed.  a_k is step 2's (a_{-1} = -Hs) and frame K's delta is known once
+ * max(a_{K-1} + D + Hs + N, a_K + D + N) <= C.  Stretched samples min(K Hs, floor(sigma(C) + 0.5)) are computed, where
+ * sigma(C) = S_{r-1} + (C - B_{r-1}) * alpha_r in the piece with B_{r-1} <= C < B_r (sigma(n) = S_m).  Output j, at
+ * step 3's pos_j in its piece r(j), is emitted once ceil(pos_j + W_{r(j)}) <= that count, as a prefix (W changes at a
+ * piece's first output).  Between chunks the stream holds the inputs from max(0, min(a_{K-2} + Hs, a_{K-1}) - D) on,
+ * fewer than max(ceil(2 Hs / alpha_min), Hs) + 2 D + N + 4 of them (alpha_min = min_r alpha_r), and the stretched
+ * samples from floor(pos_J - W_max) + 1 on (J: the first output not emitted; a later output in a wider piece reaches
+ * below pos_J - W_{r(J)}), at most 2 ceil(W_max) + 4 <= 68.  The last chunk emits everything up to n2.  Every
+ * expression is evaluated as written, each operation rounded (no fused multiply-add). */
+int32_t sb200_prosody_stream_create_contour(sb200_voice* v, const sb200_latent* z, const float* pitch_per_id,
+                                            size_t n_ids, float tempo, sb200_prosody_stream** out, sb200_error* err);
+/* Each id's delivered end (step 4 of sb200_speak_batch_ids_contour) at the voice's rate, known at creation: the ends
+ * the batch path reports for the same latent.  out[0 .. n_ids); fails with OPERATION_ERROR for a stream made without
+ * a contour or a capacity below the id count. */
+int32_t sb200_prosody_stream_bounds(const sb200_prosody_stream* s, int64_t* out, size_t capacity, sb200_error* err);
 
 /* ---- introspection for tests / bench ---- */
 /* Copy a named intermediate of the LAST run of `job` to host (time-major fp32, valid rows of
@@ -650,6 +681,20 @@ int32_t sb200_debug_prosody_stream_plan(int32_t rate, float pitch, float tempo, 
 int32_t sb200_debug_prosody_stream(int32_t device, const float* x, const int64_t* chunk_lens, size_t n_chunks,
                                    int32_t rate, float pitch, float tempo, float* y, size_t cap, int64_t* lens,
                                    int32_t* offsets, size_t offsets_cap, sb200_error* err);
+/* Test hook, no device needed: a contoured prosody stream (see sb200_prosody_stream_create_contour) over n inputs at
+ * `rate` whose id i ends at ends[i], fed chunk_lens[0 .. n_chunks), the last one ending it.  counts[5 k .. 5 k + 5)
+ * receives chunk k's outputs emitted, then the frames known, the stretched samples computed and the inputs and
+ * stretched samples held after it.  Returns 0, or 19 for bad ratios or ends, a neutral contour and tempo, a bad rate,
+ * a negative length or chunks that do not add up to n. */
+int32_t sb200_debug_prosody_contour_stream_plan(int32_t rate, int64_t n, const int64_t* ends, const float* ratios,
+                                                size_t n_ids, float tempo, const int64_t* chunk_lens, size_t n_chunks,
+                                                int64_t* counts);
+/* sb200_debug_prosody_stream for a fresh contoured stream over x[0 .. sum chunk_lens), n = sum chunk_lens, with those
+ * ends, ratios and tempo. */
+int32_t sb200_debug_prosody_contour_stream(int32_t device, const float* x, const int64_t* chunk_lens, size_t n_chunks,
+                                           int32_t rate, const int64_t* ends, const float* ratios, size_t n_ids,
+                                           float tempo, float* y, size_t cap, int64_t* lens, int32_t* offsets,
+                                           size_t offsets_cap, sb200_error* err);
 /* Test hook: G.711 (law as for sb200_job_fetch_g711) of x[0 .. n) into out[0 .. n).  device -1 runs the host copy of
  * the encoders (no device needed); otherwise the encoders run on that device over the buffer. */
 int32_t sb200_debug_g711(int32_t device, int32_t law, const int16_t* x, size_t n, uint8_t* out, sb200_error* err);

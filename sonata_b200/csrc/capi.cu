@@ -696,6 +696,39 @@ int32_t sb200_prosody_stream_create(sb200_voice* v, float pitch, float tempo, sb
         *out = new sb200_prosody_stream{create_prosody_stream(w, w->device, w->sample_rate, pitch, tempo), v->v};
     });
 }
+int32_t sb200_prosody_stream_create_contour(sb200_voice* v, const sb200_latent* z, const float* pitch_per_id,
+                                            size_t n_ids, float tempo, sb200_prosody_stream** out, sb200_error* err) {
+    return guarded(err, [&] {
+        if (!v || !z || !out || (n_ids > 0 && !pitch_per_id)) throw Error(19, "null argument");
+        Voice* w = v->v.get();
+        if (w->device < 0 || !w->emb)
+            throw Error(19, "Failed to run model inference. Error: voice was loaded config-only (device -1); libsonata_b200 has no CPU path");
+        if (z->l->v != w) throw Error(19, "the latent was not encoded by this voice");
+        const std::vector<int>& f = z->l->id_frames;
+        if (n_ids != f.size())
+            throw Error(19, "pitch contour: " + std::to_string(n_ids) + " ratios for a latent of " +
+                                std::to_string(f.size()) + " ids");
+        // the stream's input: the latent's frames at the hop, each id ending at its cumulative frames
+        const long long hop = w->a.hop();
+        std::vector<long long> ends(n_ids);
+        long long c = 0;
+        for (size_t i = 0; i < n_ids; i++) ends[i] = (c += f[i]) * hop;
+        *out = new sb200_prosody_stream{create_prosody_stream_contour(w, w->device, w->sample_rate, z->l->frames * hop,
+                                                                      ends.data(), pitch_per_id, n_ids, tempo),
+                                        v->v};
+    });
+}
+int32_t sb200_prosody_stream_bounds(const sb200_prosody_stream* s, int64_t* out, size_t capacity, sb200_error* err) {
+    return guarded(err, [&] {
+        if (!s) throw Error(19, "null argument");
+        const std::vector<long long>& b = s->p->bounds;
+        if (s->p->n_total < 0) throw Error(19, "prosody stream bounds: the stream was made without a pitch contour");
+        if (capacity < b.size() || (!out && !b.empty()))
+            throw Error(19, "prosody stream bounds: room for " + std::to_string(capacity) + " of " +
+                                std::to_string(b.size()) + " ids");
+        std::copy(b.begin(), b.end(), out);
+    });
+}
 void sb200_prosody_stream_free(sb200_prosody_stream* s) { delete s; }
 int32_t sb200_prosody_stream_profile(const sb200_prosody_stream* s, float* stretch_ms, float* pitch_ms) {
     if (!s) return 19;
@@ -1204,6 +1237,98 @@ int32_t sb200_debug_prosody_stream_plan(int32_t rate, float pitch, float tempo, 
     }
 }
 
+int32_t sb200_debug_prosody_contour_stream_plan(int32_t rate, int64_t n, const int64_t* ends, const float* ratios,
+                                                size_t n_ids, float tempo, const int64_t* chunk_lens, size_t n_chunks,
+                                                int64_t* counts) {
+    try {
+        if ((n_chunks > 0 && (!chunk_lens || !counts)) || (n_ids > 0 && (!ends || !ratios))) return 19;
+        ProsodyStream ps;
+        prosody_stream_init_contour(ps, rate, n, reinterpret_cast<const long long*>(ends), ratios, n_ids, tempo);
+        const std::vector<long long> c =
+            prosody_stream_counts(ps, reinterpret_cast<const long long*>(chunk_lens), n_chunks);
+        std::copy(c.begin(), c.end(), counts);
+        return 0;
+    } catch (const Error& e) {
+        return e.code;
+    }
+}
+
+namespace {
+// Pushes x through the fresh stream ps chunk by chunk as one-segment passes: `whole` is the whole signal's shape and
+// `counts` what prosody_stream_counts gives for the same stream and chunks, checked against the destinations before
+// any device work.
+void debug_push_stream(ProsodyStream& ps, const ProsodyShape& whole, const std::vector<long long>& counts,
+                       const float* x, const int64_t* chunk_lens, size_t n_chunks, float* y, size_t cap, int64_t* lens,
+                       int32_t* offsets, size_t offsets_cap) {
+    long long total = 0, out_total = 0;
+    for (size_t k = 0; k < n_chunks; k++) { total += chunk_lens[k]; out_total += counts[5 * k]; }
+    if ((size_t)out_total > cap) throw Error(19, "debug prosody stream: the destination is too small for the result");
+    if (offsets && ps.sh.stretch && (size_t)whole.F > offsets_cap)
+        throw Error(19, "debug prosody stream: the offsets destination is too small");
+    // buffers for the largest pass: windows of at most the history plus the whole input, every frame and output
+    DeviceBuffers d;
+    const float* dx = d.upload(x, (size_t)total, (size_t)total + 4);
+    const PcmPost post;
+    const PcmPost* dpost = d.upload(&post, 1, 1);
+    FrameSeg* dfs = d.alloc<FrameSeg>(1);
+    ProsodySeg* dg = d.alloc<ProsodySeg>(1);
+    ProsodyCarry* dc = d.alloc<ProsodyCarry>(1);
+    float* win = d.alloc<float>((size_t)ps.cap_in + (size_t)total + 4);
+    float* ds = d.alloc<float>((size_t)ps.cap_s + (size_t)whole.n1 + 4);
+    int* doff = d.alloc<int>((size_t)whole.F + 4);
+    long long* dap = ps.pieces.empty() ? nullptr : d.alloc<long long>((size_t)whole.F + 4);
+    float* dy = d.alloc<float>((size_t)whole.n2 + 4);
+    long long in_at = 0, out_at = 0;
+    for (size_t k = 0; k < n_chunks; k++) {
+        const bool last = k + 1 == n_chunks;
+        const ProsodyStep t = prosody_stream_step(ps, chunk_lens[k], last);
+        ProsodyPlan p;
+        p.add_stream(ps, t);
+        const ProsodyCarry c = prosody_carry(ps, t, 0);
+        // the chunk as one segment of single samples at in_at
+        const FrameSeg fs{0, (int)chunk_lens[k], 0, 0, in_at};
+        SB_CUDA(cudaMemcpy(dfs, &fs, sizeof(fs), cudaMemcpyHostToDevice));
+        SB_CUDA(cudaMemcpy(dg, &p.segs[0], sizeof(ProsodySeg), cudaMemcpyHostToDevice));
+        SB_CUDA(cudaMemcpy(dc, &c, sizeof(c), cudaMemcpyHostToDevice));
+        launch_prosody_stream_stretch(p, dg, dc, dx, dfs, dpost, 1, win, ds, doff, dy, 0, dap);
+        if (p.max_pitch) launch_prosody_pitch(win, ds, dg, 1, p.max_pitch, dy, 0);
+        SB_CUDA(cudaDeviceSynchronize());
+        SB_CUDA(cudaMemcpy(y + out_at, dy, (size_t)p.y_total * 4, cudaMemcpyDeviceToHost));
+        if (offsets && t.k1 > t.k0)
+            SB_CUDA(cudaMemcpy(offsets + t.k0, doff + 2, (size_t)(t.k1 - t.k0) * 4, cudaMemcpyDeviceToHost));
+        lens[k] = p.y_total;
+        out_at += p.y_total; in_at += chunk_lens[k];
+        prosody_stream_advance(ps, t, last);
+    }
+}
+}  // namespace
+
+int32_t sb200_debug_prosody_contour_stream(int32_t device, const float* x, const int64_t* chunk_lens, size_t n_chunks,
+                                           int32_t rate, const int64_t* ends, const float* ratios, size_t n_ids,
+                                           float tempo, float* y, size_t cap, int64_t* lens, int32_t* offsets,
+                                           size_t offsets_cap, sb200_error* err) {
+    return guarded(err, [&] {
+        if (!x || !chunk_lens || !y || !lens || n_chunks == 0 || !ends || !ratios || n_ids == 0)
+            throw Error(19, "debug prosody contour stream: bad arguments");
+        long long total = 0;
+        for (size_t k = 0; k < n_chunks; k++) {
+            if (chunk_lens[k] < 0) throw Error(19, "debug prosody contour stream: negative chunk length");
+            total += chunk_lens[k];
+        }
+        const long long* e = reinterpret_cast<const long long*>(ends);
+        ProsodyStream host;
+        prosody_stream_init_contour(host, rate, total, e, ratios, n_ids, tempo);
+        const std::vector<long long> counts =
+            prosody_stream_counts(host, reinterpret_cast<const long long*>(chunk_lens), n_chunks);
+        std::vector<ContourPiece> pc;
+        const ProsodyShape whole = prosody_contour_plan(rate, total, e, ratios, n_ids, NAN, tempo, pc, nullptr);
+        SB_CUDA(cudaSetDevice(device));
+        std::unique_ptr<ProsodyStream> ps(create_prosody_stream_contour(nullptr, device, rate, total, e, ratios, n_ids,
+                                                                        tempo));
+        debug_push_stream(*ps, whole, counts, x, chunk_lens, n_chunks, y, cap, lens, offsets, offsets_cap);
+    });
+}
+
 int32_t sb200_debug_prosody_stream(int32_t device, const float* x, const int64_t* chunk_lens, size_t n_chunks,
                                    int32_t rate, float pitch, float tempo, float* y, size_t cap, int64_t* lens,
                                    int32_t* offsets, size_t offsets_cap, sb200_error* err) {
@@ -1214,51 +1339,14 @@ int32_t sb200_debug_prosody_stream(int32_t device, const float* x, const int64_t
             if (chunk_lens[k] < 0) throw Error(19, "debug prosody stream: negative chunk length");
             total += chunk_lens[k];
         }
-        const std::vector<long long> e =
-            prosody_stream_plan(rate, pitch, tempo, reinterpret_cast<const long long*>(chunk_lens), n_chunks);
-        long long out_total = 0;
-        for (long long m : e) out_total += m;
-        if ((size_t)out_total > cap) throw Error(19, "debug prosody stream: the destination is too small for the result");
+        ProsodyStream host;
+        prosody_stream_init(host, rate, pitch, tempo);
+        const std::vector<long long> counts =
+            prosody_stream_counts(host, reinterpret_cast<const long long*>(chunk_lens), n_chunks);
+        const ProsodyShape whole = prosody_shape(rate, total, pitch, tempo);
         SB_CUDA(cudaSetDevice(device));
         std::unique_ptr<ProsodyStream> ps(create_prosody_stream(nullptr, device, rate, pitch, tempo));
-        if (offsets && ps->sh.stretch &&
-            (size_t)prosody_shape(rate, total, pitch, tempo).F > offsets_cap)
-            throw Error(19, "debug prosody stream: the offsets destination is too small");
-        // buffers for the largest pass: windows of at most the history plus the whole input, every frame and output
-        const ProsodyShape whole = prosody_shape(rate, total, pitch, tempo);
-        DeviceBuffers d;
-        const float* dx = d.upload(x, (size_t)total, (size_t)total + 4);
-        const PcmPost post;
-        const PcmPost* dpost = d.upload(&post, 1, 1);
-        FrameSeg* dfs = d.alloc<FrameSeg>(1);
-        ProsodySeg* dg = d.alloc<ProsodySeg>(1);
-        ProsodyCarry* dc = d.alloc<ProsodyCarry>(1);
-        float* win = d.alloc<float>((size_t)ps->cap_in + (size_t)total + 4);
-        float* ds = d.alloc<float>((size_t)ps->cap_s + (size_t)whole.n1 + 4);
-        int* doff = d.alloc<int>((size_t)whole.F + 4);
-        float* dy = d.alloc<float>((size_t)out_total + 4);
-        long long in_at = 0, out_at = 0;
-        for (size_t k = 0; k < n_chunks; k++) {
-            const bool last = k + 1 == n_chunks;
-            const ProsodyStep t = prosody_stream_step(*ps, chunk_lens[k], last);
-            ProsodyPlan p;
-            p.add_stream(*ps, t);
-            const ProsodyCarry c = prosody_carry(*ps, t, 0);
-            // the chunk as one segment of single samples at in_at
-            const FrameSeg fs{0, (int)chunk_lens[k], 0, 0, in_at};
-            SB_CUDA(cudaMemcpy(dfs, &fs, sizeof(fs), cudaMemcpyHostToDevice));
-            SB_CUDA(cudaMemcpy(dg, &p.segs[0], sizeof(ProsodySeg), cudaMemcpyHostToDevice));
-            SB_CUDA(cudaMemcpy(dc, &c, sizeof(c), cudaMemcpyHostToDevice));
-            launch_prosody_stream_stretch(p, dg, dc, dx, dfs, dpost, 1, win, ds, doff, dy, 0);
-            if (p.max_pitch) launch_prosody_pitch(win, ds, dg, 1, p.max_pitch, dy, 0);
-            SB_CUDA(cudaDeviceSynchronize());
-            SB_CUDA(cudaMemcpy(y + out_at, dy, (size_t)p.y_total * 4, cudaMemcpyDeviceToHost));
-            if (offsets && t.k1 > t.k0)
-                SB_CUDA(cudaMemcpy(offsets + t.k0, doff + 2, (size_t)(t.k1 - t.k0) * 4, cudaMemcpyDeviceToHost));
-            lens[k] = p.y_total;
-            out_at += p.y_total; in_at += chunk_lens[k];
-            prosody_stream_advance(*ps, t, last);
-        }
+        debug_push_stream(*ps, whole, counts, x, chunk_lens, n_chunks, y, cap, lens, offsets, offsets_cap);
     });
 }
 

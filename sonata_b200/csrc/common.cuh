@@ -287,8 +287,10 @@ void launch_loudness(float* wav, const LoudSeg* segs, int nseg, double* scratch,
 // and outputs [j0, j1), written from y[y_off] (the stretched samples too when there is no pitch stage, j0 = m0).  A
 // whole utterance is x0 = s0 = d0 = m0 = j0 = k0 = 0, k1 = F, m1 = n1, j1 = n2; a stream's chunk pass is a later window
 // of its stream (ProsodyStream), the frames before k0 known from earlier passes and staged at offsets[d_off].
-// A whole utterance with a pitch contour of two or more pieces (c_n > 0) runs both stages with the piece table
-// pieces[c_off, c_off + c_n] (ContourPiece) instead of alpha and p; c_n = 0 is the single-ratio path.
+// A signal with a pitch contour of two or more pieces (c_n > 0) runs both stages with the piece table
+// pieces[c_off, c_off + c_n] (ContourPiece) instead of alpha and p; c_n = 0 is the single-ratio path.  A stream's
+// window points `cp` at its stream's resident table instead (c_off 0); a whole utterance's cp is null.
+struct ContourPiece;
 struct ProsodySeg {
     long long in_off, n, s_off, n1, y_off, n2, d_off;
     int F, Hs, D, stretch, pitch;
@@ -296,11 +298,29 @@ struct ProsodySeg {
     long long x0, s0, m0, m1, j0, j1;
     int k0, k1, d0;
     int c_off, c_n;
+    const ContourPiece* cp;
 };
 // Piece r of a pitch contour (include/sonata_b200.h, sb200_speak_batch_ids_contour): input samples from B, stretched
 // samples from S, outputs from Q, stretch factor alpha = p / tempo and pitch ratio p.  A segment's table holds its c_n
 // pieces and then a sentinel whose B is n and whose S and Q are +inf, so piece r ends where piece r + 1 starts.
 struct ContourPiece { long long B; double S, Q, alpha, p; };
+// The piece of frame k (the last of pc[0, c_n) with S <= k Hs) and its analysis position
+// a_k = floor(B + (k Hs - S) / alpha + 0.5), every operation rounded as the host plan rounds it.
+__host__ __device__ inline int contour_frame_piece(const ContourPiece* pc, int c_n, double kh) {
+    int r = 0;
+    for (int top = c_n - 1; r < top;) {
+        const int mid = (r + top + 1) / 2;
+        if (pc[mid].S <= kh) r = mid; else top = mid - 1;
+    }
+    return r;
+}
+__host__ __device__ inline long long contour_analysis(const ContourPiece& q, double kh) {
+#ifdef __CUDA_ARCH__
+    return (long long)floor(__dadd_rn(__dadd_rn((double)q.B, __ddiv_rn(__dsub_rn(kh, q.S), q.alpha)), 0.5));
+#else
+    return (long long)floor((double)q.B + (kh - q.S) / q.alpha + 0.5);
+#endif
+}
 // What a stream's chunk pass stages before the prosody launches and carries after them (prosody.cu): the chunk's
 // samples after the post-path (fsegs / posts entry `chunk`) follow h_in history inputs in the segment's input window,
 // h_s stretched samples of history start its stretched window and the deltas of frames d0, d0 + 1 start its offsets.
@@ -324,12 +344,14 @@ constexpr int PP_SPAN = 640;      // shared-memory floats of their input span: 2
 static_assert((PP_OUTS - 1) * 2 + 2 * 32 + 1 <= PP_SPAN, "the pitch resampler's staging is too small for p = 2");
 // The offset chain (blockIdx.x = segment, one persistent block each; smem_ints: the largest 4 Hs + 2 D of the segments),
 // the overlap-add or copy (max_out: the most samples any segment writes) and the pitch resampler, one launch each.
-// Segments with a contour read their piece tables from `pieces`; the offset chain writes their analysis positions to
-// apos[d_off + k] and the overlap-add reads them there (both null when no segment has a contour).
+// Segments with a contour read their piece tables from `pieces` (or their cp); the offset chain writes the analysis
+// positions of a window's frames to apos[d_off + k - d0], laid out like the offsets, and the overlap-add reads them
+// there, recomputing the positions of frames before k0 from the pieces (both null when no segment has a contour).
 void launch_prosody_offsets(const float* wav, const ProsodySeg* segs, int nseg, int smem_ints, int* offsets,
                             cudaStream_t st, const ContourPiece* pieces = nullptr, long long* apos = nullptr);
 void launch_prosody_ola(const float* wav, const ProsodySeg* segs, int nseg, long long max_out, const int* offsets,
-                        float* s, float* y, cudaStream_t st, const long long* apos = nullptr);
+                        float* s, float* y, cudaStream_t st, const long long* apos = nullptr,
+                        const ContourPiece* pieces = nullptr);
 void launch_prosody_pitch(const float* wav, const float* s, const ProsodySeg* segs, int nseg, long long max_out, float* y,
                           cudaStream_t st, const ContourPiece* pieces = nullptr);
 // A stream pass's staging (before the launches above; chunks read from src through fsegs / posts, max_in: the longest

@@ -539,10 +539,8 @@ struct ProsodyBufs {
         y = nullptr;
         if (n == 0) return;
         segs.carve(dev, pin, n);
-        if (!p.pieces.empty()) {
-            pieces.carve(dev, pin, p.pieces.size());
-            apos = dev.get<long long>((size_t)p.d_total);
-        }
+        if (!p.pieces.empty()) pieces.carve(dev, pin, p.pieces.size());     // a stream's table is its own
+        if (p.contour) apos = dev.get<long long>((size_t)p.d_total);
         if (p.in_total) {
             carry.carve(dev, pin, n);
             x = dev.get<float>((size_t)p.in_total + 4);
@@ -1507,7 +1505,7 @@ void decode_chunks(Voice* v, const ChunkPass& p, ChunkResult& out) {
         b.pr.carry.upload(st);
         R.begin("stretch");
         launch_prosody_stream_stretch(pp, b.pr.segs.d, b.pr.carry.d, b.wav, b.y.fsegs.d, b.post.d, hop, b.pr.x, b.pr.s,
-                                      b.pr.offsets, py, st);
+                                      b.pr.offsets, py, st, b.pr.apos);
         R.count(pp.stretch_flops, pp.stretch_bytes, 2 + (pp.smem_ints ? 1 : 0) + (pp.max_ola ? 1 : 0));
         R.end();
         if (pp.max_pitch) {

@@ -155,6 +155,7 @@ struct ProsodyPlan {
     long long s_total = 0, y_total = 0, d_total = 0, max_ola = 0, max_pitch = 0, steps = 0;
     long long in_total = 0, max_in = 0, max_keep = 0;     // streams: the input windows, the staging and carry sizes
     int smem_ints = 0;
+    bool contour = false;                                  // some segment has a contour: a d_total table of positions
     double stretch_flops = 0, stretch_bytes = 0, pitch_flops = 0, pitch_bytes = 0;
     // Appends the segment wav[in_off, in_off + n) with shape `sh` and, when it has one, its contour's piece table.
     void add(const ProsodyShape& sh, long long in_off, long long n, const std::vector<ContourPiece>* contour = nullptr);
@@ -165,14 +166,22 @@ struct ProsodyPlan {
 // One stream's pitch and tempo state (prosody.cu): the shape of its ratios, its counts (inputs consumed, frames whose
 // delta is known, stretched samples computed, outputs emitted, and the history held of the inputs and the stretched
 // signal) and, on the device, two sets of buffers read and written alternately: the input tail (at most cap_in), the
-// stretched tail (at most cap_s, with both stages) and the deltas of the last two known frames.
+// stretched tail (at most cap_s, with both stages) and the deltas of the last two known frames.  A stream with a pitch
+// contour knows its whole input length n_total and its plan (prosody_contour_plan) at creation: its piece table, when
+// the contour makes two or more pieces, is resident on the device after the buffers (pieces_d); one piece is planned
+// as the ratio stream it equals.
 struct ProsodyCounts { long long consumed = 0, frames = 0, stretched = 0, emitted = 0; int h_in = 0, h_s = 0; };
 struct ProsodyStream {
     Voice* v = nullptr;
     int device = 0, rate = 0;
     float pitch = 1.f, tempo = 1.f;
-    ProsodyShape sh{};                    // Hs, N, D, alpha, p and the stages (lengths unused)
+    ProsodyShape sh{};                    // Hs, N, D, alpha, p and the stages (lengths unused; a contour's: its plan's)
     int cap_in = 0, cap_s = 0;
+    long long n_total = -1;               // a contour stream's input length (-1: a ratio stream)
+    std::vector<ContourPiece> pieces;     // its piece table and sentinel (empty: one piece, or a ratio stream)
+    std::vector<long long> bounds;        // its ids' delivered ends (empty: a ratio stream)
+    double w_max = 0;                     // the widest pitch kernel radius of its pieces
+    const ContourPiece* pieces_d = nullptr;
     void* mem = nullptr;
     float* in_hist[2] = {nullptr, nullptr}; float* s_hist[2] = {nullptr, nullptr}; int* d_hist[2] = {nullptr, nullptr};
     int cur = 0;
@@ -192,6 +201,13 @@ struct ProsodyStep {
 // Checks the ratios (one must ask for something) and sizes the history; no device memory.
 void prosody_stream_init(ProsodyStream& ps, int rate, float pitch, float tempo);
 ProsodyStream* create_prosody_stream(Voice* v, int device, int rate, float pitch, float tempo);
+// The same for a pitch contour of n_ids ids over n inputs (ends, ratios: as for prosody_contour_plan) and a tempo:
+// checks them as check_pitch_contour and check_prosody do (a contour and tempo that ask for nothing are refused), plans
+// the pieces and the bounds, and sizes the history by the smallest stretch factor and the widest pitch kernel.
+void prosody_stream_init_contour(ProsodyStream& ps, int rate, long long n, const long long* ends, const float* ratios,
+                                 size_t n_ids, float tempo);
+ProsodyStream* create_prosody_stream_contour(Voice* v, int device, int rate, long long n, const long long* ends,
+                                             const float* ratios, size_t n_ids, float tempo);
 // The emission rule (include/sonata_b200.h, sb200_decode_chunks_warped).  Throws OPERATION_ERROR only on an internal
 // inconsistency.
 ProsodyStep prosody_stream_step(const ProsodyStream& ps, long long n_in, bool last);
@@ -201,11 +217,14 @@ ProsodyCarry prosody_carry(const ProsodyStream& ps, const ProsodyStep& t, int ch
 // pitch stage is launch_prosody_pitch over the same tables.
 void launch_prosody_stream_stretch(const ProsodyPlan& p, const ProsodySeg* segs, const ProsodyCarry* cs,
                                    const float* src, const FrameSeg* fsegs, const PcmPost* posts, int hop, float* x,
-                                   float* s, int* offsets, float* y, cudaStream_t st);
+                                   float* s, int* offsets, float* y, cudaStream_t st, long long* apos = nullptr);
 // After the pass has synchronised: the counts become t's and the buffers swap.
 void prosody_stream_advance(ProsodyStream& ps, const ProsodyStep& t, bool last);
 // Outputs per chunk of a stream with these ratios whose chunks bring chunk_lens[0 .. n) inputs, the last one ending it.
 std::vector<long long> prosody_stream_plan(int rate, float pitch, float tempo, const long long* chunk_lens, size_t n);
+// The counts after each chunk of stream ps (fresh, no device memory) fed chunk_lens[0 .. n): 5 per chunk (outputs
+// emitted, frames, stretched samples, input and stretched history held).
+std::vector<long long> prosody_stream_counts(ProsodyStream& ps, const long long* chunk_lens, size_t n);
 
 struct Context;   // stream + arenas for one in-flight call
 

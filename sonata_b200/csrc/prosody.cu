@@ -161,17 +161,25 @@ prosody_offsets_kernel(const float* __restrict__ wav, const ProsodySeg* __restri
     const int Hs = g.Hs, N = 2 * Hs, D = g.D, L = 2 * D + 1;
     int* ref = pq;
     int* cand = pq + N;
-    // a contour (whole utterances only): the piece of frame k is carried from frame to frame, and a_k goes to ap[k]
-    const ContourPiece* pc = g.c_n ? pieces + g.c_off : nullptr;
-    long long* ap = g.c_n ? apos + g.d_off : nullptr;
-    int r = 0;
+    // a contour: the piece of the frame before the window is searched, then carried from frame to frame, and a_k goes
+    // to ap[k], laid out like the deltas
+    const ContourPiece* pc = g.c_n ? (g.cp ? g.cp : pieces + g.c_off) : nullptr;
+    long long* ap = g.c_n ? apos + g.d_off - g.d0 : nullptr;
     if (g.k0 == 0 && threadIdx.x == 0) {
         out[0] = 0;
         if (pc) ap[0] = 0;
     }
     // the frame before the first one computed: frame 0 (delta 0, at 0) or the last one an earlier pass computed
     const int k_first = max(g.k0, 1);
-    long long a_prev = prosody_analysis(Hs, g.alpha, k_first - 1);
+    int r = 0;
+    long long a_prev;
+    if (pc) {
+        const double kh = (double)((long long)(k_first - 1) * Hs);
+        r = contour_frame_piece(pc, g.c_n, kh);
+        a_prev = contour_analysis(pc[r], kh);
+    } else {
+        a_prev = prosody_analysis(Hs, g.alpha, k_first - 1);
+    }
     int d_prev = k_first == 1 ? 0 : out[k_first - 1];
     for (int k = k_first; k < g.k1; k++) {
         long long a;
@@ -179,7 +187,7 @@ prosody_offsets_kernel(const float* __restrict__ wav, const ProsodySeg* __restri
             // a_k = floor(B + (k Hs - S) / alpha + 0.5) in the piece with S <= k Hs, every operation rounded as the host
             const double kh = (double)((long long)k * Hs);
             while (r + 1 < g.c_n && kh >= pc[r + 1].S) r++;
-            a = (long long)floor(__dadd_rn(__dadd_rn((double)pc[r].B, __ddiv_rn(__dsub_rn(kh, pc[r].S), pc[r].alpha)), 0.5));
+            a = contour_analysis(pc[r], kh);
             if (threadIdx.x == 0) ap[k] = a;
         } else {
             a = prosody_analysis(Hs, g.alpha, k);
@@ -220,7 +228,7 @@ __device__ __forceinline__ float pr_window(int i, int N) { return (float)(0.5 - 
 
 __global__ void prosody_ola_kernel(const float* __restrict__ wav, const ProsodySeg* __restrict__ segs,
                                    const int* __restrict__ offsets, float* __restrict__ s, float* __restrict__ y,
-                                   const long long* __restrict__ apos) {
+                                   const long long* __restrict__ apos, const ContourPiece* __restrict__ pieces) {
     pdl_trigger(); pdl_wait();
     const ProsodySeg g = segs[blockIdx.y];
     const float* x = wav + g.in_off;
@@ -235,11 +243,19 @@ __global__ void prosody_ola_kernel(const float* __restrict__ wav, const ProsodyS
     const long long ob = g.pitch ? g.s0 : g.m0;
     const int* dl = offsets + g.d_off - g.d0;
     const int Hs = g.Hs, N = 2 * Hs;
-    const long long* ap = g.c_n ? apos + g.d_off : nullptr;      // a contour's analysis positions, from the offset chain
+    // a contour's analysis positions: the window's frames from the offset chain, an earlier pass's from the pieces
+    const long long* ap = g.c_n ? apos + g.d_off - g.d0 : nullptr;
+    const ContourPiece* pc = g.c_n ? (g.cp ? g.cp : pieces + g.c_off) : nullptr;
+    const auto contour_a = [&](int k) -> long long {
+        if (k < 0) return -(long long)Hs;
+        if (k >= g.k0) return ap[k];
+        const double kh = (double)((long long)k * Hs);
+        return contour_analysis(pc[contour_frame_piece(pc, g.c_n, kh)], kh);
+    };
     for (long long m = g.m0 + i0; m < g.m1; m += step) {
         const int k = (int)(m / Hs), r = (int)(m - (long long)k * Hs);
-        const long long a1 = ap ? ap[k] : prosody_analysis(Hs, g.alpha, k);
-        const long long a0 = ap ? (k > 0 ? ap[k - 1] : -(long long)Hs) : prosody_analysis(Hs, g.alpha, k - 1);
+        const long long a1 = ap ? contour_a(k) : prosody_analysis(Hs, g.alpha, k);
+        const long long a0 = ap ? contour_a(k - 1) : prosody_analysis(Hs, g.alpha, k - 1);
         const long long p1 = a1 + dl[k] + r;
         const long long p0 = a0 + (k > 0 ? dl[k - 1] : 0) + r + Hs;
         const float x1 = p1 >= 0 && p1 < g.n ? x[p1 - g.x0] : 0.f, x0 = p0 >= 0 && p0 < g.n ? x[p0 - g.x0] : 0.f;
@@ -308,7 +324,7 @@ prosody_pitch_kernel(const float* __restrict__ wav, const float* __restrict__ s,
         }
         return;
     }
-    const ContourPiece* pc = pieces + g.c_off;
+    const ContourPiece* pc = g.cp ? g.cp : pieces + g.c_off;
     for (long long a = g.j0 + (long long)blockIdx.x * PP_OUTS; a < g.j1; a += (long long)gridDim.x * PP_OUTS) {
         const long long jb = min(a + (long long)PP_OUTS, g.j1);
         // the piece of the block's first output (the last one with Q <= a), then each output's own
@@ -389,10 +405,10 @@ void launch_prosody_offsets(const float* wav, const ProsodySeg* segs, int nseg, 
 }
 
 void launch_prosody_ola(const float* wav, const ProsodySeg* segs, int nseg, long long max_out, const int* offsets,
-                        float* s, float* y, cudaStream_t st, const long long* apos) {
+                        float* s, float* y, cudaStream_t st, const long long* apos, const ContourPiece* pieces) {
     if (nseg <= 0) return;
     launch_pdl(prosody_ola_kernel, dim3(grid_for(max_out, 1024), nseg), dim3(256), 0, st, wav, segs, offsets, s, y,
-               apos);
+               apos, pieces);
     g_launch_count++;
 }
 
@@ -426,6 +442,7 @@ void ProsodyPlan::add(const ProsodyShape& sh, long long in_off, long long n, con
     if (contour && !contour->empty()) {
         g.c_off = (int)pieces.size(); g.c_n = (int)contour->size() - 1;
         pieces.insert(pieces.end(), contour->begin(), contour->end());
+        this->contour = true;
     }
     g.in_off = in_off; g.n = n; g.n1 = sh.n1; g.n2 = sh.n2;
     g.F = sh.F; g.Hs = sh.Hs; g.D = sh.D; g.stretch = sh.stretch; g.pitch = sh.pitch; g.alpha = sh.alpha; g.p = sh.p;
@@ -473,14 +490,45 @@ void prosody_stream_init(ProsodyStream& ps, int rate, float pitch, float tempo) 
     ps.cap_s = s.stretch ? pitch_tail : 0;
 }
 
-ProsodyStream* create_prosody_stream(Voice* v, int device, int rate, float pitch, float tempo) {
-    std::unique_ptr<ProsodyStream> ps(new ProsodyStream());
-    prosody_stream_init(*ps, rate, pitch, tempo);
+void prosody_stream_init_contour(ProsodyStream& ps, int rate, long long n, const long long* ends, const float* ratios,
+                                 size_t n_ids, float tempo) {
+    const size_t offs[2] = {0, n_ids};
+    check_pitch_contour(ratios, offs, 1, nullptr);
+    check_prosody(nullptr, &tempo, 1);
+    std::vector<ContourPiece> pc;
+    std::vector<long long> bounds(n_ids);
+    const ProsodyShape sh = prosody_contour_plan(rate, n, ends, ratios, n_ids, NAN, tempo, pc, bounds.data());
+    if (!sh.stretch && !sh.pitch)
+        throw Error(19, "a prosody stream's pitch contour and tempo ask for nothing (every ratio NaN or 1, and no tempo)");
+    if (pc.empty()) {
+        // one piece: the ratio stream it equals
+        prosody_stream_init(ps, rate, sh.pitch ? (float)sh.p : NAN, tempo);
+    } else {
+        ps.sh = sh;
+        ps.rate = rate; ps.pitch = NAN; ps.tempo = tempo;
+        double alpha_min = INFINITY;
+        for (size_t r = 0; r + 1 < pc.size(); r++) {
+            alpha_min = std::min(alpha_min, pc[r].alpha);
+            ps.w_max = std::max(ps.w_max, pitch_radius(pc[r].p));
+        }
+        ps.cap_in = (int)std::max<double>(std::ceil(2.0 * sh.Hs / alpha_min), sh.Hs) + 2 * sh.D + sh.N + 4;
+        ps.cap_s = 2 * (int)std::ceil(ps.w_max) + 4;
+        ps.pieces = std::move(pc);
+    }
+    ps.n_total = n;
+    ps.bounds = std::move(bounds);
+}
+
+namespace {
+// The history buffers (two sets of cap_in + cap_s floats and two ints) and, after them, the piece table.
+ProsodyStream* allocate_prosody_stream(std::unique_ptr<ProsodyStream> ps, Voice* v, int device) {
     ps->v = v; ps->device = device;
     SB_CUDA(cudaSetDevice(device));
     const size_t side = (size_t)ps->cap_in + ps->cap_s + 2;      // floats, floats, two ints
+    const size_t table = (2 * side * 4 + 15) / 16 * 16;
+    const size_t bytes = table + ps->pieces.size() * sizeof(ContourPiece);
     void* mem = nullptr;
-    SB_CUDA(cudaMalloc(&mem, 2 * side * 4));
+    SB_CUDA(cudaMalloc(&mem, bytes));
     ps->mem = mem;
     SB_CUDA(cudaMemset(mem, 0, 2 * side * 4));                   // delta_{-2} = delta_{-1} = 0 (unused) before frame 0
     for (int b = 0; b < 2; b++) {
@@ -488,7 +536,26 @@ ProsodyStream* create_prosody_stream(Voice* v, int device, int rate, float pitch
         ps->in_hist[b] = base; ps->s_hist[b] = base + ps->cap_in;
         ps->d_hist[b] = reinterpret_cast<int*>(base + ps->cap_in + ps->cap_s);
     }
+    if (!ps->pieces.empty()) {
+        ContourPiece* d = reinterpret_cast<ContourPiece*>(static_cast<char*>(mem) + table);
+        SB_CUDA(cudaMemcpy(d, ps->pieces.data(), ps->pieces.size() * sizeof(ContourPiece), cudaMemcpyHostToDevice));
+        ps->pieces_d = d;
+    }
     return ps.release();
+}
+}  // namespace
+
+ProsodyStream* create_prosody_stream(Voice* v, int device, int rate, float pitch, float tempo) {
+    std::unique_ptr<ProsodyStream> ps(new ProsodyStream());
+    prosody_stream_init(*ps, rate, pitch, tempo);
+    return allocate_prosody_stream(std::move(ps), v, device);
+}
+
+ProsodyStream* create_prosody_stream_contour(Voice* v, int device, int rate, long long n, const long long* ends,
+                                             const float* ratios, size_t n_ids, float tempo) {
+    std::unique_ptr<ProsodyStream> ps(new ProsodyStream());
+    prosody_stream_init_contour(*ps, rate, n, ends, ratios, n_ids, tempo);
+    return allocate_prosody_stream(std::move(ps), v, device);
 }
 
 ProsodyStream::~ProsodyStream() {
@@ -505,11 +572,44 @@ ProsodyStep prosody_stream_step(const ProsodyStream& ps, long long n_in, bool la
     t.n_in = n_in;
     t.x0 = c.consumed - c.h_in; t.s0 = c.stretched - c.h_s;
     t.k0 = (int)c.frames; t.m0 = c.stretched; t.j0 = c.emitted;
-    auto a = [&](long long k) { return prosody_analysis(sh.Hs, sh.alpha, k); };
+    // A contour of two or more pieces: a_k, sigma(C) and pos_j are piecewise (include/sonata_b200.h,
+    // sb200_decode_chunks_warped); with one piece each is the single ratio's expression.
+    const std::vector<ContourPiece>& pc = ps.pieces;
+    const int m = pc.empty() ? 0 : (int)pc.size() - 1;
+    auto a = [&](long long k) {
+        if (!m || k < 0) return prosody_analysis(sh.Hs, sh.alpha, k);
+        const double kh = (double)(k * sh.Hs);
+        return contour_analysis(pc[contour_frame_piece(pc.data(), m, kh)], kh);
+    };
+    auto sigma = [&](long long x) {          // the piece with B <= x (the last one for x = n: sigma(n) = S_m)
+        if (!m) return (double)x * sh.alpha;
+        int r = 0;
+        while (r + 1 < m && pc[r + 1].B <= x) r++;
+        return pc[r].S + (double)(x - pc[r].B) * pc[r].alpha;
+    };
+    auto piece_out = [&](long long j) {      // the piece of output j: the last with Q <= j
+        int r = 0;
+        for (int top = m - 1; r < top;) {
+            const int mid = (r + top + 1) / 2;
+            if (pc[mid].Q <= (double)j) r = mid; else top = mid - 1;
+        }
+        return r;
+    };
+    auto pos = [&](long long j, int r) { return m ? pc[r].S + ((double)j - pc[r].Q) * pc[r].p : (double)j * sh.p; };
+    auto radius = [&](int r) { return pitch_radius(m ? pc[r].p : sh.p); };
+    // a contour's plan holds for its n inputs alone: any chunk past them, or a last one short of them, fails before
+    // anything outside the plan goes out
+    if (ps.n_total >= 0 && (C > ps.n_total || (last && C != ps.n_total)))
+        throw Error(19, "internal: a contour prosody stream would " + std::string(last ? "end" : "go on") + " after " +
+                            std::to_string(C) + " inputs, not its " + std::to_string(ps.n_total));
     long long K = c.frames, S, J;
     if (last) {
-        const ProsodyShape e = prosody_shape(ps.rate, C, ps.pitch, ps.tempo);
-        K = e.F; S = e.n1; J = e.n2;
+        if (m) {
+            K = sh.F; S = sh.n1; J = sh.n2;
+        } else {
+            const ProsodyShape e = prosody_shape(ps.rate, C, ps.pitch, ps.tempo);
+            K = e.F; S = e.n1; J = e.n2;
+        }
     } else {
         S = C;
         if (sh.stretch) {
@@ -517,13 +617,17 @@ ProsodyStep prosody_stream_step(const ProsodyStream& ps, long long n_in, bool la
             // continuation point bounded by delta_{k-1} <= D; a stretched sample once it lies below the n1 of any
             // longer input
             while (std::max(a(K - 1) + sh.D + sh.Hs + sh.N, a(K) + sh.D + sh.N) <= C) K++;
-            S = std::min(K * sh.Hs, (long long)std::floor((double)C * sh.alpha + 0.5));
+            S = std::min(K * sh.Hs, (long long)std::floor(sigma(C) + 0.5));
         }
         J = S;
         if (sh.pitch) {
-            const double W = pitch_radius(sh.p);
+            // outputs go out as a prefix: the radius changes at a piece's first output
             J = c.emitted;
-            while ((long long)std::ceil((double)J * sh.p + W) <= S) J++;
+            for (int r = m ? piece_out(J) : 0;; ) {
+                if (m) while (r + 1 < m && (double)J >= pc[r + 1].Q) r++;
+                if ((long long)std::ceil(pos(J, r) + radius(r)) > S) break;
+                J++;
+            }
         }
     }
     if (K < c.frames || S < c.stretched || J < c.emitted || K > INT_MAX)
@@ -534,8 +638,11 @@ ProsodyStep prosody_stream_step(const ProsodyStream& ps, long long n_in, bool la
     // the tails the next pass reads: none after the last chunk
     long long in_from = C, s_from = S;
     if (!last) {
+        // the stretched history reaches the widest kernel below the first output not emitted
         const long long pitch_from =
-            sh.pitch ? std::min(S, std::max(0ll, (long long)std::floor((double)J * sh.p - pitch_radius(sh.p)) + 1)) : S;
+            sh.pitch ? std::min(S, std::max(0ll, (long long)std::floor(pos(J, m ? piece_out(J) : 0) -
+                                                                       (m ? ps.w_max : pitch_radius(sh.p))) + 1))
+                     : S;
         if (sh.stretch) {
             in_from = K == 0 ? 0 : std::max(0ll, std::min(a(K - 2) + sh.Hs, a(K - 1)) - sh.D);
             in_from = std::min(in_from, C);
@@ -556,6 +663,10 @@ void ProsodyPlan::add_stream(const ProsodyStream& ps, const ProsodyStep& t) {
     const ProsodyShape& sh = ps.sh;
     ProsodySeg g{};
     g.Hs = sh.Hs; g.D = sh.D; g.stretch = sh.stretch; g.pitch = sh.pitch; g.alpha = sh.alpha; g.p = sh.p;
+    if (!ps.pieces.empty()) {
+        g.c_n = (int)ps.pieces.size() - 1; g.cp = ps.pieces_d;
+        contour = true;
+    }
     const long long nx = ps.c.h_in + t.n_in;
     g.in_off = in_total; in_total += nx;
     g.x0 = t.x0; g.n = t.next.consumed;
@@ -597,11 +708,11 @@ ProsodyCarry prosody_carry(const ProsodyStream& ps, const ProsodyStep& t, int ch
 
 void launch_prosody_stream_stretch(const ProsodyPlan& p, const ProsodySeg* segs, const ProsodyCarry* cs,
                                    const float* src, const FrameSeg* fsegs, const PcmPost* posts, int hop, float* x,
-                                   float* s, int* offsets, float* y, cudaStream_t st) {
+                                   float* s, int* offsets, float* y, cudaStream_t st, long long* apos) {
     const int n = (int)p.segs.size();
     launch_prosody_stage(src, fsegs, posts, hop, segs, cs, n, p.max_in, x, s, offsets, st);
-    if (p.smem_ints) launch_prosody_offsets(x, segs, n, p.smem_ints, offsets, st);
-    if (p.max_ola) launch_prosody_ola(x, segs, n, p.max_ola, offsets, s, y, st);
+    if (p.smem_ints) launch_prosody_offsets(x, segs, n, p.smem_ints, offsets, st, nullptr, apos);
+    if (p.max_ola) launch_prosody_ola(x, segs, n, p.max_ola, offsets, s, y, st, apos);
     launch_prosody_carry(x, s, offsets, segs, cs, n, p.max_keep, st);
 }
 
@@ -611,16 +722,24 @@ void prosody_stream_advance(ProsodyStream& ps, const ProsodyStep& t, bool last) 
     ps.ended = last;
 }
 
-std::vector<long long> prosody_stream_plan(int rate, float pitch, float tempo, const long long* chunk_lens, size_t n) {
-    ProsodyStream ps;
-    prosody_stream_init(ps, rate, pitch, tempo);
-    std::vector<long long> out(n);
+std::vector<long long> prosody_stream_counts(ProsodyStream& ps, const long long* chunk_lens, size_t n) {
+    std::vector<long long> out(5 * n);
     for (size_t k = 0; k < n; k++) {
         if (chunk_lens[k] < 0) throw Error(19, "chunk " + std::to_string(k) + ": negative length");
         const ProsodyStep t = prosody_stream_step(ps, chunk_lens[k], k + 1 == n);
-        out[k] = t.j1 - t.j0;
+        const long long row[5] = {t.j1 - t.j0, t.next.frames, t.next.stretched, t.next.h_in, t.next.h_s};
+        std::copy(row, row + 5, out.begin() + 5 * k);
         prosody_stream_advance(ps, t, k + 1 == n);
     }
+    return out;
+}
+
+std::vector<long long> prosody_stream_plan(int rate, float pitch, float tempo, const long long* chunk_lens, size_t n) {
+    ProsodyStream ps;
+    prosody_stream_init(ps, rate, pitch, tempo);
+    const std::vector<long long> c = prosody_stream_counts(ps, chunk_lens, n);
+    std::vector<long long> out(n);
+    for (size_t k = 0; k < n; k++) out[k] = c[5 * k];
     return out;
 }
 

@@ -207,24 +207,30 @@ def _prosody_arrays(pitches, tempos, n: int):
     return _ratio_array(pitches, n, "pitch", *PITCH_RANGE), _ratio_array(tempos, n, "tempo", *TEMPO_RANGE)
 
 
-def _contour_value(x, b: int, i: int, unit: str = "id") -> float:
+def _who(b) -> str:
+    """What an error names: utterance b of a batch, or a label such as "stream 3" given instead of the index."""
+    return b if isinstance(b, str) else f"utterance {b}"
+
+
+def _contour_value(x, b, i: int, unit: str = "id") -> float:
     if x is None:
         return math.nan
     if isinstance(x, bool) or not isinstance(x, numbers.Real):
-        raise OperationError(f"utterance {b}, {unit} {i}: pitch ratio {x!r} is not a number")
+        raise OperationError(f"{_who(b)}, {unit} {i}: pitch ratio {x!r} is not a number")
     x = float(x)
     if not (math.isnan(x) or x == 1.0 or (math.isfinite(x) and PITCH_RANGE[0] <= x <= PITCH_RANGE[1])):
-        raise OperationError(f"utterance {b}, {unit} {i}: pitch ratio {x} is not a finite value in "
+        raise OperationError(f"{_who(b)}, {unit} {i}: pitch ratio {x} is not a finite value in "
                              f"[{PITCH_RANGE[0]}, {PITCH_RANGE[1]}] (NaN or 1: none)")
     return x
 
 
-def _contour_arrays(lens: Sequence[int], pitch_contours=None, pitches=None):
+def _contour_arrays(lens: Sequence[int], pitch_contours=None, pitches=None, who: Optional[Sequence[str]] = None):
     """The packed C image of per-id pitch ratios (f32, NaN for none), checked as the library checks them, or None when
     not given or when no utterance has a contour.  pitch_contours[b] holds one ratio per id of utterance b (in
     PITCH_RANGE, or None / NaN / 1.0 for none), or is None.  An utterance with a contour may not also have a pitch ratio
     in `pitches` (the C image of _prosody_arrays, or None).  Numeric arrays are checked in one vectorised pass; anything
-    else element by element, which also names the first bad element."""
+    else element by element, which also names the first bad element.  `who`: what the errors name instead of
+    "utterance b" (one label per entry), for callers that are not batches."""
     if pitch_contours is None:
         return None
     n = len(lens)
@@ -232,22 +238,34 @@ def _contour_arrays(lens: Sequence[int], pitch_contours=None, pitches=None):
     pos = 0
     for b, v in enumerate(_per_utterance(pitch_contours, n, "pitch contours")):
         if v is not None:
+            label = b if who is None else who[b]
             a = _numeric(v, "fiu")
             if a is None:
                 v = list(v)
-                a = np.array([_contour_value(x, b, i) for i, x in enumerate(v)] if len(v) == lens[b] else v)
+                a = np.array([_contour_value(x, label, i) for i, x in enumerate(v)] if len(v) == lens[b] else v)
             if a.size != lens[b]:
-                raise OperationError(f"utterance {b}: {a.size} pitch ratios for {lens[b]} ids")
+                raise OperationError(f"{_who(label)}: {a.size} pitch ratios for {lens[b]} ids")
             f = a.astype(np.float32)
             asked = ~np.isnan(f) & (f != 1)
             bad = np.nonzero(asked & ~(np.isfinite(f) & (f >= PITCH_RANGE[0]) & (f <= PITCH_RANGE[1])))[0]
             if bad.size:
-                _contour_value(float(f[bad[0]]), b, int(bad[0]))
+                _contour_value(float(f[bad[0]]), label, int(bad[0]))
             if asked.any() and pitches is not None and not np.isnan(pitches[b]):
-                raise OperationError(f"utterance {b}: a pitch contour and a pitch ratio together (give one or the other)")
+                raise OperationError(f"{_who(label)}: a pitch contour and a pitch ratio together (give one or the other)")
             out[pos:pos + lens[b]] = f
         pos += lens[b]
     return None if (np.isnan(out) | (out == 1)).all() else out
+
+
+def _char_values_to_ids(v, phonemes: str, src: Sequence[int], b, what: str, check) -> list:
+    """Per-character values v (one per character of `phonemes`) as per-id values: each id takes its source character's
+    value, checked by check(x, b, character, "character"); bos, eos and pads of no character take 1.0.  Characters the
+    voice drops have no id and their values are ignored.  b: the utterance's index, or a label naming the stream."""
+    v = list(v) if not isinstance(v, np.ndarray) else v.reshape(-1).tolist()
+    if len(v) != len(phonemes):
+        raise OperationError(f"{_who(b)}: {len(v)} {what} for {len(phonemes)} characters")
+    kept = {c: check(v[c], b, c, "character") for c in sorted(set(src)) if c >= 0}
+    return [1.0 if c < 0 else kept[c] for c in src]
 
 
 def _prosody_kwargs(pitches, tempos) -> dict:
@@ -264,6 +282,13 @@ def refuse_prosody(pitch, tempo, where: str) -> None:
         raise OperationError(f"{where} cannot shift pitch or tempo: the time stretch walks a whole sentence frame by "
                              "frame, and this mode hands out a sentence's first chunk before its last one is decoded "
                              "(use the lazy, parallel or file modes, speak_batch or a SynthesisJob)")
+
+
+def refuse_contour(pitch_contour, where: str) -> None:
+    """OperationError when `where`, a mode without this library's streaming voices, is asked for a pitch contour."""
+    if pitch_contour is not None:
+        raise OperationError(f"{where} cannot apply a pitch contour: only this library's streaming voices carry a "
+                             "contour from chunk to chunk (use speak_batch_with_alignment or a SynthesisJob)")
 
 
 def _encoding_list(law, n: int) -> list:
@@ -712,14 +737,8 @@ class _VitsCommons:
             id_contours = []
             for b, (ph, (ids, src)) in enumerate(zip(phoneme_batches, maps)):
                 v = char_contours[b]
-                if v is None:
-                    id_contours.append(None)
-                    continue
-                v = list(v) if not isinstance(v, np.ndarray) else v.reshape(-1).tolist()
-                if len(v) != len(ph):
-                    raise OperationError(f"utterance {b}: {len(v)} pitch ratios for {len(ph)} characters")
-                kept = {c: _contour_value(v[c], b, c, "character") for c in sorted(set(src)) if c >= 0}
-                id_contours.append([1.0 if c < 0 else kept[c] for c in src])
+                id_contours.append(None if v is None else
+                                   _char_values_to_ids(v, ph, src, b, "pitch ratios", _contour_value))
             if _contour_arrays([len(m[0]) for m in maps], id_contours, pit) is None:
                 id_contours = None
         id_scales = None
@@ -727,14 +746,8 @@ class _VitsCommons:
             id_scales = []
             for b, (ph, (ids, src)) in enumerate(zip(phoneme_batches, maps)):
                 v = per_char[b]
-                if v is None:
-                    id_scales.append(None)
-                    continue
-                v = list(v) if not isinstance(v, np.ndarray) else v.reshape(-1).tolist()
-                if len(v) != len(ph):
-                    raise OperationError(f"utterance {b}: {len(v)} duration scales for {len(ph)} characters")
-                kept = {c: _scale_value(v[c], b, c, "character") for c in sorted(set(src)) if c >= 0}
-                id_scales.append([1.0 if c < 0 else kept[c] for c in src])
+                id_scales.append(None if v is None else
+                                 _char_values_to_ids(v, ph, src, b, "duration scales", _scale_value))
         extra = {} if seeds is None else {"seeds": seeds}
         if output_rates is not None:
             extra["output_rates"] = output_rates
@@ -955,16 +968,38 @@ def _stream_resampler(model, output_rate) -> Optional[Resampler]:
 class ProsodyStream:
     """One stream's pitch and tempo state on the device (sb200_prosody_stream_*): it carries the tails of the stream's
     input and stretched signal, and its last frames' offsets, between chunks, so the concatenation of what it emits is
-    the whole stream warped at once.  `pitch` / `tempo`: ratios as for infer_batch_with_values, not both neutral."""
+    the whole stream warped at once.  `pitch` / `tempo`: ratios as for infer_batch_with_values, not both neutral.
 
-    def __init__(self, model: "_VitsCommons", pitch=None, tempo=None):
+    `pitch_contour`: one pitch ratio per id of `enc` (the EncoderOutputs of the sentence the stream carries; values as
+    for infer_batch_with_values' pitch_contours), instead of `pitch` (sb200_prosody_stream_create_contour).  Its plan is
+    fixed by enc's frames, so the stream must be fed exactly enc's chunks; `bounds` then holds each id's delivered end
+    at the voice's rate (None without a contour)."""
+
+    def __init__(self, model: "_VitsCommons", pitch=None, tempo=None, pitch_contour=None,
+                 enc: Optional["EncoderOutputs"] = None):
         p, t = _prosody_arrays([pitch], [tempo], 1)
-        if p is None and t is None:
-            raise OperationError("a prosody stream needs a pitch or a tempo ratio other than 1 (None, NaN or 1: none)")
         self._m, self._h = model, C.c_void_p()
         self.pitch = None if p is None else float(p[0])
         self.tempo = None if t is None else float(t[0])
+        self.bounds = None
         err = N.sb200_error()
+        if pitch_contour is not None:
+            if p is not None:
+                raise OperationError("stream: a pitch contour and a pitch ratio together (give one or the other)")
+            if not isinstance(enc, EncoderOutputs) or enc._m is not model or not enc._h:
+                raise OperationError("a pitch contour needs the EncoderOutputs of its sentence, from this model")
+            c = _contour_arrays([len(enc.p_duration)], [pitch_contour], None, ["stream"])
+            if c is None:
+                c = np.full(len(enc.p_duration), np.nan, np.float32)
+            _check(model._lib.sb200_prosody_stream_create_contour(
+                model._h, enc._h, _ptr(c, C.c_float), c.size, float("nan") if t is None else float(t[0]),
+                C.byref(self._h), C.byref(err)), err)
+            self.bounds = np.zeros(c.size, np.int64)
+            _check(model._lib.sb200_prosody_stream_bounds(self._h, _ptr(self.bounds, C.c_int64), c.size,
+                                                          C.byref(err)), err)
+            return
+        if p is None and t is None:
+            raise OperationError("a prosody stream needs a pitch or a tempo ratio other than 1 (None, NaN or 1: none)")
         _check(model._lib.sb200_prosody_stream_create(model._h, float("nan") if p is None else float(p[0]),
                                                       float("nan") if t is None else float(t[0]), C.byref(self._h),
                                                       C.byref(err)), err)
@@ -984,12 +1019,28 @@ class ProsodyStream:
             pass
 
 
-def _stream_prosody(model, pitch, tempo) -> Optional[ProsodyStream]:
-    """A ProsodyStream for a stream with these ratios, or None when neither asks for anything."""
+def _stream_prosody(model, pitch, tempo, pitch_contour=None, enc=None) -> Optional[ProsodyStream]:
+    """A ProsodyStream for a stream with these ratios, or with this per-id contour of enc's sentence and the tempo, or
+    None when nothing asks for anything.  A given contour makes a contoured stream (which has bounds) whenever the
+    contour or the tempo asks for something; a contour of None / NaN / 1 only is no contour beside a pitch ratio, as in
+    the batch calls, and with neither a pitch nor a tempo it leaves the plain stream, which has no bounds."""
     p, t = _prosody_arrays([pitch], [tempo], 1)
+    if pitch_contour is not None:
+        asks = _contour_arrays([len(enc.p_duration)], [pitch_contour], p, ["stream"]) is not None
+        if asks or (p is None and t is not None):
+            return ProsodyStream(model, pitch, tempo, pitch_contour, enc)
     if p is None and t is None:
         return None
     return ProsodyStream(model, pitch, tempo)
+
+
+def _delivered_bounds(warp: Optional[ProsodyStream], resampler: Optional["Resampler"]):
+    """A contoured stream's per-id delivered ends at its delivered rate: ceil(end * up / down) with an output rate, as
+    the batch alignments place them; None for a stream without a contour."""
+    if warp is None or warp.bounds is None:
+        return None
+    up, down = rate_ratio(warp._m.audio_output_info().sample_rate, None if resampler is None else resampler.rate)
+    return -((-warp.bounds * up) // down)
 
 
 def _trim_frames(trim: slice) -> Tuple[int, int]:
@@ -1011,6 +1062,12 @@ class SpeechStreamer:
         self.resampler = resampler
         self.encoding, self.gain = encoding, gain
         self.warp = warp
+
+    @property
+    def bounds(self) -> Optional[np.ndarray]:
+        """Each id's delivered end (int64, one per id) at the stream's delivered rate when the stream has a pitch
+        contour (see ProsodyStream; with an output rate at ceil(end * up / down)), else None."""
+        return _delivered_bounds(self.warp, self.resampler)
 
     def __iter__(self) -> Iterator[AudioSamples]:
         return self
@@ -1194,25 +1251,37 @@ class VitsStreamingModel(_VitsCommons):
     def stream_synthesis(self, phonemes: str, chunk_size: int, chunk_padding: int,
                          seed: Optional[int] = None, output_rate: Optional[int] = None,
                          encoding: Optional[str] = None, gain: Optional[float] = None,
-                         pitch: Optional[float] = None, tempo: Optional[float] = None) -> SpeechStreamer:
+                         pitch: Optional[float] = None, tempo: Optional[float] = None,
+                         pitch_contour: Optional[Sequence] = None) -> SpeechStreamer:
         """`seed`: the sentence's noise seed (see infer_batch_with_values), or None for positional noise.
         `output_rate`: the chunks' sample rate (see infer_batch_with_values), the sentence resampled as one stream.
         `encoding`: "mulaw" / "alaw" for chunks of G.711 `bytes`: each is G.711 of to_i16_vec of the chunk the stream
         yields without an encoding, after the linear `gain` (None: 1; encoded streams only), encoded on the device.
         `pitch` / `tempo`: ratios as for infer_batch_with_values, the sentence warped as one stream on the device
         (ProsodyStream): the concatenation of the chunks is the sentence the stream yields without ratios, warped at
-        once, then resampled and encoded as without ratios."""
+        once, then resampled and encoded as without ratios.
+        `pitch_contour`: one pitch ratio per character of `phonemes` (as for speak_batch_with_alignment), applied to
+        that character's id and pad; it combines with `tempo` but not with `pitch`.  The concatenation of the chunks is
+        the sentence the stream yields without it, with that contour applied at once (sb200_debug_prosody_contour), and
+        the streamer's `bounds` give each id's delivered end."""
         if not isinstance(self, VitsStreamingModel):
             refuse_prosody(pitch, tempo, "stream_synthesis")
-        _prosody_arrays([pitch], [tempo], 1)
+            refuse_contour(pitch_contour, "stream_synthesis")
+        pit, _ = _prosody_arrays([pitch], [tempo], 1)
         _seed_arrays([seed], 1)
         _rate_array([output_rate], 1)
         refuse_flac(encoding, "stream_synthesis")
         g = _stream_gain(encoding, gain)
-        ids = self.phonemes_to_input_ids(phonemes)
+        contour = None
+        if pitch_contour is None:
+            ids = self.phonemes_to_input_ids(phonemes)
+        else:
+            ids, src = self.phonemes_to_input_ids_map(phonemes)
+            contour = _char_values_to_ids(pitch_contour, phonemes, src, "stream", "pitch ratios", _contour_value)
+            _contour_arrays([len(ids)], [contour], pit, ["stream"])
         enc = self.infer_encoder(ids) if seed is None else self.infer_encoder_batch([ids], seeds=[seed])[0]
         return SpeechStreamer(enc, chunk_size, chunk_padding, _stream_resampler(self, output_rate), encoding, g,
-                              _stream_prosody(self, pitch, tempo))
+                              _stream_prosody(self, pitch, tempo, contour, enc))
 
 
 def _stream_gain(encoding, gain) -> float:
@@ -1233,6 +1302,7 @@ class _Stream:
         self.key, self.enc, self.resampler = key, enc, resampler
         self.encoding, self.gain = encoding, gain
         self.warp = warp
+        self.bounds = _delivered_bounds(warp, resampler)
         self.chunker = AdaptiveMelChunker(enc.num_frames, chunk_size, chunk_padding)
         self.one_shot = enc.num_frames <= (chunk_size * 2 + chunk_padding * 2)
 
@@ -1279,28 +1349,36 @@ class StreamBatch:
         _check_chunking(chunk_size, chunk_padding)
         self.model = model
         self.chunk_size, self.chunk_padding = chunk_size, chunk_padding
-        self._pending: list = []      # (key, ids, config, chunk_size, seed, output rate, encoding, gain) not encoded yet
+        self._pending: list = []      # (key, ids, config, chunk_size, seed, output rate, encoding, gain, pitch, tempo,
+                                      # per-id contour) not encoded yet
         self._active: List[_Stream] = []
+        self._retired: dict = {}      # key -> delivered ends (None: no contour) of the streams the last step ended
         self._next_key = 0
 
     def add(self, ids_or_phonemes, config: Optional[PiperSynthesisConfig] = None, seed: Optional[int] = None,
             output_rate: Optional[int] = None, encoding: Optional[str] = None, gain: Optional[float] = None,
-            pitch: Optional[float] = None, tempo: Optional[float] = None) -> int:
+            pitch: Optional[float] = None, tempo: Optional[float] = None,
+            pitch_contour: Optional[Sequence] = None) -> int:
         """`seed`: the stream's noise seed (see infer_batch_with_values); a seeded stream yields what
         `stream_synthesis(..., seed=seed)` yields, whatever other streams share its encoder pass.  `output_rate`,
         `encoding` and `gain`: the stream's sample rate and G.711 encoding, as for stream_synthesis; `pitch` / `tempo`:
-        its ratios, as there.  A warped stream's chunks go through passes of their own, so the other streams keep their
-        passes and their bits."""
+        its ratios, as there.  `pitch_contour`: one pitch ratio per phoneme character (phonemes) or per id (ids), as
+        for stream_synthesis; its length and values are checked here, and what needs the sentence's frames fails as the
+        stream's error item.  `bounds(key)` gives a contoured stream's per-id delivered ends once it is encoded.  A
+        warped stream's chunks go through passes of their own, so the other streams keep their passes and their
+        bits."""
         if not isinstance(self.model, VitsStreamingModel):
             refuse_prosody(pitch, tempo, "StreamBatch")
-        return self._add(ids_or_phonemes, config, self.chunk_size, seed, output_rate, encoding, gain, pitch, tempo)
+            refuse_contour(pitch_contour, "StreamBatch")
+        return self._add(ids_or_phonemes, config, self.chunk_size, seed, output_rate, encoding, gain, pitch, tempo,
+                         pitch_contour)
 
     def _add(self, ids_or_phonemes, config, chunk_size: int, seed: Optional[int] = None,
              output_rate: Optional[int] = None, encoding: Optional[str] = None, gain: Optional[float] = None,
-             pitch: Optional[float] = None, tempo: Optional[float] = None) -> int:
+             pitch: Optional[float] = None, tempo: Optional[float] = None, pitch_contour=None) -> int:
         if config is not None and not isinstance(config, PiperSynthesisConfig):
             raise OperationError("Invalid configuration for Vits Model")
-        _prosody_arrays([pitch], [tempo], 1)
+        pit, _ = _prosody_arrays([pitch], [tempo], 1)
         _seed_arrays([seed], 1)
         _rate_array([output_rate], 1)
         refuse_flac(encoding, "StreamBatch")
@@ -1308,16 +1386,35 @@ class StreamBatch:
         if config is not None and config.speaker is not None and config.speaker not in (self.model.get_speakers() or {}):
             raise OperationError(f"No speaker was found with the given id `{config.speaker}`")     # as check_config
         _check_chunking(chunk_size, self.chunk_padding)
-        if isinstance(ids_or_phonemes, str):
+        contour = pitch_contour
+        if isinstance(ids_or_phonemes, str) and pitch_contour is not None:
+            ids, src = self.model.phonemes_to_input_ids_map(ids_or_phonemes)
+            contour = _char_values_to_ids(pitch_contour, ids_or_phonemes, src, f"stream {self._next_key}",
+                                          "pitch ratios", _contour_value)
+        elif isinstance(ids_or_phonemes, str):
             ids = self.model.phonemes_to_input_ids(ids_or_phonemes)
         else:
             ids = [int(i) for i in ids_or_phonemes]
+        if contour is not None:
+            _contour_arrays([len(ids)], [contour], pit, [f"stream {self._next_key}"])
         if not ids:
             raise OperationError("Failed to run model inference. Error: empty input sequence")
         key = self._next_key
         self._next_key += 1
-        self._pending.append((key, ids, config, chunk_size, seed, output_rate, encoding, gain, pitch, tempo))
+        self._pending.append((key, ids, config, chunk_size, seed, output_rate, encoding, gain, pitch, tempo, contour))
         return key
+
+    def bounds(self, key) -> Optional[np.ndarray]:
+        """Stream `key`'s per-id delivered ends at its delivered rate (see SpeechStreamer.bounds), or None when it has
+        no pitch contour.  Available from the step that encodes the stream until the next step after the one that
+        returns its last chunk (or its error): the batch keeps no state for a stream once that next step has run.
+        KeyError outside that window or for an unknown key."""
+        for s in self._active:
+            if s.key == key:
+                return s.bounds
+        if key in self._retired:
+            return self._retired[key]
+        raise KeyError(f"stream {key!r} is not encoded, or ended before the last step")
 
     def __len__(self) -> int:
         """Streams added and not yet finished."""
@@ -1346,7 +1443,7 @@ class StreamBatch:
                     try:
                         active.append(_Stream(p[0], enc, p[3], self.chunk_padding,
                                               _stream_resampler(self.model, p[5]), p[6], p[7],
-                                              _stream_prosody(self.model, p[8], p[9])))
+                                              _stream_prosody(self.model, p[8], p[9], p[10], enc)))
                         continue
                     except SonataError as e:
                         err = e
@@ -1393,6 +1490,7 @@ class StreamBatch:
                 a.crossfade(42)
             out.append((s.key, a))
         self._active = [s for s in active if not s.done and s.key not in failed]
+        self._retired = {s.key: s.bounds for s in active if s.done or s.key in failed}
         return out
 
 

@@ -14,9 +14,12 @@ K, one JSON line:
                     occupies whole 128-frame granules)
 The device name and power limit are printed first, read in the same run.  With --ratios the arms are StreamBatch runs
 with every stream at one pair of pitch / tempo ratios (none, pitch 1.25, tempo 1.5, pitch 0.8 with tempo 2), whose lines
-add the "stretch" and "pitch" device ms per step; audio_s_per_s is then at the delivered length.
+add the "stretch" and "pitch" device ms per step; audio_s_per_s is then at the delivered length.  With --contour they
+are StreamBatch runs with pitch contours on the same workload: no ratios, pitch 1.25, a uniform 1.25 contour (which
+gives pitch 1.25's chunks bit for bit), the question contour (1 on the first 75 % of ids, then rising in five steps to
+1.3) and per-id ratios drawn from {0.8, 1, 1.25} with a fixed seed, with the same added figures.
 
-  python tools/bench_streams.py [--ks 1,8,32,128] [--reps 1] [--ratios]
+  python tools/bench_streams.py [--ks 1,8,32,128] [--reps 1] [--ratios | --contour]
 """
 import argparse
 import atexit
@@ -92,9 +95,28 @@ RATIO_ARMS = {"none": {}, "pitch_1.25": {"pitch": 1.25}, "tempo_1.5": {"tempo": 
               "pitch_0.8_tempo_2": {"pitch": 0.8, "tempo": 2.0}}
 
 
+def question(k):
+    """The question contour over k ids: 1 on the first 75 %, then rising in five steps to 1.3."""
+    c = [1.0] * k
+    rise = k - int(0.75 * k)
+    for i in range(int(0.75 * k), k):
+        c[i] = 1.0 + 0.06 * (1 + (i - int(0.75 * k)) * 5 // rise)
+    return c
+
+
+def contour_arms(batches):
+    rng = np.random.default_rng(1234)
+    mixed = [list(rng.choice([0.8, 1.0, 1.25], len(b))) for b in batches]
+    return {"none": {}, "pitch_1.25": {"pitch": 1.25},
+            "contour_uniform_1.25": lambda s: {"pitch_contour": [1.25] * len(batches[s])},
+            "contour_question": lambda s: {"pitch_contour": question(len(batches[s]))},
+            "contour_mixed": lambda s: {"pitch_contour": mixed[s]}}
+
+
 def run_ratios(model, batches, sr, ratios):
-    """StreamBatch with every stream at `ratios`: the batch arm's figures plus the "stretch" and "pitch" device ms per
-    step (each warped pass's regions, summed over the passes of a step, averaged over the steps)."""
+    """StreamBatch with every stream at `ratios` (keyword arguments of StreamBatch.add, or a function of the stream's
+    index giving them): the batch arm's figures plus the "stretch" and "pitch" device ms per step (each warped pass's
+    regions, summed over the passes of a step, averaged over the steps)."""
     from sonata_b200 import StreamBatch
     decode = model.infer_decoder_batch
     prof = {"stretch": 0.0, "pitch": 0.0}
@@ -112,7 +134,7 @@ def run_ratios(model, batches, sr, ratios):
     try:
         sb = StreamBatch(model, CHUNK, PAD)
         t0 = time.perf_counter()
-        keys = [sb.add(ids, **ratios) for ids in batches]
+        keys = [sb.add(ids, **(ratios(s) if callable(ratios) else ratios)) for s, ids in enumerate(batches)]
         arrivals = {k: [] for k in keys}
         lens = {k: [] for k in keys}
         while len(sb):
@@ -168,6 +190,9 @@ def main():
     ap.add_argument("--ratios", action="store_true",
                     help="StreamBatch arms with pitch / tempo ratios instead (no ratios, pitch 1.25, tempo 1.5, pitch "
                          "0.8 with tempo 2), alternated in each rep; audio_s_per_s is at the delivered length")
+    ap.add_argument("--contour", action="store_true",
+                    help="StreamBatch arms with pitch contours instead (no ratios, pitch 1.25, uniform 1.25, question, "
+                         "mixed per-id ratios), alternated in each rep")
     args = ap.parse_args()
 
     import torch
@@ -191,6 +216,8 @@ def main():
     arms = {"stream_batch": run_batch, "threads": run_threads}
     if args.ratios:
         arms = {name: (lambda m, b, s, r=r: run_ratios(m, b, s, r)) for name, r in RATIO_ARMS.items()}
+    if args.contour:
+        arms = {name: (lambda m, b, s, r=r: run_ratios(m, b, s, r)) for name, r in contour_arms(batches).items()}
     for k in ks:
         for name, fn in arms.items():            # warm-up: modules, arenas and pinned blocks at this K
             fn(model, batches[:k], sr)
