@@ -267,6 +267,45 @@ int32_t sb200_speak_batch_ids_contour(sb200_voice* v, const int64_t* ids_packed,
                                       int32_t* id_frames_out, int64_t* bounds_out, double* lufs_out, float* gain_out,
                                       sb200_error* err);
 
+/* ---- formant ratios: the spectral envelope moved on its own ----
+ * The pitch ratios and contours above multiply every frequency, the formants (the spectral envelope) included, so a
+ * shifted voice sounds like a smaller or larger speaker.  A formant ratio phi per utterance (NaN: none; else a finite
+ * value in [0.5, 2], or OPERATION_ERROR naming the utterance before any device work) gives the delivered audio the
+ * voice's own envelope with every frequency multiplied by phi: phi = 1 with a pitch ratio or contour keeps the
+ * formants where they were (so unlike the other ratios, an explicit 1 asks for something when the utterance has a
+ * pitch), and phi != 1 without one moves them at the same pitch and duration.  The stage runs at the voice's rate R
+ * on the n2 samples y the pitch stage hands out (its stretched signal with a tempo only, the decoder's waveform with
+ * neither), after it and before any output-rate resampling and loudness.  It keeps the length: n2, the delivered ends,
+ * the frame counts and the alignments are those without it.  In double:
+ *  1. Frames.  N = 1024, H = 256, periodic Hann w[i] = 0.5 - 0.5 cos(2 pi i / N).  Frame m in [-3, ceil(n2 / H)) reads
+ *     y[m H + i], i < N, zero outside [0, n2); each output sample lies in exactly 4 frames.
+ *  2. Frame ratios.  c_m = clamp(m H + N / 2, 0, n2 - 1).  p_m is the utterance's pitch ratio (1 without one), or with
+ *     a contour the p_r of the piece with Q_{r-1} <= c_m < Q_r (step 3 of sb200_speak_batch_ids_contour).
+ *     r_m = p_m / phi, Q_m = floor(Q0 / p_m + 0.5) with Q0 = floor(R / 250): a 4 ms cutoff on the unshifted voice
+ *     (half the period of a 120 Hz voice), whose harmonics and formants y carries p_m times further apart.  A 2 ms
+ *     cutoff smooths formants of 80 - 120 Hz bandwidth away: it neither keeps them through a pitch shift nor moves
+ *     them at a fixed pitch.
+ *  3. Envelope.  X = rfft(w frame), P = |X|^2 (bins 0 .. N/2), eps = 1e-10 mean(P) + 1e-30, Lambda = log(P + eps) / 2,
+ *     c = irfft(Lambda) (the real cepstrum), lifter l[0] = 1, l[q] = l[N - q] = (1 + cos(pi q / Q_m)) / 2 for
+ *     1 <= q < Q_m, else 0, and E = Re rfft(c l), bins 0 .. N/2.
+ *  4. Gain.  Bin k reads u = k r_m: E^ = E[N/2] when u >= N/2, else E[i] + (u - i)(E[i + 1] - E[i]) with i = floor(u);
+ *     g_k = clamp(E^ - E[k], -G, G) with G = 1.2 ln 10 (24 dB as a natural-log amplitude).
+ *  5. Synthesis.  z_m = irfft(X e^g); out[j] = (sum_m w[j - m H] z_m[j - m H]) / 1.5 over its 4 frames in ascending m,
+ *     rounded to f32 once.
+ * An utterance runs the stage only when phi is finite and some frame has r_m != 1; any other keeps its bits (one with
+ * phi == its pitch ratio and no contour among them).  The kernels compute in double with their own FFTs and a fixed
+ * order per utterance, so an utterance has the same bits in any batch; a sample is within half an f32 ulp of the
+ * float64 specification's value plus 1e-11 (tests/formant_reference.py).  Realtime streams do not take a formant ratio.
+ * sb200_speak_batch_ids_contour with formants (NULL: none) one ratio per utterance.  NULL formants is that call, bit for
+ * bit. */
+int32_t sb200_speak_batch_ids_formants(sb200_voice* v, const int64_t* ids_packed, const size_t* offsets, size_t batch,
+                                       const sb200_synth_config* cfgs, const float* scale_packed,
+                                       const int32_t* frames_packed, const uint64_t* seeds, const int32_t* seeded,
+                                       const uint32_t* output_rates, const float* target_lufs, const float* pitch,
+                                       const float* tempo, const float* pitch_packed, const float* formants,
+                                       sb200_audio* outs, int32_t* id_frames_out, int64_t* bounds_out,
+                                       double* lufs_out, float* gain_out, sb200_error* err);
+
 /* ---- job API: the same batched pass split into its host<->device steps (bench / multi-GPU plumbing) ----
  * create  : copies ids to the device (H2D).  `eps_w` / `eps_z` optionally inject the graph's two
  *           RandomNormalLike draws (time-major: eps_w[b] = f32[T_x][2], eps_z[b] = f32[T_y][inter]);
@@ -327,6 +366,11 @@ int32_t sb200_job_prosody(const sb200_job* job, int64_t* n1, int64_t* n2, int32_
  * batch's cumulative durations to the host with the frame counts, and after it every result call reports the warped
  * signal, as after a run with ratios. */
 int32_t sb200_job_set_pitch_contour(sb200_job* job, const float* pitch_packed, sb200_error* err);
+/* Formant ratios (see sb200_speak_batch_ids_formants) for the next sb200_job_run, one per utterance, or NULL for none
+ * (what a new job starts with; so are ratios that are all NaN).  A bad entry fails naming the utterance and leaves the
+ * job as it was.  A ratio of 1 asks for something on an utterance with a pitch ratio or contour.  The result keeps
+ * its layout: the stage changes no length or offset. */
+int32_t sb200_job_set_formants(sb200_job* job, const float* formants, sb200_error* err);
 /* Each id's delivered end in the last run (see sb200_speak_batch_ids_contour), at the voice's rate, packed like
  * ids_packed, into out_packed[0 .. capacity).  Fails before a run, or when capacity is smaller than the number of ids. */
 int32_t sb200_job_prosody_bounds(sb200_job* job, int64_t* out_packed, size_t capacity, sb200_error* err);
@@ -670,6 +714,13 @@ int32_t sb200_debug_prosody_contour(int32_t device, const float* x, size_t n, in
                                     const float* ratios, size_t n_ids, float tempo, float* y, size_t cap,
                                     int32_t* offsets, size_t offsets_cap, float* stretched, size_t stretched_cap,
                                     sb200_error* err);
+/* The prosody chain and the formant stage over one caller buffer x[0 .. n) at `rate`: the pitch / tempo ratios (NaN or
+ * 1: none) or, with ends and ratios (n_ids entries; pitch must then be NaN), that contour and the tempo, then formant
+ * ratio phi.  pre[0 .. n2) receives the signal the formant stage reads, y[0 .. n2) its output (pre itself when the
+ * stage does not run), n2_out the length; bit for bit what a job gives an utterance of those samples and ends. */
+int32_t sb200_debug_formant(int32_t device, const float* x, size_t n, int32_t rate, float pitch, float tempo,
+                            const int64_t* ends, const float* ratios, size_t n_ids, float phi, float* pre, float* y,
+                            size_t cap, int64_t* n2_out, sb200_error* err);
 /* Test hook, no device needed: the samples a prosody stream with these ratios at `rate` emits per chunk (the rule of
  * sb200_decode_chunks_warped) when its chunks bring chunk_lens[0 .. n_chunks) inputs and the last one ends it.
  * emitted[k] receives chunk k's count.  Returns 0, or 19 for bad ratios, a bad rate or a negative length. */

@@ -105,6 +105,18 @@ SIGNATURES = {
                                                   C.POINTER(C.c_float), C.POINTER(C.c_float), C.POINTER(sb200_audio),
                                                   C.POINTER(C.c_int32), C.POINTER(C.c_int64), C.POINTER(C.c_double),
                                                   C.POINTER(C.c_float), _ERR]),
+    "sb200_speak_batch_ids_formants": (C.c_int32, [_P, C.POINTER(C.c_int64), C.POINTER(C.c_size_t), C.c_size_t,
+                                                   C.POINTER(sb200_synth_config), C.POINTER(C.c_float),
+                                                   C.POINTER(C.c_int32), C.POINTER(C.c_uint64), C.POINTER(C.c_int32),
+                                                   C.POINTER(C.c_uint32), C.POINTER(C.c_float), C.POINTER(C.c_float),
+                                                   C.POINTER(C.c_float), C.POINTER(C.c_float), C.POINTER(C.c_float),
+                                                   C.POINTER(sb200_audio), C.POINTER(C.c_int32), C.POINTER(C.c_int64),
+                                                   C.POINTER(C.c_double), C.POINTER(C.c_float), _ERR]),
+    "sb200_job_set_formants": (C.c_int32, [_P, C.POINTER(C.c_float), _ERR]),
+    "sb200_debug_formant": (C.c_int32, [C.c_int32, C.POINTER(C.c_float), C.c_size_t, C.c_int32, C.c_float, C.c_float,
+                                        C.POINTER(C.c_int64), C.POINTER(C.c_float), C.c_size_t, C.c_float,
+                                        C.POINTER(C.c_float), C.POINTER(C.c_float), C.c_size_t, C.POINTER(C.c_int64),
+                                        _ERR]),
     "sb200_job_create": (C.c_int32, [_P, C.POINTER(C.c_int64), C.POINTER(C.c_size_t), C.c_size_t,
                                      C.POINTER(C.POINTER(C.c_float)), C.POINTER(C.POINTER(C.c_float)),
                                      C.POINTER(C.c_size_t), C.POINTER(_P), _ERR]),

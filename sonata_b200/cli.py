@@ -21,7 +21,7 @@ from typing import Optional
 
 from . import from_config_path
 from .core import ENCODINGS, FLAC, OperationError, check_encoding
-from .piper import PiperSynthesisConfig, VitsStreamingModel, refuse_prosody
+from .piper import PiperSynthesisConfig, VitsStreamingModel, refuse_formants, refuse_prosody
 from .synth import AudioOutputConfig, SonataSpeechSynthesizer, _check_loudness, _check_prosody
 
 MODES = ("lazy", "parallel", "realtime")
@@ -57,6 +57,10 @@ def build_parser() -> argparse.ArgumentParser:
     ap.add_argument("--tempo", type=float, metavar="RATIO",
                     help="Play the speech RATIO times faster, [0.25, 4], at the same pitch, on the GPU (a waveform time "
                          "stretch: unlike --length-scale it keeps the model's articulation).  Not in realtime mode")
+    ap.add_argument("--formant-ratio", type=float, metavar="RATIO",
+                    help="Give the speech the voice's own formants (spectral envelope) with every frequency multiplied "
+                         "by RATIO, [0.5, 2], on the GPU after --pitch-ratio: 1 with a pitch ratio keeps the speaker's "
+                         "timbre, another value without one changes it at the same pitch.  Not in realtime mode")
     ap.add_argument("--encoding", choices=("pcm16",) + ENCODINGS + (FLAC,),
                     help="Output encoding: pcm16 (default), G.711 mulaw / alaw at one byte per sample (telephony: "
                          "PCMU / PCMA), or lossless flac (one FLAC stream per request, on stdout or in the -o file; "
@@ -70,7 +74,9 @@ def process_request(synth: SonataSpeechSynthesizer, default_cfg: PiperSynthesisC
     """process_synthesis_request (main.rs:126-165).  `seed` (optional): the request's noise seed, see
     synth.sentence_seed.  `output_rate` (optional): the sample rate of the WAV or raw PCM written.  `loudness`
     (optional): every sentence's target loudness in LUFS; the PCM is then written at the fixed scale.  `pitch_ratio` /
-    `tempo` (optional): the ratios every sentence is shifted and played by, in lazy and parallel modes."""
+    `tempo` (optional): the ratios every sentence is shifted and played by, in lazy and parallel modes.
+    `formant_ratio` (optional): the ratio every sentence's formants are moved by after the pitch stage, in lazy and
+    parallel modes (realtime mode refuses it unless it writes a file)."""
     out = out or sys.stdout.buffer
     mode = (req.get("mode") or "lazy").lower()
     loudness = req.get("loudness")
@@ -88,10 +94,12 @@ def process_request(synth: SonataSpeechSynthesizer, default_cfg: PiperSynthesisC
             raise OperationError("loudness normalisation is not available in realtime mode: integrated loudness needs "
                                  "the whole sentence, and realtime mode hands out a sentence's first chunk before its "
                                  "last one is decoded (use lazy or parallel mode)")
-    pros = {k: req[k] for k in ("pitch_ratio", "tempo") if req.get(k) is not None}
-    _check_prosody(pros.get("pitch_ratio"), pros.get("tempo"))
-    if mode == "realtime" and not output_file and not isinstance(synth.model, VitsStreamingModel):
-        refuse_prosody(pros.get("pitch_ratio"), pros.get("tempo"), "realtime mode")
+    pros = {k: req[k] for k in ("pitch_ratio", "tempo", "formant_ratio") if req.get(k) is not None}
+    _check_prosody(pros.get("pitch_ratio"), pros.get("tempo"), pros.get("formant_ratio"))
+    if mode == "realtime" and not output_file:
+        refuse_formants(pros.get("formant_ratio"), "realtime mode")
+        if not isinstance(synth.model, VitsStreamingModel):
+            refuse_prosody(pros.get("pitch_ratio"), pros.get("tempo"), "realtime mode")
     synth.model.set_fallback_synthesis_config(PiperSynthesisConfig(
         req.get("speaker_id"),
         req["noise_scale"] if req.get("noise_scale") is not None else default_cfg.noise_scale,
@@ -141,7 +149,7 @@ def main(argv=None) -> int:
                "pitch": args.pitch, "appended_silence_ms": args.silence, "chunk_size": args.chunk_size,
                "chunk_padding": args.chunk_padding, "seed": args.seed, "output_rate": args.output_rate,
                "loudness": args.loudness, "encoding": args.encoding, "pitch_ratio": args.pitch_ratio,
-               "tempo": args.tempo}
+               "tempo": args.tempo, "formant_ratio": args.formant_ratio}
         process_request(synth, default_cfg, req, args.output_file)
     else:
         for i, line in enumerate(sys.stdin):
@@ -160,6 +168,8 @@ def main(argv=None) -> int:
                 req["pitch_ratio"] = args.pitch_ratio
             if req.get("tempo") is None:
                 req["tempo"] = args.tempo
+            if req.get("formant_ratio") is None:
+                req["formant_ratio"] = args.formant_ratio
             out_file = None
             if args.output_file:
                 stem, ext = os.path.splitext(args.output_file)

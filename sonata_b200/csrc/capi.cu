@@ -288,13 +288,13 @@ static void job_prosody(const Job& j, int64_t* n1, int64_t* n2, int32_t* frames)
     }
 }
 
-int32_t sb200_speak_batch_ids_contour(sb200_voice* v, const int64_t* ids, const size_t* offsets, size_t batch,
-                                      const sb200_synth_config* cfgs, const float* scale_packed,
-                                      const int32_t* frames_packed, const uint64_t* seeds, const int32_t* seeded,
-                                      const uint32_t* output_rates, const float* target_lufs, const float* pitch,
-                                      const float* tempo, const float* pitch_packed, sb200_audio* outs,
-                                      int32_t* id_frames_out, int64_t* bounds_out, double* lufs_out, float* gain_out,
-                                      sb200_error* err) {
+int32_t sb200_speak_batch_ids_formants(sb200_voice* v, const int64_t* ids, const size_t* offsets, size_t batch,
+                                       const sb200_synth_config* cfgs, const float* scale_packed,
+                                       const int32_t* frames_packed, const uint64_t* seeds, const int32_t* seeded,
+                                       const uint32_t* output_rates, const float* target_lufs, const float* pitch,
+                                       const float* tempo, const float* pitch_packed, const float* formants,
+                                       sb200_audio* outs, int32_t* id_frames_out, int64_t* bounds_out,
+                                       double* lufs_out, float* gain_out, sb200_error* err) {
     return guarded(err, [&] {
         const double t0 = now_ms();
         static_assert(sizeof(long long) == sizeof(int64_t), "");
@@ -306,6 +306,7 @@ int32_t sb200_speak_batch_ids_contour(sb200_voice* v, const int64_t* ids, const 
         const bool loud = check_loudness_targets(target_lufs, batch);
         check_prosody(pitch, tempo, batch);
         check_pitch_contour(pitch_packed, offsets, batch, pitch);
+        check_formants(formants, batch);
         std::unique_ptr<Job> j(create_job(v->v.get(), reinterpret_cast<const long long*>(ids), offsets, batch, nullptr,
                                           nullptr, nullptr, false));
         if (cfgs) set_job_configs(*j, cfgs_in(cfgs, batch).data());
@@ -315,6 +316,7 @@ int32_t sb200_speak_batch_ids_contour(sb200_voice* v, const int64_t* ids, const 
         set_job_loudness(*j, target_lufs);
         set_job_prosody(*j, pitch, tempo);
         set_job_pitch_contour(*j, pitch_packed);
+        set_job_formants(*j, formants);
         j->run(nullptr, 0);
         fetch_audio(*j, outs, 0.f);
         if (id_frames_out) {
@@ -330,6 +332,17 @@ int32_t sb200_speak_batch_ids_contour(sb200_voice* v, const int64_t* ids, const 
         for (size_t b = 0; b < batch; b++)
             outs[b].inference_ms = wall * (j->out_total ? (float)outs[b].len / (float)j->out_total : 0.f);
     });
+}
+int32_t sb200_speak_batch_ids_contour(sb200_voice* v, const int64_t* ids, const size_t* offsets, size_t batch,
+                                      const sb200_synth_config* cfgs, const float* scale_packed,
+                                      const int32_t* frames_packed, const uint64_t* seeds, const int32_t* seeded,
+                                      const uint32_t* output_rates, const float* target_lufs, const float* pitch,
+                                      const float* tempo, const float* pitch_packed, sb200_audio* outs,
+                                      int32_t* id_frames_out, int64_t* bounds_out, double* lufs_out, float* gain_out,
+                                      sb200_error* err) {
+    return sb200_speak_batch_ids_formants(v, ids, offsets, batch, cfgs, scale_packed, frames_packed, seeds, seeded,
+                                          output_rates, target_lufs, pitch, tempo, pitch_packed, nullptr, outs,
+                                          id_frames_out, bounds_out, lufs_out, gain_out, err);
 }
 int32_t sb200_speak_batch_ids_prosody(sb200_voice* v, const int64_t* ids, const size_t* offsets, size_t batch,
                                       const sb200_synth_config* cfgs, const float* scale_packed,
@@ -439,6 +452,9 @@ int32_t sb200_job_prosody(const sb200_job* job, int64_t* n1, int64_t* n2, int32_
 }
 int32_t sb200_job_set_pitch_contour(sb200_job* job, const float* pitch_packed, sb200_error* err) {
     return guarded(err, [&] { set_job_pitch_contour(*job->j, pitch_packed); });
+}
+int32_t sb200_job_set_formants(sb200_job* job, const float* formants, sb200_error* err) {
+    return guarded(err, [&] { set_job_formants(*job->j, formants); });
 }
 int32_t sb200_job_prosody_bounds(sb200_job* job, int64_t* out_packed, size_t capacity, sb200_error* err) {
     return guarded(err, [&] {
@@ -1221,6 +1237,62 @@ int32_t sb200_debug_prosody_contour(int32_t device, const float* x, size_t n, in
         if (offsets && g.F) SB_CUDA(cudaMemcpy(offsets, doff, (size_t)g.F * 4, cudaMemcpyDeviceToHost));
         if (stretched && g.stretch)
             SB_CUDA(cudaMemcpy(stretched, g.pitch ? ds : dy, (size_t)g.n1 * 4, cudaMemcpyDeviceToHost));
+    });
+}
+
+int32_t sb200_debug_formant(int32_t device, const float* x, size_t n, int32_t rate, float pitch, float tempo,
+                            const int64_t* ends, const float* ratios, size_t n_ids, float phi, float* pre, float* y,
+                            size_t cap, int64_t* n2_out, sb200_error* err) {
+    return guarded(err, [&] {
+        if (!x || !pre || !y || n == 0 || n > (size_t)INT32_MAX || (n_ids && (!ends || !ratios)))
+            throw Error(19, "debug formant: bad arguments");
+        check_prosody(&pitch, &tempo, 1);
+        check_formants(&phi, 1);
+        const size_t offs[2] = {0, n_ids};
+        if (n_ids) check_pitch_contour(ratios, offs, 1, &pitch);
+        std::vector<ContourPiece> pc;
+        ProsodyPlan p;
+        p.add(n_ids ? prosody_contour_plan(rate, (long long)n, reinterpret_cast<const long long*>(ends), ratios, n_ids,
+                                           NAN, tempo, pc, nullptr)
+                    : prosody_shape(rate, (long long)n, pitch, tempo),
+              0, (long long)n, &pc);
+        const ProsodySeg& g = p.segs[0];
+        const bool prosody = g.stretch || g.pitch;
+        FormantPlan fp;
+        if (formant_asks(g.n2, phi, g.p, p.pieces.data() + g.c_off, g.c_n))
+            fp.add(rate, 0, g.n2, phi, g.p, g.c_off, g.c_n);
+        if ((size_t)g.n2 > cap) throw Error(19, "debug formant: a destination is too small for the result");
+        SB_CUDA(cudaSetDevice(device));
+        DeviceBuffers d;
+        // the pitch stage's output and the formant stage's
+        float* dy = d.alloc<float>((size_t)g.n2 + 4);
+        float* dz = d.alloc<float>((size_t)g.n2 + 4);
+        if (prosody) {
+            const float* dx = d.upload(x, n, n);
+            const ProsodySeg* dg = d.upload(&g, 1, 1);
+            const ContourPiece* dpc = p.pieces.empty() ? nullptr : d.upload(p.pieces.data(), p.pieces.size(), p.pieces.size());
+            int* doff = d.alloc<int>((size_t)g.F + 1);
+            long long* dap = d.alloc<long long>((size_t)g.F + 1);
+            float* ds = d.alloc<float>((size_t)p.s_total + 4);
+            if (p.smem_ints) launch_prosody_offsets(dx, dg, 1, p.smem_ints, doff, 0, dpc, dap);
+            launch_prosody_ola(dx, dg, 1, p.max_ola, doff, ds, dy, 0, dap);
+            if (p.max_pitch) launch_prosody_pitch(dx, ds, dg, 1, p.max_pitch, dy, 0, dpc);
+            if (!fp.segs.empty()) {
+                const FormantSeg* dfs = d.upload(fp.segs.data(), 1, 1);
+                launch_formant(dy, dfs, 1, fp.max_runs, dpc, dz, 0);
+            }
+        } else {
+            SB_CUDA(cudaMemcpy(dy, x, n * 4, cudaMemcpyHostToDevice));
+            if (!fp.segs.empty()) {
+                const FormantSeg* dfs = d.upload(fp.segs.data(), 1, 1);
+                launch_formant(dy, dfs, 1, fp.max_runs, nullptr, dz, 0);
+            }
+        }
+        SB_CUDA(cudaDeviceSynchronize());
+        SB_CUDA(cudaGetLastError());
+        SB_CUDA(cudaMemcpy(pre, dy, (size_t)g.n2 * 4, cudaMemcpyDeviceToHost));
+        SB_CUDA(cudaMemcpy(y, fp.segs.empty() ? dy : dz, (size_t)g.n2 * 4, cudaMemcpyDeviceToHost));
+        if (n2_out) *n2_out = g.n2;
     });
 }
 

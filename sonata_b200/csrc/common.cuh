@@ -321,6 +321,21 @@ __host__ __device__ inline long long contour_analysis(const ContourPiece& q, dou
     return (long long)floor((double)q.B + (kh - q.S) / q.alpha + 0.5);
 #endif
 }
+// The formant stage of one utterance (formant.cu): its n samples in[off ..) after the pitch stage leave as
+// out[off ..), their spectral envelope moved by p_m / phi per frame (include/sonata_b200.h,
+// sb200_speak_batch_ids_formants).  p_m is p, or with a contour (c_n > 0) the p of the pieces[c_off ..] piece whose
+// outputs hold the frame's centre.  Q0 = rate / 250: the lifter's cutoff at p_m = 1.
+constexpr int FM_N = 1024, FM_H = 256;   // frame and hop
+constexpr int FM_HOPS = 32;              // hops of output per CTA (each also analyses the 3 frames before them)
+struct FormantSeg {
+    long long off, n;
+    double p, phi;
+    int Q0, c_off, c_n;
+};
+// One launch over the segments: blockIdx.y = segment, blockIdx.x = its run of FM_HOPS hops (max_runs: the most runs of
+// any segment).  `in` and `out` are different buffers.
+void launch_formant(const float* in, const FormantSeg* segs, int nseg, long long max_runs, const ContourPiece* pieces,
+                    float* out, cudaStream_t st);
 // What a stream's chunk pass stages before the prosody launches and carries after them (prosody.cu): the chunk's
 // samples after the post-path (fsegs / posts entry `chunk`) follow h_in history inputs in the segment's input window,
 // h_s stretched samples of history start its stretched window and the deltas of frames d0, d0 + 1 start its offsets.

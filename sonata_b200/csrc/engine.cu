@@ -276,6 +276,11 @@ void set_job_pitch_contour(Job& j, const float* packed) {
         j.contour.clear();
 }
 
+void set_job_formants(Job& j, const float* phi) {
+    if (check_formants(phi, j.B)) j.formant.assign(phi, phi + j.B);
+    else j.formant.clear();
+}
+
 namespace {
 
 // Launches of one pass on context c's stream, each counted in the profile region of `regions` open at the time.  cond:
@@ -566,6 +571,23 @@ struct ProsodyBufs {
     }
 };
 
+// The formant launch's segments and their pinned mirror, and its output (`y`, laid out like its input) when it is the
+// resample launch's input or the job's result in a buffer of the pass's own.
+struct FormantBufs {
+    Staged<FormantSeg> segs;
+    float* y = nullptr;
+    void carve(Arena& dev, Arena& pin, const FormantPlan& p, bool own_y) {
+        y = nullptr;
+        if (p.segs.empty()) return;
+        segs.carve(dev, pin, p.segs.size());
+        if (own_y) y = dev.get<float>((size_t)p.total + 4);
+    }
+    void upload(const FormantPlan& p, cudaStream_t st) const {
+        std::copy(p.segs.begin(), p.segs.end(), segs.h);
+        segs.upload(st);
+    }
+};
+
 // The loudness launch over what a job hands out: one segment per utterance at its delivered rate, chunk scratch laid out
 // back to back.
 struct LoudnessPlan {
@@ -630,7 +652,8 @@ struct DecoderBufs {
 // the flow the decoder and (when the caller passed no buffer) the waveforms.  With prosody or output rates the decoder's
 // waveforms are always the pass's own.  The prosody output (plan `pp`) is the pass's own too unless it is the result
 // and the caller passed a buffer; the resampled waveforms go to the caller's buffer or to `rs`, with the tables of the
-// resampling launch `rp`.
+// resampling launch `rp`.  With the formant stage (plan `fp`) the stage before it writes into a buffer of the pass's
+// own, and the formant output, laid out the same way, goes to the caller's buffer or its own (fm.y).
 struct FrameBufs {
     FrameTables y;
     float *s, *epsz, *zp, *h, *acts, *outb, *wav;
@@ -639,17 +662,20 @@ struct FrameBufs {
     ResampleTables rt; float* rs;
     LoudnessBufs ld;
     ProsodyBufs pr;
-    void carve(Arena& dev, Arena& pin, const Job& j, const ProsodyPlan& pp, const ResamplePlan& rp, const LoudnessPlan& lp,
-               bool own_wav) {
+    FormantBufs fm;
+    void carve(Arena& dev, Arena& pin, const Job& j, const ProsodyPlan& pp, const FormantPlan& fp, const ResamplePlan& rp,
+               const LoudnessPlan& lp, bool own_wav) {
         rt.carve(dev, pin, rp.segs.size());
         ld.carve(dev, pin, lp);
-        pr.carve(dev, pin, pp, own_wav || !rp.segs.empty());
+        const bool formants = !fp.segs.empty();
+        pr.carve(dev, pin, pp, own_wav || !rp.segs.empty() || formants);
+        fm.carve(dev, pin, fp, own_wav || !rp.segs.empty());
         rs = nullptr;
         if (!rp.segs.empty()) {
             if (own_wav) rs = dev.get<float>((size_t)rp.total + 4);
             own_wav = true;
         }
-        if (!pp.segs.empty()) own_wav = true;
+        if (!pp.segs.empty() || formants) own_wav = true;
         const Arch& a = j.v->a;
         const size_t RY = (size_t)j.frames.RY;
         y.carve(dev, pin, j.frames);
@@ -833,9 +859,37 @@ ProsodyPlan lay_out_prosody(const Job& j, int hop, const std::vector<int>& cum, 
     return p;
 }
 
+// The formant launch of a job whose utterances ask for a formant ratio (an empty plan when none asks): each asking
+// utterance's output of the pitch stage (plan pp), or its decoder waveform when pp is empty, with its pitch ratio or
+// contour.  Its output has that stage's layout; the utterances that do not ask are copied into it.
+FormantPlan lay_out_formants(const Job& j, int hop, const ProsodyPlan& pp) {
+    FormantPlan p;
+    if (j.formant.empty() || j.encode_only) return p;
+    p.total = pp.segs.empty() ? j.frames.total_samples : pp.y_total;
+    for (size_t b = 0; b < j.B; b++) {
+        long long in_off, n;
+        double ratio = 1.0;
+        int c_off = 0, c_n = 0;
+        if (pp.segs.empty()) {
+            in_off = j.frames.fsegs[b].out_off; n = (long long)j.frames.fsegs[b].len * hop;
+        } else {
+            const ProsodySeg& g = pp.segs[b];
+            in_off = g.y_off; n = g.n2; ratio = g.p; c_off = g.c_off; c_n = g.c_n;
+        }
+        if (!formant_asks(n, j.formant[b], ratio, pp.pieces.data() + c_off, c_n)) {
+            p.copy(in_off, n);
+            continue;
+        }
+        p.add(j.v->sample_rate, in_off, n, j.formant[b], ratio, c_off, c_n);
+    }
+    if (p.segs.empty()) return FormantPlan();
+    return p;
+}
+
 // What the job hands out (osegs, out_hop, out_total): the frame layout itself without prosody and output rates (an empty
-// plan), the prosody output without output rates (an empty plan too), else the segments of the returned plan, one
-// utterance each at its rate, back to back, resampled from the prosody output when there is one.
+// plan), the prosody output without output rates (an empty plan too; the formant stage keeps its layout), else the
+// segments of the returned plan, one utterance each at its rate, back to back, resampled from the prosody output when
+// there is one.
 ResamplePlan lay_out_output(Job& j, int hop, const ProsodyPlan& pp) {
     ResamplePlan p;
     j.osr.assign(j.B, j.v->sample_rate);
@@ -884,6 +938,18 @@ void run_prosody(Runner& R, const ProsodyPlan& p, const ProsodyBufs& t, const fl
     R.begin("pitch");
     launch_prosody_pitch(wav, t.s, t.segs.d, n, p.max_pitch, y, R.st, t.pieces.d);
     R.count(p.pitch_flops, p.pitch_bytes);
+    R.end();
+}
+
+// The formant launch of plan `p` (tables `t`) from `in` into `out`, laid out alike, and the copies of the utterances
+// that do not ask: profile region "formant".
+void run_formant(Runner& R, const FormantPlan& p, const FormantBufs& t, const ContourPiece* pieces, const float* in,
+                 float* out) {
+    R.begin("formant");
+    for (const auto& c : p.copies)
+        SB_CUDA(cudaMemcpyAsync(out + c.first, in + c.first, (size_t)c.second * 4, cudaMemcpyDeviceToDevice, R.st));
+    launch_formant(in, t.segs.d, (int)p.segs.size(), p.max_runs, pieces, out, R.st);
+    R.count(p.flops, p.bytes);
     R.end();
 }
 
@@ -1233,12 +1299,14 @@ void Job::run(float* d_out, size_t d_out_cap) {
     std::vector<long long> bounds;
     const ProsodyPlan pp = lay_out_prosody(*this, a.hop(), cum_host, bounds);
     const bool prosody = !pp.segs.empty();
+    const FormantPlan fp = lay_out_formants(*this, a.hop(), pp);
+    const bool formants = !fp.segs.empty();
     const ResamplePlan rp = lay_out_output(*this, a.hop(), pp);
     const bool resample = !rp.segs.empty();
     const LoudnessPlan lp = lay_out_loudness(*this);
     loud_ran.clear(); loud_lufs.clear(); loud_gain.clear(); pros_ran.clear(); pros_bounds.clear();
     FrameBufs f;
-    plan(C.dev_frame, C.pin, [&](Arena& dev, Arena& pin) { f.carve(dev, pin, *this, pp, rp, lp, d_out == nullptr); });
+    plan(C.dev_frame, C.pin, [&](Arena& dev, Arena& pin) { f.carve(dev, pin, *this, pp, fp, rp, lp, d_out == nullptr); });
     d_osegs = resample ? f.rt.osegs.d : prosody ? f.pr.osegs.d : f.y.fsegs.d;
     if (debug) {
         expose(*this, "z_p", f.zp, I, 1); expose(*this, "z", f.s, I, 1);
@@ -1250,6 +1318,7 @@ void Job::run(float* d_out, size_t d_out_cap) {
     }
     Level LY = upload_frames(frames, f.y, st);
     if (prosody) f.pr.upload(pp, st);
+    if (formants) f.fm.upload(fp, st);
     if (resample) f.rt.upload(rp, st);
     if (!lp.segs.empty()) {
         std::copy(lp.segs.begin(), lp.segs.end(), f.ld.segs.h);
@@ -1311,15 +1380,22 @@ void Job::run(float* d_out, size_t d_out_cap) {
         if ((size_t)out_total > d_out_cap) throw Error(19, "caller-provided device output buffer is too small");
         d_wav = d_out;
     } else {
-        d_wav = f.rs ? f.rs : f.pr.y ? f.pr.y : f.wav;
+        d_wav = f.rs ? f.rs : f.fm.y ? f.fm.y : f.pr.y ? f.pr.y : f.wav;
     }
-    run_decoder(R, LY, f.y, f.dec, f.s, resample || prosody ? f.wav : d_wav);
-    // the output stage: prosody on the decoder's waveform, the resample launch on what that left, loudness on the result
-    const float* staged = f.wav; const FrameSeg* staged_segs = f.y.fsegs.d; int staged_hop = a.hop();
+    float* staged = resample || prosody || formants ? f.wav : d_wav;
+    run_decoder(R, LY, f.y, f.dec, f.s, staged);
+    // the output stage: prosody on the decoder's waveform, formants on what that left (in the same layout), the resample
+    // launch on the result, loudness on what that gives
+    const FrameSeg* staged_segs = f.y.fsegs.d; int staged_hop = a.hop();
     if (prosody) {
-        float* py = resample ? f.pr.y : d_wav;
+        float* py = resample || formants ? f.pr.y : d_wav;
         run_prosody(R, pp, f.pr, f.wav, py);
         staged = py; staged_segs = f.pr.osegs.d; staged_hop = 1;
+    }
+    if (formants) {
+        float* fy = resample ? f.fm.y : d_wav;
+        run_formant(R, fp, f.fm, f.pr.pieces.d, staged, fy);
+        staged = fy;
     }
     if (resample) run_resample(R, rp, f.rt, staged, staged_segs, f.rt.posts.d, staged_hop, d_wav);
     if (!lp.segs.empty()) run_loudness(R, lp, f.ld, d_wav);

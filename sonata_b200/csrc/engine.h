@@ -163,6 +163,27 @@ struct ProsodyPlan {
     void add_stream(const ProsodyStream& ps, const ProsodyStep& t);
 };
 
+// Formant ratios (formant.cu).  Checks phi[0 .. B) (null: none): NaN is none, anything else must be finite and in
+// [0.5, 2], or the call fails naming the utterance.  Returns whether some utterance has a ratio.  Unlike a pitch or tempo
+// ratio, phi = 1 asks for something whenever the utterance has a pitch ratio or contour.
+bool check_formants(const float* phi, size_t B);
+// Whether an utterance of n samples after the pitch stage, with pitch ratio p (pc / c_n: its contour's pieces, c_n = 0
+// for none) and formant ratio phi, runs the formant stage: phi is not NaN and some frame has p_m / phi != 1.
+bool formant_asks(long long n, float phi, double p, const ContourPiece* pc, int c_n);
+// The formant launch's segments, read from and written to the same offsets of two buffers laid out alike (the output
+// of the stage before it, `total` samples), the copies of the utterances that do not ask ((offset, samples), adjacent
+// ones merged), the CTA runs it is sized by and what the profile counts.
+struct FormantPlan {
+    std::vector<FormantSeg> segs;
+    std::vector<std::pair<long long, long long>> copies;
+    long long total = 0, max_runs = 0;
+    double flops = 0, bytes = 0;
+    // Appends an utterance of n samples at offset `off` at the voice's `rate`, with its ratios (see FormantSeg).
+    void add(int rate, long long off, long long n, float phi, double p, int c_off, int c_n);
+    // Appends the copy of an utterance that does not ask.
+    void copy(long long off, long long n);
+};
+
 // One stream's pitch and tempo state (prosody.cu): the shape of its ratios, its counts (inputs consumed, frames whose
 // delta is known, stretched samples computed, outputs emitted, and the history held of the inputs and the stretched
 // signal) and, on the device, two sets of buffers read and written alternately: the input tail (at most cap_in), the
@@ -357,6 +378,8 @@ struct Job {
                                       // (set_job_prosody)
     std::vector<float> contour;       // per-id pitch ratios, packed like ids, NaN or 1 = none; empty when no utterance
                                       // has a contour (set_job_pitch_contour)
+    std::vector<float> formant;       // one formant ratio per utterance, NaN = none; empty when none has one
+                                      // (set_job_formants)
     std::vector<ProsodyShape> pros_ran;   // each utterance's shape in the last run (empty: it ran no prosody stage)
     std::vector<float> pitch_ran, tempo_ran;   // the ratios the last run had (empty: none)
     std::vector<long long> pros_bounds;   // each id's delivered end in the last run when it had a contour (else empty)
@@ -427,6 +450,11 @@ void set_job_prosody(Job& j, const float* pitch, const float* tempo);
 // check_pitch_contour for the checks, which also refuse an utterance with a pitch ratio.  A bad entry leaves the job's
 // contour as it was.  Each utterance with a contour runs the prosody stage with its pieces (prosody_contour_plan).
 void set_job_pitch_contour(Job& j, const float* packed);
+// Per-utterance formant ratios of the job's next run (phi[0 .. B), NaN: none), or null for none; see check_formants.
+// An utterance that asks (formant_asks) runs the formant stage after the pitch stage, before any resampling and
+// loudness; its length, bounds, alignments and place in the job's result do not change.  A bad entry leaves the job's
+// ratios as they were.
+void set_job_formants(Job& j, const float* phi);
 // Each id's delivered end (prosody_contour_plan) in the job's last run, packed like its ids, at the voice's rate: kept
 // from the run when it had a contour, else computed from job_id_frames and the ratios it had.
 std::vector<long long> job_prosody_bounds(Job& j);

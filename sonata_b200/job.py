@@ -10,8 +10,8 @@ import numpy as np
 
 from . import _native as N
 from .core import G711_LAW, Audio, OperationError, check_encoding
-from .piper import (_check, _config_array, _contour_arrays, _duration_arrays, _gain_array, _loudness_array,
-                    _prosody_arrays, _ptr, _rate_array, _seed_arrays, _take_audio, _take_bytes)
+from .piper import (_check, _config_array, _contour_arrays, _duration_arrays, _formant_array, _gain_array,
+                    _loudness_array, _prosody_arrays, _ptr, _rate_array, _seed_arrays, _take_audio, _take_bytes)
 
 
 class SynthesisJob:
@@ -19,11 +19,13 @@ class SynthesisJob:
                  eps_z: Optional[Sequence] = None, debug: bool = False, configs: Optional[Sequence] = None,
                  seeds: Optional[Sequence] = None, output_rates: Optional[Sequence] = None,
                  loudness: Optional[Sequence] = None, pitches: Optional[Sequence] = None,
-                 tempos: Optional[Sequence] = None, pitch_contours: Optional[Sequence] = None):
+                 tempos: Optional[Sequence] = None, pitch_contours: Optional[Sequence] = None,
+                 formants: Optional[Sequence] = None):
         """`configs`: one PiperSynthesisConfig per utterance (see set_configs); None keeps the voice's fallback config.
         `seeds`: noise seeds (see set_seeds).  `output_rates`: output sample rates (see set_output_rates).
         `loudness`: loudness targets (see set_loudness).  `pitches` / `tempos`: pitch and tempo ratios (see
-        set_prosody).  `pitch_contours`: per-id pitch ratios (see set_pitch_contours)."""
+        set_prosody).  `pitch_contours`: per-id pitch ratios (see set_pitch_contours).  `formants`: formant ratios (see
+        set_formants)."""
         self._m = model
         self._lib = model._lib
         n = len(batches)
@@ -34,6 +36,7 @@ class SynthesisJob:
         _rate_array(output_rates, n)
         _loudness_array(loudness, n)
         _contour_arrays(self._lens, pitch_contours, _prosody_arrays(pitches, tempos, n)[0])
+        _formant_array(formants, n)
         packed = np.ascontiguousarray(np.concatenate([np.asarray(b, dtype=np.int64) for b in batches]))
         offs = np.zeros(n + 1, dtype=np.uint64)
         offs[1:] = np.cumsum([len(b) for b in batches])
@@ -76,6 +79,8 @@ class SynthesisJob:
             self.set_prosody(pitches, tempos)
         if pitch_contours is not None:
             self.set_pitch_contours(pitch_contours)
+        if formants is not None:
+            self.set_formants(formants)
 
     def set_configs(self, configs: Optional[Sequence]) -> None:
         """Per-utterance PiperSynthesisConfigs for the next run, or None for the voice's fallback config.  A wrong
@@ -157,6 +162,14 @@ class SynthesisJob:
         c = _contour_arrays(self._lens, contours)
         err = N.sb200_error()
         _check(self._lib.sb200_job_set_pitch_contour(self._h, _ptr(c, C.c_float), C.byref(err)), err)
+
+    def set_formants(self, formants: Optional[Sequence]) -> None:
+        """Per-utterance formant ratios for the next run (see VitsModel.infer_batch_with_values), or None for none.  A
+        ratio of 1.0 asks for something on an utterance with a pitch ratio or contour: its own formants.  A bad entry
+        raises OperationError naming the utterance and leaves the job's ratios as they were."""
+        f = _formant_array(formants, self.batch)
+        err = N.sb200_error()
+        _check(self._lib.sb200_job_set_formants(self._h, _ptr(f, C.c_float), C.byref(err)), err)
 
     def prosody_bounds(self) -> List[np.ndarray]:
         """Each id's delivered end in the last run, at the voice's rate, one int64 array per utterance (see

@@ -181,6 +181,7 @@ def _loudness_array(targets, n: int):
 
 PITCH_RANGE = (0.5, 2.0)     # pitch ratios a result can be shifted by
 TEMPO_RANGE = (0.25, 4.0)    # tempo ratios a result can be played at
+FORMANT_RANGE = (0.5, 2.0)   # formant ratios a result's spectral envelope can be moved by
 
 
 def _ratio_array(values, n: int, what: str, lo: float, hi: float):
@@ -205,6 +206,34 @@ def _prosody_arrays(pitches, tempos, n: int):
     given or when no utterance asks.  pitches[b] is a ratio in PITCH_RANGE, tempos[b] one in TEMPO_RANGE, or None / NaN /
     1.0 for an utterance that keeps its samples."""
     return _ratio_array(pitches, n, "pitch", *PITCH_RANGE), _ratio_array(tempos, n, "tempo", *TEMPO_RANGE)
+
+
+def _formant_array(values, n: int):
+    """The C image of per-utterance formant ratios (f32, NaN for none), or None when not given or when every entry is
+    None / NaN.  Unlike a pitch or tempo ratio, 1.0 asks for something: the voice's own formants under a pitch ratio or
+    contour."""
+    if values is None:
+        return None
+    out = np.full(n, np.nan, np.float32)
+    for b, v in enumerate(_per_utterance(values, n, "formant ratios")):
+        if v is None:
+            continue
+        if isinstance(v, bool) or not isinstance(v, numbers.Real):
+            raise OperationError(f"utterance {b}: formant ratio {v!r} is not a number")
+        if math.isnan(float(v)):
+            continue
+        if not (math.isfinite(float(v)) and FORMANT_RANGE[0] <= float(v) <= FORMANT_RANGE[1]):
+            raise OperationError(f"utterance {b}: formant ratio {float(v)} is not a finite value in "
+                                 f"[{FORMANT_RANGE[0]}, {FORMANT_RANGE[1]}] (None or NaN: none)")
+        out[b] = float(v)
+    return None if np.isnan(out).all() else out
+
+
+def refuse_formants(formant_ratio, where: str) -> None:
+    """OperationError when `where`, a mode that hands out a sentence chunk by chunk, is asked for a formant ratio."""
+    if formant_ratio is not None and not (isinstance(formant_ratio, numbers.Real) and math.isnan(float(formant_ratio))):
+        raise OperationError(f"{where} cannot apply a formant ratio: the formant stage is not carried from chunk to "
+                             "chunk (use speak_batch, a SynthesisJob or the lazy, parallel or file modes)")
 
 
 def _who(b) -> str:
@@ -532,27 +561,30 @@ class _VitsCommons:
                     configs: Optional[Sequence[PiperSynthesisConfig]] = None, seeds: Optional[Sequence] = None,
                     output_rates: Optional[Sequence] = None, loudness: Optional[Sequence] = None,
                     pitches: Optional[Sequence] = None, tempos: Optional[Sequence] = None,
-                    pitch_contours: Optional[Sequence] = None) -> List[Audio]:
+                    pitch_contours: Optional[Sequence] = None, formants: Optional[Sequence] = None) -> List[Audio]:
         """`configs`: one PiperSynthesisConfig per utterance (speaker and scales), still synthesised as one pass;
         None uses the fallback config for every utterance.  `seeds`: noise seeds as for infer_batch_with_values.
-        `output_rates` / `loudness` / `pitches` / `tempos`: per-utterance output sample rates, loudness targets and
-        pitch and tempo ratios as for infer_batch_with_values.  `pitch_contours`: as for speak_batch_with_alignment,
-        one ratio per phoneme character."""
+        `output_rates` / `loudness` / `pitches` / `tempos` / `formants`: per-utterance output sample rates, loudness
+        targets, pitch and tempo ratios and formant ratios as for infer_batch_with_values.  `pitch_contours`: as for
+        speak_batch_with_alignment, one ratio per phoneme character."""
         n = len(phoneme_batches)
         _config_array(configs, n)             # argument errors before any id mapping
         sv, _ = _seed_arrays(seeds, n)
         rates = _rate_array(output_rates, n)
         loud = _loudness_array(loudness, n)
         pros = any(a is not None for a in _prosody_arrays(pitches, tempos, n))
+        fmt = _formant_array(formants, n)
         if n == 0:
             return []
         if pitch_contours is not None:
             return [a for a, _ in self.speak_batch_with_alignment(phoneme_batches, configs, seeds=seeds,
                                                                   output_rates=output_rates, loudness=loudness,
                                                                   pitches=pitches, tempos=tempos,
-                                                                  pitch_contours=pitch_contours)]
-        if configs is not None or sv is not None or rates is not None or loud is not None or pros:
+                                                                  pitch_contours=pitch_contours, formants=formants)]
+        if configs is not None or sv is not None or rates is not None or loud is not None or pros or fmt is not None:
             extra = {} if sv is None else {"seeds": seeds}
+            if fmt is not None:
+                extra["formants"] = formants
             if pros:
                 extra.update(_prosody_kwargs(pitches, tempos))
             if rates is not None:
@@ -581,7 +613,8 @@ class _VitsCommons:
                                 output_rates: Optional[Sequence] = None,
                                 loudness: Optional[Sequence] = None, pitches: Optional[Sequence] = None,
                                 tempos: Optional[Sequence] = None,
-                                pitch_contours: Optional[Sequence] = None) -> List[Audio]:
+                                pitch_contours: Optional[Sequence] = None,
+                                formants: Optional[Sequence] = None) -> List[Audio]:
         """Batched infer_with_values.  `configs`: one PiperSynthesisConfig per utterance (speaker and scales), or None
         for the fallback config; each utterance's result equals a single-utterance call with its config as the
         fallback, except for the on-device noise of an unseeded utterance, whose draws depend on the batch position.
@@ -609,7 +642,14 @@ class _VitsCommons:
         `pitch_contours`: one pitch ratio per id for each utterance (in PITCH_RANGE, or None / NaN / 1.0 for none), or
         None.  Each id's samples are shifted by its own ratio and the id keeps its duration (divided by the utterance's
         tempo, which a contour combines with; an utterance's pitch ratio does not).  A contour whose ratio is the same
-        on every id gives the bits of that pitch ratio (sb200_speak_batch_ids_contour)."""
+        on every id gives the bits of that pitch ratio (sb200_speak_batch_ids_contour).
+
+        `formants`: one formant ratio per utterance (in FORMANT_RANGE, or None / NaN for none), or None.  The delivered
+        audio gets the voice's own spectral envelope with every frequency multiplied by the ratio, on the device after
+        the pitch stage (sb200_speak_batch_ids_formants): 1.0 with a pitch ratio or contour keeps the formants where
+        they were, so the voice sounds like the same speaker at another pitch (unlike the other ratios, an explicit 1.0
+        asks for something there), and a ratio without a pitch moves them at the same pitch and duration.  Lengths and
+        alignments do not change."""
         n = len(batches)
         cfgs = _config_array(configs, n)
         sv, _ = _seed_arrays(seeds, n)
@@ -618,10 +658,13 @@ class _VitsCommons:
         pit, tem = _prosody_arrays(pitches, tempos, n)
         pros = pit is not None or tem is not None
         contour = _contour_arrays([len(b) for b in batches], pitch_contours, pit)
-        if sv is not None or rates is not None or loud is not None or pros or contour is not None:
+        fmt = _formant_array(formants, n)
+        if sv is not None or rates is not None or loud is not None or pros or contour is not None or fmt is not None:
             extra = _prosody_kwargs(pitches, tempos) if pros else {}
             if contour is not None:
                 extra["pitch_contours"] = pitch_contours
+            if fmt is not None:
+                extra["formants"] = formants
             return [a for a, _ in self.infer_batch_with_durations(batches, configs, seeds=seeds,
                                                                   output_rates=output_rates, loudness=loudness,
                                                                   **extra)]
@@ -643,7 +686,8 @@ class _VitsCommons:
                                    output_rates: Optional[Sequence] = None,
                                    loudness: Optional[Sequence] = None, pitches: Optional[Sequence] = None,
                                    tempos: Optional[Sequence] = None,
-                                   pitch_contours: Optional[Sequence] = None) -> List[Tuple[Audio, np.ndarray]]:
+                                   pitch_contours: Optional[Sequence] = None,
+                                   formants: Optional[Sequence] = None) -> List[Tuple[Audio, np.ndarray]]:
         """infer_batch_with_values with per-id duration control, returning (audio, frames per id) per utterance.
 
         duration_scales[b]: one scale (finite, >= 0) per id of utterance b, applied before the duration's ceil, so 1.0
@@ -651,13 +695,13 @@ class _VitsCommons:
         Either list, or any of its entries, may be None.  The frame counts times 256 are each id's samples; an
         utterance whose ids all got 0 frames is still one frame long.  `seeds`: as for infer_batch_with_values; a
         seeded frame's noise depends on its index only, so controls that move frames never reshuffle it.
-        `output_rates` / `loudness` / `pitches` / `tempos` / `pitch_contours`: as for infer_batch_with_values (the
-        frame counts stay frame counts of the utterance before any warp)."""
+        `output_rates` / `loudness` / `pitches` / `tempos` / `pitch_contours` / `formants`: as for
+        infer_batch_with_values (the frame counts stay frame counts of the utterance before any warp)."""
         return [(a, f) for a, f, _ in self._speak_ids(batches, configs, duration_scales, durations, seeds, output_rates,
-                                                       loudness, pitches, tempos, pitch_contours)]
+                                                       loudness, pitches, tempos, pitch_contours, formants)]
 
     def _speak_ids(self, batches, configs, duration_scales, durations, seeds, output_rates, loudness, pitches, tempos,
-                   pitch_contours) -> List[Tuple[Audio, np.ndarray, Optional[np.ndarray]]]:
+                   pitch_contours, formants=None) -> List[Tuple[Audio, np.ndarray, Optional[np.ndarray]]]:
         """infer_batch_with_durations with each id's delivered end (None without a contour) per utterance."""
         n = len(batches)
         cfgs = _config_array(configs, n)
@@ -668,6 +712,7 @@ class _VitsCommons:
         loud = _loudness_array(loudness, n)
         pit, tem = _prosody_arrays(pitches, tempos, n)
         contour = _contour_arrays(lens, pitch_contours, pit)
+        fmt = _formant_array(formants, n)
         if n == 0:
             return []
         if any(x == 0 for x in lens):
@@ -679,7 +724,15 @@ class _VitsCommons:
         id_frames = np.zeros(int(offs[-1]), np.int32)
         err = N.sb200_error()
         bounds = None
-        if contour is None:
+        if fmt is not None:
+            bounds = None if contour is None else np.zeros(int(offs[-1]), np.int64)
+            _check(self._lib.sb200_speak_batch_ids_formants(
+                self._h, packed.ctypes.data_as(C.POINTER(C.c_int64)), offs.ctypes.data_as(C.POINTER(C.c_size_t)), n,
+                cfgs, _ptr(scales, C.c_float), _ptr(frames, C.c_int32), _ptr(sv, C.c_uint64), _ptr(sf, C.c_int32),
+                _ptr(rates, C.c_uint32), _ptr(loud, C.c_float), _ptr(pit, C.c_float), _ptr(tem, C.c_float),
+                _ptr(contour, C.c_float), _ptr(fmt, C.c_float), outs, _ptr(id_frames, C.c_int32),
+                _ptr(bounds, C.c_int64), None, None, C.byref(err)), err)
+        elif contour is None:
             _check(self._lib.sb200_speak_batch_ids_prosody(
                 self._h, packed.ctypes.data_as(C.POINTER(C.c_int64)), offs.ctypes.data_as(C.POINTER(C.c_size_t)), n,
                 cfgs, _ptr(scales, C.c_float), _ptr(frames, C.c_int32), _ptr(sv, C.c_uint64), _ptr(sf, C.c_int32),
@@ -702,8 +755,8 @@ class _VitsCommons:
                                    seeds: Optional[Sequence] = None,
                                    output_rates: Optional[Sequence] = None,
                                    loudness: Optional[Sequence] = None, pitches: Optional[Sequence] = None,
-                                   tempos: Optional[Sequence] = None, pitch_contours: Optional[Sequence] = None
-                                   ) -> List[Tuple[Audio, List[PhonemeAlignment]]]:
+                                   tempos: Optional[Sequence] = None, pitch_contours: Optional[Sequence] = None,
+                                   formants: Optional[Sequence] = None) -> List[Tuple[Audio, List[PhonemeAlignment]]]:
         """speak_batch that also says when each phoneme is spoken: per utterance (audio, alignment), the alignment
         holding one entry for bos (`^`), one per kept phoneme character (its id and its trailing pad) and one for eos
         (`$`), contiguous from sample 0 to len(audio).
@@ -720,7 +773,8 @@ class _VitsCommons:
         pitch_contours[b] (or None): one pitch ratio per character of phoneme_batches[b] (in PITCH_RANGE, or None / NaN
         / 1.0 for none), applied to that character's id and pad, bos and eos keeping their pitch; see
         infer_batch_with_values.  An utterance with a contour is aligned from each id's delivered end
-        (sb200_speak_batch_ids_contour), exact rather than scaled: with no tempo a boundary stays where it was."""
+        (sb200_speak_batch_ids_contour), exact rather than scaled: with no tempo a boundary stays where it was.
+        `formants`: as for infer_batch_with_values; it moves no boundary."""
         n = len(phoneme_batches)
         _config_array(configs, n)
         _seed_arrays(seeds, n)
@@ -755,13 +809,15 @@ class _VitsCommons:
             extra["loudness"] = loudness
         if any(warped):
             extra.update(_prosody_kwargs(pitches, tempos))
+        if _formant_array(formants, n) is not None:
+            extra["formants"] = formants
         if id_contours is None:
             res = [(a, f, None) for a, f in self.infer_batch_with_durations([m[0] for m in maps], configs, id_scales,
                                                                             **extra)]
         else:
             res = self._speak_ids([m[0] for m in maps], configs, id_scales, None, extra.get("seeds"),
                                   extra.get("output_rates"), extra.get("loudness"), extra.get("pitches"),
-                                  extra.get("tempos"), id_contours)
+                                  extra.get("tempos"), id_contours, extra.get("formants"))
         voice_rate = self.audio_output_info().sample_rate if output_rates is not None else None
         ratio = lambda audio: (1, 1) if voice_rate is None else rate_ratio(voice_rate, audio.info.sample_rate)
         shaped = [id_contours is not None and c is not None and any(not (math.isnan(x) or x == 1.0) for x in c)
@@ -773,14 +829,14 @@ class _VitsCommons:
                          configs: Optional[Sequence[PiperSynthesisConfig]] = None, seeds: Optional[Sequence] = None,
                          output_rates: Optional[Sequence] = None, loudness: Optional[Sequence] = None,
                          gains: Optional[Sequence] = None, pitches: Optional[Sequence] = None,
-                         tempos: Optional[Sequence] = None) -> List[bytes]:
+                         tempos: Optional[Sequence] = None, formants: Optional[Sequence] = None) -> List[bytes]:
         """infer_batch_with_values delivered as G.711 telephony audio: one `bytes` per utterance, one byte per sample.
         `law`: "mulaw" (PCMU) or "alaw" (PCMA), or one of those per utterance.  The bytes are G.711 of exactly the
         16-bit samples the i16 route gives (SynthesisJob.fetch_i16): to_i16_vec of the utterance after gains[b] (None:
         1), or the fixed scale for an utterance with a loudness target.  They are encoded on the device in the i16
         conversion's launches, so only one byte per sample leaves the card.  `configs`, `seeds`, `output_rates` and
-        `loudness` as for infer_batch_with_values, and so are `pitches` and `tempos`; a batch mixing laws runs one
-        conversion per law."""
+        `loudness` as for infer_batch_with_values, and so are `pitches`, `tempos` and `formants`; a batch mixing laws
+        runs one conversion per law."""
         from .job import SynthesisJob
         n = len(batches)
         _config_array(configs, n)
@@ -790,12 +846,13 @@ class _VitsCommons:
         laws = _encoding_list(law, n)
         _gain_array(gains, n)
         _prosody_arrays(pitches, tempos, n)
+        _formant_array(formants, n)
         if n == 0:
             return []
         if any(len(b) == 0 for b in batches):
             raise OperationError("Failed to run model inference. Error: empty input sequence")
         job = SynthesisJob(self, batches, configs=configs, seeds=seeds, output_rates=output_rates, loudness=loudness,
-                           pitches=pitches, tempos=tempos)
+                           pitches=pitches, tempos=tempos, formants=formants)
         try:
             job.run()
             out: List[Optional[bytes]] = [None] * n
@@ -812,24 +869,24 @@ class _VitsCommons:
                          configs: Optional[Sequence[PiperSynthesisConfig]] = None, seeds: Optional[Sequence] = None,
                          output_rates: Optional[Sequence] = None, loudness: Optional[Sequence] = None,
                          gains: Optional[Sequence] = None, pitches: Optional[Sequence] = None,
-                         tempos: Optional[Sequence] = None) -> List[bytes]:
+                         tempos: Optional[Sequence] = None, formants: Optional[Sequence] = None) -> List[bytes]:
         """speak_batch delivered as G.711 bytes: infer_batch_g711 over the phonemes' ids."""
         n = len(phoneme_batches)
         _config_array(configs, n)
         _encoding_list(law, n)
         return self.infer_batch_g711([self.phonemes_to_input_ids(p) for p in phoneme_batches], law, configs, seeds,
-                                     output_rates, loudness, gains, pitches, tempos)
+                                     output_rates, loudness, gains, pitches, tempos, formants)
 
     def infer_batch_flac(self, batches: Sequence[Sequence[int]],
                          configs: Optional[Sequence[PiperSynthesisConfig]] = None, seeds: Optional[Sequence] = None,
                          output_rates: Optional[Sequence] = None, loudness: Optional[Sequence] = None,
                          gains: Optional[Sequence] = None, pitches: Optional[Sequence] = None,
-                         tempos: Optional[Sequence] = None) -> List[bytes]:
+                         tempos: Optional[Sequence] = None, formants: Optional[Sequence] = None) -> List[bytes]:
         """infer_batch_with_values delivered as lossless FLAC: one complete stream (`bytes`) per utterance.  Its samples
         are exactly the 16-bit samples the i16 route gives (SynthesisJob.fetch_i16): to_i16_vec of the utterance after
         gains[b] (None: 1), or the fixed scale for an utterance with a loudness target, at its delivered rate.  They are
         encoded on the device, and only the compressed bytes leave the card.  `configs`, `seeds`, `output_rates`,
-        `loudness`, `pitches` and `tempos` as for infer_batch_with_values."""
+        `loudness`, `pitches`, `tempos` and `formants` as for infer_batch_with_values."""
         from .job import SynthesisJob
         n = len(batches)
         _config_array(configs, n)
@@ -838,12 +895,13 @@ class _VitsCommons:
         _loudness_array(loudness, n)
         _gain_array(gains, n)
         _prosody_arrays(pitches, tempos, n)
+        _formant_array(formants, n)
         if n == 0:
             return []
         if any(len(b) == 0 for b in batches):
             raise OperationError("Failed to run model inference. Error: empty input sequence")
         job = SynthesisJob(self, batches, configs=configs, seeds=seeds, output_rates=output_rates, loudness=loudness,
-                           pitches=pitches, tempos=tempos)
+                           pitches=pitches, tempos=tempos, formants=formants)
         try:
             job.run()
             return job.fetch_flac(gains)
@@ -854,11 +912,11 @@ class _VitsCommons:
                          configs: Optional[Sequence[PiperSynthesisConfig]] = None, seeds: Optional[Sequence] = None,
                          output_rates: Optional[Sequence] = None, loudness: Optional[Sequence] = None,
                          gains: Optional[Sequence] = None, pitches: Optional[Sequence] = None,
-                         tempos: Optional[Sequence] = None) -> List[bytes]:
+                         tempos: Optional[Sequence] = None, formants: Optional[Sequence] = None) -> List[bytes]:
         """speak_batch delivered as FLAC streams: infer_batch_flac over the phonemes' ids."""
         _config_array(configs, len(phoneme_batches))
         return self.infer_batch_flac([self.phonemes_to_input_ids(p) for p in phoneme_batches], configs, seeds,
-                                     output_rates, loudness, gains, pitches, tempos)
+                                     output_rates, loudness, gains, pitches, tempos, formants)
 
     def _cfg(self, fn) -> PiperSynthesisConfig:
         c, err = N.sb200_synth_config(), N.sb200_error()
@@ -1252,8 +1310,10 @@ class VitsStreamingModel(_VitsCommons):
                          seed: Optional[int] = None, output_rate: Optional[int] = None,
                          encoding: Optional[str] = None, gain: Optional[float] = None,
                          pitch: Optional[float] = None, tempo: Optional[float] = None,
-                         pitch_contour: Optional[Sequence] = None) -> SpeechStreamer:
-        """`seed`: the sentence's noise seed (see infer_batch_with_values), or None for positional noise.
+                         pitch_contour: Optional[Sequence] = None,
+                         formant_ratio: Optional[float] = None) -> SpeechStreamer:
+        """`formant_ratio` is refused: streams do not carry the formant stage.
+        `seed`: the sentence's noise seed (see infer_batch_with_values), or None for positional noise.
         `output_rate`: the chunks' sample rate (see infer_batch_with_values), the sentence resampled as one stream.
         `encoding`: "mulaw" / "alaw" for chunks of G.711 `bytes`: each is G.711 of to_i16_vec of the chunk the stream
         yields without an encoding, after the linear `gain` (None: 1; encoded streams only), encoded on the device.
@@ -1264,6 +1324,7 @@ class VitsStreamingModel(_VitsCommons):
         that character's id and pad; it combines with `tempo` but not with `pitch`.  The concatenation of the chunks is
         the sentence the stream yields without it, with that contour applied at once (sb200_debug_prosody_contour), and
         the streamer's `bounds` give each id's delivered end."""
+        refuse_formants(formant_ratio, "stream_synthesis")
         if not isinstance(self, VitsStreamingModel):
             refuse_prosody(pitch, tempo, "stream_synthesis")
             refuse_contour(pitch_contour, "stream_synthesis")
@@ -1358,7 +1419,7 @@ class StreamBatch:
     def add(self, ids_or_phonemes, config: Optional[PiperSynthesisConfig] = None, seed: Optional[int] = None,
             output_rate: Optional[int] = None, encoding: Optional[str] = None, gain: Optional[float] = None,
             pitch: Optional[float] = None, tempo: Optional[float] = None,
-            pitch_contour: Optional[Sequence] = None) -> int:
+            pitch_contour: Optional[Sequence] = None, formant_ratio: Optional[float] = None) -> int:
         """`seed`: the stream's noise seed (see infer_batch_with_values); a seeded stream yields what
         `stream_synthesis(..., seed=seed)` yields, whatever other streams share its encoder pass.  `output_rate`,
         `encoding` and `gain`: the stream's sample rate and G.711 encoding, as for stream_synthesis; `pitch` / `tempo`:
@@ -1366,7 +1427,8 @@ class StreamBatch:
         for stream_synthesis; its length and values are checked here, and what needs the sentence's frames fails as the
         stream's error item.  `bounds(key)` gives a contoured stream's per-id delivered ends once it is encoded.  A
         warped stream's chunks go through passes of their own, so the other streams keep their passes and their
-        bits."""
+        bits.  `formant_ratio` is refused: streams do not carry the formant stage."""
+        refuse_formants(formant_ratio, "StreamBatch")
         if not isinstance(self.model, VitsStreamingModel):
             refuse_prosody(pitch, tempo, "StreamBatch")
             refuse_contour(pitch_contour, "StreamBatch")

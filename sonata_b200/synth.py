@@ -115,19 +115,24 @@ def _check_loudness(target) -> None:
     _loudness_array([target], 1)
 
 
-def _check_prosody(pitch_ratio, tempo) -> None:
-    """Raises OperationError unless each is None or a ratio in piper.PITCH_RANGE / piper.TEMPO_RANGE."""
-    from .piper import _prosody_arrays
+def _check_prosody(pitch_ratio, tempo, formant_ratio=None) -> None:
+    """Raises OperationError unless each is None or a ratio in piper.PITCH_RANGE / piper.TEMPO_RANGE /
+    piper.FORMANT_RANGE."""
+    from .piper import _formant_array, _prosody_arrays
     _prosody_arrays([pitch_ratio], [tempo], 1)
+    _formant_array([formant_ratio], 1)
 
 
-def _prosody_extra(n: int, pitch_ratio, tempo) -> dict:
-    """The per-utterance keywords of n sentences that share a request's pitch ratio and tempo ({} without either)."""
-    from .piper import _prosody_arrays
+def _prosody_extra(n: int, pitch_ratio, tempo, formant_ratio=None) -> dict:
+    """The per-utterance keywords of n sentences that share a request's pitch ratio, tempo and formant ratio ({}
+    without any)."""
+    from .piper import _formant_array, _prosody_arrays
     p, t = _prosody_arrays([pitch_ratio], [tempo], 1)
     out = {} if p is None else {"pitches": [pitch_ratio] * n}
     if t is not None:
         out["tempos"] = [tempo] * n
+    if _formant_array([formant_ratio], 1) is not None:
+        out["formants"] = [formant_ratio] * n
     return out
 
 
@@ -182,10 +187,13 @@ class SonataSpeechSynthesizer:
     # loudness target), the output config's volume applied on the device as a gain before the conversion and its
     # silence appended as code-of-zero bytes.  `pitch_ratio` / `tempo` (lazy, parallel and file modes): each sentence's
     # frequencies multiplied by the ratio at the same duration / played that many times faster at the same pitch, on
-    # the device before any resampling and loudness (piper.PITCH_RANGE, piper.TEMPO_RANGE).
+    # the device before any resampling and loudness (piper.PITCH_RANGE, piper.TEMPO_RANGE).  `formant_ratio` (lazy,
+    # parallel and file modes): each sentence's spectral envelope moved by the ratio after the pitch stage; 1.0 with a
+    # pitch ratio keeps the voice's own formants (piper.FORMANT_RANGE).  The streamed modes refuse it by name.
 
     def _g711_batch(self, phs: List[str], encoding: str, seeds, output_rate, loudness,
-                    cfg: Optional[AudioOutputConfig], pitch_ratio=None, tempo=None) -> List[bytes]:
+                    cfg: Optional[AudioOutputConfig], pitch_ratio=None, tempo=None,
+                    formant_ratio=None) -> List[bytes]:
         """The G.711 bytes of sentences `phs`, one synthesis pass, each followed by its appended silence."""
         if cfg is not None:
             cfg._check_supported()
@@ -195,7 +203,7 @@ class SonataSpeechSynthesizer:
             extra["output_rates"] = [output_rate] * n
         if loudness is not None:
             extra["loudness"] = [loudness] * n
-        extra.update(_prosody_extra(n, pitch_ratio, tempo))
+        extra.update(_prosody_extra(n, pitch_ratio, tempo, formant_ratio))
         if not _device_g711(self.model):
             res = self.model.speak_batch(phs, **extra) if extra else self.model.speak_batch(phs)
             return [self._process(a, cfg).samples.as_g711_bytes(encoding, fixed_scale=loudness is not None)
@@ -212,18 +220,19 @@ class SonataSpeechSynthesizer:
     def synthesize_lazy(self, text: str, output_config: Optional[AudioOutputConfig] = None,
                         seed: Optional[int] = None, output_rate: Optional[int] = None,
                         loudness: Optional[float] = None, encoding: Optional[str] = None,
-                        pitch_ratio: Optional[float] = None, tempo: Optional[float] = None) -> Iterator[Audio]:
+                        pitch_ratio: Optional[float] = None, tempo: Optional[float] = None,
+                        formant_ratio: Optional[float] = None) -> Iterator[Audio]:
         sentence_seed(seed, 0)
         _check_output_rate(output_rate)
         _check_loudness(loudness)
-        _check_prosody(pitch_ratio, tempo)
+        _check_prosody(pitch_ratio, tempo, formant_ratio)
         refuse_flac(encoding, "synthesize_lazy")
         check_encoding(encoding)
-        pros = _prosody_extra(1, pitch_ratio, tempo)
+        pros = _prosody_extra(1, pitch_ratio, tempo, formant_ratio)
         for i, ph in enumerate(self._phonemes(text)):
             if encoding is not None:
                 yield self._g711_batch([ph], encoding, None if seed is None else [sentence_seed(seed, i)], output_rate,
-                                       loudness, output_config, pitch_ratio, tempo)[0]
+                                       loudness, output_config, pitch_ratio, tempo, formant_ratio)[0]
                 continue
             if output_rate or loudness is not None or pros:
                 extra = dict(pros) if seed is None else dict(pros, seeds=[sentence_seed(seed, i)])
@@ -240,20 +249,21 @@ class SonataSpeechSynthesizer:
     def synthesize_parallel(self, text: str, output_config: Optional[AudioOutputConfig] = None,
                             seed: Optional[int] = None, output_rate: Optional[int] = None,
                             loudness: Optional[float] = None, encoding: Optional[str] = None,
-                            pitch_ratio: Optional[float] = None, tempo: Optional[float] = None) -> Iterator[Audio]:
+                            pitch_ratio: Optional[float] = None, tempo: Optional[float] = None,
+                            formant_ratio: Optional[float] = None) -> Iterator[Audio]:
         sentence_seed(seed, 0)
         _check_output_rate(output_rate)
         _check_loudness(loudness)
-        _check_prosody(pitch_ratio, tempo)
+        _check_prosody(pitch_ratio, tempo, formant_ratio)
         refuse_flac(encoding, "synthesize_parallel")
         check_encoding(encoding)
         ph = self._phonemes(text)
         if encoding is not None:
             seeds = None if seed is None else [sentence_seed(seed, i) for i in range(len(ph))]
-            return iter(self._g711_batch(ph, encoding, seeds, output_rate, loudness, output_config, pitch_ratio, tempo)
-                        if ph else [])
+            return iter(self._g711_batch(ph, encoding, seeds, output_rate, loudness, output_config, pitch_ratio, tempo,
+                                         formant_ratio) if ph else [])
         extra = {"output_rates": [output_rate] * len(ph)} if output_rate else {}
-        extra.update(_prosody_extra(len(ph), pitch_ratio, tempo))
+        extra.update(_prosody_extra(len(ph), pitch_ratio, tempo, formant_ratio))
         if loudness is not None:
             extra["loudness"] = [loudness] * len(ph)
         if not ph:
@@ -268,13 +278,17 @@ class SonataSpeechSynthesizer:
                             chunk_size: int = 72, chunk_padding: int = 3,
                             seed: Optional[int] = None, output_rate: Optional[int] = None,
                             encoding: Optional[str] = None, pitch_ratio: Optional[float] = None,
-                            tempo: Optional[float] = None) -> Iterator[AudioSamples]:
+                            tempo: Optional[float] = None, formant_ratio: Optional[float] = None
+                            ) -> Iterator[AudioSamples]:
         """RealtimeSpeechStream (:337-382): a background producer pushes chunks into an unbounded channel;
         chunk_size is multiplied by the number of chunks already produced for every following sentence.
         `output_rate`: each sentence is resampled as its own stream (zero history at its start, flushed at its end).
         `encoding`: every chunk is G.711 bytes of its to_i16_vec after the volume, encoded on the device.
         `pitch_ratio` / `tempo`: every sentence warped as its own stream on the device (a fresh piper.ProsodyStream,
-        flushed at its end); appended silence is not warped."""
+        flushed at its end); appended silence is not warped.  `formant_ratio` is refused: streams do not carry the
+        formant stage."""
+        from .piper import refuse_formants
+        refuse_formants(formant_ratio, "synthesize_streamed")
         pros = _stream_prosody_extra(self.model, pitch_ratio, tempo, "synthesize_streamed")
         sentence_seed(seed, 0)
         _check_output_rate(output_rate)
@@ -330,7 +344,8 @@ class SonataSpeechSynthesizer:
     def synthesize_to_file(self, filename, text: str, output_config: Optional[AudioOutputConfig] = None,
                            seed: Optional[int] = None, output_rate: Optional[int] = None,
                            loudness: Optional[float] = None, encoding: Optional[str] = None,
-                           pitch_ratio: Optional[float] = None, tempo: Optional[float] = None) -> None:
+                           pitch_ratio: Optional[float] = None, tempo: Optional[float] = None,
+                           formant_ratio: Optional[float] = None) -> None:
         """:168-198 — parallel mode, concatenated, peak-normalised i16 WAV (at output_rate when given).  With
         `loudness` the WAV is written at the fixed scale (trunc(clamp(x * 32767))), so it keeps the sentences' level.
         With `encoding` the WAV is 8-bit G.711 (WAVE_FORMAT_MULAW / _ALAW, with a `fact` chunk) holding the sentences'
@@ -338,7 +353,7 @@ class SonataSpeechSynthesizer:
         With encoding="flac" the file is one FLAC stream (synthesize_flac) instead of a WAV."""
         if isinstance(encoding, str) and encoding == FLAC:
             data = self.synthesize_flac(text, output_config, seed=seed, output_rate=output_rate, loudness=loudness,
-                                        pitch_ratio=pitch_ratio, tempo=tempo)
+                                        pitch_ratio=pitch_ratio, tempo=tempo, formant_ratio=formant_ratio)
             with open(filename, "wb") as f:
                 f.write(data)
             return
@@ -349,6 +364,8 @@ class SonataSpeechSynthesizer:
             extra["pitch_ratio"] = pitch_ratio
         if tempo is not None:
             extra["tempo"] = tempo
+        if formant_ratio is not None:
+            extra["formant_ratio"] = formant_ratio
         if check_encoding(encoding) is not None:
             data = b"".join(self.synthesize_parallel(text, output_config, seed=seed, encoding=encoding, **extra))
             if not data:
@@ -356,11 +373,11 @@ class SonataSpeechSynthesizer:
             with open(filename, "wb") as f:
                 f.write(g711_wave_bytes(data, encoding, output_rate or self.model.audio_output_info().sample_rate))
             return
-        self._document(text, output_config, seed, output_rate, loudness, pitch_ratio, tempo).save_to_file(
+        self._document(text, output_config, seed, output_rate, loudness, pitch_ratio, tempo, formant_ratio).save_to_file(
             filename, fixed_scale=loudness is not None)
 
     def _document(self, text: str, output_config: Optional[AudioOutputConfig], seed, output_rate, loudness,
-                  pitch_ratio=None, tempo=None) -> Audio:
+                  pitch_ratio=None, tempo=None, formant_ratio=None) -> Audio:
         """The sentences of synthesize_parallel concatenated: what synthesize_to_file writes as a WAV."""
         extra = {"output_rate": output_rate} if output_rate else {}
         if loudness is not None:
@@ -369,6 +386,8 @@ class SonataSpeechSynthesizer:
             extra["pitch_ratio"] = pitch_ratio
         if tempo is not None:
             extra["tempo"] = tempo
+        if formant_ratio is not None:
+            extra["formant_ratio"] = formant_ratio
         parts = [a.samples.as_slice() for a in self.synthesize_parallel(text, output_config, seed=seed, **extra)]
         if not parts or sum(len(p) for p in parts) == 0:
             raise OperationError("No speech data to write")
@@ -378,11 +397,11 @@ class SonataSpeechSynthesizer:
     def synthesize_flac(self, text: str, output_config: Optional[AudioOutputConfig] = None,
                         seed: Optional[int] = None, output_rate: Optional[int] = None,
                         loudness: Optional[float] = None, pitch_ratio: Optional[float] = None,
-                        tempo: Optional[float] = None) -> bytes:
+                        tempo: Optional[float] = None, formant_ratio: Optional[float] = None) -> bytes:
         """The FLAC file synthesize_to_file(..., encoding="flac") writes: one stream whose decoded samples are exactly
         the 16-bit samples of the WAV the same call writes without an encoding (the concatenation at the document's
         peak, or the fixed scale with `loudness`), encoded on the model's device by flac_encode."""
-        doc = self._document(text, output_config, seed, output_rate, loudness, pitch_ratio, tempo)
+        doc = self._document(text, output_config, seed, output_rate, loudness, pitch_ratio, tempo, formant_ratio)
         s = doc.samples
         return flac_encode(s.to_i16_fixed() if loudness is not None else s.to_i16_vec(), doc.info.sample_rate,
                            getattr(self.model, "device", 0))
@@ -427,10 +446,13 @@ class RealtimeBatch:
 
     def add(self, text: str, output_config: Optional[AudioOutputConfig] = None, config=None,
             seed: Optional[int] = None, output_rate: Optional[int] = None, encoding: Optional[str] = None,
-            pitch_ratio: Optional[float] = None, tempo: Optional[float] = None) -> int:
+            pitch_ratio: Optional[float] = None, tempo: Optional[float] = None,
+            formant_ratio: Optional[float] = None) -> int:
         """`seed`: the request's noise seed, `output_rate` its sample rate and `encoding` its G.711 encoding, as for
-        synthesize_streamed, and `pitch_ratio` / `tempo` its ratios, each sentence warped as its own stream, as there."""
-        from .piper import PiperSynthesisConfig
+        synthesize_streamed, and `pitch_ratio` / `tempo` its ratios, each sentence warped as its own stream, as there.
+        `formant_ratio` is refused, as there."""
+        from .piper import PiperSynthesisConfig, refuse_formants
+        refuse_formants(formant_ratio, "RealtimeBatch")
         pros = _stream_prosody_extra(self.model, pitch_ratio, tempo, "RealtimeBatch")
         sentence_seed(seed, 0)
         _check_output_rate(output_rate)
