@@ -306,6 +306,37 @@ int32_t sb200_speak_batch_ids_formants(sb200_voice* v, const int64_t* ids_packed
                                        sb200_audio* outs, int32_t* id_frames_out, int64_t* bounds_out,
                                        double* lufs_out, float* gain_out, sb200_error* err);
 
+/* ---- speaker blends: a voice between the speakers of a multi-speaker voice ----
+ * A speaker reaches the model through one vector g (the reference's emb_g(sid)).  A blend of an utterance or stream is
+ * n >= 1 pairs (s_i, u_i): distinct speaker ids of the voice (values of its speaker_id_map) and finite f32 weights
+ * u_i >= 0, at least one of them > 0.  Any other blend (an unknown or repeated id, a negative, NaN or infinite weight,
+ * all weights zero, an empty blend, or any blend on a single-speaker voice) fails with OPERATION_ERROR before any device
+ * work, naming the utterance (or stream) and the speaker or weight, and leaves the job or batch as it was.
+ *  1. Canonical form: drop the pairs with u_i = 0 and sort the rest by s ascending; U = sum of (double) u_i in that
+ *     order, and w_i = (float)((double) u_i / U).
+ *  2. Embedding: acc = 0.0f, then acc = fmaf(w_i, emb_g[s_i][k], acc) for each i in canonical order; g[k] = acc.
+ *  3. Conditioning: the effective biases base[r] + sum_k W[r][k] g[k] of every speaker-conditioned 1x1 conv (the
+ *     duration predictor's, every flow WaveNet's and the vocoder input's), computed as for a plain speaker with g in
+ *     place of emb_g(sid): in a batch pass, in an encoder pass and in every decoder chunk pass of its latents.
+ *  4. The blend replaces the config's speaker; the config's noise_scale, length_scale and noise_w still apply.
+ * So a blend whose canonical form is one speaker s (any positive weight, with or without zero-weight extras) has w = 1
+ * and g = emb_g[s]: the bits of that speaker.  Blends with the same canonical form (reordered, with zero weights added,
+ * or every weight scaled by a power of two) give the same bits, and a blended utterance has the same bits in any batch
+ * (with seeded or injected noise).  Equal canonical blends of a pass share one speaker slot, and a one-speaker blend
+ * shares the slot of that plain speaker; a pass in which no slot blends two or more speakers runs as it does without
+ * blends, with the same launches.
+ * A blend table is three arrays: blend_speakers and blend_weights, and blend_offsets[0 .. batch] (offsets[0] = 0):
+ * utterance b's pairs are [offsets[b], offsets[b + 1]), and an empty range means no blend for that utterance.
+ * sb200_speak_batch_ids_formants with a blend table (NULL blend_offsets: none).  NULL is that call, bit for bit. */
+int32_t sb200_speak_batch_ids_blends(sb200_voice* v, const int64_t* ids_packed, const size_t* offsets, size_t batch,
+                                     const sb200_synth_config* cfgs, const float* scale_packed,
+                                     const int32_t* frames_packed, const uint64_t* seeds, const int32_t* seeded,
+                                     const uint32_t* output_rates, const float* target_lufs, const float* pitch,
+                                     const float* tempo, const float* pitch_packed, const float* formants,
+                                     const int64_t* blend_speakers, const float* blend_weights,
+                                     const size_t* blend_offsets, sb200_audio* outs, int32_t* id_frames_out,
+                                     int64_t* bounds_out, double* lufs_out, float* gain_out, sb200_error* err);
+
 /* ---- job API: the same batched pass split into its host<->device steps (bench / multi-GPU plumbing) ----
  * create  : copies ids to the device (H2D).  `eps_w` / `eps_z` optionally inject the graph's two
  *           RandomNormalLike draws (time-major: eps_w[b] = f32[T_x][2], eps_z[b] = f32[T_y][inter]);
@@ -371,6 +402,11 @@ int32_t sb200_job_set_pitch_contour(sb200_job* job, const float* pitch_packed, s
  * job as it was.  A ratio of 1 asks for something on an utterance with a pitch ratio or contour.  The result keeps
  * its layout: the stage changes no length or offset. */
 int32_t sb200_job_set_formants(sb200_job* job, const float* formants, sb200_error* err);
+/* Speaker blends (see sb200_speak_batch_ids_blends) for the next sb200_job_run as a blend table, or NULL offsets for none
+ * (what a new job starts with).  Every entry is checked first; a bad one fails with OPERATION_ERROR naming the utterance
+ * and leaves the job's blends as they were. */
+int32_t sb200_job_set_speaker_blends(sb200_job* job, const int64_t* blend_speakers, const float* blend_weights,
+                                     const size_t* blend_offsets, sb200_error* err);
 /* Each id's delivered end in the last run (see sb200_speak_batch_ids_contour), at the voice's rate, packed like
  * ids_packed, into out_packed[0 .. capacity).  Fails before a run, or when capacity is smaller than the number of ids. */
 int32_t sb200_job_prosody_bounds(sb200_job* job, int64_t* out_packed, size_t capacity, sb200_error* err);
@@ -467,6 +503,14 @@ int32_t sb200_encode_batch_ids_seeded(sb200_voice* v, const int64_t* ids_packed,
                                       const sb200_synth_config* cfgs, const float* scale_packed,
                                       const int32_t* frames_packed, const uint64_t* seeds, const int32_t* seeded,
                                       sb200_latent** outs, sb200_error* err);
+/* sb200_encode_batch_ids_seeded with a blend table (see sb200_speak_batch_ids_blends); NULL is that call, bit for bit.
+ * Each latent keeps its utterance's canonical blend (or plain speaker), and every decoder chunk pass of it conditions on
+ * that blend. */
+int32_t sb200_encode_batch_ids_blends(sb200_voice* v, const int64_t* ids_packed, const size_t* offsets, size_t batch,
+                                      const sb200_synth_config* cfgs, const float* scale_packed,
+                                      const int32_t* frames_packed, const uint64_t* seeds, const int32_t* seeded,
+                                      const int64_t* blend_speakers, const float* blend_weights,
+                                      const size_t* blend_offsets, sb200_latent** outs, sb200_error* err);
 /* The encoder's `p_duration` (piper/src/lib.rs:675, 706-717) as frames per id of the latent's utterance (their sum is
  * its frame count, except that an utterance whose ids all got 0 frames is 1 frame long).  Returns the number of ids;
  * writes them to out only when capacity is at least that (call with NULL, 0 to learn the size). */
@@ -714,6 +758,11 @@ int32_t sb200_debug_prosody_contour(int32_t device, const float* x, size_t n, in
                                     const float* ratios, size_t n_ids, float tempo, float* y, size_t cap,
                                     int32_t* offsets, size_t offsets_cap, float* stretched, size_t stretched_cap,
                                     sb200_error* err);
+/* Test hook: the blended embedding g (gin floats) and the effective biases (cond_rows floats) a pass computes for the
+ * blend of pairs (speakers[i], weights[i]), i < n, checked as in sb200_speak_batch_ids_blends, through the same launches:
+ * bit for bit what a pass conditions on.  Fails when g_cap or bias_cap is too small. */
+int32_t sb200_debug_speaker_blend(sb200_voice* v, const int64_t* speakers, const float* weights, size_t n, float* g,
+                                  size_t g_cap, float* bias, size_t bias_cap, sb200_error* err);
 /* The prosody chain and the formant stage over one caller buffer x[0 .. n) at `rate`: the pitch / tempo ratios (NaN or
  * 1: none) or, with ends and ratios (n_ids entries; pitch must then be NaN), that contour and the tempo, then formant
  * ratio phi.  pre[0 .. n2) receives the signal the formant stage reads, y[0 .. n2) its output (pre itself when the

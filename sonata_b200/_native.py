@@ -113,6 +113,19 @@ SIGNATURES = {
                                                    C.POINTER(sb200_audio), C.POINTER(C.c_int32), C.POINTER(C.c_int64),
                                                    C.POINTER(C.c_double), C.POINTER(C.c_float), _ERR]),
     "sb200_job_set_formants": (C.c_int32, [_P, C.POINTER(C.c_float), _ERR]),
+    "sb200_speak_batch_ids_blends": (C.c_int32, [_P, C.POINTER(C.c_int64), C.POINTER(C.c_size_t), C.c_size_t,
+                                                 C.POINTER(sb200_synth_config), C.POINTER(C.c_float),
+                                                 C.POINTER(C.c_int32), C.POINTER(C.c_uint64), C.POINTER(C.c_int32),
+                                                 C.POINTER(C.c_uint32), C.POINTER(C.c_float), C.POINTER(C.c_float),
+                                                 C.POINTER(C.c_float), C.POINTER(C.c_float), C.POINTER(C.c_float),
+                                                 C.POINTER(C.c_int64), C.POINTER(C.c_float), C.POINTER(C.c_size_t),
+                                                 C.POINTER(sb200_audio), C.POINTER(C.c_int32), C.POINTER(C.c_int64),
+                                                 C.POINTER(C.c_double), C.POINTER(C.c_float), _ERR]),
+    "sb200_job_set_speaker_blends": (C.c_int32, [_P, C.POINTER(C.c_int64), C.POINTER(C.c_float),
+                                                 C.POINTER(C.c_size_t), _ERR]),
+    "sb200_debug_speaker_blend": (C.c_int32, [_P, C.POINTER(C.c_int64), C.POINTER(C.c_float), C.c_size_t,
+                                              C.POINTER(C.c_float), C.c_size_t, C.POINTER(C.c_float), C.c_size_t,
+                                              _ERR]),
     "sb200_debug_formant": (C.c_int32, [C.c_int32, C.POINTER(C.c_float), C.c_size_t, C.c_int32, C.c_float, C.c_float,
                                         C.POINTER(C.c_int64), C.POINTER(C.c_float), C.c_size_t, C.c_float,
                                         C.POINTER(C.c_float), C.POINTER(C.c_float), C.c_size_t, C.POINTER(C.c_int64),
@@ -161,6 +174,11 @@ SIGNATURES = {
     "sb200_encode_batch_ids_seeded": (C.c_int32, [_P, C.POINTER(C.c_int64), C.POINTER(C.c_size_t), C.c_size_t,
                                                   C.POINTER(sb200_synth_config), C.POINTER(C.c_float),
                                                   C.POINTER(C.c_int32), C.POINTER(C.c_uint64), C.POINTER(C.c_int32),
+                                                  C.POINTER(_P), _ERR]),
+    "sb200_encode_batch_ids_blends": (C.c_int32, [_P, C.POINTER(C.c_int64), C.POINTER(C.c_size_t), C.c_size_t,
+                                                  C.POINTER(sb200_synth_config), C.POINTER(C.c_float),
+                                                  C.POINTER(C.c_int32), C.POINTER(C.c_uint64), C.POINTER(C.c_int32),
+                                                  C.POINTER(C.c_int64), C.POINTER(C.c_float), C.POINTER(C.c_size_t),
                                                   C.POINTER(_P), _ERR]),
     "sb200_latent_id_frames":(C.c_int64, [_P, C.POINTER(C.c_int32), C.c_size_t]),
     "sb200_decode_chunks": (C.c_int32, [_P, C.POINTER(_P), C.POINTER(C.c_int64), C.POINTER(C.c_int64), C.c_size_t,

@@ -9,7 +9,9 @@ LE PCM (peak-normalised per sentence / chunk like `as_wave_bytes`) goes to stdou
 files are numbered `<stem>-<n>.<ext>` (main.rs:243-256).  `text` is phonemes, one sentence per line.  With
 `--encoding mulaw|alaw` (or a JSON "encoding") the output is G.711 instead, encoded on the GPU: raw bytes on stdout,
 or an 8-bit G.711 WAV with `-o`.  With `--encoding flac` each request is one lossless FLAC stream, encoded on the GPU:
-on stdout, or as the `-o` file (the same bytes either way); realtime mode refuses it.
+on stdout, or as the `-o` file (the same bytes either way); realtime mode refuses it.  With `--speaker-blend
+"speaker_3=0.7,speaker_12=0.3"` (or a JSON "speaker_blend": {"speaker_3": 0.7, "12": 0.3}) a multi-speaker voice speaks
+with a blend of its speakers, in every mode; a key made of digits is a speaker id, any other a speaker name.
 """
 from __future__ import annotations
 
@@ -25,6 +27,37 @@ from .piper import PiperSynthesisConfig, VitsStreamingModel, refuse_formants, re
 from .synth import AudioOutputConfig, SonataSpeechSynthesizer, _check_loudness, _check_prosody
 
 MODES = ("lazy", "parallel", "realtime")
+
+
+def _blend_key(key: str):
+    key = key.strip()
+    return int(key) if key.isdigit() else key
+
+
+def parse_speaker_blend(text: str) -> dict:
+    """The blend of a --speaker-blend value, "name_or_id=weight,...": {speaker id (digits) or name: weight}."""
+    out = {}
+    for part in text.split(","):
+        key, eq, w = part.partition("=")
+        if not eq or not key.strip():
+            raise OperationError(f"speaker blend: {part.strip()!r} is not speaker=weight")
+        try:
+            out[_blend_key(key)] = float(w)
+        except ValueError:
+            raise OperationError(f"speaker blend: the weight {w.strip()!r} of speaker {key.strip()} is not a number")
+    return out
+
+
+def speaker_blend_of(value):
+    """A request's speaker blend: None, a --speaker-blend string, or a JSON object {speaker: weight}, whose keys made of
+    digits are speaker ids."""
+    if value is None:
+        return None
+    if isinstance(value, str):
+        return parse_speaker_blend(value)
+    if isinstance(value, dict):
+        return {_blend_key(k) if isinstance(k, str) else k: w for k, w in value.items()}
+    raise OperationError(f"speaker blend: {value!r} is not an object of speakers and weights")
 
 
 def build_parser() -> argparse.ArgumentParser:
@@ -65,6 +98,9 @@ def build_parser() -> argparse.ArgumentParser:
                     help="Output encoding: pcm16 (default), G.711 mulaw / alaw at one byte per sample (telephony: "
                          "PCMU / PCMA), or lossless flac (one FLAC stream per request, on stdout or in the -o file; "
                          "not in realtime mode), encoded on the GPU")
+    ap.add_argument("--speaker-blend", metavar="SPEAKER=WEIGHT,...",
+                    help="Speak with a blend of a multi-speaker voice's speakers, e.g. \"speaker_3=0.7,speaker_12=0.3\" "
+                         "(names or ids; weights >= 0, normalised to sum 1), in place of --speaker-id")
     ap.add_argument("--device", type=int, default=int(os.environ.get("SONATA_B200_DEVICE", "0")))
     return ap
 
@@ -76,7 +112,8 @@ def process_request(synth: SonataSpeechSynthesizer, default_cfg: PiperSynthesisC
     (optional): every sentence's target loudness in LUFS; the PCM is then written at the fixed scale.  `pitch_ratio` /
     `tempo` (optional): the ratios every sentence is shifted and played by, in lazy and parallel modes.
     `formant_ratio` (optional): the ratio every sentence's formants are moved by after the pitch stage, in lazy and
-    parallel modes (realtime mode refuses it unless it writes a file)."""
+    parallel modes (realtime mode refuses it unless it writes a file).  `speaker_blend` (optional): an object
+    {speaker name or id: weight} (see speaker_blend_of) every sentence speaks with, in every mode."""
     out = out or sys.stdout.buffer
     mode = (req.get("mode") or "lazy").lower()
     loudness = req.get("loudness")
@@ -95,6 +132,7 @@ def process_request(synth: SonataSpeechSynthesizer, default_cfg: PiperSynthesisC
                                  "the whole sentence, and realtime mode hands out a sentence's first chunk before its "
                                  "last one is decoded (use lazy or parallel mode)")
     pros = {k: req[k] for k in ("pitch_ratio", "tempo", "formant_ratio") if req.get(k) is not None}
+    blend = speaker_blend_of(req.get("speaker_blend"))
     _check_prosody(pros.get("pitch_ratio"), pros.get("tempo"), pros.get("formant_ratio"))
     if mode == "realtime" and not output_file:
         refuse_formants(pros.get("formant_ratio"), "realtime mode")
@@ -111,6 +149,8 @@ def process_request(synth: SonataSpeechSynthesizer, default_cfg: PiperSynthesisC
     rate = {"output_rate": req["output_rate"]} if req.get("output_rate") else {}
     loud = {} if loudness is None else {"loudness": loudness}
     enc = {} if encoding is None else {"encoding": encoding}
+    if blend is not None:
+        pros["speaker_blend"] = blend
     if output_file:
         synth.synthesize_to_file(output_file, text, oc, seed=seed, **rate, **loud, **enc, **pros)
         return
@@ -149,7 +189,7 @@ def main(argv=None) -> int:
                "pitch": args.pitch, "appended_silence_ms": args.silence, "chunk_size": args.chunk_size,
                "chunk_padding": args.chunk_padding, "seed": args.seed, "output_rate": args.output_rate,
                "loudness": args.loudness, "encoding": args.encoding, "pitch_ratio": args.pitch_ratio,
-               "tempo": args.tempo, "formant_ratio": args.formant_ratio}
+               "tempo": args.tempo, "formant_ratio": args.formant_ratio, "speaker_blend": args.speaker_blend}
         process_request(synth, default_cfg, req, args.output_file)
     else:
         for i, line in enumerate(sys.stdin):
@@ -170,6 +210,8 @@ def main(argv=None) -> int:
                 req["tempo"] = args.tempo
             if req.get("formant_ratio") is None:
                 req["formant_ratio"] = args.formant_ratio
+            if req.get("speaker_blend") is None:
+                req["speaker_blend"] = args.speaker_blend
             out_file = None
             if args.output_file:
                 stem, ext = os.path.splitext(args.output_file)

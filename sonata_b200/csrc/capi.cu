@@ -288,13 +288,14 @@ static void job_prosody(const Job& j, int64_t* n1, int64_t* n2, int32_t* frames)
     }
 }
 
-int32_t sb200_speak_batch_ids_formants(sb200_voice* v, const int64_t* ids, const size_t* offsets, size_t batch,
-                                       const sb200_synth_config* cfgs, const float* scale_packed,
-                                       const int32_t* frames_packed, const uint64_t* seeds, const int32_t* seeded,
-                                       const uint32_t* output_rates, const float* target_lufs, const float* pitch,
-                                       const float* tempo, const float* pitch_packed, const float* formants,
-                                       sb200_audio* outs, int32_t* id_frames_out, int64_t* bounds_out,
-                                       double* lufs_out, float* gain_out, sb200_error* err) {
+int32_t sb200_speak_batch_ids_blends(sb200_voice* v, const int64_t* ids, const size_t* offsets, size_t batch,
+                                     const sb200_synth_config* cfgs, const float* scale_packed,
+                                     const int32_t* frames_packed, const uint64_t* seeds, const int32_t* seeded,
+                                     const uint32_t* output_rates, const float* target_lufs, const float* pitch,
+                                     const float* tempo, const float* pitch_packed, const float* formants,
+                                     const int64_t* blend_speakers, const float* blend_weights,
+                                     const size_t* blend_offsets, sb200_audio* outs, int32_t* id_frames_out,
+                                     int64_t* bounds_out, double* lufs_out, float* gain_out, sb200_error* err) {
     return guarded(err, [&] {
         const double t0 = now_ms();
         static_assert(sizeof(long long) == sizeof(int64_t), "");
@@ -307,6 +308,8 @@ int32_t sb200_speak_batch_ids_formants(sb200_voice* v, const int64_t* ids, const
         check_prosody(pitch, tempo, batch);
         check_pitch_contour(pitch_packed, offsets, batch, pitch);
         check_formants(formants, batch);
+        canonical_blends(*v->v, reinterpret_cast<const long long*>(blend_speakers), blend_weights, blend_offsets, batch,
+                         "utterance");
         std::unique_ptr<Job> j(create_job(v->v.get(), reinterpret_cast<const long long*>(ids), offsets, batch, nullptr,
                                           nullptr, nullptr, false));
         if (cfgs) set_job_configs(*j, cfgs_in(cfgs, batch).data());
@@ -317,6 +320,7 @@ int32_t sb200_speak_batch_ids_formants(sb200_voice* v, const int64_t* ids, const
         set_job_prosody(*j, pitch, tempo);
         set_job_pitch_contour(*j, pitch_packed);
         set_job_formants(*j, formants);
+        set_job_blends(*j, reinterpret_cast<const long long*>(blend_speakers), blend_weights, blend_offsets);
         j->run(nullptr, 0);
         fetch_audio(*j, outs, 0.f);
         if (id_frames_out) {
@@ -332,6 +336,17 @@ int32_t sb200_speak_batch_ids_formants(sb200_voice* v, const int64_t* ids, const
         for (size_t b = 0; b < batch; b++)
             outs[b].inference_ms = wall * (j->out_total ? (float)outs[b].len / (float)j->out_total : 0.f);
     });
+}
+int32_t sb200_speak_batch_ids_formants(sb200_voice* v, const int64_t* ids, const size_t* offsets, size_t batch,
+                                       const sb200_synth_config* cfgs, const float* scale_packed,
+                                       const int32_t* frames_packed, const uint64_t* seeds, const int32_t* seeded,
+                                       const uint32_t* output_rates, const float* target_lufs, const float* pitch,
+                                       const float* tempo, const float* pitch_packed, const float* formants,
+                                       sb200_audio* outs, int32_t* id_frames_out, int64_t* bounds_out,
+                                       double* lufs_out, float* gain_out, sb200_error* err) {
+    return sb200_speak_batch_ids_blends(v, ids, offsets, batch, cfgs, scale_packed, frames_packed, seeds, seeded,
+                                        output_rates, target_lufs, pitch, tempo, pitch_packed, formants, nullptr, nullptr,
+                                        nullptr, outs, id_frames_out, bounds_out, lufs_out, gain_out, err);
 }
 int32_t sb200_speak_batch_ids_contour(sb200_voice* v, const int64_t* ids, const size_t* offsets, size_t batch,
                                       const sb200_synth_config* cfgs, const float* scale_packed,
@@ -455,6 +470,12 @@ int32_t sb200_job_set_pitch_contour(sb200_job* job, const float* pitch_packed, s
 }
 int32_t sb200_job_set_formants(sb200_job* job, const float* formants, sb200_error* err) {
     return guarded(err, [&] { set_job_formants(*job->j, formants); });
+}
+int32_t sb200_job_set_speaker_blends(sb200_job* job, const int64_t* speakers, const float* weights, const size_t* offsets,
+                                     sb200_error* err) {
+    return guarded(err, [&] {
+        set_job_blends(*job->j, reinterpret_cast<const long long*>(speakers), weights, offsets);
+    });
 }
 int32_t sb200_job_prosody_bounds(sb200_job* job, int64_t* out_packed, size_t capacity, sb200_error* err) {
     return guarded(err, [&] {
@@ -607,17 +628,27 @@ int32_t sb200_decode_chunk(sb200_voice* v, const sb200_latent* z, int64_t lo, in
 }
 void sb200_latent_free(sb200_latent* z) { delete z; }
 
-int32_t sb200_encode_batch_ids_seeded(sb200_voice* v, const int64_t* ids, const size_t* offsets, size_t batch,
+int32_t sb200_encode_batch_ids_blends(sb200_voice* v, const int64_t* ids, const size_t* offsets, size_t batch,
                                       const sb200_synth_config* cfgs, const float* scale_packed,
                                       const int32_t* frames_packed, const uint64_t* seeds, const int32_t* seeded,
-                                      sb200_latent** outs, sb200_error* err) {
+                                      const int64_t* blend_speakers, const float* blend_weights,
+                                      const size_t* blend_offsets, sb200_latent** outs, sb200_error* err) {
     return guarded(err, [&] {
         const std::vector<SynthConfig> c = cfgs ? cfgs_in(cfgs, batch) : std::vector<SynthConfig>();
         std::vector<Latent*> ls = encode_latents(v->v.get(), reinterpret_cast<const long long*>(ids), offsets, batch,
                                                  cfgs ? c.data() : nullptr, scale_packed, frames_packed,
-                                                 reinterpret_cast<const unsigned long long*>(seeds), seeded);
+                                                 reinterpret_cast<const unsigned long long*>(seeds), seeded,
+                                                 reinterpret_cast<const long long*>(blend_speakers), blend_weights,
+                                                 blend_offsets);
         for (size_t b = 0; b < batch; b++) outs[b] = new sb200_latent{ls[b], v->v};
     });
+}
+int32_t sb200_encode_batch_ids_seeded(sb200_voice* v, const int64_t* ids, const size_t* offsets, size_t batch,
+                                      const sb200_synth_config* cfgs, const float* scale_packed,
+                                      const int32_t* frames_packed, const uint64_t* seeds, const int32_t* seeded,
+                                      sb200_latent** outs, sb200_error* err) {
+    return sb200_encode_batch_ids_blends(v, ids, offsets, batch, cfgs, scale_packed, frames_packed, seeds, seeded, nullptr,
+                                         nullptr, nullptr, outs, err);
 }
 int32_t sb200_encode_batch_ids_durations(sb200_voice* v, const int64_t* ids, const size_t* offsets, size_t batch,
                                          const sb200_synth_config* cfgs, const float* scale_packed,
@@ -1438,6 +1469,20 @@ int32_t sb200_debug_g711(int32_t device, int32_t law, const int16_t* x, size_t n
         launch_g711(dx, (long long)n, fmt, dy, 0);
         SB_CUDA(cudaDeviceSynchronize());
         SB_CUDA(cudaMemcpy(out, dy, n, cudaMemcpyDeviceToHost));
+    });
+}
+
+int32_t sb200_debug_speaker_blend(sb200_voice* v, const int64_t* speakers, const float* weights, size_t n, float* g,
+                                  size_t g_cap, float* bias, size_t bias_cap, sb200_error* err) {
+    return guarded(err, [&] {
+        Voice& V = *v->v;
+        const SpeakerBlend b = canonical_blend(V, reinterpret_cast<const long long*>(speakers), weights, n, "");
+        if (g_cap < (size_t)V.gin || bias_cap < (size_t)V.cond_rows)
+            throw Error(19, "debug speaker blend: a destination is too small for the result");
+        std::vector<float> gh, bh;
+        debug_speaker_blend(V, b, gh, bh);
+        std::copy(gh.begin(), gh.end(), g);
+        std::copy(bh.begin(), bh.end(), bias);
     });
 }
 

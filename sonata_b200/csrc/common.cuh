@@ -394,9 +394,15 @@ void launch_randn_seeded(float* out, int cols, unsigned tag, unsigned long long 
 // z[r][0..1] = eps * s[seg_of_gran[r / map.gran]]
 void launch_scale_copy2(const float* eps, const float* s, const int* seg_of_gran, float* z, RowMap map, cudaStream_t st);
 // out[s][r] = base[r] + sum_k w[r][k] * emb_g[sid[s]][k]  for every slot s < nslots   (speaker conditioning: effective
-// biases of the conditioned convs, one set per distinct speaker of a batch)
+// biases of the conditioned convs, one set per distinct speaker of a batch).  sid null: row s of emb_g (a blend table).
 void launch_cond_bias(const float* w, const float* base, const float* emb_g, const int* sid, int nslots, int rows, int gin,
                       float* out, cudaStream_t st);
+// One term of a canonical speaker blend: speaker row s of emb_g with normalised weight w.
+struct BlendTerm { int s; float w; };
+// g[s][k] = acc after acc = fmaf(terms[i].w, emb_g[terms[i].s][k], acc) for i in [off[s], off[s + 1]), acc from 0.f, for
+// every slot s < nslots and k < gin: the blended embeddings (include/sonata_b200.h, sb200_speak_batch_ids_blends).
+void launch_blend_g(const float* emb_g, const int* off, const BlendTerm* terms, int nslots, int gin, float* g,
+                    cudaStream_t st);
 
 // launch-configuration errors are not sticky and would otherwise be lost: throw immediately
 void check_launch(const char* what);

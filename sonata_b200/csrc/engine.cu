@@ -211,6 +211,55 @@ void set_job_configs(Job& j, const SynthConfig* cfgs) {
     j.cfgs.assign(cfgs, cfgs + j.B);
 }
 
+SpeakerBlend canonical_blend(const Voice& v, const long long* s, const float* u, size_t n, const std::string& who) {
+    const std::string p = who + "speaker blend: ";
+    if (v.num_speakers <= 1) throw Error(19, p + "the voice has a single speaker");
+    if (n == 0) throw Error(19, p + "the blend is empty");
+    std::vector<std::pair<long long, float>> terms;
+    for (size_t i = 0; i < n; i++) {
+        bool known = false;
+        for (auto& kv : v.speaker_id_map) known |= kv.second == s[i];
+        if (!known || s[i] < 0 || (v.emb_g && s[i] >= v.emb_rows))     // a config-only voice has no table to read
+            throw Error(19, p + "No speaker was found with the given id `" + std::to_string(s[i]) + "`");
+        for (size_t q = 0; q < i; q++)
+            if (s[q] == s[i]) throw Error(19, p + "speaker " + std::to_string(s[i]) + " appears more than once");
+        if (!std::isfinite(u[i]) || u[i] < 0.f)
+            throw Error(19, p + "the weight " + std::to_string(u[i]) + " of speaker " + std::to_string(s[i]) +
+                                " is not a finite number >= 0");
+        if (u[i] > 0.f) terms.emplace_back(s[i], u[i]);
+    }
+    if (terms.empty()) throw Error(19, p + "every weight is zero");
+    std::sort(terms.begin(), terms.end());
+    double U = 0.0;
+    for (auto& t : terms) U += (double)t.second;
+    SpeakerBlend b;
+    for (auto& t : terms) { b.s.push_back((int)t.first); b.w.push_back((float)((double)t.second / U)); }
+    return b;
+}
+
+std::vector<SpeakerBlend> canonical_blends(const Voice& v, const long long* s, const float* u, const size_t* offs,
+                                          size_t B, const std::string& what) {
+    std::vector<SpeakerBlend> out(B);
+    if (!offs) return out;
+    if (offs[0] != 0) throw Error(19, "the blend offsets must start at 0");
+    for (size_t b = 0; b < B; b++) {
+        const std::string who = what + " " + std::to_string(b) + ": ";
+        if (offs[b + 1] < offs[b]) throw Error(19, who + "speaker blend: the blend offsets decrease");
+        if (offs[b + 1] == offs[b]) continue;
+        if (!s || !u) throw Error(19, who + "speaker blend: no speakers or weights were given");
+        out[b] = canonical_blend(v, s + offs[b], u + offs[b], offs[b + 1] - offs[b], who);
+    }
+    return out;
+}
+
+void set_job_blends(Job& j, const long long* s, const float* u, const size_t* offs) {
+    std::vector<SpeakerBlend> b = canonical_blends(*j.v, s, u, offs, j.B, "utterance");
+    bool any = false;
+    for (const SpeakerBlend& e : b) any |= !e.s.empty();
+    if (!any) b.clear();
+    j.blends.swap(b);
+}
+
 void set_job_durations(Job& j, const float* scale, const int* frames) {
     for (size_t b = 0; b < j.B; b++)
         for (size_t i = j.offs[b]; i < j.offs[b + 1]; i++) {
@@ -369,32 +418,58 @@ template <typename T> struct Staged {
     void download(cudaStream_t st) const { SB_CUDA(cudaMemcpyAsync(h, d, n * sizeof(T), cudaMemcpyDeviceToHost, st)); }
 };
 
-// Gives the next segment of a pass the slot of speaker `sid`, a new one for a speaker not seen before; false when sid
-// is not a speaker of the voice.  On a single-speaker voice every segment has slot 0 and the pass has no slots.
-bool assign_slot(FrameLayout& l, const Voice& v, long long sid) {
+// Gives the next segment of a pass the slot of canonical blend `b` (a plain speaker: its own one-speaker blend), a new
+// one for a blend not seen before; false when a plain speaker is not a speaker of the voice.  On a single-speaker voice
+// every segment has slot 0 and the pass has no slots.
+bool assign_slot(FrameLayout& l, const Voice& v, const SpeakerBlend& b) {
     if (v.num_speakers <= 1) { l.slot_of.push_back(0); return true; }
-    if (sid < 0 || sid >= v.emb_rows) return false;
-    const auto it = std::find(l.slot_sid.begin(), l.slot_sid.end(), (int)sid);
-    l.slot_of.push_back((int)(it - l.slot_sid.begin()));
-    if (it == l.slot_sid.end()) l.slot_sid.push_back((int)sid);
+    if (b.s.size() == 1 && (b.s[0] < 0 || b.s[0] >= v.emb_rows)) return false;
+    const auto it = std::find(l.slot_spk.begin(), l.slot_spk.end(), b);
+    l.slot_of.push_back((int)(it - l.slot_spk.begin()));
+    if (it == l.slot_spk.end()) l.slot_spk.push_back(b);
     return true;
 }
+bool assign_slot(FrameLayout& l, const Voice& v, long long sid) {
+    if (v.num_speakers > 1 && (sid < 0 || sid >= v.emb_rows)) return false;
+    return assign_slot(l, v, SpeakerBlend::plain(sid));
+}
 
-// Speaker conditioning of a pass with speaker slots: the speaker of every slot and the effective biases of the
-// speaker-conditioned convs, [slot][cond_rows].  Unset without slots.
+// Speaker conditioning of a pass with speaker slots: the effective biases of the speaker-conditioned convs,
+// [slot][cond_rows], read from the voice's embeddings by speaker id when no slot blends (sid), else from the pass's
+// blend table g [slot][gin], formed from each slot's terms (boff, terms).  Unset without slots.
 struct SpeakerBias {
     Staged<int> sid; float* cond = nullptr;
+    Staged<int> boff; Staged<BlendTerm> terms; float* g = nullptr;
     void carve(Arena& dev, Arena& pin, const Voice& v, const FrameLayout& l) {
-        if (l.slot_sid.empty()) return;
-        cond = dev.get<float>(l.slot_sid.size() * v.cond_rows);
-        sid.carve(dev, pin, l.slot_sid.size());
+        if (l.slot_spk.empty()) return;
+        cond = dev.get<float>(l.slot_spk.size() * v.cond_rows);
+        if (!l.blended()) { sid.carve(dev, pin, l.slot_spk.size()); return; }
+        size_t n = 0;
+        for (const SpeakerBlend& b : l.slot_spk) n += b.s.size();
+        boff.carve(dev, pin, l.slot_spk.size() + 1);
+        terms.carve(dev, pin, n);
+        g = dev.get<float>(l.slot_spk.size() * v.gin);
     }
-    // Fills the speaker table and launches the computation of the biases.
+    // Fills the speaker or blend tables and launches the computation of the biases (after the blend table's, if any).
     void run(const Voice& v, const FrameLayout& l, cudaStream_t st) const {
         if (!cond) return;
-        std::copy(l.slot_sid.begin(), l.slot_sid.end(), sid.h);
-        sid.upload(st);
-        launch_cond_bias(v.cond_w, v.cond_base, v.emb_g, sid.d, (int)sid.n, v.cond_rows, v.gin, cond, st);
+        const int nslots = (int)l.slot_spk.size();
+        if (!g) {
+            for (int k = 0; k < nslots; k++) sid.h[k] = l.slot_spk[k].s[0];
+            sid.upload(st);
+            launch_cond_bias(v.cond_w, v.cond_base, v.emb_g, sid.d, nslots, v.cond_rows, v.gin, cond, st);
+            return;
+        }
+        int n = 0;
+        for (int k = 0; k < nslots; k++) {
+            boff.h[k] = n;
+            for (size_t i = 0; i < l.slot_spk[k].s.size(); i++) terms.h[n++] = BlendTerm{l.slot_spk[k].s[i], l.slot_spk[k].w[i]};
+        }
+        boff.h[nslots] = n;
+        boff.upload(st);
+        terms.upload(st);
+        launch_blend_g(v.emb_g, boff.d, terms.d, nslots, v.gin, g, st);
+        launch_cond_bias(v.cond_w, v.cond_base, g, nullptr, nslots, v.cond_rows, v.gin, cond, st);
     }
 };
 
@@ -436,7 +511,7 @@ struct IdBufs {
         if (tc_att) tiles.carve(dev, pin, ntiles);
         if (n_simt) att_segs.carve(dev, pin, n_simt);
         scales.carve(dev, pin, 3 * B);
-        if (!j.frames.slot_sid.empty()) xslot.carve(dev, pin, nxg);
+        if (!j.frames.slot_spk.empty()) xslot.carve(dev, pin, nxg);
         spk.carve(dev, pin, v, j.frames);
         cum = dev.get<int>(RX);
         cum_h = j.contour.empty() ? nullptr : pin.get<int>(RX);
@@ -474,7 +549,7 @@ struct FrameTables {
     void carve(Arena& dev, Arena& pin, const FrameLayout& l) {
         const int ntile = l.RY / GY;
         yend.carve(dev, pin, ntile); ftile.carve(dev, pin, ntile); fsegs.carve(dev, pin, l.fsegs.size());
-        if (!l.slot_sid.empty()) yslot.carve(dev, pin, ntile);
+        if (!l.slot_spk.empty()) yslot.carve(dev, pin, ntile);
     }
 };
 
@@ -1031,6 +1106,24 @@ void cum_to_frames(const Job& j, const int* cum, size_t b, int* out) {
 
 }  // namespace
 
+void debug_speaker_blend(Voice& v, const SpeakerBlend& b, std::vector<float>& g, std::vector<float>& bias) {
+    FrameLayout l;
+    if (v.num_speakers <= 1 || !assign_slot(l, v, b)) throw Error(19, "debug speaker blend: not a blend of this voice");
+    const auto release = [&v](Context* c) { v.release(c); };
+    const std::unique_ptr<Context, decltype(release)> ctx(v.acquire(), release);
+    SB_CUDA(cudaSetDevice(v.device));
+    SpeakerBias sb;
+    plan(ctx->dev_frame, ctx->pin, [&](Arena& dev, Arena& pin) { sb.carve(dev, pin, v, l); });
+    const cudaStream_t st = ctx->stream;
+    sb.run(v, l, st);
+    g.resize(v.gin); bias.resize(v.cond_rows);
+    const float* gd = sb.g ? sb.g : v.emb_g + (size_t)b.s[0] * v.gin;
+    SB_CUDA(cudaMemcpyAsync(g.data(), gd, g.size() * 4, cudaMemcpyDeviceToHost, st));
+    SB_CUDA(cudaMemcpyAsync(bias.data(), sb.cond, bias.size() * 4, cudaMemcpyDeviceToHost, st));
+    SB_CUDA(cudaStreamSynchronize(st));
+    SB_CUDA(cudaGetLastError());
+}
+
 const std::vector<int>& job_id_frames(Job& j) {
     if (!j.ran) throw Error(19, "job has not run: no per-id frame counts yet");
     if (!j.id_frames.empty()) return j.id_frames;
@@ -1081,9 +1174,10 @@ void Job::run(float* d_out, size_t d_out_cap) {
     for (const SegInfo& s : xsegs)
         if (!tc_voice || s.len > ATT_TC_MAX) { simt_segs.push_back(s); simt_len = std::max(simt_len, s.len); }
     const bool simt_att = !simt_segs.empty();
-    frames.slot_of.clear(); frames.slot_sid.clear();
-    for (size_t b = 0; b < B; b++)      // piper/src/lib.rs:353-358: speaker.unwrap_or(0)
-        if (!assign_slot(frames, V, cfgs[b].has_speaker ? cfgs[b].speaker : 0))
+    frames.slot_of.clear(); frames.slot_spk.clear();
+    for (size_t b = 0; b < B; b++)      // piper/src/lib.rs:353-358: speaker.unwrap_or(0), unless a blend replaces it
+        if (!(blends.empty() || blends[b].s.empty() ? assign_slot(frames, V, cfgs[b].has_speaker ? cfgs[b].speaker : 0)
+                                                    : assign_slot(frames, V, blends[b])))
             throw Error(19, "Failed to run model inference. Error: speaker id out of range (utterance " + std::to_string(b) + ")");
     IdBufs x;
     plan(C.dev_id, C.pin, [&](Arena& dev, Arena& pin) { x.carve(dev, pin, *this, tc_att, simt_segs.size()); });
@@ -1418,11 +1512,13 @@ void Job::run(float* d_out, size_t d_out_cap) {
 // ====================================================================== streaming halves
 std::vector<Latent*> encode_latents(Voice* v, const long long* ids, const size_t* offs, size_t B, const SynthConfig* cfgs,
                                     const float* scale, const int* frames, const unsigned long long* seeds,
-                                    const int* seeded) {
+                                    const int* seeded, const long long* blend_s, const float* blend_u,
+                                    const size_t* blend_offs) {
     std::unique_ptr<Job> j(create_job(v, ids, offs, B, nullptr, nullptr, nullptr, false));
     if (cfgs) set_job_configs(*j, cfgs);
     set_job_durations(*j, scale, frames);
     set_job_seeds(*j, seeds, seeded);
+    set_job_blends(*j, blend_s, blend_u, blend_offs);
     j->encode_only = true;
     j->run(nullptr, 0);
     const size_t I = (size_t)v->a.inter;
@@ -1438,7 +1534,8 @@ std::vector<Latent*> encode_latents(Voice* v, const long long* ids, const size_t
     for (size_t b = 0; b < B; b++) {
         Latent& L = *(ls[b] = std::unique_ptr<Latent>(new Latent()));
         L.v = v; L.mem = mem; L.z = p + row * I; L.frames = j->y_len[b];
-        L.sid = j->cfgs[b].has_speaker ? j->cfgs[b].speaker : 0;
+        L.spk = j->blends.empty() || j->blends[b].s.empty()
+                    ? SpeakerBlend::plain(j->cfgs[b].has_speaker ? j->cfgs[b].speaker : 0) : j->blends[b];
         SB_CUDA(cudaMemcpyAsync(L.z, j->z_dev + (size_t)j->frames.fsegs[b].off * I, (size_t)L.frames * I * 4,
                                 cudaMemcpyDeviceToDevice, j->ctx->stream));
         row += (size_t)L.frames;
@@ -1496,8 +1593,8 @@ void decode_chunks(Voice* v, const ChunkPass& p, ChunkResult& out) {
                                                   ") of a latent of " + std::to_string(c.z->frames) + ")");
         if (c.trim_lo < 0 || c.trim_hi < 0 || c.trim_lo + c.trim_hi >= c.hi - c.lo)
             fail(k, "Invalid model audio output", " (trim)");
-        // decoder.onnx takes the encoder's `g` (piper/src/lib.rs:706-735, 739-743)
-        if (!assign_slot(l, *v, c.z->sid)) fail(k, "Failed to run model inference. Error: speaker id out of range", "");
+        // decoder.onnx takes the encoder's `g` (piper/src/lib.rs:706-735, 739-743): the latent's blend
+        if (!assign_slot(l, *v, c.z->spk)) fail(k, "Failed to run model inference. Error: speaker id out of range", "");
         len[k] = (int)(c.hi - c.lo);
         if (const Resampler* r = c.rs) {
             if (r->v != v) fail(k, "the resampler was made for another voice", "");

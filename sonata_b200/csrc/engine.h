@@ -97,6 +97,15 @@ struct UpStageW { int u, k, cin, cout; std::vector<ConvW> phase; ConvW fused; st
 
 struct SynthConfig { long long speaker = 0; bool has_speaker = false; float noise_scale = 0.667f, length_scale = 1.f, noise_w = 0.8f; };
 
+// A speaker blend in canonical form (include/sonata_b200.h, sb200_speak_batch_ids_blends): distinct speaker ids in
+// ascending order, each with its normalised weight.  A plain speaker s is {s} with weight 1; empty: no blend.
+struct SpeakerBlend {
+    std::vector<int> s;
+    std::vector<float> w;
+    bool operator==(const SpeakerBlend& o) const { return s == o.s && w == o.w; }
+    static SpeakerBlend plain(long long sid) { return SpeakerBlend{{(int)sid}, {1.f}}; }
+};
+
 // resample_poly's default filter for in_rate -> out_rate (resample.cu): up / down the reduced ratio, H = 10 max(up, down)
 // and 2H + 1 taps; on the device the taps are stored phase-major, K per phase (ResampleSeg).
 struct ResampleFilter { int up = 1, down = 1, H = 0, K = 0; float* taps = nullptr; };
@@ -148,6 +157,15 @@ ProsodyShape prosody_contour_plan(int rate, long long n, const long long* ends, 
 struct Voice;
 struct ProsodyStream;
 struct ProsodyStep;
+// The canonical form of the blend of pairs (s[i], u[i]), i < n, on voice v; throws OPERATION_ERROR prefixed by `who`
+// (naming the speaker or the weight) for an empty blend, a single-speaker voice, an unknown or repeated id, a weight that
+// is negative or not finite, or weights that are all zero.
+SpeakerBlend canonical_blend(const Voice& v, const long long* s, const float* u, size_t n, const std::string& who);
+// The canonical blends of a blend table of B utterances or streams (utterance b: pairs [offs[b], offs[b + 1]); an empty
+// range: no blend, an empty entry).  `what` names an entry in errors ("utterance", "stream").  Null tables: B empty
+// entries.  Every entry is checked before anything is returned.
+std::vector<SpeakerBlend> canonical_blends(const Voice& v, const long long* s, const float* u, const size_t* offs,
+                                          size_t B, const std::string& what);
 struct ProsodyPlan {
     std::vector<ProsodySeg> segs;
     std::vector<ProsodyShape> shapes;
@@ -350,8 +368,15 @@ struct FrameLayout {
     std::vector<FrameSeg> fsegs;
     int RY = 0;
     long long total_samples = 0;
-    std::vector<int> slot_of;         // per segment: its speaker slot (index into slot_sid; 0 on single-speaker voices)
-    std::vector<int> slot_sid;        // per slot: the speaker id, distinct, in order of first use (empty: one speaker)
+    std::vector<int> slot_of;         // per segment: its speaker slot (index into slot_spk; 0 on single-speaker voices)
+    std::vector<SpeakerBlend> slot_spk;   // per slot: the canonical blend, distinct, in order of first use (empty: one
+                                          // speaker); a plain speaker is the blend of itself
+    // Whether some slot blends two or more speakers: only then does the pass form its embeddings in a blend table.
+    bool blended() const {
+        for (const SpeakerBlend& b : slot_spk)
+            if (b.s.size() > 1) return true;
+        return false;
+    }
 };
 
 struct Job {
@@ -380,6 +405,8 @@ struct Job {
                                       // has a contour (set_job_pitch_contour)
     std::vector<float> formant;       // one formant ratio per utterance, NaN = none; empty when none has one
                                       // (set_job_formants)
+    std::vector<SpeakerBlend> blends; // one canonical blend per utterance (empty entry: the config's speaker); empty when
+                                      // none has one (set_job_blends)
     std::vector<ProsodyShape> pros_ran;   // each utterance's shape in the last run (empty: it ran no prosody stage)
     std::vector<float> pitch_ran, tempo_ran;   // the ratios the last run had (empty: none)
     std::vector<long long> pros_bounds;   // each id's delivered end in the last run when it had a contour (else empty)
@@ -455,6 +482,13 @@ void set_job_pitch_contour(Job& j, const float* packed);
 // loudness; its length, bounds, alignments and place in the job's result do not change.  A bad entry leaves the job's
 // ratios as they were.
 void set_job_formants(Job& j, const float* phi);
+// Per-utterance speaker blends of the job's next run (a blend table as for canonical_blends), or null for none.  A blend
+// replaces the utterance's config speaker; its noise and length scales still apply.  Every entry is checked first; a bad
+// entry fails naming the utterance and leaves the job's blends as they were.
+void set_job_blends(Job& j, const long long* s, const float* u, const size_t* offs);
+// The blended embedding g [gin] and effective biases [cond_rows] a pass computes for blend b, through the pass's own
+// launches, copied to the host.
+void debug_speaker_blend(Voice& v, const SpeakerBlend& b, std::vector<float>& g, std::vector<float>& bias);
 // Each id's delivered end (prosody_contour_plan) in the job's last run, packed like its ids, at the voice's rate: kept
 // from the run when it had a contour, else computed from job_id_frames and the ratios it had.
 std::vector<long long> job_prosody_bounds(Job& j);
@@ -464,7 +498,8 @@ const std::vector<int>& job_id_frames(Job& j);
 
 struct Latent {
     Voice* v = nullptr;
-    long long sid = 0;    // speaker of the encoder pass (the reference hands `g` from encoder.onnx to decoder.onnx)
+    SpeakerBlend spk;     // canonical blend of the encoder pass, the plain config speaker's without one (the reference
+                          // hands `g` from encoder.onnx to decoder.onnx); its chunk passes condition on it
     std::shared_ptr<float> mem;   // device allocation shared by the latents of one encoder pass, freed with the last
     float* z = nullptr;   // device [frames][inter], inside `mem`
     long long frames = 0;
@@ -473,9 +508,12 @@ struct Latent {
 // One encoder pass over B utterances (cfgs: one per utterance, or null for the voice's fallback config; scale / frames:
 // per-id duration controls as for set_job_durations, or null; seeds / seeded: noise seeds as for set_job_seeds) -> B
 // latents sharing one device allocation.  The caller owns the returned pointers.
+// blend_s / blend_u / blend_offs: speaker blends as for set_job_blends, or null.
 std::vector<Latent*> encode_latents(Voice* v, const long long* ids, const size_t* offs, size_t B, const SynthConfig* cfgs,
                                     const float* scale = nullptr, const int* frames = nullptr,
-                                    const unsigned long long* seeds = nullptr, const int* seeded = nullptr);
+                                    const unsigned long long* seeds = nullptr, const int* seeded = nullptr,
+                                    const long long* blend_s = nullptr, const float* blend_u = nullptr,
+                                    const size_t* blend_offs = nullptr);
 Latent* encode_latent(Voice* v, const long long* ids, size_t n);
 // One stream's resampling state: the filter to its output rate, the last inputs (two device buffers of K floats each,
 // read and written alternately), and how many inputs it has consumed and outputs it has emitted.

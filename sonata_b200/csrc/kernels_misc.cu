@@ -1024,12 +1024,24 @@ __global__ void __launch_bounds__(256) cond_bias_kernel(const float* __restrict_
     pdl_trigger(); pdl_wait();
     const int r = blockIdx.x * 8 + (threadIdx.x >> 5), lane = threadIdx.x & 31;
     if (r >= rows) return;
-    const float* g = emb_g + (size_t)sid[blockIdx.y] * gin;
+    const float* g = emb_g + (size_t)(sid ? sid[blockIdx.y] : (int)blockIdx.y) * gin;
     out += (size_t)blockIdx.y * rows;
     float s = 0.f;
     for (int k = lane; k < gin; k += 32) s = fmaf(w[(size_t)r * gin + k], g[k], s);
     s = warp_sum(s);
     if (lane == 0) out[r] = base[r] + s;
+}
+
+// blended speaker embeddings: one thread per column k, one grid row (blockIdx.y) per slot; the slot's terms
+// [off[slot], off[slot + 1]) are accumulated in their (canonical) order, g[k] = fmaf(w_i, emb_g[s_i][k], g[k]) from 0
+__global__ void __launch_bounds__(128) blend_g_kernel(const float* __restrict__ emb_g, const int* __restrict__ off,
+                                                      const BlendTerm* __restrict__ terms, int gin, float* __restrict__ g) {
+    pdl_trigger(); pdl_wait();
+    const int k = blockIdx.x * 128 + threadIdx.x;
+    if (k >= gin) return;
+    float acc = 0.f;
+    for (int i = off[blockIdx.y]; i < off[blockIdx.y + 1]; i++) acc = fmaf(terms[i].w, emb_g[(size_t)terms[i].s * gin + k], acc);
+    g[(size_t)blockIdx.y * gin + k] = acc;
 }
 
 template <typename K>
@@ -1234,6 +1246,12 @@ void launch_randn_seeded(float* out, int cols, unsigned tag, unsigned long long 
 void launch_cond_bias(const float* w, const float* base, const float* emb_g, const int* sid, int nslots, int rows, int gin,
                       float* out, cudaStream_t st) {
     launch_pdl(cond_bias_kernel, dim3((rows + 7) / 8, nslots), dim3(256), 0, st, w, base, emb_g, sid, rows, gin, out);
+    g_launch_count++;
+}
+
+void launch_blend_g(const float* emb_g, const int* off, const BlendTerm* terms, int nslots, int gin, float* g,
+                    cudaStream_t st) {
+    launch_pdl(blend_g_kernel, dim3((gin + 127) / 128, nslots), dim3(128), 0, st, emb_g, off, terms, gin, g);
     g_launch_count++;
 }
 

@@ -10,7 +10,7 @@ import numpy as np
 
 from . import _native as N
 from .core import G711_LAW, Audio, OperationError, check_encoding
-from .piper import (_check, _config_array, _contour_arrays, _duration_arrays, _formant_array, _gain_array,
+from .piper import (_blend_arrays, _check, _config_array, _contour_arrays, _duration_arrays, _formant_array, _gain_array,
                     _loudness_array, _prosody_arrays, _ptr, _rate_array, _seed_arrays, _take_audio, _take_bytes)
 
 
@@ -20,12 +20,12 @@ class SynthesisJob:
                  seeds: Optional[Sequence] = None, output_rates: Optional[Sequence] = None,
                  loudness: Optional[Sequence] = None, pitches: Optional[Sequence] = None,
                  tempos: Optional[Sequence] = None, pitch_contours: Optional[Sequence] = None,
-                 formants: Optional[Sequence] = None):
+                 formants: Optional[Sequence] = None, speaker_blends: Optional[Sequence] = None):
         """`configs`: one PiperSynthesisConfig per utterance (see set_configs); None keeps the voice's fallback config.
         `seeds`: noise seeds (see set_seeds).  `output_rates`: output sample rates (see set_output_rates).
         `loudness`: loudness targets (see set_loudness).  `pitches` / `tempos`: pitch and tempo ratios (see
         set_prosody).  `pitch_contours`: per-id pitch ratios (see set_pitch_contours).  `formants`: formant ratios (see
-        set_formants)."""
+        set_formants).  `speaker_blends`: speaker blends (see set_speaker_blends)."""
         self._m = model
         self._lib = model._lib
         n = len(batches)
@@ -37,6 +37,7 @@ class SynthesisJob:
         _loudness_array(loudness, n)
         _contour_arrays(self._lens, pitch_contours, _prosody_arrays(pitches, tempos, n)[0])
         _formant_array(formants, n)
+        blend_image = _blend_arrays(model, speaker_blends, n)
         packed = np.ascontiguousarray(np.concatenate([np.asarray(b, dtype=np.int64) for b in batches]))
         offs = np.zeros(n + 1, dtype=np.uint64)
         offs[1:] = np.cumsum([len(b) for b in batches])
@@ -81,6 +82,8 @@ class SynthesisJob:
             self.set_pitch_contours(pitch_contours)
         if formants is not None:
             self.set_formants(formants)
+        if blend_image[2] is not None:
+            self._set_blend_image(*blend_image)
 
     def set_configs(self, configs: Optional[Sequence]) -> None:
         """Per-utterance PiperSynthesisConfigs for the next run, or None for the voice's fallback config.  A wrong
@@ -170,6 +173,17 @@ class SynthesisJob:
         f = _formant_array(formants, self.batch)
         err = N.sb200_error()
         _check(self._lib.sb200_job_set_formants(self._h, _ptr(f, C.c_float), C.byref(err)), err)
+
+    def set_speaker_blends(self, blends: Optional[Sequence]) -> None:
+        """Per-utterance speaker blends for the next run (see VitsModel.infer_batch_with_values): a mapping
+        {speaker: weight} or None per utterance, or None for none.  A blend replaces the utterance's config speaker.  A
+        bad entry raises OperationError naming the utterance and leaves the job's blends as they were."""
+        self._set_blend_image(*_blend_arrays(self._m, blends, self.batch))
+
+    def _set_blend_image(self, s, w, o) -> None:
+        err = N.sb200_error()
+        _check(self._lib.sb200_job_set_speaker_blends(self._h, _ptr(s, C.c_int64), _ptr(w, C.c_float),
+                                                      _ptr(o, C.c_size_t), C.byref(err)), err)
 
     def prosody_bounds(self) -> List[np.ndarray]:
         """Each id's delivered end in the last run, at the voice's rate, one int64 array per utterance (see

@@ -236,6 +236,65 @@ def refuse_formants(formant_ratio, where: str) -> None:
                              "chunk (use speak_batch, a SynthesisJob or the lazy, parallel or file modes)")
 
 
+def _blend_terms(model, blend, who: str) -> List[Tuple[int, float]]:
+    """The (speaker id, f32 weight) pairs of one blend, a mapping {speaker: weight} whose keys are ids or names of the
+    voice's speaker_id_map, checked as the library checks a blend (include/sonata_b200.h, sb200_speak_batch_ids_blends);
+    errors name `who` and the speaker or weight."""
+    p = f"{who}: speaker blend: "
+    speakers = model.get_speakers()
+    if not speakers:
+        raise OperationError(p + "the voice has a single speaker")
+    if not isinstance(blend, dict) and not hasattr(blend, "items"):
+        raise OperationError(p + f"{blend!r} is not a mapping of speakers to weights")
+    sids, seen = [], set()
+    for key, u in blend.items():
+        if isinstance(key, str):
+            sid = model.speaker_name_to_id(key)
+            if sid is None:
+                raise OperationError(p + f"No speaker was found with the name `{key}`")
+        elif type(key) is int or isinstance(key, numbers.Integral) and not isinstance(key, bool):
+            sid = int(key)
+            if sid not in speakers:
+                raise OperationError(p + f"No speaker was found with the given id `{sid}`")
+        else:
+            raise OperationError(p + f"speaker {key!r} is neither an id nor a name")
+        if sid in seen:
+            raise OperationError(p + f"speaker {sid} appears more than once")
+        if type(u) is not float and (isinstance(u, bool) or not isinstance(u, numbers.Real)):
+            raise OperationError(p + f"the weight {u!r} of speaker {sid} is not a number")
+        seen.add(sid)
+        sids.append(sid)
+    if not sids:
+        raise OperationError(p + "the blend is empty")
+    u = list(blend.values())
+    with np.errstate(over="ignore"):
+        w = np.array(u, np.float64).astype(np.float32)
+    bad = np.flatnonzero(~(np.isfinite(w) & (w >= 0)))
+    if bad.size:
+        i = int(bad[0])
+        raise OperationError(p + f"the weight {float(u[i])} of speaker {sids[i]} is not a finite number >= 0")
+    if not w.any():
+        raise OperationError(p + "every weight is zero")
+    return list(zip(sids, w.tolist()))
+
+
+def _blend_arrays(model, blends, n: int, who: Optional[Sequence[str]] = None):
+    """The C image of per-utterance speaker blends: (speakers i64, weights f32, offsets size_t [n + 1]), or
+    (None, None, None) when `blends` is None or every entry is None.  blends[b] is a mapping {speaker: weight} (see
+    _blend_terms) or None for the utterance's config speaker.  Errors name utterance b, or who[b]."""
+    if blends is None:
+        return None, None, None
+    terms = []
+    for b, v in enumerate(_per_utterance(blends, n, "speaker blends")):
+        terms.append([] if v is None else _blend_terms(model, v, f"utterance {b}" if who is None else who[b]))
+    if not any(terms):
+        return None, None, None
+    offs = np.zeros(n + 1, np.uint64)
+    offs[1:] = np.cumsum([len(t) for t in terms])
+    flat = [x for t in terms for x in t]
+    return (np.array([s for s, _ in flat], np.int64), np.array([w for _, w in flat], np.float32), offs)
+
+
 def _who(b) -> str:
     """What an error names: utterance b of a batch, or a label such as "stream 3" given instead of the index."""
     return b if isinstance(b, str) else f"utterance {b}"
@@ -561,9 +620,11 @@ class _VitsCommons:
                     configs: Optional[Sequence[PiperSynthesisConfig]] = None, seeds: Optional[Sequence] = None,
                     output_rates: Optional[Sequence] = None, loudness: Optional[Sequence] = None,
                     pitches: Optional[Sequence] = None, tempos: Optional[Sequence] = None,
-                    pitch_contours: Optional[Sequence] = None, formants: Optional[Sequence] = None) -> List[Audio]:
+                    pitch_contours: Optional[Sequence] = None, formants: Optional[Sequence] = None,
+                    speaker_blends: Optional[Sequence] = None) -> List[Audio]:
         """`configs`: one PiperSynthesisConfig per utterance (speaker and scales), still synthesised as one pass;
         None uses the fallback config for every utterance.  `seeds`: noise seeds as for infer_batch_with_values.
+        `speaker_blends`: as for infer_batch_with_values.
         `output_rates` / `loudness` / `pitches` / `tempos` / `formants`: per-utterance output sample rates, loudness
         targets, pitch and tempo ratios and formant ratios as for infer_batch_with_values.  `pitch_contours`: as for
         speak_batch_with_alignment, one ratio per phoneme character."""
@@ -574,15 +635,20 @@ class _VitsCommons:
         loud = _loudness_array(loudness, n)
         pros = any(a is not None for a in _prosody_arrays(pitches, tempos, n))
         fmt = _formant_array(formants, n)
+        blend = _blend_arrays(self, speaker_blends, n)[0] is not None
         if n == 0:
             return []
         if pitch_contours is not None:
             return [a for a, _ in self.speak_batch_with_alignment(phoneme_batches, configs, seeds=seeds,
                                                                   output_rates=output_rates, loudness=loudness,
                                                                   pitches=pitches, tempos=tempos,
-                                                                  pitch_contours=pitch_contours, formants=formants)]
-        if configs is not None or sv is not None or rates is not None or loud is not None or pros or fmt is not None:
+                                                                  pitch_contours=pitch_contours, formants=formants,
+                                                                  speaker_blends=speaker_blends)]
+        if (configs is not None or sv is not None or rates is not None or loud is not None or pros or fmt is not None
+                or blend):
             extra = {} if sv is None else {"seeds": seeds}
+            if blend:
+                extra["speaker_blends"] = speaker_blends
             if fmt is not None:
                 extra["formants"] = formants
             if pros:
@@ -614,7 +680,8 @@ class _VitsCommons:
                                 loudness: Optional[Sequence] = None, pitches: Optional[Sequence] = None,
                                 tempos: Optional[Sequence] = None,
                                 pitch_contours: Optional[Sequence] = None,
-                                formants: Optional[Sequence] = None) -> List[Audio]:
+                                formants: Optional[Sequence] = None,
+                                speaker_blends: Optional[Sequence] = None) -> List[Audio]:
         """Batched infer_with_values.  `configs`: one PiperSynthesisConfig per utterance (speaker and scales), or None
         for the fallback config; each utterance's result equals a single-utterance call with its config as the
         fallback, except for the on-device noise of an unseeded utterance, whose draws depend on the batch position.
@@ -649,7 +716,14 @@ class _VitsCommons:
         the pitch stage (sb200_speak_batch_ids_formants): 1.0 with a pitch ratio or contour keeps the formants where
         they were, so the voice sounds like the same speaker at another pitch (unlike the other ratios, an explicit 1.0
         asks for something there), and a ratio without a pitch moves them at the same pitch and duration.  Lengths and
-        alignments do not change."""
+        alignments do not change.
+
+        `speaker_blends`: one blend or None per utterance, or None.  A blend is a mapping {speaker: weight} of a
+        multi-speaker voice: keys are speaker ids or names of its speaker_id_map, weights finite and >= 0, not all zero.
+        The utterance speaks with the weighted mean of those speakers' embeddings, which replaces its config's speaker
+        (the config's scales still apply; include/sonata_b200.h, sb200_speak_batch_ids_blends).  A blend of one speaker
+        (any positive weight) gives that speaker's bits, and blends equal up to order, zero weights or a common
+        power-of-two scale give the same bits."""
         n = len(batches)
         cfgs = _config_array(configs, n)
         sv, _ = _seed_arrays(seeds, n)
@@ -659,8 +733,12 @@ class _VitsCommons:
         pros = pit is not None or tem is not None
         contour = _contour_arrays([len(b) for b in batches], pitch_contours, pit)
         fmt = _formant_array(formants, n)
-        if sv is not None or rates is not None or loud is not None or pros or contour is not None or fmt is not None:
+        blend = _blend_arrays(self, speaker_blends, n)[0] is not None
+        if (sv is not None or rates is not None or loud is not None or pros or contour is not None or fmt is not None
+                or blend):
             extra = _prosody_kwargs(pitches, tempos) if pros else {}
+            if blend:
+                extra["speaker_blends"] = speaker_blends
             if contour is not None:
                 extra["pitch_contours"] = pitch_contours
             if fmt is not None:
@@ -687,7 +765,8 @@ class _VitsCommons:
                                    loudness: Optional[Sequence] = None, pitches: Optional[Sequence] = None,
                                    tempos: Optional[Sequence] = None,
                                    pitch_contours: Optional[Sequence] = None,
-                                   formants: Optional[Sequence] = None) -> List[Tuple[Audio, np.ndarray]]:
+                                   formants: Optional[Sequence] = None,
+                                   speaker_blends: Optional[Sequence] = None) -> List[Tuple[Audio, np.ndarray]]:
         """infer_batch_with_values with per-id duration control, returning (audio, frames per id) per utterance.
 
         duration_scales[b]: one scale (finite, >= 0) per id of utterance b, applied before the duration's ceil, so 1.0
@@ -695,13 +774,15 @@ class _VitsCommons:
         Either list, or any of its entries, may be None.  The frame counts times 256 are each id's samples; an
         utterance whose ids all got 0 frames is still one frame long.  `seeds`: as for infer_batch_with_values; a
         seeded frame's noise depends on its index only, so controls that move frames never reshuffle it.
-        `output_rates` / `loudness` / `pitches` / `tempos` / `pitch_contours` / `formants`: as for
+        `output_rates` / `loudness` / `pitches` / `tempos` / `pitch_contours` / `formants` / `speaker_blends`: as for
         infer_batch_with_values (the frame counts stay frame counts of the utterance before any warp)."""
         return [(a, f) for a, f, _ in self._speak_ids(batches, configs, duration_scales, durations, seeds, output_rates,
-                                                       loudness, pitches, tempos, pitch_contours, formants)]
+                                                       loudness, pitches, tempos, pitch_contours, formants,
+                                                       speaker_blends)]
 
     def _speak_ids(self, batches, configs, duration_scales, durations, seeds, output_rates, loudness, pitches, tempos,
-                   pitch_contours, formants=None) -> List[Tuple[Audio, np.ndarray, Optional[np.ndarray]]]:
+                   pitch_contours, formants=None,
+                   speaker_blends=None) -> List[Tuple[Audio, np.ndarray, Optional[np.ndarray]]]:
         """infer_batch_with_durations with each id's delivered end (None without a contour) per utterance."""
         n = len(batches)
         cfgs = _config_array(configs, n)
@@ -713,6 +794,7 @@ class _VitsCommons:
         pit, tem = _prosody_arrays(pitches, tempos, n)
         contour = _contour_arrays(lens, pitch_contours, pit)
         fmt = _formant_array(formants, n)
+        bs, bw, bo = _blend_arrays(self, speaker_blends, n)
         if n == 0:
             return []
         if any(x == 0 for x in lens):
@@ -724,7 +806,16 @@ class _VitsCommons:
         id_frames = np.zeros(int(offs[-1]), np.int32)
         err = N.sb200_error()
         bounds = None
-        if fmt is not None:
+        if bo is not None:
+            bounds = None if contour is None else np.zeros(int(offs[-1]), np.int64)
+            _check(self._lib.sb200_speak_batch_ids_blends(
+                self._h, packed.ctypes.data_as(C.POINTER(C.c_int64)), offs.ctypes.data_as(C.POINTER(C.c_size_t)), n,
+                cfgs, _ptr(scales, C.c_float), _ptr(frames, C.c_int32), _ptr(sv, C.c_uint64), _ptr(sf, C.c_int32),
+                _ptr(rates, C.c_uint32), _ptr(loud, C.c_float), _ptr(pit, C.c_float), _ptr(tem, C.c_float),
+                _ptr(contour, C.c_float), _ptr(fmt, C.c_float), _ptr(bs, C.c_int64), _ptr(bw, C.c_float),
+                _ptr(bo, C.c_size_t), outs, _ptr(id_frames, C.c_int32), _ptr(bounds, C.c_int64), None, None,
+                C.byref(err)), err)
+        elif fmt is not None:
             bounds = None if contour is None else np.zeros(int(offs[-1]), np.int64)
             _check(self._lib.sb200_speak_batch_ids_formants(
                 self._h, packed.ctypes.data_as(C.POINTER(C.c_int64)), offs.ctypes.data_as(C.POINTER(C.c_size_t)), n,
@@ -756,7 +847,8 @@ class _VitsCommons:
                                    output_rates: Optional[Sequence] = None,
                                    loudness: Optional[Sequence] = None, pitches: Optional[Sequence] = None,
                                    tempos: Optional[Sequence] = None, pitch_contours: Optional[Sequence] = None,
-                                   formants: Optional[Sequence] = None) -> List[Tuple[Audio, List[PhonemeAlignment]]]:
+                                   formants: Optional[Sequence] = None,
+                                   speaker_blends: Optional[Sequence] = None) -> List[Tuple[Audio, List[PhonemeAlignment]]]:
         """speak_batch that also says when each phoneme is spoken: per utterance (audio, alignment), the alignment
         holding one entry for bos (`^`), one per kept phoneme character (its id and its trailing pad) and one for eos
         (`$`), contiguous from sample 0 to len(audio).
@@ -774,10 +866,13 @@ class _VitsCommons:
         / 1.0 for none), applied to that character's id and pad, bos and eos keeping their pitch; see
         infer_batch_with_values.  An utterance with a contour is aligned from each id's delivered end
         (sb200_speak_batch_ids_contour), exact rather than scaled: with no tempo a boundary stays where it was.
-        `formants`: as for infer_batch_with_values; it moves no boundary."""
+        `formants`: as for infer_batch_with_values; it moves no boundary.  `speaker_blends`: as for
+        infer_batch_with_values."""
         n = len(phoneme_batches)
         _config_array(configs, n)
         _seed_arrays(seeds, n)
+        if _blend_arrays(self, speaker_blends, n)[0] is None:
+            speaker_blends = None
         _rate_array(output_rates, n)
         _loudness_array(loudness, n)
         pit, tem = _prosody_arrays(pitches, tempos, n)
@@ -811,13 +906,15 @@ class _VitsCommons:
             extra.update(_prosody_kwargs(pitches, tempos))
         if _formant_array(formants, n) is not None:
             extra["formants"] = formants
+        if speaker_blends is not None:
+            extra["speaker_blends"] = speaker_blends
         if id_contours is None:
             res = [(a, f, None) for a, f in self.infer_batch_with_durations([m[0] for m in maps], configs, id_scales,
                                                                             **extra)]
         else:
             res = self._speak_ids([m[0] for m in maps], configs, id_scales, None, extra.get("seeds"),
                                   extra.get("output_rates"), extra.get("loudness"), extra.get("pitches"),
-                                  extra.get("tempos"), id_contours, extra.get("formants"))
+                                  extra.get("tempos"), id_contours, extra.get("formants"), speaker_blends)
         voice_rate = self.audio_output_info().sample_rate if output_rates is not None else None
         ratio = lambda audio: (1, 1) if voice_rate is None else rate_ratio(voice_rate, audio.info.sample_rate)
         shaped = [id_contours is not None and c is not None and any(not (math.isnan(x) or x == 1.0) for x in c)
@@ -829,14 +926,15 @@ class _VitsCommons:
                          configs: Optional[Sequence[PiperSynthesisConfig]] = None, seeds: Optional[Sequence] = None,
                          output_rates: Optional[Sequence] = None, loudness: Optional[Sequence] = None,
                          gains: Optional[Sequence] = None, pitches: Optional[Sequence] = None,
-                         tempos: Optional[Sequence] = None, formants: Optional[Sequence] = None) -> List[bytes]:
+                         tempos: Optional[Sequence] = None, formants: Optional[Sequence] = None,
+                         speaker_blends: Optional[Sequence] = None) -> List[bytes]:
         """infer_batch_with_values delivered as G.711 telephony audio: one `bytes` per utterance, one byte per sample.
         `law`: "mulaw" (PCMU) or "alaw" (PCMA), or one of those per utterance.  The bytes are G.711 of exactly the
         16-bit samples the i16 route gives (SynthesisJob.fetch_i16): to_i16_vec of the utterance after gains[b] (None:
         1), or the fixed scale for an utterance with a loudness target.  They are encoded on the device in the i16
         conversion's launches, so only one byte per sample leaves the card.  `configs`, `seeds`, `output_rates` and
-        `loudness` as for infer_batch_with_values, and so are `pitches`, `tempos` and `formants`; a batch mixing laws
-        runs one conversion per law."""
+        `loudness` as for infer_batch_with_values, and so are `pitches`, `tempos`, `formants` and `speaker_blends`; a
+        batch mixing laws runs one conversion per law."""
         from .job import SynthesisJob
         n = len(batches)
         _config_array(configs, n)
@@ -847,12 +945,13 @@ class _VitsCommons:
         _gain_array(gains, n)
         _prosody_arrays(pitches, tempos, n)
         _formant_array(formants, n)
+        _blend_arrays(self, speaker_blends, n)
         if n == 0:
             return []
         if any(len(b) == 0 for b in batches):
             raise OperationError("Failed to run model inference. Error: empty input sequence")
         job = SynthesisJob(self, batches, configs=configs, seeds=seeds, output_rates=output_rates, loudness=loudness,
-                           pitches=pitches, tempos=tempos, formants=formants)
+                           pitches=pitches, tempos=tempos, formants=formants, speaker_blends=speaker_blends)
         try:
             job.run()
             out: List[Optional[bytes]] = [None] * n
@@ -869,24 +968,26 @@ class _VitsCommons:
                          configs: Optional[Sequence[PiperSynthesisConfig]] = None, seeds: Optional[Sequence] = None,
                          output_rates: Optional[Sequence] = None, loudness: Optional[Sequence] = None,
                          gains: Optional[Sequence] = None, pitches: Optional[Sequence] = None,
-                         tempos: Optional[Sequence] = None, formants: Optional[Sequence] = None) -> List[bytes]:
+                         tempos: Optional[Sequence] = None, formants: Optional[Sequence] = None,
+                         speaker_blends: Optional[Sequence] = None) -> List[bytes]:
         """speak_batch delivered as G.711 bytes: infer_batch_g711 over the phonemes' ids."""
         n = len(phoneme_batches)
         _config_array(configs, n)
         _encoding_list(law, n)
         return self.infer_batch_g711([self.phonemes_to_input_ids(p) for p in phoneme_batches], law, configs, seeds,
-                                     output_rates, loudness, gains, pitches, tempos, formants)
+                                     output_rates, loudness, gains, pitches, tempos, formants, speaker_blends)
 
     def infer_batch_flac(self, batches: Sequence[Sequence[int]],
                          configs: Optional[Sequence[PiperSynthesisConfig]] = None, seeds: Optional[Sequence] = None,
                          output_rates: Optional[Sequence] = None, loudness: Optional[Sequence] = None,
                          gains: Optional[Sequence] = None, pitches: Optional[Sequence] = None,
-                         tempos: Optional[Sequence] = None, formants: Optional[Sequence] = None) -> List[bytes]:
+                         tempos: Optional[Sequence] = None, formants: Optional[Sequence] = None,
+                         speaker_blends: Optional[Sequence] = None) -> List[bytes]:
         """infer_batch_with_values delivered as lossless FLAC: one complete stream (`bytes`) per utterance.  Its samples
         are exactly the 16-bit samples the i16 route gives (SynthesisJob.fetch_i16): to_i16_vec of the utterance after
         gains[b] (None: 1), or the fixed scale for an utterance with a loudness target, at its delivered rate.  They are
         encoded on the device, and only the compressed bytes leave the card.  `configs`, `seeds`, `output_rates`,
-        `loudness`, `pitches`, `tempos` and `formants` as for infer_batch_with_values."""
+        `loudness`, `pitches`, `tempos`, `formants` and `speaker_blends` as for infer_batch_with_values."""
         from .job import SynthesisJob
         n = len(batches)
         _config_array(configs, n)
@@ -896,12 +997,13 @@ class _VitsCommons:
         _gain_array(gains, n)
         _prosody_arrays(pitches, tempos, n)
         _formant_array(formants, n)
+        _blend_arrays(self, speaker_blends, n)
         if n == 0:
             return []
         if any(len(b) == 0 for b in batches):
             raise OperationError("Failed to run model inference. Error: empty input sequence")
         job = SynthesisJob(self, batches, configs=configs, seeds=seeds, output_rates=output_rates, loudness=loudness,
-                           pitches=pitches, tempos=tempos, formants=formants)
+                           pitches=pitches, tempos=tempos, formants=formants, speaker_blends=speaker_blends)
         try:
             job.run()
             return job.fetch_flac(gains)
@@ -912,11 +1014,12 @@ class _VitsCommons:
                          configs: Optional[Sequence[PiperSynthesisConfig]] = None, seeds: Optional[Sequence] = None,
                          output_rates: Optional[Sequence] = None, loudness: Optional[Sequence] = None,
                          gains: Optional[Sequence] = None, pitches: Optional[Sequence] = None,
-                         tempos: Optional[Sequence] = None, formants: Optional[Sequence] = None) -> List[bytes]:
+                         tempos: Optional[Sequence] = None, formants: Optional[Sequence] = None,
+                         speaker_blends: Optional[Sequence] = None) -> List[bytes]:
         """speak_batch delivered as FLAC streams: infer_batch_flac over the phonemes' ids."""
         _config_array(configs, len(phoneme_batches))
         return self.infer_batch_flac([self.phonemes_to_input_ids(p) for p in phoneme_batches], configs, seeds,
-                                     output_rates, loudness, gains, pitches, tempos, formants)
+                                     output_rates, loudness, gains, pitches, tempos, formants, speaker_blends)
 
     def _cfg(self, fn) -> PiperSynthesisConfig:
         c, err = N.sb200_synth_config(), N.sb200_error()
@@ -1174,17 +1277,20 @@ class VitsStreamingModel(_VitsCommons):
                             configs: Optional[Sequence[PiperSynthesisConfig]] = None,
                             duration_scales: Optional[Sequence] = None,
                             durations: Optional[Sequence] = None,
-                            seeds: Optional[Sequence] = None) -> List[EncoderOutputs]:
+                            seeds: Optional[Sequence] = None,
+                            speaker_blends: Optional[Sequence] = None) -> List[EncoderOutputs]:
         """infer_encoder over many utterances in one encoder pass.  `configs`: one PiperSynthesisConfig per utterance,
         or None for the fallback config; each latent equals infer_encoder alone with its config as the fallback,
         except for the on-device noise of an unseeded utterance, whose draws depend on the batch position.
         `duration_scales` / `durations`: per-id duration controls as for infer_batch_with_durations; each output's
         `p_duration` holds its frames per id.  `seeds`: noise seeds as for infer_batch_with_values; a seeded latent
-        equals the `z` of the same utterance synthesised with the same seed."""
+        equals the `z` of the same utterance synthesised with the same seed.  `speaker_blends`: as for
+        infer_batch_with_values; each latent keeps its blend, and every decoder chunk of it speaks with that blend."""
         n = len(batches)
         cfgs = _config_array(configs, n)
         scales, frames = _duration_arrays([len(b) for b in batches], duration_scales, durations)
         sv, sf = _seed_arrays(seeds, n)
+        bs, bw, bo = _blend_arrays(self, speaker_blends, n)
         if any(len(b) == 0 for b in batches):
             raise OperationError("Failed to run model inference. Error: empty input sequence")
         if n == 0:
@@ -1194,11 +1300,19 @@ class VitsStreamingModel(_VitsCommons):
         offs[1:] = np.cumsum([len(b) for b in batches])
         outs = (C.c_void_p * n)()
         err = N.sb200_error()
-        _check(self._lib.sb200_encode_batch_ids_seeded(self._h, packed.ctypes.data_as(C.POINTER(C.c_int64)),
-                                                       offs.ctypes.data_as(C.POINTER(C.c_size_t)), n, cfgs,
-                                                       _ptr(scales, C.c_float), _ptr(frames, C.c_int32),
-                                                       _ptr(sv, C.c_uint64), _ptr(sf, C.c_int32), outs,
-                                                       C.byref(err)), err)
+        if bo is None:
+            _check(self._lib.sb200_encode_batch_ids_seeded(self._h, packed.ctypes.data_as(C.POINTER(C.c_int64)),
+                                                           offs.ctypes.data_as(C.POINTER(C.c_size_t)), n, cfgs,
+                                                           _ptr(scales, C.c_float), _ptr(frames, C.c_int32),
+                                                           _ptr(sv, C.c_uint64), _ptr(sf, C.c_int32), outs,
+                                                           C.byref(err)), err)
+        else:
+            _check(self._lib.sb200_encode_batch_ids_blends(self._h, packed.ctypes.data_as(C.POINTER(C.c_int64)),
+                                                           offs.ctypes.data_as(C.POINTER(C.c_size_t)), n, cfgs,
+                                                           _ptr(scales, C.c_float), _ptr(frames, C.c_int32),
+                                                           _ptr(sv, C.c_uint64), _ptr(sf, C.c_int32),
+                                                           _ptr(bs, C.c_int64), _ptr(bw, C.c_float),
+                                                           _ptr(bo, C.c_size_t), outs, C.byref(err)), err)
         return [EncoderOutputs(self, C.c_void_p(outs[i])) for i in range(n)]
 
     def infer_decoder_batch(self, chunks: Sequence[tuple], pcm16: bool = False, fade: int = 0,
@@ -1311,8 +1425,10 @@ class VitsStreamingModel(_VitsCommons):
                          encoding: Optional[str] = None, gain: Optional[float] = None,
                          pitch: Optional[float] = None, tempo: Optional[float] = None,
                          pitch_contour: Optional[Sequence] = None,
-                         formant_ratio: Optional[float] = None) -> SpeechStreamer:
+                         formant_ratio: Optional[float] = None, speaker_blend=None) -> SpeechStreamer:
         """`formant_ratio` is refused: streams do not carry the formant stage.
+        `speaker_blend`: the sentence's speaker blend (a mapping {speaker: weight}, see infer_batch_with_values), or
+        None for the fallback config's speaker; the latent keeps it, so every chunk speaks with it.
         `seed`: the sentence's noise seed (see infer_batch_with_values), or None for positional noise.
         `output_rate`: the chunks' sample rate (see infer_batch_with_values), the sentence resampled as one stream.
         `encoding`: "mulaw" / "alaw" for chunks of G.711 `bytes`: each is G.711 of to_i16_vec of the chunk the stream
@@ -1333,6 +1449,7 @@ class VitsStreamingModel(_VitsCommons):
         _rate_array([output_rate], 1)
         refuse_flac(encoding, "stream_synthesis")
         g = _stream_gain(encoding, gain)
+        blended = _blend_arrays(self, [speaker_blend], 1, ["stream"])[0] is not None
         contour = None
         if pitch_contour is None:
             ids = self.phonemes_to_input_ids(phonemes)
@@ -1340,7 +1457,10 @@ class VitsStreamingModel(_VitsCommons):
             ids, src = self.phonemes_to_input_ids_map(phonemes)
             contour = _char_values_to_ids(pitch_contour, phonemes, src, "stream", "pitch ratios", _contour_value)
             _contour_arrays([len(ids)], [contour], pit, ["stream"])
-        enc = self.infer_encoder(ids) if seed is None else self.infer_encoder_batch([ids], seeds=[seed])[0]
+        if blended:
+            enc = self.infer_encoder_batch([ids], seeds=[seed], speaker_blends=[speaker_blend])[0]
+        else:
+            enc = self.infer_encoder(ids) if seed is None else self.infer_encoder_batch([ids], seeds=[seed])[0]
         return SpeechStreamer(enc, chunk_size, chunk_padding, _stream_resampler(self, output_rate), encoding, g,
                               _stream_prosody(self, pitch, tempo, contour, enc))
 
@@ -1411,7 +1531,7 @@ class StreamBatch:
         self.model = model
         self.chunk_size, self.chunk_padding = chunk_size, chunk_padding
         self._pending: list = []      # (key, ids, config, chunk_size, seed, output rate, encoding, gain, pitch, tempo,
-                                      # per-id contour) not encoded yet
+                                      # per-id contour, speaker blend) not encoded yet
         self._active: List[_Stream] = []
         self._retired: dict = {}      # key -> delivered ends (None: no contour) of the streams the last step ended
         self._next_key = 0
@@ -1419,7 +1539,8 @@ class StreamBatch:
     def add(self, ids_or_phonemes, config: Optional[PiperSynthesisConfig] = None, seed: Optional[int] = None,
             output_rate: Optional[int] = None, encoding: Optional[str] = None, gain: Optional[float] = None,
             pitch: Optional[float] = None, tempo: Optional[float] = None,
-            pitch_contour: Optional[Sequence] = None, formant_ratio: Optional[float] = None) -> int:
+            pitch_contour: Optional[Sequence] = None, formant_ratio: Optional[float] = None,
+            speaker_blend=None) -> int:
         """`seed`: the stream's noise seed (see infer_batch_with_values); a seeded stream yields what
         `stream_synthesis(..., seed=seed)` yields, whatever other streams share its encoder pass.  `output_rate`,
         `encoding` and `gain`: the stream's sample rate and G.711 encoding, as for stream_synthesis; `pitch` / `tempo`:
@@ -1427,19 +1548,22 @@ class StreamBatch:
         for stream_synthesis; its length and values are checked here, and what needs the sentence's frames fails as the
         stream's error item.  `bounds(key)` gives a contoured stream's per-id delivered ends once it is encoded.  A
         warped stream's chunks go through passes of their own, so the other streams keep their passes and their
-        bits.  `formant_ratio` is refused: streams do not carry the formant stage."""
+        bits.  `formant_ratio` is refused: streams do not carry the formant stage.  `speaker_blend`: the stream's
+        speaker blend, as for stream_synthesis; it replaces its config's speaker and is checked here."""
         refuse_formants(formant_ratio, "StreamBatch")
         if not isinstance(self.model, VitsStreamingModel):
             refuse_prosody(pitch, tempo, "StreamBatch")
             refuse_contour(pitch_contour, "StreamBatch")
         return self._add(ids_or_phonemes, config, self.chunk_size, seed, output_rate, encoding, gain, pitch, tempo,
-                         pitch_contour)
+                         pitch_contour, speaker_blend)
 
     def _add(self, ids_or_phonemes, config, chunk_size: int, seed: Optional[int] = None,
              output_rate: Optional[int] = None, encoding: Optional[str] = None, gain: Optional[float] = None,
-             pitch: Optional[float] = None, tempo: Optional[float] = None, pitch_contour=None) -> int:
+             pitch: Optional[float] = None, tempo: Optional[float] = None, pitch_contour=None,
+             speaker_blend=None) -> int:
         if config is not None and not isinstance(config, PiperSynthesisConfig):
             raise OperationError("Invalid configuration for Vits Model")
+        _blend_arrays(self.model, [speaker_blend], 1, [f"stream {self._next_key}"])
         pit, _ = _prosody_arrays([pitch], [tempo], 1)
         _seed_arrays([seed], 1)
         _rate_array([output_rate], 1)
@@ -1463,7 +1587,8 @@ class StreamBatch:
             raise OperationError("Failed to run model inference. Error: empty input sequence")
         key = self._next_key
         self._next_key += 1
-        self._pending.append((key, ids, config, chunk_size, seed, output_rate, encoding, gain, pitch, tempo, contour))
+        self._pending.append((key, ids, config, chunk_size, seed, output_rate, encoding, gain, pitch, tempo, contour,
+                              speaker_blend))
         return key
 
     def bounds(self, key) -> Optional[np.ndarray]:
@@ -1497,9 +1622,12 @@ class StreamBatch:
 
             def encode(ps):
                 configs = None if fallback is None else [fallback if p[2] is None else p[2] for p in ps]
+                extra = {}
+                if any(p[11] is not None for p in ps):
+                    extra["speaker_blends"] = [p[11] for p in ps]
                 if all(p[4] is None for p in ps):
-                    return self.model.infer_encoder_batch([p[1] for p in ps], configs)
-                return self.model.infer_encoder_batch([p[1] for p in ps], configs, seeds=[p[4] for p in ps])
+                    return self.model.infer_encoder_batch([p[1] for p in ps], configs, **extra)
+                return self.model.infer_encoder_batch([p[1] for p in ps], configs, seeds=[p[4] for p in ps], **extra)
             for p, (enc, err) in zip(pend, _each_or_alone(encode, pend)):
                 if err is None:
                     try:

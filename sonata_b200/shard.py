@@ -11,7 +11,7 @@ from __future__ import annotations
 
 import ctypes as C
 import os
-from typing import Callable, List, Optional, Sequence
+from typing import Callable, List, Optional, Sequence, Tuple
 
 import numpy as np
 import torch
@@ -217,8 +217,8 @@ class Frontend:
     libsonata's callback receives, at half the device->host bytes.  Every device / host buffer is allocated once and
     reused; the collectives carry only ids, per-utterance configs and length tables.  `run_local(ids_list, dst, capacity,
     fmt)` is the per-rank synthesis hook (default: the CUDA job of `model`), called with `configs=` (the shard's configs in
-    its utterance order) only when the caller gave configs, and `seeds=` likewise; the gloo tests pass a deterministic
-    stand-in."""
+    its utterance order) only when the caller gave configs, and `seeds=` and `speaker_blends=` likewise; the gloo tests
+    pass a deterministic stand-in."""
 
     def __init__(self, model=None, group=None, pcm16: bool = False, pin: bool = True, run_local: Optional[Callable] = None):
         self.model, self.group, self.pcm16 = model, group, pcm16
@@ -236,7 +236,8 @@ class Frontend:
 
     # -- collective plumbing ----------------------------------------------------------------------------------------
     FIRST_BLOCK = 1 << 18      # int64 elements (2 MB) of the first broadcast: [n, total, has, lens, owner, ids ...,
-    #                            configs: 4 words per utterance when has & 1, seeds: 2 words per utterance when has & 2]
+    #                            configs: 4 words per utterance when has & 1, seeds: 2 words per utterance when has & 2,
+    #                            speaker blends when has & 4: n + 1 offsets, then the m speaker ids and m weights]
 
     @staticmethod
     def _encode_configs(configs) -> np.ndarray:
@@ -273,10 +274,43 @@ class Frontend:
         vals = w[:, 1].view(np.uint64)
         return [int(v) if f else None for f, v in zip(w[:, 0].tolist(), vals.tolist())]
 
-    def _bcast_ids(self, batches, configs=None, seeds=None):
+    def _encode_blends(self, blends, n: int) -> Optional[np.ndarray]:
+        """int64 image of per-utterance speaker blends, or None when no utterance has one: the n + 1 offsets of each
+        utterance's terms, their speaker ids, then their f32 weights as float64 bits.  Names are resolved here, with
+        the checks of piper._blend_arrays; without a model (a run_local stand-in) the keys must be ids."""
+        if blends is None:
+            return None
+        from .piper import _blend_arrays, _per_utterance
+        if self.model is not None:
+            spk, w, offs = _blend_arrays(self.model, blends, n)
+            if offs is None:
+                return None
+        else:
+            terms = [[] if b is None else [(int(k), float(np.float32(u))) for k, u in b.items()]
+                     for b in _per_utterance(blends, n, "speaker blends")]
+            if not any(terms):
+                return None
+            offs = np.concatenate([[0], np.cumsum([len(t) for t in terms])])
+            spk = np.array([k for t in terms for k, _ in t], np.int64)
+            w = np.array([u for t in terms for _, u in t], np.float32)
+        return np.concatenate([offs.astype(np.int64), spk.astype(np.int64), w.astype(np.float64).view(np.int64)])
+
+    @staticmethod
+    def _decode_blends(words: np.ndarray, n: int) -> Tuple[list, int]:
+        """The blends of _encode_blends' image at the start of `words` ({speaker id: weight} or None per utterance) and
+        the image's length."""
+        offs = words[:n + 1].astype(np.int64)
+        m = int(offs[-1])
+        spk = words[n + 1:n + 1 + m]
+        w = np.ascontiguousarray(words[n + 1 + m:n + 1 + 2 * m]).view(np.float64)
+        out = [{int(spk[i]): float(w[i]) for i in range(offs[b], offs[b + 1])} or None for b in range(n)]
+        return out, n + 1 + 2 * m
+
+    def _bcast_ids(self, batches, configs=None, seeds=None, blends=None):
         """ONE broadcast of a fixed-size block carries the header and (for up to ~260k ids) everything else, the
         per-utterance configs included; a second broadcast follows only for larger inputs.  Host staging buffers are
-        page-locked and reused.  Seeds, when given, follow the configs; without them the block is what it always was."""
+        page-locked and reused.  Seeds, when given, follow the configs, and blends the seeds; without them the block is
+        what it always was."""
         rank, world = dist.get_rank(self.group), dist.get_world_size(self.group)
         dev = _dev(self.group)
         fb = self.FIRST_BLOCK
@@ -293,19 +327,24 @@ class Frontend:
             n0 = len(batches)
             ids_end = 3 + 2 * n0 + int(lens.sum())
             seed_words = None if seeds is None else self._encode_seeds(seeds, n0)
+            blend_words = self._encode_blends(blends, n0)
             cfg_end = ids_end + (4 * n0 if configs is not None else 0)
-            total = cfg_end + (0 if seed_words is None else seed_words.size)
+            seed_end = cfg_end + (0 if seed_words is None else seed_words.size)
+            total = seed_end + (0 if blend_words is None else blend_words.size)
             if self._host.numel() < total:
                 self._host = torch.empty(int(total * 1.5), dtype=torch.int64, pin_memory=self._host.is_pinned())
             h = self._host.numpy()
-            h[0], h[1], h[2] = n0, total, (configs is not None) | (2 if seed_words is not None else 0)
+            h[0], h[1], h[2] = n0, total, ((configs is not None) | (2 if seed_words is not None else 0)
+                                           | (4 if blend_words is not None else 0))
             h[3:3 + n0] = lens
             h[3 + n0:3 + 2 * n0] = owner
             np.concatenate([np.asarray(b, dtype=np.int64) for b in batches], out=h[3 + 2 * n0:ids_end])
             if configs is not None:
                 h[ids_end:cfg_end] = self._encode_configs(configs)
             if seed_words is not None:
-                h[cfg_end:total] = seed_words
+                h[cfg_end:seed_end] = seed_words
+            if blend_words is not None:
+                h[seed_end:total] = blend_words
             self._payload.copy_(self._host[:fb], non_blocking=True)
         dist.broadcast(self._payload, 0, group=self.group)
         if rank != 0:
@@ -334,7 +373,7 @@ class Frontend:
         lens, owner = flat[3:3 + n], flat[3 + n:3 + 2 * n].copy()
         offs = 3 + 2 * n + np.concatenate([[0], np.cumsum(lens)])
         mine = np.nonzero(owner == rank)[0]
-        my_cfgs = my_seeds = None
+        my_cfgs = my_seeds = my_blends = None
         end = offs[-1]
         if flat[2] & 1:
             words = flat[end:end + 4 * n].reshape(n, 4)
@@ -342,17 +381,24 @@ class Frontend:
             end += 4 * n
         if flat[2] & 2:
             my_seeds = self._decode_seeds(flat[end:end + 2 * n].reshape(n, 2)[mine])
-        return n, owner, mine, [flat[offs[i]:offs[i + 1]].copy() for i in mine], my_cfgs, my_seeds
+            end += 2 * n
+        if flat[2] & 4:
+            every, _ = self._decode_blends(flat[end:], n)
+            my_blends = [every[i] for i in mine]
+        return n, owner, mine, [flat[offs[i]:offs[i + 1]].copy() for i in mine], my_cfgs, my_seeds, my_blends
 
     def synthesize(self, batches: Optional[Sequence[np.ndarray]], device_only: bool = False,
-                   configs: Optional[Sequence] = None, seeds: Optional[Sequence] = None):
+                   configs: Optional[Sequence] = None, seeds: Optional[Sequence] = None,
+                   speaker_blends: Optional[Sequence] = None):
         """Collective.  Rank 0 passes every utterance's ids and gets the waveforms back in utterance order (views into
         the shared segment, valid until the next call); the other ranks pass None and get None.
         `device_only`: stop after the passes (results stay in each GPU's memory): the device-resident timing of bench.py.
         `configs` (rank 0): one PiperSynthesisConfig per utterance; they travel with the ids and each rank runs its
         shard with its utterances' configs.  None: the voice's fallback config everywhere.
         `seeds` (rank 0): one noise seed (int in [0, 2**64) or None) per utterance, as for
-        VitsModel.infer_batch_with_values; a seeded utterance's samples do not depend on the rank or shard it lands on."""
+        VitsModel.infer_batch_with_values; a seeded utterance's samples do not depend on the rank or shard it lands on.
+        `speaker_blends` (rank 0): one speaker blend ({speaker name or id: weight}) or None per utterance, as for
+        VitsModel.infer_batch_with_values; names are resolved to ids on rank 0 and the blends travel with the ids."""
         rank, world = dist.get_rank(self.group), dist.get_world_size(self.group)
         dev = _dev(self.group)
         if rank == 0 and configs is not None and len(configs) != len(batches):
@@ -361,10 +407,14 @@ class Frontend:
         if rank == 0 and seeds is not None:
             from .piper import _seed_arrays
             _seed_arrays(seeds, len(batches))           # argument errors before any collective
-        n, owner, mine, my_ids, my_cfgs, my_seeds = self._bcast_ids(batches, configs, seeds)
+        if rank == 0 and speaker_blends is not None:
+            self._encode_blends(speaker_blends, len(batches))
+        n, owner, mine, my_ids, my_cfgs, my_seeds, my_blends = self._bcast_ids(batches, configs, seeds, speaker_blends)
         extra = {} if my_cfgs is None else {"configs": my_cfgs}
         if my_seeds is not None:
             extra["seeds"] = my_seeds
+        if my_blends is not None:
+            extra["speaker_blends"] = my_blends
         bps = 2 if self.pcm16 else 4
         fmt = 1 if self.pcm16 else 0
         # two-step because the layout of the segment depends on every rank's frame counts: run first (waveforms stay on
@@ -374,7 +424,7 @@ class Frontend:
             from .job import SynthesisJob
             samples_local = []
             if my_ids:
-                job = SynthesisJob(self.model, my_ids, configs=my_cfgs, seeds=my_seeds)
+                job = SynthesisJob(self.model, my_ids, configs=my_cfgs, seeds=my_seeds, speaker_blends=my_blends)
                 self.last_device_ms = job.run()
                 samples_local = job.lengths()[1]
                 if self.collect_profile:

@@ -136,6 +136,16 @@ def _prosody_extra(n: int, pitch_ratio, tempo, formant_ratio=None) -> dict:
     return out
 
 
+def _blend_extra(model, n: int, speaker_blend, where: str) -> dict:
+    """The per-utterance keywords of n sentences that share a request's speaker blend ({} without one), checked first:
+    an OperationError names `where`."""
+    if speaker_blend is None:
+        return {}
+    from .piper import _blend_arrays
+    _blend_arrays(model, [speaker_blend], 1, [where])
+    return {"speaker_blends": [speaker_blend] * n}
+
+
 def _stream_prosody_extra(model, pitch_ratio, tempo, where: str) -> dict:
     """The stream_synthesis keywords of a streaming request's ratios ({} without either).  A model that is not one of
     this library's streaming voices cannot warp a stream on the device and refuses by name (piper.refuse_prosody)."""
@@ -190,10 +200,13 @@ class SonataSpeechSynthesizer:
     # the device before any resampling and loudness (piper.PITCH_RANGE, piper.TEMPO_RANGE).  `formant_ratio` (lazy,
     # parallel and file modes): each sentence's spectral envelope moved by the ratio after the pitch stage; 1.0 with a
     # pitch ratio keeps the voice's own formants (piper.FORMANT_RANGE).  The streamed modes refuse it by name.
+    # `speaker_blend` (every mode): a mapping {speaker: weight} of a multi-speaker voice that every sentence speaks with
+    # in place of the fallback config's speaker (see piper.VitsModel.infer_batch_with_values); checked before any
+    # synthesis.
 
     def _g711_batch(self, phs: List[str], encoding: str, seeds, output_rate, loudness,
                     cfg: Optional[AudioOutputConfig], pitch_ratio=None, tempo=None,
-                    formant_ratio=None) -> List[bytes]:
+                    formant_ratio=None, speaker_blend=None) -> List[bytes]:
         """The G.711 bytes of sentences `phs`, one synthesis pass, each followed by its appended silence."""
         if cfg is not None:
             cfg._check_supported()
@@ -204,6 +217,7 @@ class SonataSpeechSynthesizer:
         if loudness is not None:
             extra["loudness"] = [loudness] * n
         extra.update(_prosody_extra(n, pitch_ratio, tempo, formant_ratio))
+        extra.update(_blend_extra(self.model, n, speaker_blend, "request"))
         if not _device_g711(self.model):
             res = self.model.speak_batch(phs, **extra) if extra else self.model.speak_batch(phs)
             return [self._process(a, cfg).samples.as_g711_bytes(encoding, fixed_scale=loudness is not None)
@@ -221,7 +235,7 @@ class SonataSpeechSynthesizer:
                         seed: Optional[int] = None, output_rate: Optional[int] = None,
                         loudness: Optional[float] = None, encoding: Optional[str] = None,
                         pitch_ratio: Optional[float] = None, tempo: Optional[float] = None,
-                        formant_ratio: Optional[float] = None) -> Iterator[Audio]:
+                        formant_ratio: Optional[float] = None, speaker_blend=None) -> Iterator[Audio]:
         sentence_seed(seed, 0)
         _check_output_rate(output_rate)
         _check_loudness(loudness)
@@ -229,10 +243,11 @@ class SonataSpeechSynthesizer:
         refuse_flac(encoding, "synthesize_lazy")
         check_encoding(encoding)
         pros = _prosody_extra(1, pitch_ratio, tempo, formant_ratio)
+        pros.update(_blend_extra(self.model, 1, speaker_blend, "request"))
         for i, ph in enumerate(self._phonemes(text)):
             if encoding is not None:
                 yield self._g711_batch([ph], encoding, None if seed is None else [sentence_seed(seed, i)], output_rate,
-                                       loudness, output_config, pitch_ratio, tempo, formant_ratio)[0]
+                                       loudness, output_config, pitch_ratio, tempo, formant_ratio, speaker_blend)[0]
                 continue
             if output_rate or loudness is not None or pros:
                 extra = dict(pros) if seed is None else dict(pros, seeds=[sentence_seed(seed, i)])
@@ -250,20 +265,22 @@ class SonataSpeechSynthesizer:
                             seed: Optional[int] = None, output_rate: Optional[int] = None,
                             loudness: Optional[float] = None, encoding: Optional[str] = None,
                             pitch_ratio: Optional[float] = None, tempo: Optional[float] = None,
-                            formant_ratio: Optional[float] = None) -> Iterator[Audio]:
+                            formant_ratio: Optional[float] = None, speaker_blend=None) -> Iterator[Audio]:
         sentence_seed(seed, 0)
         _check_output_rate(output_rate)
         _check_loudness(loudness)
         _check_prosody(pitch_ratio, tempo, formant_ratio)
         refuse_flac(encoding, "synthesize_parallel")
         check_encoding(encoding)
+        _blend_extra(self.model, 1, speaker_blend, "request")
         ph = self._phonemes(text)
         if encoding is not None:
             seeds = None if seed is None else [sentence_seed(seed, i) for i in range(len(ph))]
             return iter(self._g711_batch(ph, encoding, seeds, output_rate, loudness, output_config, pitch_ratio, tempo,
-                                         formant_ratio) if ph else [])
+                                         formant_ratio, speaker_blend) if ph else [])
         extra = {"output_rates": [output_rate] * len(ph)} if output_rate else {}
         extra.update(_prosody_extra(len(ph), pitch_ratio, tempo, formant_ratio))
+        extra.update(_blend_extra(self.model, len(ph), speaker_blend, "request"))
         if loudness is not None:
             extra["loudness"] = [loudness] * len(ph)
         if not ph:
@@ -278,8 +295,8 @@ class SonataSpeechSynthesizer:
                             chunk_size: int = 72, chunk_padding: int = 3,
                             seed: Optional[int] = None, output_rate: Optional[int] = None,
                             encoding: Optional[str] = None, pitch_ratio: Optional[float] = None,
-                            tempo: Optional[float] = None, formant_ratio: Optional[float] = None
-                            ) -> Iterator[AudioSamples]:
+                            tempo: Optional[float] = None, formant_ratio: Optional[float] = None,
+                            speaker_blend=None) -> Iterator[AudioSamples]:
         """RealtimeSpeechStream (:337-382): a background producer pushes chunks into an unbounded channel;
         chunk_size is multiplied by the number of chunks already produced for every following sentence.
         `output_rate`: each sentence is resampled as its own stream (zero history at its start, flushed at its end).
@@ -304,6 +321,8 @@ class SonataSpeechSynthesizer:
             if output_config is not None and output_config.gain() is not None:
                 rate["gain"] = output_config.gain()
         rate.update(pros)
+        if _blend_extra(self.model, 1, speaker_blend, "request"):
+            rate["speaker_blend"] = speaker_blend
         extra = lambda i: dict(rate) if seed is None else dict(rate, seed=sentence_seed(seed, i))
 
         def emit(chunk):
@@ -345,7 +364,7 @@ class SonataSpeechSynthesizer:
                            seed: Optional[int] = None, output_rate: Optional[int] = None,
                            loudness: Optional[float] = None, encoding: Optional[str] = None,
                            pitch_ratio: Optional[float] = None, tempo: Optional[float] = None,
-                           formant_ratio: Optional[float] = None) -> None:
+                           formant_ratio: Optional[float] = None, speaker_blend=None) -> None:
         """:168-198 — parallel mode, concatenated, peak-normalised i16 WAV (at output_rate when given).  With
         `loudness` the WAV is written at the fixed scale (trunc(clamp(x * 32767))), so it keeps the sentences' level.
         With `encoding` the WAV is 8-bit G.711 (WAVE_FORMAT_MULAW / _ALAW, with a `fact` chunk) holding the sentences'
@@ -353,7 +372,8 @@ class SonataSpeechSynthesizer:
         With encoding="flac" the file is one FLAC stream (synthesize_flac) instead of a WAV."""
         if isinstance(encoding, str) and encoding == FLAC:
             data = self.synthesize_flac(text, output_config, seed=seed, output_rate=output_rate, loudness=loudness,
-                                        pitch_ratio=pitch_ratio, tempo=tempo, formant_ratio=formant_ratio)
+                                        pitch_ratio=pitch_ratio, tempo=tempo, formant_ratio=formant_ratio,
+                                        speaker_blend=speaker_blend)
             with open(filename, "wb") as f:
                 f.write(data)
             return
@@ -366,6 +386,8 @@ class SonataSpeechSynthesizer:
             extra["tempo"] = tempo
         if formant_ratio is not None:
             extra["formant_ratio"] = formant_ratio
+        if speaker_blend is not None:
+            extra["speaker_blend"] = speaker_blend
         if check_encoding(encoding) is not None:
             data = b"".join(self.synthesize_parallel(text, output_config, seed=seed, encoding=encoding, **extra))
             if not data:
@@ -373,11 +395,11 @@ class SonataSpeechSynthesizer:
             with open(filename, "wb") as f:
                 f.write(g711_wave_bytes(data, encoding, output_rate or self.model.audio_output_info().sample_rate))
             return
-        self._document(text, output_config, seed, output_rate, loudness, pitch_ratio, tempo, formant_ratio).save_to_file(
-            filename, fixed_scale=loudness is not None)
+        self._document(text, output_config, seed, output_rate, loudness, pitch_ratio, tempo, formant_ratio,
+                       speaker_blend).save_to_file(filename, fixed_scale=loudness is not None)
 
     def _document(self, text: str, output_config: Optional[AudioOutputConfig], seed, output_rate, loudness,
-                  pitch_ratio=None, tempo=None, formant_ratio=None) -> Audio:
+                  pitch_ratio=None, tempo=None, formant_ratio=None, speaker_blend=None) -> Audio:
         """The sentences of synthesize_parallel concatenated: what synthesize_to_file writes as a WAV."""
         extra = {"output_rate": output_rate} if output_rate else {}
         if loudness is not None:
@@ -388,6 +410,8 @@ class SonataSpeechSynthesizer:
             extra["tempo"] = tempo
         if formant_ratio is not None:
             extra["formant_ratio"] = formant_ratio
+        if speaker_blend is not None:
+            extra["speaker_blend"] = speaker_blend
         parts = [a.samples.as_slice() for a in self.synthesize_parallel(text, output_config, seed=seed, **extra)]
         if not parts or sum(len(p) for p in parts) == 0:
             raise OperationError("No speech data to write")
@@ -397,11 +421,13 @@ class SonataSpeechSynthesizer:
     def synthesize_flac(self, text: str, output_config: Optional[AudioOutputConfig] = None,
                         seed: Optional[int] = None, output_rate: Optional[int] = None,
                         loudness: Optional[float] = None, pitch_ratio: Optional[float] = None,
-                        tempo: Optional[float] = None, formant_ratio: Optional[float] = None) -> bytes:
+                        tempo: Optional[float] = None, formant_ratio: Optional[float] = None,
+                        speaker_blend=None) -> bytes:
         """The FLAC file synthesize_to_file(..., encoding="flac") writes: one stream whose decoded samples are exactly
         the 16-bit samples of the WAV the same call writes without an encoding (the concatenation at the document's
         peak, or the fixed scale with `loudness`), encoded on the model's device by flac_encode."""
-        doc = self._document(text, output_config, seed, output_rate, loudness, pitch_ratio, tempo, formant_ratio)
+        doc = self._document(text, output_config, seed, output_rate, loudness, pitch_ratio, tempo, formant_ratio,
+                             speaker_blend)
         s = doc.samples
         return flac_encode(s.to_i16_fixed() if loudness is not None else s.to_i16_vec(), doc.info.sample_rate,
                            getattr(self.model, "device", 0))
@@ -447,10 +473,11 @@ class RealtimeBatch:
     def add(self, text: str, output_config: Optional[AudioOutputConfig] = None, config=None,
             seed: Optional[int] = None, output_rate: Optional[int] = None, encoding: Optional[str] = None,
             pitch_ratio: Optional[float] = None, tempo: Optional[float] = None,
-            formant_ratio: Optional[float] = None) -> int:
+            formant_ratio: Optional[float] = None, speaker_blend=None) -> int:
         """`seed`: the request's noise seed, `output_rate` its sample rate and `encoding` its G.711 encoding, as for
         synthesize_streamed, and `pitch_ratio` / `tempo` its ratios, each sentence warped as its own stream, as there.
-        `formant_ratio` is refused, as there."""
+        `formant_ratio` is refused, as there.  `speaker_blend`: the request's speaker blend, as for synthesize_streamed;
+        it replaces the config's speaker and is checked here, naming the request."""
         from .piper import PiperSynthesisConfig, refuse_formants
         refuse_formants(formant_ratio, "RealtimeBatch")
         pros = _stream_prosody_extra(self.model, pitch_ratio, tempo, "RealtimeBatch")
@@ -464,11 +491,12 @@ class RealtimeBatch:
             raise OperationError("Invalid configuration for Vits Model")
         if config is not None and config.speaker is not None and config.speaker not in (self.model.get_speakers() or {}):
             raise OperationError(f"No speaker was found with the given id `{config.speaker}`")
+        _blend_extra(self.model, 1, speaker_blend, f"request {self._next_key}")
         ids = [self.model.phonemes_to_input_ids(ph) for ph in _sentences(self.model, text)]
         if any(len(i) == 0 for i in ids):
             raise OperationError("Failed to run model inference. Error: empty input sequence")
         req = _Request(self._next_key, ids, output_config, config, self.chunk_size, seed, output_rate or None, encoding)
-        req.prosody = pros
+        req.prosody, req.blend = pros, speaker_blend
         self._next_key += 1
         self._start_sentence(req)
         return req.key
@@ -484,6 +512,8 @@ class RealtimeBatch:
             if req.output_config is not None and req.output_config.gain() is not None:
                 rate["gain"] = req.output_config.gain()
         rate.update(req.prosody)
+        if req.blend is not None:
+            rate["speaker_blend"] = req.blend
         self._by_stream[self._streams._add(req.ids[req.next], req.config, req.cs, sentence_seed(req.seed, req.next),
                                            **rate)] = req
         req.next += 1
