@@ -295,7 +295,8 @@ int32_t sb200_speak_batch_ids_contour(sb200_voice* v, const int64_t* ids_packed,
  * An utterance runs the stage only when phi is finite and some frame has r_m != 1; any other keeps its bits (one with
  * phi == its pitch ratio and no contour among them).  The kernels compute in double with their own FFTs and a fixed
  * order per utterance, so an utterance has the same bits in any batch; a sample is within half an f32 ulp of the
- * float64 specification's value plus 1e-11 (tests/formant_reference.py).  Realtime streams do not take a formant ratio.
+ * float64 specification's value plus 1e-11 (tests/formant_reference.py).  Realtime streams take a formant ratio through
+ * sb200_prosody_stream_create_formant, with the same bits as this call.
  * sb200_speak_batch_ids_contour with formants (NULL: none) one ratio per utterance.  NULL formants is that call, bit for
  * bit. */
 int32_t sb200_speak_batch_ids_formants(sb200_voice* v, const int64_t* ids_packed, const size_t* offsets, size_t batch,
@@ -621,6 +622,32 @@ int32_t sb200_prosody_stream_create_contour(sb200_voice* v, const sb200_latent* 
  * the batch path reports for the same latent.  out[0 .. n_ids); fails with OPERATION_ERROR for a stream made without
  * a contour or a capacity below the id count. */
 int32_t sb200_prosody_stream_bounds(const sb200_prosody_stream* s, int64_t* out, size_t capacity, sb200_error* err);
+/* ---- streams with a formant ratio (see sb200_speak_batch_ids_formants) ----
+ * A prosody stream with a formant ratio phi (NaN: none; else a finite value in [0.5, 2]) on top of a pitch ratio and a
+ * tempo (pitch_per_id NULL: a ratio stream, z may be NULL), or of latent z's contour pitch_per_id[0 .. n_ids) and a
+ * tempo (as sb200_prosody_stream_create_contour; pitch must then be NaN or 1), or of neither.  Unlike the other
+ * creators it accepts ratios that ask for nothing when phi asks for something: a formant-only stream, which changes the
+ * timbre of a plain stream.  The stage runs only when formant_asks holds: phi finite and some frame with p_m / phi != 1
+ * (a contour stream knows n2 at creation); a stream whose phi asks for nothing (phi NaN, or equal to its pitch ratio
+ * without a contour) is the stream without phi: the same chunk counts, bits and launches.  A bad phi fails naming it,
+ * as do ratios and a phi that all ask for nothing and every failure of the other creators, all with OPERATION_ERROR
+ * before any device work.  Lengths, sb200_prosody_stream_bounds and the delivered ends do not depend on phi.
+ * Contract: join the chunks such a stream emits through sb200_decode_chunks_warped; the result is, bit for bit, the y
+ * of sb200_debug_formant over the joined samples appended to the stream (the chunks after the post-path, as for a ratio
+ * stream) with the stream's pitch, tempo, contour (ends = 256 C_i) and phi, then resampled and converted as without phi.
+ * Emission rule: let G be the formant stage's inputs so far (the outputs the pitch stage has emitted or, without pitch
+ * and tempo, the samples appended), N = 1024 and H = 256.  A chunk that does not end the stream emits the stage's outputs
+ * [0, E), E = H max(0, floor((G - (N - H)) / H)): every hop whose 4 frames lie inside the input.  Those frames neither
+ * read past G nor reach the clamp of their centres at n2 - 1, so nothing before the last chunk depends on n2.  The last
+ * chunk emits everything up to n2, reading zeros past the end.  Between chunks the stream holds its inputs from
+ * max(0, E - 3 H) on, fewer than N + 3 H = 1792 of them: the 3 H before E recompute the frames whose overlap-add
+ * reaches E.  The stage holds back G - E = 768 .. 1023 samples on top of the pitch stage's hold-back (35 - 46 ms at
+ * 22.05 kHz, 48 - 64 ms at 16 kHz).  A one-shot stream's single chunk is its last, so it emits everything. */
+int32_t sb200_prosody_stream_create_formant(sb200_voice* v, const sb200_latent* z, float pitch,
+                                            const float* pitch_per_id, size_t n_ids, float tempo, float formant,
+                                            sb200_prosody_stream** out, sb200_error* err);
+/* The "formant" device time (ms) of the last chunk pass the stream was in (0: its stage did not run). */
+int32_t sb200_prosody_stream_profile_formant(const sb200_prosody_stream* s, float* formant_ms);
 
 /* ---- introspection for tests / bench ---- */
 /* Copy a named intermediate of the LAST run of `job` to host (time-major fp32, valid rows of
@@ -795,6 +822,18 @@ int32_t sb200_debug_prosody_contour_stream(int32_t device, const float* x, const
                                            int32_t rate, const int64_t* ends, const float* ratios, size_t n_ids,
                                            float tempo, float* y, size_t cap, int64_t* lens, int32_t* offsets,
                                            size_t offsets_cap, sb200_error* err);
+/* Test hook, no device needed: the samples a stream of sb200_prosody_stream_create_formant emits per chunk at `rate`,
+ * with pitch and tempo, or (ends, ratios: n_ids entries; n_ids 0: none) a contour over n = sum chunk_lens inputs, and
+ * formant ratio `formant`, when its chunks bring chunk_lens[0 .. n_chunks) inputs and the last one ends it.  emitted[k]
+ * receives chunk k's count.  Fails with the creator's errors, or for a negative length. */
+int32_t sb200_debug_formant_stream_plan(int32_t rate, float pitch, float tempo, const int64_t* ends, const float* ratios,
+                                        size_t n_ids, float formant, const int64_t* chunk_lens, size_t n_chunks,
+                                        int64_t* emitted, sb200_error* err);
+/* That stream, fresh on `device`, fed x[0 .. sum chunk_lens) in those chunks with no decoder involved: y receives the
+ * concatenated outputs (cap: its size) and lens[k] chunk k's count. */
+int32_t sb200_debug_formant_stream(int32_t device, const float* x, const int64_t* chunk_lens, size_t n_chunks,
+                                   int32_t rate, float pitch, float tempo, const int64_t* ends, const float* ratios,
+                                   size_t n_ids, float formant, float* y, size_t cap, int64_t* lens, sb200_error* err);
 /* Test hook: G.711 (law as for sb200_job_fetch_g711) of x[0 .. n) into out[0 .. n).  device -1 runs the host copy of
  * the encoders (no device needed); otherwise the encoders run on that device over the buffer. */
 int32_t sb200_debug_g711(int32_t device, int32_t law, const int16_t* x, size_t n, uint8_t* out, sb200_error* err);

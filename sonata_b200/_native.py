@@ -247,6 +247,16 @@ SIGNATURES = {
     "sb200_prosody_stream_create_contour": (C.c_int32, [_P, _P, C.POINTER(C.c_float), C.c_size_t, C.c_float,
                                                         C.POINTER(_P), _ERR]),
     "sb200_prosody_stream_bounds": (C.c_int32, [_P, C.POINTER(C.c_int64), C.c_size_t, _ERR]),
+    "sb200_prosody_stream_create_formant": (C.c_int32, [_P, _P, C.c_float, C.POINTER(C.c_float), C.c_size_t,
+                                                        C.c_float, C.c_float, C.POINTER(_P), _ERR]),
+    "sb200_prosody_stream_profile_formant": (C.c_int32, [_P, C.POINTER(C.c_float)]),
+    "sb200_debug_formant_stream_plan": (C.c_int32, [C.c_int32, C.c_float, C.c_float, C.POINTER(C.c_int64),
+                                                    C.POINTER(C.c_float), C.c_size_t, C.c_float, C.POINTER(C.c_int64),
+                                                    C.c_size_t, C.POINTER(C.c_int64), _ERR]),
+    "sb200_debug_formant_stream": (C.c_int32, [C.c_int32, C.POINTER(C.c_float), C.POINTER(C.c_int64), C.c_size_t,
+                                               C.c_int32, C.c_float, C.c_float, C.POINTER(C.c_int64),
+                                               C.POINTER(C.c_float), C.c_size_t, C.c_float, C.POINTER(C.c_float),
+                                               C.c_size_t, C.POINTER(C.c_int64), _ERR]),
     "sb200_debug_prosody_contour_stream_plan": (C.c_int32, [C.c_int32, C.c_int64, C.POINTER(C.c_int64),
                                                             C.POINTER(C.c_float), C.c_size_t, C.c_float,
                                                             C.POINTER(C.c_int64), C.c_size_t, C.POINTER(C.c_int64)]),

@@ -93,7 +93,8 @@ def build_parser() -> argparse.ArgumentParser:
     ap.add_argument("--formant-ratio", type=float, metavar="RATIO",
                     help="Give the speech the voice's own formants (spectral envelope) with every frequency multiplied "
                          "by RATIO, [0.5, 2], on the GPU after --pitch-ratio: 1 with a pitch ratio keeps the speaker's "
-                         "timbre, another value without one changes it at the same pitch.  Not in realtime mode")
+                         "timbre, another value without one changes it at the same pitch.  In realtime mode (streaming "
+                         "voices only) it holds back 35 - 64 ms more audio")
     ap.add_argument("--encoding", choices=("pcm16",) + ENCODINGS + (FLAC,),
                     help="Output encoding: pcm16 (default), G.711 mulaw / alaw at one byte per sample (telephony: "
                          "PCMU / PCMA), or lossless flac (one FLAC stream per request, on stdout or in the -o file; "
@@ -111,8 +112,8 @@ def process_request(synth: SonataSpeechSynthesizer, default_cfg: PiperSynthesisC
     synth.sentence_seed.  `output_rate` (optional): the sample rate of the WAV or raw PCM written.  `loudness`
     (optional): every sentence's target loudness in LUFS; the PCM is then written at the fixed scale.  `pitch_ratio` /
     `tempo` (optional): the ratios every sentence is shifted and played by, in lazy and parallel modes.
-    `formant_ratio` (optional): the ratio every sentence's formants are moved by after the pitch stage, in lazy and
-    parallel modes (realtime mode refuses it unless it writes a file).  `speaker_blend` (optional): an object
+    `formant_ratio` (optional): the ratio every sentence's formants are moved by after the pitch stage, in every mode
+    (realtime mode carries it as a stream on this library's streaming voices).  `speaker_blend` (optional): an object
     {speaker name or id: weight} (see speaker_blend_of) every sentence speaks with, in every mode."""
     out = out or sys.stdout.buffer
     mode = (req.get("mode") or "lazy").lower()
@@ -134,10 +135,9 @@ def process_request(synth: SonataSpeechSynthesizer, default_cfg: PiperSynthesisC
     pros = {k: req[k] for k in ("pitch_ratio", "tempo", "formant_ratio") if req.get(k) is not None}
     blend = speaker_blend_of(req.get("speaker_blend"))
     _check_prosody(pros.get("pitch_ratio"), pros.get("tempo"), pros.get("formant_ratio"))
-    if mode == "realtime" and not output_file:
+    if mode == "realtime" and not output_file and not isinstance(synth.model, VitsStreamingModel):
         refuse_formants(pros.get("formant_ratio"), "realtime mode")
-        if not isinstance(synth.model, VitsStreamingModel):
-            refuse_prosody(pros.get("pitch_ratio"), pros.get("tempo"), "realtime mode")
+        refuse_prosody(pros.get("pitch_ratio"), pros.get("tempo"), "realtime mode")
     synth.model.set_fallback_synthesis_config(PiperSynthesisConfig(
         req.get("speaker_id"),
         req["noise_scale"] if req.get("noise_scale") is not None else default_cfg.noise_scale,

@@ -765,6 +765,33 @@ int32_t sb200_prosody_stream_create_contour(sb200_voice* v, const sb200_latent* 
                                         v->v};
     });
 }
+int32_t sb200_prosody_stream_create_formant(sb200_voice* v, const sb200_latent* z, float pitch,
+                                            const float* pitch_per_id, size_t n_ids, float tempo, float formant,
+                                            sb200_prosody_stream** out, sb200_error* err) {
+    return guarded(err, [&] {
+        if (!v || !out || (pitch_per_id && !z)) throw Error(19, "null argument");
+        Voice* w = v->v.get();
+        if (w->device < 0 || !w->emb)
+            throw Error(19, "Failed to run model inference. Error: voice was loaded config-only (device -1); libsonata_b200 has no CPU path");
+        std::vector<long long> ends;
+        long long n = -1;
+        if (pitch_per_id) {
+            if (z->l->v != w) throw Error(19, "the latent was not encoded by this voice");
+            const std::vector<int>& f = z->l->id_frames;
+            if (n_ids != f.size())
+                throw Error(19, "pitch contour: " + std::to_string(n_ids) + " ratios for a latent of " +
+                                    std::to_string(f.size()) + " ids");
+            const long long hop = w->a.hop();
+            ends.resize(n_ids);
+            long long c = 0;
+            for (size_t i = 0; i < n_ids; i++) ends[i] = (c += f[i]) * hop;
+            n = z->l->frames * hop;
+        }
+        *out = new sb200_prosody_stream{create_prosody_stream_formant(w, w->device, w->sample_rate, n, ends.data(),
+                                                                      pitch_per_id, n_ids, pitch, tempo, formant),
+                                        v->v};
+    });
+}
 int32_t sb200_prosody_stream_bounds(const sb200_prosody_stream* s, int64_t* out, size_t capacity, sb200_error* err) {
     return guarded(err, [&] {
         if (!s) throw Error(19, "null argument");
@@ -781,6 +808,11 @@ int32_t sb200_prosody_stream_profile(const sb200_prosody_stream* s, float* stret
     if (!s) return 19;
     if (stretch_ms) *stretch_ms = s->p->last_ms[0];
     if (pitch_ms) *pitch_ms = s->p->last_ms[1];
+    return 0;
+}
+int32_t sb200_prosody_stream_profile_formant(const sb200_prosody_stream* s, float* formant_ms) {
+    if (!s) return 19;
+    if (formant_ms) *formant_ms = s->p->last_fm_ms;
     return 0;
 }
 
@@ -1358,13 +1390,14 @@ int32_t sb200_debug_prosody_contour_stream_plan(int32_t rate, int64_t n, const i
 
 namespace {
 // Pushes x through the fresh stream ps chunk by chunk as one-segment passes: `whole` is the whole signal's shape and
-// `counts` what prosody_stream_counts gives for the same stream and chunks, checked against the destinations before
-// any device work.
-void debug_push_stream(ProsodyStream& ps, const ProsodyShape& whole, const std::vector<long long>& counts,
+// `counts` what the stream emits per chunk (prosody_stream_counts' first column every `stride` entries), checked
+// against the destinations before any device work.  A formant stream's stage runs after its pitch stage, or on the
+// chunk itself without one.
+void debug_push_stream(ProsodyStream& ps, const ProsodyShape& whole, const std::vector<long long>& counts, size_t stride,
                        const float* x, const int64_t* chunk_lens, size_t n_chunks, float* y, size_t cap, int64_t* lens,
                        int32_t* offsets, size_t offsets_cap) {
     long long total = 0, out_total = 0;
-    for (size_t k = 0; k < n_chunks; k++) { total += chunk_lens[k]; out_total += counts[5 * k]; }
+    for (size_t k = 0; k < n_chunks; k++) { total += chunk_lens[k]; out_total += counts[stride * k]; }
     if ((size_t)out_total > cap) throw Error(19, "debug prosody stream: the destination is too small for the result");
     if (offsets && ps.sh.stretch && (size_t)whole.F > offsets_cap)
         throw Error(19, "debug prosody stream: the offsets destination is too small");
@@ -1381,26 +1414,47 @@ void debug_push_stream(ProsodyStream& ps, const ProsodyShape& whole, const std::
     int* doff = d.alloc<int>((size_t)whole.F + 4);
     long long* dap = ps.pieces.empty() ? nullptr : d.alloc<long long>((size_t)whole.F + 4);
     float* dy = d.alloc<float>((size_t)whole.n2 + 4);
+    FormantSeg* dfg = ps.fm ? d.alloc<FormantSeg>(1) : nullptr;
+    FormantCarry* dfc = ps.fm ? d.alloc<FormantCarry>(1) : nullptr;
+    float* fwin = ps.fm ? d.alloc<float>((size_t)FM_CARRY + (size_t)whole.n2 + 4) : nullptr;
+    float* dz = ps.fm ? d.alloc<float>((size_t)whole.n2 + 4) : nullptr;
+    const bool warps = prosody_stream_warps(ps);
     long long in_at = 0, out_at = 0;
     for (size_t k = 0; k < n_chunks; k++) {
         const bool last = k + 1 == n_chunks;
         const ProsodyStep t = prosody_stream_step(ps, chunk_lens[k], last);
         ProsodyPlan p;
-        p.add_stream(ps, t);
-        const ProsodyCarry c = prosody_carry(ps, t, 0);
         // the chunk as one segment of single samples at in_at
         const FrameSeg fs{0, (int)chunk_lens[k], 0, 0, in_at};
         SB_CUDA(cudaMemcpy(dfs, &fs, sizeof(fs), cudaMemcpyHostToDevice));
-        SB_CUDA(cudaMemcpy(dg, &p.segs[0], sizeof(ProsodySeg), cudaMemcpyHostToDevice));
-        SB_CUDA(cudaMemcpy(dc, &c, sizeof(c), cudaMemcpyHostToDevice));
-        launch_prosody_stream_stretch(p, dg, dc, dx, dfs, dpost, 1, win, ds, doff, dy, 0, dap);
-        if (p.max_pitch) launch_prosody_pitch(win, ds, dg, 1, p.max_pitch, dy, 0);
+        if (warps) {
+            p.add_stream(ps, t);
+            const ProsodyCarry c = prosody_carry(ps, t, 0);
+            SB_CUDA(cudaMemcpy(dg, &p.segs[0], sizeof(ProsodySeg), cudaMemcpyHostToDevice));
+            SB_CUDA(cudaMemcpy(dc, &c, sizeof(c), cudaMemcpyHostToDevice));
+            launch_prosody_stream_stretch(p, dg, dc, dx, dfs, dpost, 1, win, ds, doff, dy, 0, dap);
+            if (p.max_pitch) launch_prosody_pitch(win, ds, dg, 1, p.max_pitch, dy, 0);
+        }
+        long long m = t.j1 - t.j0;
+        const float* res = dy;
+        if (ps.fm) {
+            const FormantStep f = formant_stream_step(ps, t.next.emitted, last);
+            FormantPlan fp;
+            fp.add_stream(ps, f);
+            const FormantCarry fc = formant_carry(ps, f, 0, warps ? dy : nullptr);
+            SB_CUDA(cudaMemcpy(dfg, &fp.segs[0], sizeof(FormantSeg), cudaMemcpyHostToDevice));
+            SB_CUDA(cudaMemcpy(dfc, &fc, sizeof(fc), cudaMemcpyHostToDevice));
+            launch_formant_stream(fp, dfg, dfc, dx, dfs, dpost, 1, fwin, dz, 0);
+            m = fp.total; res = dz;
+            formant_stream_advance(ps, f);
+        }
         SB_CUDA(cudaDeviceSynchronize());
-        SB_CUDA(cudaMemcpy(y + out_at, dy, (size_t)p.y_total * 4, cudaMemcpyDeviceToHost));
+        SB_CUDA(cudaGetLastError());
+        SB_CUDA(cudaMemcpy(y + out_at, res, (size_t)m * 4, cudaMemcpyDeviceToHost));
         if (offsets && t.k1 > t.k0)
             SB_CUDA(cudaMemcpy(offsets + t.k0, doff + 2, (size_t)(t.k1 - t.k0) * 4, cudaMemcpyDeviceToHost));
-        lens[k] = p.y_total;
-        out_at += p.y_total; in_at += chunk_lens[k];
+        lens[k] = m;
+        out_at += m; in_at += chunk_lens[k];
         prosody_stream_advance(ps, t, last);
     }
 }
@@ -1428,7 +1482,7 @@ int32_t sb200_debug_prosody_contour_stream(int32_t device, const float* x, const
         SB_CUDA(cudaSetDevice(device));
         std::unique_ptr<ProsodyStream> ps(create_prosody_stream_contour(nullptr, device, rate, total, e, ratios, n_ids,
                                                                         tempo));
-        debug_push_stream(*ps, whole, counts, x, chunk_lens, n_chunks, y, cap, lens, offsets, offsets_cap);
+        debug_push_stream(*ps, whole, counts, 5, x, chunk_lens, n_chunks, y, cap, lens, offsets, offsets_cap);
     });
 }
 
@@ -1449,7 +1503,58 @@ int32_t sb200_debug_prosody_stream(int32_t device, const float* x, const int64_t
         const ProsodyShape whole = prosody_shape(rate, total, pitch, tempo);
         SB_CUDA(cudaSetDevice(device));
         std::unique_ptr<ProsodyStream> ps(create_prosody_stream(nullptr, device, rate, pitch, tempo));
-        debug_push_stream(*ps, whole, counts, x, chunk_lens, n_chunks, y, cap, lens, offsets, offsets_cap);
+        debug_push_stream(*ps, whole, counts, 5, x, chunk_lens, n_chunks, y, cap, lens, offsets, offsets_cap);
+    });
+}
+
+namespace {
+// A fresh formant stream on the host (no device memory) for the debug hooks, and the whole signal's shape of n inputs.
+ProsodyShape debug_formant_stream(ProsodyStream& ps, int32_t rate, long long n, float pitch, float tempo,
+                                  const int64_t* ends, const float* ratios, size_t n_ids, float formant) {
+    const long long* e = reinterpret_cast<const long long*>(ends);
+    prosody_stream_init_formant(ps, rate, n, e, n_ids ? ratios : nullptr, n_ids, pitch, tempo, formant);
+    if (!n_ids) return prosody_shape(rate, n, pitch, tempo);
+    std::vector<ContourPiece> pc;
+    return prosody_contour_plan(rate, n, e, ratios, n_ids, NAN, tempo, pc, nullptr);
+}
+}  // namespace
+
+int32_t sb200_debug_formant_stream_plan(int32_t rate, float pitch, float tempo, const int64_t* ends, const float* ratios,
+                                        size_t n_ids, float formant, const int64_t* chunk_lens, size_t n_chunks,
+                                        int64_t* emitted, sb200_error* err) {
+    return guarded(err, [&] {
+        if ((n_chunks > 0 && (!chunk_lens || !emitted)) || (n_ids > 0 && (!ends || !ratios)))
+            throw Error(19, "debug formant stream plan: bad arguments");
+        long long total = 0;
+        for (size_t k = 0; k < n_chunks; k++) total += std::max<long long>(chunk_lens[k], 0);
+        ProsodyStream ps;
+        debug_formant_stream(ps, rate, total, pitch, tempo, ends, ratios, n_ids, formant);
+        const std::vector<long long> e =
+            formant_stream_counts(ps, reinterpret_cast<const long long*>(chunk_lens), n_chunks);
+        std::copy(e.begin(), e.end(), emitted);
+    });
+}
+
+int32_t sb200_debug_formant_stream(int32_t device, const float* x, const int64_t* chunk_lens, size_t n_chunks,
+                                   int32_t rate, float pitch, float tempo, const int64_t* ends, const float* ratios,
+                                   size_t n_ids, float formant, float* y, size_t cap, int64_t* lens, sb200_error* err) {
+    return guarded(err, [&] {
+        if (!x || !chunk_lens || !y || !lens || n_chunks == 0 || (n_ids > 0 && (!ends || !ratios)))
+            throw Error(19, "debug formant stream: bad arguments");
+        long long total = 0;
+        for (size_t k = 0; k < n_chunks; k++) {
+            if (chunk_lens[k] < 0) throw Error(19, "debug formant stream: negative chunk length");
+            total += chunk_lens[k];
+        }
+        ProsodyStream host;
+        const ProsodyShape whole = debug_formant_stream(host, rate, total, pitch, tempo, ends, ratios, n_ids, formant);
+        const std::vector<long long> counts =
+            formant_stream_counts(host, reinterpret_cast<const long long*>(chunk_lens), n_chunks);
+        SB_CUDA(cudaSetDevice(device));
+        std::unique_ptr<ProsodyStream> ps(create_prosody_stream_formant(
+            nullptr, device, rate, n_ids ? total : -1, reinterpret_cast<const long long*>(ends),
+            n_ids ? ratios : nullptr, n_ids, pitch, tempo, formant));
+        debug_push_stream(*ps, whole, counts, 1, x, chunk_lens, n_chunks, y, cap, lens, nullptr, 0);
     });
 }
 

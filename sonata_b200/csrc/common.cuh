@@ -327,15 +327,32 @@ __host__ __device__ inline long long contour_analysis(const ContourPiece& q, dou
 // outputs hold the frame's centre.  Q0 = rate / 250: the lifter's cutoff at p_m = 1.
 constexpr int FM_N = 1024, FM_H = 256;   // frame and hop
 constexpr int FM_HOPS = 32;              // hops of output per CTA (each also analyses the 3 frames before them)
+constexpr int FM_STREAM_HOPS = 8;        // the same in a stream's chunk pass, whose window holds a few dozen hops
+// A stream's chunk pass computes hops [h0, h1) of an utterance from a window of it: in[off ..) holds its samples from
+// x0 on (x0 <= max(0, (h0 - 3) H)), the hops leave at out[y_off ..), and cp, when set, is the stream's own piece table.
+// The whole utterance is x0 = h0 = 0, h1 = ceil(n / H) and y_off = off.  A sample's bits do not depend on the window.
 struct FormantSeg {
     long long off, n;
     double p, phi;
     int Q0, c_off, c_n;
+    long long x0, h0, h1, y_off;
+    const ContourPiece* cp;
 };
-// One launch over the segments: blockIdx.y = segment, blockIdx.x = its run of FM_HOPS hops (max_runs: the most runs of
+// One launch over the segments: blockIdx.y = segment, blockIdx.x = its run of `run` hops (max_runs: the most runs of
 // any segment).  `in` and `out` are different buffers.
 void launch_formant(const float* in, const FormantSeg* segs, int nseg, long long max_runs, const ContourPiece* pieces,
-                    float* out, cudaStream_t st);
+                    float* out, cudaStream_t st, int run = FM_HOPS);
+// What a stream's chunk pass stages before the formant launch (formant.cu): the segment's window is the h carried
+// samples of hist, then n_new new ones, read from `direct` (the pitch stage's output) or, when that is null, from the
+// chunk's samples after the post-path (fsegs / posts entry `chunk`).  The keep window samples from `from` on go to next.
+struct FormantCarry {
+    int chunk, h, keep;
+    long long from, n_new;
+    const float* direct;
+    const float* hist; float* next;
+};
+void launch_formant_stage(const float* src, const FrameSeg* fsegs, const PcmPost* posts, int hop, const FormantSeg* segs,
+                          const FormantCarry* cs, int nseg, long long max_in, float* win, cudaStream_t st);
 // What a stream's chunk pass stages before the prosody launches and carries after them (prosody.cu): the chunk's
 // samples after the post-path (fsegs / posts entry `chunk`) follow h_in history inputs in the segment's input window,
 // h_s stretched samples of history start its stretched window and the deltas of frames d0, d0 + 1 start its offsets.

@@ -784,20 +784,27 @@ struct ChunkBufs {
     void* pcm; unsigned* max;
     void* out_h;
     // warped chunks (plan `pp`): the prosody buffers, the output after the waveforms in `wav`, and the resample
-    // launch's input table (the prosody output for a warped chunk, the post-path's chunk for the others)
+    // launch's input table (the prosody output for a warped chunk, the post-path's chunk for the others); chunks with
+    // a formant stage (plan `fp`): its tables and windows, its output after the prosody output in `wav`, and the
+    // resample launch reads that output instead
     ProsodyBufs pr;
+    Staged<FormantSeg> fsegs; Staged<FormantCarry> fcarry; float* fwin = nullptr;
     Staged<FrameSeg> rin; Staged<PcmPost> rpost;
     void carve(Arena& dev, Arena& pin, const Voice& v, const FrameLayout& l, const ChunkPass& p, const ResamplePlan& rp,
-               const ProsodyPlan& pp, size_t total) {
+               const ProsodyPlan& pp, const FormantPlan& fp, size_t total) {
         const bool i16_out = p.format != PCM_F32;
         const size_t n = l.fsegs.size();
         spk.carve(dev, pin, v, l);
         y.carve(dev, pin, l);
         src.carve(dev, pin, n);
         s = dev.get<float>((size_t)l.RY * v.a.inter);
-        wav = dev.get<float>((size_t)l.total_samples + (size_t)pp.y_total + 4);
+        wav = dev.get<float>((size_t)l.total_samples + (size_t)pp.y_total + (size_t)fp.total + 4);
         pr.carve(dev, pin, pp, false);
-        if (!pp.segs.empty()) { rin.carve(dev, pin, n); rpost.carve(dev, pin, n); }
+        if (!fp.segs.empty()) {
+            fsegs.carve(dev, pin, fp.segs.size()); fcarry.carve(dev, pin, fp.segs.size());
+            fwin = dev.get<float>((size_t)fp.in_total + 4);
+        }
+        if (!pp.segs.empty() || !fp.segs.empty()) { rin.carve(dev, pin, n); rpost.carve(dev, pin, n); }
         dec.carve(dev, v, l.RY, p.debug);
         if (p.resample || i16_out) post.carve(dev, pin, n);
         rt.carve(dev, pin, rp.segs.size());
@@ -1571,7 +1578,7 @@ static void fill_fade(PcmPost& p, int fade, long long len) {
 // context's page-locked staging, and only then do the resamplers and prosody streams advance.
 void decode_chunks(Voice* v, const ChunkPass& p, ChunkResult& out) {
     out.f32.clear(); out.i16.clear(); out.g711.clear(); out.captures.clear();
-    out.ms = out.stretch_ms = out.pitch_ms = 0.f;
+    out.ms = out.stretch_ms = out.pitch_ms = out.formant_ms = 0.f;
     const size_t n = p.chunks.size();
     if (n == 0) return;
     if (p.format < PCM_F32 || p.format > PCM_ALAW)
@@ -1614,10 +1621,13 @@ void decode_chunks(Voice* v, const ChunkPass& p, ChunkResult& out) {
             fail(k, "last flag " + std::to_string(c.last) + " is neither 0 nor 1", "");
     }
     // samples of each chunk after its trims, what its prosody stream emits for them, and the resample launch
-    std::vector<long long> n_in(n), n_res(n);     // n_res: what the resample launch takes (a warped chunk's output)
+    // n_res: what the resample launch takes (a warped chunk's output, or its formant stage's)
+    std::vector<long long> n_in(n), n_res(n);
     std::vector<ProsodyStep> steps(n);
-    std::vector<int> warped;
+    std::vector<FormantStep> fsteps(n);
+    std::vector<int> warped, formed, warp_of(n, -1);     // warp_of[k]: chunk k's segment of pp
     ProsodyPlan pp;
+    FormantPlan fp;
     ResamplePlan rp;
     for (size_t k = 0; k < n; k++) {
         const ChunkSpec& c = p.chunks[k];
@@ -1625,9 +1635,18 @@ void decode_chunks(Voice* v, const ChunkPass& p, ChunkResult& out) {
         n_res[k] = n_in[k];
         if (c.ps) {
             steps[k] = prosody_stream_step(*c.ps, n_in[k], c.last != 0);
-            pp.add_stream(*c.ps, steps[k]);
-            warped.push_back((int)k);
+            if (prosody_stream_warps(*c.ps)) {
+                pp.add_stream(*c.ps, steps[k]);
+                warp_of[k] = (int)warped.size();
+                warped.push_back((int)k);
+            }
             n_res[k] = steps[k].j1 - steps[k].j0;
+            if (c.ps->fm) {
+                fsteps[k] = formant_stream_step(*c.ps, steps[k].next.emitted, c.last != 0);
+                fp.add_stream(*c.ps, fsteps[k]);
+                formed.push_back((int)k);
+                n_res[k] = fsteps[k].e1 - fsteps[k].e0;
+            }
         }
         if (p.resample) rp.add(c.rs ? &c.rs->f : nullptr, n_res[k], c.rs, c.last != 0);
     }
@@ -1639,7 +1658,7 @@ void decode_chunks(Voice* v, const ChunkPass& p, ChunkResult& out) {
     lay_out_frames(l, len, hop, {});
     const size_t total = p.resample ? (size_t)rp.total : (size_t)l.total_samples;
     ChunkBufs b;
-    plan(C.dev_frame, C.pin, [&](Arena& dev, Arena& pin) { b.carve(dev, pin, *v, l, p, rp, pp, total); });
+    plan(C.dev_frame, C.pin, [&](Arena& dev, Arena& pin) { b.carve(dev, pin, *v, l, p, rp, pp, fp, total); });
     cudaStream_t st = C.stream;
     std::vector<Region> regions;
     Runner R(*v, C, regions, b.spk.cond);
@@ -1668,10 +1687,21 @@ void decode_chunks(Voice* v, const ChunkPass& p, ChunkResult& out) {
         b.post.upload(st);
     }
     // warped chunks: prosody on the post-path's samples, then the resample launch reads its output (n samples at
-    // `off` as a segment of ceil(n / hop) frames less a trim, with no post-path of its own)
+    // `off` as a segment of ceil(n / hop) frames less a trim, with no post-path of its own); chunks with a formant
+    // stage: the stage on that output (or on the post-path's samples), and the resample launch reads the stage's output
     const FrameSeg* rs_in = b.y.fsegs.d; const PcmPost* rs_post = b.post.d;
+    float* py = b.wav + l.total_samples;
+    const auto resample_from = [&](int k, long long off, long long m) {
+        const long long frames = (m + hop - 1) / hop;
+        b.rin.h[k] = FrameSeg{0, (int)frames, 0, 0, off};
+        b.rpost.h[k] = PcmPost();
+        b.rpost.h[k].trim_hi = frames * hop - m;
+    };
+    if (!warped.empty() || !formed.empty()) {
+        std::copy(l.fsegs.begin(), l.fsegs.end(), b.rin.h);
+        std::copy(b.post.h, b.post.h + n, b.rpost.h);
+    }
     if (!warped.empty()) {
-        float* py = b.wav + l.total_samples;
         b.pr.upload(pp, st);
         for (size_t q = 0; q < warped.size(); q++)
             b.pr.carry.h[q] = prosody_carry(*p.chunks[warped[q]].ps, steps[warped[q]], warped[q]);
@@ -1687,15 +1717,29 @@ void decode_chunks(Voice* v, const ChunkPass& p, ChunkResult& out) {
             R.count(pp.pitch_flops, pp.pitch_bytes);
             R.end();
         }
-        std::copy(l.fsegs.begin(), l.fsegs.end(), b.rin.h);
-        std::copy(b.post.h, b.post.h + n, b.rpost.h);
         for (size_t q = 0; q < warped.size(); q++) {
             const ProsodySeg& g = pp.segs[q];
-            const long long m = g.j1 - g.j0, frames = (m + hop - 1) / hop;
-            b.rin.h[warped[q]] = FrameSeg{0, (int)frames, 0, 0, l.total_samples + g.y_off};
-            b.rpost.h[warped[q]] = PcmPost();
-            b.rpost.h[warped[q]].trim_hi = frames * hop - m;
+            resample_from(warped[q], l.total_samples + g.y_off, g.j1 - g.j0);
         }
+    }
+    if (!formed.empty()) {
+        float* fy = py + pp.y_total;
+        std::copy(fp.segs.begin(), fp.segs.end(), b.fsegs.h);
+        b.fsegs.upload(st);
+        for (size_t q = 0; q < formed.size(); q++) {
+            const int k = formed[q], w = warp_of[k];
+            b.fcarry.h[q] = formant_carry(*p.chunks[k].ps, fsteps[k], k, w < 0 ? nullptr : py + pp.segs[w].y_off);
+        }
+        b.fcarry.upload(st);
+        R.begin("formant");
+        launch_formant_stream(fp, b.fsegs.d, b.fcarry.d, b.wav, b.y.fsegs.d, b.post.d, hop, b.fwin, fy, st);
+        R.count(fp.flops, fp.bytes, fp.max_runs ? 2 : 1);
+        R.end();
+        for (size_t q = 0; q < formed.size(); q++)
+            resample_from(formed[q], l.total_samples + pp.y_total + fp.segs[q].y_off,
+                          fsteps[formed[q]].e1 - fsteps[formed[q]].e0);
+    }
+    if (!warped.empty() || !formed.empty()) {
         b.rin.upload(st);
         b.rpost.upload(st);
         rs_in = b.rin.d; rs_post = b.rpost.d;
@@ -1725,14 +1769,18 @@ void decode_chunks(Voice* v, const ChunkPass& p, ChunkResult& out) {
         r->ended = p.chunks[k].last != 0;
     }
     for (Region& g : regions) {
-        if (g.name != "stretch" && g.name != "pitch") continue;
+        if (g.name != "stretch" && g.name != "pitch" && g.name != "formant") continue;
         cudaEventElapsedTime(&g.ms, g.e0, g.e1);
-        (g.name == "stretch" ? out.stretch_ms : out.pitch_ms) = g.ms;
+        (g.name == "stretch" ? out.stretch_ms : g.name == "pitch" ? out.pitch_ms : out.formant_ms) = g.ms;
     }
-    for (int k : warped) {
-        ProsodyStream& w = *p.chunks[k].ps;
-        prosody_stream_advance(w, steps[k], p.chunks[k].last != 0);
-        w.last_ms[0] = out.stretch_ms; w.last_ms[1] = out.pitch_ms;
+    for (size_t k = 0; k < n; k++) {
+        ProsodyStream* w = p.chunks[k].ps;
+        if (!w) continue;
+        if (w->fm) formant_stream_advance(*w, fsteps[k]);
+        prosody_stream_advance(*w, steps[k], p.chunks[k].last != 0);
+        const bool warps = prosody_stream_warps(*w);
+        w->last_ms[0] = warps ? out.stretch_ms : 0.f; w->last_ms[1] = warps ? out.pitch_ms : 0.f;
+        w->last_fm_ms = w->fm ? out.formant_ms : 0.f;
     }
     if (p.format == PCM_I16) out.i16.resize(n); else if (b.pcm) out.g711.resize(n); else out.f32.resize(n);
     for (size_t k = 0; k < n; k++) {

@@ -5,6 +5,7 @@
 #pragma once
 #include "common.cuh"
 #include <atomic>
+#include <cmath>
 #include <map>
 #include <memory>
 #include <mutex>
@@ -191,15 +192,21 @@ bool formant_asks(long long n, float phi, double p, const ContourPiece* pc, int 
 // The formant launch's segments, read from and written to the same offsets of two buffers laid out alike (the output
 // of the stage before it, `total` samples), the copies of the utterances that do not ask ((offset, samples), adjacent
 // ones merged), the CTA runs it is sized by and what the profile counts.
+// A stream pass's plan instead holds one segment per stream: its window at in[off ..) (in_total samples in all, the
+// largest max_in) and the hops it emits at out[y_off ..) (total samples), in runs of FM_STREAM_HOPS.
+struct FormantStep;
 struct FormantPlan {
     std::vector<FormantSeg> segs;
     std::vector<std::pair<long long, long long>> copies;
     long long total = 0, max_runs = 0;
+    long long in_total = 0, max_in = 0;
     double flops = 0, bytes = 0;
     // Appends an utterance of n samples at offset `off` at the voice's `rate`, with its ratios (see FormantSeg).
     void add(int rate, long long off, long long n, float phi, double p, int c_off, int c_n);
     // Appends the copy of an utterance that does not ask.
     void copy(long long off, long long n);
+    // Appends stream ps's window for its chunk pass step t.
+    void add_stream(const ProsodyStream& ps, const FormantStep& t);
 };
 
 // One stream's pitch and tempo state (prosody.cu): the shape of its ratios, its counts (inputs consumed, frames whose
@@ -227,8 +234,34 @@ struct ProsodyStream {
     ProsodyCounts c;
     bool ended = false;
     float last_ms[2] = {0.f, 0.f};        // the "stretch" and "pitch" device time of the last pass it was in
+    // The formant stage (formant.cu): phi (NaN: none), whether the stage runs (formant_asks), its inputs taken (the
+    // pitch stage's outputs, or the chunks' samples without pitch and tempo) and outputs emitted, the h carried inputs
+    // [fm_in - fm_h, fm_in) in fm_hist[cur] (FM_CARRY floats each, after the prosody buffers) and its last region time.
+    float formant = NAN;
+    bool fm = false;
+    long long fm_in = 0, fm_out = 0;
+    int fm_h = 0;
+    float* fm_hist[2] = {nullptr, nullptr};
+    float last_fm_ms = 0.f;
     ~ProsodyStream();
 };
+// Whether stream ps runs the stretch or pitch stage (a formant-only stream runs neither).
+inline bool prosody_stream_warps(const ProsodyStream& ps) { return ps.sh.stretch || ps.sh.pitch; }
+// The most inputs a formant stream carries between passes: fewer than N, and the 3 H that recompute the frames before
+// its next hop.
+constexpr int FM_CARRY = FM_N + 3 * FM_H;
+// What one chunk pass does to a stream's formant stage (include/sonata_b200.h, sb200_prosody_stream_create_formant): its
+// inputs become g1, it emits hops [h0, h1) (outputs [e0, e1)) and the next pass carries its inputs from `from` on.
+struct FormantStep { long long g1, h0, h1, e0, e1, from; };
+FormantStep formant_stream_step(const ProsodyStream& ps, long long g1, bool last);
+// The stage / carry entry of chunk `chunk` for step t of ps; direct: where its new inputs are (the pitch stage's output),
+// or null for the chunk's samples after the post-path.
+FormantCarry formant_carry(const ProsodyStream& ps, const FormantStep& t, int chunk, const float* direct);
+// The launches of a stream pass's "formant" region: the staging (and carry), then the stage over every window.
+void launch_formant_stream(const FormantPlan& p, const FormantSeg* segs, const FormantCarry* cs, const float* src,
+                           const FrameSeg* fsegs, const PcmPost* posts, int hop, float* win, float* y, cudaStream_t st);
+// After the pass has synchronised: the stage's counts become t's (prosody_stream_advance swaps the buffers).
+void formant_stream_advance(ProsodyStream& ps, const FormantStep& t);
 // What one chunk pass does to a stream: n_in new inputs, the frames [k0, k1), stretched samples [m0, m1) and outputs
 // [j0, j1) it computes, the first absolute positions of its input and stretched windows (x0, s0), where the tails the
 // next pass reads start (in_from, s_from), and the counts after it.  Computed on the host from the counts alone.
@@ -237,14 +270,25 @@ struct ProsodyStep {
     int k0, k1;
     ProsodyCounts next;
 };
-// Checks the ratios (one must ask for something) and sizes the history; no device memory.
-void prosody_stream_init(ProsodyStream& ps, int rate, float pitch, float tempo);
+// Checks the ratios (one must ask for something unless allow_none) and sizes the history; no device memory.
+void prosody_stream_init(ProsodyStream& ps, int rate, float pitch, float tempo, bool allow_none = false);
 ProsodyStream* create_prosody_stream(Voice* v, int device, int rate, float pitch, float tempo);
 // The same for a pitch contour of n_ids ids over n inputs (ends, ratios: as for prosody_contour_plan) and a tempo:
 // checks them as check_pitch_contour and check_prosody do (a contour and tempo that ask for nothing are refused), plans
 // the pieces and the bounds, and sizes the history by the smallest stretch factor and the widest pitch kernel.
 void prosody_stream_init_contour(ProsodyStream& ps, int rate, long long n, const long long* ends, const float* ratios,
-                                 size_t n_ids, float tempo);
+                                 size_t n_ids, float tempo, bool allow_none = false);
+// A stream with a formant ratio phi (NaN: none) on top of a pitch ratio and a tempo (ratios null) or of a contour of
+// n_ids ids over n inputs and a tempo: the checks of the two above, which here accept ratios that ask for nothing when
+// phi asks, and phi's own (finite, in [0.5, 2]); a pitch ratio beside a contour, and a stream that asks for nothing at
+// all, are refused.
+void prosody_stream_init_formant(ProsodyStream& ps, int rate, long long n, const long long* ends, const float* ratios,
+                                 size_t n_ids, float pitch, float tempo, float phi);
+ProsodyStream* create_prosody_stream_formant(Voice* v, int device, int rate, long long n, const long long* ends,
+                                             const float* ratios, size_t n_ids, float pitch, float tempo, float phi);
+// Outputs per chunk of fresh stream ps (no device memory) fed chunk_lens[0 .. n), the last one ending it: what its
+// formant stage emits when it runs, else what its pitch stage emits.
+std::vector<long long> formant_stream_counts(ProsodyStream& ps, const long long* chunk_lens, size_t n);
 ProsodyStream* create_prosody_stream_contour(Voice* v, int device, int rate, long long n, const long long* ends,
                                              const float* ratios, size_t n_ids, float tempo);
 // The emission rule (include/sonata_b200.h, sb200_decode_chunks_warped).  Throws OPERATION_ERROR only on an internal
@@ -574,6 +618,7 @@ struct ChunkResult {
     std::vector<std::vector<uint8_t>> g711;   // formats 2 and 3
     float ms = 0;                             // the pass's device time
     float stretch_ms = 0, pitch_ms = 0;       // its "stretch" and "pitch" regions (0: none ran)
+    float formant_ms = 0;                     // its "formant" region (0: none ran)
     std::vector<ChunkCapture> captures;       // ChunkPass::debug only
 };
 void decode_chunks(Voice* v, const ChunkPass& p, ChunkResult& out);

@@ -52,6 +52,7 @@ void FormantPlan::add(int rate, long long off, long long n, float phi, double p,
     g.off = off; g.n = n;
     g.p = p; g.phi = (double)phi; g.Q0 = rate / 250; g.c_off = c_off; g.c_n = c_n;
     const long long hops = (n + FM_H - 1) / FM_H, runs = (hops + FM_HOPS - 1) / FM_HOPS;
+    g.h1 = hops; g.y_off = off;
     max_runs = std::max(max_runs, runs);
     // every CTA analyses its hops and the 3 frames before them: 4 FFTs of N points and about 40 operations per bin
     const double frames = (double)hops + 3.0 * (double)runs;
@@ -64,6 +65,57 @@ void FormantPlan::copy(long long off, long long n) {
     if (!copies.empty() && copies.back().first + copies.back().second == off) copies.back().second += n;
     else copies.emplace_back(off, n);
     bytes += 8.0 * (double)n;
+}
+
+// ------------------------------------------------------------------ host: streams
+// Hop h needs frames h - 3 .. h, so inputs up to (h + 4) H: before its last chunk a stream emits the hops whose 4 frames
+// lie inside its G inputs, and those frames neither reach the clamp at n2 - 1 nor read past G, so they are the whole
+// signal's.  The last chunk emits the rest up to n2 = G.  The next pass recomputes the 3 frames before its first hop,
+// so it carries the inputs from (h1 - 3) H on.
+FormantStep formant_stream_step(const ProsodyStream& ps, long long g1, bool last) {
+    FormantStep t{};
+    t.g1 = g1; t.e0 = ps.fm_out; t.h0 = ps.fm_out / FM_H;
+    if (last) {
+        t.h1 = (g1 + FM_H - 1) / FM_H; t.e1 = g1; t.from = g1;
+    } else {
+        t.h1 = std::max(0ll, g1 / FM_H - (FM_N / FM_H - 1)); t.e1 = t.h1 * FM_H;
+        t.from = std::max(0ll, (t.h1 - 3) * FM_H);
+    }
+    if (g1 < ps.fm_in || t.h1 < t.h0 || t.e1 < t.e0 || ps.fm_out % FM_H != 0)
+        throw Error(19, "internal: a formant stream would go back");
+    if (g1 - t.from > FM_CARRY || ps.fm_in - ps.fm_h > std::max(0ll, (t.h0 - 3) * FM_H))
+        throw Error(19, "internal: a formant stream's carry exceeds its buffers");
+    return t;
+}
+
+void FormantPlan::add_stream(const ProsodyStream& ps, const FormantStep& t) {
+    FormantSeg g{};
+    const long long nx = ps.fm_h + (t.g1 - ps.fm_in);
+    g.off = in_total; in_total += nx; max_in = std::max(max_in, nx);
+    g.n = t.g1; g.x0 = ps.fm_in - ps.fm_h; g.h0 = t.h0; g.h1 = t.h1;
+    g.y_off = total; total += t.e1 - t.e0;
+    g.p = ps.sh.p; g.phi = (double)ps.formant; g.Q0 = ps.rate / 250;
+    if (!ps.pieces.empty()) { g.c_n = (int)ps.pieces.size() - 1; g.cp = ps.pieces_d; }
+    const long long hops = t.h1 - t.h0, runs = (hops + FM_STREAM_HOPS - 1) / FM_STREAM_HOPS;
+    max_runs = std::max(max_runs, runs);
+    const double frames = (double)hops + 3.0 * (double)runs;
+    flops += frames * (4.0 * 5.0 * FM_N * 10.0 + 40.0 * FM_N);
+    bytes += 4.0 * (2.0 * (double)nx + (double)(t.g1 - t.from)) + 4.0 * (frames * FM_H + 3.0 * FM_H * (double)runs) +
+             4.0 * (double)(t.e1 - t.e0);
+    segs.push_back(g);
+}
+
+FormantCarry formant_carry(const ProsodyStream& ps, const FormantStep& t, int chunk, const float* direct) {
+    FormantCarry c{};
+    c.chunk = chunk; c.h = ps.fm_h; c.n_new = t.g1 - ps.fm_in;
+    c.from = t.from - (ps.fm_in - ps.fm_h); c.keep = (int)(t.g1 - t.from);
+    c.direct = direct;
+    c.hist = ps.fm_hist[ps.cur]; c.next = ps.fm_hist[1 - ps.cur];
+    return c;
+}
+
+void formant_stream_advance(ProsodyStream& ps, const FormantStep& t) {
+    ps.fm_in = t.g1; ps.fm_out = t.e1; ps.fm_h = (int)(t.g1 - t.from);
 }
 
 // ------------------------------------------------------------------ the kernel
@@ -106,7 +158,7 @@ __device__ void fm_fft(double2* x, const double2* tw, bool inverse) {
 
 __global__ void __launch_bounds__(FM_THREADS)
 formant_kernel(const float* __restrict__ in, const FormantSeg* __restrict__ segs, const ContourPiece* __restrict__ pieces,
-               float* __restrict__ out) {
+               float* __restrict__ out, int run) {
     extern __shared__ __align__(16) unsigned char fm_raw[];
     FmSmem& sm = *reinterpret_cast<FmSmem*>(fm_raw);
     const int t = threadIdx.x;
@@ -118,14 +170,14 @@ formant_kernel(const float* __restrict__ in, const FormantSeg* __restrict__ segs
     }
     pdl_trigger(); pdl_wait();
     const FormantSeg g = segs[blockIdx.y];
-    const long long n = g.n, hops = (n + FM_H - 1) / FM_H;
-    const long long h0 = (long long)blockIdx.x * FM_HOPS;
-    if (h0 >= hops) return;
-    const long long h1 = min(h0 + FM_HOPS, hops);
+    const long long n = g.n;
+    const long long h0 = g.h0 + (long long)blockIdx.x * run;
+    if (h0 >= g.h1) return;
+    const long long h1 = min(h0 + run, g.h1);
     const long long j_lo = h0 * FM_H, j_hi = min(h1 * FM_H, n);
-    const float* y = in + g.off;
-    float* o = out + g.off;
-    const ContourPiece* pc = g.c_n ? pieces + g.c_off : nullptr;
+    const float* y = in + g.off - g.x0;              // y[j]: sample j, for j >= x0
+    float* o = out + g.y_off - g.h0 * FM_H;          // o[j]: where sample j leaves
+    const ContourPiece* pc = g.c_n ? (g.cp ? g.cp : pieces + g.c_off) : nullptr;
     const double clamp = 1.2 * 2.30258509299404568402;      // 24 dB as a natural-log amplitude
     __syncthreads();
     for (long long m = h0 - 3; m < h1; m++) {
@@ -226,7 +278,7 @@ formant_kernel(const float* __restrict__ in, const FormantSeg* __restrict__ segs
 }
 
 void launch_formant(const float* in, const FormantSeg* segs, int nseg, long long max_runs, const ContourPiece* pieces,
-                    float* out, cudaStream_t st) {
+                    float* out, cudaStream_t st, int run) {
     if (nseg <= 0 || max_runs <= 0) return;
     if (max_runs > INT_MAX) throw_launch_error("formant: an utterance too long for the grid");
     static PerDeviceOnce once;
@@ -234,8 +286,41 @@ void launch_formant(const float* in, const FormantSeg* segs, int nseg, long long
         cudaFuncSetAttribute(formant_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(FmSmem));
     });
     launch_pdl(formant_kernel, dim3((unsigned)max_runs, nseg), dim3(FM_THREADS), sizeof(FmSmem), st, in, segs, pieces,
-               out);
+               out, run);
     g_launch_count++;
+}
+
+// ------------------------------------------------------------------ a stream's chunk pass: staging and carry
+// Writes each segment's window (the carried samples, then the new ones) and, from the same values, the samples the
+// stream's next pass carries into its other buffer.
+__global__ void formant_stage_kernel(const float* __restrict__ src, const FrameSeg* __restrict__ fsegs,
+                                     const PcmPost* __restrict__ posts, int hop, const FormantSeg* __restrict__ segs,
+                                     const FormantCarry* __restrict__ cs, float* __restrict__ win) {
+    pdl_trigger(); pdl_wait();
+    const FormantCarry c = cs[blockIdx.y];
+    float* w = win + segs[blockIdx.y].off;
+    const PcmSeg x = c.direct ? PcmSeg{} : pcm_seg(src, fsegs[c.chunk], posts + c.chunk, hop);
+    const long long i0 = (long long)blockIdx.x * blockDim.x + threadIdx.x, step = (long long)gridDim.x * blockDim.x;
+    for (long long i = i0; i < c.h + c.n_new; i += step) {
+        const float v = i < c.h ? c.hist[i] : c.direct ? c.direct[i - c.h] : pcm_value(x, i - c.h);
+        w[i] = v;
+        if (i >= c.from) c.next[i - c.from] = v;
+    }
+}
+
+void launch_formant_stage(const float* src, const FrameSeg* fsegs, const PcmPost* posts, int hop, const FormantSeg* segs,
+                          const FormantCarry* cs, int nseg, long long max_in, float* win, cudaStream_t st) {
+    if (nseg <= 0) return;
+    const unsigned grid = (unsigned)std::min<long long>(std::max<long long>((max_in + 1023) / 1024, 1), 4096);
+    launch_pdl(formant_stage_kernel, dim3(grid, nseg), dim3(256), 0, st, src, fsegs, posts, hop, segs, cs, win);
+    g_launch_count++;
+}
+
+void launch_formant_stream(const FormantPlan& p, const FormantSeg* segs, const FormantCarry* cs, const float* src,
+                           const FrameSeg* fsegs, const PcmPost* posts, int hop, float* win, float* y, cudaStream_t st) {
+    const int n = (int)p.segs.size();
+    launch_formant_stage(src, fsegs, posts, hop, segs, cs, n, p.max_in, win, st);
+    launch_formant(win, segs, n, p.max_runs, nullptr, y, st, FM_STREAM_HOPS);
 }
 
 }  // namespace sb200

@@ -475,9 +475,9 @@ namespace {
 double pitch_radius(double p) { return 16.0 / (p > 1.0 ? 1.0 / p : 1.0); }     // W, as the pitch kernel computes it
 }  // namespace
 
-void prosody_stream_init(ProsodyStream& ps, int rate, float pitch, float tempo) {
+void prosody_stream_init(ProsodyStream& ps, int rate, float pitch, float tempo, bool allow_none) {
     check_prosody(&pitch, &tempo, 1);
-    if (!prosody_asked(pitch) && !prosody_asked(tempo))
+    if (!allow_none && !prosody_asked(pitch) && !prosody_asked(tempo))
         throw Error(19, "a prosody stream needs a pitch or a tempo ratio other than 1 (NaN or 1: none)");
     ps.sh = prosody_shape(rate, 0, pitch, tempo);
     ps.rate = rate; ps.pitch = pitch; ps.tempo = tempo;
@@ -491,18 +491,18 @@ void prosody_stream_init(ProsodyStream& ps, int rate, float pitch, float tempo) 
 }
 
 void prosody_stream_init_contour(ProsodyStream& ps, int rate, long long n, const long long* ends, const float* ratios,
-                                 size_t n_ids, float tempo) {
+                                 size_t n_ids, float tempo, bool allow_none) {
     const size_t offs[2] = {0, n_ids};
     check_pitch_contour(ratios, offs, 1, nullptr);
     check_prosody(nullptr, &tempo, 1);
     std::vector<ContourPiece> pc;
     std::vector<long long> bounds(n_ids);
     const ProsodyShape sh = prosody_contour_plan(rate, n, ends, ratios, n_ids, NAN, tempo, pc, bounds.data());
-    if (!sh.stretch && !sh.pitch)
+    if (!allow_none && !sh.stretch && !sh.pitch)
         throw Error(19, "a prosody stream's pitch contour and tempo ask for nothing (every ratio NaN or 1, and no tempo)");
     if (pc.empty()) {
         // one piece: the ratio stream it equals
-        prosody_stream_init(ps, rate, sh.pitch ? (float)sh.p : NAN, tempo);
+        prosody_stream_init(ps, rate, sh.pitch ? (float)sh.p : NAN, tempo, allow_none);
     } else {
         ps.sh = sh;
         ps.rate = rate; ps.pitch = NAN; ps.tempo = tempo;
@@ -519,13 +519,35 @@ void prosody_stream_init_contour(ProsodyStream& ps, int rate, long long n, const
     ps.bounds = std::move(bounds);
 }
 
+void prosody_stream_init_formant(ProsodyStream& ps, int rate, long long n, const long long* ends, const float* ratios,
+                                 size_t n_ids, float pitch, float tempo, float phi) {
+    if (!std::isnan(phi) && !(std::isfinite(phi) && phi >= 0.5f && phi <= 2.f))
+        throw Error(19, "formant ratio " + std::to_string(phi) + " is not a finite value in [0.5, 2] (NaN: none)");
+    if (ratios) {
+        check_prosody(&pitch, nullptr, 1);
+        if (prosody_asked(pitch)) throw Error(19, "a pitch contour and a pitch ratio together (give one or the other)");
+        prosody_stream_init_contour(ps, rate, n, ends, ratios, n_ids, tempo, true);
+    } else {
+        prosody_stream_init(ps, rate, pitch, tempo, true);
+    }
+    ps.formant = phi;
+    // a stream of one ratio runs the stage on every frame or on none, whatever its length; a contour's plan knows n2
+    const int c_n = ps.pieces.empty() ? 0 : (int)ps.pieces.size() - 1;
+    ps.fm = formant_asks(c_n ? ps.sh.n2 : 1, phi, ps.sh.p, ps.pieces.data(), c_n);
+    if (!ps.fm && !prosody_stream_warps(ps))
+        throw Error(19, "a prosody stream needs a pitch or tempo ratio, a pitch contour or a formant ratio that asks for "
+                        "something (ratios NaN or 1, and a formant ratio NaN or equal to the pitch: none)");
+}
+
 namespace {
-// The history buffers (two sets of cap_in + cap_s floats and two ints) and, after them, the piece table.
+// The history buffers (two sets of cap_in + cap_s floats and two ints), the formant stage's two carry buffers when it
+// runs and, after them, the piece table.
 ProsodyStream* allocate_prosody_stream(std::unique_ptr<ProsodyStream> ps, Voice* v, int device) {
     ps->v = v; ps->device = device;
     SB_CUDA(cudaSetDevice(device));
     const size_t side = (size_t)ps->cap_in + ps->cap_s + 2;      // floats, floats, two ints
-    const size_t table = (2 * side * 4 + 15) / 16 * 16;
+    const size_t fm = ps->fm ? (size_t)FM_CARRY : 0;
+    const size_t table = (2 * (side + fm) * 4 + 15) / 16 * 16;
     const size_t bytes = table + ps->pieces.size() * sizeof(ContourPiece);
     void* mem = nullptr;
     SB_CUDA(cudaMalloc(&mem, bytes));
@@ -535,6 +557,7 @@ ProsodyStream* allocate_prosody_stream(std::unique_ptr<ProsodyStream> ps, Voice*
         float* base = static_cast<float*>(mem) + b * side;
         ps->in_hist[b] = base; ps->s_hist[b] = base + ps->cap_in;
         ps->d_hist[b] = reinterpret_cast<int*>(base + ps->cap_in + ps->cap_s);
+        if (fm) ps->fm_hist[b] = static_cast<float*>(mem) + 2 * side + b * fm;
     }
     if (!ps->pieces.empty()) {
         ContourPiece* d = reinterpret_cast<ContourPiece*>(static_cast<char*>(mem) + table);
@@ -555,6 +578,13 @@ ProsodyStream* create_prosody_stream_contour(Voice* v, int device, int rate, lon
                                              const float* ratios, size_t n_ids, float tempo) {
     std::unique_ptr<ProsodyStream> ps(new ProsodyStream());
     prosody_stream_init_contour(*ps, rate, n, ends, ratios, n_ids, tempo);
+    return allocate_prosody_stream(std::move(ps), v, device);
+}
+
+ProsodyStream* create_prosody_stream_formant(Voice* v, int device, int rate, long long n, const long long* ends,
+                                             const float* ratios, size_t n_ids, float pitch, float tempo, float phi) {
+    std::unique_ptr<ProsodyStream> ps(new ProsodyStream());
+    prosody_stream_init_formant(*ps, rate, n, ends, ratios, n_ids, pitch, tempo, phi);
     return allocate_prosody_stream(std::move(ps), v, device);
 }
 
@@ -730,6 +760,23 @@ std::vector<long long> prosody_stream_counts(ProsodyStream& ps, const long long*
         const long long row[5] = {t.j1 - t.j0, t.next.frames, t.next.stretched, t.next.h_in, t.next.h_s};
         std::copy(row, row + 5, out.begin() + 5 * k);
         prosody_stream_advance(ps, t, k + 1 == n);
+    }
+    return out;
+}
+
+std::vector<long long> formant_stream_counts(ProsodyStream& ps, const long long* chunk_lens, size_t n) {
+    std::vector<long long> out(n);
+    for (size_t k = 0; k < n; k++) {
+        if (chunk_lens[k] < 0) throw Error(19, "chunk " + std::to_string(k) + ": negative length");
+        const bool last = k + 1 == n;
+        const ProsodyStep t = prosody_stream_step(ps, chunk_lens[k], last);
+        out[k] = t.j1 - t.j0;
+        if (ps.fm) {
+            const FormantStep f = formant_stream_step(ps, t.next.emitted, last);
+            out[k] = f.e1 - f.e0;
+            formant_stream_advance(ps, f);
+        }
+        prosody_stream_advance(ps, t, last);
     }
     return out;
 }

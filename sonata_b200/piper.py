@@ -229,6 +229,21 @@ def _formant_array(values, n: int):
     return None if np.isnan(out).all() else out
 
 
+def _stream_formant(formant_ratio, who: str) -> Optional[float]:
+    """A stream's formant ratio as a float, or None for None / NaN; an OperationError names the stream `who`."""
+    if formant_ratio is None:
+        return None
+    if isinstance(formant_ratio, bool) or not isinstance(formant_ratio, numbers.Real):
+        raise OperationError(f"{who}: formant ratio {formant_ratio!r} is not a number")
+    v = float(formant_ratio)
+    if math.isnan(v):
+        return None
+    if not (math.isfinite(v) and FORMANT_RANGE[0] <= v <= FORMANT_RANGE[1]):
+        raise OperationError(f"{who}: formant ratio {v} is not a finite value in "
+                             f"[{FORMANT_RANGE[0]}, {FORMANT_RANGE[1]}] (None or NaN: none)")
+    return v
+
+
 def refuse_formants(formant_ratio, where: str) -> None:
     """OperationError when `where`, a mode that hands out a sentence chunk by chunk, is asked for a formant ratio."""
     if formant_ratio is not None and not (isinstance(formant_ratio, numbers.Real) and math.isnan(float(formant_ratio))):
@@ -1134,16 +1149,42 @@ class ProsodyStream:
     `pitch_contour`: one pitch ratio per id of `enc` (the EncoderOutputs of the sentence the stream carries; values as
     for infer_batch_with_values' pitch_contours), instead of `pitch` (sb200_prosody_stream_create_contour).  Its plan is
     fixed by enc's frames, so the stream must be fed exactly enc's chunks; `bounds` then holds each id's delivered end
-    at the voice's rate (None without a contour)."""
+    at the voice's rate (None without a contour).
+
+    `formant`: a formant ratio as for infer_batch_with_values' formants (None / NaN: none), applied on top of the
+    ratios or contour, or alone when they ask for nothing (sb200_prosody_stream_create_formant): the concatenation of
+    what the stream emits is the formant stage of the sentence it warps, applied at once.  Its stage holds back 768 -
+    1023 samples more than the warp alone."""
 
     def __init__(self, model: "_VitsCommons", pitch=None, tempo=None, pitch_contour=None,
-                 enc: Optional["EncoderOutputs"] = None):
+                 enc: Optional["EncoderOutputs"] = None, formant=None):
         p, t = _prosody_arrays([pitch], [tempo], 1)
+        phi = _stream_formant(formant, "stream")
         self._m, self._h = model, C.c_void_p()
         self.pitch = None if p is None else float(p[0])
         self.tempo = None if t is None else float(t[0])
+        self.formant = phi
         self.bounds = None
         err = N.sb200_error()
+        if phi is not None:
+            # sb200_prosody_stream_create_formant: the ratio or contour stream with phi on top, or phi alone
+            c = None
+            if pitch_contour is not None:
+                if not isinstance(enc, EncoderOutputs) or enc._m is not model or not enc._h:
+                    raise OperationError("a pitch contour needs the EncoderOutputs of its sentence, from this model")
+                c = _contour_arrays([len(enc.p_duration)], [pitch_contour], None, ["stream"])
+                if c is None:
+                    c = np.full(len(enc.p_duration), np.nan, np.float32)
+            nan = float("nan")
+            _check(model._lib.sb200_prosody_stream_create_formant(
+                model._h, None if c is None else enc._h, nan if p is None else float(p[0]), _ptr(c, C.c_float),
+                0 if c is None else c.size, nan if t is None else float(t[0]), phi, C.byref(self._h), C.byref(err)),
+                err)
+            if c is not None:
+                self.bounds = np.zeros(c.size, np.int64)
+                _check(model._lib.sb200_prosody_stream_bounds(self._h, _ptr(self.bounds, C.c_int64), c.size,
+                                                              C.byref(err)), err)
+            return
         if pitch_contour is not None:
             if p is not None:
                 raise OperationError("stream: a pitch contour and a pitch ratio together (give one or the other)")
@@ -1171,6 +1212,12 @@ class ProsodyStream:
         self._m._lib.sb200_prosody_stream_profile(self._h, C.byref(s), C.byref(p))
         return float(s.value), float(p.value)
 
+    def last_formant_ms(self) -> float:
+        """The "formant" device time (ms) of the last chunk pass this stream was in (0: its stage did not run)."""
+        f = C.c_float()
+        self._m._lib.sb200_prosody_stream_profile_formant(self._h, C.byref(f))
+        return float(f.value)
+
     def __del__(self):
         try:
             if self._h:
@@ -1180,19 +1227,24 @@ class ProsodyStream:
             pass
 
 
-def _stream_prosody(model, pitch, tempo, pitch_contour=None, enc=None) -> Optional[ProsodyStream]:
-    """A ProsodyStream for a stream with these ratios, or with this per-id contour of enc's sentence and the tempo, or
-    None when nothing asks for anything.  A given contour makes a contoured stream (which has bounds) whenever the
-    contour or the tempo asks for something; a contour of None / NaN / 1 only is no contour beside a pitch ratio, as in
-    the batch calls, and with neither a pitch nor a tempo it leaves the plain stream, which has no bounds."""
+def _stream_prosody(model, pitch, tempo, pitch_contour=None, enc=None, formant=None) -> Optional[ProsodyStream]:
+    """A ProsodyStream for a stream with these ratios, or with this per-id contour of enc's sentence and the tempo, and
+    the formant ratio, or None when nothing asks for anything.  A given contour makes a contoured stream (which has
+    bounds) whenever the contour or the tempo asks for something; a contour of None / NaN / 1 only is no contour beside a
+    pitch ratio, as in the batch calls, and with neither a pitch nor a tempo it leaves the plain stream, which has no
+    bounds.  A formant ratio asks for something unless it equals the pitch ratio (1 without one): it then makes a
+    formant-only stream of a plain one."""
     p, t = _prosody_arrays([pitch], [tempo], 1)
+    phi = _stream_formant(formant, "stream")
     if pitch_contour is not None:
         asks = _contour_arrays([len(enc.p_duration)], [pitch_contour], p, ["stream"]) is not None
         if asks or (p is None and t is not None):
-            return ProsodyStream(model, pitch, tempo, pitch_contour, enc)
-    if p is None and t is None:
+            return ProsodyStream(model, pitch, tempo, pitch_contour, enc, phi)
+    if phi is not None and np.float32(phi) == (np.float32(1.0) if p is None else p[0]):
+        phi = None                      # r_m = 1 on every frame: the stage would not run
+    if p is None and t is None and phi is None:
         return None
-    return ProsodyStream(model, pitch, tempo)
+    return ProsodyStream(model, pitch, tempo, formant=phi)
 
 
 def _delivered_bounds(warp: Optional[ProsodyStream], resampler: Optional["Resampler"]):
@@ -1426,7 +1478,10 @@ class VitsStreamingModel(_VitsCommons):
                          pitch: Optional[float] = None, tempo: Optional[float] = None,
                          pitch_contour: Optional[Sequence] = None,
                          formant_ratio: Optional[float] = None, speaker_blend=None) -> SpeechStreamer:
-        """`formant_ratio` is refused: streams do not carry the formant stage.
+        """`formant_ratio`: as for infer_batch_with_values' formants, on top of `pitch` / `tempo` / `pitch_contour` or
+        alone, the sentence's formant stage carried as one stream on the device (ProsodyStream): the concatenation of
+        the chunks is the formant stage applied at once to the sentence the stream yields without it, then resampled and
+        encoded as without it.  The stage holds back 768 - 1023 samples (35 - 46 ms at 22.05 kHz) more.
         `speaker_blend`: the sentence's speaker blend (a mapping {speaker: weight}, see infer_batch_with_values), or
         None for the fallback config's speaker; the latent keeps it, so every chunk speaks with it.
         `seed`: the sentence's noise seed (see infer_batch_with_values), or None for positional noise.
@@ -1440,10 +1495,11 @@ class VitsStreamingModel(_VitsCommons):
         that character's id and pad; it combines with `tempo` but not with `pitch`.  The concatenation of the chunks is
         the sentence the stream yields without it, with that contour applied at once (sb200_debug_prosody_contour), and
         the streamer's `bounds` give each id's delivered end."""
-        refuse_formants(formant_ratio, "stream_synthesis")
         if not isinstance(self, VitsStreamingModel):
+            refuse_formants(formant_ratio, "stream_synthesis")
             refuse_prosody(pitch, tempo, "stream_synthesis")
             refuse_contour(pitch_contour, "stream_synthesis")
+        phi = _stream_formant(formant_ratio, "stream")
         pit, _ = _prosody_arrays([pitch], [tempo], 1)
         _seed_arrays([seed], 1)
         _rate_array([output_rate], 1)
@@ -1462,7 +1518,7 @@ class VitsStreamingModel(_VitsCommons):
         else:
             enc = self.infer_encoder(ids) if seed is None else self.infer_encoder_batch([ids], seeds=[seed])[0]
         return SpeechStreamer(enc, chunk_size, chunk_padding, _stream_resampler(self, output_rate), encoding, g,
-                              _stream_prosody(self, pitch, tempo, contour, enc))
+                              _stream_prosody(self, pitch, tempo, contour, enc, phi))
 
 
 def _stream_gain(encoding, gain) -> float:
@@ -1531,7 +1587,7 @@ class StreamBatch:
         self.model = model
         self.chunk_size, self.chunk_padding = chunk_size, chunk_padding
         self._pending: list = []      # (key, ids, config, chunk_size, seed, output rate, encoding, gain, pitch, tempo,
-                                      # per-id contour, speaker blend) not encoded yet
+                                      # per-id contour, speaker blend, formant ratio) not encoded yet
         self._active: List[_Stream] = []
         self._retired: dict = {}      # key -> delivered ends (None: no contour) of the streams the last step ended
         self._next_key = 0
@@ -1548,22 +1604,24 @@ class StreamBatch:
         for stream_synthesis; its length and values are checked here, and what needs the sentence's frames fails as the
         stream's error item.  `bounds(key)` gives a contoured stream's per-id delivered ends once it is encoded.  A
         warped stream's chunks go through passes of their own, so the other streams keep their passes and their
-        bits.  `formant_ratio` is refused: streams do not carry the formant stage.  `speaker_blend`: the stream's
-        speaker blend, as for stream_synthesis; it replaces its config's speaker and is checked here."""
-        refuse_formants(formant_ratio, "StreamBatch")
+        bits.  `formant_ratio`: the stream's formant ratio, as for stream_synthesis; it is checked here, naming the
+        stream, and a stream with one is warped (in those passes) even without pitch or tempo.  `speaker_blend`: the
+        stream's speaker blend, as for stream_synthesis; it replaces its config's speaker and is checked here."""
         if not isinstance(self.model, VitsStreamingModel):
+            refuse_formants(formant_ratio, "StreamBatch")
             refuse_prosody(pitch, tempo, "StreamBatch")
             refuse_contour(pitch_contour, "StreamBatch")
         return self._add(ids_or_phonemes, config, self.chunk_size, seed, output_rate, encoding, gain, pitch, tempo,
-                         pitch_contour, speaker_blend)
+                         pitch_contour, speaker_blend, formant_ratio)
 
     def _add(self, ids_or_phonemes, config, chunk_size: int, seed: Optional[int] = None,
              output_rate: Optional[int] = None, encoding: Optional[str] = None, gain: Optional[float] = None,
              pitch: Optional[float] = None, tempo: Optional[float] = None, pitch_contour=None,
-             speaker_blend=None) -> int:
+             speaker_blend=None, formant_ratio=None) -> int:
         if config is not None and not isinstance(config, PiperSynthesisConfig):
             raise OperationError("Invalid configuration for Vits Model")
         _blend_arrays(self.model, [speaker_blend], 1, [f"stream {self._next_key}"])
+        phi = _stream_formant(formant_ratio, f"stream {self._next_key}")
         pit, _ = _prosody_arrays([pitch], [tempo], 1)
         _seed_arrays([seed], 1)
         _rate_array([output_rate], 1)
@@ -1588,7 +1646,7 @@ class StreamBatch:
         key = self._next_key
         self._next_key += 1
         self._pending.append((key, ids, config, chunk_size, seed, output_rate, encoding, gain, pitch, tempo, contour,
-                              speaker_blend))
+                              speaker_blend, phi))
         return key
 
     def bounds(self, key) -> Optional[np.ndarray]:
@@ -1633,7 +1691,7 @@ class StreamBatch:
                     try:
                         active.append(_Stream(p[0], enc, p[3], self.chunk_padding,
                                               _stream_resampler(self.model, p[5]), p[6], p[7],
-                                              _stream_prosody(self.model, p[8], p[9], p[10], enc)))
+                                              _stream_prosody(self.model, p[8], p[9], p[10], enc, p[12])))
                         continue
                     except SonataError as e:
                         err = e

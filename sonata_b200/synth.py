@@ -146,16 +146,21 @@ def _blend_extra(model, n: int, speaker_blend, where: str) -> dict:
     return {"speaker_blends": [speaker_blend] * n}
 
 
-def _stream_prosody_extra(model, pitch_ratio, tempo, where: str) -> dict:
-    """The stream_synthesis keywords of a streaming request's ratios ({} without either).  A model that is not one of
-    this library's streaming voices cannot warp a stream on the device and refuses by name (piper.refuse_prosody)."""
-    from .piper import VitsStreamingModel, _prosody_arrays, refuse_prosody
+def _stream_prosody_extra(model, pitch_ratio, tempo, where: str, formant_ratio=None) -> dict:
+    """The stream_synthesis keywords of a streaming request's ratios ({} without any).  A model that is not one of
+    this library's streaming voices cannot warp a stream on the device and refuses by name (piper.refuse_prosody,
+    piper.refuse_formants)."""
+    from .piper import VitsStreamingModel, _prosody_arrays, _stream_formant, refuse_formants, refuse_prosody
     if not isinstance(model, VitsStreamingModel):
+        refuse_formants(formant_ratio, where)
         refuse_prosody(pitch_ratio, tempo, where)
     p, t = _prosody_arrays([pitch_ratio], [tempo], 1)
     out = {} if p is None else {"pitch": pitch_ratio}
     if t is not None:
         out["tempo"] = tempo
+    phi = _stream_formant(formant_ratio, "request")
+    if phi is not None:
+        out["formant_ratio"] = phi
     return out
 
 
@@ -199,7 +204,8 @@ class SonataSpeechSynthesizer:
     # frequencies multiplied by the ratio at the same duration / played that many times faster at the same pitch, on
     # the device before any resampling and loudness (piper.PITCH_RANGE, piper.TEMPO_RANGE).  `formant_ratio` (lazy,
     # parallel and file modes): each sentence's spectral envelope moved by the ratio after the pitch stage; 1.0 with a
-    # pitch ratio keeps the voice's own formants (piper.FORMANT_RANGE).  The streamed modes refuse it by name.
+    # pitch ratio keeps the voice's own formants (piper.FORMANT_RANGE).  The streamed modes carry it as a stream on
+    # this library's streaming voices and refuse it by name on other models.
     # `speaker_blend` (every mode): a mapping {speaker: weight} of a multi-speaker voice that every sentence speaks with
     # in place of the fallback config's speaker (see piper.VitsModel.infer_batch_with_values); checked before any
     # synthesis.
@@ -302,11 +308,9 @@ class SonataSpeechSynthesizer:
         `output_rate`: each sentence is resampled as its own stream (zero history at its start, flushed at its end).
         `encoding`: every chunk is G.711 bytes of its to_i16_vec after the volume, encoded on the device.
         `pitch_ratio` / `tempo`: every sentence warped as its own stream on the device (a fresh piper.ProsodyStream,
-        flushed at its end); appended silence is not warped.  `formant_ratio` is refused: streams do not carry the
-        formant stage."""
-        from .piper import refuse_formants
-        refuse_formants(formant_ratio, "synthesize_streamed")
-        pros = _stream_prosody_extra(self.model, pitch_ratio, tempo, "synthesize_streamed")
+        flushed at its end); appended silence is not warped.  `formant_ratio`: every sentence's formant stage carried
+        as its own stream on the device, with or without the ratios (see stream_synthesis)."""
+        pros = _stream_prosody_extra(self.model, pitch_ratio, tempo, "synthesize_streamed", formant_ratio)
         sentence_seed(seed, 0)
         _check_output_rate(output_rate)
         refuse_flac(encoding, "synthesize_streamed")
@@ -476,11 +480,10 @@ class RealtimeBatch:
             formant_ratio: Optional[float] = None, speaker_blend=None) -> int:
         """`seed`: the request's noise seed, `output_rate` its sample rate and `encoding` its G.711 encoding, as for
         synthesize_streamed, and `pitch_ratio` / `tempo` its ratios, each sentence warped as its own stream, as there.
-        `formant_ratio` is refused, as there.  `speaker_blend`: the request's speaker blend, as for synthesize_streamed;
-        it replaces the config's speaker and is checked here, naming the request."""
-        from .piper import PiperSynthesisConfig, refuse_formants
-        refuse_formants(formant_ratio, "RealtimeBatch")
-        pros = _stream_prosody_extra(self.model, pitch_ratio, tempo, "RealtimeBatch")
+        `formant_ratio` its formant ratio, as there.  `speaker_blend`: the request's speaker blend, as for
+        synthesize_streamed; it replaces the config's speaker and is checked here, naming the request."""
+        from .piper import PiperSynthesisConfig
+        pros = _stream_prosody_extra(self.model, pitch_ratio, tempo, "RealtimeBatch", formant_ratio)
         sentence_seed(seed, 0)
         _check_output_rate(output_rate)
         refuse_flac(encoding, "RealtimeBatch")

@@ -17,9 +17,11 @@ with every stream at one pair of pitch / tempo ratios (none, pitch 1.25, tempo 1
 add the "stretch" and "pitch" device ms per step; audio_s_per_s is then at the delivered length.  With --contour they
 are StreamBatch runs with pitch contours on the same workload: no ratios, pitch 1.25, a uniform 1.25 contour (which
 gives pitch 1.25's chunks bit for bit), the question contour (1 on the first 75 % of ids, then rising in five steps to
-1.3) and per-id ratios drawn from {0.8, 1, 1.25} with a fixed seed, with the same added figures.
+1.3) and per-id ratios drawn from {0.8, 1, 1.25} with a fixed seed, with the same added figures.  With --formants they
+are StreamBatch runs with formant ratios: no ratios, pitch 1.25, pitch 1.25 with formant ratio 1 (the pitch shift that
+keeps the voice's formants) and formant ratio 1.2 alone, whose lines also add the "formant" device ms per step.
 
-  python tools/bench_streams.py [--ks 1,8,32,128] [--reps 1] [--ratios | --contour]
+  python tools/bench_streams.py [--ks 1,8,32,128] [--reps 1] [--ratios | --contour | --formants]
 """
 import argparse
 import atexit
@@ -95,6 +97,10 @@ RATIO_ARMS = {"none": {}, "pitch_1.25": {"pitch": 1.25}, "tempo_1.5": {"tempo": 
               "pitch_0.8_tempo_2": {"pitch": 0.8, "tempo": 2.0}}
 
 
+FORMANT_ARMS = {"none": {}, "pitch_1.25": {"pitch": 1.25}, "pitch_1.25_formant_1": {"pitch": 1.25, "formant_ratio": 1.0},
+                "formant_1.2": {"formant_ratio": 1.2}}
+
+
 def question(k):
     """The question contour over k ids: 1 on the first 75 %, then rising in five steps to 1.3."""
     c = [1.0] * k
@@ -116,10 +122,11 @@ def contour_arms(batches):
 def run_ratios(model, batches, sr, ratios):
     """StreamBatch with every stream at `ratios` (keyword arguments of StreamBatch.add, or a function of the stream's
     index giving them): the batch arm's figures plus the "stretch" and "pitch" device ms per step (each warped pass's
-    regions, summed over the passes of a step, averaged over the steps)."""
+    regions, summed over the passes of a step, averaged over the steps), and the "formant" ms when a stream has a
+    formant ratio."""
     from sonata_b200 import StreamBatch
     decode = model.infer_decoder_batch
-    prof = {"stretch": 0.0, "pitch": 0.0}
+    prof = {"stretch": 0.0, "pitch": 0.0, "formant": 0.0}
 
     def timed(chunks, **kw):
         out = decode(chunks, **kw)
@@ -128,6 +135,7 @@ def run_ratios(model, batches, sr, ratios):
             s, p = w.last_pass_ms()
             prof["stretch"] += s
             prof["pitch"] += p
+            prof["formant"] += w.last_formant_ms()
         return out
     model.infer_decoder_batch = timed
     steps = 0
@@ -149,9 +157,11 @@ def run_ratios(model, batches, sr, ratios):
         wall = time.perf_counter() - t0
     finally:
         del model.infer_decoder_batch
-    return wall, [arrivals[k] for k in keys], [lens[k] for k in keys], {
-        "stretch_ms_per_step": round(prof["stretch"] / max(steps, 1), 3),
-        "pitch_ms_per_step": round(prof["pitch"] / max(steps, 1), 3), "steps": steps}
+    extra = {"stretch_ms_per_step": round(prof["stretch"] / max(steps, 1), 3),
+             "pitch_ms_per_step": round(prof["pitch"] / max(steps, 1), 3), "steps": steps}
+    if any("formant_ratio" in (ratios(s) if callable(ratios) else ratios) for s in range(len(batches))):
+        extra["formant_ms_per_step"] = round(prof["formant"] / max(steps, 1), 3)
+    return wall, [arrivals[k] for k in keys], [lens[k] for k in keys], extra
 
 
 def run_threads(model, batches, sr):
@@ -193,6 +203,9 @@ def main():
     ap.add_argument("--contour", action="store_true",
                     help="StreamBatch arms with pitch contours instead (no ratios, pitch 1.25, uniform 1.25, question, "
                          "mixed per-id ratios), alternated in each rep")
+    ap.add_argument("--formants", action="store_true",
+                    help="StreamBatch arms with formant ratios instead (no ratios, pitch 1.25, pitch 1.25 with formant "
+                         "ratio 1, formant ratio 1.2 alone), alternated in each rep")
     args = ap.parse_args()
 
     import torch
@@ -218,6 +231,8 @@ def main():
         arms = {name: (lambda m, b, s, r=r: run_ratios(m, b, s, r)) for name, r in RATIO_ARMS.items()}
     if args.contour:
         arms = {name: (lambda m, b, s, r=r: run_ratios(m, b, s, r)) for name, r in contour_arms(batches).items()}
+    if args.formants:
+        arms = {name: (lambda m, b, s, r=r: run_ratios(m, b, s, r)) for name, r in FORMANT_ARMS.items()}
     for k in ks:
         for name, fn in arms.items():            # warm-up: modules, arenas and pinned blocks at this K
             fn(model, batches[:k], sr)
