@@ -649,6 +649,53 @@ int32_t sb200_prosody_stream_create_formant(sb200_voice* v, const sb200_latent* 
 /* The "formant" device time (ms) of the last chunk pass the stream was in (0: its stage did not run). */
 int32_t sb200_prosody_stream_profile_formant(const sb200_prosody_stream* s, float* formant_ms);
 
+/* ---- live loudness: a stream held to a target by a causal BS.1770 meter carried on the device ----
+ * A loudness stream (a meter) belongs to a voice, and so to its device, and meters one delivered rate r.  Its target T
+ * (LUFS) is finite and in [-70, 0]; its maximum gain M (dB) is finite and in [0, 40] (20 is the usual choice).  Its input
+ * x_0, x_1, .. is the concatenation of the f32 samples that every chunk passed with it would deliver without it: after
+ * the post-path (trims, crossfade), the prosody and formant stages and resampling, before the chunk's gain and before
+ * conversion.  Across chunks, and across the sentences of one request, the signal just continues.
+ * With S = (r + 5) / 10 and q_c the sum of y^2 over step c (samples [cS, (c + 1)S)) of the K-weighted signal, computed
+ * as sb200_debug_loudness's kernel computes it (each step filtered from zero state to e_c, states chained as
+ * s_{c+1} = A^S s_c + e_c, then y^2 summed in sample order from the true s_c; the same bits as the batch kernel's q_c):
+ * - the reading at step boundary m >= 1 (time mS) uses x[0, mS) only.  For m >= 4 it is the gated integrated loudness
+ *   L_m over blocks 0 .. m - 4 with the batch gates and reduction order: sb200_debug_loudness(x, mS, r), bit for bit.
+ *   For 1 <= m <= 3, before the first 400 ms block exists, it is provisional:
+ *   L_m = -0.691 + 10 log10((q_0 + .. + q_{m-1}) / (mS)), summed left to right, and -inf when that is <= -70 or the
+ *   sum is 0.
+ * - gains at the boundaries: a_0 = 1 for a new meter (a meter that continues keeps its last a); for m >= 1,
+ *   a_m = a_{m-1} when L_m = -inf, else f32(min(10^((T - L_m)/20), 10^(M/20))), computed in double.
+ * - sample i of step m >= 1 gets G_i = f32(a_{m-1} + (a_m - a_{m-1}) (i - mS + 1) / S), in double as written with each
+ *   operation rounded: a linear ramp across each 100 ms step.  Step 0 gets a_0.  The output is
+ *   y_i = clamp(x_i * G_i, -1, 1) (an f32 product); the meter counts the samples it clamped.
+ * So G_i depends only on samples before mS: the meter holds nothing back and adds no latency, and every chunk delivers
+ * exactly as many samples as it would without it.  The result does not depend on how the signal is chunked, or on what
+ * shares the pass.  When a request ends at n samples, its last reading is the batch meter's L of x[0, floor(n/S) S).
+ * The first 100 ms of a new meter play at gain 1, readings before 400 ms are provisional, and peaks are held by the
+ * clamp, not by a look-ahead limiter.  A meter keeps q of at most 2^16 steps (about 109 minutes of audio).
+ * out_rate: r (0: the voice's rate; else one of the output rates). */
+typedef struct sb200_loudness_stream sb200_loudness_stream;
+int32_t sb200_loudness_stream_create(sb200_voice* v, uint32_t out_rate, float target_lufs, float max_gain_db,
+                                     sb200_loudness_stream** out, sb200_error* err);
+void sb200_loudness_stream_free(sb200_loudness_stream* s);
+/* The meter's last reading (LUFS; -inf before any or without one), its last gain a, the samples it has metered and
+ * clamped, and the "loudness" device time (ms) of the last chunk pass it was in.  Any pointer may be NULL. */
+int32_t sb200_loudness_stream_state(const sb200_loudness_stream* s, double* lufs, float* gain, int64_t* samples,
+                                    int64_t* clipped, float* ms, sb200_error* err);
+/* sb200_decode_chunks_warped with meters[k] (NULL entries: none; meters NULL: that call, bit for bit) metering chunk
+ * k's delivered samples as above, in the pass's "loudness" region after resampling.  A metered chunk's gain[k] scales y
+ * after the meter, in every format; its i16 is trunc(clamp(y * 32767)) at the fixed scale, not peak-normalised, and
+ * G.711 encodes those samples.  Joined, what a metered stream delivers (f32) is, bit for bit,
+ * sb200_debug_loudness_stream over the joined chunks the same stream delivers without a meter, however they are
+ * chunked.  Each of these fails with OPERATION_ERROR naming the chunk, before any device work or state change: a meter
+ * made for another voice, a meter used twice in one call, a chunk whose delivered rate is not the meter's, a meter
+ * whose history would pass 2^16 steps. */
+int32_t sb200_decode_chunks_metered(sb200_voice* v, const sb200_latent* const* zs, const int64_t* lo, const int64_t* hi,
+                                    const int64_t* trim_lo_frames, const int64_t* trim_hi_frames, size_t n, int32_t fade,
+                                    const float* gain, sb200_resampler* const* resamplers,
+                                    sb200_prosody_stream* const* warps, sb200_loudness_stream* const* meters,
+                                    const int32_t* last, int32_t format, void** outs, size_t* lens, sb200_error* err);
+
 /* ---- introspection for tests / bench ---- */
 /* Copy a named intermediate of the LAST run of `job` to host (time-major fp32, valid rows of
  * utterance b only).  Names: "x","stats","logw","z_p","z","dec.pre","dec.up<i>","dec.mrf<i>", and the first encoder
@@ -762,6 +809,12 @@ int32_t sb200_debug_loudness_filter(int32_t rate, double* coeffs);
 /* The loudness kernel over one caller buffer x[0 .. n) at `rate`, measured only: *lufs receives its integrated loudness,
  * bit for bit what a job measures for an utterance of those samples. */
 int32_t sb200_debug_loudness(int32_t device, const float* x, size_t n, int32_t rate, double* lufs, sb200_error* err);
+/* A fresh meter (see sb200_loudness_stream_create) at `rate` with target_lufs and max_gain_db on `device`, fed x in
+ * chunks of chunk_lens[0 .. n_chunks) samples, one loudness launch per chunk: y receives the metered samples (as many as
+ * x), lufs_steps / gain_steps every reading L_m and gain a_m, m = 1 .. floor(total / S), and *clipped the clamp count. */
+int32_t sb200_debug_loudness_stream(int32_t device, const float* x, const size_t* chunk_lens, size_t n_chunks,
+                                    int32_t rate, float target_lufs, float max_gain_db, float* y, double* lufs_steps,
+                                    float* gain_steps, int64_t* clipped, sb200_error* err);
 /* Test hook, no device needed: the prosody plan (see sb200_speak_batch_ids_prosody) of n samples at `rate` with the two
  * ratios: shape6 receives Hs, N, D, n1, n2, F, and positions[0 .. min(F, cap)) the analysis positions a_k.  Returns 0, or
  * 19 for a ratio out of range or a rate outside 1000 .. 48000. */

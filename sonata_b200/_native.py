@@ -250,6 +250,16 @@ SIGNATURES = {
     "sb200_prosody_stream_create_formant": (C.c_int32, [_P, _P, C.c_float, C.POINTER(C.c_float), C.c_size_t,
                                                         C.c_float, C.c_float, C.POINTER(_P), _ERR]),
     "sb200_prosody_stream_profile_formant": (C.c_int32, [_P, C.POINTER(C.c_float)]),
+    "sb200_loudness_stream_create": (C.c_int32, [_P, C.c_uint32, C.c_float, C.c_float, C.POINTER(_P), _ERR]),
+    "sb200_loudness_stream_free": (None, [_P]),
+    "sb200_loudness_stream_state": (C.c_int32, [_P, C.POINTER(C.c_double), C.POINTER(C.c_float),
+                                                C.POINTER(C.c_int64), C.POINTER(C.c_int64), C.POINTER(C.c_float),
+                                                _ERR]),
+    "sb200_decode_chunks_metered": (C.c_int32, [_P, C.POINTER(_P), C.POINTER(C.c_int64), C.POINTER(C.c_int64),
+                                                C.POINTER(C.c_int64), C.POINTER(C.c_int64), C.c_size_t, C.c_int32,
+                                                C.POINTER(C.c_float), C.POINTER(_P), C.POINTER(_P), C.POINTER(_P),
+                                                C.POINTER(C.c_int32), C.c_int32, C.POINTER(C.c_void_p),
+                                                C.POINTER(C.c_size_t), _ERR]),
     "sb200_debug_formant_stream_plan": (C.c_int32, [C.c_int32, C.c_float, C.c_float, C.POINTER(C.c_int64),
                                                     C.POINTER(C.c_float), C.c_size_t, C.c_float, C.POINTER(C.c_int64),
                                                     C.c_size_t, C.POINTER(C.c_int64), _ERR]),
@@ -272,6 +282,10 @@ SIGNATURES = {
     "sb200_debug_loudness_filter": (C.c_int32, [C.c_int32, C.POINTER(C.c_double)]),
     "sb200_debug_loudness": (C.c_int32, [C.c_int32, C.POINTER(C.c_float), C.c_size_t, C.c_int32, C.POINTER(C.c_double),
                                          _ERR]),
+    "sb200_debug_loudness_stream": (C.c_int32, [C.c_int32, C.POINTER(C.c_float), C.POINTER(C.c_size_t), C.c_size_t,
+                                                C.c_int32, C.c_float, C.c_float, C.POINTER(C.c_float),
+                                                C.POINTER(C.c_double), C.POINTER(C.c_float), C.POINTER(C.c_int64),
+                                                _ERR]),
     "sb200_debug_prosody_plan": (C.c_int32, [C.c_int32, C.c_int64, C.c_float, C.c_float, C.POINTER(C.c_int64),
                                              C.POINTER(C.c_int64), C.c_size_t]),
     "sb200_debug_prosody": (C.c_int32, [C.c_int32, C.POINTER(C.c_float), C.c_size_t, C.c_int32, C.c_float, C.c_float,

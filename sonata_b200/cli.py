@@ -23,7 +23,8 @@ from typing import Optional
 
 from . import from_config_path
 from .core import ENCODINGS, FLAC, OperationError, check_encoding
-from .piper import PiperSynthesisConfig, VitsStreamingModel, refuse_formants, refuse_prosody
+from .piper import (PiperSynthesisConfig, VitsStreamingModel, _check_live_loudness, refuse_formants,
+                    refuse_live_loudness, refuse_prosody)
 from .synth import AudioOutputConfig, SonataSpeechSynthesizer, _check_loudness, _check_prosody
 
 MODES = ("lazy", "parallel", "realtime")
@@ -84,6 +85,13 @@ def build_parser() -> argparse.ArgumentParser:
                     help="Target integrated loudness of every sentence in LUFS, [-70, 0] (ITU-R BS.1770-4; e.g. -23 "
                          "EBU R128, -16 podcasts), measured and applied on the GPU; output is then written at a fixed "
                          "scale instead of peak-normalised.  Not in realtime mode")
+    ap.add_argument("--live-loudness", type=float, metavar="LUFS",
+                    help="Realtime mode only (streaming voices): hold the stream at this loudness in LUFS, [-70, 0], "
+                         "with a causal BS.1770 meter of everything delivered so far driving a gain ramped over each "
+                         "100 ms, on the GPU, adding no latency; output is then written at a fixed scale.  The first "
+                         "100 ms play at gain 1 and peaks are clamped, not limited.  Other modes: use --loudness")
+    ap.add_argument("--max-gain-db", type=float, metavar="DB",
+                    help="The most gain --live-loudness may apply, in dB, [0, 40] (default 20)")
     ap.add_argument("--pitch-ratio", type=float, metavar="RATIO",
                     help="Multiply every frequency of the speech by RATIO, [0.5, 2], at the same duration, on the GPU.  "
                          "Not in realtime mode")
@@ -114,7 +122,9 @@ def process_request(synth: SonataSpeechSynthesizer, default_cfg: PiperSynthesisC
     `tempo` (optional): the ratios every sentence is shifted and played by, in lazy and parallel modes.
     `formant_ratio` (optional): the ratio every sentence's formants are moved by after the pitch stage, in every mode
     (realtime mode carries it as a stream on this library's streaming voices).  `speaker_blend` (optional): an object
-    {speaker name or id: weight} (see speaker_blend_of) every sentence speaks with, in every mode."""
+    {speaker name or id: weight} (see speaker_blend_of) every sentence speaks with, in every mode.  `live_loudness` /
+    `max_gain_db` (optional, realtime mode only): the request's live loudness target in LUFS and the meter's maximum
+    gain (see SonataSpeechSynthesizer.synthesize_streamed); the PCM is then written at the fixed scale."""
     out = out or sys.stdout.buffer
     mode = (req.get("mode") or "lazy").lower()
     loudness = req.get("loudness")
@@ -132,6 +142,17 @@ def process_request(synth: SonataSpeechSynthesizer, default_cfg: PiperSynthesisC
             raise OperationError("loudness normalisation is not available in realtime mode: integrated loudness needs "
                                  "the whole sentence, and realtime mode hands out a sentence's first chunk before its "
                                  "last one is decoded (use lazy or parallel mode)")
+    live = {k: req[k] for k in ("live_loudness", "max_gain_db") if req.get(k) is not None}
+    if live:
+        if "live_loudness" not in live:
+            raise OperationError("request: a maximum gain is the cap of a live loudness meter: give live_loudness")
+        if mode != "realtime" or output_file:
+            raise OperationError("live loudness is a realtime mode meter of a stream as it is delivered: for lazy, "
+                                 "parallel and file output use loudness (--loudness), which normalises each whole "
+                                 "sentence")
+        _check_live_loudness(live["live_loudness"], live.get("max_gain_db"), encoding, "request")
+        if not isinstance(synth.model, VitsStreamingModel):
+            refuse_live_loudness(live["live_loudness"], "realtime mode")
     pros = {k: req[k] for k in ("pitch_ratio", "tempo", "formant_ratio") if req.get(k) is not None}
     blend = speaker_blend_of(req.get("speaker_blend"))
     _check_prosody(pros.get("pitch_ratio"), pros.get("tempo"), pros.get("formant_ratio"))
@@ -164,7 +185,7 @@ def process_request(synth: SonataSpeechSynthesizer, default_cfg: PiperSynthesisC
         stream = synth.synthesize_parallel(text, oc, seed=seed, **rate, **loud, **enc, **pros)
     elif mode == "realtime":
         stream = synth.synthesize_streamed(text, oc, req.get("chunk_size") or 100, req.get("chunk_padding") or 3,
-                                          seed=seed, **rate, **enc, **pros)
+                                          seed=seed, **rate, **enc, **pros, **live)
     else:
         raise ValueError(f"unknown synthesis mode `{mode}`")
     for item in stream:
@@ -172,7 +193,7 @@ def process_request(synth: SonataSpeechSynthesizer, default_cfg: PiperSynthesisC
             out.write(item)
         else:
             samples = item if mode == "realtime" else item.samples
-            out.write(samples.as_wave_bytes(fixed_scale=loudness is not None))
+            out.write(samples.as_wave_bytes(fixed_scale=loudness is not None or bool(live)))
         out.flush()
 
 
@@ -189,7 +210,8 @@ def main(argv=None) -> int:
                "pitch": args.pitch, "appended_silence_ms": args.silence, "chunk_size": args.chunk_size,
                "chunk_padding": args.chunk_padding, "seed": args.seed, "output_rate": args.output_rate,
                "loudness": args.loudness, "encoding": args.encoding, "pitch_ratio": args.pitch_ratio,
-               "tempo": args.tempo, "formant_ratio": args.formant_ratio, "speaker_blend": args.speaker_blend}
+               "tempo": args.tempo, "formant_ratio": args.formant_ratio, "speaker_blend": args.speaker_blend,
+               "live_loudness": args.live_loudness, "max_gain_db": args.max_gain_db}
         process_request(synth, default_cfg, req, args.output_file)
     else:
         for i, line in enumerate(sys.stdin):
@@ -212,6 +234,10 @@ def main(argv=None) -> int:
                 req["formant_ratio"] = args.formant_ratio
             if req.get("speaker_blend") is None:
                 req["speaker_blend"] = args.speaker_blend
+            if req.get("live_loudness") is None:
+                req["live_loudness"] = args.live_loudness
+            if req.get("max_gain_db") is None:
+                req["max_gain_db"] = args.max_gain_db
             out_file = None
             if args.output_file:
                 stem, ext = os.path.splitext(args.output_file)

@@ -31,6 +31,10 @@ struct sb200_resampler {
     Resampler* r; std::shared_ptr<Voice> keep;
     ~sb200_resampler() { delete r; }
 };
+struct sb200_loudness_stream {
+    LoudnessStream* s; std::shared_ptr<Voice> keep;
+    ~sb200_loudness_stream() { delete s; }
+};
 
 namespace {
 
@@ -829,12 +833,22 @@ int32_t sb200_decode_chunks_warped(sb200_voice* v, const sb200_latent* const* zs
                                    const float* gain, sb200_resampler* const* resamplers,
                                    sb200_prosody_stream* const* warps, const int32_t* last, int32_t format, void** outs,
                                    size_t* lens, sb200_error* err) {
+    return sb200_decode_chunks_metered(v, zs, lo, hi, trim_lo_frames, trim_hi_frames, n, fade, gain, resamplers, warps,
+                                       nullptr, last, format, outs, lens, err);
+}
+
+int32_t sb200_decode_chunks_metered(sb200_voice* v, const sb200_latent* const* zs, const int64_t* lo, const int64_t* hi,
+                                    const int64_t* trim_lo_frames, const int64_t* trim_hi_frames, size_t n, int32_t fade,
+                                    const float* gain, sb200_resampler* const* resamplers,
+                                    sb200_prosody_stream* const* warps, sb200_loudness_stream* const* meters,
+                                    const int32_t* last, int32_t format, void** outs, size_t* lens, sb200_error* err) {
     return guarded(err, [&] {
         ChunkPass p = chunk_pass(zs, lo, hi, n, trim_lo_frames, trim_hi_frames, gain);
         if (n > 0 && (!resamplers || !outs || !lens)) throw Error(19, "null argument");
         for (size_t k = 0; k < n; k++) {
             p.chunks[k].rs = resamplers[k] ? resamplers[k]->r : nullptr;
             p.chunks[k].ps = warps && warps[k] ? warps[k]->p : nullptr;
+            p.chunks[k].ls = meters && meters[k] ? meters[k]->s : nullptr;
             if (last) p.chunks[k].last = last[k];
         }
         p.fade = fade; p.resample = true; p.format = format;
@@ -843,6 +857,35 @@ int32_t sb200_decode_chunks_warped(sb200_voice* v, const sb200_latent* const* zs
         if (format == PCM_I16) copy_out(r.i16, outs, lens);
         else if (format == PCM_F32) copy_out(r.f32, outs, lens);
         else copy_out(r.g711, outs, lens);
+    });
+}
+
+int32_t sb200_loudness_stream_create(sb200_voice* v, uint32_t out_rate, float target_lufs, float max_gain_db,
+                                     sb200_loudness_stream** out, sb200_error* err) {
+    return guarded(err, [&] {
+        if (!v || !out) throw Error(19, "null argument");
+        Voice* w = v->v.get();
+        if (w->device < 0 || !w->emb)
+            throw Error(19, "Failed to run model inference. Error: voice was loaded config-only (device -1); libsonata_b200 has no CPU path");
+        long long rate = w->sample_rate;
+        if (out_rate && out_rate != (uint32_t)w->sample_rate) {
+            resample_ratio(w->sample_rate, out_rate, "loudness stream: ");
+            rate = out_rate;
+        }
+        *out = new sb200_loudness_stream{create_loudness_stream(w, w->device, rate, target_lufs, max_gain_db), v->v};
+    });
+}
+void sb200_loudness_stream_free(sb200_loudness_stream* s) { delete s; }
+int32_t sb200_loudness_stream_state(const sb200_loudness_stream* s, double* lufs, float* gain, int64_t* samples,
+                                    int64_t* clipped, float* ms, sb200_error* err) {
+    return guarded(err, [&] {
+        if (!s) throw Error(19, "null argument");
+        const LoudnessStream& m = *s->s;
+        if (lufs) *lufs = m.lufs;
+        if (gain) *gain = m.a;
+        if (samples) *samples = m.samples;
+        if (clipped) *clipped = m.clipped;
+        if (ms) *ms = m.last_ms;
     });
 }
 
@@ -1190,6 +1233,52 @@ int32_t sb200_debug_loudness(int32_t device, const float* x, size_t n, int32_t r
         launch_loudness(dx, ds, 1, scratch, dl, dg, 0);
         SB_CUDA(cudaDeviceSynchronize());
         SB_CUDA(cudaMemcpy(lufs, dl, sizeof(double), cudaMemcpyDeviceToHost));
+    });
+}
+
+int32_t sb200_debug_loudness_stream(int32_t device, const float* x, const size_t* chunk_lens, size_t n_chunks,
+                                    int32_t rate, float target_lufs, float max_gain_db, float* y, double* lufs_steps,
+                                    float* gain_steps, int64_t* clipped, sb200_error* err) {
+    return guarded(err, [&] {
+        if ((n_chunks && (!chunk_lens || !y)) || !lufs_steps || !gain_steps || !clipped)
+            throw Error(19, "debug loudness stream: bad arguments");
+        size_t total = 0;
+        for (size_t c = 0; c < n_chunks; c++) total += chunk_lens[c];
+        if (total && !x) throw Error(19, "debug loudness stream: bad arguments");
+        SB_CUDA(cudaSetDevice(device));
+        std::unique_ptr<LoudnessStream> m(create_loudness_stream(nullptr, device, rate, target_lufs, max_gain_db));
+        loudness_stream_steps(*m, (long long)total, "debug loudness stream: ");
+        const long long S = m->d.S, steps = (long long)total / S;
+        DeviceBuffers d;
+        float* dx = d.upload(x, total, total + 1);
+        float* win = d.alloc<float>(total + (size_t)S + 1);
+        double* e = d.alloc<double>(8 * (size_t)steps + 8);
+        double* dl = d.alloc<double>((size_t)steps + 1);
+        float* dg = d.alloc<float>((size_t)steps + 1);
+        unsigned long long* dc = d.alloc<unsigned long long>(1);
+        LoudStreamSeg* ds = d.alloc<LoudStreamSeg>(1);
+        // chunk by chunk, each in its own launch, as passes feed a meter
+        size_t off = 0;
+        for (size_t c = 0; c < n_chunks; c++) {
+            const long long n = (long long)chunk_lens[c], nc = loudness_stream_steps(*m, n, "debug loudness stream: ");
+            LoudStreamSeg g = loudness_stream_seg(*m, dx + off, n, 1.f);
+            g.win = win; g.e = e; g.lufs = dl + m->steps; g.gains = dg + m->steps; g.clipped = dc;
+            SB_CUDA(cudaMemcpy(ds, &g, sizeof(g), cudaMemcpyHostToDevice));
+            launch_loudness_stream(ds, 1, 0);
+            SB_CUDA(cudaDeviceSynchronize());
+            std::vector<double> l((size_t)nc + 1);
+            std::vector<float> a((size_t)nc + 1);
+            unsigned long long clip = 0;
+            SB_CUDA(cudaMemcpy(l.data(), g.lufs, (size_t)nc * sizeof(double), cudaMemcpyDeviceToHost));
+            SB_CUDA(cudaMemcpy(a.data(), g.gains, (size_t)nc * sizeof(float), cudaMemcpyDeviceToHost));
+            SB_CUDA(cudaMemcpy(&clip, dc, sizeof(clip), cudaMemcpyDeviceToHost));
+            loudness_stream_advance(*m, n, l.data(), a.data(), clip);
+            off += (size_t)n;
+        }
+        if (total) SB_CUDA(cudaMemcpy(y, dx, total * 4, cudaMemcpyDeviceToHost));
+        SB_CUDA(cudaMemcpy(lufs_steps, dl, (size_t)steps * sizeof(double), cudaMemcpyDeviceToHost));
+        SB_CUDA(cudaMemcpy(gain_steps, dg, (size_t)steps * sizeof(float), cudaMemcpyDeviceToHost));
+        *clipped = m->clipped;
     });
 }
 

@@ -277,6 +277,23 @@ constexpr int LD_SCRATCH = 6;     // doubles per chunk: its 4 states, its sum of
 // One launch over nseg segments (blockIdx.x = segment): lufs[b] = the integrated loudness (-inf when no block passes the
 // gates), gain[b] = the gain applied to the segment (1 without a target).
 void launch_loudness(float* wav, const LoudSeg* segs, int nseg, double* scratch, double* lufs, float* gain, cudaStream_t st);
+// One chunk of a live loudness stream in a pass (kernels_misc.cu loudness_stream_kernel; the meter is loudness.cu's
+// LoudnessStream, the contract include/sonata_b200.h's sb200_loudness_stream_create).  y[0 .. n): the chunk's delivered
+// samples, metered and scaled in place.  cin / cout: the carry read and the one written, each the K-weighting state at
+// the meter's last complete step boundary (4 doubles) followed by the p < S samples since it (floats).  The window
+// (p + n samples) is staged in win; e holds 8 doubles per step it completes (nc = (p + n) / S).  q: the meter's step
+// energies, q[m0 + c] written for the completed steps.  lufs[c] / gains[c]: the reading and gain at boundary m0 + 1 + c.
+// a_prev / a_cur: the gains at boundaries m0 - 1 and m0; gain: the chunk's own gain, applied after the meter.
+struct LoudStreamSeg {
+    float* y; long long n;
+    const double* cin; double* cout;
+    double* q; float* win; double* e;
+    double* lufs; float* gains; unsigned long long* clipped;
+    long long m0; int p, S;
+    float a_prev, a_cur, target, max_gain_db, gain;
+    double k[10], AS[16];
+};
+void launch_loudness_stream(const LoudStreamSeg* segs, int nseg, cudaStream_t st);
 // Pitch and tempo of one segment (prosody.cu): x = wav[in_off, in_off + n) is time-stretched by alpha = pitch / tempo
 // (WSOLA: synthesis hop Hs, frame 2 Hs, search radius D, F frames whose offsets go to offsets[d_off ..)) into n1 samples
 // when `stretch`, then resampled by p into n2 samples when `pitch`.  The delivered signal is y[y_off, y_off + n2); with

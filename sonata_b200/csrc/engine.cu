@@ -587,18 +587,20 @@ struct ResamplePlan {
 };
 
 // Device tables of a resample launch and their pinned mirrors: the segments, identity posts (for a launch whose input
-// has no post-path, or for the i16 conversion of its output; out_gain[k], when given, is output k's gain there) and the
-// output segments, n_out samples at out_off.
+// has no post-path, or for the i16 conversion of its output; out_gain[k], when given, is output k's gain there, and
+// fixed_scale[k] its PcmPost::fixed_scale) and the output segments, n_out samples at out_off.
 struct ResampleTables {
     Staged<ResampleSeg> segs; Staged<PcmPost> posts; Staged<FrameSeg> osegs;
     void carve(Arena& dev, Arena& pin, size_t n) {
         segs.carve(dev, pin, n); posts.carve(dev, pin, n); osegs.carve(dev, pin, n);
     }
-    void upload(const ResamplePlan& p, cudaStream_t st, const std::vector<float>* out_gain = nullptr) {
+    void upload(const ResamplePlan& p, cudaStream_t st, const std::vector<float>* out_gain = nullptr,
+                const std::vector<int>* fixed_scale = nullptr) {
         for (size_t k = 0; k < p.segs.size(); k++) {
             segs.h[k] = p.segs[k];
             posts.h[k] = PcmPost();
             if (out_gain) posts.h[k].gain = (*out_gain)[k];
+            if (fixed_scale) posts.h[k].fixed_scale = (*fixed_scale)[k];
             osegs.h[k] = FrameSeg{0, (int)p.segs[k].n_out, 0, 0, p.segs[k].out_off};
         }
         segs.upload(st); posts.upload(st); osegs.upload(st);
@@ -769,6 +771,20 @@ struct FrameBufs {
     }
 };
 
+// The metered chunks of a chunk pass: chunks[q] has n[q] samples, its window at win_off[q] of the pass's window buffer
+// and the steps[q] steps it completes at step_off[q] of its step tables.
+struct MeterPlan {
+    std::vector<int> chunks;
+    std::vector<long long> n, win_off, step_off, steps;
+    long long win_total = 0, steps_total = 0;
+    void add(int k, const LoudnessStream& s, long long samples, long long completes) {
+        chunks.push_back(k); n.push_back(samples);
+        win_off.push_back(win_total); step_off.push_back(steps_total); steps.push_back(completes);
+        win_total += s.samples - s.steps * s.d.S + samples;
+        steps_total += completes;
+    }
+};
+
 // One pass of streaming decoder chunks (layout l): speaker biases of every slot, tables, the gather table and the
 // latent slices, the decoder (one buffer per stage for a debug pass) and the waveforms; the post-path table when an
 // output stage runs, the resample launch's tables and output, the i16 or G.711 scratch; and the pinned block the packed
@@ -790,8 +806,12 @@ struct ChunkBufs {
     ProsodyBufs pr;
     Staged<FormantSeg> fsegs; Staged<FormantCarry> fcarry; float* fwin = nullptr;
     Staged<FrameSeg> rin; Staged<PcmPost> rpost;
+    // metered chunks (plan `mp`): their entries, windows and step scratch, and the readings, gains and clamp counts
+    // they return
+    Staged<LoudStreamSeg> lsegs; float* lwin = nullptr; double* le = nullptr;
+    Staged<double> llufs; Staged<float> lgains; Staged<unsigned long long> lclip;
     void carve(Arena& dev, Arena& pin, const Voice& v, const FrameLayout& l, const ChunkPass& p, const ResamplePlan& rp,
-               const ProsodyPlan& pp, const FormantPlan& fp, size_t total) {
+               const ProsodyPlan& pp, const FormantPlan& fp, const MeterPlan& mp, size_t total) {
         const bool i16_out = p.format != PCM_F32;
         const size_t n = l.fsegs.size();
         spk.carve(dev, pin, v, l);
@@ -805,6 +825,13 @@ struct ChunkBufs {
             fwin = dev.get<float>((size_t)fp.in_total + 4);
         }
         if (!pp.segs.empty() || !fp.segs.empty()) { rin.carve(dev, pin, n); rpost.carve(dev, pin, n); }
+        if (!mp.chunks.empty()) {
+            const size_t m = mp.chunks.size(), steps = (size_t)std::max<long long>(mp.steps_total, 1);
+            lsegs.carve(dev, pin, m);
+            lwin = dev.get<float>((size_t)mp.win_total + 4);
+            le = dev.get<double>(8 * steps);
+            llufs.carve(dev, pin, steps); lgains.carve(dev, pin, steps); lclip.carve(dev, pin, m);
+        }
         dec.carve(dev, v, l.RY, p.debug);
         if (p.resample || i16_out) post.carve(dev, pin, n);
         rt.carve(dev, pin, rp.segs.size());
@@ -1574,11 +1601,12 @@ static void fill_fade(PcmPost& p, int fade, long long len) {
 // The chunks are laid out as the segments of one frame level.  The pass runs the decoder, then its output stage: the
 // prosody launches of the chunks with a pitch / tempo stream, which read the waveforms through the post-path, the
 // resample launch, which reads their output or the waveforms through the post-path, and the i16 (or G.711) conversion,
-// which applies the post-path itself when no resample launch ran.  The packed result comes back in one copy through the
-// context's page-locked staging, and only then do the resamplers and prosody streams advance.
+// which applies the post-path itself when no resample launch ran.  The loudness launch meters the resampled output of the
+// chunks with a meter in place, before the conversion.  The packed result comes back in one copy through the context's
+// page-locked staging, and only then do the resamplers, prosody streams and meters advance.
 void decode_chunks(Voice* v, const ChunkPass& p, ChunkResult& out) {
     out.f32.clear(); out.i16.clear(); out.g711.clear(); out.captures.clear();
-    out.ms = out.stretch_ms = out.pitch_ms = out.formant_ms = 0.f;
+    out.ms = out.stretch_ms = out.pitch_ms = out.formant_ms = out.loudness_ms = 0.f;
     const size_t n = p.chunks.size();
     if (n == 0) return;
     if (p.format < PCM_F32 || p.format > PCM_ALAW)
@@ -1617,6 +1645,17 @@ void decode_chunks(Voice* v, const ChunkPass& p, ChunkResult& out) {
                 if (p.chunks[q].ps == w)
                     fail(k, "the prosody stream of chunk " + std::to_string(q) + " appears twice in one call", "");
         }
+        if (const LoudnessStream* m = c.ls) {
+            if (!p.resample) fail(k, "a loudness stream needs a resampled chunk pass", "");
+            if (m->v != v) fail(k, "the loudness stream was made for another voice", "");
+            for (size_t q = 0; q < k; q++)
+                if (p.chunks[q].ls == m)
+                    fail(k, "the loudness stream of chunk " + std::to_string(q) + " appears twice in one call", "");
+            const long long rate = c.rs ? (long long)v->sample_rate * c.rs->f.up / c.rs->f.down : v->sample_rate;
+            if (rate != m->rate)
+                fail(k, "the chunk is delivered at " + std::to_string(rate) + " Hz and its loudness stream meters " +
+                            std::to_string(m->rate) + " Hz", "");
+        }
         if ((c.rs || c.ps) && c.last != 0 && c.last != 1)
             fail(k, "last flag " + std::to_string(c.last) + " is neither 0 nor 1", "");
     }
@@ -1650,6 +1689,13 @@ void decode_chunks(Voice* v, const ChunkPass& p, ChunkResult& out) {
         }
         if (p.resample) rp.add(c.rs ? &c.rs->f : nullptr, n_res[k], c.rs, c.last != 0);
     }
+    // metered chunks: what the resample launch delivers for them, and the steps that completes
+    MeterPlan mp;
+    for (size_t k = 0; k < n; k++)
+        if (LoudnessStream* m = p.chunks[k].ls) {
+            const long long d = rp.segs[k].n_out;
+            mp.add((int)k, *m, d, loudness_stream_steps(*m, d, "chunk " + std::to_string(k) + ": "));
+        }
 
     const auto release = [v](Context* c) { v->release(c); };
     const std::unique_ptr<Context, decltype(release)> ctx(v->acquire(), release);
@@ -1658,7 +1704,7 @@ void decode_chunks(Voice* v, const ChunkPass& p, ChunkResult& out) {
     lay_out_frames(l, len, hop, {});
     const size_t total = p.resample ? (size_t)rp.total : (size_t)l.total_samples;
     ChunkBufs b;
-    plan(C.dev_frame, C.pin, [&](Arena& dev, Arena& pin) { b.carve(dev, pin, *v, l, p, rp, pp, fp, total); });
+    plan(C.dev_frame, C.pin, [&](Arena& dev, Arena& pin) { b.carve(dev, pin, *v, l, p, rp, pp, fp, mp, total); });
     cudaStream_t st = C.stream;
     std::vector<Region> regions;
     Runner R(*v, C, regions, b.spk.cond);
@@ -1671,15 +1717,19 @@ void decode_chunks(Voice* v, const ChunkPass& p, ChunkResult& out) {
     run_decoder(R, LY, b.y, b.dec, b.s, b.wav);
     // G.711 of resampled chunks: the gain scales the resampled samples just before the conversion, as a volume on the
     // delivered audio (resampling x * g is not bit for bit resampling x, then times g)
+    // A metered chunk's gain applies after its meter, which the loudness launch does, and it converts at the fixed scale
     const bool gain_after = p.resample && p.format >= PCM_MULAW;
     std::vector<float> out_gain;
+    std::vector<int> fixed_scale;
     if (gain_after)
-        for (const ChunkSpec& c : p.chunks) out_gain.push_back(c.gain);
+        for (const ChunkSpec& c : p.chunks) out_gain.push_back(c.ls ? 1.f : c.gain);
+    if (!mp.chunks.empty())
+        for (const ChunkSpec& c : p.chunks) fixed_scale.push_back(c.ls ? 1 : 0);
     if (b.post.d) {
         for (size_t k = 0; k < n; k++) {
             PcmPost& q = b.post.h[k];
             q = PcmPost();
-            q.gain = gain_after ? 1.f : p.chunks[k].gain;
+            q.gain = gain_after || p.chunks[k].ls ? 1.f : p.chunks[k].gain;
             q.trim_lo = p.chunks[k].trim_lo * hop;
             q.trim_hi = p.chunks[k].trim_hi * hop;
             if (p.fade > 0) fill_fade(q, p.fade, n_in[k]);
@@ -1745,8 +1795,28 @@ void decode_chunks(Voice* v, const ChunkPass& p, ChunkResult& out) {
         rs_in = b.rin.d; rs_post = b.rpost.d;
     }
     if (p.resample) {
-        b.rt.upload(rp, st, gain_after ? &out_gain : nullptr);
+        b.rt.upload(rp, st, gain_after ? &out_gain : nullptr, fixed_scale.empty() ? nullptr : &fixed_scale);
         run_resample(R, rp, b.rt, b.wav, rs_in, rs_post, hop, b.rs);
+        if (!mp.chunks.empty()) {
+            double window = 0, samples = 0;
+            for (size_t q = 0; q < mp.chunks.size(); q++) {
+                const int k = mp.chunks[q];
+                LoudStreamSeg g = loudness_stream_seg(*p.chunks[k].ls, b.rs + rp.segs[k].out_off, mp.n[q],
+                                                      p.chunks[k].gain);
+                g.win = b.lwin + mp.win_off[q]; g.e = b.le + 8 * mp.step_off[q];
+                g.lufs = b.llufs.d + mp.step_off[q]; g.gains = b.lgains.d + mp.step_off[q]; g.clipped = b.lclip.d + q;
+                b.lsegs.h[q] = g;
+                window += (double)(g.p + g.n);
+                samples += (double)g.n;
+            }
+            b.lsegs.upload(st);
+            R.begin("loudness");
+            launch_loudness_stream(b.lsegs.d, (int)mp.chunks.size(), st);
+            // the window filtered twice; read, staged, read again and written
+            R.count(2.0 * 22.0 * window, 4.0 * (3.0 * window + samples));
+            R.end();
+            b.llufs.download(st); b.lgains.download(st); b.lclip.download(st);
+        }
         if (b.pcm) launch_pcm(b.rs, b.rt.osegs.d, b.rt.posts.d, (int)n, 1, rp.max_out, b.max, p.format, b.pcm, st);
     } else if (b.pcm) {
         launch_pcm(b.wav, b.y.fsegs.d, b.post.d, (int)n, hop, (long long)*std::max_element(len.begin(), len.end()) * hop,
@@ -1769,9 +1839,15 @@ void decode_chunks(Voice* v, const ChunkPass& p, ChunkResult& out) {
         r->ended = p.chunks[k].last != 0;
     }
     for (Region& g : regions) {
-        if (g.name != "stretch" && g.name != "pitch" && g.name != "formant") continue;
+        if (g.name != "stretch" && g.name != "pitch" && g.name != "formant" && g.name != "loudness") continue;
         cudaEventElapsedTime(&g.ms, g.e0, g.e1);
-        (g.name == "stretch" ? out.stretch_ms : g.name == "pitch" ? out.pitch_ms : out.formant_ms) = g.ms;
+        (g.name == "stretch" ? out.stretch_ms : g.name == "pitch" ? out.pitch_ms
+                                              : g.name == "formant" ? out.formant_ms : out.loudness_ms) = g.ms;
+    }
+    for (size_t q = 0; q < mp.chunks.size(); q++) {
+        LoudnessStream* m = p.chunks[mp.chunks[q]].ls;
+        loudness_stream_advance(*m, mp.n[q], b.llufs.h + mp.step_off[q], b.lgains.h + mp.step_off[q], b.lclip.h[q]);
+        m->last_ms = out.loudness_ms;
     }
     for (size_t k = 0; k < n; k++) {
         ProsodyStream* w = p.chunks[k].ps;

@@ -128,6 +128,41 @@ void loudness_design(long long rate, LoudSeg& s);
 // Checks targets t[0 .. B) (null: none): NaN is no target, anything else must be finite and in [-70, 0] LUFS, or the
 // call fails naming the utterance.  Returns whether some utterance has a target.
 bool check_loudness_targets(const float* t, size_t B);
+// One stream's live loudness meter (include/sonata_b200.h, sb200_loudness_stream_create): its voice (null for a test
+// hook's meter) and device, its delivered rate, target T and maximum gain M, the K-weighting design (d.S, d.k, d.AS);
+// on the device two carries read and written alternately (the state at the last complete step boundary, 4 doubles,
+// then the samples since it, S floats) and q of every complete step (LS_MAX_STEPS doubles), in one allocation; its
+// counts, the gains at its last two boundaries and its last reading, and its "loudness" time of the last pass.
+constexpr long long LS_MAX_STEPS = 1 << 16;
+struct Voice;
+struct LoudnessStream {
+    Voice* v = nullptr;
+    int device = 0;
+    long long rate = 0;
+    float target = 0.f, max_gain_db = 20.f;
+    LoudSeg d{};
+    void* mem = nullptr;
+    double* carry[2] = {nullptr, nullptr};
+    double* q = nullptr;
+    int cur = 0;
+    long long samples = 0, steps = 0, clipped = 0;
+    float a_prev = 1.f, a = 1.f;
+    double lufs = -INFINITY;
+    float last_ms = 0.f;
+    ~LoudnessStream();
+};
+// Checks T (finite, in [-70, 0]) and M (finite, in [0, 40]) and the rate, then allocates the meter's device state.
+LoudnessStream* create_loudness_stream(Voice* v, int device, long long rate, float target, float max_gain_db);
+// The steps a chunk of n more samples completes; throws OPERATION_ERROR prefixed by `who` when they would take the
+// meter past LS_MAX_STEPS.
+long long loudness_stream_steps(const LoudnessStream& s, long long n, const std::string& who);
+// The chunk entry of n samples at y with gain `gain` after the meter; the scratch pointers (win, e, lufs, gains,
+// clipped) are the caller's to set.
+LoudStreamSeg loudness_stream_seg(const LoudnessStream& s, float* y, long long n, float gain);
+// After the pass has synchronised: n samples more, the readings and gains of the boundaries it reached and the samples
+// it clamped; the carries swap.
+void loudness_stream_advance(LoudnessStream& s, long long n, const double* lufs, const float* gains,
+                             unsigned long long clipped);
 
 // Pitch and tempo (prosody.cu).  What one utterance of n samples at `rate` becomes with its two ratios: the WSOLA
 // frame sizes (synthesis hop Hs = rate / 100, frame N = 2 Hs, search radius D = rate / 160), the stretch factor
@@ -582,6 +617,7 @@ struct ChunkSpec {
     float gain = 1.f;                     // linear gain of the post-path
     Resampler* rs = nullptr;              // the chunk's stream (resample passes; null: none)
     ProsodyStream* ps = nullptr;          // the chunk's pitch / tempo stream (resample passes; null: none)
+    LoudnessStream* ls = nullptr;         // the chunk's live loudness meter (resample passes; null: none)
     int last = 0;                         // 1: the chunk ends its stream, which is flushed
 };
 // One frame-level decoder pass over chunks of latents of one voice; chunk k equals the same chunk decoded alone, bit for
@@ -591,7 +627,8 @@ struct ChunkSpec {
 // emitting every output it can (a chunk without one leaves at the voice's rate as the post-path leaves it); a resampler
 // may appear once per pass and must belong to the voice.  A chunk with a prosody stream (resample passes only) is warped
 // first, and what that stream emits is what the resampler, or the voice-rate copy, takes; the same rules hold for
-// prosody streams.  i16: to_i16_vec (samples.rs:51-75) normalised to each emitted
+// prosody streams.  A chunk with a loudness meter (resample passes only) is metered after all that, in place, and its
+// gain applies after the meter, in every format; its i16 / G.711 conversion is at the fixed scale.  i16: to_i16_vec (samples.rs:51-75) normalised to each emitted
 // chunk's own peak; mu-law / A-law: the G.711 bytes of those same i16 samples, from the same launches.  Every check runs
 // before any device work and any resampler changes; errors name the chunk, except with `single`, which keeps the
 // single-chunk entry point's messages.  With `debug` the decoder keeps one buffer per stage and every stage is copied
@@ -619,6 +656,7 @@ struct ChunkResult {
     float ms = 0;                             // the pass's device time
     float stretch_ms = 0, pitch_ms = 0;       // its "stretch" and "pitch" regions (0: none ran)
     float formant_ms = 0;                     // its "formant" region (0: none ran)
+    float loudness_ms = 0;                    // its "loudness" region (0: none ran)
     std::vector<ChunkCapture> captures;       // ChunkPass::debug only
 };
 void decode_chunks(Voice* v, const ChunkPass& p, ChunkResult& out);

@@ -819,6 +819,52 @@ __device__ __forceinline__ double ld_block_sum(double v, double* red) {
 
 __device__ __forceinline__ double ld_block_loudness(double z) { return -0.691 + 10.0 * log10(z); }
 
+// One step of the state chain: s <- A^S s + e, each row summed in a fixed order.
+__device__ __forceinline__ void ld_chain_step(const double* AS, const double* e, double* s) {
+    double t[4];
+#pragma unroll
+    for (int r = 0; r < 4; r++) {
+        double a = e[r];
+#pragma unroll
+        for (int q = 0; q < 4; q++) a = fma(AS[4 * r + q], s[q], a);
+        t[r] = a;
+    }
+#pragma unroll
+    for (int r = 0; r < 4; r++) s[r] = t[r];
+}
+
+// z_j of block j, whose four steps' energies are q[0], q[stride], q[2 stride], q[3 stride]; blk = 4S.
+__device__ __forceinline__ double ld_block_z(const double* q, long long stride, double blk) {
+    return (((q[0] + q[stride]) + q[2 * stride]) + q[3 * stride]) / blk;
+}
+
+// The gated integrated loudness of the nb blocks whose step energies are q[c * stride] (block j: steps j .. j + 3):
+// the absolute gate at -70 LUFS, the relative gate 10 LU under the mean of the blocks that pass it, each sum taken per
+// thread in stride order and then over the block in a fixed tree order.  -inf when no block passes.  Every thread of
+// the block calls it and gets the result.
+__device__ __forceinline__ double ld_gates(const double* q, long long stride, long long nb, double blk, double* red) {
+    double sum = 0.0, cnt = 0.0;
+    for (long long j = threadIdx.x; j < nb; j += LD_THREADS) {
+        const double z = ld_block_z(q + stride * j, stride, blk);
+        if (ld_block_loudness(z) > -70.0) { sum += z; cnt += 1.0; }
+    }
+    sum = ld_block_sum(sum, red);
+    cnt = ld_block_sum(cnt, red);
+    double L = -INFINITY;
+    if (cnt > 0.0) {
+        const double rel = ld_block_loudness(sum / cnt) - 10.0;
+        double sum2 = 0.0, cnt2 = 0.0;
+        for (long long j = threadIdx.x; j < nb; j += LD_THREADS) {
+            const double z = ld_block_z(q + stride * j, stride, blk), l = ld_block_loudness(z);
+            if (l > -70.0 && l > rel) { sum2 += z; cnt2 += 1.0; }
+        }
+        sum2 = ld_block_sum(sum2, red);
+        cnt2 = ld_block_sum(cnt2, red);
+        if (cnt2 > 0.0) L = ld_block_loudness(sum2 / cnt2);
+    }
+    return L;
+}
+
 __global__ void __launch_bounds__(LD_THREADS) loudness_kernel(float* __restrict__ wav, const LoudSeg* __restrict__ segs,
                                                               double* __restrict__ scratch, double* __restrict__ lufs,
                                                               float* __restrict__ gain) {
@@ -849,17 +895,8 @@ __global__ void __launch_bounds__(LD_THREADS) loudness_kernel(float* __restrict_
         for (long long c = 0; c + 1 < nch; c++) {
             double* d = sc + LD_SCRATCH * c;
             const double e[4] = {d[0], d[1], d[2], d[3]};
-            double t[4];
-#pragma unroll
-            for (int r = 0; r < 4; r++) {
-                double a = e[r];
-#pragma unroll
-                for (int q = 0; q < 4; q++) a = fma(G.AS[4 * r + q], s[q], a);
-                t[r] = a;
-            }
             d[0] = s[0]; d[1] = s[1]; d[2] = s[2]; d[3] = s[3];
-#pragma unroll
-            for (int r = 0; r < 4; r++) s[r] = t[r];
+            ld_chain_step(G.AS, e, s);
         }
         if (nch > 0) {
             double* d = sc + LD_SCRATCH * (nch - 1);
@@ -888,30 +925,7 @@ __global__ void __launch_bounds__(LD_THREADS) loudness_kernel(float* __restrict_
     peak = (float)red[LD_THREADS - 1];
     // (4) gates over the nb blocks
     const long long nb = n >= 4 * S ? (n - 4 * S) / S + 1 : 0;
-    const double blk = 4.0 * (double)S;
-    auto z_of = [&](long long j) {
-        const double* q = sc + LD_SCRATCH * j + 4;
-        return (((q[0] + q[LD_SCRATCH]) + q[2 * LD_SCRATCH]) + q[3 * LD_SCRATCH]) / blk;
-    };
-    double sum = 0.0, cnt = 0.0;
-    for (long long j = threadIdx.x; j < nb; j += LD_THREADS) {
-        const double z = z_of(j);
-        if (ld_block_loudness(z) > -70.0) { sum += z; cnt += 1.0; }
-    }
-    sum = ld_block_sum(sum, red);
-    cnt = ld_block_sum(cnt, red);
-    double L = -INFINITY;
-    if (cnt > 0.0) {
-        const double rel = ld_block_loudness(sum / cnt) - 10.0;
-        double sum2 = 0.0, cnt2 = 0.0;
-        for (long long j = threadIdx.x; j < nb; j += LD_THREADS) {
-            const double z = z_of(j), l = ld_block_loudness(z);
-            if (l > -70.0 && l > rel) { sum2 += z; cnt2 += 1.0; }
-        }
-        sum2 = ld_block_sum(sum2, red);
-        cnt2 = ld_block_sum(cnt2, red);
-        if (cnt2 > 0.0) L = ld_block_loudness(sum2 / cnt2);
-    }
+    const double L = ld_gates(sc + 4, LD_SCRATCH, nb, 4.0 * (double)S, red);
     // (5) the gain, never taking the peak above full scale
     float g = 1.f;
     if (!isnan(G.target) && L > -INFINITY && peak > 0.f) {
@@ -921,6 +935,97 @@ __global__ void __launch_bounds__(LD_THREADS) loudness_kernel(float* __restrict_
     if (threadIdx.x == 0) { lufs[blockIdx.x] = L; gain[blockIdx.x] = g; }
     if (g != 1.f)
         for (long long i = threadIdx.x; i < n; i += LD_THREADS) x[i] = __fmul_rn(x[i], g);
+}
+
+// ------------------------------------------------------------------ live loudness of a stream (one block per chunk)
+// The chunk continues its meter's signal: the carried partial step (p samples) and the chunk's n samples are staged
+// as one window, every step the window completes is filtered from zero state by one thread, thread 0 chains the states
+// from the carried one, and each step's q is summed again from its true state, exactly as loudness_kernel does it.
+// Then the readings at each step boundary the window reaches, the gains they give, and the ramp, scale and clamp of the
+// chunk in place; the carry of the next chunk goes to the other buffer.
+__global__ void __launch_bounds__(LD_THREADS) loudness_stream_kernel(const LoudStreamSeg* __restrict__ segs) {
+    __shared__ double red[LD_THREADS];
+    pdl_trigger(); pdl_wait();
+    const LoudStreamSeg& G = segs[blockIdx.x];
+    const long long n = G.n, S = G.S, p = G.p, w = p + n, nc = w / S, m0 = G.m0;
+    float* win = G.win;
+    double k[10];
+#pragma unroll
+    for (int i = 0; i < 10; i++) k[i] = G.k[i];
+    // (1) the window: the carried samples, then the chunk's
+    const float* tail = reinterpret_cast<const float*>(G.cin + 4);
+    for (long long i = threadIdx.x; i < w; i += LD_THREADS) win[i] = i < p ? tail[i] : G.y[i - p];
+    if (threadIdx.x == 0) *G.clipped = 0ull;
+    __syncthreads();
+    // (2) zero-state end states of the completed steps
+    for (long long c = threadIdx.x; c < nc; c += LD_THREADS) {
+        double s[4] = {0.0, 0.0, 0.0, 0.0};
+        float m;
+        kweight_run(win, c * S, (c + 1) * S, k, s, &m);
+        double* d = G.e + 8 * c;
+        d[0] = s[0]; d[1] = s[1]; d[2] = s[2]; d[3] = s[3];
+    }
+    __syncthreads();
+    // (3) true initial states from the carried one; the state at the new last boundary is carried
+    if (threadIdx.x == 0) {
+        double s[4] = {G.cin[0], G.cin[1], G.cin[2], G.cin[3]};
+        for (long long c = 0; c < nc; c++) {
+            double* d = G.e + 8 * c;
+            d[4] = s[0]; d[5] = s[1]; d[6] = s[2]; d[7] = s[3];
+            ld_chain_step(G.AS, d, s);
+        }
+        G.cout[0] = s[0]; G.cout[1] = s[1]; G.cout[2] = s[2]; G.cout[3] = s[3];
+    }
+    __syncthreads();
+    // (4) q of every completed step, and the samples past the last boundary into the carry
+    for (long long c = threadIdx.x; c < nc; c += LD_THREADS) {
+        const double* d = G.e + 8 * c;
+        double s[4] = {d[4], d[5], d[6], d[7]};
+        float m;
+        G.q[m0 + c] = kweight_run(win, c * S, (c + 1) * S, k, s, &m);
+    }
+    float* tail_out = reinterpret_cast<float*>(G.cout + 4);
+    for (long long i = nc * S + threadIdx.x; i < w; i += LD_THREADS) tail_out[i - nc * S] = win[i];
+    __syncthreads();
+    // (5) the reading and gain at every boundary m0 + 1 .. m0 + nc: the batch gates over blocks 0 .. m - 4 from m = 4
+    // on, the provisional mean before it; a boundary without a reading keeps the gain
+    const double amax = exp10((double)G.max_gain_db / 20.0);
+    float a = G.a_cur;
+    for (long long c = 1; c <= nc; c++) {
+        const long long m = m0 + c;
+        double L;
+        if (m >= 4) {
+            L = ld_gates(G.q, 1, m - 3, 4.0 * (double)S, red);
+        } else {
+            double sum = 0.0;
+            for (long long j = 0; j < m; j++) sum += G.q[j];
+            L = sum > 0.0 ? ld_block_loudness(sum / (double)(m * S)) : -INFINITY;
+            if (L <= -70.0) L = -INFINITY;
+        }
+        if (L > -INFINITY) a = (float)fmin(exp10(((double)G.target - L) / 20.0), amax);
+        if (threadIdx.x == 0) { G.lufs[c - 1] = L; G.gains[c - 1] = a; }
+    }
+    __syncthreads();
+    // (6) each sample's gain, ramped over its step from the gain at the step's start to the one at its end; then the
+    // clamp and the chunk's own gain
+    const auto a_at = [&](long long m) { return m == m0 - 1 ? G.a_prev : m == m0 ? G.a_cur : G.gains[m - m0 - 1]; };
+    unsigned long long clip = 0;
+    const float vol = G.gain;
+    for (long long i = threadIdx.x; i < n; i += LD_THREADS) {
+        const long long t = m0 * S + p + i, m = t / S;
+        float g;
+        if (m == 0) {
+            g = a_at(0);
+        } else {
+            const double a0 = (double)a_at(m - 1), a1 = (double)a_at(m);
+            g = (float)__dadd_rn(a0, __ddiv_rn(__dmul_rn(__dsub_rn(a1, a0), (double)(t - m * S + 1)), (double)S));
+        }
+        float v = __fmul_rn(win[p + i], g);
+        if (v > 1.f) { v = 1.f; clip++; }
+        else if (v < -1.f) { v = -1.f; clip++; }
+        G.y[i] = vol == 1.f ? v : __fmul_rn(v, vol);
+    }
+    if (clip) atomicAdd(G.clipped, clip);
 }
 
 // Frame-level input of a chunk pass: every row is a plain 16-byte copy of its segment's latent row or exact zeros, so a
@@ -1209,6 +1314,12 @@ void launch_resample(const float* wav, const FrameSeg* fsegs, const PcmPost* pos
 void launch_loudness(float* wav, const LoudSeg* segs, int nseg, double* scratch, double* lufs, float* gain, cudaStream_t st) {
     if (nseg <= 0) return;
     launch_pdl(loudness_kernel, dim3(nseg), dim3(LD_THREADS), 0, st, wav, segs, scratch, lufs, gain);
+    g_launch_count++;
+}
+
+void launch_loudness_stream(const LoudStreamSeg* segs, int nseg, cudaStream_t st) {
+    if (nseg == 0) return;
+    launch_pdl(loudness_stream_kernel, dim3(nseg), dim3(LD_THREADS), 0, st, segs);
     g_launch_count++;
 }
 

@@ -1,9 +1,11 @@
 // Host side of loudness normalisation: the K-weighting filter of ITU-R BS.1770-4 designed for any rate the way
 // libebur128 designs it (in double), the state recurrence of its two-biquad cascade raised to the gating step, and the
-// check of per-utterance targets.  The kernel is loudness_kernel (kernels_misc.cu).
+// check of per-utterance targets; and the live meters of streams.  The kernels are loudness_kernel and
+// loudness_stream_kernel (kernels_misc.cu).
 #include "engine.h"
 #include <algorithm>
 #include <cmath>
+#include <memory>
 
 namespace sb200 {
 
@@ -73,6 +75,67 @@ bool check_loudness_targets(const float* t, size_t B) {
         any = true;
     }
     return any;
+}
+
+LoudnessStream* create_loudness_stream(Voice* v, int device, long long rate, float target, float max_gain_db) {
+    if (!(std::isfinite(target) && target >= -70.f && target <= 0.f))
+        throw Error(19, "live loudness target " + std::to_string(target) + " LUFS is not a finite value in [-70, 0]");
+    if (!(std::isfinite(max_gain_db) && max_gain_db >= 0.f && max_gain_db <= 40.f))
+        throw Error(19, "live loudness maximum gain " + std::to_string(max_gain_db) +
+                            " dB is not a finite value in [0, 40]");
+    std::unique_ptr<LoudnessStream> s(new LoudnessStream());
+    loudness_design(rate, s->d);
+    s->v = v; s->device = device; s->rate = rate;
+    s->target = target; s->max_gain_db = max_gain_db;
+    // two carries of 4 doubles and S floats each, then q
+    const size_t carry = 4 + ((size_t)s->d.S + 1) / 2;
+    SB_CUDA(cudaSetDevice(device));
+    SB_CUDA(cudaMalloc(&s->mem, sizeof(double) * (2 * carry + (size_t)LS_MAX_STEPS)));
+    double* base = static_cast<double*>(s->mem);
+    SB_CUDA(cudaMemset(base, 0, sizeof(double) * 2 * carry));
+    s->carry[0] = base; s->carry[1] = base + carry;
+    s->q = base + 2 * carry;
+    return s.release();
+}
+
+LoudnessStream::~LoudnessStream() {
+    if (!mem) return;
+    cudaSetDevice(device);
+    cudaFree(mem);
+}
+
+long long loudness_stream_steps(const LoudnessStream& s, long long n, const std::string& who) {
+    const long long steps = (s.samples + n) / s.d.S;
+    if (steps > LS_MAX_STEPS)
+        throw Error(19, who + "the loudness stream would pass its capacity of " + std::to_string(LS_MAX_STEPS) +
+                            " steps of 100 ms (" + std::to_string(s.samples + n) + " samples at " +
+                            std::to_string(s.rate) + " Hz)");
+    return steps - s.steps;
+}
+
+LoudStreamSeg loudness_stream_seg(const LoudnessStream& s, float* y, long long n, float gain) {
+    LoudStreamSeg g{};
+    g.y = y; g.n = n;
+    g.cin = s.carry[s.cur]; g.cout = s.carry[1 - s.cur];
+    g.q = s.q;
+    g.m0 = s.steps; g.p = (int)(s.samples - s.steps * s.d.S); g.S = s.d.S;
+    g.a_prev = s.a_prev; g.a_cur = s.a;
+    g.target = s.target; g.max_gain_db = s.max_gain_db; g.gain = gain;
+    std::copy(s.d.k, s.d.k + 10, g.k);
+    std::copy(s.d.AS, s.d.AS + 16, g.AS);
+    return g;
+}
+
+void loudness_stream_advance(LoudnessStream& s, long long n, const double* lufs, const float* gains,
+                             unsigned long long clipped) {
+    const long long nc = (s.samples + n) / s.d.S - s.steps;
+    if (nc >= 2) s.a_prev = gains[nc - 2];
+    else if (nc == 1) s.a_prev = s.a;
+    if (nc >= 1) { s.a = gains[nc - 1]; s.lufs = lufs[nc - 1]; }
+    s.samples += n;
+    s.steps += nc;
+    s.clipped += (long long)clipped;
+    s.cur ^= 1;
 }
 
 }  // namespace sb200

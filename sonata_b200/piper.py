@@ -160,23 +160,38 @@ def _rate_array(rates, n: int):
     return out
 
 
-def _loudness_array(targets, n: int):
+def _loudness_array(targets, n: int, who: Optional[Sequence[str]] = None):
     """The C image of per-utterance loudness targets (f32, NaN for none), or None when `targets` is None or holds no
-    target.  targets[b] is a LUFS value, finite and in [-70, 0], or None / NaN (utterance b is measured only)."""
+    target.  targets[b] is a LUFS value, finite and in [-70, 0], or None / NaN (utterance b is measured only).  Errors
+    name who[b] (default "utterance b")."""
     if targets is None:
         return None
     out = np.full(n, np.nan, np.float32)
     for b, t in enumerate(_per_utterance(targets, n, "loudness targets")):
+        name = f"utterance {b}" if who is None else who[b]
         if t is None:
             continue
         if isinstance(t, bool) or not isinstance(t, numbers.Real):
-            raise OperationError(f"utterance {b}: loudness target {t!r} is not a number")
+            raise OperationError(f"{name}: loudness target {t!r} is not a number")
         if math.isnan(float(t)):
             continue
         if not (math.isfinite(float(t)) and -70.0 <= float(t) <= 0.0):
-            raise OperationError(f"utterance {b}: loudness target {float(t)} LUFS is not a finite value in [-70, 0]")
+            raise OperationError(f"{name}: loudness target {float(t)} LUFS is not a finite value in [-70, 0]")
         out[b] = float(t)
     return None if np.isnan(out).all() else out
+
+
+MAX_GAIN_RANGE = (0.0, 40.0)     # the maximum gains (dB) a live loudness meter may apply
+
+
+def _check_max_gain(max_gain_db, who: str) -> float:
+    """A live loudness meter's maximum gain in dB as a float: finite and in [0, 40], or the call fails naming `who`."""
+    if isinstance(max_gain_db, bool) or not isinstance(max_gain_db, numbers.Real):
+        raise OperationError(f"{who}: maximum gain {max_gain_db!r} is not a number")
+    g = float(max_gain_db)
+    if not (math.isfinite(g) and MAX_GAIN_RANGE[0] <= g <= MAX_GAIN_RANGE[1]):
+        raise OperationError(f"{who}: maximum gain {g} dB is not a finite value in [0, 40]")
+    return g
 
 
 PITCH_RANGE = (0.5, 2.0)     # pitch ratios a result can be shifted by
@@ -1247,6 +1262,95 @@ def _stream_prosody(model, pitch, tempo, pitch_contour=None, enc=None, formant=N
     return ProsodyStream(model, pitch, tempo, formant=phi)
 
 
+class LoudnessStream:
+    """One stream's live loudness meter on the device (sb200_loudness_stream_*): a causal ITU-R BS.1770 meter of
+    everything the stream has delivered so far drives a gain ramped across each 100 ms step, so the stream holds
+    `target` LUFS (finite, in [-70, 0]) without holding anything back.  `max_gain_db` (finite, in [0, 40]) caps the
+    gain; `output_rate` is the rate it meters (None: the voice's).  The first 100 ms play at gain 1, readings before
+    400 ms are provisional, and peaks are held by clamping to [-1, 1], not by a look-ahead limiter.  A meter may be
+    passed with the chunks of several sentences in turn: their signal just continues.  See include/sonata_b200.h."""
+
+    def __init__(self, model: "_VitsCommons", target, max_gain_db=20.0, output_rate: Optional[int] = None,
+                 who: str = "stream"):
+        t = _loudness_array([target], 1, [who])
+        if t is None:
+            raise OperationError(f"{who}: a live loudness stream needs a target in LUFS")
+        g = _check_max_gain(max_gain_db, who)
+        _rate_array([output_rate], 1)
+        self._m, self._h = model, C.c_void_p()
+        self.target, self.max_gain_db = float(t[0]), g
+        self.rate = int(output_rate) if output_rate else model.audio_output_info().sample_rate
+        err = N.sb200_error()
+        _check(model._lib.sb200_loudness_stream_create(model._h, int(output_rate or 0), self.target, g,
+                                                       C.byref(self._h), C.byref(err)), err)
+
+    def state(self) -> dict:
+        """{"lufs": the last reading (-inf before any), "gain": the last gain, "samples": samples metered, "clipped":
+        samples clamped}."""
+        lufs, gain, n, clipped = C.c_double(), C.c_float(), C.c_int64(), C.c_int64()
+        err = N.sb200_error()
+        _check(self._m._lib.sb200_loudness_stream_state(self._h, C.byref(lufs), C.byref(gain), C.byref(n),
+                                                        C.byref(clipped), None, C.byref(err)), err)
+        return {"lufs": float(lufs.value), "gain": float(gain.value), "samples": int(n.value),
+                "clipped": int(clipped.value)}
+
+    @property
+    def last_pass_ms(self) -> float:
+        """The "loudness" device time (ms) of the last chunk pass this meter was in."""
+        ms, err = C.c_float(), N.sb200_error()
+        _check(self._m._lib.sb200_loudness_stream_state(self._h, None, None, None, None, C.byref(ms), C.byref(err)),
+               err)
+        return float(ms.value)
+
+    def __del__(self):
+        try:
+            if self._h:
+                self._m._lib.sb200_loudness_stream_free(self._h)
+                self._h = None
+        except Exception:
+            pass
+
+
+def _stream_meter(model, live_loudness, max_gain_db, output_rate, who: str) -> Optional[LoudnessStream]:
+    """The meter of a stream with `live_loudness` (None: none; a target in LUFS: a fresh meter; a LoudnessStream: that
+    meter, continued), checked against the stream's output rate.  Errors name `who`."""
+    if live_loudness is None:
+        return None
+    if isinstance(live_loudness, LoudnessStream):
+        rate = int(output_rate) if output_rate else model.audio_output_info().sample_rate
+        if live_loudness._m is not model or not live_loudness._h:
+            raise OperationError(f"{who}: the loudness stream was made for another voice")
+        if live_loudness.rate != rate:
+            raise OperationError(f"{who}: the loudness stream meters {live_loudness.rate} Hz and the stream is "
+                                 f"delivered at {rate} Hz")
+        return live_loudness
+    return LoudnessStream(model, live_loudness, 20.0 if max_gain_db is None else max_gain_db, output_rate, who)
+
+
+def _check_live_loudness(live_loudness, max_gain_db, encoding, who: str) -> None:
+    """The checks of a stream's live loudness that need no device: its target, its maximum gain, and an encoding that
+    can be metered (FLAC cannot stream)."""
+    if live_loudness is None:
+        if max_gain_db is not None:
+            raise OperationError(f"{who}: a maximum gain is the cap of a live loudness meter: give live_loudness")
+        return
+    if encoding == "flac":
+        raise OperationError(f"{who}: live loudness cannot meter FLAC, which does not stream")
+    if not isinstance(live_loudness, LoudnessStream):
+        if _loudness_array([live_loudness], 1, [who]) is None:
+            raise OperationError(f"{who}: live loudness target {live_loudness!r} is not a target in LUFS")
+    elif max_gain_db is not None:
+        raise OperationError(f"{who}: a LoudnessStream keeps its own maximum gain")
+    if max_gain_db is not None:
+        _check_max_gain(max_gain_db, who)
+
+
+def refuse_live_loudness(live_loudness, where: str) -> None:
+    """Models without device streaming cannot meter a stream."""
+    if live_loudness is not None:
+        raise OperationError(f"{where}: live loudness needs a streaming voice of this library")
+
+
 def _delivered_bounds(warp: Optional[ProsodyStream], resampler: Optional["Resampler"]):
     """A contoured stream's per-id delivered ends at its delivered rate: ceil(end * up / down) with an output rate, as
     the batch alignments place them; None for a stream without a contour."""
@@ -1268,8 +1372,9 @@ class SpeechStreamer:
 
     def __init__(self, enc: EncoderOutputs, chunk_size: int, chunk_padding: int,
                  resampler: Optional[Resampler] = None, encoding: Optional[str] = None, gain: float = 1.0,
-                 warp: Optional[ProsodyStream] = None):
+                 warp: Optional[ProsodyStream] = None, meter: Optional[LoudnessStream] = None):
         self.enc = enc
+        self.meter = meter
         self.chunker = AdaptiveMelChunker(enc.num_frames, chunk_size, chunk_padding)
         self.one_shot = enc.num_frames <= (chunk_size * 2 + chunk_padding * 2)
         self.resampler = resampler
@@ -1288,7 +1393,7 @@ class SpeechStreamer:
     def __next__(self) -> AudioSamples:
         (m0, m1), (a0, a1) = next(self.chunker)
         # encoded, resampled or warped: the post-path runs on the device, then the stream's resampler / prosody stream
-        if self.encoding is not None or self.resampler is not None or self.warp is not None:
+        if self.encoding is not None or self.resampler is not None or self.warp is not None or self.meter is not None:
             if self.one_shot:
                 self.chunker.consume()
                 chunk, fade = (self.enc, 0, self.enc.num_frames, 0, 0), 0
@@ -1296,11 +1401,13 @@ class SpeechStreamer:
                 hi = self.enc.num_frames if m1 is None else m1
                 chunk, fade = (self.enc, m0, hi) + _trim_frames(slice(a0, a1)), 42
             kw = {}
-            if self.resampler is not None or self.warp is not None:     # whether this chunk ends the stream: after
-                kw.update(resamplers=[self.resampler],                  # the one-shot consume()
-                          last=[self.chunker.last_end_index is None])
+            if self.resampler is not None or self.warp is not None or self.meter is not None:
+                kw.update(resamplers=[self.resampler],                  # whether this chunk ends the stream: after
+                          last=[self.chunker.last_end_index is None])   # the one-shot consume()
             if self.warp is not None:
                 kw["warps"] = [self.warp]
+            if self.meter is not None:
+                kw["meters"] = [self.meter]
             if self.encoding is not None:
                 kw.update(gains=[self.gain], encoding=self.encoding)
             return self.enc._m.infer_decoder_batch([chunk], fade=fade, **kw)[0]
@@ -1370,7 +1477,7 @@ class VitsStreamingModel(_VitsCommons):
     def infer_decoder_batch(self, chunks: Sequence[tuple], pcm16: bool = False, fade: int = 0,
                             gains: Optional[Sequence[float]] = None, resamplers: Optional[Sequence] = None,
                             last: Optional[Sequence[bool]] = None, encoding: Optional[str] = None,
-                            warps: Optional[Sequence] = None) -> list:
+                            warps: Optional[Sequence] = None, meters: Optional[Sequence] = None) -> list:
         """Many `EncoderOutputs.infer_decoder(lo, hi)` calls as one decoder pass.  `chunks`: (encoder outputs, lo, hi)
         per chunk; each result equals that chunk decoded alone, bit for bit.
 
@@ -1389,7 +1496,11 @@ class VitsStreamingModel(_VitsCommons):
 
         With `warps` (one ProsodyStream or None per chunk; chunks may carry trims, as with resamplers), chunk k after
         the post-path is appended to its prosody stream first, and what that emits goes on to resamplers[k] (None
-        entries, or resamplers None: the voice's rate) and the conversion; last[k] flushes both streams."""
+        entries, or resamplers None: the voice's rate) and the conversion; last[k] flushes both streams.
+
+        With `meters` (one LoudnessStream or None per chunk; chunks may carry trims, as with resamplers), what chunk k
+        delivers is metered by its live loudness stream after all that, gains[k] applies after the meter, and pcm16 /
+        G.711 convert it at the fixed scale (sb200_decode_chunks_metered)."""
         refuse_flac(encoding, "a decoder chunk pass")
         check_encoding(encoding)
         if encoding is not None and pcm16:
@@ -1399,7 +1510,8 @@ class VitsStreamingModel(_VitsCommons):
         tlo, thi = np.zeros(n, np.int64), np.zeros(n, np.int64)
         hs = (C.c_void_p * n)()
         for k, c in enumerate(chunks):
-            if len(c) not in ((3, 5) if pcm16 or encoding or resamplers is not None or warps is not None else (3,)):
+            if len(c) not in ((3, 5) if pcm16 or encoding or resamplers is not None or warps is not None
+                              or meters is not None else (3,)):
                 raise OperationError(f"Invalid decoder chunk {k}: expected (encoder outputs, lo, hi"
                                      + (", trim_lo, trim_hi)" if pcm16 else ")"))
             enc = c[0]
@@ -1415,7 +1527,7 @@ class VitsStreamingModel(_VitsCommons):
             return []
         p64 = lambda a: a.ctypes.data_as(C.POINTER(C.c_int64))
         err = N.sb200_error()
-        if resamplers is not None or warps is not None:
+        if resamplers is not None or warps is not None or meters is not None:
             resamplers = _per_utterance([None] * n if resamplers is None else resamplers, n, "resamplers")
             rs = (C.c_void_p * n)()
             for k, r in enumerate(resamplers):
@@ -1429,6 +1541,13 @@ class VitsStreamingModel(_VitsCommons):
                     if w is not None and (not isinstance(w, ProsodyStream) or not w._h):
                         raise OperationError(f"chunk {k}: not a ProsodyStream")
                     ws[k] = None if w is None else w._h.value
+            ms = None
+            if meters is not None:
+                ms = (C.c_void_p * n)()
+                for k, m in enumerate(_per_utterance(meters, n, "meters")):
+                    if m is not None and (not isinstance(m, LoudnessStream) or not m._h):
+                        raise OperationError(f"chunk {k}: not a LoudnessStream")
+                    ms[k] = None if m is None else m._h.value
             fl = np.zeros(n, np.int32) if last is None else np.array([1 if x else 0 for x in
                                                                         _per_utterance(last, n, "last flags")], np.int32)
             g = None if gains is None else np.ascontiguousarray(gains, dtype=np.float32)
@@ -1436,7 +1555,11 @@ class VitsStreamingModel(_VitsCommons):
             lens = (C.c_size_t * n)()
             fmt = G711_LAW[encoding] + 2 if encoding else 1 if pcm16 else 0
             gp = None if g is None else g.ctypes.data_as(C.POINTER(C.c_float))
-            if ws is None:
+            if ms is not None:
+                _check(self._lib.sb200_decode_chunks_metered(
+                    self._h, hs, p64(lo), p64(hi), p64(tlo), p64(thi), n, int(fade), gp, rs, ws, ms,
+                    _ptr(fl, C.c_int32), fmt, outs, lens, C.byref(err)), err)
+            elif ws is None:
                 _check(self._lib.sb200_decode_chunks_resampled(
                     self._h, hs, p64(lo), p64(hi), p64(tlo), p64(thi), n, int(fade), gp, rs, _ptr(fl, C.c_int32), fmt,
                     outs, lens, C.byref(err)), err)
@@ -1477,7 +1600,8 @@ class VitsStreamingModel(_VitsCommons):
                          encoding: Optional[str] = None, gain: Optional[float] = None,
                          pitch: Optional[float] = None, tempo: Optional[float] = None,
                          pitch_contour: Optional[Sequence] = None,
-                         formant_ratio: Optional[float] = None, speaker_blend=None) -> SpeechStreamer:
+                         formant_ratio: Optional[float] = None, speaker_blend=None,
+                         live_loudness=None, max_gain_db: Optional[float] = None) -> SpeechStreamer:
         """`formant_ratio`: as for infer_batch_with_values' formants, on top of `pitch` / `tempo` / `pitch_contour` or
         alone, the sentence's formant stage carried as one stream on the device (ProsodyStream): the concatenation of
         the chunks is the formant stage applied at once to the sentence the stream yields without it, then resampled and
@@ -1494,8 +1618,13 @@ class VitsStreamingModel(_VitsCommons):
         `pitch_contour`: one pitch ratio per character of `phonemes` (as for speak_batch_with_alignment), applied to
         that character's id and pad; it combines with `tempo` but not with `pitch`.  The concatenation of the chunks is
         the sentence the stream yields without it, with that contour applied at once (sb200_debug_prosody_contour), and
-        the streamer's `bounds` give each id's delivered end."""
+        the streamer's `bounds` give each id's delivered end.
+        `live_loudness`: a target in LUFS, for a fresh live loudness meter (LoudnessStream, capped at `max_gain_db`,
+        default 20), or a LoudnessStream to continue (a request's meter across its sentences).  What the stream
+        delivers is metered and scaled on the device as it leaves, holding nothing back; `gain` applies after the
+        meter, and G.711 is taken at the fixed scale."""
         if not isinstance(self, VitsStreamingModel):
+            refuse_live_loudness(live_loudness, "stream_synthesis")
             refuse_formants(formant_ratio, "stream_synthesis")
             refuse_prosody(pitch, tempo, "stream_synthesis")
             refuse_contour(pitch_contour, "stream_synthesis")
@@ -1503,6 +1632,7 @@ class VitsStreamingModel(_VitsCommons):
         pit, _ = _prosody_arrays([pitch], [tempo], 1)
         _seed_arrays([seed], 1)
         _rate_array([output_rate], 1)
+        _check_live_loudness(live_loudness, max_gain_db, encoding, "stream")
         refuse_flac(encoding, "stream_synthesis")
         g = _stream_gain(encoding, gain)
         blended = _blend_arrays(self, [speaker_blend], 1, ["stream"])[0] is not None
@@ -1517,8 +1647,9 @@ class VitsStreamingModel(_VitsCommons):
             enc = self.infer_encoder_batch([ids], seeds=[seed], speaker_blends=[speaker_blend])[0]
         else:
             enc = self.infer_encoder(ids) if seed is None else self.infer_encoder_batch([ids], seeds=[seed])[0]
+        meter = _stream_meter(self, live_loudness, max_gain_db, output_rate, "stream")
         return SpeechStreamer(enc, chunk_size, chunk_padding, _stream_resampler(self, output_rate), encoding, g,
-                              _stream_prosody(self, pitch, tempo, contour, enc, phi))
+                              _stream_prosody(self, pitch, tempo, contour, enc, phi), meter)
 
 
 def _stream_gain(encoding, gain) -> float:
@@ -1535,8 +1666,10 @@ class _Stream:
     """One sentence of a StreamBatch: its latent and its own chunk schedule, with SpeechStreamer's one-shot rule."""
 
     def __init__(self, key, enc, chunk_size: int, chunk_padding: int, resampler: Optional[Resampler] = None,
-                 encoding: Optional[str] = None, gain: float = 1.0, warp: Optional[ProsodyStream] = None):
+                 encoding: Optional[str] = None, gain: float = 1.0, warp: Optional[ProsodyStream] = None,
+                 meter: Optional[LoudnessStream] = None):
         self.key, self.enc, self.resampler = key, enc, resampler
+        self.meter = meter
         self.encoding, self.gain = encoding, gain
         self.warp = warp
         self.bounds = _delivered_bounds(warp, resampler)
@@ -1587,7 +1720,8 @@ class StreamBatch:
         self.model = model
         self.chunk_size, self.chunk_padding = chunk_size, chunk_padding
         self._pending: list = []      # (key, ids, config, chunk_size, seed, output rate, encoding, gain, pitch, tempo,
-                                      # per-id contour, speaker blend, formant ratio) not encoded yet
+                                      # per-id contour, speaker blend, formant ratio, live loudness, maximum gain) not
+                                      # encoded yet
         self._active: List[_Stream] = []
         self._retired: dict = {}      # key -> delivered ends (None: no contour) of the streams the last step ended
         self._next_key = 0
@@ -1596,7 +1730,7 @@ class StreamBatch:
             output_rate: Optional[int] = None, encoding: Optional[str] = None, gain: Optional[float] = None,
             pitch: Optional[float] = None, tempo: Optional[float] = None,
             pitch_contour: Optional[Sequence] = None, formant_ratio: Optional[float] = None,
-            speaker_blend=None) -> int:
+            speaker_blend=None, live_loudness=None, max_gain_db: Optional[float] = None) -> int:
         """`seed`: the stream's noise seed (see infer_batch_with_values); a seeded stream yields what
         `stream_synthesis(..., seed=seed)` yields, whatever other streams share its encoder pass.  `output_rate`,
         `encoding` and `gain`: the stream's sample rate and G.711 encoding, as for stream_synthesis; `pitch` / `tempo`:
@@ -1606,20 +1740,32 @@ class StreamBatch:
         warped stream's chunks go through passes of their own, so the other streams keep their passes and their
         bits.  `formant_ratio`: the stream's formant ratio, as for stream_synthesis; it is checked here, naming the
         stream, and a stream with one is warped (in those passes) even without pitch or tempo.  `speaker_blend`: the
-        stream's speaker blend, as for stream_synthesis; it replaces its config's speaker and is checked here."""
+        stream's speaker blend, as for stream_synthesis; it replaces its config's speaker and is checked here.
+        `live_loudness` / `max_gain_db`: the stream's live loudness, as for stream_synthesis; a LoudnessStream that an
+        unfinished stream of this batch already carries is refused.  Metered streams go through passes of their own,
+        so the other streams keep their passes and their bits."""
         if not isinstance(self.model, VitsStreamingModel):
+            refuse_live_loudness(live_loudness, "StreamBatch")
             refuse_formants(formant_ratio, "StreamBatch")
             refuse_prosody(pitch, tempo, "StreamBatch")
             refuse_contour(pitch_contour, "StreamBatch")
         return self._add(ids_or_phonemes, config, self.chunk_size, seed, output_rate, encoding, gain, pitch, tempo,
-                         pitch_contour, speaker_blend, formant_ratio)
+                         pitch_contour, speaker_blend, formant_ratio, live_loudness, max_gain_db)
 
     def _add(self, ids_or_phonemes, config, chunk_size: int, seed: Optional[int] = None,
              output_rate: Optional[int] = None, encoding: Optional[str] = None, gain: Optional[float] = None,
              pitch: Optional[float] = None, tempo: Optional[float] = None, pitch_contour=None,
-             speaker_blend=None, formant_ratio=None) -> int:
+             speaker_blend=None, formant_ratio=None, live_loudness=None, max_gain_db=None) -> int:
         if config is not None and not isinstance(config, PiperSynthesisConfig):
             raise OperationError("Invalid configuration for Vits Model")
+        who = f"stream {self._next_key}"
+        _check_live_loudness(live_loudness, max_gain_db, encoding, who)
+        if isinstance(live_loudness, LoudnessStream):
+            if any(p[13] is live_loudness for p in self._pending) or any(s.meter is live_loudness
+                                                                         for s in self._active):
+                raise OperationError(f"{who}: the LoudnessStream is already carried by an unfinished stream of this "
+                                     "batch")
+            _stream_meter(self.model, live_loudness, None, output_rate, who)
         _blend_arrays(self.model, [speaker_blend], 1, [f"stream {self._next_key}"])
         phi = _stream_formant(formant_ratio, f"stream {self._next_key}")
         pit, _ = _prosody_arrays([pitch], [tempo], 1)
@@ -1646,7 +1792,7 @@ class StreamBatch:
         key = self._next_key
         self._next_key += 1
         self._pending.append((key, ids, config, chunk_size, seed, output_rate, encoding, gain, pitch, tempo, contour,
-                              speaker_blend, phi))
+                              speaker_blend, phi, live_loudness, max_gain_db))
         return key
 
     def bounds(self, key) -> Optional[np.ndarray]:
@@ -1691,30 +1837,34 @@ class StreamBatch:
                     try:
                         active.append(_Stream(p[0], enc, p[3], self.chunk_padding,
                                               _stream_resampler(self.model, p[5]), p[6], p[7],
-                                              _stream_prosody(self.model, p[8], p[9], p[10], enc, p[12])))
+                                              _stream_prosody(self.model, p[8], p[9], p[10], enc, p[12]),
+                                              _stream_meter(self.model, p[13], p[14], p[5], f"stream {p[0]}")))
                         continue
                     except SonataError as e:
                         err = e
                 out.append((p[0], err))
         plan = [(s,) + s.next_chunk() for s in active]
         failed = set()
-        # one pass per (encoding, resampled, one-shot, warped): the streams without an encoding first, in their usual
-        # passes; warped streams in passes of their own
-        plain_key = (None, False, False, False)
-        groups = {plain_key: [], (None, True, False, False): [], (None, True, True, False): []}
+        # one pass per (encoding, resampled, one-shot, warped, metered): the streams without an encoding first, in
+        # their usual passes; warped and metered streams in passes of their own
+        plain_key = (None, False, False, False, False)
+        groups = {plain_key: [], (None, True, False, False, False): [], (None, True, True, False, False): []}
         for p in plan:
             s = p[0]
-            plain = s.encoding is None and s.resampler is None and s.warp is None
-            k = plain_key if plain else (s.encoding, s.resampler is not None, p[3] is None, s.warp is not None)
+            plain = s.encoding is None and s.resampler is None and s.warp is None and s.meter is None
+            k = plain_key if plain else (s.encoding, s.resampler is not None, p[3] is None, s.warp is not None,
+                                         s.meter is not None)
             groups.setdefault(k, []).append(p)
 
         def device_post(pl, key):
-            encoding, resampled, whole, warped = key
+            encoding, resampled, whole, warped, metered = key
             chunks = [(s.enc, lo, hi) + ((0, 0) if trim is None else _trim_frames(trim)) for s, lo, hi, trim in pl]
-            extra = {} if not (resampled or warped) else {"resamplers": [p[0].resampler for p in pl],
-                                                          "last": [p[0].done for p in pl]}
+            extra = {} if not (resampled or warped or metered) else {"resamplers": [p[0].resampler for p in pl],
+                                                                     "last": [p[0].done for p in pl]}
             if warped:
                 extra["warps"] = [p[0].warp for p in pl]
+            if metered:
+                extra["meters"] = [p[0].meter for p in pl]
             if encoding is not None:
                 extra.update(encoding=encoding, gains=[p[0].gain for p in pl])
             return self.model.infer_decoder_batch(chunks, fade=0 if whole else 42, **extra)
@@ -1733,7 +1883,7 @@ class StreamBatch:
                 out.append((s.key, err))
                 failed.add(s.key)
                 continue
-            if trim is not None and s.resampler is None and s.encoding is None and s.warp is None:
+            if trim is not None and s.resampler is None and s.encoding is None and s.warp is None and s.meter is None:
                 a = AudioSamples(a.as_slice()[trim])
                 a.crossfade(42)
             out.append((s.key, a))

@@ -164,6 +164,21 @@ def _stream_prosody_extra(model, pitch_ratio, tempo, where: str, formant_ratio=N
     return out
 
 
+def _request_meter(model, live_loudness, max_gain_db, output_rate, encoding, where: str, who: str):
+    """The live loudness meter of a streaming request (None without a target): one piper.LoudnessStream at the
+    request's output rate, carried across its sentences.  Models that are not this library's streaming voices refuse
+    it by name."""
+    from .piper import LoudnessStream, VitsStreamingModel, _check_live_loudness, refuse_live_loudness
+    if not isinstance(model, VitsStreamingModel):
+        refuse_live_loudness(live_loudness, where)
+    _check_live_loudness(live_loudness, max_gain_db, encoding, who)
+    if live_loudness is None:
+        return None
+    if isinstance(live_loudness, LoudnessStream):
+        raise OperationError(f"{who}: a request makes its own meter: give live_loudness as a target in LUFS")
+    return LoudnessStream(model, live_loudness, 20.0 if max_gain_db is None else max_gain_db, output_rate or None, who)
+
+
 def _device_g711(model) -> bool:
     """Whether `model` encodes G.711 on the device (VitsModel / VitsStreamingModel).  Other SonataModels (fakes in
     tests) get the host definition, AudioSamples.as_g711_bytes, of the audio they return."""
@@ -302,15 +317,22 @@ class SonataSpeechSynthesizer:
                             seed: Optional[int] = None, output_rate: Optional[int] = None,
                             encoding: Optional[str] = None, pitch_ratio: Optional[float] = None,
                             tempo: Optional[float] = None, formant_ratio: Optional[float] = None,
-                            speaker_blend=None) -> Iterator[AudioSamples]:
+                            speaker_blend=None, live_loudness: Optional[float] = None,
+                            max_gain_db: Optional[float] = None) -> Iterator[AudioSamples]:
         """RealtimeSpeechStream (:337-382): a background producer pushes chunks into an unbounded channel;
         chunk_size is multiplied by the number of chunks already produced for every following sentence.
         `output_rate`: each sentence is resampled as its own stream (zero history at its start, flushed at its end).
         `encoding`: every chunk is G.711 bytes of its to_i16_vec after the volume, encoded on the device.
         `pitch_ratio` / `tempo`: every sentence warped as its own stream on the device (a fresh piper.ProsodyStream,
         flushed at its end); appended silence is not warped.  `formant_ratio`: every sentence's formant stage carried
-        as its own stream on the device, with or without the ratios (see stream_synthesis)."""
+        as its own stream on the device, with or without the ratios (see stream_synthesis).  `live_loudness`: a target
+        in LUFS that one live loudness meter (piper.LoudnessStream, capped at `max_gain_db`, default 20) holds the
+        request to, carried across its sentences; appended silence is not metered, and the volume applies after the
+        meter (G.711 is then taken at the fixed scale)."""
         pros = _stream_prosody_extra(self.model, pitch_ratio, tempo, "synthesize_streamed", formant_ratio)
+        refuse_flac(encoding, "synthesize_streamed")
+        meter = _request_meter(self.model, live_loudness, max_gain_db, output_rate, encoding, "synthesize_streamed",
+                               "request")
         sentence_seed(seed, 0)
         _check_output_rate(output_rate)
         refuse_flac(encoding, "synthesize_streamed")
@@ -327,6 +349,8 @@ class SonataSpeechSynthesizer:
         rate.update(pros)
         if _blend_extra(self.model, 1, speaker_blend, "request"):
             rate["speaker_blend"] = speaker_blend
+        if meter is not None:
+            rate["live_loudness"] = meter
         extra = lambda i: dict(rate) if seed is None else dict(rate, seed=sentence_seed(seed, i))
 
         def emit(chunk):
@@ -477,13 +501,16 @@ class RealtimeBatch:
     def add(self, text: str, output_config: Optional[AudioOutputConfig] = None, config=None,
             seed: Optional[int] = None, output_rate: Optional[int] = None, encoding: Optional[str] = None,
             pitch_ratio: Optional[float] = None, tempo: Optional[float] = None,
-            formant_ratio: Optional[float] = None, speaker_blend=None) -> int:
+            formant_ratio: Optional[float] = None, speaker_blend=None, live_loudness: Optional[float] = None,
+            max_gain_db: Optional[float] = None) -> int:
         """`seed`: the request's noise seed, `output_rate` its sample rate and `encoding` its G.711 encoding, as for
         synthesize_streamed, and `pitch_ratio` / `tempo` its ratios, each sentence warped as its own stream, as there.
         `formant_ratio` its formant ratio, as there.  `speaker_blend`: the request's speaker blend, as for
-        synthesize_streamed; it replaces the config's speaker and is checked here, naming the request."""
+        synthesize_streamed; it replaces the config's speaker and is checked here, naming the request.
+        `live_loudness` / `max_gain_db`: the request's live loudness, one meter across its sentences, as there."""
         from .piper import PiperSynthesisConfig
         pros = _stream_prosody_extra(self.model, pitch_ratio, tempo, "RealtimeBatch", formant_ratio)
+        refuse_flac(encoding, "RealtimeBatch")
         sentence_seed(seed, 0)
         _check_output_rate(output_rate)
         refuse_flac(encoding, "RealtimeBatch")
@@ -500,6 +527,8 @@ class RealtimeBatch:
             raise OperationError("Failed to run model inference. Error: empty input sequence")
         req = _Request(self._next_key, ids, output_config, config, self.chunk_size, seed, output_rate or None, encoding)
         req.prosody, req.blend = pros, speaker_blend
+        req.meter = _request_meter(self.model, live_loudness, max_gain_db, output_rate, encoding, "RealtimeBatch",
+                                   f"request {req.key}")
         self._next_key += 1
         self._start_sentence(req)
         return req.key
@@ -517,6 +546,8 @@ class RealtimeBatch:
         rate.update(req.prosody)
         if req.blend is not None:
             rate["speaker_blend"] = req.blend
+        if req.meter is not None:
+            rate["live_loudness"] = req.meter
         self._by_stream[self._streams._add(req.ids[req.next], req.config, req.cs, sentence_seed(req.seed, req.next),
                                            **rate)] = req
         req.next += 1
