@@ -158,6 +158,39 @@ struct DeviceBuffers {
     }
 };
 
+// The output stage of a debug hook's plan o run on stream 0 over the n samples at x, one segment at hop 1 read plainly,
+// with its buffers carved from arenas of the call's own, freed however the call ends.  taps (when given): the filter
+// the plan's resample segments read, put on the device here.  The stage has finished when the constructor returns.
+struct HookStage {
+    struct Arenas {
+        Arena dev, pin{true};
+        ~Arenas() { dev.release(); pin.release(); }
+    } a;
+    OutputBufs b;
+    Wave out;
+    HookStage(OutputPlan& o, const float* x, size_t n, const std::vector<float>& taps = {}) {
+        Staged<FrameSeg> seg; Staged<PcmPost> post; float* dt = nullptr;
+        plan(a.dev, a.pin, [&](Arena& dev, Arena& pin) {
+            seg.carve(dev, pin, 1); post.carve(dev, pin, 1);
+            dt = taps.empty() ? nullptr : dev.get<float>(taps.size());
+            b.carve(dev, pin, o, (long long)n, nullptr);
+        });
+        if (dt) {
+            SB_CUDA(cudaMemcpy(dt, taps.data(), taps.size() * 4, cudaMemcpyHostToDevice));
+            for (ResampleSeg& r : o.rp.segs) r.taps = dt;
+        }
+        seg.h[0] = FrameSeg{0, (int)n, 0, 0, 0}; post.h[0] = PcmPost();
+        seg.upload(0); post.upload(0);
+        SB_CUDA(cudaMemset(b.in + n, 0, 4 * sizeof(float)));
+        if (n) SB_CUDA(cudaMemcpy(b.in, x, n * 4, cudaMemcpyHostToDevice));
+        b.upload(o, 1, seg.h, post.h, 0);
+        Profile none;
+        out = run_output_stage(none, o, b, Wave{b.in, seg.d, post.d, 1}, 0);
+        SB_CUDA(cudaDeviceSynchronize());
+        SB_CUDA(cudaGetLastError());
+    }
+};
+
 // The branches of a 64-channel ResBlock2 stage of kernel sizes ks[b] and dilations dils[2b], dils[2b + 1]; each conv's
 // ConvW from `make` (weights and images, or only the shape).  False on a malformed description.
 template <typename Make> bool debug_stage(int32_t nbr, const int32_t* ks, const int32_t* dils, std::vector<ResBW>& res, Make&& make) {
@@ -1185,23 +1218,13 @@ int32_t sb200_debug_resample(int32_t device, const float* x, size_t n, int32_t i
                              sb200_error* err) {
     return guarded(err, [&] {
         if (!x || !y || n == 0 || n > (size_t)INT32_MAX) throw Error(19, "debug resample: bad arguments");
-        ResampleFilter f = resample_ratio(in_rate, out_rate, "");
+        const ResampleFilter f = resample_ratio(in_rate, out_rate, "");
         const std::vector<float> t = resample_phase_major(resample_taps(f.up, f.down), f.up, f.K);
-        const long long n_out = ((long long)n * f.up + f.down - 1) / f.down;
         SB_CUDA(cudaSetDevice(device));
-        DeviceBuffers d;
-        f.taps = d.upload(t.data(), t.size(), t.size());
-        const float* dx = d.upload(x, n, n);
-        float* dy = d.alloc<float>((size_t)n_out);
-        const FrameSeg fs{0, (int)n, 0, 0, 0};               // one segment of n samples at hop 1
-        const PcmPost post;
-        const ResampleSeg rs{f.taps, 0, n_out, f.up, f.down, f.H, f.K};
-        const FrameSeg* dfs = d.upload(&fs, 1, 1);
-        const PcmPost* dpost = d.upload(&post, 1, 1);
-        const ResampleSeg* drs = d.upload(&rs, 1, 1);
-        launch_resample(dx, dfs, dpost, 1, drs, 1, n_out, resample_span(f.up, f.down, f.K), dy, 0);
-        SB_CUDA(cudaDeviceSynchronize());
-        SB_CUDA(cudaMemcpy(y, dy, (size_t)n_out * 4, cudaMemcpyDeviceToHost));
+        OutputPlan o;
+        o.rp.add(&f, (long long)n);
+        HookStage h(o, x, n, t);
+        SB_CUDA(cudaMemcpy(y, h.out.buf, (size_t)o.rp.total * 4, cudaMemcpyDeviceToHost));
     });
 }
 
@@ -1223,16 +1246,12 @@ int32_t sb200_debug_loudness(int32_t device, const float* x, size_t n, int32_t r
         LoudSeg s{};
         loudness_design(rate, s);
         s.off = 0; s.n = (long long)n; s.c0 = 0; s.target = NAN;
+        OutputPlan o;
+        o.lp.segs.push_back(s);
+        o.lp.chunks = ((long long)n + s.S - 1) / s.S;
         SB_CUDA(cudaSetDevice(device));
-        DeviceBuffers d;
-        float* dx = d.upload(x, n, n);
-        const LoudSeg* ds = d.upload(&s, 1, 1);
-        double* scratch = d.alloc<double>((size_t)LD_SCRATCH * ((n + s.S - 1) / s.S));
-        double* dl = d.alloc<double>(1);
-        float* dg = d.alloc<float>(1);
-        launch_loudness(dx, ds, 1, scratch, dl, dg, 0);
-        SB_CUDA(cudaDeviceSynchronize());
-        SB_CUDA(cudaMemcpy(lufs, dl, sizeof(double), cudaMemcpyDeviceToHost));
+        HookStage h(o, x, n);
+        *lufs = h.b.lufs.h[0];
     });
 }
 
@@ -1248,36 +1267,19 @@ int32_t sb200_debug_loudness_stream(int32_t device, const float* x, const size_t
         SB_CUDA(cudaSetDevice(device));
         std::unique_ptr<LoudnessStream> m(create_loudness_stream(nullptr, device, rate, target_lufs, max_gain_db));
         loudness_stream_steps(*m, (long long)total, "debug loudness stream: ");
-        const long long S = m->d.S, steps = (long long)total / S;
-        DeviceBuffers d;
-        float* dx = d.upload(x, total, total + 1);
-        float* win = d.alloc<float>(total + (size_t)S + 1);
-        double* e = d.alloc<double>(8 * (size_t)steps + 8);
-        double* dl = d.alloc<double>((size_t)steps + 1);
-        float* dg = d.alloc<float>((size_t)steps + 1);
-        unsigned long long* dc = d.alloc<unsigned long long>(1);
-        LoudStreamSeg* ds = d.alloc<LoudStreamSeg>(1);
-        // chunk by chunk, each in its own launch, as passes feed a meter
+        // chunk by chunk, each in its own pass, as passes feed a meter
         size_t off = 0;
         for (size_t c = 0; c < n_chunks; c++) {
-            const long long n = (long long)chunk_lens[c], nc = loudness_stream_steps(*m, n, "debug loudness stream: ");
-            LoudStreamSeg g = loudness_stream_seg(*m, dx + off, n, 1.f);
-            g.win = win; g.e = e; g.lufs = dl + m->steps; g.gains = dg + m->steps; g.clipped = dc;
-            SB_CUDA(cudaMemcpy(ds, &g, sizeof(g), cudaMemcpyHostToDevice));
-            launch_loudness_stream(ds, 1, 0);
-            SB_CUDA(cudaDeviceSynchronize());
-            std::vector<double> l((size_t)nc + 1);
-            std::vector<float> a((size_t)nc + 1);
-            unsigned long long clip = 0;
-            SB_CUDA(cudaMemcpy(l.data(), g.lufs, (size_t)nc * sizeof(double), cudaMemcpyDeviceToHost));
-            SB_CUDA(cudaMemcpy(a.data(), g.gains, (size_t)nc * sizeof(float), cudaMemcpyDeviceToHost));
-            SB_CUDA(cudaMemcpy(&clip, dc, sizeof(clip), cudaMemcpyDeviceToHost));
-            loudness_stream_advance(*m, n, l.data(), a.data(), clip);
-            off += (size_t)n;
+            ChunkSpec spec;
+            spec.ls = m.get();
+            OutputPlan o = plan_chunk_output({spec}, {(long long)chunk_lens[c]}, false);
+            HookStage h(o, x + off, chunk_lens[c]);
+            if (chunk_lens[c]) SB_CUDA(cudaMemcpy(y + off, h.b.in, chunk_lens[c] * 4, cudaMemcpyDeviceToHost));
+            std::copy(h.b.mlufs.h, h.b.mlufs.h + o.mp.steps[0], lufs_steps + m->steps);
+            std::copy(h.b.mgains.h, h.b.mgains.h + o.mp.steps[0], gain_steps + m->steps);
+            advance_streams(o, h.b, Profile());
+            off += chunk_lens[c];
         }
-        if (total) SB_CUDA(cudaMemcpy(y, dx, total * 4, cudaMemcpyDeviceToHost));
-        SB_CUDA(cudaMemcpy(lufs_steps, dl, (size_t)steps * sizeof(double), cudaMemcpyDeviceToHost));
-        SB_CUDA(cudaMemcpy(gain_steps, dg, (size_t)steps * sizeof(float), cudaMemcpyDeviceToHost));
         *clipped = m->clipped;
     });
 }
@@ -1297,34 +1299,32 @@ int32_t sb200_debug_prosody_plan(int32_t rate, int64_t n, float pitch, float tem
     }
 }
 
+namespace {
+// A prosody hook's results: the output, every frame's offset and the stretched signal (the scratch when the pitch stage
+// follows, else the output itself).
+void debug_prosody_out(const HookStage& h, const ProsodySeg& g, float* y, int32_t* offsets, float* stretched) {
+    SB_CUDA(cudaMemcpy(y, h.b.py, (size_t)g.n2 * 4, cudaMemcpyDeviceToHost));
+    if (offsets && g.F) SB_CUDA(cudaMemcpy(offsets, h.b.offsets, (size_t)g.F * 4, cudaMemcpyDeviceToHost));
+    if (stretched && g.stretch)
+        SB_CUDA(cudaMemcpy(stretched, g.pitch ? h.b.ps : h.b.py, (size_t)g.n1 * 4, cudaMemcpyDeviceToHost));
+}
+}  // namespace
+
 int32_t sb200_debug_prosody(int32_t device, const float* x, size_t n, int32_t rate, float pitch, float tempo, float* y,
                             size_t cap, int32_t* offsets, size_t offsets_cap, float* stretched, size_t stretched_cap,
                             sb200_error* err) {
     return guarded(err, [&] {
         if (!x || !y || n == 0 || n > (size_t)INT32_MAX) throw Error(19, "debug prosody: bad arguments");
         check_prosody(&pitch, &tempo, 1);
-        ProsodyPlan p;
-        p.add(prosody_shape(rate, (long long)n, pitch, tempo), 0, (long long)n);
-        const ProsodySeg& g = p.segs[0];
+        OutputPlan p;
+        p.pp.add(prosody_shape(rate, (long long)n, pitch, tempo), 0, (long long)n);
+        const ProsodySeg& g = p.pp.segs[0];
         if ((size_t)g.n2 > cap || (offsets && (size_t)g.F > offsets_cap) ||
             (stretched && g.stretch && (size_t)g.n1 > stretched_cap))
             throw Error(19, "debug prosody: a destination is too small for the result");
         SB_CUDA(cudaSetDevice(device));
-        DeviceBuffers d;
-        const float* dx = d.upload(x, n, n);
-        const ProsodySeg* dg = d.upload(&g, 1, 1);
-        int* doff = d.alloc<int>((size_t)g.F + 1);
-        float* ds = d.alloc<float>((size_t)p.s_total + 4);
-        float* dy = d.alloc<float>((size_t)g.n2 + 4);
-        if (p.smem_ints) launch_prosody_offsets(dx, dg, 1, p.smem_ints, doff, 0);
-        launch_prosody_ola(dx, dg, 1, p.max_ola, doff, ds, dy, 0);
-        if (p.max_pitch) launch_prosody_pitch(dx, ds, dg, 1, p.max_pitch, dy, 0);
-        SB_CUDA(cudaDeviceSynchronize());
-        SB_CUDA(cudaMemcpy(y, dy, (size_t)g.n2 * 4, cudaMemcpyDeviceToHost));
-        if (offsets && g.F) SB_CUDA(cudaMemcpy(offsets, doff, (size_t)g.F * 4, cudaMemcpyDeviceToHost));
-        // the stretched signal: the scratch when the pitch stage follows, else the result itself
-        if (stretched && g.stretch)
-            SB_CUDA(cudaMemcpy(stretched, g.pitch ? ds : dy, (size_t)g.n1 * 4, cudaMemcpyDeviceToHost));
+        HookStage h(p, x, n);
+        debug_prosody_out(h, g, y, offsets, stretched);
     });
 }
 
@@ -1364,31 +1364,17 @@ int32_t sb200_debug_prosody_contour(int32_t device, const float* x, size_t n, in
         check_pitch_contour(ratios, offs, 1, nullptr);
         check_prosody(nullptr, &tempo, 1);
         std::vector<ContourPiece> pc;
-        ProsodyPlan p;
-        p.add(prosody_contour_plan(rate, (long long)n, reinterpret_cast<const long long*>(ends), ratios, n_ids, NAN, tempo,
-                                   pc, nullptr),
-              0, (long long)n, &pc);
-        const ProsodySeg& g = p.segs[0];
+        OutputPlan p;
+        p.pp.add(prosody_contour_plan(rate, (long long)n, reinterpret_cast<const long long*>(ends), ratios, n_ids, NAN,
+                                      tempo, pc, nullptr),
+                 0, (long long)n, &pc);
+        const ProsodySeg& g = p.pp.segs[0];
         if ((size_t)g.n2 > cap || (offsets && (size_t)g.F > offsets_cap) ||
             (stretched && g.stretch && (size_t)g.n1 > stretched_cap))
             throw Error(19, "debug prosody contour: a destination is too small for the result");
         SB_CUDA(cudaSetDevice(device));
-        DeviceBuffers d;
-        const float* dx = d.upload(x, n, n);
-        const ProsodySeg* dg = d.upload(&g, 1, 1);
-        const ContourPiece* dpc = p.pieces.empty() ? nullptr : d.upload(p.pieces.data(), p.pieces.size(), p.pieces.size());
-        int* doff = d.alloc<int>((size_t)g.F + 1);
-        long long* dap = d.alloc<long long>((size_t)g.F + 1);
-        float* ds = d.alloc<float>((size_t)p.s_total + 4);
-        float* dy = d.alloc<float>((size_t)g.n2 + 4);
-        if (p.smem_ints) launch_prosody_offsets(dx, dg, 1, p.smem_ints, doff, 0, dpc, dap);
-        launch_prosody_ola(dx, dg, 1, p.max_ola, doff, ds, dy, 0, dap);
-        if (p.max_pitch) launch_prosody_pitch(dx, ds, dg, 1, p.max_pitch, dy, 0, dpc);
-        SB_CUDA(cudaDeviceSynchronize());
-        SB_CUDA(cudaMemcpy(y, dy, (size_t)g.n2 * 4, cudaMemcpyDeviceToHost));
-        if (offsets && g.F) SB_CUDA(cudaMemcpy(offsets, doff, (size_t)g.F * 4, cudaMemcpyDeviceToHost));
-        if (stretched && g.stretch)
-            SB_CUDA(cudaMemcpy(stretched, g.pitch ? ds : dy, (size_t)g.n1 * 4, cudaMemcpyDeviceToHost));
+        HookStage h(p, x, n);
+        debug_prosody_out(h, g, y, offsets, stretched);
     });
 }
 
@@ -1409,41 +1395,19 @@ int32_t sb200_debug_formant(int32_t device, const float* x, size_t n, int32_t ra
                     : prosody_shape(rate, (long long)n, pitch, tempo),
               0, (long long)n, &pc);
         const ProsodySeg& g = p.segs[0];
-        const bool prosody = g.stretch || g.pitch;
-        FormantPlan fp;
-        if (formant_asks(g.n2, phi, g.p, p.pieces.data() + g.c_off, g.c_n))
-            fp.add(rate, 0, g.n2, phi, g.p, g.c_off, g.c_n);
+        OutputPlan o;
+        if (g.stretch || g.pitch) o.pp = p;
+        if (formant_asks(g.n2, phi, g.p, p.pieces.data() + g.c_off, g.c_n)) {
+            o.fp.add(rate, 0, g.n2, phi, g.p, g.c_off, g.c_n);
+            o.fp.total = g.n2;
+        }
         if ((size_t)g.n2 > cap) throw Error(19, "debug formant: a destination is too small for the result");
         SB_CUDA(cudaSetDevice(device));
-        DeviceBuffers d;
+        HookStage h(o, x, n);
         // the pitch stage's output and the formant stage's
-        float* dy = d.alloc<float>((size_t)g.n2 + 4);
-        float* dz = d.alloc<float>((size_t)g.n2 + 4);
-        if (prosody) {
-            const float* dx = d.upload(x, n, n);
-            const ProsodySeg* dg = d.upload(&g, 1, 1);
-            const ContourPiece* dpc = p.pieces.empty() ? nullptr : d.upload(p.pieces.data(), p.pieces.size(), p.pieces.size());
-            int* doff = d.alloc<int>((size_t)g.F + 1);
-            long long* dap = d.alloc<long long>((size_t)g.F + 1);
-            float* ds = d.alloc<float>((size_t)p.s_total + 4);
-            if (p.smem_ints) launch_prosody_offsets(dx, dg, 1, p.smem_ints, doff, 0, dpc, dap);
-            launch_prosody_ola(dx, dg, 1, p.max_ola, doff, ds, dy, 0, dap);
-            if (p.max_pitch) launch_prosody_pitch(dx, ds, dg, 1, p.max_pitch, dy, 0, dpc);
-            if (!fp.segs.empty()) {
-                const FormantSeg* dfs = d.upload(fp.segs.data(), 1, 1);
-                launch_formant(dy, dfs, 1, fp.max_runs, dpc, dz, 0);
-            }
-        } else {
-            SB_CUDA(cudaMemcpy(dy, x, n * 4, cudaMemcpyHostToDevice));
-            if (!fp.segs.empty()) {
-                const FormantSeg* dfs = d.upload(fp.segs.data(), 1, 1);
-                launch_formant(dy, dfs, 1, fp.max_runs, nullptr, dz, 0);
-            }
-        }
-        SB_CUDA(cudaDeviceSynchronize());
-        SB_CUDA(cudaGetLastError());
-        SB_CUDA(cudaMemcpy(pre, dy, (size_t)g.n2 * 4, cudaMemcpyDeviceToHost));
-        SB_CUDA(cudaMemcpy(y, fp.segs.empty() ? dy : dz, (size_t)g.n2 * 4, cudaMemcpyDeviceToHost));
+        const float* before = o.pp.segs.empty() ? h.b.in : h.b.py;
+        SB_CUDA(cudaMemcpy(pre, before, (size_t)g.n2 * 4, cudaMemcpyDeviceToHost));
+        SB_CUDA(cudaMemcpy(y, o.fp.segs.empty() ? before : h.b.fy, (size_t)g.n2 * 4, cudaMemcpyDeviceToHost));
         if (n2_out) *n2_out = g.n2;
     });
 }
@@ -1485,66 +1449,25 @@ namespace {
 void debug_push_stream(ProsodyStream& ps, const ProsodyShape& whole, const std::vector<long long>& counts, size_t stride,
                        const float* x, const int64_t* chunk_lens, size_t n_chunks, float* y, size_t cap, int64_t* lens,
                        int32_t* offsets, size_t offsets_cap) {
-    long long total = 0, out_total = 0;
-    for (size_t k = 0; k < n_chunks; k++) { total += chunk_lens[k]; out_total += counts[stride * k]; }
+    long long out_total = 0;
+    for (size_t k = 0; k < n_chunks; k++) out_total += counts[stride * k];
     if ((size_t)out_total > cap) throw Error(19, "debug prosody stream: the destination is too small for the result");
     if (offsets && ps.sh.stretch && (size_t)whole.F > offsets_cap)
         throw Error(19, "debug prosody stream: the offsets destination is too small");
-    // buffers for the largest pass: windows of at most the history plus the whole input, every frame and output
-    DeviceBuffers d;
-    const float* dx = d.upload(x, (size_t)total, (size_t)total + 4);
-    const PcmPost post;
-    const PcmPost* dpost = d.upload(&post, 1, 1);
-    FrameSeg* dfs = d.alloc<FrameSeg>(1);
-    ProsodySeg* dg = d.alloc<ProsodySeg>(1);
-    ProsodyCarry* dc = d.alloc<ProsodyCarry>(1);
-    float* win = d.alloc<float>((size_t)ps.cap_in + (size_t)total + 4);
-    float* ds = d.alloc<float>((size_t)ps.cap_s + (size_t)whole.n1 + 4);
-    int* doff = d.alloc<int>((size_t)whole.F + 4);
-    long long* dap = ps.pieces.empty() ? nullptr : d.alloc<long long>((size_t)whole.F + 4);
-    float* dy = d.alloc<float>((size_t)whole.n2 + 4);
-    FormantSeg* dfg = ps.fm ? d.alloc<FormantSeg>(1) : nullptr;
-    FormantCarry* dfc = ps.fm ? d.alloc<FormantCarry>(1) : nullptr;
-    float* fwin = ps.fm ? d.alloc<float>((size_t)FM_CARRY + (size_t)whole.n2 + 4) : nullptr;
-    float* dz = ps.fm ? d.alloc<float>((size_t)whole.n2 + 4) : nullptr;
-    const bool warps = prosody_stream_warps(ps);
     long long in_at = 0, out_at = 0;
     for (size_t k = 0; k < n_chunks; k++) {
-        const bool last = k + 1 == n_chunks;
-        const ProsodyStep t = prosody_stream_step(ps, chunk_lens[k], last);
-        ProsodyPlan p;
-        // the chunk as one segment of single samples at in_at
-        const FrameSeg fs{0, (int)chunk_lens[k], 0, 0, in_at};
-        SB_CUDA(cudaMemcpy(dfs, &fs, sizeof(fs), cudaMemcpyHostToDevice));
-        if (warps) {
-            p.add_stream(ps, t);
-            const ProsodyCarry c = prosody_carry(ps, t, 0);
-            SB_CUDA(cudaMemcpy(dg, &p.segs[0], sizeof(ProsodySeg), cudaMemcpyHostToDevice));
-            SB_CUDA(cudaMemcpy(dc, &c, sizeof(c), cudaMemcpyHostToDevice));
-            launch_prosody_stream_stretch(p, dg, dc, dx, dfs, dpost, 1, win, ds, doff, dy, 0, dap);
-            if (p.max_pitch) launch_prosody_pitch(win, ds, dg, 1, p.max_pitch, dy, 0);
-        }
-        long long m = t.j1 - t.j0;
-        const float* res = dy;
-        if (ps.fm) {
-            const FormantStep f = formant_stream_step(ps, t.next.emitted, last);
-            FormantPlan fp;
-            fp.add_stream(ps, f);
-            const FormantCarry fc = formant_carry(ps, f, 0, warps ? dy : nullptr);
-            SB_CUDA(cudaMemcpy(dfg, &fp.segs[0], sizeof(FormantSeg), cudaMemcpyHostToDevice));
-            SB_CUDA(cudaMemcpy(dfc, &fc, sizeof(fc), cudaMemcpyHostToDevice));
-            launch_formant_stream(fp, dfg, dfc, dx, dfs, dpost, 1, fwin, dz, 0);
-            m = fp.total; res = dz;
-            formant_stream_advance(ps, f);
-        }
-        SB_CUDA(cudaDeviceSynchronize());
-        SB_CUDA(cudaGetLastError());
-        SB_CUDA(cudaMemcpy(y + out_at, res, (size_t)m * 4, cudaMemcpyDeviceToHost));
+        ChunkSpec c;
+        c.ps = &ps; c.last = k + 1 == n_chunks;
+        OutputPlan o = plan_chunk_output({c}, {(long long)chunk_lens[k]}, false);
+        HookStage h(o, x + in_at, (size_t)chunk_lens[k]);
+        const long long m = o.n_res[0];
+        const ProsodyStep& t = o.steps[0];
+        SB_CUDA(cudaMemcpy(y + out_at, o.fp.segs.empty() ? h.b.py : h.b.fy, (size_t)m * 4, cudaMemcpyDeviceToHost));
         if (offsets && t.k1 > t.k0)
-            SB_CUDA(cudaMemcpy(offsets + t.k0, doff + 2, (size_t)(t.k1 - t.k0) * 4, cudaMemcpyDeviceToHost));
+            SB_CUDA(cudaMemcpy(offsets + t.k0, h.b.offsets + 2, (size_t)(t.k1 - t.k0) * 4, cudaMemcpyDeviceToHost));
         lens[k] = m;
         out_at += m; in_at += chunk_lens[k];
-        prosody_stream_advance(ps, t, last);
+        advance_streams(o, h.b, Profile());
     }
 }
 }  // namespace

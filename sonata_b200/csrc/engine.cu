@@ -330,27 +330,35 @@ void set_job_formants(Job& j, const float* phi) {
     else j.formant.clear();
 }
 
+void Profile::begin(const std::string& name) {
+    if (!regions) return;
+    regions->emplace_back();
+    cur = &regions->back();
+    cur->name = name;
+    cur->e0 = c->next_event(); cur->e1 = c->next_event();
+    cudaEventRecord(cur->e0, st);
+}
+void Profile::end() {
+    if (!cur) return;
+    cudaEventRecord(cur->e1, st);
+    cur = nullptr;
+}
+float Profile::ms(const std::string& name) const {
+    float ms = 0.f;
+    if (regions)
+        for (Region& g : *regions)
+            if (g.name == name) { cudaEventElapsedTime(&g.ms, g.e0, g.e1); ms = g.ms; }
+    return ms;
+}
+
 namespace {
 
-// Launches of one pass on context c's stream, each counted in the profile region of `regions` open at the time.  cond:
+// Launches of one pass on context c's stream, each counted in the profile region of `regs` open at the time.  cond:
 // the effective biases of the speaker-conditioned convs, [slot][cond_rows] (null on a single-speaker voice).
-struct Runner {
-    Voice& v; Context& c; std::vector<Region>& regions; const float* cond; const Arch& a; cudaStream_t st;
-    Region* cur = nullptr;
+struct Runner : Profile {
+    Voice& v; const float* cond; const Arch& a;
     Runner(Voice& voice, Context& ctx, std::vector<Region>& regs, const float* cond_bias)
-        : v(voice), c(ctx), regions(regs), cond(cond_bias), a(voice.a), st(ctx.stream) {}
-
-    void begin(const std::string& name) {
-        regions.emplace_back();
-        cur = &regions.back();
-        cur->name = name;
-        cur->e0 = c.next_event(); cur->e1 = c.next_event();
-        cudaEventRecord(cur->e0, st);
-    }
-    void end() { cudaEventRecord(cur->e1, st); cur = nullptr; }
-    void count(double flops, double bytes, int launches = 1) {
-        if (cur) { cur->flops += flops; cur->bytes += bytes; cur->launches += launches; }
-    }
+        : Profile{&ctx, &regs, ctx.stream}, v(voice), cond(cond_bias), a(voice.a) {}
 
     void conv(const ConvW& w, const float* x, int ldx, const Level& lin, const ConvCall& o) {
         ConvArgs p = conv_args(w, x, ldx, lin.map, o);
@@ -397,26 +405,6 @@ void expose(Job& j, const std::string& name, float* p, int cols, int level) {
     j.dbg[name] = {p, cols};
     j.dbg_level[name] = level;
 }
-
-// Each workspace below hands out its buffers in one carve(dev, pin).  plan() runs it on dry arenas to learn the sizes,
-// makes room in the context's arenas and carves again for real, so no size is written down twice.
-template <typename Carve> void plan(Arena& dev, Arena& pin, Carve&& carve) {
-    Arena dry_dev, dry_pin;
-    dry_dev.dry = dry_pin.dry = true;
-    carve(dry_dev, dry_pin);
-    dev.reserve(dry_dev.used);
-    pin.reserve(dry_pin.used);
-    carve(dev, pin);
-}
-
-// A table the host fills and the device reads, or the reverse: the device table `d` and its page-locked mirror `h`,
-// carved together with one element count, so every copy moves exactly the carved table.  Unset (null) when not carved.
-template <typename T> struct Staged {
-    T* d = nullptr; T* h = nullptr; size_t n = 0;
-    void carve(Arena& dev, Arena& pin, size_t count) { n = count; d = dev.get<T>(n); h = pin.get<T>(n); }
-    void upload(cudaStream_t st) const { SB_CUDA(cudaMemcpyAsync(d, h, n * sizeof(T), cudaMemcpyHostToDevice, st)); }
-    void download(cudaStream_t st) const { SB_CUDA(cudaMemcpyAsync(h, d, n * sizeof(T), cudaMemcpyDeviceToHost, st)); }
-};
 
 // Gives the next segment of a pass the slot of canonical blend `b` (a plain speaker: its own one-speaker blend), a new
 // one for a blend not seen before; false when a plain speaker is not a speaker of the voice.  On a single-speaker voice
@@ -553,139 +541,6 @@ struct FrameTables {
     }
 };
 
-// One resample launch over segments laid out back to back: each segment's ResampleSeg, what the launch is sized by and
-// what the profile counts.
-struct ResamplePlan {
-    std::vector<ResampleSeg> segs;
-    long long total = 0, max_out = 0; int smem = 0;
-    double flops = 0, bytes = 0;
-    // Appends a segment of n_in inputs through `f` (null: copied unchanged).  A whole signal emits every output; with a
-    // stream's resampler `r` (whose filter is f) the segment continues r's stream, emits every output whose inputs have
-    // all arrived, and flushes the stream when `last`.
-    void add(const ResampleFilter* f, long long n_in, const Resampler* r = nullptr, bool last = false) {
-        ResampleSeg s{};
-        s.out_off = total; s.n_out = n_in; s.down = 1;
-        if (f) {
-            const long long N = (r ? r->consumed : 0) + n_in;
-            s.taps = f->taps; s.up = f->up; s.down = f->down; s.H = f->H; s.K = f->K;
-            s.n_out = resample_emit_end(*f, N, !r || last) - (r ? r->emitted : 0);
-            if (r) {
-                s.hist = r->hist[r->cur]; s.hist_out = r->hist[1 - r->cur];
-                s.c = r->consumed; s.j0 = r->emitted; s.h = r->h; s.h_out = (int)std::min<long long>(N, f->K - 1);
-            }
-        }
-        bytes += 4.0 * ((double)n_in + s.n_out);
-        if (f) {
-            smem = std::max(smem, resample_span(f->up, f->down, f->K));
-            flops += 2.0 * (double)s.n_out * (2.0 * f->H + 1.0) / f->up;
-            bytes += 4.0 * (double)f->up * f->K;
-        }
-        max_out = std::max(max_out, s.n_out);
-        total += s.n_out;
-        segs.push_back(s);
-    }
-};
-
-// Device tables of a resample launch and their pinned mirrors: the segments, identity posts (for a launch whose input
-// has no post-path, or for the i16 conversion of its output; out_gain[k], when given, is output k's gain there, and
-// fixed_scale[k] its PcmPost::fixed_scale) and the output segments, n_out samples at out_off.
-struct ResampleTables {
-    Staged<ResampleSeg> segs; Staged<PcmPost> posts; Staged<FrameSeg> osegs;
-    void carve(Arena& dev, Arena& pin, size_t n) {
-        segs.carve(dev, pin, n); posts.carve(dev, pin, n); osegs.carve(dev, pin, n);
-    }
-    void upload(const ResamplePlan& p, cudaStream_t st, const std::vector<float>* out_gain = nullptr,
-                const std::vector<int>* fixed_scale = nullptr) {
-        for (size_t k = 0; k < p.segs.size(); k++) {
-            segs.h[k] = p.segs[k];
-            posts.h[k] = PcmPost();
-            if (out_gain) posts.h[k].gain = (*out_gain)[k];
-            if (fixed_scale) posts.h[k].fixed_scale = (*fixed_scale)[k];
-            osegs.h[k] = FrameSeg{0, (int)p.segs[k].n_out, 0, 0, p.segs[k].out_off};
-        }
-        segs.upload(st); posts.upload(st); osegs.upload(st);
-    }
-};
-
-// Device buffers of the prosody launches of plan p and the pinned mirrors of their tables: the segments, every frame's
-// offset, the stretched signals of the segments that run both stages, and the output unless it goes elsewhere.  A plan
-// of whole signals adds the output segments (n2 samples at y_off, for the launches that read the prosody output); a
-// plan of stream windows the carry entry of every window and the staged input windows.
-struct ProsodyBufs {
-    Staged<ProsodySeg> segs; Staged<FrameSeg> osegs; Staged<ProsodyCarry> carry;
-    Staged<ContourPiece> pieces;               // the contours' piece tables (only when a segment has one)
-    long long* apos = nullptr;                 // and their analysis positions, indexed like the offsets
-    int* offsets = nullptr; float *x = nullptr, *s = nullptr, *y = nullptr;
-    void carve(Arena& dev, Arena& pin, const ProsodyPlan& p, bool own_y) {
-        const size_t n = p.segs.size();
-        y = nullptr;
-        if (n == 0) return;
-        segs.carve(dev, pin, n);
-        if (!p.pieces.empty()) pieces.carve(dev, pin, p.pieces.size());     // a stream's table is its own
-        if (p.contour) apos = dev.get<long long>((size_t)p.d_total);
-        if (p.in_total) {
-            carry.carve(dev, pin, n);
-            x = dev.get<float>((size_t)p.in_total + 4);
-        } else {
-            osegs.carve(dev, pin, n);
-        }
-        offsets = p.d_total ? dev.get<int>((size_t)p.d_total) : nullptr;
-        s = p.s_total ? dev.get<float>((size_t)p.s_total + 4) : nullptr;
-        if (own_y) y = dev.get<float>((size_t)p.y_total + 4);
-    }
-    // Fills and uploads the segments and, for whole signals, the output segments; a stream pass fills the carry.
-    void upload(const ProsodyPlan& p, cudaStream_t st) const {
-        for (size_t k = 0; k < p.segs.size(); k++) {
-            segs.h[k] = p.segs[k];
-            if (osegs.d) osegs.h[k] = FrameSeg{0, (int)p.segs[k].n2, 0, 0, p.segs[k].y_off};
-        }
-        segs.upload(st);
-        if (osegs.d) osegs.upload(st);
-        if (pieces.d) {
-            std::copy(p.pieces.begin(), p.pieces.end(), pieces.h);
-            pieces.upload(st);
-        }
-    }
-};
-
-// The formant launch's segments and their pinned mirror, and its output (`y`, laid out like its input) when it is the
-// resample launch's input or the job's result in a buffer of the pass's own.
-struct FormantBufs {
-    Staged<FormantSeg> segs;
-    float* y = nullptr;
-    void carve(Arena& dev, Arena& pin, const FormantPlan& p, bool own_y) {
-        y = nullptr;
-        if (p.segs.empty()) return;
-        segs.carve(dev, pin, p.segs.size());
-        if (own_y) y = dev.get<float>((size_t)p.total + 4);
-    }
-    void upload(const FormantPlan& p, cudaStream_t st) const {
-        std::copy(p.segs.begin(), p.segs.end(), segs.h);
-        segs.upload(st);
-    }
-};
-
-// The loudness launch over what a job hands out: one segment per utterance at its delivered rate, chunk scratch laid out
-// back to back.
-struct LoudnessPlan {
-    std::vector<LoudSeg> segs;
-    long long chunks = 0;
-};
-
-// Device tables of the loudness launch and their pinned mirrors: the segments, the chunk scratch and the results.
-struct LoudnessBufs {
-    Staged<LoudSeg> segs;
-    double* scratch = nullptr;
-    Staged<double> lufs; Staged<float> gain;
-    void carve(Arena& dev, Arena& pin, const LoudnessPlan& p) {
-        const size_t n = p.segs.size();
-        if (n == 0) return;
-        segs.carve(dev, pin, n);
-        scratch = dev.get<double>((size_t)LD_SCRATCH * std::max<long long>(p.chunks, 1));
-        lufs.carve(dev, pin, n); gain.carve(dev, pin, n);
-    }
-};
-
 // Decoder over RY frames: conv_pre's output, then ping-pong stage buffers sized for the widest stage, or with debug one
 // set per stage so every stage can be fetched.
 struct DecoderBufs {
@@ -726,33 +581,13 @@ struct DecoderBufs {
 };
 
 // Frame level of a synthesis pass (phase 2): tables, the latent, the flow's scratch, and unless the pass stops after
-// the flow the decoder and (when the caller passed no buffer) the waveforms.  With prosody or output rates the decoder's
-// waveforms are always the pass's own.  The prosody output (plan `pp`) is the pass's own too unless it is the result
-// and the caller passed a buffer; the resampled waveforms go to the caller's buffer or to `rs`, with the tables of the
-// resampling launch `rp`.  With the formant stage (plan `fp`) the stage before it writes into a buffer of the pass's
-// own, and the formant output, laid out the same way, goes to the caller's buffer or its own (fm.y).
+// the flow the output stage's buffers (plan `o`; the decoder's waveforms are their input) and the decoder.
 struct FrameBufs {
     FrameTables y;
-    float *s, *epsz, *zp, *h, *acts, *outb, *wav;
+    float *s, *epsz, *zp, *h, *acts, *outb;
     std::vector<float*> flow;                  // debug: z after each coupling layer, in the engine's channel order
     DecoderBufs dec;
-    ResampleTables rt; float* rs;
-    LoudnessBufs ld;
-    ProsodyBufs pr;
-    FormantBufs fm;
-    void carve(Arena& dev, Arena& pin, const Job& j, const ProsodyPlan& pp, const FormantPlan& fp, const ResamplePlan& rp,
-               const LoudnessPlan& lp, bool own_wav) {
-        rt.carve(dev, pin, rp.segs.size());
-        ld.carve(dev, pin, lp);
-        const bool formants = !fp.segs.empty();
-        pr.carve(dev, pin, pp, own_wav || !rp.segs.empty() || formants);
-        fm.carve(dev, pin, fp, own_wav || !rp.segs.empty());
-        rs = nullptr;
-        if (!rp.segs.empty()) {
-            if (own_wav) rs = dev.get<float>((size_t)rp.total + 4);
-            own_wav = true;
-        }
-        if (!pp.segs.empty() || formants) own_wav = true;
+    void carve(Arena& dev, Arena& pin, const Job& j, const OutputPlan& o, OutputBufs& out, float* d_out) {
         const Arch& a = j.v->a;
         const size_t RY = (size_t)j.frames.RY;
         y.carve(dev, pin, j.frames);
@@ -764,78 +599,37 @@ struct FrameBufs {
         flow.assign(j.debug ? j.v->flows.size() : 0, nullptr);
         for (auto& p : flow) p = dev.get<float>(RY * a.inter);
         h = dev.get<float>(RY * a.hidden); acts = dev.get<float>(RY * a.hidden); outb = dev.get<float>(RY * a.hidden);
-        wav = nullptr;
         if (j.encode_only) return;
-        if (own_wav) wav = dev.get<float>((size_t)j.frames.total_samples + 4);
+        out.carve(dev, pin, o, j.frames.total_samples, d_out);
         dec.carve(dev, *j.v, j.frames.RY, j.debug);
     }
 };
 
-// The metered chunks of a chunk pass: chunks[q] has n[q] samples, its window at win_off[q] of the pass's window buffer
-// and the steps[q] steps it completes at step_off[q] of its step tables.
-struct MeterPlan {
-    std::vector<int> chunks;
-    std::vector<long long> n, win_off, step_off, steps;
-    long long win_total = 0, steps_total = 0;
-    void add(int k, const LoudnessStream& s, long long samples, long long completes) {
-        chunks.push_back(k); n.push_back(samples);
-        win_off.push_back(win_total); step_off.push_back(steps_total); steps.push_back(completes);
-        win_total += s.samples - s.steps * s.d.S + samples;
-        steps_total += completes;
-    }
-};
-
 // One pass of streaming decoder chunks (layout l): speaker biases of every slot, tables, the gather table and the
-// latent slices, the decoder (one buffer per stage for a debug pass) and the waveforms; the post-path table when an
-// output stage runs, the resample launch's tables and output, the i16 or G.711 scratch; and the pinned block the packed
-// result (`total` values) is copied to.
+// latent slices, the decoder (one buffer per stage for a debug pass), the output stage (plan `o`; the decoder's
+// waveforms are its input), the post-path table when the output stage or a conversion reads it, the i16 or G.711
+// scratch; and the pinned block the packed result (`total` values) is copied to.
 struct ChunkBufs {
     SpeakerBias spk;
     FrameTables y;
     Staged<GatherSeg> src;
-    float *s, *wav;
+    float* s;
+    OutputBufs out;
     DecoderBufs dec;
     Staged<PcmPost> post;
-    ResampleTables rt; float* rs;
     void* pcm; unsigned* max;
     void* out_h;
-    // warped chunks (plan `pp`): the prosody buffers, the output after the waveforms in `wav`, and the resample
-    // launch's input table (the prosody output for a warped chunk, the post-path's chunk for the others); chunks with
-    // a formant stage (plan `fp`): its tables and windows, its output after the prosody output in `wav`, and the
-    // resample launch reads that output instead
-    ProsodyBufs pr;
-    Staged<FormantSeg> fsegs; Staged<FormantCarry> fcarry; float* fwin = nullptr;
-    Staged<FrameSeg> rin; Staged<PcmPost> rpost;
-    // metered chunks (plan `mp`): their entries, windows and step scratch, and the readings, gains and clamp counts
-    // they return
-    Staged<LoudStreamSeg> lsegs; float* lwin = nullptr; double* le = nullptr;
-    Staged<double> llufs; Staged<float> lgains; Staged<unsigned long long> lclip;
-    void carve(Arena& dev, Arena& pin, const Voice& v, const FrameLayout& l, const ChunkPass& p, const ResamplePlan& rp,
-               const ProsodyPlan& pp, const FormantPlan& fp, const MeterPlan& mp, size_t total) {
+    void carve(Arena& dev, Arena& pin, const Voice& v, const FrameLayout& l, const ChunkPass& p, const OutputPlan& o,
+               size_t total) {
         const bool i16_out = p.format != PCM_F32;
         const size_t n = l.fsegs.size();
         spk.carve(dev, pin, v, l);
         y.carve(dev, pin, l);
         src.carve(dev, pin, n);
         s = dev.get<float>((size_t)l.RY * v.a.inter);
-        wav = dev.get<float>((size_t)l.total_samples + (size_t)pp.y_total + (size_t)fp.total + 4);
-        pr.carve(dev, pin, pp, false);
-        if (!fp.segs.empty()) {
-            fsegs.carve(dev, pin, fp.segs.size()); fcarry.carve(dev, pin, fp.segs.size());
-            fwin = dev.get<float>((size_t)fp.in_total + 4);
-        }
-        if (!pp.segs.empty() || !fp.segs.empty()) { rin.carve(dev, pin, n); rpost.carve(dev, pin, n); }
-        if (!mp.chunks.empty()) {
-            const size_t m = mp.chunks.size(), steps = (size_t)std::max<long long>(mp.steps_total, 1);
-            lsegs.carve(dev, pin, m);
-            lwin = dev.get<float>((size_t)mp.win_total + 4);
-            le = dev.get<double>(8 * steps);
-            llufs.carve(dev, pin, steps); lgains.carve(dev, pin, steps); lclip.carve(dev, pin, m);
-        }
+        out.carve(dev, pin, o, l.total_samples, nullptr);
         dec.carve(dev, v, l.RY, p.debug);
         if (p.resample || i16_out) post.carve(dev, pin, n);
-        rt.carve(dev, pin, rp.segs.size());
-        rs = p.resample ? dev.get<float>(total + 4) : nullptr;
         pcm = i16_out ? dev.alloc((total + 8) * pcm_bytes(p.format)) : nullptr;
         max = i16_out ? dev.get<unsigned>(n) : nullptr;
         out_h = pin.alloc(total * pcm_bytes(p.format));
@@ -932,169 +726,6 @@ void lay_out_frames(FrameLayout& l, const std::vector<int>& y_len, int hop, cons
         cur += round_up(y_len[b] + HY, GY);
     }
     l.RY = cur; l.total_samples = out;
-}
-
-// The prosody launches of a job whose utterances ask for a pitch, a tempo or a contour (an empty plan when none does):
-// every utterance's decoder waveform, with its ratios or NaN.  With a contour (cum: the batch's cum rows on the host),
-// every utterance is planned from its ids' ends, and bounds receives each id's delivered end, packed like the ids.
-ProsodyPlan lay_out_prosody(const Job& j, int hop, const std::vector<int>& cum, std::vector<long long>& bounds) {
-    ProsodyPlan p;
-    bounds.clear();
-    if ((j.pitch.empty() && j.contour.empty()) || j.encode_only) return p;
-    if (j.contour.empty()) {
-        for (size_t b = 0; b < j.B; b++) {
-            const FrameSeg& f = j.frames.fsegs[b];
-            const long long n = (long long)f.len * hop;
-            p.add(prosody_shape(j.v->sample_rate, n, j.pitch[b], j.tempo[b]), f.out_off, n);
-        }
-        return p;
-    }
-    bounds.resize(j.ids.size());
-    std::vector<long long> ends;
-    std::vector<ContourPiece> pieces;
-    for (size_t b = 0; b < j.B; b++) {
-        const FrameSeg& f = j.frames.fsegs[b];
-        const long long n = (long long)f.len * hop;
-        const size_t n_ids = j.offs[b + 1] - j.offs[b];
-        ends.resize(n_ids);
-        for (size_t i = 0; i < n_ids; i++) ends[i] = (long long)cum[j.xsegs[b].off + i] * hop;
-        const float* r = j.contour.data() + j.offs[b];
-        const bool has = std::any_of(r, r + n_ids, [](float v) { return !std::isnan(v) && v != 1.f; });
-        const float pitch = j.pitch.empty() ? NAN : j.pitch[b], tempo = j.tempo.empty() ? NAN : j.tempo[b];
-        const ProsodyShape sh = prosody_contour_plan(j.v->sample_rate, n, ends.data(), has ? r : nullptr, n_ids, pitch,
-                                                     tempo, pieces, bounds.data() + j.offs[b]);
-        p.add(sh, f.out_off, n, &pieces);
-    }
-    return p;
-}
-
-// The formant launch of a job whose utterances ask for a formant ratio (an empty plan when none asks): each asking
-// utterance's output of the pitch stage (plan pp), or its decoder waveform when pp is empty, with its pitch ratio or
-// contour.  Its output has that stage's layout; the utterances that do not ask are copied into it.
-FormantPlan lay_out_formants(const Job& j, int hop, const ProsodyPlan& pp) {
-    FormantPlan p;
-    if (j.formant.empty() || j.encode_only) return p;
-    p.total = pp.segs.empty() ? j.frames.total_samples : pp.y_total;
-    for (size_t b = 0; b < j.B; b++) {
-        long long in_off, n;
-        double ratio = 1.0;
-        int c_off = 0, c_n = 0;
-        if (pp.segs.empty()) {
-            in_off = j.frames.fsegs[b].out_off; n = (long long)j.frames.fsegs[b].len * hop;
-        } else {
-            const ProsodySeg& g = pp.segs[b];
-            in_off = g.y_off; n = g.n2; ratio = g.p; c_off = g.c_off; c_n = g.c_n;
-        }
-        if (!formant_asks(n, j.formant[b], ratio, pp.pieces.data() + c_off, c_n)) {
-            p.copy(in_off, n);
-            continue;
-        }
-        p.add(j.v->sample_rate, in_off, n, j.formant[b], ratio, c_off, c_n);
-    }
-    if (p.segs.empty()) return FormantPlan();
-    return p;
-}
-
-// What the job hands out (osegs, out_hop, out_total): the frame layout itself without prosody and output rates (an empty
-// plan), the prosody output without output rates (an empty plan too; the formant stage keeps its layout), else the
-// segments of the returned plan, one utterance each at its rate, back to back, resampled from the prosody output when
-// there is one.
-ResamplePlan lay_out_output(Job& j, int hop, const ProsodyPlan& pp) {
-    ResamplePlan p;
-    j.osr.assign(j.B, j.v->sample_rate);
-    if (j.out_rates.empty() || j.encode_only) {
-        j.osegs = j.frames.fsegs; j.out_hop = hop; j.out_total = j.frames.total_samples;
-        if (!pp.segs.empty()) {
-            for (size_t b = 0; b < j.B; b++) j.osegs[b] = FrameSeg{0, (int)pp.segs[b].n2, 0, 0, pp.segs[b].y_off};
-            j.out_hop = 1; j.out_total = pp.y_total;
-        }
-        return p;
-    }
-    j.osegs.assign(j.B, FrameSeg{});
-    for (size_t b = 0; b < j.B; b++) {
-        const ResampleFilter* f = nullptr;
-        if (j.out_rates[b]) {
-            j.osr[b] = j.out_rates[b];
-            f = &voice_resampler(*j.v, j.out_rates[b], "utterance " + std::to_string(b) + ": ");
-        }
-        p.add(f, pp.segs.empty() ? (long long)j.frames.fsegs[b].len * hop : pp.segs[b].n2);
-        j.osegs[b] = FrameSeg{0, (int)p.segs[b].n_out, 0, 0, p.segs[b].out_off};
-    }
-    j.out_hop = 1; j.out_total = p.total;
-    return p;
-}
-
-// The resample launch of plan `p` (tables `t`) over the segments of wav, read through `posts`, into out: profile region
-// "resample".
-void run_resample(Runner& R, const ResamplePlan& p, const ResampleTables& t, const float* wav, const FrameSeg* fsegs,
-                  const PcmPost* posts, int hop, float* out) {
-    R.begin("resample");
-    launch_resample(wav, fsegs, posts, hop, t.segs.d, (int)p.segs.size(), p.max_out, p.smem, out, R.st);
-    R.count(p.flops, p.bytes);
-    R.end();
-}
-
-// The prosody launches of plan `p` (buffers `t`) over the segments of wav into y: profile regions "stretch" (the offset
-// chain and the overlap-add, which also copies the segments without a ratio) and "pitch".
-void run_prosody(Runner& R, const ProsodyPlan& p, const ProsodyBufs& t, const float* wav, float* y) {
-    const int n = (int)p.segs.size();
-    R.begin("stretch");
-    if (p.smem_ints) launch_prosody_offsets(wav, t.segs.d, n, p.smem_ints, t.offsets, R.st, t.pieces.d, t.apos);
-    launch_prosody_ola(wav, t.segs.d, n, p.max_ola, t.offsets, t.s, y, R.st, t.apos);
-    R.count(p.stretch_flops, p.stretch_bytes, p.smem_ints ? 2 : 1);
-    R.end();
-    if (p.max_pitch == 0) return;
-    R.begin("pitch");
-    launch_prosody_pitch(wav, t.s, t.segs.d, n, p.max_pitch, y, R.st, t.pieces.d);
-    R.count(p.pitch_flops, p.pitch_bytes);
-    R.end();
-}
-
-// The formant launch of plan `p` (tables `t`) from `in` into `out`, laid out alike, and the copies of the utterances
-// that do not ask: profile region "formant".
-void run_formant(Runner& R, const FormantPlan& p, const FormantBufs& t, const ContourPiece* pieces, const float* in,
-                 float* out) {
-    R.begin("formant");
-    for (const auto& c : p.copies)
-        SB_CUDA(cudaMemcpyAsync(out + c.first, in + c.first, (size_t)c.second * 4, cudaMemcpyDeviceToDevice, R.st));
-    launch_formant(in, t.segs.d, (int)p.segs.size(), p.max_runs, pieces, out, R.st);
-    R.count(p.flops, p.bytes);
-    R.end();
-}
-
-// The loudness launch of a job with targets (an empty plan without): every utterance as the job hands it out, at its
-// rate, with its target or NaN.
-LoudnessPlan lay_out_loudness(const Job& j) {
-    LoudnessPlan p;
-    if (j.loud_target.empty() || j.encode_only) return p;
-    p.segs.resize(j.B);
-    for (size_t b = 0; b < j.B; b++) {
-        LoudSeg& s = p.segs[b];
-        loudness_design(j.osr[b], s);
-        s.off = j.osegs[b].out_off;
-        s.n = (long long)j.osegs[b].len * j.out_hop;
-        s.c0 = p.chunks;
-        s.target = j.loud_target[b];
-        p.chunks += (s.n + s.S - 1) / s.S;
-    }
-    return p;
-}
-
-// The loudness launch of plan `p` over wav in place, and the copy of its results to the pinned mirrors: profile region
-// "loudness".  Its bytes are the samples read and, where a target scales them, written.
-void run_loudness(Runner& R, const LoudnessPlan& p, const LoudnessBufs& t, float* wav) {
-    const size_t n = p.segs.size();
-    double samples = 0, scaled = 0;
-    for (const LoudSeg& s : p.segs) {
-        samples += (double)s.n;
-        if (!std::isnan(s.target)) scaled += (double)s.n;
-    }
-    R.begin("loudness");
-    launch_loudness(wav, t.segs.d, (int)n, t.scratch, t.lufs.d, t.gain.d, R.st);
-    R.count(2.0 * 22.0 * samples, 4.0 * (samples + scaled));
-    R.end();
-    t.lufs.download(R.st);
-    t.gain.download(R.st);
 }
 
 // Fills the frame-level tables of layout l through their pinned mirrors; returns the level.
@@ -1425,17 +1056,13 @@ void Job::run(float* d_out, size_t d_out_cap) {
     // The stream is idle here, so the pinned staging of the X tables can be reused for the Y tables.
     lay_out_frames(frames, y_len, a.hop(), xsegs);
     std::vector<long long> bounds;
-    const ProsodyPlan pp = lay_out_prosody(*this, a.hop(), cum_host, bounds);
-    const bool prosody = !pp.segs.empty();
-    const FormantPlan fp = lay_out_formants(*this, a.hop(), pp);
-    const bool formants = !fp.segs.empty();
-    const ResamplePlan rp = lay_out_output(*this, a.hop(), pp);
-    const bool resample = !rp.segs.empty();
-    const LoudnessPlan lp = lay_out_loudness(*this);
+    const OutputPlan op = plan_job_output(*this, a.hop(), cum_host, bounds);
     loud_ran.clear(); loud_lufs.clear(); loud_gain.clear(); pros_ran.clear(); pros_bounds.clear();
+    if (d_out && !encode_only && (size_t)out_total > d_out_cap)
+        throw Error(19, "caller-provided device output buffer is too small");
     FrameBufs f;
-    plan(C.dev_frame, C.pin, [&](Arena& dev, Arena& pin) { f.carve(dev, pin, *this, pp, fp, rp, lp, d_out == nullptr); });
-    d_osegs = resample ? f.rt.osegs.d : prosody ? f.pr.osegs.d : f.y.fsegs.d;
+    OutputBufs ob;
+    plan(C.dev_frame, C.pin, [&](Arena& dev, Arena& pin) { f.carve(dev, pin, *this, op, ob, d_out); });
     if (debug) {
         expose(*this, "z_p", f.zp, I, 1); expose(*this, "z", f.s, I, 1);
         // flow.{f}: z after the coupling layer of the graph's flow.flows.{2f} (f = flow_n - 1 first).  The graph's Flip
@@ -1445,13 +1072,7 @@ void Job::run(float* d_out, size_t d_out_cap) {
         if (!encode_only) f.dec.expose_to(*this);
     }
     Level LY = upload_frames(frames, f.y, st);
-    if (prosody) f.pr.upload(pp, st);
-    if (formants) f.fm.upload(fp, st);
-    if (resample) f.rt.upload(rp, st);
-    if (!lp.segs.empty()) {
-        std::copy(lp.segs.begin(), lp.segs.end(), f.ld.segs.h);
-        f.ld.segs.upload(st);
-    }
+    if (!encode_only) ob.upload(op, a.hop(), nullptr, nullptr, st);
 
     // ---------------- alignment expansion ----------------
     R.begin("align");
@@ -1504,41 +1125,21 @@ void Job::run(float* d_out, size_t d_out_cap) {
         ran = true;
         return;
     }
-    if (d_out) {
-        if ((size_t)out_total > d_out_cap) throw Error(19, "caller-provided device output buffer is too small");
-        d_wav = d_out;
-    } else {
-        d_wav = f.rs ? f.rs : f.fm.y ? f.fm.y : f.pr.y ? f.pr.y : f.wav;
-    }
-    float* staged = resample || prosody || formants ? f.wav : d_wav;
-    run_decoder(R, LY, f.y, f.dec, f.s, staged);
-    // the output stage: prosody on the decoder's waveform, formants on what that left (in the same layout), the resample
-    // launch on the result, loudness on what that gives
-    const FrameSeg* staged_segs = f.y.fsegs.d; int staged_hop = a.hop();
-    if (prosody) {
-        float* py = resample || formants ? f.pr.y : d_wav;
-        run_prosody(R, pp, f.pr, f.wav, py);
-        staged = py; staged_segs = f.pr.osegs.d; staged_hop = 1;
-    }
-    if (formants) {
-        float* fy = resample ? f.fm.y : d_wav;
-        run_formant(R, fp, f.fm, f.pr.pieces.d, staged, fy);
-        staged = fy;
-    }
-    if (resample) run_resample(R, rp, f.rt, staged, staged_segs, f.rt.posts.d, staged_hop, d_wav);
-    if (!lp.segs.empty()) run_loudness(R, lp, f.ld, d_wav);
+    run_decoder(R, LY, f.y, f.dec, f.s, ob.in);
+    const Wave res = run_output_stage(R, op, ob, Wave{ob.in, f.y.fsegs.d, nullptr, a.hop()}, st);
+    d_wav = res.buf; d_osegs = res.segs;
     SB_CUDA(cudaEventRecord(C.ev_end, st));
     SB_CUDA(cudaStreamSynchronize(st));
     SB_CUDA(cudaGetLastError());
     SB_CUDA(cudaEventElapsedTime(&last_ms, C.ev_begin, C.ev_end));
     for (Region& r : regions) cudaEventElapsedTime(&r.ms, r.e0, r.e1);
-    pros_ran = pp.shapes;
+    pros_ran = op.pp.shapes;
     pros_bounds.swap(bounds);
     pitch_ran = pitch; tempo_ran = tempo;
-    if (!lp.segs.empty()) {
+    if (!op.lp.segs.empty()) {
         loud_ran = loud_target;
-        loud_lufs.assign(f.ld.lufs.h, f.ld.lufs.h + B);
-        loud_gain.assign(f.ld.gain.h, f.ld.gain.h + B);
+        loud_lufs.assign(ob.lufs.h, ob.lufs.h + B);
+        loud_gain.assign(ob.gain.h, ob.gain.h + B);
     }
     ran = true;
 }
@@ -1620,6 +1221,15 @@ void decode_chunks(Voice* v, const ChunkPass& p, ChunkResult& out) {
     auto fail = [&p](size_t k, const std::string& what, const std::string& detail) {
         throw Error(19, p.single ? what : "chunk " + std::to_string(k) + ": " + what + detail);
     };
+    // chunk k's stream (its field `of`, named `what`): made for this voice, not flushed, and in no earlier chunk
+    const auto check_stream = [&](size_t k, auto of, const std::string& what, bool ended, const std::string& flushed) {
+        const auto* s = p.chunks[k].*of;
+        if (s->v != v) fail(k, "the " + what + " was made for another voice", "");
+        if (ended) fail(k, flushed, "");
+        for (size_t q = 0; q < k; q++)
+            if (p.chunks[q].*of == s)
+                fail(k, "the " + what + " of chunk " + std::to_string(q) + " appears twice in one call", "");
+    };
     for (size_t k = 0; k < n; k++) {
         const ChunkSpec& c = p.chunks[k];
         if (!c.z || c.z->v != v) fail(k, "the latent was not encoded by this voice", "");
@@ -1631,26 +1241,15 @@ void decode_chunks(Voice* v, const ChunkPass& p, ChunkResult& out) {
         // decoder.onnx takes the encoder's `g` (piper/src/lib.rs:706-735, 739-743): the latent's blend
         if (!assign_slot(l, *v, c.z->spk)) fail(k, "Failed to run model inference. Error: speaker id out of range", "");
         len[k] = (int)(c.hi - c.lo);
-        if (const Resampler* r = c.rs) {
-            if (r->v != v) fail(k, "the resampler was made for another voice", "");
-            if (r->ended) fail(k, "the resampler's stream has already been flushed", "");
-            for (size_t q = 0; q < k; q++)
-                if (p.chunks[q].rs == r) fail(k, "the resampler of chunk " + std::to_string(q) + " appears twice in one call", "");
-        }
-        if (const ProsodyStream* w = c.ps) {
+        if (c.rs)
+            check_stream(k, &ChunkSpec::rs, "resampler", c.rs->ended, "the resampler's stream has already been flushed");
+        if (c.ps) {
             if (!p.resample) fail(k, "a prosody stream needs a resampled chunk pass", "");
-            if (w->v != v) fail(k, "the prosody stream was made for another voice", "");
-            if (w->ended) fail(k, "the prosody stream has already been flushed", "");
-            for (size_t q = 0; q < k; q++)
-                if (p.chunks[q].ps == w)
-                    fail(k, "the prosody stream of chunk " + std::to_string(q) + " appears twice in one call", "");
+            check_stream(k, &ChunkSpec::ps, "prosody stream", c.ps->ended, "the prosody stream has already been flushed");
         }
         if (const LoudnessStream* m = c.ls) {
             if (!p.resample) fail(k, "a loudness stream needs a resampled chunk pass", "");
-            if (m->v != v) fail(k, "the loudness stream was made for another voice", "");
-            for (size_t q = 0; q < k; q++)
-                if (p.chunks[q].ls == m)
-                    fail(k, "the loudness stream of chunk " + std::to_string(q) + " appears twice in one call", "");
+            check_stream(k, &ChunkSpec::ls, "loudness stream", false, "");
             const long long rate = c.rs ? (long long)v->sample_rate * c.rs->f.up / c.rs->f.down : v->sample_rate;
             if (rate != m->rate)
                 fail(k, "the chunk is delivered at " + std::to_string(rate) + " Hz and its loudness stream meters " +
@@ -1659,43 +1258,22 @@ void decode_chunks(Voice* v, const ChunkPass& p, ChunkResult& out) {
         if ((c.rs || c.ps) && c.last != 0 && c.last != 1)
             fail(k, "last flag " + std::to_string(c.last) + " is neither 0 nor 1", "");
     }
-    // samples of each chunk after its trims, what its prosody stream emits for them, and the resample launch
-    // n_res: what the resample launch takes (a warped chunk's output, or its formant stage's)
-    std::vector<long long> n_in(n), n_res(n);
-    std::vector<ProsodyStep> steps(n);
-    std::vector<FormantStep> fsteps(n);
-    std::vector<int> warped, formed, warp_of(n, -1);     // warp_of[k]: chunk k's segment of pp
-    ProsodyPlan pp;
-    FormantPlan fp;
-    ResamplePlan rp;
+    // samples of each chunk after its trims
+    std::vector<long long> n_in(n);
     for (size_t k = 0; k < n; k++) {
         const ChunkSpec& c = p.chunks[k];
         n_in[k] = (c.hi - c.lo - c.trim_lo - c.trim_hi) * hop;
-        n_res[k] = n_in[k];
-        if (c.ps) {
-            steps[k] = prosody_stream_step(*c.ps, n_in[k], c.last != 0);
-            if (prosody_stream_warps(*c.ps)) {
-                pp.add_stream(*c.ps, steps[k]);
-                warp_of[k] = (int)warped.size();
-                warped.push_back((int)k);
-            }
-            n_res[k] = steps[k].j1 - steps[k].j0;
-            if (c.ps->fm) {
-                fsteps[k] = formant_stream_step(*c.ps, steps[k].next.emitted, c.last != 0);
-                fp.add_stream(*c.ps, fsteps[k]);
-                formed.push_back((int)k);
-                n_res[k] = fsteps[k].e1 - fsteps[k].e0;
-            }
-        }
-        if (p.resample) rp.add(c.rs ? &c.rs->f : nullptr, n_res[k], c.rs, c.last != 0);
     }
-    // metered chunks: what the resample launch delivers for them, and the steps that completes
-    MeterPlan mp;
-    for (size_t k = 0; k < n; k++)
-        if (LoudnessStream* m = p.chunks[k].ls) {
-            const long long d = rp.segs[k].n_out;
-            mp.add((int)k, *m, d, loudness_stream_steps(*m, d, "chunk " + std::to_string(k) + ": "));
-        }
+    OutputPlan op = plan_chunk_output(p.chunks, n_in, p.resample);
+    const ResamplePlan& rp = op.rp;
+    // G.711 of resampled chunks: the gain scales the resampled samples just before the conversion, as a volume on the
+    // delivered audio (resampling x * g is not bit for bit resampling x, then times g)
+    // A metered chunk's gain applies after its meter, which the loudness launch does, and it converts at the fixed scale
+    const bool gain_after = p.resample && p.format >= PCM_MULAW;
+    if (gain_after)
+        for (const ChunkSpec& c : p.chunks) op.out_gain.push_back(c.ls ? 1.f : c.gain);
+    if (!op.mp.chunks.empty())
+        for (const ChunkSpec& c : p.chunks) op.fixed_scale.push_back(c.ls ? 1 : 0);
 
     const auto release = [v](Context* c) { v->release(c); };
     const std::unique_ptr<Context, decltype(release)> ctx(v->acquire(), release);
@@ -1704,7 +1282,7 @@ void decode_chunks(Voice* v, const ChunkPass& p, ChunkResult& out) {
     lay_out_frames(l, len, hop, {});
     const size_t total = p.resample ? (size_t)rp.total : (size_t)l.total_samples;
     ChunkBufs b;
-    plan(C.dev_frame, C.pin, [&](Arena& dev, Arena& pin) { b.carve(dev, pin, *v, l, p, rp, pp, fp, mp, total); });
+    plan(C.dev_frame, C.pin, [&](Arena& dev, Arena& pin) { b.carve(dev, pin, *v, l, p, op, total); });
     cudaStream_t st = C.stream;
     std::vector<Region> regions;
     Runner R(*v, C, regions, b.spk.cond);
@@ -1713,18 +1291,6 @@ void decode_chunks(Voice* v, const ChunkPass& p, ChunkResult& out) {
     Level LY = upload_frames(l, b.y, st);
     for (size_t k = 0; k < n; k++) b.src.h[k] = GatherSeg{p.chunks[k].z->z, p.chunks[k].lo, l.fsegs[k].off, len[k]};
     b.src.upload(st);
-    launch_gather_rows(b.src.d, b.y.ftile.d, GY, l.RY, v->a.inter, b.s, st);
-    run_decoder(R, LY, b.y, b.dec, b.s, b.wav);
-    // G.711 of resampled chunks: the gain scales the resampled samples just before the conversion, as a volume on the
-    // delivered audio (resampling x * g is not bit for bit resampling x, then times g)
-    // A metered chunk's gain applies after its meter, which the loudness launch does, and it converts at the fixed scale
-    const bool gain_after = p.resample && p.format >= PCM_MULAW;
-    std::vector<float> out_gain;
-    std::vector<int> fixed_scale;
-    if (gain_after)
-        for (const ChunkSpec& c : p.chunks) out_gain.push_back(c.ls ? 1.f : c.gain);
-    if (!mp.chunks.empty())
-        for (const ChunkSpec& c : p.chunks) fixed_scale.push_back(c.ls ? 1 : 0);
     if (b.post.d) {
         for (size_t k = 0; k < n; k++) {
             PcmPost& q = b.post.h[k];
@@ -1736,128 +1302,22 @@ void decode_chunks(Voice* v, const ChunkPass& p, ChunkResult& out) {
         }
         b.post.upload(st);
     }
-    // warped chunks: prosody on the post-path's samples, then the resample launch reads its output (n samples at
-    // `off` as a segment of ceil(n / hop) frames less a trim, with no post-path of its own); chunks with a formant
-    // stage: the stage on that output (or on the post-path's samples), and the resample launch reads the stage's output
-    const FrameSeg* rs_in = b.y.fsegs.d; const PcmPost* rs_post = b.post.d;
-    float* py = b.wav + l.total_samples;
-    const auto resample_from = [&](int k, long long off, long long m) {
-        const long long frames = (m + hop - 1) / hop;
-        b.rin.h[k] = FrameSeg{0, (int)frames, 0, 0, off};
-        b.rpost.h[k] = PcmPost();
-        b.rpost.h[k].trim_hi = frames * hop - m;
-    };
-    if (!warped.empty() || !formed.empty()) {
-        std::copy(l.fsegs.begin(), l.fsegs.end(), b.rin.h);
-        std::copy(b.post.h, b.post.h + n, b.rpost.h);
-    }
-    if (!warped.empty()) {
-        b.pr.upload(pp, st);
-        for (size_t q = 0; q < warped.size(); q++)
-            b.pr.carry.h[q] = prosody_carry(*p.chunks[warped[q]].ps, steps[warped[q]], warped[q]);
-        b.pr.carry.upload(st);
-        R.begin("stretch");
-        launch_prosody_stream_stretch(pp, b.pr.segs.d, b.pr.carry.d, b.wav, b.y.fsegs.d, b.post.d, hop, b.pr.x, b.pr.s,
-                                      b.pr.offsets, py, st, b.pr.apos);
-        R.count(pp.stretch_flops, pp.stretch_bytes, 2 + (pp.smem_ints ? 1 : 0) + (pp.max_ola ? 1 : 0));
-        R.end();
-        if (pp.max_pitch) {
-            R.begin("pitch");
-            launch_prosody_pitch(b.pr.x, b.pr.s, b.pr.segs.d, (int)warped.size(), pp.max_pitch, py, st);
-            R.count(pp.pitch_flops, pp.pitch_bytes);
-            R.end();
-        }
-        for (size_t q = 0; q < warped.size(); q++) {
-            const ProsodySeg& g = pp.segs[q];
-            resample_from(warped[q], l.total_samples + g.y_off, g.j1 - g.j0);
-        }
-    }
-    if (!formed.empty()) {
-        float* fy = py + pp.y_total;
-        std::copy(fp.segs.begin(), fp.segs.end(), b.fsegs.h);
-        b.fsegs.upload(st);
-        for (size_t q = 0; q < formed.size(); q++) {
-            const int k = formed[q], w = warp_of[k];
-            b.fcarry.h[q] = formant_carry(*p.chunks[k].ps, fsteps[k], k, w < 0 ? nullptr : py + pp.segs[w].y_off);
-        }
-        b.fcarry.upload(st);
-        R.begin("formant");
-        launch_formant_stream(fp, b.fsegs.d, b.fcarry.d, b.wav, b.y.fsegs.d, b.post.d, hop, b.fwin, fy, st);
-        R.count(fp.flops, fp.bytes, fp.max_runs ? 2 : 1);
-        R.end();
-        for (size_t q = 0; q < formed.size(); q++)
-            resample_from(formed[q], l.total_samples + pp.y_total + fp.segs[q].y_off,
-                          fsteps[formed[q]].e1 - fsteps[formed[q]].e0);
-    }
-    if (!warped.empty() || !formed.empty()) {
-        b.rin.upload(st);
-        b.rpost.upload(st);
-        rs_in = b.rin.d; rs_post = b.rpost.d;
-    }
-    if (p.resample) {
-        b.rt.upload(rp, st, gain_after ? &out_gain : nullptr, fixed_scale.empty() ? nullptr : &fixed_scale);
-        run_resample(R, rp, b.rt, b.wav, rs_in, rs_post, hop, b.rs);
-        if (!mp.chunks.empty()) {
-            double window = 0, samples = 0;
-            for (size_t q = 0; q < mp.chunks.size(); q++) {
-                const int k = mp.chunks[q];
-                LoudStreamSeg g = loudness_stream_seg(*p.chunks[k].ls, b.rs + rp.segs[k].out_off, mp.n[q],
-                                                      p.chunks[k].gain);
-                g.win = b.lwin + mp.win_off[q]; g.e = b.le + 8 * mp.step_off[q];
-                g.lufs = b.llufs.d + mp.step_off[q]; g.gains = b.lgains.d + mp.step_off[q]; g.clipped = b.lclip.d + q;
-                b.lsegs.h[q] = g;
-                window += (double)(g.p + g.n);
-                samples += (double)g.n;
-            }
-            b.lsegs.upload(st);
-            R.begin("loudness");
-            launch_loudness_stream(b.lsegs.d, (int)mp.chunks.size(), st);
-            // the window filtered twice; read, staged, read again and written
-            R.count(2.0 * 22.0 * window, 4.0 * (3.0 * window + samples));
-            R.end();
-            b.llufs.download(st); b.lgains.download(st); b.lclip.download(st);
-        }
-        if (b.pcm) launch_pcm(b.rs, b.rt.osegs.d, b.rt.posts.d, (int)n, 1, rp.max_out, b.max, p.format, b.pcm, st);
-    } else if (b.pcm) {
-        launch_pcm(b.wav, b.y.fsegs.d, b.post.d, (int)n, hop, (long long)*std::max_element(len.begin(), len.end()) * hop,
-                   b.max, p.format, b.pcm, st);
+    b.out.upload(op, hop, l.fsegs.data(), b.post.h, st);
+    launch_gather_rows(b.src.d, b.y.ftile.d, GY, l.RY, v->a.inter, b.s, st);
+    run_decoder(R, LY, b.y, b.dec, b.s, b.out.in);
+    const Wave res = run_output_stage(R, op, b.out, Wave{b.out.in, b.y.fsegs.d, b.post.d, hop}, st);
+    if (b.pcm) {
+        const long long longest = p.resample ? rp.max_out : (long long)*std::max_element(len.begin(), len.end()) * hop;
+        launch_pcm(res.buf, res.segs, res.posts, (int)n, res.hop, longest, b.max, p.format, b.pcm, st);
     }
     SB_CUDA(cudaEventRecord(C.ev_end, st));
-    const void* res = b.pcm ? (const void*)b.pcm : b.rs ? (const void*)b.rs : (const void*)b.wav;
-    SB_CUDA(cudaMemcpyAsync(b.out_h, res, total * pcm_bytes(p.format), cudaMemcpyDeviceToHost, st));
+    SB_CUDA(cudaMemcpyAsync(b.out_h, b.pcm ? b.pcm : (const void*)res.buf, total * pcm_bytes(p.format),
+                            cudaMemcpyDeviceToHost, st));
     SB_CUDA(cudaStreamSynchronize(st));
     SB_CUDA(cudaGetLastError());
-
-    for (size_t k = 0; k < n; k++) {
-        Resampler* r = p.chunks[k].rs;
-        if (!r) continue;
-        const ResampleSeg& s = rp.segs[k];
-        r->consumed = s.c + n_res[k];
-        r->emitted = s.j0 + s.n_out;
-        r->cur ^= 1;
-        r->h = s.h_out;
-        r->ended = p.chunks[k].last != 0;
-    }
-    for (Region& g : regions) {
-        if (g.name != "stretch" && g.name != "pitch" && g.name != "formant" && g.name != "loudness") continue;
-        cudaEventElapsedTime(&g.ms, g.e0, g.e1);
-        (g.name == "stretch" ? out.stretch_ms : g.name == "pitch" ? out.pitch_ms
-                                              : g.name == "formant" ? out.formant_ms : out.loudness_ms) = g.ms;
-    }
-    for (size_t q = 0; q < mp.chunks.size(); q++) {
-        LoudnessStream* m = p.chunks[mp.chunks[q]].ls;
-        loudness_stream_advance(*m, mp.n[q], b.llufs.h + mp.step_off[q], b.lgains.h + mp.step_off[q], b.lclip.h[q]);
-        m->last_ms = out.loudness_ms;
-    }
-    for (size_t k = 0; k < n; k++) {
-        ProsodyStream* w = p.chunks[k].ps;
-        if (!w) continue;
-        if (w->fm) formant_stream_advance(*w, fsteps[k]);
-        prosody_stream_advance(*w, steps[k], p.chunks[k].last != 0);
-        const bool warps = prosody_stream_warps(*w);
-        w->last_ms[0] = warps ? out.stretch_ms : 0.f; w->last_ms[1] = warps ? out.pitch_ms : 0.f;
-        w->last_fm_ms = w->fm ? out.formant_ms : 0.f;
-    }
+    advance_streams(op, b.out, R);
+    out.stretch_ms = R.ms("stretch"); out.pitch_ms = R.ms("pitch");
+    out.formant_ms = R.ms("formant"); out.loudness_ms = R.ms("loudness");
     if (p.format == PCM_I16) out.i16.resize(n); else if (b.pcm) out.g711.resize(n); else out.f32.resize(n);
     for (size_t k = 0; k < n; k++) {
         const long long o = p.resample ? rp.segs[k].out_off : l.fsegs[k].out_off;

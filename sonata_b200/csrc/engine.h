@@ -424,6 +424,26 @@ struct Arena {
     void release();
 };
 
+// Each workspace hands out its buffers in one carve(dev, pin).  plan() runs it on dry arenas to learn the sizes, makes
+// room in the arenas and carves again for real, so no size is written down twice.
+template <typename Carve> void plan(Arena& dev, Arena& pin, Carve&& carve) {
+    Arena dry_dev, dry_pin;
+    dry_dev.dry = dry_pin.dry = true;
+    carve(dry_dev, dry_pin);
+    dev.reserve(dry_dev.used);
+    pin.reserve(dry_pin.used);
+    carve(dev, pin);
+}
+
+// A table the host fills and the device reads, or the reverse: the device table `d` and its page-locked mirror `h`,
+// carved together with one element count, so every copy moves exactly the carved table.  Unset (null) when not carved.
+template <typename T> struct Staged {
+    T* d = nullptr; T* h = nullptr; size_t n = 0;
+    void carve(Arena& dev, Arena& pin, size_t count) { n = count; d = dev.get<T>(n); h = pin.get<T>(n); }
+    void upload(cudaStream_t st) const { SB_CUDA(cudaMemcpyAsync(d, h, n * sizeof(T), cudaMemcpyHostToDevice, st)); }
+    void download(cudaStream_t st) const { SB_CUDA(cudaMemcpyAsync(h, d, n * sizeof(T), cudaMemcpyDeviceToHost, st)); }
+};
+
 struct Context {
     int device = 0;
     cudaStream_t stream = nullptr;
@@ -434,6 +454,21 @@ struct Context {
     cudaEvent_t ev_begin = nullptr, ev_end = nullptr;
     cudaEvent_t next_event();
     ~Context();
+};
+
+// The profile of a pass: each region between begin() and end() records its device time on a pair of the context's
+// events and counts the flops, bytes and launches of the launches made inside it.  Without a region list it records
+// nothing (the test hooks).
+struct Profile {
+    Context* c = nullptr; std::vector<Region>* regions = nullptr; cudaStream_t st = nullptr;
+    Region* cur = nullptr;
+    void begin(const std::string& name);
+    void end();
+    void count(double flops, double bytes, int launches = 1) {
+        if (cur) { cur->flops += flops; cur->bytes += bytes; cur->launches += launches; }
+    }
+    // After the pass has synchronised: the device time of the region `name` (0 when none ran).
+    float ms(const std::string& name) const;
 };
 
 struct Level {          // one time resolution of the packed batch
@@ -510,7 +545,7 @@ struct Job {
     // with either, one segment of len = its delivered samples per utterance at out_hop = 1.
     std::vector<FrameSeg> osegs; int out_hop = 1; long long out_total = 0;
     std::vector<int> osr;             // sample rate of each handed-out utterance
-    FrameSeg* d_osegs = nullptr;
+    const FrameSeg* d_osegs = nullptr;
     std::map<std::string, std::pair<float*, int>> dbg;   // name -> (device ptr, cols)
     std::map<std::string, int> dbg_level;                // name -> U (rows per frame), 0 for X level, -1 for an X-level
                                                          // buffer stored transposed ([cols][RX])
@@ -660,6 +695,105 @@ struct ChunkResult {
     std::vector<ChunkCapture> captures;       // ChunkPass::debug only
 };
 void decode_chunks(Voice* v, const ChunkPass& p, ChunkResult& out);
+
+// ---- the waveform output stage (output_stage.cu) ----
+// After the decoder: prosody (stretch, pitch), formants, resampling, then loudness in place on what that leaves.
+
+// What a stage reads: segment k is buf[segs[k].out_off ..), segs[k].len * hop samples read through posts[k] (trims,
+// fade, gain; null: read plainly).  The whole-signal prosody and formant launches read buf at their plans' offsets.
+struct Wave {
+    float* buf = nullptr;
+    const FrameSeg* segs = nullptr;
+    const PcmPost* posts = nullptr;
+    int hop = 1;
+};
+
+// One resample launch over segments laid out back to back: each segment's ResampleSeg, what the launch is sized by and
+// what the profile counts.
+struct ResamplePlan {
+    std::vector<ResampleSeg> segs;
+    long long total = 0, max_out = 0; int smem = 0;
+    double flops = 0, bytes = 0;
+    // Appends a segment of n_in inputs through `f` (null: copied unchanged).  A whole signal emits every output; with a
+    // stream's resampler `r` (whose filter is f) the segment continues r's stream, emits every output whose inputs have
+    // all arrived, and flushes the stream when `last`.
+    void add(const ResampleFilter* f, long long n_in, const Resampler* r = nullptr, bool last = false);
+};
+
+// The loudness launch over what a job hands out: one segment per utterance at its delivered rate, chunk scratch laid out
+// back to back.
+struct LoudnessPlan {
+    std::vector<LoudSeg> segs;
+    long long chunks = 0;
+};
+
+// The metered chunks of a chunk pass: chunks[q] has n[q] samples, its window at win_off[q] of the pass's window buffer
+// and the steps[q] steps it completes at step_off[q] of its step tables.
+struct MeterPlan {
+    std::vector<int> chunks;
+    std::vector<long long> n, win_off, step_off, steps;
+    long long win_total = 0, steps_total = 0;
+    void add(int k, const LoudnessStream& s, long long samples, long long completes);
+};
+
+// The output stage of one pass.  A job's (plan_job_output) runs each stage on whole utterances; a chunk pass's
+// (plan_chunk_output) runs each chunk's streams, one window each, and keeps the chunks and their steps so the streams
+// can advance after the pass.  An empty plan of either kind runs nothing.
+struct OutputPlan {
+    ProsodyPlan pp;
+    FormantPlan fp;
+    ResamplePlan rp;
+    LoudnessPlan lp;                          // whole signals
+    MeterPlan mp;                             // chunk passes
+    std::vector<ChunkSpec> chunks;            // chunk passes: empty for a job
+    std::vector<ProsodyStep> steps;           // per chunk with a prosody stream
+    std::vector<FormantStep> fsteps;          // per chunk whose stream runs the formant stage
+    std::vector<int> warped, formed, warp_of; // the chunks of pp's and fp's segments; warp_of[k]: chunk k's segment of pp
+    std::vector<long long> n_res;             // per chunk: the samples the resample launch takes
+    std::vector<float> out_gain;              // per chunk (or empty): the gain of its resampled output's PcmPost
+    std::vector<int> fixed_scale;             // per chunk (or empty): that PcmPost's fixed_scale
+    bool streams() const { return !chunks.empty(); }
+};
+// The output stage of job j's utterances on the frame layout j.frames with `hop` samples per frame, and what the job
+// hands out (osegs, out_hop, out_total, osr).  With a contour (cum: the batch's cum rows on the host) every utterance is
+// planned from its ids' ends, and bounds receives each id's delivered end, packed like the ids.
+OutputPlan plan_job_output(Job& j, int hop, const std::vector<int>& cum, std::vector<long long>& bounds);
+// The output stage of chunk pass chunks, chunk k bringing n_in[k] samples after its trims: each chunk's prosody stream,
+// its formant stage, with `resample` the resample launch (a chunk without a resampler is copied), and its meter, which
+// reads what the resample launch delivers (without it: the chunk's stage output).
+OutputPlan plan_chunk_output(const std::vector<ChunkSpec>& chunks, const std::vector<long long>& n_in, bool resample);
+
+// The device buffers and tables of plan p and their pinned mirrors.  `in` is where the stage's input goes (the decoder's
+// waveforms, in_total samples): a buffer of the pass's own, followed by the prosody output `py` and the formant output
+// `fy`, or the caller's d_out when no stage writes a result of its own.  With d_out the last stage that writes writes
+// there; the resample output `ry` is otherwise the pass's own.  offsets, ps (the stretched signal) and py stay
+// reachable after the pass.
+struct OutputBufs {
+    Staged<ProsodySeg> psegs; Staged<FrameSeg> posegs; Staged<ProsodyCarry> pcarry;
+    Staged<ContourPiece> pieces;              // the contours' piece tables (only when a segment has one)
+    long long* apos = nullptr;                // and their analysis positions, indexed like the offsets
+    int* offsets = nullptr; float *px = nullptr, *ps = nullptr, *py = nullptr;
+    Staged<FormantSeg> fsegs; Staged<FormantCarry> fcarry; float *fwin = nullptr, *fy = nullptr;
+    Staged<FrameSeg> rin; Staged<PcmPost> rpost;  // chunk passes: what the resample launch reads after the stages
+    Staged<ResampleSeg> rsegs; Staged<PcmPost> rposts; Staged<FrameSeg> rosegs; float* ry = nullptr;
+    Staged<LoudSeg> lsegs; double* lscratch = nullptr; Staged<double> lufs; Staged<float> gain;
+    Staged<LoudStreamSeg> msegs; float* mwin = nullptr; double* me = nullptr;
+    Staged<double> mlufs; Staged<float> mgains; Staged<unsigned long long> mclip;
+    float* in = nullptr;
+    void carve(Arena& dev, Arena& pin, const OutputPlan& p, long long in_total, float* d_out);
+    // Fills and uploads every table.  A chunk pass's input is read at `hop` samples per frame through the host mirrors
+    // of its segment and post tables (in_segs, in_posts; null posts: read plainly); a job's needs neither.
+    void upload(const OutputPlan& p, int hop, const FrameSeg* in_segs, const PcmPost* in_posts, cudaStream_t st);
+};
+
+// The launches of plan p from the input wave `in` (in.buf == b.in) on st: profile regions "stretch", "pitch",
+// "formant", "resample" and "loudness", each only when its stage runs.  Returns what the stage delivers: the last
+// output's wave (a job's: its segments at hop 1 once a stage has changed their lengths).  The loudness results are
+// downloaded to their pinned mirrors.
+Wave run_output_stage(Profile& prof, const OutputPlan& p, const OutputBufs& b, Wave in, cudaStream_t st);
+// After a chunk pass's plan p has run and synchronised: its resamplers, prosody and formant stages and meters take their
+// new counts, and each stream the region times of the pass in prof.
+void advance_streams(const OutputPlan& p, const OutputBufs& b, const Profile& prof);
 
 void job_pcm16(Job& j, float gain, std::vector<std::vector<int16_t>>& out);
 // Peak-normalised 16-bit PCM of every utterance of a finished job (to_i16_vec after a linear gain), converted on the

@@ -1,0 +1,412 @@
+// The waveform output stage: what runs after the decoder, in this order: prosody (the stretch and the pitch stage), the
+// formant stage, resampling, and loudness in place on what those leave.  Jobs, chunk passes and the test hooks plan,
+// carve and launch it here only, so they run the same launches.
+#include "engine.h"
+#include <algorithm>
+#include <cmath>
+
+namespace sb200 {
+
+void ResamplePlan::add(const ResampleFilter* f, long long n_in, const Resampler* r, bool last) {
+    ResampleSeg s{};
+    s.out_off = total; s.n_out = n_in; s.down = 1;
+    if (f) {
+        const long long N = (r ? r->consumed : 0) + n_in;
+        s.taps = f->taps; s.up = f->up; s.down = f->down; s.H = f->H; s.K = f->K;
+        s.n_out = resample_emit_end(*f, N, !r || last) - (r ? r->emitted : 0);
+        if (r) {
+            s.hist = r->hist[r->cur]; s.hist_out = r->hist[1 - r->cur];
+            s.c = r->consumed; s.j0 = r->emitted; s.h = r->h; s.h_out = (int)std::min<long long>(N, f->K - 1);
+        }
+    }
+    bytes += 4.0 * ((double)n_in + s.n_out);
+    if (f) {
+        smem = std::max(smem, resample_span(f->up, f->down, f->K));
+        flops += 2.0 * (double)s.n_out * (2.0 * f->H + 1.0) / f->up;
+        bytes += 4.0 * (double)f->up * f->K;
+    }
+    max_out = std::max(max_out, s.n_out);
+    total += s.n_out;
+    segs.push_back(s);
+}
+
+void MeterPlan::add(int k, const LoudnessStream& s, long long samples, long long completes) {
+    chunks.push_back(k); n.push_back(samples);
+    win_off.push_back(win_total); step_off.push_back(steps_total); steps.push_back(completes);
+    win_total += s.samples - s.steps * s.d.S + samples;
+    steps_total += completes;
+}
+
+OutputPlan plan_job_output(Job& j, int hop, const std::vector<int>& cum, std::vector<long long>& bounds) {
+    OutputPlan o;
+    const size_t B = j.B;
+    const std::vector<FrameSeg>& fs = j.frames.fsegs;
+    const bool audio = !j.encode_only;
+    // prosody: every utterance's decoder waveform, with its ratios or NaN, or with a contour planned from its ids' ends
+    ProsodyPlan& pp = o.pp;
+    bounds.clear();
+    if (audio && j.contour.empty() && !j.pitch.empty()) {
+        for (size_t b = 0; b < B; b++) {
+            const long long n = (long long)fs[b].len * hop;
+            pp.add(prosody_shape(j.v->sample_rate, n, j.pitch[b], j.tempo[b]), fs[b].out_off, n);
+        }
+    } else if (audio && !j.contour.empty()) {
+        bounds.resize(j.ids.size());
+        std::vector<long long> ends;
+        std::vector<ContourPiece> pieces;
+        for (size_t b = 0; b < B; b++) {
+            const long long n = (long long)fs[b].len * hop;
+            const size_t n_ids = j.offs[b + 1] - j.offs[b];
+            ends.resize(n_ids);
+            for (size_t i = 0; i < n_ids; i++) ends[i] = (long long)cum[j.xsegs[b].off + i] * hop;
+            const float* r = j.contour.data() + j.offs[b];
+            const bool has = std::any_of(r, r + n_ids, [](float v) { return !std::isnan(v) && v != 1.f; });
+            const float pitch = j.pitch.empty() ? NAN : j.pitch[b], tempo = j.tempo.empty() ? NAN : j.tempo[b];
+            const ProsodyShape sh = prosody_contour_plan(j.v->sample_rate, n, ends.data(), has ? r : nullptr, n_ids,
+                                                         pitch, tempo, pieces, bounds.data() + j.offs[b]);
+            pp.add(sh, fs[b].out_off, n, &pieces);
+        }
+    }
+    // formants: each asking utterance's output of the pitch stage (or its decoder waveform), with its pitch ratio or
+    // contour, in that stage's layout; the utterances that do not ask are copied into it
+    if (audio && !j.formant.empty()) {
+        FormantPlan& fp = o.fp;
+        fp.total = pp.segs.empty() ? j.frames.total_samples : pp.y_total;
+        for (size_t b = 0; b < B; b++) {
+            long long in_off = fs[b].out_off, n = (long long)fs[b].len * hop;
+            double ratio = 1.0;
+            int c_off = 0, c_n = 0;
+            if (!pp.segs.empty()) {
+                const ProsodySeg& g = pp.segs[b];
+                in_off = g.y_off; n = g.n2; ratio = g.p; c_off = g.c_off; c_n = g.c_n;
+            }
+            if (formant_asks(n, j.formant[b], ratio, pp.pieces.data() + c_off, c_n))
+                fp.add(j.v->sample_rate, in_off, n, j.formant[b], ratio, c_off, c_n);
+            else
+                fp.copy(in_off, n);
+        }
+        if (fp.segs.empty()) fp = FormantPlan();
+    }
+    // what the job hands out: the frame layout itself, the prosody output (the formant stage keeps its layout), or with
+    // output rates one resampled segment per utterance at its rate, back to back
+    j.osr.assign(B, j.v->sample_rate);
+    if (j.out_rates.empty() || !audio) {
+        j.osegs = fs; j.out_hop = hop; j.out_total = j.frames.total_samples;
+        if (!pp.segs.empty()) {
+            for (size_t b = 0; b < B; b++) j.osegs[b] = FrameSeg{0, (int)pp.segs[b].n2, 0, 0, pp.segs[b].y_off};
+            j.out_hop = 1; j.out_total = pp.y_total;
+        }
+    } else {
+        j.osegs.assign(B, FrameSeg{});
+        for (size_t b = 0; b < B; b++) {
+            const ResampleFilter* f = nullptr;
+            if (j.out_rates[b]) {
+                j.osr[b] = j.out_rates[b];
+                f = &voice_resampler(*j.v, j.out_rates[b], "utterance " + std::to_string(b) + ": ");
+            }
+            o.rp.add(f, pp.segs.empty() ? (long long)fs[b].len * hop : pp.segs[b].n2);
+            j.osegs[b] = FrameSeg{0, (int)o.rp.segs[b].n_out, 0, 0, o.rp.segs[b].out_off};
+        }
+        j.out_hop = 1; j.out_total = o.rp.total;
+    }
+    // loudness: every utterance as the job hands it out, at its rate, with its target or NaN
+    if (audio && !j.loud_target.empty()) {
+        LoudnessPlan& lp = o.lp;
+        lp.segs.resize(B);
+        for (size_t b = 0; b < B; b++) {
+            LoudSeg& s = lp.segs[b];
+            loudness_design(j.osr[b], s);
+            s.off = j.osegs[b].out_off;
+            s.n = (long long)j.osegs[b].len * j.out_hop;
+            s.c0 = lp.chunks;
+            s.target = j.loud_target[b];
+            lp.chunks += (s.n + s.S - 1) / s.S;
+        }
+    }
+    return o;
+}
+
+OutputPlan plan_chunk_output(const std::vector<ChunkSpec>& chunks, const std::vector<long long>& n_in, bool resample) {
+    OutputPlan o;
+    const size_t n = chunks.size();
+    o.chunks = chunks;
+    o.steps.resize(n); o.fsteps.resize(n); o.warp_of.assign(n, -1);
+    o.n_res = n_in;
+    for (size_t k = 0; k < n; k++) {
+        const ChunkSpec& c = chunks[k];
+        if (c.ps) {
+            o.steps[k] = prosody_stream_step(*c.ps, n_in[k], c.last != 0);
+            if (prosody_stream_warps(*c.ps)) {
+                o.pp.add_stream(*c.ps, o.steps[k]);
+                o.warp_of[k] = (int)o.warped.size();
+                o.warped.push_back((int)k);
+            }
+            o.n_res[k] = o.steps[k].j1 - o.steps[k].j0;
+            if (c.ps->fm) {
+                o.fsteps[k] = formant_stream_step(*c.ps, o.steps[k].next.emitted, c.last != 0);
+                o.fp.add_stream(*c.ps, o.fsteps[k]);
+                o.formed.push_back((int)k);
+                o.n_res[k] = o.fsteps[k].e1 - o.fsteps[k].e0;
+            }
+        }
+        if (resample) o.rp.add(c.rs ? &c.rs->f : nullptr, o.n_res[k], c.rs, c.last != 0);
+    }
+    for (size_t k = 0; k < n; k++)
+        if (const LoudnessStream* m = chunks[k].ls) {
+            const long long d = resample ? o.rp.segs[k].n_out : o.n_res[k];
+            o.mp.add((int)k, *m, d, loudness_stream_steps(*m, d, "chunk " + std::to_string(k) + ": "));
+        }
+    return o;
+}
+
+void OutputBufs::carve(Arena& dev, Arena& pin, const OutputPlan& p, long long in_total, float* d_out) {
+    *this = OutputBufs();
+    const ProsodyPlan& pp = p.pp;
+    const FormantPlan& fp = p.fp;
+    if (const size_t n = pp.segs.size()) {
+        psegs.carve(dev, pin, n);
+        if (!pp.pieces.empty()) pieces.carve(dev, pin, pp.pieces.size());     // a stream's table is its own
+        if (pp.contour) apos = dev.get<long long>((size_t)pp.d_total);
+        if (p.streams()) {
+            pcarry.carve(dev, pin, n);
+            px = dev.get<float>((size_t)pp.in_total + 4);
+        } else {
+            posegs.carve(dev, pin, n);
+        }
+        offsets = pp.d_total ? dev.get<int>((size_t)pp.d_total) : nullptr;
+        ps = pp.s_total ? dev.get<float>((size_t)pp.s_total + 4) : nullptr;
+    }
+    if (const size_t n = fp.segs.size()) {
+        fsegs.carve(dev, pin, n);
+        if (p.streams()) {
+            fcarry.carve(dev, pin, n);
+            fwin = dev.get<float>((size_t)fp.in_total + 4);
+        }
+    }
+    if (p.streams() && (!pp.segs.empty() || !fp.segs.empty())) {
+        rin.carve(dev, pin, p.chunks.size());
+        rpost.carve(dev, pin, p.chunks.size());
+    }
+    if (const size_t n = p.rp.segs.size()) {
+        rsegs.carve(dev, pin, n); rposts.carve(dev, pin, n); rosegs.carve(dev, pin, n);
+    }
+    if (const size_t n = p.lp.segs.size()) {
+        lsegs.carve(dev, pin, n);
+        lscratch = dev.get<double>((size_t)LD_SCRATCH * std::max<long long>(p.lp.chunks, 1));
+        lufs.carve(dev, pin, n); gain.carve(dev, pin, n);
+    }
+    if (const size_t m = p.mp.chunks.size()) {
+        const size_t steps = (size_t)std::max<long long>(p.mp.steps_total, 1);
+        msegs.carve(dev, pin, m);
+        mwin = dev.get<float>((size_t)p.mp.win_total + 4);
+        me = dev.get<double>(8 * steps);
+        mlufs.carve(dev, pin, steps); mgains.carve(dev, pin, steps); mclip.carve(dev, pin, m);
+    }
+    const bool staged = !pp.segs.empty() || !fp.segs.empty() || !p.rp.segs.empty();
+    in = staged || !d_out ? dev.get<float>((size_t)(in_total + pp.y_total + fp.total) + 4) : d_out;
+    py = in + in_total;
+    fy = py + pp.y_total;
+    if (!p.rp.segs.empty()) ry = d_out ? d_out : dev.get<float>((size_t)p.rp.total + 4);
+    else if (d_out && !fp.segs.empty()) fy = d_out;
+    else if (d_out && !pp.segs.empty()) py = d_out;
+}
+
+void OutputBufs::upload(const OutputPlan& p, int hop, const FrameSeg* in_segs, const PcmPost* in_posts,
+                        cudaStream_t st) {
+    const ProsodyPlan& pp = p.pp;
+    const FormantPlan& fp = p.fp;
+    const size_t n = p.chunks.size();
+    if (psegs.d) {
+        std::copy(pp.segs.begin(), pp.segs.end(), psegs.h);
+        psegs.upload(st);
+        if (posegs.d) {
+            for (size_t k = 0; k < pp.segs.size(); k++) posegs.h[k] = FrameSeg{0, (int)pp.segs[k].n2, 0, 0, pp.segs[k].y_off};
+            posegs.upload(st);
+        }
+        if (pieces.d) {
+            std::copy(pp.pieces.begin(), pp.pieces.end(), pieces.h);
+            pieces.upload(st);
+        }
+        if (pcarry.d) {
+            for (size_t q = 0; q < p.warped.size(); q++) {
+                const int k = p.warped[q];
+                pcarry.h[q] = prosody_carry(*p.chunks[k].ps, p.steps[k], k);
+            }
+            pcarry.upload(st);
+        }
+    }
+    if (fsegs.d) {
+        std::copy(fp.segs.begin(), fp.segs.end(), fsegs.h);
+        fsegs.upload(st);
+        if (fcarry.d) {
+            for (size_t q = 0; q < p.formed.size(); q++) {
+                const int k = p.formed[q], w = p.warp_of[k];
+                fcarry.h[q] = formant_carry(*p.chunks[k].ps, p.fsteps[k], k, w < 0 ? nullptr : py + pp.segs[w].y_off);
+            }
+            fcarry.upload(st);
+        }
+    }
+    // chunk passes: where each chunk's samples are after the stages, its input or its last stage's output
+    std::vector<float*> at(n);
+    for (size_t k = 0; k < n; k++) at[k] = in + in_segs[k].out_off;
+    for (size_t q = 0; q < p.warped.size(); q++) at[p.warped[q]] = py + pp.segs[q].y_off;
+    for (size_t q = 0; q < p.formed.size(); q++) at[p.formed[q]] = fy + fp.segs[q].y_off;
+    if (rin.d) {
+        // a chunk a stage ran on is read from that stage's output: its m samples as a segment of ceil(m / hop) frames
+        // less a trim, with no post-path of its own
+        for (size_t k = 0; k < n; k++) {
+            rin.h[k] = in_segs[k];
+            rpost.h[k] = in_posts ? in_posts[k] : PcmPost();
+            if (!p.chunks[k].ps) continue;
+            const long long m = p.n_res[k], frames = (m + hop - 1) / hop;
+            rin.h[k] = FrameSeg{0, (int)frames, 0, 0, at[k] - in};
+            rpost.h[k] = PcmPost();
+            rpost.h[k].trim_hi = frames * hop - m;
+        }
+        rin.upload(st);
+        rpost.upload(st);
+    }
+    if (rsegs.d) {
+        // identity posts, for a launch whose input has no post-path or for the PCM conversion of its output
+        for (size_t k = 0; k < p.rp.segs.size(); k++) {
+            rsegs.h[k] = p.rp.segs[k];
+            rposts.h[k] = PcmPost();
+            if (!p.out_gain.empty()) rposts.h[k].gain = p.out_gain[k];
+            if (!p.fixed_scale.empty()) rposts.h[k].fixed_scale = p.fixed_scale[k];
+            rosegs.h[k] = FrameSeg{0, (int)p.rp.segs[k].n_out, 0, 0, p.rp.segs[k].out_off};
+        }
+        rsegs.upload(st); rposts.upload(st); rosegs.upload(st);
+    }
+    if (lsegs.d) {
+        std::copy(p.lp.segs.begin(), p.lp.segs.end(), lsegs.h);
+        lsegs.upload(st);
+    }
+    if (msegs.d) {
+        // a metered chunk is what the resample launch delivers for it, or without one its samples after the stages
+        const MeterPlan& mp = p.mp;
+        for (size_t q = 0; q < mp.chunks.size(); q++) {
+            const int k = mp.chunks[q];
+            float* y = ry ? ry + p.rp.segs[k].out_off : at[k];
+            LoudStreamSeg g = loudness_stream_seg(*p.chunks[k].ls, y, mp.n[q], p.chunks[k].gain);
+            g.win = mwin + mp.win_off[q]; g.e = me + 8 * mp.step_off[q];
+            g.lufs = mlufs.d + mp.step_off[q]; g.gains = mgains.d + mp.step_off[q]; g.clipped = mclip.d + q;
+            msegs.h[q] = g;
+        }
+        msegs.upload(st);
+    }
+}
+
+Wave run_output_stage(Profile& prof, const OutputPlan& p, const OutputBufs& b, Wave in, cudaStream_t st) {
+    const bool streams = p.streams();
+    // a chunk pass's later stages read every chunk from one table: the stage outputs of its staged chunks, the input
+    // of the others
+    const Wave restaged{in.buf, b.rin.d, b.rpost.d, in.hop};
+    Wave cur = in;
+    const ProsodyPlan& pp = p.pp;
+    if (const int n = (int)pp.segs.size()) {
+        prof.begin("stretch");
+        if (streams) {
+            launch_prosody_stream_stretch(pp, b.psegs.d, b.pcarry.d, in.buf, in.segs, in.posts, in.hop, b.px, b.ps,
+                                          b.offsets, b.py, st, b.apos);
+            prof.count(pp.stretch_flops, pp.stretch_bytes, 2 + (pp.smem_ints ? 1 : 0) + (pp.max_ola ? 1 : 0));
+        } else {
+            // the offset chain and the overlap-add, which also copies the segments without a ratio
+            if (pp.smem_ints)
+                launch_prosody_offsets(in.buf, b.psegs.d, n, pp.smem_ints, b.offsets, st, b.pieces.d, b.apos);
+            launch_prosody_ola(in.buf, b.psegs.d, n, pp.max_ola, b.offsets, b.ps, b.py, st, b.apos);
+            prof.count(pp.stretch_flops, pp.stretch_bytes, pp.smem_ints ? 2 : 1);
+        }
+        prof.end();
+        if (pp.max_pitch) {
+            prof.begin("pitch");
+            launch_prosody_pitch(streams ? b.px : in.buf, b.ps, b.psegs.d, n, pp.max_pitch, b.py, st, b.pieces.d);
+            prof.count(pp.pitch_flops, pp.pitch_bytes);
+            prof.end();
+        }
+        cur = streams ? restaged : Wave{b.py, b.posegs.d, nullptr, 1};
+    }
+    const FormantPlan& fp = p.fp;
+    if (!fp.segs.empty()) {
+        prof.begin("formant");
+        if (streams) {
+            launch_formant_stream(fp, b.fsegs.d, b.fcarry.d, in.buf, in.segs, in.posts, in.hop, b.fwin, b.fy, st);
+            prof.count(fp.flops, fp.bytes, fp.max_runs ? 2 : 1);
+        } else {
+            for (const auto& c : fp.copies)
+                SB_CUDA(cudaMemcpyAsync(b.fy + c.first, cur.buf + c.first, (size_t)c.second * 4, cudaMemcpyDeviceToDevice,
+                                        st));
+            launch_formant(cur.buf, b.fsegs.d, (int)fp.segs.size(), fp.max_runs, b.pieces.d, b.fy, st);
+            prof.count(fp.flops, fp.bytes);
+        }
+        prof.end();
+        cur = streams ? restaged : Wave{b.fy, cur.segs, cur.posts, cur.hop};
+    }
+    const ResamplePlan& rp = p.rp;
+    if (!rp.segs.empty()) {
+        prof.begin("resample");
+        launch_resample(cur.buf, cur.segs, cur.posts ? cur.posts : b.rposts.d, cur.hop, b.rsegs.d, (int)rp.segs.size(),
+                        rp.max_out, rp.smem, b.ry, st);
+        prof.count(rp.flops, rp.bytes);
+        prof.end();
+        cur = Wave{b.ry, b.rosegs.d, b.rposts.d, 1};
+    }
+    if (!p.lp.segs.empty()) {
+        // the samples read and, where a target scales them, written
+        double samples = 0, scaled = 0;
+        for (const LoudSeg& s : p.lp.segs) {
+            samples += (double)s.n;
+            if (!std::isnan(s.target)) scaled += (double)s.n;
+        }
+        prof.begin("loudness");
+        launch_loudness(cur.buf, b.lsegs.d, (int)p.lp.segs.size(), b.lscratch, b.lufs.d, b.gain.d, st);
+        prof.count(2.0 * 22.0 * samples, 4.0 * (samples + scaled));
+        prof.end();
+        b.lufs.download(st);
+        b.gain.download(st);
+    }
+    if (const size_t m = p.mp.chunks.size()) {
+        double window = 0, samples = 0;
+        for (size_t q = 0; q < m; q++) {
+            window += (double)(b.msegs.h[q].p + b.msegs.h[q].n);
+            samples += (double)b.msegs.h[q].n;
+        }
+        prof.begin("loudness");
+        launch_loudness_stream(b.msegs.d, (int)m, st);
+        // the window filtered twice; read, staged, read again and written
+        prof.count(2.0 * 22.0 * window, 4.0 * (3.0 * window + samples));
+        prof.end();
+        b.mlufs.download(st); b.mgains.download(st); b.mclip.download(st);
+    }
+    return cur;
+}
+
+void advance_streams(const OutputPlan& p, const OutputBufs& b, const Profile& prof) {
+    const float stretch_ms = prof.ms("stretch"), pitch_ms = prof.ms("pitch"), formant_ms = prof.ms("formant"),
+                loudness_ms = prof.ms("loudness");
+    for (size_t k = 0; k < p.chunks.size(); k++) {
+        const ChunkSpec& c = p.chunks[k];
+        if (Resampler* r = c.rs) {
+            const ResampleSeg& s = p.rp.segs[k];
+            r->consumed = s.c + p.n_res[k];
+            r->emitted = s.j0 + s.n_out;
+            r->cur ^= 1;
+            r->h = s.h_out;
+            r->ended = c.last != 0;
+        }
+        if (ProsodyStream* w = c.ps) {
+            if (w->fm) formant_stream_advance(*w, p.fsteps[k]);
+            prosody_stream_advance(*w, p.steps[k], c.last != 0);
+            const bool warps = prosody_stream_warps(*w);
+            w->last_ms[0] = warps ? stretch_ms : 0.f; w->last_ms[1] = warps ? pitch_ms : 0.f;
+            w->last_fm_ms = w->fm ? formant_ms : 0.f;
+        }
+    }
+    const MeterPlan& mp = p.mp;
+    for (size_t q = 0; q < mp.chunks.size(); q++) {
+        LoudnessStream* m = p.chunks[mp.chunks[q]].ls;
+        loudness_stream_advance(*m, mp.n[q], b.mlufs.h + mp.step_off[q], b.mgains.h + mp.step_off[q], b.mclip.h[q]);
+        m->last_ms = loudness_ms;
+    }
+}
+
+}  // namespace sb200
