@@ -10,8 +10,9 @@ import numpy as np
 
 from . import _native as N
 from .core import G711_LAW, Audio, OperationError, check_encoding
-from .piper import (_blend_arrays, _check, _config_array, _contour_arrays, _duration_arrays, _formant_array, _gain_array,
-                    _loudness_array, _prosody_arrays, _ptr, _rate_array, _seed_arrays, _take_audio, _take_bytes)
+from .piper import (_batch_options, _blend_arrays, _check, _config_array, _contour_arrays, _duration_arrays,
+                    _formant_array, _gain_array, _loudness_array, _pack_ids, _prosody_arrays, _ptr, _rate_array,
+                    _seed_arrays, _take_audio, _take_bytes)
 
 
 class SynthesisJob:
@@ -26,21 +27,28 @@ class SynthesisJob:
         `loudness`: loudness targets (see set_loudness).  `pitches` / `tempos`: pitch and tempo ratios (see
         set_prosody).  `pitch_contours`: per-id pitch ratios (see set_pitch_contours).  `formants`: formant ratios (see
         set_formants).  `speaker_blends`: speaker blends (see set_speaker_blends)."""
+        # argument errors before the job exists
+        options = _batch_options(model, len(batches), [len(b) for b in batches], configs, seeds=seeds,
+                                 output_rates=output_rates, loudness=loudness, pitches=pitches, tempos=tempos,
+                                 pitch_contours=pitch_contours, formants=formants, speaker_blends=speaker_blends)
+        self._open(model, batches, options, eps_w, eps_z, debug)
+
+    @classmethod
+    def _of(cls, model, batches: Sequence[Sequence[int]], options) -> "SynthesisJob":
+        """A job of `batches` with options already checked by piper._batch_options."""
+        job = cls.__new__(cls)
+        job._open(model, batches, options)
+        return job
+
+    def _open(self, model, batches, o, eps_w=None, eps_z=None, debug: bool = False) -> None:
+        """Creates the job and sets the checked images of options `o`, in the order the library's batch entry points
+        set them; what o does not ask for keeps the new job's default."""
         self._m = model
         self._lib = model._lib
         n = len(batches)
         self.batch = n
         self._lens = [len(b) for b in batches]
-        _config_array(configs, n)             # argument errors before the job exists
-        _seed_arrays(seeds, n)
-        _rate_array(output_rates, n)
-        _loudness_array(loudness, n)
-        _contour_arrays(self._lens, pitch_contours, _prosody_arrays(pitches, tempos, n)[0])
-        _formant_array(formants, n)
-        blend_image = _blend_arrays(model, speaker_blends, n)
-        packed = np.ascontiguousarray(np.concatenate([np.asarray(b, dtype=np.int64) for b in batches]))
-        offs = np.zeros(n + 1, dtype=np.uint64)
-        offs[1:] = np.cumsum([len(b) for b in batches])
+        packed, offs = _pack_ids(batches)
         keep = []
 
         def ptrs(arrs):
@@ -68,36 +76,43 @@ class SynthesisJob:
             C.byref(err)), err)
         if debug:
             self._lib.sb200_job_set_debug(self._h, 1)
-        if configs is not None:
-            self.set_configs(configs)
-        if seeds is not None:
-            self.set_seeds(seeds)
-        if output_rates is not None:
-            self.set_output_rates(output_rates)
-        if loudness is not None:
-            self.set_loudness(loudness)
-        if pitches is not None or tempos is not None:
-            self.set_prosody(pitches, tempos)
-        if pitch_contours is not None:
-            self.set_pitch_contours(pitch_contours)
-        if formants is not None:
-            self.set_formants(formants)
-        if blend_image[2] is not None:
-            self._set_blend_image(*blend_image)
+        lib = self._lib
+        if o.cfgs is not None:
+            self._set(lib.sb200_job_set_configs, o.cfgs)
+        if o.scales is not None or o.frames is not None:
+            self._set(lib.sb200_job_set_durations, _ptr(o.scales, C.c_float), _ptr(o.frames, C.c_int32))
+        if o.seeds is not None:
+            self._set(lib.sb200_job_set_seeds, _ptr(o.seeds, C.c_uint64), _ptr(o.seeded, C.c_int32))
+        if o.rates is not None:
+            self._set(lib.sb200_job_set_output_rates, _ptr(o.rates, C.c_uint32))
+        if o.loudness is not None:
+            self._set(lib.sb200_job_set_loudness, _ptr(o.loudness, C.c_float))
+        if o.pitch is not None or o.tempo is not None:
+            self._set(lib.sb200_job_set_prosody, _ptr(o.pitch, C.c_float), _ptr(o.tempo, C.c_float))
+        if o.contour is not None:
+            self._set(lib.sb200_job_set_pitch_contour, _ptr(o.contour, C.c_float))
+        if o.formants is not None:
+            self._set(lib.sb200_job_set_formants, _ptr(o.formants, C.c_float))
+        if o.blend_offsets is not None:
+            self._set(lib.sb200_job_set_speaker_blends, _ptr(o.blend_speakers, C.c_int64),
+                      _ptr(o.blend_weights, C.c_float), _ptr(o.blend_offsets, C.c_size_t))
+
+    def _set(self, fn, *images) -> None:
+        """One sb200_job_set_* call with its C images."""
+        err = N.sb200_error()
+        _check(fn(self._h, *images, C.byref(err)), err)
 
     def set_configs(self, configs: Optional[Sequence]) -> None:
         """Per-utterance PiperSynthesisConfigs for the next run, or None for the voice's fallback config.  A wrong
         length or an unknown speaker raises OperationError and leaves the job's configs as they were."""
-        err = N.sb200_error()
-        _check(self._lib.sb200_job_set_configs(self._h, _config_array(configs, self.batch), C.byref(err)), err)
+        self._set(self._lib.sb200_job_set_configs, _config_array(configs, self.batch))
 
     def set_durations(self, scales: Optional[Sequence] = None, frames: Optional[Sequence] = None) -> None:
         """Per-id duration controls for the next run (see VitsModel.infer_batch_with_durations): scales[b] / frames[b]
         hold one value per id of utterance b, or None.  None and None restores the default.  A bad entry raises
         OperationError naming the utterance and the id, and leaves the job's controls as they were."""
         sc, fr = _duration_arrays(self._lens, scales, frames)
-        err = N.sb200_error()
-        _check(self._lib.sb200_job_set_durations(self._h, _ptr(sc, C.c_float), _ptr(fr, C.c_int32), C.byref(err)), err)
+        self._set(self._lib.sb200_job_set_durations, _ptr(sc, C.c_float), _ptr(fr, C.c_int32))
 
     def set_seeds(self, seeds: Optional[Sequence]) -> None:
         """Per-utterance noise seeds for the next run (see VitsModel.infer_batch_with_values): an int in [0, 2**64) or
@@ -105,17 +120,14 @@ class SynthesisJob:
         fetchable as "eps_w" and "eps_z".  A bad entry, or seeds on a job with injected noise, raises OperationError
         and leaves the job's seeds as they were."""
         sv, sf = _seed_arrays(seeds, self.batch)
-        err = N.sb200_error()
-        _check(self._lib.sb200_job_set_seeds(self._h, _ptr(sv, C.c_uint64), _ptr(sf, C.c_int32), C.byref(err)), err)
+        self._set(self._lib.sb200_job_set_seeds, _ptr(sv, C.c_uint64), _ptr(sf, C.c_int32))
 
     def set_output_rates(self, rates: Optional[Sequence]) -> None:
         """Per-utterance output sample rates for the next run (see VitsModel.infer_batch_with_values), or None for the
         voice's rate throughout.  After such a run, fetch, fetch_i16, copy_out and the samples and offsets of lengths
         all report the resampled signal.  An unsupported rate raises OperationError naming the utterance and leaves the
         job's rates as they were."""
-        r = _rate_array(rates, self.batch)
-        err = N.sb200_error()
-        _check(self._lib.sb200_job_set_output_rates(self._h, _ptr(r, C.c_uint32), C.byref(err)), err)
+        self._set(self._lib.sb200_job_set_output_rates, _ptr(_rate_array(rates, self.batch), C.c_uint32))
 
     def set_loudness(self, targets: Optional[Sequence]) -> None:
         """Per-utterance loudness targets for the next run (see VitsModel.infer_batch_with_values): LUFS in [-70, 0] or
@@ -123,9 +135,7 @@ class SynthesisJob:
         utterance, scales those with a target in place on the device (d_out included), and fetch_i16 / copy_out(fmt=1)
         convert those at the fixed scale 32767 instead of their peak.  A bad entry raises OperationError naming the
         utterance and leaves the job's targets as they were."""
-        t = _loudness_array(targets, self.batch)
-        err = N.sb200_error()
-        _check(self._lib.sb200_job_set_loudness(self._h, _ptr(t, C.c_float), C.byref(err)), err)
+        self._set(self._lib.sb200_job_set_loudness, _ptr(_loudness_array(targets, self.batch), C.c_float))
 
     def loudness(self) -> Tuple[np.ndarray, np.ndarray]:
         """(integrated loudness in LUFS as float64, -inf when no block passes the gates; gain applied as float32) per
@@ -143,8 +153,7 @@ class SynthesisJob:
         lengths all report the warped signal.  A bad entry raises OperationError naming the utterance and leaves the
         job's ratios as they were."""
         p, t = _prosody_arrays(pitches, tempos, self.batch)
-        err = N.sb200_error()
-        _check(self._lib.sb200_job_set_prosody(self._h, _ptr(p, C.c_float), _ptr(t, C.c_float), C.byref(err)), err)
+        self._set(self._lib.sb200_job_set_prosody, _ptr(p, C.c_float), _ptr(t, C.c_float))
 
     def prosody(self) -> Tuple[np.ndarray, np.ndarray, np.ndarray]:
         """(stretched length n1, delivered length before any output-rate resampling n2, WSOLA frames F) per utterance of
@@ -162,28 +171,20 @@ class SynthesisJob:
         off.  A contour combines with the job's tempos and not with its pitch ratios.  After a run with a contour the
         results report the warped signal, as after set_prosody, and prosody_bounds gives each id's delivered end.  A bad
         entry raises OperationError naming the utterance and the id, and leaves the job's contours as they were."""
-        c = _contour_arrays(self._lens, contours)
-        err = N.sb200_error()
-        _check(self._lib.sb200_job_set_pitch_contour(self._h, _ptr(c, C.c_float), C.byref(err)), err)
+        self._set(self._lib.sb200_job_set_pitch_contour, _ptr(_contour_arrays(self._lens, contours), C.c_float))
 
     def set_formants(self, formants: Optional[Sequence]) -> None:
         """Per-utterance formant ratios for the next run (see VitsModel.infer_batch_with_values), or None for none.  A
         ratio of 1.0 asks for something on an utterance with a pitch ratio or contour: its own formants.  A bad entry
         raises OperationError naming the utterance and leaves the job's ratios as they were."""
-        f = _formant_array(formants, self.batch)
-        err = N.sb200_error()
-        _check(self._lib.sb200_job_set_formants(self._h, _ptr(f, C.c_float), C.byref(err)), err)
+        self._set(self._lib.sb200_job_set_formants, _ptr(_formant_array(formants, self.batch), C.c_float))
 
     def set_speaker_blends(self, blends: Optional[Sequence]) -> None:
         """Per-utterance speaker blends for the next run (see VitsModel.infer_batch_with_values): a mapping
         {speaker: weight} or None per utterance, or None for none.  A blend replaces the utterance's config speaker.  A
         bad entry raises OperationError naming the utterance and leaves the job's blends as they were."""
-        self._set_blend_image(*_blend_arrays(self._m, blends, self.batch))
-
-    def _set_blend_image(self, s, w, o) -> None:
-        err = N.sb200_error()
-        _check(self._lib.sb200_job_set_speaker_blends(self._h, _ptr(s, C.c_int64), _ptr(w, C.c_float),
-                                                      _ptr(o, C.c_size_t), C.byref(err)), err)
+        s, w, o = _blend_arrays(self._m, blends, self.batch)
+        self._set(self._lib.sb200_job_set_speaker_blends, _ptr(s, C.c_int64), _ptr(w, C.c_float), _ptr(o, C.c_size_t))
 
     def prosody_bounds(self) -> List[np.ndarray]:
         """Each id's delivered end in the last run, at the voice's rate, one int64 array per utterance (see
@@ -235,22 +236,21 @@ class SynthesisJob:
         returns, after gains[b] (None: 1), computed on the device in the i16 conversion's launches."""
         if law is None or check_encoding(law) is None:
             raise OperationError(f"law {law!r} is neither 'mulaw' nor 'alaw'")
-        g = _gain_array(gains, self.batch)
-        outs = (C.POINTER(C.c_uint8) * self.batch)()
-        lens = (C.c_size_t * self.batch)()
-        err = N.sb200_error()
-        _check(self._lib.sb200_job_fetch_g711(self._h, G711_LAW[law], _ptr(g, C.c_float), outs, lens, C.byref(err)), err)
-        return _take_bytes(self._lib, outs, lens)
+        return self._fetch_bytes(self._lib.sb200_job_fetch_g711, G711_LAW[law],
+                                 _ptr(_gain_array(gains, self.batch), C.c_float))
 
     def fetch_flac(self, gains: Optional[Sequence] = None) -> List[bytes]:
         """One complete FLAC stream per utterance (see sb200_job_fetch_flac): lossless, of exactly the 16-bit samples
         fetch_i16 returns after gains[b] (None: 1), at the utterance's delivered rate.  Analysed, laid out and packed on
         the device; only the compressed bytes leave the card."""
-        g = _gain_array(gains, self.batch)
+        return self._fetch_bytes(self._lib.sb200_job_fetch_flac, _ptr(_gain_array(gains, self.batch), C.c_float))
+
+    def _fetch_bytes(self, fn, *args) -> List[bytes]:
+        """One byte buffer per utterance from fetch entry point `fn` (sb200_job_fetch_g711 / _flac) with `args`."""
         outs = (C.POINTER(C.c_uint8) * self.batch)()
         lens = (C.c_size_t * self.batch)()
         err = N.sb200_error()
-        _check(self._lib.sb200_job_fetch_flac(self._h, _ptr(g, C.c_float), outs, lens, C.byref(err)), err)
+        _check(fn(self._h, *args, outs, lens, C.byref(err)), err)
         return _take_bytes(self._lib, outs, lens)
 
     def copy_out(self, dst_address: int, capacity_bytes: int, fmt: int = 0) -> int:

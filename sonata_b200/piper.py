@@ -386,13 +386,6 @@ def _char_values_to_ids(v, phonemes: str, src: Sequence[int], b, what: str, chec
     return [1.0 if c < 0 else kept[c] for c in src]
 
 
-def _prosody_kwargs(pitches, tempos) -> dict:
-    out = {} if pitches is None else {"pitches": pitches}
-    if tempos is not None:
-        out["tempos"] = tempos
-    return out
-
-
 def refuse_prosody(pitch, tempo, where: str) -> None:
     """OperationError when `where`, a mode that hands out a sentence chunk by chunk, is asked for a pitch or tempo
     ratio."""
@@ -431,6 +424,86 @@ def _gain_array(gains, n: int):
             raise OperationError(f"utterance {b}: gain {g!r} is not a finite number")
         out[b] = float(g)
     return out
+
+
+@dataclass
+class _BatchOptions:
+    """A batch's options, checked once by _batch_options, as the C images the library takes: each None when not given
+    or when no utterance asks for it.  A phoneme surface's per-character controls (char_scales, char_contours: one
+    entry or None per utterance) become the per-id images `scales` and `contour` once its phonemes are mapped
+    (map_characters)."""
+    n: int
+    cfgs: object = None                       # sb200_synth_config [n]
+    scales: Optional[np.ndarray] = None       # per id, packed
+    frames: Optional[np.ndarray] = None       # per id, packed
+    seeds: Optional[np.ndarray] = None
+    seeded: Optional[np.ndarray] = None
+    rates: Optional[np.ndarray] = None
+    loudness: Optional[np.ndarray] = None
+    laws: Optional[list] = None               # G.711 surfaces only
+    gains: Optional[np.ndarray] = None
+    pitch: Optional[np.ndarray] = None
+    tempo: Optional[np.ndarray] = None
+    contour: Optional[np.ndarray] = None      # per id, packed
+    formants: Optional[np.ndarray] = None
+    blend_speakers: Optional[np.ndarray] = None
+    blend_weights: Optional[np.ndarray] = None
+    blend_offsets: Optional[np.ndarray] = None
+    char_scales: Optional[list] = None
+    char_contours: Optional[list] = None
+
+    def map_characters(self, phonemes: Sequence[str], maps) -> None:
+        """Makes the per-id images of the per-character controls once the phonemes are mapped: maps[b] is (ids, source
+        character of each id) of phonemes[b], as phonemes_to_input_ids_map gives it."""
+        def per_id(values, what, check):
+            return None if values is None else [
+                None if v is None else _char_values_to_ids(v, ph, src, b, what, check)
+                for b, (v, ph, (_, src)) in enumerate(zip(values, phonemes, maps))]
+        lens = [len(ids) for ids, _ in maps]
+        self.scales, _ = _duration_arrays(lens, per_id(self.char_scales, "duration scales", _scale_value))
+        self.contour = _contour_arrays(lens, per_id(self.char_contours, "pitch ratios", _contour_value), self.pitch)
+
+
+def _batch_options(model, n: int, lens: Optional[Sequence[int]] = None, configs=None, duration_scales=None,
+                   durations=None, seeds=None, output_rates=None, loudness=None, law=None, gains=None, pitches=None,
+                   tempos=None, pitch_contours=None, formants=None, speaker_blends=None,
+                   g711: bool = False) -> _BatchOptions:
+    """The options of a batch of n utterances, each checked as its C image is made, in one order at every surface:
+    configs, duration scales, durations, seeds, output rates, loudness, law (with `g711`), gains, pitch and tempo, pitch
+    contours, formants, speaker blends.  `lens`: the utterances' id counts, for per-id controls; None for a phoneme
+    surface, whose per-character controls are only counted here, before any phoneme is mapped (see map_characters)."""
+    o = _BatchOptions(n, _config_array(configs, n))
+    if lens is None:
+        o.char_scales = None if duration_scales is None else _per_utterance(duration_scales, n, "duration scales")
+    else:
+        o.scales, o.frames = _duration_arrays(lens, duration_scales, durations)
+    o.seeds, o.seeded = _seed_arrays(seeds, n)
+    o.rates = _rate_array(output_rates, n)
+    o.loudness = _loudness_array(loudness, n)
+    if g711:
+        o.laws = _encoding_list(law, n)
+    o.gains = _gain_array(gains, n)
+    o.pitch, o.tempo = _prosody_arrays(pitches, tempos, n)
+    if lens is None:
+        o.char_contours = None if pitch_contours is None else _per_utterance(pitch_contours, n, "pitch contours")
+    else:
+        o.contour = _contour_arrays(lens, pitch_contours, o.pitch)
+    o.formants = _formant_array(formants, n)
+    o.blend_speakers, o.blend_weights, o.blend_offsets = _blend_arrays(model, speaker_blends, n)
+    return o
+
+
+def _pack_ids(batches):
+    """The ids of a batch back to back (int64) and each utterance's offset into them (size_t [n + 1])."""
+    packed = np.ascontiguousarray(np.concatenate([np.asarray(b, dtype=np.int64) for b in batches]))
+    offs = np.zeros(len(batches) + 1, dtype=np.uint64)
+    offs[1:] = np.cumsum([len(b) for b in batches])
+    return packed, offs
+
+
+def _check_not_empty(batches) -> None:
+    if any(len(b) == 0 for b in batches):
+        raise OperationError("Failed to run model inference. Error: empty input sequence")
 
 
 def rate_ratio(in_rate: int, out_rate: Optional[int]) -> Tuple[int, int]:
@@ -659,36 +732,18 @@ class _VitsCommons:
         targets, pitch and tempo ratios and formant ratios as for infer_batch_with_values.  `pitch_contours`: as for
         speak_batch_with_alignment, one ratio per phoneme character."""
         n = len(phoneme_batches)
-        _config_array(configs, n)             # argument errors before any id mapping
-        sv, _ = _seed_arrays(seeds, n)
-        rates = _rate_array(output_rates, n)
-        loud = _loudness_array(loudness, n)
-        pros = any(a is not None for a in _prosody_arrays(pitches, tempos, n))
-        fmt = _formant_array(formants, n)
-        blend = _blend_arrays(self, speaker_blends, n)[0] is not None
+        o = _batch_options(self, n, None, configs, seeds=seeds, output_rates=output_rates, loudness=loudness,
+                           pitches=pitches, tempos=tempos, pitch_contours=pitch_contours, formants=formants,
+                           speaker_blends=speaker_blends)
         if n == 0:
             return []
         if pitch_contours is not None:
-            return [a for a, _ in self.speak_batch_with_alignment(phoneme_batches, configs, seeds=seeds,
-                                                                  output_rates=output_rates, loudness=loudness,
-                                                                  pitches=pitches, tempos=tempos,
-                                                                  pitch_contours=pitch_contours, formants=formants,
-                                                                  speaker_blends=speaker_blends)]
-        if (configs is not None or sv is not None or rates is not None or loud is not None or pros or fmt is not None
-                or blend):
-            extra = {} if sv is None else {"seeds": seeds}
-            if blend:
-                extra["speaker_blends"] = speaker_blends
-            if fmt is not None:
-                extra["formants"] = formants
-            if pros:
-                extra.update(_prosody_kwargs(pitches, tempos))
-            if rates is not None:
-                extra["output_rates"] = output_rates
-            if loud is not None:
-                extra["loudness"] = loudness
-            return self.infer_batch_with_values([self.phonemes_to_input_ids(p) for p in phoneme_batches], configs,
-                                                **extra)
+            maps = [self.phonemes_to_input_ids_map(p) for p in phoneme_batches]
+            o.map_characters(phoneme_batches, maps)
+            return [a for a, _, _ in self._speak_ids([ids for ids, _ in maps], o)]
+        if any(x is not None for x in (o.cfgs, o.seeds, o.rates, o.loudness, o.pitch, o.tempo, o.formants,
+                                       o.blend_offsets)):
+            return [a for a, _, _ in self._speak_ids([self.phonemes_to_input_ids(p) for p in phoneme_batches], o)]
         arr = (C.c_char_p * n)(*[p.encode("utf-8") for p in phoneme_batches])
         outs = (N.sb200_audio * n)()
         err = N.sb200_error()
@@ -754,37 +809,10 @@ class _VitsCommons:
         (the config's scales still apply; include/sonata_b200.h, sb200_speak_batch_ids_blends).  A blend of one speaker
         (any positive weight) gives that speaker's bits, and blends equal up to order, zero weights or a common
         power-of-two scale give the same bits."""
-        n = len(batches)
-        cfgs = _config_array(configs, n)
-        sv, _ = _seed_arrays(seeds, n)
-        rates = _rate_array(output_rates, n)
-        loud = _loudness_array(loudness, n)
-        pit, tem = _prosody_arrays(pitches, tempos, n)
-        pros = pit is not None or tem is not None
-        contour = _contour_arrays([len(b) for b in batches], pitch_contours, pit)
-        fmt = _formant_array(formants, n)
-        blend = _blend_arrays(self, speaker_blends, n)[0] is not None
-        if (sv is not None or rates is not None or loud is not None or pros or contour is not None or fmt is not None
-                or blend):
-            extra = _prosody_kwargs(pitches, tempos) if pros else {}
-            if blend:
-                extra["speaker_blends"] = speaker_blends
-            if contour is not None:
-                extra["pitch_contours"] = pitch_contours
-            if fmt is not None:
-                extra["formants"] = formants
-            return [a for a, _ in self.infer_batch_with_durations(batches, configs, seeds=seeds,
-                                                                  output_rates=output_rates, loudness=loudness,
-                                                                  **extra)]
-        packed = np.ascontiguousarray(np.concatenate([np.asarray(b, dtype=np.int64) for b in batches]))
-        offs = np.zeros(n + 1, dtype=np.uint64)
-        offs[1:] = np.cumsum([len(b) for b in batches])
-        outs = (N.sb200_audio * n)()
-        err = N.sb200_error()
-        _check(self._lib.sb200_speak_batch_ids_configs(self._h, packed.ctypes.data_as(C.POINTER(C.c_int64)),
-                                                       offs.ctypes.data_as(C.POINTER(C.c_size_t)), n, cfgs, outs,
-                                                       C.byref(err)), err)
-        return [_take_audio(outs[i]) for i in range(n)]
+        o = _batch_options(self, len(batches), [len(b) for b in batches], configs, seeds=seeds,
+                           output_rates=output_rates, loudness=loudness, pitches=pitches, tempos=tempos,
+                           pitch_contours=pitch_contours, formants=formants, speaker_blends=speaker_blends)
+        return [a for a, _, _ in self._speak_ids(batches, o)]
 
     def infer_batch_with_durations(self, batches: Sequence[Sequence[int]],
                                    configs: Optional[Sequence[PiperSynthesisConfig]] = None,
@@ -806,67 +834,31 @@ class _VitsCommons:
         seeded frame's noise depends on its index only, so controls that move frames never reshuffle it.
         `output_rates` / `loudness` / `pitches` / `tempos` / `pitch_contours` / `formants` / `speaker_blends`: as for
         infer_batch_with_values (the frame counts stay frame counts of the utterance before any warp)."""
-        return [(a, f) for a, f, _ in self._speak_ids(batches, configs, duration_scales, durations, seeds, output_rates,
-                                                       loudness, pitches, tempos, pitch_contours, formants,
-                                                       speaker_blends)]
+        o = _batch_options(self, len(batches), [len(b) for b in batches], configs, duration_scales, durations, seeds,
+                           output_rates, loudness, pitches=pitches, tempos=tempos, pitch_contours=pitch_contours,
+                           formants=formants, speaker_blends=speaker_blends)
+        return [(a, f) for a, f, _ in self._speak_ids(batches, o, frames=True)]
 
-    def _speak_ids(self, batches, configs, duration_scales, durations, seeds, output_rates, loudness, pitches, tempos,
-                   pitch_contours, formants=None,
-                   speaker_blends=None) -> List[Tuple[Audio, np.ndarray, Optional[np.ndarray]]]:
-        """infer_batch_with_durations with each id's delivered end (None without a contour) per utterance."""
+    def _speak_ids(self, batches, o: _BatchOptions, frames: bool = False) -> List[tuple]:
+        """The f32 batch route: `batches` with options `o` in one sb200_speak_batch_ids_blends call.  Per utterance
+        (audio, frames per id, each id's delivered end): the frames only when asked for, since fetching them costs a
+        device->host copy and a synchronise, and the ends only when o has a pitch contour (None otherwise)."""
         n = len(batches)
-        cfgs = _config_array(configs, n)
-        lens = [len(b) for b in batches]
-        scales, frames = _duration_arrays(lens, duration_scales, durations)
-        sv, sf = _seed_arrays(seeds, n)
-        rates = _rate_array(output_rates, n)
-        loud = _loudness_array(loudness, n)
-        pit, tem = _prosody_arrays(pitches, tempos, n)
-        contour = _contour_arrays(lens, pitch_contours, pit)
-        fmt = _formant_array(formants, n)
-        bs, bw, bo = _blend_arrays(self, speaker_blends, n)
         if n == 0:
             return []
-        if any(x == 0 for x in lens):
-            raise OperationError("Failed to run model inference. Error: empty input sequence")
-        packed = np.ascontiguousarray(np.concatenate([np.asarray(b, dtype=np.int64) for b in batches]))
-        offs = np.zeros(n + 1, dtype=np.uint64)
-        offs[1:] = np.cumsum(lens)
+        _check_not_empty(batches)
+        packed, offs = _pack_ids(batches)
         outs = (N.sb200_audio * n)()
-        id_frames = np.zeros(int(offs[-1]), np.int32)
+        id_frames = np.zeros(int(offs[-1]), np.int32) if frames else None
+        bounds = None if o.contour is None else np.zeros(int(offs[-1]), np.int64)
         err = N.sb200_error()
-        bounds = None
-        if bo is not None:
-            bounds = None if contour is None else np.zeros(int(offs[-1]), np.int64)
-            _check(self._lib.sb200_speak_batch_ids_blends(
-                self._h, packed.ctypes.data_as(C.POINTER(C.c_int64)), offs.ctypes.data_as(C.POINTER(C.c_size_t)), n,
-                cfgs, _ptr(scales, C.c_float), _ptr(frames, C.c_int32), _ptr(sv, C.c_uint64), _ptr(sf, C.c_int32),
-                _ptr(rates, C.c_uint32), _ptr(loud, C.c_float), _ptr(pit, C.c_float), _ptr(tem, C.c_float),
-                _ptr(contour, C.c_float), _ptr(fmt, C.c_float), _ptr(bs, C.c_int64), _ptr(bw, C.c_float),
-                _ptr(bo, C.c_size_t), outs, _ptr(id_frames, C.c_int32), _ptr(bounds, C.c_int64), None, None,
-                C.byref(err)), err)
-        elif fmt is not None:
-            bounds = None if contour is None else np.zeros(int(offs[-1]), np.int64)
-            _check(self._lib.sb200_speak_batch_ids_formants(
-                self._h, packed.ctypes.data_as(C.POINTER(C.c_int64)), offs.ctypes.data_as(C.POINTER(C.c_size_t)), n,
-                cfgs, _ptr(scales, C.c_float), _ptr(frames, C.c_int32), _ptr(sv, C.c_uint64), _ptr(sf, C.c_int32),
-                _ptr(rates, C.c_uint32), _ptr(loud, C.c_float), _ptr(pit, C.c_float), _ptr(tem, C.c_float),
-                _ptr(contour, C.c_float), _ptr(fmt, C.c_float), outs, _ptr(id_frames, C.c_int32),
-                _ptr(bounds, C.c_int64), None, None, C.byref(err)), err)
-        elif contour is None:
-            _check(self._lib.sb200_speak_batch_ids_prosody(
-                self._h, packed.ctypes.data_as(C.POINTER(C.c_int64)), offs.ctypes.data_as(C.POINTER(C.c_size_t)), n,
-                cfgs, _ptr(scales, C.c_float), _ptr(frames, C.c_int32), _ptr(sv, C.c_uint64), _ptr(sf, C.c_int32),
-                _ptr(rates, C.c_uint32), _ptr(loud, C.c_float), _ptr(pit, C.c_float), _ptr(tem, C.c_float), outs,
-                _ptr(id_frames, C.c_int32), None, None, C.byref(err)), err)
-        else:
-            bounds = np.zeros(int(offs[-1]), np.int64)
-            _check(self._lib.sb200_speak_batch_ids_contour(
-                self._h, packed.ctypes.data_as(C.POINTER(C.c_int64)), offs.ctypes.data_as(C.POINTER(C.c_size_t)), n,
-                cfgs, _ptr(scales, C.c_float), _ptr(frames, C.c_int32), _ptr(sv, C.c_uint64), _ptr(sf, C.c_int32),
-                _ptr(rates, C.c_uint32), _ptr(loud, C.c_float), _ptr(pit, C.c_float), _ptr(tem, C.c_float),
-                _ptr(contour, C.c_float), outs, _ptr(id_frames, C.c_int32), _ptr(bounds, C.c_int64), None, None,
-                C.byref(err)), err)
+        _check(self._lib.sb200_speak_batch_ids_blends(
+            self._h, _ptr(packed, C.c_int64), _ptr(offs, C.c_size_t), n, o.cfgs, _ptr(o.scales, C.c_float),
+            _ptr(o.frames, C.c_int32), _ptr(o.seeds, C.c_uint64), _ptr(o.seeded, C.c_int32), _ptr(o.rates, C.c_uint32),
+            _ptr(o.loudness, C.c_float), _ptr(o.pitch, C.c_float), _ptr(o.tempo, C.c_float), _ptr(o.contour, C.c_float),
+            _ptr(o.formants, C.c_float), _ptr(o.blend_speakers, C.c_int64), _ptr(o.blend_weights, C.c_float),
+            _ptr(o.blend_offsets, C.c_size_t), outs, _ptr(id_frames, C.c_int32), _ptr(bounds, C.c_int64), None, None,
+            C.byref(err)), err)
         cut = lambda a, b: None if a is None else a[int(offs[b]):int(offs[b + 1])].copy()
         return [(_take_audio(outs[b]), cut(id_frames, b), cut(bounds, b)) for b in range(n)]
 
@@ -899,58 +891,23 @@ class _VitsCommons:
         `formants`: as for infer_batch_with_values; it moves no boundary.  `speaker_blends`: as for
         infer_batch_with_values."""
         n = len(phoneme_batches)
-        _config_array(configs, n)
-        _seed_arrays(seeds, n)
-        if _blend_arrays(self, speaker_blends, n)[0] is None:
-            speaker_blends = None
-        _rate_array(output_rates, n)
-        _loudness_array(loudness, n)
-        pit, tem = _prosody_arrays(pitches, tempos, n)
-        warped = [(pit is not None and not np.isnan(pit[b])) or (tem is not None and not np.isnan(tem[b]))
-                  for b in range(n)]
-        per_char = None if duration_scales is None else _per_utterance(duration_scales, n, "duration scales")
-        char_contours = None if pitch_contours is None else _per_utterance(pitch_contours, n, "pitch contours")
+        o = _batch_options(self, n, None, configs, duration_scales, seeds=seeds, output_rates=output_rates,
+                           loudness=loudness, pitches=pitches, tempos=tempos, pitch_contours=pitch_contours,
+                           formants=formants, speaker_blends=speaker_blends)
         maps = [self.phonemes_to_input_ids_map(p) for p in phoneme_batches]
-        id_contours = None
-        if char_contours is not None:
-            id_contours = []
-            for b, (ph, (ids, src)) in enumerate(zip(phoneme_batches, maps)):
-                v = char_contours[b]
-                id_contours.append(None if v is None else
-                                   _char_values_to_ids(v, ph, src, b, "pitch ratios", _contour_value))
-            if _contour_arrays([len(m[0]) for m in maps], id_contours, pit) is None:
-                id_contours = None
-        id_scales = None
-        if per_char is not None:
-            id_scales = []
-            for b, (ph, (ids, src)) in enumerate(zip(phoneme_batches, maps)):
-                v = per_char[b]
-                id_scales.append(None if v is None else
-                                 _char_values_to_ids(v, ph, src, b, "duration scales", _scale_value))
-        extra = {} if seeds is None else {"seeds": seeds}
-        if output_rates is not None:
-            extra["output_rates"] = output_rates
-        if loudness is not None:
-            extra["loudness"] = loudness
-        if any(warped):
-            extra.update(_prosody_kwargs(pitches, tempos))
-        if _formant_array(formants, n) is not None:
-            extra["formants"] = formants
-        if speaker_blends is not None:
-            extra["speaker_blends"] = speaker_blends
-        if id_contours is None:
-            res = [(a, f, None) for a, f in self.infer_batch_with_durations([m[0] for m in maps], configs, id_scales,
-                                                                            **extra)]
-        else:
-            res = self._speak_ids([m[0] for m in maps], configs, id_scales, None, extra.get("seeds"),
-                                  extra.get("output_rates"), extra.get("loudness"), extra.get("pitches"),
-                                  extra.get("tempos"), id_contours, extra.get("formants"), speaker_blends)
-        voice_rate = self.audio_output_info().sample_rate if output_rates is not None else None
+        o.map_characters(phoneme_batches, maps)
+        res = self._speak_ids([ids for ids, _ in maps], o, frames=True)
+        voice_rate = self.audio_output_info().sample_rate if o.rates is not None else None
         ratio = lambda audio: (1, 1) if voice_rate is None else rate_ratio(voice_rate, audio.info.sample_rate)
-        shaped = [id_contours is not None and c is not None and any(not (math.isnan(x) or x == 1.0) for x in c)
-                  for c in (id_contours or [None] * n)]
-        return [(audio, _alignment(ph, src, frames, len(audio), *ratio(audio), warped=w, bounds=bounds if c else None))
-                for ph, (_, src), (audio, frames, bounds), w, c in zip(phoneme_batches, maps, res, warped, shaped)]
+        warped = lambda b: any(r is not None and not np.isnan(r[b]) for r in (o.pitch, o.tempo))
+        offs = np.cumsum([0] + [len(ids) for ids, _ in maps])
+
+        def shaped(b):          # utterance b has a contour that asks for something: aligned from its delivered ends
+            c = None if o.contour is None else o.contour[offs[b]:offs[b + 1]]
+            return c is not None and bool(np.any(~np.isnan(c) & (c != 1)))
+        return [(audio, _alignment(ph, src, frames, len(audio), *ratio(audio), warped=warped(b),
+                                   bounds=bounds if shaped(b) else None))
+                for b, (ph, (_, src), (audio, frames, bounds)) in enumerate(zip(phoneme_batches, maps, res))]
 
     def infer_batch_g711(self, batches: Sequence[Sequence[int]], law,
                          configs: Optional[Sequence[PiperSynthesisConfig]] = None, seeds: Optional[Sequence] = None,
@@ -965,34 +922,10 @@ class _VitsCommons:
         conversion's launches, so only one byte per sample leaves the card.  `configs`, `seeds`, `output_rates` and
         `loudness` as for infer_batch_with_values, and so are `pitches`, `tempos`, `formants` and `speaker_blends`; a
         batch mixing laws runs one conversion per law."""
-        from .job import SynthesisJob
-        n = len(batches)
-        _config_array(configs, n)
-        _seed_arrays(seeds, n)
-        _rate_array(output_rates, n)
-        _loudness_array(loudness, n)
-        laws = _encoding_list(law, n)
-        _gain_array(gains, n)
-        _prosody_arrays(pitches, tempos, n)
-        _formant_array(formants, n)
-        _blend_arrays(self, speaker_blends, n)
-        if n == 0:
-            return []
-        if any(len(b) == 0 for b in batches):
-            raise OperationError("Failed to run model inference. Error: empty input sequence")
-        job = SynthesisJob(self, batches, configs=configs, seeds=seeds, output_rates=output_rates, loudness=loudness,
-                           pitches=pitches, tempos=tempos, formants=formants, speaker_blends=speaker_blends)
-        try:
-            job.run()
-            out: List[Optional[bytes]] = [None] * n
-            for e in dict.fromkeys(laws):
-                res = job.fetch_g711(e, gains)
-                for b in range(n):
-                    if laws[b] == e:
-                        out[b] = res[b]
-            return out
-        finally:
-            job.close()
+        o = _batch_options(self, len(batches), [len(b) for b in batches], configs, seeds=seeds,
+                           output_rates=output_rates, loudness=loudness, law=law, gains=gains, pitches=pitches,
+                           tempos=tempos, formants=formants, speaker_blends=speaker_blends, g711=True)
+        return self._encode_batch(batches, o)
 
     def speak_batch_g711(self, phoneme_batches: Sequence[str], law,
                          configs: Optional[Sequence[PiperSynthesisConfig]] = None, seeds: Optional[Sequence] = None,
@@ -1001,11 +934,10 @@ class _VitsCommons:
                          tempos: Optional[Sequence] = None, formants: Optional[Sequence] = None,
                          speaker_blends: Optional[Sequence] = None) -> List[bytes]:
         """speak_batch delivered as G.711 bytes: infer_batch_g711 over the phonemes' ids."""
-        n = len(phoneme_batches)
-        _config_array(configs, n)
-        _encoding_list(law, n)
-        return self.infer_batch_g711([self.phonemes_to_input_ids(p) for p in phoneme_batches], law, configs, seeds,
-                                     output_rates, loudness, gains, pitches, tempos, formants, speaker_blends)
+        o = _batch_options(self, len(phoneme_batches), None, configs, seeds=seeds, output_rates=output_rates,
+                           loudness=loudness, law=law, gains=gains, pitches=pitches, tempos=tempos, formants=formants,
+                           speaker_blends=speaker_blends, g711=True)
+        return self._encode_batch([self.phonemes_to_input_ids(p) for p in phoneme_batches], o)
 
     def infer_batch_flac(self, batches: Sequence[Sequence[int]],
                          configs: Optional[Sequence[PiperSynthesisConfig]] = None, seeds: Optional[Sequence] = None,
@@ -1018,27 +950,10 @@ class _VitsCommons:
         gains[b] (None: 1), or the fixed scale for an utterance with a loudness target, at its delivered rate.  They are
         encoded on the device, and only the compressed bytes leave the card.  `configs`, `seeds`, `output_rates`,
         `loudness`, `pitches`, `tempos`, `formants` and `speaker_blends` as for infer_batch_with_values."""
-        from .job import SynthesisJob
-        n = len(batches)
-        _config_array(configs, n)
-        _seed_arrays(seeds, n)
-        _rate_array(output_rates, n)
-        _loudness_array(loudness, n)
-        _gain_array(gains, n)
-        _prosody_arrays(pitches, tempos, n)
-        _formant_array(formants, n)
-        _blend_arrays(self, speaker_blends, n)
-        if n == 0:
-            return []
-        if any(len(b) == 0 for b in batches):
-            raise OperationError("Failed to run model inference. Error: empty input sequence")
-        job = SynthesisJob(self, batches, configs=configs, seeds=seeds, output_rates=output_rates, loudness=loudness,
-                           pitches=pitches, tempos=tempos, formants=formants, speaker_blends=speaker_blends)
-        try:
-            job.run()
-            return job.fetch_flac(gains)
-        finally:
-            job.close()
+        o = _batch_options(self, len(batches), [len(b) for b in batches], configs, seeds=seeds,
+                           output_rates=output_rates, loudness=loudness, gains=gains, pitches=pitches, tempos=tempos,
+                           formants=formants, speaker_blends=speaker_blends)
+        return self._encode_batch(batches, o)
 
     def speak_batch_flac(self, phoneme_batches: Sequence[str],
                          configs: Optional[Sequence[PiperSynthesisConfig]] = None, seeds: Optional[Sequence] = None,
@@ -1047,9 +962,33 @@ class _VitsCommons:
                          tempos: Optional[Sequence] = None, formants: Optional[Sequence] = None,
                          speaker_blends: Optional[Sequence] = None) -> List[bytes]:
         """speak_batch delivered as FLAC streams: infer_batch_flac over the phonemes' ids."""
-        _config_array(configs, len(phoneme_batches))
-        return self.infer_batch_flac([self.phonemes_to_input_ids(p) for p in phoneme_batches], configs, seeds,
-                                     output_rates, loudness, gains, pitches, tempos, formants, speaker_blends)
+        o = _batch_options(self, len(phoneme_batches), None, configs, seeds=seeds, output_rates=output_rates,
+                           loudness=loudness, gains=gains, pitches=pitches, tempos=tempos, formants=formants,
+                           speaker_blends=speaker_blends)
+        return self._encode_batch([self.phonemes_to_input_ids(p) for p in phoneme_batches], o)
+
+    def _encode_batch(self, batches, o: _BatchOptions) -> List[bytes]:
+        """The G.711 bytes (when o has laws) or FLAC streams of `batches` with options `o`: one SynthesisJob run, then
+        one fetch per law."""
+        from .job import SynthesisJob
+        if o.n == 0:
+            return []
+        _check_not_empty(batches)
+        job = SynthesisJob._of(self, batches, o)
+        try:
+            job.run()
+            g = _ptr(o.gains, C.c_float)
+            if o.laws is None:
+                return job._fetch_bytes(self._lib.sb200_job_fetch_flac, g)
+            out: List[Optional[bytes]] = [None] * o.n
+            for e in dict.fromkeys(o.laws):
+                res = job._fetch_bytes(self._lib.sb200_job_fetch_g711, G711_LAW[e], g)
+                for b in range(o.n):
+                    if o.laws[b] == e:
+                        out[b] = res[b]
+            return out
+        finally:
+            job.close()
 
     def _cfg(self, fn) -> PiperSynthesisConfig:
         c, err = N.sb200_synth_config(), N.sb200_error()
@@ -1148,6 +1087,16 @@ class Resampler:
             pass
 
 
+def _handles(objs, n: int, kind, what: str):
+    """The C handles of one `kind` (Resampler, ProsodyStream or LoudnessStream) or None per chunk of a decoder pass."""
+    out = (C.c_void_p * n)()
+    for k, x in enumerate(_per_utterance(objs, n, what)):
+        if x is not None and (not isinstance(x, kind) or not x._h):
+            raise OperationError(f"chunk {k}: not a {kind.__name__}")
+        out[k] = None if x is None else x._h.value
+    return out
+
+
 def _stream_resampler(model, output_rate) -> Optional[Resampler]:
     """A Resampler for a stream at output_rate, or None when the stream stays at the voice's rate."""
     _rate_array([output_rate], 1)
@@ -1180,46 +1129,34 @@ class ProsodyStream:
         self.tempo = None if t is None else float(t[0])
         self.formant = phi
         self.bounds = None
-        err = N.sb200_error()
-        if phi is not None:
-            # sb200_prosody_stream_create_formant: the ratio or contour stream with phi on top, or phi alone
-            c = None
-            if pitch_contour is not None:
-                if not isinstance(enc, EncoderOutputs) or enc._m is not model or not enc._h:
-                    raise OperationError("a pitch contour needs the EncoderOutputs of its sentence, from this model")
-                c = _contour_arrays([len(enc.p_duration)], [pitch_contour], None, ["stream"])
-                if c is None:
-                    c = np.full(len(enc.p_duration), np.nan, np.float32)
-            nan = float("nan")
-            _check(model._lib.sb200_prosody_stream_create_formant(
-                model._h, None if c is None else enc._h, nan if p is None else float(p[0]), _ptr(c, C.c_float),
-                0 if c is None else c.size, nan if t is None else float(t[0]), phi, C.byref(self._h), C.byref(err)),
-                err)
-            if c is not None:
-                self.bounds = np.zeros(c.size, np.int64)
-                _check(model._lib.sb200_prosody_stream_bounds(self._h, _ptr(self.bounds, C.c_int64), c.size,
-                                                              C.byref(err)), err)
-            return
+        c = None                        # the contour's per-id image
         if pitch_contour is not None:
-            if p is not None:
+            if phi is None and p is not None:
                 raise OperationError("stream: a pitch contour and a pitch ratio together (give one or the other)")
             if not isinstance(enc, EncoderOutputs) or enc._m is not model or not enc._h:
                 raise OperationError("a pitch contour needs the EncoderOutputs of its sentence, from this model")
             c = _contour_arrays([len(enc.p_duration)], [pitch_contour], None, ["stream"])
             if c is None:
                 c = np.full(len(enc.p_duration), np.nan, np.float32)
-            _check(model._lib.sb200_prosody_stream_create_contour(
-                model._h, enc._h, _ptr(c, C.c_float), c.size, float("nan") if t is None else float(t[0]),
+        nan = float("nan")
+        pv, tv = nan if p is None else float(p[0]), nan if t is None else float(t[0])
+        err = N.sb200_error()
+        if phi is not None:
+            # the ratio or contour stream with phi on top, or phi alone
+            _check(model._lib.sb200_prosody_stream_create_formant(
+                model._h, None if c is None else enc._h, pv, _ptr(c, C.c_float), 0 if c is None else c.size, tv, phi,
                 C.byref(self._h), C.byref(err)), err)
+        elif c is not None:
+            _check(model._lib.sb200_prosody_stream_create_contour(model._h, enc._h, _ptr(c, C.c_float), c.size, tv,
+                                                                  C.byref(self._h), C.byref(err)), err)
+        elif p is None and t is None:
+            raise OperationError("a prosody stream needs a pitch or a tempo ratio other than 1 (None, NaN or 1: none)")
+        else:
+            _check(model._lib.sb200_prosody_stream_create(model._h, pv, tv, C.byref(self._h), C.byref(err)), err)
+        if c is not None:
             self.bounds = np.zeros(c.size, np.int64)
             _check(model._lib.sb200_prosody_stream_bounds(self._h, _ptr(self.bounds, C.c_int64), c.size,
                                                           C.byref(err)), err)
-            return
-        if p is None and t is None:
-            raise OperationError("a prosody stream needs a pitch or a tempo ratio other than 1 (None, NaN or 1: none)")
-        _check(model._lib.sb200_prosody_stream_create(model._h, float("nan") if p is None else float(p[0]),
-                                                      float("nan") if t is None else float(t[0]), C.byref(self._h),
-                                                      C.byref(err)), err)
 
     def last_pass_ms(self) -> Tuple[float, float]:
         """The "stretch" and "pitch" device time (ms) of the last chunk pass this stream was in."""
@@ -1365,21 +1302,20 @@ def _trim_frames(trim: slice) -> Tuple[int, int]:
     return (trim.start or 0) // HOP, (-trim.stop // HOP) if trim.stop is not None else 0
 
 
-class SpeechStreamer:
-    """piper/src/lib.rs:765-858: chunked decoder runs with overlap trimming + crossfade(42).  With a resampler, each
-    chunk's trim and crossfade run on the device and the chunk leaves at the resampler's rate.  With an encoding, they
-    run on the device too and each chunk leaves as G.711 bytes of its to_i16_vec after `gain`."""
+class _Stream:
+    """One sentence streamed from its latent `enc`: its own chunk schedule with the one-shot rule of piper/src/lib.rs
+    (a sentence of at most 2 chunks and 2 paddings is decoded whole), and the stream objects its chunks pass through
+    on the device.  `key`: what a StreamBatch calls it."""
 
-    def __init__(self, enc: EncoderOutputs, chunk_size: int, chunk_padding: int,
-                 resampler: Optional[Resampler] = None, encoding: Optional[str] = None, gain: float = 1.0,
-                 warp: Optional[ProsodyStream] = None, meter: Optional[LoudnessStream] = None):
-        self.enc = enc
+    def __init__(self, key, enc, chunk_size: int, chunk_padding: int, resampler: Optional[Resampler] = None,
+                 encoding: Optional[str] = None, gain: float = 1.0, warp: Optional[ProsodyStream] = None,
+                 meter: Optional[LoudnessStream] = None):
+        self.key, self.enc, self.resampler = key, enc, resampler
         self.meter = meter
-        self.chunker = AdaptiveMelChunker(enc.num_frames, chunk_size, chunk_padding)
-        self.one_shot = enc.num_frames <= (chunk_size * 2 + chunk_padding * 2)
-        self.resampler = resampler
         self.encoding, self.gain = encoding, gain
         self.warp = warp
+        self.chunker = AdaptiveMelChunker(enc.num_frames, chunk_size, chunk_padding)
+        self.one_shot = enc.num_frames <= (chunk_size * 2 + chunk_padding * 2)
 
     @property
     def bounds(self) -> Optional[np.ndarray]:
@@ -1387,37 +1323,65 @@ class SpeechStreamer:
         contour (see ProsodyStream; with an output rate at ceil(end * up / down)), else None."""
         return _delivered_bounds(self.warp, self.resampler)
 
+    @property
+    def on_device(self) -> bool:
+        """Whether the chunks' trim and crossfade run on the device, with the stream's encoding, resampler, prosody
+        stream or meter."""
+        return not (self.encoding is None and self.resampler is None and self.warp is None and self.meter is None)
+
+    def next_chunk(self):
+        """(lo, hi, audio slice or None): the frames to decode next, and how the plain path trims them (None: the
+        one-shot chunk, returned as decoded)."""
+        (m0, m1), (a0, a1) = next(self.chunker)
+        if self.one_shot:
+            self.chunker.consume()
+            return 0, self.enc.num_frames, None
+        return m0, self.enc.num_frames if m1 is None else m1, slice(a0, a1)
+
+    @property
+    def done(self) -> bool:
+        return self.chunker.last_end_index is None
+
+
+def _device_post(model, plan) -> list:
+    """One infer_decoder_batch call for planned chunks [(stream, lo, hi, trim)] of streams with the same encoding,
+    trim kind (one-shot or not) and kinds of resampler, prosody stream and meter: each chunk trimmed and crossfaded on
+    the device, then passed through its stream's objects, whose last chunk flushes them."""
+    s0 = plan[0][0]
+    streams = [s for s, _, _, _ in plan]
+    kw = {}
+    if s0.resampler is not None or s0.warp is not None or s0.meter is not None:
+        kw.update(resamplers=[s.resampler for s in streams], last=[s.done for s in streams])
+    if s0.warp is not None:
+        kw["warps"] = [s.warp for s in streams]
+    if s0.meter is not None:
+        kw["meters"] = [s.meter for s in streams]
+    if s0.encoding is not None:
+        kw.update(gains=[s.gain for s in streams], encoding=s0.encoding)
+    chunks = [(s.enc, lo, hi) + ((0, 0) if trim is None else _trim_frames(trim)) for s, lo, hi, trim in plan]
+    return model.infer_decoder_batch(chunks, fade=0 if plan[0][3] is None else 42, **kw)
+
+
+class SpeechStreamer(_Stream):
+    """piper/src/lib.rs:765-858: chunked decoder runs with overlap trimming + crossfade(42).  With a resampler, each
+    chunk's trim and crossfade run on the device and the chunk leaves at the resampler's rate.  With an encoding, they
+    run on the device too and each chunk leaves as G.711 bytes of its to_i16_vec after `gain`."""
+
+    def __init__(self, enc: EncoderOutputs, chunk_size: int, chunk_padding: int,
+                 resampler: Optional[Resampler] = None, encoding: Optional[str] = None, gain: float = 1.0,
+                 warp: Optional[ProsodyStream] = None, meter: Optional[LoudnessStream] = None):
+        super().__init__(None, enc, chunk_size, chunk_padding, resampler, encoding, gain, warp, meter)
+
     def __iter__(self) -> Iterator[AudioSamples]:
         return self
 
     def __next__(self) -> AudioSamples:
-        (m0, m1), (a0, a1) = next(self.chunker)
-        # encoded, resampled or warped: the post-path runs on the device, then the stream's resampler / prosody stream
-        if self.encoding is not None or self.resampler is not None or self.warp is not None or self.meter is not None:
-            if self.one_shot:
-                self.chunker.consume()
-                chunk, fade = (self.enc, 0, self.enc.num_frames, 0, 0), 0
-            else:
-                hi = self.enc.num_frames if m1 is None else m1
-                chunk, fade = (self.enc, m0, hi) + _trim_frames(slice(a0, a1)), 42
-            kw = {}
-            if self.resampler is not None or self.warp is not None or self.meter is not None:
-                kw.update(resamplers=[self.resampler],                  # whether this chunk ends the stream: after
-                          last=[self.chunker.last_end_index is None])   # the one-shot consume()
-            if self.warp is not None:
-                kw["warps"] = [self.warp]
-            if self.meter is not None:
-                kw["meters"] = [self.meter]
-            if self.encoding is not None:
-                kw.update(gains=[self.gain], encoding=self.encoding)
-            return self.enc._m.infer_decoder_batch([chunk], fade=fade, **kw)[0]
-        if self.one_shot:
-            self.chunker.consume()
+        lo, hi, trim = self.next_chunk()
+        if self.on_device:
+            return _device_post(self.enc._m, [(self, lo, hi, trim)])[0]
+        if trim is None:
             return self.enc.infer_decoder()
-        hi = self.enc.num_frames if m1 is None else m1
-        audio = self.enc.infer_decoder(m0, hi).as_slice()
-        audio = audio[a0:a1] if a1 is not None else audio[a0:]
-        out = AudioSamples(audio)
+        out = AudioSamples(self.enc.infer_decoder(lo, hi).as_slice()[trim])
         out.crossfade(42)
         return out
 
@@ -1446,32 +1410,19 @@ class VitsStreamingModel(_VitsCommons):
         equals the `z` of the same utterance synthesised with the same seed.  `speaker_blends`: as for
         infer_batch_with_values; each latent keeps its blend, and every decoder chunk of it speaks with that blend."""
         n = len(batches)
-        cfgs = _config_array(configs, n)
-        scales, frames = _duration_arrays([len(b) for b in batches], duration_scales, durations)
-        sv, sf = _seed_arrays(seeds, n)
-        bs, bw, bo = _blend_arrays(self, speaker_blends, n)
-        if any(len(b) == 0 for b in batches):
-            raise OperationError("Failed to run model inference. Error: empty input sequence")
+        o = _batch_options(self, n, [len(b) for b in batches], configs, duration_scales, durations, seeds,
+                           speaker_blends=speaker_blends)
+        _check_not_empty(batches)
         if n == 0:
             return []
-        packed = np.ascontiguousarray(np.concatenate([np.asarray(b, dtype=np.int64) for b in batches]))
-        offs = np.zeros(n + 1, dtype=np.uint64)
-        offs[1:] = np.cumsum([len(b) for b in batches])
+        packed, offs = _pack_ids(batches)
         outs = (C.c_void_p * n)()
         err = N.sb200_error()
-        if bo is None:
-            _check(self._lib.sb200_encode_batch_ids_seeded(self._h, packed.ctypes.data_as(C.POINTER(C.c_int64)),
-                                                           offs.ctypes.data_as(C.POINTER(C.c_size_t)), n, cfgs,
-                                                           _ptr(scales, C.c_float), _ptr(frames, C.c_int32),
-                                                           _ptr(sv, C.c_uint64), _ptr(sf, C.c_int32), outs,
-                                                           C.byref(err)), err)
-        else:
-            _check(self._lib.sb200_encode_batch_ids_blends(self._h, packed.ctypes.data_as(C.POINTER(C.c_int64)),
-                                                           offs.ctypes.data_as(C.POINTER(C.c_size_t)), n, cfgs,
-                                                           _ptr(scales, C.c_float), _ptr(frames, C.c_int32),
-                                                           _ptr(sv, C.c_uint64), _ptr(sf, C.c_int32),
-                                                           _ptr(bs, C.c_int64), _ptr(bw, C.c_float),
-                                                           _ptr(bo, C.c_size_t), outs, C.byref(err)), err)
+        _check(self._lib.sb200_encode_batch_ids_blends(
+            self._h, _ptr(packed, C.c_int64), _ptr(offs, C.c_size_t), n, o.cfgs, _ptr(o.scales, C.c_float),
+            _ptr(o.frames, C.c_int32), _ptr(o.seeds, C.c_uint64), _ptr(o.seeded, C.c_int32),
+            _ptr(o.blend_speakers, C.c_int64), _ptr(o.blend_weights, C.c_float), _ptr(o.blend_offsets, C.c_size_t),
+            outs, C.byref(err)), err)
         return [EncoderOutputs(self, C.c_void_p(outs[i])) for i in range(n)]
 
     def infer_decoder_batch(self, chunks: Sequence[tuple], pcm16: bool = False, fade: int = 0,
@@ -1528,26 +1479,9 @@ class VitsStreamingModel(_VitsCommons):
         p64 = lambda a: a.ctypes.data_as(C.POINTER(C.c_int64))
         err = N.sb200_error()
         if resamplers is not None or warps is not None or meters is not None:
-            resamplers = _per_utterance([None] * n if resamplers is None else resamplers, n, "resamplers")
-            rs = (C.c_void_p * n)()
-            for k, r in enumerate(resamplers):
-                if r is not None and (not isinstance(r, Resampler) or not r._h):
-                    raise OperationError(f"chunk {k}: not a Resampler")
-                rs[k] = None if r is None else r._h.value
-            ws = None
-            if warps is not None:
-                ws = (C.c_void_p * n)()
-                for k, w in enumerate(_per_utterance(warps, n, "warps")):
-                    if w is not None and (not isinstance(w, ProsodyStream) or not w._h):
-                        raise OperationError(f"chunk {k}: not a ProsodyStream")
-                    ws[k] = None if w is None else w._h.value
-            ms = None
-            if meters is not None:
-                ms = (C.c_void_p * n)()
-                for k, m in enumerate(_per_utterance(meters, n, "meters")):
-                    if m is not None and (not isinstance(m, LoudnessStream) or not m._h):
-                        raise OperationError(f"chunk {k}: not a LoudnessStream")
-                    ms[k] = None if m is None else m._h.value
+            rs = _handles([None] * n if resamplers is None else resamplers, n, Resampler, "resamplers")
+            ws = None if warps is None else _handles(warps, n, ProsodyStream, "warps")
+            ms = None if meters is None else _handles(meters, n, LoudnessStream, "meters")
             fl = np.zeros(n, np.int32) if last is None else np.array([1 if x else 0 for x in
                                                                         _per_utterance(last, n, "last flags")], np.int32)
             g = None if gains is None else np.ascontiguousarray(gains, dtype=np.float32)
@@ -1555,18 +1489,9 @@ class VitsStreamingModel(_VitsCommons):
             lens = (C.c_size_t * n)()
             fmt = G711_LAW[encoding] + 2 if encoding else 1 if pcm16 else 0
             gp = None if g is None else g.ctypes.data_as(C.POINTER(C.c_float))
-            if ms is not None:
-                _check(self._lib.sb200_decode_chunks_metered(
-                    self._h, hs, p64(lo), p64(hi), p64(tlo), p64(thi), n, int(fade), gp, rs, ws, ms,
-                    _ptr(fl, C.c_int32), fmt, outs, lens, C.byref(err)), err)
-            elif ws is None:
-                _check(self._lib.sb200_decode_chunks_resampled(
-                    self._h, hs, p64(lo), p64(hi), p64(tlo), p64(thi), n, int(fade), gp, rs, _ptr(fl, C.c_int32), fmt,
-                    outs, lens, C.byref(err)), err)
-            else:
-                _check(self._lib.sb200_decode_chunks_warped(
-                    self._h, hs, p64(lo), p64(hi), p64(tlo), p64(thi), n, int(fade), gp, rs, ws, _ptr(fl, C.c_int32),
-                    fmt, outs, lens, C.byref(err)), err)
+            _check(self._lib.sb200_decode_chunks_metered(
+                self._h, hs, p64(lo), p64(hi), p64(tlo), p64(thi), n, int(fade), gp, rs, ws, ms, _ptr(fl, C.c_int32),
+                fmt, outs, lens, C.byref(err)), err)
             if encoding:
                 return _take_bytes(self._lib, outs, lens)
             if pcm16:
@@ -1628,28 +1553,16 @@ class VitsStreamingModel(_VitsCommons):
             refuse_formants(formant_ratio, "stream_synthesis")
             refuse_prosody(pitch, tempo, "stream_synthesis")
             refuse_contour(pitch_contour, "stream_synthesis")
-        phi = _stream_formant(formant_ratio, "stream")
-        pit, _ = _prosody_arrays([pitch], [tempo], 1)
-        _seed_arrays([seed], 1)
-        _rate_array([output_rate], 1)
-        _check_live_loudness(live_loudness, max_gain_db, encoding, "stream")
-        refuse_flac(encoding, "stream_synthesis")
-        g = _stream_gain(encoding, gain)
-        blended = _blend_arrays(self, [speaker_blend], 1, ["stream"])[0] is not None
-        contour = None
-        if pitch_contour is None:
-            ids = self.phonemes_to_input_ids(phonemes)
+        o = _stream_options(self, "stream_synthesis", None, phonemes, seed=seed, output_rate=output_rate,
+                            encoding=encoding, gain=gain, pitch=pitch, tempo=tempo, pitch_contour=pitch_contour,
+                            formant_ratio=formant_ratio, speaker_blend=speaker_blend, live_loudness=live_loudness,
+                            max_gain_db=max_gain_db)
+        if o.seed is None and o.blend is None:
+            enc = self.infer_encoder(o.ids)
         else:
-            ids, src = self.phonemes_to_input_ids_map(phonemes)
-            contour = _char_values_to_ids(pitch_contour, phonemes, src, "stream", "pitch ratios", _contour_value)
-            _contour_arrays([len(ids)], [contour], pit, ["stream"])
-        if blended:
-            enc = self.infer_encoder_batch([ids], seeds=[seed], speaker_blends=[speaker_blend])[0]
-        else:
-            enc = self.infer_encoder(ids) if seed is None else self.infer_encoder_batch([ids], seeds=[seed])[0]
-        meter = _stream_meter(self, live_loudness, max_gain_db, output_rate, "stream")
-        return SpeechStreamer(enc, chunk_size, chunk_padding, _stream_resampler(self, output_rate), encoding, g,
-                              _stream_prosody(self, pitch, tempo, contour, enc, phi), meter)
+            enc = self.infer_encoder_batch([o.ids], seeds=[o.seed], speaker_blends=[o.blend])[0]
+        resampler, warp, meter = _open_stream(self, o, enc)
+        return SpeechStreamer(enc, chunk_size, chunk_padding, resampler, o.encoding, o.gain, warp, meter)
 
 
 def _stream_gain(encoding, gain) -> float:
@@ -1662,39 +1575,83 @@ def _stream_gain(encoding, gain) -> float:
     return float(_gain_array([gain], 1)[0])
 
 
-class _Stream:
-    """One sentence of a StreamBatch: its latent and its own chunk schedule, with SpeechStreamer's one-shot rule."""
-
-    def __init__(self, key, enc, chunk_size: int, chunk_padding: int, resampler: Optional[Resampler] = None,
-                 encoding: Optional[str] = None, gain: float = 1.0, warp: Optional[ProsodyStream] = None,
-                 meter: Optional[LoudnessStream] = None):
-        self.key, self.enc, self.resampler = key, enc, resampler
-        self.meter = meter
-        self.encoding, self.gain = encoding, gain
-        self.warp = warp
-        self.bounds = _delivered_bounds(warp, resampler)
-        self.chunker = AdaptiveMelChunker(enc.num_frames, chunk_size, chunk_padding)
-        self.one_shot = enc.num_frames <= (chunk_size * 2 + chunk_padding * 2)
-
-    def next_chunk(self):
-        """(lo, hi, audio slice or None): the frames to decode next, and how SpeechStreamer.__next__ trims them (None:
-        the one-shot chunk, returned as decoded)."""
-        (m0, m1), (a0, a1) = next(self.chunker)
-        if self.one_shot:
-            self.chunker.consume()
-            return 0, self.enc.num_frames, None
-        return m0, self.enc.num_frames if m1 is None else m1, slice(a0, a1)
-
-    @property
-    def done(self) -> bool:
-        return self.chunker.last_end_index is None
-
-
 def _check_chunking(chunk_size, chunk_padding):
     if not isinstance(chunk_size, int) or chunk_size < 1:
         raise OperationError(f"Invalid chunk size {chunk_size!r}: expected a positive integer")
     if not isinstance(chunk_padding, int) or chunk_padding < 0:
         raise OperationError(f"Invalid chunk padding {chunk_padding!r}: expected a non-negative integer")
+
+
+@dataclass
+class _StreamOptions:
+    """One stream's options, checked once by _stream_options."""
+    key: Optional[int]                  # its StreamBatch key (None: a stream_synthesis stream)
+    who: str                            # what its errors name
+    ids: List[int]
+    config: Optional[PiperSynthesisConfig]
+    chunk_size: Optional[int]
+    seed: Optional[int]
+    output_rate: Optional[int]
+    encoding: Optional[str]
+    gain: float
+    pitch: Optional[float]
+    tempo: Optional[float]
+    contour: Optional[Sequence]         # per id
+    formant: Optional[float]
+    blend: Optional[dict]
+    live_loudness: object               # None, a target in LUFS or a LoudnessStream to continue
+    max_gain_db: Optional[float]
+
+
+def _stream_options(model, where: str, key: Optional[int], ids_or_phonemes, config=None, chunk_size=None,
+                    chunk_padding=None, seed=None, output_rate=None, encoding=None, gain=None, pitch=None, tempo=None,
+                    pitch_contour=None, formant_ratio=None, speaker_blend=None, live_loudness=None, max_gain_db=None,
+                    carried=()) -> _StreamOptions:
+    """The options of one stream of `model`, checked in one order: config, live loudness, speaker blend, formant ratio,
+    pitch and tempo, seed, output rate, FLAC (refused by the name `where`), encoding and gain, the config's speaker,
+    chunking, then the ids (phonemes are mapped) and the contour.  Errors name "stream" (key None) or "stream {key}".
+    `chunk_size`: checked with `chunk_padding` when given.  `carried`: the LoudnessStreams the caller's unfinished
+    streams carry, which live_loudness may not be."""
+    if config is not None and not isinstance(config, PiperSynthesisConfig):
+        raise OperationError("Invalid configuration for Vits Model")
+    who = "stream" if key is None else f"stream {key}"
+    _check_live_loudness(live_loudness, max_gain_db, encoding, who)
+    if isinstance(live_loudness, LoudnessStream):
+        if any(m is live_loudness for m in carried):
+            raise OperationError(f"{who}: the LoudnessStream is already carried by an unfinished stream of this batch")
+        _stream_meter(model, live_loudness, None, output_rate, who)
+    _blend_arrays(model, [speaker_blend], 1, [who])
+    phi = _stream_formant(formant_ratio, who)
+    pit, _ = _prosody_arrays([pitch], [tempo], 1)
+    _seed_arrays([seed], 1)
+    _rate_array([output_rate], 1)
+    refuse_flac(encoding, where)
+    g = _stream_gain(encoding, gain)
+    if config is not None and config.speaker is not None and config.speaker not in (model.get_speakers() or {}):
+        raise OperationError(f"No speaker was found with the given id `{config.speaker}`")     # as check_config
+    if chunk_size is not None:
+        _check_chunking(chunk_size, chunk_padding)
+    contour = pitch_contour
+    if isinstance(ids_or_phonemes, str) and pitch_contour is not None:
+        ids, src = model.phonemes_to_input_ids_map(ids_or_phonemes)
+        contour = _char_values_to_ids(pitch_contour, ids_or_phonemes, src, who, "pitch ratios", _contour_value)
+    elif isinstance(ids_or_phonemes, str):
+        ids = model.phonemes_to_input_ids(ids_or_phonemes)
+    else:
+        ids = [int(i) for i in ids_or_phonemes]
+    if contour is not None:
+        _contour_arrays([len(ids)], [contour], pit, [who])
+    if not ids:
+        raise OperationError("Failed to run model inference. Error: empty input sequence")
+    return _StreamOptions(key, who, ids, config, chunk_size, seed, output_rate, encoding, g, pitch, tempo, contour, phi,
+                          speaker_blend, live_loudness, max_gain_db)
+
+
+def _open_stream(model, o: _StreamOptions, enc):
+    """(resampler, ProsodyStream, meter) of a stream with options `o` and latent `enc`, each None when not asked for."""
+    return (_stream_resampler(model, o.output_rate),
+            _stream_prosody(model, o.pitch, o.tempo, o.contour, enc, o.formant),
+            _stream_meter(model, o.live_loudness, o.max_gain_db, o.output_rate, o.who))
 
 
 class StreamBatch:
@@ -1719,9 +1676,7 @@ class StreamBatch:
         _check_chunking(chunk_size, chunk_padding)
         self.model = model
         self.chunk_size, self.chunk_padding = chunk_size, chunk_padding
-        self._pending: list = []      # (key, ids, config, chunk_size, seed, output rate, encoding, gain, pitch, tempo,
-                                      # per-id contour, speaker blend, formant ratio, live loudness, maximum gain) not
-                                      # encoded yet
+        self._pending: List[_StreamOptions] = []      # the streams not encoded yet
         self._active: List[_Stream] = []
         self._retired: dict = {}      # key -> delivered ends (None: no contour) of the streams the last step ended
         self._next_key = 0
@@ -1756,44 +1711,15 @@ class StreamBatch:
              output_rate: Optional[int] = None, encoding: Optional[str] = None, gain: Optional[float] = None,
              pitch: Optional[float] = None, tempo: Optional[float] = None, pitch_contour=None,
              speaker_blend=None, formant_ratio=None, live_loudness=None, max_gain_db=None) -> int:
-        if config is not None and not isinstance(config, PiperSynthesisConfig):
-            raise OperationError("Invalid configuration for Vits Model")
-        who = f"stream {self._next_key}"
-        _check_live_loudness(live_loudness, max_gain_db, encoding, who)
-        if isinstance(live_loudness, LoudnessStream):
-            if any(p[13] is live_loudness for p in self._pending) or any(s.meter is live_loudness
-                                                                         for s in self._active):
-                raise OperationError(f"{who}: the LoudnessStream is already carried by an unfinished stream of this "
-                                     "batch")
-            _stream_meter(self.model, live_loudness, None, output_rate, who)
-        _blend_arrays(self.model, [speaker_blend], 1, [f"stream {self._next_key}"])
-        phi = _stream_formant(formant_ratio, f"stream {self._next_key}")
-        pit, _ = _prosody_arrays([pitch], [tempo], 1)
-        _seed_arrays([seed], 1)
-        _rate_array([output_rate], 1)
-        refuse_flac(encoding, "StreamBatch")
-        gain = _stream_gain(encoding, gain)
-        if config is not None and config.speaker is not None and config.speaker not in (self.model.get_speakers() or {}):
-            raise OperationError(f"No speaker was found with the given id `{config.speaker}`")     # as check_config
-        _check_chunking(chunk_size, self.chunk_padding)
-        contour = pitch_contour
-        if isinstance(ids_or_phonemes, str) and pitch_contour is not None:
-            ids, src = self.model.phonemes_to_input_ids_map(ids_or_phonemes)
-            contour = _char_values_to_ids(pitch_contour, ids_or_phonemes, src, f"stream {self._next_key}",
-                                          "pitch ratios", _contour_value)
-        elif isinstance(ids_or_phonemes, str):
-            ids = self.model.phonemes_to_input_ids(ids_or_phonemes)
-        else:
-            ids = [int(i) for i in ids_or_phonemes]
-        if contour is not None:
-            _contour_arrays([len(ids)], [contour], pit, [f"stream {self._next_key}"])
-        if not ids:
-            raise OperationError("Failed to run model inference. Error: empty input sequence")
-        key = self._next_key
+        carried = [o.live_loudness for o in self._pending] + [s.meter for s in self._active]
+        o = _stream_options(self.model, "StreamBatch", self._next_key, ids_or_phonemes, config, chunk_size,
+                            self.chunk_padding, seed=seed, output_rate=output_rate, encoding=encoding, gain=gain,
+                            pitch=pitch, tempo=tempo, pitch_contour=pitch_contour, formant_ratio=formant_ratio,
+                            speaker_blend=speaker_blend, live_loudness=live_loudness, max_gain_db=max_gain_db,
+                            carried=carried)
         self._next_key += 1
-        self._pending.append((key, ids, config, chunk_size, seed, output_rate, encoding, gain, pitch, tempo, contour,
-                              speaker_blend, phi, live_loudness, max_gain_db))
-        return key
+        self._pending.append(o)
+        return o.key
 
     def bounds(self, key) -> Optional[np.ndarray]:
         """Stream `key`'s per-id delivered ends at its delivered rate (see SpeechStreamer.bounds), or None when it has
@@ -1813,7 +1739,7 @@ class StreamBatch:
 
     def __contains__(self, key) -> bool:
         """Whether stream `key` has chunks still to come."""
-        return any(p[0] == key for p in self._pending) or any(s.key == key for s in self._active)
+        return any(o.key == key for o in self._pending) or any(s.key == key for s in self._active)
 
     def step(self) -> List[tuple]:
         out = []
@@ -1821,28 +1747,26 @@ class StreamBatch:
         if self._pending:
             pend, self._pending = self._pending, []
             fallback = None
-            if any(p[2] is not None for p in pend):
+            if any(o.config is not None for o in pend):
                 fallback = self.model.get_fallback_synthesis_config()
 
             def encode(ps):
-                configs = None if fallback is None else [fallback if p[2] is None else p[2] for p in ps]
-                extra = {}
-                if any(p[11] is not None for p in ps):
-                    extra["speaker_blends"] = [p[11] for p in ps]
-                if all(p[4] is None for p in ps):
-                    return self.model.infer_encoder_batch([p[1] for p in ps], configs, **extra)
-                return self.model.infer_encoder_batch([p[1] for p in ps], configs, seeds=[p[4] for p in ps], **extra)
-            for p, (enc, err) in zip(pend, _each_or_alone(encode, pend)):
+                ids = [o.ids for o in ps]
+                configs = None if fallback is None else [fallback if o.config is None else o.config for o in ps]
+                if all(o.seed is None and o.blend is None for o in ps):
+                    return self.model.infer_encoder_batch(ids, configs)
+                return self.model.infer_encoder_batch(ids, configs, seeds=[o.seed for o in ps],
+                                                      speaker_blends=[o.blend for o in ps])
+            for o, (enc, err) in zip(pend, _each_or_alone(encode, pend)):
                 if err is None:
                     try:
-                        active.append(_Stream(p[0], enc, p[3], self.chunk_padding,
-                                              _stream_resampler(self.model, p[5]), p[6], p[7],
-                                              _stream_prosody(self.model, p[8], p[9], p[10], enc, p[12]),
-                                              _stream_meter(self.model, p[13], p[14], p[5], f"stream {p[0]}")))
+                        resampler, warp, meter = _open_stream(self.model, o, enc)
+                        active.append(_Stream(o.key, enc, o.chunk_size, self.chunk_padding, resampler, o.encoding,
+                                              o.gain, warp, meter))
                         continue
                     except SonataError as e:
                         err = e
-                out.append((p[0], err))
+                out.append((o.key, err))
         plan = [(s,) + s.next_chunk() for s in active]
         failed = set()
         # one pass per (encoding, resampled, one-shot, warped, metered): the streams without an encoding first, in
@@ -1851,29 +1775,15 @@ class StreamBatch:
         groups = {plain_key: [], (None, True, False, False, False): [], (None, True, True, False, False): []}
         for p in plan:
             s = p[0]
-            plain = s.encoding is None and s.resampler is None and s.warp is None and s.meter is None
-            k = plain_key if plain else (s.encoding, s.resampler is not None, p[3] is None, s.warp is not None,
-                                         s.meter is not None)
+            k = plain_key if not s.on_device else (s.encoding, s.resampler is not None, p[3] is None,
+                                                   s.warp is not None, s.meter is not None)
             groups.setdefault(k, []).append(p)
-
-        def device_post(pl, key):
-            encoding, resampled, whole, warped, metered = key
-            chunks = [(s.enc, lo, hi) + ((0, 0) if trim is None else _trim_frames(trim)) for s, lo, hi, trim in pl]
-            extra = {} if not (resampled or warped or metered) else {"resamplers": [p[0].resampler for p in pl],
-                                                                     "last": [p[0].done for p in pl]}
-            if warped:
-                extra["warps"] = [p[0].warp for p in pl]
-            if metered:
-                extra["meters"] = [p[0].meter for p in pl]
-            if encoding is not None:
-                extra.update(encoding=encoding, gains=[p[0].gain for p in pl])
-            return self.model.infer_decoder_batch(chunks, fade=0 if whole else 42, **extra)
         decoded = {}
         for key, group in groups.items():
             if key == plain_key:
                 call = lambda pl: self.model.infer_decoder_batch([(s.enc, lo, hi) for s, lo, hi, _ in pl])
             else:
-                call = lambda pl, key=key: device_post(pl, key)
+                call = lambda pl: _device_post(self.model, pl)
             if group:
                 decoded.update({id(p): r for p, r in zip(group, _each_or_alone(call, group))})
         for p in plan:
@@ -1883,7 +1793,7 @@ class StreamBatch:
                 out.append((s.key, err))
                 failed.add(s.key)
                 continue
-            if trim is not None and s.resampler is None and s.encoding is None and s.warp is None and s.meter is None:
+            if trim is not None and not s.on_device:
                 a = AudioSamples(a.as_slice()[trim])
                 a.crossfade(42)
             out.append((s.key, a))

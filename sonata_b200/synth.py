@@ -335,7 +335,6 @@ class SonataSpeechSynthesizer:
                                "request")
         sentence_seed(seed, 0)
         _check_output_rate(output_rate)
-        refuse_flac(encoding, "synthesize_streamed")
         check_encoding(encoding)
         if encoding is not None and output_config is not None:
             output_config._check_supported()
@@ -513,7 +512,6 @@ class RealtimeBatch:
         refuse_flac(encoding, "RealtimeBatch")
         sentence_seed(seed, 0)
         _check_output_rate(output_rate)
-        refuse_flac(encoding, "RealtimeBatch")
         check_encoding(encoding)
         if output_config is not None:
             output_config._check_supported()
@@ -538,18 +536,12 @@ class RealtimeBatch:
             return
         req.cs = next_chunk_size(req.cs, req.produced)
         req.n = 0
-        rate = {} if req.output_rate is None else {"output_rate": req.output_rate}
-        if req.encoding is not None:
-            rate["encoding"] = req.encoding
-            if req.output_config is not None and req.output_config.gain() is not None:
-                rate["gain"] = req.output_config.gain()
-        rate.update(req.prosody)
-        if req.blend is not None:
-            rate["speaker_blend"] = req.blend
-        if req.meter is not None:
-            rate["live_loudness"] = req.meter
-        self._by_stream[self._streams._add(req.ids[req.next], req.config, req.cs, sentence_seed(req.seed, req.next),
-                                           **rate)] = req
+        # the volume of an encoded request is a gain before its encoding; otherwise it applies to the chunks here
+        gain = req.output_config.gain() if req.encoding is not None and req.output_config is not None else None
+        key = self._streams._add(req.ids[req.next], req.config, req.cs, sentence_seed(req.seed, req.next),
+                                 req.output_rate, req.encoding, gain, speaker_blend=req.blend,
+                                 live_loudness=req.meter, **req.prosody)
+        self._by_stream[key] = req
         req.next += 1
 
     def __len__(self) -> int:

@@ -140,25 +140,27 @@ class FakeModel:
                 src += [c, c]
         return ids + [2], src + [-1]
 
-    def infer_batch_with_durations(self, batches, configs=None, duration_scales=None, durations=None):
-        self.calls.append((batches, configs, duration_scales))
+    def _speak_ids(self, batches, o, frames=False):
+        offs = np.cumsum([0] + [len(ids) for ids in batches])
+        scales = None if o.scales is None else [o.scales[offs[b]:offs[b + 1]].tolist() for b in range(len(batches))]
+        self.calls.append((batches, o.cfgs, scales))
         out = []
         for b, ids in enumerate(batches):
-            s = duration_scales[b] if duration_scales and duration_scales[b] is not None else [1.0] * len(ids)
+            s = scales[b] if scales else [1.0] * len(ids)
             f = np.array([math.ceil(x * (i % 4)) for i, x in zip(ids, s)], np.int32)
             n = max(int(f.sum()), 1) * 256
-            out.append((Audio(np.zeros(n, np.float32), 22050), f))
+            out.append((Audio(np.zeros(n, np.float32), 22050), f, None))
         return out
 
 
-def test_alignment_groups_ids_by_character():
+def test_alignment_groups_ids_by_character_through_the_f32_route():
     fake = FakeModel()
     ph = "ab~c"
     res = _VitsCommons.speak_batch_with_alignment(fake, [ph, "~"], duration_scales=[[2.0, 1.0, float("nan"), 0.5], None])
     (audio, al), (audio2, al2) = res
     ids, src = fake.phonemes_to_input_ids_map(ph)
     assert fake.calls[0][2][0] == [1.0, 2.0, 2.0, 1.0, 1.0, 0.5, 0.5, 1.0]      # the NaN of a dropped character is ignored
-    assert fake.calls[0][2][1] is None
+    assert fake.calls[0][2][1] == [1.0, 1.0]                                     # bos and eos of "~": no scales
     assert [a.phoneme for a in al] == ["^", "a", "b", "c", "$"]
     assert al[0].start_sample == 0 and all(x.start_sample + x.num_samples == y.start_sample for x, y in zip(al, al[1:]))
     assert al[-1].start_sample + al[-1].num_samples == len(audio)

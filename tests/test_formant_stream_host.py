@@ -185,7 +185,7 @@ class _Streaming(VitsStreamingModel):
         pass
 
 
-def test_stream_batch_checks_each_stream(monkeypatch):
+def test_stream_batch_checks_each_stream_option(monkeypatch):
     m = _Streaming()
     sb = StreamBatch(m, 40, 3)
     sb.add([1, 2, 3])
@@ -195,8 +195,8 @@ def test_stream_batch_checks_each_stream(monkeypatch):
     with pytest.raises(OperationError, match="stream 2: formant ratio 'a' is not a number"):
         sb.add([1, 2, 3], formant_ratio="a")
     k = sb.add([1, 2, 3], formant_ratio=NAN, pitch=1.25)
-    assert [p[12] for p in sb._pending] == [None, 1.2, None]
-    assert sb._pending[-1][0] == k == 2
+    assert [o.formant for o in sb._pending] == [None, 1.2, None]
+    assert sb._pending[-1].key == k == 2
 
 
 def test_stream_prosody_decides_what_asks(monkeypatch):
