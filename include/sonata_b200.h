@@ -338,6 +338,41 @@ int32_t sb200_speak_batch_ids_blends(sb200_voice* v, const int64_t* ids_packed, 
                                      const size_t* blend_offsets, sb200_audio* outs, int32_t* id_frames_out,
                                      int64_t* bounds_out, double* lufs_out, float* gain_out, sb200_error* err);
 
+/* ---- volume contours: a level in dB per id ----
+ * A volume contour gives each id of an utterance a level, packed like ids_packed: a finite value in [-60, 20] dB,
+ * -inf for silence (gain 0), or NaN or exactly 0 for no change.  Any other value fails with OPERATION_ERROR naming the
+ * utterance and the id, before any device work; a contour of NaN / 0 only asks for nothing.  The stage runs at the
+ * voice's rate R on the n2 samples x the formant stage hands out (the pitch stage's output without one, the decoder's
+ * waveform without prosody), after those stages and before any output-rate resampling and loudness, which see its
+ * output as they see a waveform.  It changes no length, delivered end, frame count or alignment.  In double, each
+ * operation rounded (no fused multiply-add):
+ *  1. Pieces.  Id i covers the delivered samples [E_{i-1}, E_i), E_{-1} = 0, with E the ends of step 4 of
+ *     sb200_speak_batch_ids_contour (what sb200_job_prosody_bounds reports; 256 C_i without pitch, tempo or contour;
+ *     the last id always ends at n2).  Ids whose span is empty are dropped, and runs of consecutive ids with equal f32
+ *     levels (NaN -> 0) merge: pieces r = 1 .. m with boundaries 0 = B_0 < B_1 < .. < B_m = n2 and levels v_r, and
+ *     g_r = f32(10^(v_r / 20)) computed on the host (-inf: 0).
+ *  2. Gain curve.  L = 2 (R / 200) samples (integer division: 220 at 22.05 kHz, 160 at 16 kHz, about 10 ms).  Boundary
+ *     r (1 <= r < m) ramps the samples B_r - L/2 <= j < B_r + L/2 with t = (j - B_r + L/2 + 0.5) / L and
+ *     S_r(j) = t t (3 - 2 t).  G_j = g_a + sum (g_{r+1} - g_r) S_r(j) over the boundaries whose ramp covers j, in
+ *     ascending r, with a the piece before the first of them (the piece holding j when none does), rounded to f32 once.
+ *  3. Output.  y_j = x_j G_j, one f32 multiply, with no clamp.
+ * So a contour that merges into one piece is the utterance times g_1 bit for bit, an utterance whose pieces all have
+ * gain 1 runs nothing and keeps its bits, and a contoured utterance has the same bits in any batch.  A loudness target
+ * normalises the contoured utterance as a whole, so the contour's relative levels survive it.  The executable
+ * specification is tests/volume_reference.py.  Realtime streams take a contour through
+ * sb200_prosody_stream_create_volume, with the same bits as this call.
+ * sb200_speak_batch_ids_blends with volume_db_packed (NULL: none) the contours of the batch, packed like ids_packed.
+ * NULL is that call, bit for bit. */
+int32_t sb200_speak_batch_ids_volume(sb200_voice* v, const int64_t* ids_packed, const size_t* offsets, size_t batch,
+                                     const sb200_synth_config* cfgs, const float* scale_packed,
+                                     const int32_t* frames_packed, const uint64_t* seeds, const int32_t* seeded,
+                                     const uint32_t* output_rates, const float* target_lufs, const float* pitch,
+                                     const float* tempo, const float* pitch_packed, const float* formants,
+                                     const int64_t* blend_speakers, const float* blend_weights,
+                                     const size_t* blend_offsets, const float* volume_db_packed, sb200_audio* outs,
+                                     int32_t* id_frames_out, int64_t* bounds_out, double* lufs_out, float* gain_out,
+                                     sb200_error* err);
+
 /* ---- job API: the same batched pass split into its host<->device steps (bench / multi-GPU plumbing) ----
  * create  : copies ids to the device (H2D).  `eps_w` / `eps_z` optionally inject the graph's two
  *           RandomNormalLike draws (time-major: eps_w[b] = f32[T_x][2], eps_z[b] = f32[T_y][inter]);
@@ -403,6 +438,12 @@ int32_t sb200_job_set_pitch_contour(sb200_job* job, const float* pitch_packed, s
  * job as it was.  A ratio of 1 asks for something on an utterance with a pitch ratio or contour.  The result keeps
  * its layout: the stage changes no length or offset. */
 int32_t sb200_job_set_formants(sb200_job* job, const float* formants, sb200_error* err);
+/* A volume contour (see sb200_speak_batch_ids_volume) for the next sb200_job_run, packed like ids_packed, or NULL for
+ * none (what a new job starts with; so is a contour that is all NaN or 0).  Checked like sb200_job_set_pitch_contour: a
+ * bad entry fails with OPERATION_ERROR naming the utterance and the id, and leaves the job as it was.  A run with a
+ * contour copies the batch's cumulative durations to the host with the frame counts, and sb200_job_profile reports the
+ * stage as the region "volume".  The result keeps its layout: the stage scales it in place. */
+int32_t sb200_job_set_volume_contour(sb200_job* job, const float* volume_db_packed, sb200_error* err);
 /* Speaker blends (see sb200_speak_batch_ids_blends) for the next sb200_job_run as a blend table, or NULL offsets for none
  * (what a new job starts with).  Every entry is checked first; a bad one fails with OPERATION_ERROR naming the utterance
  * and leaves the job's blends as they were. */
@@ -648,6 +689,26 @@ int32_t sb200_prosody_stream_create_formant(sb200_voice* v, const sb200_latent* 
                                             sb200_prosody_stream** out, sb200_error* err);
 /* The "formant" device time (ms) of the last chunk pass the stream was in (0: its stage did not run). */
 int32_t sb200_prosody_stream_profile_formant(const sb200_prosody_stream* s, float* formant_ms);
+/* ---- streams with a volume contour (see sb200_speak_batch_ids_volume) ----
+ * sb200_prosody_stream_create_formant with volume_db_per_id[0 .. n_ids) (NULL: none), one level per id of latent z
+ * (required with a contour; n_ids its id count, shared with pitch_per_id when both are given).  Like the formant
+ * creator it accepts ratios and a phi that ask for nothing when the contour asks for something: a volume-only stream.
+ * A contour that asks for nothing gives the stream sb200_prosody_stream_create_formant gives: the same chunk counts,
+ * bits and launches.  The ends and pieces are fixed at creation from the latent's frames (the ends the batch path
+ * gives for the same latent, ratios and contour) and the piece table is uploaded once, into the stream's own
+ * allocation.  A bad level fails naming the id, as do a wrong n_ids and another voice's latent, all with
+ * OPERATION_ERROR before any device work.
+ * Emission: G_j depends only on j and the ends, so the stage holds nothing back.  Every sample the stages before it
+ * emit is scaled at its delivered position, in the chunk pass's region "volume", after "formant" and before
+ * resampling and any meter.  Contract: join the chunks such a stream emits through sb200_decode_chunks_warped or
+ * sb200_decode_chunks_metered; the result is, bit for bit, the batch contract applied to the joined chunks the same
+ * stream yields without the contour, then resampled, metered and converted as without it. */
+int32_t sb200_prosody_stream_create_volume(sb200_voice* v, const sb200_latent* z, float pitch,
+                                           const float* pitch_per_id, size_t n_ids, float tempo, float formant,
+                                           const float* volume_db_per_id, sb200_prosody_stream** out,
+                                           sb200_error* err);
+/* The "volume" device time (ms) of the last chunk pass the stream was in (0: its stage did not run). */
+int32_t sb200_prosody_stream_profile_volume(const sb200_prosody_stream* s, float* volume_ms);
 
 /* ---- live loudness: a stream held to a target by a causal BS.1770 meter carried on the device ----
  * A loudness stream (a meter) belongs to a voice, and so to its device, and meters one delivered rate r.  Its target T
@@ -850,6 +911,12 @@ int32_t sb200_debug_speaker_blend(sb200_voice* v, const int64_t* speakers, const
 int32_t sb200_debug_formant(int32_t device, const float* x, size_t n, int32_t rate, float pitch, float tempo,
                             const int64_t* ends, const float* ratios, size_t n_ids, float phi, float* pre, float* y,
                             size_t cap, int64_t* n2_out, sb200_error* err);
+/* The volume stage over one caller buffer x[0 .. n) at `rate`, whose id i ends at delivered sample ends[i]
+ * (non-decreasing, the last at n) with levels[i] (n_ids entries, checked as sb200_speak_batch_ids_volume checks them):
+ * y[0 .. n) receives the result, x itself when the pieces ask for nothing; bit for bit what a job gives an utterance
+ * of those samples and ends. */
+int32_t sb200_debug_volume(int32_t device, const float* x, size_t n, const int64_t* ends, const float* levels,
+                           size_t n_ids, int32_t rate, float* y, sb200_error* err);
 /* Test hook, no device needed: the samples a prosody stream with these ratios at `rate` emits per chunk (the rule of
  * sb200_decode_chunks_warped) when its chunks bring chunk_lens[0 .. n_chunks) inputs and the last one ends it.
  * emitted[k] receives chunk k's count.  Returns 0, or 19 for bad ratios, a bad rate or a negative length. */

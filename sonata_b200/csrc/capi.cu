@@ -325,14 +325,15 @@ static void job_prosody(const Job& j, int64_t* n1, int64_t* n2, int32_t* frames)
     }
 }
 
-int32_t sb200_speak_batch_ids_blends(sb200_voice* v, const int64_t* ids, const size_t* offsets, size_t batch,
+int32_t sb200_speak_batch_ids_volume(sb200_voice* v, const int64_t* ids, const size_t* offsets, size_t batch,
                                      const sb200_synth_config* cfgs, const float* scale_packed,
                                      const int32_t* frames_packed, const uint64_t* seeds, const int32_t* seeded,
                                      const uint32_t* output_rates, const float* target_lufs, const float* pitch,
                                      const float* tempo, const float* pitch_packed, const float* formants,
                                      const int64_t* blend_speakers, const float* blend_weights,
-                                     const size_t* blend_offsets, sb200_audio* outs, int32_t* id_frames_out,
-                                     int64_t* bounds_out, double* lufs_out, float* gain_out, sb200_error* err) {
+                                     const size_t* blend_offsets, const float* volume_db_packed, sb200_audio* outs,
+                                     int32_t* id_frames_out, int64_t* bounds_out, double* lufs_out, float* gain_out,
+                                     sb200_error* err) {
     return guarded(err, [&] {
         const double t0 = now_ms();
         static_assert(sizeof(long long) == sizeof(int64_t), "");
@@ -347,6 +348,7 @@ int32_t sb200_speak_batch_ids_blends(sb200_voice* v, const int64_t* ids, const s
         check_formants(formants, batch);
         canonical_blends(*v->v, reinterpret_cast<const long long*>(blend_speakers), blend_weights, blend_offsets, batch,
                          "utterance");
+        check_volume_contour(volume_db_packed, offsets, batch);
         std::unique_ptr<Job> j(create_job(v->v.get(), reinterpret_cast<const long long*>(ids), offsets, batch, nullptr,
                                           nullptr, nullptr, false));
         if (cfgs) set_job_configs(*j, cfgs_in(cfgs, batch).data());
@@ -358,6 +360,7 @@ int32_t sb200_speak_batch_ids_blends(sb200_voice* v, const int64_t* ids, const s
         set_job_pitch_contour(*j, pitch_packed);
         set_job_formants(*j, formants);
         set_job_blends(*j, reinterpret_cast<const long long*>(blend_speakers), blend_weights, blend_offsets);
+        set_job_volume_contour(*j, volume_db_packed);
         j->run(nullptr, 0);
         fetch_audio(*j, outs, 0.f);
         if (id_frames_out) {
@@ -373,6 +376,19 @@ int32_t sb200_speak_batch_ids_blends(sb200_voice* v, const int64_t* ids, const s
         for (size_t b = 0; b < batch; b++)
             outs[b].inference_ms = wall * (j->out_total ? (float)outs[b].len / (float)j->out_total : 0.f);
     });
+}
+int32_t sb200_speak_batch_ids_blends(sb200_voice* v, const int64_t* ids, const size_t* offsets, size_t batch,
+                                     const sb200_synth_config* cfgs, const float* scale_packed,
+                                     const int32_t* frames_packed, const uint64_t* seeds, const int32_t* seeded,
+                                     const uint32_t* output_rates, const float* target_lufs, const float* pitch,
+                                     const float* tempo, const float* pitch_packed, const float* formants,
+                                     const int64_t* blend_speakers, const float* blend_weights,
+                                     const size_t* blend_offsets, sb200_audio* outs, int32_t* id_frames_out,
+                                     int64_t* bounds_out, double* lufs_out, float* gain_out, sb200_error* err) {
+    return sb200_speak_batch_ids_volume(v, ids, offsets, batch, cfgs, scale_packed, frames_packed, seeds, seeded,
+                                        output_rates, target_lufs, pitch, tempo, pitch_packed, formants, blend_speakers,
+                                        blend_weights, blend_offsets, nullptr, outs, id_frames_out, bounds_out, lufs_out,
+                                        gain_out, err);
 }
 int32_t sb200_speak_batch_ids_formants(sb200_voice* v, const int64_t* ids, const size_t* offsets, size_t batch,
                                        const sb200_synth_config* cfgs, const float* scale_packed,
@@ -507,6 +523,9 @@ int32_t sb200_job_set_pitch_contour(sb200_job* job, const float* pitch_packed, s
 }
 int32_t sb200_job_set_formants(sb200_job* job, const float* formants, sb200_error* err) {
     return guarded(err, [&] { set_job_formants(*job->j, formants); });
+}
+int32_t sb200_job_set_volume_contour(sb200_job* job, const float* volume_db_packed, sb200_error* err) {
+    return guarded(err, [&] { set_job_volume_contour(*job->j, volume_db_packed); });
 }
 int32_t sb200_job_set_speaker_blends(sb200_job* job, const int64_t* speakers, const float* weights, const size_t* offsets,
                                      sb200_error* err) {
@@ -805,27 +824,35 @@ int32_t sb200_prosody_stream_create_contour(sb200_voice* v, const sb200_latent* 
 int32_t sb200_prosody_stream_create_formant(sb200_voice* v, const sb200_latent* z, float pitch,
                                             const float* pitch_per_id, size_t n_ids, float tempo, float formant,
                                             sb200_prosody_stream** out, sb200_error* err) {
+    return sb200_prosody_stream_create_volume(v, z, pitch, pitch_per_id, n_ids, tempo, formant, nullptr, out, err);
+}
+int32_t sb200_prosody_stream_create_volume(sb200_voice* v, const sb200_latent* z, float pitch,
+                                           const float* pitch_per_id, size_t n_ids, float tempo, float formant,
+                                           const float* volume_db_per_id, sb200_prosody_stream** out,
+                                           sb200_error* err) {
     return guarded(err, [&] {
-        if (!v || !out || (pitch_per_id && !z)) throw Error(19, "null argument");
+        if (!v || !out || ((pitch_per_id || volume_db_per_id) && !z)) throw Error(19, "null argument");
         Voice* w = v->v.get();
         if (w->device < 0 || !w->emb)
             throw Error(19, "Failed to run model inference. Error: voice was loaded config-only (device -1); libsonata_b200 has no CPU path");
         std::vector<long long> ends;
         long long n = -1;
-        if (pitch_per_id) {
+        if (pitch_per_id || volume_db_per_id) {
             if (z->l->v != w) throw Error(19, "the latent was not encoded by this voice");
             const std::vector<int>& f = z->l->id_frames;
             if (n_ids != f.size())
-                throw Error(19, "pitch contour: " + std::to_string(n_ids) + " ratios for a latent of " +
-                                    std::to_string(f.size()) + " ids");
+                throw Error(19, std::string(pitch_per_id ? "pitch contour: " : "volume contour: ") +
+                                    std::to_string(n_ids) + (pitch_per_id ? " ratios" : " levels") +
+                                    " for a latent of " + std::to_string(f.size()) + " ids");
             const long long hop = w->a.hop();
             ends.resize(n_ids);
             long long c = 0;
             for (size_t i = 0; i < n_ids; i++) ends[i] = (c += f[i]) * hop;
             n = z->l->frames * hop;
         }
-        *out = new sb200_prosody_stream{create_prosody_stream_formant(w, w->device, w->sample_rate, n, ends.data(),
-                                                                      pitch_per_id, n_ids, pitch, tempo, formant),
+        *out = new sb200_prosody_stream{create_prosody_stream_volume(w, w->device, w->sample_rate, n, ends.data(),
+                                                                     pitch_per_id, n_ids, pitch, tempo, formant,
+                                                                     volume_db_per_id),
                                         v->v};
     });
 }
@@ -850,6 +877,11 @@ int32_t sb200_prosody_stream_profile(const sb200_prosody_stream* s, float* stret
 int32_t sb200_prosody_stream_profile_formant(const sb200_prosody_stream* s, float* formant_ms) {
     if (!s) return 19;
     if (formant_ms) *formant_ms = s->p->last_fm_ms;
+    return 0;
+}
+int32_t sb200_prosody_stream_profile_volume(const sb200_prosody_stream* s, float* volume_ms) {
+    if (!s) return 19;
+    if (volume_ms) *volume_ms = s->p->last_vol_ms;
     return 0;
 }
 
@@ -1409,6 +1441,23 @@ int32_t sb200_debug_formant(int32_t device, const float* x, size_t n, int32_t ra
         SB_CUDA(cudaMemcpy(pre, before, (size_t)g.n2 * 4, cudaMemcpyDeviceToHost));
         SB_CUDA(cudaMemcpy(y, o.fp.segs.empty() ? before : h.b.fy, (size_t)g.n2 * 4, cudaMemcpyDeviceToHost));
         if (n2_out) *n2_out = g.n2;
+    });
+}
+
+int32_t sb200_debug_volume(int32_t device, const float* x, size_t n, const int64_t* ends, const float* levels,
+                           size_t n_ids, int32_t rate, float* y, sb200_error* err) {
+    return guarded(err, [&] {
+        if ((n && (!x || !y)) || (n_ids && (!ends || !levels)) || rate < 200)
+            throw Error(19, "debug volume: bad arguments");
+        const size_t offs[2] = {0, n_ids};
+        check_volume_contour(levels, offs, 1, false);
+        const std::vector<VolumePiece> pc =
+            volume_pieces(reinterpret_cast<const long long*>(ends), levels, n_ids, (long long)n);
+        OutputPlan o;
+        if (!pc.empty()) o.vp.add(0, (long long)n, 0, volume_half(rate), pc);
+        SB_CUDA(cudaSetDevice(device));
+        HookStage h(o, x, n);
+        if (n) SB_CUDA(cudaMemcpy(y, h.b.in, n * 4, cudaMemcpyDeviceToHost));
     });
 }
 

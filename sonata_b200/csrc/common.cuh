@@ -381,6 +381,21 @@ struct ProsodyCarry {
     const float *in_hist, *s_hist; const int* d_hist;
     float *in_next, *s_next; int* d_next;
 };
+// Volume contours (volume.cu; include/sonata_b200.h, sb200_speak_batch_ids_volume).  Piece r of a contour starts at
+// delivered sample B (B = 0 for the first) and has gain g.
+struct VolumePiece { long long B; float g; };
+// One signal's volume stage: samples [j0, j0 + n) of the delivered signal become y[0 .. n), y_j = x_j G_j, with the
+// gain curve of its m pieces pc and ramps of 2 half samples.  x: the samples, read plainly, or null for chunk `chunk` of
+// the pass's input read through its post-path (fsegs / posts).  x may equal y.
+struct VolumeSeg {
+    const float* x; float* y;
+    long long n, j0;
+    int chunk, half, m;
+    const VolumePiece* pc;
+};
+// One launch over the segments: blockIdx.y = segment, max_n: the most samples of any segment.
+void launch_volume(const VolumeSeg* segs, int nseg, long long max_n, const float* src, const FrameSeg* fsegs,
+                   const PcmPost* posts, int hop, cudaStream_t st);
 // Analysis position of WSOLA frame k: floor(k Hs / alpha + 0.5), every operation exactly rounded in double, so the host
 // plan and the kernels agree; the virtual frame -1 sits at -Hs.
 __host__ __device__ inline long long prosody_analysis(int Hs, double alpha, long long k) {

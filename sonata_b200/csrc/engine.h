@@ -278,10 +278,40 @@ struct ProsodyStream {
     int fm_h = 0;
     float* fm_hist[2] = {nullptr, nullptr};
     float last_fm_ms = 0.f;
+    // The volume stage (volume.cu): the contour's pieces over the delivered samples, fixed at creation (empty: none),
+    // resident on the device after the pitch contour's table (vol_d), and its last region time.
+    std::vector<VolumePiece> vol;
+    const VolumePiece* vol_d = nullptr;
+    float last_vol_ms = 0.f;
     ~ProsodyStream();
 };
 // Whether stream ps runs the stretch or pitch stage (a formant-only stream runs neither).
 inline bool prosody_stream_warps(const ProsodyStream& ps) { return ps.sh.stretch || ps.sh.pitch; }
+// Volume contours (volume.cu).  Checks a volume contour packed[0 .. offs[B]) of B utterances or, with !per_utterance,
+// of one stream: a level is NaN or 0 (none), -inf (silence) or a finite value in [-60, 20] dB, or the call fails naming
+// the utterance (per_utterance) and the id.  Returns whether some level asks for something.
+bool check_volume_contour(const float* packed, const size_t* offs, size_t B, bool per_utterance = true);
+// The f32 gain of a level: 1 for NaN, 0 for -inf, else 10^(level / 20) in double.
+float volume_gain_of(float level);
+// The pieces of a signal of n2 delivered samples whose id i ends at ends[i] (non-decreasing, the last at n2) with
+// levels[i] (include/sonata_b200.h, sb200_speak_batch_ids_volume): empty ids dropped, runs of equal levels merged.
+// Empty when every piece has gain 1, which asks for nothing.  Throws OPERATION_ERROR for bad ends.
+std::vector<VolumePiece> volume_pieces(const long long* ends, const float* levels, size_t n_ids, long long n2);
+// The ramp's half length L / 2 = rate / 200 samples (about 5 ms).
+inline int volume_half(int rate) { return rate / 200; }
+// The volume launch's segments.  at[q]: a job's segment is in place at offset at[q] of the stage's input; a chunk
+// pass's is chunk at[q], written at y_off[q] of the pass's own output (total samples).  A job's piece tables are laid
+// out back to back in `pieces` (p_off[q]; -1: the segment's pc is already a stream's resident table).
+struct VolumePlan {
+    std::vector<VolumeSeg> segs;
+    std::vector<long long> at, p_off, y_off;
+    std::vector<VolumePiece> pieces;
+    long long total = 0, max_n = 0;
+    double bytes = 0;
+    void add(long long at_, long long n, long long j0, int half, const std::vector<VolumePiece>& pc,
+             const VolumePiece* pc_d = nullptr);
+};
+
 // The most inputs a formant stream carries between passes: fewer than N, and the 3 H that recompute the frames before
 // its next hop.
 constexpr int FM_CARRY = FM_N + 3 * FM_H;
@@ -318,7 +348,15 @@ void prosody_stream_init_contour(ProsodyStream& ps, int rate, long long n, const
 // phi asks, and phi's own (finite, in [0.5, 2]); a pitch ratio beside a contour, and a stream that asks for nothing at
 // all, are refused.
 void prosody_stream_init_formant(ProsodyStream& ps, int rate, long long n, const long long* ends, const float* ratios,
-                                 size_t n_ids, float pitch, float tempo, float phi);
+                                 size_t n_ids, float pitch, float tempo, float phi, bool allow_none = false);
+// The same with a volume contour levels[0 .. n_ids) (null: none) over the stream's delivered samples, with ends
+// (n_ids ids over n inputs, required with levels) giving each id's delivered end as prosody_contour_plan does: the
+// checks of check_volume_contour, and ratios and a phi that ask for nothing are accepted when the contour asks.
+void prosody_stream_init_volume(ProsodyStream& ps, int rate, long long n, const long long* ends, const float* ratios,
+                                size_t n_ids, float pitch, float tempo, float phi, const float* levels);
+ProsodyStream* create_prosody_stream_volume(Voice* v, int device, int rate, long long n, const long long* ends,
+                                            const float* ratios, size_t n_ids, float pitch, float tempo, float phi,
+                                            const float* levels);
 ProsodyStream* create_prosody_stream_formant(Voice* v, int device, int rate, long long n, const long long* ends,
                                              const float* ratios, size_t n_ids, float pitch, float tempo, float phi);
 // Outputs per chunk of fresh stream ps (no device memory) fed chunk_lens[0 .. n), the last one ending it: what its
@@ -519,6 +557,8 @@ struct Job {
                                       // has a contour (set_job_pitch_contour)
     std::vector<float> formant;       // one formant ratio per utterance, NaN = none; empty when none has one
                                       // (set_job_formants)
+    std::vector<float> volume;        // per-id levels in dB, packed like ids, NaN or 0 = none; empty when no utterance
+                                      // has a volume contour (set_job_volume_contour)
     std::vector<SpeakerBlend> blends; // one canonical blend per utterance (empty entry: the config's speaker); empty when
                                       // none has one (set_job_blends)
     std::vector<ProsodyShape> pros_ran;   // each utterance's shape in the last run (empty: it ran no prosody stage)
@@ -596,6 +636,10 @@ void set_job_pitch_contour(Job& j, const float* packed);
 // loudness; its length, bounds, alignments and place in the job's result do not change.  A bad entry leaves the job's
 // ratios as they were.
 void set_job_formants(Job& j, const float* phi);
+// Per-id volume levels of the job's next run, packed like its ids (NaN or 0: none), or null for none; see
+// check_volume_contour.  A bad entry leaves the job's contour as it was.  Each utterance whose pieces (volume_pieces,
+// over its ids' delivered ends) ask runs the volume stage after the formant stage, before any resampling and loudness.
+void set_job_volume_contour(Job& j, const float* packed);
 // Per-utterance speaker blends of the job's next run (a blend table as for canonical_blends), or null for none.  A blend
 // replaces the utterance's config speaker; its noise and length scales still apply.  Every entry is checked first; a bad
 // entry fails naming the utterance and leaves the job's blends as they were.
@@ -697,7 +741,7 @@ struct ChunkResult {
 void decode_chunks(Voice* v, const ChunkPass& p, ChunkResult& out);
 
 // ---- the waveform output stage (output_stage.cu) ----
-// After the decoder: prosody (stretch, pitch), formants, resampling, then loudness in place on what that leaves.
+// After the decoder: prosody (stretch, pitch), formants, volume, resampling, then loudness in place on what that leaves.
 
 // What a stage reads: segment k is buf[segs[k].out_off ..), segs[k].len * hop samples read through posts[k] (trims,
 // fade, gain; null: read plainly).  The whole-signal prosody and formant launches read buf at their plans' offsets.
@@ -742,6 +786,7 @@ struct MeterPlan {
 struct OutputPlan {
     ProsodyPlan pp;
     FormantPlan fp;
+    VolumePlan vp;
     ResamplePlan rp;
     LoudnessPlan lp;                          // whole signals
     MeterPlan mp;                             // chunk passes
@@ -756,7 +801,8 @@ struct OutputPlan {
 };
 // The output stage of job j's utterances on the frame layout j.frames with `hop` samples per frame, and what the job
 // hands out (osegs, out_hop, out_total, osr).  With a contour (cum: the batch's cum rows on the host) every utterance is
-// planned from its ids' ends, and bounds receives each id's delivered end, packed like the ids.
+// planned from its ids' ends, and bounds receives each id's delivered end, packed like the ids.  A volume contour's
+// pieces are planned over the same ends (cum is then on the host too).
 OutputPlan plan_job_output(Job& j, int hop, const std::vector<int>& cum, std::vector<long long>& bounds);
 // The output stage of chunk pass chunks, chunk k bringing n_in[k] samples after its trims: each chunk's prosody stream,
 // its formant stage, with `resample` the resample launch (a chunk without a resampler is copied), and its meter, which
@@ -774,6 +820,7 @@ struct OutputBufs {
     long long* apos = nullptr;                // and their analysis positions, indexed like the offsets
     int* offsets = nullptr; float *px = nullptr, *ps = nullptr, *py = nullptr;
     Staged<FormantSeg> fsegs; Staged<FormantCarry> fcarry; float *fwin = nullptr, *fy = nullptr;
+    Staged<VolumeSeg> vsegs; Staged<VolumePiece> vpieces; float* vy = nullptr;
     Staged<FrameSeg> rin; Staged<PcmPost> rpost;  // chunk passes: what the resample launch reads after the stages
     Staged<ResampleSeg> rsegs; Staged<PcmPost> rposts; Staged<FrameSeg> rosegs; float* ry = nullptr;
     Staged<LoudSeg> lsegs; double* lscratch = nullptr; Staged<double> lufs; Staged<float> gain;
@@ -787,7 +834,8 @@ struct OutputBufs {
 };
 
 // The launches of plan p from the input wave `in` (in.buf == b.in) on st: profile regions "stretch", "pitch",
-// "formant", "resample" and "loudness", each only when its stage runs.  Returns what the stage delivers: the last
+// "formant", "volume", "resample" and "loudness", each only when its stage runs.  A job's volume stage scales its
+// utterances in place; a chunk pass's writes each chunk to vy (after fy).  Returns what the stage delivers: the last
 // output's wave (a job's: its segments at hop 1 once a stage has changed their lengths).  The loudness results are
 // downloaded to their pinned mirrors.
 Wave run_output_stage(Profile& prof, const OutputPlan& p, const OutputBufs& b, Wave in, cudaStream_t st);

@@ -1,6 +1,6 @@
 // The waveform output stage: what runs after the decoder, in this order: prosody (the stretch and the pitch stage), the
-// formant stage, resampling, and loudness in place on what those leave.  Jobs, chunk passes and the test hooks plan,
-// carve and launch it here only, so they run the same launches.
+// formant stage, the volume stage, resampling, and loudness in place on what those leave.  Jobs, chunk passes and the
+// test hooks plan, carve and launch it here only, so they run the same launches.
 #include "engine.h"
 #include <algorithm>
 #include <cmath>
@@ -87,6 +87,30 @@ OutputPlan plan_job_output(Job& j, int hop, const std::vector<int>& cum, std::ve
         }
         if (fp.segs.empty()) fp = FormantPlan();
     }
+    // volume: each asking utterance in place in the layout the stages before it leave, its pieces over its ids'
+    // delivered ends (the contour's bounds, or those the utterance's ratios give)
+    if (audio && !j.volume.empty()) {
+        std::vector<long long> ends, e2;
+        std::vector<ContourPiece> unused;
+        for (size_t b = 0; b < B; b++) {
+            const size_t n_ids = j.offs[b + 1] - j.offs[b];
+            const float* lv = j.volume.data() + j.offs[b];
+            if (!std::any_of(lv, lv + n_ids, [](float v) { return !std::isnan(v) && v != 0.f; })) continue;
+            const long long n = (long long)fs[b].len * hop, n2 = pp.segs.empty() ? n : pp.segs[b].n2;
+            if (!bounds.empty()) {
+                e2.assign(bounds.begin() + j.offs[b], bounds.begin() + j.offs[b + 1]);
+            } else {
+                ends.resize(n_ids); e2.resize(n_ids);
+                for (size_t i = 0; i < n_ids; i++) ends[i] = (long long)cum[j.xsegs[b].off + i] * hop;
+                prosody_contour_plan(j.v->sample_rate, n, ends.data(), nullptr, n_ids,
+                                     j.pitch.empty() ? NAN : j.pitch[b], j.tempo.empty() ? NAN : j.tempo[b], unused,
+                                     e2.data());
+            }
+            const std::vector<VolumePiece> pc = volume_pieces(e2.data(), lv, n_ids, n2);
+            if (!pc.empty())
+                o.vp.add(pp.segs.empty() ? fs[b].out_off : pp.segs[b].y_off, n2, 0, volume_half(j.v->sample_rate), pc);
+        }
+    }
     // what the job hands out: the frame layout itself, the prosody output (the formant stage keeps its layout), or with
     // output rates one resampled segment per utterance at its rate, back to back
     j.osr.assign(B, j.v->sample_rate);
@@ -148,6 +172,13 @@ OutputPlan plan_chunk_output(const std::vector<ChunkSpec>& chunks, const std::ve
                 o.formed.push_back((int)k);
                 o.n_res[k] = o.fsteps[k].e1 - o.fsteps[k].e0;
             }
+            if (!c.ps->vol.empty()) {
+                // what the stages before it emit, at its delivered positions
+                o.vp.add((long long)k, o.n_res[k], c.ps->fm ? o.fsteps[k].e0 : o.steps[k].j0, volume_half(c.ps->rate),
+                         c.ps->vol, c.ps->vol_d);
+                o.vp.y_off.push_back(o.vp.total);
+                o.vp.total += o.n_res[k];
+            }
         }
         if (resample) o.rp.add(c.rs ? &c.rs->f : nullptr, o.n_res[k], c.rs, c.last != 0);
     }
@@ -183,7 +214,11 @@ void OutputBufs::carve(Arena& dev, Arena& pin, const OutputPlan& p, long long in
             fwin = dev.get<float>((size_t)fp.in_total + 4);
         }
     }
-    if (p.streams() && (!pp.segs.empty() || !fp.segs.empty())) {
+    if (const size_t n = p.vp.segs.size()) {
+        vsegs.carve(dev, pin, n);
+        if (!p.vp.pieces.empty()) vpieces.carve(dev, pin, p.vp.pieces.size());
+    }
+    if (p.streams() && (!pp.segs.empty() || !fp.segs.empty() || !p.vp.segs.empty())) {
         rin.carve(dev, pin, p.chunks.size());
         rpost.carve(dev, pin, p.chunks.size());
     }
@@ -203,9 +238,10 @@ void OutputBufs::carve(Arena& dev, Arena& pin, const OutputPlan& p, long long in
         mlufs.carve(dev, pin, steps); mgains.carve(dev, pin, steps); mclip.carve(dev, pin, m);
     }
     const bool staged = !pp.segs.empty() || !fp.segs.empty() || !p.rp.segs.empty();
-    in = staged || !d_out ? dev.get<float>((size_t)(in_total + pp.y_total + fp.total) + 4) : d_out;
+    in = staged || !d_out ? dev.get<float>((size_t)(in_total + pp.y_total + fp.total + p.vp.total) + 4) : d_out;
     py = in + in_total;
     fy = py + pp.y_total;
+    vy = fy + fp.total;
     if (!p.rp.segs.empty()) ry = d_out ? d_out : dev.get<float>((size_t)p.rp.total + 4);
     else if (d_out && !fp.segs.empty()) fy = d_out;
     else if (d_out && !pp.segs.empty()) py = d_out;
@@ -251,6 +287,34 @@ void OutputBufs::upload(const OutputPlan& p, int hop, const FrameSeg* in_segs, c
     for (size_t k = 0; k < n; k++) at[k] = in + in_segs[k].out_off;
     for (size_t q = 0; q < p.warped.size(); q++) at[p.warped[q]] = py + pp.segs[q].y_off;
     for (size_t q = 0; q < p.formed.size(); q++) at[p.formed[q]] = fy + fp.segs[q].y_off;
+    if (vsegs.d) {
+        // a job's utterances in place in the last stage's output; a chunk read where the stages before it leave it
+        // (without one, through its post-path) and written to vy
+        const VolumePlan& vp = p.vp;
+        float* base = !fp.segs.empty() ? fy : !pp.segs.empty() ? py : in;
+        std::vector<char> staged(n, 0);
+        for (int k : p.warped) staged[k] = 1;
+        for (int k : p.formed) staged[k] = 1;
+        for (size_t q = 0; q < vp.segs.size(); q++) {
+            VolumeSeg g = vp.segs[q];
+            if (p.streams()) {
+                const size_t k = (size_t)vp.at[q];
+                g.chunk = (int)k;
+                g.x = staged[k] ? at[k] : nullptr;
+                g.y = at[k] = vy + vp.y_off[q];
+            } else {
+                g.y = base + vp.at[q];
+                g.x = g.y;
+            }
+            if (vp.p_off[q] >= 0) g.pc = vpieces.d + vp.p_off[q];
+            vsegs.h[q] = g;
+        }
+        vsegs.upload(st);
+        if (vpieces.d) {
+            std::copy(vp.pieces.begin(), vp.pieces.end(), vpieces.h);
+            vpieces.upload(st);
+        }
+    }
     if (rin.d) {
         // a chunk a stage ran on is read from that stage's output: its m samples as a segment of ceil(m / hop) frames
         // less a trim, with no post-path of its own
@@ -341,6 +405,14 @@ Wave run_output_stage(Profile& prof, const OutputPlan& p, const OutputBufs& b, W
         prof.end();
         cur = streams ? restaged : Wave{b.fy, cur.segs, cur.posts, cur.hop};
     }
+    const VolumePlan& vp = p.vp;
+    if (!vp.segs.empty()) {
+        prof.begin("volume");
+        launch_volume(b.vsegs.d, (int)vp.segs.size(), vp.max_n, in.buf, in.segs, in.posts, in.hop, st);
+        prof.count(0, vp.bytes);
+        prof.end();
+        if (streams) cur = restaged;
+    }
     const ResamplePlan& rp = p.rp;
     if (!rp.segs.empty()) {
         prof.begin("resample");
@@ -382,7 +454,7 @@ Wave run_output_stage(Profile& prof, const OutputPlan& p, const OutputBufs& b, W
 
 void advance_streams(const OutputPlan& p, const OutputBufs& b, const Profile& prof) {
     const float stretch_ms = prof.ms("stretch"), pitch_ms = prof.ms("pitch"), formant_ms = prof.ms("formant"),
-                loudness_ms = prof.ms("loudness");
+                volume_ms = prof.ms("volume"), loudness_ms = prof.ms("loudness");
     for (size_t k = 0; k < p.chunks.size(); k++) {
         const ChunkSpec& c = p.chunks[k];
         if (Resampler* r = c.rs) {
@@ -399,6 +471,7 @@ void advance_streams(const OutputPlan& p, const OutputBufs& b, const Profile& pr
             const bool warps = prosody_stream_warps(*w);
             w->last_ms[0] = warps ? stretch_ms : 0.f; w->last_ms[1] = warps ? pitch_ms : 0.f;
             w->last_fm_ms = w->fm ? formant_ms : 0.f;
+            w->last_vol_ms = w->vol.empty() ? 0.f : volume_ms;
         }
     }
     const MeterPlan& mp = p.mp;

@@ -520,7 +520,7 @@ void prosody_stream_init_contour(ProsodyStream& ps, int rate, long long n, const
 }
 
 void prosody_stream_init_formant(ProsodyStream& ps, int rate, long long n, const long long* ends, const float* ratios,
-                                 size_t n_ids, float pitch, float tempo, float phi) {
+                                 size_t n_ids, float pitch, float tempo, float phi, bool allow_none) {
     if (!std::isnan(phi) && !(std::isfinite(phi) && phi >= 0.5f && phi <= 2.f))
         throw Error(19, "formant ratio " + std::to_string(phi) + " is not a finite value in [0.5, 2] (NaN: none)");
     if (ratios) {
@@ -534,21 +534,39 @@ void prosody_stream_init_formant(ProsodyStream& ps, int rate, long long n, const
     // a stream of one ratio runs the stage on every frame or on none, whatever its length; a contour's plan knows n2
     const int c_n = ps.pieces.empty() ? 0 : (int)ps.pieces.size() - 1;
     ps.fm = formant_asks(c_n ? ps.sh.n2 : 1, phi, ps.sh.p, ps.pieces.data(), c_n);
-    if (!ps.fm && !prosody_stream_warps(ps))
+    if (!allow_none && !ps.fm && !prosody_stream_warps(ps))
         throw Error(19, "a prosody stream needs a pitch or tempo ratio, a pitch contour or a formant ratio that asks for "
                         "something (ratios NaN or 1, and a formant ratio NaN or equal to the pitch: none)");
 }
 
+void prosody_stream_init_volume(ProsodyStream& ps, int rate, long long n, const long long* ends, const float* ratios,
+                                size_t n_ids, float pitch, float tempo, float phi, const float* levels) {
+    const size_t offs[2] = {0, n_ids};
+    const bool asks = check_volume_contour(levels, offs, 1, false);
+    prosody_stream_init_formant(ps, rate, n, ends, ratios, n_ids, pitch, tempo, phi, asks);
+    if (!asks) return;
+    // each id's delivered end, as the batch path computes it for the same ratios or contour
+    std::vector<long long> e2(n_ids);
+    std::vector<ContourPiece> unused;
+    const ProsodyShape sh = prosody_contour_plan(rate, n, ends, ratios, n_ids, ratios ? NAN : pitch, tempo, unused,
+                                                 e2.data());
+    ps.vol = volume_pieces(e2.data(), levels, n_ids, sh.n2);
+    if (ps.vol.empty() && !ps.fm && !prosody_stream_warps(ps))
+        throw Error(19, "a prosody stream's ratios, formant ratio and volume contour ask for nothing (the contour's "
+                        "levels apply only to ids without samples)");
+}
+
 namespace {
 // The history buffers (two sets of cap_in + cap_s floats and two ints), the formant stage's two carry buffers when it
-// runs and, after them, the piece table.
+// runs and, after them, the pitch contour's piece table and the volume contour's.
 ProsodyStream* allocate_prosody_stream(std::unique_ptr<ProsodyStream> ps, Voice* v, int device) {
     ps->v = v; ps->device = device;
     SB_CUDA(cudaSetDevice(device));
     const size_t side = (size_t)ps->cap_in + ps->cap_s + 2;      // floats, floats, two ints
     const size_t fm = ps->fm ? (size_t)FM_CARRY : 0;
     const size_t table = (2 * (side + fm) * 4 + 15) / 16 * 16;
-    const size_t bytes = table + ps->pieces.size() * sizeof(ContourPiece);
+    const size_t vol_at = (table + ps->pieces.size() * sizeof(ContourPiece) + 15) / 16 * 16;
+    const size_t bytes = vol_at + ps->vol.size() * sizeof(VolumePiece);
     void* mem = nullptr;
     SB_CUDA(cudaMalloc(&mem, bytes));
     ps->mem = mem;
@@ -563,6 +581,11 @@ ProsodyStream* allocate_prosody_stream(std::unique_ptr<ProsodyStream> ps, Voice*
         ContourPiece* d = reinterpret_cast<ContourPiece*>(static_cast<char*>(mem) + table);
         SB_CUDA(cudaMemcpy(d, ps->pieces.data(), ps->pieces.size() * sizeof(ContourPiece), cudaMemcpyHostToDevice));
         ps->pieces_d = d;
+    }
+    if (!ps->vol.empty()) {
+        VolumePiece* d = reinterpret_cast<VolumePiece*>(static_cast<char*>(mem) + vol_at);
+        SB_CUDA(cudaMemcpy(d, ps->vol.data(), ps->vol.size() * sizeof(VolumePiece), cudaMemcpyHostToDevice));
+        ps->vol_d = d;
     }
     return ps.release();
 }
@@ -585,6 +608,14 @@ ProsodyStream* create_prosody_stream_formant(Voice* v, int device, int rate, lon
                                              const float* ratios, size_t n_ids, float pitch, float tempo, float phi) {
     std::unique_ptr<ProsodyStream> ps(new ProsodyStream());
     prosody_stream_init_formant(*ps, rate, n, ends, ratios, n_ids, pitch, tempo, phi);
+    return allocate_prosody_stream(std::move(ps), v, device);
+}
+
+ProsodyStream* create_prosody_stream_volume(Voice* v, int device, int rate, long long n, const long long* ends,
+                                            const float* ratios, size_t n_ids, float pitch, float tempo, float phi,
+                                            const float* levels) {
+    std::unique_ptr<ProsodyStream> ps(new ProsodyStream());
+    prosody_stream_init_volume(*ps, rate, n, ends, ratios, n_ids, pitch, tempo, phi, levels);
     return allocate_prosody_stream(std::move(ps), v, device);
 }
 

@@ -12,7 +12,7 @@ from . import _native as N
 from .core import G711_LAW, Audio, OperationError, check_encoding
 from .piper import (_batch_options, _blend_arrays, _check, _config_array, _contour_arrays, _duration_arrays,
                     _formant_array, _gain_array, _loudness_array, _pack_ids, _prosody_arrays, _ptr, _rate_array,
-                    _seed_arrays, _take_audio, _take_bytes)
+                    _seed_arrays, _take_audio, _take_bytes, _volume_arrays)
 
 
 class SynthesisJob:
@@ -21,16 +21,19 @@ class SynthesisJob:
                  seeds: Optional[Sequence] = None, output_rates: Optional[Sequence] = None,
                  loudness: Optional[Sequence] = None, pitches: Optional[Sequence] = None,
                  tempos: Optional[Sequence] = None, pitch_contours: Optional[Sequence] = None,
-                 formants: Optional[Sequence] = None, speaker_blends: Optional[Sequence] = None):
+                 formants: Optional[Sequence] = None, speaker_blends: Optional[Sequence] = None,
+                 volume_contours: Optional[Sequence] = None):
         """`configs`: one PiperSynthesisConfig per utterance (see set_configs); None keeps the voice's fallback config.
         `seeds`: noise seeds (see set_seeds).  `output_rates`: output sample rates (see set_output_rates).
         `loudness`: loudness targets (see set_loudness).  `pitches` / `tempos`: pitch and tempo ratios (see
         set_prosody).  `pitch_contours`: per-id pitch ratios (see set_pitch_contours).  `formants`: formant ratios (see
-        set_formants).  `speaker_blends`: speaker blends (see set_speaker_blends)."""
+        set_formants).  `speaker_blends`: speaker blends (see set_speaker_blends).  `volume_contours`: per-id volume
+        levels (see set_volume_contours)."""
         # argument errors before the job exists
         options = _batch_options(model, len(batches), [len(b) for b in batches], configs, seeds=seeds,
                                  output_rates=output_rates, loudness=loudness, pitches=pitches, tempos=tempos,
-                                 pitch_contours=pitch_contours, formants=formants, speaker_blends=speaker_blends)
+                                 pitch_contours=pitch_contours, formants=formants, speaker_blends=speaker_blends,
+                                 volume_contours=volume_contours)
         self._open(model, batches, options, eps_w, eps_z, debug)
 
     @classmethod
@@ -96,6 +99,8 @@ class SynthesisJob:
         if o.blend_offsets is not None:
             self._set(lib.sb200_job_set_speaker_blends, _ptr(o.blend_speakers, C.c_int64),
                       _ptr(o.blend_weights, C.c_float), _ptr(o.blend_offsets, C.c_size_t))
+        if o.volume is not None:
+            self._set(lib.sb200_job_set_volume_contour, _ptr(o.volume, C.c_float))
 
     def _set(self, fn, *images) -> None:
         """One sb200_job_set_* call with its C images."""
@@ -178,6 +183,13 @@ class SynthesisJob:
         ratio of 1.0 asks for something on an utterance with a pitch ratio or contour: its own formants.  A bad entry
         raises OperationError naming the utterance and leaves the job's ratios as they were."""
         self._set(self._lib.sb200_job_set_formants, _ptr(_formant_array(formants, self.batch), C.c_float))
+
+    def set_volume_contours(self, contours: Optional[Sequence]) -> None:
+        """Per-id volume levels in dB for the next run (see VitsModel.infer_batch_with_values): contours[b] holds one
+        level per id of utterance b, or is None; None for the whole list, or levels that are all None / NaN / 0, turn
+        contours off.  The results keep their lengths and layout, and profile() reports the stage as "volume".  A bad
+        entry raises OperationError naming the utterance and the id, and leaves the job's contours as they were."""
+        self._set(self._lib.sb200_job_set_volume_contour, _ptr(_volume_arrays(self._lens, contours), C.c_float))
 
     def set_speaker_blends(self, blends: Optional[Sequence]) -> None:
         """Per-utterance speaker blends for the next run (see VitsModel.infer_batch_with_values): a mapping

@@ -375,15 +375,60 @@ def _contour_arrays(lens: Sequence[int], pitch_contours=None, pitches=None, who:
     return None if (np.isnan(out) | (out == 1)).all() else out
 
 
-def _char_values_to_ids(v, phonemes: str, src: Sequence[int], b, what: str, check) -> list:
+def _char_values_to_ids(v, phonemes: str, src: Sequence[int], b, what: str, check, none: float = 1.0) -> list:
     """Per-character values v (one per character of `phonemes`) as per-id values: each id takes its source character's
-    value, checked by check(x, b, character, "character"); bos, eos and pads of no character take 1.0.  Characters the
-    voice drops have no id and their values are ignored.  b: the utterance's index, or a label naming the stream."""
+    value, checked by check(x, b, character, "character"); bos, eos and pads of no character take `none`.  Characters
+    the voice drops have no id and their values are ignored.  b: the utterance's index, or a label naming the stream."""
     v = list(v) if not isinstance(v, np.ndarray) else v.reshape(-1).tolist()
     if len(v) != len(phonemes):
         raise OperationError(f"{_who(b)}: {len(v)} {what} for {len(phonemes)} characters")
     kept = {c: check(v[c], b, c, "character") for c in sorted(set(src)) if c >= 0}
-    return [1.0 if c < 0 else kept[c] for c in src]
+    return [none if c < 0 else kept[c] for c in src]
+
+
+VOLUME_RANGE = (-60.0, 20.0)   # volume levels (dB) an id can be given, besides -inf (silence)
+
+
+def _volume_value(x, b, i: int, unit: str = "id") -> float:
+    if x is None:
+        return math.nan
+    if isinstance(x, bool) or not isinstance(x, numbers.Real):
+        raise OperationError(f"{_who(b)}, {unit} {i}: volume level {x!r} is not a number")
+    x = float(x)
+    if not (math.isnan(x) or x == 0.0 or x == -math.inf or
+            (math.isfinite(x) and VOLUME_RANGE[0] <= x <= VOLUME_RANGE[1])):
+        raise OperationError(f"{_who(b)}, {unit} {i}: volume level {x} dB is not a finite value in "
+                             f"[{VOLUME_RANGE[0]}, {VOLUME_RANGE[1]}] or -inf (None, NaN or 0: none)")
+    return x
+
+
+def _volume_arrays(lens: Sequence[int], volume_contours=None, who: Optional[Sequence[str]] = None):
+    """The packed C image of per-id volume levels in dB (f32, NaN for none), checked as the library checks them, or None
+    when not given or when every level is None / NaN / 0.  volume_contours[b] holds one level per id of utterance b (in
+    VOLUME_RANGE, -inf for silence, or None / NaN / 0 for none), or is None.  `who`: as for _contour_arrays."""
+    if volume_contours is None:
+        return None
+    n = len(lens)
+    out = np.full(int(sum(lens)), np.nan, np.float32)
+    pos = 0
+    for b, v in enumerate(_per_utterance(volume_contours, n, "volume contours")):
+        if v is not None:
+            label = b if who is None else who[b]
+            a = _numeric(v, "fiu")
+            if a is None:
+                v = list(v)
+                a = np.array([_volume_value(x, label, i) for i, x in enumerate(v)] if len(v) == lens[b] else v)
+            if a.size != lens[b]:
+                raise OperationError(f"{_who(label)}: {a.size} volume levels for {lens[b]} ids")
+            f = a.astype(np.float32).reshape(-1)
+            asked = ~np.isnan(f) & (f != 0)
+            ok = (f == -np.inf) | (np.isfinite(f) & (f >= VOLUME_RANGE[0]) & (f <= VOLUME_RANGE[1]))
+            bad = np.nonzero(asked & ~ok)[0]
+            if bad.size:
+                _volume_value(float(f[bad[0]]), label, int(bad[0]))
+            out[pos:pos + lens[b]] = f
+        pos += lens[b]
+    return None if (np.isnan(out) | (out == 0)).all() else out
 
 
 def refuse_prosody(pitch, tempo, where: str) -> None:
@@ -393,6 +438,13 @@ def refuse_prosody(pitch, tempo, where: str) -> None:
         raise OperationError(f"{where} cannot shift pitch or tempo: the time stretch walks a whole sentence frame by "
                              "frame, and this mode hands out a sentence's first chunk before its last one is decoded "
                              "(use the lazy, parallel or file modes, speak_batch or a SynthesisJob)")
+
+
+def refuse_volume(volume_contour, where: str) -> None:
+    """OperationError when `where`, a mode without this library's streaming voices, is asked for a volume contour."""
+    if volume_contour is not None:
+        raise OperationError(f"{where} cannot apply a volume contour: only this library's streaming voices carry a "
+                             "contour from chunk to chunk (use speak_batch or a SynthesisJob)")
 
 
 def refuse_contour(pitch_contour, where: str) -> None:
@@ -429,9 +481,9 @@ def _gain_array(gains, n: int):
 @dataclass
 class _BatchOptions:
     """A batch's options, checked once by _batch_options, as the C images the library takes: each None when not given
-    or when no utterance asks for it.  A phoneme surface's per-character controls (char_scales, char_contours: one
-    entry or None per utterance) become the per-id images `scales` and `contour` once its phonemes are mapped
-    (map_characters)."""
+    or when no utterance asks for it.  A phoneme surface's per-character controls (char_scales, char_contours,
+    char_volumes: one entry or None per utterance) become the per-id images `scales`, `contour` and `volume` once its
+    phonemes are mapped (map_characters)."""
     n: int
     cfgs: object = None                       # sb200_synth_config [n]
     scales: Optional[np.ndarray] = None       # per id, packed
@@ -449,28 +501,31 @@ class _BatchOptions:
     blend_speakers: Optional[np.ndarray] = None
     blend_weights: Optional[np.ndarray] = None
     blend_offsets: Optional[np.ndarray] = None
+    volume: Optional[np.ndarray] = None       # per id, packed
     char_scales: Optional[list] = None
     char_contours: Optional[list] = None
+    char_volumes: Optional[list] = None
 
     def map_characters(self, phonemes: Sequence[str], maps) -> None:
         """Makes the per-id images of the per-character controls once the phonemes are mapped: maps[b] is (ids, source
         character of each id) of phonemes[b], as phonemes_to_input_ids_map gives it."""
-        def per_id(values, what, check):
+        def per_id(values, what, check, none=1.0):
             return None if values is None else [
-                None if v is None else _char_values_to_ids(v, ph, src, b, what, check)
+                None if v is None else _char_values_to_ids(v, ph, src, b, what, check, none)
                 for b, (v, ph, (_, src)) in enumerate(zip(values, phonemes, maps))]
         lens = [len(ids) for ids, _ in maps]
         self.scales, _ = _duration_arrays(lens, per_id(self.char_scales, "duration scales", _scale_value))
         self.contour = _contour_arrays(lens, per_id(self.char_contours, "pitch ratios", _contour_value), self.pitch)
+        self.volume = _volume_arrays(lens, per_id(self.char_volumes, "volume levels", _volume_value, 0.0))
 
 
 def _batch_options(model, n: int, lens: Optional[Sequence[int]] = None, configs=None, duration_scales=None,
                    durations=None, seeds=None, output_rates=None, loudness=None, law=None, gains=None, pitches=None,
-                   tempos=None, pitch_contours=None, formants=None, speaker_blends=None,
+                   tempos=None, pitch_contours=None, formants=None, speaker_blends=None, volume_contours=None,
                    g711: bool = False) -> _BatchOptions:
     """The options of a batch of n utterances, each checked as its C image is made, in one order at every surface:
     configs, duration scales, durations, seeds, output rates, loudness, law (with `g711`), gains, pitch and tempo, pitch
-    contours, formants, speaker blends.  `lens`: the utterances' id counts, for per-id controls; None for a phoneme
+    contours, formants, speaker blends, volume contours.  `lens`: the utterances' id counts, for per-id controls; None for a phoneme
     surface, whose per-character controls are only counted here, before any phoneme is mapped (see map_characters)."""
     o = _BatchOptions(n, _config_array(configs, n))
     if lens is None:
@@ -490,6 +545,10 @@ def _batch_options(model, n: int, lens: Optional[Sequence[int]] = None, configs=
         o.contour = _contour_arrays(lens, pitch_contours, o.pitch)
     o.formants = _formant_array(formants, n)
     o.blend_speakers, o.blend_weights, o.blend_offsets = _blend_arrays(model, speaker_blends, n)
+    if lens is None:
+        o.char_volumes = None if volume_contours is None else _per_utterance(volume_contours, n, "volume contours")
+    else:
+        o.volume = _volume_arrays(lens, volume_contours)
     return o
 
 
@@ -724,20 +783,21 @@ class _VitsCommons:
                     output_rates: Optional[Sequence] = None, loudness: Optional[Sequence] = None,
                     pitches: Optional[Sequence] = None, tempos: Optional[Sequence] = None,
                     pitch_contours: Optional[Sequence] = None, formants: Optional[Sequence] = None,
-                    speaker_blends: Optional[Sequence] = None) -> List[Audio]:
+                    speaker_blends: Optional[Sequence] = None,
+                    volume_contours: Optional[Sequence] = None) -> List[Audio]:
         """`configs`: one PiperSynthesisConfig per utterance (speaker and scales), still synthesised as one pass;
         None uses the fallback config for every utterance.  `seeds`: noise seeds as for infer_batch_with_values.
         `speaker_blends`: as for infer_batch_with_values.
         `output_rates` / `loudness` / `pitches` / `tempos` / `formants`: per-utterance output sample rates, loudness
-        targets, pitch and tempo ratios and formant ratios as for infer_batch_with_values.  `pitch_contours`: as for
-        speak_batch_with_alignment, one ratio per phoneme character."""
+        targets, pitch and tempo ratios and formant ratios as for infer_batch_with_values.  `pitch_contours` /
+        `volume_contours`: as for speak_batch_with_alignment, one ratio or level per phoneme character."""
         n = len(phoneme_batches)
         o = _batch_options(self, n, None, configs, seeds=seeds, output_rates=output_rates, loudness=loudness,
                            pitches=pitches, tempos=tempos, pitch_contours=pitch_contours, formants=formants,
-                           speaker_blends=speaker_blends)
+                           speaker_blends=speaker_blends, volume_contours=volume_contours)
         if n == 0:
             return []
-        if pitch_contours is not None:
+        if pitch_contours is not None or volume_contours is not None:
             maps = [self.phonemes_to_input_ids_map(p) for p in phoneme_batches]
             o.map_characters(phoneme_batches, maps)
             return [a for a, _, _ in self._speak_ids([ids for ids, _ in maps], o)]
@@ -766,7 +826,8 @@ class _VitsCommons:
                                 tempos: Optional[Sequence] = None,
                                 pitch_contours: Optional[Sequence] = None,
                                 formants: Optional[Sequence] = None,
-                                speaker_blends: Optional[Sequence] = None) -> List[Audio]:
+                                speaker_blends: Optional[Sequence] = None,
+                                volume_contours: Optional[Sequence] = None) -> List[Audio]:
         """Batched infer_with_values.  `configs`: one PiperSynthesisConfig per utterance (speaker and scales), or None
         for the fallback config; each utterance's result equals a single-utterance call with its config as the
         fallback, except for the on-device noise of an unseeded utterance, whose draws depend on the batch position.
@@ -808,10 +869,17 @@ class _VitsCommons:
         The utterance speaks with the weighted mean of those speakers' embeddings, which replaces its config's speaker
         (the config's scales still apply; include/sonata_b200.h, sb200_speak_batch_ids_blends).  A blend of one speaker
         (any positive weight) gives that speaker's bits, and blends equal up to order, zero weights or a common
-        power-of-two scale give the same bits."""
+        power-of-two scale give the same bits.
+
+        `volume_contours`: one volume level in dB per id for each utterance (in VOLUME_RANGE, -inf to mute, or None /
+        NaN / 0 for none), or None: SSML's <prosody volume> on a span.  Each id's delivered samples are scaled by its
+        level, with a 10 ms smoothstep between levels, on the device after the formant stage and before any resampling
+        and loudness (sb200_speak_batch_ids_volume); a loudness target then normalises the utterance as a whole, so the
+        relative levels survive.  Lengths and alignments do not change, and there is no clamp."""
         o = _batch_options(self, len(batches), [len(b) for b in batches], configs, seeds=seeds,
                            output_rates=output_rates, loudness=loudness, pitches=pitches, tempos=tempos,
-                           pitch_contours=pitch_contours, formants=formants, speaker_blends=speaker_blends)
+                           pitch_contours=pitch_contours, formants=formants, speaker_blends=speaker_blends,
+                           volume_contours=volume_contours)
         return [a for a, _, _ in self._speak_ids(batches, o)]
 
     def infer_batch_with_durations(self, batches: Sequence[Sequence[int]],
@@ -824,7 +892,8 @@ class _VitsCommons:
                                    tempos: Optional[Sequence] = None,
                                    pitch_contours: Optional[Sequence] = None,
                                    formants: Optional[Sequence] = None,
-                                   speaker_blends: Optional[Sequence] = None) -> List[Tuple[Audio, np.ndarray]]:
+                                   speaker_blends: Optional[Sequence] = None,
+                                   volume_contours: Optional[Sequence] = None) -> List[Tuple[Audio, np.ndarray]]:
         """infer_batch_with_values with per-id duration control, returning (audio, frames per id) per utterance.
 
         duration_scales[b]: one scale (finite, >= 0) per id of utterance b, applied before the duration's ceil, so 1.0
@@ -832,15 +901,16 @@ class _VitsCommons:
         Either list, or any of its entries, may be None.  The frame counts times 256 are each id's samples; an
         utterance whose ids all got 0 frames is still one frame long.  `seeds`: as for infer_batch_with_values; a
         seeded frame's noise depends on its index only, so controls that move frames never reshuffle it.
-        `output_rates` / `loudness` / `pitches` / `tempos` / `pitch_contours` / `formants` / `speaker_blends`: as for
-        infer_batch_with_values (the frame counts stay frame counts of the utterance before any warp)."""
+        `output_rates` / `loudness` / `pitches` / `tempos` / `pitch_contours` / `formants` / `speaker_blends` /
+        `volume_contours`: as for infer_batch_with_values (the frame counts stay frame counts of the utterance before
+        any warp)."""
         o = _batch_options(self, len(batches), [len(b) for b in batches], configs, duration_scales, durations, seeds,
                            output_rates, loudness, pitches=pitches, tempos=tempos, pitch_contours=pitch_contours,
-                           formants=formants, speaker_blends=speaker_blends)
+                           formants=formants, speaker_blends=speaker_blends, volume_contours=volume_contours)
         return [(a, f) for a, f, _ in self._speak_ids(batches, o, frames=True)]
 
     def _speak_ids(self, batches, o: _BatchOptions, frames: bool = False) -> List[tuple]:
-        """The f32 batch route: `batches` with options `o` in one sb200_speak_batch_ids_blends call.  Per utterance
+        """The f32 batch route: `batches` with options `o` in one sb200_speak_batch_ids_volume call.  Per utterance
         (audio, frames per id, each id's delivered end): the frames only when asked for, since fetching them costs a
         device->host copy and a synchronise, and the ends only when o has a pitch contour (None otherwise)."""
         n = len(batches)
@@ -852,12 +922,12 @@ class _VitsCommons:
         id_frames = np.zeros(int(offs[-1]), np.int32) if frames else None
         bounds = None if o.contour is None else np.zeros(int(offs[-1]), np.int64)
         err = N.sb200_error()
-        _check(self._lib.sb200_speak_batch_ids_blends(
+        _check(self._lib.sb200_speak_batch_ids_volume(
             self._h, _ptr(packed, C.c_int64), _ptr(offs, C.c_size_t), n, o.cfgs, _ptr(o.scales, C.c_float),
             _ptr(o.frames, C.c_int32), _ptr(o.seeds, C.c_uint64), _ptr(o.seeded, C.c_int32), _ptr(o.rates, C.c_uint32),
             _ptr(o.loudness, C.c_float), _ptr(o.pitch, C.c_float), _ptr(o.tempo, C.c_float), _ptr(o.contour, C.c_float),
             _ptr(o.formants, C.c_float), _ptr(o.blend_speakers, C.c_int64), _ptr(o.blend_weights, C.c_float),
-            _ptr(o.blend_offsets, C.c_size_t), outs, _ptr(id_frames, C.c_int32), _ptr(bounds, C.c_int64), None, None,
+            _ptr(o.blend_offsets, C.c_size_t), _ptr(o.volume, C.c_float), outs, _ptr(id_frames, C.c_int32), _ptr(bounds, C.c_int64), None, None,
             C.byref(err)), err)
         cut = lambda a, b: None if a is None else a[int(offs[b]):int(offs[b + 1])].copy()
         return [(_take_audio(outs[b]), cut(id_frames, b), cut(bounds, b)) for b in range(n)]
@@ -870,7 +940,8 @@ class _VitsCommons:
                                    loudness: Optional[Sequence] = None, pitches: Optional[Sequence] = None,
                                    tempos: Optional[Sequence] = None, pitch_contours: Optional[Sequence] = None,
                                    formants: Optional[Sequence] = None,
-                                   speaker_blends: Optional[Sequence] = None) -> List[Tuple[Audio, List[PhonemeAlignment]]]:
+                                   speaker_blends: Optional[Sequence] = None,
+                                   volume_contours: Optional[Sequence] = None) -> List[Tuple[Audio, List[PhonemeAlignment]]]:
         """speak_batch that also says when each phoneme is spoken: per utterance (audio, alignment), the alignment
         holding one entry for bos (`^`), one per kept phoneme character (its id and its trailing pad) and one for eos
         (`$`), contiguous from sample 0 to len(audio).
@@ -889,11 +960,13 @@ class _VitsCommons:
         infer_batch_with_values.  An utterance with a contour is aligned from each id's delivered end
         (sb200_speak_batch_ids_contour), exact rather than scaled: with no tempo a boundary stays where it was.
         `formants`: as for infer_batch_with_values; it moves no boundary.  `speaker_blends`: as for
-        infer_batch_with_values."""
+        infer_batch_with_values.  volume_contours[b] (or None): one volume level per character of phoneme_batches[b]
+        (see infer_batch_with_values), applied to that character's id and pad, bos and eos keeping their level; it
+        moves no boundary."""
         n = len(phoneme_batches)
         o = _batch_options(self, n, None, configs, duration_scales, seeds=seeds, output_rates=output_rates,
                            loudness=loudness, pitches=pitches, tempos=tempos, pitch_contours=pitch_contours,
-                           formants=formants, speaker_blends=speaker_blends)
+                           formants=formants, speaker_blends=speaker_blends, volume_contours=volume_contours)
         maps = [self.phonemes_to_input_ids_map(p) for p in phoneme_batches]
         o.map_characters(phoneme_batches, maps)
         res = self._speak_ids([ids for ids, _ in maps], o, frames=True)
@@ -1118,12 +1191,21 @@ class ProsodyStream:
     `formant`: a formant ratio as for infer_batch_with_values' formants (None / NaN: none), applied on top of the
     ratios or contour, or alone when they ask for nothing (sb200_prosody_stream_create_formant): the concatenation of
     what the stream emits is the formant stage of the sentence it warps, applied at once.  Its stage holds back 768 -
-    1023 samples more than the warp alone."""
+    1023 samples more than the warp alone.
+
+    `volume`: one volume level in dB per id of `enc` (values as for infer_batch_with_values' volume_contours), applied
+    on top of the rest, or alone when it asks for nothing (sb200_prosody_stream_create_volume): each sample the stream
+    emits is scaled at its delivered position, holding nothing back."""
 
     def __init__(self, model: "_VitsCommons", pitch=None, tempo=None, pitch_contour=None,
-                 enc: Optional["EncoderOutputs"] = None, formant=None):
+                 enc: Optional["EncoderOutputs"] = None, formant=None, volume=None):
         p, t = _prosody_arrays([pitch], [tempo], 1)
         phi = _stream_formant(formant, "stream")
+        vol = None                      # the volume contour's per-id image
+        if volume is not None:
+            if not isinstance(enc, EncoderOutputs) or enc._m is not model or not enc._h:
+                raise OperationError("a volume contour needs the EncoderOutputs of its sentence, from this model")
+            vol = _volume_arrays([len(enc.p_duration)], [volume], ["stream"])
         self._m, self._h = model, C.c_void_p()
         self.pitch = None if p is None else float(p[0])
         self.tempo = None if t is None else float(t[0])
@@ -1141,7 +1223,12 @@ class ProsodyStream:
         nan = float("nan")
         pv, tv = nan if p is None else float(p[0]), nan if t is None else float(t[0])
         err = N.sb200_error()
-        if phi is not None:
+        if vol is not None:
+            # any of the above with the volume contour on top, or the contour alone
+            _check(model._lib.sb200_prosody_stream_create_volume(
+                model._h, enc._h, pv, _ptr(c, C.c_float), vol.size, tv, nan if phi is None else phi,
+                _ptr(vol, C.c_float), C.byref(self._h), C.byref(err)), err)
+        elif phi is not None:
             # the ratio or contour stream with phi on top, or phi alone
             _check(model._lib.sb200_prosody_stream_create_formant(
                 model._h, None if c is None else enc._h, pv, _ptr(c, C.c_float), 0 if c is None else c.size, tv, phi,
@@ -1170,6 +1257,12 @@ class ProsodyStream:
         self._m._lib.sb200_prosody_stream_profile_formant(self._h, C.byref(f))
         return float(f.value)
 
+    def last_volume_ms(self) -> float:
+        """The "volume" device time (ms) of the last chunk pass this stream was in (0: its stage did not run)."""
+        f = C.c_float()
+        self._m._lib.sb200_prosody_stream_profile_volume(self._h, C.byref(f))
+        return float(f.value)
+
     def __del__(self):
         try:
             if self._h:
@@ -1179,14 +1272,21 @@ class ProsodyStream:
             pass
 
 
-def _stream_prosody(model, pitch, tempo, pitch_contour=None, enc=None, formant=None) -> Optional[ProsodyStream]:
+def _stream_prosody(model, pitch, tempo, pitch_contour=None, enc=None, formant=None,
+                    volume=None) -> Optional[ProsodyStream]:
     """A ProsodyStream for a stream with these ratios, or with this per-id contour of enc's sentence and the tempo, and
     the formant ratio, or None when nothing asks for anything.  A given contour makes a contoured stream (which has
     bounds) whenever the contour or the tempo asks for something; a contour of None / NaN / 1 only is no contour beside a
     pitch ratio, as in the batch calls, and with neither a pitch nor a tempo it leaves the plain stream, which has no
     bounds.  A formant ratio asks for something unless it equals the pitch ratio (1 without one): it then makes a
-    formant-only stream of a plain one."""
+    formant-only stream of a plain one.  A volume contour that asks for something (see _volume_arrays) is carried on
+    top of the rest, or alone."""
     p, t = _prosody_arrays([pitch], [tempo], 1)
+    if volume is not None and _volume_arrays([len(enc.p_duration)], [volume], ["stream"]) is not None:
+        if pitch_contour is not None and _contour_arrays([len(enc.p_duration)], [pitch_contour], p, ["stream"]) is None \
+                and (p is not None or t is None):
+            pitch_contour = None
+        return ProsodyStream(model, pitch, tempo, pitch_contour, enc, formant, volume)
     phi = _stream_formant(formant, "stream")
     if pitch_contour is not None:
         asks = _contour_arrays([len(enc.p_duration)], [pitch_contour], p, ["stream"]) is not None
@@ -1526,7 +1626,8 @@ class VitsStreamingModel(_VitsCommons):
                          pitch: Optional[float] = None, tempo: Optional[float] = None,
                          pitch_contour: Optional[Sequence] = None,
                          formant_ratio: Optional[float] = None, speaker_blend=None,
-                         live_loudness=None, max_gain_db: Optional[float] = None) -> SpeechStreamer:
+                         live_loudness=None, max_gain_db: Optional[float] = None,
+                         volume_contour: Optional[Sequence] = None) -> SpeechStreamer:
         """`formant_ratio`: as for infer_batch_with_values' formants, on top of `pitch` / `tempo` / `pitch_contour` or
         alone, the sentence's formant stage carried as one stream on the device (ProsodyStream): the concatenation of
         the chunks is the formant stage applied at once to the sentence the stream yields without it, then resampled and
@@ -1547,8 +1648,13 @@ class VitsStreamingModel(_VitsCommons):
         `live_loudness`: a target in LUFS, for a fresh live loudness meter (LoudnessStream, capped at `max_gain_db`,
         default 20), or a LoudnessStream to continue (a request's meter across its sentences).  What the stream
         delivers is metered and scaled on the device as it leaves, holding nothing back; `gain` applies after the
-        meter, and G.711 is taken at the fixed scale."""
+        meter, and G.711 is taken at the fixed scale.
+        `volume_contour`: one volume level per character of `phonemes` (as for speak_batch_with_alignment's
+        volume_contours), applied to that character's id and pad, on top of the rest or alone (ProsodyStream): the
+        concatenation of the chunks is the sentence the stream yields without it with that contour applied at once,
+        before resampling, metering and encoding.  It holds nothing back."""
         if not isinstance(self, VitsStreamingModel):
+            refuse_volume(volume_contour, "stream_synthesis")
             refuse_live_loudness(live_loudness, "stream_synthesis")
             refuse_formants(formant_ratio, "stream_synthesis")
             refuse_prosody(pitch, tempo, "stream_synthesis")
@@ -1556,7 +1662,7 @@ class VitsStreamingModel(_VitsCommons):
         o = _stream_options(self, "stream_synthesis", None, phonemes, seed=seed, output_rate=output_rate,
                             encoding=encoding, gain=gain, pitch=pitch, tempo=tempo, pitch_contour=pitch_contour,
                             formant_ratio=formant_ratio, speaker_blend=speaker_blend, live_loudness=live_loudness,
-                            max_gain_db=max_gain_db)
+                            max_gain_db=max_gain_db, volume_contour=volume_contour)
         if o.seed is None and o.blend is None:
             enc = self.infer_encoder(o.ids)
         else:
@@ -1601,15 +1707,16 @@ class _StreamOptions:
     blend: Optional[dict]
     live_loudness: object               # None, a target in LUFS or a LoudnessStream to continue
     max_gain_db: Optional[float]
+    volume: Optional[Sequence] = None   # per id
 
 
 def _stream_options(model, where: str, key: Optional[int], ids_or_phonemes, config=None, chunk_size=None,
                     chunk_padding=None, seed=None, output_rate=None, encoding=None, gain=None, pitch=None, tempo=None,
                     pitch_contour=None, formant_ratio=None, speaker_blend=None, live_loudness=None, max_gain_db=None,
-                    carried=()) -> _StreamOptions:
+                    carried=(), volume_contour=None) -> _StreamOptions:
     """The options of one stream of `model`, checked in one order: config, live loudness, speaker blend, formant ratio,
     pitch and tempo, seed, output rate, FLAC (refused by the name `where`), encoding and gain, the config's speaker,
-    chunking, then the ids (phonemes are mapped) and the contour.  Errors name "stream" (key None) or "stream {key}".
+    chunking, then the ids (phonemes are mapped), the contour and the volume contour.  Errors name "stream" (key None) or "stream {key}".
     `chunk_size`: checked with `chunk_padding` when given.  `carried`: the LoudnessStreams the caller's unfinished
     streams carry, which live_loudness may not be."""
     if config is not None and not isinstance(config, PiperSynthesisConfig):
@@ -1631,26 +1738,32 @@ def _stream_options(model, where: str, key: Optional[int], ids_or_phonemes, conf
         raise OperationError(f"No speaker was found with the given id `{config.speaker}`")     # as check_config
     if chunk_size is not None:
         _check_chunking(chunk_size, chunk_padding)
-    contour = pitch_contour
-    if isinstance(ids_or_phonemes, str) and pitch_contour is not None:
+    contour, volume = pitch_contour, volume_contour
+    if isinstance(ids_or_phonemes, str) and (pitch_contour is not None or volume_contour is not None):
         ids, src = model.phonemes_to_input_ids_map(ids_or_phonemes)
-        contour = _char_values_to_ids(pitch_contour, ids_or_phonemes, src, who, "pitch ratios", _contour_value)
+        if pitch_contour is not None:
+            contour = _char_values_to_ids(pitch_contour, ids_or_phonemes, src, who, "pitch ratios", _contour_value)
+        if volume_contour is not None:
+            volume = _char_values_to_ids(volume_contour, ids_or_phonemes, src, who, "volume levels", _volume_value,
+                                         0.0)
     elif isinstance(ids_or_phonemes, str):
         ids = model.phonemes_to_input_ids(ids_or_phonemes)
     else:
         ids = [int(i) for i in ids_or_phonemes]
     if contour is not None:
         _contour_arrays([len(ids)], [contour], pit, [who])
+    if volume is not None:
+        _volume_arrays([len(ids)], [volume], [who])
     if not ids:
         raise OperationError("Failed to run model inference. Error: empty input sequence")
     return _StreamOptions(key, who, ids, config, chunk_size, seed, output_rate, encoding, g, pitch, tempo, contour, phi,
-                          speaker_blend, live_loudness, max_gain_db)
+                          speaker_blend, live_loudness, max_gain_db, volume)
 
 
 def _open_stream(model, o: _StreamOptions, enc):
     """(resampler, ProsodyStream, meter) of a stream with options `o` and latent `enc`, each None when not asked for."""
     return (_stream_resampler(model, o.output_rate),
-            _stream_prosody(model, o.pitch, o.tempo, o.contour, enc, o.formant),
+            _stream_prosody(model, o.pitch, o.tempo, o.contour, enc, o.formant, o.volume),
             _stream_meter(model, o.live_loudness, o.max_gain_db, o.output_rate, o.who))
 
 
@@ -1685,7 +1798,8 @@ class StreamBatch:
             output_rate: Optional[int] = None, encoding: Optional[str] = None, gain: Optional[float] = None,
             pitch: Optional[float] = None, tempo: Optional[float] = None,
             pitch_contour: Optional[Sequence] = None, formant_ratio: Optional[float] = None,
-            speaker_blend=None, live_loudness=None, max_gain_db: Optional[float] = None) -> int:
+            speaker_blend=None, live_loudness=None, max_gain_db: Optional[float] = None,
+            volume_contour: Optional[Sequence] = None) -> int:
         """`seed`: the stream's noise seed (see infer_batch_with_values); a seeded stream yields what
         `stream_synthesis(..., seed=seed)` yields, whatever other streams share its encoder pass.  `output_rate`,
         `encoding` and `gain`: the stream's sample rate and G.711 encoding, as for stream_synthesis; `pitch` / `tempo`:
@@ -1698,25 +1812,28 @@ class StreamBatch:
         stream's speaker blend, as for stream_synthesis; it replaces its config's speaker and is checked here.
         `live_loudness` / `max_gain_db`: the stream's live loudness, as for stream_synthesis; a LoudnessStream that an
         unfinished stream of this batch already carries is refused.  Metered streams go through passes of their own,
-        so the other streams keep their passes and their bits."""
+        so the other streams keep their passes and their bits.  `volume_contour`: one volume level per phoneme
+        character (phonemes) or per id (ids), as for stream_synthesis; checked here, naming the stream.  A stream with
+        one goes through the warped passes."""
         if not isinstance(self.model, VitsStreamingModel):
+            refuse_volume(volume_contour, "StreamBatch")
             refuse_live_loudness(live_loudness, "StreamBatch")
             refuse_formants(formant_ratio, "StreamBatch")
             refuse_prosody(pitch, tempo, "StreamBatch")
             refuse_contour(pitch_contour, "StreamBatch")
         return self._add(ids_or_phonemes, config, self.chunk_size, seed, output_rate, encoding, gain, pitch, tempo,
-                         pitch_contour, speaker_blend, formant_ratio, live_loudness, max_gain_db)
+                         pitch_contour, speaker_blend, formant_ratio, live_loudness, max_gain_db, volume_contour)
 
     def _add(self, ids_or_phonemes, config, chunk_size: int, seed: Optional[int] = None,
              output_rate: Optional[int] = None, encoding: Optional[str] = None, gain: Optional[float] = None,
              pitch: Optional[float] = None, tempo: Optional[float] = None, pitch_contour=None,
-             speaker_blend=None, formant_ratio=None, live_loudness=None, max_gain_db=None) -> int:
+             speaker_blend=None, formant_ratio=None, live_loudness=None, max_gain_db=None, volume_contour=None) -> int:
         carried = [o.live_loudness for o in self._pending] + [s.meter for s in self._active]
         o = _stream_options(self.model, "StreamBatch", self._next_key, ids_or_phonemes, config, chunk_size,
                             self.chunk_padding, seed=seed, output_rate=output_rate, encoding=encoding, gain=gain,
                             pitch=pitch, tempo=tempo, pitch_contour=pitch_contour, formant_ratio=formant_ratio,
                             speaker_blend=speaker_blend, live_loudness=live_loudness, max_gain_db=max_gain_db,
-                            carried=carried)
+                            carried=carried, volume_contour=volume_contour)
         self._next_key += 1
         self._pending.append(o)
         return o.key
