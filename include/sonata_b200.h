@@ -373,6 +373,46 @@ int32_t sb200_speak_batch_ids_volume(sb200_voice* v, const int64_t* ids_packed, 
                                      int32_t* id_frames_out, int64_t* bounds_out, double* lufs_out, float* gain_out,
                                      sb200_error* err);
 
+/* ---- breaks: a pause in milliseconds after any id ----
+ * A break image gives each id of an utterance a pause after it, packed like ids_packed (f32): a finite value in
+ * (0, 10000] ms, or NaN or exactly 0 for none.  Any other value (negative, +-inf, above 10 s) fails with
+ * OPERATION_ERROR naming the utterance and the id, before any device work, as does an utterance whose paused length
+ * would pass 2^31 - 1 samples.  The stage runs at the voice's rate R on the n2 samples x the volume stage hands out
+ * (the formant stage's, the pitch stage's or the decoder's without one), after it and before any output-rate
+ * resampling, loudness target, live meter and encoder, which see its output as they see a waveform.  In double, each
+ * operation rounded (no fused multiply-add):
+ *  1. Lengths.  N_i = floor(ms_i R / 1000 + 0.5); a break with N_i = 0 asks for nothing.
+ *  2. Positions.  Break i sits at E_i, id i's delivered end before breaks (the ends of step 4 of
+ *     sb200_speak_batch_ids_contour, what sb200_job_prosody_bounds reported before breaks: 256 C_i without prosody; the
+ *     last end is n2).  Breaks at equal positions merge in ascending id order, their lengths summed: breaks k = 1 .. m at
+ *     P_1 < .. < P_m of lengths M_k, with running totals D_k = M_1 + .. + M_k, D_0 = 0.
+ *  3. Fades.  F = R / 200 (integer division, volume's half ramp), S(t) = t t (3 - 2 t).  Input sample j gets h_j: 1.0
+ *     multiplied, in ascending k, by S(((P_k - j) - 0.5) / F) for every k with P_k - F <= j < P_k (fade-out) and by
+ *     S(((j - P_k) + 0.5) / F) for every k with P_k <= j < P_k + F (fade-in), rounded to f32 once; y_j = x_j h_j, one
+ *     f32 multiply, no clamp.
+ *  4. Output.  n2 + D_m samples: input sample j lands at j + D_{k(j)}, k(j) = #{k : P_k <= j}, and outputs
+ *     [P_k + D_{k-1}, P_k + D_k) hold +0.0f.  A break at n2 is trailing silence; one at 0 (after ids with no samples)
+ *     leading silence.
+ *  5. Delivered ends.  E'_i = E_i + sum of M_k over P_k <= E_i: a pause belongs to the id it follows, so alignments stay
+ *     contiguous from sample 0 and the last end is the delivered length.  bounds_out, sb200_job_prosody_bounds and the
+ *     stream bounds report E' (at an output rate: ceil(E' up / down)).  The volume stage still uses E.
+ * An image of NaN / 0 only, or whose breaks all round to 0 samples, runs nothing and keeps every bit; an utterance with
+ * breaks has the same bits in any batch; a loudness target normalises the paused utterance as a whole (its silent
+ * blocks fall under the absolute gate); the i16 route's peak scale does not move.  When some utterance of a batch asks,
+ * every utterance goes through the one break launch (one that does not ask is copied).  sb200_job_lengths, the fetches
+ * (f32, i16, G.711, FLAC), sb200_job_copy_out and the d_out capacity all count the paused signal.  The executable
+ * specification is tests/break_reference.py.  Realtime streams take breaks through sb200_prosody_stream_create_breaks.
+ * sb200_speak_batch_ids_volume with breaks_ms_packed (NULL: none); NULL is that call, bit for bit. */
+int32_t sb200_speak_batch_ids_breaks(sb200_voice* v, const int64_t* ids_packed, const size_t* offsets, size_t batch,
+                                     const sb200_synth_config* cfgs, const float* scale_packed,
+                                     const int32_t* frames_packed, const uint64_t* seeds, const int32_t* seeded,
+                                     const uint32_t* output_rates, const float* target_lufs, const float* pitch,
+                                     const float* tempo, const float* pitch_packed, const float* formants,
+                                     const int64_t* blend_speakers, const float* blend_weights,
+                                     const size_t* blend_offsets, const float* volume_db_packed,
+                                     const float* breaks_ms_packed, sb200_audio* outs, int32_t* id_frames_out,
+                                     int64_t* bounds_out, double* lufs_out, float* gain_out, sb200_error* err);
+
 /* ---- job API: the same batched pass split into its host<->device steps (bench / multi-GPU plumbing) ----
  * create  : copies ids to the device (H2D).  `eps_w` / `eps_z` optionally inject the graph's two
  *           RandomNormalLike draws (time-major: eps_w[b] = f32[T_x][2], eps_z[b] = f32[T_y][inter]);
@@ -444,6 +484,12 @@ int32_t sb200_job_set_formants(sb200_job* job, const float* formants, sb200_erro
  * contour copies the batch's cumulative durations to the host with the frame counts, and sb200_job_profile reports the
  * stage as the region "volume".  The result keeps its layout: the stage scales it in place. */
 int32_t sb200_job_set_volume_contour(sb200_job* job, const float* volume_db_packed, sb200_error* err);
+/* Breaks (see sb200_speak_batch_ids_breaks) for the next sb200_job_run, packed like ids_packed, or NULL for none (what a
+ * new job starts with; so is an image that is all NaN or 0).  A bad entry fails with OPERATION_ERROR naming the
+ * utterance and the id, and leaves the job as it was.  A run with breaks copies the batch's cumulative durations to the
+ * host, and sb200_job_profile reports the stage as the region "break".  The result's lengths, offsets and
+ * sb200_job_prosody_bounds count the pauses. */
+int32_t sb200_job_set_breaks(sb200_job* job, const float* breaks_ms_packed, sb200_error* err);
 /* Speaker blends (see sb200_speak_batch_ids_blends) for the next sb200_job_run as a blend table, or NULL offsets for none
  * (what a new job starts with).  Every entry is checked first; a bad one fails with OPERATION_ERROR naming the utterance
  * and leaves the job's blends as they were. */
@@ -659,9 +705,9 @@ int32_t sb200_decode_chunks_warped(sb200_voice* v, const sb200_latent* const* zs
  * expression is evaluated as written, each operation rounded (no fused multiply-add). */
 int32_t sb200_prosody_stream_create_contour(sb200_voice* v, const sb200_latent* z, const float* pitch_per_id,
                                             size_t n_ids, float tempo, sb200_prosody_stream** out, sb200_error* err);
-/* Each id's delivered end (step 4 of sb200_speak_batch_ids_contour) at the voice's rate, known at creation: the ends
- * the batch path reports for the same latent.  out[0 .. n_ids); fails with OPERATION_ERROR for a stream made without
- * a contour or a capacity below the id count. */
+/* Each id's delivered end (step 4 of sb200_speak_batch_ids_contour; after its pauses for a stream with breaks) at the
+ * voice's rate, known at creation: the ends the batch path reports for the same latent.  out[0 .. n_ids); fails with
+ * OPERATION_ERROR for a stream made without a contour or breaks, or a capacity below the id count. */
 int32_t sb200_prosody_stream_bounds(const sb200_prosody_stream* s, int64_t* out, size_t capacity, sb200_error* err);
 /* ---- streams with a formant ratio (see sb200_speak_batch_ids_formants) ----
  * A prosody stream with a formant ratio phi (NaN: none; else a finite value in [0.5, 2]) on top of a pitch ratio and a
@@ -709,6 +755,25 @@ int32_t sb200_prosody_stream_create_volume(sb200_voice* v, const sb200_latent* z
                                            sb200_error* err);
 /* The "volume" device time (ms) of the last chunk pass the stream was in (0: its stage did not run). */
 int32_t sb200_prosody_stream_profile_volume(const sb200_prosody_stream* s, float* volume_ms);
+/* ---- streams with breaks (see sb200_speak_batch_ids_breaks) ----
+ * sb200_prosody_stream_create_volume with breaks_ms_per_id[0 .. n_ids) (NULL: none), one break per id of latent z
+ * (required with breaks).  Ratios, a phi and a volume contour that ask for nothing are accepted when a break asks: a
+ * break-only stream.  Breaks that ask for nothing give the stream sb200_prosody_stream_create_volume gives.  The
+ * positions and lengths are fixed at creation from the latent's frames and the table is uploaded once, into the
+ * stream's own allocation; the stream must then be fed exactly its latent's frames.  A bad break fails naming the id.
+ * Emission: with J the samples the stage has received so far, after every chunk pass it has emitted exactly
+ * O(J) = J + sum of M_k over P_k <= J samples, so a chunk whose input reaches P_k emits break k's zeros in that pass; the
+ * stage holds nothing back, adds no latency and changes no chunk count, and the last chunk brings the total to
+ * n2 + D_m.  It runs in the chunk pass's region "break", after "volume" and before resampling and any meter.
+ * Contract: join the chunks such a stream emits through sb200_decode_chunks_warped or sb200_decode_chunks_metered; the
+ * result is, bit for bit, the batch contract applied to the joined chunks the same stream yields without breaks, then
+ * resampled, metered and converted as without them.  sb200_prosody_stream_bounds gives E' for such a stream. */
+int32_t sb200_prosody_stream_create_breaks(sb200_voice* v, const sb200_latent* z, float pitch,
+                                           const float* pitch_per_id, size_t n_ids, float tempo, float formant,
+                                           const float* volume_db_per_id, const float* breaks_ms_per_id,
+                                           sb200_prosody_stream** out, sb200_error* err);
+/* The "break" device time (ms) of the last chunk pass the stream was in (0: its stage did not run). */
+int32_t sb200_prosody_stream_profile_breaks(const sb200_prosody_stream* s, float* break_ms);
 
 /* ---- live loudness: a stream held to a target by a causal BS.1770 meter carried on the device ----
  * A loudness stream (a meter) belongs to a voice, and so to its device, and meters one delivered rate r.  Its target T
@@ -917,6 +982,12 @@ int32_t sb200_debug_formant(int32_t device, const float* x, size_t n, int32_t ra
  * of those samples and ends. */
 int32_t sb200_debug_volume(int32_t device, const float* x, size_t n, const int64_t* ends, const float* levels,
                            size_t n_ids, int32_t rate, float* y, sb200_error* err);
+/* The break stage over one caller buffer x[0 .. n) at `rate`, whose id i ends at ends[i] (non-decreasing, the last at
+ * n) with a break of ms[i] after it (n_ids entries, checked as sb200_speak_batch_ids_breaks checks them): *n_out
+ * receives the paused length and y[0 .. *n_out) the result (cap: y's room; too little fails after *n_out is set); bit
+ * for bit what a job gives an utterance of those samples and ends. */
+int32_t sb200_debug_breaks(int32_t device, const float* x, size_t n, const int64_t* ends, const float* ms, size_t n_ids,
+                           int32_t rate, float* y, size_t cap, int64_t* n_out, sb200_error* err);
 /* Test hook, no device needed: the samples a prosody stream with these ratios at `rate` emits per chunk (the rule of
  * sb200_decode_chunks_warped) when its chunks bring chunk_lens[0 .. n_chunks) inputs and the last one ends it.
  * emitted[k] receives chunk k's count.  Returns 0, or 19 for bad ratios, a bad rate or a negative length. */

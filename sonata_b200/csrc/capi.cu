@@ -325,15 +325,15 @@ static void job_prosody(const Job& j, int64_t* n1, int64_t* n2, int32_t* frames)
     }
 }
 
-int32_t sb200_speak_batch_ids_volume(sb200_voice* v, const int64_t* ids, const size_t* offsets, size_t batch,
+int32_t sb200_speak_batch_ids_breaks(sb200_voice* v, const int64_t* ids, const size_t* offsets, size_t batch,
                                      const sb200_synth_config* cfgs, const float* scale_packed,
                                      const int32_t* frames_packed, const uint64_t* seeds, const int32_t* seeded,
                                      const uint32_t* output_rates, const float* target_lufs, const float* pitch,
                                      const float* tempo, const float* pitch_packed, const float* formants,
                                      const int64_t* blend_speakers, const float* blend_weights,
-                                     const size_t* blend_offsets, const float* volume_db_packed, sb200_audio* outs,
-                                     int32_t* id_frames_out, int64_t* bounds_out, double* lufs_out, float* gain_out,
-                                     sb200_error* err) {
+                                     const size_t* blend_offsets, const float* volume_db_packed,
+                                     const float* breaks_ms_packed, sb200_audio* outs, int32_t* id_frames_out,
+                                     int64_t* bounds_out, double* lufs_out, float* gain_out, sb200_error* err) {
     return guarded(err, [&] {
         const double t0 = now_ms();
         static_assert(sizeof(long long) == sizeof(int64_t), "");
@@ -349,6 +349,7 @@ int32_t sb200_speak_batch_ids_volume(sb200_voice* v, const int64_t* ids, const s
         canonical_blends(*v->v, reinterpret_cast<const long long*>(blend_speakers), blend_weights, blend_offsets, batch,
                          "utterance");
         check_volume_contour(volume_db_packed, offsets, batch);
+        check_breaks(breaks_ms_packed, offsets, batch);
         std::unique_ptr<Job> j(create_job(v->v.get(), reinterpret_cast<const long long*>(ids), offsets, batch, nullptr,
                                           nullptr, nullptr, false));
         if (cfgs) set_job_configs(*j, cfgs_in(cfgs, batch).data());
@@ -361,6 +362,7 @@ int32_t sb200_speak_batch_ids_volume(sb200_voice* v, const int64_t* ids, const s
         set_job_formants(*j, formants);
         set_job_blends(*j, reinterpret_cast<const long long*>(blend_speakers), blend_weights, blend_offsets);
         set_job_volume_contour(*j, volume_db_packed);
+        set_job_breaks(*j, breaks_ms_packed);
         j->run(nullptr, 0);
         fetch_audio(*j, outs, 0.f);
         if (id_frames_out) {
@@ -376,6 +378,20 @@ int32_t sb200_speak_batch_ids_volume(sb200_voice* v, const int64_t* ids, const s
         for (size_t b = 0; b < batch; b++)
             outs[b].inference_ms = wall * (j->out_total ? (float)outs[b].len / (float)j->out_total : 0.f);
     });
+}
+int32_t sb200_speak_batch_ids_volume(sb200_voice* v, const int64_t* ids, const size_t* offsets, size_t batch,
+                                     const sb200_synth_config* cfgs, const float* scale_packed,
+                                     const int32_t* frames_packed, const uint64_t* seeds, const int32_t* seeded,
+                                     const uint32_t* output_rates, const float* target_lufs, const float* pitch,
+                                     const float* tempo, const float* pitch_packed, const float* formants,
+                                     const int64_t* blend_speakers, const float* blend_weights,
+                                     const size_t* blend_offsets, const float* volume_db_packed, sb200_audio* outs,
+                                     int32_t* id_frames_out, int64_t* bounds_out, double* lufs_out, float* gain_out,
+                                     sb200_error* err) {
+    return sb200_speak_batch_ids_breaks(v, ids, offsets, batch, cfgs, scale_packed, frames_packed, seeds, seeded,
+                                        output_rates, target_lufs, pitch, tempo, pitch_packed, formants, blend_speakers,
+                                        blend_weights, blend_offsets, volume_db_packed, nullptr, outs, id_frames_out,
+                                        bounds_out, lufs_out, gain_out, err);
 }
 int32_t sb200_speak_batch_ids_blends(sb200_voice* v, const int64_t* ids, const size_t* offsets, size_t batch,
                                      const sb200_synth_config* cfgs, const float* scale_packed,
@@ -526,6 +542,9 @@ int32_t sb200_job_set_formants(sb200_job* job, const float* formants, sb200_erro
 }
 int32_t sb200_job_set_volume_contour(sb200_job* job, const float* volume_db_packed, sb200_error* err) {
     return guarded(err, [&] { set_job_volume_contour(*job->j, volume_db_packed); });
+}
+int32_t sb200_job_set_breaks(sb200_job* job, const float* breaks_ms_packed, sb200_error* err) {
+    return guarded(err, [&] { set_job_breaks(*job->j, breaks_ms_packed); });
 }
 int32_t sb200_job_set_speaker_blends(sb200_job* job, const int64_t* speakers, const float* weights, const size_t* offsets,
                                      sb200_error* err) {
@@ -830,19 +849,29 @@ int32_t sb200_prosody_stream_create_volume(sb200_voice* v, const sb200_latent* z
                                            const float* pitch_per_id, size_t n_ids, float tempo, float formant,
                                            const float* volume_db_per_id, sb200_prosody_stream** out,
                                            sb200_error* err) {
+    return sb200_prosody_stream_create_breaks(v, z, pitch, pitch_per_id, n_ids, tempo, formant, volume_db_per_id,
+                                              nullptr, out, err);
+}
+int32_t sb200_prosody_stream_create_breaks(sb200_voice* v, const sb200_latent* z, float pitch,
+                                           const float* pitch_per_id, size_t n_ids, float tempo, float formant,
+                                           const float* volume_db_per_id, const float* breaks_ms_per_id,
+                                           sb200_prosody_stream** out, sb200_error* err) {
     return guarded(err, [&] {
-        if (!v || !out || ((pitch_per_id || volume_db_per_id) && !z)) throw Error(19, "null argument");
+        const bool per_id = pitch_per_id || volume_db_per_id || breaks_ms_per_id;
+        if (!v || !out || (per_id && !z)) throw Error(19, "null argument");
         Voice* w = v->v.get();
         if (w->device < 0 || !w->emb)
             throw Error(19, "Failed to run model inference. Error: voice was loaded config-only (device -1); libsonata_b200 has no CPU path");
         std::vector<long long> ends;
         long long n = -1;
-        if (pitch_per_id || volume_db_per_id) {
+        if (per_id) {
             if (z->l->v != w) throw Error(19, "the latent was not encoded by this voice");
             const std::vector<int>& f = z->l->id_frames;
             if (n_ids != f.size())
-                throw Error(19, std::string(pitch_per_id ? "pitch contour: " : "volume contour: ") +
-                                    std::to_string(n_ids) + (pitch_per_id ? " ratios" : " levels") +
+                throw Error(19, std::string(pitch_per_id ? "pitch contour: " : volume_db_per_id ? "volume contour: "
+                                                                                                : "breaks: ") +
+                                    std::to_string(n_ids) +
+                                    (pitch_per_id ? " ratios" : volume_db_per_id ? " levels" : " breaks") +
                                     " for a latent of " + std::to_string(f.size()) + " ids");
             const long long hop = w->a.hop();
             ends.resize(n_ids);
@@ -850,9 +879,9 @@ int32_t sb200_prosody_stream_create_volume(sb200_voice* v, const sb200_latent* z
             for (size_t i = 0; i < n_ids; i++) ends[i] = (c += f[i]) * hop;
             n = z->l->frames * hop;
         }
-        *out = new sb200_prosody_stream{create_prosody_stream_volume(w, w->device, w->sample_rate, n, ends.data(),
+        *out = new sb200_prosody_stream{create_prosody_stream_breaks(w, w->device, w->sample_rate, n, ends.data(),
                                                                      pitch_per_id, n_ids, pitch, tempo, formant,
-                                                                     volume_db_per_id),
+                                                                     volume_db_per_id, breaks_ms_per_id),
                                         v->v};
     });
 }
@@ -860,7 +889,8 @@ int32_t sb200_prosody_stream_bounds(const sb200_prosody_stream* s, int64_t* out,
     return guarded(err, [&] {
         if (!s) throw Error(19, "null argument");
         const std::vector<long long>& b = s->p->bounds;
-        if (s->p->n_total < 0) throw Error(19, "prosody stream bounds: the stream was made without a pitch contour");
+        if (s->p->n_total < 0 && s->p->brk.empty())
+            throw Error(19, "prosody stream bounds: the stream was made without a pitch contour or breaks");
         if (capacity < b.size() || (!out && !b.empty()))
             throw Error(19, "prosody stream bounds: room for " + std::to_string(capacity) + " of " +
                                 std::to_string(b.size()) + " ids");
@@ -882,6 +912,11 @@ int32_t sb200_prosody_stream_profile_formant(const sb200_prosody_stream* s, floa
 int32_t sb200_prosody_stream_profile_volume(const sb200_prosody_stream* s, float* volume_ms) {
     if (!s) return 19;
     if (volume_ms) *volume_ms = s->p->last_vol_ms;
+    return 0;
+}
+int32_t sb200_prosody_stream_profile_breaks(const sb200_prosody_stream* s, float* break_ms) {
+    if (!s) return 19;
+    if (break_ms) *break_ms = s->p->last_brk_ms;
     return 0;
 }
 
@@ -1458,6 +1493,28 @@ int32_t sb200_debug_volume(int32_t device, const float* x, size_t n, const int64
         SB_CUDA(cudaSetDevice(device));
         HookStage h(o, x, n);
         if (n) SB_CUDA(cudaMemcpy(y, h.b.in, n * 4, cudaMemcpyDeviceToHost));
+    });
+}
+
+int32_t sb200_debug_breaks(int32_t device, const float* x, size_t n, const int64_t* ends, const float* ms, size_t n_ids,
+                           int32_t rate, float* y, size_t cap, int64_t* n_out, sb200_error* err) {
+    return guarded(err, [&] {
+        if ((n && !x) || (n_ids && (!ends || !ms)) || !n_out || rate < 200)
+            throw Error(19, "debug breaks: bad arguments");
+        const size_t offs[2] = {0, n_ids};
+        check_breaks(ms, offs, 1, false);
+        const std::vector<BreakPiece> bk =
+            break_plan(reinterpret_cast<const long long*>(ends), ms, n_ids, (long long)n, rate, "");
+        const long long total = (long long)n + (bk.empty() ? 0 : bk.back().D);
+        *n_out = total;
+        if ((size_t)total > cap || (total && !y))
+            throw Error(19, "debug breaks: the destination holds " + std::to_string(cap) + " samples, the result has " +
+                                std::to_string(total));
+        OutputPlan o;
+        if (!bk.empty()) o.bp.add(0, (long long)n, 0, 0, total, volume_half(rate), bk);
+        SB_CUDA(cudaSetDevice(device));
+        HookStage h(o, x, n);
+        if (total) SB_CUDA(cudaMemcpy(y, h.out.buf, (size_t)total * 4, cudaMemcpyDeviceToHost));
     });
 }
 

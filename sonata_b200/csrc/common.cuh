@@ -396,6 +396,21 @@ struct VolumeSeg {
 // One launch over the segments: blockIdx.y = segment, max_n: the most samples of any segment.
 void launch_volume(const VolumeSeg* segs, int nseg, long long max_n, const float* src, const FrameSeg* fsegs,
                    const PcmPost* posts, int hop, cudaStream_t st);
+// Pauses (breaks.cu; include/sonata_b200.h, sb200_speak_batch_ids_breaks).  Break k of a signal sits at input sample P
+// (ascending, merged), and D is the running length of breaks 1 .. k in samples.
+struct BreakPiece { long long P, D; };
+// One signal's break stage: output samples [o0, o0 + n) of the paused signal become y[0 .. n), from the input samples
+// j0 .. of x (x[j - j0]), with the fades of half samples around each of its m breaks bk.  x: the samples, read plainly,
+// or null for chunk `chunk` of the pass's input read through its post-path (fsegs / posts).
+struct BreakSeg {
+    const float* x; float* y;
+    long long n, o0, j0;
+    int chunk, half, m;
+    const BreakPiece* bk;
+};
+// One launch over the segments: blockIdx.y = segment, max_n: the most outputs of any segment.
+void launch_breaks(const BreakSeg* segs, int nseg, long long max_n, const float* src, const FrameSeg* fsegs,
+                   const PcmPost* posts, int hop, cudaStream_t st);
 // Analysis position of WSOLA frame k: floor(k Hs / alpha + 0.5), every operation exactly rounded in double, so the host
 // plan and the kernels agree; the virtual frame -1 sits at -Hs.
 __host__ __device__ inline long long prosody_analysis(int Hs, double alpha, long long k) {

@@ -335,6 +335,11 @@ void set_job_volume_contour(Job& j, const float* packed) {
     else j.volume.clear();
 }
 
+void set_job_breaks(Job& j, const float* packed) {
+    if (check_breaks(packed, j.offs.data(), j.B)) j.breaks.assign(packed, packed + j.ids.size());
+    else j.breaks.clear();
+}
+
 void Profile::begin(const std::string& name) {
     if (!regions) return;
     regions->emplace_back();
@@ -481,7 +486,7 @@ struct IdBufs {
     Staged<int> xslot;                         // multi-speaker voices: speaker slot of every X granule
     SpeakerBias spk;
     int* cum;
-    int* cum_h;                                // pinned mirror of cum (only when the job has a pitch or volume contour)
+    int* cum_h;                                // pinned mirror of cum (only with a pitch or volume contour or breaks)
     float *xa, *xb, *qkv, *att, *ffn, *stats, *d0, *t1, *t2, *g, *h29, *zz, *logw;
     float *att_s, *att_vt, *att_orel;          // tensor-core attention: scores of every head, V^T, relative-value term
     float* epsw;
@@ -507,7 +512,7 @@ struct IdBufs {
         if (!j.frames.slot_spk.empty()) xslot.carve(dev, pin, nxg);
         spk.carve(dev, pin, v, j.frames);
         cum = dev.get<int>(RX);
-        cum_h = j.contour.empty() && j.volume.empty() ? nullptr : pin.get<int>(RX);
+        cum_h = j.contour.empty() && j.volume.empty() && j.breaks.empty() ? nullptr : pin.get<int>(RX);
         xa = rows(H); xb = rows(H); qkv = rows(3 * H); att = rows(H); ffn = rows(a.filter); stats = rows(2 * a.inter);
         d0 = rows(H); t1 = rows(H); t2 = rows(H); g = rows(H); h29 = rows(32); zz = rows(2); logw = rows(1);
         att_s = att_vt = att_orel = nullptr;

@@ -283,6 +283,13 @@ struct ProsodyStream {
     std::vector<VolumePiece> vol;
     const VolumePiece* vol_d = nullptr;
     float last_vol_ms = 0.f;
+    // The break stage (breaks.cu): the table of pauses over the delivered samples before them, fixed at creation
+    // (empty: none), resident on the device after the volume table (brk_d); the stage's input length brk_n2, inputs
+    // taken (J) and outputs emitted, and its last region time.
+    std::vector<BreakPiece> brk;
+    const BreakPiece* brk_d = nullptr;
+    long long brk_n2 = 0, brk_in = 0, brk_out = 0;
+    float last_brk_ms = 0.f;
     ~ProsodyStream();
 };
 // Whether stream ps runs the stretch or pitch stage (a formant-only stream runs neither).
@@ -310,6 +317,33 @@ struct VolumePlan {
     double bytes = 0;
     void add(long long at_, long long n, long long j0, int half, const std::vector<VolumePiece>& pc,
              const VolumePiece* pc_d = nullptr);
+};
+// Pauses (breaks.cu).  Checks breaks packed[0 .. offs[B]) of B utterances or, with !per_utterance, of one stream: a
+// break is NaN or 0 (none) or a finite value in (0, 10000] ms, or the call fails naming the utterance (per_utterance)
+// and the id.  Returns whether some break asks for something.
+bool check_breaks(const float* packed, const size_t* offs, size_t B, bool per_utterance = true);
+// The samples of a break of ms milliseconds at `rate`: floor(ms R / 1000 + 0.5) in double, 0 for none.
+long long break_samples(float ms, int rate);
+// The break table of a signal of n2 delivered samples whose id i ends at ends[i] (non-decreasing, the last at n2) with
+// a break of ms[i] after it (include/sonata_b200.h, sb200_speak_batch_ids_breaks): breaks of 0 samples dropped, those
+// at equal positions merged.  Empty when none asks.  Throws OPERATION_ERROR, prefixed by `who`, for bad ends and for a
+// paused length past 2^31 - 1.
+std::vector<BreakPiece> break_plan(const long long* ends, const float* ms, size_t n_ids, long long n2, int rate,
+                                   const std::string& who);
+// The samples the breaks at or before input position pos add: sum of M_k over P_k <= pos.
+long long break_shift(const std::vector<BreakPiece>& bk, long long pos);
+// The break launch's segments.  at[q]: a job's segment reads offset at[q] of the stage's input; a chunk pass's is
+// chunk at[q].  Every segment writes at y_off[q] of the stage's own output (total samples).  A job's tables are laid out
+// back to back in `pieces` (p_off[q]; -1: the segment's table is already a stream's resident one).
+struct BreakPlan {
+    std::vector<BreakSeg> segs;
+    std::vector<long long> at, p_off, y_off;
+    std::vector<BreakPiece> pieces;
+    long long total = 0, max_n = 0;
+    double bytes = 0;
+    // Appends a segment of n_in inputs from input position j0 that emits outputs [o0, o0 + n_out).
+    void add(long long at_, long long n_in, long long j0, long long o0, long long n_out, int half,
+             const std::vector<BreakPiece>& bk, const BreakPiece* bk_d = nullptr);
 };
 
 // The most inputs a formant stream carries between passes: fewer than N, and the 3 H that recompute the frames before
@@ -353,7 +387,17 @@ void prosody_stream_init_formant(ProsodyStream& ps, int rate, long long n, const
 // (n_ids ids over n inputs, required with levels) giving each id's delivered end as prosody_contour_plan does: the
 // checks of check_volume_contour, and ratios and a phi that ask for nothing are accepted when the contour asks.
 void prosody_stream_init_volume(ProsodyStream& ps, int rate, long long n, const long long* ends, const float* ratios,
-                                size_t n_ids, float pitch, float tempo, float phi, const float* levels);
+                                size_t n_ids, float pitch, float tempo, float phi, const float* levels,
+                                bool allow_none = false);
+// The same with breaks ms[0 .. n_ids) (null: none) after the ids (ends required with breaks): the checks of
+// check_breaks, and ratios, a phi and a contour that ask for nothing are accepted when a break asks.  The table is
+// planned over the delivered ends before breaks, and bounds becomes the ends after them.
+void prosody_stream_init_breaks(ProsodyStream& ps, int rate, long long n, const long long* ends, const float* ratios,
+                                size_t n_ids, float pitch, float tempo, float phi, const float* levels,
+                                const float* ms);
+ProsodyStream* create_prosody_stream_breaks(Voice* v, int device, int rate, long long n, const long long* ends,
+                                            const float* ratios, size_t n_ids, float pitch, float tempo, float phi,
+                                            const float* levels, const float* ms);
 ProsodyStream* create_prosody_stream_volume(Voice* v, int device, int rate, long long n, const long long* ends,
                                             const float* ratios, size_t n_ids, float pitch, float tempo, float phi,
                                             const float* levels);
@@ -559,11 +603,14 @@ struct Job {
                                       // (set_job_formants)
     std::vector<float> volume;        // per-id levels in dB, packed like ids, NaN or 0 = none; empty when no utterance
                                       // has a volume contour (set_job_volume_contour)
+    std::vector<float> breaks;        // per-id pauses in ms, packed like ids, NaN or 0 = none; empty when no utterance
+                                      // has one (set_job_breaks)
     std::vector<SpeakerBlend> blends; // one canonical blend per utterance (empty entry: the config's speaker); empty when
                                       // none has one (set_job_blends)
     std::vector<ProsodyShape> pros_ran;   // each utterance's shape in the last run (empty: it ran no prosody stage)
     std::vector<float> pitch_ran, tempo_ran;   // the ratios the last run had (empty: none)
-    std::vector<long long> pros_bounds;   // each id's delivered end in the last run when it had a contour (else empty)
+    std::vector<long long> pros_bounds;   // each id's delivered end in the last run when it had a contour, a volume
+                                          // contour or breaks (after its pauses; else empty)
     // Loudness of the last run: the targets it ran with (empty: it measured nothing), each utterance's integrated
     // loudness and the gain applied to it
     std::vector<float> loud_ran; std::vector<double> loud_lufs; std::vector<float> loud_gain;
@@ -640,6 +687,11 @@ void set_job_formants(Job& j, const float* phi);
 // check_volume_contour.  A bad entry leaves the job's contour as it was.  Each utterance whose pieces (volume_pieces,
 // over its ids' delivered ends) ask runs the volume stage after the formant stage, before any resampling and loudness.
 void set_job_volume_contour(Job& j, const float* packed);
+// Per-id breaks of the job's next run in ms, packed like its ids (NaN or 0: none), or null for none; see check_breaks.
+// A bad entry leaves the job's breaks as they were.  When some utterance's breaks ask for samples, every utterance runs
+// the break stage after the volume stage, before any resampling and loudness, and its length, bounds and place in the
+// job's result count its pauses.
+void set_job_breaks(Job& j, const float* packed);
 // Per-utterance speaker blends of the job's next run (a blend table as for canonical_blends), or null for none.  A blend
 // replaces the utterance's config speaker; its noise and length scales still apply.  Every entry is checked first; a bad
 // entry fails naming the utterance and leaves the job's blends as they were.
@@ -741,7 +793,8 @@ struct ChunkResult {
 void decode_chunks(Voice* v, const ChunkPass& p, ChunkResult& out);
 
 // ---- the waveform output stage (output_stage.cu) ----
-// After the decoder: prosody (stretch, pitch), formants, volume, resampling, then loudness in place on what that leaves.
+// After the decoder: prosody (stretch, pitch), formants, volume, breaks, resampling, then loudness in place on what that
+// leaves.
 
 // What a stage reads: segment k is buf[segs[k].out_off ..), segs[k].len * hop samples read through posts[k] (trims,
 // fade, gain; null: read plainly).  The whole-signal prosody and formant launches read buf at their plans' offsets.
@@ -787,6 +840,7 @@ struct OutputPlan {
     ProsodyPlan pp;
     FormantPlan fp;
     VolumePlan vp;
+    BreakPlan bp;
     ResamplePlan rp;
     LoudnessPlan lp;                          // whole signals
     MeterPlan mp;                             // chunk passes
@@ -802,16 +856,17 @@ struct OutputPlan {
 // The output stage of job j's utterances on the frame layout j.frames with `hop` samples per frame, and what the job
 // hands out (osegs, out_hop, out_total, osr).  With a contour (cum: the batch's cum rows on the host) every utterance is
 // planned from its ids' ends, and bounds receives each id's delivered end, packed like the ids.  A volume contour's
-// pieces are planned over the same ends (cum is then on the host too).
+// pieces and the breaks' tables are planned over the same ends (cum is then on the host too); with breaks, bounds
+// receives every utterance's ends after its pauses.
 OutputPlan plan_job_output(Job& j, int hop, const std::vector<int>& cum, std::vector<long long>& bounds);
 // The output stage of chunk pass chunks, chunk k bringing n_in[k] samples after its trims: each chunk's prosody stream,
-// its formant stage, with `resample` the resample launch (a chunk without a resampler is copied), and its meter, which
+// its formant, volume and break stages, with `resample` the resample launch (a chunk without a resampler is copied), and its meter, which
 // reads what the resample launch delivers (without it: the chunk's stage output).
 OutputPlan plan_chunk_output(const std::vector<ChunkSpec>& chunks, const std::vector<long long>& n_in, bool resample);
 
 // The device buffers and tables of plan p and their pinned mirrors.  `in` is where the stage's input goes (the decoder's
-// waveforms, in_total samples): a buffer of the pass's own, followed by the prosody output `py` and the formant output
-// `fy`, or the caller's d_out when no stage writes a result of its own.  With d_out the last stage that writes writes
+// waveforms, in_total samples): a buffer of the pass's own, followed by the prosody output `py`, the formant output
+// `fy`, a chunk pass's volume output `vy` and the break output `by`, or the caller's d_out when no stage writes a result of its own.  With d_out the last stage that writes writes
 // there; the resample output `ry` is otherwise the pass's own.  offsets, ps (the stretched signal) and py stay
 // reachable after the pass.
 struct OutputBufs {
@@ -821,6 +876,7 @@ struct OutputBufs {
     int* offsets = nullptr; float *px = nullptr, *ps = nullptr, *py = nullptr;
     Staged<FormantSeg> fsegs; Staged<FormantCarry> fcarry; float *fwin = nullptr, *fy = nullptr;
     Staged<VolumeSeg> vsegs; Staged<VolumePiece> vpieces; float* vy = nullptr;
+    Staged<BreakSeg> bsegs; Staged<BreakPiece> bpieces; Staged<FrameSeg> bosegs; float* by = nullptr;
     Staged<FrameSeg> rin; Staged<PcmPost> rpost;  // chunk passes: what the resample launch reads after the stages
     Staged<ResampleSeg> rsegs; Staged<PcmPost> rposts; Staged<FrameSeg> rosegs; float* ry = nullptr;
     Staged<LoudSeg> lsegs; double* lscratch = nullptr; Staged<double> lufs; Staged<float> gain;
@@ -834,8 +890,9 @@ struct OutputBufs {
 };
 
 // The launches of plan p from the input wave `in` (in.buf == b.in) on st: profile regions "stretch", "pitch",
-// "formant", "volume", "resample" and "loudness", each only when its stage runs.  A job's volume stage scales its
-// utterances in place; a chunk pass's writes each chunk to vy (after fy).  Returns what the stage delivers: the last
+// "formant", "volume", "break", "resample" and "loudness", each only when its stage runs.  A job's volume stage scales
+// its utterances in place; a chunk pass's writes each chunk to vy (after fy).  The break stage writes every segment to
+// by, longer by its pauses.  Returns what the stage delivers: the last
 // output's wave (a job's: its segments at hop 1 once a stage has changed their lengths).  The loudness results are
 // downloaded to their pinned mirrors.
 Wave run_output_stage(Profile& prof, const OutputPlan& p, const OutputBufs& b, Wave in, cudaStream_t st);

@@ -1,5 +1,5 @@
 // The waveform output stage: what runs after the decoder, in this order: prosody (the stretch and the pitch stage), the
-// formant stage, the volume stage, resampling, and loudness in place on what those leave.  Jobs, chunk passes and the
+// formant stage, the volume stage, the break stage, resampling, and loudness in place on what those leave.  Jobs, chunk passes and the
 // test hooks plan, carve and launch it here only, so they run the same launches.
 #include "engine.h"
 #include <algorithm>
@@ -87,36 +87,62 @@ OutputPlan plan_job_output(Job& j, int hop, const std::vector<int>& cum, std::ve
         }
         if (fp.segs.empty()) fp = FormantPlan();
     }
-    // volume: each asking utterance in place in the layout the stages before it leave, its pieces over its ids'
-    // delivered ends (the contour's bounds, or those the utterance's ratios give)
-    if (audio && !j.volume.empty()) {
-        std::vector<long long> ends, e2;
+    // each id's delivered end before any pause, which the volume and break stages share: the contour's bounds, or
+    // those the utterance's ratios give
+    if (audio && bounds.empty() && (!j.volume.empty() || !j.breaks.empty())) {
+        bounds.resize(j.ids.size());
+        std::vector<long long> ends;
         std::vector<ContourPiece> unused;
+        for (size_t b = 0; b < B; b++) {
+            const size_t n_ids = j.offs[b + 1] - j.offs[b];
+            ends.resize(n_ids);
+            for (size_t i = 0; i < n_ids; i++) ends[i] = (long long)cum[j.xsegs[b].off + i] * hop;
+            prosody_contour_plan(j.v->sample_rate, (long long)fs[b].len * hop, ends.data(), nullptr, n_ids,
+                                 j.pitch.empty() ? NAN : j.pitch[b], j.tempo.empty() ? NAN : j.tempo[b], unused,
+                                 bounds.data() + j.offs[b]);
+        }
+    }
+    // where each utterance is, and how long, after the stages before volume (the formant stage keeps their layout)
+    const auto at = [&](size_t b) { return pp.segs.empty() ? fs[b].out_off : pp.segs[b].y_off; };
+    const auto n2_of = [&](size_t b) { return pp.segs.empty() ? (long long)fs[b].len * hop : pp.segs[b].n2; };
+    // volume: each asking utterance in place, its pieces over its ids' delivered ends
+    if (audio && !j.volume.empty()) {
         for (size_t b = 0; b < B; b++) {
             const size_t n_ids = j.offs[b + 1] - j.offs[b];
             const float* lv = j.volume.data() + j.offs[b];
             if (!std::any_of(lv, lv + n_ids, [](float v) { return !std::isnan(v) && v != 0.f; })) continue;
-            const long long n = (long long)fs[b].len * hop, n2 = pp.segs.empty() ? n : pp.segs[b].n2;
-            if (!bounds.empty()) {
-                e2.assign(bounds.begin() + j.offs[b], bounds.begin() + j.offs[b + 1]);
-            } else {
-                ends.resize(n_ids); e2.resize(n_ids);
-                for (size_t i = 0; i < n_ids; i++) ends[i] = (long long)cum[j.xsegs[b].off + i] * hop;
-                prosody_contour_plan(j.v->sample_rate, n, ends.data(), nullptr, n_ids,
-                                     j.pitch.empty() ? NAN : j.pitch[b], j.tempo.empty() ? NAN : j.tempo[b], unused,
-                                     e2.data());
-            }
-            const std::vector<VolumePiece> pc = volume_pieces(e2.data(), lv, n_ids, n2);
-            if (!pc.empty())
-                o.vp.add(pp.segs.empty() ? fs[b].out_off : pp.segs[b].y_off, n2, 0, volume_half(j.v->sample_rate), pc);
+            const std::vector<VolumePiece> pc = volume_pieces(bounds.data() + j.offs[b], lv, n_ids, n2_of(b));
+            if (!pc.empty()) o.vp.add(at(b), n2_of(b), 0, volume_half(j.v->sample_rate), pc);
         }
     }
-    // what the job hands out: the frame layout itself, the prosody output (the formant stage keeps its layout), or with
-    // output rates one resampled segment per utterance at its rate, back to back
+    // breaks: when any utterance asks, every utterance into the stage's own output, back to back (one that does not
+    // ask is copied), and its ends moved past the pauses before them
+    if (audio && !j.breaks.empty()) {
+        std::vector<std::vector<BreakPiece>> bk(B);
+        bool any = false;
+        for (size_t b = 0; b < B; b++) {
+            const size_t n_ids = j.offs[b + 1] - j.offs[b];
+            bk[b] = break_plan(bounds.data() + j.offs[b], j.breaks.data() + j.offs[b], n_ids, n2_of(b),
+                               j.v->sample_rate, "utterance " + std::to_string(b) + ": ");
+            any |= !bk[b].empty();
+        }
+        if (any)
+            for (size_t b = 0; b < B; b++) {
+                const long long n2 = n2_of(b), d = bk[b].empty() ? 0 : bk[b].back().D;
+                o.bp.add(at(b), n2, 0, 0, n2 + d, volume_half(j.v->sample_rate), bk[b]);
+                for (size_t i = j.offs[b]; i < j.offs[b + 1]; i++) bounds[i] += break_shift(bk[b], bounds[i]);
+            }
+    }
+    // what the job hands out: the frame layout itself, the prosody output (the formant stage keeps its layout), the
+    // break output, or with output rates one resampled segment per utterance at its rate, back to back
     j.osr.assign(B, j.v->sample_rate);
+    const BreakPlan& bp = o.bp;
     if (j.out_rates.empty() || !audio) {
         j.osegs = fs; j.out_hop = hop; j.out_total = j.frames.total_samples;
-        if (!pp.segs.empty()) {
+        if (!bp.segs.empty()) {
+            for (size_t b = 0; b < B; b++) j.osegs[b] = FrameSeg{0, (int)bp.segs[b].n, 0, 0, bp.y_off[b]};
+            j.out_hop = 1; j.out_total = bp.total;
+        } else if (!pp.segs.empty()) {
             for (size_t b = 0; b < B; b++) j.osegs[b] = FrameSeg{0, (int)pp.segs[b].n2, 0, 0, pp.segs[b].y_off};
             j.out_hop = 1; j.out_total = pp.y_total;
         }
@@ -128,7 +154,7 @@ OutputPlan plan_job_output(Job& j, int hop, const std::vector<int>& cum, std::ve
                 j.osr[b] = j.out_rates[b];
                 f = &voice_resampler(*j.v, j.out_rates[b], "utterance " + std::to_string(b) + ": ");
             }
-            o.rp.add(f, pp.segs.empty() ? (long long)fs[b].len * hop : pp.segs[b].n2);
+            o.rp.add(f, bp.segs.empty() ? n2_of(b) : bp.segs[b].n);
             j.osegs[b] = FrameSeg{0, (int)o.rp.segs[b].n_out, 0, 0, o.rp.segs[b].out_off};
         }
         j.out_hop = 1; j.out_total = o.rp.total;
@@ -179,6 +205,17 @@ OutputPlan plan_chunk_output(const std::vector<ChunkSpec>& chunks, const std::ve
                 o.vp.y_off.push_back(o.vp.total);
                 o.vp.total += o.n_res[k];
             }
+            if (!c.ps->brk.empty()) {
+                // the inputs [J0, J1) it receives, and every output up to O(J1) = J1 + the pauses at or before J1
+                const ProsodyStream& w = *c.ps;
+                const long long J1 = w.brk_in + o.n_res[k];
+                if (J1 > w.brk_n2 || (c.last && J1 != w.brk_n2))
+                    throw Error(19, "internal: a prosody stream with breaks would " + std::string(c.last ? "end" : "go on") +
+                                        " after " + std::to_string(J1) + " inputs, not its " + std::to_string(w.brk_n2));
+                const long long n_out = J1 + break_shift(w.brk, J1) - w.brk_out;
+                o.bp.add((long long)k, o.n_res[k], w.brk_in, w.brk_out, n_out, volume_half(w.rate), w.brk, w.brk_d);
+                o.n_res[k] = n_out;
+            }
         }
         if (resample) o.rp.add(c.rs ? &c.rs->f : nullptr, o.n_res[k], c.rs, c.last != 0);
     }
@@ -218,7 +255,12 @@ void OutputBufs::carve(Arena& dev, Arena& pin, const OutputPlan& p, long long in
         vsegs.carve(dev, pin, n);
         if (!p.vp.pieces.empty()) vpieces.carve(dev, pin, p.vp.pieces.size());
     }
-    if (p.streams() && (!pp.segs.empty() || !fp.segs.empty() || !p.vp.segs.empty())) {
+    if (const size_t n = p.bp.segs.size()) {
+        bsegs.carve(dev, pin, n);
+        if (!p.bp.pieces.empty()) bpieces.carve(dev, pin, p.bp.pieces.size());
+        if (!p.streams()) bosegs.carve(dev, pin, n);
+    }
+    if (p.streams() && (!pp.segs.empty() || !fp.segs.empty() || !p.vp.segs.empty() || !p.bp.segs.empty())) {
         rin.carve(dev, pin, p.chunks.size());
         rpost.carve(dev, pin, p.chunks.size());
     }
@@ -237,12 +279,15 @@ void OutputBufs::carve(Arena& dev, Arena& pin, const OutputPlan& p, long long in
         me = dev.get<double>(8 * steps);
         mlufs.carve(dev, pin, steps); mgains.carve(dev, pin, steps); mclip.carve(dev, pin, m);
     }
-    const bool staged = !pp.segs.empty() || !fp.segs.empty() || !p.rp.segs.empty();
-    in = staged || !d_out ? dev.get<float>((size_t)(in_total + pp.y_total + fp.total + p.vp.total) + 4) : d_out;
+    const bool staged = !pp.segs.empty() || !fp.segs.empty() || !p.bp.segs.empty() || !p.rp.segs.empty();
+    in = staged || !d_out ? dev.get<float>((size_t)(in_total + pp.y_total + fp.total + p.vp.total + p.bp.total) + 4)
+                          : d_out;
     py = in + in_total;
     fy = py + pp.y_total;
     vy = fy + fp.total;
+    by = vy + p.vp.total;
     if (!p.rp.segs.empty()) ry = d_out ? d_out : dev.get<float>((size_t)p.rp.total + 4);
+    else if (d_out && !p.bp.segs.empty()) by = d_out;
     else if (d_out && !fp.segs.empty()) fy = d_out;
     else if (d_out && !pp.segs.empty()) py = d_out;
 }
@@ -287,14 +332,15 @@ void OutputBufs::upload(const OutputPlan& p, int hop, const FrameSeg* in_segs, c
     for (size_t k = 0; k < n; k++) at[k] = in + in_segs[k].out_off;
     for (size_t q = 0; q < p.warped.size(); q++) at[p.warped[q]] = py + pp.segs[q].y_off;
     for (size_t q = 0; q < p.formed.size(); q++) at[p.formed[q]] = fy + fp.segs[q].y_off;
+    // a job's utterances are in the last stage's output; a chunk is where the stages before it leave it (without one,
+    // read through its post-path)
+    float* base = !fp.segs.empty() ? fy : !pp.segs.empty() ? py : in;
+    std::vector<char> staged(n, 0);
+    for (int k : p.warped) staged[k] = 1;
+    for (int k : p.formed) staged[k] = 1;
     if (vsegs.d) {
-        // a job's utterances in place in the last stage's output; a chunk read where the stages before it leave it
-        // (without one, through its post-path) and written to vy
+        // a job's utterances scaled in place; a chunk written to vy
         const VolumePlan& vp = p.vp;
-        float* base = !fp.segs.empty() ? fy : !pp.segs.empty() ? py : in;
-        std::vector<char> staged(n, 0);
-        for (int k : p.warped) staged[k] = 1;
-        for (int k : p.formed) staged[k] = 1;
         for (size_t q = 0; q < vp.segs.size(); q++) {
             VolumeSeg g = vp.segs[q];
             if (p.streams()) {
@@ -302,6 +348,7 @@ void OutputBufs::upload(const OutputPlan& p, int hop, const FrameSeg* in_segs, c
                 g.chunk = (int)k;
                 g.x = staged[k] ? at[k] : nullptr;
                 g.y = at[k] = vy + vp.y_off[q];
+                staged[k] = 1;
             } else {
                 g.y = base + vp.at[q];
                 g.x = g.y;
@@ -313,6 +360,31 @@ void OutputBufs::upload(const OutputPlan& p, int hop, const FrameSeg* in_segs, c
         if (vpieces.d) {
             std::copy(vp.pieces.begin(), vp.pieces.end(), vpieces.h);
             vpieces.upload(st);
+        }
+    }
+    if (bsegs.d) {
+        // every segment written to by, longer by its pauses
+        const BreakPlan& bp = p.bp;
+        for (size_t q = 0; q < bp.segs.size(); q++) {
+            BreakSeg g = bp.segs[q];
+            g.y = by + bp.y_off[q];
+            if (p.streams()) {
+                const size_t k = (size_t)bp.at[q];
+                g.chunk = (int)k;
+                g.x = staged[k] ? at[k] : nullptr;
+                at[k] = g.y;
+            } else {
+                g.x = base + bp.at[q];
+                bosegs.h[q] = FrameSeg{0, (int)g.n, 0, 0, bp.y_off[q]};
+            }
+            if (bp.p_off[q] >= 0) g.bk = bpieces.d + bp.p_off[q];
+            bsegs.h[q] = g;
+        }
+        bsegs.upload(st);
+        if (bosegs.d) bosegs.upload(st);
+        if (bpieces.d) {
+            std::copy(bp.pieces.begin(), bp.pieces.end(), bpieces.h);
+            bpieces.upload(st);
         }
     }
     if (rin.d) {
@@ -413,6 +485,14 @@ Wave run_output_stage(Profile& prof, const OutputPlan& p, const OutputBufs& b, W
         prof.end();
         if (streams) cur = restaged;
     }
+    const BreakPlan& bp = p.bp;
+    if (!bp.segs.empty()) {
+        prof.begin("break");
+        launch_breaks(b.bsegs.d, (int)bp.segs.size(), bp.max_n, in.buf, in.segs, in.posts, in.hop, st);
+        prof.count(0, bp.bytes);
+        prof.end();
+        cur = streams ? restaged : Wave{b.by, b.bosegs.d, nullptr, 1};
+    }
     const ResamplePlan& rp = p.rp;
     if (!rp.segs.empty()) {
         prof.begin("resample");
@@ -454,7 +534,7 @@ Wave run_output_stage(Profile& prof, const OutputPlan& p, const OutputBufs& b, W
 
 void advance_streams(const OutputPlan& p, const OutputBufs& b, const Profile& prof) {
     const float stretch_ms = prof.ms("stretch"), pitch_ms = prof.ms("pitch"), formant_ms = prof.ms("formant"),
-                volume_ms = prof.ms("volume"), loudness_ms = prof.ms("loudness");
+                volume_ms = prof.ms("volume"), break_ms = prof.ms("break"), loudness_ms = prof.ms("loudness");
     for (size_t k = 0; k < p.chunks.size(); k++) {
         const ChunkSpec& c = p.chunks[k];
         if (Resampler* r = c.rs) {
@@ -467,11 +547,17 @@ void advance_streams(const OutputPlan& p, const OutputBufs& b, const Profile& pr
         }
         if (ProsodyStream* w = c.ps) {
             if (w->fm) formant_stream_advance(*w, p.fsteps[k]);
+            if (!w->brk.empty()) {
+                // the inputs it took (what the stages before it emitted), and the outputs emitted for them
+                w->brk_in = w->fm ? p.fsteps[k].e1 : p.steps[k].j1;
+                w->brk_out += p.n_res[k];
+            }
             prosody_stream_advance(*w, p.steps[k], c.last != 0);
             const bool warps = prosody_stream_warps(*w);
             w->last_ms[0] = warps ? stretch_ms : 0.f; w->last_ms[1] = warps ? pitch_ms : 0.f;
             w->last_fm_ms = w->fm ? formant_ms : 0.f;
             w->last_vol_ms = w->vol.empty() ? 0.f : volume_ms;
+            w->last_brk_ms = w->brk.empty() ? 0.f : break_ms;
         }
     }
     const MeterPlan& mp = p.mp;

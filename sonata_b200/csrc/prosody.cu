@@ -540,10 +540,11 @@ void prosody_stream_init_formant(ProsodyStream& ps, int rate, long long n, const
 }
 
 void prosody_stream_init_volume(ProsodyStream& ps, int rate, long long n, const long long* ends, const float* ratios,
-                                size_t n_ids, float pitch, float tempo, float phi, const float* levels) {
+                                size_t n_ids, float pitch, float tempo, float phi, const float* levels,
+                                bool allow_none) {
     const size_t offs[2] = {0, n_ids};
     const bool asks = check_volume_contour(levels, offs, 1, false);
-    prosody_stream_init_formant(ps, rate, n, ends, ratios, n_ids, pitch, tempo, phi, asks);
+    prosody_stream_init_formant(ps, rate, n, ends, ratios, n_ids, pitch, tempo, phi, asks || allow_none);
     if (!asks) return;
     // each id's delivered end, as the batch path computes it for the same ratios or contour
     std::vector<long long> e2(n_ids);
@@ -551,14 +552,37 @@ void prosody_stream_init_volume(ProsodyStream& ps, int rate, long long n, const 
     const ProsodyShape sh = prosody_contour_plan(rate, n, ends, ratios, n_ids, ratios ? NAN : pitch, tempo, unused,
                                                  e2.data());
     ps.vol = volume_pieces(e2.data(), levels, n_ids, sh.n2);
-    if (ps.vol.empty() && !ps.fm && !prosody_stream_warps(ps))
+    if (!allow_none && ps.vol.empty() && !ps.fm && !prosody_stream_warps(ps))
         throw Error(19, "a prosody stream's ratios, formant ratio and volume contour ask for nothing (the contour's "
                         "levels apply only to ids without samples)");
 }
 
+void prosody_stream_init_breaks(ProsodyStream& ps, int rate, long long n, const long long* ends, const float* ratios,
+                                size_t n_ids, float pitch, float tempo, float phi, const float* levels,
+                                const float* ms) {
+    const size_t offs[2] = {0, n_ids};
+    const bool asks = check_breaks(ms, offs, 1, false);
+    prosody_stream_init_volume(ps, rate, n, ends, ratios, n_ids, pitch, tempo, phi, levels, asks);
+    if (!asks) return;
+    // each id's delivered end before breaks, as the batch path computes it for the same ratios or contour
+    std::vector<long long> e2(n_ids);
+    std::vector<ContourPiece> unused;
+    const ProsodyShape sh = prosody_contour_plan(rate, n, ends, ratios, n_ids, ratios ? NAN : pitch, tempo, unused,
+                                                 e2.data());
+    ps.brk = break_plan(e2.data(), ms, n_ids, sh.n2, rate, "");
+    if (ps.brk.empty() && ps.vol.empty() && !ps.fm && !prosody_stream_warps(ps))
+        throw Error(19, "a prosody stream's ratios, formant ratio, volume contour and breaks ask for nothing (every "
+                        "break rounds to 0 samples)");
+    ps.brk_n2 = sh.n2;
+    if (!ps.brk.empty()) {
+        for (long long& e : e2) e += break_shift(ps.brk, e);
+        ps.bounds = std::move(e2);
+    }
+}
+
 namespace {
 // The history buffers (two sets of cap_in + cap_s floats and two ints), the formant stage's two carry buffers when it
-// runs and, after them, the pitch contour's piece table and the volume contour's.
+// runs and, after them, the pitch contour's piece table, the volume contour's and the break table.
 ProsodyStream* allocate_prosody_stream(std::unique_ptr<ProsodyStream> ps, Voice* v, int device) {
     ps->v = v; ps->device = device;
     SB_CUDA(cudaSetDevice(device));
@@ -566,7 +590,8 @@ ProsodyStream* allocate_prosody_stream(std::unique_ptr<ProsodyStream> ps, Voice*
     const size_t fm = ps->fm ? (size_t)FM_CARRY : 0;
     const size_t table = (2 * (side + fm) * 4 + 15) / 16 * 16;
     const size_t vol_at = (table + ps->pieces.size() * sizeof(ContourPiece) + 15) / 16 * 16;
-    const size_t bytes = vol_at + ps->vol.size() * sizeof(VolumePiece);
+    const size_t brk_at = (vol_at + ps->vol.size() * sizeof(VolumePiece) + 15) / 16 * 16;
+    const size_t bytes = brk_at + ps->brk.size() * sizeof(BreakPiece);
     void* mem = nullptr;
     SB_CUDA(cudaMalloc(&mem, bytes));
     ps->mem = mem;
@@ -586,6 +611,11 @@ ProsodyStream* allocate_prosody_stream(std::unique_ptr<ProsodyStream> ps, Voice*
         VolumePiece* d = reinterpret_cast<VolumePiece*>(static_cast<char*>(mem) + vol_at);
         SB_CUDA(cudaMemcpy(d, ps->vol.data(), ps->vol.size() * sizeof(VolumePiece), cudaMemcpyHostToDevice));
         ps->vol_d = d;
+    }
+    if (!ps->brk.empty()) {
+        BreakPiece* d = reinterpret_cast<BreakPiece*>(static_cast<char*>(mem) + brk_at);
+        SB_CUDA(cudaMemcpy(d, ps->brk.data(), ps->brk.size() * sizeof(BreakPiece), cudaMemcpyHostToDevice));
+        ps->brk_d = d;
     }
     return ps.release();
 }
@@ -616,6 +646,14 @@ ProsodyStream* create_prosody_stream_volume(Voice* v, int device, int rate, long
                                             const float* levels) {
     std::unique_ptr<ProsodyStream> ps(new ProsodyStream());
     prosody_stream_init_volume(*ps, rate, n, ends, ratios, n_ids, pitch, tempo, phi, levels);
+    return allocate_prosody_stream(std::move(ps), v, device);
+}
+
+ProsodyStream* create_prosody_stream_breaks(Voice* v, int device, int rate, long long n, const long long* ends,
+                                            const float* ratios, size_t n_ids, float pitch, float tempo, float phi,
+                                            const float* levels, const float* ms) {
+    std::unique_ptr<ProsodyStream> ps(new ProsodyStream());
+    prosody_stream_init_breaks(*ps, rate, n, ends, ratios, n_ids, pitch, tempo, phi, levels, ms);
     return allocate_prosody_stream(std::move(ps), v, device);
 }
 

@@ -10,7 +10,7 @@ import numpy as np
 
 from . import _native as N
 from .core import G711_LAW, Audio, OperationError, check_encoding
-from .piper import (_batch_options, _blend_arrays, _check, _config_array, _contour_arrays, _duration_arrays,
+from .piper import (_batch_options, _blend_arrays, _break_arrays, _check, _config_array, _contour_arrays, _duration_arrays,
                     _formant_array, _gain_array, _loudness_array, _pack_ids, _prosody_arrays, _ptr, _rate_array,
                     _seed_arrays, _take_audio, _take_bytes, _volume_arrays)
 
@@ -22,18 +22,18 @@ class SynthesisJob:
                  loudness: Optional[Sequence] = None, pitches: Optional[Sequence] = None,
                  tempos: Optional[Sequence] = None, pitch_contours: Optional[Sequence] = None,
                  formants: Optional[Sequence] = None, speaker_blends: Optional[Sequence] = None,
-                 volume_contours: Optional[Sequence] = None):
+                 volume_contours: Optional[Sequence] = None, breaks: Optional[Sequence] = None):
         """`configs`: one PiperSynthesisConfig per utterance (see set_configs); None keeps the voice's fallback config.
         `seeds`: noise seeds (see set_seeds).  `output_rates`: output sample rates (see set_output_rates).
         `loudness`: loudness targets (see set_loudness).  `pitches` / `tempos`: pitch and tempo ratios (see
         set_prosody).  `pitch_contours`: per-id pitch ratios (see set_pitch_contours).  `formants`: formant ratios (see
         set_formants).  `speaker_blends`: speaker blends (see set_speaker_blends).  `volume_contours`: per-id volume
-        levels (see set_volume_contours)."""
+        levels (see set_volume_contours).  `breaks`: per-id pauses (see set_breaks)."""
         # argument errors before the job exists
         options = _batch_options(model, len(batches), [len(b) for b in batches], configs, seeds=seeds,
                                  output_rates=output_rates, loudness=loudness, pitches=pitches, tempos=tempos,
                                  pitch_contours=pitch_contours, formants=formants, speaker_blends=speaker_blends,
-                                 volume_contours=volume_contours)
+                                 volume_contours=volume_contours, breaks=breaks)
         self._open(model, batches, options, eps_w, eps_z, debug)
 
     @classmethod
@@ -101,6 +101,8 @@ class SynthesisJob:
                       _ptr(o.blend_weights, C.c_float), _ptr(o.blend_offsets, C.c_size_t))
         if o.volume is not None:
             self._set(lib.sb200_job_set_volume_contour, _ptr(o.volume, C.c_float))
+        if o.breaks is not None:
+            self._set(lib.sb200_job_set_breaks, _ptr(o.breaks, C.c_float))
 
     def _set(self, fn, *images) -> None:
         """One sb200_job_set_* call with its C images."""
@@ -190,6 +192,13 @@ class SynthesisJob:
         contours off.  The results keep their lengths and layout, and profile() reports the stage as "volume".  A bad
         entry raises OperationError naming the utterance and the id, and leaves the job's contours as they were."""
         self._set(self._lib.sb200_job_set_volume_contour, _ptr(_volume_arrays(self._lens, contours), C.c_float))
+
+    def set_breaks(self, breaks: Optional[Sequence]) -> None:
+        """Per-id pauses in ms for the next run (see VitsModel.infer_batch_with_values): breaks[b] holds one break per
+        id of utterance b, or is None; None for the whole list, or breaks that are all None / NaN / 0, turn pauses off.
+        The results, their lengths and prosody_bounds count the pauses, and profile() reports the stage as "break".  A
+        bad entry raises OperationError naming the utterance and the id, and leaves the job's breaks as they were."""
+        self._set(self._lib.sb200_job_set_breaks, _ptr(_break_arrays(self._lens, breaks), C.c_float))
 
     def set_speaker_blends(self, blends: Optional[Sequence]) -> None:
         """Per-utterance speaker blends for the next run (see VitsModel.infer_batch_with_values): a mapping

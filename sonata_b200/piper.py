@@ -431,6 +431,79 @@ def _volume_arrays(lens: Sequence[int], volume_contours=None, who: Optional[Sequ
     return None if (np.isnan(out) | (out == 0)).all() else out
 
 
+BREAK_RANGE_MS = (0.0, 10000.0)   # a break (ms) is in (low, high]; None, NaN or 0 ask for none
+
+
+def _break_value(x, b, i: int, unit: str = "id") -> float:
+    if x is None:
+        return math.nan
+    if isinstance(x, bool) or not isinstance(x, numbers.Real):
+        raise OperationError(f"{_who(b)}, {unit} {i}: break {x!r} is not a number")
+    x = float(x)
+    if not (math.isnan(x) or x == 0.0 or (math.isfinite(x) and BREAK_RANGE_MS[0] < x <= BREAK_RANGE_MS[1])):
+        raise OperationError(f"{_who(b)}, {unit} {i}: break {x} ms is not a finite value in "
+                             f"({BREAK_RANGE_MS[0]}, {BREAK_RANGE_MS[1]}] (None, NaN or 0: none)")
+    return x
+
+
+def _break_arrays(lens: Sequence[int], breaks=None, who: Optional[Sequence[str]] = None):
+    """The packed C image of per-id breaks in ms (f32, NaN for none), checked as the library checks them, or None when
+    not given or when every break is None / NaN / 0.  breaks[b] holds one break per id of utterance b, the pause after
+    that id (in BREAK_RANGE_MS, or None / NaN / 0 for none), or is None.  `who`: as for _contour_arrays."""
+    if breaks is None:
+        return None
+    n = len(lens)
+    out = np.full(int(sum(lens)), np.nan, np.float32)
+    pos = 0
+    for b, v in enumerate(_per_utterance(breaks, n, "breaks")):
+        if v is not None:
+            label = b if who is None else who[b]
+            a = _numeric(v, "fiu")
+            if a is None:
+                v = list(v)
+                a = np.array([_break_value(x, label, i) for i, x in enumerate(v)] if len(v) == lens[b] else v)
+            if a.size != lens[b]:
+                raise OperationError(f"{_who(label)}: {a.size} breaks for {lens[b]} ids")
+            f = a.astype(np.float32).reshape(-1)
+            asked = ~np.isnan(f) & (f != 0)
+            bad = np.nonzero(asked & ~(np.isfinite(f) & (f > BREAK_RANGE_MS[0]) & (f <= BREAK_RANGE_MS[1])))[0]
+            if bad.size:
+                _break_value(float(f[bad[0]]), label, int(bad[0]))
+            out[pos:pos + lens[b]] = f
+        pos += lens[b]
+    return None if (np.isnan(out) | (out == 0)).all() else out
+
+
+def _char_breaks_to_ids(v, phonemes: str, src: Sequence[int], b) -> list:
+    """Per-character breaks v (one per character of `phonemes`) as per-id breaks: a character's break goes after the
+    last id it maps to (its pad); a character the voice drops puts its break after the last id before it (bos when no
+    kept character precedes it), so no requested pause is lost.  Breaks that land on one id add up.  Each break is
+    checked by _break_value, naming its character."""
+    v = list(v) if not isinstance(v, np.ndarray) else v.reshape(-1).tolist()
+    if len(v) != len(phonemes):
+        raise OperationError(f"{_who(b)}: {len(v)} breaks for {len(phonemes)} characters")
+    ms = [_break_value(x, b, c, "character") for c, x in enumerate(v)]
+    # the ids a break can follow: bos (before every character) and each id of a kept character, in order
+    keys = [(-1 if i == 0 else int(c), i) for i, c in enumerate(src) if i == 0 or int(c) >= 0]
+    out = [math.nan] * len(src)
+    for c, x in enumerate(ms):
+        if math.isnan(x) or x == 0.0:
+            continue
+        i = [i for k, i in keys if k <= c][-1]
+        out[i] = x if math.isnan(out[i]) else out[i] + x
+    return out
+
+
+def _breaks_ask(image, rate: int) -> bool:
+    """Whether a per-id breaks image (of _break_arrays, or None) asks for a pause of one sample or more at `rate`: some
+    floor(ms * rate / 1000 + 0.5) > 0, in double as the library computes it."""
+    if image is None:
+        return False
+    ms = image.astype(np.float64)
+    ms = ms[~np.isnan(ms)]
+    return bool(np.any(np.floor(ms * rate / 1000.0 + 0.5) > 0))
+
+
 def refuse_prosody(pitch, tempo, where: str) -> None:
     """OperationError when `where`, a mode that hands out a sentence chunk by chunk, is asked for a pitch or tempo
     ratio."""
@@ -445,6 +518,13 @@ def refuse_volume(volume_contour, where: str) -> None:
     if volume_contour is not None:
         raise OperationError(f"{where} cannot apply a volume contour: only this library's streaming voices carry a "
                              "contour from chunk to chunk (use speak_batch or a SynthesisJob)")
+
+
+def refuse_breaks(breaks, where: str) -> None:
+    """OperationError when `where`, a mode without this library's streaming voices, is asked for breaks."""
+    if breaks is not None:
+        raise OperationError(f"{where} cannot insert breaks: only this library's streaming voices carry them from chunk "
+                             "to chunk (use speak_batch or a SynthesisJob)")
 
 
 def refuse_contour(pitch_contour, where: str) -> None:
@@ -482,8 +562,8 @@ def _gain_array(gains, n: int):
 class _BatchOptions:
     """A batch's options, checked once by _batch_options, as the C images the library takes: each None when not given
     or when no utterance asks for it.  A phoneme surface's per-character controls (char_scales, char_contours,
-    char_volumes: one entry or None per utterance) become the per-id images `scales`, `contour` and `volume` once its
-    phonemes are mapped (map_characters)."""
+    char_volumes, char_breaks: one entry or None per utterance) become the per-id images `scales`, `contour`, `volume`
+    and `breaks` once its phonemes are mapped (map_characters)."""
     n: int
     cfgs: object = None                       # sb200_synth_config [n]
     scales: Optional[np.ndarray] = None       # per id, packed
@@ -502,9 +582,11 @@ class _BatchOptions:
     blend_weights: Optional[np.ndarray] = None
     blend_offsets: Optional[np.ndarray] = None
     volume: Optional[np.ndarray] = None       # per id, packed
+    breaks: Optional[np.ndarray] = None       # per id, packed
     char_scales: Optional[list] = None
     char_contours: Optional[list] = None
     char_volumes: Optional[list] = None
+    char_breaks: Optional[list] = None
 
     def map_characters(self, phonemes: Sequence[str], maps) -> None:
         """Makes the per-id images of the per-character controls once the phonemes are mapped: maps[b] is (ids, source
@@ -517,15 +599,23 @@ class _BatchOptions:
         self.scales, _ = _duration_arrays(lens, per_id(self.char_scales, "duration scales", _scale_value))
         self.contour = _contour_arrays(lens, per_id(self.char_contours, "pitch ratios", _contour_value), self.pitch)
         self.volume = _volume_arrays(lens, per_id(self.char_volumes, "volume levels", _volume_value, 0.0))
+        self.breaks = None if self.char_breaks is None else _break_arrays(lens, [
+            None if v is None else _char_breaks_to_ids(v, ph, src, b)
+            for b, (v, ph, (_, src)) in enumerate(zip(self.char_breaks, phonemes, maps))])
+
+    @property
+    def per_character(self) -> bool:
+        """Whether a per-character control needs the phonemes' character map."""
+        return any(x is not None for x in (self.char_scales, self.char_contours, self.char_volumes, self.char_breaks))
 
 
 def _batch_options(model, n: int, lens: Optional[Sequence[int]] = None, configs=None, duration_scales=None,
                    durations=None, seeds=None, output_rates=None, loudness=None, law=None, gains=None, pitches=None,
                    tempos=None, pitch_contours=None, formants=None, speaker_blends=None, volume_contours=None,
-                   g711: bool = False) -> _BatchOptions:
+                   breaks=None, g711: bool = False) -> _BatchOptions:
     """The options of a batch of n utterances, each checked as its C image is made, in one order at every surface:
     configs, duration scales, durations, seeds, output rates, loudness, law (with `g711`), gains, pitch and tempo, pitch
-    contours, formants, speaker blends, volume contours.  `lens`: the utterances' id counts, for per-id controls; None for a phoneme
+    contours, formants, speaker blends, volume contours, breaks.  `lens`: the utterances' id counts, for per-id controls; None for a phoneme
     surface, whose per-character controls are only counted here, before any phoneme is mapped (see map_characters)."""
     o = _BatchOptions(n, _config_array(configs, n))
     if lens is None:
@@ -549,6 +639,10 @@ def _batch_options(model, n: int, lens: Optional[Sequence[int]] = None, configs=
         o.char_volumes = None if volume_contours is None else _per_utterance(volume_contours, n, "volume contours")
     else:
         o.volume = _volume_arrays(lens, volume_contours)
+    if lens is None:
+        o.char_breaks = None if breaks is None else _per_utterance(breaks, n, "breaks")
+    else:
+        o.breaks = _break_arrays(lens, breaks)
     return o
 
 
@@ -784,20 +878,21 @@ class _VitsCommons:
                     pitches: Optional[Sequence] = None, tempos: Optional[Sequence] = None,
                     pitch_contours: Optional[Sequence] = None, formants: Optional[Sequence] = None,
                     speaker_blends: Optional[Sequence] = None,
-                    volume_contours: Optional[Sequence] = None) -> List[Audio]:
+                    volume_contours: Optional[Sequence] = None, breaks: Optional[Sequence] = None) -> List[Audio]:
         """`configs`: one PiperSynthesisConfig per utterance (speaker and scales), still synthesised as one pass;
         None uses the fallback config for every utterance.  `seeds`: noise seeds as for infer_batch_with_values.
         `speaker_blends`: as for infer_batch_with_values.
         `output_rates` / `loudness` / `pitches` / `tempos` / `formants`: per-utterance output sample rates, loudness
         targets, pitch and tempo ratios and formant ratios as for infer_batch_with_values.  `pitch_contours` /
-        `volume_contours`: as for speak_batch_with_alignment, one ratio or level per phoneme character."""
+        `volume_contours` / `breaks`: as for speak_batch_with_alignment, one ratio, level or break per phoneme
+        character."""
         n = len(phoneme_batches)
         o = _batch_options(self, n, None, configs, seeds=seeds, output_rates=output_rates, loudness=loudness,
                            pitches=pitches, tempos=tempos, pitch_contours=pitch_contours, formants=formants,
-                           speaker_blends=speaker_blends, volume_contours=volume_contours)
+                           speaker_blends=speaker_blends, volume_contours=volume_contours, breaks=breaks)
         if n == 0:
             return []
-        if pitch_contours is not None or volume_contours is not None:
+        if pitch_contours is not None or volume_contours is not None or breaks is not None:
             maps = [self.phonemes_to_input_ids_map(p) for p in phoneme_batches]
             o.map_characters(phoneme_batches, maps)
             return [a for a, _, _ in self._speak_ids([ids for ids, _ in maps], o)]
@@ -827,7 +922,8 @@ class _VitsCommons:
                                 pitch_contours: Optional[Sequence] = None,
                                 formants: Optional[Sequence] = None,
                                 speaker_blends: Optional[Sequence] = None,
-                                volume_contours: Optional[Sequence] = None) -> List[Audio]:
+                                volume_contours: Optional[Sequence] = None,
+                                breaks: Optional[Sequence] = None) -> List[Audio]:
         """Batched infer_with_values.  `configs`: one PiperSynthesisConfig per utterance (speaker and scales), or None
         for the fallback config; each utterance's result equals a single-utterance call with its config as the
         fallback, except for the on-device noise of an unseeded utterance, whose draws depend on the batch position.
@@ -875,11 +971,17 @@ class _VitsCommons:
         NaN / 0 for none), or None: SSML's <prosody volume> on a span.  Each id's delivered samples are scaled by its
         level, with a 10 ms smoothstep between levels, on the device after the formant stage and before any resampling
         and loudness (sb200_speak_batch_ids_volume); a loudness target then normalises the utterance as a whole, so the
-        relative levels survive.  Lengths and alignments do not change, and there is no clamp."""
+        relative levels survive.  Lengths and alignments do not change, and there is no clamp.
+
+        `breaks`: one pause in ms per id for each utterance, inserted after that id (in BREAK_RANGE_MS, or None / NaN
+        / 0 for none), or None: SSML's <break time>.  Each pause is round(ms * rate / 1000) samples of silence at the
+        voice's rate, with a 5 ms smoothstep fade of the speech on either side, inserted on the device after the
+        volume stage and before any resampling and loudness (sb200_speak_batch_ids_breaks); a loudness target then
+        normalises the paused utterance as a whole.  The utterance gets longer by its pauses."""
         o = _batch_options(self, len(batches), [len(b) for b in batches], configs, seeds=seeds,
                            output_rates=output_rates, loudness=loudness, pitches=pitches, tempos=tempos,
                            pitch_contours=pitch_contours, formants=formants, speaker_blends=speaker_blends,
-                           volume_contours=volume_contours)
+                           volume_contours=volume_contours, breaks=breaks)
         return [a for a, _, _ in self._speak_ids(batches, o)]
 
     def infer_batch_with_durations(self, batches: Sequence[Sequence[int]],
@@ -893,7 +995,8 @@ class _VitsCommons:
                                    pitch_contours: Optional[Sequence] = None,
                                    formants: Optional[Sequence] = None,
                                    speaker_blends: Optional[Sequence] = None,
-                                   volume_contours: Optional[Sequence] = None) -> List[Tuple[Audio, np.ndarray]]:
+                                   volume_contours: Optional[Sequence] = None,
+                                   breaks: Optional[Sequence] = None) -> List[Tuple[Audio, np.ndarray]]:
         """infer_batch_with_values with per-id duration control, returning (audio, frames per id) per utterance.
 
         duration_scales[b]: one scale (finite, >= 0) per id of utterance b, applied before the duration's ceil, so 1.0
@@ -902,17 +1005,19 @@ class _VitsCommons:
         utterance whose ids all got 0 frames is still one frame long.  `seeds`: as for infer_batch_with_values; a
         seeded frame's noise depends on its index only, so controls that move frames never reshuffle it.
         `output_rates` / `loudness` / `pitches` / `tempos` / `pitch_contours` / `formants` / `speaker_blends` /
-        `volume_contours`: as for infer_batch_with_values (the frame counts stay frame counts of the utterance before
-        any warp)."""
+        `volume_contours` / `breaks`: as for infer_batch_with_values (the frame counts stay frame counts of the
+        utterance before any warp or pause)."""
         o = _batch_options(self, len(batches), [len(b) for b in batches], configs, duration_scales, durations, seeds,
                            output_rates, loudness, pitches=pitches, tempos=tempos, pitch_contours=pitch_contours,
-                           formants=formants, speaker_blends=speaker_blends, volume_contours=volume_contours)
+                           formants=formants, speaker_blends=speaker_blends, volume_contours=volume_contours,
+                           breaks=breaks)
         return [(a, f) for a, f, _ in self._speak_ids(batches, o, frames=True)]
 
     def _speak_ids(self, batches, o: _BatchOptions, frames: bool = False) -> List[tuple]:
-        """The f32 batch route: `batches` with options `o` in one sb200_speak_batch_ids_volume call.  Per utterance
+        """The f32 batch route: `batches` with options `o` in one sb200_speak_batch_ids_breaks call.  Per utterance
         (audio, frames per id, each id's delivered end): the frames only when asked for, since fetching them costs a
-        device->host copy and a synchronise, and the ends only when o has a pitch contour (None otherwise)."""
+        device->host copy and a synchronise, and the ends only when o has a pitch contour or breaks (None
+        otherwise)."""
         n = len(batches)
         if n == 0:
             return []
@@ -920,15 +1025,15 @@ class _VitsCommons:
         packed, offs = _pack_ids(batches)
         outs = (N.sb200_audio * n)()
         id_frames = np.zeros(int(offs[-1]), np.int32) if frames else None
-        bounds = None if o.contour is None else np.zeros(int(offs[-1]), np.int64)
+        bounds = None if o.contour is None and o.breaks is None else np.zeros(int(offs[-1]), np.int64)
         err = N.sb200_error()
-        _check(self._lib.sb200_speak_batch_ids_volume(
+        _check(self._lib.sb200_speak_batch_ids_breaks(
             self._h, _ptr(packed, C.c_int64), _ptr(offs, C.c_size_t), n, o.cfgs, _ptr(o.scales, C.c_float),
             _ptr(o.frames, C.c_int32), _ptr(o.seeds, C.c_uint64), _ptr(o.seeded, C.c_int32), _ptr(o.rates, C.c_uint32),
             _ptr(o.loudness, C.c_float), _ptr(o.pitch, C.c_float), _ptr(o.tempo, C.c_float), _ptr(o.contour, C.c_float),
             _ptr(o.formants, C.c_float), _ptr(o.blend_speakers, C.c_int64), _ptr(o.blend_weights, C.c_float),
-            _ptr(o.blend_offsets, C.c_size_t), _ptr(o.volume, C.c_float), outs, _ptr(id_frames, C.c_int32), _ptr(bounds, C.c_int64), None, None,
-            C.byref(err)), err)
+            _ptr(o.blend_offsets, C.c_size_t), _ptr(o.volume, C.c_float), _ptr(o.breaks, C.c_float), outs,
+            _ptr(id_frames, C.c_int32), _ptr(bounds, C.c_int64), None, None, C.byref(err)), err)
         cut = lambda a, b: None if a is None else a[int(offs[b]):int(offs[b + 1])].copy()
         return [(_take_audio(outs[b]), cut(id_frames, b), cut(bounds, b)) for b in range(n)]
 
@@ -941,7 +1046,8 @@ class _VitsCommons:
                                    tempos: Optional[Sequence] = None, pitch_contours: Optional[Sequence] = None,
                                    formants: Optional[Sequence] = None,
                                    speaker_blends: Optional[Sequence] = None,
-                                   volume_contours: Optional[Sequence] = None) -> List[Tuple[Audio, List[PhonemeAlignment]]]:
+                                   volume_contours: Optional[Sequence] = None,
+                                   breaks: Optional[Sequence] = None) -> List[Tuple[Audio, List[PhonemeAlignment]]]:
         """speak_batch that also says when each phoneme is spoken: per utterance (audio, alignment), the alignment
         holding one entry for bos (`^`), one per kept phoneme character (its id and its trailing pad) and one for eos
         (`$`), contiguous from sample 0 to len(audio).
@@ -962,11 +1068,15 @@ class _VitsCommons:
         `formants`: as for infer_batch_with_values; it moves no boundary.  `speaker_blends`: as for
         infer_batch_with_values.  volume_contours[b] (or None): one volume level per character of phoneme_batches[b]
         (see infer_batch_with_values), applied to that character's id and pad, bos and eos keeping their level; it
-        moves no boundary."""
+        moves no boundary.  breaks[b] (or None): one pause in ms per character of phoneme_batches[b] (see
+        infer_batch_with_values), after that character's pad; a character the voice drops puts its pause after the
+        last id before it.  An utterance with breaks is aligned from each id's delivered end after the pauses before
+        it, so a pause belongs to the entry it follows and the entries still end at len(audio)."""
         n = len(phoneme_batches)
         o = _batch_options(self, n, None, configs, duration_scales, seeds=seeds, output_rates=output_rates,
                            loudness=loudness, pitches=pitches, tempos=tempos, pitch_contours=pitch_contours,
-                           formants=formants, speaker_blends=speaker_blends, volume_contours=volume_contours)
+                           formants=formants, speaker_blends=speaker_blends, volume_contours=volume_contours,
+                           breaks=breaks)
         maps = [self.phonemes_to_input_ids_map(p) for p in phoneme_batches]
         o.map_characters(phoneme_batches, maps)
         res = self._speak_ids([ids for ids, _ in maps], o, frames=True)
@@ -975,9 +1085,11 @@ class _VitsCommons:
         warped = lambda b: any(r is not None and not np.isnan(r[b]) for r in (o.pitch, o.tempo))
         offs = np.cumsum([0] + [len(ids) for ids, _ in maps])
 
-        def shaped(b):          # utterance b has a contour that asks for something: aligned from its delivered ends
+        def shaped(b):          # utterance b has a contour or breaks that ask: aligned from its delivered ends
             c = None if o.contour is None else o.contour[offs[b]:offs[b + 1]]
-            return c is not None and bool(np.any(~np.isnan(c) & (c != 1)))
+            k = None if o.breaks is None else o.breaks[offs[b]:offs[b + 1]]
+            return ((c is not None and bool(np.any(~np.isnan(c) & (c != 1)))) or
+                    (k is not None and bool(np.any(~np.isnan(k) & (k != 0)))))
         return [(audio, _alignment(ph, src, frames, len(audio), *ratio(audio), warped=warped(b),
                                    bounds=bounds if shaped(b) else None))
                 for b, (ph, (_, src), (audio, frames, bounds)) in enumerate(zip(phoneme_batches, maps, res))]
@@ -987,17 +1099,17 @@ class _VitsCommons:
                          output_rates: Optional[Sequence] = None, loudness: Optional[Sequence] = None,
                          gains: Optional[Sequence] = None, pitches: Optional[Sequence] = None,
                          tempos: Optional[Sequence] = None, formants: Optional[Sequence] = None,
-                         speaker_blends: Optional[Sequence] = None) -> List[bytes]:
+                         speaker_blends: Optional[Sequence] = None, breaks: Optional[Sequence] = None) -> List[bytes]:
         """infer_batch_with_values delivered as G.711 telephony audio: one `bytes` per utterance, one byte per sample.
         `law`: "mulaw" (PCMU) or "alaw" (PCMA), or one of those per utterance.  The bytes are G.711 of exactly the
         16-bit samples the i16 route gives (SynthesisJob.fetch_i16): to_i16_vec of the utterance after gains[b] (None:
         1), or the fixed scale for an utterance with a loudness target.  They are encoded on the device in the i16
         conversion's launches, so only one byte per sample leaves the card.  `configs`, `seeds`, `output_rates` and
-        `loudness` as for infer_batch_with_values, and so are `pitches`, `tempos`, `formants` and `speaker_blends`; a
-        batch mixing laws runs one conversion per law."""
+        `loudness` as for infer_batch_with_values, and so are `pitches`, `tempos`, `formants`, `speaker_blends` and
+        `breaks`; a batch mixing laws runs one conversion per law."""
         o = _batch_options(self, len(batches), [len(b) for b in batches], configs, seeds=seeds,
                            output_rates=output_rates, loudness=loudness, law=law, gains=gains, pitches=pitches,
-                           tempos=tempos, formants=formants, speaker_blends=speaker_blends, g711=True)
+                           tempos=tempos, formants=formants, speaker_blends=speaker_blends, breaks=breaks, g711=True)
         return self._encode_batch(batches, o)
 
     def speak_batch_g711(self, phoneme_batches: Sequence[str], law,
@@ -1005,27 +1117,28 @@ class _VitsCommons:
                          output_rates: Optional[Sequence] = None, loudness: Optional[Sequence] = None,
                          gains: Optional[Sequence] = None, pitches: Optional[Sequence] = None,
                          tempos: Optional[Sequence] = None, formants: Optional[Sequence] = None,
-                         speaker_blends: Optional[Sequence] = None) -> List[bytes]:
-        """speak_batch delivered as G.711 bytes: infer_batch_g711 over the phonemes' ids."""
+                         speaker_blends: Optional[Sequence] = None, breaks: Optional[Sequence] = None) -> List[bytes]:
+        """speak_batch delivered as G.711 bytes: infer_batch_g711 over the phonemes' ids (`breaks`: one per phoneme
+        character, as for speak_batch_with_alignment)."""
         o = _batch_options(self, len(phoneme_batches), None, configs, seeds=seeds, output_rates=output_rates,
                            loudness=loudness, law=law, gains=gains, pitches=pitches, tempos=tempos, formants=formants,
-                           speaker_blends=speaker_blends, g711=True)
-        return self._encode_batch([self.phonemes_to_input_ids(p) for p in phoneme_batches], o)
+                           speaker_blends=speaker_blends, breaks=breaks, g711=True)
+        return self._encode_batch(self._phoneme_ids(phoneme_batches, o), o)
 
     def infer_batch_flac(self, batches: Sequence[Sequence[int]],
                          configs: Optional[Sequence[PiperSynthesisConfig]] = None, seeds: Optional[Sequence] = None,
                          output_rates: Optional[Sequence] = None, loudness: Optional[Sequence] = None,
                          gains: Optional[Sequence] = None, pitches: Optional[Sequence] = None,
                          tempos: Optional[Sequence] = None, formants: Optional[Sequence] = None,
-                         speaker_blends: Optional[Sequence] = None) -> List[bytes]:
+                         speaker_blends: Optional[Sequence] = None, breaks: Optional[Sequence] = None) -> List[bytes]:
         """infer_batch_with_values delivered as lossless FLAC: one complete stream (`bytes`) per utterance.  Its samples
         are exactly the 16-bit samples the i16 route gives (SynthesisJob.fetch_i16): to_i16_vec of the utterance after
         gains[b] (None: 1), or the fixed scale for an utterance with a loudness target, at its delivered rate.  They are
         encoded on the device, and only the compressed bytes leave the card.  `configs`, `seeds`, `output_rates`,
-        `loudness`, `pitches`, `tempos`, `formants` and `speaker_blends` as for infer_batch_with_values."""
+        `loudness`, `pitches`, `tempos`, `formants`, `speaker_blends` and `breaks` as for infer_batch_with_values."""
         o = _batch_options(self, len(batches), [len(b) for b in batches], configs, seeds=seeds,
                            output_rates=output_rates, loudness=loudness, gains=gains, pitches=pitches, tempos=tempos,
-                           formants=formants, speaker_blends=speaker_blends)
+                           formants=formants, speaker_blends=speaker_blends, breaks=breaks)
         return self._encode_batch(batches, o)
 
     def speak_batch_flac(self, phoneme_batches: Sequence[str],
@@ -1033,12 +1146,21 @@ class _VitsCommons:
                          output_rates: Optional[Sequence] = None, loudness: Optional[Sequence] = None,
                          gains: Optional[Sequence] = None, pitches: Optional[Sequence] = None,
                          tempos: Optional[Sequence] = None, formants: Optional[Sequence] = None,
-                         speaker_blends: Optional[Sequence] = None) -> List[bytes]:
-        """speak_batch delivered as FLAC streams: infer_batch_flac over the phonemes' ids."""
+                         speaker_blends: Optional[Sequence] = None, breaks: Optional[Sequence] = None) -> List[bytes]:
+        """speak_batch delivered as FLAC streams: infer_batch_flac over the phonemes' ids (`breaks`: one per phoneme
+        character, as for speak_batch_with_alignment)."""
         o = _batch_options(self, len(phoneme_batches), None, configs, seeds=seeds, output_rates=output_rates,
                            loudness=loudness, gains=gains, pitches=pitches, tempos=tempos, formants=formants,
-                           speaker_blends=speaker_blends)
-        return self._encode_batch([self.phonemes_to_input_ids(p) for p in phoneme_batches], o)
+                           speaker_blends=speaker_blends, breaks=breaks)
+        return self._encode_batch(self._phoneme_ids(phoneme_batches, o), o)
+
+    def _phoneme_ids(self, phoneme_batches: Sequence[str], o: _BatchOptions) -> list:
+        """The ids of each phoneme string; with per-character controls in `o`, mapped so o gets their per-id images."""
+        if not o.per_character:
+            return [self.phonemes_to_input_ids(p) for p in phoneme_batches]
+        maps = [self.phonemes_to_input_ids_map(p) for p in phoneme_batches]
+        o.map_characters(phoneme_batches, maps)
+        return [ids for ids, _ in maps]
 
     def _encode_batch(self, batches, o: _BatchOptions) -> List[bytes]:
         """The G.711 bytes (when o has laws) or FLAC streams of `batches` with options `o`: one SynthesisJob run, then
@@ -1195,10 +1317,15 @@ class ProsodyStream:
 
     `volume`: one volume level in dB per id of `enc` (values as for infer_batch_with_values' volume_contours), applied
     on top of the rest, or alone when it asks for nothing (sb200_prosody_stream_create_volume): each sample the stream
-    emits is scaled at its delivered position, holding nothing back."""
+    emits is scaled at its delivered position, holding nothing back.
+
+    `breaks`: one pause in ms per id of `enc` (values as for infer_batch_with_values' breaks), inserted after that id,
+    on top of the rest or alone (sb200_prosody_stream_create_breaks): each chunk emits the pauses its input reaches,
+    holding nothing back, and `bounds` then holds each id's delivered end after the pauses before it.  The stream must
+    be fed exactly enc's chunks."""
 
     def __init__(self, model: "_VitsCommons", pitch=None, tempo=None, pitch_contour=None,
-                 enc: Optional["EncoderOutputs"] = None, formant=None, volume=None):
+                 enc: Optional["EncoderOutputs"] = None, formant=None, volume=None, breaks=None):
         p, t = _prosody_arrays([pitch], [tempo], 1)
         phi = _stream_formant(formant, "stream")
         vol = None                      # the volume contour's per-id image
@@ -1206,6 +1333,11 @@ class ProsodyStream:
             if not isinstance(enc, EncoderOutputs) or enc._m is not model or not enc._h:
                 raise OperationError("a volume contour needs the EncoderOutputs of its sentence, from this model")
             vol = _volume_arrays([len(enc.p_duration)], [volume], ["stream"])
+        bk = None                       # the breaks' per-id image
+        if breaks is not None:
+            if not isinstance(enc, EncoderOutputs) or enc._m is not model or not enc._h:
+                raise OperationError("breaks need the EncoderOutputs of their sentence, from this model")
+            bk = _break_arrays([len(enc.p_duration)], [breaks], ["stream"])
         self._m, self._h = model, C.c_void_p()
         self.pitch = None if p is None else float(p[0])
         self.tempo = None if t is None else float(t[0])
@@ -1223,7 +1355,12 @@ class ProsodyStream:
         nan = float("nan")
         pv, tv = nan if p is None else float(p[0]), nan if t is None else float(t[0])
         err = N.sb200_error()
-        if vol is not None:
+        if bk is not None:
+            # any of the above with the breaks on top, or the breaks alone
+            _check(model._lib.sb200_prosody_stream_create_breaks(
+                model._h, enc._h, pv, _ptr(c, C.c_float), bk.size, tv, nan if phi is None else phi,
+                _ptr(vol, C.c_float), _ptr(bk, C.c_float), C.byref(self._h), C.byref(err)), err)
+        elif vol is not None:
             # any of the above with the volume contour on top, or the contour alone
             _check(model._lib.sb200_prosody_stream_create_volume(
                 model._h, enc._h, pv, _ptr(c, C.c_float), vol.size, tv, nan if phi is None else phi,
@@ -1240,9 +1377,10 @@ class ProsodyStream:
             raise OperationError("a prosody stream needs a pitch or a tempo ratio other than 1 (None, NaN or 1: none)")
         else:
             _check(model._lib.sb200_prosody_stream_create(model._h, pv, tv, C.byref(self._h), C.byref(err)), err)
-        if c is not None:
-            self.bounds = np.zeros(c.size, np.int64)
-            _check(model._lib.sb200_prosody_stream_bounds(self._h, _ptr(self.bounds, C.c_int64), c.size,
+        if c is not None or _breaks_ask(bk, model.audio_output_info().sample_rate):
+            n_ids = len(enc.p_duration)
+            self.bounds = np.zeros(n_ids, np.int64)
+            _check(model._lib.sb200_prosody_stream_bounds(self._h, _ptr(self.bounds, C.c_int64), n_ids,
                                                           C.byref(err)), err)
 
     def last_pass_ms(self) -> Tuple[float, float]:
@@ -1263,6 +1401,12 @@ class ProsodyStream:
         self._m._lib.sb200_prosody_stream_profile_volume(self._h, C.byref(f))
         return float(f.value)
 
+    def last_break_ms(self) -> float:
+        """The "break" device time (ms) of the last chunk pass this stream was in (0: its stage did not run)."""
+        f = C.c_float()
+        self._m._lib.sb200_prosody_stream_profile_breaks(self._h, C.byref(f))
+        return float(f.value)
+
     def __del__(self):
         try:
             if self._h:
@@ -1273,15 +1417,21 @@ class ProsodyStream:
 
 
 def _stream_prosody(model, pitch, tempo, pitch_contour=None, enc=None, formant=None,
-                    volume=None) -> Optional[ProsodyStream]:
+                    volume=None, breaks=None) -> Optional[ProsodyStream]:
     """A ProsodyStream for a stream with these ratios, or with this per-id contour of enc's sentence and the tempo, and
     the formant ratio, or None when nothing asks for anything.  A given contour makes a contoured stream (which has
     bounds) whenever the contour or the tempo asks for something; a contour of None / NaN / 1 only is no contour beside a
     pitch ratio, as in the batch calls, and with neither a pitch nor a tempo it leaves the plain stream, which has no
     bounds.  A formant ratio asks for something unless it equals the pitch ratio (1 without one): it then makes a
     formant-only stream of a plain one.  A volume contour that asks for something (see _volume_arrays) is carried on
-    top of the rest, or alone."""
+    top of the rest, or alone, and so are breaks of one sample or more (see _breaks_ask)."""
     p, t = _prosody_arrays([pitch], [tempo], 1)
+    if breaks is not None and _breaks_ask(_break_arrays([len(enc.p_duration)], [breaks], ["stream"]),
+                                          model.audio_output_info().sample_rate):
+        if pitch_contour is not None and _contour_arrays([len(enc.p_duration)], [pitch_contour], p, ["stream"]) is None \
+                and (p is not None or t is None):
+            pitch_contour = None
+        return ProsodyStream(model, pitch, tempo, pitch_contour, enc, formant, volume, breaks)
     if volume is not None and _volume_arrays([len(enc.p_duration)], [volume], ["stream"]) is not None:
         if pitch_contour is not None and _contour_arrays([len(enc.p_duration)], [pitch_contour], p, ["stream"]) is None \
                 and (p is not None or t is None):
@@ -1389,7 +1539,7 @@ def refuse_live_loudness(live_loudness, where: str) -> None:
 
 
 def _delivered_bounds(warp: Optional[ProsodyStream], resampler: Optional["Resampler"]):
-    """A contoured stream's per-id delivered ends at its delivered rate: ceil(end * up / down) with an output rate, as
+    """A contoured stream's (or one with breaks) per-id delivered ends at its delivered rate: ceil(end * up / down) with an output rate, as
     the batch alignments place them; None for a stream without a contour."""
     if warp is None or warp.bounds is None:
         return None
@@ -1627,7 +1777,8 @@ class VitsStreamingModel(_VitsCommons):
                          pitch_contour: Optional[Sequence] = None,
                          formant_ratio: Optional[float] = None, speaker_blend=None,
                          live_loudness=None, max_gain_db: Optional[float] = None,
-                         volume_contour: Optional[Sequence] = None) -> SpeechStreamer:
+                         volume_contour: Optional[Sequence] = None,
+                         breaks: Optional[Sequence] = None) -> SpeechStreamer:
         """`formant_ratio`: as for infer_batch_with_values' formants, on top of `pitch` / `tempo` / `pitch_contour` or
         alone, the sentence's formant stage carried as one stream on the device (ProsodyStream): the concatenation of
         the chunks is the formant stage applied at once to the sentence the stream yields without it, then resampled and
@@ -1652,8 +1803,13 @@ class VitsStreamingModel(_VitsCommons):
         `volume_contour`: one volume level per character of `phonemes` (as for speak_batch_with_alignment's
         volume_contours), applied to that character's id and pad, on top of the rest or alone (ProsodyStream): the
         concatenation of the chunks is the sentence the stream yields without it with that contour applied at once,
-        before resampling, metering and encoding.  It holds nothing back."""
+        before resampling, metering and encoding.  It holds nothing back.
+        `breaks`: one pause in ms per character of `phonemes` (as for speak_batch_with_alignment's breaks), on top of
+        the rest or alone (ProsodyStream): the concatenation of the chunks is the sentence the stream yields without
+        them with those pauses inserted at once, before resampling, metering and encoding.  A chunk emits the pauses its
+        input reaches, holding nothing back, and the streamer's `bounds` give each id's delivered end."""
         if not isinstance(self, VitsStreamingModel):
+            refuse_breaks(breaks, "stream_synthesis")
             refuse_volume(volume_contour, "stream_synthesis")
             refuse_live_loudness(live_loudness, "stream_synthesis")
             refuse_formants(formant_ratio, "stream_synthesis")
@@ -1662,7 +1818,7 @@ class VitsStreamingModel(_VitsCommons):
         o = _stream_options(self, "stream_synthesis", None, phonemes, seed=seed, output_rate=output_rate,
                             encoding=encoding, gain=gain, pitch=pitch, tempo=tempo, pitch_contour=pitch_contour,
                             formant_ratio=formant_ratio, speaker_blend=speaker_blend, live_loudness=live_loudness,
-                            max_gain_db=max_gain_db, volume_contour=volume_contour)
+                            max_gain_db=max_gain_db, volume_contour=volume_contour, breaks=breaks)
         if o.seed is None and o.blend is None:
             enc = self.infer_encoder(o.ids)
         else:
@@ -1708,15 +1864,16 @@ class _StreamOptions:
     live_loudness: object               # None, a target in LUFS or a LoudnessStream to continue
     max_gain_db: Optional[float]
     volume: Optional[Sequence] = None   # per id
+    breaks: Optional[Sequence] = None   # per id
 
 
 def _stream_options(model, where: str, key: Optional[int], ids_or_phonemes, config=None, chunk_size=None,
                     chunk_padding=None, seed=None, output_rate=None, encoding=None, gain=None, pitch=None, tempo=None,
                     pitch_contour=None, formant_ratio=None, speaker_blend=None, live_loudness=None, max_gain_db=None,
-                    carried=(), volume_contour=None) -> _StreamOptions:
+                    carried=(), volume_contour=None, breaks=None) -> _StreamOptions:
     """The options of one stream of `model`, checked in one order: config, live loudness, speaker blend, formant ratio,
     pitch and tempo, seed, output rate, FLAC (refused by the name `where`), encoding and gain, the config's speaker,
-    chunking, then the ids (phonemes are mapped), the contour and the volume contour.  Errors name "stream" (key None) or "stream {key}".
+    chunking, then the ids (phonemes are mapped), the contour, the volume contour and the breaks.  Errors name "stream" (key None) or "stream {key}".
     `chunk_size`: checked with `chunk_padding` when given.  `carried`: the LoudnessStreams the caller's unfinished
     streams carry, which live_loudness may not be."""
     if config is not None and not isinstance(config, PiperSynthesisConfig):
@@ -1738,14 +1895,17 @@ def _stream_options(model, where: str, key: Optional[int], ids_or_phonemes, conf
         raise OperationError(f"No speaker was found with the given id `{config.speaker}`")     # as check_config
     if chunk_size is not None:
         _check_chunking(chunk_size, chunk_padding)
-    contour, volume = pitch_contour, volume_contour
-    if isinstance(ids_or_phonemes, str) and (pitch_contour is not None or volume_contour is not None):
+    contour, volume, brk = pitch_contour, volume_contour, breaks
+    if isinstance(ids_or_phonemes, str) and (pitch_contour is not None or volume_contour is not None or
+                                             breaks is not None):
         ids, src = model.phonemes_to_input_ids_map(ids_or_phonemes)
         if pitch_contour is not None:
             contour = _char_values_to_ids(pitch_contour, ids_or_phonemes, src, who, "pitch ratios", _contour_value)
         if volume_contour is not None:
             volume = _char_values_to_ids(volume_contour, ids_or_phonemes, src, who, "volume levels", _volume_value,
                                          0.0)
+        if breaks is not None:
+            brk = _char_breaks_to_ids(breaks, ids_or_phonemes, src, who)
     elif isinstance(ids_or_phonemes, str):
         ids = model.phonemes_to_input_ids(ids_or_phonemes)
     else:
@@ -1754,16 +1914,18 @@ def _stream_options(model, where: str, key: Optional[int], ids_or_phonemes, conf
         _contour_arrays([len(ids)], [contour], pit, [who])
     if volume is not None:
         _volume_arrays([len(ids)], [volume], [who])
+    if brk is not None:
+        _break_arrays([len(ids)], [brk], [who])
     if not ids:
         raise OperationError("Failed to run model inference. Error: empty input sequence")
     return _StreamOptions(key, who, ids, config, chunk_size, seed, output_rate, encoding, g, pitch, tempo, contour, phi,
-                          speaker_blend, live_loudness, max_gain_db, volume)
+                          speaker_blend, live_loudness, max_gain_db, volume, brk)
 
 
 def _open_stream(model, o: _StreamOptions, enc):
     """(resampler, ProsodyStream, meter) of a stream with options `o` and latent `enc`, each None when not asked for."""
     return (_stream_resampler(model, o.output_rate),
-            _stream_prosody(model, o.pitch, o.tempo, o.contour, enc, o.formant, o.volume),
+            _stream_prosody(model, o.pitch, o.tempo, o.contour, enc, o.formant, o.volume, o.breaks),
             _stream_meter(model, o.live_loudness, o.max_gain_db, o.output_rate, o.who))
 
 
@@ -1799,7 +1961,7 @@ class StreamBatch:
             pitch: Optional[float] = None, tempo: Optional[float] = None,
             pitch_contour: Optional[Sequence] = None, formant_ratio: Optional[float] = None,
             speaker_blend=None, live_loudness=None, max_gain_db: Optional[float] = None,
-            volume_contour: Optional[Sequence] = None) -> int:
+            volume_contour: Optional[Sequence] = None, breaks: Optional[Sequence] = None) -> int:
         """`seed`: the stream's noise seed (see infer_batch_with_values); a seeded stream yields what
         `stream_synthesis(..., seed=seed)` yields, whatever other streams share its encoder pass.  `output_rate`,
         `encoding` and `gain`: the stream's sample rate and G.711 encoding, as for stream_synthesis; `pitch` / `tempo`:
@@ -1814,26 +1976,30 @@ class StreamBatch:
         unfinished stream of this batch already carries is refused.  Metered streams go through passes of their own,
         so the other streams keep their passes and their bits.  `volume_contour`: one volume level per phoneme
         character (phonemes) or per id (ids), as for stream_synthesis; checked here, naming the stream.  A stream with
-        one goes through the warped passes."""
+        one goes through the warped passes.  `breaks`: one pause in ms per phoneme character (phonemes) or per id
+        (ids), as for stream_synthesis; checked here, naming the stream.  A stream with pauses goes through the warped
+        passes, and `bounds(key)` gives its per-id delivered ends once it is encoded."""
         if not isinstance(self.model, VitsStreamingModel):
+            refuse_breaks(breaks, "StreamBatch")
             refuse_volume(volume_contour, "StreamBatch")
             refuse_live_loudness(live_loudness, "StreamBatch")
             refuse_formants(formant_ratio, "StreamBatch")
             refuse_prosody(pitch, tempo, "StreamBatch")
             refuse_contour(pitch_contour, "StreamBatch")
         return self._add(ids_or_phonemes, config, self.chunk_size, seed, output_rate, encoding, gain, pitch, tempo,
-                         pitch_contour, speaker_blend, formant_ratio, live_loudness, max_gain_db, volume_contour)
+                         pitch_contour, speaker_blend, formant_ratio, live_loudness, max_gain_db, volume_contour, breaks)
 
     def _add(self, ids_or_phonemes, config, chunk_size: int, seed: Optional[int] = None,
              output_rate: Optional[int] = None, encoding: Optional[str] = None, gain: Optional[float] = None,
              pitch: Optional[float] = None, tempo: Optional[float] = None, pitch_contour=None,
-             speaker_blend=None, formant_ratio=None, live_loudness=None, max_gain_db=None, volume_contour=None) -> int:
+             speaker_blend=None, formant_ratio=None, live_loudness=None, max_gain_db=None, volume_contour=None,
+             breaks=None) -> int:
         carried = [o.live_loudness for o in self._pending] + [s.meter for s in self._active]
         o = _stream_options(self.model, "StreamBatch", self._next_key, ids_or_phonemes, config, chunk_size,
                             self.chunk_padding, seed=seed, output_rate=output_rate, encoding=encoding, gain=gain,
                             pitch=pitch, tempo=tempo, pitch_contour=pitch_contour, formant_ratio=formant_ratio,
                             speaker_blend=speaker_blend, live_loudness=live_loudness, max_gain_db=max_gain_db,
-                            carried=carried, volume_contour=volume_contour)
+                            carried=carried, volume_contour=volume_contour, breaks=breaks)
         self._next_key += 1
         self._pending.append(o)
         return o.key
