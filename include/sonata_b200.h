@@ -413,6 +413,45 @@ int32_t sb200_speak_batch_ids_breaks(sb200_voice* v, const int64_t* ids_packed, 
                                      const float* breaks_ms_packed, sb200_audio* outs, int32_t* id_frames_out,
                                      int64_t* bounds_out, double* lufs_out, float* gain_out, sb200_error* err);
 
+/* ---- target durations: fit an utterance, or spans of it, to a duration in milliseconds ----
+ * A target table gives utterance b the spans k in [fit_offsets[b], fit_offsets[b + 1]) (fit_offsets: batch + 1
+ * entries from 0, as blend_offsets): ids [fit_first[k], fit_end[k]) of the utterance (0-based, end exclusive) and the
+ * duration fit_ms[k] they should take.  A whole utterance is the span [0, n_ids), bos and eos included.  Spans must be
+ * non-empty, inside the utterance, ascending and disjoint, and fit_ms finite in (0, 600000], or NaN for a span that
+ * asks for nothing; any other entry fails with OPERATION_ERROR naming the utterance and the span, before any device
+ * work, as does a span that asks on an utterance with a tempo ratio (the two set the same length).  Solving span S at
+ * the voice's rate R:
+ *  1. T = floor(ms R / 1000 + 0.5) samples, in double.
+ *  2. P = the break samples of S's ids (step 1 of sb200_speak_batch_ids_breaks: a pause belongs to the id it follows).
+ *  3. Each predicted id i of S gets c_i(u) = ceil(w_i u) frames for an f32 factor u, where w_i = (exp(logw_i)
+ *     length_scale) scale_i is rounded exactly as without a target, and the multiply by u is one more f32 multiply,
+ *     applied last.  An id with a fixed count (frames_packed >= 0) keeps it; counts saturate at INT_MAX.
+ *  4. L(u) = 256 sum c_i(u) + P samples (the hop times S's frames), in int64.
+ *  5. u* is the largest f32 u in [0.5, 2] with L(u) <= T: the longest delivery that does not overrun the slot.  When
+ *     even L(0.5) > T, u* = 0.5 and the span is over its target.  Every c_i is nondecreasing in u, so u* is unique and
+ *     any u of its plateau gives the same counts.  A span without a predicted id asks for nothing (u* = 1).
+ * Ids outside every span keep their counts; without a span that asks, nothing is multiplied, launched or copied, and
+ * every bit is that of a call without targets.  u* is found on the device between the duration predictor and the
+ * durations' scan (one warp per span, bisection over the f32 bit patterns of [0.5, 2]: at most 25 integer sums), so a
+ * fitted utterance has the bits of the same utterance run with frames_packed fixed to its fitted counts, in any batch.
+ * Everything after the durations composes as it does with fixed counts: pitch ratios and contours, formants, volume,
+ * breaks, output rates, loudness, G.711 and FLAC; the delivered ends are what bounds_out reports.  fit_factor_out /
+ * fit_len_out (per span, either may be NULL) receive u* and L(u*) in samples at R (NaN and -1 for a span that asks
+ * nothing).  The executable specification is tests/fit_reference.py.  Realtime streams are fitted in their encoder
+ * pass (sb200_encode_batch_ids_targets).  sb200_speak_batch_ids_breaks with a target table (NULL fit_offsets: none);
+ * NULL is that call, bit for bit. */
+int32_t sb200_speak_batch_ids_fit(sb200_voice* v, const int64_t* ids_packed, const size_t* offsets, size_t batch,
+                                  const sb200_synth_config* cfgs, const float* scale_packed,
+                                  const int32_t* frames_packed, const uint64_t* seeds, const int32_t* seeded,
+                                  const uint32_t* output_rates, const float* target_lufs, const float* pitch,
+                                  const float* tempo, const float* pitch_packed, const float* formants,
+                                  const int64_t* blend_speakers, const float* blend_weights,
+                                  const size_t* blend_offsets, const float* volume_db_packed,
+                                  const float* breaks_ms_packed, const int64_t* fit_first, const int64_t* fit_end,
+                                  const float* fit_ms, const size_t* fit_offsets, sb200_audio* outs,
+                                  int32_t* id_frames_out, int64_t* bounds_out, double* lufs_out, float* gain_out,
+                                  float* fit_factor_out, int64_t* fit_len_out, sb200_error* err);
+
 /* ---- job API: the same batched pass split into its host<->device steps (bench / multi-GPU plumbing) ----
  * create  : copies ids to the device (H2D).  `eps_w` / `eps_z` optionally inject the graph's two
  *           RandomNormalLike draws (time-major: eps_w[b] = f32[T_x][2], eps_z[b] = f32[T_y][inter]);
@@ -490,6 +529,16 @@ int32_t sb200_job_set_volume_contour(sb200_job* job, const float* volume_db_pack
  * host, and sb200_job_profile reports the stage as the region "break".  The result's lengths, offsets and
  * sb200_job_prosody_bounds count the pauses. */
 int32_t sb200_job_set_breaks(sb200_job* job, const float* breaks_ms_packed, sb200_error* err);
+/* Target durations (see sb200_speak_batch_ids_fit) for the next sb200_job_run, or NULL fit_offsets for none (what a new
+ * job starts with; so is a table whose spans all ask nothing).  A bad entry fails with OPERATION_ERROR naming the
+ * utterance and the span, and leaves the job's targets as they were.  A run with targets reports the fit as the
+ * profile region "fit" and, with debug set, keeps each span's predicted w_i fetchable as "fit.w" (X level, one column;
+ * rows outside the spans and of fixed ids are not written). */
+int32_t sb200_job_set_targets(sb200_job* job, const int64_t* fit_first, const int64_t* fit_end, const float* fit_ms,
+                              const size_t* fit_offsets, sb200_error* err);
+/* u* and L(u*) of every span of the last run's targets, packed as the table (capacity: its spans; either may be NULL);
+ * fails when the last run had none. */
+int32_t sb200_job_targets(const sb200_job* job, float* fit_factor, int64_t* fit_len, size_t capacity, sb200_error* err);
 /* Speaker blends (see sb200_speak_batch_ids_blends) for the next sb200_job_run as a blend table, or NULL offsets for none
  * (what a new job starts with).  Every entry is checked first; a bad one fails with OPERATION_ERROR naming the utterance
  * and leaves the job's blends as they were. */
@@ -599,6 +648,19 @@ int32_t sb200_encode_batch_ids_blends(sb200_voice* v, const int64_t* ids_packed,
                                       const int32_t* frames_packed, const uint64_t* seeds, const int32_t* seeded,
                                       const int64_t* blend_speakers, const float* blend_weights,
                                       const size_t* blend_offsets, sb200_latent** outs, sb200_error* err);
+/* sb200_encode_batch_ids_blends with a target table (see sb200_speak_batch_ids_fit; NULL fit_offsets: none, that call
+ * bit for bit): each latent's frames are fitted in the encoder pass, and its chunks then decode unchanged.
+ * breaks_ms_packed (NULL: none, checked as sb200_speak_batch_ids_breaks checks them) are the pauses the latents'
+ * prosody streams will insert; the fit counts them in P, and the pass inserts none.  fit_factor_out / fit_len_out as
+ * there. */
+int32_t sb200_encode_batch_ids_targets(sb200_voice* v, const int64_t* ids_packed, const size_t* offsets, size_t batch,
+                                       const sb200_synth_config* cfgs, const float* scale_packed,
+                                       const int32_t* frames_packed, const uint64_t* seeds, const int32_t* seeded,
+                                       const int64_t* blend_speakers, const float* blend_weights,
+                                       const size_t* blend_offsets, const float* breaks_ms_packed,
+                                       const int64_t* fit_first, const int64_t* fit_end, const float* fit_ms,
+                                       const size_t* fit_offsets, float* fit_factor_out, int64_t* fit_len_out,
+                                       sb200_latent** outs, sb200_error* err);
 /* The encoder's `p_duration` (piper/src/lib.rs:675, 706-717) as frames per id of the latent's utterance (their sum is
  * its frame count, except that an utterance whose ids all got 0 frames is 1 frame long).  Returns the number of ids;
  * writes them to out only when capacity is at least that (call with NULL, 0 to learn the size). */
@@ -986,6 +1048,13 @@ int32_t sb200_debug_volume(int32_t device, const float* x, size_t n, const int64
  * n) with a break of ms[i] after it (n_ids entries, checked as sb200_speak_batch_ids_breaks checks them): *n_out
  * receives the paused length and y[0 .. *n_out) the result (cap: y's room; too little fails after *n_out is set); bit
  * for bit what a job gives an utterance of those samples and ends. */
+/* The fit kernel over caller values: w[0 .. n) the ids' w_i, frames (NULL: all predicted) their fixed counts as
+ * frames_packed, and n_spans spans [first[k], end[k]) with budget[k] = floor((T - P) / 256) frames.  factor[0 .. n)
+ * receives the factor image (1 outside the spans), u_out / frames_out per span u* and its frames (L(u*) = 256 frames +
+ * P); any output may be NULL.  Bit for bit what the synthesis path's fit does with those w. */
+int32_t sb200_debug_fit(int32_t device, const float* w, size_t n, const int32_t* frames, const int64_t* first,
+                        const int64_t* end, const int64_t* budget, size_t n_spans, float* factor, float* u_out,
+                        int64_t* frames_out, sb200_error* err);
 int32_t sb200_debug_breaks(int32_t device, const float* x, size_t n, const int64_t* ends, const float* ms, size_t n_ids,
                            int32_t rate, float* y, size_t cap, int64_t* n_out, sb200_error* err);
 /* Test hook, no device needed: the samples a prosody stream with these ratios at `rate` emits per chunk (the rule of

@@ -325,15 +325,24 @@ static void job_prosody(const Job& j, int64_t* n1, int64_t* n2, int32_t* frames)
     }
 }
 
-int32_t sb200_speak_batch_ids_breaks(sb200_voice* v, const int64_t* ids, const size_t* offsets, size_t batch,
-                                     const sb200_synth_config* cfgs, const float* scale_packed,
-                                     const int32_t* frames_packed, const uint64_t* seeds, const int32_t* seeded,
-                                     const uint32_t* output_rates, const float* target_lufs, const float* pitch,
-                                     const float* tempo, const float* pitch_packed, const float* formants,
-                                     const int64_t* blend_speakers, const float* blend_weights,
-                                     const size_t* blend_offsets, const float* volume_db_packed,
-                                     const float* breaks_ms_packed, sb200_audio* outs, int32_t* id_frames_out,
-                                     int64_t* bounds_out, double* lufs_out, float* gain_out, sb200_error* err) {
+// u* and L(u*) of every span of a job's last run's targets (each may be null).
+static void job_targets(const Job& j, float* factor, int64_t* len) {
+    if (!j.ran || j.fit_u.empty()) throw Error(19, "the job's last run had no target durations");
+    if (factor) std::copy(j.fit_u.begin(), j.fit_u.end(), factor);
+    if (len) std::copy(j.fit_len.begin(), j.fit_len.end(), len);
+}
+
+int32_t sb200_speak_batch_ids_fit(sb200_voice* v, const int64_t* ids, const size_t* offsets, size_t batch,
+                                  const sb200_synth_config* cfgs, const float* scale_packed,
+                                  const int32_t* frames_packed, const uint64_t* seeds, const int32_t* seeded,
+                                  const uint32_t* output_rates, const float* target_lufs, const float* pitch,
+                                  const float* tempo, const float* pitch_packed, const float* formants,
+                                  const int64_t* blend_speakers, const float* blend_weights,
+                                  const size_t* blend_offsets, const float* volume_db_packed,
+                                  const float* breaks_ms_packed, const int64_t* fit_first, const int64_t* fit_end,
+                                  const float* fit_ms, const size_t* fit_offsets, sb200_audio* outs,
+                                  int32_t* id_frames_out, int64_t* bounds_out, double* lufs_out, float* gain_out,
+                                  float* fit_factor_out, int64_t* fit_len_out, sb200_error* err) {
     return guarded(err, [&] {
         const double t0 = now_ms();
         static_assert(sizeof(long long) == sizeof(int64_t), "");
@@ -350,6 +359,9 @@ int32_t sb200_speak_batch_ids_breaks(sb200_voice* v, const int64_t* ids, const s
                          "utterance");
         check_volume_contour(volume_db_packed, offsets, batch);
         check_breaks(breaks_ms_packed, offsets, batch);
+        const long long* ff = reinterpret_cast<const long long*>(fit_first);
+        const long long* fe = reinterpret_cast<const long long*>(fit_end);
+        const bool fit = check_targets(ff, fe, fit_ms, fit_offsets, offsets, batch, tempo);
         std::unique_ptr<Job> j(create_job(v->v.get(), reinterpret_cast<const long long*>(ids), offsets, batch, nullptr,
                                           nullptr, nullptr, false));
         if (cfgs) set_job_configs(*j, cfgs_in(cfgs, batch).data());
@@ -363,6 +375,7 @@ int32_t sb200_speak_batch_ids_breaks(sb200_voice* v, const int64_t* ids, const s
         set_job_blends(*j, reinterpret_cast<const long long*>(blend_speakers), blend_weights, blend_offsets);
         set_job_volume_contour(*j, volume_db_packed);
         set_job_breaks(*j, breaks_ms_packed);
+        set_job_targets(*j, ff, fe, fit_ms, fit_offsets);
         j->run(nullptr, 0);
         fetch_audio(*j, outs, 0.f);
         if (id_frames_out) {
@@ -374,10 +387,26 @@ int32_t sb200_speak_batch_ids_breaks(sb200_voice* v, const int64_t* ids, const s
             std::copy(e.begin(), e.end(), bounds_out);
         }
         if (loud) job_loudness(*j, lufs_out, gain_out);
+        if (fit) job_targets(*j, fit_factor_out, fit_len_out);
         const float wall = (float)(now_ms() - t0);
         for (size_t b = 0; b < batch; b++)
             outs[b].inference_ms = wall * (j->out_total ? (float)outs[b].len / (float)j->out_total : 0.f);
     });
+}
+int32_t sb200_speak_batch_ids_breaks(sb200_voice* v, const int64_t* ids, const size_t* offsets, size_t batch,
+                                     const sb200_synth_config* cfgs, const float* scale_packed,
+                                     const int32_t* frames_packed, const uint64_t* seeds, const int32_t* seeded,
+                                     const uint32_t* output_rates, const float* target_lufs, const float* pitch,
+                                     const float* tempo, const float* pitch_packed, const float* formants,
+                                     const int64_t* blend_speakers, const float* blend_weights,
+                                     const size_t* blend_offsets, const float* volume_db_packed,
+                                     const float* breaks_ms_packed, sb200_audio* outs, int32_t* id_frames_out,
+                                     int64_t* bounds_out, double* lufs_out, float* gain_out, sb200_error* err) {
+    return sb200_speak_batch_ids_fit(v, ids, offsets, batch, cfgs, scale_packed, frames_packed, seeds, seeded,
+                                     output_rates, target_lufs, pitch, tempo, pitch_packed, formants, blend_speakers,
+                                     blend_weights, blend_offsets, volume_db_packed, breaks_ms_packed, nullptr, nullptr,
+                                     nullptr, nullptr, outs, id_frames_out, bounds_out, lufs_out, gain_out, nullptr,
+                                     nullptr, err);
 }
 int32_t sb200_speak_batch_ids_volume(sb200_voice* v, const int64_t* ids, const size_t* offsets, size_t batch,
                                      const sb200_synth_config* cfgs, const float* scale_packed,
@@ -546,6 +575,22 @@ int32_t sb200_job_set_volume_contour(sb200_job* job, const float* volume_db_pack
 int32_t sb200_job_set_breaks(sb200_job* job, const float* breaks_ms_packed, sb200_error* err) {
     return guarded(err, [&] { set_job_breaks(*job->j, breaks_ms_packed); });
 }
+int32_t sb200_job_set_targets(sb200_job* job, const int64_t* fit_first, const int64_t* fit_end, const float* fit_ms,
+                              const size_t* fit_offsets, sb200_error* err) {
+    return guarded(err, [&] {
+        set_job_targets(*job->j, reinterpret_cast<const long long*>(fit_first),
+                        reinterpret_cast<const long long*>(fit_end), fit_ms, fit_offsets);
+    });
+}
+int32_t sb200_job_targets(const sb200_job* job, float* fit_factor, int64_t* fit_len, size_t capacity, sb200_error* err) {
+    return guarded(err, [&] {
+        const Job& j = *job->j;
+        if (j.ran && capacity < j.fit_u.size())
+            throw Error(19, "target durations: the destination holds " + std::to_string(capacity) + " spans, the job has " +
+                                std::to_string(j.fit_u.size()));
+        job_targets(j, fit_factor, fit_len);
+    });
+}
 int32_t sb200_job_set_speaker_blends(sb200_job* job, const int64_t* speakers, const float* weights, const size_t* offsets,
                                      sb200_error* err) {
     return guarded(err, [&] {
@@ -703,20 +748,36 @@ int32_t sb200_decode_chunk(sb200_voice* v, const sb200_latent* z, int64_t lo, in
 }
 void sb200_latent_free(sb200_latent* z) { delete z; }
 
+int32_t sb200_encode_batch_ids_targets(sb200_voice* v, const int64_t* ids, const size_t* offsets, size_t batch,
+                                       const sb200_synth_config* cfgs, const float* scale_packed,
+                                       const int32_t* frames_packed, const uint64_t* seeds, const int32_t* seeded,
+                                       const int64_t* blend_speakers, const float* blend_weights,
+                                       const size_t* blend_offsets, const float* breaks_ms_packed,
+                                       const int64_t* fit_first, const int64_t* fit_end, const float* fit_ms,
+                                       const size_t* fit_offsets, float* fit_factor_out, int64_t* fit_len_out,
+                                       sb200_latent** outs, sb200_error* err) {
+    return guarded(err, [&] {
+        const std::vector<SynthConfig> c = cfgs ? cfgs_in(cfgs, batch) : std::vector<SynthConfig>();
+        check_breaks(breaks_ms_packed, offsets, batch);
+        std::vector<Latent*> ls = encode_latents(v->v.get(), reinterpret_cast<const long long*>(ids), offsets, batch,
+                                                 cfgs ? c.data() : nullptr, scale_packed, frames_packed,
+                                                 reinterpret_cast<const unsigned long long*>(seeds), seeded,
+                                                 reinterpret_cast<const long long*>(blend_speakers), blend_weights,
+                                                 blend_offsets, breaks_ms_packed,
+                                                 reinterpret_cast<const long long*>(fit_first),
+                                                 reinterpret_cast<const long long*>(fit_end), fit_ms, fit_offsets,
+                                                 fit_factor_out, reinterpret_cast<long long*>(fit_len_out));
+        for (size_t b = 0; b < batch; b++) outs[b] = new sb200_latent{ls[b], v->v};
+    });
+}
 int32_t sb200_encode_batch_ids_blends(sb200_voice* v, const int64_t* ids, const size_t* offsets, size_t batch,
                                       const sb200_synth_config* cfgs, const float* scale_packed,
                                       const int32_t* frames_packed, const uint64_t* seeds, const int32_t* seeded,
                                       const int64_t* blend_speakers, const float* blend_weights,
                                       const size_t* blend_offsets, sb200_latent** outs, sb200_error* err) {
-    return guarded(err, [&] {
-        const std::vector<SynthConfig> c = cfgs ? cfgs_in(cfgs, batch) : std::vector<SynthConfig>();
-        std::vector<Latent*> ls = encode_latents(v->v.get(), reinterpret_cast<const long long*>(ids), offsets, batch,
-                                                 cfgs ? c.data() : nullptr, scale_packed, frames_packed,
-                                                 reinterpret_cast<const unsigned long long*>(seeds), seeded,
-                                                 reinterpret_cast<const long long*>(blend_speakers), blend_weights,
-                                                 blend_offsets);
-        for (size_t b = 0; b < batch; b++) outs[b] = new sb200_latent{ls[b], v->v};
-    });
+    return sb200_encode_batch_ids_targets(v, ids, offsets, batch, cfgs, scale_packed, frames_packed, seeds, seeded,
+                                          blend_speakers, blend_weights, blend_offsets, nullptr, nullptr, nullptr,
+                                          nullptr, nullptr, nullptr, nullptr, outs, err);
 }
 int32_t sb200_encode_batch_ids_seeded(sb200_voice* v, const int64_t* ids, const size_t* offsets, size_t batch,
                                       const sb200_synth_config* cfgs, const float* scale_packed,
@@ -1243,6 +1304,35 @@ int32_t sb200_debug_durations(int32_t device, const float* z, int32_t rows, cons
         SB_CUDA(cudaMemcpy(logw, dlogw, (size_t)rows * 4, cudaMemcpyDeviceToHost));
         SB_CUDA(cudaMemcpy(cum, dcum, (size_t)rows * 4, cudaMemcpyDeviceToHost));
         SB_CUDA(cudaMemcpy(y_len, dylen, (size_t)nseg * 4, cudaMemcpyDeviceToHost));
+    });
+}
+
+int32_t sb200_debug_fit(int32_t device, const float* w, size_t n, const int32_t* frames, const int64_t* first,
+                        const int64_t* end, const int64_t* budget, size_t n_spans, float* factor, float* u_out,
+                        int64_t* frames_out, sb200_error* err) {
+    return guarded(err, [&] {
+        if (n == 0 || n > (size_t)INT_MAX || !w || (n_spans && (!first || !end || !budget)))
+            throw Error(19, "debug fit: bad arguments");
+        std::vector<FitSpan> spans(n_spans);
+        for (size_t k = 0; k < n_spans; k++) {
+            if (!(first[k] >= 0 && first[k] < end[k] && end[k] <= (int64_t)n))
+                throw Error(19, "debug fit: span " + std::to_string(k) + " is not a non-empty range of the ids");
+            spans[k] = FitSpan{(int)first[k], (int)(end[k] - first[k]), 0, (long long)budget[k]};
+        }
+        SB_CUDA(cudaSetDevice(device));
+        std::vector<float> ones(n, 1.f);
+        DeviceBuffers d;
+        float* dw = d.upload(w, n, n);
+        const int* df = frames ? d.upload(frames, n, n) : nullptr;
+        float* dfac = d.upload(ones.data(), n, n);
+        float* du = d.alloc<float>(std::max<size_t>(n_spans, 1));
+        long long* dfr = d.alloc<long long>(std::max<size_t>(n_spans, 1));
+        const FitSpan* ds = n_spans ? d.upload(spans.data(), n_spans, n_spans) : nullptr;
+        launch_fit(ds, (int)n_spans, nullptr, 0.f, 0.f, nullptr, nullptr, df, dw, dfac, du, dfr, 0);
+        SB_CUDA(cudaDeviceSynchronize());
+        if (factor) SB_CUDA(cudaMemcpy(factor, dfac, n * 4, cudaMemcpyDeviceToHost));
+        if (n_spans && u_out) SB_CUDA(cudaMemcpy(u_out, du, n_spans * 4, cudaMemcpyDeviceToHost));
+        if (n_spans && frames_out) SB_CUDA(cudaMemcpy(frames_out, dfr, n_spans * 8, cudaMemcpyDeviceToHost));
     });
 }
 

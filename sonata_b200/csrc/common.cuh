@@ -10,6 +10,7 @@
 // buffers untouched there), which keeps that invariant without memsets.
 #pragma once
 #include <cuda_runtime.h>
+#include <climits>
 #include <stdint.h>
 #include <stdlib.h>
 #include <mutex>
@@ -180,9 +181,36 @@ void launch_spline(const float* h29, int ldh, float* z, int tcol, int bins, floa
                    RowMap map, cudaStream_t st);
 // logw = (z[:,0]-m0)*exp(-logs0); w = exp(logw)*length_scale[b]; w_ceil; per-segment inclusive scan.  Optional per-id
 // controls at the id level (null: none): w_ceil = ceil(w * dur_scale[r]), and dur_frames[r] >= 0 replaces w_ceil.
+// fit (null: none) is the fit's per-id factor image: w_ceil = ceil(w * fit[r]), one more f32 multiply applied last.
 void launch_durations(const float* z, float m0, float logs0, const float* length_scale, const SegInfo* segs, int nseg,
                       float* logw, int* cum, int* y_len, cudaStream_t st, const float* dur_scale = nullptr,
-                      const int* dur_frames = nullptr);
+                      const int* dur_frames = nullptr, const float* fit = nullptr);
+// An id's predicted duration before its ceil: logw = (z[row][0] - m0) * exp(-logs0) (einv), then
+// w = (exp(logw) * length_scale) * dur_scale[row], each product rounded in that order (no dur_scale: no multiply).
+// durations_kernel and fit_kernel both round w here, so the fit searches the very values the scan rounds up.
+__device__ __forceinline__ float dur_logw(const float* z, int row, float m0, float einv) { return (z[2 * row] - m0) * einv; }
+__device__ __forceinline__ float dur_weight(float lw, float length_scale, const float* dur_scale, int row) {
+    float wf = expf(lw) * length_scale;
+    if (dur_scale) wf = wf * dur_scale[row];
+    return wf;
+}
+// ceil(w) as a frame count, saturating at INT_MAX (NaN and inf too).
+__device__ __forceinline__ long long dur_count(float wf) {
+    const float wc = ceilf(wf);
+    return wc < 2147483648.f ? (long long)(int)wc : (long long)INT_MAX;
+}
+// Target durations (fit.cu; include/sonata_b200.h, sb200_speak_batch_ids_fit).  One span of one utterance: X rows
+// [row0, row0 + len), its utterance `seg` (whose length scale it reads) and the most frames its ids may take,
+// budget = floor((T - P) / hop).
+struct FitSpan { int row0, len, seg; long long budget; };
+// One warp per span.  With z, each predicted id's w (dur_weight) is computed and written to w[row]; without z, w holds
+// the caller's values.  Then u* = the largest f32 u in [0.5, 2] with sum of ceil(w u) (plus the fixed counts of
+// dur_frames) <= budget, or 0.5 when none fits, found by bisection over the f32 bit patterns; a span without a
+// predicted id gets u = 1.  factor[row] = u* over the span's rows, u_out[k] = u*, frames_out[k] = the span's frames at
+// u*.  dur_scale / dur_frames: as for launch_durations (null: none).
+void launch_fit(const FitSpan* spans, int nspans, const float* z, float m0, float logs0, const float* length_scales,
+                const float* dur_scale, const int* dur_frames, float* w, float* factor, float* u_out,
+                long long* frames_out, cudaStream_t st);
 struct FrameSeg { int off; int len; int xoff; int xlen; long long out_off; };
 // z_p rows: gather m_p/logs_p of the token whose cumulative duration covers the frame, add noise scaled by the noise_scale
 // of the frame's segment (ftile_seg)

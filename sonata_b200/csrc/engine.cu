@@ -312,6 +312,14 @@ void set_job_loudness(Job& j, const float* targets) {
 void set_job_prosody(Job& j, const float* pitch, const float* tempo) {
     const bool any = check_prosody(pitch, tempo, j.B);
     if (!j.contour.empty()) check_pitch_contour(j.contour.data(), j.offs.data(), j.B, pitch);
+    if (!j.targets.empty()) {
+        std::vector<long long> first(j.targets.size()), end(j.targets.size());
+        std::vector<float> ms(j.targets.size());
+        for (size_t k = 0; k < j.targets.size(); k++) {
+            first[k] = j.targets[k].first; end[k] = j.targets[k].end; ms[k] = j.targets[k].ms;
+        }
+        check_targets(first.data(), end.data(), ms.data(), j.target_offs.data(), j.offs.data(), j.B, tempo);
+    }
     if (!any) { j.pitch.clear(); j.tempo.clear(); return; }
     const std::vector<float> none(j.B, NAN);
     j.pitch.assign(pitch ? pitch : none.data(), (pitch ? pitch : none.data()) + j.B);
@@ -491,6 +499,9 @@ struct IdBufs {
     float *att_s, *att_vt, *att_orel;          // tensor-core attention: scores of every head, V^T, relative-value term
     float* epsw;
     Staged<float> dscale; Staged<int> dframes; // per-id duration controls (only when the job has them)
+    // target fit (only when a span asks): the spans, the per-id factor image (1 outside the spans), w, and per span u*
+    // and its frames
+    Staged<FitSpan> fspans; Staged<float> fitu; float* fitw = nullptr; Staged<float> fit_uo; Staged<long long> fit_fo;
     Staged<NoiseSeed> seeds;                   // per utterance (only when the job has seeds; read at both levels)
     float *qkv0, *att0, *p0, *vt0;             // debug: layer 0's attention operands and result
     std::vector<std::array<float*, 4>> dpf;    // debug: each duration flow's input, DDSConv output, spline parameters, output
@@ -499,7 +510,7 @@ struct IdBufs {
     enum { ENC_QKV, ENC_VT, ENC_ATT, ENC_O, ENC_LN1, ENC_FFN1, ENC_FFN2, ENC_LN2, ENC_NCAP };
     std::vector<std::array<float*, ENC_NCAP>> encl;
 
-    void carve(Arena& dev, Arena& pin, const Job& j, bool tc_att, size_t n_simt) {
+    void carve(Arena& dev, Arena& pin, const Job& j, bool tc_att, size_t n_simt, size_t n_fit) {
         const Voice& v = *j.v; const Arch& a = v.a;
         const int RX = j.RX, nxg = RX / GX, H = a.hidden;
         const size_t B = j.B, ntiles = j.tiles_s.size() + j.tiles_o.size();
@@ -522,6 +533,11 @@ struct IdBufs {
         epsw = any_noise_w ? rows(2) : nullptr;
         if (!j.dur_scale.empty()) dscale.carve(dev, pin, RX);
         if (!j.dur_frames.empty()) dframes.carve(dev, pin, RX);
+        fitw = nullptr;
+        if (n_fit) {
+            fspans.carve(dev, pin, n_fit); fitu.carve(dev, pin, RX); fitw = rows(1);
+            fit_uo.carve(dev, pin, n_fit); fit_fo.carve(dev, pin, n_fit);
+        }
         if (!j.seeds.empty()) seeds.carve(dev, pin, B);
         qkv0 =att0 = p0 = vt0 = nullptr;
         emb0 = nullptr;
@@ -854,8 +870,9 @@ void Job::run(float* d_out, size_t d_out_cap) {
         if (!(blends.empty() || blends[b].s.empty() ? assign_slot(frames, V, cfgs[b].has_speaker ? cfgs[b].speaker : 0)
                                                     : assign_slot(frames, V, blends[b])))
             throw Error(19, "Failed to run model inference. Error: speaker id out of range (utterance " + std::to_string(b) + ")");
+    const FitPlan fp = fit_plan(*this);
     IdBufs x;
-    plan(C.dev_id, C.pin, [&](Arena& dev, Arena& pin) { x.carve(dev, pin, *this, tc_att, simt_segs.size()); });
+    plan(C.dev_id, C.pin, [&](Arena& dev, Arena& pin) { x.carve(dev, pin, *this, tc_att, simt_segs.size(), fp.spans.size()); });
     d_cum = x.cum;
     Runner R(V, C, regions, x.spk.cond);
 
@@ -891,6 +908,12 @@ void Job::run(float* d_out, size_t d_out_cap) {
     };
     per_id(x.dscale, dur_scale, 1.f);
     per_id(x.dframes, dur_frames, -1);
+    if (x.fspans.d) {
+        std::copy(fp.spans.begin(), fp.spans.end(), x.fspans.h);
+        x.fspans.upload(st);
+        std::fill(x.fitu.h, x.fitu.h + RX, 1.f);
+        x.fitu.upload(st);
+    }
     if (x.seeds.d) {
         std::copy(seeds.begin(), seeds.end(), x.seeds.h);
         x.seeds.upload(st);
@@ -925,6 +948,7 @@ void Job::run(float* d_out, size_t d_out_cap) {
             expose(*this, "vt0", x.vt0, H, -1);        // stored as [H][RX]
         }
         expose(*this, "dp.g", x.g, H, 0); expose(*this, "logw", x.logw, 1, 0);
+        if (x.fitw) expose(*this, "fit.w", x.fitw, 1, 0);    // w of the spans' predicted ids only
         for (size_t s = 0; s < x.dpf.size(); s++) {
             const std::string fs = "dp.f" + std::to_string(s) + ".";
             expose(*this, fs + "in", x.dpf[s][0], 2, 0); expose(*this, fs + "h", x.dpf[s][1], H, 0);
@@ -1044,15 +1068,34 @@ void Job::run(float* d_out, size_t d_out_cap) {
         R.count(0, 4.0 * LX.valid_rows * 34);
         if (debug) d2d(x.dpf[s][3], x.zz, (size_t)RX * 2, st);
     }
+    if (x.fspans.d) {
+        R.end();
+        R.begin("fit");
+        launch_fit(x.fspans.d, (int)fp.spans.size(), x.zz, V.ea_m0, V.ea_logs0, x.scales.d + B, x.dscale.d, x.dframes.d,
+                   x.fitw, x.fitu.d, x.fit_uo.d, x.fit_fo.d, st);
+        // up to 26 passes over each span id, reading its w and its fixed count
+        { double n = 0; for (const FitSpan& q : fp.spans) n += q.len; R.count(0, 26.0 * 8.0 * n); }
+        R.end();
+        R.begin("dp");
+    }
     launch_durations(x.zz, V.ea_m0, V.ea_logs0, x.scales.d + B, x.xsegs.d, (int)B, x.logw, x.cum, x.ylen.d, st,
-                     x.dscale.d, x.dframes.d);
+                     x.dscale.d, x.dframes.d, x.fitu.d);
     R.end();
 
     // ---------------- host learns the frame counts (the graph's data-dependent shape) ----------------
     x.ylen.download(st);
+    if (x.fspans.d) { x.fit_uo.download(st); x.fit_fo.download(st); }
     if (x.cum_h) SB_CUDA(cudaMemcpyAsync(x.cum_h, x.cum, (size_t)RX * sizeof(int), cudaMemcpyDeviceToHost, st));
     SB_CUDA(cudaStreamSynchronize(st));
     y_len.assign(x.ylen.h, x.ylen.h + B);
+    fit_u.clear(); fit_len.clear();
+    if (!targets.empty()) {
+        fit_u.assign(targets.size(), NAN); fit_len.assign(targets.size(), -1);
+        for (size_t q = 0; q < fp.spans.size(); q++) {
+            fit_u[fp.index[q]] = x.fit_uo.h[q];
+            fit_len[fp.index[q]] = (long long)a.hop() * x.fit_fo.h[q] + fp.pause[q];
+        }
+    }
     const std::vector<int> cum_host = x.cum_h ? std::vector<int>(x.cum_h, x.cum_h + RX) : std::vector<int>();
     long long tot_frames = 0;
     for (int y : y_len) tot_frames += y;
@@ -1158,14 +1201,24 @@ void Job::run(float* d_out, size_t d_out_cap) {
 std::vector<Latent*> encode_latents(Voice* v, const long long* ids, const size_t* offs, size_t B, const SynthConfig* cfgs,
                                     const float* scale, const int* frames, const unsigned long long* seeds,
                                     const int* seeded, const long long* blend_s, const float* blend_u,
-                                    const size_t* blend_offs) {
+                                    const size_t* blend_offs, const float* breaks, const long long* fit_first,
+                                    const long long* fit_end, const float* fit_ms, const size_t* fit_offs,
+                                    float* fit_u, long long* fit_len) {
     std::unique_ptr<Job> j(create_job(v, ids, offs, B, nullptr, nullptr, nullptr, false));
     if (cfgs) set_job_configs(*j, cfgs);
     set_job_durations(*j, scale, frames);
     set_job_seeds(*j, seeds, seeded);
     set_job_blends(*j, blend_s, blend_u, blend_offs);
+    set_job_targets(*j, fit_first, fit_end, fit_ms, fit_offs);
+    if (!j->targets.empty()) set_job_breaks(*j, breaks);    // only the fit reads them: an encoder pass inserts no pause
     j->encode_only = true;
     j->run(nullptr, 0);
+    if (fit_offs && fit_offs[B]) {
+        for (size_t k = 0; k < fit_offs[B]; k++) {
+            if (fit_u) fit_u[k] = j->fit_u.empty() ? NAN : j->fit_u[k];
+            if (fit_len) fit_len[k] = j->fit_len.empty() ? -1 : j->fit_len[k];
+        }
+    }
     const size_t I = (size_t)v->a.inter;
     size_t total = 0;
     for (int f : j->y_len) total += (size_t)f;

@@ -575,6 +575,10 @@ struct FrameLayout {
     }
 };
 
+// One span of a target table (include/sonata_b200.h, sb200_speak_batch_ids_fit): ids [first, end) of its utterance and
+// the duration in ms they should take (NaN: none).
+struct FitTarget { long long first, end; float ms; };
+
 struct Job {
     Voice* v = nullptr;
     Context* ctx = nullptr;
@@ -605,6 +609,10 @@ struct Job {
                                       // has a volume contour (set_job_volume_contour)
     std::vector<float> breaks;        // per-id pauses in ms, packed like ids, NaN or 0 = none; empty when no utterance
                                       // has one (set_job_breaks)
+    std::vector<FitTarget> targets;   // target durations: each utterance's spans, target_offs[b] .. target_offs[b + 1];
+    std::vector<size_t> target_offs;  // both empty when no span asks (set_job_targets)
+    std::vector<float> fit_u;         // per span of the last run's targets: u* and L(u*) in samples at the voice's
+    std::vector<long long> fit_len;   // rate (NaN and -1 for a span that asked nothing); empty when it had none
     std::vector<SpeakerBlend> blends; // one canonical blend per utterance (empty entry: the config's speaker); empty when
                                       // none has one (set_job_blends)
     std::vector<ProsodyShape> pros_ran;   // each utterance's shape in the last run (empty: it ran no prosody stage)
@@ -692,6 +700,26 @@ void set_job_volume_contour(Job& j, const float* packed);
 // the break stage after the volume stage, before any resampling and loudness, and its length, bounds and place in the
 // job's result count its pauses.
 void set_job_breaks(Job& j, const float* packed);
+// Target durations of the job's next run: spans [first[k], end[k]) of ids with ms[k] each, utterance b's spans being
+// k in [fit_offs[b], fit_offs[b + 1]), or null fit_offs for none; see check_targets.  A bad entry leaves the job's
+// targets as they were.  The run fits each span that asks between the duration predictor and the durations' scan
+// (fit_kernel) and keeps u* and L(u*) of every span in fit_u / fit_len.
+void set_job_targets(Job& j, const long long* first, const long long* end, const float* ms, const size_t* fit_offs);
+// Checks a target table of B utterances (offs: their id offsets) or, with !per_utterance, of one stream: spans
+// non-empty, inside the utterance, ascending and disjoint; ms NaN (none) or a finite value in (0, 600000]; no span
+// that asks on an utterance whose tempo[b] (null: none) asks.  Errors name the utterance and the span.  Returns whether
+// some span asks.
+bool check_targets(const long long* first, const long long* end, const float* ms, const size_t* fit_offs,
+                   const size_t* offs, size_t B, const float* tempo, bool per_utterance = true);
+// The samples of a target of ms milliseconds at `rate`: floor(ms R / 1000 + 0.5) in double.
+long long target_samples(float ms, int rate);
+// The fit launch of job j: the spans that ask, each with its break samples P and its index into j.targets.
+struct FitPlan {
+    std::vector<FitSpan> spans;
+    std::vector<long long> pause;
+    std::vector<size_t> index;
+};
+FitPlan fit_plan(const Job& j);
 // Per-utterance speaker blends of the job's next run (a blend table as for canonical_blends), or null for none.  A blend
 // replaces the utterance's config speaker; its noise and length scales still apply.  Every entry is checked first; a bad
 // entry fails naming the utterance and leaves the job's blends as they were.
@@ -718,12 +746,17 @@ struct Latent {
 // One encoder pass over B utterances (cfgs: one per utterance, or null for the voice's fallback config; scale / frames:
 // per-id duration controls as for set_job_durations, or null; seeds / seeded: noise seeds as for set_job_seeds) -> B
 // latents sharing one device allocation.  The caller owns the returned pointers.
-// blend_s / blend_u / blend_offs: speaker blends as for set_job_blends, or null.
+// blend_s / blend_u / blend_offs: speaker blends as for set_job_blends, or null.  fit_*: target durations as for
+// set_job_targets (their u* and L(u*) into fit_u / fit_len when given), with `breaks` (per id, as for set_job_breaks)
+// counted in each span's P: the breaks its latent's prosody stream will insert.
 std::vector<Latent*> encode_latents(Voice* v, const long long* ids, const size_t* offs, size_t B, const SynthConfig* cfgs,
                                     const float* scale = nullptr, const int* frames = nullptr,
                                     const unsigned long long* seeds = nullptr, const int* seeded = nullptr,
                                     const long long* blend_s = nullptr, const float* blend_u = nullptr,
-                                    const size_t* blend_offs = nullptr);
+                                    const size_t* blend_offs = nullptr, const float* breaks = nullptr,
+                                    const long long* fit_first = nullptr, const long long* fit_end = nullptr,
+                                    const float* fit_ms = nullptr, const size_t* fit_offs = nullptr,
+                                    float* fit_u = nullptr, long long* fit_len = nullptr);
 Latent* encode_latent(Voice* v, const long long* ids, size_t n);
 // One stream's resampling state: the filter to its output rate, the last inputs (two device buffers of K floats each,
 // read and written alternately), and how many inputs it has consumed and outputs it has emitted.

@@ -490,6 +490,7 @@ __global__ void scale_copy2_kernel(const float* __restrict__ eps, const float* _
 //   dur_scale  : the predicted count is ceil((exp(logw) * length_scale) * s); the product is rounded in that order, so
 //                s = 1 gives the bits of a call without scales
 //   dur_frames : a value >= 0 replaces the count (no ceil involved); -1 keeps the predicted one
+//   fit        : the target fit's factor u (fit.cu), multiplied in after s as one more f32 multiply
 // logw is written for every id either way.
 __device__ __forceinline__ int sat_int(long long v) { return (int)min(v, (long long)INT_MAX); }
 
@@ -498,6 +499,7 @@ __global__ void __launch_bounds__(256) durations_kernel(const float* __restrict_
                                                         const SegInfo* __restrict__ segs,
                                                         const float* __restrict__ dur_scale,
                                                         const int* __restrict__ dur_frames,
+                                                        const float* __restrict__ fit,
                                                         float* __restrict__ logw, int* __restrict__ cum,
                                                         int* __restrict__ y_len) {
     pdl_trigger(); pdl_wait();
@@ -514,12 +516,11 @@ __global__ void __launch_bounds__(256) durations_kernel(const float* __restrict_
         long long w = 0;
         if (i < sg.len) {
             const int row = sg.off + i;
-            const float lw = (z[2 * row] - m0) * einv;
+            const float lw = dur_logw(z, row, m0, einv);
             logw[row] = lw;
-            float wf = expf(lw) * length_scale;
-            if (dur_scale) wf = wf * dur_scale[row];
-            const float wc = ceilf(wf);
-            w = wc < 2147483648.f ? (long long)(int)wc : (long long)INT_MAX;     // NaN and inf saturate too
+            float wf = dur_weight(lw, length_scale, dur_scale, row);
+            if (fit) wf = wf * fit[row];
+            w = dur_count(wf);
             if (dur_frames) {
                 const int f = dur_frames[row];
                 if (f >= 0) w = f;
@@ -1242,9 +1243,10 @@ void launch_scale_copy2(const float* eps, const float* s, const int* seg_of_gran
 }
 
 void launch_durations(const float* z, float m0, float logs0, const float* length_scale, const SegInfo* segs, int nseg,
-                      float* logw, int* cum, int* y_len, cudaStream_t st, const float* dur_scale, const int* dur_frames) {
+                      float* logw, int* cum, int* y_len, cudaStream_t st, const float* dur_scale, const int* dur_frames,
+                      const float* fit) {
     launch_pdl(durations_kernel, dim3(nseg), dim3(256), 0, st, z, m0, logs0, length_scale, segs, dur_scale, dur_frames,
-               logw, cum, y_len);
+               fit, logw, cum, y_len);
     g_launch_count++;
 }
 

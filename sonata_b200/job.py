@@ -12,7 +12,8 @@ from . import _native as N
 from .core import G711_LAW, Audio, OperationError, check_encoding
 from .piper import (_batch_options, _blend_arrays, _break_arrays, _check, _config_array, _contour_arrays, _duration_arrays,
                     _formant_array, _gain_array, _loudness_array, _pack_ids, _prosody_arrays, _ptr, _rate_array,
-                    _seed_arrays, _take_audio, _take_bytes, _volume_arrays)
+                    _seed_arrays, _take_audio, _take_bytes, _volume_arrays, _target_arrays, _target_images,
+                    _check_target_list)
 
 
 class SynthesisJob:
@@ -22,18 +23,20 @@ class SynthesisJob:
                  loudness: Optional[Sequence] = None, pitches: Optional[Sequence] = None,
                  tempos: Optional[Sequence] = None, pitch_contours: Optional[Sequence] = None,
                  formants: Optional[Sequence] = None, speaker_blends: Optional[Sequence] = None,
-                 volume_contours: Optional[Sequence] = None, breaks: Optional[Sequence] = None):
+                 volume_contours: Optional[Sequence] = None, breaks: Optional[Sequence] = None,
+                 target_durations: Optional[Sequence] = None):
         """`configs`: one PiperSynthesisConfig per utterance (see set_configs); None keeps the voice's fallback config.
         `seeds`: noise seeds (see set_seeds).  `output_rates`: output sample rates (see set_output_rates).
         `loudness`: loudness targets (see set_loudness).  `pitches` / `tempos`: pitch and tempo ratios (see
         set_prosody).  `pitch_contours`: per-id pitch ratios (see set_pitch_contours).  `formants`: formant ratios (see
         set_formants).  `speaker_blends`: speaker blends (see set_speaker_blends).  `volume_contours`: per-id volume
-        levels (see set_volume_contours).  `breaks`: per-id pauses (see set_breaks)."""
+        levels (see set_volume_contours).  `breaks`: per-id pauses (see set_breaks).  `target_durations`: target
+        durations (see set_target_durations)."""
         # argument errors before the job exists
         options = _batch_options(model, len(batches), [len(b) for b in batches], configs, seeds=seeds,
                                  output_rates=output_rates, loudness=loudness, pitches=pitches, tempos=tempos,
                                  pitch_contours=pitch_contours, formants=formants, speaker_blends=speaker_blends,
-                                 volume_contours=volume_contours, breaks=breaks)
+                                 volume_contours=volume_contours, breaks=breaks, target_durations=target_durations)
         self._open(model, batches, options, eps_w, eps_z, debug)
 
     @classmethod
@@ -103,6 +106,9 @@ class SynthesisJob:
             self._set(lib.sb200_job_set_volume_contour, _ptr(o.volume, C.c_float))
         if o.breaks is not None:
             self._set(lib.sb200_job_set_breaks, _ptr(o.breaks, C.c_float))
+        if o.targets is not None:
+            self._set(lib.sb200_job_set_targets, *_target_images(o.targets))
+        self._spans = None if o.targets is None else [int(x) for x in o.targets[3]]
 
     def _set(self, fn, *images) -> None:
         """One sb200_job_set_* call with its C images."""
@@ -199,6 +205,28 @@ class SynthesisJob:
         The results, their lengths and prosody_bounds count the pauses, and profile() reports the stage as "break".  A
         bad entry raises OperationError naming the utterance and the id, and leaves the job's breaks as they were."""
         self._set(self._lib.sb200_job_set_breaks, _ptr(_break_arrays(self._lens, breaks), C.c_float))
+
+    def set_target_durations(self, targets: Optional[Sequence]) -> None:
+        """Target durations for the next run (see VitsModel.infer_batch_with_values): per utterance None, a duration in
+        ms for the whole utterance or a list of (first, last, ms) spans of ids; None for the whole list, or entries
+        that all ask for nothing, turn fitting off.  A bad entry, or one on an utterance with a tempo ratio, raises
+        OperationError naming the utterance and the span, and leaves the job's targets as they were."""
+        t = _target_arrays(self._lens, _check_target_list(targets, self.batch, None, self._lens))
+        self._set(self._lib.sb200_job_set_targets, *_target_images(t))
+        self._spans = None if t is None else [int(x) for x in t[3]]
+
+    def targets(self) -> List[List[Tuple[float, int]]]:
+        """Per utterance, each target span's (u, delivered length) of the last run: u the factor its predicted
+        durations got, and the span's samples at the voice's rate, breaks included (NaN and -1 for a span that asked
+        for nothing).  OperationError when the last run had no targets."""
+        if self._spans is None:
+            raise OperationError("the job's last run had no target durations")
+        n = self._spans[-1]
+        u, ln = np.zeros(max(n, 1), np.float32), np.zeros(max(n, 1), np.int64)
+        err = N.sb200_error()
+        _check(self._lib.sb200_job_targets(self._h, _ptr(u, C.c_float), _ptr(ln, C.c_int64), n, C.byref(err)), err)
+        return [[(float(u[k]), int(ln[k])) for k in range(self._spans[b], self._spans[b + 1])]
+                for b in range(self.batch)]
 
     def set_speaker_blends(self, blends: Optional[Sequence]) -> None:
         """Per-utterance speaker blends for the next run (see VitsModel.infer_batch_with_values): a mapping

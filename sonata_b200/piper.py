@@ -504,6 +504,111 @@ def _breaks_ask(image, rate: int) -> bool:
     return bool(np.any(np.floor(ms * rate / 1000.0 + 0.5) > 0))
 
 
+TARGET_RANGE_MS = (0.0, 600000.0)   # a target duration (ms) is in (low, high]; None or NaN ask for none
+
+
+def _target_ms(x, label, k: Optional[int]) -> float:
+    """A target duration checked as the library checks it (NaN for None); k: its span, or None for a whole utterance."""
+    where = _who(label) if k is None else f"{_who(label)}, span {k}"
+    if x is None:
+        return math.nan
+    if isinstance(x, bool) or not isinstance(x, numbers.Real):
+        raise OperationError(f"{where}: target duration {x!r} is not a number")
+    x = float(x)
+    if not (math.isnan(x) or (math.isfinite(x) and TARGET_RANGE_MS[0] < x <= TARGET_RANGE_MS[1])):
+        raise OperationError(f"{where}: target duration {x} ms is not a finite value in "
+                             f"({TARGET_RANGE_MS[0]}, {TARGET_RANGE_MS[1]}] (None or NaN: none)")
+    return x
+
+
+def _target_entry(v, label, tempo=None, count: Optional[int] = None, unit: str = "id"):
+    """One utterance's target durations, checked for form: None, a duration in ms for the whole utterance (a float, NaN
+    for none), or a list of (first, last, ms) spans, inclusive, ascending and disjoint (a list of (int, int, float)).
+    `count`: the ids (or characters) the spans index, None when not known yet.  An entry that asks for something with a
+    tempo ratio (tempo not None / NaN) is refused."""
+    if v is None:
+        return None
+    if isinstance(v, numbers.Real) and not isinstance(v, bool):
+        out = _target_ms(v, label, None)
+        asks = not math.isnan(out)
+    else:
+        if isinstance(v, (str, bytes)) or not hasattr(v, "__iter__"):
+            raise OperationError(f"{_who(label)}: target durations {v!r} are neither a duration in ms nor a list of "
+                                 "(first, last, ms) spans")
+        out, prev, asks = [], -1, False
+        for k, sp in enumerate(v):
+            if isinstance(sp, (str, bytes)) or not hasattr(sp, "__len__") or len(sp) != 3:
+                raise OperationError(f"{_who(label)}, span {k}: {sp!r} is not a (first, last, ms) span")
+            a, b, ms = sp
+            if any(isinstance(x, bool) or not isinstance(x, numbers.Integral) for x in (a, b)):
+                raise OperationError(f"{_who(label)}, span {k}: {unit}s {a!r} .. {b!r} are not integers")
+            a, b = int(a), int(b)
+            if not (0 <= a <= b and (count is None or b < count)):
+                raise OperationError(f"{_who(label)}, span {k}: {unit}s {a} .. {b} are not a range of the "
+                                     + (f"{count} {unit}s" if count is not None else f"{unit}s"))
+            if a <= prev:
+                raise OperationError(f"{_who(label)}, span {k}: {unit}s {a} .. {b} overlap or precede the span before "
+                                     f"it, which ends at {unit} {prev}")
+            prev = b
+            ms = _target_ms(ms, label, k)
+            asks |= not math.isnan(ms)
+            out.append((a, b, ms))
+    if asks and tempo is not None and not math.isnan(float(tempo)):
+        raise OperationError(f"{_who(label)}: a target duration and a tempo ratio together (give one or the other)")
+    return out
+
+
+def _char_targets_to_ids(entry, phonemes: str, src: Sequence[int], label):
+    """A checked phoneme-surface target entry (of _target_entry) as id spans: a span of characters [a, b] covers the
+    ids whose source character lies in it (its ids and pads, as pitch contours map characters); one that covers no id
+    is refused.  A whole-utterance duration stays one."""
+    if entry is None or isinstance(entry, float):
+        return entry
+    out = []
+    for k, (a, b, ms) in enumerate(entry):
+        if b >= len(phonemes):
+            raise OperationError(f"{_who(label)}, span {k}: characters {a} .. {b} are not a range of the "
+                                 f"{len(phonemes)} characters")
+        ids = [i for i, c in enumerate(src) if a <= int(c) <= b]
+        if not ids:
+            raise OperationError(f"{_who(label)}, span {k}: characters {a} .. {b} map to no id (the voice drops them)")
+        out.append((ids[0], ids[-1], ms))
+    return out
+
+
+def _target_arrays(lens: Sequence[int], entries):
+    """The C target table (first i64, end i64, ms f32, offsets size_t [n + 1]) of checked per-utterance entries (of
+    _target_entry, in ids; a whole-utterance duration is the span of every id), or None when no span asks."""
+    if entries is None:
+        return None
+    first, end, ms, offs = [], [], [], [0]
+    for n_ids, e in zip(lens, entries):
+        spans = [] if e is None else [(0, n_ids - 1, e)] if isinstance(e, float) else e
+        for a, b, m in spans:
+            first.append(a); end.append(b + 1); ms.append(m)
+        offs.append(len(first))
+    if all(math.isnan(m) for m in ms):
+        return None
+    return (np.array(first, np.int64), np.array(end, np.int64), np.array(ms, np.float32),
+            np.array(offs, np.uint64))
+
+
+def _target_images(t):
+    """The four C pointers of a target table of _target_arrays (all None for none)."""
+    if t is None:
+        return None, None, None, None
+    return _ptr(t[0], C.c_int64), _ptr(t[1], C.c_int64), _ptr(t[2], C.c_float), _ptr(t[3], C.c_size_t)
+
+
+def _check_target_list(targets, n: int, tempo, lens: Optional[Sequence[int]]):
+    """Each utterance's entry of `targets` (one per utterance, or None) checked by _target_entry; None when not given."""
+    if targets is None:
+        return None
+    return [_target_entry(v, b, None if tempo is None else tempo[b], None if lens is None else lens[b],
+                          "id" if lens is not None else "character")
+            for b, v in enumerate(_per_utterance(targets, n, "target durations"))]
+
+
 def refuse_prosody(pitch, tempo, where: str) -> None:
     """OperationError when `where`, a mode that hands out a sentence chunk by chunk, is asked for a pitch or tempo
     ratio."""
@@ -525,6 +630,13 @@ def refuse_breaks(breaks, where: str) -> None:
     if breaks is not None:
         raise OperationError(f"{where} cannot insert breaks: only this library's streaming voices carry them from chunk "
                              "to chunk (use speak_batch or a SynthesisJob)")
+
+
+def refuse_targets(target_duration, where: str) -> None:
+    """OperationError when `where`, a mode without this library's streaming voices, is asked for a target duration."""
+    if target_duration is not None:
+        raise OperationError(f"{where} cannot fit a target duration: only this library's streaming voices fit a "
+                             "sentence's latent (use speak_batch or a SynthesisJob)")
 
 
 def refuse_contour(pitch_contour, where: str) -> None:
@@ -583,10 +695,12 @@ class _BatchOptions:
     blend_offsets: Optional[np.ndarray] = None
     volume: Optional[np.ndarray] = None       # per id, packed
     breaks: Optional[np.ndarray] = None       # per id, packed
+    targets: Optional[tuple] = None           # target table (_target_arrays)
     char_scales: Optional[list] = None
     char_contours: Optional[list] = None
     char_volumes: Optional[list] = None
     char_breaks: Optional[list] = None
+    char_targets: Optional[list] = None       # checked entries in characters (_target_entry)
 
     def map_characters(self, phonemes: Sequence[str], maps) -> None:
         """Makes the per-id images of the per-character controls once the phonemes are mapped: maps[b] is (ids, source
@@ -602,20 +716,24 @@ class _BatchOptions:
         self.breaks = None if self.char_breaks is None else _break_arrays(lens, [
             None if v is None else _char_breaks_to_ids(v, ph, src, b)
             for b, (v, ph, (_, src)) in enumerate(zip(self.char_breaks, phonemes, maps))])
+        if self.char_targets is not None:
+            self.targets = _target_arrays(lens, [_char_targets_to_ids(e, ph, src, b) for b, (e, ph, (_, src)) in
+                                                 enumerate(zip(self.char_targets, phonemes, maps))])
 
     @property
     def per_character(self) -> bool:
         """Whether a per-character control needs the phonemes' character map."""
-        return any(x is not None for x in (self.char_scales, self.char_contours, self.char_volumes, self.char_breaks))
+        return any(x is not None for x in (self.char_scales, self.char_contours, self.char_volumes, self.char_breaks,
+                                           self.char_targets))
 
 
 def _batch_options(model, n: int, lens: Optional[Sequence[int]] = None, configs=None, duration_scales=None,
                    durations=None, seeds=None, output_rates=None, loudness=None, law=None, gains=None, pitches=None,
                    tempos=None, pitch_contours=None, formants=None, speaker_blends=None, volume_contours=None,
-                   breaks=None, g711: bool = False) -> _BatchOptions:
+                   breaks=None, g711: bool = False, target_durations=None) -> _BatchOptions:
     """The options of a batch of n utterances, each checked as its C image is made, in one order at every surface:
     configs, duration scales, durations, seeds, output rates, loudness, law (with `g711`), gains, pitch and tempo, pitch
-    contours, formants, speaker blends, volume contours, breaks.  `lens`: the utterances' id counts, for per-id controls; None for a phoneme
+    contours, formants, speaker blends, volume contours, breaks, target durations.  `lens`: the utterances' id counts, for per-id controls; None for a phoneme
     surface, whose per-character controls are only counted here, before any phoneme is mapped (see map_characters)."""
     o = _BatchOptions(n, _config_array(configs, n))
     if lens is None:
@@ -643,6 +761,11 @@ def _batch_options(model, n: int, lens: Optional[Sequence[int]] = None, configs=
         o.char_breaks = None if breaks is None else _per_utterance(breaks, n, "breaks")
     else:
         o.breaks = _break_arrays(lens, breaks)
+    checked = _check_target_list(target_durations, n, o.tempo, lens)
+    if lens is None:
+        o.char_targets = checked
+    else:
+        o.targets = _target_arrays(lens, checked)
     return o
 
 
@@ -878,21 +1001,23 @@ class _VitsCommons:
                     pitches: Optional[Sequence] = None, tempos: Optional[Sequence] = None,
                     pitch_contours: Optional[Sequence] = None, formants: Optional[Sequence] = None,
                     speaker_blends: Optional[Sequence] = None,
-                    volume_contours: Optional[Sequence] = None, breaks: Optional[Sequence] = None) -> List[Audio]:
+                    volume_contours: Optional[Sequence] = None, breaks: Optional[Sequence] = None,
+                    target_durations: Optional[Sequence] = None) -> List[Audio]:
         """`configs`: one PiperSynthesisConfig per utterance (speaker and scales), still synthesised as one pass;
         None uses the fallback config for every utterance.  `seeds`: noise seeds as for infer_batch_with_values.
         `speaker_blends`: as for infer_batch_with_values.
         `output_rates` / `loudness` / `pitches` / `tempos` / `formants`: per-utterance output sample rates, loudness
         targets, pitch and tempo ratios and formant ratios as for infer_batch_with_values.  `pitch_contours` /
         `volume_contours` / `breaks`: as for speak_batch_with_alignment, one ratio, level or break per phoneme
-        character."""
+        character.  `target_durations`: as for speak_batch_with_alignment, spans in phoneme characters."""
         n = len(phoneme_batches)
         o = _batch_options(self, n, None, configs, seeds=seeds, output_rates=output_rates, loudness=loudness,
                            pitches=pitches, tempos=tempos, pitch_contours=pitch_contours, formants=formants,
-                           speaker_blends=speaker_blends, volume_contours=volume_contours, breaks=breaks)
+                           speaker_blends=speaker_blends, volume_contours=volume_contours, breaks=breaks,
+                           target_durations=target_durations)
         if n == 0:
             return []
-        if pitch_contours is not None or volume_contours is not None or breaks is not None:
+        if o.per_character:
             maps = [self.phonemes_to_input_ids_map(p) for p in phoneme_batches]
             o.map_characters(phoneme_batches, maps)
             return [a for a, _, _ in self._speak_ids([ids for ids, _ in maps], o)]
@@ -923,7 +1048,8 @@ class _VitsCommons:
                                 formants: Optional[Sequence] = None,
                                 speaker_blends: Optional[Sequence] = None,
                                 volume_contours: Optional[Sequence] = None,
-                                breaks: Optional[Sequence] = None) -> List[Audio]:
+                                breaks: Optional[Sequence] = None,
+                                target_durations: Optional[Sequence] = None) -> List[Audio]:
         """Batched infer_with_values.  `configs`: one PiperSynthesisConfig per utterance (speaker and scales), or None
         for the fallback config; each utterance's result equals a single-utterance call with its config as the
         fallback, except for the on-device noise of an unseeded utterance, whose draws depend on the batch position.
@@ -977,11 +1103,20 @@ class _VitsCommons:
         / 0 for none), or None: SSML's <break time>.  Each pause is round(ms * rate / 1000) samples of silence at the
         voice's rate, with a 5 ms smoothstep fade of the speech on either side, inserted on the device after the
         volume stage and before any resampling and loudness (sb200_speak_batch_ids_breaks); a loudness target then
-        normalises the paused utterance as a whole.  The utterance gets longer by its pauses."""
+        normalises the paused utterance as a whole.  The utterance gets longer by its pauses.
+
+        `target_durations`: one entry per utterance, or None: None, a duration in ms for the whole utterance (bos and
+        eos included), or a list of (first, last, ms) spans of ids, inclusive, ascending and disjoint; ms in
+        TARGET_RANGE_MS, or None / NaN for none.  Each span's predicted durations are multiplied by one factor u in
+        [0.5, 2] before their ceil, the largest whose frames (times 256, plus the span's breaks) do not pass the target
+        (u = 0.5 when even that overruns), found on the device in the same pass (include/sonata_b200.h,
+        sb200_speak_batch_ids_fit).  Ids outside the spans and fixed durations keep their counts, and the rest of the
+        pass runs as with those counts fixed.  A target may not go with a tempo ratio.  SynthesisJob.targets()
+        reports each span's u and delivered length."""
         o = _batch_options(self, len(batches), [len(b) for b in batches], configs, seeds=seeds,
                            output_rates=output_rates, loudness=loudness, pitches=pitches, tempos=tempos,
                            pitch_contours=pitch_contours, formants=formants, speaker_blends=speaker_blends,
-                           volume_contours=volume_contours, breaks=breaks)
+                           volume_contours=volume_contours, breaks=breaks, target_durations=target_durations)
         return [a for a, _, _ in self._speak_ids(batches, o)]
 
     def infer_batch_with_durations(self, batches: Sequence[Sequence[int]],
@@ -996,7 +1131,8 @@ class _VitsCommons:
                                    formants: Optional[Sequence] = None,
                                    speaker_blends: Optional[Sequence] = None,
                                    volume_contours: Optional[Sequence] = None,
-                                   breaks: Optional[Sequence] = None) -> List[Tuple[Audio, np.ndarray]]:
+                                   breaks: Optional[Sequence] = None,
+                                   target_durations: Optional[Sequence] = None) -> List[Tuple[Audio, np.ndarray]]:
         """infer_batch_with_values with per-id duration control, returning (audio, frames per id) per utterance.
 
         duration_scales[b]: one scale (finite, >= 0) per id of utterance b, applied before the duration's ceil, so 1.0
@@ -1005,16 +1141,16 @@ class _VitsCommons:
         utterance whose ids all got 0 frames is still one frame long.  `seeds`: as for infer_batch_with_values; a
         seeded frame's noise depends on its index only, so controls that move frames never reshuffle it.
         `output_rates` / `loudness` / `pitches` / `tempos` / `pitch_contours` / `formants` / `speaker_blends` /
-        `volume_contours` / `breaks`: as for infer_batch_with_values (the frame counts stay frame counts of the
-        utterance before any warp or pause)."""
+        `volume_contours` / `breaks` / `target_durations`: as for infer_batch_with_values (the frame counts stay
+        frame counts of the utterance before any warp or pause, and are the fitted ones with a target)."""
         o = _batch_options(self, len(batches), [len(b) for b in batches], configs, duration_scales, durations, seeds,
                            output_rates, loudness, pitches=pitches, tempos=tempos, pitch_contours=pitch_contours,
                            formants=formants, speaker_blends=speaker_blends, volume_contours=volume_contours,
-                           breaks=breaks)
+                           breaks=breaks, target_durations=target_durations)
         return [(a, f) for a, f, _ in self._speak_ids(batches, o, frames=True)]
 
     def _speak_ids(self, batches, o: _BatchOptions, frames: bool = False) -> List[tuple]:
-        """The f32 batch route: `batches` with options `o` in one sb200_speak_batch_ids_breaks call.  Per utterance
+        """The f32 batch route: `batches` with options `o` in one sb200_speak_batch_ids_fit call.  Per utterance
         (audio, frames per id, each id's delivered end): the frames only when asked for, since fetching them costs a
         device->host copy and a synchronise, and the ends only when o has a pitch contour or breaks (None
         otherwise)."""
@@ -1027,13 +1163,14 @@ class _VitsCommons:
         id_frames = np.zeros(int(offs[-1]), np.int32) if frames else None
         bounds = None if o.contour is None and o.breaks is None else np.zeros(int(offs[-1]), np.int64)
         err = N.sb200_error()
-        _check(self._lib.sb200_speak_batch_ids_breaks(
+        _check(self._lib.sb200_speak_batch_ids_fit(
             self._h, _ptr(packed, C.c_int64), _ptr(offs, C.c_size_t), n, o.cfgs, _ptr(o.scales, C.c_float),
             _ptr(o.frames, C.c_int32), _ptr(o.seeds, C.c_uint64), _ptr(o.seeded, C.c_int32), _ptr(o.rates, C.c_uint32),
             _ptr(o.loudness, C.c_float), _ptr(o.pitch, C.c_float), _ptr(o.tempo, C.c_float), _ptr(o.contour, C.c_float),
             _ptr(o.formants, C.c_float), _ptr(o.blend_speakers, C.c_int64), _ptr(o.blend_weights, C.c_float),
-            _ptr(o.blend_offsets, C.c_size_t), _ptr(o.volume, C.c_float), _ptr(o.breaks, C.c_float), outs,
-            _ptr(id_frames, C.c_int32), _ptr(bounds, C.c_int64), None, None, C.byref(err)), err)
+            _ptr(o.blend_offsets, C.c_size_t), _ptr(o.volume, C.c_float), _ptr(o.breaks, C.c_float),
+            *_target_images(o.targets), outs, _ptr(id_frames, C.c_int32), _ptr(bounds, C.c_int64), None, None, None,
+            None, C.byref(err)), err)
         cut = lambda a, b: None if a is None else a[int(offs[b]):int(offs[b + 1])].copy()
         return [(_take_audio(outs[b]), cut(id_frames, b), cut(bounds, b)) for b in range(n)]
 
@@ -1047,7 +1184,9 @@ class _VitsCommons:
                                    formants: Optional[Sequence] = None,
                                    speaker_blends: Optional[Sequence] = None,
                                    volume_contours: Optional[Sequence] = None,
-                                   breaks: Optional[Sequence] = None) -> List[Tuple[Audio, List[PhonemeAlignment]]]:
+                                   breaks: Optional[Sequence] = None,
+                                   target_durations: Optional[Sequence] = None
+                                   ) -> List[Tuple[Audio, List[PhonemeAlignment]]]:
         """speak_batch that also says when each phoneme is spoken: per utterance (audio, alignment), the alignment
         holding one entry for bos (`^`), one per kept phoneme character (its id and its trailing pad) and one for eos
         (`$`), contiguous from sample 0 to len(audio).
@@ -1071,12 +1210,15 @@ class _VitsCommons:
         moves no boundary.  breaks[b] (or None): one pause in ms per character of phoneme_batches[b] (see
         infer_batch_with_values), after that character's pad; a character the voice drops puts its pause after the
         last id before it.  An utterance with breaks is aligned from each id's delivered end after the pauses before
-        it, so a pause belongs to the entry it follows and the entries still end at len(audio)."""
+        it, so a pause belongs to the entry it follows and the entries still end at len(audio).
+        target_durations[b] (or None): as for infer_batch_with_values, with spans (first, last, ms) of phoneme
+        characters, inclusive: a span covers the ids (and pads) of the characters in it, and one whose characters the
+        voice all drops is refused.  The alignment then holds the fitted durations."""
         n = len(phoneme_batches)
         o = _batch_options(self, n, None, configs, duration_scales, seeds=seeds, output_rates=output_rates,
                            loudness=loudness, pitches=pitches, tempos=tempos, pitch_contours=pitch_contours,
                            formants=formants, speaker_blends=speaker_blends, volume_contours=volume_contours,
-                           breaks=breaks)
+                           breaks=breaks, target_durations=target_durations)
         maps = [self.phonemes_to_input_ids_map(p) for p in phoneme_batches]
         o.map_characters(phoneme_batches, maps)
         res = self._speak_ids([ids for ids, _ in maps], o, frames=True)
@@ -1099,17 +1241,19 @@ class _VitsCommons:
                          output_rates: Optional[Sequence] = None, loudness: Optional[Sequence] = None,
                          gains: Optional[Sequence] = None, pitches: Optional[Sequence] = None,
                          tempos: Optional[Sequence] = None, formants: Optional[Sequence] = None,
-                         speaker_blends: Optional[Sequence] = None, breaks: Optional[Sequence] = None) -> List[bytes]:
+                         speaker_blends: Optional[Sequence] = None, breaks: Optional[Sequence] = None,
+                         target_durations: Optional[Sequence] = None) -> List[bytes]:
         """infer_batch_with_values delivered as G.711 telephony audio: one `bytes` per utterance, one byte per sample.
         `law`: "mulaw" (PCMU) or "alaw" (PCMA), or one of those per utterance.  The bytes are G.711 of exactly the
         16-bit samples the i16 route gives (SynthesisJob.fetch_i16): to_i16_vec of the utterance after gains[b] (None:
         1), or the fixed scale for an utterance with a loudness target.  They are encoded on the device in the i16
         conversion's launches, so only one byte per sample leaves the card.  `configs`, `seeds`, `output_rates` and
-        `loudness` as for infer_batch_with_values, and so are `pitches`, `tempos`, `formants`, `speaker_blends` and
-        `breaks`; a batch mixing laws runs one conversion per law."""
+        `loudness` as for infer_batch_with_values, and so are `pitches`, `tempos`, `formants`, `speaker_blends`,
+        `breaks` and `target_durations`; a batch mixing laws runs one conversion per law."""
         o = _batch_options(self, len(batches), [len(b) for b in batches], configs, seeds=seeds,
                            output_rates=output_rates, loudness=loudness, law=law, gains=gains, pitches=pitches,
-                           tempos=tempos, formants=formants, speaker_blends=speaker_blends, breaks=breaks, g711=True)
+                           tempos=tempos, formants=formants, speaker_blends=speaker_blends, breaks=breaks, g711=True,
+                           target_durations=target_durations)
         return self._encode_batch(batches, o)
 
     def speak_batch_g711(self, phoneme_batches: Sequence[str], law,
@@ -1117,12 +1261,14 @@ class _VitsCommons:
                          output_rates: Optional[Sequence] = None, loudness: Optional[Sequence] = None,
                          gains: Optional[Sequence] = None, pitches: Optional[Sequence] = None,
                          tempos: Optional[Sequence] = None, formants: Optional[Sequence] = None,
-                         speaker_blends: Optional[Sequence] = None, breaks: Optional[Sequence] = None) -> List[bytes]:
+                         speaker_blends: Optional[Sequence] = None, breaks: Optional[Sequence] = None,
+                         target_durations: Optional[Sequence] = None) -> List[bytes]:
         """speak_batch delivered as G.711 bytes: infer_batch_g711 over the phonemes' ids (`breaks`: one per phoneme
-        character, as for speak_batch_with_alignment)."""
+        character, and `target_durations` in characters, as for speak_batch_with_alignment)."""
         o = _batch_options(self, len(phoneme_batches), None, configs, seeds=seeds, output_rates=output_rates,
                            loudness=loudness, law=law, gains=gains, pitches=pitches, tempos=tempos, formants=formants,
-                           speaker_blends=speaker_blends, breaks=breaks, g711=True)
+                           speaker_blends=speaker_blends, breaks=breaks, g711=True,
+                           target_durations=target_durations)
         return self._encode_batch(self._phoneme_ids(phoneme_batches, o), o)
 
     def infer_batch_flac(self, batches: Sequence[Sequence[int]],
@@ -1130,15 +1276,18 @@ class _VitsCommons:
                          output_rates: Optional[Sequence] = None, loudness: Optional[Sequence] = None,
                          gains: Optional[Sequence] = None, pitches: Optional[Sequence] = None,
                          tempos: Optional[Sequence] = None, formants: Optional[Sequence] = None,
-                         speaker_blends: Optional[Sequence] = None, breaks: Optional[Sequence] = None) -> List[bytes]:
+                         speaker_blends: Optional[Sequence] = None, breaks: Optional[Sequence] = None,
+                         target_durations: Optional[Sequence] = None) -> List[bytes]:
         """infer_batch_with_values delivered as lossless FLAC: one complete stream (`bytes`) per utterance.  Its samples
         are exactly the 16-bit samples the i16 route gives (SynthesisJob.fetch_i16): to_i16_vec of the utterance after
         gains[b] (None: 1), or the fixed scale for an utterance with a loudness target, at its delivered rate.  They are
         encoded on the device, and only the compressed bytes leave the card.  `configs`, `seeds`, `output_rates`,
-        `loudness`, `pitches`, `tempos`, `formants`, `speaker_blends` and `breaks` as for infer_batch_with_values."""
+        `loudness`, `pitches`, `tempos`, `formants`, `speaker_blends`, `breaks` and `target_durations` as for
+        infer_batch_with_values."""
         o = _batch_options(self, len(batches), [len(b) for b in batches], configs, seeds=seeds,
                            output_rates=output_rates, loudness=loudness, gains=gains, pitches=pitches, tempos=tempos,
-                           formants=formants, speaker_blends=speaker_blends, breaks=breaks)
+                           formants=formants, speaker_blends=speaker_blends, breaks=breaks,
+                           target_durations=target_durations)
         return self._encode_batch(batches, o)
 
     def speak_batch_flac(self, phoneme_batches: Sequence[str],
@@ -1146,12 +1295,14 @@ class _VitsCommons:
                          output_rates: Optional[Sequence] = None, loudness: Optional[Sequence] = None,
                          gains: Optional[Sequence] = None, pitches: Optional[Sequence] = None,
                          tempos: Optional[Sequence] = None, formants: Optional[Sequence] = None,
-                         speaker_blends: Optional[Sequence] = None, breaks: Optional[Sequence] = None) -> List[bytes]:
+                         speaker_blends: Optional[Sequence] = None, breaks: Optional[Sequence] = None,
+                         target_durations: Optional[Sequence] = None) -> List[bytes]:
         """speak_batch delivered as FLAC streams: infer_batch_flac over the phonemes' ids (`breaks`: one per phoneme
-        character, as for speak_batch_with_alignment)."""
+        character, and `target_durations` in characters, as for speak_batch_with_alignment)."""
         o = _batch_options(self, len(phoneme_batches), None, configs, seeds=seeds, output_rates=output_rates,
                            loudness=loudness, gains=gains, pitches=pitches, tempos=tempos, formants=formants,
-                           speaker_blends=speaker_blends, breaks=breaks)
+                           speaker_blends=speaker_blends, breaks=breaks,
+                           target_durations=target_durations)
         return self._encode_batch(self._phoneme_ids(phoneme_batches, o), o)
 
     def _phoneme_ids(self, phoneme_batches: Sequence[str], o: _BatchOptions) -> list:
@@ -1246,6 +1397,7 @@ class EncoderOutputs:
         n = int(model._lib.sb200_latent_id_frames(handle, None, 0))
         self.p_duration = np.zeros(n, np.int32)
         model._lib.sb200_latent_id_frames(handle, _ptr(self.p_duration, C.c_int32), n)
+        self.fit: Optional[List[Tuple[float, int]]] = None     # per target span: (u, delivered length) of the fit
 
     def infer_decoder(self, lo: int = 0, hi: Optional[int] = None) -> AudioSamples:
         hi = self.num_frames if hi is None else hi
@@ -1651,29 +1803,44 @@ class VitsStreamingModel(_VitsCommons):
                             duration_scales: Optional[Sequence] = None,
                             durations: Optional[Sequence] = None,
                             seeds: Optional[Sequence] = None,
-                            speaker_blends: Optional[Sequence] = None) -> List[EncoderOutputs]:
+                            speaker_blends: Optional[Sequence] = None,
+                            target_durations: Optional[Sequence] = None,
+                            breaks: Optional[Sequence] = None) -> List[EncoderOutputs]:
         """infer_encoder over many utterances in one encoder pass.  `configs`: one PiperSynthesisConfig per utterance,
         or None for the fallback config; each latent equals infer_encoder alone with its config as the fallback,
         except for the on-device noise of an unseeded utterance, whose draws depend on the batch position.
         `duration_scales` / `durations`: per-id duration controls as for infer_batch_with_durations; each output's
         `p_duration` holds its frames per id.  `seeds`: noise seeds as for infer_batch_with_values; a seeded latent
         equals the `z` of the same utterance synthesised with the same seed.  `speaker_blends`: as for
-        infer_batch_with_values; each latent keeps its blend, and every decoder chunk of it speaks with that blend."""
+        infer_batch_with_values; each latent keeps its blend, and every decoder chunk of it speaks with that blend.
+        `target_durations`: as for infer_batch_with_values: each latent's frames are fitted in this encoder pass, and
+        its chunks then decode unchanged; each output's `fit` holds (u, delivered length) per span (None without).
+        `breaks`: the pauses (per id, as for infer_batch_with_values) the latent's stream will insert, counted in its
+        targets; this pass inserts none, and without targets they are only checked."""
         n = len(batches)
         o = _batch_options(self, n, [len(b) for b in batches], configs, duration_scales, durations, seeds,
-                           speaker_blends=speaker_blends)
+                           speaker_blends=speaker_blends, breaks=breaks, target_durations=target_durations)
         _check_not_empty(batches)
         if n == 0:
             return []
         packed, offs = _pack_ids(batches)
         outs = (C.c_void_p * n)()
         err = N.sb200_error()
-        _check(self._lib.sb200_encode_batch_ids_blends(
+        t = o.targets
+        u = None if t is None else np.zeros(len(t[2]), np.float32)
+        ln = None if t is None else np.zeros(len(t[2]), np.int64)
+        _check(self._lib.sb200_encode_batch_ids_targets(
             self._h, _ptr(packed, C.c_int64), _ptr(offs, C.c_size_t), n, o.cfgs, _ptr(o.scales, C.c_float),
             _ptr(o.frames, C.c_int32), _ptr(o.seeds, C.c_uint64), _ptr(o.seeded, C.c_int32),
             _ptr(o.blend_speakers, C.c_int64), _ptr(o.blend_weights, C.c_float), _ptr(o.blend_offsets, C.c_size_t),
-            outs, C.byref(err)), err)
-        return [EncoderOutputs(self, C.c_void_p(outs[i])) for i in range(n)]
+            _ptr(o.breaks if t is not None else None, C.c_float), *_target_images(t), _ptr(u, C.c_float),
+            _ptr(ln, C.c_int64), outs, C.byref(err)), err)
+        res = [EncoderOutputs(self, C.c_void_p(outs[i])) for i in range(n)]
+        if t is not None:
+            for b, e in enumerate(res):
+                k0, k1 = int(t[3][b]), int(t[3][b + 1])
+                e.fit = [(float(u[k]), int(ln[k])) for k in range(k0, k1)]
+        return res
 
     def infer_decoder_batch(self, chunks: Sequence[tuple], pcm16: bool = False, fade: int = 0,
                             gains: Optional[Sequence[float]] = None, resamplers: Optional[Sequence] = None,
@@ -1778,7 +1945,7 @@ class VitsStreamingModel(_VitsCommons):
                          formant_ratio: Optional[float] = None, speaker_blend=None,
                          live_loudness=None, max_gain_db: Optional[float] = None,
                          volume_contour: Optional[Sequence] = None,
-                         breaks: Optional[Sequence] = None) -> SpeechStreamer:
+                         breaks: Optional[Sequence] = None, target_duration=None) -> SpeechStreamer:
         """`formant_ratio`: as for infer_batch_with_values' formants, on top of `pitch` / `tempo` / `pitch_contour` or
         alone, the sentence's formant stage carried as one stream on the device (ProsodyStream): the concatenation of
         the chunks is the formant stage applied at once to the sentence the stream yields without it, then resampled and
@@ -1807,8 +1974,13 @@ class VitsStreamingModel(_VitsCommons):
         `breaks`: one pause in ms per character of `phonemes` (as for speak_batch_with_alignment's breaks), on top of
         the rest or alone (ProsodyStream): the concatenation of the chunks is the sentence the stream yields without
         them with those pauses inserted at once, before resampling, metering and encoding.  A chunk emits the pauses its
-        input reaches, holding nothing back, and the streamer's `bounds` give each id's delivered end."""
+        input reaches, holding nothing back, and the streamer's `bounds` give each id's delivered end.
+        `target_duration`: the sentence's target durations (as for speak_batch_with_alignment's target_durations: a
+        duration in ms, or (first, last, ms) spans of phoneme characters); the latent's frames are fitted in its
+        encoder pass, with its breaks counted, and its chunks then run unchanged.  The encoder outputs' `fit` holds
+        each span's (u, delivered length)."""
         if not isinstance(self, VitsStreamingModel):
+            refuse_targets(target_duration, "stream_synthesis")
             refuse_breaks(breaks, "stream_synthesis")
             refuse_volume(volume_contour, "stream_synthesis")
             refuse_live_loudness(live_loudness, "stream_synthesis")
@@ -1818,8 +1990,12 @@ class VitsStreamingModel(_VitsCommons):
         o = _stream_options(self, "stream_synthesis", None, phonemes, seed=seed, output_rate=output_rate,
                             encoding=encoding, gain=gain, pitch=pitch, tempo=tempo, pitch_contour=pitch_contour,
                             formant_ratio=formant_ratio, speaker_blend=speaker_blend, live_loudness=live_loudness,
-                            max_gain_db=max_gain_db, volume_contour=volume_contour, breaks=breaks)
-        if o.seed is None and o.blend is None:
+                            max_gain_db=max_gain_db, volume_contour=volume_contour, breaks=breaks,
+                            target_duration=target_duration)
+        if o.target is not None:
+            enc = self.infer_encoder_batch([o.ids], seeds=[o.seed], speaker_blends=[o.blend], target_durations=[o.target],
+                                           breaks=[o.breaks])[0]
+        elif o.seed is None and o.blend is None:
             enc = self.infer_encoder(o.ids)
         else:
             enc = self.infer_encoder_batch([o.ids], seeds=[o.seed], speaker_blends=[o.blend])[0]
@@ -1865,15 +2041,17 @@ class _StreamOptions:
     max_gain_db: Optional[float]
     volume: Optional[Sequence] = None   # per id
     breaks: Optional[Sequence] = None   # per id
+    target: object = None               # checked target entry in ids (_target_entry), or None
 
 
 def _stream_options(model, where: str, key: Optional[int], ids_or_phonemes, config=None, chunk_size=None,
                     chunk_padding=None, seed=None, output_rate=None, encoding=None, gain=None, pitch=None, tempo=None,
                     pitch_contour=None, formant_ratio=None, speaker_blend=None, live_loudness=None, max_gain_db=None,
-                    carried=(), volume_contour=None, breaks=None) -> _StreamOptions:
+                    carried=(), volume_contour=None, breaks=None, target_duration=None) -> _StreamOptions:
     """The options of one stream of `model`, checked in one order: config, live loudness, speaker blend, formant ratio,
     pitch and tempo, seed, output rate, FLAC (refused by the name `where`), encoding and gain, the config's speaker,
-    chunking, then the ids (phonemes are mapped), the contour, the volume contour and the breaks.  Errors name "stream" (key None) or "stream {key}".
+    chunking, then the ids (phonemes are mapped), the contour, the volume contour, the breaks and the target duration.
+    Errors name "stream" (key None) or "stream {key}".
     `chunk_size`: checked with `chunk_padding` when given.  `carried`: the LoudnessStreams the caller's unfinished
     streams carry, which live_loudness may not be."""
     if config is not None and not isinstance(config, PiperSynthesisConfig):
@@ -1886,7 +2064,7 @@ def _stream_options(model, where: str, key: Optional[int], ids_or_phonemes, conf
         _stream_meter(model, live_loudness, None, output_rate, who)
     _blend_arrays(model, [speaker_blend], 1, [who])
     phi = _stream_formant(formant_ratio, who)
-    pit, _ = _prosody_arrays([pitch], [tempo], 1)
+    pit, tmp = _prosody_arrays([pitch], [tempo], 1)
     _seed_arrays([seed], 1)
     _rate_array([output_rate], 1)
     refuse_flac(encoding, where)
@@ -1895,10 +2073,15 @@ def _stream_options(model, where: str, key: Optional[int], ids_or_phonemes, conf
         raise OperationError(f"No speaker was found with the given id `{config.speaker}`")     # as check_config
     if chunk_size is not None:
         _check_chunking(chunk_size, chunk_padding)
-    contour, volume, brk = pitch_contour, volume_contour, breaks
-    if isinstance(ids_or_phonemes, str) and (pitch_contour is not None or volume_contour is not None or
-                                             breaks is not None):
+    contour, volume, brk, target = pitch_contour, volume_contour, breaks, None
+    chars = isinstance(ids_or_phonemes, str)
+    if target_duration is not None:
+        target = _target_entry(target_duration, who, None if tmp is None else tmp[0], len(ids_or_phonemes),
+                               "character" if chars else "id")
+    if chars and (pitch_contour is not None or volume_contour is not None or breaks is not None or
+                  target_duration is not None):
         ids, src = model.phonemes_to_input_ids_map(ids_or_phonemes)
+        target = _char_targets_to_ids(target, ids_or_phonemes, src, who)
         if pitch_contour is not None:
             contour = _char_values_to_ids(pitch_contour, ids_or_phonemes, src, who, "pitch ratios", _contour_value)
         if volume_contour is not None:
@@ -1919,7 +2102,7 @@ def _stream_options(model, where: str, key: Optional[int], ids_or_phonemes, conf
     if not ids:
         raise OperationError("Failed to run model inference. Error: empty input sequence")
     return _StreamOptions(key, who, ids, config, chunk_size, seed, output_rate, encoding, g, pitch, tempo, contour, phi,
-                          speaker_blend, live_loudness, max_gain_db, volume, brk)
+                          speaker_blend, live_loudness, max_gain_db, volume, brk, target)
 
 
 def _open_stream(model, o: _StreamOptions, enc):
@@ -1961,7 +2144,8 @@ class StreamBatch:
             pitch: Optional[float] = None, tempo: Optional[float] = None,
             pitch_contour: Optional[Sequence] = None, formant_ratio: Optional[float] = None,
             speaker_blend=None, live_loudness=None, max_gain_db: Optional[float] = None,
-            volume_contour: Optional[Sequence] = None, breaks: Optional[Sequence] = None) -> int:
+            volume_contour: Optional[Sequence] = None, breaks: Optional[Sequence] = None,
+            target_duration=None) -> int:
         """`seed`: the stream's noise seed (see infer_batch_with_values); a seeded stream yields what
         `stream_synthesis(..., seed=seed)` yields, whatever other streams share its encoder pass.  `output_rate`,
         `encoding` and `gain`: the stream's sample rate and G.711 encoding, as for stream_synthesis; `pitch` / `tempo`:
@@ -1978,8 +2162,11 @@ class StreamBatch:
         character (phonemes) or per id (ids), as for stream_synthesis; checked here, naming the stream.  A stream with
         one goes through the warped passes.  `breaks`: one pause in ms per phoneme character (phonemes) or per id
         (ids), as for stream_synthesis; checked here, naming the stream.  A stream with pauses goes through the warped
-        passes, and `bounds(key)` gives its per-id delivered ends once it is encoded."""
+        passes, and `bounds(key)` gives its per-id delivered ends once it is encoded.  `target_duration`: the
+        stream's target durations, as for stream_synthesis (spans of phoneme characters or of ids); checked here,
+        naming the stream, and fitted in the step's encoder pass, which the other streams share unchanged."""
         if not isinstance(self.model, VitsStreamingModel):
+            refuse_targets(target_duration, "StreamBatch")
             refuse_breaks(breaks, "StreamBatch")
             refuse_volume(volume_contour, "StreamBatch")
             refuse_live_loudness(live_loudness, "StreamBatch")
@@ -1987,19 +2174,21 @@ class StreamBatch:
             refuse_prosody(pitch, tempo, "StreamBatch")
             refuse_contour(pitch_contour, "StreamBatch")
         return self._add(ids_or_phonemes, config, self.chunk_size, seed, output_rate, encoding, gain, pitch, tempo,
-                         pitch_contour, speaker_blend, formant_ratio, live_loudness, max_gain_db, volume_contour, breaks)
+                         pitch_contour, speaker_blend, formant_ratio, live_loudness, max_gain_db, volume_contour, breaks,
+                         target_duration)
 
     def _add(self, ids_or_phonemes, config, chunk_size: int, seed: Optional[int] = None,
              output_rate: Optional[int] = None, encoding: Optional[str] = None, gain: Optional[float] = None,
              pitch: Optional[float] = None, tempo: Optional[float] = None, pitch_contour=None,
              speaker_blend=None, formant_ratio=None, live_loudness=None, max_gain_db=None, volume_contour=None,
-             breaks=None) -> int:
+             breaks=None, target_duration=None) -> int:
         carried = [o.live_loudness for o in self._pending] + [s.meter for s in self._active]
         o = _stream_options(self.model, "StreamBatch", self._next_key, ids_or_phonemes, config, chunk_size,
                             self.chunk_padding, seed=seed, output_rate=output_rate, encoding=encoding, gain=gain,
                             pitch=pitch, tempo=tempo, pitch_contour=pitch_contour, formant_ratio=formant_ratio,
                             speaker_blend=speaker_blend, live_loudness=live_loudness, max_gain_db=max_gain_db,
-                            carried=carried, volume_contour=volume_contour, breaks=breaks)
+                            carried=carried, volume_contour=volume_contour, breaks=breaks,
+                            target_duration=target_duration)
         self._next_key += 1
         self._pending.append(o)
         return o.key
@@ -2036,6 +2225,11 @@ class StreamBatch:
             def encode(ps):
                 ids = [o.ids for o in ps]
                 configs = None if fallback is None else [fallback if o.config is None else o.config for o in ps]
+                if any(o.target is not None for o in ps):
+                    return self.model.infer_encoder_batch(ids, configs, seeds=[o.seed for o in ps],
+                                                          speaker_blends=[o.blend for o in ps],
+                                                          target_durations=[o.target for o in ps],
+                                                          breaks=[o.breaks for o in ps])
                 if all(o.seed is None and o.blend is None for o in ps):
                     return self.model.infer_encoder_batch(ids, configs)
                 return self.model.infer_encoder_batch(ids, configs, seeds=[o.seed for o in ps],
