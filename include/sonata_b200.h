@@ -594,6 +594,58 @@ int32_t sb200_job_fetch_flac(sb200_job* job, const float* gains, uint8_t** outs,
  * rates (8000, 11025, 16000, 22050, 24000, 32000, 44100, 48000) fails with OPERATION_ERROR before any device work. */
 int32_t sb200_flac_encode(int32_t device, const int16_t* x, size_t n, uint32_t sample_rate, uint8_t** out, size_t* len,
                           sb200_error* err);
+
+/* ---- Watermark: a keyed provenance mark on everything a voice delivers (tests/watermark_reference.py) ----
+ * Set on the voice, not per call: once set, every job of the voice is marked, through every batch route (f32, i16,
+ * G.711, FLAC, output rates, loudness targets), and every realtime stream made while it is set
+ * (sb200_watermark_stream_create).
+ *
+ * Where: at each utterance's delivered rate R, after the last waveform stage (the resampler with an output rate, else
+ * breaks, volume, formant, pitch or the decoder) and before loudness and the encoders, over exactly the samples the
+ * caller receives.  n counts them from 0 at the utterance's first delivered sample (pauses count).  Loudness and the
+ * peak-scaled i16 conversion only apply a gain afterwards, and detection does not depend on gain.
+ * Chips: P = 4096.  c_j[m] = +1 when bit 0 of word 0 of Philox4x32-10 with counter (m, j, 0, 0) and key
+ * (key mod 2^32, key >> 32) is 1, else -1, for j in {0, 1}, m in [0, P).  c0 is the sync sequence; c1 carries the
+ * payload s as a cyclic shift: c[n] = c0[n mod P] + c1[(n - s) mod P], one of {-2, 0, 2}.
+ * Envelope: blocks of B = floor(R / 100) samples (the last may be shorter, L_k its length); q[n] the sample quantised
+ * as the pitch stage quantises it, (int)(clamp(x, -1, 1) * 32767) with an f32 product and a truncating cast;
+ * S_k = sum of q^2 over block k in int64; E_k = min(S_{k-1} / L_{k-1}, S_k / L_k) in double, block -1 taken as block 0.
+ * So the 10 ms after speech, and silences and pauses, get no mark.
+ * Gain: alpha = 10^(strength_db / 20) in double on the host; a_k = (float)((alpha * sqrt(E_k * 0.5)) / 32767), each
+ * double operation correctly rounded; y[n] = x[n] + a_k * c[n] as one f32 multiply and one f32 add.  The mark's power
+ * is alpha^2 E_k.  Nothing is clamped; lengths, ends, alignments and prosody bounds do not change.
+ * Scope: a provenance mark, not a tamper-proof one (folding many marked clips estimates the P-periodic sequence).  It
+ * survives gain, i16, G.711, FLAC, cropping and additive noise; it is not designed to survive resampling, time-scaling,
+ * pitch-shifting or lossy codecs after delivery.  A file that joins separately marked utterances splits its evidence
+ * over several offsets, so detecting each utterance is stronger than detecting the whole file. */
+typedef struct sb200_watermark {
+    uint64_t key;
+    int32_t payload;     /* [0, 4096) */
+    float strength_db;   /* finite, in [-40, -10] */
+} sb200_watermark;
+/* wm == NULL turns the mark off.  A bad payload or strength fails with OPERATION_ERROR naming the field and leaves the
+ * voice as it was.  The first use of a key builds its two chip tables on the voice's device.  A job reads the setting
+ * once, when it starts to run. */
+int32_t sb200_voice_set_watermark(sb200_voice* v, const sb200_watermark* wm, sb200_error* err);
+/* *on receives 1 and *out the setting when the voice marks, else *on = 0 (out untouched). */
+int32_t sb200_voice_watermark(const sb200_voice* v, sb200_watermark* out, int32_t* on, sb200_error* err);
+typedef struct sb200_watermark_result {
+    int32_t marked;      /* 1: z0 >= 6.5 */
+    int32_t payload;     /* (o0 - o1) mod P when marked and z1 >= 6.5, else -1 */
+    int32_t offset;      /* o0: the clip start's position mod P */
+    double z0, z1;
+} sb200_watermark_result;
+/* Detection in clips packed[offsets[b] .. offsets[b + 1]) for b < batch, f32 (fmt 0, quantised as above) or i16
+ * (fmt 1) samples, each possibly cropped anywhere, on `device`:
+ *   fold F[m] = sum of q[i] over i = m mod P (int64, exact); X = FFT_P(F); W = X / |X| (0 where |X| = 0);
+ *   r_j[o] = sum_m w[m] c_j[(m + o) mod P] = Re IFFT(conj(W) FFT_P(c_j)) [o];
+ *   o_j = argmax r_j (smallest o on ties); z_j = (r_j[o_j] - mu_j) / sigma_j, mu_j and sigma_j the population mean and
+ *   standard deviation of the other P - 1 lags (z_j = 0 when sigma_j = 0).
+ * Without a mark the standardised lags are about N(0, 1), so a false detection per clip and key is bounded by about
+ * P Q(6.5) = 1.6e-7.  A bad format fails with OPERATION_ERROR before any device work. */
+int32_t sb200_watermark_detect(int32_t device, uint64_t key, int32_t fmt, const void* packed, const size_t* offsets,
+                               size_t batch, sb200_watermark_result* out, sb200_error* err);
+
 int32_t sb200_job_lengths(const sb200_job* job, int64_t* frames, int64_t* samples, int64_t* out_offsets);
 /* Copy the result of a finished job into CALLER-OWNED host memory, utterances back to back in batch order.
  * format 0: f32 samples (what infer_with_values returns, piper/src/lib.rs:382-392);
@@ -883,6 +935,27 @@ int32_t sb200_decode_chunks_metered(sb200_voice* v, const sb200_latent* const* z
                                     const float* gain, sb200_resampler* const* resamplers,
                                     sb200_prosody_stream* const* warps, sb200_loudness_stream* const* meters,
                                     const int32_t* last, int32_t format, void** outs, size_t* lens, sb200_error* err);
+/* Watermarked realtime streams.  sb200_watermark_stream_create reads the voice's watermark once: *out is a stream that
+ * marks with that setting to its end, or NULL when the voice marks nothing (such a stream stays unmarked to its end).
+ * out_rate: the stream's delivered rate (0: the voice's).  sb200_decode_chunks_marked is sb200_decode_chunks_metered
+ * with one such stream (or NULL) per chunk: what the chunk delivers after resampling goes through the watermark stage
+ * before its meter and conversion, at stream positions n counted from the stream's first delivered sample.  After a
+ * pass in which a stream's stage has received J samples it has emitted floor(J / B) B of them (B = rate / 100), and
+ * all of them once a chunk with last = 1 ends it: it holds back fewer than B samples, and its chunk count does not
+ * change.  The joined chunks equal the whole-signal mark of the joined unmarked chunks, bit for bit.  A chunk's
+ * stream must be delivered at the chunk's rate and may appear once per pass. */
+typedef struct sb200_watermark_stream sb200_watermark_stream;
+int32_t sb200_watermark_stream_create(sb200_voice* v, uint32_t out_rate, sb200_watermark_stream** out,
+                                      sb200_error* err);
+void sb200_watermark_stream_free(sb200_watermark_stream* s);
+/* the "watermark" device time (ms) of the last chunk pass the stream was in; 19 for a null argument */
+int32_t sb200_watermark_stream_profile(const sb200_watermark_stream* s, float* ms);
+int32_t sb200_decode_chunks_marked(sb200_voice* v, const sb200_latent* const* zs, const int64_t* lo, const int64_t* hi,
+                                   const int64_t* trim_lo_frames, const int64_t* trim_hi_frames, size_t n, int32_t fade,
+                                   const float* gain, sb200_resampler* const* resamplers,
+                                   sb200_prosody_stream* const* warps, sb200_loudness_stream* const* meters,
+                                   sb200_watermark_stream* const* marks, const int32_t* last, int32_t format, void** outs,
+                                   size_t* lens, sb200_error* err);
 
 /* ---- introspection for tests / bench ---- */
 /* Copy a named intermediate of the LAST run of `job` to host (time-major fp32, valid rows of
@@ -1057,6 +1130,11 @@ int32_t sb200_debug_fit(int32_t device, const float* w, size_t n, const int32_t*
                         int64_t* frames_out, sb200_error* err);
 int32_t sb200_debug_breaks(int32_t device, const float* x, size_t n, const int64_t* ends, const float* ms, size_t n_ids,
                            int32_t rate, float* y, size_t cap, int64_t* n_out, sb200_error* err);
+/* The watermark stage over one caller buffer x[0 .. n) delivered at `rate` (8000 .. 48000), marked with *wm (checked as
+ * sb200_voice_set_watermark checks it): y[0 .. n) receives the result; bit for bit what a job gives an utterance of
+ * those samples. */
+int32_t sb200_debug_watermark(const float* x, size_t n, int32_t rate, const sb200_watermark* wm, float* y,
+                              sb200_error* err);
 /* Test hook, no device needed: the samples a prosody stream with these ratios at `rate` emits per chunk (the rule of
  * sb200_decode_chunks_warped) when its chunks bring chunk_lens[0 .. n_chunks) inputs and the last one ends it.
  * emitted[k] receives chunk k's count.  Returns 0, or 19 for bad ratios, a bad rate or a negative length. */

@@ -110,8 +110,30 @@ def build_parser() -> argparse.ArgumentParser:
     ap.add_argument("--speaker-blend", metavar="SPEAKER=WEIGHT,...",
                     help="Speak with a blend of a multi-speaker voice's speakers, e.g. \"speaker_3=0.7,speaker_12=0.3\" "
                          "(names or ids; weights >= 0, normalised to sum 1), in place of --speaker-id")
+    ap.add_argument("--watermark-key", type=_watermark_key, metavar="KEY",
+                    help="Mark all audio with this key's watermark (decimal or 0x-hex, [0, 2^64)), added on the GPU at "
+                         "the delivered rate, in every mode; core.watermark_detect finds it")
+    ap.add_argument("--watermark-payload", type=int, metavar="N", help="The mark's payload, [0, 4096) (default 0)")
+    ap.add_argument("--watermark-strength-db", type=float, metavar="DB",
+                    help="The mark's level relative to the local envelope, [-40, -10] dB (default -26)")
     ap.add_argument("--device", type=int, default=int(os.environ.get("SONATA_B200_DEVICE", "0")))
     return ap
+
+
+def _watermark_key(s: str) -> int:
+    return int(s, 16) if s.strip().lower().startswith("0x") else int(s, 10)
+
+
+def set_watermark_of(model, args) -> None:
+    """Mark `model` with the --watermark-* options, if a key is given; a payload or strength without a key is an
+    error."""
+    if args.watermark_key is None:
+        if args.watermark_payload is not None or args.watermark_strength_db is not None:
+            raise OperationError("--watermark-payload and --watermark-strength-db need --watermark-key")
+        return
+    model.set_watermark(args.watermark_key,
+                        0 if args.watermark_payload is None else args.watermark_payload,
+                        -26.0 if args.watermark_strength_db is None else args.watermark_strength_db)
 
 
 def process_request(synth: SonataSpeechSynthesizer, default_cfg: PiperSynthesisConfig, req: dict,
@@ -200,6 +222,7 @@ def process_request(synth: SonataSpeechSynthesizer, default_cfg: PiperSynthesisC
 def main(argv=None) -> int:
     args = build_parser().parse_args(argv)
     model = from_config_path(args.config, device=args.device)
+    set_watermark_of(model, args)
     synth = SonataSpeechSynthesizer(model)
     default_cfg = model.get_default_synthesis_config()
     if args.input_file:

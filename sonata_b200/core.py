@@ -165,6 +165,66 @@ def flac_encode(samples_i16: np.ndarray, sample_rate: int, device: int = 0) -> b
         lib.sb200_bytes_free(out)
 
 
+WATERMARK_PERIOD = 4096
+
+
+@dataclass
+class WatermarkResult:
+    """One clip's detection (include/sonata_b200.h, sb200_watermark_detect): whether it carries the key's mark (z0 >=
+    6.5), its payload (-1 unless marked and z1 >= 6.5), the clip start's position mod 4096, and both scores."""
+    marked: bool
+    payload: int
+    offset: int
+    z0: float
+    z1: float
+
+
+def check_watermark(key, payload, strength_db):
+    """(key, payload, strength_db) as the library takes them, or OperationError with the library's messages: a key in
+    [0, 2^64), a payload in [0, 4096), a finite strength in [-40, -10] dB."""
+    if isinstance(key, bool) or not isinstance(key, (int, np.integer)) or not 0 <= int(key) < 1 << 64:
+        raise OperationError(f"watermark: key {key!r} is not an integer in [0, 2^64)")
+    if isinstance(payload, bool) or not isinstance(payload, (int, np.integer)) or not 0 <= int(payload) < WATERMARK_PERIOD:
+        raise OperationError(f"watermark: payload {payload!r} is not in [0, 4096)")
+    ok = isinstance(strength_db, (int, float, np.integer, np.floating)) and not isinstance(strength_db, bool)
+    s = float(np.float32(strength_db)) if ok else math.nan
+    if not (ok and math.isfinite(s) and -40.0 <= s <= -10.0):
+        raise OperationError(f"watermark: strength_db {f'{s:g}' if ok else repr(strength_db)} is not a finite value in "
+                             "[-40, -10] dB")
+    return int(key), int(payload), s
+
+
+def watermark_detect(clips, key, device: int = 0):
+    """Detect key's watermark in each clip of `clips` (1-D float32 or int16 arrays, all of one dtype, each possibly
+    cropped anywhere) on CUDA device `device`, in one batched call: a list of WatermarkResult."""
+    import ctypes as C
+    from . import _native as N
+    from .piper import _check
+    if isinstance(key, bool) or not isinstance(key, (int, np.integer)) or not 0 <= int(key) < 1 << 64:
+        raise OperationError(f"watermark: key {key!r} is not an integer in [0, 2^64)")
+    if isinstance(device, bool) or not isinstance(device, (int, np.integer)) or int(device) < 0:
+        raise OperationError(f"device {device!r} is not a CUDA device index")
+    clips = list(clips)
+    dtypes = {c.dtype for c in clips if isinstance(c, np.ndarray)}
+    if any(not isinstance(c, np.ndarray) or c.ndim != 1 for c in clips) or not dtypes <= {np.dtype(np.float32),
+                                                                                          np.dtype(np.int16)}:
+        raise OperationError("watermark_detect takes 1-D numpy arrays of float32 or int16 samples")
+    if len(dtypes) > 1:
+        raise OperationError("watermark_detect takes clips of one dtype: all float32 or all int16")
+    if not clips:
+        return []
+    fmt = 1 if dtypes == {np.dtype(np.int16)} else 0
+    packed = np.ascontiguousarray(np.concatenate(clips))
+    offs = np.zeros(len(clips) + 1, np.uint64)
+    offs[1:] = np.cumsum([c.size for c in clips])
+    out = (N.sb200_watermark_result * len(clips))()
+    err = N.sb200_error()
+    _check(N.lib().sb200_watermark_detect(int(device), int(key), fmt, packed.ctypes.data_as(C.c_void_p),
+                                          offs.ctypes.data_as(C.POINTER(C.c_size_t)), len(clips), out, C.byref(err)),
+           err)
+    return [WatermarkResult(bool(r.marked), int(r.payload), int(r.offset), float(r.z0), float(r.z1)) for r in out]
+
+
 class AudioSamples:
     """struct AudioSamples(Vec<f32>) (audio/ops/src/samples.rs:16-18)."""
 

@@ -35,6 +35,10 @@ struct sb200_loudness_stream {
     LoudnessStream* s; std::shared_ptr<Voice> keep;
     ~sb200_loudness_stream() { delete s; }
 };
+struct sb200_watermark_stream {
+    WatermarkStream* w; std::shared_ptr<Voice> keep;
+    ~sb200_watermark_stream() { delete w; }
+};
 
 namespace {
 
@@ -682,6 +686,72 @@ int32_t sb200_flac_encode(int32_t device, const int16_t* x, size_t n, uint32_t s
     });
 }
 
+int32_t sb200_voice_set_watermark(sb200_voice* v, const sb200_watermark* wm, sb200_error* err) {
+    return guarded(err, [&] {
+        Voice& V = *v->v;
+        if (!wm) {
+            std::unique_lock<std::shared_mutex> g(V.cfg_mu);
+            V.wm_on = false;
+            return;
+        }
+        check_watermark(wm->payload, wm->strength_db);
+        bool known;
+        {
+            std::shared_lock<std::shared_mutex> g(V.cfg_mu);
+            known = V.wm_chips.count(wm->key) != 0;
+        }
+        // a new key's tables are built before the lock is taken, so running jobs of the voice do not wait for them
+        signed char* built = nullptr;
+        if (!known) {
+            SB_CUDA(cudaSetDevice(V.device));
+            built = build_watermark_chips(wm->key);
+        }
+        std::unique_lock<std::shared_mutex> g(V.cfg_mu);
+        const signed char*& chips = V.wm_chips[wm->key];
+        if (!chips && built) {
+            V.dev_allocs.push_back(built);
+            chips = built;
+        } else if (built) {
+            cudaFree(built);       // another thread set the same key meanwhile
+        }
+        V.wm = Watermark{wm->key, wm->payload, wm->strength_db, chips};
+        V.wm_on = true;
+    });
+}
+int32_t sb200_voice_watermark(const sb200_voice* v, sb200_watermark* out, int32_t* on, sb200_error* err) {
+    return guarded(err, [&] {
+        if (!on) throw Error(19, "null argument");
+        const Voice& V = *v->v;
+        std::shared_lock<std::shared_mutex> g(V.cfg_mu);
+        *on = V.wm_on ? 1 : 0;
+        if (V.wm_on && out) *out = sb200_watermark{V.wm.key, V.wm.payload, V.wm.strength_db};
+    });
+}
+int32_t sb200_watermark_detect(int32_t device, uint64_t key, int32_t fmt, const void* packed, const size_t* offsets,
+                               size_t batch, sb200_watermark_result* out, sb200_error* err) {
+    return guarded(err, [&] {
+        if (fmt != 0 && fmt != 1)
+            throw Error(19, "watermark detect: format " + std::to_string(fmt) + " is not 0 (f32) or 1 (i16)");
+        if (batch && (!offsets || !out)) throw Error(19, "null argument");
+        if (batch == 0) return;
+        for (size_t b = 0; b < batch; b++)
+            if (offsets[b + 1] < offsets[b])
+                throw Error(19, "watermark detect: clip " + std::to_string(b) + " ends before it starts");
+        const size_t n = offsets[batch] - offsets[0];
+        if (n && !packed) throw Error(19, "null argument");
+        SB_CUDA(cudaSetDevice(device));
+        DeviceBuffers d;
+        const size_t es = fmt == 0 ? 4 : 2;
+        char* dx = d.alloc<char>(n * es + 16);
+        if (n) SB_CUDA(cudaMemcpy(dx, static_cast<const char*>(packed) + offsets[0] * es, n * es, cudaMemcpyHostToDevice));
+        std::vector<size_t> offs(offsets, offsets + batch + 1);
+        for (size_t& o : offs) o -= offsets[0];
+        std::vector<WatermarkScore> s(batch);
+        watermark_detect(key, fmt, dx, offs.data(), batch, s.data(), 0);
+        for (size_t b = 0; b < batch; b++) out[b] = sb200_watermark_result{s[b].marked, s[b].payload, s[b].offset, s[b].z0, s[b].z1};
+    });
+}
+
 int32_t sb200_job_copy_out(sb200_job* job, void* dst, size_t cap, int32_t format, size_t* written, sb200_error* err) {
     return guarded(err, [&] {
         Job& j = *job->j;
@@ -1003,6 +1073,16 @@ int32_t sb200_decode_chunks_metered(sb200_voice* v, const sb200_latent* const* z
                                     const float* gain, sb200_resampler* const* resamplers,
                                     sb200_prosody_stream* const* warps, sb200_loudness_stream* const* meters,
                                     const int32_t* last, int32_t format, void** outs, size_t* lens, sb200_error* err) {
+    return sb200_decode_chunks_marked(v, zs, lo, hi, trim_lo_frames, trim_hi_frames, n, fade, gain, resamplers, warps,
+                                      meters, nullptr, last, format, outs, lens, err);
+}
+
+int32_t sb200_decode_chunks_marked(sb200_voice* v, const sb200_latent* const* zs, const int64_t* lo, const int64_t* hi,
+                                   const int64_t* trim_lo_frames, const int64_t* trim_hi_frames, size_t n, int32_t fade,
+                                   const float* gain, sb200_resampler* const* resamplers,
+                                   sb200_prosody_stream* const* warps, sb200_loudness_stream* const* meters,
+                                   sb200_watermark_stream* const* marks, const int32_t* last, int32_t format, void** outs,
+                                   size_t* lens, sb200_error* err) {
     return guarded(err, [&] {
         ChunkPass p = chunk_pass(zs, lo, hi, n, trim_lo_frames, trim_hi_frames, gain);
         if (n > 0 && (!resamplers || !outs || !lens)) throw Error(19, "null argument");
@@ -1010,6 +1090,7 @@ int32_t sb200_decode_chunks_metered(sb200_voice* v, const sb200_latent* const* z
             p.chunks[k].rs = resamplers[k] ? resamplers[k]->r : nullptr;
             p.chunks[k].ps = warps && warps[k] ? warps[k]->p : nullptr;
             p.chunks[k].ls = meters && meters[k] ? meters[k]->s : nullptr;
+            p.chunks[k].ws = marks && marks[k] ? marks[k]->w : nullptr;
             if (last) p.chunks[k].last = last[k];
         }
         p.fade = fade; p.resample = true; p.format = format;
@@ -1037,6 +1118,27 @@ int32_t sb200_loudness_stream_create(sb200_voice* v, uint32_t out_rate, float ta
     });
 }
 void sb200_loudness_stream_free(sb200_loudness_stream* s) { delete s; }
+
+int32_t sb200_watermark_stream_create(sb200_voice* v, uint32_t out_rate, sb200_watermark_stream** out,
+                                      sb200_error* err) {
+    return guarded(err, [&] {
+        if (!v || !out) throw Error(19, "null argument");
+        *out = nullptr;
+        Voice* w = v->v.get();
+        long long rate = w->sample_rate;
+        if (out_rate && out_rate != (uint32_t)w->sample_rate) {
+            resample_ratio(w->sample_rate, out_rate, "watermark stream: ");
+            rate = out_rate;
+        }
+        if (WatermarkStream* s = create_watermark_stream(w, rate)) *out = new sb200_watermark_stream{s, v->v};
+    });
+}
+void sb200_watermark_stream_free(sb200_watermark_stream* s) { delete s; }
+int32_t sb200_watermark_stream_profile(const sb200_watermark_stream* s, float* ms) {
+    if (!s || !ms) return 19;
+    *ms = s->w->last_ms;
+    return 0;
+}
 int32_t sb200_loudness_stream_state(const sb200_loudness_stream* s, double* lufs, float* gain, int64_t* samples,
                                     int64_t* clipped, float* ms, sb200_error* err) {
     return guarded(err, [&] {
@@ -1583,6 +1685,22 @@ int32_t sb200_debug_volume(int32_t device, const float* x, size_t n, const int64
         SB_CUDA(cudaSetDevice(device));
         HookStage h(o, x, n);
         if (n) SB_CUDA(cudaMemcpy(y, h.b.in, n * 4, cudaMemcpyDeviceToHost));
+    });
+}
+
+int32_t sb200_debug_watermark(const float* x, size_t n, int32_t rate, const sb200_watermark* wm, float* y,
+                              sb200_error* err) {
+    return guarded(err, [&] {
+        if ((n && (!x || !y)) || !wm || rate < 8000 || rate > 48000) throw Error(19, "debug watermark: bad arguments");
+        check_watermark(wm->payload, wm->strength_db);
+        DeviceBuffers d;
+        signed char* chips = build_watermark_chips(wm->key);
+        d.ptrs.push_back(chips);
+        OutputPlan o;
+        o.wp.add(Watermark{wm->key, wm->payload, wm->strength_db, chips}, 0, (long long)n, rate);
+        o.wp.total = (long long)n;
+        HookStage h(o, x, n);
+        if (n) SB_CUDA(cudaMemcpy(y, h.out.buf, n * 4, cudaMemcpyDeviceToHost));
     });
 }
 

@@ -118,6 +118,18 @@ struct PerDeviceOnce {
 __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
 __device__ __forceinline__ void pdl_trigger() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
 
+// One round of Philox4x32 (the noise draws in kernels_misc.cu, the watermark chips in watermark.cu).
+__device__ __forceinline__ void philox_round(unsigned& c0, unsigned& c1, unsigned& c2, unsigned& c3, unsigned k0,
+                                             unsigned k1) {
+    const unsigned long long p0 = (unsigned long long)0xD2511F53u * c0;
+    const unsigned long long p1 = (unsigned long long)0xCD9E8D57u * c2;
+    const unsigned n0 = (unsigned)(p1 >> 32) ^ c1 ^ k0;
+    const unsigned n1 = (unsigned)p1;
+    const unsigned n2 = (unsigned)(p0 >> 32) ^ c3 ^ k1;
+    const unsigned n3 = (unsigned)p0;
+    c0 = n0; c1 = n1; c2 = n2; c3 = n3;
+}
+
 template <typename... KArgs, typename... Args>
 inline void launch_pdl(void (*kern)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t st, Args&&... args) {
     static const int allowed = getenv("SB200_NO_PDL") ? 0 : 1;

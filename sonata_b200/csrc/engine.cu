@@ -851,6 +851,10 @@ void Job::run(float* d_out, size_t d_out_cap) {
     cudaStream_t st = C.stream;
     const int H = a.hidden, I = a.inter, F = a.filter;
     regions.clear(); dbg.clear(); dbg_level.clear(); id_frames.clear();
+    {
+        std::shared_lock<std::shared_mutex> g(V.cfg_mu);
+        wm_on = V.wm_on; wm = V.wm;
+    }
 
     // ---------------- id level (phase 1) workspace ----------------
     // Each utterance takes the attention it would take alone: the tensor-core attention (two grouped GEMMs around a
@@ -1318,7 +1322,15 @@ void decode_chunks(Voice* v, const ChunkPass& p, ChunkResult& out) {
                 fail(k, "the chunk is delivered at " + std::to_string(rate) + " Hz and its loudness stream meters " +
                             std::to_string(m->rate) + " Hz", "");
         }
-        if ((c.rs || c.ps) && c.last != 0 && c.last != 1)
+        if (const WatermarkStream* w = c.ws) {
+            if (!p.resample) fail(k, "a watermark stream needs a resampled chunk pass", "");
+            check_stream(k, &ChunkSpec::ws, "watermark stream", w->ended, "the watermark stream has already ended");
+            const long long rate = c.rs ? (long long)v->sample_rate * c.rs->f.up / c.rs->f.down : v->sample_rate;
+            if (rate != w->rate)
+                fail(k, "the chunk is delivered at " + std::to_string(rate) + " Hz and its watermark stream marks " +
+                            std::to_string(w->rate) + " Hz", "");
+        }
+        if ((c.rs || c.ps || c.ws) && c.last != 0 && c.last != 1)
             fail(k, "last flag " + std::to_string(c.last) + " is neither 0 nor 1", "");
     }
     // samples of each chunk after its trims
@@ -1343,7 +1355,8 @@ void decode_chunks(Voice* v, const ChunkPass& p, ChunkResult& out) {
     Context& C = *ctx;
     SB_CUDA(cudaSetDevice(v->device));
     lay_out_frames(l, len, hop, {});
-    const size_t total = p.resample ? (size_t)rp.total : (size_t)l.total_samples;
+    const WatermarkPlan& wp = op.wp;
+    const size_t total = !wp.segs.empty() ? (size_t)wp.total : p.resample ? (size_t)rp.total : (size_t)l.total_samples;
     ChunkBufs b;
     plan(C.dev_frame, C.pin, [&](Arena& dev, Arena& pin) { b.carve(dev, pin, *v, l, p, op, total); });
     cudaStream_t st = C.stream;
@@ -1370,7 +1383,8 @@ void decode_chunks(Voice* v, const ChunkPass& p, ChunkResult& out) {
     run_decoder(R, LY, b.y, b.dec, b.s, b.out.in);
     const Wave res = run_output_stage(R, op, b.out, Wave{b.out.in, b.y.fsegs.d, b.post.d, hop}, st);
     if (b.pcm) {
-        const long long longest = p.resample ? rp.max_out : (long long)*std::max_element(len.begin(), len.end()) * hop;
+        const long long longest = !wp.segs.empty() ? wp.max_n : p.resample ? rp.max_out
+                                                                             : (long long)*std::max_element(len.begin(), len.end()) * hop;
         launch_pcm(res.buf, res.segs, res.posts, (int)n, res.hop, longest, b.max, p.format, b.pcm, st);
     }
     SB_CUDA(cudaEventRecord(C.ev_end, st));
@@ -1383,8 +1397,8 @@ void decode_chunks(Voice* v, const ChunkPass& p, ChunkResult& out) {
     out.formant_ms = R.ms("formant"); out.loudness_ms = R.ms("loudness");
     if (p.format == PCM_I16) out.i16.resize(n); else if (b.pcm) out.g711.resize(n); else out.f32.resize(n);
     for (size_t k = 0; k < n; k++) {
-        const long long o = p.resample ? rp.segs[k].out_off : l.fsegs[k].out_off;
-        const long long m = p.resample ? rp.segs[k].n_out : n_in[k];
+        const long long o = !wp.segs.empty() ? wp.segs[k].y_off : p.resample ? rp.segs[k].out_off : l.fsegs[k].out_off;
+        const long long m = !wp.segs.empty() ? wp.segs[k].n : p.resample ? rp.segs[k].n_out : n_in[k];
         if (p.format == PCM_I16) {
             const int16_t* h = static_cast<const int16_t*>(b.out_h);
             out.i16[k].assign(h + o, h + o + m);

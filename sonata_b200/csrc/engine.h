@@ -426,6 +426,38 @@ std::vector<long long> prosody_stream_plan(int rate, float pitch, float tempo, c
 // emitted, frames, stretched samples, input and stretched history held).
 std::vector<long long> prosody_stream_counts(ProsodyStream& ps, const long long* chunk_lens, size_t n);
 
+// The watermark (watermark.cu; include/sonata_b200.h, sb200_voice_set_watermark): key, payload, strength and the key's
+// chip tables on the voice's device (c0 then c1, WM_P signed chars each).
+constexpr int WM_P = 4096;
+struct Watermark {
+    unsigned long long key = 0;
+    int payload = 0;
+    float strength_db = 0.f;
+    const signed char* chips = nullptr;
+};
+// One stream's watermark (include/sonata_b200.h, sb200_watermark_stream_create): the voice's setting when the stream was
+// made, its delivered rate and block, the inputs it has received and the outputs it has emitted (a multiple of blk
+// until the last chunk), and on the device two sets, read and written alternately, of the held inputs (fewer than blk)
+// and the S of the last block emitted.
+struct WatermarkStream {
+    Voice* v = nullptr;
+    Watermark wm;
+    long long rate = 0, blk = 0, in = 0, out = 0;
+    void* mem = nullptr;
+    float* hold[2] = {nullptr, nullptr};
+    long long* s[2] = {nullptr, nullptr};
+    int cur = 0;
+    bool ended = false;
+    float last_ms = 0.f;
+    ~WatermarkStream();
+};
+// The stream of voice v delivered at `rate`: null when the voice does not mark.
+WatermarkStream* create_watermark_stream(Voice* v, long long rate);
+// Checks a payload in [0, WM_P) and a finite strength in [-40, -10] dB; an error names the field.
+void check_watermark(long long payload, float strength_db);
+// The key's chip tables, built on the current device in memory the caller frees (cudaFree).
+signed char* build_watermark_chips(unsigned long long key);
+
 struct Context;   // stream + arenas for one in-flight call
 
 struct Voice {
@@ -440,6 +472,11 @@ struct Voice {
     SynthConfig factory_cfg;
     mutable std::shared_mutex cfg_mu;     // RwLock<PiperSynthesisConfig> (piper/src/lib.rs:292)
     SynthConfig cfg;
+    // under cfg_mu: the watermark when wm_on, and the chip tables of every key ever set (in dev_allocs), kept because
+    // a job that started under an earlier key may still read its table
+    bool wm_on = false;
+    Watermark wm;
+    std::map<unsigned long long, const signed char*> wm_chips;
 
     // ---- weights ----
     int device = 0;
@@ -615,6 +652,8 @@ struct Job {
     std::vector<long long> fit_len;   // rate (NaN and -1 for a span that asked nothing); empty when it had none
     std::vector<SpeakerBlend> blends; // one canonical blend per utterance (empty entry: the config's speaker); empty when
                                       // none has one (set_job_blends)
+    bool wm_on = false;               // the voice's watermark, read when the run starts
+    Watermark wm;
     std::vector<ProsodyShape> pros_ran;   // each utterance's shape in the last run (empty: it ran no prosody stage)
     std::vector<float> pitch_ran, tempo_ran;   // the ratios the last run had (empty: none)
     std::vector<long long> pros_bounds;   // each id's delivered end in the last run when it had a contour, a volume
@@ -782,6 +821,7 @@ struct ChunkSpec {
     Resampler* rs = nullptr;              // the chunk's stream (resample passes; null: none)
     ProsodyStream* ps = nullptr;          // the chunk's pitch / tempo stream (resample passes; null: none)
     LoudnessStream* ls = nullptr;         // the chunk's live loudness meter (resample passes; null: none)
+    WatermarkStream* ws = nullptr;        // the chunk's watermark (resample passes; null: none)
     int last = 0;                         // 1: the chunk ends its stream, which is flushed
 };
 // One frame-level decoder pass over chunks of latents of one voice; chunk k equals the same chunk decoded alone, bit for
@@ -850,6 +890,38 @@ struct ResamplePlan {
     void add(const ResampleFilter* f, long long n_in, const Resampler* r = nullptr, bool last = false);
 };
 
+// The watermark launch.  Segment q emits n samples of its input at y[y_off ..): the h samples at hold, then the m at
+// x[x_off ..), the mark at positions pos0 + i in blocks of blk = R / 100 samples (chips null: copied unchanged).  The
+// block before the first is block 0, or with s_in the block whose S is *s_in.  A job's segments are whole utterances,
+// read and written at the same offset (h = 0, m = n, pos0 = 0).  A stream's also put the inputs past n into hold_out
+// and the S of the last block they emit into s_out (WatermarkStream).
+struct WatermarkSeg {
+    long long x_off, y_off, n, m, pos0;
+    int h, blk, payload;
+    double alpha;
+    const signed char* chips;
+    const float* hold; float* hold_out;
+    const long long* s_in; long long* s_out;
+};
+struct WatermarkStream;
+struct WatermarkPlan {
+    std::vector<WatermarkSeg> segs;
+    long long total = 0, max_runs = 0, max_n = 0;
+    double bytes = 0;
+    // A job's utterance of n samples at offset off, delivered at `rate`.
+    void add(const Watermark& wm, long long off, long long n, int rate);
+    // A chunk of m new samples at x_off: with its stream ws, what the stream emits for it (the hold-back rule of
+    // include/sonata_b200.h, sb200_watermark_stream_create), else the chunk copied; written at total ..
+    void add_chunk(const WatermarkStream* ws, long long x_off, long long m, bool last);
+};
+void launch_watermark(const WatermarkPlan& p, const WatermarkSeg* segs, const float* x, float* y, cudaStream_t st);
+// Detection (include/sonata_b200.h, sb200_watermark_detect) of `batch` clips of fmt 0 (f32) or 1 (i16) samples at
+// d_x[offs[b] .. offs[b + 1]) on the device, into out[0 .. batch); the device work runs on st.  F (null: not wanted)
+// receives every clip's fold, WM_P int64 each.
+struct WatermarkScore { int marked, payload, offset; double z0, z1; };
+void watermark_detect(unsigned long long key, int fmt, const void* d_x, const size_t* offs, size_t batch,
+                      WatermarkScore* out, cudaStream_t st, long long* F = nullptr);
+
 // The loudness launch over what a job hands out: one segment per utterance at its delivered rate, chunk scratch laid out
 // back to back.
 struct LoudnessPlan {
@@ -875,6 +947,7 @@ struct OutputPlan {
     VolumePlan vp;
     BreakPlan bp;
     ResamplePlan rp;
+    WatermarkPlan wp;                         // jobs of a marked voice
     LoudnessPlan lp;                          // whole signals
     MeterPlan mp;                             // chunk passes
     std::vector<ChunkSpec> chunks;            // chunk passes: empty for a job
@@ -912,6 +985,7 @@ struct OutputBufs {
     Staged<BreakSeg> bsegs; Staged<BreakPiece> bpieces; Staged<FrameSeg> bosegs; float* by = nullptr;
     Staged<FrameSeg> rin; Staged<PcmPost> rpost;  // chunk passes: what the resample launch reads after the stages
     Staged<ResampleSeg> rsegs; Staged<PcmPost> rposts; Staged<FrameSeg> rosegs; float* ry = nullptr;
+    Staged<WatermarkSeg> wsegs; Staged<FrameSeg> wosegs; Staged<PcmPost> wposts; float* wy = nullptr;
     Staged<LoudSeg> lsegs; double* lscratch = nullptr; Staged<double> lufs; Staged<float> gain;
     Staged<LoudStreamSeg> msegs; float* mwin = nullptr; double* me = nullptr;
     Staged<double> mlufs; Staged<float> mgains; Staged<unsigned long long> mclip;
@@ -923,7 +997,8 @@ struct OutputBufs {
 };
 
 // The launches of plan p from the input wave `in` (in.buf == b.in) on st: profile regions "stretch", "pitch",
-// "formant", "volume", "break", "resample" and "loudness", each only when its stage runs.  A job's volume stage scales
+// "formant", "volume", "break", "resample", "watermark" (a job of a marked voice: into wy, at the same offsets) and
+// "loudness", each only when its stage runs.  A job's volume stage scales
 // its utterances in place; a chunk pass's writes each chunk to vy (after fy).  The break stage writes every segment to
 // by, longer by its pauses.  Returns what the stage delivers: the last
 // output's wave (a job's: its segments at hop 1 once a stage has changed their lengths).  The loudness results are

@@ -1045,17 +1045,6 @@ __global__ void gather_rows_kernel(const GatherSeg* __restrict__ segs, const int
 }
 
 // ------------------------------------------------------------------ Philox4x32-10 -> N(0,1)
-__device__ __forceinline__ void philox_round(unsigned& c0, unsigned& c1, unsigned& c2, unsigned& c3, unsigned k0,
-                                             unsigned k1) {
-    const unsigned long long p0 = (unsigned long long)0xD2511F53u * c0;
-    const unsigned long long p1 = (unsigned long long)0xCD9E8D57u * c2;
-    const unsigned n0 = (unsigned)(p1 >> 32) ^ c1 ^ k0;
-    const unsigned n1 = (unsigned)p1;
-    const unsigned n2 = (unsigned)(p0 >> 32) ^ c3 ^ k1;
-    const unsigned n3 = (unsigned)p0;
-    c0 = n0; c1 = n1; c2 = n2; c3 = n3;
-}
-
 // Four N(0,1) values from one Philox4x32-10 block of counter (c0..c3) under key (k0, k1), by Box-Muller
 // (tests/noise_reference.py restates it on the host).
 __device__ __forceinline__ void philox_normal4(unsigned c0, unsigned c1, unsigned c2, unsigned c3, unsigned k0,

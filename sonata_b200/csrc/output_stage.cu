@@ -1,5 +1,6 @@
 // The waveform output stage: what runs after the decoder, in this order: prosody (the stretch and the pitch stage), the
-// formant stage, the volume stage, the break stage, resampling, and loudness in place on what those leave.  Jobs, chunk passes and the
+// formant stage, the volume stage, the break stage, resampling, the watermark, and loudness in place on what those
+// leave.  Jobs, chunk passes and the
 // test hooks plan, carve and launch it here only, so they run the same launches.
 #include "engine.h"
 #include <algorithm>
@@ -159,6 +160,13 @@ OutputPlan plan_job_output(Job& j, int hop, const std::vector<int>& cum, std::ve
         }
         j.out_hop = 1; j.out_total = o.rp.total;
     }
+    // watermark: a marked voice's every utterance as the job hands it out, at its rate, into the stage's own output at
+    // the same offsets
+    if (audio && j.wm_on) {
+        for (size_t b = 0; b < B; b++)
+            o.wp.add(j.wm, j.osegs[b].out_off, (long long)j.osegs[b].len * j.out_hop, j.osr[b]);
+        o.wp.total = j.out_total;
+    }
     // loudness: every utterance as the job hands it out, at its rate, with its target or NaN
     if (audio && !j.loud_target.empty()) {
         LoudnessPlan& lp = o.lp;
@@ -219,9 +227,14 @@ OutputPlan plan_chunk_output(const std::vector<ChunkSpec>& chunks, const std::ve
         }
         if (resample) o.rp.add(c.rs ? &c.rs->f : nullptr, o.n_res[k], c.rs, c.last != 0);
     }
+    // watermark: when some chunk's stream marks, every chunk of the pass at its delivered rate, a marked one as its
+    // stream emits it and the others copied, back to back
+    if (resample && std::any_of(chunks.begin(), chunks.end(), [](const ChunkSpec& c) { return c.ws != nullptr; }))
+        for (size_t k = 0; k < n; k++)
+            o.wp.add_chunk(chunks[k].ws, o.rp.segs[k].out_off, o.rp.segs[k].n_out, chunks[k].last != 0);
     for (size_t k = 0; k < n; k++)
         if (const LoudnessStream* m = chunks[k].ls) {
-            const long long d = resample ? o.rp.segs[k].n_out : o.n_res[k];
+            const long long d = !o.wp.segs.empty() ? o.wp.segs[k].n : resample ? o.rp.segs[k].n_out : o.n_res[k];
             o.mp.add((int)k, *m, d, loudness_stream_steps(*m, d, "chunk " + std::to_string(k) + ": "));
         }
     return o;
@@ -231,6 +244,13 @@ void OutputBufs::carve(Arena& dev, Arena& pin, const OutputPlan& p, long long in
     *this = OutputBufs();
     const ProsodyPlan& pp = p.pp;
     const FormantPlan& fp = p.fp;
+    if (const size_t n = p.wp.segs.size()) {
+        // the watermark is the last stage that writes: into d_out, and every stage before it into the pass's own
+        wsegs.carve(dev, pin, n);
+        if (p.streams()) { wosegs.carve(dev, pin, n); wposts.carve(dev, pin, n); }
+        wy = d_out ? d_out : dev.get<float>((size_t)p.wp.total + 4);
+        d_out = nullptr;
+    }
     if (const size_t n = pp.segs.size()) {
         psegs.carve(dev, pin, n);
         if (!pp.pieces.empty()) pieces.carve(dev, pin, pp.pieces.size());     // a stream's table is its own
@@ -413,6 +433,21 @@ void OutputBufs::upload(const OutputPlan& p, int hop, const FrameSeg* in_segs, c
         }
         rsegs.upload(st); rposts.upload(st); rosegs.upload(st);
     }
+    if (wsegs.d) {
+        std::copy(p.wp.segs.begin(), p.wp.segs.end(), wsegs.h);
+        for (size_t k = 0; wosegs.d && k < p.wp.segs.size(); k++) {
+            // a stream's held samples and carried S, read from one set and written to the other
+            if (const WatermarkStream* w = p.chunks[k].ws) {
+                WatermarkSeg& g = wsegs.h[k];
+                g.hold = w->hold[w->cur]; g.hold_out = w->hold[1 - w->cur];
+                g.s_in = w->out > 0 ? w->s[w->cur] : nullptr; g.s_out = w->s[1 - w->cur];
+            }
+            wosegs.h[k] = FrameSeg{0, (int)p.wp.segs[k].n, 0, 0, p.wp.segs[k].y_off};
+            wposts.h[k] = rposts.h[k];
+        }
+        wsegs.upload(st);
+        if (wosegs.d) { wosegs.upload(st); wposts.upload(st); }
+    }
     if (lsegs.d) {
         std::copy(p.lp.segs.begin(), p.lp.segs.end(), lsegs.h);
         lsegs.upload(st);
@@ -422,7 +457,7 @@ void OutputBufs::upload(const OutputPlan& p, int hop, const FrameSeg* in_segs, c
         const MeterPlan& mp = p.mp;
         for (size_t q = 0; q < mp.chunks.size(); q++) {
             const int k = mp.chunks[q];
-            float* y = ry ? ry + p.rp.segs[k].out_off : at[k];
+            float* y = wy ? wy + p.wp.segs[k].y_off : ry ? ry + p.rp.segs[k].out_off : at[k];
             LoudStreamSeg g = loudness_stream_seg(*p.chunks[k].ls, y, mp.n[q], p.chunks[k].gain);
             g.win = mwin + mp.win_off[q]; g.e = me + 8 * mp.step_off[q];
             g.lufs = mlufs.d + mp.step_off[q]; g.gains = mgains.d + mp.step_off[q]; g.clipped = mclip.d + q;
@@ -502,6 +537,17 @@ Wave run_output_stage(Profile& prof, const OutputPlan& p, const OutputBufs& b, W
         prof.end();
         cur = Wave{b.ry, b.rosegs.d, b.rposts.d, 1};
     }
+    const WatermarkPlan& wp = p.wp;
+    if (!wp.segs.empty()) {
+        // segments are read plainly: a job's waves carry no post-path, or the resampler's identity one, and a chunk
+        // pass's resampled output keeps its post-path (the gain of G.711, the fixed scale) for the conversion
+        prof.begin("watermark");
+        launch_watermark(wp, b.wsegs.d, cur.buf, b.wy, st);
+        prof.count(0, wp.bytes);
+        prof.end();
+        if (streams) cur = Wave{b.wy, b.wosegs.d, b.wposts.d, 1};
+        else cur.buf = b.wy;
+    }
     if (!p.lp.segs.empty()) {
         // the samples read and, where a target scales them, written
         double samples = 0, scaled = 0;
@@ -560,6 +606,16 @@ void advance_streams(const OutputPlan& p, const OutputBufs& b, const Profile& pr
             w->last_brk_ms = w->brk.empty() ? 0.f : break_ms;
         }
     }
+    const float watermark_ms = prof.ms("watermark");
+    for (size_t k = 0; k < p.chunks.size() && !p.wp.segs.empty(); k++)
+        if (WatermarkStream* w = p.chunks[k].ws) {
+            const WatermarkSeg& g = p.wp.segs[k];
+            w->in += g.m;
+            w->out += g.n;
+            w->cur ^= 1;
+            w->ended = p.chunks[k].last != 0;
+            w->last_ms = watermark_ms;
+        }
     const MeterPlan& mp = p.mp;
     for (size_t q = 0; q < mp.chunks.size(); q++) {
         LoudnessStream* m = p.chunks[mp.chunks[q]].ls;

@@ -18,7 +18,7 @@ import numpy as np
 
 from . import _native as N
 from .core import (G711_LAW, Audio, AudioInfo, AudioSamples, OperationError, PhonemeAlignment, Phonemes,
-                   PhonemizationError, SonataError, check_encoding, refuse_flac)
+                   PhonemizationError, SonataError, check_encoding, check_watermark, refuse_flac)
 
 MIN_CHUNK_SIZE = 44      # piper/src/lib.rs:18
 MAX_CHUNK_SIZE = 1024    # piper/src/lib.rs:19
@@ -945,6 +945,25 @@ class _VitsCommons:
             self._speakers = {int(v): k for k, v in m.items()}
         return self._speakers or None
 
+    def set_watermark(self, key, payload: int = 0, strength_db: float = -26.0):
+        """Mark everything this voice delivers from now on with key's watermark carrying `payload` (include/sonata_b200.h,
+        sb200_voice_set_watermark): every job and batch route, at each utterance's delivered rate.  key None turns it
+        off.  A realtime stream reads the setting when it is made and keeps it to its end.  Bad values raise
+        OperationError and leave the voice as it was."""
+        err = N.sb200_error()
+        if key is None:
+            _check(self._lib.sb200_voice_set_watermark(self._h, None, C.byref(err)), err)
+            return
+        k, p, s = check_watermark(key, payload, strength_db)
+        wm = N.sb200_watermark(k, p, s)
+        _check(self._lib.sb200_voice_set_watermark(self._h, C.byref(wm), C.byref(err)), err)
+
+    def watermark(self) -> Optional[Tuple[int, int, float]]:
+        """(key, payload, strength_db) of the voice's watermark, or None when it marks nothing."""
+        wm, on, err = N.sb200_watermark(), C.c_int32(), N.sb200_error()
+        _check(self._lib.sb200_voice_watermark(self._h, C.byref(wm), C.byref(on), C.byref(err)), err)
+        return (int(wm.key), int(wm.payload), float(wm.strength_db)) if on.value else None
+
     def close(self):
         if getattr(self, "_h", None) and self._h.value:
             self._lib.sb200_voice_free(self._h)
@@ -1650,6 +1669,48 @@ class LoudnessStream:
             pass
 
 
+class WatermarkStream:
+    """One realtime stream's watermark on the device (sb200_watermark_stream_*): the voice's watermark as it was when
+    the stream was made, kept to the stream's end, at the stream's delivered rate `output_rate` (None: the voice's).
+    The stage holds back fewer than 10 ms (the samples past the last whole block) until the stream's last chunk.
+    Made by `open`, which gives None for a voice that marks nothing."""
+
+    def __init__(self, model: "_VitsCommons", handle: C.c_void_p, rate: int):
+        self._m, self._h, self.rate = model, handle, rate
+
+    @classmethod
+    def open(cls, model: "_VitsCommons", output_rate: Optional[int] = None) -> Optional["WatermarkStream"]:
+        h, err = C.c_void_p(), N.sb200_error()
+        _check(model._lib.sb200_watermark_stream_create(model._h, int(output_rate or 0), C.byref(h), C.byref(err)),
+               err)
+        if not h.value:
+            return None
+        return cls(model, h, int(output_rate) if output_rate else model.audio_output_info().sample_rate)
+
+    @property
+    def last_pass_ms(self) -> float:
+        """The "watermark" device time (ms) of the last chunk pass this stream was in."""
+        ms = C.c_float()
+        self._m._lib.sb200_watermark_stream_profile(self._h, C.byref(ms))
+        return float(ms.value)
+
+    def __del__(self):
+        try:
+            if self._h:
+                self._m._lib.sb200_watermark_stream_free(self._h)
+                self._h = None
+        except Exception:
+            pass
+
+
+def _stream_mark(model, output_rate) -> Optional[WatermarkStream]:
+    """The watermark of a new stream of `model` (None when the voice marks nothing, or is not a loaded streaming voice
+    of this library, which holds no setting)."""
+    if not isinstance(model, VitsStreamingModel) or not getattr(model, "_h", None):
+        return None
+    return WatermarkStream.open(model, output_rate)
+
+
 def _stream_meter(model, live_loudness, max_gain_db, output_rate, who: str) -> Optional[LoudnessStream]:
     """The meter of a stream with `live_loudness` (None: none; a target in LUFS: a fresh meter; a LoudnessStream: that
     meter, continued), checked against the stream's output rate.  Errors name `who`."""
@@ -1711,9 +1772,9 @@ class _Stream:
 
     def __init__(self, key, enc, chunk_size: int, chunk_padding: int, resampler: Optional[Resampler] = None,
                  encoding: Optional[str] = None, gain: float = 1.0, warp: Optional[ProsodyStream] = None,
-                 meter: Optional[LoudnessStream] = None):
+                 meter: Optional[LoudnessStream] = None, mark: Optional[WatermarkStream] = None):
         self.key, self.enc, self.resampler = key, enc, resampler
-        self.meter = meter
+        self.meter, self.mark = meter, mark
         self.encoding, self.gain = encoding, gain
         self.warp = warp
         self.chunker = AdaptiveMelChunker(enc.num_frames, chunk_size, chunk_padding)
@@ -1729,7 +1790,8 @@ class _Stream:
     def on_device(self) -> bool:
         """Whether the chunks' trim and crossfade run on the device, with the stream's encoding, resampler, prosody
         stream or meter."""
-        return not (self.encoding is None and self.resampler is None and self.warp is None and self.meter is None)
+        return not (self.encoding is None and self.resampler is None and self.warp is None and self.meter is None
+                    and self.mark is None)
 
     def next_chunk(self):
         """(lo, hi, audio slice or None): the frames to decode next, and how the plain path trims them (None: the
@@ -1752,8 +1814,10 @@ def _device_post(model, plan) -> list:
     s0 = plan[0][0]
     streams = [s for s, _, _, _ in plan]
     kw = {}
-    if s0.resampler is not None or s0.warp is not None or s0.meter is not None:
+    if s0.resampler is not None or s0.warp is not None or s0.meter is not None or s0.mark is not None:
         kw.update(resamplers=[s.resampler for s in streams], last=[s.done for s in streams])
+    if s0.mark is not None:
+        kw["marks"] = [s.mark for s in streams]
     if s0.warp is not None:
         kw["warps"] = [s.warp for s in streams]
     if s0.meter is not None:
@@ -1771,8 +1835,9 @@ class SpeechStreamer(_Stream):
 
     def __init__(self, enc: EncoderOutputs, chunk_size: int, chunk_padding: int,
                  resampler: Optional[Resampler] = None, encoding: Optional[str] = None, gain: float = 1.0,
-                 warp: Optional[ProsodyStream] = None, meter: Optional[LoudnessStream] = None):
-        super().__init__(None, enc, chunk_size, chunk_padding, resampler, encoding, gain, warp, meter)
+                 warp: Optional[ProsodyStream] = None, meter: Optional[LoudnessStream] = None,
+                 mark: Optional[WatermarkStream] = None):
+        super().__init__(None, enc, chunk_size, chunk_padding, resampler, encoding, gain, warp, meter, mark)
 
     def __iter__(self) -> Iterator[AudioSamples]:
         return self
@@ -1845,7 +1910,8 @@ class VitsStreamingModel(_VitsCommons):
     def infer_decoder_batch(self, chunks: Sequence[tuple], pcm16: bool = False, fade: int = 0,
                             gains: Optional[Sequence[float]] = None, resamplers: Optional[Sequence] = None,
                             last: Optional[Sequence[bool]] = None, encoding: Optional[str] = None,
-                            warps: Optional[Sequence] = None, meters: Optional[Sequence] = None) -> list:
+                            warps: Optional[Sequence] = None, meters: Optional[Sequence] = None,
+                            marks: Optional[Sequence] = None) -> list:
         """Many `EncoderOutputs.infer_decoder(lo, hi)` calls as one decoder pass.  `chunks`: (encoder outputs, lo, hi)
         per chunk; each result equals that chunk decoded alone, bit for bit.
 
@@ -1868,7 +1934,11 @@ class VitsStreamingModel(_VitsCommons):
 
         With `meters` (one LoudnessStream or None per chunk; chunks may carry trims, as with resamplers), what chunk k
         delivers is metered by its live loudness stream after all that, gains[k] applies after the meter, and pcm16 /
-        G.711 convert it at the fixed scale (sb200_decode_chunks_metered)."""
+        G.711 convert it at the fixed scale (sb200_decode_chunks_metered).
+
+        With `marks` (one WatermarkStream or None per chunk; chunks may carry trims, as with resamplers), what chunk k
+        delivers after resampling is marked by its stream before any meter and conversion: the stream emits its
+        whole 10 ms blocks and holds back the rest until its last chunk (sb200_decode_chunks_marked)."""
         refuse_flac(encoding, "a decoder chunk pass")
         check_encoding(encoding)
         if encoding is not None and pcm16:
@@ -1879,7 +1949,7 @@ class VitsStreamingModel(_VitsCommons):
         hs = (C.c_void_p * n)()
         for k, c in enumerate(chunks):
             if len(c) not in ((3, 5) if pcm16 or encoding or resamplers is not None or warps is not None
-                              or meters is not None else (3,)):
+                              or meters is not None or marks is not None else (3,)):
                 raise OperationError(f"Invalid decoder chunk {k}: expected (encoder outputs, lo, hi"
                                      + (", trim_lo, trim_hi)" if pcm16 else ")"))
             enc = c[0]
@@ -1895,8 +1965,9 @@ class VitsStreamingModel(_VitsCommons):
             return []
         p64 = lambda a: a.ctypes.data_as(C.POINTER(C.c_int64))
         err = N.sb200_error()
-        if resamplers is not None or warps is not None or meters is not None:
+        if resamplers is not None or warps is not None or meters is not None or marks is not None:
             rs = _handles([None] * n if resamplers is None else resamplers, n, Resampler, "resamplers")
+            mk = None if marks is None else _handles(marks, n, WatermarkStream, "marks")
             ws = None if warps is None else _handles(warps, n, ProsodyStream, "warps")
             ms = None if meters is None else _handles(meters, n, LoudnessStream, "meters")
             fl = np.zeros(n, np.int32) if last is None else np.array([1 if x else 0 for x in
@@ -1906,9 +1977,9 @@ class VitsStreamingModel(_VitsCommons):
             lens = (C.c_size_t * n)()
             fmt = G711_LAW[encoding] + 2 if encoding else 1 if pcm16 else 0
             gp = None if g is None else g.ctypes.data_as(C.POINTER(C.c_float))
-            _check(self._lib.sb200_decode_chunks_metered(
-                self._h, hs, p64(lo), p64(hi), p64(tlo), p64(thi), n, int(fade), gp, rs, ws, ms, _ptr(fl, C.c_int32),
-                fmt, outs, lens, C.byref(err)), err)
+            _check(self._lib.sb200_decode_chunks_marked(
+                self._h, hs, p64(lo), p64(hi), p64(tlo), p64(thi), n, int(fade), gp, rs, ws, ms, mk,
+                _ptr(fl, C.c_int32), fmt, outs, lens, C.byref(err)), err)
             if encoding:
                 return _take_bytes(self._lib, outs, lens)
             if pcm16:
@@ -2000,7 +2071,8 @@ class VitsStreamingModel(_VitsCommons):
         else:
             enc = self.infer_encoder_batch([o.ids], seeds=[o.seed], speaker_blends=[o.blend])[0]
         resampler, warp, meter = _open_stream(self, o, enc)
-        return SpeechStreamer(enc, chunk_size, chunk_padding, resampler, o.encoding, o.gain, warp, meter)
+        return SpeechStreamer(enc, chunk_size, chunk_padding, resampler, o.encoding, o.gain, warp, meter,
+                              _stream_mark(self, o.output_rate))
 
 
 def _stream_gain(encoding, gain) -> float:
@@ -2042,6 +2114,7 @@ class _StreamOptions:
     volume: Optional[Sequence] = None   # per id
     breaks: Optional[Sequence] = None   # per id
     target: object = None               # checked target entry in ids (_target_entry), or None
+    mark: object = None                 # StreamBatch: the WatermarkStream read when the stream was added, or None
 
 
 def _stream_options(model, where: str, key: Optional[int], ids_or_phonemes, config=None, chunk_size=None,
@@ -2189,6 +2262,7 @@ class StreamBatch:
                             speaker_blend=speaker_blend, live_loudness=live_loudness, max_gain_db=max_gain_db,
                             carried=carried, volume_contour=volume_contour, breaks=breaks,
                             target_duration=target_duration)
+        o.mark = _stream_mark(self.model, o.output_rate)      # the voice's watermark as it is when the stream is added
         self._next_key += 1
         self._pending.append(o)
         return o.key
@@ -2239,7 +2313,7 @@ class StreamBatch:
                     try:
                         resampler, warp, meter = _open_stream(self.model, o, enc)
                         active.append(_Stream(o.key, enc, o.chunk_size, self.chunk_padding, resampler, o.encoding,
-                                              o.gain, warp, meter))
+                                              o.gain, warp, meter, o.mark))
                         continue
                     except SonataError as e:
                         err = e
@@ -2248,12 +2322,13 @@ class StreamBatch:
         failed = set()
         # one pass per (encoding, resampled, one-shot, warped, metered): the streams without an encoding first, in
         # their usual passes; warped and metered streams in passes of their own
-        plain_key = (None, False, False, False, False)
-        groups = {plain_key: [], (None, True, False, False, False): [], (None, True, True, False, False): []}
+        plain_key = (None, False, False, False, False, False)
+        groups = {plain_key: [], (None, True, False, False, False, False): [],
+                  (None, True, True, False, False, False): []}
         for p in plan:
             s = p[0]
             k = plain_key if not s.on_device else (s.encoding, s.resampler is not None, p[3] is None,
-                                                   s.warp is not None, s.meter is not None)
+                                                   s.warp is not None, s.meter is not None, s.mark is not None)
             groups.setdefault(k, []).append(p)
         decoded = {}
         for key, group in groups.items():
